@@ -243,7 +243,7 @@ enum b200_pool { B200_POOL_MEAN = 0, B200_POOL_CLS = 1 };
 typedef struct b200_tower_desc {
     int32_t width;      /* hidden size */
     int32_t layers;     /* transformer blocks */
-    int32_t heads;      /* head_dim = width / heads must be 64 */
+    int32_t heads;      /* head_dim = width / heads must be 32 or 64 */
     int32_t mlp;        /* MLP hidden size */
     int32_t ctx;        /* text: context length (77 / 512); vision: unused */
     int32_t vocab;      /* text: vocabulary size; vision: unused */

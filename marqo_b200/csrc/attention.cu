@@ -3,10 +3,11 @@
 namespace mb {
 namespace attention {
 
-constexpr int HD = 64;        // head dim
 constexpr int BQ = 64;        // query rows per CTA (4 warps x 16)
 constexpr int BKV = 64;       // keys per block
 constexpr int THREADS = 128;
+template <int HD>
+constexpr int CH_LOG2 = HD == 64 ? 3 : 2;   // log2 of the HD / 8 16-byte chunks per tile row
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -37,24 +38,28 @@ __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
     return *reinterpret_cast<uint32_t*>(&v);
 }
 
-// tile: 64 rows x 64 bf16 (128 B per row), 16-byte chunks XOR-swizzled by (row & 7)
+// tile: 64 rows x HD bf16 (HD / 8 16-byte chunks per row), chunks XOR-swizzled so that the 8 rows one ldmatrix reads
+// cover all 32 banks: HD = 64 (128 B rows) by (row & 7); HD = 32 (64 B rows, two per 128 B line) by ((row >> 1) & 3).
+template <int HD>
 __device__ __forceinline__ __nv_bfloat16* tile_ptr(__nv_bfloat16* tile, int row, int chunk) {
-    return tile + row * HD + ((chunk ^ (row & 7)) << 3);
+    const int swz = HD == 64 ? (row & 7) : ((row >> 1) & 3);
+    return tile + row * HD + ((chunk ^ swz) << 3);
 }
 
+template <int HD>
 __device__ __forceinline__ void load_tile(__nv_bfloat16* tile, const __nv_bfloat16* base, int row0, int nrows, int ld) {
     // base points at (sequence row 0, first column of this head's q/k/v slice)
 #pragma unroll
-    for (int i = 0; i < (64 * 8) / THREADS; ++i) {
+    for (int i = 0; i < (64 << CH_LOG2<HD>) / THREADS; ++i) {
         const int idx = threadIdx.x + i * THREADS;
-        const int r = idx >> 3, c = idx & 7;
+        const int r = idx >> CH_LOG2<HD>, c = idx & ((1 << CH_LOG2<HD>) - 1);
         const bool ok = row0 + r < nrows;
         const __nv_bfloat16* src = base + (size_t)(ok ? row0 + r : 0) * ld + c * 8;
-        cp_async16(tile_ptr(tile, r, c), src, ok);
+        cp_async16(tile_ptr<HD>(tile, r, c), src, ok);
     }
 }
 
-template <int MASK>
+template <int HD, int MASK>
 __global__ void __launch_bounds__(THREADS)
 attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out, int S, int W,
                  const int32_t* __restrict__ kv_len, float scale_log2e) {
@@ -77,17 +82,17 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
     if (MASK == MASK_CAUSAL) kend = min(len, q0 + BQ);
     const int nkb = (kend + BKV - 1) / BKV;
 
-    load_tile(sQ, qbase, q0, S, ld);
+    load_tile<HD>(sQ, qbase, q0, S, ld);
     if (nkb > 0) {
-        load_tile(sK[0], kbase, 0, len, ld);
-        load_tile(sV[0], vbase, 0, len, ld);
+        load_tile<HD>(sK[0], kbase, 0, len, ld);
+        load_tile<HD>(sV[0], vbase, 0, len, ld);
     }
     cp_async_commit();
 
-    uint32_t qf[4][4];
-    float o[8][4];
+    uint32_t qf[HD / 16][4];
+    float o[HD / 8][4];
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
+    for (int i = 0; i < HD / 8; ++i)
 #pragma unroll
         for (int j = 0; j < 4; ++j) o[i][j] = 0.f;
     float row_max[2] = {-INFINITY, -INFINITY};
@@ -97,8 +102,8 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
     for (int kb = 0; kb < nkb; ++kb) {
         const int buf = kb & 1;
         if (kb + 1 < nkb) {
-            load_tile(sK[buf ^ 1], kbase, (kb + 1) * BKV, len, ld);
-            load_tile(sV[buf ^ 1], vbase, (kb + 1) * BKV, len, ld);
+            load_tile<HD>(sK[buf ^ 1], kbase, (kb + 1) * BKV, len, ld);
+            load_tile<HD>(sV[buf ^ 1], vbase, (kb + 1) * BKV, len, ld);
             cp_async_commit();
             cp_async_wait<1>();
         } else {
@@ -107,9 +112,9 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
         __syncthreads();
         if (kb == 0) {
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
+            for (int ks = 0; ks < HD / 16; ++ks) {
                 const int mat = lane >> 3, r = lane & 7;
-                ldmatrix_x4(qf[ks], tile_ptr(sQ, warp * 16 + (mat & 1) * 8 + r, ks * 2 + (mat >> 1)));
+                ldmatrix_x4(qf[ks], tile_ptr<HD>(sQ, warp * 16 + (mat & 1) * 8 + r, ks * 2 + (mat >> 1)));
             }
         }
         // ---- S = Q K^T (16 x 64 per warp)
@@ -119,12 +124,12 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
 #pragma unroll
             for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
+        for (int ks = 0; ks < HD / 16; ++ks) {
 #pragma unroll
             for (int np = 0; np < 4; ++np) {
                 uint32_t kf[4];
                 const int mat = lane >> 3, r = lane & 7;
-                ldmatrix_x4(kf, tile_ptr(sK[buf], np * 16 + (mat >> 1) * 8 + r, ks * 2 + (mat & 1)));
+                ldmatrix_x4(kf, tile_ptr<HD>(sK[buf], np * 16 + (mat >> 1) * 8 + r, ks * 2 + (mat & 1)));
                 mma_bf16(s[2 * np], qf[ks], kf[0], kf[1]);
                 mma_bf16(s[2 * np + 1], qf[ks], kf[2], kf[3]);
             }
@@ -158,7 +163,7 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
             row_sum[rr] *= corr[rr];
         }
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
+        for (int nt = 0; nt < HD / 8; ++nt) {
             o[nt][0] *= corr[0];
             o[nt][1] *= corr[0];
             o[nt][2] *= corr[1];
@@ -185,10 +190,10 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
             pa[2] = pack2(s[2 * ks + 1][0], s[2 * ks + 1][1]);
             pa[3] = pack2(s[2 * ks + 1][2], s[2 * ks + 1][3]);
 #pragma unroll
-            for (int dp = 0; dp < 4; ++dp) {
+            for (int dp = 0; dp < HD / 16; ++dp) {
                 uint32_t vf[4];
                 const int mat = lane >> 3, r = lane & 7;
-                ldmatrix_x4_trans(vf, tile_ptr(sV[buf], ks * 16 + (mat & 1) * 8 + r, dp * 2 + (mat >> 1)));
+                ldmatrix_x4_trans(vf, tile_ptr<HD>(sV[buf], ks * 16 + (mat & 1) * 8 + r, dp * 2 + (mat >> 1)));
                 mma_bf16(o[2 * dp], pa, vf[0], vf[1]);
                 mma_bf16(o[2 * dp + 1], pa, vf[2], vf[3]);
             }
@@ -207,21 +212,42 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
     }
     const float inv[2] = {row_sum[0] > 0.f ? 1.f / row_sum[0] : 0.f, row_sum[1] > 0.f ? 1.f / row_sum[1] : 0.f};
 #pragma unroll
-    for (int nt = 0; nt < 8; ++nt) {
+    for (int nt = 0; nt < HD / 8; ++nt) {
         const int r0 = warp * 16 + g;
-        *reinterpret_cast<uint32_t*>(tile_ptr(sQ, r0, nt) + 2 * t) = pack2(o[nt][0] * inv[0], o[nt][1] * inv[0]);
-        *reinterpret_cast<uint32_t*>(tile_ptr(sQ, r0 + 8, nt) + 2 * t) = pack2(o[nt][2] * inv[1], o[nt][3] * inv[1]);
+        *reinterpret_cast<uint32_t*>(tile_ptr<HD>(sQ, r0, nt) + 2 * t) = pack2(o[nt][0] * inv[0], o[nt][1] * inv[0]);
+        *reinterpret_cast<uint32_t*>(tile_ptr<HD>(sQ, r0 + 8, nt) + 2 * t) = pack2(o[nt][2] * inv[1], o[nt][3] * inv[1]);
     }
     __syncwarp();
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
+    for (int i = 0; i < HD / 16; ++i) {
         const int idx = lane + i * 32;
-        const int r = warp * 16 + (idx >> 3), c = idx & 7;
+        const int r = warp * 16 + (idx >> CH_LOG2<HD>), c = idx & ((1 << CH_LOG2<HD>) - 1);
         const int tok = q0 + r;
         if (tok < S) {
-            const uint4 val = *reinterpret_cast<const uint4*>(tile_ptr(sQ, r, c));
+            const uint4 val = *reinterpret_cast<const uint4*>(tile_ptr<HD>(sQ, r, c));
             *reinterpret_cast<uint4*>(out + ((size_t)b * S + tok) * W + h * HD + c * 8) = val;
         }
+    }
+}
+
+template <int HD>
+void launch_hd(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask, const int32_t* kv_len,
+               cudaStream_t stream) {
+    const dim3 grid((S + BQ - 1) / BQ, H, B);
+    const float scale_log2e = head_scale_log2e(HD);
+    switch (mask) {
+        case MASK_NONE:
+            attention_kernel<HD, MASK_NONE><<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e);
+            break;
+        case MASK_CAUSAL:
+            attention_kernel<HD, MASK_CAUSAL><<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e);
+            break;
+        case MASK_KEYLEN:
+            if (!kv_len) fail(B200_ERR_INTERNAL, "attention: kv_len required for key-length masking");
+            attention_kernel<HD, MASK_KEYLEN><<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e);
+            break;
+        default:
+            fail(B200_ERR_INTERNAL, "attention: unknown mask mode %d", mask);
     }
 }
 
@@ -229,23 +255,10 @@ int launch(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, in
            cudaStream_t stream) {
     if (B <= 0 || S <= 0) return 0;
     if (S >= 128) return launch_wgmma(qkv, out, B, S, W, H, mask, kv_len, stream);
-    if (W != H * HD) fail(B200_ERR_UNSUPPORTED, "attention: head_dim must be 64 (width %d, heads %d)", W, H);
-    const dim3 grid((S + BQ - 1) / BQ, H, B);
-    const float scale_log2e = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
-    switch (mask) {
-        case MASK_NONE:
-            attention_kernel<MASK_NONE><<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e);
-            break;
-        case MASK_CAUSAL:
-            attention_kernel<MASK_CAUSAL><<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e);
-            break;
-        case MASK_KEYLEN:
-            if (!kv_len) fail(B200_ERR_INTERNAL, "attention: kv_len required for key-length masking");
-            attention_kernel<MASK_KEYLEN><<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e);
-            break;
-        default:
-            fail(B200_ERR_INTERNAL, "attention: unknown mask mode %d", mask);
-    }
+    if (head_dim(W, H) == 64)
+        launch_hd<64>(qkv, out, B, S, W, H, mask, kv_len, stream);
+    else
+        launch_hd<32>(qkv, out, B, S, W, H, mask, kv_len, stream);
     MB_CUDA(cudaGetLastError());
     return 1;
 }

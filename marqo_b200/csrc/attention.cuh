@@ -1,4 +1,4 @@
-// Multi-head attention over packed QKV (head_dim 64), flash-style online softmax in fp32, one CTA per (64 queries, head,
+// Multi-head attention over packed QKV (head_dim 32 or 64), flash-style online softmax in fp32, one CTA per (64 queries, head,
 // sequence):
 //   S >= 128: wgmma kernel (attention_wgmma.cu) — TMA-fed 128-key K / V tiles, one MMA warpgroup, P from registers.
 //   S <  128: warp-level kernel (attention.cu, mma.sync m16n8k16, 64-key blocks) — a ViT-B-32 (50 tokens) or CLIP text
@@ -11,11 +11,22 @@ namespace attention {
 
 enum Mask { MASK_NONE = 0, MASK_CAUSAL = 1, MASK_KEYLEN = 2 };
 
-// qkv: bf16 [B*S, 3*W] rows = tokens, columns = [q | k | v], head h occupies columns h*64..h*64+63 of each part.
+// qkv: bf16 [B*S, 3*W] rows = tokens, columns = [q | k | v], head h occupies columns h*D..h*D+D-1 of each part, where
+// D = W / H is the head dim, 32 or 64; both kernels take it as the compile-time parameter HD.
 // out: bf16 [B*S, W].  kv_len: int32 [B] valid key count per sequence (MASK_KEYLEN only).
 // Returns the number of kernels launched.
 int launch(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask, const int32_t* kv_len,
            cudaStream_t stream);
+
+// W / H when it is a head dim the kernels are built for (32 or 64); anything else fails with B200_ERR_UNSUPPORTED.
+inline int head_dim(int W, int H) {
+    if (H > 0 && W == H * 64) return 64;
+    if (H > 0 && W == H * 32) return 32;
+    fail(B200_ERR_UNSUPPORTED, "attention: head_dim must be 32 or 64 (width %d, heads %d)", W, H);
+}
+
+// softmax scale 1/sqrt(head_dim), times log2(e): the kernels exponentiate with exp2
+inline float head_scale_log2e(int hd) { return (hd == 64 ? 0.125f : 0.17677669529663687f) * 1.4426950408889634f; }
 
 // wgmma implementation (attention_wgmma.cu); any S, chosen by launch() for S >= 128
 int launch_wgmma(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask, const int32_t* kv_len,

@@ -3,8 +3,10 @@
 //               full / empty pairs), all straight from the packed qkv matrix with the 128-byte swizzle;
 //   warps 0-3   one MMA warpgroup: S = Q K^T with wgmma m64n128k16 (both operands K-major in smem), online softmax in
 //               fp32 on the accumulator registers (log2 domain, quad shuffles for the row maxima), then O += P V with
-//               wgmma m64n64k16 taking P from registers (bf16, the m16n8k16 A fragment the S accumulator layout maps to)
-//               and V as the transposed (MN-major) B operand.
+//               wgmma m64n{HD}k16 taking P from registers (bf16, the m16n8k16 A fragment the S accumulator layout maps
+//               to) and V as the transposed (MN-major) B operand.
+// The head dim HD (32 or 64) is a template parameter.  A Q / K / V row is HD * 2 bytes, so HD = 64 tiles use the 128-byte
+// swizzle and HD = 32 tiles the 64-byte one, in the tensor maps and in the wgmma descriptors alike.
 // Keys past the sequence's length (S, kv_len[b]) and, for MASK_CAUSAL, past the query are masked to -inf; the tiles TMA
 // reads beyond a sequence belong to the next one (or are zero-filled past the matrix) and only ever meet masked scores.
 #include <mutex>
@@ -17,26 +19,51 @@ namespace attention {
 
 namespace {
 
-constexpr int HD = 64;
 constexpr int BQ = 64;
 constexpr int BKV = 128;
 constexpr int KV_STAGES = 2;
 constexpr int THREADS = 160;
-constexpr uint32_t Q_BYTES = BQ * HD * 2;
-constexpr uint32_t KV_TILE_BYTES = BKV * HD * 2;
-constexpr uint32_t STAGE_BYTES = 2 * KV_TILE_BYTES;   // K then V
-constexpr size_t SMEM_BYTES = Q_BYTES + KV_STAGES * STAGE_BYTES + 1024 /*align*/ + 64 /*barriers*/;
+
+template <int HD>
+struct Tiles {
+    static constexpr uint32_t Q_BYTES = BQ * HD * 2;
+    static constexpr uint32_t KV_TILE_BYTES = BKV * HD * 2;
+    static constexpr uint32_t STAGE_BYTES = 2 * KV_TILE_BYTES;   // K then V
+    static constexpr size_t SMEM_BYTES = Q_BYTES + KV_STAGES * STAGE_BYTES + 1024 /*align*/ + 64 /*barriers*/;
+};
+
+// K-major descriptor of a Q / K tile, and MN-major descriptor of a V tile, for the swizzle that goes with HD
+template <int HD>
+__device__ __forceinline__ uint64_t desc_k(uint32_t smem_addr) {
+    if constexpr (HD == 64) return ptx::make_desc_k_sw128(smem_addr);
+    else return ptx::make_desc_k_sw64(smem_addr);
+}
+template <int HD>
+__device__ __forceinline__ uint64_t desc_mn(uint32_t smem_addr) {
+    if constexpr (HD == 64) return ptx::make_desc_mn_sw128(smem_addr, 0);
+    else return ptx::make_desc_mn_sw64(smem_addr, 0);
+}
+
+// O[64 x HD] += P[64 x 16] V[16 x HD]
+template <int HD>
+__device__ __forceinline__ void wgmma_pv(float (&o)[HD / 2], const uint32_t (&a)[4], uint64_t desc_v) {
+    if constexpr (HD == 64) ptx::wgmma_m64n64k16_bf16_rs_tb(o, a, desc_v, 1u);
+    else ptx::wgmma_m64n32k16_bf16_rs_tb(o, a, desc_v, 1u);
+}
 
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
     __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
     return *reinterpret_cast<uint32_t*>(&v);
 }
 
-template <int MASK>
+template <int HD, int MASK>
 __global__ void __launch_bounds__(THREADS)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
                        __nv_bfloat16* __restrict__ out, int S, int W, const int32_t* __restrict__ kv_len,
                        float scale_log2e) {
+    constexpr uint32_t Q_BYTES = Tiles<HD>::Q_BYTES;
+    constexpr uint32_t KV_TILE_BYTES = Tiles<HD>::KV_TILE_BYTES;
+    constexpr uint32_t STAGE_BYTES = Tiles<HD>::STAGE_BYTES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sq = smem;
@@ -101,8 +128,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
         ptx::wgmma_fence();
 #pragma unroll
         for (int k = 0; k < HD / 16; ++k)
-            ptx::wgmma_m64n128k16_bf16(s, ptx::make_desc_k_sw128(q_base + k * 32), ptx::make_desc_k_sw128(k_base + k * 32),
-                                       k != 0 ? 1u : 0u);
+            ptx::wgmma_m64n128k16_bf16(s, desc_k<HD>(q_base + k * 32), desc_k<HD>(k_base + k * 32), k != 0 ? 1u : 0u);
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         // ---- mask, scale (log2 domain), online softmax
@@ -148,11 +174,10 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
             pa[i >> 1][(i & 1) * 2] = pack_bf16(p0, p1);
             pa[i >> 1][(i & 1) * 2 + 1] = pack_bf16(p2, p3);
         }
-        // ---- O += P V (64 x 64, K = 128 keys)
+        // ---- O += P V (64 x HD, K = 128 keys; 16 keys = 16 V rows of HD * 2 bytes per k-step)
         ptx::wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BKV / 16; ++k)
-            ptx::wgmma_m64n64k16_bf16_rs_tb(o, pa[k], ptx::make_desc_mn_sw128(v_base + k * 2048, 0), 1u);
+        for (int k = 0; k < BKV / 16; ++k) wgmma_pv<HD>(o, pa[k], desc_mn<HD>(v_base + k * 32 * HD));
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         __syncwarp();
@@ -175,39 +200,50 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
     }
 }
 
-template <int MASK>
+template <int HD, int MASK>
 void launch_mask(const CUtensorMap& tq, const CUtensorMap& tkv, __nv_bfloat16* out, int B, int S, int W, int H,
                  const int32_t* kv_len, cudaStream_t stream) {
+    constexpr size_t SMEM_BYTES = Tiles<HD>::SMEM_BYTES;
     static std::once_flag once;
     std::call_once(once, [] {
-        MB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel<MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        MB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel<HD, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)SMEM_BYTES));
     });
     const dim3 grid((S + BQ - 1) / BQ, H, B);
-    const float scale_log2e = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
-    attention_wgmma_kernel<MASK><<<grid, THREADS, SMEM_BYTES, stream>>>(tq, tkv, out, S, W, kv_len, scale_log2e);
+    const float scale_log2e = head_scale_log2e(HD);
+    attention_wgmma_kernel<HD, MASK><<<grid, THREADS, SMEM_BYTES, stream>>>(tq, tkv, out, S, W, kv_len, scale_log2e);
+}
+
+template <int HD>
+void launch_hd(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask,
+               const int32_t* kv_len, cudaStream_t stream) {
+    const uint64_t rows = (uint64_t)B * S;
+    const CUtensorMapSwizzle swz = HD == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    const CUtensorMap tq = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows, (uint64_t)3 * W * 2,
+                                        HD, BQ, swz);
+    const CUtensorMap tkv = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows,
+                                         (uint64_t)3 * W * 2, HD, BKV, swz);
+    switch (mask) {
+        case MASK_NONE: launch_mask<HD, MASK_NONE>(tq, tkv, out, B, S, W, H, kv_len, stream); break;
+        case MASK_CAUSAL: launch_mask<HD, MASK_CAUSAL>(tq, tkv, out, B, S, W, H, kv_len, stream); break;
+        case MASK_KEYLEN:
+            if (!kv_len) fail(B200_ERR_INTERNAL, "attention: kv_len required for key-length masking");
+            launch_mask<HD, MASK_KEYLEN>(tq, tkv, out, B, S, W, H, kv_len, stream);
+            break;
+        default: fail(B200_ERR_INTERNAL, "attention: unknown mask mode %d", mask);
+    }
 }
 
 }  // namespace
 
 int launch_wgmma(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask,
                  const int32_t* kv_len, cudaStream_t stream) {
-    if (W != H * HD) fail(B200_ERR_UNSUPPORTED, "attention: head_dim must be 64 (width %d, heads %d)", W, H);
+    const int hd = head_dim(W, H);
     if (B > 65535) fail(B200_ERR_UNSUPPORTED, "attention: batch %d is too large", B);
-    const uint64_t rows = (uint64_t)B * S;
-    const CUtensorMap tq = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows, (uint64_t)3 * W * 2,
-                                        HD, BQ, CU_TENSOR_MAP_SWIZZLE_128B);
-    const CUtensorMap tkv = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows,
-                                         (uint64_t)3 * W * 2, HD, BKV, CU_TENSOR_MAP_SWIZZLE_128B);
-    switch (mask) {
-        case MASK_NONE: launch_mask<MASK_NONE>(tq, tkv, out, B, S, W, H, kv_len, stream); break;
-        case MASK_CAUSAL: launch_mask<MASK_CAUSAL>(tq, tkv, out, B, S, W, H, kv_len, stream); break;
-        case MASK_KEYLEN:
-            if (!kv_len) fail(B200_ERR_INTERNAL, "attention: kv_len required for key-length masking");
-            launch_mask<MASK_KEYLEN>(tq, tkv, out, B, S, W, H, kv_len, stream);
-            break;
-        default: fail(B200_ERR_INTERNAL, "attention: unknown mask mode %d", mask);
-    }
+    if (hd == 64)
+        launch_hd<64>(qkv, out, B, S, W, H, mask, kv_len, stream);
+    else
+        launch_hd<32>(qkv, out, B, S, W, H, mask, kv_len, stream);
     MB_CUDA(cudaGetLastError());
     return 1;
 }

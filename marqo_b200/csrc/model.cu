@@ -145,8 +145,8 @@ void check_tower(const b200_tower_desc& t, const char* name) {
     MB_CHECK_ARG(t.width > 0 && t.width % 128 == 0 && t.width <= 1024, "%s.width %d must be a multiple of 128, <= 1024",
                  name, t.width);
     MB_CHECK_ARG(t.layers > 0, "%s.layers must be positive", name);
-    MB_CHECK_ARG(t.heads > 0 && t.width == t.heads * 64, "%s: head_dim must be 64 (width %d, heads %d)", name, t.width,
-                 t.heads);
+    MB_CHECK_ARG(t.heads > 0 && (t.width == t.heads * 32 || t.width == t.heads * 64),
+                 "%s: head_dim must be 32 or 64 (width %d, heads %d)", name, t.width, t.heads);
     MB_CHECK_ARG(t.mlp > 0 && t.mlp % 64 == 0, "%s.mlp %d must be a multiple of 64", name, t.mlp);
 }
 

@@ -142,6 +142,30 @@ __device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr, uint3
     return d;
 }
 
+// K-major operand, 64-byte swizzle: rows are 64 B (32 x 16-bit) apart inside an 8-row / 512 B swizzle atom, atoms
+// SBO = 512 B apart; layout = 2 (SWIZZLE_64B).  The tile base must be 512-byte aligned; advancing K by 16 elements =
+// +32 B on the start address (two k-steps per 32-element row).
+__device__ __forceinline__ uint64_t make_desc_k_sw64(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+    d |= static_cast<uint64_t>(1) << 16;
+    d |= static_cast<uint64_t>(512 >> 4) << 32;
+    d |= static_cast<uint64_t>(2) << 62;
+    return d;
+}
+
+// MN-major operand, 64-byte swizzle: rows of 32 contiguous MN elements (64 B), one row per K index, 8 K rows form a
+// 512 B swizzle atom; SBO = 512 B between successive 8-K groups, LBO = byte stride between 32-element MN blocks (unused
+// when N = 32).  Advancing K by 16 = +1024 B on the start address.
+__device__ __forceinline__ uint64_t make_desc_mn_sw64(uint32_t smem_addr, uint32_t lbo_bytes) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
+    d |= static_cast<uint64_t>(512 >> 4) << 32;
+    d |= static_cast<uint64_t>(2) << 62;
+    return d;
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -215,6 +239,22 @@ __device__ __forceinline__ void wgmma_m64n64k16_bf16_rs_tb(float (&d)[32], const
           "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
           "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
           "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
+}
+// D[64 x 32] (+)= A[64 x 16] * B[16 x 32], A in registers as above, B MN-major in shared memory (descriptor from
+// make_desc_mn_sw64), fp32 accumulators in the layout above.
+__device__ __forceinline__ void wgmma_m64n32k16_bf16_rs_tb(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %21, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, {%16, %17, %18, %19}, %20, p, 1, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
 }
 // named barrier among COUNT threads (COUNT % 32 == 0); id 0 is __syncthreads().  The id must be an immediate: with a

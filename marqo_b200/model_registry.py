@@ -1,10 +1,20 @@
 """Model name -> properties + architecture for the models the engine serves.
 
-Property dicts (`name`, `dimensions`, `type`, `tokens`, prefixes) are the reference's registry entries
-(src/marqo/s2_inference/model_registry.py:142-231 for open_clip/*, :771-788 for hf/e5-*); `type` is rewritten to the
-engine's loader types ("b200_open_clip" / "b200_hf") so that both engines can be registered side by side in
-MODEL_PROPERTIES['loaders'] (model_registry.py:2133-2145).  The `arch` blocks are the shapes that live in
-open_clip 2.24.0 `model_configs/*.json` and the HF `config.json` files (SURVEY.md §8)."""
+Property dicts (`name`, `dimensions`, `type`, `tokens`, `model_size`, prefixes, `poolingMethod`, `notes`) are the
+reference's registry entries (src/marqo/s2_inference/model_registry.py:142-231 for open_clip/*, :616-851 for hf/*);
+`type` is rewritten to the engine's loader types ("b200_open_clip" / "b200_hf") so that both engines can be registered
+side by side in MODEL_PROPERTIES['loaders'] (model_registry.py:2133-2145).  The `arch` blocks are the shapes that live
+in open_clip 2.24.0 `model_configs/*.json` and the HF `config.json` files (SURVEY.md §8).
+
+The hf/* shapes come from the upstream HF `config.json` files, which cannot be re-read offline (like the ViT shapes of
+SURVEY.md §8).  All are uncased-WordPiece BERTs (vocabulary 30522, 512 positions, 2 token types, erf-GELU, mlp = 4 x
+width), mean-pooled:
+    MiniLM-L6  (all-MiniLM-L6-v1/v2, all_datasets_v3/v4_MiniLM-L6)                 width  384, 6 layers, 12 heads
+    MiniLM-L12 (all_datasets_v3/v4_MiniLM-L12)                                      width  384, 12 layers, 12 heads
+    e5-small, e5-small-v2, e5-small-unsupervised, bge-small-en-v1.5                width  384, 12 layers, 12 heads
+    e5-base, e5-base-v2, e5-base-unsupervised, bge-base-en-v1.5                    width  768, 12 layers, 12 heads
+    e5-large, e5-large-v2, e5-large-unsupervised, bge-large-en-v1.5                width 1024, 24 layers, 16 heads
+The 384-wide models have head_dim 32, the others head_dim 64."""
 from __future__ import annotations
 
 import copy
@@ -35,6 +45,21 @@ _VIT_B_16 = dict(embed=512, vw=768, vl=12, vh=12, patch=16, tw=512, tl=12, th=8)
 _VIT_L_14 = dict(embed=768, vw=1024, vl=24, vh=16, patch=14, tw=768, tl=12, th=12)
 
 
+# (width, layers, heads) of the hf/* BERTs (module docstring)
+_MINILM_L6 = (384, 6, 12)
+_MINILM_L12 = (384, 12, 12)
+_BERT_SMALL = (384, 12, 12)
+_BERT_BASE = (768, 12, 12)
+_BERT_LARGE = (1024, 24, 16)
+_BGE_QUERY_PREFIX = "Represent this sentence for searching relevant passages: "
+
+
+def _hf(name: str, tokens: int, shape: tuple, **props) -> dict:
+    """A reference hf/* entry (`dimensions` = width: every one of them mean-pools the last hidden state) + its arch."""
+    return {"name": name, "dimensions": shape[0], "tokens": tokens, "type": TYPE_HF, **props, "notes": "",
+            "arch": _bert_arch(*shape)}
+
+
 def _open_clip(name: str, dims: int, pretrained: str, shape: dict, act: str) -> dict:
     return {"name": name, "dimensions": dims, "note": "open_clip models", "type": TYPE_OPEN_CLIP,
             "pretrained": pretrained, "arch": _clip_arch(**shape, act=act)}
@@ -56,14 +81,31 @@ def _models() -> Dict[str, dict]:
     # (verify) upstream uses 0.5/0.5 image statistics for this tag (SURVEY.md Appendix B)
     m["open_clip/ViT-L-14/laion2b_s32b_b82k"]["arch"]["mean"] = (0.5, 0.5, 0.5)
     m["open_clip/ViT-L-14/laion2b_s32b_b82k"]["arch"]["std"] = (0.5, 0.5, 0.5)
-    for short, repo, w, layers, heads, size in (("e5-small-v2", "intfloat/e5-small-v2", 384, 12, 6, 0.134),
-                                                ("e5-base-v2", "intfloat/e5-base-v2", 768, 12, 12, 0.438),
-                                                ("e5-large-v2", "intfloat/e5-large-v2", 1024, 24, 16, 1.34),
-                                                ("e5-base", "intfloat/e5-base", 768, 12, 12, 0.438),
-                                                ("e5-large", "intfloat/e5-large", 1024, 24, 16, 1.34)):
-        m[f"hf/{short}"] = {"name": repo, "dimensions": w, "tokens": 512, "type": TYPE_HF, "model_size": size,
-                            "text_query_prefix": "query: ", "text_chunk_prefix": "passage: ", "notes": "",
-                            "arch": _bert_arch(w, layers, heads)}
+    for short, repo, tokens, shape in (("all-MiniLM-L6-v1", "sentence-transformers/all-MiniLM-L6-v1", 128, _MINILM_L6),
+                                       ("all-MiniLM-L6-v2", "sentence-transformers/all-MiniLM-L6-v2", 256, _MINILM_L6),
+                                       ("all_datasets_v3_MiniLM-L12", "flax-sentence-embeddings/all_datasets_v3_MiniLM-L12",
+                                        128, _MINILM_L12),
+                                       ("all_datasets_v3_MiniLM-L6", "flax-sentence-embeddings/all_datasets_v3_MiniLM-L6",
+                                        128, _MINILM_L6),
+                                       ("all_datasets_v4_MiniLM-L12", "flax-sentence-embeddings/all_datasets_v4_MiniLM-L12",
+                                        128, _MINILM_L12),
+                                       ("all_datasets_v4_MiniLM-L6", "flax-sentence-embeddings/all_datasets_v4_MiniLM-L6",
+                                        128, _MINILM_L6)):
+        m[f"hf/{short}"] = _hf(repo, tokens, shape)
+    for short, tokens, size, shape in (("e5-small", 192, 0.1342, _BERT_SMALL),
+                                       ("e5-base", 192, 0.438, _BERT_BASE),
+                                       ("e5-large", 192, 1.3, _BERT_LARGE),
+                                       ("e5-large-unsupervised", 128, 1.3, _BERT_LARGE),
+                                       ("e5-base-unsupervised", 128, 0.438, _BERT_BASE),
+                                       ("e5-small-unsupervised", 128, 0.134, _BERT_SMALL),
+                                       ("e5-small-v2", 512, 0.134, _BERT_SMALL),
+                                       ("e5-base-v2", 512, 0.438, _BERT_BASE),
+                                       ("e5-large-v2", 512, 1.34, _BERT_LARGE)):
+        m[f"hf/{short}"] = _hf(f"intfloat/{short}", tokens, shape, model_size=size, text_query_prefix="query: ",
+                               text_chunk_prefix="passage: ")
+    for size, shape in (("small", _BERT_SMALL), ("base", _BERT_BASE), ("large", _BERT_LARGE)):
+        m[f"hf/bge-{size}-en-v1.5"] = _hf(f"BAAI/bge-{size}-en-v1.5", 512, shape, text_query_prefix=_BGE_QUERY_PREFIX,
+                                          poolingMethod="mean")
     return m
 
 

@@ -14,5 +14,5 @@ lib = N.load()
 for B, S, W, H, mask in cases:
     ms = C.c_float(0)
     N.check(lib.b200_debug_attention_time(0, B, S, W, H, mask, iters, C.byref(ms)))
-    flops = 4.0 * B * H * S * S * 64
+    flops = 4.0 * B * H * S * S * (W // H)
     print(json.dumps({"B": B, "S": S, "W": W, "H": H, "mask": mask, "us": ms.value * 1e3, "TFLOPs": flops / ms.value / 1e9}))
