@@ -412,6 +412,10 @@ int b200_debug_jpeg_decode_host(const uint8_t* file, size_t nbytes, uint8_t* out
                                 int32_t* out_height, int32_t* out_width);
 /* Pillow-compatible bicubic resize (shortest side -> S) + centre crop of uint8 HWC images [n,h,w,3] -> [n,S,S,3]. */
 int b200_debug_resize(int device, const uint8_t* hwc, int n, int h, int w, int S, uint8_t* out);
+/* Bytes of device memory the library holds right now, over all devices and handles of this process (indexes,
+ * exchanges, models and the scratch of calls in flight).  Memory from b200_host_alloc is not counted.  Returns to its
+ * earlier value once every handle created in between is destroyed: a leak check. */
+int b200_debug_device_bytes(int64_t* out_live_bytes);
 
 #ifdef __cplusplus
 }

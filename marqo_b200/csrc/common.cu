@@ -1,4 +1,5 @@
 #include <algorithm>
+#include <atomic>
 #include <vector>
 
 #include "common.cuh"
@@ -8,8 +9,65 @@
 namespace mb {
 
 static thread_local std::string g_last_error;
+static std::atomic<int64_t> g_device_bytes{0};
 
 void set_last_error(const std::string& msg) { g_last_error = msg; }
+
+void require_sm90_device(int device) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+        cudaGetLastError();
+        fail(B200_ERR_NO_DEVICE, "no CUDA device available (marqo_b200 has no CPU fallback)");
+    }
+    MB_CHECK_ARG(device >= 0 && device < ndev, "device %d out of range (%d devices)", device, ndev);
+    int major = 0;
+    MB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
+    if (major != 9) fail(B200_ERR_NO_DEVICE, "device %d has compute capability %d.x; sm_90 required", device, major);
+}
+
+void* device_alloc(size_t bytes, cudaStream_t stream, bool stream_ordered) {
+    void* p = nullptr;
+    const cudaError_t e = stream_ordered ? cudaMallocAsync(&p, bytes, stream) : cudaMalloc(&p, bytes);
+    if (e == cudaErrorMemoryAllocation) {
+        cudaGetLastError();
+        fail(B200_ERR_OOM, "cudaMalloc(%zu bytes) failed: out of device memory", bytes);
+    }
+    if (e != cudaSuccess)
+        fail(B200_ERR_CUDA, "%s(%zu bytes) failed: %s", stream_ordered ? "cudaMallocAsync" : "cudaMalloc", bytes,
+             cudaGetErrorString(e));
+    g_device_bytes += (int64_t)bytes;
+    return p;
+}
+
+void device_free(void* p, size_t bytes, cudaStream_t stream, bool stream_ordered) noexcept {
+    if (stream_ordered) cudaFreeAsync(p, stream);
+    else cudaFree(p);
+    g_device_bytes -= (int64_t)bytes;
+}
+
+UniqueStream make_stream(unsigned flags) {
+    cudaStream_t s = nullptr;
+    MB_CUDA(cudaStreamCreateWithFlags(&s, flags));
+    return UniqueStream(s);
+}
+
+UniqueEvent make_event() {
+    cudaEvent_t e = nullptr;
+    MB_CUDA(cudaEventCreate(&e));
+    return UniqueEvent(e);
+}
+
+void* pinned_alloc(size_t bytes) {
+    void* p = nullptr;
+    MB_CUDA(cudaHostAlloc(&p, bytes, cudaHostAllocPortable));
+    return p;
+}
+
+IpcMapping open_ipc_mapping(const cudaIpcMemHandle_t& h) {
+    void* p = nullptr;
+    MB_CUDA(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
+    return IpcMapping(static_cast<uint8_t*>(p));
+}
 
 using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -103,6 +161,13 @@ int b200_host_alloc(size_t bytes, void** out) {
 int b200_host_free(void* p) {
     return mb::guarded([&] {
         if (p) MB_CUDA(cudaFreeHost(p));
+    });
+}
+
+int b200_debug_device_bytes(int64_t* out_live_bytes) {
+    return mb::guarded([&] {
+        MB_CHECK_ARG(out_live_bytes != nullptr, "out_live_bytes is NULL");
+        *out_live_bytes = mb::g_device_bytes.load();
     });
 }
 

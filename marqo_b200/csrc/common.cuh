@@ -1,5 +1,6 @@
 // Host-side helpers shared by every translation unit of libmarqo_b200.so:
-// status codes, thread-local error text, CUDA error checks, TMA tensor-map encoding.
+// status codes, thread-local error text, CUDA error checks, owners of device memory and CUDA handles,
+// TMA tensor-map encoding.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -9,8 +10,11 @@
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
+#include <memory>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
+#include <utility>
 
 #include "../../include/marqo_b200.h"
 
@@ -70,6 +74,82 @@ struct DeviceGuard {
         if (prev >= 0) cudaSetDevice(prev);
     }
 };
+
+// Raises B200_ERR_NO_DEVICE / B200_ERR_INVALID_ARG unless `device` is an sm_90 device of this process.
+void require_sm90_device(int device);
+
+// ---------------------------------------------------------------------------------------------------- ownership
+// Every device allocation of the library goes through device_alloc / device_free: out of memory is reported as
+// B200_ERR_OOM, and the process-wide count of live bytes (b200_debug_device_bytes) stays exact.  `stream_ordered`
+// selects cudaMallocAsync / cudaFreeAsync on `stream`.
+void* device_alloc(size_t bytes, cudaStream_t stream, bool stream_ordered);
+void device_free(void* p, size_t bytes, cudaStream_t stream, bool stream_ordered) noexcept;
+
+// Move-only owner of a device array of size() elements.  Default-constructed, moved-from and zero-sized buffers are
+// empty (null).
+template <class T>
+class DeviceBuffer {
+  public:
+    DeviceBuffer() = default;
+    explicit DeviceBuffer(size_t n) : p_(static_cast<T*>(device_alloc(n * sizeof(T), nullptr, false))), n_(n) {}
+    // stream-ordered: allocated and released on `s`
+    DeviceBuffer(size_t n, cudaStream_t s)
+        : p_(static_cast<T*>(device_alloc(n * sizeof(T), s, true))), n_(n), stream_(s), stream_ordered_(true) {}
+    DeviceBuffer(DeviceBuffer&& o) noexcept { swap(o); }
+    DeviceBuffer& operator=(DeviceBuffer&& o) noexcept {
+        DeviceBuffer(std::move(o)).swap(*this);
+        return *this;
+    }
+    ~DeviceBuffer() {
+        if (p_) device_free(p_, n_ * sizeof(T), stream_, stream_ordered_);
+    }
+    T* get() const { return p_; }
+    size_t size() const { return n_; }
+    explicit operator bool() const { return p_ != nullptr; }
+    void swap(DeviceBuffer& o) noexcept {
+        std::swap(p_, o.p_);
+        std::swap(n_, o.n_);
+        std::swap(stream_, o.stream_);
+        std::swap(stream_ordered_, o.stream_ordered_);
+    }
+
+  private:
+    T* p_ = nullptr;
+    size_t n_ = 0;
+    cudaStream_t stream_ = nullptr;
+    bool stream_ordered_ = false;
+};
+
+struct StreamDeleter {
+    void operator()(cudaStream_t s) const { cudaStreamDestroy(s); }
+};
+struct EventDeleter {
+    void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
+};
+struct GraphExecDeleter {
+    void operator()(cudaGraphExec_t g) const { cudaGraphExecDestroy(g); }
+};
+struct PinnedDeleter {
+    void operator()(void* p) const { cudaFreeHost(p); }
+};
+struct IpcDeleter {
+    void operator()(void* p) const { cudaIpcCloseMemHandle(p); }
+};
+using UniqueStream = std::unique_ptr<std::remove_pointer_t<cudaStream_t>, StreamDeleter>;
+using UniqueEvent = std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, EventDeleter>;
+using UniqueGraphExec = std::unique_ptr<std::remove_pointer_t<cudaGraphExec_t>, GraphExecDeleter>;
+template <class T>
+using PinnedPtr = std::unique_ptr<T, PinnedDeleter>;
+using IpcMapping = std::unique_ptr<uint8_t, IpcDeleter>;   // another process's device buffer mapped here
+
+UniqueStream make_stream(unsigned flags);
+UniqueEvent make_event();
+void* pinned_alloc(size_t bytes);   // portable page-locked host memory
+template <class T>
+PinnedPtr<T> make_pinned() {
+    return PinnedPtr<T>(static_cast<T*>(pinned_alloc(sizeof(T))));
+}
+IpcMapping open_ipc_mapping(const cudaIpcMemHandle_t& h);
 
 // 2D row-major tensor map: inner dim `cols` (contiguous), outer dim `rows`, row pitch in bytes.
 // box = {box_cols, box_rows}; swizzle 128B requires box_cols * elem_size == 128.

@@ -10,19 +10,14 @@ using namespace mb;
 
 namespace {
 
-struct Scratch {
-    std::vector<void*> ptrs;
-    cudaStream_t s = nullptr;
-    ~Scratch() {
-        for (void* p : ptrs) cudaFree(p);
-        if (s) cudaStreamDestroy(s);
-    }
+struct Scratch {   // a stream and the device buffers of one call
+    UniqueStream stream = make_stream(cudaStreamDefault);
+    cudaStream_t s = stream.get();
+    std::vector<DeviceBuffer<uint8_t>> bufs;
     template <class T>
     T* alloc(size_t n) {
-        void* p = nullptr;
-        MB_CUDA(cudaMalloc(&p, std::max<size_t>(n * sizeof(T), 16)));
-        ptrs.push_back(p);
-        return reinterpret_cast<T*>(p);
+        bufs.emplace_back(std::max<size_t>(n * sizeof(T), 16));
+        return reinterpret_cast<T*>(bufs.back().get());
     }
     template <class T>
     T* upload(const T* h, size_t n) {
@@ -74,7 +69,6 @@ int b200_debug_patch_embed(int device, const uint8_t* hwc, int n, int S, int pat
         require_device(device);
         DeviceGuard g(device);
         Scratch sc;
-        MB_CUDA(cudaStreamCreate(&sc.s));
         const int G = (S / patch) * (S / patch), K = 3 * patch * patch;
         uint8_t* dImg = sc.upload(hwc, (size_t)n * S * S * 3);
         float* dW = sc.upload(conv_w, (size_t)N * K);
@@ -125,7 +119,6 @@ int b200_debug_gemm_ln(int device, const float* A, const float* W, const float* 
         require_device(device);
         DeviceGuard g(device);
         Scratch sc;
-        MB_CUDA(cudaStreamCreate(&sc.s));
         __nv_bfloat16* dA = sc.upload_bf16(A, (size_t)M * K);
         __nv_bfloat16* dW = sc.upload_bf16(W, (size_t)N * K);
         float* dOut = sc.alloc<float>((size_t)M * N);
@@ -163,7 +156,6 @@ int b200_debug_gemm(int device, const float* A, const float* W, const float* bia
         require_device(device);
         DeviceGuard g(device);
         Scratch sc;
-        MB_CUDA(cudaStreamCreate(&sc.s));
         __nv_bfloat16* dA = sc.upload_bf16(A, (size_t)M * K);
         __nv_bfloat16* dW = sc.upload_bf16(W, (size_t)N * K);
         float* dOut = sc.alloc<float>((size_t)M * N);
@@ -201,7 +193,6 @@ int b200_debug_attention(int device, const float* qkv, int B, int S, int W, int 
         require_device(device);
         DeviceGuard g(device);
         Scratch sc;
-        MB_CUDA(cudaStreamCreate(&sc.s));
         const size_t M = (size_t)B * S;
         __nv_bfloat16* dq = sc.upload_bf16(qkv, M * 3 * W);
         __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>(M * W);
@@ -223,7 +214,6 @@ int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, 
         require_device(device);
         DeviceGuard g(device);
         Scratch sc;
-        MB_CUDA(cudaStreamCreate(&sc.s));
         const size_t M = (size_t)B * S;
         __nv_bfloat16* dq = sc.alloc<__nv_bfloat16>(M * 3 * W);
         __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>(M * W);
@@ -232,18 +222,14 @@ int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, 
         MB_CUDA(cudaGetLastError());
         std::vector<int32_t> lens((size_t)B, S);
         const int32_t* dlen = mask == attention::MASK_KEYLEN ? sc.upload(lens.data(), (size_t)B) : nullptr;
-        cudaEvent_t e0, e1;
-        MB_CUDA(cudaEventCreate(&e0));
-        MB_CUDA(cudaEventCreate(&e1));
+        UniqueEvent e0 = make_event(), e1 = make_event();
         for (int i = 0; i < 3; ++i) attention::launch(dq, dO, B, S, W, H, mask, dlen, sc.s);   // warm-up
-        MB_CUDA(cudaEventRecord(e0, sc.s));
+        MB_CUDA(cudaEventRecord(e0.get(), sc.s));
         for (int i = 0; i < iters; ++i) attention::launch(dq, dO, B, S, W, H, mask, dlen, sc.s);
-        MB_CUDA(cudaEventRecord(e1, sc.s));
+        MB_CUDA(cudaEventRecord(e1.get(), sc.s));
         MB_CUDA(cudaStreamSynchronize(sc.s));
         float ms = 0.f;
-        MB_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-        cudaEventDestroy(e0);
-        cudaEventDestroy(e1);
+        MB_CUDA(cudaEventElapsedTime(&ms, e0.get(), e1.get()));
         *out_ms = ms / (float)iters;
     });
 }
@@ -255,7 +241,6 @@ int b200_debug_layernorm(int device, const float* x, const float* gamma, const f
         require_device(device);
         DeviceGuard g(device);
         Scratch sc;
-        MB_CUDA(cudaStreamCreate(&sc.s));
         float* dx = sc.upload(x, (size_t)rows * w);
         float* dg = sc.upload(gamma, (size_t)w);
         float* db = sc.upload(beta, (size_t)w);
@@ -273,7 +258,6 @@ int b200_debug_resize(int device, const uint8_t* hwc, int n, int h, int w, int S
         require_device(device);
         DeviceGuard g(device);
         Scratch sc;
-        MB_CUDA(cudaStreamCreate(&sc.s));
         uint8_t* din = sc.upload(hwc, (size_t)n * h * w * 3);
         uint8_t* dout = sc.alloc<uint8_t>((size_t)n * S * S * 3);
         kernels::resize_crop_u8(din, n, h, w, S, dout, sc.s);

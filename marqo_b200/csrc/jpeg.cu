@@ -648,37 +648,25 @@ int b200_jpeg_decode_batch(int device, const uint8_t* const* files, const size_t
         std::vector<ImageDesc> descs;
         long long total_blocks, total_pixels, plane_bytes;
         layout_batch(imgs, ok, descs, total_blocks, total_pixels, plane_bytes);
-        void *d_desc = nullptr, *d_coef = nullptr, *d_planes = nullptr;
-        cudaStream_t stream = nullptr;
-        try {
-            MB_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-            MB_CUDA(cudaMalloc(&d_desc, descs.size() * sizeof(ImageDesc)));
-            MB_CUDA(cudaMalloc(&d_coef, (size_t)total_blocks * 64 * sizeof(int16_t)));
-            MB_CUDA(cudaMalloc(&d_planes, (size_t)plane_bytes));
-            MB_CUDA(cudaMemcpyAsync(d_desc, descs.data(), descs.size() * sizeof(ImageDesc), cudaMemcpyHostToDevice, stream));
-            for (size_t k = 0; k < ok.size(); ++k) {
-                const Parsed& p = imgs[ok[k]];
-                MB_CUDA(cudaMemcpyAsync((int16_t*)d_coef + (size_t)descs[k].block_base * 64, p.coefs.data(),
-                                        p.coefs.size() * sizeof(int16_t), cudaMemcpyHostToDevice, stream));
-            }
-            idct_kernel<<<(unsigned)((total_blocks + 127) / 128), 128, 0, stream>>>(
-                (const ImageDesc*)d_desc, (int)descs.size(), (const int16_t*)d_coef, (uint8_t*)d_planes, total_blocks);
-            MB_CUDA(cudaGetLastError());
-            upsample_rgb_kernel<<<(unsigned)((total_pixels + 255) / 256), 256, 0, stream>>>(
-                (const ImageDesc*)d_desc, (int)descs.size(), (const uint8_t*)d_planes, total_pixels);
-            MB_CUDA(cudaGetLastError());
-            MB_CUDA(cudaStreamSynchronize(stream));
-        } catch (...) {
-            cudaFree(d_desc);
-            cudaFree(d_coef);
-            cudaFree(d_planes);
-            if (stream) cudaStreamDestroy(stream);
-            throw;
+        UniqueStream owned_stream = make_stream(cudaStreamNonBlocking);
+        cudaStream_t stream = owned_stream.get();
+        DeviceBuffer<ImageDesc> d_desc(descs.size());
+        DeviceBuffer<int16_t> d_coef((size_t)total_blocks * 64);
+        DeviceBuffer<uint8_t> d_planes((size_t)plane_bytes);
+        MB_CUDA(cudaMemcpyAsync(d_desc.get(), descs.data(), descs.size() * sizeof(ImageDesc), cudaMemcpyHostToDevice,
+                                stream));
+        for (size_t k = 0; k < ok.size(); ++k) {
+            const Parsed& p = imgs[ok[k]];
+            MB_CUDA(cudaMemcpyAsync(d_coef.get() + (size_t)descs[k].block_base * 64, p.coefs.data(),
+                                    p.coefs.size() * sizeof(int16_t), cudaMemcpyHostToDevice, stream));
         }
-        cudaFree(d_desc);
-        cudaFree(d_coef);
-        cudaFree(d_planes);
-        cudaStreamDestroy(stream);
+        idct_kernel<<<(unsigned)((total_blocks + 127) / 128), 128, 0, stream>>>(
+            d_desc.get(), (int)descs.size(), d_coef.get(), d_planes.get(), total_blocks);
+        MB_CUDA(cudaGetLastError());
+        upsample_rgb_kernel<<<(unsigned)((total_pixels + 255) / 256), 256, 0, stream>>>(
+            d_desc.get(), (int)descs.size(), d_planes.get(), total_pixels);
+        MB_CUDA(cudaGetLastError());
+        MB_CUDA(cudaStreamSynchronize(stream));
     });
 }
 

@@ -573,29 +573,24 @@ void resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst
     const int top = py_round_half_even((new_h - S) / 2.0);
     const ResampleTable th = precompute(w, new_w);
     const ResampleTable tv = precompute(h, new_h);
-    int *d_hb = nullptr, *d_hc = nullptr, *d_vb = nullptr, *d_vc = nullptr;
-    uint8_t* tmp = nullptr;
-    auto up = [&](const std::vector<int>& v, int** d) {
-        MB_CUDA(cudaMallocAsync((void**)d, v.size() * sizeof(int), s));
-        MB_CUDA(cudaMemcpyAsync(*d, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-    };
-    up(th.bounds, &d_hb);
-    up(th.coeffs, &d_hc);
-    up(tv.bounds, &d_vb);
-    up(tv.coeffs, &d_vc);
-    MB_CUDA(cudaMallocAsync((void**)&tmp, (size_t)n * h * S * 3, s));
+    {   // stream-ordered temporaries, released on `s` at the end of this block
+        auto up = [&](const std::vector<int>& v) {
+            DeviceBuffer<int> d(v.size(), s);
+            MB_CUDA(cudaMemcpyAsync(d.get(), v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+            return d;
+        };
+        const DeviceBuffer<int> d_hb = up(th.bounds), d_hc = up(th.coeffs), d_vb = up(tv.bounds), d_vc = up(tv.coeffs);
+        const DeviceBuffer<uint8_t> tmp((size_t)n * h * S * 3, s);
+        const long long nh = (long long)n * h * S;
+        resample_h_kernel<<<(unsigned)((nh + 255) / 256), 256, 0, s>>>(src, n, h, w, S, left, d_hb.get(), d_hc.get(),
+                                                                       th.ksize, tmp.get());
+        MB_CUDA(cudaGetLastError());
+        const long long nv = (long long)n * S * S;
+        resample_v_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, s>>>(tmp.get(), n, h, S, top, d_vb.get(), d_vc.get(),
+                                                                       tv.ksize, dst);
+        MB_CUDA(cudaGetLastError());
+    }
     // the pageable host vectors above must outlive the async copies: synchronise before they go out of scope
-    const long long nh = (long long)n * h * S;
-    resample_h_kernel<<<(unsigned)((nh + 255) / 256), 256, 0, s>>>(src, n, h, w, S, left, d_hb, d_hc, th.ksize, tmp);
-    MB_CUDA(cudaGetLastError());
-    const long long nv = (long long)n * S * S;
-    resample_v_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, s>>>(tmp, n, h, S, top, d_vb, d_vc, tv.ksize, dst);
-    MB_CUDA(cudaGetLastError());
-    MB_CUDA(cudaFreeAsync(d_hb, s));
-    MB_CUDA(cudaFreeAsync(d_hc, s));
-    MB_CUDA(cudaFreeAsync(d_vb, s));
-    MB_CUDA(cudaFreeAsync(d_vc, s));
-    MB_CUDA(cudaFreeAsync(tmp, s));
     MB_CUDA(cudaStreamSynchronize(s));
 }
 

@@ -31,11 +31,6 @@ using namespace mb;
 
 namespace {
 
-struct Buf {
-    void* p = nullptr;
-    size_t bytes = 0;
-};
-
 struct LayerW {
     const float *ln1_w = nullptr, *ln1_b = nullptr, *ln2_w = nullptr, *ln2_b = nullptr;
     const float *b_qkv = nullptr, *b_o = nullptr, *b_fc = nullptr, *b_proj = nullptr;
@@ -65,27 +60,26 @@ struct b200_model {
     int sms = 0;
     b200_model_desc desc{};
     bool finalized = false;
-    std::map<std::string, Buf> raw;   // uploaded fp32 parameters by checkpoint name
-    std::vector<void*> owned;         // derived device buffers
+    std::map<std::string, DeviceBuffer<float>> raw;   // uploaded fp32 parameters by checkpoint name
+    std::vector<DeviceBuffer<uint8_t>> derived;        // device buffers built from them by b200_model_finalize
     TowerW vision, text;
     // workspaces (sized for max_tokens tokens)
     long long max_tokens = 0;
-    float* x = nullptr;
-    __nv_bfloat16 *h = nullptr, *qkv = nullptr, *o = nullptr, *u = nullptr, *patches = nullptr;
-    int32_t *aux = nullptr;           // [max_batch] eot index / kv_len
-    float* out_dev = nullptr;         // [max_batch, embed]
-    float* pooled = nullptr;          // [max_batch, width] LayerNorm-ed pooled rows (CLIP heads)
-    void* in_dev = nullptr;           // staging for host inputs
-    size_t in_dev_bytes = 0;
-    uint8_t* resized = nullptr;       // [max_batch, S, S, 3]
+    DeviceBuffer<float> x;
+    DeviceBuffer<__nv_bfloat16> h, qkv, o, u, patches;
+    DeviceBuffer<int32_t> aux;        // [max_batch] eot index / kv_len
+    DeviceBuffer<float> out_dev;      // [max_batch, embed]
+    DeviceBuffer<float> pooled;       // [max_batch, width] LayerNorm-ed pooled rows (CLIP heads)
+    DeviceBuffer<uint8_t> in_dev;     // staging for host inputs
+    DeviceBuffer<uint8_t> resized;    // [max_batch, S, S, 3]
     cudaStream_t stream = nullptr;
-    cudaStream_t own_stream = nullptr;  // created by the handle; `stream` may be replaced by a caller's stream
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    UniqueStream own_stream;          // created by the handle; `stream` may be replaced by a caller's stream
+    UniqueEvent ev0, ev1;
     bool timing_valid = false;
     int last_launches = 0;
     // optional per-kernel-class device timing (bench.py's roofline numerator)
     bool profiling = false;
-    std::vector<cudaEvent_t> prof_ev;  // pairs
+    std::vector<UniqueEvent> prof_ev;  // pairs
     std::vector<int> prof_cls;         // 0 = gemm, 1 = attention
     int prof_n = 0;
     // CUDA graphs of small (launch-bound) forward passes, keyed by everything the captured launches depend on
@@ -97,7 +91,7 @@ struct b200_model {
         }
     };
     struct GraphEntry {
-        cudaGraphExec_t exec = nullptr;   // null: seen once (ran eagerly), captured on the next use
+        UniqueGraphExec exec;   // null: seen once (ran eagerly), captured on the next use
         int launches = 0;
     };
     std::map<GraphKey, GraphEntry> graphs;
@@ -107,38 +101,11 @@ struct b200_model {
 
 namespace {
 
-void dev_alloc(void** p, size_t bytes) {
-    cudaError_t e = cudaMalloc(p, std::max<size_t>(bytes, 16));
-    if (e == cudaErrorMemoryAllocation) {
-        cudaGetLastError();
-        fail(B200_ERR_OOM, "cudaMalloc(%zu bytes) failed: out of device memory", bytes);
-    }
-    MB_CUDA(e);
-}
-
-void model_free(b200_model* m) {
-    if (!m) return;
-    cudaSetDevice(m->device);
-    for (auto& kv : m->raw) cudaFree(kv.second.p);
-    for (void* p : m->owned) cudaFree(p);
-    cudaFree(m->x);
-    cudaFree(m->h);
-    cudaFree(m->qkv);
-    cudaFree(m->o);
-    cudaFree(m->u);
-    cudaFree(m->patches);
-    cudaFree(m->aux);
-    cudaFree(m->out_dev);
-    cudaFree(m->pooled);
-    cudaFree(m->in_dev);
-    cudaFree(m->resized);
-    if (m->ev0) cudaEventDestroy(m->ev0);
-    if (m->ev1) cudaEventDestroy(m->ev1);
-    for (cudaEvent_t e : m->prof_ev) cudaEventDestroy(e);
-    for (auto& kv : m->graphs)
-        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-    if (m->own_stream) cudaStreamDestroy(m->own_stream);
-    delete m;
+// A device buffer built from the checkpoint, owned by the model until it is destroyed.
+template <class T>
+T* derived_buffer(b200_model* m, size_t n) {
+    m->derived.emplace_back(n * sizeof(T));
+    return reinterpret_cast<T*>(m->derived.back().get());
 }
 
 void check_tower(const b200_tower_desc& t, const char* name) {
@@ -153,21 +120,18 @@ void check_tower(const b200_tower_desc& t, const char* name) {
 const float* param(b200_model* m, const std::string& name, long long numel) {
     auto it = m->raw.find(name);
     if (it == m->raw.end()) fail(B200_ERR_MISSING_WEIGHT, "missing parameter '%s'", name.c_str());
-    if ((long long)(it->second.bytes / sizeof(float)) != numel)
-        fail(B200_ERR_INVALID_ARG, "parameter '%s' has %zu elements, expected %lld", name.c_str(),
-             it->second.bytes / sizeof(float), numel);
-    return reinterpret_cast<const float*>(it->second.p);
+    if ((long long)it->second.size() != numel)
+        fail(B200_ERR_INVALID_ARG, "parameter '%s' has %zu elements, expected %lld", name.c_str(), it->second.size(),
+             numel);
+    return it->second.get();
 }
 
 // fp32 parameter -> owned bf16 copy; the fp32 original is released.
 const __nv_bfloat16* to_bf16(b200_model* m, const std::string& name, long long numel) {
     const float* src = param(m, name, numel);
-    __nv_bfloat16* dst = nullptr;
-    dev_alloc((void**)&dst, (size_t)numel * 2);
-    m->owned.push_back(dst);
+    __nv_bfloat16* dst = derived_buffer<__nv_bfloat16>(m, (size_t)numel);
     kernels::f32_to_bf16(src, dst, numel, m->stream);
     MB_CUDA(cudaStreamSynchronize(m->stream));
-    cudaFree(m->raw[name].p);
     m->raw.erase(name);
     return dst;
 }
@@ -200,12 +164,8 @@ void build_bert_layers(b200_model* m, TowerW& T) {
         const std::string p = "encoder.layer." + std::to_string(i) + ".";
         LayerW& L = T.layers[i];
         // fuse query / key / value into one [3w, w] weight and one [3w] bias
-        __nv_bfloat16* wq = nullptr;
-        float* bq = nullptr;
-        dev_alloc((void**)&wq, (size_t)3 * w * w * 2);
-        dev_alloc((void**)&bq, (size_t)3 * w * 4);
-        m->owned.push_back(wq);
-        m->owned.push_back(bq);
+        __nv_bfloat16* wq = derived_buffer<__nv_bfloat16>(m, (size_t)3 * w * w);
+        float* bq = derived_buffer<float>(m, (size_t)3 * w);
         const char* names[3] = {"query", "key", "value"};
         for (int j = 0; j < 3; ++j) {
             const std::string base = p + "attention.self." + names[j];
@@ -214,11 +174,7 @@ void build_bert_layers(b200_model* m, TowerW& T) {
                                     m->stream));
         }
         MB_CUDA(cudaStreamSynchronize(m->stream));
-        for (int j = 0; j < 3; ++j) {
-            const std::string nm = p + "attention.self." + names[j] + ".weight";
-            cudaFree(m->raw[nm].p);
-            m->raw.erase(nm);
-        }
+        for (int j = 0; j < 3; ++j) m->raw.erase(p + "attention.self." + names[j] + ".weight");
         L.w_qkv = wq;
         L.b_qkv = bq;
         L.w_o = to_bf16(m, p + "attention.output.dense.weight", w * w);
@@ -244,19 +200,15 @@ struct ProfScope {
     ProfScope(b200_model* mm, int cls) : m(mm), on(mm->profiling) {
         if (!on) return;
         if ((size_t)(2 * m->prof_n + 2) > m->prof_ev.size()) {
-            for (int i = 0; i < 64; ++i) {
-                cudaEvent_t e;
-                MB_CUDA(cudaEventCreate(&e));
-                m->prof_ev.push_back(e);
-            }
+            for (int i = 0; i < 64; ++i) m->prof_ev.push_back(make_event());
             m->prof_cls.resize(m->prof_ev.size() / 2);
         }
         m->prof_cls[m->prof_n] = cls;
-        MB_CUDA(cudaEventRecord(m->prof_ev[2 * m->prof_n], m->stream));
+        MB_CUDA(cudaEventRecord(m->prof_ev[2 * m->prof_n].get(), m->stream));
     }
     ~ProfScope() {
         if (!on) return;
-        cudaEventRecord(m->prof_ev[2 * m->prof_n + 1], m->stream);
+        cudaEventRecord(m->prof_ev[2 * m->prof_n + 1].get(), m->stream);
         ++m->prof_n;
     }
 };
@@ -270,7 +222,7 @@ void linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, con
 
 void attend(b200_model* m, Counter& c, int B, int S, int w, int heads, int mask_mode, const int32_t* kv_len) {
     ProfScope ps(m, 1);
-    c.n += attention::launch(m->qkv, m->o, B, S, w, heads, mask_mode, kv_len, m->stream);
+    c.n += attention::launch(m->qkv.get(), m->o.get(), B, S, w, heads, mask_mode, kv_len, m->stream);
 }
 
 // MARQO_B200_GELU_FP32=1: evaluate fc1's erf-GELU in fp32 instead of packed fp16 (A/B timing and accuracy comparisons)
@@ -285,39 +237,39 @@ void run_clip_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, i
     const int M = B * S, w = T.d.width, mlp = T.d.mlp;
     const int act = m->desc.act == B200_ACT_QUICKGELU ? gemm::ACT_QUICKGELU : gemm::ACT_GELU;
     for (const LayerW& L : T.layers) {
-        kernels::layernorm(m->x, w, L.ln1_w, L.ln1_b, 1e-5f, M, w, nullptr, m->h, m->stream);
+        kernels::layernorm(m->x.get(), w, L.ln1_w, L.ln1_b, 1e-5f, M, w, nullptr, m->h.get(), m->stream);
         ++c.n;
         gemm::Epilogue e1;
         e1.bias = L.b_qkv;
-        e1.out = m->qkv;
+        e1.out = m->qkv.get();
         e1.ldo = 3 * w;
-        linear(m, c, m->h, M, w, L.w_qkv, 3 * w, e1);
+        linear(m, c, m->h.get(), M, w, L.w_qkv, 3 * w, e1);
         attend(m, c, B, S, w, T.d.heads, mask_mode, nullptr);
         gemm::Epilogue e2;
         e2.bias = L.b_o;
-        e2.residual = m->x;
+        e2.residual = m->x.get();
         e2.ldr = w;
-        e2.out = m->x;
+        e2.out = m->x.get();
         e2.ldo = w;
         e2.out_fp32 = 1;
-        linear(m, c, m->o, M, w, L.w_o, w, e2);
-        kernels::layernorm(m->x, w, L.ln2_w, L.ln2_b, 1e-5f, M, w, nullptr, m->h, m->stream);
+        linear(m, c, m->o.get(), M, w, L.w_o, w, e2);
+        kernels::layernorm(m->x.get(), w, L.ln2_w, L.ln2_b, 1e-5f, M, w, nullptr, m->h.get(), m->stream);
         ++c.n;
         gemm::Epilogue e3;
         e3.bias = L.b_fc;
         e3.act = act;
-        e3.out = m->u;
+        e3.out = m->u.get();
         e3.ldo = mlp;
         e3.act_fp32 = gelu_fp32() ? 1 : 0;
-        linear(m, c, m->h, M, w, L.w_fc, mlp, e3);
+        linear(m, c, m->h.get(), M, w, L.w_fc, mlp, e3);
         gemm::Epilogue e4;
         e4.bias = L.b_proj;
-        e4.residual = m->x;
+        e4.residual = m->x.get();
         e4.ldr = w;
-        e4.out = m->x;
+        e4.out = m->x.get();
         e4.ldo = w;
         e4.out_fp32 = 1;
-        linear(m, c, m->u, M, mlp, L.w_proj, w, e4);
+        linear(m, c, m->u.get(), M, mlp, L.w_proj, w, e4);
     }
 }
 
@@ -329,36 +281,36 @@ void run_bert_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S) {
     for (const LayerW& L : T.layers) {
         gemm::Epilogue e1;
         e1.bias = L.b_qkv;
-        e1.out = m->qkv;
+        e1.out = m->qkv.get();
         e1.ldo = 3 * w;
-        linear(m, c, m->h, M, w, L.w_qkv, 3 * w, e1);
-        attend(m, c, B, S, w, T.d.heads, attention::MASK_KEYLEN, m->aux);
+        linear(m, c, m->h.get(), M, w, L.w_qkv, 3 * w, e1);
+        attend(m, c, B, S, w, T.d.heads, attention::MASK_KEYLEN, m->aux.get());
         gemm::Epilogue e2;
         e2.bias = L.b_o;
-        e2.residual = m->x;
+        e2.residual = m->x.get();
         e2.ldr = w;
-        e2.out = m->x;
+        e2.out = m->x.get();
         e2.ldo = w;
         e2.out_fp32 = 1;
-        linear(m, c, m->o, M, w, L.w_o, w, e2);
-        kernels::layernorm(m->x, w, L.ln1_w, L.ln1_b, eps, M, w, m->x, m->h, m->stream);
+        linear(m, c, m->o.get(), M, w, L.w_o, w, e2);
+        kernels::layernorm(m->x.get(), w, L.ln1_w, L.ln1_b, eps, M, w, m->x.get(), m->h.get(), m->stream);
         ++c.n;
         gemm::Epilogue e3;
         e3.bias = L.b_fc;
         e3.act = gemm::ACT_GELU;
-        e3.out = m->u;
+        e3.out = m->u.get();
         e3.ldo = mlp;
         e3.act_fp32 = gelu_fp32() ? 1 : 0;
-        linear(m, c, m->h, M, w, L.w_fc, mlp, e3);
+        linear(m, c, m->h.get(), M, w, L.w_fc, mlp, e3);
         gemm::Epilogue e4;
         e4.bias = L.b_proj;
-        e4.residual = m->x;
+        e4.residual = m->x.get();
         e4.ldr = w;
-        e4.out = m->x;
+        e4.out = m->x.get();
         e4.ldo = w;
         e4.out_fp32 = 1;
-        linear(m, c, m->u, M, mlp, L.w_proj, w, e4);
-        kernels::layernorm(m->x, w, L.ln2_w, L.ln2_b, eps, M, w, m->x, m->h, m->stream);
+        linear(m, c, m->u.get(), M, mlp, L.w_proj, w, e4);
+        kernels::layernorm(m->x.get(), w, L.ln2_w, L.ln2_b, eps, M, w, m->x.get(), m->h.get(), m->stream);
         ++c.n;
     }
 }
@@ -369,7 +321,7 @@ void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const fl
     const TowerW& T = m->vision;
     const int S = T.d.image_size, p = T.d.patch, w = T.d.width, G = T.grid * T.grid;
     gemm::Epilogue e;  // conv1 (no bias) + positional embedding, scattered to token rows 1..G of each image
-    e.out = m->x;
+    e.out = m->x.get();
     e.ldo = w;
     e.out_fp32 = 1;
     e.remap_group = G;
@@ -391,20 +343,20 @@ void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const fl
         ++c.n;
     } else {
         // preprocessed fp32 CHW tensors (the reference's parity path) and shapes the gather does not cover
-        if (!m->patches) dev_alloc((void**)&m->patches, (size_t)m->desc.max_batch * G * T.kpad * 2);
+        if (!m->patches) m->patches = DeviceBuffer<__nv_bfloat16>((size_t)m->desc.max_batch * G * T.kpad);
         if (u8)
-            kernels::im2col_u8(u8, n, S, p, T.kpad, m->desc.image_mean, m->desc.image_std, m->patches, m->stream);
+            kernels::im2col_u8(u8, n, S, p, T.kpad, m->desc.image_mean, m->desc.image_std, m->patches.get(), m->stream);
         else
-            kernels::im2col_f32(f32, n, S, p, T.kpad, m->patches, m->stream);
-        linear(m, c, m->patches, n * G, T.kpad, T.conv_w, w, e);
+            kernels::im2col_f32(f32, n, S, p, T.kpad, m->patches.get(), m->stream);
+        linear(m, c, m->patches.get(), n * G, T.kpad, T.conv_w, w, e);
         ++c.n;
     }
-    kernels::vit_cls_rows(m->x, T.cls, T.pos, n, T.tokens, w, m->stream);
-    kernels::layernorm(m->x, w, T.ln_pre_w, T.ln_pre_b, 1e-5f, n * T.tokens, w, m->x, nullptr, m->stream);
+    kernels::vit_cls_rows(m->x.get(), T.cls, T.pos, n, T.tokens, w, m->stream);
+    kernels::layernorm(m->x.get(), w, T.ln_pre_w, T.ln_pre_b, 1e-5f, n * T.tokens, w, m->x.get(), nullptr, m->stream);
     c.n += 2;
     run_clip_blocks(m, c, T, n, T.tokens, attention::MASK_NONE);
-    kernels::clip_head(m->x, T.tokens, nullptr, T.ln_out_w, T.ln_out_b, 1e-5f, T.proj, n, w, m->desc.embed_dim, normalize,
-                       d_out, m->pooled, m->stream);
+    kernels::clip_head(m->x.get(), T.tokens, nullptr, T.ln_out_w, T.ln_out_b, 1e-5f, T.proj, n, w, m->desc.embed_dim,
+                       normalize, d_out, m->pooled.get(), m->stream);
     c.n += 3;
 }
 
@@ -413,18 +365,18 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
     const TowerW& T = m->text;
     const int w = T.d.width;
     if (m->desc.arch == B200_ARCH_CLIP) {
-        kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, m->x, m->aux, m->stream);
+        kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, m->x.get(), m->aux.get(), m->stream);
         c.n += 1;
         run_clip_blocks(m, c, T, n, S, attention::MASK_CAUSAL);
-        kernels::clip_head(m->x, S, m->aux, T.ln_out_w, T.ln_out_b, 1e-5f, T.proj, n, w, m->desc.embed_dim, normalize,
-                           d_out, m->pooled, m->stream);
+        kernels::clip_head(m->x.get(), S, m->aux.get(), T.ln_out_w, T.ln_out_b, 1e-5f, T.proj, n, w, m->desc.embed_dim,
+                           normalize, d_out, m->pooled.get(), m->stream);
         c.n += 3;
     } else {
         kernels::bert_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, 1e-12f, n, S, w, T.d.vocab,
-                               m->x, m->h, m->aux, m->stream);
+                               m->x.get(), m->h.get(), m->aux.get(), m->stream);
         c.n += 1;
         run_bert_blocks(m, c, T, n, S);
-        kernels::bert_head(m->x, m->aux, n, S, w, m->desc.pool, normalize, d_out, m->stream);
+        kernels::bert_head(m->x.get(), m->aux.get(), n, S, w, m->desc.pool, normalize, d_out, m->stream);
         c.n += 1;
     }
 }
@@ -465,20 +417,15 @@ void run_graphed(b200_model* m, Counter& c, const b200_model::GraphKey& key, lon
         const cudaError_t e = cudaGraphInstantiate(&exec, graph, 0);
         cudaGraphDestroy(graph);
         MB_CUDA(e);
-        it->second.exec = exec;
+        it->second.exec.reset(exec);
         it->second.launches = cc.n;
     }
-    MB_CUDA(cudaGraphLaunch(it->second.exec, m->stream));
+    MB_CUDA(cudaGraphLaunch(it->second.exec.get(), m->stream));
     c.n += it->second.launches;
 }
 
 void ensure_in_dev(b200_model* m, size_t bytes) {
-    if (bytes <= m->in_dev_bytes) return;
-    cudaFree(m->in_dev);
-    m->in_dev = nullptr;
-    m->in_dev_bytes = 0;
-    dev_alloc(&m->in_dev, bytes);
-    m->in_dev_bytes = bytes;
+    if (bytes > m->in_dev.size()) m->in_dev = DeviceBuffer<uint8_t>(bytes);
 }
 
 void forward_images(b200_model* m, Counter& c, const uint8_t* u8, const float* f32, int n, int normalize, float* d_out) {
@@ -506,9 +453,9 @@ int batch_cap_tokens(b200_model* m, int tokens_per_item) {
 struct TimedRegion {
     b200_model* m;
     Counter c;
-    explicit TimedRegion(b200_model* mm) : m(mm) { MB_CUDA(cudaEventRecord(m->ev0, m->stream)); }
+    explicit TimedRegion(b200_model* mm) : m(mm) { MB_CUDA(cudaEventRecord(m->ev0.get(), m->stream)); }
     void finish() {
-        MB_CUDA(cudaEventRecord(m->ev1, m->stream));
+        MB_CUDA(cudaEventRecord(m->ev1.get(), m->stream));
         m->timing_valid = true;
         m->last_launches = c.n;
     }
@@ -524,9 +471,9 @@ void encode_images_u8_dev(b200_model* m, Counter& c, const uint8_t* d_img, int n
         const int nb = std::min(cap, n - o);
         const uint8_t* src = d_img + (size_t)o * h * w * 3;
         if (h != S || w != S) {
-            kernels::resize_crop_u8(src, nb, h, w, S, m->resized, m->stream);
+            kernels::resize_crop_u8(src, nb, h, w, S, m->resized.get(), m->stream);
             c.n += 2;
-            src = m->resized;
+            src = m->resized.get();
         }
         forward_images(m, c, src, nullptr, nb, normalize, d_out + (size_t)o * m->desc.embed_dim);
     }
@@ -556,15 +503,7 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
     return guarded([&] {
         MB_CHECK_ARG(desc && out, "NULL argument");
         *out = nullptr;
-        int ndev = 0;
-        if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-            cudaGetLastError();
-            fail(B200_ERR_NO_DEVICE, "no CUDA device available (marqo_b200 has no CPU fallback)");
-        }
-        MB_CHECK_ARG(device >= 0 && device < ndev, "device %d out of range (%d devices)", device, ndev);
-        int major = 0;
-        MB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-        if (major != 9) fail(B200_ERR_NO_DEVICE, "device %d has compute capability %d.x; sm_90 required", device, major);
+        require_sm90_device(device);
         MB_CHECK_ARG(desc->arch == B200_ARCH_CLIP || desc->arch == B200_ARCH_BERT, "unknown arch %d", desc->arch);
         MB_CHECK_ARG(desc->max_batch > 0, "max_batch must be positive");
         MB_CHECK_ARG(desc->embed_dim > 0 && desc->embed_dim <= 4096, "embed_dim out of range");
@@ -584,30 +523,29 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
                 MB_CHECK_ARG(desc->embed_dim == desc->text.width, "BERT embed_dim must equal width");
         }
         DeviceGuard g(device);
-        b200_model* m = new b200_model();
-        try {
-            m->device = device;
-            m->desc = *desc;
-            m->sms = sm_count(device);
-            MB_CUDA(cudaStreamCreateWithFlags(&m->own_stream, cudaStreamNonBlocking));
-            m->stream = m->own_stream;
-            MB_CUDA(cudaEventCreate(&m->ev0));
-            MB_CUDA(cudaEventCreate(&m->ev1));
-            m->vision.present = has_vision;
-            m->vision.d = desc->vision;
-            m->text.present = has_text;
-            m->text.d = desc->text;
-            gemm::configure();
-        } catch (...) {
-            model_free(m);
-            throw;
-        }
-        *out = m;
+        std::unique_ptr<b200_model> m(new b200_model());   // released under the guard if the set-up fails
+        m->device = device;
+        m->desc = *desc;
+        m->sms = sm_count(device);
+        m->own_stream = make_stream(cudaStreamNonBlocking);
+        m->stream = m->own_stream.get();
+        m->ev0 = make_event();
+        m->ev1 = make_event();
+        m->vision.present = has_vision;
+        m->vision.d = desc->vision;
+        m->text.present = has_text;
+        m->text.d = desc->text;
+        gemm::configure();
+        *out = m.release();
     });
 }
 
 int b200_model_destroy(b200_model* m) {
-    return guarded([&] { model_free(m); });
+    return guarded([&] {
+        if (!m) return;
+        DeviceGuard g(m->device);
+        delete m;
+    });
 }
 
 int b200_model_load_tensor(b200_model* m, const char* name, const float* data, int64_t numel) {
@@ -617,20 +555,9 @@ int b200_model_load_tensor(b200_model* m, const char* name, const float* data, i
         std::lock_guard<std::mutex> lk(m->mu);
         if (m->finalized) fail(B200_ERR_INVALID_ARG, "model is already finalized");
         DeviceGuard g(m->device);
-        Buf b;
-        b.bytes = (size_t)numel * sizeof(float);
-        dev_alloc(&b.p, b.bytes);
-        cudaError_t e = cudaMemcpy(b.p, data, b.bytes, cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) {
-            cudaFree(b.p);
-            MB_CUDA(e);
-        }
-        auto it = m->raw.find(name);
-        if (it != m->raw.end()) {
-            cudaFree(it->second.p);
-            m->raw.erase(it);
-        }
-        m->raw[name] = b;
+        DeviceBuffer<float> b((size_t)numel);
+        MB_CUDA(cudaMemcpy(b.get(), data, (size_t)numel * sizeof(float), cudaMemcpyHostToDevice));
+        m->raw[name] = std::move(b);
     });
 }
 
@@ -650,16 +577,12 @@ int b200_model_finalize(b200_model* m) {
             const int K = 3 * (int)p * (int)p;
             T.kpad = (int)round_up((size_t)K, 64);
             const float* conv = param(m, "visual.conv1.weight", w * K);
-            __nv_bfloat16* cw = nullptr;
-            dev_alloc((void**)&cw, (size_t)w * T.kpad * 2);
-            m->owned.push_back(cw);
+            __nv_bfloat16* cw = derived_buffer<__nv_bfloat16>(m, (size_t)w * T.kpad);
             kernels::pad_rows_to_bf16(conv, (int)w, K, T.kpad, cw, m->stream);
             MB_CUDA(cudaStreamSynchronize(m->stream));
             T.conv_w = cw;
             if (gemm::patch_gather_supported(T.d.image_size, (int)p)) {
-                __nv_bfloat16* cg = nullptr;
-                dev_alloc((void**)&cg, (size_t)w * gemm::patch_gather_k((int)p) * 2);
-                m->owned.push_back(cg);
+                __nv_bfloat16* cg = derived_buffer<__nv_bfloat16>(m, (size_t)w * gemm::patch_gather_k((int)p));
                 kernels::patch_weight_rows(conv, (int)w, (int)p, gemm::patch_gather_kbpd((int)p), cg, m->stream);
                 MB_CUDA(cudaStreamSynchronize(m->stream));
                 T.conv_wg = cg;
@@ -677,8 +600,8 @@ int b200_model_finalize(b200_model* m) {
             max_mlp = std::max(max_mlp, (long long)T.d.mlp);
             // the bf16 patch matrix of the im2col path is allocated on first use (fp32 CHW input / unsupported shapes)
             if (!T.conv_wg)
-                dev_alloc((void**)&m->patches, (size_t)m->desc.max_batch * T.grid * T.grid * T.kpad * 2);
-            dev_alloc((void**)&m->resized, (size_t)m->desc.max_batch * T.d.image_size * T.d.image_size * 3);
+                m->patches = DeviceBuffer<__nv_bfloat16>((size_t)m->desc.max_batch * T.grid * T.grid * T.kpad);
+            m->resized = DeviceBuffer<uint8_t>((size_t)m->desc.max_batch * T.d.image_size * T.d.image_size * 3);
         }
         if (m->text.present) {
             TowerW& T = m->text;
@@ -708,15 +631,15 @@ int b200_model_finalize(b200_model* m) {
         const long long bytes_per_tok = max_w * (4 + 2 + 6 + 2) + max_mlp * 2;
         const long long cap_tok = (24LL << 30) / bytes_per_tok;
         m->max_tokens = std::min(max_tok, std::max<long long>(cap_tok, 1024));
-        dev_alloc((void**)&m->x, (size_t)m->max_tokens * max_w * 4);
-        dev_alloc((void**)&m->h, (size_t)m->max_tokens * max_w * 2);
-        dev_alloc((void**)&m->qkv, (size_t)m->max_tokens * max_w * 6);
-        dev_alloc((void**)&m->o, (size_t)m->max_tokens * max_w * 2);
-        dev_alloc((void**)&m->u, (size_t)m->max_tokens * max_mlp * 2);
+        m->x = DeviceBuffer<float>((size_t)m->max_tokens * max_w);
+        m->h = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_w);
+        m->qkv = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_w * 3);
+        m->o = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_w);
+        m->u = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_mlp);
         MB_CUDA(cudaStreamSynchronize(m->stream));
-        dev_alloc((void**)&m->aux, (size_t)m->desc.max_batch * 4);
-        dev_alloc((void**)&m->out_dev, (size_t)m->desc.max_batch * E * 4);
-        dev_alloc((void**)&m->pooled, (size_t)m->desc.max_batch * max_w * 4);
+        m->aux = DeviceBuffer<int32_t>((size_t)m->desc.max_batch);
+        m->out_dev = DeviceBuffer<float>((size_t)m->desc.max_batch * E);
+        m->pooled = DeviceBuffer<float>((size_t)m->desc.max_batch * max_w);
         MB_CUDA(cudaStreamSynchronize(m->stream));
         m->finalized = true;
     });
@@ -737,10 +660,11 @@ int b200_model_encode_images_u8(b200_model* m, const uint8_t* hwc, int n, int h,
         TimedRegion tr(m);
         for (int o = 0; o < n; o += cap) {
             const int nb = std::min(cap, n - o);
-            MB_CUDA(cudaMemcpyAsync(m->in_dev, hwc + (size_t)o * img_bytes, (size_t)nb * img_bytes, cudaMemcpyHostToDevice,
+            MB_CUDA(cudaMemcpyAsync(m->in_dev.get(), hwc + (size_t)o * img_bytes, (size_t)nb * img_bytes,
+                                    cudaMemcpyHostToDevice, m->stream));
+            encode_images_u8_dev(m, tr.c, m->in_dev.get(), nb, h, w, normalize, m->out_dev.get());
+            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
                                     m->stream));
-            encode_images_u8_dev(m, tr.c, reinterpret_cast<const uint8_t*>(m->in_dev), nb, h, w, normalize, m->out_dev);
-            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev, (size_t)nb * E * 4, cudaMemcpyDeviceToHost, m->stream));
             MB_CUDA(cudaStreamSynchronize(m->stream));
         }
         tr.finish();
@@ -762,10 +686,12 @@ int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int nor
         TimedRegion tr(m);
         for (int o = 0; o < n; o += cap) {
             const int nb = std::min(cap, n - o);
-            MB_CUDA(cudaMemcpyAsync(m->in_dev, chw + (size_t)o * 3 * S * S, (size_t)nb * img_bytes, cudaMemcpyHostToDevice,
+            MB_CUDA(cudaMemcpyAsync(m->in_dev.get(), chw + (size_t)o * 3 * S * S, (size_t)nb * img_bytes,
+                                    cudaMemcpyHostToDevice, m->stream));
+            forward_images(m, tr.c, nullptr, reinterpret_cast<const float*>(m->in_dev.get()), nb, normalize,
+                           m->out_dev.get());
+            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
                                     m->stream));
-            forward_images(m, tr.c, nullptr, reinterpret_cast<const float*>(m->in_dev), nb, normalize, m->out_dev);
-            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev, (size_t)nb * E * 4, cudaMemcpyDeviceToHost, m->stream));
             MB_CUDA(cudaStreamSynchronize(m->stream));
         }
         tr.finish();
@@ -796,7 +722,7 @@ int b200_model_encode_tokens(b200_model* m, const int32_t* ids, const int32_t* a
         const int cap = batch_cap_tokens(m, seq);
         const size_t row_bytes = (size_t)seq * 4;
         ensure_in_dev(m, (size_t)std::min(n, cap) * row_bytes * 2);
-        int32_t* d_ids = reinterpret_cast<int32_t*>(m->in_dev);
+        int32_t* d_ids = reinterpret_cast<int32_t*>(m->in_dev.get());
         int32_t* d_mask = d_ids + (size_t)std::min(n, cap) * seq;
         TimedRegion tr(m);
         for (int o = 0; o < n; o += cap) {
@@ -805,8 +731,9 @@ int b200_model_encode_tokens(b200_model* m, const int32_t* ids, const int32_t* a
             if (attn_mask)
                 MB_CUDA(cudaMemcpyAsync(d_mask, attn_mask + (size_t)o * seq, (size_t)nb * row_bytes, cudaMemcpyHostToDevice,
                                         m->stream));
-            forward_tokens(m, tr.c, d_ids, attn_mask ? d_mask : nullptr, nb, seq, normalize, m->out_dev);
-            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev, (size_t)nb * E * 4, cudaMemcpyDeviceToHost, m->stream));
+            forward_tokens(m, tr.c, d_ids, attn_mask ? d_mask : nullptr, nb, seq, normalize, m->out_dev.get());
+            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
+                                    m->stream));
             MB_CUDA(cudaStreamSynchronize(m->stream));
         }
         tr.finish();
@@ -850,7 +777,7 @@ int b200_model_set_stream(b200_model* m, void* cuda_stream, int use_external) {
         std::lock_guard<std::mutex> lk(m->mu);
         DeviceGuard g(m->device);
         MB_CUDA(cudaStreamSynchronize(m->stream));
-        m->stream = use_external ? reinterpret_cast<cudaStream_t>(cuda_stream) : m->own_stream;
+        m->stream = use_external ? reinterpret_cast<cudaStream_t>(cuda_stream) : m->own_stream.get();
         m->external_stream = use_external != 0;   // a caller's stream may itself be under capture: no graphs there
     });
 }
@@ -872,9 +799,9 @@ int b200_model_profile(b200_model* m, float* gemm_ms, int* gemm_launches, float*
         float ms[2] = {0.f, 0.f};
         int cnt[2] = {0, 0};
         for (int i = 0; i < m->prof_n; ++i) {
-            MB_CUDA(cudaEventSynchronize(m->prof_ev[2 * i + 1]));
+            MB_CUDA(cudaEventSynchronize(m->prof_ev[2 * i + 1].get()));
             float t = 0.f;
-            MB_CUDA(cudaEventElapsedTime(&t, m->prof_ev[2 * i], m->prof_ev[2 * i + 1]));
+            MB_CUDA(cudaEventElapsedTime(&t, m->prof_ev[2 * i].get(), m->prof_ev[2 * i + 1].get()));
             ms[m->prof_cls[i]] += t;
             ++cnt[m->prof_cls[i]];
         }
@@ -891,8 +818,8 @@ int b200_model_last_timing(b200_model* m, float* ms, int* launches) {
         std::lock_guard<std::mutex> lk(m->mu);
         DeviceGuard g(m->device);
         if (!m->timing_valid) fail(B200_ERR_INVALID_ARG, "no encode call has been timed yet");
-        MB_CUDA(cudaEventSynchronize(m->ev1));
-        MB_CUDA(cudaEventElapsedTime(ms, m->ev0, m->ev1));
+        MB_CUDA(cudaEventSynchronize(m->ev1.get()));
+        MB_CUDA(cudaEventElapsedTime(ms, m->ev0.get(), m->ev1.get()));
         *launches = m->last_launches;
     });
 }

@@ -1151,11 +1151,10 @@ using namespace mb::score;
 struct b200_exchange {
     int device = 0;
     int rank = 0, world = 1;
-    size_t slot_stride = 0;      // bytes per (parity, source rank) slot
-    size_t buf_bytes = 0;
-    uint8_t* local = nullptr;    // cudaMalloc'ed: [2][world][slot_stride] blocks, then [2][world] u64 flags
+    size_t slot_stride = 0;         // bytes per (parity, source rank) slot
+    DeviceBuffer<uint8_t> local;    // [2][world][slot_stride] blocks, then [2][world] u64 flags
+    IpcMapping mapped[8];           // the other ranks' buffers, opened by b200_exchange_open
     uint8_t* peer[8] = {nullptr};   // peer[s] = rank s's buffer mapped here (peer[rank] == local)
-    bool opened[8] = {false};
     unsigned long long epoch = 0;
 };
 
@@ -1169,136 +1168,84 @@ struct b200_index {
     int64_t dead_rows = 0;  // tombstoned rows still occupying the matrix
     bool has_docs = false;  // false while doc_of_row[i] == i for every row (identity fast path)
     int32_t doc_offset = 0; // added to returned document numbers (shard -> global numbering)
-    __half* corpus = nullptr;
-    int32_t* doc_of_row = nullptr;
-    float* row_n2 = nullptr;       // [capacity] squared norms (euclidean metric only)
-    float* max_n2 = nullptr;       // [1] largest squared norm of a stored row
-    int* d_flags = nullptr;        // [2]: bit 0 of [0] = non-finite / out-of-fp16-range input; [1] = negative multiplier
+    DeviceBuffer<__half> corpus;       // [capacity, dim]
+    DeviceBuffer<int32_t> doc_of_row;  // [capacity]
+    DeviceBuffer<float> row_n2;        // [capacity] squared norms (euclidean metric only)
+    DeviceBuffer<float> max_n2;        // [1] largest squared norm of a stored row
+    DeviceBuffer<int> d_flags;         // [2]: bit 0 of [0] = non-finite / out-of-fp16-range input;
+                                       //      [1] = negative multiplier
     // per-search workspaces
-    __half* qh = nullptr;          // [MQ, dim]
-    float* q_stage = nullptr;      // [MQ, dim] fp32 staging for host queries
-    float* list_score = nullptr;   // [grid][MQ][KP]
-    int32_t* list_row = nullptr;
-    int32_t* list_doc = nullptr;
-    int out_k = 0;                 // the resident output block holds [MQ, out_k]
-    int32_t* o_doc = nullptr;
-    int32_t* o_row = nullptr;
-    double* o_score = nullptr;
-    QState* qs = nullptr;          // device
-    QState* h_qs = nullptr;        // pinned host mirror
-    int32_t* cbuf = nullptr;       // [MQ][ccap] rows appended by the collect pass
+    DeviceBuffer<__half> qh;           // [MQ, dim]
+    DeviceBuffer<float> q_stage;       // [MQ, dim] fp32 staging for host queries
+    DeviceBuffer<float> list_score;    // [grid][MQ][KP]
+    DeviceBuffer<int32_t> list_row;
+    DeviceBuffer<int32_t> list_doc;
+    int out_k = 0;                     // the resident output block holds [MQ, out_k]
+    DeviceBuffer<int32_t> o_doc;
+    DeviceBuffer<int32_t> o_row;
+    DeviceBuffer<double> o_score;
+    DeviceBuffer<QState> qs;           // device
+    PinnedPtr<QState> h_qs;            // pinned host mirror
+    DeviceBuffer<int32_t> cbuf;        // [MQ][ccap] rows appended by the collect pass
     int ccap = 0;
-    // score modifiers: per-document numeric attributes (one device column per attribute name, NaN = missing)
-    std::vector<double*> attr_cols;
-    double** d_cols_table = nullptr;  // device copy of attr_cols (B200_MAX_ATTRIBUTE_COLUMNS entries)
+    // score modifiers: per-document numeric attributes (one device column per attribute name, NaN = missing; an empty
+    // buffer is a column that was never set)
+    std::vector<DeviceBuffer<double>> attr_cols;
+    DeviceBuffer<double*> d_cols_table;  // device copy of the attr_cols pointers (B200_MAX_ATTRIBUTE_COLUMNS entries)
     bool cols_table_dirty = true;
     int64_t attr_cap = 0;          // documents each column can hold
     int64_t max_doc = -1;          // largest explicit document number seen by add()
-    double2* mod64 = nullptr;      // [mod_cap] (mult, add) of the current modified search
-    float2* mod32 = nullptr;
+    DeviceBuffer<double2> mod64;   // [mod_cap] (mult, add) of the current modified search
+    DeviceBuffer<float2> mod32;
     int64_t mod_cap = 0;
-    double* mod_max = nullptr;     // [2] max |mult|, max |add|
+    DeviceBuffer<double> mod_max;  // [2] max |mult|, max |add|
     bool mod_active = false;
     // document filter of the current search (device bitset over local document numbers)
-    uint32_t* filter_bits = nullptr;
+    DeviceBuffer<uint32_t> filter_bits;
     int64_t filter_cap_words = 0;
     int64_t filter_docs = 0;
     uint64_t filter_tag = 0;       // identity of the bitset held in filter_bits (0 = none cached)
     bool filter_active = false;
     // statistics of the exactness machinery (b200_index_search_stats)
     int64_t stat_groups = 0, stat_flagged = 0, stat_collect_passes = 0, stat_host_finalize = 0;
-    cudaStream_t stream = nullptr;
-    cudaStream_t own_stream = nullptr;
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    cudaStream_t stream = nullptr;   // own_stream, or the caller's stream set by b200_index_set_stream
+    UniqueStream own_stream;
+    UniqueEvent ev[4];
     bool timing_valid = false;
     std::mutex mu;
 };
 
 namespace {
 
-void index_free(b200_index* ix) {
-    if (!ix) return;
-    cudaSetDevice(ix->device);
-    cudaFree(ix->corpus);
-    cudaFree(ix->doc_of_row);
-    cudaFree(ix->row_n2);
-    cudaFree(ix->max_n2);
-    cudaFree(ix->d_flags);
-    cudaFree(ix->qh);
-    cudaFree(ix->q_stage);
-    cudaFree(ix->list_score);
-    cudaFree(ix->list_row);
-    cudaFree(ix->list_doc);
-    cudaFree(ix->o_doc);
-    cudaFree(ix->o_row);
-    cudaFree(ix->o_score);
-    cudaFree(ix->qs);
-    if (ix->h_qs) cudaFreeHost(ix->h_qs);
-    cudaFree(ix->cbuf);
-    for (double* c : ix->attr_cols) cudaFree(c);
-    cudaFree(ix->d_cols_table);
-    cudaFree(ix->mod64);
-    cudaFree(ix->mod32);
-    cudaFree(ix->mod_max);
-    cudaFree(ix->filter_bits);
-    for (auto& e : ix->ev)
-        if (e) cudaEventDestroy(e);
-    if (ix->own_stream) cudaStreamDestroy(ix->own_stream);
-    delete ix;
-}
-
-void cuda_alloc(void** p, size_t bytes) {
-    cudaError_t e = cudaMalloc(p, bytes);
-    if (e == cudaErrorMemoryAllocation) {
-        cudaGetLastError();
-        fail(B200_ERR_OOM, "cudaMalloc(%zu bytes) failed: out of device memory", bytes);
-    }
-    MB_CUDA(e);
-}
-
-struct DevBuf {   // RAII scratch allocation
-    void* p = nullptr;
-    DevBuf() = default;
-    explicit DevBuf(size_t bytes) { cuda_alloc(&p, bytes); }
-    DevBuf(const DevBuf&) = delete;
-    DevBuf& operator=(const DevBuf&) = delete;
-    ~DevBuf() { cudaFree(p); }
-    template <class T>
-    T* as() const { return reinterpret_cast<T*>(p); }
+struct RowArrays {   // the per-row arrays of an index, allocated together for one capacity
+    DeviceBuffer<__half> corpus;
+    DeviceBuffer<int32_t> doc_of_row;
+    DeviceBuffer<float> row_n2;
 };
+
+RowArrays alloc_rows(const b200_index* ix, int64_t cap) {
+    return {DeviceBuffer<__half>((size_t)cap * ix->dim), DeviceBuffer<int32_t>((size_t)cap),
+            ix->metric == B200_METRIC_EUCLIDEAN ? DeviceBuffer<float>((size_t)cap) : DeviceBuffer<float>()};
+}
 
 void ensure_capacity(b200_index* ix, int64_t need_rows) {
     if (need_rows <= ix->capacity) return;
     int64_t cap = std::max<int64_t>(need_rows, ix->capacity + ix->capacity / 2);
     cap = (int64_t)round_up((size_t)cap, TILE_N);
-    __half* nc = nullptr;
-    int32_t* nd = nullptr;
-    float* nn = nullptr;
-    try {
-        cuda_alloc((void**)&nc, (size_t)cap * ix->dim * sizeof(__half));
-        cuda_alloc((void**)&nd, (size_t)cap * sizeof(int32_t));
-        if (ix->metric == B200_METRIC_EUCLIDEAN) cuda_alloc((void**)&nn, (size_t)cap * sizeof(float));
-    } catch (...) {
-        cudaFree(nc);
-        cudaFree(nd);
-        cudaFree(nn);
-        throw;
-    }
+    RowArrays r = alloc_rows(ix, cap);
     if (ix->n_rows > 0) {
-        MB_CUDA(cudaMemcpyAsync(nc, ix->corpus, (size_t)ix->n_rows * ix->dim * sizeof(__half), cudaMemcpyDeviceToDevice,
-                                ix->stream));
-        MB_CUDA(cudaMemcpyAsync(nd, ix->doc_of_row, (size_t)ix->n_rows * sizeof(int32_t), cudaMemcpyDeviceToDevice,
-                                ix->stream));
-        if (nn)
-            MB_CUDA(cudaMemcpyAsync(nn, ix->row_n2, (size_t)ix->n_rows * sizeof(float), cudaMemcpyDeviceToDevice, ix->stream));
+        MB_CUDA(cudaMemcpyAsync(r.corpus.get(), ix->corpus.get(), (size_t)ix->n_rows * ix->dim * sizeof(__half),
+                                cudaMemcpyDeviceToDevice, ix->stream));
+        MB_CUDA(cudaMemcpyAsync(r.doc_of_row.get(), ix->doc_of_row.get(), (size_t)ix->n_rows * sizeof(int32_t),
+                                cudaMemcpyDeviceToDevice, ix->stream));
+        if (r.row_n2)
+            MB_CUDA(cudaMemcpyAsync(r.row_n2.get(), ix->row_n2.get(), (size_t)ix->n_rows * sizeof(float),
+                                    cudaMemcpyDeviceToDevice, ix->stream));
     }
     MB_CUDA(cudaStreamSynchronize(ix->stream));
-    cudaFree(ix->corpus);
-    cudaFree(ix->doc_of_row);
-    cudaFree(ix->row_n2);
-    ix->corpus = nc;
-    ix->doc_of_row = nd;
-    ix->row_n2 = nn;
+    ix->corpus = std::move(r.corpus);
+    ix->doc_of_row = std::move(r.doc_of_row);
+    ix->row_n2 = std::move(r.row_n2);
     ix->capacity = cap;
 }
 
@@ -1306,25 +1253,16 @@ void ensure_out_k(b200_index* ix, int k) {
     if (k <= ix->out_k) return;
     const int nk = std::max(k, 16);
     MB_CUDA(cudaStreamSynchronize(ix->stream));
-    cudaFree(ix->o_doc);
-    cudaFree(ix->o_row);
-    cudaFree(ix->o_score);
-    ix->o_doc = ix->o_row = nullptr;
-    ix->o_score = nullptr;
-    ix->out_k = 0;
-    cuda_alloc((void**)&ix->o_doc, (size_t)MQ * nk * sizeof(int32_t));
-    cuda_alloc((void**)&ix->o_row, (size_t)MQ * nk * sizeof(int32_t));
-    cuda_alloc((void**)&ix->o_score, (size_t)MQ * nk * sizeof(double));
+    ix->o_doc = DeviceBuffer<int32_t>((size_t)MQ * nk);
+    ix->o_row = DeviceBuffer<int32_t>((size_t)MQ * nk);
+    ix->o_score = DeviceBuffer<double>((size_t)MQ * nk);
     ix->out_k = nk;
 }
 
 void ensure_ccap(b200_index* ix, int cap) {
     if (cap <= ix->ccap) return;
     MB_CUDA(cudaStreamSynchronize(ix->stream));
-    cudaFree(ix->cbuf);
-    ix->cbuf = nullptr;
-    ix->ccap = 0;
-    cuda_alloc((void**)&ix->cbuf, (size_t)MQ * cap * sizeof(int32_t));
+    ix->cbuf = DeviceBuffer<int32_t>((size_t)MQ * cap);
     ix->ccap = cap;
 }
 
@@ -1339,70 +1277,57 @@ ScanFn scan_fn(int idx) {
 }
 
 b200_index* index_new(int device, int dim, int metric, int64_t capacity_rows) {
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        fail(B200_ERR_NO_DEVICE, "no CUDA device available (marqo_b200 has no CPU fallback)");
-    }
-    MB_CHECK_ARG(device >= 0 && device < ndev, "device %d out of range (%d devices)", device, ndev);
-    int major = 0;
-    MB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    if (major != 9) fail(B200_ERR_NO_DEVICE, "device %d has compute capability %d.x; sm_90 required", device, major);
+    require_sm90_device(device);
     MB_CHECK_ARG(dim > 0 && dim % BLOCK_K == 0 && dim <= MAX_DIM, "dim must be a multiple of %d and <= %d (got %d)",
                  BLOCK_K, MAX_DIM, dim);
     MB_CHECK_ARG(metric >= 0 && metric <= B200_METRIC_EUCLIDEAN, "unknown metric %d", metric);
     MB_CHECK_ARG(capacity_rows >= 0, "capacity_rows must be >= 0");
     DeviceGuard g(device);
-    b200_index* ix = new b200_index();
-    try {
-        ix->device = device;
-        ix->dim = dim;
-        ix->metric = metric;
-        ix->sms = std::min(sm_count(device), MAX_LISTS);   // merge_kernel's list-head table holds MAX_LISTS lists
-        MB_CUDA(cudaStreamCreateWithFlags(&ix->own_stream, cudaStreamNonBlocking));
-        ix->stream = ix->own_stream;
-        for (auto& e : ix->ev) MB_CUDA(cudaEventCreate(&e));
-        cuda_alloc((void**)&ix->qh, (size_t)MQ * dim * sizeof(__half));
-        cuda_alloc((void**)&ix->q_stage, (size_t)MQ * dim * sizeof(float));
-        const size_t nl = (size_t)ix->sms * MQ * KP;
-        cuda_alloc((void**)&ix->list_score, nl * sizeof(float));
-        cuda_alloc((void**)&ix->list_row, nl * sizeof(int32_t));
-        cuda_alloc((void**)&ix->list_doc, nl * sizeof(int32_t));
-        cuda_alloc((void**)&ix->qs, sizeof(QState));
-        MB_CUDA(cudaMemset(ix->qs, 0, sizeof(QState)));
-        MB_CUDA(cudaHostAlloc((void**)&ix->h_qs, sizeof(QState), cudaHostAllocPortable));
-        cuda_alloc((void**)&ix->max_n2, sizeof(float));
-        MB_CUDA(cudaMemset(ix->max_n2, 0, sizeof(float)));
-        cuda_alloc((void**)&ix->d_flags, 2 * sizeof(int));
-        MB_CUDA(cudaMemset(ix->d_flags, 0, 2 * sizeof(int)));
-        cuda_alloc((void**)&ix->mod_max, 2 * sizeof(double));
-        MB_CUDA(cudaMemset(ix->mod_max, 0, 2 * sizeof(double)));
-        cuda_alloc((void**)&ix->d_cols_table, B200_MAX_ATTRIBUTE_COLUMNS * sizeof(double*));
-        ensure_out_k(ix, 16);
-        ensure_ccap(ix, FIN_CAP);
-        ensure_capacity(ix, std::max<int64_t>(capacity_rows, TILE_N));
-        const auto smem_attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
-        for (int i = 0; i < 8; ++i) {
-            MB_CUDA(cudaFuncSetAttribute(scan_fn<false>(i), smem_attr, SMEM_LIMIT));
-            MB_CUDA(cudaFuncSetAttribute(scan_fn<true>(i), smem_attr, SMEM_LIMIT));
-        }
-        MB_CUDA(cudaFuncSetAttribute(merge_kernel, smem_attr, 64 * 1024));
-        MB_CUDA(cudaFuncSetAttribute(finalize_kernel, smem_attr, (int)finalize_smem_bytes(FIN_CAP)));
-    } catch (...) {
-        index_free(ix);
-        throw;
+    std::unique_ptr<b200_index> ix(new b200_index());   // released under the guard if the set-up fails
+    ix->device = device;
+    ix->dim = dim;
+    ix->metric = metric;
+    ix->sms = std::min(sm_count(device), MAX_LISTS);   // merge_kernel's list-head table holds MAX_LISTS lists
+    ix->own_stream = make_stream(cudaStreamNonBlocking);
+    ix->stream = ix->own_stream.get();
+    for (auto& e : ix->ev) e = make_event();
+    ix->qh = DeviceBuffer<__half>((size_t)MQ * dim);
+    ix->q_stage = DeviceBuffer<float>((size_t)MQ * dim);
+    const size_t nl = (size_t)ix->sms * MQ * KP;
+    ix->list_score = DeviceBuffer<float>(nl);
+    ix->list_row = DeviceBuffer<int32_t>(nl);
+    ix->list_doc = DeviceBuffer<int32_t>(nl);
+    ix->qs = DeviceBuffer<QState>(1);
+    MB_CUDA(cudaMemset(ix->qs.get(), 0, sizeof(QState)));
+    ix->h_qs = make_pinned<QState>();
+    ix->max_n2 = DeviceBuffer<float>(1);
+    MB_CUDA(cudaMemset(ix->max_n2.get(), 0, sizeof(float)));
+    ix->d_flags = DeviceBuffer<int>(2);
+    MB_CUDA(cudaMemset(ix->d_flags.get(), 0, 2 * sizeof(int)));
+    ix->mod_max = DeviceBuffer<double>(2);
+    MB_CUDA(cudaMemset(ix->mod_max.get(), 0, 2 * sizeof(double)));
+    ix->d_cols_table = DeviceBuffer<double*>(B200_MAX_ATTRIBUTE_COLUMNS);
+    ensure_out_k(ix.get(), 16);
+    ensure_ccap(ix.get(), FIN_CAP);
+    ensure_capacity(ix.get(), std::max<int64_t>(capacity_rows, TILE_N));
+    const auto smem_attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
+    for (int i = 0; i < 8; ++i) {
+        MB_CUDA(cudaFuncSetAttribute(scan_fn<false>(i), smem_attr, SMEM_LIMIT));
+        MB_CUDA(cudaFuncSetAttribute(scan_fn<true>(i), smem_attr, SMEM_LIMIT));
     }
-    return ix;
+    MB_CUDA(cudaFuncSetAttribute(merge_kernel, smem_attr, 64 * 1024));
+    MB_CUDA(cudaFuncSetAttribute(finalize_kernel, smem_attr, (int)finalize_smem_bytes(FIN_CAP)));
+    return ix.release();
 }
 
 // Raises B200_ERR_INVALID_ARG when the last conversion saw a non-finite / out-of-fp16-range value (needs a
 // synchronised stream).
 void check_input_flags(b200_index* ix, const char* what) {
     int flags = 0;
-    MB_CUDA(cudaMemcpyAsync(&flags, ix->d_flags, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
+    MB_CUDA(cudaMemcpyAsync(&flags, ix->d_flags.get(), sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
     MB_CUDA(cudaStreamSynchronize(ix->stream));
     if (flags & 1) {
-        MB_CUDA(cudaMemsetAsync(ix->d_flags, 0, sizeof(int), ix->stream));
+        MB_CUDA(cudaMemsetAsync(ix->d_flags.get(), 0, sizeof(int), ix->stream));
         fail(B200_ERR_INVALID_ARG,
              "%s contain a value that is not finite or does not fit the fp16 row store (|x| <= 65504 after "
              "normalisation)", what);
@@ -1414,15 +1339,16 @@ void add_rows_device(b200_index* ix, const float* d_vecs, const int32_t* d_doc_i
     const int wpb = 8;
     const int64_t blocks = (m + wpb - 1) / wpb;
     convert_rows_kernel<<<(unsigned)blocks, wpb * 32, 0, ix->stream>>>(
-        d_vecs, ix->corpus + (size_t)ix->n_rows * ix->dim, m, ix->dim, m, ix->metric == B200_METRIC_ANGULAR,
-        ix->metric == B200_METRIC_EUCLIDEAN ? ix->row_n2 + ix->n_rows : nullptr, ix->max_n2, ix->d_flags);
+        d_vecs, ix->corpus.get() + (size_t)ix->n_rows * ix->dim, m, ix->dim, m, ix->metric == B200_METRIC_ANGULAR,
+        ix->metric == B200_METRIC_EUCLIDEAN ? ix->row_n2.get() + ix->n_rows : nullptr, ix->max_n2.get(),
+        ix->d_flags.get());
     MB_CUDA(cudaGetLastError());
     if (d_doc_ids) {
-        MB_CUDA(cudaMemcpyAsync(ix->doc_of_row + ix->n_rows, d_doc_ids, (size_t)m * sizeof(int32_t),
+        MB_CUDA(cudaMemcpyAsync(ix->doc_of_row.get() + ix->n_rows, d_doc_ids, (size_t)m * sizeof(int32_t),
                                 cudaMemcpyDeviceToDevice, ix->stream));
         ix->has_docs = true;
     } else {
-        iota_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ix->stream>>>(ix->doc_of_row + ix->n_rows, m,
+        iota_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ix->stream>>>(ix->doc_of_row.get() + ix->n_rows, m,
                                                                         (int32_t)ix->n_rows);
         MB_CUDA(cudaGetLastError());
     }
@@ -1442,11 +1368,11 @@ ExactParams exact_params(b200_index* ix, int nq, int k, const GroupOut& out) {
     ex.dim = ix->dim;
     ex.metric = ix->metric;
     ex.doc_offset = ix->doc_offset;
-    ex.qh = ix->qh;
-    ex.corpus = ix->corpus;
-    ex.doc_of_row = ix->doc_of_row;
-    ex.mod64 = ix->mod_active ? ix->mod64 : nullptr;
-    ex.qs = ix->qs;
+    ex.qh = ix->qh.get();
+    ex.corpus = ix->corpus.get();
+    ex.doc_of_row = ix->doc_of_row.get();
+    ex.mod64 = ix->mod_active ? ix->mod64.get() : nullptr;
+    ex.qs = ix->qs.get();
     ex.out_doc = out.doc;
     ex.out_row = out.row;
     ex.out_score = out.score;
@@ -1470,9 +1396,9 @@ ScanLaunch prepare_scan(b200_index* ix, int nq) {
     while (stages > 2 && scan_smem_bytes(ix->dim, stages, mod) > (size_t)SMEM_LIMIT) --stages;
     L.smem = scan_smem_bytes(ix->dim, stages, mod);
     if (L.smem > (size_t)SMEM_LIMIT) fail(B200_ERR_INTERNAL, "scan kernel shared memory budget exceeded");
-    L.tmap_c = make_tmap_2d(ix->corpus, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (uint64_t)ix->dim, (uint64_t)ix->n_rows,
-                            (uint64_t)ix->dim * 2, BLOCK_K, TILE_N, CU_TENSOR_MAP_SWIZZLE_128B);
-    L.tmap_q = make_tmap_2d(ix->qh, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (uint64_t)ix->dim, (uint64_t)MQ,
+    L.tmap_c = make_tmap_2d(ix->corpus.get(), CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (uint64_t)ix->dim,
+                            (uint64_t)ix->n_rows, (uint64_t)ix->dim * 2, BLOCK_K, TILE_N, CU_TENSOR_MAP_SWIZZLE_128B);
+    L.tmap_q = make_tmap_2d(ix->qh.get(), CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (uint64_t)ix->dim, (uint64_t)MQ,
                             (uint64_t)ix->dim * 2, BLOCK_K, MQ, CU_TENSOR_MAP_SWIZZLE_128B);
     ScanParams& sp = L.sp;
     sp.n_rows = (int)ix->n_rows;
@@ -1481,16 +1407,16 @@ ScanLaunch prepare_scan(b200_index* ix, int nq) {
     sp.num_stages = stages;
     sp.nq = nq;
     sp.metric = ix->metric;
-    sp.doc_of_row = ix->doc_of_row;
-    sp.row_bias = ix->row_n2;
-    sp.mod = mod ? ix->mod32 : nullptr;
-    sp.filter = ix->filter_active ? ix->filter_bits : nullptr;
+    sp.doc_of_row = ix->doc_of_row.get();
+    sp.row_bias = ix->row_n2.get();
+    sp.mod = mod ? ix->mod32.get() : nullptr;
+    sp.filter = ix->filter_active ? ix->filter_bits.get() : nullptr;
     sp.filter_docs = ix->filter_docs;
-    sp.qs = ix->qs;
-    sp.out_score = ix->list_score;
-    sp.out_row = ix->list_row;
-    sp.out_doc = ix->list_doc;
-    sp.cbuf = ix->cbuf;
+    sp.qs = ix->qs.get();
+    sp.out_score = ix->list_score.get();
+    sp.out_row = ix->list_row.get();
+    sp.out_doc = ix->list_doc.get();
+    sp.cbuf = ix->cbuf.get();
     sp.ccap = ix->ccap;
     const bool bias = ix->metric == B200_METRIC_EUCLIDEAN;
     const bool docs = ix->has_docs || ix->filter_active;   // the filter is applied where the document numbers are read
@@ -1499,7 +1425,7 @@ ScanLaunch prepare_scan(b200_index* ix, int nq) {
 }
 
 void launch_collect(b200_index* ix, ScanLaunch& L) {
-    L.sp.cbuf = ix->cbuf;
+    L.sp.cbuf = ix->cbuf.get();
     L.sp.ccap = ix->ccap;
     scan_fn<true>(L.fn_index)<<<L.grid, THREADS, L.smem, ix->stream>>>(L.tmap_c, L.tmap_q, L.sp);
     MB_CUDA(cudaGetLastError());
@@ -1507,17 +1433,17 @@ void launch_collect(b200_index* ix, ScanLaunch& L) {
 
 void launch_finalize(b200_index* ix, int nq, int k, const GroupOut& out) {
     FinalizeParams fp{};
-    fp.cbuf = ix->cbuf;
+    fp.cbuf = ix->cbuf.get();
     fp.ccap = ix->ccap;
     fp.live_bound = ix->n_rows;
     fp.ex = exact_params(ix, nq, k, out);
-    reset_need_kernel<<<1, 1, 0, ix->stream>>>(ix->qs);
+    reset_need_kernel<<<1, 1, 0, ix->stream>>>(ix->qs.get());
     finalize_kernel<<<nq, FIN_THREADS, finalize_smem_bytes(std::min(ix->ccap, FIN_CAP)), ix->stream>>>(fp);
     MB_CUDA(cudaGetLastError());
 }
 
 void fetch_qstate(b200_index* ix) {
-    MB_CUDA(cudaMemcpyAsync(ix->h_qs, ix->qs, sizeof(QState), cudaMemcpyDeviceToHost, ix->stream));
+    MB_CUDA(cudaMemcpyAsync(ix->h_qs.get(), ix->qs.get(), sizeof(QState), cudaMemcpyDeviceToHost, ix->stream));
     MB_CUDA(cudaStreamSynchronize(ix->stream));
 }
 
@@ -1526,12 +1452,12 @@ void fetch_qstate(b200_index* ix) {
 // dedup / sort is the same rule as exact_select.  Returns true when the query is resolved.
 bool host_finalize(b200_index* ix, int q, int nq, int k, const GroupOut& out, int cnt) {
     ++ix->stat_host_finalize;
-    DevBuf d_dot((size_t)cnt * 8), d_key((size_t)cnt * 8), d_doc((size_t)cnt * 4);
+    DeviceBuffer<double> d_dot((size_t)cnt), d_key((size_t)cnt);
+    DeviceBuffer<int32_t> d_doc((size_t)cnt);
     GroupOut dummy{nullptr, nullptr, nullptr};
     ExactParams ex = exact_params(ix, nq, k, dummy);
-    const int32_t* rows = ix->cbuf + (size_t)q * ix->ccap;
-    exact_keys_kernel<<<(cnt + 7) / 8, 256, 0, ix->stream>>>(ex, q, rows, cnt, d_dot.as<double>(), d_key.as<double>(),
-                                                            d_doc.as<int32_t>());
+    const int32_t* rows = ix->cbuf.get() + (size_t)q * ix->ccap;
+    exact_keys_kernel<<<(cnt + 7) / 8, 256, 0, ix->stream>>>(ex, q, rows, cnt, d_dot.get(), d_key.get(), d_doc.get());
     MB_CUDA(cudaGetLastError());
     struct Hit {
         double dot, key;
@@ -1539,9 +1465,9 @@ bool host_finalize(b200_index* ix, int q, int nq, int k, const GroupOut& out, in
     };
     std::vector<double> h_dot(cnt), h_key(cnt);
     std::vector<int32_t> h_doc(cnt), h_row(cnt);
-    MB_CUDA(cudaMemcpyAsync(h_dot.data(), d_dot.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, ix->stream));
-    MB_CUDA(cudaMemcpyAsync(h_key.data(), d_key.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, ix->stream));
-    MB_CUDA(cudaMemcpyAsync(h_doc.data(), d_doc.p, (size_t)cnt * 4, cudaMemcpyDeviceToHost, ix->stream));
+    MB_CUDA(cudaMemcpyAsync(h_dot.data(), d_dot.get(), (size_t)cnt * 8, cudaMemcpyDeviceToHost, ix->stream));
+    MB_CUDA(cudaMemcpyAsync(h_key.data(), d_key.get(), (size_t)cnt * 8, cudaMemcpyDeviceToHost, ix->stream));
+    MB_CUDA(cudaMemcpyAsync(h_doc.data(), d_doc.get(), (size_t)cnt * 4, cudaMemcpyDeviceToHost, ix->stream));
     MB_CUDA(cudaMemcpyAsync(h_row.data(), rows, (size_t)cnt * 4, cudaMemcpyDeviceToHost, ix->stream));
     MB_CUDA(cudaStreamSynchronize(ix->stream));
     std::vector<Hit> v(cnt);
@@ -1556,7 +1482,7 @@ bool host_finalize(b200_index* ix, int q, int nq, int k, const GroupOut& out, in
     v.resize(w);
     std::sort(v.begin(), v.end(), [](const Hit& a, const Hit& b) { return a.key > b.key || (a.key == b.key && a.doc < b.doc); });
     const int nd = (int)v.size();
-    QState* h = ix->h_qs;
+    QState* h = ix->h_qs.get();
     const double L = h->L[q], eps = h->eps[q];
     double ek = -std::numeric_limits<double>::infinity();
     if (nd >= k) ek = ix->mod_active ? v[k - 1].key : (ix->metric == B200_METRIC_EUCLIDEAN ? v[k - 1].key + h->qn2x[q] : v[k - 1].key);
@@ -1596,7 +1522,7 @@ bool host_finalize(b200_index* ix, int q, int nq, int k, const GroupOut& out, in
     return resolved;
 }
 
-// One group of <= MQ queries already converted into ix->qh.
+// One group of <= MQ queries already converted into ix->qh.get().
 //   may_sync: the caller tolerates host synchronisation — flagged queries are driven to resolution here.
 //   otherwise: one collect + finalize pass is enqueued unconditionally (both exit at once when nothing is flagged);
 //   queries still unresolved after it are counted in QState::rounds (b200_index_search_stats).
@@ -1608,14 +1534,14 @@ void search_group(b200_index* ix, int nq, int k, const GroupOut& out, bool recor
         MB_CUDA(cudaGetLastError());
         return;
     }
-    query_prep_kernel<<<MQ / 8, 256, 0, ix->stream>>>(ix->qh, ix->dim, ix->metric, ix->mod_active ? 1 : 0, ix->max_n2,
-                                                     ix->mod_max, ix->qs);
+    query_prep_kernel<<<MQ / 8, 256, 0, ix->stream>>>(ix->qh.get(), ix->dim, ix->metric, ix->mod_active ? 1 : 0,
+                                                     ix->max_n2.get(), ix->mod_max.get(), ix->qs.get());
     MB_CUDA(cudaGetLastError());
     ScanLaunch L = prepare_scan(ix, nq);
-    if (record_timing) MB_CUDA(cudaEventRecord(ix->ev[0], ix->stream));
+    if (record_timing) MB_CUDA(cudaEventRecord(ix->ev[0].get(), ix->stream));
     scan_fn<false>(L.fn_index)<<<L.grid, THREADS, L.smem, ix->stream>>>(L.tmap_c, L.tmap_q, L.sp);
     MB_CUDA(cudaGetLastError());
-    if (record_timing) MB_CUDA(cudaEventRecord(ix->ev[1], ix->stream));
+    if (record_timing) MB_CUDA(cudaEventRecord(ix->ev[1].get(), ix->stream));
 
     MergeParams mp{};
     mp.num_lists = L.grid;
@@ -1623,25 +1549,25 @@ void search_group(b200_index* ix, int nq, int k, const GroupOut& out, bool recor
     while (sort_n < L.grid * KP) sort_n <<= 1;
     mp.sort_n = sort_n;
     mp.l_only = k > K_MERGE_MAX ? 1 : 0;
-    mp.in_score = ix->list_score;
-    mp.in_row = ix->list_row;
-    mp.in_doc = ix->list_doc;
+    mp.in_score = ix->list_score.get();
+    mp.in_row = ix->list_row.get();
+    mp.in_doc = ix->list_doc.get();
     mp.ex = exact_params(ix, nq, k, out);
     merge_kernel<<<nq, MERGE_THREADS, (size_t)sort_n * 12, ix->stream>>>(mp);
     MB_CUDA(cudaGetLastError());
     if (record_timing) {
-        MB_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
+        MB_CUDA(cudaEventRecord(ix->ev[2].get(), ix->stream));
         ix->timing_valid = true;
     }
     if (!may_sync) {
         launch_collect(ix, L);
         launch_finalize(ix, nq, k, out);
-        note_unresolved_kernel<<<1, 1, 0, ix->stream>>>(ix->qs);
+        note_unresolved_kernel<<<1, 1, 0, ix->stream>>>(ix->qs.get());
         MB_CUDA(cudaGetLastError());
         return;
     }
     fetch_qstate(ix);
-    QState* h = ix->h_qs;
+    QState* h = ix->h_qs.get();
     if (h->n_need == 0) return;
     ix->stat_flagged += h->n_need;
     for (int round = 0; h->n_need > 0; ++round) {
@@ -1650,7 +1576,7 @@ void search_group(b200_index* ix, int nq, int k, const GroupOut& out, bool recor
         if (round >= 12)   // stop lowering L step by step: take everything
             for (int q = 0; q < nq; ++q)
                 if (h->status[q] == Q_NEED) h->L[q] = -INFINITY;
-        MB_CUDA(cudaMemcpyAsync(ix->qs, h, sizeof(QState), cudaMemcpyHostToDevice, ix->stream));
+        MB_CUDA(cudaMemcpyAsync(ix->qs.get(), h, sizeof(QState), cudaMemcpyHostToDevice, ix->stream));
         launch_collect(ix, L);
         fetch_qstate(ix);
         int max_cnt = 0;
@@ -1681,8 +1607,9 @@ void search_group(b200_index* ix, int nq, int k, const GroupOut& out, bool recor
 }
 
 void convert_queries(b200_index* ix, const float* d_q, int g) {
-    convert_rows_kernel<<<MQ / 8, 256, 0, ix->stream>>>(d_q, ix->qh, g, ix->dim, MQ, ix->metric == B200_METRIC_ANGULAR,
-                                                        nullptr, nullptr, ix->d_flags);
+    convert_rows_kernel<<<MQ / 8, 256, 0, ix->stream>>>(d_q, ix->qh.get(), g, ix->dim, MQ,
+                                                        ix->metric == B200_METRIC_ANGULAR, nullptr, nullptr,
+                                                        ix->d_flags.get());
     MB_CUDA(cudaGetLastError());
 }
 
@@ -1722,36 +1649,36 @@ void fill_nan(b200_index* ix, double* dst, int64_t n) {
 void ensure_attr_capacity(b200_index* ix, int64_t need_docs) {
     if (need_docs <= ix->attr_cap) return;
     const int64_t cap = (int64_t)round_up((size_t)std::max<int64_t>(need_docs, ix->attr_cap + ix->attr_cap / 2), 1024);
-    for (double*& col : ix->attr_cols) {
+    for (DeviceBuffer<double>& col : ix->attr_cols) {
         if (!col) continue;
-        double* nc = nullptr;
-        cuda_alloc((void**)&nc, (size_t)cap * sizeof(double));
+        DeviceBuffer<double> nc((size_t)cap);
         if (ix->attr_cap > 0)
-            MB_CUDA(cudaMemcpyAsync(nc, col, (size_t)ix->attr_cap * sizeof(double), cudaMemcpyDeviceToDevice, ix->stream));
-        fill_nan(ix, nc + ix->attr_cap, cap - ix->attr_cap);
+            MB_CUDA(cudaMemcpyAsync(nc.get(), col.get(), (size_t)ix->attr_cap * sizeof(double),
+                                    cudaMemcpyDeviceToDevice, ix->stream));
+        fill_nan(ix, nc.get() + ix->attr_cap, cap - ix->attr_cap);
         MB_CUDA(cudaStreamSynchronize(ix->stream));
-        cudaFree(col);
-        col = nc;
+        col = std::move(nc);
     }
     ix->attr_cap = cap;
     ix->cols_table_dirty = true;
 }
 
 double* attr_column(b200_index* ix, int column) {
-    if ((int)ix->attr_cols.size() <= column) ix->attr_cols.resize(column + 1, nullptr);
-    if (!ix->attr_cols[column]) {
-        cuda_alloc((void**)&ix->attr_cols[column], (size_t)ix->attr_cap * sizeof(double));
-        fill_nan(ix, ix->attr_cols[column], ix->attr_cap);
+    if ((int)ix->attr_cols.size() <= column) ix->attr_cols.resize(column + 1);
+    DeviceBuffer<double>& col = ix->attr_cols[column];
+    if (!col) {
+        col = DeviceBuffer<double>((size_t)ix->attr_cap);
+        fill_nan(ix, col.get(), ix->attr_cap);
         ix->cols_table_dirty = true;
     }
-    return ix->attr_cols[column];
+    return col.get();
 }
 
 void sync_cols_table(b200_index* ix) {
     if (!ix->cols_table_dirty) return;
     double* table[B200_MAX_ATTRIBUTE_COLUMNS] = {nullptr};
-    for (size_t c = 0; c < ix->attr_cols.size(); ++c) table[c] = ix->attr_cols[c];
-    MB_CUDA(cudaMemcpyAsync(ix->d_cols_table, table, sizeof(table), cudaMemcpyHostToDevice, ix->stream));
+    for (size_t c = 0; c < ix->attr_cols.size(); ++c) table[c] = ix->attr_cols[c].get();
+    MB_CUDA(cudaMemcpyAsync(ix->d_cols_table.get(), table, sizeof(table), cudaMemcpyHostToDevice, ix->stream));
     MB_CUDA(cudaStreamSynchronize(ix->stream));   // `table` is a stack array
     ix->cols_table_dirty = false;
 }
@@ -1771,14 +1698,9 @@ void prepare_modifiers(b200_index* ix, const int32_t* mult_cols, const double* m
                        const int32_t* add_cols, const double* add_w, int n_add) {
     const int64_t nd = num_docs(ix);
     if (nd > ix->mod_cap) {
-        cudaFree(ix->mod64);
-        cudaFree(ix->mod32);
-        ix->mod64 = nullptr;
-        ix->mod32 = nullptr;
-        ix->mod_cap = 0;
         const int64_t cap = (int64_t)round_up((size_t)nd + (size_t)nd / 2, 1024);
-        cuda_alloc((void**)&ix->mod64, (size_t)cap * sizeof(double2));
-        cuda_alloc((void**)&ix->mod32, (size_t)cap * sizeof(float2));
+        ix->mod64 = DeviceBuffer<double2>((size_t)cap);
+        ix->mod32 = DeviceBuffer<float2>((size_t)cap);
         ix->mod_cap = cap;
     }
     if (nd == 0) return;
@@ -1789,7 +1711,8 @@ void prepare_modifiers(b200_index* ix, const int32_t* mult_cols, const double* m
     mp.n_add = n_add;
     auto col = [&](int c) -> const double* {
         MB_CHECK_ARG(c >= 0 && c < B200_MAX_ATTRIBUTE_COLUMNS, "attribute column %d out of range", c);
-        return c < (int)ix->attr_cols.size() ? ix->attr_cols[c] : nullptr;   // never-set column: missing everywhere
+        // a column that was never set is missing everywhere
+        return c < (int)ix->attr_cols.size() ? ix->attr_cols[c].get() : nullptr;
     };
     for (int i = 0; i < n_mult; ++i) {
         mp.mult_col[i] = col(mult_cols[i]);
@@ -1799,16 +1722,16 @@ void prepare_modifiers(b200_index* ix, const int32_t* mult_cols, const double* m
         mp.add_col[i] = col(add_cols[i]);
         mp.add_w[i] = add_w[i];
     }
-    mp.out64 = ix->mod64;
-    mp.out32 = ix->mod32;
-    mp.negative_flag = ix->d_flags + 1;
-    mp.mod_max = ix->mod_max;
-    MB_CUDA(cudaMemsetAsync(ix->d_flags + 1, 0, sizeof(int), ix->stream));
-    MB_CUDA(cudaMemsetAsync(ix->mod_max, 0, 2 * sizeof(double), ix->stream));
+    mp.out64 = ix->mod64.get();
+    mp.out32 = ix->mod32.get();
+    mp.negative_flag = ix->d_flags.get() + 1;
+    mp.mod_max = ix->mod_max.get();
+    MB_CUDA(cudaMemsetAsync(ix->d_flags.get() + 1, 0, sizeof(int), ix->stream));
+    MB_CUDA(cudaMemsetAsync(ix->mod_max.get(), 0, 2 * sizeof(double), ix->stream));
     modifier_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, ix->stream>>>(mp);
     MB_CUDA(cudaGetLastError());
     int flag = 0;
-    MB_CUDA(cudaMemcpyAsync(&flag, ix->d_flags + 1, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
+    MB_CUDA(cudaMemcpyAsync(&flag, ix->d_flags.get() + 1, sizeof(int), cudaMemcpyDeviceToHost, ix->stream));
     MB_CUDA(cudaStreamSynchronize(ix->stream));
     // closeness(field, embeddings) is the best chunk's closeness; the scan keeps, per document, the chunk with the best
     // MODIFIED key, which is the same chunk only while the multiplier is >= 0.
@@ -1825,16 +1748,13 @@ void prepare_filter(b200_index* ix, const uint32_t* bits, int64_t n_docs, uint64
     if (tag != 0 && tag == ix->filter_tag && n_docs == ix->filter_docs) return;
     if (words > ix->filter_cap_words) {
         MB_CUDA(cudaStreamSynchronize(ix->stream));
-        cudaFree(ix->filter_bits);
-        ix->filter_bits = nullptr;
-        ix->filter_cap_words = 0;
         ix->filter_tag = 0;
         const int64_t cap = (int64_t)round_up((size_t)words + (size_t)words / 2 + 1, 256);
-        cuda_alloc((void**)&ix->filter_bits, (size_t)cap * 4);
+        ix->filter_bits = DeviceBuffer<uint32_t>((size_t)cap);
         ix->filter_cap_words = cap;
     }
     if (words > 0)
-        MB_CUDA(cudaMemcpyAsync(ix->filter_bits, bits, (size_t)words * 4, cudaMemcpyHostToDevice, ix->stream));
+        MB_CUDA(cudaMemcpyAsync(ix->filter_bits.get(), bits, (size_t)words * 4, cudaMemcpyHostToDevice, ix->stream));
     MB_CUDA(cudaStreamSynchronize(ix->stream));   // the caller's buffer may be pageable and short-lived
     ix->filter_docs = n_docs;
     ix->filter_tag = tag;
@@ -1844,14 +1764,14 @@ void search_host(b200_index* ix, const float* q, int nq, int k, int32_t* out_doc
     ensure_out_k(ix, k);
     for (int q0 = 0; q0 < nq; q0 += MQ) {
         const int gq = std::min(MQ, nq - q0);
-        MB_CUDA(cudaMemcpyAsync(ix->q_stage, q + (size_t)q0 * ix->dim, (size_t)gq * ix->dim * sizeof(float),
+        MB_CUDA(cudaMemcpyAsync(ix->q_stage.get(), q + (size_t)q0 * ix->dim, (size_t)gq * ix->dim * sizeof(float),
                                 cudaMemcpyHostToDevice, ix->stream));
-        search_device(ix, ix->q_stage, gq, k, ix->o_doc, ix->o_row, ix->o_score, true);
-        MB_CUDA(cudaMemcpyAsync(out_doc + (size_t)q0 * k, ix->o_doc, (size_t)gq * k * sizeof(int32_t),
+        search_device(ix, ix->q_stage.get(), gq, k, ix->o_doc.get(), ix->o_row.get(), ix->o_score.get(), true);
+        MB_CUDA(cudaMemcpyAsync(out_doc + (size_t)q0 * k, ix->o_doc.get(), (size_t)gq * k * sizeof(int32_t),
                                 cudaMemcpyDeviceToHost, ix->stream));
-        MB_CUDA(cudaMemcpyAsync(out_row + (size_t)q0 * k, ix->o_row, (size_t)gq * k * sizeof(int32_t),
+        MB_CUDA(cudaMemcpyAsync(out_row + (size_t)q0 * k, ix->o_row.get(), (size_t)gq * k * sizeof(int32_t),
                                 cudaMemcpyDeviceToHost, ix->stream));
-        MB_CUDA(cudaMemcpyAsync(out_score + (size_t)q0 * k, ix->o_score, (size_t)gq * k * sizeof(double),
+        MB_CUDA(cudaMemcpyAsync(out_score + (size_t)q0 * k, ix->o_score.get(), (size_t)gq * k * sizeof(double),
                                 cudaMemcpyDeviceToHost, ix->stream));
         check_input_flags(ix, "queries");   // synchronises
     }
@@ -1868,6 +1788,21 @@ void validate_opts(const b200_search_opts* o) {
     MB_CHECK_ARG(o->filter_bits != nullptr || o->filter_docs == 0, "filter_docs > 0 with filter_bits == NULL");
 }
 
+// Runs `append` (add_rows_device calls) and checks the appended values; nothing of a rejected batch stays searchable.
+template <class F>
+void add_checked(b200_index* ix, F&& append) {
+    const int64_t rows_before = ix->n_rows;
+    const bool docs_before = ix->has_docs;
+    try {
+        append();
+        check_input_flags(ix, "embeddings");
+    } catch (...) {
+        ix->n_rows = rows_before;
+        ix->has_docs = docs_before;
+        throw;
+    }
+}
+
 }  // namespace
 
 extern "C" {
@@ -1881,7 +1816,11 @@ int b200_index_create(int device, int dim, int metric, int64_t capacity_rows, b2
 }
 
 int b200_index_destroy(b200_index* ix) {
-    return guarded([&] { index_free(ix); });
+    return guarded([&] {
+        if (!ix) return;
+        DeviceGuard g(ix->device);
+        delete ix;
+    });
 }
 
 int b200_index_add(b200_index* ix, const float* vecs, const int32_t* doc_ids, int64_t m) {
@@ -1900,27 +1839,20 @@ int b200_index_add(b200_index* ix, const float* vecs, const int32_t* doc_ids, in
                 hi = std::max<int64_t>(hi, doc_ids[i]);
             }
         const int64_t chunk = 1 << 16;
-        DevBuf d_v((size_t)std::min(m, chunk) * ix->dim * sizeof(float));
-        DevBuf d_d(doc_ids ? (size_t)std::min(m, chunk) * sizeof(int32_t) : 16);
-        const int64_t rows_before = ix->n_rows;
-        const bool docs_before = ix->has_docs;
-        try {
+        DeviceBuffer<float> d_v((size_t)std::min(m, chunk) * ix->dim);
+        DeviceBuffer<int32_t> d_d(doc_ids ? (size_t)std::min(m, chunk) : 0);
+        add_checked(ix, [&] {
             for (int64_t o = 0; o < m; o += chunk) {
                 const int64_t c = std::min(chunk, m - o);
-                MB_CUDA(cudaMemcpyAsync(d_v.p, vecs + (size_t)o * ix->dim, (size_t)c * ix->dim * sizeof(float),
+                MB_CUDA(cudaMemcpyAsync(d_v.get(), vecs + (size_t)o * ix->dim, (size_t)c * ix->dim * sizeof(float),
                                         cudaMemcpyHostToDevice, ix->stream));
                 if (doc_ids)
-                    MB_CUDA(cudaMemcpyAsync(d_d.p, doc_ids + o, (size_t)c * sizeof(int32_t), cudaMemcpyHostToDevice,
+                    MB_CUDA(cudaMemcpyAsync(d_d.get(), doc_ids + o, (size_t)c * sizeof(int32_t), cudaMemcpyHostToDevice,
                                             ix->stream));
-                add_rows_device(ix, d_v.as<float>(), doc_ids ? d_d.as<int32_t>() : nullptr, c);
+                add_rows_device(ix, d_v.get(), doc_ids ? d_d.get() : nullptr, c);
                 MB_CUDA(cudaStreamSynchronize(ix->stream));
             }
-            check_input_flags(ix, "embeddings");
-        } catch (...) {   // nothing of a rejected batch stays searchable
-            ix->n_rows = rows_before;
-            ix->has_docs = docs_before;
-            throw;
-        }
+        });
         ix->max_doc = hi;
     });
 }
@@ -1934,16 +1866,7 @@ int b200_index_add_device(b200_index* ix, const float* d_vecs, const int32_t* d_
         std::lock_guard<std::mutex> lk(ix->mu);
         DeviceGuard g(ix->device);
         MB_CHECK_ARG(ix->n_rows + m < (int64_t)INT32_MAX, "row count would exceed 2^31-1");
-        const int64_t rows_before = ix->n_rows;
-        const bool docs_before = ix->has_docs;
-        add_rows_device(ix, d_vecs, d_doc_ids, m);
-        try {
-            check_input_flags(ix, "embeddings");
-        } catch (...) {
-            ix->n_rows = rows_before;
-            ix->has_docs = docs_before;
-            throw;
-        }
+        add_checked(ix, [&] { add_rows_device(ix, d_vecs, d_doc_ids, m); });
         if (d_doc_ids) track_max_doc(ix, d_doc_ids, m);
     });
 }
@@ -1962,18 +1885,9 @@ int b200_index_add_device_docs(b200_index* ix, const float* d_vecs, const int32_
             MB_CHECK_ARG(doc_ids[i] >= 0, "doc_ids[%lld] is negative", (long long)i);
             hi = std::max<int64_t>(hi, doc_ids[i]);
         }
-        DevBuf d_d((size_t)m * sizeof(int32_t));
-        MB_CUDA(cudaMemcpyAsync(d_d.p, doc_ids, (size_t)m * sizeof(int32_t), cudaMemcpyHostToDevice, ix->stream));
-        const int64_t rows_before = ix->n_rows;
-        const bool docs_before = ix->has_docs;
-        add_rows_device(ix, d_vecs, d_d.as<int32_t>(), m);
-        try {
-            check_input_flags(ix, "embeddings");
-        } catch (...) {
-            ix->n_rows = rows_before;
-            ix->has_docs = docs_before;
-            throw;
-        }
+        DeviceBuffer<int32_t> d_d((size_t)m);
+        MB_CUDA(cudaMemcpyAsync(d_d.get(), doc_ids, (size_t)m * sizeof(int32_t), cudaMemcpyHostToDevice, ix->stream));
+        add_checked(ix, [&] { add_rows_device(ix, d_vecs, d_d.get(), m); });
         ix->max_doc = hi;
     });
 }
@@ -1984,7 +1898,7 @@ int b200_index_delete_doc(b200_index* ix, int32_t doc_id) {
         std::lock_guard<std::mutex> lk(ix->mu);
         DeviceGuard g(ix->device);
         if (ix->n_rows == 0) return;
-        tombstone_kernel<<<(unsigned)((ix->n_rows + 255) / 256), 256, 0, ix->stream>>>(ix->doc_of_row, ix->n_rows,
+        tombstone_kernel<<<(unsigned)((ix->n_rows + 255) / 256), 256, 0, ix->stream>>>(ix->doc_of_row.get(), ix->n_rows,
                                                                                       doc_id);
         MB_CUDA(cudaGetLastError());
         MB_CUDA(cudaStreamSynchronize(ix->stream));
@@ -2002,9 +1916,9 @@ int b200_index_delete_rows(b200_index* ix, const int32_t* rows, int64_t n) {
         DeviceGuard g(ix->device);
         for (int64_t i = 0; i < n; ++i)
             MB_CHECK_ARG(rows[i] >= 0 && rows[i] < ix->n_rows, "rows[%lld] = %d out of range", (long long)i, rows[i]);
-        DevBuf d_r((size_t)n * sizeof(int32_t));
-        MB_CUDA(cudaMemcpyAsync(d_r.p, rows, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, ix->stream));
-        tombstone_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ix->stream>>>(ix->doc_of_row, d_r.as<int32_t>(), n);
+        DeviceBuffer<int32_t> d_r((size_t)n);
+        MB_CUDA(cudaMemcpyAsync(d_r.get(), rows, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, ix->stream));
+        tombstone_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ix->stream>>>(ix->doc_of_row.get(), d_r.get(), n);
         MB_CUDA(cudaGetLastError());
         MB_CUDA(cudaStreamSynchronize(ix->stream));
         ix->has_docs = true;
@@ -2020,7 +1934,8 @@ int b200_index_compact(b200_index* ix, int32_t* out_new_of_old, int64_t* out_row
         const int64_t n = ix->n_rows;
         std::vector<int32_t> doc((size_t)n);
         if (n > 0) {
-            MB_CUDA(cudaMemcpyAsync(doc.data(), ix->doc_of_row, (size_t)n * 4, cudaMemcpyDeviceToHost, ix->stream));
+            MB_CUDA(cudaMemcpyAsync(doc.data(), ix->doc_of_row.get(), (size_t)n * 4, cudaMemcpyDeviceToHost,
+                                    ix->stream));
             MB_CUDA(cudaStreamSynchronize(ix->stream));
         }
         int64_t live = 0;
@@ -2031,32 +1946,17 @@ int b200_index_compact(b200_index* ix, int32_t* out_new_of_old, int64_t* out_row
             return;
         }
         const int64_t cap = (int64_t)round_up((size_t)std::max<int64_t>(live, TILE_N), TILE_N);
-        __half* nc = nullptr;
-        int32_t* nd = nullptr;
-        float* nn = nullptr;
-        DevBuf d_map((size_t)std::max<int64_t>(n, 1) * 4);
-        try {
-            cuda_alloc((void**)&nc, (size_t)cap * ix->dim * sizeof(__half));
-            cuda_alloc((void**)&nd, (size_t)cap * sizeof(int32_t));
-            if (ix->row_n2) cuda_alloc((void**)&nn, (size_t)cap * sizeof(float));
-            MB_CUDA(cudaMemcpyAsync(d_map.p, out_new_of_old, (size_t)n * 4, cudaMemcpyHostToDevice, ix->stream));
-            compact_rows_kernel<<<(unsigned)((n + 7) / 8), 256, 0, ix->stream>>>(ix->corpus, nc, ix->doc_of_row, nd,
-                                                                                ix->row_n2, nn, d_map.as<int32_t>(), n,
-                                                                                ix->dim);
-            MB_CUDA(cudaGetLastError());
-            MB_CUDA(cudaStreamSynchronize(ix->stream));
-        } catch (...) {
-            cudaFree(nc);
-            cudaFree(nd);
-            cudaFree(nn);
-            throw;
-        }
-        cudaFree(ix->corpus);
-        cudaFree(ix->doc_of_row);
-        cudaFree(ix->row_n2);
-        ix->corpus = nc;
-        ix->doc_of_row = nd;
-        ix->row_n2 = nn;
+        DeviceBuffer<int32_t> d_map((size_t)n);   // n > live >= 0
+        RowArrays r = alloc_rows(ix, cap);
+        MB_CUDA(cudaMemcpyAsync(d_map.get(), out_new_of_old, (size_t)n * 4, cudaMemcpyHostToDevice, ix->stream));
+        compact_rows_kernel<<<(unsigned)((n + 7) / 8), 256, 0, ix->stream>>>(
+            ix->corpus.get(), r.corpus.get(), ix->doc_of_row.get(), r.doc_of_row.get(), ix->row_n2.get(), r.row_n2.get(),
+            d_map.get(), n, ix->dim);
+        MB_CUDA(cudaGetLastError());
+        MB_CUDA(cudaStreamSynchronize(ix->stream));
+        ix->corpus = std::move(r.corpus);
+        ix->doc_of_row = std::move(r.doc_of_row);
+        ix->row_n2 = std::move(r.row_n2);
         ix->capacity = cap;
         ix->n_rows = live;
         ix->dead_rows = 0;
@@ -2094,7 +1994,7 @@ int b200_index_get_rows(b200_index* ix, const int64_t* rows, int64_t n, float* o
         std::vector<__half> tmp((size_t)n * ix->dim);
         for (int64_t i = 0; i < n; ++i) {
             MB_CHECK_ARG(rows[i] >= 0 && rows[i] < ix->n_rows, "row %lld out of range", (long long)rows[i]);
-            MB_CUDA(cudaMemcpyAsync(tmp.data() + (size_t)i * ix->dim, ix->corpus + (size_t)rows[i] * ix->dim,
+            MB_CUDA(cudaMemcpyAsync(tmp.data() + (size_t)i * ix->dim, ix->corpus.get() + (size_t)rows[i] * ix->dim,
                                     (size_t)ix->dim * sizeof(__half), cudaMemcpyDeviceToHost, ix->stream));
         }
         MB_CUDA(cudaStreamSynchronize(ix->stream));
@@ -2155,20 +2055,20 @@ int b200_index_set_attributes(b200_index* ix, int column, const int32_t* doc_ids
         DeviceGuard g(ix->device);
         if (column < 0 && ix->attr_cols.empty()) return;
         ensure_attr_capacity(ix, hi + 1);
-        DevBuf d_ids((size_t)n * sizeof(int32_t));
-        DevBuf d_vals(values ? (size_t)n * sizeof(double) : 16);
-        MB_CUDA(cudaMemcpyAsync(d_ids.p, doc_ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, ix->stream));
+        DeviceBuffer<int32_t> d_ids((size_t)n);
+        DeviceBuffer<double> d_vals(values ? (size_t)n : 0);
+        MB_CUDA(cudaMemcpyAsync(d_ids.get(), doc_ids, (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, ix->stream));
         if (values)
-            MB_CUDA(cudaMemcpyAsync(d_vals.p, values, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, ix->stream));
+            MB_CUDA(cudaMemcpyAsync(d_vals.get(), values, (size_t)n * sizeof(double), cudaMemcpyHostToDevice,
+                                    ix->stream));
         const unsigned blocks = (unsigned)((n + 255) / 256);
         if (column >= 0) {
-            scatter_attr_kernel<<<blocks, 256, 0, ix->stream>>>(attr_column(ix, column), d_ids.as<int32_t>(),
-                                                                values ? d_vals.as<double>() : nullptr, n);
+            scatter_attr_kernel<<<blocks, 256, 0, ix->stream>>>(attr_column(ix, column), d_ids.get(), d_vals.get(), n);
             MB_CUDA(cudaGetLastError());
         } else {
             sync_cols_table(ix);
-            clear_attr_kernel<<<blocks, 256, 0, ix->stream>>>(ix->d_cols_table, (int)ix->attr_cols.size(),
-                                                              d_ids.as<int32_t>(), n, ix->attr_cap);
+            clear_attr_kernel<<<blocks, 256, 0, ix->stream>>>(ix->d_cols_table.get(), (int)ix->attr_cols.size(),
+                                                              d_ids.get(), n, ix->attr_cap);
             MB_CUDA(cudaGetLastError());
         }
         MB_CUDA(cudaStreamSynchronize(ix->stream));
@@ -2200,12 +2100,13 @@ int b200_index_set_attributes_multi(b200_index* ix, const int32_t* columns, cons
         for (int c = 0; c <= max_col; ++c)
             if (used[c]) attr_column(ix, c);
         sync_cols_table(ix);
-        DevBuf d_cols((size_t)n * 4), d_ids((size_t)n * 4), d_vals((size_t)n * 8);
-        MB_CUDA(cudaMemcpyAsync(d_cols.p, columns, (size_t)n * 4, cudaMemcpyHostToDevice, ix->stream));
-        MB_CUDA(cudaMemcpyAsync(d_ids.p, doc_ids, (size_t)n * 4, cudaMemcpyHostToDevice, ix->stream));
-        MB_CUDA(cudaMemcpyAsync(d_vals.p, values, (size_t)n * 8, cudaMemcpyHostToDevice, ix->stream));
+        DeviceBuffer<int32_t> d_cols((size_t)n), d_ids((size_t)n);
+        DeviceBuffer<double> d_vals((size_t)n);
+        MB_CUDA(cudaMemcpyAsync(d_cols.get(), columns, (size_t)n * 4, cudaMemcpyHostToDevice, ix->stream));
+        MB_CUDA(cudaMemcpyAsync(d_ids.get(), doc_ids, (size_t)n * 4, cudaMemcpyHostToDevice, ix->stream));
+        MB_CUDA(cudaMemcpyAsync(d_vals.get(), values, (size_t)n * 8, cudaMemcpyHostToDevice, ix->stream));
         scatter_attr_multi_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ix->stream>>>(
-            ix->d_cols_table, d_cols.as<int32_t>(), d_ids.as<int32_t>(), d_vals.as<double>(), n);
+            ix->d_cols_table.get(), d_cols.get(), d_ids.get(), d_vals.get(), n);
         MB_CUDA(cudaGetLastError());
         MB_CUDA(cudaStreamSynchronize(ix->stream));
     });
@@ -2242,7 +2143,7 @@ int b200_index_set_stream(b200_index* ix, void* cuda_stream, int use_external) {
         std::lock_guard<std::mutex> lk(ix->mu);
         DeviceGuard g(ix->device);
         MB_CUDA(cudaStreamSynchronize(ix->stream));
-        ix->stream = use_external ? reinterpret_cast<cudaStream_t>(cuda_stream) : ix->own_stream;
+        ix->stream = use_external ? reinterpret_cast<cudaStream_t>(cuda_stream) : ix->own_stream.get();
     });
 }
 
@@ -2276,9 +2177,9 @@ int b200_index_last_timing(b200_index* ix, float* scan_ms, float* merge_ms) {
         std::lock_guard<std::mutex> lk(ix->mu);
         DeviceGuard g(ix->device);
         if (!ix->timing_valid) fail(B200_ERR_INVALID_ARG, "no search has been timed yet");
-        MB_CUDA(cudaEventSynchronize(ix->ev[2]));
-        MB_CUDA(cudaEventElapsedTime(scan_ms, ix->ev[0], ix->ev[1]));
-        MB_CUDA(cudaEventElapsedTime(merge_ms, ix->ev[1], ix->ev[2]));
+        MB_CUDA(cudaEventSynchronize(ix->ev[2].get()));
+        MB_CUDA(cudaEventElapsedTime(scan_ms, ix->ev[0].get(), ix->ev[1].get()));
+        MB_CUDA(cudaEventElapsedTime(merge_ms, ix->ev[1].get(), ix->ev[2].get()));
     });
 }
 
@@ -2330,13 +2231,13 @@ int b200_exchange_create(int device, int rank, int world, int max_nq, int max_k,
         ex->rank = rank;
         ex->world = world;
         ex->slot_stride = round_up((size_t)max_nq * max_k * 16, 256);
-        ex->buf_bytes = 2 * (size_t)world * ex->slot_stride + 2 * (size_t)world * sizeof(unsigned long long);
-        cuda_alloc((void**)&ex->local, ex->buf_bytes);
-        MB_CUDA(cudaMemset(ex->local, 0, ex->buf_bytes));
+        ex->local =
+            DeviceBuffer<uint8_t>(2 * (size_t)world * ex->slot_stride + 2 * (size_t)world * sizeof(unsigned long long));
+        MB_CUDA(cudaMemset(ex->local.get(), 0, ex->local.size()));
         MB_CUDA(cudaDeviceSynchronize());
-        ex->peer[rank] = ex->local;
+        ex->peer[rank] = ex->local.get();
         cudaIpcMemHandle_t h;
-        MB_CUDA(cudaIpcGetMemHandle(&h, ex->local));
+        MB_CUDA(cudaIpcGetMemHandle(&h, ex->local.get()));
         static_assert(sizeof(cudaIpcMemHandle_t) == B200_EXCHANGE_HANDLE_BYTES, "handle size");
         memcpy(out_handle, &h, sizeof(h));
         *out = ex.release();
@@ -2349,13 +2250,11 @@ int b200_exchange_open(b200_exchange* ex, const void* handles) {
         DeviceGuard g(ex->device);
         const uint8_t* hp = reinterpret_cast<const uint8_t*>(handles);
         for (int s = 0; s < ex->world; ++s) {
-            if (s == ex->rank || ex->opened[s]) continue;
+            if (s == ex->rank || ex->mapped[s]) continue;
             cudaIpcMemHandle_t h;
             memcpy(&h, hp + (size_t)s * B200_EXCHANGE_HANDLE_BYTES, sizeof(h));
-            void* p = nullptr;
-            MB_CUDA(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-            ex->peer[s] = reinterpret_cast<uint8_t*>(p);
-            ex->opened[s] = true;
+            ex->mapped[s] = open_ipc_mapping(h);
+            ex->peer[s] = ex->mapped[s].get();
         }
     });
 }
@@ -2363,11 +2262,8 @@ int b200_exchange_open(b200_exchange* ex, const void* handles) {
 int b200_exchange_destroy(b200_exchange* ex) {
     return guarded([&] {
         if (!ex) return;
-        cudaSetDevice(ex->device);
+        DeviceGuard g(ex->device);
         cudaDeviceSynchronize();
-        for (int s = 0; s < ex->world; ++s)
-            if (ex->opened[s]) cudaIpcCloseMemHandle(ex->peer[s]);
-        cudaFree(ex->local);
         delete ex;
     });
 }
@@ -2452,15 +2348,15 @@ int b200_index_save(b200_index* ix, const char* path) {
         };
         try {
             MB_CUDA(cudaStreamSynchronize(ix->stream));
-            dump(ix->corpus, (size_t)ix->n_rows * ix->dim * sizeof(__half));
-            dump(ix->doc_of_row, (size_t)ix->n_rows * sizeof(int32_t));
+            dump(ix->corpus.get(), (size_t)ix->n_rows * ix->dim * sizeof(__half));
+            dump(ix->doc_of_row.get(), (size_t)ix->n_rows * sizeof(int32_t));
             // trailer: score-modifier attribute columns
             const int64_t trailer[3] = {ix->max_doc, ix->attr_cap, (int64_t)ix->attr_cols.size()};
             ok = ok && fwrite(trailer, sizeof(trailer), 1, f.get()) == 1;
-            for (double* col : ix->attr_cols) {
+            for (const DeviceBuffer<double>& col : ix->attr_cols) {
                 const int32_t present = col ? 1 : 0;
                 ok = ok && fwrite(&present, sizeof(present), 1, f.get()) == 1;
-                if (col) dump(col, (size_t)ix->attr_cap * sizeof(double));
+                if (col) dump(col.get(), (size_t)ix->attr_cap * sizeof(double));
             }
             ok = ok && fflush(f.get()) == 0;
         } catch (...) {
@@ -2488,55 +2384,52 @@ int b200_index_load(int device, const char* path, b200_index** out) {
         std::unique_ptr<FILE, FileCloser> f(fopen(path, "rb"));
         if (!f) fail(B200_ERR_INVALID_ARG, "cannot open %s", path);
         SnapshotHeader hdr;
-        b200_index* ix = nullptr;
-        try {
-            if (fread(&hdr, sizeof(hdr), 1, f.get()) != 1 || memcmp(hdr.magic, "B200IDX\0", 8) != 0 ||
-                (hdr.version != 1 && hdr.version != 2))
-                fail(B200_ERR_INVALID_ARG, "%s is not a marqo_b200 index snapshot", path);
-            ix = index_new(device, hdr.dim, hdr.metric, hdr.n_rows);
-            DeviceGuard g(device);
-            std::vector<uint8_t> buf((size_t)1 << 24);
-            auto slurp = [&](void* dptr, size_t bytes) {
-                for (size_t o = 0; o < bytes; o += buf.size()) {
-                    const size_t c = std::min(buf.size(), bytes - o);
-                    if (fread(buf.data(), 1, c, f.get()) != c) fail(B200_ERR_INVALID_ARG, "%s is truncated", path);
-                    MB_CUDA(cudaMemcpy((uint8_t*)dptr + o, buf.data(), c, cudaMemcpyHostToDevice));
-                }
-            };
-            slurp(ix->corpus, (size_t)hdr.n_rows * hdr.dim * sizeof(__half));
-            slurp(ix->doc_of_row, (size_t)hdr.n_rows * sizeof(int32_t));
-            ix->n_rows = hdr.n_rows;
-            ix->has_docs = hdr.has_docs != 0;
-            if (hdr.version >= 2) {
-                int64_t trailer[3];
-                if (fread(trailer, sizeof(trailer), 1, f.get()) != 1) fail(B200_ERR_INVALID_ARG, "%s is truncated", path);
-                MB_CHECK_ARG(trailer[2] >= 0 && trailer[2] <= B200_MAX_ATTRIBUTE_COLUMNS && trailer[1] >= 0,
-                             "%s has a corrupt attribute trailer", path);
-                ix->max_doc = trailer[0];
-                ix->attr_cap = trailer[1];
-                ix->attr_cols.assign((size_t)trailer[2], nullptr);
-                for (size_t c = 0; c < ix->attr_cols.size(); ++c) {
-                    int32_t present = 0;
-                    if (fread(&present, sizeof(present), 1, f.get()) != 1) fail(B200_ERR_INVALID_ARG, "%s is truncated", path);
-                    if (!present) continue;
-                    cuda_alloc((void**)&ix->attr_cols[c], (size_t)ix->attr_cap * sizeof(double));
-                    slurp(ix->attr_cols[c], (size_t)ix->attr_cap * sizeof(double));
-                }
-                ix->cols_table_dirty = true;
-            } else if (ix->has_docs && hdr.n_rows > 0) {
-                track_max_doc(ix, ix->doc_of_row, hdr.n_rows);
+        if (fread(&hdr, sizeof(hdr), 1, f.get()) != 1 || memcmp(hdr.magic, "B200IDX\0", 8) != 0 ||
+            (hdr.version != 1 && hdr.version != 2))
+            fail(B200_ERR_INVALID_ARG, "%s is not a marqo_b200 index snapshot", path);
+        require_sm90_device(device);
+        DeviceGuard g(device);
+        std::unique_ptr<b200_index> owner(index_new(device, hdr.dim, hdr.metric, hdr.n_rows));   // freed under the guard
+        b200_index* ix = owner.get();
+        std::vector<uint8_t> buf((size_t)1 << 24);
+        auto slurp = [&](void* dptr, size_t bytes) {
+            for (size_t o = 0; o < bytes; o += buf.size()) {
+                const size_t c = std::min(buf.size(), bytes - o);
+                if (fread(buf.data(), 1, c, f.get()) != c) fail(B200_ERR_INVALID_ARG, "%s is truncated", path);
+                MB_CUDA(cudaMemcpy((uint8_t*)dptr + o, buf.data(), c, cudaMemcpyHostToDevice));
             }
-            if (hdr.n_rows > 0) {   // per-row norms (euclidean) and the largest norm (error bound of the scan)
-                row_norms_kernel<<<(unsigned)((hdr.n_rows + 7) / 8), 256, 0, ix->stream>>>(
-                    ix->corpus, hdr.n_rows, hdr.dim, ix->metric == B200_METRIC_EUCLIDEAN ? ix->row_n2 : nullptr, ix->max_n2);
-                MB_CUDA(cudaGetLastError());
-                MB_CUDA(cudaStreamSynchronize(ix->stream));
+        };
+        slurp(ix->corpus.get(), (size_t)hdr.n_rows * hdr.dim * sizeof(__half));
+        slurp(ix->doc_of_row.get(), (size_t)hdr.n_rows * sizeof(int32_t));
+        ix->n_rows = hdr.n_rows;
+        ix->has_docs = hdr.has_docs != 0;
+        if (hdr.version >= 2) {
+            int64_t trailer[3];
+            if (fread(trailer, sizeof(trailer), 1, f.get()) != 1) fail(B200_ERR_INVALID_ARG, "%s is truncated", path);
+            MB_CHECK_ARG(trailer[2] >= 0 && trailer[2] <= B200_MAX_ATTRIBUTE_COLUMNS && trailer[1] >= 0,
+                         "%s has a corrupt attribute trailer", path);
+            ix->max_doc = trailer[0];
+            ix->attr_cap = trailer[1];
+            ix->attr_cols.resize((size_t)trailer[2]);
+            for (DeviceBuffer<double>& col : ix->attr_cols) {
+                int32_t present = 0;
+                if (fread(&present, sizeof(present), 1, f.get()) != 1) fail(B200_ERR_INVALID_ARG, "%s is truncated", path);
+                if (!present) continue;
+                col = DeviceBuffer<double>((size_t)ix->attr_cap);
+                slurp(col.get(), (size_t)ix->attr_cap * sizeof(double));
             }
-        } catch (...) {
-            index_free(ix);
-            throw;
+            ix->cols_table_dirty = true;
+        } else if (ix->has_docs && hdr.n_rows > 0) {
+            track_max_doc(ix, ix->doc_of_row.get(), hdr.n_rows);
         }
-        *out = ix;
+        if (hdr.n_rows > 0) {   // per-row norms (euclidean) and the largest norm (error bound of the scan)
+            row_norms_kernel<<<(unsigned)((hdr.n_rows + 7) / 8), 256, 0, ix->stream>>>(
+                ix->corpus.get(), hdr.n_rows, hdr.dim, ix->metric == B200_METRIC_EUCLIDEAN ? ix->row_n2.get() : nullptr,
+                ix->max_n2.get());
+            MB_CUDA(cudaGetLastError());
+            MB_CUDA(cudaStreamSynchronize(ix->stream));
+        }
+        *out = owner.release();
     });
 }
 
