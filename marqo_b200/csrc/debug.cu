@@ -38,15 +38,21 @@ __global__ void bf16_to_f32_kernel(const __nv_bfloat16* src, float* dst, long lo
     if (i < n) dst[i] = __bfloat162float(src[i]);
 }
 
-// pseudo-random bf16 values in [-1, 1) (kernel timing probes: no 200 MB host upload)
-__global__ void fill_bf16_kernel(__nv_bfloat16* dst, long long n, uint32_t seed) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+// pseudo-random values in [-1, 1) (kernel timing probes: no 200 MB host upload)
+__device__ __forceinline__ float fill_value(long long i, uint32_t seed) {
     uint32_t x = (uint32_t)i * 2654435761u + seed;
     x ^= x >> 16;
     x *= 0x85ebca6bu;
     x ^= x >> 13;
-    dst[i] = __float2bfloat16_rn((float)(x & 0xFFFF) / 32768.0f - 1.0f);
+    return (float)(x & 0xFFFF) / 32768.0f - 1.0f;
+}
+__global__ void fill_bf16_kernel(__nv_bfloat16* dst, long long n, uint32_t seed) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) dst[i] = __float2bfloat16_rn(fill_value(i, seed));
+}
+__global__ void fill_f32_kernel(float* dst, long long n, uint32_t seed) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) dst[i] = fill_value(i, seed);
 }
 
 void require_device(int device) {
@@ -182,6 +188,87 @@ int b200_debug_gemm(int device, const float* A, const float* W, const float* bia
         MB_CUDA(cudaGetLastError());
         MB_CUDA(cudaStreamSynchronize(sc.s));
         MB_CUDA(cudaMemcpy(out, dOut, (size_t)M * N * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int b200_debug_gemm_into(int device, const float* A, const float* W, const float* bias, int M, int N, int K, int act,
+                         int act_fp32, int out_bf16, int residual_in_place, int out_rows, int ldo, float* io) {
+    return guarded([&] {
+        MB_CHECK_ARG(A && W && io, "NULL buffer");
+        MB_CHECK_ARG(M > 0 && N > 0 && K > 0 && out_rows >= M && ldo >= N, "bad shape");
+        MB_CHECK_ARG(!(residual_in_place && out_bf16), "the in-place residual is fp32");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        __nv_bfloat16* dA = sc.upload_bf16(A, (size_t)M * K);
+        __nv_bfloat16* dW = sc.upload_bf16(W, (size_t)N * K);
+        const size_t n = (size_t)out_rows * ldo;
+        float* dIo = sc.upload(io, n);
+        __nv_bfloat16* dIoB = out_bf16 ? sc.upload_bf16(io, n) : nullptr;
+        gemm::Epilogue ep;
+        ep.bias = bias ? sc.upload(bias, (size_t)N) : nullptr;
+        ep.act = act;
+        ep.act_fp32 = act_fp32;
+        ep.out = out_bf16 ? static_cast<void*>(dIoB) : static_cast<void*>(dIo);
+        ep.ldo = ldo;
+        ep.out_fp32 = out_bf16 ? 0 : 1;
+        if (residual_in_place) {   // as the encoder layers update the fp32 residual stream: residual == out
+            ep.residual = dIo;
+            ep.ldr = ldo;
+        }
+        gemm::launch(dA, K, dW, M, N, K, ep, sm_count(device), sc.s);
+        if (out_bf16) bf16_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, sc.s>>>(dIoB, dIo, (long long)n);
+        MB_CUDA(cudaGetLastError());
+        MB_CUDA(cudaStreamSynchronize(sc.s));
+        MB_CUDA(cudaMemcpy(io, dIo, n * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16, int has_bias, int residual_in_place,
+                         int iters, float* out_ms) {
+    return guarded([&] {
+        MB_CHECK_ARG(out_ms != nullptr, "NULL buffer");
+        MB_CHECK_ARG(M > 0 && N > 0 && K > 0 && iters > 0, "M, N, K, iters must be positive");
+        MB_CHECK_ARG(!(residual_in_place && out_bf16), "the in-place residual is fp32");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        __nv_bfloat16* dA = sc.alloc<__nv_bfloat16>((size_t)M * K);
+        __nv_bfloat16* dW = sc.alloc<__nv_bfloat16>((size_t)N * K);
+        const long long na = (long long)M * K, nw = (long long)N * K, no = (long long)M * N;
+        fill_bf16_kernel<<<(unsigned)((na + 255) / 256), 256, 0, sc.s>>>(dA, na, 12345u);
+        fill_bf16_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, sc.s>>>(dW, nw, 777u);
+        gemm::Epilogue ep;
+        ep.act = act;
+        ep.ldo = N;
+        if (has_bias) {
+            float* dBias = sc.alloc<float>((size_t)N);
+            fill_f32_kernel<<<(unsigned)((N + 255) / 256), 256, 0, sc.s>>>(dBias, N, 99u);
+            ep.bias = dBias;
+        }
+        if (out_bf16) {
+            ep.out = sc.alloc<__nv_bfloat16>((size_t)no);
+        } else {
+            float* dOut = sc.alloc<float>((size_t)no);
+            fill_f32_kernel<<<(unsigned)((no + 255) / 256), 256, 0, sc.s>>>(dOut, no, 4242u);
+            ep.out = dOut;
+            ep.out_fp32 = 1;
+            if (residual_in_place) {   // residual == out, as run_clip_blocks updates x
+                ep.residual = dOut;
+                ep.ldr = N;
+            }
+        }
+        MB_CUDA(cudaGetLastError());
+        const int sms = sm_count(device);
+        UniqueEvent e0 = make_event(), e1 = make_event();
+        for (int i = 0; i < 3; ++i) gemm::launch(dA, K, dW, M, N, K, ep, sms, sc.s);   // warm-up
+        MB_CUDA(cudaEventRecord(e0.get(), sc.s));
+        for (int i = 0; i < iters; ++i) gemm::launch(dA, K, dW, M, N, K, ep, sms, sc.s);
+        MB_CUDA(cudaEventRecord(e1.get(), sc.s));
+        MB_CUDA(cudaStreamSynchronize(sc.s));
+        float ms = 0.f;
+        MB_CUDA(cudaEventElapsedTime(&ms, e0.get(), e1.get()));
+        *out_ms = ms / (float)iters;
     });
 }
 

@@ -9,11 +9,22 @@ namespace gemm {
 
 // Warp-specialised wgmma GEMM.  One CTA computes a BM x BN = 128 x 128 tile:
 //   warps 0-7   two MMA warpgroups, 64 rows of the tile each (wgmma m64n128k16, fp32 accumulators in registers), then
-//               the epilogue straight from those registers (bias, activation, positional embedding, residual, store);
+//               the epilogue (bias, activation, residual) on those registers;
 //   warps 8..   the producer: one warp issuing TMA loads of A and W k-blocks (128B swizzle) into a STAGES-deep smem ring,
 //               or, for the ViT patch embedding (GATHER), four warps that build the A stage from the uint8 image while
 //               one of them still loads W by TMA.
 // Two CTAs share an SM (3 x 32 KB stages each), so one CTA's epilogue overlaps the other's main loop.
+//
+// Epilogues (chosen on the host, a template parameter):
+//   STAGED     every GEMM whose output rows are the A rows.  Warpgroup wg's 64 x 128 block of the output goes through
+//              one ring stage, the one of virtual k-block kblocks + wg: the producer takes that stage through the usual
+//              empty/full protocol once the main loop has released it (k-block kblocks + wg - 3), and fills it with
+//              the fp32 residual rows by TMA when there is a residual, so the load overlaps the last MMAs.  The MMA
+//              threads write act(acc + bias) (+ residual) over it, and one thread per warpgroup stores the block by
+//              TMA, which clips it at M and N.  The bias columns are read once per CTA into shared memory.
+//   register   the ViT token scatter (remap_group > 0: patch embed, gather kernel or im2col): GEMM row r goes to token
+//              row b (G + 1) + 1 + i, so the 64 rows of a warpgroup are not one contiguous output block; each thread
+//              stores its fragments from registers.
 constexpr int BM = 128;
 constexpr int BN = 128;
 constexpr int BK = 64;
@@ -23,7 +34,14 @@ constexpr int MMA_THREADS = 256;
 constexpr uint32_t A_STAGE_BYTES = BM * BK * 2;
 constexpr uint32_t B_STAGE_BYTES = BN * BK * 2;
 constexpr uint32_t STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+constexpr uint32_t BARRIER_BYTES = 256;
+constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + BARRIER_BYTES + 2 * BN * 4 /*bias*/;
+// Staged epilogue: a warpgroup's 64 output rows as 128-byte-wide TMA boxes with the 128B swizzle, 8 KB each, one
+// after the other in its stage: fp32 -> 4 boxes of 32 columns (the residual arrives in the same layout), bf16 -> 2
+// boxes of 64 columns.
+constexpr int EPI_ROWS = BM / 2;
+constexpr uint32_t EPI_BOX_BYTES = EPI_ROWS * 128;
+static_assert(4 * EPI_BOX_BYTES == STAGE_BYTES, "a warpgroup's fp32 64 x 128 block is one ring stage");
 
 template <bool GATHER>
 constexpr int threads() { return MMA_THREADS + (GATHER ? 128 : 32); }
@@ -109,13 +127,35 @@ __device__ __forceinline__ uint32_t sw128_offset(int row, int unit) {
     return (uint32_t)row * 128u + (uint32_t)((unit ^ (row & 7)) << 4);
 }
 
-template <bool GATHER>
+// Offset of element (row, col) of a warpgroup's staged 64 x 128 block (EPI_BOX_BYTES boxes of 128 / ELEM columns).  A
+// warp's store of one fragment (8 rows x 4 column pairs) touches 8 different 16-byte units per row phase: no bank
+// conflicts.
+template <int ELEM>
+__device__ __forceinline__ uint32_t epi_offset(int row, int col) {
+    constexpr int BOX_COLS = 128 / ELEM;
+    const int byte = (col % BOX_COLS) * ELEM;
+    return (uint32_t)(col / BOX_COLS) * EPI_BOX_BYTES + sw128_offset(row, byte >> 4) + (uint32_t)(byte & 15);
+}
+
+// Named barrier over the 128 threads of MMA warpgroup wg (ids 1 and 2; 0 is __syncthreads).
+__device__ __forceinline__ void warpgroup_sync(int wg) {
+    if (wg == 0)
+        ptx::bar_sync<1, 128>();
+    else
+        ptx::bar_sync<2, 128>();
+}
+
+// tmap_r / tmap_o (STAGED only): the fp32 residual and the output, boxes of EPI_ROWS rows x 128 bytes.
+template <bool GATHER, bool STAGED>
 __global__ void __launch_bounds__(threads<GATHER>(), GATHER ? 1 : 2)
-gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, Params p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+            const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_o, Params p) {
+    static_assert(!(GATHER && STAGED), "the patch embed scatters token rows: register epilogue");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * STAGE_BYTES);
     uint64_t* empty = full + STAGES;
+    float* bias_s = reinterpret_cast<float*>(smem + (size_t)STAGES * STAGE_BYTES + BARRIER_BYTES);   // [2][BN]
 
     const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
     const int lane = threadIdx.x & 31;
@@ -126,6 +166,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     if (threadIdx.x == MMA_THREADS) {
         ptx::prefetch_tmap(&tmap_b);
         if (!GATHER) ptx::prefetch_tmap(&tmap_a);
+        if (STAGED) {
+            ptx::prefetch_tmap(&tmap_o);
+            if (p.ep.residual) ptx::prefetch_tmap(&tmap_r);
+        }
         for (int i = 0; i < STAGES; ++i) {
             ptx::mbar_init(&full[i], GATHER ? 1 + 128 : 1);
             ptx::mbar_init(&empty[i], MMA_THREADS / 32);
@@ -185,11 +229,32 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                 ptx::mbar_arrive(&full[stage]);
             }
         }
+        if (STAGED) {
+            // virtual k-blocks kblocks, kblocks + 1: the epilogue stages of warpgroups 0 and 1, with their residual rows
+            for (int wg = 0; wg < 2; ++wg) {
+                const int kb = kblocks + wg;
+                const int stage = kb % STAGES;
+                uint8_t* s = smem + (size_t)stage * STAGE_BYTES;
+                ptx::mbar_wait(&empty[stage], ((uint32_t)(kb / STAGES) & 1u) ^ 1);
+                if (pt != 0) continue;   // full[] counts one producer arrival
+                // Residual boxes that overlap [0, M) x [0, N); the others are never stored.  A box that straddles M
+                // is zero-filled past it and still counts all its bytes.
+                const int row0 = m0 + EPI_ROWS * wg;
+                const int boxes = p.ep.residual != nullptr && row0 < p.M ? min(4, (p.N - n0) / 32) : 0;
+                ptx::mbar_arrive_expect_tx(&full[stage], (uint32_t)boxes * EPI_BOX_BYTES);
+                for (int b = 0; b < boxes; ++b)
+                    ptx::tma_load_2d(s + b * EPI_BOX_BYTES, &tmap_r, &full[stage], n0 + 32 * b, row0, ptx::kEvictNormal);
+            }
+        }
         return;
     }
 
     // ---------------------------------------------------------------- MMA warpgroups
     const int wg = warp >> 2;
+    const Epilogue& ep = p.ep;
+    // STAGED: thread t of the warpgroup fetches bias column n0 + t now; the load completes under the main loop
+    float bias_t = 0.f;
+    if (STAGED && ep.bias != nullptr && n0 + (int)(threadIdx.x & 127) < p.N) bias_t = __ldg(ep.bias + n0 + (threadIdx.x & 127));
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -209,62 +274,99 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     }
     ptx::wgmma_wait<0>();
 
-    // ---------------------------------------------------------------- epilogue from registers
-    const Epilogue& ep = p.ep;
-    const int rbase = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    // bf16 output without residual or token scatter (QKV, fc1): erf-GELU on packed fp16 pairs (see gelu_erf_h2)
-    const bool half_gelu = ep.act == ACT_GELU && !ep.act_fp32 && !ep.out_fp32 && ep.residual == nullptr &&
-                           ep.rowbias == nullptr && ep.remap_group == 0;
-    long long orow[2];
-    bool rok[2];
+    if constexpr (STAGED) {
+        // ------------------------------------------------------------ epilogue staged in shared memory, TMA store
+        const int t = threadIdx.x & 127;
+        float* wbias = bias_s + wg * BN;
+        wbias[t] = bias_t;
+        const int kb = kblocks + wg;
+        ptx::mbar_wait(&full[kb % STAGES], (uint32_t)(kb / STAGES) & 1u);   // the stage is ours, the residual in it
+        uint8_t* tile = smem + (size_t)(kb % STAGES) * STAGE_BYTES;
+        warpgroup_sync(wg);   // wbias complete
+        const int rbase = (warp & 3) * 16 + (lane >> 2);   // row inside the warpgroup's 64
+        // bf16 output (QKV, fc1): erf-GELU on packed fp16 pairs (see gelu_erf_h2)
+        const bool half_gelu = ep.act == ACT_GELU && !ep.act_fp32 && !ep.out_fp32;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int r = rbase + 8 * h;
-        rok[h] = r < p.M;
-        orow[h] = r;
-        if (ep.remap_group > 0) {
-            const int b = r / ep.remap_group;
-            orow[h] = (long long)b * (ep.remap_group + 1) + 1 + (r - b * ep.remap_group);
+        for (int i = 0; i < BN / 8; ++i) {
+            const int col = 8 * i + 2 * (lane & 3);
+            const float2 bv = *reinterpret_cast<const float2*>(wbias + col);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = rbase + 8 * h;
+                float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
+                if (half_gelu) {
+                    const float2 y = __half22float2(gelu_erf_h2(__floats2half2_rn(x0, x1)));
+                    *reinterpret_cast<uint32_t*>(tile + epi_offset<2>(r, col)) = pack_bf16x2(y.x, y.y);
+                    continue;
+                }
+                if (ep.act == ACT_GELU) {
+                    x0 = gelu_erf(x0);
+                    x1 = gelu_erf(x1);
+                } else if (ep.act == ACT_QUICKGELU) {
+                    x0 = quick_gelu(x0);
+                    x1 = quick_gelu(x1);
+                }
+                if (ep.out_fp32) {
+                    float2* dst = reinterpret_cast<float2*>(tile + epi_offset<4>(r, col));
+                    if (ep.residual) {   // in the stage already, where the result goes
+                        const float2 rv = *dst;
+                        x0 += rv.x;
+                        x1 += rv.y;
+                    }
+                    *dst = make_float2(x0, x1);
+                } else {
+                    *reinterpret_cast<uint32_t*>(tile + epi_offset<2>(r, col)) = pack_bf16x2(x0, x1);
+                }
+            }
         }
-    }
-#pragma unroll
-    for (int i = 0; i < BN / 8; ++i) {
-        const int col = n0 + 8 * i + 2 * (lane & 3);
-        if (col >= p.N) continue;   // N % 32 == 0: col + 1 < N as well
-        float2 bv = make_float2(0.f, 0.f);
-        if (ep.bias) bv = __ldg(reinterpret_cast<const float2*>(ep.bias + col));
+        ptx::fence_proxy_async_smem();   // generic-proxy stores -> visible to the TMA store
+        warpgroup_sync(wg);
+        const int row0 = m0 + EPI_ROWS * wg;
+        if (t == 0 && row0 < p.M) {
+            const int box_cols = ep.out_fp32 ? 32 : 64;
+            for (int b = 0; b * box_cols < BN && n0 + b * box_cols < p.N; ++b)
+                ptx::tma_store_2d(&tmap_o, tile + b * EPI_BOX_BYTES, n0 + b * box_cols, row0);
+            ptx::tma_store_commit();
+            ptx::tma_store_wait_read<0>();   // the stage must outlive the store's reads of it
+        }
+    } else {
+        // ------------------------------------------------------------ token scatter from registers (fp32 output)
+        const int rbase = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        long long orow[2];
+        bool rok[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            if (!rok[h]) continue;
             const int r = rbase + 8 * h;
-            float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
-            if (half_gelu) {
-                const float2 y = __half22float2(gelu_erf_h2(__floats2half2_rn(x0, x1)));
-                *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(ep.out) + orow[h] * ep.ldo + col) =
-                    pack_bf16x2(y.x, y.y);
-                continue;
-            }
-            if (ep.act == ACT_GELU) {
-                x0 = gelu_erf(x0);
-                x1 = gelu_erf(x1);
-            } else if (ep.act == ACT_QUICKGELU) {
-                x0 = quick_gelu(x0);
-                x1 = quick_gelu(x1);
-            }
-            if (ep.rowbias) {   // ViT patch-embed: positional embedding of this row's patch
-                const float2 pb = __ldg(reinterpret_cast<const float2*>(ep.rowbias + (size_t)(1 + r % ep.remap_group) * p.N + col));
-                x0 += pb.x;
-                x1 += pb.y;
-            }
-            if (ep.residual) {
-                const float2 rv = *reinterpret_cast<const float2*>(ep.residual + (size_t)r * ep.ldr + col);
-                x0 += rv.x;
-                x1 += rv.y;
-            }
-            if (ep.out_fp32)
+            const int b = r / ep.remap_group;
+            rok[h] = r < p.M;
+            orow[h] = (long long)b * (ep.remap_group + 1) + 1 + (r - b * ep.remap_group);
+        }
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) {
+            const int col = n0 + 8 * i + 2 * (lane & 3);
+            if (col >= p.N) continue;   // N % 32 == 0: col + 1 < N as well
+            float2 bv = make_float2(0.f, 0.f);
+            if (ep.bias) bv = __ldg(reinterpret_cast<const float2*>(ep.bias + col));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (!rok[h]) continue;
+                const int r = rbase + 8 * h;
+                float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
+                if (ep.act == ACT_GELU) {
+                    x0 = gelu_erf(x0);
+                    x1 = gelu_erf(x1);
+                } else if (ep.act == ACT_QUICKGELU) {
+                    x0 = quick_gelu(x0);
+                    x1 = quick_gelu(x1);
+                }
+                if (ep.rowbias) {   // ViT patch-embed: positional embedding of this row's patch
+                    const float2 pb =
+                        __ldg(reinterpret_cast<const float2*>(ep.rowbias + (size_t)(1 + r % ep.remap_group) * p.N + col));
+                    x0 += pb.x;
+                    x1 += pb.y;
+                }
                 *reinterpret_cast<float2*>(static_cast<float*>(ep.out) + orow[h] * ep.ldo + col) = make_float2(x0, x1);
-            else
-                *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(ep.out) + orow[h] * ep.ldo + col) = pack_bf16x2(x0, x1);
+            }
         }
     }
 }
@@ -273,12 +375,13 @@ void configure() {
     static std::once_flag once;
     std::call_once(once, [] {
         const auto attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
-        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false>, attr, (int)SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<true>, attr, (int)SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, true>, attr, (int)SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, false>, attr, (int)SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<true, false>, attr, (int)SMEM_BYTES));
     });
 }
 
-template <bool GATHER>
+template <bool GATHER, bool STAGED>
 static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep,
                          cudaStream_t stream, const PatchGather* pg = nullptr) {
     Params p{};
@@ -301,13 +404,24 @@ static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W
     p.ep = ep;
     const long long tiles = (long long)((M + BM - 1) / BM) * p.tiles_n;
     if (tiles > 0x7fffffffLL) fail(B200_ERR_UNSUPPORTED, "gemm: %lld tiles is too many", tiles);
-    // (GATHER has no A matrix: the A map is a second, unused view of W so the kernel signature stays the same)
+    // (GATHER has no A matrix, and the register epilogue no residual or output map: those maps are further, unused views
+    // of W so the kernel signature stays the same)
     CUtensorMap tb = make_tmap_2d(W, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)K, (uint64_t)N, (uint64_t)K * 2, BK, BN,
                                   CU_TENSOR_MAP_SWIZZLE_128B);
     CUtensorMap ta = GATHER ? tb
                             : make_tmap_2d(A, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)K, (uint64_t)M,
                                            (uint64_t)lda * 2, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);
-    gemm_kernel<GATHER><<<(unsigned)tiles, threads<GATHER>(), SMEM_BYTES, stream>>>(ta, tb, p);
+    CUtensorMap tr = tb, to = tb;
+    if (STAGED) {
+        if (ep.residual)
+            tr = make_tmap_2d(ep.residual, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
+                              (uint64_t)ep.ldr * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
+        to = ep.out_fp32 ? make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
+                                        (uint64_t)ep.ldo * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B)
+                         : make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)N, (uint64_t)M,
+                                        (uint64_t)ep.ldo * 2, 64, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
+    }
+    gemm_kernel<GATHER, STAGED><<<(unsigned)tiles, threads<GATHER>(), SMEM_BYTES, stream>>>(ta, tb, tr, to, p);
     MB_CUDA(cudaGetLastError());
 }
 
@@ -322,12 +436,13 @@ void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, c
     if (!patch_gather_supported(pg.S, pg.patch))
         fail(B200_ERR_INTERNAL, "patch gather: image %d / patch %d is not supported", pg.S, pg.patch);
     if (N % 32 != 0 || ep.ldo % 8 != 0) fail(B200_ERR_INTERNAL, "patch gather: N = %d, ldo = %d", N, ep.ldo);
-    if (ep.residual != nullptr || !ep.out_fp32) fail(B200_ERR_INTERNAL, "patch gather: fp32 output without residual only");
+    if (ep.remap_group <= 0 || ep.residual != nullptr || !ep.out_fp32)
+        fail(B200_ERR_INTERNAL, "patch gather: token scatter to fp32 output without residual only");
     configure();
     const int g = pg.S / pg.patch;
     const long long M = (long long)pg.n * g * g;
     if (M > 0x7fffffffLL) fail(B200_ERR_INVALID_ARG, "patch gather: batch of %d images is too large", pg.n);
-    launch_tiles<true>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
+    launch_tiles<true, false>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
 }
 
 void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep, int sms,
@@ -337,9 +452,21 @@ void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int 
     if (K <= 0 || K % BK != 0) fail(B200_ERR_INTERNAL, "gemm: K = %d must be a positive multiple of %d", K, BK);
     if (N % 32 != 0) fail(B200_ERR_INTERNAL, "gemm: N = %d must be a multiple of 32", N);
     if (lda % 8 != 0 || ep.ldo % 8 != 0) fail(B200_ERR_INTERNAL, "gemm: leading dimensions must be multiples of 8");
-    if (ep.residual != nullptr && ep.ldr % 2 != 0) fail(B200_ERR_INTERNAL, "gemm: residual leading dimension must be even");
+    if (ep.remap_group > 0) {
+        if (ep.residual != nullptr || !ep.out_fp32)
+            fail(B200_ERR_INTERNAL, "gemm: token scatter to fp32 output without residual only");
+        configure();
+        launch_tiles<false, false>(A, lda, W, M, N, K, ep, stream);
+        return;
+    }
+    // TMA: 16-byte aligned bases and row pitches
+    if ((reinterpret_cast<uintptr_t>(ep.out) & 15) != 0) fail(B200_ERR_INTERNAL, "gemm: output not 16-byte aligned");
+    if (ep.rowbias != nullptr) fail(B200_ERR_INTERNAL, "gemm: the positional bias goes with the token scatter");
+    if (ep.residual != nullptr &&
+        (!ep.out_fp32 || ep.ldr % 4 != 0 || (reinterpret_cast<uintptr_t>(ep.residual) & 15) != 0))
+        fail(B200_ERR_INTERNAL, "gemm: the residual needs an fp32 output, ldr %% 4 == 0 and 16-byte alignment");
     configure();
-    launch_tiles<false>(A, lda, W, M, N, K, ep, stream);
+    launch_tiles<false, true>(A, lda, W, M, N, K, ep, stream);
 }
 
 }  // namespace gemm

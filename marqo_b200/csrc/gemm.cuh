@@ -1,6 +1,8 @@
 // Warp-specialised wgmma GEMM:  out[M,N] = epilogue( A[M,K] (bf16, K-major) x W[N,K]^T (bf16, K-major) )
-// 128 x 128 tiles, TMA-fed 128B-swizzled smem ring, two MMA warpgroups with fp32 accumulators in registers and the
-// epilogue applied straight from those registers (gemm.cu).
+// 128 x 128 tiles, TMA-fed 128B-swizzled smem ring, two MMA warpgroups with fp32 accumulators in registers.  The
+// epilogue stages each warpgroup's output block in a ring stage (the fp32 residual TMA-loaded into it ahead of time)
+// and writes it with TMA stores; only the ViT token scatter (remap_group > 0) stores from registers (gemm.cu).
+// Output and residual must be 16-byte aligned; a residual needs an fp32 output and ldr % 4 == 0.
 #pragma once
 #include "common.cuh"
 
