@@ -25,6 +25,21 @@ namespace gemm {
 //   register   the ViT token scatter (remap_group > 0: patch embed, gather kernel or im2col): GEMM row r goes to token
 //              row b (G + 1) + 1 + i, so the 64 rows of a warpgroup are not one contiguous output block; each thread
 //              stores its fragments from registers.
+//
+// gemm_persistent_kernel: GEMMs with K >= 1024, N % 256 == 0 and at least one full wave of tiles (the ViT-L-14
+// layers).  128 x 256 tiles on a persistent grid, one CTA per SM walking the tiles t = blockIdx.x + i * gridDim.x,
+// m-major (tile_m = t / tiles_n), so the W columns in use stay in L2.  384 threads:
+//   warpgroup 0     the producer: one thread issues the TMA loads into a 3-stage ring of 48 KB; the warpgroup gives its
+//                   registers to the MMA warpgroups (setmaxnreg 40).
+//   warpgroups 1-2  wgmma m64n256k16 on 64 rows each (128 accumulators per thread, setmaxnreg 232), then the STAGED
+//                   epilogue arithmetic through the warpgroup's own EPI_BYTES shared-memory buffer, stored by TMA.
+//   The ring position `it` is one running counter over every k-block of every tile of the CTA, in the producer and in
+//   the MMA warpgroups alike (stage it % 3, phase (it / 3) & 1); it never restarts for a new tile, so the producer runs
+//   on into the next tile's k-blocks while the MMA warpgroups are in the epilogue.
+//   Per 64-wide k-block a 128 x 256 tile moves 48 KB of TMA writes and 80 KB of wgmma reads through shared memory for
+//   4.2 MFLOP, against 32 + 48 KB per 2.1 MFLOP for 128 x 128: its main loop alone runs QKV at 793 TFLOP/s where the
+//   same kernel with 128 x 128 tiles reaches 576 (DESIGN.md §7.5c).  With one CTA per SM nothing covers its epilogue,
+//   so it pays only where a tile has enough k-blocks; launch() picks it for K >= 1024 and whole 256-wide column tiles.
 constexpr int BM = 128;
 constexpr int BN = 128;
 constexpr int BK = 64;
@@ -43,12 +58,25 @@ constexpr int EPI_ROWS = BM / 2;
 constexpr uint32_t EPI_BOX_BYTES = EPI_ROWS * 128;
 static_assert(4 * EPI_BOX_BYTES == STAGE_BYTES, "a warpgroup's fp32 64 x 128 block is one ring stage");
 
+// gemm_persistent_kernel: ring, two epilogue buffers (a warpgroup's bf16 64 x 256 block, or one 128-column half of its
+// fp32 block), bias [2][P_BN], barriers
+constexpr int P_BN = 256;
+constexpr int P_STAGES = 3;
+constexpr uint32_t P_STAGE_BYTES = A_STAGE_BYTES + P_BN * BK * 2;
+constexpr uint32_t P_RING_BYTES = P_STAGES * P_STAGE_BYTES;
+constexpr uint32_t EPI_BYTES = 4 * EPI_BOX_BYTES;
+constexpr int PERSISTENT_THREADS = 128 + MMA_THREADS;
+constexpr int ACT_GELU_H2 = 3;   // the persistent kernel's ACT for erf-GELU on packed fp16 pairs (gelu_erf_h2)
+constexpr size_t P_SMEM_BYTES = 1024 /*align*/ + P_RING_BYTES + 2 * EPI_BYTES + 2 * P_BN * 4 + BARRIER_BYTES;
+static_assert(P_SMEM_BYTES <= 227 * 1024, "over the opt-in shared memory of an H100 CTA");
+static_assert(P_BN * 2 * EPI_ROWS == EPI_BYTES, "a warpgroup's bf16 64 x 256 block is one epilogue buffer");
+
 template <bool GATHER>
 constexpr int threads() { return MMA_THREADS + (GATHER ? 128 : 32); }
 
 struct Params {
     int M, N, K;
-    int tiles_n;
+    int tiles_m, tiles_n;
     Epilogue ep;
     // GATHER only: uint8 HWC images [n, S, S, 3]; A row r = patch r (image r / (g*g), then row-major in the grid).
     // k index of the A row = dy * (64 * kbpd) + dx * 3 + c (kernels::patch_weight_rows lays W out the same way).
@@ -371,6 +399,226 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     }
 }
 
+// tmap_r / tmap_o: the fp32 residual (an unused view when there is none) and the output, boxes of EPI_ROWS rows x 128
+// bytes.
+//
+// The epilogue buffer of MMA warpgroup wg is written by three parties, in this order for every use:
+//   1. the TMA store of the previous use reads it: issued by thread 0 of the warpgroup (the only thread that stores
+//      from it), which is therefore the one that waits for those reads (cp.async.bulk.wait_group.read 0);
+//   2. then, with a residual, thread 0 TMA-loads the residual columns of this use into it, completing on epi_full[wg];
+//   3. then the 128 threads write act(acc + bias) (+ residual) over it: they wait on epi_full[wg] (residual) or on a
+//      warpgroup barrier that thread 0 reaches only after step 1 (no residual); fence.proxy.async and a warpgroup
+//      barrier order their writes before thread 0 issues the store of this use.
+// Thread 0 waits for the previous tile's last store after it has issued the first k-block of the new tile, so the
+// store overlaps the main loop, and the first residual load goes out then too, from L2 (the CTA prefetched the
+// tile's second residual half together with its first half).  An fp32 block of P_BN = 256 columns is 64 KB, twice the
+// buffer: it goes in two 128-column uses, and the second waits for the first's store inside the epilogue.
+// Running in place (residual == out) is safe: the residual rows and columns a tile reads are the ones it writes, and
+// no other tile touches them.
+// OUT_FP32 and ACT (ACT_NONE, ACT_GELU, ACT_QUICKGELU, or ACT_GELU_H2: erf-GELU on packed fp16 pairs for a bf16
+// output) are template parameters so that each instantiation holds only the epilogue it runs: the epilogue is unrolled
+// over the 128 accumulators, and with every variant behind runtime branches the kernel was 218 KB of code, which each
+// tile's epilogue fetched into a cold instruction cache while the tensor cores idled.
+template <bool OUT_FP32, int ACT>
+__global__ void __launch_bounds__(PERSISTENT_THREADS, 1)
+gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_o, Params p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* epi_s = smem + P_RING_BYTES;                                // [2][EPI_BYTES]
+    float* bias_s = reinterpret_cast<float*>(epi_s + 2 * EPI_BYTES);      // [2][P_BN]
+    uint64_t* full = reinterpret_cast<uint64_t*>(bias_s + 2 * P_BN);
+    uint64_t* empty = full + P_STAGES;
+    uint64_t* epi_full = empty + P_STAGES;                                  // [2]
+
+    const int tiles = p.tiles_m * p.tiles_n;
+    const int kblocks = p.K / BK;
+    const Epilogue& ep = p.ep;
+    const bool has_res = ep.residual != nullptr;
+
+    if (threadIdx.x == 0) {
+        ptx::prefetch_tmap(&tmap_a);
+        ptx::prefetch_tmap(&tmap_b);
+        ptx::prefetch_tmap(&tmap_o);
+        if (has_res) ptx::prefetch_tmap(&tmap_r);
+        for (int i = 0; i < P_STAGES; ++i) {
+            ptx::mbar_init(&full[i], 1);
+            ptx::mbar_init(&empty[i], MMA_THREADS / 32);
+        }
+        ptx::mbar_init(&epi_full[0], 1);
+        ptx::mbar_init(&epi_full[1], 1);
+        ptx::fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (threadIdx.x < 128) {
+        // ------------------------------------------------------------ producer
+        ptx::setmaxnreg_dec<40>();
+        if (threadIdx.x != 0) return;
+        uint32_t it = 0;
+        for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+            const int m0 = (tile / p.tiles_n) * BM, n0 = (tile % p.tiles_n) * P_BN;
+            for (int kb = 0; kb < kblocks; ++kb, ++it) {
+                const int stage = it % P_STAGES;
+                uint8_t* sa = smem + (size_t)stage * P_STAGE_BYTES;
+                ptx::mbar_wait(&empty[stage], ((it / P_STAGES) & 1u) ^ 1);
+                ptx::mbar_arrive_expect_tx(&full[stage], P_STAGE_BYTES);
+                ptx::tma_load_2d(sa, &tmap_a, &full[stage], kb * BK, m0, ptx::kEvictNormal);
+                ptx::tma_load_2d(sa + A_STAGE_BYTES, &tmap_b, &full[stage], kb * BK, n0, ptx::kEvictLast);
+            }
+        }
+        return;
+    }
+
+    // ---------------------------------------------------------------- MMA warpgroups
+    ptx::setmaxnreg_inc<232>();
+    const int wg = (threadIdx.x >> 7) - 1;
+    const int t = threadIdx.x & 127;
+    const int warp = t >> 5, lane = t & 31;
+    uint8_t* buf = epi_s + wg * EPI_BYTES;
+    float* wbias = bias_s + wg * P_BN;
+    const uint32_t buf_s = ptx::smem_u32(buf), wbias_s = ptx::smem_u32(wbias);
+    const int rbase = warp * 16 + (lane >> 2);   // row inside the warpgroup's 64
+    static_assert(!(OUT_FP32 && ACT == ACT_GELU_H2), "packed fp16 GELU is for bf16 outputs");
+    constexpr int HALVES = P_BN / 128;   // 128-column uses of the buffer by an fp32 block
+    uint32_t it = 0, epi_phase = 0;
+
+    // thread 0: residual columns [c0, c0 + 128) of rows row0.. into the buffer (boxes past N are never stored)
+    auto load_residual = [&](int row0, int c0) {
+        const int boxes = row0 < p.M && c0 < p.N ? min(4, (p.N - c0) / 32) : 0;
+        ptx::mbar_arrive_expect_tx(&epi_full[wg], (uint32_t)boxes * EPI_BOX_BYTES);
+        for (int b = 0; b < boxes; ++b)
+            ptx::tma_load_2d(buf + b * EPI_BOX_BYTES, &tmap_r, &epi_full[wg], c0 + 32 * b, row0, ptx::kEvictNormal);
+    };
+
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const int m0 = (tile / p.tiles_n) * BM, n0 = (tile % p.tiles_n) * P_BN;
+        const int row0 = m0 + EPI_ROWS * wg;
+        // thread t fetches bias columns n0 + t + 128 j now; the loads complete under the main loop
+        float bias_r[P_BN / 128];
+#pragma unroll
+        for (int j = 0; j < P_BN / 128; ++j) {
+            const int c = n0 + t + 128 * j;
+            bias_r[j] = ep.bias != nullptr && c < p.N ? __ldg(ep.bias + c) : 0.f;
+        }
+        float acc[P_BN / 2];
+#pragma unroll
+        for (int i = 0; i < P_BN / 2; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < kblocks; ++kb, ++it) {
+            const int stage = it % P_STAGES;
+            ptx::mbar_wait(&full[stage], (it / P_STAGES) & 1u);
+            const uint32_t a_base = ptx::smem_u32(smem + (size_t)stage * P_STAGE_BYTES) + wg * (64 * 128);
+            const uint32_t b_base = ptx::smem_u32(smem + (size_t)stage * P_STAGE_BYTES + A_STAGE_BYTES);
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / WG_K; ++k) {
+                const uint64_t da = ptx::make_desc_k_sw128(a_base + k * WG_K * 2);
+                const uint64_t db = ptx::make_desc_k_sw128(b_base + k * WG_K * 2);
+                ptx::wgmma_m64n256k16_bf16(acc, da, db, (kb | k) != 0 ? 1u : 0u);
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<1>();   // the previous k-block's MMAs are done: its stage goes back to the producer
+            if (kb > 0 && lane == 0) ptx::mbar_arrive(&empty[(it - 1) % P_STAGES]);
+            if (kb == 0 && t == 0) {
+                ptx::tma_store_wait_read<0>();   // the previous tile's last store has read the buffer
+                if (has_res) {
+                    load_residual(row0, n0);
+                    if (row0 < p.M)
+                        for (int b = 0; b < 4 && n0 + 128 + 32 * b < p.N; ++b)
+                            ptx::tma_prefetch_l2_2d(&tmap_r, n0 + 128 + 32 * b, row0);
+                }
+            }
+        }
+        ptx::wgmma_wait<0>();
+        if (lane == 0) ptx::mbar_arrive(&empty[(it - 1) % P_STAGES]);
+
+        // ------------------------------------------------------------ epilogue through the buffer, TMA store
+#pragma unroll
+        for (int j = 0; j < P_BN / 128; ++j) wbias[t + 128 * j] = bias_r[j];
+        warpgroup_sync(wg);   // wbias complete; without a residual, the buffer is free (thread 0 waited above)
+        if constexpr (!OUT_FP32) {
+#pragma unroll
+            for (int i = 0; i < P_BN / 8; ++i) {
+                const int col = 8 * i + 2 * (lane & 3);
+                const float2 bv = ptx::ld_shared_f32x2(wbias_s + 4 * col);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = rbase + 8 * h;
+                    float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
+                    if constexpr (ACT == ACT_GELU_H2) {
+                        const float2 y = __half22float2(gelu_erf_h2(__floats2half2_rn(x0, x1)));
+                        x0 = y.x;
+                        x1 = y.y;
+                    } else if constexpr (ACT == ACT_GELU) {
+                        x0 = gelu_erf(x0);
+                        x1 = gelu_erf(x1);
+                    } else if constexpr (ACT == ACT_QUICKGELU) {
+                        x0 = quick_gelu(x0);
+                        x1 = quick_gelu(x1);
+                    }
+                    ptx::st_shared_u32(buf_s + epi_offset<2>(r, col), pack_bf16x2(x0, x1));
+                }
+            }
+            ptx::fence_proxy_async_smem();   // generic-proxy stores -> visible to the TMA store
+            warpgroup_sync(wg);
+            if (t == 0 && row0 < p.M) {
+                for (int b = 0; b < P_BN / 64 && n0 + 64 * b < p.N; ++b)
+                    ptx::tma_store_2d(&tmap_o, buf + b * EPI_BOX_BYTES, n0 + 64 * b, row0);
+                ptx::tma_store_commit();
+            }
+        } else {
+#pragma unroll
+            for (int hf = 0; hf < HALVES; ++hf) {
+                if (hf > 0) {   // the buffer holds half hf - 1 until its store has read it
+                    if (t == 0) {
+                        ptx::tma_store_wait_read<0>();
+                        if (has_res) load_residual(row0, n0 + 128 * hf);
+                    }
+                    if (!has_res) warpgroup_sync(wg);
+                }
+                if (has_res) {
+                    ptx::mbar_wait(&epi_full[wg], epi_phase);
+                    epi_phase ^= 1;
+                }
+#pragma unroll
+                for (int i = 0; i < 16; ++i) {
+                    const int col = 8 * i + 2 * (lane & 3);   // inside the half
+                    const int ai = 4 * (16 * hf + i);
+                    const float2 bv = ptx::ld_shared_f32x2(wbias_s + 4 * (128 * hf + col));
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int r = rbase + 8 * h;
+                        float x0 = acc[ai + 2 * h] + bv.x, x1 = acc[ai + 2 * h + 1] + bv.y;
+                        if constexpr (ACT == ACT_GELU) {
+                            x0 = gelu_erf(x0);
+                            x1 = gelu_erf(x1);
+                        } else if constexpr (ACT == ACT_QUICKGELU) {
+                            x0 = quick_gelu(x0);
+                            x1 = quick_gelu(x1);
+                        }
+                        const uint32_t dst = buf_s + epi_offset<4>(r, col);
+                        if (has_res) {   // in the buffer already, where the result goes
+                            const float2 rv = ptx::ld_shared_f32x2(dst);
+                            x0 += rv.x;
+                            x1 += rv.y;
+                        }
+                        ptx::st_shared_f32x2(dst, x0, x1);
+                    }
+                }
+                ptx::fence_proxy_async_smem();
+                warpgroup_sync(wg);
+                const int c0 = n0 + 128 * hf;
+                if (t == 0 && row0 < p.M && c0 < p.N) {
+                    for (int b = 0; b < 4 && c0 + 32 * b < p.N; ++b)
+                        ptx::tma_store_2d(&tmap_o, buf + b * EPI_BOX_BYTES, c0 + 32 * b, row0);
+                    ptx::tma_store_commit();
+                }
+            }
+        }
+    }
+    if (t == 0) ptx::tma_store_wait_read<0>();   // shared memory must outlive the last store's reads of it
+}
+
 void configure() {
     static std::once_flag once;
     std::call_once(once, [] {
@@ -378,6 +626,13 @@ void configure() {
         MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, true>, attr, (int)SMEM_BYTES));
         MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, false>, attr, (int)SMEM_BYTES));
         MB_CUDA(cudaFuncSetAttribute(gemm_kernel<true, false>, attr, (int)SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<false, ACT_NONE>, attr, (int)P_SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<false, ACT_GELU>, attr, (int)P_SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<false, ACT_QUICKGELU>, attr, (int)P_SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<false, ACT_GELU_H2>, attr, (int)P_SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<true, ACT_NONE>, attr, (int)P_SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<true, ACT_GELU>, attr, (int)P_SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<true, ACT_QUICKGELU>, attr, (int)P_SMEM_BYTES));
     });
 }
 
@@ -425,6 +680,57 @@ static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W
     MB_CUDA(cudaGetLastError());
 }
 
+template <bool OUT_FP32, int ACT>
+static void launch_persistent(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K,
+                              const Epilogue& ep, int sms, cudaStream_t stream) {
+    Params p{};
+    p.M = M;
+    p.N = N;
+    p.K = K;
+    p.tiles_m = (M + BM - 1) / BM;
+    p.tiles_n = (N + P_BN - 1) / P_BN;
+    p.ep = ep;
+    const long long tiles = (long long)p.tiles_m * p.tiles_n;
+    if (tiles > 0x7fffffffLL) fail(B200_ERR_UNSUPPORTED, "gemm: %lld tiles is too many", tiles);
+    CUtensorMap ta = make_tmap_2d(A, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2,
+                                  BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);
+    CUtensorMap tb = make_tmap_2d(W, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)K, (uint64_t)N, (uint64_t)K * 2, BK,
+                                  P_BN, CU_TENSOR_MAP_SWIZZLE_128B);
+    // (without a residual its map is a further, unused view of W so the kernel signature stays the same)
+    CUtensorMap tr = ep.residual ? make_tmap_2d(ep.residual, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
+                                                (uint64_t)ep.ldr * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B)
+                                 : tb;
+    CUtensorMap to = ep.out_fp32 ? make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
+                                                (uint64_t)ep.ldo * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B)
+                                 : make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)N, (uint64_t)M,
+                                                (uint64_t)ep.ldo * 2, 64, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
+    const int grid = (int)std::min<long long>(tiles, std::max(sms, 1));
+    gemm_persistent_kernel<OUT_FP32, ACT><<<grid, PERSISTENT_THREADS, P_SMEM_BYTES, stream>>>(ta, tb, tr, to, p);
+    MB_CUDA(cudaGetLastError());
+}
+
+static void launch_persistent(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K,
+                              const Epilogue& ep, int sms, cudaStream_t stream) {
+    const int act = ep.act == ACT_GELU && !ep.act_fp32 && !ep.out_fp32 ? ACT_GELU_H2 : ep.act;
+    if (ep.out_fp32) {
+        if (act == ACT_GELU)
+            launch_persistent<true, ACT_GELU>(A, lda, W, M, N, K, ep, sms, stream);
+        else if (act == ACT_QUICKGELU)
+            launch_persistent<true, ACT_QUICKGELU>(A, lda, W, M, N, K, ep, sms, stream);
+        else
+            launch_persistent<true, ACT_NONE>(A, lda, W, M, N, K, ep, sms, stream);
+    } else {
+        if (act == ACT_GELU_H2)
+            launch_persistent<false, ACT_GELU_H2>(A, lda, W, M, N, K, ep, sms, stream);
+        else if (act == ACT_GELU)
+            launch_persistent<false, ACT_GELU>(A, lda, W, M, N, K, ep, sms, stream);
+        else if (act == ACT_QUICKGELU)
+            launch_persistent<false, ACT_QUICKGELU>(A, lda, W, M, N, K, ep, sms, stream);
+        else
+            launch_persistent<false, ACT_NONE>(A, lda, W, M, N, K, ep, sms, stream);
+    }
+}
+
 bool patch_gather_supported(int S, int patch) {
     return S > 0 && patch > 0 && S % patch == 0;
 }
@@ -447,7 +753,6 @@ void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, c
 
 void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep, int sms,
             cudaStream_t stream) {
-    (void)sms;
     if (M <= 0 || N <= 0) return;
     if (K <= 0 || K % BK != 0) fail(B200_ERR_INTERNAL, "gemm: K = %d must be a positive multiple of %d", K, BK);
     if (N % 32 != 0) fail(B200_ERR_INTERNAL, "gemm: N = %d must be a multiple of 32", N);
@@ -466,7 +771,14 @@ void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int 
         (!ep.out_fp32 || ep.ldr % 4 != 0 || (reinterpret_cast<uintptr_t>(ep.residual) & 15) != 0))
         fail(B200_ERR_INTERNAL, "gemm: the residual needs an fp32 output, ldr %% 4 == 0 and 16-byte alignment");
     configure();
-    launch_tiles<false, true>(A, lda, W, M, N, K, ep, stream);
+    // The persistent kernel's main loop is faster, but its epilogue is not overlapped: it pays with enough k-blocks per
+    // tile (all four ViT-L-14 layer GEMMs, K >= 1024), at least one full wave of tiles, and no half-empty 256-wide
+    // column tile (the 384-wide BERTs run slower with one; DESIGN.md §7.5c).
+    const long long tiles256 = (long long)((M + BM - 1) / BM) * (N / P_BN);
+    if (K >= 1024 && N % P_BN == 0 && tiles256 >= sms)
+        launch_persistent(A, lda, W, M, N, K, ep, sms, stream);
+    else
+        launch_tiles<false, true>(A, lda, W, M, N, K, ep, stream);
 }
 
 }  // namespace gemm

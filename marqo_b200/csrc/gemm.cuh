@@ -1,7 +1,9 @@
 // Warp-specialised wgmma GEMM:  out[M,N] = epilogue( A[M,K] (bf16, K-major) x W[N,K]^T (bf16, K-major) )
 // 128 x 128 tiles, TMA-fed 128B-swizzled smem ring, two MMA warpgroups with fp32 accumulators in registers.  The
 // epilogue stages each warpgroup's output block in a ring stage (the fp32 residual TMA-loaded into it ahead of time)
-// and writes it with TMA stores; only the ViT token scatter (remap_group > 0) stores from registers (gemm.cu).
+// and writes it with TMA stores; only the ViT token scatter (remap_group > 0) stores from registers.  For K >= 1024,
+// N % 256 == 0 and at least one full wave of tiles, a persistent kernel of 128 x 256 tiles (one CTA per SM) runs instead, with
+// the same epilogue arithmetic through a shared-memory buffer of its own (gemm.cu).
 // Output and residual must be 16-byte aligned; a residual needs an fp32 output and ldr % 4 == 0.
 #pragma once
 #include "common.cuh"
