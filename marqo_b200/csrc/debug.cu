@@ -192,7 +192,7 @@ int b200_debug_gemm(int device, const float* A, const float* W, const float* bia
 }
 
 int b200_debug_gemm_into(int device, const float* A, const float* W, const float* bias, int M, int N, int K, int act,
-                         int act_fp32, int out_bf16, int residual_in_place, int out_rows, int ldo, float* io) {
+                         int out_bf16, int residual_in_place, int out_rows, int ldo, float* io) {
     return guarded([&] {
         MB_CHECK_ARG(A && W && io, "NULL buffer");
         MB_CHECK_ARG(M > 0 && N > 0 && K > 0 && out_rows >= M && ldo >= N, "bad shape");
@@ -208,7 +208,6 @@ int b200_debug_gemm_into(int device, const float* A, const float* W, const float
         gemm::Epilogue ep;
         ep.bias = bias ? sc.upload(bias, (size_t)N) : nullptr;
         ep.act = act;
-        ep.act_fp32 = act_fp32;
         ep.out = out_bf16 ? static_cast<void*>(dIoB) : static_cast<void*>(dIo);
         ep.ldo = ldo;
         ep.out_fp32 = out_bf16 ? 0 : 1;

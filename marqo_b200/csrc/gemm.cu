@@ -1,30 +1,37 @@
 #include "gemm.cuh"
 
 #include <mutex>
+#include <type_traits>
 
 #include "ptx.cuh"
 
 namespace mb {
 namespace gemm {
 
-// Warp-specialised wgmma GEMM.  One CTA computes a BM x BN = 128 x 128 tile:
+// Two warp-specialised wgmma GEMM kernels share one STAGED epilogue: a warpgroup's 64-row output block goes through
+// shared memory as 128-byte-wide TMA boxes with the 128B swizzle (the fp32 residual TMA-loaded into the same boxes
+// beforehand), the MMA threads write act(acc + bias) (+ residual) over it (epilogue_to_smem), and one thread per
+// warpgroup stores the boxes by TMA, which clips them at M and N.  The output type and the activation are template
+// parameters of both kernels, so each instantiation holds only the epilogue it runs; the host maps an Epilogue to its
+// instantiation in one place (dispatch).
+//
+// gemm_kernel: one CTA computes a BM x BN = 128 x 128 tile:
 //   warps 0-7   two MMA warpgroups, 64 rows of the tile each (wgmma m64n128k16, fp32 accumulators in registers), then
-//               the epilogue (bias, activation, residual) on those registers;
+//               the epilogue;
 //   warps 8..   the producer: one warp issuing TMA loads of A and W k-blocks (128B swizzle) into a STAGES-deep smem ring,
 //               or, for the ViT patch embedding (GATHER), four warps that build the A stage from the uint8 image while
 //               one of them still loads W by TMA.
 // Two CTAs share an SM (3 x 32 KB stages each), so one CTA's epilogue overlaps the other's main loop.
 //
-// Epilogues (chosen on the host, a template parameter):
+// Its epilogues (chosen on the host, a template parameter):
 //   STAGED     every GEMM whose output rows are the A rows.  Warpgroup wg's 64 x 128 block of the output goes through
 //              one ring stage, the one of virtual k-block kblocks + wg: the producer takes that stage through the usual
 //              empty/full protocol once the main loop has released it (k-block kblocks + wg - 3), and fills it with
-//              the fp32 residual rows by TMA when there is a residual, so the load overlaps the last MMAs.  The MMA
-//              threads write act(acc + bias) (+ residual) over it, and one thread per warpgroup stores the block by
-//              TMA, which clips it at M and N.  The bias columns are read once per CTA into shared memory.
+//              the fp32 residual rows by TMA when there is a residual, so the load overlaps the last MMAs.  The bias
+//              columns are read once per CTA into shared memory.
 //   register   the ViT token scatter (remap_group > 0: patch embed, gather kernel or im2col): GEMM row r goes to token
 //              row b (G + 1) + 1 + i, so the 64 rows of a warpgroup are not one contiguous output block; each thread
-//              stores its fragments from registers.
+//              adds the positional embedding and stores its fp32 fragments from registers.  No bias, no activation.
 //
 // gemm_persistent_kernel: GEMMs with K >= 1024, N % 256 == 0 and at least one full wave of tiles (the ViT-L-14
 // layers).  128 x 256 tiles on a persistent grid, one CTA per SM walking the tiles t = blockIdx.x + i * gridDim.x,
@@ -32,7 +39,7 @@ namespace gemm {
 //   warpgroup 0     the producer: one thread issues the TMA loads into a 3-stage ring of 48 KB; the warpgroup gives its
 //                   registers to the MMA warpgroups (setmaxnreg 40).
 //   warpgroups 1-2  wgmma m64n256k16 on 64 rows each (128 accumulators per thread, setmaxnreg 232), then the STAGED
-//                   epilogue arithmetic through the warpgroup's own EPI_BYTES shared-memory buffer, stored by TMA.
+//                   epilogue through the warpgroup's own EPI_BYTES shared-memory buffer.
 //   The ring position `it` is one running counter over every k-block of every tile of the CTA, in the producer and in
 //   the MMA warpgroups alike (stage it % 3, phase (it / 3) & 1); it never restarts for a new tile, so the producer runs
 //   on into the next tile's k-blocks while the MMA warpgroups are in the epilogue.
@@ -66,7 +73,6 @@ constexpr uint32_t P_STAGE_BYTES = A_STAGE_BYTES + P_BN * BK * 2;
 constexpr uint32_t P_RING_BYTES = P_STAGES * P_STAGE_BYTES;
 constexpr uint32_t EPI_BYTES = 4 * EPI_BOX_BYTES;
 constexpr int PERSISTENT_THREADS = 128 + MMA_THREADS;
-constexpr int ACT_GELU_H2 = 3;   // the persistent kernel's ACT for erf-GELU on packed fp16 pairs (gelu_erf_h2)
 constexpr size_t P_SMEM_BYTES = 1024 /*align*/ + P_RING_BYTES + 2 * EPI_BYTES + 2 * P_BN * 4 + BARRIER_BYTES;
 static_assert(P_SMEM_BYTES <= 227 * 1024, "over the opt-in shared memory of an H100 CTA");
 static_assert(P_BN * 2 * EPI_ROWS == EPI_BYTES, "a warpgroup's bf16 64 x 256 block is one epilogue buffer");
@@ -173,12 +179,81 @@ __device__ __forceinline__ void warpgroup_sync(int wg) {
         ptx::bar_sync<2, 128>();
 }
 
-// tmap_r / tmap_o (STAGED only): the fp32 residual and the output, boxes of EPI_ROWS rows x 128 bytes.
-template <bool GATHER, bool STAGED>
+// The activation of an adjacent column pair.  A bf16 output (QKV, fc1) evaluates erf-GELU on packed fp16 pairs (see
+// gelu_erf_h2), an fp32 output in fp32.
+template <bool OUT_FP32, int ACT>
+__device__ __forceinline__ float2 act(float x0, float x1) {
+    if constexpr (ACT == ACT_GELU && !OUT_FP32)
+        return __half22float2(gelu_erf_h2(__floats2half2_rn(x0, x1)));
+    else if constexpr (ACT == ACT_GELU)
+        return make_float2(gelu_erf(x0), gelu_erf(x1));
+    else if constexpr (ACT == ACT_QUICKGELU)
+        return make_float2(quick_gelu(x0), quick_gelu(x1));
+    else
+        return make_float2(x0, x1);
+}
+
+// The STAGED epilogue of COLS output columns of a warpgroup's 64 rows, held in acc[0, COLS / 2) (fragment i: columns
+// 8 i + 2 (lane & 3) + {0, 1} of rows rbase and rbase + 8): act(acc + bias) with the bias row at shared address bias_s,
+// plus the fp32 residual already in the buffer when there is one, written at epi_offset into the buffer at shared
+// address buf_s.
+template <bool OUT_FP32, int ACT, int COLS>
+__device__ __forceinline__ void epilogue_to_smem(const float* acc, uint32_t bias_s, uint32_t buf_s, bool residual,
+                                                 int rbase, int lane) {
+#pragma unroll
+    for (int i = 0; i < COLS / 8; ++i) {
+        const int col = 8 * i + 2 * (lane & 3);
+        const float2 bv = ptx::ld_shared_f32x2(bias_s + 4 * col);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = rbase + 8 * h;
+            float2 y = act<OUT_FP32, ACT>(acc[4 * i + 2 * h] + bv.x, acc[4 * i + 2 * h + 1] + bv.y);
+            if constexpr (OUT_FP32) {
+                const uint32_t dst = buf_s + epi_offset<4>(r, col);
+                if (residual) {   // in the buffer already, where the result goes
+                    const float2 rv = ptx::ld_shared_f32x2(dst);
+                    y.x += rv.x;
+                    y.y += rv.y;
+                }
+                ptx::st_shared_f32x2(dst, y.x, y.y);
+            } else {
+                ptx::st_shared_u32(buf_s + epi_offset<2>(r, col), pack_bf16x2(y.x, y.y));
+            }
+        }
+    }
+}
+
+// Arrives on bar expecting the fp32 residual boxes of the 64-row, 128-column block at (row0, c0), and TMA-loads them
+// into buf.  Only the boxes that overlap [0, M) x [0, N) are loaded, as the others are never stored; a box that
+// straddles M is zero-filled past it and still counts all its bytes.
+__device__ __forceinline__ void load_residual_boxes(const CUtensorMap* tmap_r, uint64_t* bar, uint8_t* buf, int row0,
+                                                    int c0, int M, int N) {
+    const int boxes = row0 < M && c0 < N ? min(4, (N - c0) / 32) : 0;
+    ptx::mbar_arrive_expect_tx(bar, (uint32_t)boxes * EPI_BOX_BYTES);
+    for (int b = 0; b < boxes; ++b)
+        ptx::tma_load_2d(buf + b * EPI_BOX_BYTES, tmap_r, bar, c0 + 32 * b, row0, ptx::kEvictNormal);
+}
+
+// TMA-stores the 64-row, COLS-column output block at (row0, c0) from its boxes in buf, clipped at M and N, as one bulk
+// group.
+template <bool OUT_FP32, int COLS>
+__device__ __forceinline__ void store_output_boxes(const CUtensorMap* tmap_o, const uint8_t* buf, int row0, int c0,
+                                                   int M, int N) {
+    constexpr int BOX_COLS = OUT_FP32 ? 32 : 64;
+    if (row0 >= M) return;
+    for (int b = 0; b * BOX_COLS < COLS && c0 + b * BOX_COLS < N; ++b)
+        ptx::tma_store_2d(tmap_o, buf + b * EPI_BOX_BYTES, c0 + b * BOX_COLS, row0);
+    ptx::tma_store_commit();
+}
+
+// tmap_r / tmap_o (STAGED only): the fp32 residual and the output, boxes of EPI_ROWS rows x 128 bytes.  The token
+// scatter (!STAGED) is gemm_kernel<GATHER, false, true, ACT_NONE>.
+template <bool GATHER, bool STAGED, bool OUT_FP32, int ACT>
 __global__ void __launch_bounds__(threads<GATHER>(), GATHER ? 1 : 2)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_o, Params p) {
     static_assert(!(GATHER && STAGED), "the patch embed scatters token rows: register epilogue");
+    static_assert(STAGED || (OUT_FP32 && ACT == ACT_NONE), "the token scatter writes fp32 with no activation");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * STAGE_BYTES);
@@ -265,13 +340,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                 uint8_t* s = smem + (size_t)stage * STAGE_BYTES;
                 ptx::mbar_wait(&empty[stage], ((uint32_t)(kb / STAGES) & 1u) ^ 1);
                 if (pt != 0) continue;   // full[] counts one producer arrival
-                // Residual boxes that overlap [0, M) x [0, N); the others are never stored.  A box that straddles M
-                // is zero-filled past it and still counts all its bytes.
-                const int row0 = m0 + EPI_ROWS * wg;
-                const int boxes = p.ep.residual != nullptr && row0 < p.M ? min(4, (p.N - n0) / 32) : 0;
-                ptx::mbar_arrive_expect_tx(&full[stage], (uint32_t)boxes * EPI_BOX_BYTES);
-                for (int b = 0; b < boxes; ++b)
-                    ptx::tma_load_2d(s + b * EPI_BOX_BYTES, &tmap_r, &full[stage], n0 + 32 * b, row0, ptx::kEvictNormal);
+                if (p.ep.residual != nullptr)
+                    load_residual_boxes(&tmap_r, &full[stage], s, m0 + EPI_ROWS * wg, n0, p.M, p.N);
+                else
+                    ptx::mbar_arrive(&full[stage]);
             }
         }
         return;
@@ -312,88 +384,42 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         uint8_t* tile = smem + (size_t)(kb % STAGES) * STAGE_BYTES;
         warpgroup_sync(wg);   // wbias complete
         const int rbase = (warp & 3) * 16 + (lane >> 2);   // row inside the warpgroup's 64
-        // bf16 output (QKV, fc1): erf-GELU on packed fp16 pairs (see gelu_erf_h2)
-        const bool half_gelu = ep.act == ACT_GELU && !ep.act_fp32 && !ep.out_fp32;
-#pragma unroll
-        for (int i = 0; i < BN / 8; ++i) {
-            const int col = 8 * i + 2 * (lane & 3);
-            const float2 bv = *reinterpret_cast<const float2*>(wbias + col);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int r = rbase + 8 * h;
-                float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
-                if (half_gelu) {
-                    const float2 y = __half22float2(gelu_erf_h2(__floats2half2_rn(x0, x1)));
-                    *reinterpret_cast<uint32_t*>(tile + epi_offset<2>(r, col)) = pack_bf16x2(y.x, y.y);
-                    continue;
-                }
-                if (ep.act == ACT_GELU) {
-                    x0 = gelu_erf(x0);
-                    x1 = gelu_erf(x1);
-                } else if (ep.act == ACT_QUICKGELU) {
-                    x0 = quick_gelu(x0);
-                    x1 = quick_gelu(x1);
-                }
-                if (ep.out_fp32) {
-                    float2* dst = reinterpret_cast<float2*>(tile + epi_offset<4>(r, col));
-                    if (ep.residual) {   // in the stage already, where the result goes
-                        const float2 rv = *dst;
-                        x0 += rv.x;
-                        x1 += rv.y;
-                    }
-                    *dst = make_float2(x0, x1);
-                } else {
-                    *reinterpret_cast<uint32_t*>(tile + epi_offset<2>(r, col)) = pack_bf16x2(x0, x1);
-                }
-            }
-        }
+        epilogue_to_smem<OUT_FP32, ACT, BN>(acc, ptx::smem_u32(wbias), ptx::smem_u32(tile), ep.residual != nullptr,
+                                            rbase, lane);
         ptx::fence_proxy_async_smem();   // generic-proxy stores -> visible to the TMA store
         warpgroup_sync(wg);
-        const int row0 = m0 + EPI_ROWS * wg;
-        if (t == 0 && row0 < p.M) {
-            const int box_cols = ep.out_fp32 ? 32 : 64;
-            for (int b = 0; b * box_cols < BN && n0 + b * box_cols < p.N; ++b)
-                ptx::tma_store_2d(&tmap_o, tile + b * EPI_BOX_BYTES, n0 + b * box_cols, row0);
-            ptx::tma_store_commit();
+        if (t == 0) {
+            store_output_boxes<OUT_FP32, BN>(&tmap_o, tile, m0 + EPI_ROWS * wg, n0, p.M, p.N);
             ptx::tma_store_wait_read<0>();   // the stage must outlive the store's reads of it
         }
     } else {
-        // ------------------------------------------------------------ token scatter from registers (fp32 output)
+        // ------------------------------------------------------------ token scatter from registers
         const int rbase = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-        long long orow[2];
+        float* orow[2];
+        const float* pos[2];
         bool rok[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int r = rbase + 8 * h;
-            const int b = r / ep.remap_group;
+            const int b = r / ep.remap_group, i = r - b * ep.remap_group;
             rok[h] = r < p.M;
-            orow[h] = (long long)b * (ep.remap_group + 1) + 1 + (r - b * ep.remap_group);
+            orow[h] = static_cast<float*>(ep.out) + ((long long)b * (ep.remap_group + 1) + 1 + i) * ep.ldo;
+            pos[h] = ep.rowbias ? ep.rowbias + (size_t)(1 + i) * p.N : nullptr;
         }
 #pragma unroll
         for (int i = 0; i < BN / 8; ++i) {
             const int col = n0 + 8 * i + 2 * (lane & 3);
             if (col >= p.N) continue;   // N % 32 == 0: col + 1 < N as well
-            float2 bv = make_float2(0.f, 0.f);
-            if (ep.bias) bv = __ldg(reinterpret_cast<const float2*>(ep.bias + col));
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 if (!rok[h]) continue;
-                const int r = rbase + 8 * h;
-                float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
-                if (ep.act == ACT_GELU) {
-                    x0 = gelu_erf(x0);
-                    x1 = gelu_erf(x1);
-                } else if (ep.act == ACT_QUICKGELU) {
-                    x0 = quick_gelu(x0);
-                    x1 = quick_gelu(x1);
-                }
-                if (ep.rowbias) {   // ViT patch-embed: positional embedding of this row's patch
-                    const float2 pb =
-                        __ldg(reinterpret_cast<const float2*>(ep.rowbias + (size_t)(1 + r % ep.remap_group) * p.N + col));
+                float x0 = acc[4 * i + 2 * h], x1 = acc[4 * i + 2 * h + 1];
+                if (pos[h]) {   // ViT patch-embed: positional embedding of this row's patch
+                    const float2 pb = __ldg(reinterpret_cast<const float2*>(pos[h] + col));
                     x0 += pb.x;
                     x1 += pb.y;
                 }
-                *reinterpret_cast<float2*>(static_cast<float*>(ep.out) + orow[h] * ep.ldo + col) = make_float2(x0, x1);
+                *reinterpret_cast<float2*>(orow[h] + col) = make_float2(x0, x1);
             }
         }
     }
@@ -415,10 +441,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 // buffer: it goes in two 128-column uses, and the second waits for the first's store inside the epilogue.
 // Running in place (residual == out) is safe: the residual rows and columns a tile reads are the ones it writes, and
 // no other tile touches them.
-// OUT_FP32 and ACT (ACT_NONE, ACT_GELU, ACT_QUICKGELU, or ACT_GELU_H2: erf-GELU on packed fp16 pairs for a bf16
-// output) are template parameters so that each instantiation holds only the epilogue it runs: the epilogue is unrolled
-// over the 128 accumulators, and with every variant behind runtime branches the kernel was 218 KB of code, which each
-// tile's epilogue fetched into a cold instruction cache while the tensor cores idled.
+// OUT_FP32 and ACT are template parameters so that each instantiation holds only the epilogue it runs: the epilogue is
+// unrolled over the 128 accumulators, and with every variant behind runtime branches the kernel was 218 KB of code,
+// which each tile's epilogue fetched into a cold instruction cache while the tensor cores idled.
 template <bool OUT_FP32, int ACT>
 __global__ void __launch_bounds__(PERSISTENT_THREADS, 1)
 gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
@@ -434,7 +459,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     const int tiles = p.tiles_m * p.tiles_n;
     const int kblocks = p.K / BK;
     const Epilogue& ep = p.ep;
-    const bool has_res = ep.residual != nullptr;
+    const bool has_res = OUT_FP32 && ep.residual != nullptr;
 
     if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmap_a);
@@ -479,17 +504,9 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     float* wbias = bias_s + wg * P_BN;
     const uint32_t buf_s = ptx::smem_u32(buf), wbias_s = ptx::smem_u32(wbias);
     const int rbase = warp * 16 + (lane >> 2);   // row inside the warpgroup's 64
-    static_assert(!(OUT_FP32 && ACT == ACT_GELU_H2), "packed fp16 GELU is for bf16 outputs");
-    constexpr int HALVES = P_BN / 128;   // 128-column uses of the buffer by an fp32 block
+    // columns per use of the buffer: a bf16 block in one use, an fp32 block in two
+    constexpr int COLS = OUT_FP32 ? 128 : P_BN;
     uint32_t it = 0, epi_phase = 0;
-
-    // thread 0: residual columns [c0, c0 + 128) of rows row0.. into the buffer (boxes past N are never stored)
-    auto load_residual = [&](int row0, int c0) {
-        const int boxes = row0 < p.M && c0 < p.N ? min(4, (p.N - c0) / 32) : 0;
-        ptx::mbar_arrive_expect_tx(&epi_full[wg], (uint32_t)boxes * EPI_BOX_BYTES);
-        for (int b = 0; b < boxes; ++b)
-            ptx::tma_load_2d(buf + b * EPI_BOX_BYTES, &tmap_r, &epi_full[wg], c0 + 32 * b, row0, ptx::kEvictNormal);
-    };
 
     for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const int m0 = (tile / p.tiles_n) * BM, n0 = (tile % p.tiles_n) * P_BN;
@@ -522,7 +539,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
             if (kb == 0 && t == 0) {
                 ptx::tma_store_wait_read<0>();   // the previous tile's last store has read the buffer
                 if (has_res) {
-                    load_residual(row0, n0);
+                    load_residual_boxes(&tmap_r, &epi_full[wg], buf, row0, n0, p.M, p.N);
                     if (row0 < p.M)
                         for (int b = 0; b < 4 && n0 + 128 + 32 * b < p.N; ++b)
                             ptx::tma_prefetch_l2_2d(&tmap_r, n0 + 128 + 32 * b, row0);
@@ -536,107 +553,78 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 #pragma unroll
         for (int j = 0; j < P_BN / 128; ++j) wbias[t + 128 * j] = bias_r[j];
         warpgroup_sync(wg);   // wbias complete; without a residual, the buffer is free (thread 0 waited above)
-        if constexpr (!OUT_FP32) {
 #pragma unroll
-            for (int i = 0; i < P_BN / 8; ++i) {
-                const int col = 8 * i + 2 * (lane & 3);
-                const float2 bv = ptx::ld_shared_f32x2(wbias_s + 4 * col);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int r = rbase + 8 * h;
-                    float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
-                    if constexpr (ACT == ACT_GELU_H2) {
-                        const float2 y = __half22float2(gelu_erf_h2(__floats2half2_rn(x0, x1)));
-                        x0 = y.x;
-                        x1 = y.y;
-                    } else if constexpr (ACT == ACT_GELU) {
-                        x0 = gelu_erf(x0);
-                        x1 = gelu_erf(x1);
-                    } else if constexpr (ACT == ACT_QUICKGELU) {
-                        x0 = quick_gelu(x0);
-                        x1 = quick_gelu(x1);
-                    }
-                    ptx::st_shared_u32(buf_s + epi_offset<2>(r, col), pack_bf16x2(x0, x1));
+        for (int hf = 0; hf < P_BN / COLS; ++hf) {
+            if (hf > 0) {   // the buffer holds half hf - 1 until its store has read it
+                if (t == 0) {
+                    ptx::tma_store_wait_read<0>();
+                    if (has_res) load_residual_boxes(&tmap_r, &epi_full[wg], buf, row0, n0 + COLS * hf, p.M, p.N);
                 }
+                if (!has_res) warpgroup_sync(wg);
             }
+            if (has_res) {
+                ptx::mbar_wait(&epi_full[wg], epi_phase);
+                epi_phase ^= 1;
+            }
+            epilogue_to_smem<OUT_FP32, ACT, COLS>(acc + COLS / 2 * hf, wbias_s + 4 * COLS * hf, buf_s, has_res, rbase,
+                                                  lane);
             ptx::fence_proxy_async_smem();   // generic-proxy stores -> visible to the TMA store
             warpgroup_sync(wg);
-            if (t == 0 && row0 < p.M) {
-                for (int b = 0; b < P_BN / 64 && n0 + 64 * b < p.N; ++b)
-                    ptx::tma_store_2d(&tmap_o, buf + b * EPI_BOX_BYTES, n0 + 64 * b, row0);
-                ptx::tma_store_commit();
-            }
-        } else {
-#pragma unroll
-            for (int hf = 0; hf < HALVES; ++hf) {
-                if (hf > 0) {   // the buffer holds half hf - 1 until its store has read it
-                    if (t == 0) {
-                        ptx::tma_store_wait_read<0>();
-                        if (has_res) load_residual(row0, n0 + 128 * hf);
-                    }
-                    if (!has_res) warpgroup_sync(wg);
-                }
-                if (has_res) {
-                    ptx::mbar_wait(&epi_full[wg], epi_phase);
-                    epi_phase ^= 1;
-                }
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const int col = 8 * i + 2 * (lane & 3);   // inside the half
-                    const int ai = 4 * (16 * hf + i);
-                    const float2 bv = ptx::ld_shared_f32x2(wbias_s + 4 * (128 * hf + col));
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int r = rbase + 8 * h;
-                        float x0 = acc[ai + 2 * h] + bv.x, x1 = acc[ai + 2 * h + 1] + bv.y;
-                        if constexpr (ACT == ACT_GELU) {
-                            x0 = gelu_erf(x0);
-                            x1 = gelu_erf(x1);
-                        } else if constexpr (ACT == ACT_QUICKGELU) {
-                            x0 = quick_gelu(x0);
-                            x1 = quick_gelu(x1);
-                        }
-                        const uint32_t dst = buf_s + epi_offset<4>(r, col);
-                        if (has_res) {   // in the buffer already, where the result goes
-                            const float2 rv = ptx::ld_shared_f32x2(dst);
-                            x0 += rv.x;
-                            x1 += rv.y;
-                        }
-                        ptx::st_shared_f32x2(dst, x0, x1);
-                    }
-                }
-                ptx::fence_proxy_async_smem();
-                warpgroup_sync(wg);
-                const int c0 = n0 + 128 * hf;
-                if (t == 0 && row0 < p.M && c0 < p.N) {
-                    for (int b = 0; b < 4 && c0 + 32 * b < p.N; ++b)
-                        ptx::tma_store_2d(&tmap_o, buf + b * EPI_BOX_BYTES, c0 + 32 * b, row0);
-                    ptx::tma_store_commit();
-                }
-            }
+            if (t == 0) store_output_boxes<OUT_FP32, COLS>(&tmap_o, buf, row0, n0 + COLS * hf, p.M, p.N);
         }
     }
     if (t == 0) ptx::tma_store_wait_read<0>();   // shared memory must outlive the last store's reads of it
+}
+
+// Calls f(std::bool_constant<OUT_FP32>, std::integral_constant<int, ACT>) for the STAGED epilogue instantiation of
+// (out_fp32, act), an activation other than GELU and QuickGELU being none: the one list of instantiations, from which
+// both launches and configure() take theirs.
+template <class F>
+static void dispatch(bool out_fp32, int act, F&& f) {
+    const auto with_act = [&](auto out) {
+        if (act == ACT_GELU)
+            f(out, std::integral_constant<int, ACT_GELU>{});
+        else if (act == ACT_QUICKGELU)
+            f(out, std::integral_constant<int, ACT_QUICKGELU>{});
+        else
+            f(out, std::integral_constant<int, ACT_NONE>{});
+    };
+    if (out_fp32)
+        with_act(std::true_type{});
+    else
+        with_act(std::false_type{});
 }
 
 void configure() {
     static std::once_flag once;
     std::call_once(once, [] {
         const auto attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
-        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, true>, attr, (int)SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, false>, attr, (int)SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<true, false>, attr, (int)SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<false, ACT_NONE>, attr, (int)P_SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<false, ACT_GELU>, attr, (int)P_SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<false, ACT_QUICKGELU>, attr, (int)P_SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<false, ACT_GELU_H2>, attr, (int)P_SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<true, ACT_NONE>, attr, (int)P_SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<true, ACT_GELU>, attr, (int)P_SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<true, ACT_QUICKGELU>, attr, (int)P_SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, false, true, ACT_NONE>, attr, (int)SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<true, false, true, ACT_NONE>, attr, (int)SMEM_BYTES));
+        for (int out_fp32 = 0; out_fp32 < 2; ++out_fp32)
+            for (int act = ACT_NONE; act <= ACT_QUICKGELU; ++act)
+                dispatch(out_fp32, act, [&](auto out, auto a) {
+                    constexpr bool OUT_FP32 = decltype(out)::value;
+                    constexpr int ACT = decltype(a)::value;
+                    MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, true, OUT_FP32, ACT>, attr, (int)SMEM_BYTES));
+                    MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<OUT_FP32, ACT>, attr, (int)P_SMEM_BYTES));
+                });
     });
 }
 
-template <bool GATHER, bool STAGED>
+// The STAGED epilogue's maps, boxes of EPI_ROWS rows x 128 bytes with the 128B swizzle: the fp32 residual (tr is left
+// as it is without one) and the output.
+static void epilogue_tmaps(const Epilogue& ep, int M, int N, CUtensorMap& tr, CUtensorMap& to) {
+    if (ep.residual)
+        tr = make_tmap_2d(ep.residual, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
+                          (uint64_t)ep.ldr * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
+    to = ep.out_fp32 ? make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
+                                    (uint64_t)ep.ldo * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B)
+                     : make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)N, (uint64_t)M,
+                                    (uint64_t)ep.ldo * 2, 64, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
+template <bool GATHER, bool STAGED, bool OUT_FP32, int ACT>
 static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep,
                          cudaStream_t stream, const PatchGather* pg = nullptr) {
     Params p{};
@@ -667,16 +655,9 @@ static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W
                             : make_tmap_2d(A, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)K, (uint64_t)M,
                                            (uint64_t)lda * 2, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);
     CUtensorMap tr = tb, to = tb;
-    if (STAGED) {
-        if (ep.residual)
-            tr = make_tmap_2d(ep.residual, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
-                              (uint64_t)ep.ldr * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
-        to = ep.out_fp32 ? make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
-                                        (uint64_t)ep.ldo * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B)
-                         : make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)N, (uint64_t)M,
-                                        (uint64_t)ep.ldo * 2, 64, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
-    }
-    gemm_kernel<GATHER, STAGED><<<(unsigned)tiles, threads<GATHER>(), SMEM_BYTES, stream>>>(ta, tb, tr, to, p);
+    if (STAGED) epilogue_tmaps(ep, M, N, tr, to);
+    gemm_kernel<GATHER, STAGED, OUT_FP32, ACT>
+        <<<(unsigned)tiles, threads<GATHER>(), SMEM_BYTES, stream>>>(ta, tb, tr, to, p);
     MB_CUDA(cudaGetLastError());
 }
 
@@ -697,38 +678,11 @@ static void launch_persistent(const __nv_bfloat16* A, int lda, const __nv_bfloat
     CUtensorMap tb = make_tmap_2d(W, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)K, (uint64_t)N, (uint64_t)K * 2, BK,
                                   P_BN, CU_TENSOR_MAP_SWIZZLE_128B);
     // (without a residual its map is a further, unused view of W so the kernel signature stays the same)
-    CUtensorMap tr = ep.residual ? make_tmap_2d(ep.residual, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
-                                                (uint64_t)ep.ldr * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B)
-                                 : tb;
-    CUtensorMap to = ep.out_fp32 ? make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
-                                                (uint64_t)ep.ldo * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B)
-                                 : make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)N, (uint64_t)M,
-                                                (uint64_t)ep.ldo * 2, 64, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
+    CUtensorMap tr = tb, to;
+    epilogue_tmaps(ep, M, N, tr, to);
     const int grid = (int)std::min<long long>(tiles, std::max(sms, 1));
     gemm_persistent_kernel<OUT_FP32, ACT><<<grid, PERSISTENT_THREADS, P_SMEM_BYTES, stream>>>(ta, tb, tr, to, p);
     MB_CUDA(cudaGetLastError());
-}
-
-static void launch_persistent(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K,
-                              const Epilogue& ep, int sms, cudaStream_t stream) {
-    const int act = ep.act == ACT_GELU && !ep.act_fp32 && !ep.out_fp32 ? ACT_GELU_H2 : ep.act;
-    if (ep.out_fp32) {
-        if (act == ACT_GELU)
-            launch_persistent<true, ACT_GELU>(A, lda, W, M, N, K, ep, sms, stream);
-        else if (act == ACT_QUICKGELU)
-            launch_persistent<true, ACT_QUICKGELU>(A, lda, W, M, N, K, ep, sms, stream);
-        else
-            launch_persistent<true, ACT_NONE>(A, lda, W, M, N, K, ep, sms, stream);
-    } else {
-        if (act == ACT_GELU_H2)
-            launch_persistent<false, ACT_GELU_H2>(A, lda, W, M, N, K, ep, sms, stream);
-        else if (act == ACT_GELU)
-            launch_persistent<false, ACT_GELU>(A, lda, W, M, N, K, ep, sms, stream);
-        else if (act == ACT_QUICKGELU)
-            launch_persistent<false, ACT_QUICKGELU>(A, lda, W, M, N, K, ep, sms, stream);
-        else
-            launch_persistent<false, ACT_NONE>(A, lda, W, M, N, K, ep, sms, stream);
-    }
 }
 
 bool patch_gather_supported(int S, int patch) {
@@ -742,13 +696,13 @@ void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, c
     if (!patch_gather_supported(pg.S, pg.patch))
         fail(B200_ERR_INTERNAL, "patch gather: image %d / patch %d is not supported", pg.S, pg.patch);
     if (N % 32 != 0 || ep.ldo % 8 != 0) fail(B200_ERR_INTERNAL, "patch gather: N = %d, ldo = %d", N, ep.ldo);
-    if (ep.remap_group <= 0 || ep.residual != nullptr || !ep.out_fp32)
-        fail(B200_ERR_INTERNAL, "patch gather: token scatter to fp32 output without residual only");
+    if (ep.remap_group <= 0 || ep.residual != nullptr || ep.bias != nullptr || ep.act != ACT_NONE || !ep.out_fp32)
+        fail(B200_ERR_INTERNAL, "patch gather: fp32 token scatter without bias, activation or residual only");
     configure();
     const int g = pg.S / pg.patch;
     const long long M = (long long)pg.n * g * g;
     if (M > 0x7fffffffLL) fail(B200_ERR_INVALID_ARG, "patch gather: batch of %d images is too large", pg.n);
-    launch_tiles<true, false>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
+    launch_tiles<true, false, true, ACT_NONE>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
 }
 
 void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep, int sms,
@@ -758,10 +712,10 @@ void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int 
     if (N % 32 != 0) fail(B200_ERR_INTERNAL, "gemm: N = %d must be a multiple of 32", N);
     if (lda % 8 != 0 || ep.ldo % 8 != 0) fail(B200_ERR_INTERNAL, "gemm: leading dimensions must be multiples of 8");
     if (ep.remap_group > 0) {
-        if (ep.residual != nullptr || !ep.out_fp32)
-            fail(B200_ERR_INTERNAL, "gemm: token scatter to fp32 output without residual only");
+        if (ep.residual != nullptr || ep.bias != nullptr || ep.act != ACT_NONE || !ep.out_fp32)
+            fail(B200_ERR_INTERNAL, "gemm: fp32 token scatter without bias, activation or residual only");
         configure();
-        launch_tiles<false, false>(A, lda, W, M, N, K, ep, stream);
+        launch_tiles<false, false, true, ACT_NONE>(A, lda, W, M, N, K, ep, stream);
         return;
     }
     // TMA: 16-byte aligned bases and row pitches
@@ -775,10 +729,15 @@ void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int 
     // tile (all four ViT-L-14 layer GEMMs, K >= 1024), at least one full wave of tiles, and no half-empty 256-wide
     // column tile (the 384-wide BERTs run slower with one; DESIGN.md §7.5c).
     const long long tiles256 = (long long)((M + BM - 1) / BM) * (N / P_BN);
-    if (K >= 1024 && N % P_BN == 0 && tiles256 >= sms)
-        launch_persistent(A, lda, W, M, N, K, ep, sms, stream);
-    else
-        launch_tiles<false, true>(A, lda, W, M, N, K, ep, stream);
+    const bool persistent = K >= 1024 && N % P_BN == 0 && tiles256 >= sms;
+    dispatch(ep.out_fp32, ep.act, [&](auto out, auto a) {
+        constexpr bool OUT_FP32 = decltype(out)::value;
+        constexpr int ACT = decltype(a)::value;
+        if (persistent)
+            launch_persistent<OUT_FP32, ACT>(A, lda, W, M, N, K, ep, sms, stream);
+        else
+            launch_tiles<false, true, OUT_FP32, ACT>(A, lda, W, M, N, K, ep, stream);
+    });
 }
 
 }  // namespace gemm

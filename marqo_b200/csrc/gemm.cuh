@@ -1,9 +1,9 @@
 // Warp-specialised wgmma GEMM:  out[M,N] = epilogue( A[M,K] (bf16, K-major) x W[N,K]^T (bf16, K-major) )
-// 128 x 128 tiles, TMA-fed 128B-swizzled smem ring, two MMA warpgroups with fp32 accumulators in registers.  The
-// epilogue stages each warpgroup's output block in a ring stage (the fp32 residual TMA-loaded into it ahead of time)
-// and writes it with TMA stores; only the ViT token scatter (remap_group > 0) stores from registers.  For K >= 1024,
-// N % 256 == 0 and at least one full wave of tiles, a persistent kernel of 128 x 256 tiles (one CTA per SM) runs instead, with
-// the same epilogue arithmetic through a shared-memory buffer of its own (gemm.cu).
+// 128 x 128 tiles, TMA-fed 128B-swizzled smem ring, two MMA warpgroups with fp32 accumulators in registers.  For
+// K >= 1024, N % 256 == 0 and at least one full wave of tiles, a persistent kernel of 128 x 256 tiles (one CTA per SM)
+// runs instead.  Both kernels run one epilogue, act(acc + bias) (+ residual): each warpgroup's output block goes
+// through shared memory (the fp32 residual TMA-loaded into it ahead of time) and out by TMA stores (gemm.cu).  Only the
+// ViT token scatter (remap_group > 0) stores from registers; it takes no bias and no activation.
 // Output and residual must be 16-byte aligned; a residual needs an fp32 output and ldr % 4 == 0.
 #pragma once
 #include "common.cuh"
@@ -17,8 +17,7 @@ struct Epilogue {
     const float* bias = nullptr;      // [N]
     const float* residual = nullptr;  // fp32 [M, ldr], added after the activation
     int ldr = 0;
-    int act = ACT_NONE;
-    int act_fp32 = 0;     // 1: evaluate erf-GELU in fp32 even for a bf16 output (default: packed fp16, see gemm.cu gelu_erf_h2)
+    int act = ACT_NONE;   // erf-GELU on packed fp16 pairs for a bf16 output (see gemm.cu gelu_erf_h2), fp32 otherwise
     void* out = nullptr;  // bf16 or fp32 [*, ldo]
     int ldo = 0;
     int out_fp32 = 0;

@@ -225,12 +225,6 @@ void attend(b200_model* m, Counter& c, int B, int S, int w, int heads, int mask_
     c.n += attention::launch(m->qkv.get(), m->o.get(), B, S, w, heads, mask_mode, kv_len, m->stream);
 }
 
-// MARQO_B200_GELU_FP32=1: evaluate fc1's erf-GELU in fp32 instead of packed fp16 (A/B timing and accuracy comparisons)
-bool gelu_fp32() {
-    static const bool on = getenv("MARQO_B200_GELU_FP32") != nullptr;
-    return on;
-}
-
 // Pre-LN residual blocks (open_clip ResidualAttentionBlock).  x (fp32) is the residual stream, h (bf16) the LayerNorm
 // output the next GEMM consumes.
 void run_clip_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, int mask_mode) {
@@ -260,7 +254,6 @@ void run_clip_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, i
         e3.act = act;
         e3.out = m->u.get();
         e3.ldo = mlp;
-        e3.act_fp32 = gelu_fp32() ? 1 : 0;
         linear(m, c, m->h.get(), M, w, L.w_fc, mlp, e3);
         gemm::Epilogue e4;
         e4.bias = L.b_proj;
@@ -300,7 +293,6 @@ void run_bert_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S) {
         e3.act = gemm::ACT_GELU;
         e3.out = m->u.get();
         e3.ldo = mlp;
-        e3.act_fp32 = gelu_fp32() ? 1 : 0;
         linear(m, c, m->h.get(), M, w, L.w_fc, mlp, e3);
         gemm::Epilogue e4;
         e4.bias = L.b_proj;

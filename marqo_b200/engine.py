@@ -489,8 +489,8 @@ def debug_gemm(A, W, bias=None, residual=None, act: int = 0, out_bf16: bool = Fa
     return out
 
 
-def debug_gemm_into(A, W, io, bias=None, act: int = 0, act_fp32: bool = False, out_bf16: bool = False,
-                    residual_in_place: bool = False, device: int = 0) -> np.ndarray:
+def debug_gemm_into(A, W, io, bias=None, act: int = 0, out_bf16: bool = False, residual_in_place: bool = False,
+                    device: int = 0) -> np.ndarray:
     """GEMM into a copy of io (fp32 [rows >= M, cols >= N], bf16 on the device when out_bf16): rows [0, M) x columns
     [0, N) become act(A W^T + bias), plus their old values when residual_in_place (residual == out); the rest of the
     buffer is returned as the kernel left it."""
@@ -499,9 +499,8 @@ def debug_gemm_into(A, W, io, bias=None, act: int = 0, act_fp32: bool = False, o
     Nn = W.shape[0]
     b = None if bias is None else _as(bias, np.float32)
     out = np.array(io, dtype=np.float32, order="C", copy=True)
-    N.check(N.load().b200_debug_gemm_into(device, _ptr(A), _ptr(W), _ptr(b), M, Nn, K, act, int(act_fp32),
-                                          int(out_bf16), int(residual_in_place), out.shape[0], out.shape[1],
-                                          _ptr(out)))
+    N.check(N.load().b200_debug_gemm_into(device, _ptr(A), _ptr(W), _ptr(b), M, Nn, K, act, int(out_bf16),
+                                          int(residual_in_place), out.shape[0], out.shape[1], _ptr(out)))
     return out
 
 

@@ -24,23 +24,23 @@ def _act(z: torch.Tensor, act: int) -> torch.Tensor:
     return z
 
 
-@pytest.mark.parametrize("M,N,K,act,act_fp32,out_bf16,residual,bias", [
-    (333, 96, 256, 0, 0, 0, True, True),            # residual in place, partial row and column tiles
-    (40, 384, 128, 0, 0, 0, True, True),            # the second warpgroup's rows are all past M
-    (333, 1024, 64, 0, 0, 0, True, True),           # K = 64: one k-block, the epilogue stages never held operands
-    (128 * 300 + 5, 128, 128, 0, 0, 0, True, True),    # 301 tiles: more than 2 x 132 SMs
-    (300, 256, 192, 1, 0, 0, True, True),           # GELU, then the residual
-    (300, 256, 192, 2, 0, 0, True, True),           # QuickGELU, then the residual
-    (333, 96, 256, 0, 0, 1, False, True),           # bias only, bf16
-    (333, 96, 256, 0, 0, 0, False, True),           # bias only, fp32
-    (200, 384, 128, 0, 0, 0, False, False),         # no bias, fp32, two k-blocks
-    (333, 384, 256, 1, 0, 1, False, True),          # GELU, bf16 (packed fp16 evaluation)
-    (333, 384, 256, 1, 1, 1, False, True),          # GELU, bf16 (fp32 evaluation)
-    (333, 384, 256, 1, 0, 0, False, True),          # GELU, fp32
-    (40, 96, 64, 2, 0, 1, False, True),             # QuickGELU, bf16
-    (333, 384, 256, 2, 0, 0, False, True),          # QuickGELU, fp32
+@pytest.mark.parametrize("M,N,K,act,out_bf16,residual,bias", [
+    (333, 96, 256, 0, 0, True, True),            # residual in place, partial row and column tiles
+    (40, 384, 128, 0, 0, True, True),            # the second warpgroup's rows are all past M
+    (333, 1024, 64, 0, 0, True, True),           # K = 64: one k-block, the epilogue stages never held operands
+    (128 * 300 + 5, 128, 128, 0, 0, True, True),    # 301 tiles: more than 2 x 132 SMs
+    (300, 256, 192, 1, 0, True, True),           # GELU, then the residual
+    (300, 256, 192, 2, 0, True, True),           # QuickGELU, then the residual
+    (333, 96, 256, 0, 1, False, True),           # bias only, bf16
+    (333, 96, 256, 0, 0, False, True),           # bias only, fp32
+    (200, 384, 128, 0, 0, False, False),         # no bias, fp32, two k-blocks
+    (200, 384, 128, 1, 1, False, False),         # no bias, bf16 GELU
+    (333, 384, 256, 1, 1, False, True),          # GELU, bf16 (packed fp16 evaluation)
+    (333, 384, 256, 1, 0, False, True),          # GELU, fp32
+    (40, 96, 64, 2, 1, False, True),             # QuickGELU, bf16
+    (333, 384, 256, 2, 0, False, True),          # QuickGELU, fp32
 ])
-def test_gemm_epilogue_into_buffer(gpu_required, M, N, K, act, act_fp32, out_bf16, residual, bias):
+def test_gemm_epilogue_into_buffer(gpu_required, M, N, K, act, out_bf16, residual, bias):
     from marqo_b200.engine import debug_gemm_into
     g = torch.Generator().manual_seed(M * 7 + N + K + act)
     A = _bf16(torch.randn(M, K, generator=g))
@@ -51,8 +51,7 @@ def test_gemm_epilogue_into_buffer(gpu_required, M, N, K, act, act_fp32, out_bf1
     if residual:
         io[:M, :N] = res
     got = torch.from_numpy(debug_gemm_into(A.numpy(), W.numpy(), io.numpy(), None if b is None else b.numpy(), act=act,
-                                           act_fp32=bool(act_fp32), out_bf16=bool(out_bf16),
-                                           residual_in_place=residual))
+                                           out_bf16=bool(out_bf16), residual_in_place=residual))
     z = A.double() @ W.double().t()
     if b is not None:
         z = z + b.double()
