@@ -235,7 +235,8 @@ typedef struct b200_model b200_model;
 
 enum b200_arch {
     B200_ARCH_CLIP = 0, /* open_clip CLIP: vision tower + text tower */
-    B200_ARCH_BERT = 1  /* HF BertModel + pooling */
+    B200_ARCH_BERT = 1, /* HF BertModel + pooling */
+    B200_ARCH_MPNET = 2 /* HF MPNetModel + pooling: BERT layers with a relative-position bias in the attention logits */
 };
 enum b200_act { B200_ACT_GELU = 0, B200_ACT_QUICKGELU = 1 };
 enum b200_pool { B200_POOL_MEAN = 0, B200_POOL_CLS = 1 };
@@ -261,7 +262,13 @@ typedef struct b200_model_desc {
     float image_mean[3]; /* Normalize() constants, src/marqo/s2_inference/clip_utils.py:32-33 */
     float image_std[3];
     b200_tower_desc vision; /* CLIP only */
-    b200_tower_desc text;   /* CLIP text tower, or the BERT encoder */
+    b200_tower_desc text;   /* CLIP text tower, or the BERT / MPNet encoder (MPNet: ctx = longest sequence, which is
+                               max_position_embeddings - pad_id - 1 because positions start after the pad id) */
+    /* MPNet only (MPNetConfig): */
+    float layer_norm_eps;     /* 1e-5 for the sentence-transformers checkpoints */
+    int32_t pad_id;           /* pad_token_id (1): the position ids count from it */
+    int32_t rel_buckets;      /* relative_attention_num_buckets (32) */
+    int32_t rel_max_distance; /* max_distance of relative_position_bucket (128) */
 } b200_model_desc;
 
 int b200_model_create(int device, const b200_model_desc* desc, b200_model** out);
@@ -286,7 +293,9 @@ int b200_model_encode_images_u8(b200_model* m, const uint8_t* hwc, int n, int h,
  * unchanged: abstract_clip_model.py:108-111). */
 int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int normalize, float* out);
 /* Token ids int32 [n, seq] (host).  CLIP: causal text tower, EOT = arg-max id pooling.
- * BERT: attn_mask int32 [n, seq] (1 = token, 0 = pad; NULL = all ones), token_type 0. */
+ * BERT: attn_mask int32 [n, seq] (1 = token, 0 = pad; NULL = all ones), token_type 0.
+ * MPNet: as BERT, without token types; position ids follow the ids (HF create_position_ids_from_input_ids), the key
+ * mask follows attn_mask.  seq > text.ctx is refused with B200_ERR_INVALID_ARG. */
 int b200_model_encode_tokens(b200_model* m, const int32_t* ids, const int32_t* attn_mask, int n, int seq,
                              int normalize, float* out);
 /* Device-resident variants: inputs/outputs are device pointers on the model's device,
@@ -322,6 +331,13 @@ typedef struct b200_tokenizer b200_tokenizer;
  * (one token per line, id = line number; must contain [PAD] [UNK] [CLS] [SEP]).  do_lower_case != 0 also strips
  * accents (BertNormalizer's strip_accents=None follows lowercase). */
 int b200_tokenizer_create_wordpiece(const char* vocab_utf8, size_t nbytes, int do_lower_case, b200_tokenizer** out);
+/* The same WordPiece with the special tokens named by the caller: rows are "cls ids sep", padded with `pad`, words
+ * without a piece become `unk`, and exactly the n_specials strings of `specials` are matched verbatim in the raw text
+ * (MPNetTokenizer: "<s>", "</s>", "<pad>", "[UNK]" and specials <s> <pad> </s> [UNK] <mask>).  Every named token must be
+ * in the vocabulary. */
+int b200_tokenizer_create_wordpiece_ex(const char* vocab_utf8, size_t nbytes, int do_lower_case, const char* cls,
+                                       const char* sep, const char* pad, const char* unk, const char* const* specials,
+                                       int n_specials, b200_tokenizer** out);
 /* CLIP byte-level BPE — open_clip's SimpleTokenizer, the tokenizer OPEN_CLIP.load_tokenizer() returns for non-hf-hub
  * models (src/marqo/core/inference/embedding_models/open_clip_model.py:211-222; cleaning rules restated at
  * src/marqo/core/inference/embedding_models/hf_tokenizer.py:9-17).  merges_utf8: the DECOMPRESSED bytes of
@@ -410,6 +426,16 @@ int b200_debug_patch_embed(int device, const uint8_t* hwc, int n, int S, int pat
  * 2 key length (kv_len int32 [B]).  out fp32 [B*S, W]. */
 int b200_debug_attention(int device, const float* qkv, int B, int S, int W, int H, int mask, const int32_t* kv_len,
                          float* out);
+/* The same with key-length masking (kv_len int32 [B]) and MPNet's relative-position bias: rel_bias fp32 [H, 2*smax - 1]
+ * (natural-log domain, as it enters softmax) adds rel_bias[h, j - i + smax - 1] to the logit of query i and key j.
+ * head_dim 64, S <= smax. */
+int b200_debug_attention_bias(int device, const float* qkv, int B, int S, int W, int H, const int32_t* kv_len,
+                              const float* rel_bias, int smax, float* out);
+/* Mean device time (ms) of `iters` launches of the biased attention on device-generated data (all keys kept). */
+int b200_debug_attention_bias_time(int device, int B, int S, int W, int H, int iters, float* out_ms);
+/* MPNet's relative_position_bucket as the model builds its bias table: out[d + max_len - 1] = bucket of
+ * key - query = d for |d| < max_len (host-only). */
+int b200_debug_relative_position_buckets(int num_buckets, int max_distance, int max_len, int32_t* out);
 /* LayerNorm over rows of fp32 [rows, w]. */
 /* Mean device time (ms, CUDA events) of `iters` back-to-back attention launches on device-generated data. */
 int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, int iters, float* out_ms);

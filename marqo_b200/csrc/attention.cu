@@ -59,13 +59,19 @@ __device__ __forceinline__ void load_tile(__nv_bfloat16* tile, const __nv_bfloat
     }
 }
 
-template <int HD, int MASK>
+// BIAS: add the relative-position bias (attention.cuh: RelBias) to the logits.  The kernel serves S < 128, so the
+// band of the bias row one CTA meets is at most 2 key blocks + BQ entries.
+constexpr int BIAS_BAND = 2 * BKV + BQ;
+
+template <int HD, int MASK, bool BIAS>
 __global__ void __launch_bounds__(THREADS)
 attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out, int S, int W,
-                 const int32_t* __restrict__ kv_len, float scale_log2e) {
+                 const int32_t* __restrict__ kv_len, float scale_log2e, const float* __restrict__ rel_bias,
+                 int bias_smax) {
     __shared__ __align__(128) __nv_bfloat16 sQ[BQ * HD];
     __shared__ __align__(128) __nv_bfloat16 sK[2][BKV * HD];
     __shared__ __align__(128) __nv_bfloat16 sV[2][BKV * HD];
+    __shared__ float sBias[BIAS ? BIAS_BAND : 1];
 
     const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * BQ;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -88,6 +94,10 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
         load_tile<HD>(sV[0], vbase, 0, len, ld);
     }
     cp_async_commit();
+    if constexpr (BIAS) {   // band entry t: key - query = t - (q0 + BQ - 1); read after the first block's barrier
+        const float* row = rel_bias + (size_t)h * (2 * bias_smax - 1);
+        for (int t = threadIdx.x; t < nkb * BKV + BQ; t += THREADS) sBias[t] = rel_bias_band_value(row, bias_smax, q0, t);
+    }
 
     uint32_t qf[HD / 16][4];
     float o[HD / 8][4];
@@ -144,7 +154,11 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
                 const int rr = e >> 1;
                 bool ok = key < len;
                 if (MASK == MASK_CAUSAL) ok = ok && key <= qrow[rr];
-                const float v = ok ? s[nt][e] * scale_log2e : -INFINITY;
+                float v;
+                if constexpr (BIAS)
+                    v = ok ? s[nt][e] * scale_log2e + sBias[key - qrow[rr] + (q0 + BQ - 1)] : -INFINITY;
+                else
+                    v = ok ? s[nt][e] * scale_log2e : -INFINITY;
                 s[nt][e] = v;
                 mx[rr] = fmaxf(mx[rr], v);
             }
@@ -237,14 +251,17 @@ void launch_hd(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W
     const float scale_log2e = head_scale_log2e(HD);
     switch (mask) {
         case MASK_NONE:
-            attention_kernel<HD, MASK_NONE><<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e);
+            attention_kernel<HD, MASK_NONE, false>
+                <<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e, nullptr, 0);
             break;
         case MASK_CAUSAL:
-            attention_kernel<HD, MASK_CAUSAL><<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e);
+            attention_kernel<HD, MASK_CAUSAL, false>
+                <<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e, nullptr, 0);
             break;
         case MASK_KEYLEN:
             if (!kv_len) fail(B200_ERR_INTERNAL, "attention: kv_len required for key-length masking");
-            attention_kernel<HD, MASK_KEYLEN><<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e);
+            attention_kernel<HD, MASK_KEYLEN, false>
+                <<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e, nullptr, 0);
             break;
         default:
             fail(B200_ERR_INTERNAL, "attention: unknown mask mode %d", mask);
@@ -259,6 +276,20 @@ int launch(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, in
         launch_hd<64>(qkv, out, B, S, W, H, mask, kv_len, stream);
     else
         launch_hd<32>(qkv, out, B, S, W, H, mask, kv_len, stream);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int launch_rel_bias(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, const int32_t* kv_len,
+                    const RelBias& bias, cudaStream_t stream) {
+    if (B <= 0 || S <= 0) return 0;
+    if (head_dim(W, H) != 64) fail(B200_ERR_UNSUPPORTED, "attention: the relative bias is built for head_dim 64 only");
+    if (!kv_len || !bias.table) fail(B200_ERR_INTERNAL, "attention: the relative bias needs kv_len and a table");
+    if (S > bias.smax) fail(B200_ERR_INVALID_ARG, "attention: sequence %d is longer than the bias table (%d)", S, bias.smax);
+    if (S >= 128) return launch_wgmma_rel_bias(qkv, out, B, S, W, H, kv_len, bias, stream);
+    const dim3 grid((S + BQ - 1) / BQ, H, B);
+    attention_kernel<64, MASK_KEYLEN, true>
+        <<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, head_scale_log2e(64), bias.table, bias.smax);
     MB_CUDA(cudaGetLastError());
     return 1;
 }

@@ -18,6 +18,16 @@ enum Mask { MASK_NONE = 0, MASK_CAUSAL = 1, MASK_KEYLEN = 2 };
 int launch(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask, const int32_t* kv_len,
            cudaStream_t stream);
 
+// Additive relative-position bias of the attention logits (MPNet): table fp32 [H][2 * smax - 1], already multiplied by
+// log2(e); query i and key j of head h add table[h][j - i + smax - 1] to their log2-domain logit.  Each CTA stages the
+// diagonal band its 64 queries reach in shared memory.  Built for head_dim 64 with MASK_KEYLEN only; S <= smax.
+struct RelBias {
+    const float* table = nullptr;
+    int smax = 0;
+};
+int launch_rel_bias(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, const int32_t* kv_len,
+                    const RelBias& bias, cudaStream_t stream);
+
 // W / H when it is a head dim the kernels are built for (32 or 64); anything else fails with B200_ERR_UNSUPPORTED.
 inline int head_dim(int W, int H) {
     if (H > 0 && W == H * 64) return 64;
@@ -31,6 +41,15 @@ inline float head_scale_log2e(int hd) { return (hd == 64 ? 0.125f : 0.1767766952
 // wgmma implementation (attention_wgmma.cu); any S, chosen by launch() for S >= 128
 int launch_wgmma(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask, const int32_t* kv_len,
                  cudaStream_t stream);
+int launch_wgmma_rel_bias(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, const int32_t* kv_len,
+                          const RelBias& bias, cudaStream_t stream);
+
+// Table index of band entry t for a CTA whose queries start at q0: the band covers key - query = t - (q0 + 63).
+// Entries outside the table (never met by a key that is kept) are 0.
+__device__ __forceinline__ float rel_bias_band_value(const float* __restrict__ row, int smax, int q0, int t) {
+    const int idx = t - (q0 + 63) + smax - 1;
+    return idx >= 0 && idx < 2 * smax - 1 ? __ldg(row + idx) : 0.f;
+}
 
 }  // namespace attention
 }  // namespace mb

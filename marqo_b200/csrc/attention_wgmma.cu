@@ -56,11 +56,16 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
     return *reinterpret_cast<uint32_t*>(&v);
 }
 
-template <int HD, int MASK>
+// bytes of the relative-bias band behind the barriers: one float per key of the CTA's key tiles, plus BQ - 1
+inline size_t bias_band_bytes(int S) { return ((size_t)(S + BKV - 1) / BKV * BKV + BQ) * sizeof(float); }
+
+// BIAS: add the relative-position bias (attention.cuh: RelBias) to the logits, read from a band of the head's bias row
+// staged in shared memory behind the barriers.
+template <int HD, int MASK, bool BIAS>
 __global__ void __launch_bounds__(THREADS)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
                        __nv_bfloat16* __restrict__ out, int S, int W, const int32_t* __restrict__ kv_len,
-                       float scale_log2e) {
+                       float scale_log2e, const float* __restrict__ rel_bias, int bias_smax) {
     constexpr uint32_t Q_BYTES = Tiles<HD>::Q_BYTES;
     constexpr uint32_t KV_TILE_BYTES = Tiles<HD>::KV_TILE_BYTES;
     constexpr uint32_t STAGE_BYTES = Tiles<HD>::STAGE_BYTES;
@@ -88,6 +93,11 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
         }
         ptx::mbar_init(qfull, 1);
         ptx::fence_barrier_init();
+    }
+    float* sbias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 64);
+    if constexpr (BIAS) {   // band entry t: key - query = t - (q0 + BQ - 1)
+        const float* row = rel_bias + (size_t)h * (2 * bias_smax - 1);
+        for (int t = threadIdx.x; t < nkb * BKV + BQ; t += THREADS) sbias[t] = rel_bias_band_value(row, bias_smax, q0, t);
     }
     __syncthreads();
 
@@ -141,7 +151,11 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
                 const int rr = e >> 1;
                 bool ok = key < len;
                 if (MASK == MASK_CAUSAL) ok = ok && key <= qrow[rr];
-                const float v = ok ? s[4 * i + e] * scale_log2e : -INFINITY;
+                float v;
+                if constexpr (BIAS)
+                    v = ok ? s[4 * i + e] * scale_log2e + sbias[key - qrow[rr] + (q0 + BQ - 1)] : -INFINITY;
+                else
+                    v = ok ? s[4 * i + e] * scale_log2e : -INFINITY;
                 s[4 * i + e] = v;
                 mx[rr] = fmaxf(mx[rr], v);
             }
@@ -206,23 +220,29 @@ void launch_mask(const CUtensorMap& tq, const CUtensorMap& tkv, __nv_bfloat16* o
     constexpr size_t SMEM_BYTES = Tiles<HD>::SMEM_BYTES;
     static std::once_flag once;
     std::call_once(once, [] {
-        MB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel<HD, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        MB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel<HD, MASK, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)SMEM_BYTES));
     });
     const dim3 grid((S + BQ - 1) / BQ, H, B);
     const float scale_log2e = head_scale_log2e(HD);
-    attention_wgmma_kernel<HD, MASK><<<grid, THREADS, SMEM_BYTES, stream>>>(tq, tkv, out, S, W, kv_len, scale_log2e);
+    attention_wgmma_kernel<HD, MASK, false>
+        <<<grid, THREADS, SMEM_BYTES, stream>>>(tq, tkv, out, S, W, kv_len, scale_log2e, nullptr, 0);
+}
+
+// Q tiles of BQ rows and K / V tiles of BKV rows out of the packed qkv matrix
+template <int HD>
+void make_tmaps(const __nv_bfloat16* qkv, int B, int S, int W, CUtensorMap& tq, CUtensorMap& tkv) {
+    const uint64_t rows = (uint64_t)B * S;
+    const CUtensorMapSwizzle swz = HD == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    tq = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows, (uint64_t)3 * W * 2, HD, BQ, swz);
+    tkv = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows, (uint64_t)3 * W * 2, HD, BKV, swz);
 }
 
 template <int HD>
 void launch_hd(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask,
                const int32_t* kv_len, cudaStream_t stream) {
-    const uint64_t rows = (uint64_t)B * S;
-    const CUtensorMapSwizzle swz = HD == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-    const CUtensorMap tq = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows, (uint64_t)3 * W * 2,
-                                        HD, BQ, swz);
-    const CUtensorMap tkv = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows,
-                                         (uint64_t)3 * W * 2, HD, BKV, swz);
+    CUtensorMap tq, tkv;
+    make_tmaps<HD>(qkv, B, S, W, tq, tkv);
     switch (mask) {
         case MASK_NONE: launch_mask<HD, MASK_NONE>(tq, tkv, out, B, S, W, H, kv_len, stream); break;
         case MASK_CAUSAL: launch_mask<HD, MASK_CAUSAL>(tq, tkv, out, B, S, W, H, kv_len, stream); break;
@@ -244,6 +264,27 @@ int launch_wgmma(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int
         launch_hd<64>(qkv, out, B, S, W, H, mask, kv_len, stream);
     else
         launch_hd<32>(qkv, out, B, S, W, H, mask, kv_len, stream);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int launch_wgmma_rel_bias(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, const int32_t* kv_len,
+                          const RelBias& bias, cudaStream_t stream) {
+    constexpr int MAX_S = 1024;   // the shared-memory limit set once below covers the band of S <= MAX_S
+    if (B > 65535) fail(B200_ERR_UNSUPPORTED, "attention: batch %d is too large", B);
+    if (head_dim(W, H) != 64) fail(B200_ERR_UNSUPPORTED, "attention: the relative bias is built for head_dim 64 only");
+    if (S > MAX_S) fail(B200_ERR_UNSUPPORTED, "attention: the relative bias supports sequences of at most %d", MAX_S);
+    constexpr size_t BASE = Tiles<64>::SMEM_BYTES;
+    static std::once_flag once;
+    std::call_once(once, [] {
+        MB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel<64, MASK_KEYLEN, true>,
+                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(BASE + bias_band_bytes(MAX_S))));
+    });
+    CUtensorMap tq, tkv;
+    make_tmaps<64>(qkv, B, S, W, tq, tkv);
+    const dim3 grid((S + BQ - 1) / BQ, H, B);
+    attention_wgmma_kernel<64, MASK_KEYLEN, true><<<grid, THREADS, BASE + bias_band_bytes(S), stream>>>(
+        tq, tkv, out, S, W, kv_len, head_scale_log2e(64), bias.table, bias.smax);
     MB_CUDA(cudaGetLastError());
     return 1;
 }

@@ -252,6 +252,57 @@ void bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, c
     MB_CUDA(cudaGetLastError());
 }
 
+__global__ void __launch_bounds__(256) mpnet_embed_ln_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ mask,
+                                                             const float* __restrict__ word, const float* __restrict__ pos,
+                                                             const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                             float eps, int n, int S, int w, int vocab, int pad,
+                                                             float* __restrict__ x, __nv_bfloat16* __restrict__ h,
+                                                             int32_t* __restrict__ kv_len) {
+    const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (row >= (long long)n * S) return;
+    const int s = (int)(row % S);
+    const int32_t* seq = ids + (row - s);
+    // HF create_position_ids_from_input_ids: cumsum(ids != pad) * (ids != pad) + pad, from the ids, not the mask
+    int cnt = 0;
+    for (int j = lane; j <= s; j += 32) cnt += seq[j] != pad;
+    cnt = __reduce_add_sync(0xffffffffu, cnt);
+    int id = ids[row];
+    const int p = id != pad ? pad + cnt : pad;
+    id = min(max(id, 0), vocab - 1);
+    const int nv = w / 128;
+    const float4* w4 = reinterpret_cast<const float4*>(word + (long long)id * w);
+    const float4* p4 = reinterpret_cast<const float4*>(pos + (long long)p * w);
+    float4 v[LN_MAX_V4];
+#pragma unroll
+    for (int j = 0; j < LN_MAX_V4; ++j)
+        if (j < nv) {
+            const int i4 = lane + 32 * j;
+            const float4 a = __ldg(w4 + i4), b = __ldg(p4 + i4);
+            v[j] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);   // HF: inputs_embeds + position_embeddings
+        }
+    ln_row<true>(v, nv, w, gamma, beta, eps, lane, x + row * w, h + row * w);
+    if (s == 0 && lane == 0) {
+        int c = S;
+        if (mask) {
+            c = 0;
+            for (int j = 0; j < S; ++j) c += mask[row + j] != 0;
+        }
+        kv_len[row / S] = c;
+    }
+}
+
+void mpnet_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* gamma,
+                    const float* beta, float eps, int n, int S, int w, int vocab, int pad, float* x, __nv_bfloat16* h,
+                    int32_t* kv_len, cudaStream_t s) {
+    if (n <= 0) return;
+    check_ln_width(w);
+    const long long rows = (long long)n * S;
+    mpnet_embed_ln_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(ids, mask, word, pos, gamma, beta, eps, n, S, w, vocab,
+                                                                    pad, x, h, kv_len);
+    MB_CUDA(cudaGetLastError());
+}
+
 // ------------------------------------------------------------------------------------------------ heads
 __device__ __forceinline__ float block_sum_256(float v, float* red) {
     v = warp_sum(v);

@@ -1,4 +1,4 @@
-// Encoder runtime: CLIP ViT image tower, CLIP text tower, BERT (e5) — SURVEY §8 a2-a5.
+// Encoder runtime: CLIP ViT image tower, CLIP text tower, BERT (e5, MiniLM, bge), MPNet — SURVEY §8 a2-a5.
 //
 // What the reference calls (third-party, restated in oracle/encoders.py):
 //   OPEN_CLIP.encode_image / encode_text   src/marqo/core/inference/embedding_models/open_clip_model.py:249-286
@@ -15,6 +15,7 @@
 //   patches   bf16 [images * grid^2, kpad]  normalised im2col of the uint8 input (ToTensor + Normalize fused)
 // Every Linear is the wgmma GEMM of gemm.cu with bias / activation / residual-add fused into its epilogue.
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <map>
 #include <tuple>
@@ -51,6 +52,8 @@ struct TowerW {
     // text / bert embeddings
     const float *tok = nullptr, *type0 = nullptr, *emb_ln_w = nullptr, *emb_ln_b = nullptr;
     int max_pos = 0;
+    // MPNet: relative-position bias of every layer, fp32 [heads, 2 * max_pos - 1] pre-scaled by log2(e)
+    attention::RelBias rel_bias;
 };
 
 }  // namespace
@@ -157,7 +160,18 @@ void build_clip_layers(b200_model* m, TowerW& T, const std::string& prefix) {
     }
 }
 
-void build_bert_layers(b200_model* m, TowerW& T) {
+// Checkpoint names of the attention half of a post-LN layer: HF BertLayer and MPNetLayer differ only there.
+struct PostLnNames {
+    const char* qkv[3];    // query / key / value Linear, under encoder.layer.{i}.
+    const char* out;       // attention output Linear
+    const char* out_ln;    // LayerNorm after the attention residual
+};
+const PostLnNames BERT_NAMES{{"attention.self.query", "attention.self.key", "attention.self.value"},
+                             "attention.output.dense", "attention.output.LayerNorm"};
+const PostLnNames MPNET_NAMES{{"attention.attn.q", "attention.attn.k", "attention.attn.v"}, "attention.attn.o",
+                              "attention.LayerNorm"};
+
+void build_bert_layers(b200_model* m, TowerW& T, const PostLnNames& nm) {
     const long long w = T.d.width, mlp = T.d.mlp;
     T.layers.resize(T.d.layers);
     for (int i = 0; i < T.d.layers; ++i) {
@@ -166,21 +180,20 @@ void build_bert_layers(b200_model* m, TowerW& T) {
         // fuse query / key / value into one [3w, w] weight and one [3w] bias
         __nv_bfloat16* wq = derived_buffer<__nv_bfloat16>(m, (size_t)3 * w * w);
         float* bq = derived_buffer<float>(m, (size_t)3 * w);
-        const char* names[3] = {"query", "key", "value"};
         for (int j = 0; j < 3; ++j) {
-            const std::string base = p + "attention.self." + names[j];
+            const std::string base = p + nm.qkv[j];
             kernels::f32_to_bf16(param(m, base + ".weight", w * w), wq + (size_t)j * w * w, w * w, m->stream);
             MB_CUDA(cudaMemcpyAsync(bq + (size_t)j * w, param(m, base + ".bias", w), (size_t)w * 4, cudaMemcpyDeviceToDevice,
                                     m->stream));
         }
         MB_CUDA(cudaStreamSynchronize(m->stream));
-        for (int j = 0; j < 3; ++j) m->raw.erase(p + "attention.self." + names[j] + ".weight");
+        for (int j = 0; j < 3; ++j) m->raw.erase(p + nm.qkv[j] + ".weight");
         L.w_qkv = wq;
         L.b_qkv = bq;
-        L.w_o = to_bf16(m, p + "attention.output.dense.weight", w * w);
-        L.b_o = param(m, p + "attention.output.dense.bias", w);
-        L.ln1_w = param(m, p + "attention.output.LayerNorm.weight", w);  // post-LN after attention
-        L.ln1_b = param(m, p + "attention.output.LayerNorm.bias", w);
+        L.w_o = to_bf16(m, p + nm.out + ".weight", w * w);
+        L.b_o = param(m, p + nm.out + ".bias", w);
+        L.ln1_w = param(m, p + nm.out_ln + ".weight", w);  // post-LN after attention
+        L.ln1_b = param(m, p + nm.out_ln + ".bias", w);
         L.w_fc = to_bf16(m, p + "intermediate.dense.weight", mlp * w);
         L.b_fc = param(m, p + "intermediate.dense.bias", mlp);
         L.w_proj = to_bf16(m, p + "output.dense.weight", w * mlp);
@@ -188,6 +201,49 @@ void build_bert_layers(b200_model* m, TowerW& T) {
         L.ln2_w = param(m, p + "output.LayerNorm.weight", w);  // post-LN after the MLP
         L.ln2_b = param(m, p + "output.LayerNorm.bias", w);
     }
+}
+
+// Rows of a parameter stored as [rows, w]; its element count must be a multiple of w.
+long long param_rows(b200_model* m, const std::string& name, long long w) {
+    auto it = m->raw.find(name);
+    if (it == m->raw.end()) fail(B200_ERR_MISSING_WEIGHT, "missing parameter '%s'", name.c_str());
+    if ((long long)it->second.size() % w != 0)
+        fail(B200_ERR_INVALID_ARG, "parameter '%s' has %zu elements, not a multiple of %lld", name.c_str(),
+             it->second.size(), w);
+    return (long long)it->second.size() / w;
+}
+
+// transformers MPNetEncoder.relative_position_bucket for relative_position = key - query, in the same fp32 arithmetic:
+// n = query - key; keys after the query take the upper half of the buckets; |n| < half / 2 is exact, larger distances
+// are log-spaced up to max_distance, truncated toward zero.
+int relative_position_bucket(int rel, int num_buckets, int max_distance) {
+    const int half = num_buckets / 2, max_exact = half / 2;
+    const int base = rel > 0 ? half : 0;
+    const int n = rel < 0 ? -rel : rel;
+    if (n < max_exact) return base + n;
+    const float lg = std::log((float)n / (float)max_exact) / (float)std::log((double)max_distance / max_exact);
+    const int large = max_exact + (int)(lg * (float)(half - max_exact));
+    return base + std::min(large, half - 1);
+}
+
+// MPNet's relative-position bias, built once per handle: table[h][d + ctx - 1] = weight[bucket(d)][h] * log2(e) for
+// every key - query distance d of a sequence of up to ctx tokens.  Every layer reads the same table (a fixed pointer,
+// so captured CUDA graphs replay it).
+attention::RelBias build_rel_bias(b200_model* m, const TowerW& T) {
+    const int H = T.d.heads, nb = m->desc.rel_buckets, smax = T.d.ctx, span = 2 * smax - 1;
+    const float* w = param(m, "encoder.relative_attention_bias.weight", (long long)nb * H);
+    std::vector<float> wh((size_t)nb * H), table((size_t)H * span);
+    MB_CUDA(cudaMemcpy(wh.data(), w, wh.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    for (int d = -(smax - 1); d <= smax - 1; ++d) {
+        const int bucket = relative_position_bucket(d, nb, m->desc.rel_max_distance);
+        for (int h = 0; h < H; ++h) table[(size_t)h * span + d + smax - 1] = wh[(size_t)bucket * H + h] * 1.4426950408889634f;
+    }
+    float* dev = derived_buffer<float>(m, table.size());
+    MB_CUDA(cudaMemcpy(dev, table.data(), table.size() * sizeof(float), cudaMemcpyHostToDevice));
+    attention::RelBias b;
+    b.table = dev;
+    b.smax = smax;
+    return b;
 }
 
 struct Counter {
@@ -220,9 +276,13 @@ void linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, con
     ++c.n;
 }
 
-void attend(b200_model* m, Counter& c, int B, int S, int w, int heads, int mask_mode, const int32_t* kv_len) {
+void attend(b200_model* m, Counter& c, int B, int S, int w, int heads, int mask_mode, const int32_t* kv_len,
+            const attention::RelBias& bias = {}) {
     ProfScope ps(m, 1);
-    c.n += attention::launch(m->qkv.get(), m->o.get(), B, S, w, heads, mask_mode, kv_len, m->stream);
+    if (bias.table)
+        c.n += attention::launch_rel_bias(m->qkv.get(), m->o.get(), B, S, w, heads, kv_len, bias, m->stream);
+    else
+        c.n += attention::launch(m->qkv.get(), m->o.get(), B, S, w, heads, mask_mode, kv_len, m->stream);
 }
 
 // Pre-LN residual blocks (open_clip ResidualAttentionBlock).  x (fp32) is the residual stream, h (bf16) the LayerNorm
@@ -266,18 +326,17 @@ void run_clip_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, i
     }
 }
 
-// Post-LN blocks (HF BertLayer); on entry x (fp32) and h (bf16) both hold the embedding LayerNorm output.  Both
-// LayerNorms of a layer rewrite x in place.
-void run_bert_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S) {
+// Post-LN blocks (HF BertLayer, MPNetLayer with the tower's relative-position bias); on entry x (fp32) and h (bf16)
+// both hold the embedding LayerNorm output.  Both LayerNorms of a layer rewrite x in place.
+void run_bert_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, float eps) {
     const int M = B * S, w = T.d.width, mlp = T.d.mlp;
-    const float eps = 1e-12f;
     for (const LayerW& L : T.layers) {
         gemm::Epilogue e1;
         e1.bias = L.b_qkv;
         e1.out = m->qkv.get();
         e1.ldo = 3 * w;
         linear(m, c, m->h.get(), M, w, L.w_qkv, 3 * w, e1);
-        attend(m, c, B, S, w, T.d.heads, attention::MASK_KEYLEN, m->aux.get());
+        attend(m, c, B, S, w, T.d.heads, attention::MASK_KEYLEN, m->aux.get(), T.rel_bias);
         gemm::Epilogue e2;
         e2.bias = L.b_o;
         e2.residual = m->x.get();
@@ -363,11 +422,19 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
         kernels::clip_head(m->x.get(), S, m->aux.get(), T.ln_out_w, T.ln_out_b, 1e-5f, T.proj, n, w, m->desc.embed_dim,
                            normalize, d_out, m->pooled.get(), m->stream);
         c.n += 3;
+    } else if (m->desc.arch == B200_ARCH_MPNET) {
+        const float eps = m->desc.layer_norm_eps;
+        kernels::mpnet_embed_ln(d_ids, d_mask, T.tok, T.pos, T.emb_ln_w, T.emb_ln_b, eps, n, S, w, T.d.vocab,
+                                m->desc.pad_id, m->x.get(), m->h.get(), m->aux.get(), m->stream);
+        c.n += 1;
+        run_bert_blocks(m, c, T, n, S, eps);
+        kernels::bert_head(m->x.get(), m->aux.get(), n, S, w, m->desc.pool, normalize, d_out, m->stream);
+        c.n += 1;
     } else {
         kernels::bert_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, 1e-12f, n, S, w, T.d.vocab,
                                m->x.get(), m->h.get(), m->aux.get(), m->stream);
         c.n += 1;
-        run_bert_blocks(m, c, T, n, S);
+        run_bert_blocks(m, c, T, n, S, 1e-12f);
         kernels::bert_head(m->x.get(), m->aux.get(), n, S, w, m->desc.pool, normalize, d_out, m->stream);
         c.n += 1;
     }
@@ -496,7 +563,8 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         MB_CHECK_ARG(desc && out, "NULL argument");
         *out = nullptr;
         require_sm90_device(device);
-        MB_CHECK_ARG(desc->arch == B200_ARCH_CLIP || desc->arch == B200_ARCH_BERT, "unknown arch %d", desc->arch);
+        MB_CHECK_ARG(desc->arch == B200_ARCH_CLIP || desc->arch == B200_ARCH_BERT || desc->arch == B200_ARCH_MPNET,
+                     "unknown arch %d", desc->arch);
         MB_CHECK_ARG(desc->max_batch > 0, "max_batch must be positive");
         MB_CHECK_ARG(desc->embed_dim > 0 && desc->embed_dim <= 4096, "embed_dim out of range");
         const bool has_vision = desc->arch == B200_ARCH_CLIP && desc->vision.layers > 0;
@@ -511,8 +579,20 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         if (has_text) {
             check_tower(desc->text, "text");
             MB_CHECK_ARG(desc->text.ctx > 0 && desc->text.vocab > 0, "text.ctx and text.vocab must be positive");
-            if (desc->arch == B200_ARCH_BERT)
-                MB_CHECK_ARG(desc->embed_dim == desc->text.width, "BERT embed_dim must equal width");
+            if (desc->arch != B200_ARCH_CLIP)
+                MB_CHECK_ARG(desc->embed_dim == desc->text.width, "BERT / MPNet embed_dim must equal width");
+            if (desc->arch == B200_ARCH_MPNET) {
+                MB_CHECK_ARG(desc->text.width == desc->text.heads * 64, "MPNet: head_dim must be 64 (width %d, heads %d)",
+                             desc->text.width, desc->text.heads);
+                MB_CHECK_ARG(desc->layer_norm_eps > 0.f, "MPNet: layer_norm_eps must be positive");
+                MB_CHECK_ARG(desc->pad_id >= 0 && desc->pad_id < desc->text.vocab, "MPNet: pad_id %d out of range",
+                             desc->pad_id);
+                MB_CHECK_ARG(desc->rel_buckets >= 4 && desc->rel_buckets % 2 == 0 && desc->rel_max_distance > desc->rel_buckets / 4,
+                             "MPNet: bad relative-bias buckets (%d) / max distance (%d)", desc->rel_buckets,
+                             desc->rel_max_distance);
+                MB_CHECK_ARG(desc->text.ctx <= 1024, "MPNet: sequences of up to 1024 tokens are supported (ctx %d)",
+                             desc->text.ctx);
+            }
         }
         DeviceGuard g(device);
         std::unique_ptr<b200_model> m(new b200_model());   // released under the guard if the set-up fails
@@ -606,6 +686,18 @@ int b200_model_finalize(b200_model* m) {
                 T.ln_out_w = param(m, "ln_final.weight", w);
                 T.ln_out_b = param(m, "ln_final.bias", w);
                 T.proj = param(m, "text_projection", w * E);
+            } else if (m->desc.arch == B200_ARCH_MPNET) {
+                T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
+                // positions run pad_id + 1 .. pad_id + ctx (pads take pad_id): the table has at least ctx + pad_id + 1 rows
+                const long long pos_rows = param_rows(m, "embeddings.position_embeddings.weight", w);
+                MB_CHECK_ARG(pos_rows >= (long long)T.d.ctx + m->desc.pad_id + 1,
+                             "embeddings.position_embeddings has %lld rows; %d tokens with pad id %d need %d", pos_rows,
+                             T.d.ctx, m->desc.pad_id, T.d.ctx + m->desc.pad_id + 1);
+                T.pos = param(m, "embeddings.position_embeddings.weight", pos_rows * w);
+                T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
+                T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
+                build_bert_layers(m, T, MPNET_NAMES);
+                T.rel_bias = build_rel_bias(m, T);
             } else {
                 T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
                 T.pos = param(m, "embeddings.position_embeddings.weight", (long long)T.d.ctx * w);
@@ -613,7 +705,7 @@ int b200_model_finalize(b200_model* m) {
                 T.type0 = param(m, "embeddings.token_type_embeddings.weight", (long long)tv * w);  // row 0 is used
                 T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
                 T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
-                build_bert_layers(m, T);
+                build_bert_layers(m, T, BERT_NAMES);
             }
             max_tok = std::max(max_tok, (long long)m->desc.max_batch * T.d.ctx);
             max_w = std::max(max_w, w);
@@ -696,7 +788,7 @@ int b200_model_encode_tokens(b200_model* m, const int32_t* ids, const int32_t* a
         require_ready(m);
         MB_CHECK_ARG(ids && out, "NULL buffer");
         check_tokens_args(m, n, seq);
-        if (attn_mask && m->desc.arch == B200_ARCH_BERT) {
+        if (attn_mask && m->desc.arch != B200_ARCH_CLIP) {
             // the kernels implement prefix (right-padded) masks, which is what the tokenizer call at
             // hugging_face_model.py:179-185 produces
             for (int b = 0; b < n; ++b) {
@@ -801,6 +893,16 @@ int b200_model_profile(b200_model* m, float* gemm_ms, int* gemm_launches, float*
         *gemm_launches = cnt[0];
         *attention_ms = ms[1];
         *attention_launches = cnt[1];
+    });
+}
+
+int b200_debug_relative_position_buckets(int num_buckets, int max_distance, int max_len, int32_t* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(out != nullptr, "NULL buffer");
+        MB_CHECK_ARG(num_buckets >= 4 && num_buckets % 2 == 0 && max_distance > num_buckets / 4 && max_len > 0,
+                     "bad bucket parameters");
+        for (int d = -(max_len - 1); d <= max_len - 1; ++d)
+            out[d + max_len - 1] = relative_position_bucket(d, num_buckets, max_distance);
     });
 }
 

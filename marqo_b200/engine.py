@@ -289,12 +289,13 @@ def _to_numpy_f32(t) -> np.ndarray:
 
 
 class Encoder:
-    """A CLIP (vision + text towers) or BERT encoder resident on one GPU.
+    """A CLIP (vision + text towers), BERT or MPNet encoder resident on one GPU.
 
     `config` keys — CLIP: embed_dim, act ("gelu"|"quickgelu"), mean, std, vision{width,layers,heads,mlp,patch,
     image_size}, text{width,layers,heads,mlp,ctx,vocab};  BERT: width, layers, heads, mlp, vocab, max_pos, type_vocab,
-    pool ("mean"|"cls").  `weights` maps checkpoint parameter names (open_clip state_dict names / HF BertModel names) to
-    fp32 arrays or torch tensors.
+    pool ("mean"|"cls");  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
+    max_pos - pad_id - 1 tokens), pad_id, ln_eps, rel_buckets, rel_max_distance, pool.  `weights` maps checkpoint
+    parameter names (open_clip state_dict names / HF BertModel / MPNetModel names) to fp32 arrays or torch tensors.
     """
 
     def __init__(self, arch: str, config: dict, weights: dict, device: int = 0, max_batch: int = 256):
@@ -326,6 +327,18 @@ class Encoder:
             d.type_vocab = int(config.get("type_vocab", 2))
             d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"],
                                  config.get("max_pos", 512), config["vocab"], 0, 0)
+            self.image_size = 0
+        elif arch == "mpnet":
+            d.arch = N.ARCH_MPNET
+            d.embed_dim = int(config["width"])
+            d.pool = N.POOL_CLS if config.get("pool", "mean") == "cls" else N.POOL_MEAN
+            d.pad_id = int(config.get("pad_id", 1))
+            d.layer_norm_eps = float(config["ln_eps"])      # MPNetConfig's default (1e-12) is not the checkpoints' value
+            d.rel_buckets = int(config.get("rel_buckets", 32))
+            d.rel_max_distance = int(config.get("rel_max_distance", 128))
+            ctx = int(config.get("max_pos", 514)) - d.pad_id - 1
+            d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"], ctx, config["vocab"],
+                                 0, 0)
             self.image_size = 0
         else:
             raise ValueError(f"unknown arch {arch!r}")
@@ -536,11 +549,39 @@ def debug_patch_embed(images_u8, patch: int, conv_w, mean, std, pos=None, use_ga
     return out
 
 
-def debug_attention(qkv, B: int, S: int, W: int, H: int, mask: int = 0, kv_len=None, device: int = 0) -> np.ndarray:
+def debug_attention(qkv, B: int, S: int, W: int, H: int, mask: int = 0, kv_len=None, device: int = 0,
+                    rel_bias=None) -> np.ndarray:
+    """softmax(q k^T / sqrt(hd) + mask) v over packed qkv.  rel_bias: MPNet's relative-position bias, fp32
+    [H, 2 * smax - 1], adds rel_bias[h, j - i + smax - 1] to the logit of query i and key j (key-length mask only,
+    head_dim 64, S <= smax)."""
     q = _as(qkv, np.float32)
     kl = None if kv_len is None else _as(kv_len, np.int32)
     out = np.empty((B * S, W), np.float32)
-    N.check(N.load().b200_debug_attention(device, _ptr(q), B, S, W, H, mask, _ptr(kl), _ptr(out)))
+    if rel_bias is None:
+        N.check(N.load().b200_debug_attention(device, _ptr(q), B, S, W, H, mask, _ptr(kl), _ptr(out)))
+        return out
+    rb = _as(rel_bias, np.float32)
+    if mask != 2 or kl is None:
+        raise ValueError("the relative bias runs with the key-length mask (mask=2, kv_len)")
+    if rb.ndim != 2 or rb.shape[0] != H or rb.shape[1] % 2 != 1:
+        raise ValueError(f"expected rel_bias [{H}, 2 * smax - 1], got {rb.shape}")
+    N.check(N.load().b200_debug_attention_bias(device, _ptr(q), B, S, W, H, _ptr(kl), _ptr(rb), (rb.shape[1] + 1) // 2,
+                                               _ptr(out)))
+    return out
+
+
+def debug_attention_bias_time(B: int, S: int, W: int, H: int, iters: int = 20, device: int = 0) -> float:
+    """Mean device time (ms) of the biased attention launch on generated data."""
+    ms = C.c_float(0)
+    N.check(N.load().b200_debug_attention_bias_time(device, B, S, W, H, iters, C.byref(ms)))
+    return ms.value
+
+
+def relative_position_buckets(max_len: int, num_buckets: int = 32, max_distance: int = 128) -> np.ndarray:
+    """The bucket of every key - query distance d, |d| < max_len, as the MPNet runtime builds its bias table:
+    out[d + max_len - 1]."""
+    out = np.empty(2 * max_len - 1, np.int32)
+    N.check(N.load().b200_debug_relative_position_buckets(num_buckets, max_distance, max_len, _ptr(out)))
     return out
 
 

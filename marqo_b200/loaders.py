@@ -32,13 +32,15 @@ def _resolve_weights(props: dict, arch: dict, kind: str) -> Dict[str, np.ndarray
     w = props.get("weights")
     if w is None and props.get("random_init") is not None:
         seed = int(props["random_init"])
-        return weights_mod.random_clip_weights(arch, seed) if kind == "clip" else weights_mod.random_bert_weights(arch, seed)
+        random = {"clip": weights_mod.random_clip_weights, "bert": weights_mod.random_bert_weights,
+                  "mpnet": weights_mod.random_mpnet_weights}[kind]
+        return random(arch, seed)
     if w is None:
         raise ModelLoadError("model_properties needs `weights` (state dict or checkpoint path) or `random_init`; "
                              "checkpoint download is Marqo's job (open_clip_model.py:107-131) and out of scope here")
     if isinstance(w, (str, bytes)) or hasattr(w, "__fspath__"):
         w = weights_mod.load_state_dict(w)
-    if kind == "bert":
+    if kind in ("bert", "mpnet"):
         w = weights_mod.strip_hf_prefix(w)
     return w
 
@@ -284,15 +286,17 @@ class B200HuggingFace:
         if props.get("poolingMethod") or props.get("pooling_method"):  # hugging_face_model_properties.py
             arch = dict(arch, pool=(props.get("poolingMethod") or props.get("pooling_method")))
         self.arch = arch
-        self._model = Encoder("bert", arch, _resolve_weights(props, arch, "bert"), device=_validate_device(self.device),
+        kind = arch.get("kind", "bert")   # "mpnet": MPNetModel (model_registry.MPNET_MODELS); else BertModel
+        self._model = Encoder(kind, arch, _resolve_weights(props, arch, kind), device=_validate_device(self.device),
                               max_batch=int(props.get("max_batch", 256)))
         self._tokenizer = props.get("tokenizer") or self._default_tokenizer()
 
     def _default_tokenizer(self):
         if self.model_properties.get("vocab_file"):
-            from .tokenizers import WordPieceTokenizer
-            return WordPieceTokenizer(self.model_properties["vocab_file"],
-                                      do_lower_case=bool(self.model_properties.get("do_lower_case", True)))
+            from .tokenizers import MPNetTokenizer, WordPieceTokenizer
+            cls = MPNetTokenizer if self.arch.get("kind") == "mpnet" else WordPieceTokenizer
+            return cls(self.model_properties["vocab_file"],
+                       do_lower_case=bool(self.model_properties.get("do_lower_case", True)))
         try:
             from transformers import AutoTokenizer
             return AutoTokenizer.from_pretrained(self.model_properties["name"])
@@ -370,4 +374,4 @@ def register_with_marqo() -> None:
     """Install the two loader types into a live Marqo process (see INTEGRATION.md)."""
     from marqo.s2_inference import s2_inference as marqo_s2  # type: ignore
     marqo_s2.MODEL_PROPERTIES['loaders'].update(LOADERS)
-    marqo_s2.MODEL_PROPERTIES['models'].update(model_registry.MODELS)
+    marqo_s2.MODEL_PROPERTIES['models'].update(model_registry.all_models())

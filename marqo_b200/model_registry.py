@@ -14,11 +14,18 @@ width), mean-pooled:
     e5-small, e5-small-v2, e5-small-unsupervised, bge-small-en-v1.5                width  384, 12 layers, 12 heads
     e5-base, e5-base-v2, e5-base-unsupervised, bge-base-en-v1.5                    width  768, 12 layers, 12 heads
     e5-large, e5-large-v2, e5-large-unsupervised, bge-large-en-v1.5                width 1024, 24 layers, 16 heads
-The 384-wide models have head_dim 32, the others head_dim 64."""
+The 384-wide models have head_dim 32, the others head_dim 64.
+
+The MPNet entries (all-mpnet-base-v1/v2, all_datasets_v3/v4_mpnet-base; model_registry.py:630-641,668-679) live in a
+table of their own, MPNET_MODELS, behind `find_model` / `all_models`: they are MPNet-base checkpoints (`arch["kind"] ==
+"mpnet"`), which the same `b200_hf` loader serves with the MPNet runtime and tokenizer.  Their shapes come from the
+upstream config.json files and cannot be re-read offline (verify): width 768, 12 layers, 12 heads, mlp 3072, vocabulary
+30527, max_position_embeddings 514 (positions start after pad_token_id 1, so at most 512 tokens), layer_norm_eps 1e-5
+(MPNetConfig's default is 1e-12), 32 relative-attention buckets with max distance 128, mean pooling."""
 from __future__ import annotations
 
 import copy
-from typing import Dict
+from typing import Dict, Optional
 
 OPENAI_MEAN = (0.48145466, 0.4578275, 0.40821073)   # src/marqo/s2_inference/clip_utils.py:32-33
 OPENAI_STD = (0.26862954, 0.26130258, 0.27577711)
@@ -112,9 +119,41 @@ def _models() -> Dict[str, dict]:
 MODELS: Dict[str, dict] = _models()
 
 
+def _mpnet_arch() -> dict:
+    """MPNet-base (module docstring, verify)."""
+    return {"kind": "mpnet", "width": 768, "layers": 12, "heads": 12, "mlp": 3072, "vocab": 30527, "max_pos": 514,
+            "pad_id": 1, "ln_eps": 1e-5, "rel_buckets": 32, "rel_max_distance": 128, "pool": "mean"}
+
+
+def _mpnet_models() -> Dict[str, dict]:
+    m: Dict[str, dict] = {}
+    for short, repo in (("all-mpnet-base-v1", "sentence-transformers/all-mpnet-base-v1"),
+                        ("all-mpnet-base-v2", "sentence-transformers/all-mpnet-base-v2"),
+                        ("all_datasets_v3_mpnet-base", "flax-sentence-embeddings/all_datasets_v3_mpnet-base"),
+                        ("all_datasets_v4_mpnet-base", "flax-sentence-embeddings/all_datasets_v4_mpnet-base")):
+        m[f"hf/{short}"] = {"name": repo, "dimensions": 768, "tokens": 128, "type": TYPE_HF, "notes": "",
+                            "arch": _mpnet_arch()}
+    return m
+
+
+MPNET_MODELS: Dict[str, dict] = _mpnet_models()
+
+
+def find_model(model_name: str) -> Optional[dict]:
+    """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
+    entry = MODELS.get(model_name)
+    return entry if entry is not None else MPNET_MODELS.get(model_name)
+
+
+def all_models() -> Dict[str, dict]:
+    """Every served registry entry by name (a new dict over the same entries)."""
+    return {**MODELS, **MPNET_MODELS}
+
+
 def get_model_properties(model_name: str) -> dict:
     from .errors import UnknownModelError
-    if model_name not in MODELS:
+    entry = find_model(model_name)
+    if entry is None:
         raise UnknownModelError(f"Could not find model properties in model registry for model={model_name}. "
                                 f"Model is not supported by default.")
-    return copy.deepcopy(MODELS[model_name])
+    return copy.deepcopy(entry)

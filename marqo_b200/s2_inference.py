@@ -102,9 +102,9 @@ def validate_model_properties(model_name: str, model_properties: Optional[dict])
         raise InvalidModelPropertiesError(
             f"model type `{mtype}` is not served by the H100 engine (supported: open_clip, hf)")
     if "arch" not in props:
-        base = model_registry.MODELS.get(model_name)
+        base = model_registry.find_model(model_name)
         if base is None:
-            base = next((e for e in model_registry.MODELS.values() if e["name"] == props.get("name")), None)
+            base = next((e for e in model_registry.all_models().values() if e["name"] == props.get("name")), None)
         if base is None:
             raise InvalidModelPropertiesError(
                 f"model_properties for {model_name} needs an `arch` block (or a registry name) to size the encoder")

@@ -3,6 +3,8 @@
 * `WordPieceTokenizer` is called the way hugging_face_model.py:179-185 calls its AutoTokenizer:
   `tok(sentences, padding=True, truncation=True, max_length=N, return_tensors="np")` -> {input_ids, attention_mask,
   token_type_ids}.
+* `MPNetTokenizer` is the same WordPiece pipeline with MPNetTokenizer's special tokens ("<s> A </s>", <pad>, [UNK]) and
+  the same call -> {input_ids, attention_mask}.
 * `ClipBpeTokenizer` is called the way open_clip_model.py:277-279 calls open_clip's tokenizer:
   `tok(texts) -> int64 [n, context_length]`.
 
@@ -64,6 +66,8 @@ def _read(path_or_bytes: Union[str, Path, bytes]) -> bytes:
 
 
 class WordPieceTokenizer(_Tokenizer):
+    _token_type_ids = True
+
     def __init__(self, vocab: Union[str, Path, bytes], do_lower_case: bool = True, model_max_length: int = 512):
         data = _read(vocab)
         h = C.c_void_p()
@@ -77,12 +81,32 @@ class WordPieceTokenizer(_Tokenizer):
             raise ValueError("WordPieceTokenizer implements the reference's call only: padding=True, truncation=True")
         single = isinstance(sentences, str)
         ids, mask = self._encode([sentences] if single else list(sentences), max_length or self.model_max_length)
-        out = {"input_ids": ids.astype(np.int64), "token_type_ids": np.zeros_like(ids, dtype=np.int64),
-               "attention_mask": mask.astype(np.int64)}
+        out = {"input_ids": ids.astype(np.int64)}
+        if self._token_type_ids:
+            out["token_type_ids"] = np.zeros_like(ids, dtype=np.int64)
+        out["attention_mask"] = mask.astype(np.int64)
         if return_tensors == "pt":
             import torch
             return {k: torch.from_numpy(v) for k, v in out.items()}
         return out
+
+
+class MPNetTokenizer(WordPieceTokenizer):
+    """transformers' MPNetTokenizer on a vocab.txt: BertNormalizer + BertPreTokenizer + WordPiece with [UNK], rows
+    "<s> A </s>" padded with <pad>; the added special tokens matched in the raw text are exactly SPECIALS ("[CLS]",
+    "[SEP]", "[MASK]" and "<unk>" are ordinary text).  No token_type_ids."""
+    SPECIALS = ("<s>", "<pad>", "</s>", "[UNK]", "<mask>")
+    _token_type_ids = False
+
+    def __init__(self, vocab: Union[str, Path, bytes], do_lower_case: bool = True, model_max_length: int = 512):
+        data = _read(vocab)
+        specials = (C.c_char_p * len(self.SPECIALS))(*[t.encode() for t in self.SPECIALS])
+        h = C.c_void_p()
+        N.check(N.load().b200_tokenizer_create_wordpiece_ex(data, len(data), 1 if do_lower_case else 0, b"<s>", b"</s>",
+                                                            b"<pad>", b"[UNK]", C.cast(specials, C.c_void_p),
+                                                            len(self.SPECIALS), C.byref(h)))
+        _Tokenizer.__init__(self, h)
+        self.model_max_length = model_max_length
 
 
 class ClipBpeTokenizer(_Tokenizer):

@@ -33,9 +33,11 @@ def load_state_dict(path: str) -> Dict[str, np.ndarray]:
 
 
 def strip_hf_prefix(sd: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
-    """HF checkpoints saved from BertForXxx carry a 'bert.' prefix; BertModel checkpoints do not."""
-    if any(k.startswith("bert.") for k in sd):
-        return {k[len("bert."):]: v for k, v in sd.items() if k.startswith("bert.")}
+    """HF checkpoints saved from BertForXxx / MPNetForXxx carry a 'bert.' / 'mpnet.' prefix; BertModel and MPNetModel
+    checkpoints do not."""
+    for prefix in ("bert.", "mpnet."):
+        if any(k.startswith(prefix) for k in sd):
+            return {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
     return sd
 
 
@@ -115,6 +117,35 @@ def random_bert_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
         sd[p + "attention.output.dense.bias"] = _vec(g, w)
         sd[p + "attention.output.LayerNorm.weight"] = _vec(g, w, 0.1, 1.0)
         sd[p + "attention.output.LayerNorm.bias"] = _vec(g, w)
+        sd[p + "intermediate.dense.weight"] = _lin(g, mlp, w)
+        sd[p + "intermediate.dense.bias"] = _vec(g, mlp)
+        sd[p + "output.dense.weight"] = _lin(g, w, mlp)
+        sd[p + "output.dense.bias"] = _vec(g, w)
+        sd[p + "output.LayerNorm.weight"] = _vec(g, w, 0.1, 1.0)
+        sd[p + "output.LayerNorm.bias"] = _vec(g, w)
+    return sd
+
+
+def random_mpnet_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
+    """Seeded random weights under HF MPNetModel parameter names (arch: the registry's MPNet block)."""
+    g = _rng(seed)
+    w, mlp = arch["width"], arch["mlp"]
+    sd: Dict[str, np.ndarray] = {}
+    sd["embeddings.word_embeddings.weight"] = g.standard_normal((arch["vocab"], w), dtype=np.float32)
+    sd["embeddings.position_embeddings.weight"] = 0.5 * g.standard_normal((arch["max_pos"], w), dtype=np.float32)
+    sd["embeddings.LayerNorm.weight"] = _vec(g, w, 0.1, 1.0)
+    sd["embeddings.LayerNorm.bias"] = _vec(g, w)
+    sd["encoder.relative_attention_bias.weight"] = _vec(g, arch.get("rel_buckets", 32) * arch["heads"], 1.0).reshape(
+        -1, arch["heads"])
+    for i in range(arch["layers"]):
+        p = f"encoder.layer.{i}."
+        for nm in ("q", "k", "v"):
+            sd[p + f"attention.attn.{nm}.weight"] = _lin(g, w, w, 1.5)
+            sd[p + f"attention.attn.{nm}.bias"] = _vec(g, w)
+        sd[p + "attention.attn.o.weight"] = _lin(g, w, w)
+        sd[p + "attention.attn.o.bias"] = _vec(g, w)
+        sd[p + "attention.LayerNorm.weight"] = _vec(g, w, 0.1, 1.0)
+        sd[p + "attention.LayerNorm.bias"] = _vec(g, w)
         sd[p + "intermediate.dense.weight"] = _lin(g, mlp, w)
         sd[p + "intermediate.dense.bias"] = _vec(g, mlp)
         sd[p + "output.dense.weight"] = _lin(g, w, mlp)

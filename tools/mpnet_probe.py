@@ -1,0 +1,101 @@
+"""Dev probe for the MPNet embedders (hf/all-mpnet-base-*), not a bench line.  Needs a GPU; prints JSON lines.
+
+  1. attention kernel alone at the MPNet-base shape (12 heads of 64, key-length mask, every key valid), with and without
+     the relative-position bias (b200_debug_attention_bias_time / b200_debug_attention_time);
+  2. device-resident forward (ids on the device, mean pooling + L2 normalise, seeded weights) vs transformers'
+     MPNetModel built from the same config and weights, in fp32 (what the reference runs on CUDA) and in bf16.
+Times are host clocks around `iters` calls that end in a device synchronise, after `warmup` calls of the same shape.
+
+    python tools/mpnet_probe.py [iters]
+"""
+import ctypes as C
+import json
+import subprocess
+import sys
+import time
+
+import torch
+
+sys.path.insert(0, ".")
+from marqo_b200 import _native as N, model_registry as R, weights as Wt  # noqa: E402
+from marqo_b200.engine import Encoder, debug_attention_bias_time  # noqa: E402
+
+ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 50
+WARMUP = 5
+NAME = "hf/all-mpnet-base-v2"
+
+
+def _card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
+    name, power, clock = (x.strip() for x in q.split(","))
+    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
+
+
+def _wall(fn, iters):
+    for _ in range(WARMUP):
+        fn()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(iters):
+        fn()
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) / iters * 1e3
+
+
+def attention(B, S, H=12, hd=64):
+    W = H * hd
+    ms = C.c_float(0)
+    N.check(N.load().b200_debug_attention_time(0, B, S, W, H, 2, ITERS, C.byref(ms)))
+    biased = debug_attention_bias_time(B, S, W, H, ITERS)
+    return {"probe": "attention", "B": B, "S": S, "H": H, "head_dim": hd, "no_bias_us": ms.value * 1e3,
+            "rel_bias_us": biased * 1e3, "bias_overhead": biased / ms.value - 1.0}
+
+
+def forward(B, S):
+    from transformers import MPNetConfig, MPNetModel
+    arch = R.get_model_properties(NAME)["arch"]
+    sd = Wt.random_mpnet_weights(arch, 1234)
+    enc = Encoder("mpnet", arch, sd, max_batch=B)
+    g = torch.Generator(device="cuda").manual_seed(0)
+    ids = torch.randint(5, arch["vocab"], (B, S), dtype=torch.int32, device="cuda", generator=g)
+    out = torch.empty(B, arch["width"], dtype=torch.float32, device="cuda")
+    engine = _wall(lambda: enc.encode_tokens_device(ids.data_ptr(), None, B, S, out.data_ptr()), ITERS)
+    hc = MPNetConfig(vocab_size=arch["vocab"], hidden_size=arch["width"], num_hidden_layers=arch["layers"],
+                     num_attention_heads=arch["heads"], intermediate_size=arch["mlp"],
+                     max_position_embeddings=arch["max_pos"], pad_token_id=arch["pad_id"], layer_norm_eps=arch["ln_eps"],
+                     relative_attention_num_buckets=arch["rel_buckets"], hidden_act="gelu")
+    model = MPNetModel(hc, add_pooling_layer=False).cuda().eval()
+    model.load_state_dict({k: torch.from_numpy(v) for k, v in sd.items()}, strict=False)
+    ids64, mask = ids.long(), torch.ones(B, S, dtype=torch.long, device="cuda")
+
+    def hf():
+        with torch.no_grad():
+            last = model(input_ids=ids64, attention_mask=mask).last_hidden_state
+            emb = (last * mask[..., None]).sum(1) / mask.sum(1, keepdim=True)
+            return torch.nn.functional.normalize(emb.float(), dim=-1)
+
+    ref32 = hf()
+    fp32 = _wall(hf, ITERS)
+    model = model.to(torch.bfloat16)
+    bf16 = _wall(hf, ITERS)
+    cos = float(torch.nn.functional.cosine_similarity(out.double(), ref32.double(), dim=-1).min())
+    enc.close()
+    return {"probe": "forward", "model": NAME, "B": B, "S": S, "hf_attention": model.config._attn_implementation,
+            "engine_ms": engine, "hf_fp32_ms": fp32, "hf_bf16_ms": bf16, "engine_items_per_s": B / engine * 1e3,
+            "hf_fp32_items_per_s": B / fp32 * 1e3, "hf_bf16_items_per_s": B / bf16 * 1e3, "min_cos_vs_hf_fp32": cos}
+
+
+def main():
+    if not torch.cuda.is_available() or N.device_count() < 1:
+        sys.exit("mpnet_probe: needs an sm_90 GPU")
+    torch.backends.cuda.matmul.allow_tf32 = False
+    print(json.dumps(_card()), flush=True)
+    for B, S in ((256, 128), (64, 512)):
+        print(json.dumps(attention(B, S)), flush=True)
+    for B, S in ((256, 128), (1, 16), (64, 512)):
+        print(json.dumps(forward(B, S)), flush=True)
+
+
+if __name__ == "__main__":
+    main()
