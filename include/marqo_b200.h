@@ -409,9 +409,12 @@ int b200_debug_gemm_ln(int device, const float* A, const float* W, const float* 
                        float* out_ln);
 /* GEMM into an existing output buffer: io fp32 [out_rows, ldo] (out_rows >= M, ldo >= N) is uploaded (as bf16 when
  * out_bf16 != 0), rows [0, M) x columns [0, N) are overwritten with act(A W^T + bias) (+ the old contents when
- * residual_in_place != 0: residual == out, fp32 only), and the whole buffer is copied back into io. */
+ * residual_in_place != 0: residual == out, fp32 only), and the whole buffer is copied back into io.  The library picks
+ * the kernel by its usual rule for an SM count of sms (0: the device's own); *kernel_out (when not NULL) receives the
+ * kernel it ran: 0 the 128 x 128 tiles, 1 the persistent 128 x 256 tiles. */
 int b200_debug_gemm_into(int device, const float* A, const float* W, const float* bias, int M, int N, int K, int act,
-                         int out_bf16, int residual_in_place, int out_rows, int ldo, float* io);
+                         int out_bf16, int residual_in_place, int out_rows, int ldo, int sms, float* io,
+                         int* kernel_out);
 /* Mean device time (ms, CUDA events) of `iters` back-to-back GEMM launches [M,K] x [N,K]^T on device-generated data,
  * with the epilogue given by act, out_bf16, has_bias and residual_in_place (residual == out, fp32 only). */
 int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16, int has_bias, int residual_in_place,

@@ -192,10 +192,11 @@ int b200_debug_gemm(int device, const float* A, const float* W, const float* bia
 }
 
 int b200_debug_gemm_into(int device, const float* A, const float* W, const float* bias, int M, int N, int K, int act,
-                         int out_bf16, int residual_in_place, int out_rows, int ldo, float* io) {
+                         int out_bf16, int residual_in_place, int out_rows, int ldo, int sms, float* io,
+                         int* kernel_out) {
     return guarded([&] {
         MB_CHECK_ARG(A && W && io, "NULL buffer");
-        MB_CHECK_ARG(M > 0 && N > 0 && K > 0 && out_rows >= M && ldo >= N, "bad shape");
+        MB_CHECK_ARG(M > 0 && N > 0 && K > 0 && out_rows >= M && ldo >= N && sms >= 0, "bad shape");
         MB_CHECK_ARG(!(residual_in_place && out_bf16), "the in-place residual is fp32");
         require_device(device);
         DeviceGuard g(device);
@@ -215,7 +216,8 @@ int b200_debug_gemm_into(int device, const float* A, const float* W, const float
             ep.residual = dIo;
             ep.ldr = ldo;
         }
-        gemm::launch(dA, K, dW, M, N, K, ep, sm_count(device), sc.s);
+        const int kernel = gemm::launch(dA, K, dW, M, N, K, ep, sms > 0 ? sms : sm_count(device), sc.s);
+        if (kernel_out) *kernel_out = kernel;
         if (out_bf16) bf16_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, sc.s>>>(dIoB, dIo, (long long)n);
         MB_CUDA(cudaGetLastError());
         MB_CUDA(cudaStreamSynchronize(sc.s));

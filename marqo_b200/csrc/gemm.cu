@@ -123,9 +123,12 @@ __device__ __forceinline__ float gelu_erf(float x) {
 
 // The same erf-GELU on TWO elements per instruction (HFMA2 / ex2.approx.f16x2), for outputs that are rounded to bf16 anyway
 // (fc1's epilogue: the r02 profile had it at 16 fp32 instructions per element and the GEMM epilogue-bound at 75 % tensor
-// pipe).  fp16 has 11 significand bits against bf16's 8: the result carries ~1e-3 relative error before the bf16 rounding
-// of 4e-3 (tests/test_kernels_gpu.py::test_gemm_epilogues; the reference's own CUDA path evaluates GELU in fp16 under
-// torch.autocast, open_clip_model.py:256-258).  |x| up to 360 keeps a * a inside fp16 range.
+// pipe).  The error is absolute, not relative: fp16 roundings of 2^-11 (of 1 - e, of ex2's argument and result, of the
+// final fma) scale with |x| / 2, so the bf16 result y obeys |y - GELU(x)| <= 2^-8 |GELU(x)| + 2^-9 |x| + 2^-24 (bf16
+// rounding, fp16 evaluation, fp16 subnormal spacing; tests/test_gemm_shapes_gpu.py::test_activation_edges).  In the
+// negative tail that is far from relative: x = -3 gives -0.00439 for -0.00405.  The reference's own CUDA path
+// evaluates GELU in fp16 under torch.autocast too (open_clip_model.py:256-258).  Past |x| = 360 a * a overflows to
+// inf and the result is x or 0, as it should be; |x| >= 65520 is an fp16 infinity, which act() keeps away from here.
 __device__ __forceinline__ __half2 gelu_erf_h2(__half2 x) {
     const __half2 a = __hmul2(x, __float2half2_rn(0.70710678118654752440f));
     const __half2 t = __habs2(a);
@@ -183,9 +186,14 @@ __device__ __forceinline__ void warpgroup_sync(int wg) {
 // gelu_erf_h2), an fp32 output in fp32.
 template <bool OUT_FP32, int ACT>
 __device__ __forceinline__ float2 act(float x0, float x1) {
-    if constexpr (ACT == ACT_GELU && !OUT_FP32)
-        return __half22float2(gelu_erf_h2(__floats2half2_rn(x0, x1)));
-    else if constexpr (ACT == ACT_GELU)
+    if constexpr (ACT == ACT_GELU && !OUT_FP32) {
+        // |x| >= 65520 rounds to an fp16 infinity, which gelu_erf_h2 turns into +inf or NaN; beyond the fp16 range
+        // GELU(x) is x or -0 to far better than bf16 precision, so those elements take it in fp32
+        float2 y = __half22float2(gelu_erf_h2(__floats2half2_rn(x0, x1)));
+        y.x = x0 >= 65504.f ? x0 : x0 <= -65504.f ? -0.f : y.x;
+        y.y = x1 >= 65504.f ? x1 : x1 <= -65504.f ? -0.f : y.y;
+        return y;
+    } else if constexpr (ACT == ACT_GELU)
         return make_float2(gelu_erf(x0), gelu_erf(x1));
     else if constexpr (ACT == ACT_QUICKGELU)
         return make_float2(quick_gelu(x0), quick_gelu(x1));
@@ -705,9 +713,9 @@ void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, c
     launch_tiles<true, false, true, ACT_NONE>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
 }
 
-void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep, int sms,
-            cudaStream_t stream) {
-    if (M <= 0 || N <= 0) return;
+int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep, int sms,
+           cudaStream_t stream) {
+    if (M <= 0 || N <= 0) return KERNEL_NONE;
     if (K <= 0 || K % BK != 0) fail(B200_ERR_INTERNAL, "gemm: K = %d must be a positive multiple of %d", K, BK);
     if (N % 32 != 0) fail(B200_ERR_INTERNAL, "gemm: N = %d must be a multiple of 32", N);
     if (lda % 8 != 0 || ep.ldo % 8 != 0) fail(B200_ERR_INTERNAL, "gemm: leading dimensions must be multiples of 8");
@@ -716,7 +724,7 @@ void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int 
             fail(B200_ERR_INTERNAL, "gemm: fp32 token scatter without bias, activation or residual only");
         configure();
         launch_tiles<false, false, true, ACT_NONE>(A, lda, W, M, N, K, ep, stream);
-        return;
+        return KERNEL_128x128;
     }
     // TMA: 16-byte aligned bases and row pitches
     if ((reinterpret_cast<uintptr_t>(ep.out) & 15) != 0) fail(B200_ERR_INTERNAL, "gemm: output not 16-byte aligned");
@@ -738,6 +746,7 @@ void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int 
         else
             launch_tiles<false, true, OUT_FP32, ACT>(A, lda, W, M, N, K, ep, stream);
     });
+    return persistent ? KERNEL_PERSISTENT : KERNEL_128x128;
 }
 
 }  // namespace gemm

@@ -29,8 +29,11 @@ struct Epilogue {
 
 // A: bf16 [M, K] row-major with leading dimension lda (elements); W: bf16 [N, K] row-major (nn.Linear layout).
 // Requirements: K % 64 == 0, N % 32 == 0, lda % 8 == 0.
-void launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep,
-            int sm_count, cudaStream_t stream);
+// Returns the kernel it launched: KERNEL_PERSISTENT for K >= 1024, N % 256 == 0 and at least sm_count 128 x 256 tiles,
+// KERNEL_128x128 otherwise, KERNEL_NONE when M or N is 0.
+enum Kernel { KERNEL_NONE = -1, KERNEL_128x128 = 0, KERNEL_PERSISTENT = 1 };
+int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep,
+           int sm_count, cudaStream_t stream);
 
 // ViT patch embedding straight from uint8 pixels (SURVEY §8 a2; add_docs.py:129-134 + clip_utils.py:48-67 fused into the
 // conv1 GEMM's operand load): out = epilogue( patches(img) x Wg^T ), where row r of the virtual A matrix is patch r of the

@@ -503,18 +503,22 @@ def debug_gemm(A, W, bias=None, residual=None, act: int = 0, out_bf16: bool = Fa
 
 
 def debug_gemm_into(A, W, io, bias=None, act: int = 0, out_bf16: bool = False, residual_in_place: bool = False,
-                    device: int = 0) -> np.ndarray:
+                    sms: Optional[int] = None, return_kernel: bool = False, device: int = 0):
     """GEMM into a copy of io (fp32 [rows >= M, cols >= N], bf16 on the device when out_bf16): rows [0, M) x columns
     [0, N) become act(A W^T + bias), plus their old values when residual_in_place (residual == out); the rest of the
-    buffer is returned as the kernel left it."""
+    buffer is returned as the kernel left it.  The kernel is chosen by the library's rule for an SM count of sms (None:
+    the device's own).  Returns the buffer, or with return_kernel (the buffer, the kernel that ran:
+    _native.GEMM_128x128 or _native.GEMM_PERSISTENT)."""
     A, W = _as(A, np.float32), _as(W, np.float32)
     M, K = A.shape
     Nn = W.shape[0]
     b = None if bias is None else _as(bias, np.float32)
     out = np.array(io, dtype=np.float32, order="C", copy=True)
+    kernel = C.c_int(-1)
     N.check(N.load().b200_debug_gemm_into(device, _ptr(A), _ptr(W), _ptr(b), M, Nn, K, act, int(out_bf16),
-                                          int(residual_in_place), out.shape[0], out.shape[1], _ptr(out)))
-    return out
+                                          int(residual_in_place), out.shape[0], out.shape[1], sms or 0, _ptr(out),
+                                          C.byref(kernel)))
+    return (out, kernel.value) if return_kernel else out
 
 
 def debug_gemm_ln(A, W, bias, residual, gamma, beta, eps: float, in_place: bool = False, repeats: int = 1,

@@ -6,6 +6,8 @@ import math
 import pytest
 import torch
 
+from marqo_b200._native import GEMM_128x128
+
 pytestmark = pytest.mark.gpu
 
 SENTINEL = -7.5      # exact in bf16 and fp32
@@ -50,8 +52,10 @@ def test_gemm_epilogue_into_buffer(gpu_required, M, N, K, act, out_bf16, residua
     res = torch.randn(M, N, generator=g)
     if residual:
         io[:M, :N] = res
-    got = torch.from_numpy(debug_gemm_into(A.numpy(), W.numpy(), io.numpy(), None if b is None else b.numpy(), act=act,
-                                           out_bf16=bool(out_bf16), residual_in_place=residual))
+    got, kernel = debug_gemm_into(A.numpy(), W.numpy(), io.numpy(), None if b is None else b.numpy(), act=act,
+                                  out_bf16=bool(out_bf16), residual_in_place=residual, return_kernel=True)
+    assert kernel == GEMM_128x128, "the shape no longer runs the 128 x 128 kernel"
+    got = torch.from_numpy(got)
     z = A.double() @ W.double().t()
     if b is not None:
         z = z + b.double()

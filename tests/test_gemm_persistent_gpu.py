@@ -8,6 +8,8 @@ import math
 import pytest
 import torch
 
+from marqo_b200._native import GEMM_PERSISTENT
+
 pytestmark = pytest.mark.gpu
 
 SENTINEL = -7.5      # exact in bf16 and fp32
@@ -47,8 +49,10 @@ def test_persistent_gemm_into_buffer(gpu_required, M, N, K, act, out_bf16, resid
     res = torch.randn(M, N, generator=g)
     if residual:
         io[:M, :N] = res
-    got = torch.from_numpy(debug_gemm_into(A.numpy(), W.numpy(), io.numpy(), b.numpy(), act=act,
-                                           out_bf16=bool(out_bf16), residual_in_place=residual))
+    got, kernel = debug_gemm_into(A.numpy(), W.numpy(), io.numpy(), b.numpy(), act=act, out_bf16=bool(out_bf16),
+                                  residual_in_place=residual, return_kernel=True)
+    assert kernel == GEMM_PERSISTENT, "the shape no longer runs the persistent kernel"
+    got = torch.from_numpy(got)
     ref = _act(A.double() @ W.double().t() + b.double(), act)
     if residual:
         ref = ref + res.double()
