@@ -74,7 +74,8 @@ enum b200_metric {
 };
 
 /* Create an empty row store of fp16[capacity_rows, dim] on `device` (grows on demand).
- * dim must be a multiple of 64 and <= 1024. */
+ * dim must be a multiple of 64 and <= 4096; any other dim returns B200_ERR_INVALID_ARG.  Up to 1024 the scan keeps the
+ * query block resident in shared memory; above it the query block is streamed beside the corpus. */
 int b200_index_create(int device, int dim, int metric, int64_t capacity_rows, b200_index** out);
 int b200_index_destroy(b200_index* ix);
 
@@ -415,6 +416,11 @@ int b200_debug_gemm_ln(int device, const float* A, const float* W, const float* 
 int b200_debug_gemm_into(int device, const float* A, const float* W, const float* bias, int M, int N, int K, int act,
                          int out_bf16, int residual_in_place, int out_rows, int ldo, int sms, float* io,
                          int* kernel_out);
+/* Scan kernel of a row store.  force_streamed: 1 makes every later search of ix scan with the streamed-query kernel
+ * whatever its dim (so both kernels can run on one corpus), 0 restores the library's rule (resident query block up to
+ * dim 1024, streamed above), -1 leaves the setting unchanged.  *last_kernel (when not NULL) receives the kernel the last
+ * search ran: 0 resident query block, 1 streamed query block, -1 no search yet. */
+int b200_debug_index_scan_kernel(b200_index* ix, int force_streamed, int* last_kernel);
 /* Mean device time (ms, CUDA events) of `iters` back-to-back GEMM launches [M,K] x [N,K]^T on device-generated data,
  * with the epilogue given by act, out_bf16, has_bias and residual_in_place (residual == out, fp32 only). */
 int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16, int has_bias, int residual_in_place,

@@ -5,6 +5,7 @@
 #include "common.cuh"
 #include "gemm.cuh"
 #include "kernels.cuh"
+#include "score.cuh"
 
 using namespace mb;
 
@@ -223,6 +224,10 @@ int b200_debug_gemm_into(int device, const float* A, const float* W, const float
         MB_CUDA(cudaStreamSynchronize(sc.s));
         MB_CUDA(cudaMemcpy(io, dIo, n * 4, cudaMemcpyDeviceToHost));
     });
+}
+
+int b200_debug_index_scan_kernel(b200_index* ix, int force_streamed, int* last_kernel) {
+    return guarded([&] { score::debug_scan_kernel(ix, force_streamed, last_kernel); });
 }
 
 int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16, int has_bias, int residual_in_place,

@@ -7,8 +7,9 @@
 //
 // Pipeline per group of <= 64 queries:
 //   1. scan_kernel<SELECT>  persistent, one CTA per SM.  The corpus is streamed once from HBM by TMA (128-byte
-//        swizzle, 16 KB stages) and multiplied against the smem-resident query block by one wgmma warpgroup (M = 64
-//        queries, N = 128 rows, fp16 x fp16 -> fp32), which stores each tile's scores to shared memory.  Four
+//        swizzle, 16 KB stages) and multiplied against the query block by one wgmma warpgroup (M = 64 queries,
+//        N = 128 rows, fp16 x fp16 -> fp32), which stores each tile's scores to shared memory.  Up to dim 1024 the
+//        query block is resident in shared memory; above it each stage carries its query k-block (STREAM_Q).  Four
 //        epilogue warps read them back (one thread per query) and each keeps a sorted register list of the KP best
 //        (key, row, doc) of its query.  Rows of a document that is already listed are dropped only when they are PROVABLY not its best
 //        chunk (approximate key more than tol = 2 eps below the listed one).
@@ -37,6 +38,7 @@
 
 #include "common.cuh"
 #include "ptx.cuh"
+#include "score.cuh"
 
 namespace mb {
 namespace score {
@@ -56,7 +58,7 @@ constexpr int ACC_LD = TILE_N + 4;   // fp32 row pitch of the smem accumulator t
 constexpr int THREADS = 288;    // warps 0-3 epilogue, warps 4-7 MMA warpgroup, warp 8 TMA
 constexpr uint32_t STAGE_BYTES = TILE_N * BLOCK_K * 2;
 constexpr uint32_t QCHUNK_BYTES = MQ * BLOCK_K * 2;
-constexpr int MAX_DIM = 1024;
+constexpr int MAX_DIM = 4096;
 constexpr int SMEM_LIMIT = 232448;  // 227 KB
 static_assert(K_MERGE_MAX + K_MERGE_MAX / 4 + 16 <= KP * KP, "list-entry threshold trick covers at most KP*KP entries");
 static_assert(M_CAP >= K_MERGE_MAX + K_MERGE_MAX / 4 + 16, "M_CAP must cover the candidates needed for K_MERGE_MAX");
@@ -100,8 +102,18 @@ struct ScanParams {
     int ccap;
 };
 
-__host__ __device__ inline size_t scan_smem_bytes(int dim, int stages, bool has_mod = false) {
-    return (size_t)(dim / BLOCK_K) * QCHUNK_BYTES + (size_t)stages * STAGE_BYTES + (size_t)MQ * ACC_LD * sizeof(float) +
+// Two ways to feed the wgmma A operand (the query block):
+//   resident (dim <= RESIDENT_MAX_DIM): all dim / 64 query k-blocks are loaded once per CTA and stay in shared memory;
+//     they take dim / 64 * 8 KB, so the ring stages get what is left of the 227 KB.
+//   streamed: every ring stage carries the query k-block (64 x 64, 8 KB) beside the corpus k-block it multiplies, so
+//     shared memory does not grow with dim; the price is 8 KB of L2 -> SM query traffic per 16 KB corpus k-block.
+constexpr int RESIDENT_MAX_DIM = 1024;
+enum ScanKernel : int { SCAN_RESIDENT_Q = 0, SCAN_STREAMED_Q = 1 };
+
+__host__ __device__ inline size_t scan_smem_bytes(int dim, int stages, bool has_mod = false, bool stream_q = false) {
+    const size_t resident_q = stream_q ? 0 : (size_t)(dim / BLOCK_K) * QCHUNK_BYTES;
+    const size_t stage_bytes = STAGE_BYTES + (stream_q ? QCHUNK_BYTES : 0);
+    return resident_q + (size_t)stages * stage_bytes + (size_t)MQ * ACC_LD * sizeof(float) +
            2 * 4 * TILE_N * sizeof(int32_t) + (has_mod ? 4 * TILE_N * sizeof(float2) : 0) + (2 * 16 + 3) * sizeof(uint64_t) +
            1024 /* alignment slack */;
 }
@@ -176,20 +188,22 @@ __device__ __forceinline__ void list_insert(float (&ls)[KP], int (&lr)[KP], int 
     }
 }
 
-template <bool HAS_DOCS, bool HAS_BIAS, bool HAS_MOD, bool COLLECT>
+// STREAM_Q: the query k-block travels in each ring stage (at byte STAGE_BYTES of the stage) instead of being resident.
+template <bool HAS_DOCS, bool HAS_BIAS, bool HAS_MOD, bool COLLECT, bool STREAM_Q>
 __global__ void __launch_bounds__(THREADS, 1)
 scan_kernel(const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_q, ScanParams p) {
     if (COLLECT) {
         // the fallback pass is always enqueued by the asynchronous entry point; nothing flagged -> nothing to do
         if (*reinterpret_cast<volatile int*>(&p.qs->n_need) == 0) return;
     }
+    constexpr uint32_t RING_BYTES = STAGE_BYTES + (STREAM_Q ? QCHUNK_BYTES : 0);   // bytes per ring stage
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int kblocks = p.dim / BLOCK_K;
     const int S = p.num_stages;
     uint8_t* smem_q = smem;
-    uint8_t* smem_c = smem_q + (size_t)kblocks * QCHUNK_BYTES;
-    float* smem_acc = reinterpret_cast<float*>(smem_c + (size_t)S * STAGE_BYTES);
+    uint8_t* smem_c = smem_q + (STREAM_Q ? 0 : (size_t)kblocks * QCHUNK_BYTES);
+    float* smem_acc = reinterpret_cast<float*>(smem_c + (size_t)S * RING_BYTES);
     int32_t* smem_docs = reinterpret_cast<int32_t*>(smem_acc + MQ * ACC_LD);
     float* smem_bias = reinterpret_cast<float*>(smem_docs + 4 * TILE_N);
     float2* smem_mod = reinterpret_cast<float2*>(smem_bias + 4 * TILE_N);
@@ -219,17 +233,22 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ 
     if (warp == 8) {
         // ------------------------------------------------------------ TMA producer
         if (lane == 0) {
-            ptx::mbar_arrive_expect_tx(qfull, kblocks * QCHUNK_BYTES);
-            for (int kb = 0; kb < kblocks; ++kb)
-                ptx::tma_load_2d(smem_q + (size_t)kb * QCHUNK_BYTES, &tmap_q, qfull, kb * BLOCK_K, 0, ptx::kEvictLast);
+            if constexpr (!STREAM_Q) {
+                ptx::mbar_arrive_expect_tx(qfull, kblocks * QCHUNK_BYTES);
+                for (int kb = 0; kb < kblocks; ++kb)
+                    ptx::tma_load_2d(smem_q + (size_t)kb * QCHUNK_BYTES, &tmap_q, qfull, kb * BLOCK_K, 0, ptx::kEvictLast);
+            }
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
                 for (int kb = 0; kb < kblocks; ++kb) {
                     ptx::mbar_wait(&empty[stage], phase ^ 1);
-                    ptx::mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
-                    ptx::tma_load_2d(smem_c + (size_t)stage * STAGE_BYTES, &tmap_c, &full[stage], kb * BLOCK_K,
+                    ptx::mbar_arrive_expect_tx(&full[stage], RING_BYTES);
+                    ptx::tma_load_2d(smem_c + (size_t)stage * RING_BYTES, &tmap_c, &full[stage], kb * BLOCK_K,
                                      tile * TILE_N, ptx::kEvictFirst);
+                    if constexpr (STREAM_Q)   // the query block is re-read by every CTA for every tile: keep it in L2
+                        ptx::tma_load_2d(smem_c + (size_t)stage * RING_BYTES + STAGE_BYTES, &tmap_q, &full[stage],
+                                         kb * BLOCK_K, 0, ptx::kEvictLast);
                     if (++stage == S) {
                         stage = 0;
                         phase ^= 1;
@@ -239,7 +258,7 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ 
         }
     } else if (warp >= 4) {
         // ------------------------------------------------------------ MMA warpgroup: S = Q C^T for one tile (64 x 128)
-        ptx::mbar_wait(qfull, 0);
+        if constexpr (!STREAM_Q) ptx::mbar_wait(qfull, 0);
         const int r0 = (warp - 4) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
         int stage = 0;
         uint32_t phase = 0, acc_phase = 0;
@@ -247,8 +266,9 @@ scan_kernel(const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ 
         for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
             for (int kb = 0; kb < kblocks; ++kb) {
                 ptx::mbar_wait(&full[stage], phase);
-                const uint32_t a_base = ptx::smem_u32(smem_q + (size_t)kb * QCHUNK_BYTES);
-                const uint32_t b_base = ptx::smem_u32(smem_c + (size_t)stage * STAGE_BYTES);
+                const uint32_t a_base = ptx::smem_u32(STREAM_Q ? smem_c + (size_t)stage * RING_BYTES + STAGE_BYTES
+                                                               : smem_q + (size_t)kb * QCHUNK_BYTES);
+                const uint32_t b_base = ptx::smem_u32(smem_c + (size_t)stage * RING_BYTES);
                 ptx::wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < BLOCK_K / WG_K; ++k)
@@ -1208,6 +1228,10 @@ struct b200_index {
     bool filter_active = false;
     // statistics of the exactness machinery (b200_index_search_stats)
     int64_t stat_groups = 0, stat_flagged = 0, stat_collect_passes = 0, stat_host_finalize = 0;
+    // scan kernel selection: the streamed-query kernel is forced at any dim (test hook), and the kernel the last scan
+    // ran (-1 before the first scan)
+    bool force_streamed_q = false;
+    int last_scan_kernel = -1;
     cudaStream_t stream = nullptr;   // own_stream, or the caller's stream set by b200_index_set_stream
     UniqueStream own_stream;
     UniqueEvent ev[4];
@@ -1267,12 +1291,19 @@ void ensure_ccap(b200_index* ix, int cap) {
 }
 
 using ScanFn = void (*)(const CUtensorMap, const CUtensorMap, ScanParams);
+constexpr int NUM_SCAN_FNS = 16;
+// idx bits: 1 docs, 2 bias, 4 modifiers, 8 streamed query block
 template <bool C>
 ScanFn scan_fn(int idx) {
-    static const ScanFn table[8] = {scan_kernel<false, false, false, C>, scan_kernel<true, false, false, C>,
-                                    scan_kernel<false, true, false, C>,  scan_kernel<true, true, false, C>,
-                                    scan_kernel<false, false, true, C>,  scan_kernel<true, false, true, C>,
-                                    scan_kernel<false, true, true, C>,   scan_kernel<true, true, true, C>};
+    static const ScanFn table[NUM_SCAN_FNS] = {
+        scan_kernel<false, false, false, C, false>, scan_kernel<true, false, false, C, false>,
+        scan_kernel<false, true, false, C, false>,  scan_kernel<true, true, false, C, false>,
+        scan_kernel<false, false, true, C, false>,  scan_kernel<true, false, true, C, false>,
+        scan_kernel<false, true, true, C, false>,   scan_kernel<true, true, true, C, false>,
+        scan_kernel<false, false, false, C, true>,  scan_kernel<true, false, false, C, true>,
+        scan_kernel<false, true, false, C, true>,   scan_kernel<true, true, false, C, true>,
+        scan_kernel<false, false, true, C, true>,   scan_kernel<true, false, true, C, true>,
+        scan_kernel<false, true, true, C, true>,    scan_kernel<true, true, true, C, true>};
     return table[idx];
 }
 
@@ -1311,7 +1342,7 @@ b200_index* index_new(int device, int dim, int metric, int64_t capacity_rows) {
     ensure_ccap(ix.get(), FIN_CAP);
     ensure_capacity(ix.get(), std::max<int64_t>(capacity_rows, TILE_N));
     const auto smem_attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
-    for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < NUM_SCAN_FNS; ++i) {
         MB_CUDA(cudaFuncSetAttribute(scan_fn<false>(i), smem_attr, SMEM_LIMIT));
         MB_CUDA(cudaFuncSetAttribute(scan_fn<true>(i), smem_attr, SMEM_LIMIT));
     }
@@ -1392,9 +1423,10 @@ ScanLaunch prepare_scan(b200_index* ix, int nq) {
     const int num_tiles = (int)((ix->n_rows + TILE_N - 1) / TILE_N);
     L.grid = std::min(num_tiles, ix->sms);
     const bool mod = ix->mod_active;
+    const bool stream_q = ix->dim > RESIDENT_MAX_DIM || ix->force_streamed_q;
     int stages = 16;
-    while (stages > 2 && scan_smem_bytes(ix->dim, stages, mod) > (size_t)SMEM_LIMIT) --stages;
-    L.smem = scan_smem_bytes(ix->dim, stages, mod);
+    while (stages > 2 && scan_smem_bytes(ix->dim, stages, mod, stream_q) > (size_t)SMEM_LIMIT) --stages;
+    L.smem = scan_smem_bytes(ix->dim, stages, mod, stream_q);
     if (L.smem > (size_t)SMEM_LIMIT) fail(B200_ERR_INTERNAL, "scan kernel shared memory budget exceeded");
     L.tmap_c = make_tmap_2d(ix->corpus.get(), CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (uint64_t)ix->dim,
                             (uint64_t)ix->n_rows, (uint64_t)ix->dim * 2, BLOCK_K, TILE_N, CU_TENSOR_MAP_SWIZZLE_128B);
@@ -1420,7 +1452,8 @@ ScanLaunch prepare_scan(b200_index* ix, int nq) {
     sp.ccap = ix->ccap;
     const bool bias = ix->metric == B200_METRIC_EUCLIDEAN;
     const bool docs = ix->has_docs || ix->filter_active;   // the filter is applied where the document numbers are read
-    L.fn_index = (docs ? 1 : 0) | (bias ? 2 : 0) | (mod ? 4 : 0);
+    L.fn_index = (docs ? 1 : 0) | (bias ? 2 : 0) | (mod ? 4 : 0) | (stream_q ? 8 : 0);
+    ix->last_scan_kernel = stream_q ? SCAN_STREAMED_Q : SCAN_RESIDENT_Q;
     return L;
 }
 
@@ -1804,6 +1837,15 @@ void add_checked(b200_index* ix, F&& append) {
 }
 
 }  // namespace
+
+void mb::score::debug_scan_kernel(b200_index* ix, int force_streamed, int* last_kernel) {
+    MB_CHECK_ARG(ix != nullptr, "index is NULL");
+    MB_CHECK_ARG(force_streamed >= -1 && force_streamed <= 1, "force_streamed must be -1, 0 or 1 (got %d)",
+                 force_streamed);
+    std::lock_guard<std::mutex> lk(ix->mu);
+    if (force_streamed >= 0) ix->force_streamed_q = force_streamed != 0;
+    if (last_kernel) *last_kernel = ix->last_scan_kernel;
+}
 
 extern "C" {
 

@@ -1,0 +1,14 @@
+// Test hooks of the score + top-k row store (score.cu) that the diagnostic entry points (debug.cu) reach.
+#pragma once
+#include "common.cuh"
+
+namespace mb {
+namespace score {
+
+// force_streamed: 1 makes every later scan of `ix` run the streamed-query kernel whatever its dim, 0 restores the
+// library's rule (streamed only above 1024), -1 leaves the setting as it is.  *last_kernel (when not NULL) receives
+// the kernel the last scan ran: 0 resident query block, 1 streamed, -1 no scan yet.
+void debug_scan_kernel(b200_index* ix, int force_streamed, int* last_kernel);
+
+}  // namespace score
+}  // namespace mb

@@ -521,6 +521,16 @@ def debug_gemm_into(A, W, io, bias=None, act: int = 0, out_bf16: bool = False, r
     return (out, kernel.value) if return_kernel else out
 
 
+def debug_scan_kernel(store: RowStore, force_streamed: Optional[bool] = None) -> int:
+    """The scan kernel `store`'s last search ran (_native.SCAN_RESIDENT_Q or SCAN_STREAMED_Q; -1 before any search).
+    force_streamed True makes later searches use the streamed-query kernel at any dim, False restores the library's
+    rule, None leaves the setting as it is."""
+    last = C.c_int(-1)
+    force = -1 if force_streamed is None else int(bool(force_streamed))
+    N.check(N.load().b200_debug_index_scan_kernel(store._handle(), force, C.byref(last)))
+    return last.value
+
+
 def debug_gemm_ln(A, W, bias, residual, gamma, beta, eps: float, in_place: bool = False, repeats: int = 1,
                   device: int = 0):
     """Residual GEMM followed by the LayerNorm launch -> (x fp32 [M, N], LayerNorm(x) rounded to bf16 [M, N])."""

@@ -28,7 +28,7 @@ from typing import Any, Dict, List, Optional, Tuple
 
 import numpy as np
 
-from ._native import ERR_UNSUPPORTED, NativeError
+from ._native import ERR_UNSUPPORTED, MAX_INDEX_DIM, NativeError
 from .engine import RowStore
 from .yql_filter import FilterSyntaxError, compile_filter
 from .errors import VespaError, VespaStatusError
@@ -47,6 +47,23 @@ QUERY_INPUT_EMBEDDINGS = ("marqo__query_embedding", "embedding_query")
 EMBEDDINGS_PREFIX = "marqo__embeddings"
 CHUNKS_PREFIX = "marqo__chunks"
 MATCH_FEATURES = "matchfeatures"
+
+ROW_ALIGN = 64   # the row store's width is a multiple of this; narrower fields are stored with zero columns appended
+
+
+def _padded_width(dim: int) -> int:
+    return -(-dim // ROW_ALIGN) * ROW_ALIGN
+
+
+def _pad_columns(mat: np.ndarray, width: int) -> np.ndarray:
+    """[m, d] -> [m, width] with zero columns appended.  Zero columns add exact zeros to every dot product, norm and
+    fp64 re-score sum, so ids, rows and scores are those of the unpadded vectors."""
+    if mat.shape[-1] == width:
+        return mat
+    out = np.zeros(mat.shape[:-1] + (width,), dtype=np.float32)
+    out[..., :mat.shape[-1]] = mat
+    return out
+
 
 _NN_TERM = re.compile(r"\(\s*\{([^}]*)\}\s*nearestNeighbor\(\s*([A-Za-z0-9_]+)\s*,\s*([A-Za-z0-9_]+)\s*\)\s*\)")
 _WHERE = re.compile(r"\bwhere\b(.*)$", re.IGNORECASE | re.DOTALL)
@@ -133,6 +150,7 @@ class _FilterEntry:
 class _Schema:
     def __init__(self):
         self.stores: Dict[str, RowStore] = {}          # embeddings field -> row store
+        self.dims: Dict[str, int] = {}                 # embeddings field -> its vectors' dimension (<= store width)
         self.row_chunk: Dict[str, List[Tuple[int, str]]] = {}  # embeddings field -> row -> (doc number, chunk key)
         self.doc_num: Dict[str, int] = {}              # external id -> document number
         self.doc_ids: List[Optional[str]] = []         # document number -> external id (None = deleted)
@@ -288,10 +306,13 @@ class GpuTensorIndex:
                     raise ValueError(f"field {f}: embedding values beyond +-{limit:g} do not fit the fp16 row store")
                 dim = mat.shape[1]
             store = s.stores.get(f)
-            if store is not None and dim != store.dim:
-                raise ValueError(f"field {f}: embedding dimension {dim} != index dimension {store.dim}")
-            if store is None and (dim <= 0 or dim % 64 != 0 or dim > 1024):
-                raise ValueError(f"field {f}: embedding dimension {dim} is not a multiple of 64 in [64, 1024]")
+            if store is not None and dim != s.dims[f]:
+                raise ValueError(f"field {f}: embedding dimension {dim} != index dimension {s.dims[f]}")
+            if store is None and not 0 < dim <= MAX_INDEX_DIM:
+                raise ValueError(f"field {f}: embedding dimension {dim} is not in [1, {MAX_INDEX_DIM}]")
+            if isinstance(mat, DeviceChunks) and dim != _padded_width(dim):
+                raise ValueError(f"field {f}: device-resident embeddings of dimension {dim} are not a multiple of "
+                                 f"{ROW_ALIGN}; send them as host vectors")
             staged[f] = (keys, mat)
         attrs: Dict[str, float] = {}
         for tensor_field in SCORE_MODIFIER_FIELDS:
@@ -384,8 +405,9 @@ class GpuTensorIndex:
                         d = m.dim if isinstance(m, DeviceChunks) else m.shape[1]
                         if d != dim:
                             raise ValueError(f"field {f}: embedding dimension {d} != index dimension {dim}")
-                    store = RowStore(dim, metric=self.metric, device=self.device)
+                    store = RowStore(_padded_width(dim), metric=self.metric, device=self.device)
                     s.stores[f] = store
+                    s.dims[f] = dim
                     s.row_chunk[f] = []
                     s.dead[f] = 0
                     created.append(f)
@@ -416,7 +438,7 @@ class GpuTensorIndex:
                         dev_ids.extend([num] * len(keys))      # the vectoriser hands out consecutive slices of one
                     else:                                      # tensor: a whole batch becomes ONE device append
                         flush_dev()
-                        host_rows.append(mat)
+                        host_rows.append(_pad_columns(mat, store.dim))
                         host_ids.append(np.full(len(keys), num, dtype=np.int32))
                 flush_host()
                 flush_dev()
@@ -456,6 +478,7 @@ class GpuTensorIndex:
             for f in created:
                 if f not in appended:
                     s.stores.pop(f).close()
+                    s.dims.pop(f, None)
                     s.row_chunk.pop(f, None)
             try:
                 rc, ri, rv = [], [], []
@@ -693,9 +716,10 @@ class GpuTensorIndex:
                     store = s.stores.get(f)
                     if store is None or len(store) == 0:
                         continue
-                    if q.shape[-1] != store.dim:
-                        raise VespaStatusError(400, f"Expected a tensor of dimension {store.dim} for query input but "
+                    if q.shape[-1] != s.dims[f]:
+                        raise VespaStatusError(400, f"Expected a tensor of dimension {s.dims[f]} for query input but "
                                                     f"got {q.shape[-1]}")
+                    qf = _pad_columns(q, store.dim)
                     if epoch is None:
                         epoch = s.epoch
                     # a weight on an attribute no document has multiplies / adds nothing anywhere: drop the term
@@ -712,7 +736,7 @@ class GpuTensorIndex:
                         return store.search(Q, kmax, mult=mult_cols, add=add_cols, **kw)
 
                 key = (id(store), mult_cols, add_cols, filter_text)
-                found[f] = self._coalescer.submit(key, q, k, run)
+                found[f] = self._coalescer.submit(key, qf, k, run)
             with self._lock:
                 if epoch is not None and epoch != s.epoch:
                     continue      # a compaction renumbered rows between the scan and now: search again
@@ -769,7 +793,7 @@ class GpuTensorIndex:
                 out = dict(s.fields[num] or {})
                 for f, rows in s.doc_rows[num].items():
                     if rows:
-                        vecs = s.stores[f].get_rows(rows)
+                        vecs = s.stores[f].get_rows(rows)[:, :s.dims[f]]
                         out[f] = {s.row_chunk[f][r][1]: vecs[i].tolist() for i, r in enumerate(rows)}
                 if fields is not None:
                     out = {k: v for k, v in out.items() if k in fields}
@@ -826,6 +850,8 @@ class GpuTensorIndex:
                     fname = f"{len(manifest['schemas'])}_{i}.b200idx"
                     st.save(os.path.join(directory, fname))
                     stores[f] = {"file": fname, "row_chunk": s.row_chunk[f]}
+                    if s.dims[f] != st.dim:   # stored with zero columns appended
+                        stores[f]["dim"] = s.dims[f]
                 manifest["schemas"][name] = {"stores": stores, "doc_ids": s.doc_ids, "fields": s.fields,
                                              "doc_rows": s.doc_rows, "attr_col": s.attr_col, "attrs": s.attrs}
             tmp = os.path.join(directory, "manifest.json.tmp")
@@ -852,6 +878,7 @@ class GpuTensorIndex:
             s.attrs = [dict(a) for a in js["attrs"]]
             for f, st in js["stores"].items():
                 s.stores[f] = RowStore.load(os.path.join(directory, st["file"]), device=device)
+                s.dims[f] = int(st.get("dim", s.stores[f].dim))
                 s.row_chunk[f] = [(int(n), str(k)) for n, k in st["row_chunk"]]
                 live = sum(len(d.get(f, ())) for d in s.doc_rows)
                 s.dead[f] = len(s.row_chunk[f]) - live

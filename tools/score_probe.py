@@ -1,9 +1,15 @@
-"""Dev probe: time the scan/merge kernels on a shard-sized corpus generated on the device (not a bench line)."""
+"""Dev probe: time the scan/merge kernels on a shard-sized corpus generated on the device (not a bench line).
+
+usage: python tools/score_probe.py ROWS DIM [mod] [streamed]
+  mod       also time the score-modifier variant
+  streamed  force the streamed-query scan kernel (the one dims above 1024 use) whatever DIM is
+The JSON line reports the kernel that ran and search_stats(): queries the guard flagged and collect passes run."""
 import sys, time, json
 import numpy as np
 import torch
 sys.path.insert(0, ".")
-from marqo_b200.engine import RowStore
+from marqo_b200 import _native
+from marqo_b200.engine import RowStore, debug_scan_kernel
 
 n = int(float(sys.argv[1])) if len(sys.argv) > 1 else 1_250_000
 d = int(sys.argv[2]) if len(sys.argv) > 2 else 768
@@ -11,6 +17,8 @@ nq, k = 64, 10
 torch.cuda.set_device(0)
 g = torch.Generator(device="cuda").manual_seed(0)
 store = RowStore(d, capacity=n)
+if "streamed" in sys.argv[3:]:
+    debug_scan_kernel(store, force_streamed=True)
 chunk = 125_000
 for lo in range(0, n, chunk):
     m = min(chunk, n - lo)
@@ -30,13 +38,15 @@ for it in range(8):
 scan = sorted(r[0] for r in res[2:])
 merge = sorted(r[1] for r in res[2:])
 bytes_ = n * d * 2
-out = {"n": n, "d": d, "scan_ms_med": scan[len(scan)//2], "scan_ms_min": scan[0], "merge_ms_med": merge[len(merge)//2],
-       "GBps_med": bytes_ / scan[len(scan)//2] / 1e6, "GBps_best": bytes_ / scan[0] / 1e6, "all": res}
+kernel = {_native.SCAN_RESIDENT_Q: "resident_q", _native.SCAN_STREAMED_Q: "streamed_q"}[debug_scan_kernel(store)]
+out = {"n": n, "d": d, "kernel": kernel, "scan_ms_med": scan[len(scan)//2], "scan_ms_min": scan[0],
+       "merge_ms_med": merge[len(merge)//2], "GBps_med": bytes_ / scan[len(scan)//2] / 1e6, "GBps_best": bytes_ / scan[0] / 1e6,
+       "qps_med": nq * 1e3 / (scan[len(scan)//2] + merge[len(merge)//2]), "search_stats": store.search_stats(), "all": res}
 print(json.dumps(out))
 print(od[:2].tolist(), osc[:2].tolist())
 
 # score modifiers (f3): same corpus, 3 attribute columns, the scan kernel's HAS_MOD variant through the host entry point
-if len(sys.argv) > 3 and sys.argv[3] == "mod":
+if "mod" in sys.argv[3:]:
     rng = np.random.default_rng(0)
     ids = np.arange(n, dtype=np.int32)
     for c in range(3):
