@@ -425,12 +425,13 @@ int b200_debug_index_scan_kernel(b200_index* ix, int force_streamed, int* last_k
  * with the epilogue given by act, out_bf16, has_bias and residual_in_place (residual == out, fp32 only). */
 int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16, int has_bias, int residual_in_place,
                          int iters, float* out_ms);
-/* ViT patch embedding of uint8 HWC images [n,S,S,3]: ToTensor + Normalize (mean3/std3) -> conv1 (conv_w fp32
- * [N, 3*patch*patch], no bias) -> token rows: out fp32 [n*(G+1), N], row b*(G+1)+1+i = patch i of image b (+ pos[1+i]
- * when pos != NULL), class-token rows left zero.  use_gather != 0: the fused gather GEMM (no patch matrix in HBM,
- * src/marqo/tensor_search/add_docs.py:129-134 folded into the operand load); 0: im2col kernel + plain GEMM. */
+/* ViT patch embedding of uint8 HWC images [n,S,S,3], the token rows the image forward feeds to ln_pre: out fp32
+ * [n*(G+1), N], row b*(G+1) = cls + pos[0], row b*(G+1)+1+i = conv1(patch i of image b) + pos[1+i], where the patch is
+ * ToTensor + Normalize (mean3/std3)-ed and conv1 is conv_w fp32 [N, 3*patch*patch] without bias.  cls fp32 [N] and pos
+ * fp32 [G+1, N] may be NULL (zeros).  The fused gather GEMM: no patch matrix in HBM,
+ * src/marqo/tensor_search/add_docs.py:129-134 folded into the operand load. */
 int b200_debug_patch_embed(int device, const uint8_t* hwc, int n, int S, int patch, const float* conv_w, int N,
-                           const float* mean3, const float* std3, const float* pos, int use_gather, float* out);
+                           const float* mean3, const float* std3, const float* cls, const float* pos, float* out);
 /* softmax(q k^T / 8 + mask) v over packed qkv fp32 [B*S, 3*W] (rounded to bf16); mask: 0 none, 1 causal,
  * 2 key length (kv_len int32 [B]).  out fp32 [B*S, W]. */
 int b200_debug_attention(int device, const float* qkv, int B, int S, int W, int H, int mask, const int32_t* kv_len,

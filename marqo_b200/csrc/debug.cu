@@ -69,7 +69,7 @@ void require_device(int device) {
 extern "C" {
 
 int b200_debug_patch_embed(int device, const uint8_t* hwc, int n, int S, int patch, const float* conv_w, int N,
-                           const float* mean3, const float* std3, const float* pos, int use_gather, float* out) {
+                           const float* mean3, const float* std3, const float* cls, const float* pos, float* out) {
     return guarded([&] {
         MB_CHECK_ARG(hwc && conv_w && mean3 && std3 && out, "NULL buffer");
         MB_CHECK_ARG(n > 0 && S > 0 && patch > 0 && S % patch == 0 && N > 0 && N % 32 == 0, "bad shape");
@@ -79,40 +79,31 @@ int b200_debug_patch_embed(int device, const uint8_t* hwc, int n, int S, int pat
         const int G = (S / patch) * (S / patch), K = 3 * patch * patch;
         uint8_t* dImg = sc.upload(hwc, (size_t)n * S * S * 3);
         float* dW = sc.upload(conv_w, (size_t)N * K);
-        float* dOut = sc.alloc<float>((size_t)n * (G + 1) * N);
-        MB_CUDA(cudaMemsetAsync(dOut, 0, (size_t)n * (G + 1) * N * 4, sc.s));
+        const std::vector<float> zeros((size_t)(G + 1) * N, 0.f);   // a missing cls / pos
+        const float* dCls = sc.upload(cls ? cls : zeros.data(), (size_t)N);
+        const float* dPos = sc.upload(pos ? pos : zeros.data(), (size_t)(G + 1) * N);
+        __nv_bfloat16* dWg = sc.alloc<__nv_bfloat16>((size_t)N * gemm::patch_gather_k(patch));
+        kernels::patch_weight_rows(dW, N, patch, gemm::patch_gather_kbpd(patch), dWg, sc.s);
+        // as the ViT forward does: x = pos (+ cls), then the gather GEMM adds conv1 onto it in place
+        float* dX = sc.alloc<float>((size_t)n * (G + 1) * N);
+        kernels::vit_embed_rows(dX, dCls, dPos, n, G + 1, N, sc.s);
         gemm::Epilogue ep;
-        ep.out = dOut;
+        ep.residual = dX;
+        ep.ldr = N;
+        ep.out = dX;
         ep.ldo = N;
         ep.out_fp32 = 1;
-        ep.remap_group = G;                                   // token row b * (G + 1) + 1 + i, as the ViT forward does
-        ep.rowbias = pos ? sc.upload(pos, (size_t)(G + 1) * N) : nullptr;
-        if (!pos) ep.rowbias = nullptr;
-        int sms = sm_count(device);
-        if (use_gather) {
-            MB_CHECK_ARG(gemm::patch_gather_supported(S, patch), "the gather GEMM does not support image %d / patch %d", S,
-                         patch);
-            __nv_bfloat16* dWg = sc.alloc<__nv_bfloat16>((size_t)N * gemm::patch_gather_k(patch));
-            kernels::patch_weight_rows(dW, N, patch, gemm::patch_gather_kbpd(patch), dWg, sc.s);
-            gemm::PatchGather pg;
-            pg.img = dImg;
-            pg.n = n;
-            pg.S = S;
-            pg.patch = patch;
-            for (int i = 0; i < 3; ++i) {
-                pg.mean[i] = mean3[i];
-                pg.std[i] = std3[i];
-            }
-            gemm::launch_patch_embed(pg, dWg, N, ep, sms, sc.s);
-        } else {
-            const int kpad = (int)round_up((size_t)K, 64);
-            __nv_bfloat16* dWp = sc.alloc<__nv_bfloat16>((size_t)N * kpad);
-            kernels::pad_rows_to_bf16(dW, N, K, kpad, dWp, sc.s);
-            __nv_bfloat16* dP = sc.alloc<__nv_bfloat16>((size_t)n * G * kpad);
-            kernels::im2col_u8(dImg, n, S, patch, kpad, mean3, std3, dP, sc.s);
-            gemm::launch(dP, kpad, dWp, n * G, N, kpad, ep, sms, sc.s);
+        gemm::PatchGather pg;
+        pg.img = dImg;
+        pg.n = n;
+        pg.S = S;
+        pg.patch = patch;
+        for (int i = 0; i < 3; ++i) {
+            pg.mean[i] = mean3[i];
+            pg.std[i] = std3[i];
         }
-        MB_CUDA(cudaMemcpyAsync(out, dOut, (size_t)n * (G + 1) * N * 4, cudaMemcpyDeviceToHost, sc.s));
+        gemm::launch_patch_embed(pg, dWg, N, ep, sc.s);
+        MB_CUDA(cudaMemcpyAsync(out, dX, (size_t)n * (G + 1) * N * 4, cudaMemcpyDeviceToHost, sc.s));
         MB_CUDA(cudaStreamSynchronize(sc.s));
     });
 }

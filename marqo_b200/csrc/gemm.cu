@@ -8,8 +8,8 @@
 namespace mb {
 namespace gemm {
 
-// Two warp-specialised wgmma GEMM kernels share one STAGED epilogue: a warpgroup's 64-row output block goes through
-// shared memory as 128-byte-wide TMA boxes with the 128B swizzle (the fp32 residual TMA-loaded into the same boxes
+// Two warp-specialised wgmma GEMM kernels share one epilogue: a warpgroup's 64-row output block goes through shared
+// memory as 128-byte-wide TMA boxes with the 128B swizzle (the fp32 residual TMA-loaded into the same boxes
 // beforehand), the MMA threads write act(acc + bias) (+ residual) over it (epilogue_to_smem), and one thread per
 // warpgroup stores the boxes by TMA, which clips them at M and N.  The output type and the activation are template
 // parameters of both kernels, so each instantiation holds only the epilogue it runs; the host maps an Epilogue to its
@@ -22,23 +22,17 @@ namespace gemm {
 //               or, for the ViT patch embedding (GATHER), four warps that build the A stage from the uint8 image while
 //               one of them still loads W by TMA.
 // Two CTAs share an SM (3 x 32 KB stages each), so one CTA's epilogue overlaps the other's main loop.
-//
-// Its epilogues (chosen on the host, a template parameter):
-//   STAGED     every GEMM whose output rows are the A rows.  Warpgroup wg's 64 x 128 block of the output goes through
-//              one ring stage, the one of virtual k-block kblocks + wg: the producer takes that stage through the usual
-//              empty/full protocol once the main loop has released it (k-block kblocks + wg - 3), and fills it with
-//              the fp32 residual rows by TMA when there is a residual, so the load overlaps the last MMAs.  The bias
-//              columns are read once per CTA into shared memory.
-//   register   the ViT token scatter (remap_group > 0: patch embed, gather kernel or im2col): GEMM row r goes to token
-//              row b (G + 1) + 1 + i, so the 64 rows of a warpgroup are not one contiguous output block; each thread
-//              adds the positional embedding and stores its fp32 fragments from registers.  No bias, no activation.
+// Warpgroup wg's 64 x 128 block of the output goes through one ring stage, the one of virtual k-block kblocks + wg:
+// the producer takes that stage through the usual empty/full protocol once the main loop has released it (k-block
+// kblocks + wg - 3), and fills it with the fp32 residual rows by TMA when there is a residual, so the load overlaps the
+// last MMAs.  The bias columns are read once per CTA into shared memory.
 //
 // gemm_persistent_kernel: GEMMs with K >= 1024, N % 256 == 0 and at least one full wave of tiles (the ViT-L-14
 // layers).  128 x 256 tiles on a persistent grid, one CTA per SM walking the tiles t = blockIdx.x + i * gridDim.x,
 // m-major (tile_m = t / tiles_n), so the W columns in use stay in L2.  384 threads:
 //   warpgroup 0     the producer: one thread issues the TMA loads into a 3-stage ring of 48 KB; the warpgroup gives its
 //                   registers to the MMA warpgroups (setmaxnreg 40).
-//   warpgroups 1-2  wgmma m64n256k16 on 64 rows each (128 accumulators per thread, setmaxnreg 232), then the STAGED
+//   warpgroups 1-2  wgmma m64n256k16 on 64 rows each (128 accumulators per thread, setmaxnreg 232), then the
 //                   epilogue through the warpgroup's own EPI_BYTES shared-memory buffer.
 //   The ring position `it` is one running counter over every k-block of every tile of the CTA, in the producer and in
 //   the MMA warpgroups alike (stage it % 3, phase (it / 3) & 1); it never restarts for a new tile, so the producer runs
@@ -58,7 +52,7 @@ constexpr uint32_t B_STAGE_BYTES = BN * BK * 2;
 constexpr uint32_t STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
 constexpr uint32_t BARRIER_BYTES = 256;
 constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + BARRIER_BYTES + 2 * BN * 4 /*bias*/;
-// Staged epilogue: a warpgroup's 64 output rows as 128-byte-wide TMA boxes with the 128B swizzle, 8 KB each, one
+// Epilogue: a warpgroup's 64 output rows as 128-byte-wide TMA boxes with the 128B swizzle, 8 KB each, one
 // after the other in its stage: fp32 -> 4 boxes of 32 columns (the residual arrives in the same layout), bf16 -> 2
 // boxes of 64 columns.
 constexpr int EPI_ROWS = BM / 2;
@@ -84,7 +78,8 @@ struct Params {
     int M, N, K;
     int tiles_m, tiles_n;
     Epilogue ep;
-    // GATHER only: uint8 HWC images [n, S, S, 3]; A row r = patch r (image r / (g*g), then row-major in the grid).
+    // GATHER only: uint8 HWC images [n, S, S, 3]; A row r = token t = r % (g*g + 1) of image r / (g*g + 1): zero for
+    // t = 0 (the class token), else patch t - 1, row-major in the grid.
     // k index of the A row = dy * (64 * kbpd) + dx * 3 + c (kernels::patch_weight_rows lays W out the same way).
     const uint8_t* img;
     int g;                  // patches per image side
@@ -201,7 +196,7 @@ __device__ __forceinline__ float2 act(float x0, float x1) {
         return make_float2(x0, x1);
 }
 
-// The STAGED epilogue of COLS output columns of a warpgroup's 64 rows, held in acc[0, COLS / 2) (fragment i: columns
+// The epilogue of COLS output columns of a warpgroup's 64 rows, held in acc[0, COLS / 2) (fragment i: columns
 // 8 i + 2 (lane & 3) + {0, 1} of rows rbase and rbase + 8): act(acc + bias) with the bias row at shared address bias_s,
 // plus the fp32 residual already in the buffer when there is one, written at epi_offset into the buffer at shared
 // address buf_s.
@@ -254,14 +249,13 @@ __device__ __forceinline__ void store_output_boxes(const CUtensorMap* tmap_o, co
     ptx::tma_store_commit();
 }
 
-// tmap_r / tmap_o (STAGED only): the fp32 residual and the output, boxes of EPI_ROWS rows x 128 bytes.  The token
-// scatter (!STAGED) is gemm_kernel<GATHER, false, true, ACT_NONE>.
-template <bool GATHER, bool STAGED, bool OUT_FP32, int ACT>
+// tmap_r / tmap_o: the fp32 residual and the output, boxes of EPI_ROWS rows x 128 bytes.  p is a grid constant so that
+// the gather's run-time index into p.nscale / p.nshift reads the parameter space instead of a local copy of p.
+template <bool GATHER, bool OUT_FP32, int ACT>
 __global__ void __launch_bounds__(threads<GATHER>(), GATHER ? 1 : 2)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-            const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_o, Params p) {
-    static_assert(!(GATHER && STAGED), "the patch embed scatters token rows: register epilogue");
-    static_assert(STAGED || (OUT_FP32 && ACT == ACT_NONE), "the token scatter writes fp32 with no activation");
+            const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_o,
+            const __grid_constant__ Params p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * STAGE_BYTES);
@@ -277,10 +271,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     if (threadIdx.x == MMA_THREADS) {
         ptx::prefetch_tmap(&tmap_b);
         if (!GATHER) ptx::prefetch_tmap(&tmap_a);
-        if (STAGED) {
-            ptx::prefetch_tmap(&tmap_o);
-            if (p.ep.residual) ptx::prefetch_tmap(&tmap_r);
-        }
+        ptx::prefetch_tmap(&tmap_o);
+        if (p.ep.residual) ptx::prefetch_tmap(&tmap_r);
         for (int i = 0; i < STAGES; ++i) {
             ptx::mbar_init(&full[i], GATHER ? 1 + 128 : 1);
             ptx::mbar_init(&empty[i], MMA_THREADS / 32);
@@ -293,14 +285,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         // ------------------------------------------------------------ producer
         const int pt = threadIdx.x - MMA_THREADS;
         if (!GATHER && pt >= 32) return;
-        // GATHER: thread pt builds A row pt of every stage: patch m0 + pt
+        // GATHER: thread pt builds A row pt of every stage: token row m0 + pt, zero (prow == nullptr) for a class token
         const uint8_t* prow = nullptr;
         if (GATHER) {
             const int r = m0 + pt;
-            if (r < p.M) {
-                const int gg = p.g * p.g;
-                const int b = r / gg, pi = r - b * gg;
-                const int py = pi / p.g, px = pi - py * p.g;
+            const int tokens = p.g * p.g + 1;
+            const int b = r / tokens, t = r - b * tokens;
+            if (r < p.M && t > 0) {
+                const int py = (t - 1) / p.g, px = (t - 1) - py * p.g;
                 prow = p.img + ((size_t)b * p.g * p.patch + (size_t)py * p.patch) * p.row_bytes + (size_t)px * p.patch * 3;
             }
         }
@@ -340,19 +332,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                 ptx::mbar_arrive(&full[stage]);
             }
         }
-        if (STAGED) {
-            // virtual k-blocks kblocks, kblocks + 1: the epilogue stages of warpgroups 0 and 1, with their residual rows
-            for (int wg = 0; wg < 2; ++wg) {
-                const int kb = kblocks + wg;
-                const int stage = kb % STAGES;
-                uint8_t* s = smem + (size_t)stage * STAGE_BYTES;
-                ptx::mbar_wait(&empty[stage], ((uint32_t)(kb / STAGES) & 1u) ^ 1);
-                if (pt != 0) continue;   // full[] counts one producer arrival
+        // virtual k-blocks kblocks, kblocks + 1: the epilogue stages of warpgroups 0 and 1, with their residual rows
+        for (int wg = 0; wg < 2; ++wg) {
+            const int kb = kblocks + wg;
+            const int stage = kb % STAGES;
+            uint8_t* s = smem + (size_t)stage * STAGE_BYTES;
+            ptx::mbar_wait(&empty[stage], ((uint32_t)(kb / STAGES) & 1u) ^ 1);
+            if (pt == 0) {
                 if (p.ep.residual != nullptr)
                     load_residual_boxes(&tmap_r, &full[stage], s, m0 + EPI_ROWS * wg, n0, p.M, p.N);
                 else
                     ptx::mbar_arrive(&full[stage]);
             }
+            if (GATHER) ptx::mbar_arrive(&full[stage]);   // full[] also counts every gather thread
         }
         return;
     }
@@ -360,9 +352,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     // ---------------------------------------------------------------- MMA warpgroups
     const int wg = warp >> 2;
     const Epilogue& ep = p.ep;
-    // STAGED: thread t of the warpgroup fetches bias column n0 + t now; the load completes under the main loop
+    // thread t of the warpgroup fetches bias column n0 + t now; the load completes under the main loop
     float bias_t = 0.f;
-    if (STAGED && ep.bias != nullptr && n0 + (int)(threadIdx.x & 127) < p.N) bias_t = __ldg(ep.bias + n0 + (threadIdx.x & 127));
+    if (ep.bias != nullptr && n0 + (int)(threadIdx.x & 127) < p.N) bias_t = __ldg(ep.bias + n0 + (threadIdx.x & 127));
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -382,54 +374,22 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     }
     ptx::wgmma_wait<0>();
 
-    if constexpr (STAGED) {
-        // ------------------------------------------------------------ epilogue staged in shared memory, TMA store
-        const int t = threadIdx.x & 127;
-        float* wbias = bias_s + wg * BN;
-        wbias[t] = bias_t;
-        const int kb = kblocks + wg;
-        ptx::mbar_wait(&full[kb % STAGES], (uint32_t)(kb / STAGES) & 1u);   // the stage is ours, the residual in it
-        uint8_t* tile = smem + (size_t)(kb % STAGES) * STAGE_BYTES;
-        warpgroup_sync(wg);   // wbias complete
-        const int rbase = (warp & 3) * 16 + (lane >> 2);   // row inside the warpgroup's 64
-        epilogue_to_smem<OUT_FP32, ACT, BN>(acc, ptx::smem_u32(wbias), ptx::smem_u32(tile), ep.residual != nullptr,
-                                            rbase, lane);
-        ptx::fence_proxy_async_smem();   // generic-proxy stores -> visible to the TMA store
-        warpgroup_sync(wg);
-        if (t == 0) {
-            store_output_boxes<OUT_FP32, BN>(&tmap_o, tile, m0 + EPI_ROWS * wg, n0, p.M, p.N);
-            ptx::tma_store_wait_read<0>();   // the stage must outlive the store's reads of it
-        }
-    } else {
-        // ------------------------------------------------------------ token scatter from registers
-        const int rbase = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-        float* orow[2];
-        const float* pos[2];
-        bool rok[2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int r = rbase + 8 * h;
-            const int b = r / ep.remap_group, i = r - b * ep.remap_group;
-            rok[h] = r < p.M;
-            orow[h] = static_cast<float*>(ep.out) + ((long long)b * (ep.remap_group + 1) + 1 + i) * ep.ldo;
-            pos[h] = ep.rowbias ? ep.rowbias + (size_t)(1 + i) * p.N : nullptr;
-        }
-#pragma unroll
-        for (int i = 0; i < BN / 8; ++i) {
-            const int col = n0 + 8 * i + 2 * (lane & 3);
-            if (col >= p.N) continue;   // N % 32 == 0: col + 1 < N as well
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                if (!rok[h]) continue;
-                float x0 = acc[4 * i + 2 * h], x1 = acc[4 * i + 2 * h + 1];
-                if (pos[h]) {   // ViT patch-embed: positional embedding of this row's patch
-                    const float2 pb = __ldg(reinterpret_cast<const float2*>(pos[h] + col));
-                    x0 += pb.x;
-                    x1 += pb.y;
-                }
-                *reinterpret_cast<float2*>(orow[h] + col) = make_float2(x0, x1);
-            }
-        }
+    // ---------------------------------------------------------------- epilogue through shared memory, TMA store
+    const int t = threadIdx.x & 127;
+    float* wbias = bias_s + wg * BN;
+    wbias[t] = bias_t;
+    const int kb = kblocks + wg;
+    ptx::mbar_wait(&full[kb % STAGES], (uint32_t)(kb / STAGES) & 1u);   // the stage is ours, the residual in it
+    uint8_t* tile = smem + (size_t)(kb % STAGES) * STAGE_BYTES;
+    warpgroup_sync(wg);   // wbias complete
+    const int rbase = (warp & 3) * 16 + (lane >> 2);   // row inside the warpgroup's 64
+    epilogue_to_smem<OUT_FP32, ACT, BN>(acc, ptx::smem_u32(wbias), ptx::smem_u32(tile), ep.residual != nullptr, rbase,
+                                        lane);
+    ptx::fence_proxy_async_smem();   // generic-proxy stores -> visible to the TMA store
+    warpgroup_sync(wg);
+    if (t == 0) {
+        store_output_boxes<OUT_FP32, BN>(&tmap_o, tile, m0 + EPI_ROWS * wg, n0, p.M, p.N);
+        ptx::tma_store_wait_read<0>();   // the stage must outlive the store's reads of it
     }
 }
 
@@ -584,7 +544,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     if (t == 0) ptx::tma_store_wait_read<0>();   // shared memory must outlive the last store's reads of it
 }
 
-// Calls f(std::bool_constant<OUT_FP32>, std::integral_constant<int, ACT>) for the STAGED epilogue instantiation of
+// Calls f(std::bool_constant<OUT_FP32>, std::integral_constant<int, ACT>) for the epilogue instantiation of
 // (out_fp32, act), an activation other than GELU and QuickGELU being none: the one list of instantiations, from which
 // both launches and configure() take theirs.
 template <class F>
@@ -607,21 +567,29 @@ void configure() {
     static std::once_flag once;
     std::call_once(once, [] {
         const auto attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
-        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, false, true, ACT_NONE>, attr, (int)SMEM_BYTES));
-        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<true, false, true, ACT_NONE>, attr, (int)SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<true, true, ACT_NONE>, attr, (int)SMEM_BYTES));
         for (int out_fp32 = 0; out_fp32 < 2; ++out_fp32)
             for (int act = ACT_NONE; act <= ACT_QUICKGELU; ++act)
                 dispatch(out_fp32, act, [&](auto out, auto a) {
                     constexpr bool OUT_FP32 = decltype(out)::value;
                     constexpr int ACT = decltype(a)::value;
-                    MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, true, OUT_FP32, ACT>, attr, (int)SMEM_BYTES));
+                    MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, OUT_FP32, ACT>, attr, (int)SMEM_BYTES));
                     MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<OUT_FP32, ACT>, attr, (int)P_SMEM_BYTES));
                 });
     });
 }
 
-// The STAGED epilogue's maps, boxes of EPI_ROWS rows x 128 bytes with the 128B swizzle: the fp32 residual (tr is left
-// as it is without one) and the output.
+// TMA: 16-byte aligned bases and row pitches
+static void check_epilogue(const Epilogue& ep) {
+    if (ep.ldo % 8 != 0) fail(B200_ERR_INTERNAL, "gemm: ldo = %d must be a multiple of 8", ep.ldo);
+    if ((reinterpret_cast<uintptr_t>(ep.out) & 15) != 0) fail(B200_ERR_INTERNAL, "gemm: output not 16-byte aligned");
+    if (ep.residual != nullptr &&
+        (!ep.out_fp32 || ep.ldr % 4 != 0 || (reinterpret_cast<uintptr_t>(ep.residual) & 15) != 0))
+        fail(B200_ERR_INTERNAL, "gemm: the residual needs an fp32 output, ldr %% 4 == 0 and 16-byte alignment");
+}
+
+// The epilogue's maps, boxes of EPI_ROWS rows x 128 bytes with the 128B swizzle: the fp32 residual (tr is left as it
+// is without one) and the output.
 static void epilogue_tmaps(const Epilogue& ep, int M, int N, CUtensorMap& tr, CUtensorMap& to) {
     if (ep.residual)
         tr = make_tmap_2d(ep.residual, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
@@ -632,7 +600,7 @@ static void epilogue_tmaps(const Epilogue& ep, int M, int N, CUtensorMap& tr, CU
                                     (uint64_t)ep.ldo * 2, 64, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-template <bool GATHER, bool STAGED, bool OUT_FP32, int ACT>
+template <bool GATHER, bool OUT_FP32, int ACT>
 static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep,
                          cudaStream_t stream, const PatchGather* pg = nullptr) {
     Params p{};
@@ -655,17 +623,16 @@ static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W
     p.ep = ep;
     const long long tiles = (long long)((M + BM - 1) / BM) * p.tiles_n;
     if (tiles > 0x7fffffffLL) fail(B200_ERR_UNSUPPORTED, "gemm: %lld tiles is too many", tiles);
-    // (GATHER has no A matrix, and the register epilogue no residual or output map: those maps are further, unused views
-    // of W so the kernel signature stays the same)
+    // (GATHER has no A matrix, and without a residual there is no residual map: those maps are further, unused views of
+    // W so the kernel signature stays the same)
     CUtensorMap tb = make_tmap_2d(W, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)K, (uint64_t)N, (uint64_t)K * 2, BK, BN,
                                   CU_TENSOR_MAP_SWIZZLE_128B);
     CUtensorMap ta = GATHER ? tb
                             : make_tmap_2d(A, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)K, (uint64_t)M,
                                            (uint64_t)lda * 2, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);
-    CUtensorMap tr = tb, to = tb;
-    if (STAGED) epilogue_tmaps(ep, M, N, tr, to);
-    gemm_kernel<GATHER, STAGED, OUT_FP32, ACT>
-        <<<(unsigned)tiles, threads<GATHER>(), SMEM_BYTES, stream>>>(ta, tb, tr, to, p);
+    CUtensorMap tr = tb, to;
+    epilogue_tmaps(ep, M, N, tr, to);
+    gemm_kernel<GATHER, OUT_FP32, ACT><<<(unsigned)tiles, threads<GATHER>(), SMEM_BYTES, stream>>>(ta, tb, tr, to, p);
     MB_CUDA(cudaGetLastError());
 }
 
@@ -693,24 +660,18 @@ static void launch_persistent(const __nv_bfloat16* A, int lda, const __nv_bfloat
     MB_CUDA(cudaGetLastError());
 }
 
-bool patch_gather_supported(int S, int patch) {
-    return S > 0 && patch > 0 && S % patch == 0;
-}
-
-void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, const Epilogue& ep, int sms,
-                        cudaStream_t stream) {
-    (void)sms;
+void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, const Epilogue& ep, cudaStream_t stream) {
     if (pg.n <= 0 || N <= 0) return;
-    if (!patch_gather_supported(pg.S, pg.patch))
-        fail(B200_ERR_INTERNAL, "patch gather: image %d / patch %d is not supported", pg.S, pg.patch);
-    if (N % 32 != 0 || ep.ldo % 8 != 0) fail(B200_ERR_INTERNAL, "patch gather: N = %d, ldo = %d", N, ep.ldo);
-    if (ep.remap_group <= 0 || ep.residual != nullptr || ep.bias != nullptr || ep.act != ACT_NONE || !ep.out_fp32)
-        fail(B200_ERR_INTERNAL, "patch gather: fp32 token scatter without bias, activation or residual only");
+    if (pg.S <= 0 || pg.patch <= 0 || pg.S % pg.patch != 0)
+        fail(B200_ERR_INTERNAL, "patch gather: image %d is not a multiple of patch %d", pg.S, pg.patch);
+    if (N % 32 != 0) fail(B200_ERR_INTERNAL, "patch gather: N = %d must be a multiple of 32", N);
+    if (!ep.out_fp32 || ep.act != ACT_NONE) fail(B200_ERR_INTERNAL, "patch gather: fp32 output without activation only");
+    check_epilogue(ep);
     configure();
     const int g = pg.S / pg.patch;
-    const long long M = (long long)pg.n * g * g;
+    const long long M = (long long)pg.n * (g * g + 1);
     if (M > 0x7fffffffLL) fail(B200_ERR_INVALID_ARG, "patch gather: batch of %d images is too large", pg.n);
-    launch_tiles<true, false, true, ACT_NONE>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
+    launch_tiles<true, true, ACT_NONE>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
 }
 
 int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep, int sms,
@@ -718,20 +679,8 @@ int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N
     if (M <= 0 || N <= 0) return KERNEL_NONE;
     if (K <= 0 || K % BK != 0) fail(B200_ERR_INTERNAL, "gemm: K = %d must be a positive multiple of %d", K, BK);
     if (N % 32 != 0) fail(B200_ERR_INTERNAL, "gemm: N = %d must be a multiple of 32", N);
-    if (lda % 8 != 0 || ep.ldo % 8 != 0) fail(B200_ERR_INTERNAL, "gemm: leading dimensions must be multiples of 8");
-    if (ep.remap_group > 0) {
-        if (ep.residual != nullptr || ep.bias != nullptr || ep.act != ACT_NONE || !ep.out_fp32)
-            fail(B200_ERR_INTERNAL, "gemm: fp32 token scatter without bias, activation or residual only");
-        configure();
-        launch_tiles<false, false, true, ACT_NONE>(A, lda, W, M, N, K, ep, stream);
-        return KERNEL_128x128;
-    }
-    // TMA: 16-byte aligned bases and row pitches
-    if ((reinterpret_cast<uintptr_t>(ep.out) & 15) != 0) fail(B200_ERR_INTERNAL, "gemm: output not 16-byte aligned");
-    if (ep.rowbias != nullptr) fail(B200_ERR_INTERNAL, "gemm: the positional bias goes with the token scatter");
-    if (ep.residual != nullptr &&
-        (!ep.out_fp32 || ep.ldr % 4 != 0 || (reinterpret_cast<uintptr_t>(ep.residual) & 15) != 0))
-        fail(B200_ERR_INTERNAL, "gemm: the residual needs an fp32 output, ldr %% 4 == 0 and 16-byte alignment");
+    if (lda % 8 != 0) fail(B200_ERR_INTERNAL, "gemm: lda = %d must be a multiple of 8", lda);
+    check_epilogue(ep);
     configure();
     // The persistent kernel's main loop is faster, but its epilogue is not overlapped: it pays with enough k-blocks per
     // tile (all four ViT-L-14 layer GEMMs, K >= 1024), at least one full wave of tiles, and no half-empty 256-wide
@@ -744,7 +693,7 @@ int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N
         if (persistent)
             launch_persistent<OUT_FP32, ACT>(A, lda, W, M, N, K, ep, sms, stream);
         else
-            launch_tiles<false, true, OUT_FP32, ACT>(A, lda, W, M, N, K, ep, stream);
+            launch_tiles<false, OUT_FP32, ACT>(A, lda, W, M, N, K, ep, stream);
     });
     return persistent ? KERNEL_PERSISTENT : KERNEL_128x128;
 }

@@ -2,8 +2,7 @@
 // 128 x 128 tiles, TMA-fed 128B-swizzled smem ring, two MMA warpgroups with fp32 accumulators in registers.  For
 // K >= 1024, N % 256 == 0 and at least one full wave of tiles, a persistent kernel of 128 x 256 tiles (one CTA per SM)
 // runs instead.  Both kernels run one epilogue, act(acc + bias) (+ residual): each warpgroup's output block goes
-// through shared memory (the fp32 residual TMA-loaded into it ahead of time) and out by TMA stores (gemm.cu).  Only the
-// ViT token scatter (remap_group > 0) stores from registers; it takes no bias and no activation.
+// through shared memory (the fp32 residual TMA-loaded into it ahead of time) and out by TMA stores (gemm.cu).
 // Output and residual must be 16-byte aligned; a residual needs an fp32 output and ldr % 4 == 0.
 #pragma once
 #include "common.cuh"
@@ -21,10 +20,6 @@ struct Epilogue {
     void* out = nullptr;  // bf16 or fp32 [*, ldo]
     int ldo = 0;
     int out_fp32 = 0;
-    // ViT token assembly (patch-embed): GEMM row r = (image b, patch i) with G patches per image is written to token
-    // row b * (G + 1) + 1 + i and gets rowbias[(1 + i), :] (the positional embedding) added.
-    int remap_group = 0;
-    const float* rowbias = nullptr;  // fp32 [G + 1, N]
 };
 
 // A: bf16 [M, K] row-major with leading dimension lda (elements); W: bf16 [N, K] row-major (nn.Linear layout).
@@ -36,20 +31,20 @@ int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N
            int sm_count, cudaStream_t stream);
 
 // ViT patch embedding straight from uint8 pixels (SURVEY §8 a2; add_docs.py:129-134 + clip_utils.py:48-67 fused into the
-// conv1 GEMM's operand load): out = epilogue( patches(img) x Wg^T ), where row r of the virtual A matrix is patch r of the
-// uint8 HWC batch [n, S, S, 3] (image r / g^2, row-major in the g x g grid), normalised as ToTensor + Normalize, and
-// Wg [N, patch_gather_k(patch)] is conv1.weight re-laid by kernels::patch_weight_rows.  No patch matrix exists in HBM:
-// the gather warps of the GEMM read the image rows, convert and write the swizzled smem A stage.
+// conv1 GEMM's operand load): out = epilogue( patches(img) x Wg^T ) over the n (g^2 + 1) ViT token rows of the uint8
+// HWC batch [n, S, S, 3] (S % patch == 0, g = S / patch).  Row r of the virtual A matrix is token t = r % (g^2 + 1) of
+// image r / (g^2 + 1): zero for the class token t = 0, else patch t - 1 (row-major in the g x g grid), normalised as
+// ToTensor + Normalize.  Wg [N, patch_gather_k(patch)] is conv1.weight re-laid by kernels::patch_weight_rows.  No patch
+// matrix exists in HBM: the gather warps of the GEMM read the image rows, convert and write the swizzled smem A stage.
+// The epilogue must have an fp32 output and no activation.
 struct PatchGather {
     const uint8_t* img = nullptr;
     int n = 0, S = 0, patch = 0;
     float mean[3] = {0.f, 0.f, 0.f}, std[3] = {1.f, 1.f, 1.f};
 };
-bool patch_gather_supported(int S, int patch);   // S % patch == 0
 inline int patch_gather_kbpd(int patch) { return (3 * patch + 63) / 64; }
 inline int patch_gather_k(int patch) { return patch * patch_gather_kbpd(patch) * 64; }
-void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, const Epilogue& ep, int sm_count,
-                        cudaStream_t stream);
+void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, const Epilogue& ep, cudaStream_t stream);
 
 void configure();  // one-time cudaFuncSetAttribute calls
 

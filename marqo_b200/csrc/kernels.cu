@@ -91,40 +91,32 @@ void layernorm(const float* x, long long in_stride, const float* gamma, const fl
 }
 
 // ------------------------------------------------------------------------------------------------ im2col
-template <bool U8>
-__global__ void __launch_bounds__(256) im2col_kernel(const void* __restrict__ img, int n, int S, int p, int kpad,
-                                                     float3 scale, float3 shift, __nv_bfloat16* __restrict__ out) {
-    // one thread = 8 consecutive k of one patch row
+__global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ chw, int n, int S, int p, int kpad,
+                                                     __nv_bfloat16* __restrict__ out) {
+    // one thread = 8 consecutive k of one token row; the class-token row (t == 0) of each image is zero
     const int g = S / p;
+    const int tokens = g * g + 1;
     const int groups = kpad / 8;
     const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long total = (long long)n * g * g * groups;
+    const long long total = (long long)n * tokens * groups;
     if (gid >= total) return;
     const int kg = (int)(gid % groups);
-    const long long prow = gid / groups;
-    const int px = (int)(prow % g);
-    const int py = (int)((prow / g) % g);
-    const long long b = prow / ((long long)g * g);
+    const long long row = gid / groups;
+    const long long b = row / tokens;
+    const int t = (int)(row - b * tokens);
+    const int px = (t - 1) % g, py = (t - 1) / g;
     const int K = 3 * p * p;
     float f[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
         const int k = kg * 8 + e;
         float val = 0.f;
-        if (k < K) {
+        if (t > 0 && k < K) {
             const int c = k / (p * p);
             const int rem = k - c * p * p;
             const int dy = rem / p, dx = rem - dy * p;
             const int y = py * p + dy, x = px * p + dx;
-            if (U8) {
-                const uint8_t u = reinterpret_cast<const uint8_t*>(img)[((b * S + y) * S + x) * 3 + c];
-                const float sc = c == 0 ? scale.x : (c == 1 ? scale.y : scale.z);
-                const float sh = c == 0 ? shift.x : (c == 1 ? shift.y : shift.z);
-                // ToTensor then Normalize: (u/255 - mean)/std, evaluated as torchvision does (div, sub, div)
-                val = ((float)u / 255.0f - sh) / sc;
-            } else {
-                val = reinterpret_cast<const float*>(img)[((b * 3 + c) * S + y) * S + x];
-            }
+            val = chw[((b * 3 + c) * S + y) * S + x];
         }
         f[e] = val;
     }
@@ -132,38 +124,37 @@ __global__ void __launch_bounds__(256) im2col_kernel(const void* __restrict__ im
         make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
 }
 
-void im2col_u8(const uint8_t* img, int n, int S, int p, int kpad, const float* mean3, const float* std3,
-               __nv_bfloat16* out, cudaStream_t s) {
-    if (n <= 0) return;
-    const int g = S / p;
-    const long long total = (long long)n * g * g * (kpad / 8);
-    const float3 sc = make_float3(std3[0], std3[1], std3[2]);
-    const float3 sh = make_float3(mean3[0], mean3[1], mean3[2]);
-    im2col_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, s>>>(img, n, S, p, kpad, sc, sh, out);
-    MB_CUDA(cudaGetLastError());
-}
-
 void im2col_f32(const float* chw, int n, int S, int p, int kpad, __nv_bfloat16* out, cudaStream_t s) {
     if (n <= 0) return;
     const int g = S / p;
-    const long long total = (long long)n * g * g * (kpad / 8);
-    im2col_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, s>>>(chw, n, S, p, kpad, make_float3(1, 1, 1),
-                                                                        make_float3(0, 0, 0), out);
+    const long long total = (long long)n * (g * g + 1) * (kpad / 8);
+    im2col_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(chw, n, S, p, kpad, out);
     MB_CUDA(cudaGetLastError());
 }
 
 // ------------------------------------------------------------------------------------------------ embeddings
-__global__ void vit_cls_kernel(float* x, const float* __restrict__ cls, const float* __restrict__ pos, int n,
-                               int tokens_per_image, int w) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n * w) return;
-    const int b = i / w, c = i - b * w;
-    x[(long long)b * tokens_per_image * w + c] = cls[c] + pos[c];
+__global__ void __launch_bounds__(256) vit_embed_kernel(float4* __restrict__ x, const float4* __restrict__ cls,
+                                                        const float4* __restrict__ pos, long long total,
+                                                        int tokens_per_image, int w4) {
+    // one thread = 4 columns of one token row
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const long long row = i / w4;
+    const int c = (int)(i - row * w4), t = (int)(row % tokens_per_image);
+    float4 v = __ldg(pos + (long long)t * w4 + c);
+    if (t == 0) {
+        const float4 a = __ldg(cls + c);
+        v = make_float4(a.x + v.x, a.y + v.y, a.z + v.z, a.w + v.w);
+    }
+    x[i] = v;
 }
 
-void vit_cls_rows(float* x, const float* cls, const float* pos, int n, int tokens_per_image, int w, cudaStream_t s) {
+void vit_embed_rows(float* x, const float* cls, const float* pos, int n, int tokens_per_image, int w, cudaStream_t s) {
     if (n <= 0) return;
-    vit_cls_kernel<<<(n * w + 255) / 256, 256, 0, s>>>(x, cls, pos, n, tokens_per_image, w);
+    const long long total = (long long)n * tokens_per_image * (w / 4);
+    vit_embed_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
+        reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(cls), reinterpret_cast<const float4*>(pos), total,
+        tokens_per_image, w / 4);
     MB_CUDA(cudaGetLastError());
 }
 

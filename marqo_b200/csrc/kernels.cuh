@@ -1,5 +1,5 @@
-// Memory-bound helper kernels of the encoders (LayerNorm, embeddings, im2col + image normalise, pooling +
-// projection + L2 normalise, dtype conversion).  All are coalesced / vectorised; none is GEMM-shaped.
+// Memory-bound helper kernels of the encoders (LayerNorm, embeddings, im2col, pooling + projection + L2 normalise,
+// dtype conversion).  All are coalesced / vectorised; none is GEMM-shaped.
 #pragma once
 #include "common.cuh"
 
@@ -11,15 +11,14 @@ namespace kernels {
 void layernorm(const float* x, long long in_stride, const float* gamma, const float* beta, float eps, int rows, int w,
                float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s);
 
-// uint8 HWC images [n, S, S, 3] -> normalised bf16 patch matrix [n * g * g, kpad], k = c*p*p + dy*p + dx
-// ((u8/255 - mean[c]) / std[c]; zero for k >= 3*p*p).  This is the CLIP ToTensor + Normalize fused into im2col.
-void im2col_u8(const uint8_t* img, int n, int S, int p, int kpad, const float* mean3, const float* std3,
-               __nv_bfloat16* out, cudaStream_t s);
-// Already-normalised fp32 CHW [n, 3, S, S] -> bf16 patch matrix.
+// Already-normalised fp32 CHW [n, 3, S, S] -> bf16 A matrix of the ViT token rows [n * (g*g + 1), kpad]: row
+// b * (g*g + 1) + t is zero for the class token t = 0, else patch t - 1 (row-major in the g x g grid) with
+// k = c*p*p + dy*p + dx, zero for k >= 3*p*p.
 void im2col_f32(const float* chw, int n, int S, int p, int kpad, __nv_bfloat16* out, cudaStream_t s);
 
-// x[b*(G+1), :] = class_embedding + positional_embedding[0]
-void vit_cls_rows(float* x, const float* cls, const float* pos, int n, int tokens_per_image, int w, cudaStream_t s);
+// x[b * tokens_per_image + t, :] = positional_embedding[t], plus class_embedding for t == 0 (w % 4 == 0): the rows the
+// patch-embed GEMM then adds conv1(patch) onto in place
+void vit_embed_rows(float* x, const float* cls, const float* pos, int n, int tokens_per_image, int w, cudaStream_t s);
 
 // CLIP text: x[b, s, :] = token_embedding[ids[b, s]] + positional_embedding[s]; also eot[b] = arg-max_s ids[b, s]
 void clip_text_embed(const int32_t* ids, const float* tok, const float* pos, int n, int S, int w, int vocab, float* x,

@@ -12,7 +12,7 @@
 //   qkv       bf16 [tokens, 3*width] fused QKV projection
 //   o         bf16 [tokens, width]   attention output
 //   u         bf16 [tokens, mlp]     MLP hidden
-//   patches   bf16 [images * grid^2, kpad]  normalised im2col of the uint8 input (ToTensor + Normalize fused)
+//   patches   bf16 [images * (grid^2 + 1), kpad]  im2col of preprocessed fp32 CHW input (zero class-token rows)
 // Every Linear is the wgmma GEMM of gemm.cu with bias / activation / residual-add fused into its epilogue.
 #include <algorithm>
 #include <cmath>
@@ -44,7 +44,7 @@ struct TowerW {
     std::vector<LayerW> layers;
     // vision
     const __nv_bfloat16* conv_w = nullptr;  // [width, kpad]
-    const __nv_bfloat16* conv_wg = nullptr; // [width, gemm::patch_gather_k(patch)]: gather GEMM order, or NULL if unsupported
+    const __nv_bfloat16* conv_wg = nullptr; // [width, gemm::patch_gather_k(patch)]: gather GEMM order
     int kpad = 0, grid = 0, tokens = 0;
     const float *cls = nullptr, *pos = nullptr, *ln_pre_w = nullptr, *ln_pre_b = nullptr;
     // final LN (ln_post / ln_final) and projection [width, embed]
@@ -370,15 +370,17 @@ void run_bert_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, f
 void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const float* f32, int n, int normalize,
                           float* d_out) {
     const TowerW& T = m->vision;
-    const int S = T.d.image_size, p = T.d.patch, w = T.d.width, G = T.grid * T.grid;
-    gemm::Epilogue e;  // conv1 (no bias) + positional embedding, scattered to token rows 1..G of each image
+    const int S = T.d.image_size, p = T.d.patch, w = T.d.width;
+    // x = positional embedding (+ class embedding on each image's first row), then conv1 (no bias) of every token row
+    // added onto it in place; a class-token row multiplies a zero A row
+    kernels::vit_embed_rows(m->x.get(), T.cls, T.pos, n, T.tokens, w, m->stream);
+    gemm::Epilogue e;
+    e.residual = m->x.get();
+    e.ldr = w;
     e.out = m->x.get();
     e.ldo = w;
     e.out_fp32 = 1;
-    e.remap_group = G;
-    e.rowbias = T.pos;
-    static const bool no_gather = getenv("MARQO_B200_NO_PATCH_GATHER") != nullptr;   // A/B timing switch
-    if (u8 && T.conv_wg && !no_gather && (reinterpret_cast<uintptr_t>(u8) & 15) == 0) {
+    if (u8) {
         // uint8 pixels -> ToTensor + Normalize -> bf16 inside the GEMM's operand load: no patch matrix in HBM
         gemm::PatchGather pg;
         pg.img = u8;
@@ -390,19 +392,15 @@ void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const fl
             pg.std[i] = m->desc.image_std[i];
         }
         ProfScope ps(m, 0);
-        gemm::launch_patch_embed(pg, T.conv_wg, w, e, m->sms, m->stream);
+        gemm::launch_patch_embed(pg, T.conv_wg, w, e, m->stream);
         ++c.n;
     } else {
-        // preprocessed fp32 CHW tensors (the reference's parity path) and shapes the gather does not cover
-        if (!m->patches) m->patches = DeviceBuffer<__nv_bfloat16>((size_t)m->desc.max_batch * G * T.kpad);
-        if (u8)
-            kernels::im2col_u8(u8, n, S, p, T.kpad, m->desc.image_mean, m->desc.image_std, m->patches.get(), m->stream);
-        else
-            kernels::im2col_f32(f32, n, S, p, T.kpad, m->patches.get(), m->stream);
-        linear(m, c, m->patches.get(), n * G, T.kpad, T.conv_w, w, e);
+        // preprocessed fp32 CHW tensors (the reference's parity path)
+        if (!m->patches) m->patches = DeviceBuffer<__nv_bfloat16>((size_t)m->desc.max_batch * T.tokens * T.kpad);
+        kernels::im2col_f32(f32, n, S, p, T.kpad, m->patches.get(), m->stream);
+        linear(m, c, m->patches.get(), n * T.tokens, T.kpad, T.conv_w, w, e);
         ++c.n;
     }
-    kernels::vit_cls_rows(m->x.get(), T.cls, T.pos, n, T.tokens, w, m->stream);
     kernels::layernorm(m->x.get(), w, T.ln_pre_w, T.ln_pre_b, 1e-5f, n * T.tokens, w, m->x.get(), nullptr, m->stream);
     c.n += 2;
     run_clip_blocks(m, c, T, n, T.tokens, attention::MASK_NONE);
@@ -653,12 +651,10 @@ int b200_model_finalize(b200_model* m) {
             kernels::pad_rows_to_bf16(conv, (int)w, K, T.kpad, cw, m->stream);
             MB_CUDA(cudaStreamSynchronize(m->stream));
             T.conv_w = cw;
-            if (gemm::patch_gather_supported(T.d.image_size, (int)p)) {
-                __nv_bfloat16* cg = derived_buffer<__nv_bfloat16>(m, (size_t)w * gemm::patch_gather_k((int)p));
-                kernels::patch_weight_rows(conv, (int)w, (int)p, gemm::patch_gather_kbpd((int)p), cg, m->stream);
-                MB_CUDA(cudaStreamSynchronize(m->stream));
-                T.conv_wg = cg;
-            }
+            __nv_bfloat16* cg = derived_buffer<__nv_bfloat16>(m, (size_t)w * gemm::patch_gather_k((int)p));
+            kernels::patch_weight_rows(conv, (int)w, (int)p, gemm::patch_gather_kbpd((int)p), cg, m->stream);
+            MB_CUDA(cudaStreamSynchronize(m->stream));
+            T.conv_wg = cg;
             T.cls = param(m, "visual.class_embedding", w);
             T.pos = param(m, "visual.positional_embedding", (long long)T.tokens * w);
             T.ln_pre_w = param(m, "visual.ln_pre.weight", w);
@@ -670,9 +666,6 @@ int b200_model_finalize(b200_model* m) {
             max_tok = std::max(max_tok, (long long)m->desc.max_batch * T.tokens);
             max_w = std::max(max_w, w);
             max_mlp = std::max(max_mlp, (long long)T.d.mlp);
-            // the bf16 patch matrix of the im2col path is allocated on first use (fp32 CHW input / unsupported shapes)
-            if (!T.conv_wg)
-                m->patches = DeviceBuffer<__nv_bfloat16>((size_t)m->desc.max_batch * T.grid * T.grid * T.kpad);
             m->resized = DeviceBuffer<uint8_t>((size_t)m->desc.max_batch * T.d.image_size * T.d.image_size * 3);
         }
         if (m->text.present) {

@@ -547,19 +547,20 @@ def debug_gemm_ln(A, W, bias, residual, gamma, beta, eps: float, in_place: bool 
     return out_x, out_ln
 
 
-def debug_patch_embed(images_u8, patch: int, conv_w, mean, std, pos=None, use_gather: bool = True,
-                      device: int = 0) -> np.ndarray:
-    """ViT patch embedding of uint8 HWC images [n, S, S, 3] -> token rows fp32 [n * (G + 1), N] (class rows zero)."""
+def debug_patch_embed(images_u8, patch: int, conv_w, mean, std, pos=None, cls=None, device: int = 0) -> np.ndarray:
+    """ViT patch embedding of uint8 HWC images [n, S, S, 3] -> the token rows fp32 [n * (G + 1), N] the image forward
+    feeds to ln_pre: cls + pos[0] for the class rows, conv1(patch) + pos[1:] for the others (cls / pos None: zeros)."""
     img = _as(images_u8, np.uint8)
     n, S = img.shape[0], img.shape[1]
     w = _as(conv_w, np.float32).reshape(conv_w.shape[0], -1)
     Nn = w.shape[0]
     G = (S // patch) ** 2
     m3, s3 = _as(mean, np.float32), _as(std, np.float32)
+    cs = None if cls is None else _as(cls, np.float32)
     ps = None if pos is None else _as(pos, np.float32)
     out = np.empty((n * (G + 1), Nn), np.float32)
-    N.check(N.load().b200_debug_patch_embed(device, _ptr(img), n, S, patch, _ptr(w), Nn, _ptr(m3), _ptr(s3), _ptr(ps),
-                                            1 if use_gather else 0, _ptr(out)))
+    N.check(N.load().b200_debug_patch_embed(device, _ptr(img), n, S, patch, _ptr(w), Nn, _ptr(m3), _ptr(s3), _ptr(cs),
+                                            _ptr(ps), _ptr(out)))
     return out
 
 

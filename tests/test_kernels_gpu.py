@@ -81,9 +81,10 @@ def test_gemm_fused_layernorm(gpu_required, M, N, K, in_place):
     (300, 224, 32, 128),   # more tiles than SMs
     (1, 112, 8, 256),      # small image: 336-byte rows
 ])
-def test_patch_embed_gather_matches_conv(gpu_required, n, S, patch, N):
-    """SURVEY §8 (a2): uint8 HWC -> ToTensor -> Normalize -> conv1 fused into the GEMM's operand load.  Reference: the
-    torchvision formula (u8/255 - mean)/std in fp32, rounded to bf16 like the kernel's A operand, conv2d in fp32."""
+def test_patch_embed_token_rows_match_conv(gpu_required, n, S, patch, N):
+    """SURVEY §8 (a2): uint8 HWC -> ToTensor -> Normalize -> conv1 fused into the GEMM's operand load, added onto the
+    positional (+ class) embedding rows in place.  Reference: the torchvision formula (u8/255 - mean)/std in fp32,
+    rounded to bf16 like the kernel's A operand, conv2d in fp32."""
     from marqo_b200.engine import debug_patch_embed
     g = torch.Generator().manual_seed(n * 31 + patch)
     img = torch.randint(0, 256, (n, S, S, 3), generator=g, dtype=torch.uint8)
@@ -91,21 +92,20 @@ def test_patch_embed_gather_matches_conv(gpu_required, n, S, patch, N):
     w = _bf16(torch.randn(N, 3, patch, patch, generator=g) / math.sqrt(K))
     G = (S // patch) ** 2
     pos = torch.randn(G + 1, N, generator=g)
+    cls = torch.randn(N, generator=g)
     mean = torch.tensor([0.48145466, 0.4578275, 0.40821073])
     std = torch.tensor([0.26862954, 0.26130258, 0.27577711])
     x = (img.permute(0, 3, 1, 2).float() / 255.0 - mean[None, :, None, None]) / std[None, :, None, None]
     ref = torch.nn.functional.conv2d(_bf16(x).double(), w.double(), stride=patch)       # [n, N, g, g]
     ref = ref.flatten(2).transpose(1, 2) + pos[None, 1:, :].double()                      # [n, G, N]
-    got = torch.from_numpy(debug_patch_embed(img.numpy(), patch, w.numpy(), mean.numpy(), std.numpy(), pos.numpy()))
+    got = torch.from_numpy(debug_patch_embed(img.numpy(), patch, w.numpy(), mean.numpy(), std.numpy(), pos.numpy(),
+                                             cls=cls.numpy()))
     got = got.view(n, G + 1, N)
-    assert float(got[:, 0].abs().max()) == 0.0                                            # class rows are not this kernel's
+    assert torch.equal(got[:, 0], (cls + pos[0]).expand(n, N))       # class rows: a zero A row adds nothing
     # the kernel normalises with one fma (u * 1/(255 std) - mean/std): a few values land on the other side of a bf16
-    # rounding boundary (2^-9 relative) -> compare at bf16-product accuracy, and against the im2col path the same way
+    # rounding boundary (2^-9 relative) -> compare at bf16-product accuracy
     torch.testing.assert_close(got[:, 1:].double(), ref, rtol=0, atol=2e-2)
     assert float((got[:, 1:].double() - ref).abs().mean()) < 1e-3
-    old = torch.from_numpy(debug_patch_embed(img.numpy(), patch, w.numpy(), mean.numpy(), std.numpy(), pos.numpy(),
-                                             use_gather=False)).view(n, G + 1, N)
-    torch.testing.assert_close(got, old, rtol=0, atol=2e-2)
 
 
 @pytest.mark.parametrize("B,S,H,mask", [
