@@ -237,7 +237,8 @@ typedef struct b200_model b200_model;
 enum b200_arch {
     B200_ARCH_CLIP = 0, /* open_clip CLIP: vision tower + text tower */
     B200_ARCH_BERT = 1, /* HF BertModel + pooling */
-    B200_ARCH_MPNET = 2 /* HF MPNetModel + pooling: BERT layers with a relative-position bias in the attention logits */
+    B200_ARCH_MPNET = 2, /* HF MPNetModel + pooling: BERT layers with a relative-position bias in the attention logits */
+    B200_ARCH_SIGLIP = 3 /* open_clip SigLIP: class-token-free ViT with a MAP pooling head + bidirectional text tower */
 };
 enum b200_act { B200_ACT_GELU = 0, B200_ACT_QUICKGELU = 1 };
 enum b200_pool { B200_POOL_MEAN = 0, B200_POOL_CLS = 1 };
@@ -265,8 +266,9 @@ typedef struct b200_model_desc {
     b200_tower_desc vision; /* CLIP only */
     b200_tower_desc text;   /* CLIP text tower, or the BERT / MPNet encoder (MPNet: ctx = longest sequence, which is
                                max_position_embeddings - pad_id - 1 because positions start after the pad id) */
-    /* MPNet only (MPNetConfig): */
-    float layer_norm_eps;     /* 1e-5 for the sentence-transformers checkpoints */
+    /* MPNet (MPNetConfig) and SigLIP: */
+    float layer_norm_eps;     /* 1e-5 for the sentence-transformers MPNet checkpoints, 1e-6 for SigLIP */
+    /* MPNet only: */
     int32_t pad_id;           /* pad_token_id (1): the position ids count from it */
     int32_t rel_buckets;      /* relative_attention_num_buckets (32) */
     int32_t rel_max_distance; /* max_distance of relative_position_bucket (128) */
@@ -276,7 +278,12 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
 int b200_model_destroy(b200_model* m);
 /* Upload one parameter (fp32, host, contiguous) under its checkpoint name: open_clip
  * state_dict names for CLIP ("visual.conv1.weight", "transformer.resblocks.0.attn.in_proj_weight",
- * ...), HF BertModel names for BERT ("embeddings.word_embeddings.weight", ...). */
+ * ...), HF BertModel names for BERT ("embeddings.word_embeddings.weight", ...).  SigLIP: open_clip's names for its
+ * timm trunk and text tower (verify): visual.trunk.patch_embed.proj.{weight,bias}, visual.trunk.pos_embed [1, G*G, W],
+ * visual.trunk.blocks.{i}.{norm1,attn.qkv,attn.proj,norm2,mlp.fc1,mlp.fc2}.{weight,bias}, visual.trunk.norm.*,
+ * visual.trunk.attn_pool.{latent [1, 1, W], q, kv, proj, norm, mlp.fc1, mlp.fc2}.*, text.token_embedding.weight,
+ * text.positional_embedding, text.transformer.resblocks.{i}.* (the CLIP block names), text.ln_final.*,
+ * text.text_projection.{weight [E, W], bias}. */
 int b200_model_load_tensor(b200_model* m, const char* name, const float* data, int64_t numel);
 /* Verifies every required parameter has been supplied, builds derived buffers. */
 int b200_model_finalize(b200_model* m);
@@ -293,7 +300,11 @@ int b200_model_encode_images_u8(b200_model* m, const uint8_t* hwc, int n, int h,
 /* Already-preprocessed fp32 CHW tensors [n,3,S,S] (the reference passes these through
  * unchanged: abstract_clip_model.py:108-111). */
 int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int normalize, float* out);
+/* SigLIP images: the resize squashes the image to S x S (independent x and y scales, no crop); the tower has no class
+ * token and pools with its MAP head (embed_dim == vision width, no projection). */
 /* Token ids int32 [n, seq] (host).  CLIP: causal text tower, EOT = arg-max id pooling.
+ * SigLIP: bidirectional text tower (no mask), the last position of each row is pooled, then ln_final and the biased
+ * text projection; attn_mask is ignored (the tokenizer pads every row to the context length).
  * BERT: attn_mask int32 [n, seq] (1 = token, 0 = pad; NULL = all ones), token_type 0.
  * MPNet: as BERT, without token types; position ids follow the ids (HF create_position_ids_from_input_ids), the key
  * mask follows attn_mask.  seq > text.ctx is refused with B200_ERR_INVALID_ARG. */
@@ -457,6 +468,13 @@ int b200_debug_jpeg_decode_host(const uint8_t* file, size_t nbytes, uint8_t* out
                                 int32_t* out_height, int32_t* out_width);
 /* Pillow-compatible bicubic resize (shortest side -> S) + centre crop of uint8 HWC images [n,h,w,3] -> [n,S,S,3]. */
 int b200_debug_resize(int device, const uint8_t* hwc, int n, int h, int w, int S, uint8_t* out);
+/* The same bicubic resampling squashed to S x S (x and y scaled independently, no crop): PIL resize((S, S), BICUBIC),
+ * SigLIP's preprocessing. */
+int b200_debug_resize_squash(int device, const uint8_t* hwc, int n, int h, int w, int S, uint8_t* out);
+/* SigLIP's MAP pooling attention: for image b and head h, softmax(q_h . k_{b,s} / sqrt(64)) over the S tokens of image
+ * b, times v_{b,s}.  q fp32 [W] (one latent query, shared by every image); kv fp32 [B*S, 2W] (K columns then V columns,
+ * rounded to bf16); head_dim 64.  out fp32 [B, W] (rounded to bf16). */
+int b200_debug_map_attention(int device, const float* q, const float* kv, int B, int S, int W, int H, float* out);
 /* Bytes of device memory the library holds right now, over all devices and handles of this process (indexes,
  * exchanges, models and the scratch of calls in flight).  Memory from b200_host_alloc is not counted.  Returns to its
  * earlier value once every handle created in between is destroyed: a leak check. */

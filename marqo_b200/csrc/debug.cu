@@ -408,4 +408,41 @@ int b200_debug_resize(int device, const uint8_t* hwc, int n, int h, int w, int S
     });
 }
 
+int b200_debug_resize_squash(int device, const uint8_t* hwc, int n, int h, int w, int S, uint8_t* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(hwc && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && h > 0 && w > 0 && S > 0, "n, h, w, S must be positive");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        uint8_t* din = sc.upload(hwc, (size_t)n * h * w * 3);
+        uint8_t* dout = sc.alloc<uint8_t>((size_t)n * S * S * 3);
+        kernels::resize_squash_u8(din, n, h, w, S, dout, sc.s);
+        MB_CUDA(cudaStreamSynchronize(sc.s));
+        MB_CUDA(cudaMemcpy(out, dout, (size_t)n * S * S * 3, cudaMemcpyDeviceToHost));
+    });
+}
+
+int b200_debug_map_attention(int device, const float* q, const float* kv, int B, int S, int W, int H, float* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(q && kv && out, "NULL buffer");
+        MB_CHECK_ARG(B > 0 && S > 0 && W > 0 && H > 0, "B, S, W, H must be positive");
+        MB_CHECK_ARG(W == H * 64, "head_dim must be 64 (W %d, H %d)", W, H);
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const size_t M = (size_t)B * S;
+        const float* dq = sc.upload(q, (size_t)W);
+        __nv_bfloat16* dkv = sc.upload_bf16(kv, M * 2 * W);
+        __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>((size_t)B * W);
+        float* dOut = sc.alloc<float>((size_t)B * W);
+        kernels::map_attention(dq, dkv, B, S, W, H, dO, sc.s);
+        const long long n = (long long)B * W;
+        bf16_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, sc.s>>>(dO, dOut, n);
+        MB_CUDA(cudaGetLastError());
+        MB_CUDA(cudaStreamSynchronize(sc.s));
+        MB_CUDA(cudaMemcpy(out, dOut, (size_t)B * W * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
 }  // extern "C"

@@ -78,8 +78,8 @@ struct Params {
     int M, N, K;
     int tiles_m, tiles_n;
     Epilogue ep;
-    // GATHER only: uint8 HWC images [n, S, S, 3]; A row r = token t = r % (g*g + 1) of image r / (g*g + 1): zero for
-    // t = 0 (the class token), else patch t - 1, row-major in the grid.
+    // GATHER only: uint8 HWC images [n, S, S, 3]; A row r = token t = r % (g*g + cls) of image r / (g*g + cls): zero
+    // for t < cls (the class token), else patch t - cls, row-major in the grid.
     // k index of the A row = dy * (64 * kbpd) + dx * 3 + c (kernels::patch_weight_rows lays W out the same way).
     const uint8_t* img;
     int g;                  // patches per image side
@@ -88,6 +88,7 @@ struct Params {
     int seg;                // 3 * patch: bytes (= k values) of one patch pixel row
     int kbpd;               // 64-slot k-blocks per patch pixel row: ceil(seg / 64)
     float nscale[3], nshift[3];   // (u8 * nscale[c] + nshift[c]) == (u8/255 - mean[c]) / std[c]
+    int cls;                // class-token rows per image: 1 (CLIP) or 0 (SigLIP)
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -289,10 +290,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         const uint8_t* prow = nullptr;
         if (GATHER) {
             const int r = m0 + pt;
-            const int tokens = p.g * p.g + 1;
-            const int b = r / tokens, t = r - b * tokens;
-            if (r < p.M && t > 0) {
-                const int py = (t - 1) / p.g, px = (t - 1) - py * p.g;
+            const int tokens = p.g * p.g + p.cls;
+            const int b = r / tokens, t = r - b * tokens - p.cls;
+            if (r < p.M && t >= 0) {
+                const int py = t / p.g, px = t - py * p.g;
                 prow = p.img + ((size_t)b * p.g * p.patch + (size_t)py * p.patch) * p.row_bytes + (size_t)px * p.patch * 3;
             }
         }
@@ -611,6 +612,7 @@ static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W
         p.row_bytes = 3 * pg->S;
         p.seg = 3 * pg->patch;
         p.kbpd = patch_gather_kbpd(pg->patch);
+        p.cls = pg->cls;
         for (int c = 0; c < 3; ++c) {
             p.nscale[c] = (float)(1.0 / (255.0 * (double)pg->std[c]));
             p.nshift[c] = (float)(-(double)pg->mean[c] / (double)pg->std[c]);
@@ -668,8 +670,9 @@ void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, c
     if (!ep.out_fp32 || ep.act != ACT_NONE) fail(B200_ERR_INTERNAL, "patch gather: fp32 output without activation only");
     check_epilogue(ep);
     configure();
+    if (pg.cls != 0 && pg.cls != 1) fail(B200_ERR_INTERNAL, "patch gather: cls = %d must be 0 or 1", pg.cls);
     const int g = pg.S / pg.patch;
-    const long long M = (long long)pg.n * (g * g + 1);
+    const long long M = (long long)pg.n * (g * g + pg.cls);
     if (M > 0x7fffffffLL) fail(B200_ERR_INVALID_ARG, "patch gather: batch of %d images is too large", pg.n);
     launch_tiles<true, true, ACT_NONE>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
 }

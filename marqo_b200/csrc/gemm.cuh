@@ -31,15 +31,17 @@ int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N
            int sm_count, cudaStream_t stream);
 
 // ViT patch embedding straight from uint8 pixels (SURVEY §8 a2; add_docs.py:129-134 + clip_utils.py:48-67 fused into the
-// conv1 GEMM's operand load): out = epilogue( patches(img) x Wg^T ) over the n (g^2 + 1) ViT token rows of the uint8
-// HWC batch [n, S, S, 3] (S % patch == 0, g = S / patch).  Row r of the virtual A matrix is token t = r % (g^2 + 1) of
-// image r / (g^2 + 1): zero for the class token t = 0, else patch t - 1 (row-major in the g x g grid), normalised as
-// ToTensor + Normalize.  Wg [N, patch_gather_k(patch)] is conv1.weight re-laid by kernels::patch_weight_rows.  No patch
-// matrix exists in HBM: the gather warps of the GEMM read the image rows, convert and write the swizzled smem A stage.
-// The epilogue must have an fp32 output and no activation.
+// conv1 GEMM's operand load): out = epilogue( patches(img) x Wg^T ) over the n (g^2 + cls) ViT token rows of the uint8
+// HWC batch [n, S, S, 3] (S % patch == 0, g = S / patch).  Row r of the virtual A matrix is token t = r % (g^2 + cls)
+// of image r / (g^2 + cls): zero for the class token t < cls, else patch t - cls (row-major in the g x g grid),
+// normalised as ToTensor + Normalize.  cls is 1 for CLIP and 0 for the class-token-free SigLIP tower.  Wg [N,
+// patch_gather_k(patch)] is conv1.weight re-laid by kernels::patch_weight_rows.  No patch matrix exists in HBM: the
+// gather warps of the GEMM read the image rows, convert and write the swizzled smem A stage.  The epilogue must have an
+// fp32 output and no activation.
 struct PatchGather {
     const uint8_t* img = nullptr;
     int n = 0, S = 0, patch = 0;
+    int cls = 1;
     float mean[3] = {0.f, 0.f, 0.f}, std[3] = {1.f, 1.f, 1.f};
 };
 inline int patch_gather_kbpd(int patch) { return (3 * patch + 63) / 64; }

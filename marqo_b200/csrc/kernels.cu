@@ -92,10 +92,10 @@ void layernorm(const float* x, long long in_stride, const float* gamma, const fl
 
 // ------------------------------------------------------------------------------------------------ im2col
 __global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ chw, int n, int S, int p, int kpad,
-                                                     __nv_bfloat16* __restrict__ out) {
-    // one thread = 8 consecutive k of one token row; the class-token row (t == 0) of each image is zero
+                                                     int cls, __nv_bfloat16* __restrict__ out) {
+    // one thread = 8 consecutive k of one token row; the class-token row (t < cls) of each image is zero
     const int g = S / p;
-    const int tokens = g * g + 1;
+    const int tokens = g * g + cls;
     const int groups = kpad / 8;
     const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long total = (long long)n * tokens * groups;
@@ -103,15 +103,15 @@ __global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ c
     const int kg = (int)(gid % groups);
     const long long row = gid / groups;
     const long long b = row / tokens;
-    const int t = (int)(row - b * tokens);
-    const int px = (t - 1) % g, py = (t - 1) / g;
+    const int t = (int)(row - b * tokens) - cls;
+    const int px = t % g, py = t / g;
     const int K = 3 * p * p;
     float f[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
         const int k = kg * 8 + e;
         float val = 0.f;
-        if (t > 0 && k < K) {
+        if (t >= 0 && k < K) {
             const int c = k / (p * p);
             const int rem = k - c * p * p;
             const int dy = rem / p, dx = rem - dy * p;
@@ -124,11 +124,11 @@ __global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ c
         make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
 }
 
-void im2col_f32(const float* chw, int n, int S, int p, int kpad, __nv_bfloat16* out, cudaStream_t s) {
+void im2col_f32(const float* chw, int n, int S, int p, int kpad, int cls, __nv_bfloat16* out, cudaStream_t s) {
     if (n <= 0) return;
     const int g = S / p;
-    const long long total = (long long)n * (g * g + 1) * (kpad / 8);
-    im2col_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(chw, n, S, p, kpad, out);
+    const long long total = (long long)n * (g * g + cls) * (kpad / 8);
+    im2col_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(chw, n, S, p, kpad, cls, out);
     MB_CUDA(cudaGetLastError());
 }
 
@@ -142,7 +142,7 @@ __global__ void __launch_bounds__(256) vit_embed_kernel(float4* __restrict__ x, 
     const long long row = i / w4;
     const int c = (int)(i - row * w4), t = (int)(row % tokens_per_image);
     float4 v = __ldg(pos + (long long)t * w4 + c);
-    if (t == 0) {
+    if (t == 0 && cls != nullptr) {
         const float4 a = __ldg(cls + c);
         v = make_float4(a.x + v.x, a.y + v.y, a.z + v.z, a.w + v.w);
     }
@@ -600,19 +600,9 @@ __global__ void resample_v_kernel(const uint8_t* __restrict__ tmp, int n, int h,
 
 static int py_round_half_even(double v) { return (int)nearbyint(v); }
 
-void resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s) {
-    if (n <= 0) return;
-    // torchvision Resize(S): shortest side -> S, the other int(S * long / short); CenterCrop(S)
-    int new_w, new_h;
-    if (w <= h) {
-        new_w = S;
-        new_h = (int)((double)((long long)S * h) / (double)w);  // int(S * long / short): Python true division
-    } else {
-        new_h = S;
-        new_w = (int)((double)((long long)S * w) / (double)h);
-    }
-    const int left = py_round_half_even((new_w - S) / 2.0);
-    const int top = py_round_half_even((new_h - S) / 2.0);
+// Resample [n, h, w, 3] to new_h x new_w and keep the S x S window at (top, left).
+static void resample_window_u8(const uint8_t* src, int n, int h, int w, int new_h, int new_w, int top, int left, int S,
+                               uint8_t* dst, cudaStream_t s) {
     const ResampleTable th = precompute(w, new_w);
     const ResampleTable tv = precompute(h, new_h);
     {   // stream-ordered temporaries, released on `s` at the end of this block
@@ -634,6 +624,135 @@ void resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst
     }
     // the pageable host vectors above must outlive the async copies: synchronise before they go out of scope
     MB_CUDA(cudaStreamSynchronize(s));
+}
+
+void resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s) {
+    if (n <= 0) return;
+    // torchvision Resize(S): shortest side -> S, the other int(S * long / short); CenterCrop(S)
+    int new_w, new_h;
+    if (w <= h) {
+        new_w = S;
+        new_h = (int)((double)((long long)S * h) / (double)w);  // int(S * long / short): Python true division
+    } else {
+        new_h = S;
+        new_w = (int)((double)((long long)S * w) / (double)h);
+    }
+    const int left = py_round_half_even((new_w - S) / 2.0);
+    const int top = py_round_half_even((new_h - S) / 2.0);
+    resample_window_u8(src, n, h, w, new_h, new_w, top, left, S, dst, s);
+}
+
+void resize_squash_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s) {
+    if (n <= 0) return;
+    // PIL resize((S, S), BICUBIC) = torchvision Resize((S, S)) on a PIL image: both axes to S, nothing cropped.  An axis
+    // that already has S pixels gets the identity coefficients (a single 1.0 tap), so running its pass is exact.
+    resample_window_u8(src, n, h, w, S, S, 0, 0, S, dst, s);
+}
+
+// ------------------------------------------------------------------------------------------------ SigLIP MAP head
+// One CTA (128 threads) per (image, head).  Pass 1: thread s takes key s (its 64 bf16 values are one 128-byte line)
+// and stores the base-2 logit q.k / 8 * log2(e) in shared memory; pass 2: block max, p = exp2(l - max) in place, block
+// sum; pass 3: warp w accumulates p_s v_s over keys s = w (mod 4), lane l owning columns 2l, 2l + 1; the four partial
+// sums are added in a fixed order and divided by the sum.  Two exact passes over the logits instead of an online
+// softmax: S <= MAP_MAX_TOKENS logits fit in shared memory.
+constexpr int MAP_THREADS = 128;
+constexpr int MAP_MAX_TOKENS = 12288;   // 48 KB of logits
+
+__device__ __forceinline__ float block_reduce_128(float v, float* red, bool is_max) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float u = __shfl_xor_sync(0xffffffffu, v, o);
+        v = is_max ? fmaxf(v, u) : v + u;
+    }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    __syncthreads();   // red[] may still be read by the previous reduction
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    return is_max ? fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3])) : ((red[0] + red[1]) + red[2]) + red[3];
+}
+
+__global__ void __launch_bounds__(MAP_THREADS) map_attention_kernel(const float* __restrict__ q,
+                                                                    const __nv_bfloat16* __restrict__ kv, int S, int W,
+                                                                    __nv_bfloat16* __restrict__ out) {
+    extern __shared__ float logit[];   // [S]
+    __shared__ float qs[64];
+    __shared__ float red[4];
+    __shared__ float part[4][64];
+    const int b = blockIdx.x, h = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if (tid < 64) qs[tid] = q[h * 64 + tid] * (0.125f * 1.4426950408889634f);
+    __syncthreads();
+    const long long ld = 2LL * W;
+    const __nv_bfloat16* keys = kv + (long long)b * S * ld + h * 64;
+    const __nv_bfloat16* vals = keys + W;
+    float mx = -INFINITY;
+    for (int s = tid; s < S; s += MAP_THREADS) {
+        const uint4* k4 = reinterpret_cast<const uint4*>(keys + s * ld);
+        float acc = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const uint4 u = __ldg(k4 + j);
+            const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&u);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 f = __bfloat1622float2(p2[e]);
+                acc = fmaf(qs[8 * j + 2 * e], f.x, acc);
+                acc = fmaf(qs[8 * j + 2 * e + 1], f.y, acc);
+            }
+        }
+        logit[s] = acc;
+        mx = fmaxf(mx, acc);
+    }
+    mx = block_reduce_128(mx, red, true);
+    float sum = 0.f;
+    for (int s = tid; s < S; s += MAP_THREADS) {
+        const float p = exp2f(logit[s] - mx);
+        logit[s] = p;
+        sum += p;
+    }
+    sum = block_reduce_128(sum, red, false);   // its barriers also publish the p values
+    float2 acc = make_float2(0.f, 0.f);
+    for (int s = warp; s < S; s += 4) {
+        const float p = logit[s];
+        const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(vals + s * ld + 2 * lane));
+        acc.x = fmaf(p, f.x, acc.x);
+        acc.y = fmaf(p, f.y, acc.y);
+    }
+    part[warp][2 * lane] = acc.x;
+    part[warp][2 * lane + 1] = acc.y;
+    __syncthreads();
+    if (tid < 64) {
+        const float o = ((part[0][tid] + part[1][tid]) + part[2][tid]) + part[3][tid];
+        out[(long long)b * W + h * 64 + tid] = __float2bfloat16_rn(o / sum);
+    }
+}
+
+void map_attention(const float* q, const __nv_bfloat16* kv, int n, int S, int W, int heads, __nv_bfloat16* out,
+                   cudaStream_t s) {
+    if (n <= 0) return;
+    if (W != heads * 64) fail(B200_ERR_UNSUPPORTED, "map_attention: head_dim must be 64 (width %d, heads %d)", W, heads);
+    if (S <= 0 || S > MAP_MAX_TOKENS) fail(B200_ERR_UNSUPPORTED, "map_attention: %d tokens (1..%d)", S, MAP_MAX_TOKENS);
+    map_attention_kernel<<<dim3((unsigned)n, (unsigned)heads), MAP_THREADS, (size_t)S * sizeof(float), s>>>(q, kv, S, W,
+                                                                                                        out);
+    MB_CUDA(cudaGetLastError());
+}
+
+__global__ void __launch_bounds__(256) l2_rows_kernel(const float* __restrict__ src, int n, int E, int normalize,
+                                                      float* __restrict__ out) {
+    const int b = blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (b >= n) return;
+    const float* row = src + (long long)b * E;
+    float ss = 0.f;
+    if (normalize)
+        for (int i = lane; i < E; i += 32) ss += row[i] * row[i];
+    const float nrm = sqrtf(warp_sum(ss));
+    for (int i = lane; i < E; i += 32) out[(long long)b * E + i] = normalize ? row[i] / nrm : row[i];
+}
+
+void l2_rows(const float* src, int n, int E, int normalize, float* out, cudaStream_t s) {
+    if (n <= 0) return;
+    l2_rows_kernel<<<(n + 7) / 8, 256, 0, s>>>(src, n, E, normalize, out);
+    MB_CUDA(cudaGetLastError());
 }
 
 }  // namespace kernels

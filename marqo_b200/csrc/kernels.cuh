@@ -11,13 +11,13 @@ namespace kernels {
 void layernorm(const float* x, long long in_stride, const float* gamma, const float* beta, float eps, int rows, int w,
                float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s);
 
-// Already-normalised fp32 CHW [n, 3, S, S] -> bf16 A matrix of the ViT token rows [n * (g*g + 1), kpad]: row
-// b * (g*g + 1) + t is zero for the class token t = 0, else patch t - 1 (row-major in the g x g grid) with
-// k = c*p*p + dy*p + dx, zero for k >= 3*p*p.
-void im2col_f32(const float* chw, int n, int S, int p, int kpad, __nv_bfloat16* out, cudaStream_t s);
+// Already-normalised fp32 CHW [n, 3, S, S] -> bf16 A matrix of the ViT token rows [n * (g*g + cls), kpad]: row
+// b * (g*g + cls) + t is zero for the class token t < cls (cls is 1 for CLIP, 0 for SigLIP), else patch t - cls
+// (row-major in the g x g grid) with k = c*p*p + dy*p + dx, zero for k >= 3*p*p.
+void im2col_f32(const float* chw, int n, int S, int p, int kpad, int cls, __nv_bfloat16* out, cudaStream_t s);
 
-// x[b * tokens_per_image + t, :] = positional_embedding[t], plus class_embedding for t == 0 (w % 4 == 0): the rows the
-// patch-embed GEMM then adds conv1(patch) onto in place
+// x[b * tokens_per_image + t, :] = positional_embedding[t], plus class_embedding for t == 0 unless cls is NULL
+// (w % 4 == 0): the rows the patch-embed GEMM then adds conv1(patch) onto in place
 void vit_embed_rows(float* x, const float* cls, const float* pos, int n, int tokens_per_image, int w, cudaStream_t s);
 
 // CLIP text: x[b, s, :] = token_embedding[ids[b, s]] + positional_embedding[s]; also eot[b] = arg-max_s ids[b, s]
@@ -57,6 +57,16 @@ void patch_weight_rows(const float* src, int rows, int p, int kbpd, __nv_bfloat1
 
 // PIL-compatible antialiased bicubic resize (shortest side -> S) + centre crop, uint8 HWC in/out.
 void resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s);
+// The same resampling squashed to S x S (x and y scaled independently, no crop): PIL resize((S, S), BICUBIC).
+void resize_squash_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s);
+
+// SigLIP MAP pooling attention, one latent query per head: out[b, h*64 .. h*64+63] = softmax_s(q_h . k_{b,s} / 8) v_{b,s}
+// (bf16).  q fp32 [W] (shared by every image); kv bf16 [n*S, 2W] (K columns, then V columns, head-major); head_dim 64.
+void map_attention(const float* q, const __nv_bfloat16* kv, int n, int S, int W, int heads, __nv_bfloat16* out,
+                   cudaStream_t s);
+
+// out[b] = src[b] / |src[b]| if normalize (no epsilon: abstract_clip_model.py:83-85), else src[b]; rows of E floats.
+void l2_rows(const float* src, int n, int E, int normalize, float* out, cudaStream_t s);
 
 }  // namespace kernels
 }  // namespace mb

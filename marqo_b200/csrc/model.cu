@@ -1,4 +1,4 @@
-// Encoder runtime: CLIP ViT image tower, CLIP text tower, BERT (e5, MiniLM, bge), MPNet — SURVEY §8 a2-a5.
+// Encoder runtime: CLIP ViT image tower, CLIP text tower, SigLIP towers, BERT (e5, MiniLM, bge), MPNet — SURVEY §8 a2-a5.
 //
 // What the reference calls (third-party, restated in oracle/encoders.py):
 //   OPEN_CLIP.encode_image / encode_text   src/marqo/core/inference/embedding_models/open_clip_model.py:249-286
@@ -38,17 +38,34 @@ struct LayerW {
     const __nv_bfloat16 *w_qkv = nullptr, *w_o = nullptr, *w_fc = nullptr, *w_proj = nullptr;
 };
 
+// SigLIP's MAP pooling head (timm AttentionPoolLatent with one latent): q = latent W_q^T + b_q is batch-independent and
+// built once by b200_model_finalize.
+struct MapW {
+    const float* q = nullptr;                                    // fp32 [width]
+    const __nv_bfloat16 *w_kv = nullptr, *w_proj = nullptr, *w_fc1 = nullptr, *w_fc2 = nullptr;
+    const float *b_kv = nullptr, *b_proj = nullptr, *b_fc1 = nullptr, *b_fc2 = nullptr, *ln_w = nullptr, *ln_b = nullptr;
+    int mlp = 0;
+};
+
 struct TowerW {
     b200_tower_desc d{};
     bool present = false;
     std::vector<LayerW> layers;
+    float eps = 1e-5f;                      // every LayerNorm of the tower
     // vision
     const __nv_bfloat16* conv_w = nullptr;  // [width, kpad]
     const __nv_bfloat16* conv_wg = nullptr; // [width, gemm::patch_gather_k(patch)]: gather GEMM order
     int kpad = 0, grid = 0, tokens = 0;
+    int cls_rows = 1;                       // class-token rows per image: 1 (CLIP), 0 (SigLIP)
+    // pos: CLIP positional_embedding [grid^2 + 1, width]; SigLIP pos_embed + the patch conv's bias [grid^2, width].
+    // ln_pre is NULL for SigLIP.
     const float *cls = nullptr, *pos = nullptr, *ln_pre_w = nullptr, *ln_pre_b = nullptr;
-    // final LN (ln_post / ln_final) and projection [width, embed]
+    // final LN (ln_post / ln_final / trunk.norm) and CLIP's projection [width, embed]
     const float *ln_out_w = nullptr, *ln_out_b = nullptr, *proj = nullptr;
+    // SigLIP text projection (nn.Linear [embed, width] + bias) and vision MAP head
+    const __nv_bfloat16* w_tproj = nullptr;
+    const float* b_tproj = nullptr;
+    MapW map;
     // text / bert embeddings
     const float *tok = nullptr, *type0 = nullptr, *emb_ln_w = nullptr, *emb_ln_b = nullptr;
     int max_pos = 0;
@@ -139,24 +156,34 @@ const __nv_bfloat16* to_bf16(b200_model* m, const std::string& name, long long n
     return dst;
 }
 
-void build_clip_layers(b200_model* m, TowerW& T, const std::string& prefix) {
+// Checkpoint names of a pre-LN block: open_clip ResidualAttentionBlock and timm's ViT Block (SigLIP's vision trunk)
+// have the same arithmetic and the same fused q|k|v layout.
+struct PreLnNames {
+    const char *ln1, *qkv_w, *qkv_b, *out, *ln2, *fc, *proj;
+};
+const PreLnNames OPEN_CLIP_BLOCK{"ln_1", "attn.in_proj_weight", "attn.in_proj_bias", "attn.out_proj", "ln_2", "mlp.c_fc",
+                                 "mlp.c_proj"};
+const PreLnNames TIMM_BLOCK{"norm1", "attn.qkv.weight", "attn.qkv.bias", "attn.proj", "norm2", "mlp.fc1", "mlp.fc2"};
+
+// blocks: the prefix of block i's names up to the index ("visual.transformer.resblocks.", "visual.trunk.blocks.", ...)
+void build_preln_layers(b200_model* m, TowerW& T, const std::string& blocks, const PreLnNames& nm) {
     const long long w = T.d.width, mlp = T.d.mlp;
     T.layers.resize(T.d.layers);
     for (int i = 0; i < T.d.layers; ++i) {
-        const std::string p = prefix + "transformer.resblocks." + std::to_string(i) + ".";
+        const std::string p = blocks + std::to_string(i) + ".";
         LayerW& L = T.layers[i];
-        L.ln1_w = param(m, p + "ln_1.weight", w);
-        L.ln1_b = param(m, p + "ln_1.bias", w);
-        L.w_qkv = to_bf16(m, p + "attn.in_proj_weight", 3 * w * w);
-        L.b_qkv = param(m, p + "attn.in_proj_bias", 3 * w);
-        L.w_o = to_bf16(m, p + "attn.out_proj.weight", w * w);
-        L.b_o = param(m, p + "attn.out_proj.bias", w);
-        L.ln2_w = param(m, p + "ln_2.weight", w);
-        L.ln2_b = param(m, p + "ln_2.bias", w);
-        L.w_fc = to_bf16(m, p + "mlp.c_fc.weight", mlp * w);
-        L.b_fc = param(m, p + "mlp.c_fc.bias", mlp);
-        L.w_proj = to_bf16(m, p + "mlp.c_proj.weight", w * mlp);
-        L.b_proj = param(m, p + "mlp.c_proj.bias", w);
+        L.ln1_w = param(m, p + nm.ln1 + ".weight", w);
+        L.ln1_b = param(m, p + nm.ln1 + ".bias", w);
+        L.w_qkv = to_bf16(m, p + nm.qkv_w, 3 * w * w);
+        L.b_qkv = param(m, p + nm.qkv_b, 3 * w);
+        L.w_o = to_bf16(m, p + nm.out + ".weight", w * w);
+        L.b_o = param(m, p + nm.out + ".bias", w);
+        L.ln2_w = param(m, p + nm.ln2 + ".weight", w);
+        L.ln2_b = param(m, p + nm.ln2 + ".bias", w);
+        L.w_fc = to_bf16(m, p + nm.fc + ".weight", mlp * w);
+        L.b_fc = param(m, p + nm.fc + ".bias", mlp);
+        L.w_proj = to_bf16(m, p + nm.proj + ".weight", w * mlp);
+        L.b_proj = param(m, p + nm.proj + ".bias", w);
     }
 }
 
@@ -246,6 +273,58 @@ attention::RelBias build_rel_bias(b200_model* m, const TowerW& T) {
     return b;
 }
 
+std::vector<float> to_host(const float* d, size_t n) {
+    std::vector<float> h(n);
+    MB_CUDA(cudaMemcpy(h.data(), d, n * sizeof(float), cudaMemcpyDeviceToHost));
+    return h;
+}
+
+const float* upload_derived(b200_model* m, const std::vector<float>& h) {
+    float* d = derived_buffer<float>(m, h.size());
+    MB_CUDA(cudaMemcpy(d, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice));
+    return d;
+}
+
+// SigLIP's timm trunk after the patch conv (open_clip names, verify): pos_embed with the conv bias folded in (the bias
+// is the same for every token, so pos[t] + bias + conv(patch) == pos'[t] + conv(patch)), the blocks, the final norm and
+// the MAP head, whose latent query projection q = latent W_q^T + b_q is computed here once, in double.
+void build_siglip_vision(b200_model* m, TowerW& T) {
+    const long long w = T.d.width;
+    const std::string t = "visual.trunk.";
+    std::vector<float> pos = to_host(param(m, t + "pos_embed", (long long)T.tokens * w), (size_t)T.tokens * w);
+    const std::vector<float> bias = to_host(param(m, t + "patch_embed.proj.bias", w), (size_t)w);
+    for (long long i = 0; i < (long long)pos.size(); ++i) pos[i] += bias[i % w];
+    T.pos = upload_derived(m, pos);
+    build_preln_layers(m, T, t + "blocks.", TIMM_BLOCK);
+    T.ln_out_w = param(m, t + "norm.weight", w);
+    T.ln_out_b = param(m, t + "norm.bias", w);
+    const std::string a = t + "attn_pool.";
+    const std::vector<float> latent = to_host(param(m, a + "latent", w), (size_t)w);
+    const std::vector<float> wq = to_host(param(m, a + "q.weight", w * w), (size_t)(w * w));
+    const std::vector<float> bq = to_host(param(m, a + "q.bias", w), (size_t)w);
+    std::vector<float> q((size_t)w);
+    for (long long o = 0; o < w; ++o) {
+        double acc = bq[o];
+        for (long long i = 0; i < w; ++i) acc += (double)wq[o * w + i] * latent[i];
+        q[o] = (float)acc;
+    }
+    MapW& P = T.map;
+    P.q = upload_derived(m, q);
+    P.w_kv = to_bf16(m, a + "kv.weight", 2 * w * w);
+    P.b_kv = param(m, a + "kv.bias", 2 * w);
+    P.w_proj = to_bf16(m, a + "proj.weight", w * w);
+    P.b_proj = param(m, a + "proj.bias", w);
+    P.ln_w = param(m, a + "norm.weight", w);
+    P.ln_b = param(m, a + "norm.bias", w);
+    const long long mlp = param_rows(m, a + "mlp.fc1.weight", w);
+    MB_CHECK_ARG(mlp > 0 && mlp % 64 == 0, "%smlp.fc1 has %lld rows: a positive multiple of 64 is needed", a.c_str(), mlp);
+    P.mlp = (int)mlp;
+    P.w_fc1 = to_bf16(m, a + "mlp.fc1.weight", mlp * w);
+    P.b_fc1 = param(m, a + "mlp.fc1.bias", mlp);
+    P.w_fc2 = to_bf16(m, a + "mlp.fc2.weight", w * mlp);
+    P.b_fc2 = param(m, a + "mlp.fc2.bias", w);
+}
+
 struct Counter {
     int n = 0;
 };
@@ -291,7 +370,7 @@ void run_clip_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, i
     const int M = B * S, w = T.d.width, mlp = T.d.mlp;
     const int act = m->desc.act == B200_ACT_QUICKGELU ? gemm::ACT_QUICKGELU : gemm::ACT_GELU;
     for (const LayerW& L : T.layers) {
-        kernels::layernorm(m->x.get(), w, L.ln1_w, L.ln1_b, 1e-5f, M, w, nullptr, m->h.get(), m->stream);
+        kernels::layernorm(m->x.get(), w, L.ln1_w, L.ln1_b, T.eps, M, w, nullptr, m->h.get(), m->stream);
         ++c.n;
         gemm::Epilogue e1;
         e1.bias = L.b_qkv;
@@ -307,7 +386,7 @@ void run_clip_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, i
         e2.ldo = w;
         e2.out_fp32 = 1;
         linear(m, c, m->o.get(), M, w, L.w_o, w, e2);
-        kernels::layernorm(m->x.get(), w, L.ln2_w, L.ln2_b, 1e-5f, M, w, nullptr, m->h.get(), m->stream);
+        kernels::layernorm(m->x.get(), w, L.ln2_w, L.ln2_b, T.eps, M, w, nullptr, m->h.get(), m->stream);
         ++c.n;
         gemm::Epilogue e3;
         e3.bias = L.b_fc;
@@ -366,13 +445,50 @@ void run_bert_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, f
     }
 }
 
+// The small-M GEMMs of the SigLIP heads: out = act(A[M, K] W[N, K]^T + bias) (+ residual == out, fp32)
+void head_linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, const __nv_bfloat16* W, int N,
+                 const float* bias, int act, void* out, bool out_fp32, bool residual) {
+    gemm::Epilogue e;
+    e.bias = bias;
+    e.act = act;
+    e.out = out;
+    e.ldo = N;
+    e.out_fp32 = out_fp32 ? 1 : 0;
+    if (residual) {
+        e.residual = static_cast<const float*>(out);
+        e.ldr = N;
+    }
+    linear(m, c, A, M, K, W, N, e);
+}
+
+// SigLIP vision head over the n * S token rows in x: final LayerNorm of every token -> h, K|V projection -> qkv
+// [n * S, 2w], one latent query per head attending over its image's tokens -> o [n, w], then proj -> pooled (fp32),
+// pooled + MLP(LN(pooled)), optional L2 -> d_out.
+void map_head(b200_model* m, Counter& c, const TowerW& T, int n, int normalize, float* d_out) {
+    const int S = T.tokens, w = T.d.width, M = n * S;
+    const MapW& P = T.map;
+    kernels::layernorm(m->x.get(), w, T.ln_out_w, T.ln_out_b, T.eps, M, w, nullptr, m->h.get(), m->stream);
+    head_linear(m, c, m->h.get(), M, w, P.w_kv, 2 * w, P.b_kv, gemm::ACT_NONE, m->qkv.get(), false, false);
+    {
+        ProfScope ps(m, 1);
+        kernels::map_attention(P.q, m->qkv.get(), n, S, w, T.d.heads, m->o.get(), m->stream);
+    }
+    head_linear(m, c, m->o.get(), n, w, P.w_proj, w, P.b_proj, gemm::ACT_NONE, m->pooled.get(), true, false);
+    kernels::layernorm(m->pooled.get(), w, P.ln_w, P.ln_b, T.eps, n, w, nullptr, m->h.get(), m->stream);
+    head_linear(m, c, m->h.get(), n, w, P.w_fc1, P.mlp, P.b_fc1, gemm::ACT_GELU, m->u.get(), false, false);
+    head_linear(m, c, m->u.get(), n, P.mlp, P.w_fc2, w, P.b_fc2, gemm::ACT_NONE, m->pooled.get(), true, true);
+    kernels::l2_rows(m->pooled.get(), n, w, normalize, d_out, m->stream);
+    c.n += 4;
+}
+
 // images already as device uint8 [n, S, S, 3] (u8 != nullptr) or device fp32 CHW (f32 != nullptr)
 void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const float* f32, int n, int normalize,
                           float* d_out) {
     const TowerW& T = m->vision;
     const int S = T.d.image_size, p = T.d.patch, w = T.d.width;
     // x = positional embedding (+ class embedding on each image's first row), then conv1 (no bias) of every token row
-    // added onto it in place; a class-token row multiplies a zero A row
+    // added onto it in place; a class-token row multiplies a zero A row.  SigLIP has no class row, and its conv bias is
+    // already in T.pos.
     kernels::vit_embed_rows(m->x.get(), T.cls, T.pos, n, T.tokens, w, m->stream);
     gemm::Epilogue e;
     e.residual = m->x.get();
@@ -387,6 +503,7 @@ void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const fl
         pg.n = n;
         pg.S = S;
         pg.patch = p;
+        pg.cls = T.cls_rows;
         for (int i = 0; i < 3; ++i) {
             pg.mean[i] = m->desc.image_mean[i];
             pg.std[i] = m->desc.image_std[i];
@@ -397,14 +514,21 @@ void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const fl
     } else {
         // preprocessed fp32 CHW tensors (the reference's parity path)
         if (!m->patches) m->patches = DeviceBuffer<__nv_bfloat16>((size_t)m->desc.max_batch * T.tokens * T.kpad);
-        kernels::im2col_f32(f32, n, S, p, T.kpad, m->patches.get(), m->stream);
+        kernels::im2col_f32(f32, n, S, p, T.kpad, T.cls_rows, m->patches.get(), m->stream);
         linear(m, c, m->patches.get(), n * T.tokens, T.kpad, T.conv_w, w, e);
         ++c.n;
     }
-    kernels::layernorm(m->x.get(), w, T.ln_pre_w, T.ln_pre_b, 1e-5f, n * T.tokens, w, m->x.get(), nullptr, m->stream);
-    c.n += 2;
+    ++c.n;
+    if (T.ln_pre_w) {
+        kernels::layernorm(m->x.get(), w, T.ln_pre_w, T.ln_pre_b, T.eps, n * T.tokens, w, m->x.get(), nullptr, m->stream);
+        ++c.n;
+    }
     run_clip_blocks(m, c, T, n, T.tokens, attention::MASK_NONE);
-    kernels::clip_head(m->x.get(), T.tokens, nullptr, T.ln_out_w, T.ln_out_b, 1e-5f, T.proj, n, w, m->desc.embed_dim,
+    if (m->desc.arch == B200_ARCH_SIGLIP) {
+        map_head(m, c, T, n, normalize, d_out);
+        return;
+    }
+    kernels::clip_head(m->x.get(), T.tokens, nullptr, T.ln_out_w, T.ln_out_b, T.eps, T.proj, n, w, m->desc.embed_dim,
                        normalize, d_out, m->pooled.get(), m->stream);
     c.n += 3;
 }
@@ -417,8 +541,18 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
         kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, m->x.get(), m->aux.get(), m->stream);
         c.n += 1;
         run_clip_blocks(m, c, T, n, S, attention::MASK_CAUSAL);
-        kernels::clip_head(m->x.get(), S, m->aux.get(), T.ln_out_w, T.ln_out_b, 1e-5f, T.proj, n, w, m->desc.embed_dim,
+        kernels::clip_head(m->x.get(), S, m->aux.get(), T.ln_out_w, T.ln_out_b, T.eps, T.proj, n, w, m->desc.embed_dim,
                            normalize, d_out, m->pooled.get(), m->stream);
+        c.n += 3;
+    } else if (m->desc.arch == B200_ARCH_SIGLIP) {
+        // bidirectional blocks; ln_final of each sequence's last row (stride S rows) -> h [n, w], biased projection
+        const int E = m->desc.embed_dim;
+        kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, m->x.get(), m->aux.get(), m->stream);
+        run_clip_blocks(m, c, T, n, S, attention::MASK_NONE);
+        kernels::layernorm(m->x.get() + (size_t)(S - 1) * w, (long long)S * w, T.ln_out_w, T.ln_out_b, T.eps, n, w,
+                           nullptr, m->h.get(), m->stream);
+        head_linear(m, c, m->h.get(), n, w, T.w_tproj, E, T.b_tproj, gemm::ACT_NONE, m->pooled.get(), true, false);
+        kernels::l2_rows(m->pooled.get(), n, E, normalize, d_out, m->stream);
         c.n += 3;
     } else if (m->desc.arch == B200_ARCH_MPNET) {
         const float eps = m->desc.layer_norm_eps;
@@ -528,7 +662,10 @@ void encode_images_u8_dev(b200_model* m, Counter& c, const uint8_t* d_img, int n
         const int nb = std::min(cap, n - o);
         const uint8_t* src = d_img + (size_t)o * h * w * 3;
         if (h != S || w != S) {
-            kernels::resize_crop_u8(src, nb, h, w, S, m->resized.get(), m->stream);
+            if (m->desc.arch == B200_ARCH_SIGLIP)   // open_clip's SigLIP preprocessing squashes (no aspect, no crop)
+                kernels::resize_squash_u8(src, nb, h, w, S, m->resized.get(), m->stream);
+            else
+                kernels::resize_crop_u8(src, nb, h, w, S, m->resized.get(), m->stream);
             c.n += 2;
             src = m->resized.get();
         }
@@ -561,11 +698,17 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         MB_CHECK_ARG(desc && out, "NULL argument");
         *out = nullptr;
         require_sm90_device(device);
-        MB_CHECK_ARG(desc->arch == B200_ARCH_CLIP || desc->arch == B200_ARCH_BERT || desc->arch == B200_ARCH_MPNET,
+        MB_CHECK_ARG(desc->arch == B200_ARCH_CLIP || desc->arch == B200_ARCH_BERT || desc->arch == B200_ARCH_MPNET ||
+                         desc->arch == B200_ARCH_SIGLIP,
                      "unknown arch %d", desc->arch);
         MB_CHECK_ARG(desc->max_batch > 0, "max_batch must be positive");
         MB_CHECK_ARG(desc->embed_dim > 0 && desc->embed_dim <= 4096, "embed_dim out of range");
-        const bool has_vision = desc->arch == B200_ARCH_CLIP && desc->vision.layers > 0;
+        const bool siglip = desc->arch == B200_ARCH_SIGLIP;
+        const bool has_vision = (desc->arch == B200_ARCH_CLIP || siglip) && desc->vision.layers > 0;
+        if (siglip) {
+            MB_CHECK_ARG(desc->layer_norm_eps > 0.f, "SigLIP: layer_norm_eps must be positive");
+            MB_CHECK_ARG(desc->embed_dim % 32 == 0, "SigLIP: embed_dim %d must be a multiple of 32", desc->embed_dim);
+        }
         const bool has_text = desc->text.layers > 0;
         MB_CHECK_ARG(has_vision || has_text, "model has no tower");
         if (has_vision) {
@@ -573,11 +716,19 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
             MB_CHECK_ARG(desc->vision.patch > 0 && desc->vision.image_size % desc->vision.patch == 0,
                          "image_size must be a multiple of patch");
             for (int i = 0; i < 3; ++i) MB_CHECK_ARG(desc->image_std[i] > 0.f, "image_std must be positive");
+            if (siglip) {
+                // the MAP head has no projection; its single-query attention runs head_dim 64 only
+                MB_CHECK_ARG(desc->embed_dim == desc->vision.width, "SigLIP: embed_dim %d must equal the vision width %d",
+                             desc->embed_dim, desc->vision.width);
+                MB_CHECK_ARG(desc->vision.width == desc->vision.heads * 64,
+                             "SigLIP: vision head_dim must be 64 (width %d, heads %d)", desc->vision.width,
+                             desc->vision.heads);
+            }
         }
         if (has_text) {
             check_tower(desc->text, "text");
             MB_CHECK_ARG(desc->text.ctx > 0 && desc->text.vocab > 0, "text.ctx and text.vocab must be positive");
-            if (desc->arch != B200_ARCH_CLIP)
+            if (desc->arch != B200_ARCH_CLIP && !siglip)
                 MB_CHECK_ARG(desc->embed_dim == desc->text.width, "BERT / MPNet embed_dim must equal width");
             if (desc->arch == B200_ARCH_MPNET) {
                 MB_CHECK_ARG(desc->text.width == desc->text.heads * 64, "MPNet: head_dim must be 64 (width %d, heads %d)",
@@ -639,14 +790,17 @@ int b200_model_finalize(b200_model* m) {
         DeviceGuard g(m->device);
         const int E = m->desc.embed_dim;
         long long max_tok = 0, max_w = 0, max_mlp = 0;
+        const bool siglip = m->desc.arch == B200_ARCH_SIGLIP;
+        if (siglip) m->vision.eps = m->text.eps = m->desc.layer_norm_eps;
         if (m->vision.present) {
             TowerW& T = m->vision;
             const long long w = T.d.width, p = T.d.patch;
             T.grid = T.d.image_size / T.d.patch;
-            T.tokens = T.grid * T.grid + 1;
+            T.cls_rows = siglip ? 0 : 1;
+            T.tokens = T.grid * T.grid + T.cls_rows;
             const int K = 3 * (int)p * (int)p;
             T.kpad = (int)round_up((size_t)K, 64);
-            const float* conv = param(m, "visual.conv1.weight", w * K);
+            const float* conv = param(m, siglip ? "visual.trunk.patch_embed.proj.weight" : "visual.conv1.weight", w * K);
             __nv_bfloat16* cw = derived_buffer<__nv_bfloat16>(m, (size_t)w * T.kpad);
             kernels::pad_rows_to_bf16(conv, (int)w, K, T.kpad, cw, m->stream);
             MB_CUDA(cudaStreamSynchronize(m->stream));
@@ -655,17 +809,21 @@ int b200_model_finalize(b200_model* m) {
             kernels::patch_weight_rows(conv, (int)w, (int)p, gemm::patch_gather_kbpd((int)p), cg, m->stream);
             MB_CUDA(cudaStreamSynchronize(m->stream));
             T.conv_wg = cg;
-            T.cls = param(m, "visual.class_embedding", w);
-            T.pos = param(m, "visual.positional_embedding", (long long)T.tokens * w);
-            T.ln_pre_w = param(m, "visual.ln_pre.weight", w);
-            T.ln_pre_b = param(m, "visual.ln_pre.bias", w);
-            build_clip_layers(m, T, "visual.");
-            T.ln_out_w = param(m, "visual.ln_post.weight", w);
-            T.ln_out_b = param(m, "visual.ln_post.bias", w);
-            T.proj = param(m, "visual.proj", w * E);
+            if (siglip) {
+                build_siglip_vision(m, T);
+            } else {
+                T.cls = param(m, "visual.class_embedding", w);
+                T.pos = param(m, "visual.positional_embedding", (long long)T.tokens * w);
+                T.ln_pre_w = param(m, "visual.ln_pre.weight", w);
+                T.ln_pre_b = param(m, "visual.ln_pre.bias", w);
+                build_preln_layers(m, T, "visual.transformer.resblocks.", OPEN_CLIP_BLOCK);
+                T.ln_out_w = param(m, "visual.ln_post.weight", w);
+                T.ln_out_b = param(m, "visual.ln_post.bias", w);
+                T.proj = param(m, "visual.proj", w * E);
+            }
             max_tok = std::max(max_tok, (long long)m->desc.max_batch * T.tokens);
             max_w = std::max(max_w, w);
-            max_mlp = std::max(max_mlp, (long long)T.d.mlp);
+            max_mlp = std::max(max_mlp, (long long)std::max(T.d.mlp, T.map.mlp));
             m->resized = DeviceBuffer<uint8_t>((size_t)m->desc.max_batch * T.d.image_size * T.d.image_size * 3);
         }
         if (m->text.present) {
@@ -675,10 +833,18 @@ int b200_model_finalize(b200_model* m) {
             if (m->desc.arch == B200_ARCH_CLIP) {
                 T.tok = param(m, "token_embedding.weight", (long long)T.d.vocab * w);
                 T.pos = param(m, "positional_embedding", (long long)T.d.ctx * w);
-                build_clip_layers(m, T, "");
+                build_preln_layers(m, T, "transformer.resblocks.", OPEN_CLIP_BLOCK);
                 T.ln_out_w = param(m, "ln_final.weight", w);
                 T.ln_out_b = param(m, "ln_final.bias", w);
                 T.proj = param(m, "text_projection", w * E);
+            } else if (siglip) {
+                T.tok = param(m, "text.token_embedding.weight", (long long)T.d.vocab * w);
+                T.pos = param(m, "text.positional_embedding", (long long)T.d.ctx * w);
+                build_preln_layers(m, T, "text.transformer.resblocks.", OPEN_CLIP_BLOCK);
+                T.ln_out_w = param(m, "text.ln_final.weight", w);
+                T.ln_out_b = param(m, "text.ln_final.bias", w);
+                T.w_tproj = to_bf16(m, "text.text_projection.weight", E * w);
+                T.b_tproj = param(m, "text.text_projection.bias", E);
             } else if (m->desc.arch == B200_ARCH_MPNET) {
                 T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
                 // positions run pad_id + 1 .. pad_id + ctx (pads take pad_id): the table has at least ctx + pad_id + 1 rows
@@ -716,7 +882,7 @@ int b200_model_finalize(b200_model* m) {
         MB_CUDA(cudaStreamSynchronize(m->stream));
         m->aux = DeviceBuffer<int32_t>((size_t)m->desc.max_batch);
         m->out_dev = DeviceBuffer<float>((size_t)m->desc.max_batch * E);
-        m->pooled = DeviceBuffer<float>((size_t)m->desc.max_batch * max_w);
+        m->pooled = DeviceBuffer<float>((size_t)m->desc.max_batch * std::max<long long>(max_w, E));
         MB_CUDA(cudaStreamSynchronize(m->stream));
         m->finalized = true;
     });

@@ -289,10 +289,11 @@ def _to_numpy_f32(t) -> np.ndarray:
 
 
 class Encoder:
-    """A CLIP (vision + text towers), BERT or MPNet encoder resident on one GPU.
+    """A CLIP or SigLIP (vision + text towers), BERT or MPNet encoder resident on one GPU.
 
     `config` keys — CLIP: embed_dim, act ("gelu"|"quickgelu"), mean, std, vision{width,layers,heads,mlp,patch,
-    image_size}, text{width,layers,heads,mlp,ctx,vocab};  BERT: width, layers, heads, mlp, vocab, max_pos, type_vocab,
+    image_size}, text{width,layers,heads,mlp,ctx,vocab};  SigLIP: the CLIP keys plus ln_eps (embed_dim == vision
+    width);  BERT: width, layers, heads, mlp, vocab, max_pos, type_vocab,
     pool ("mean"|"cls");  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
     max_pos - pad_id - 1 tokens), pad_id, ln_eps, rel_buckets, rel_max_distance, pool.  `weights` maps checkpoint
     parameter names (open_clip state_dict names / HF BertModel / MPNetModel names) to fp32 arrays or torch tensors.
@@ -304,8 +305,10 @@ class Encoder:
         self.device = int(device)
         d = N.ModelDesc()
         d.max_batch = int(max_batch)
-        if arch == "clip":
-            d.arch = N.ARCH_CLIP
+        if arch in ("clip", "siglip"):
+            d.arch = N.ARCH_CLIP if arch == "clip" else N.ARCH_SIGLIP
+            if arch == "siglip":
+                d.layer_norm_eps = float(config["ln_eps"])
             d.embed_dim = int(config["embed_dim"])
             d.act = N.ACT_QUICKGELU if config.get("act", "gelu") == "quickgelu" else N.ACT_GELU
             mean = config.get("mean", (0.48145466, 0.4578275, 0.40821073))
@@ -611,4 +614,24 @@ def debug_resize(hwc, S: int, device: int = 0) -> np.ndarray:
     a = _as(hwc, np.uint8)
     out = np.empty((a.shape[0], S, S, 3), np.uint8)
     N.check(N.load().b200_debug_resize(device, _ptr(a), a.shape[0], a.shape[1], a.shape[2], S, _ptr(out)))
+    return out
+
+
+def debug_resize_squash(hwc, S: int, device: int = 0) -> np.ndarray:
+    """uint8 [n, h, w, 3] -> [n, S, S, 3] as PIL resize((S, S), BICUBIC) does (SigLIP's squash resize)."""
+    a = _as(hwc, np.uint8)
+    out = np.empty((a.shape[0], S, S, 3), np.uint8)
+    N.check(N.load().b200_debug_resize_squash(device, _ptr(a), a.shape[0], a.shape[1], a.shape[2], S, _ptr(out)))
+    return out
+
+
+def debug_map_attention(q, kv, B: int, S: int, H: int, device: int = 0) -> np.ndarray:
+    """SigLIP's MAP pooling attention: q fp32 [W] (one latent query), kv [B * S, 2W] (K then V columns, rounded to
+    bf16) -> fp32 [B, W], softmax(q_h k_h^T / 8) v_h per image and head (rounded to bf16)."""
+    qa, kva = _as(q, np.float32), _as(kv, np.float32)
+    W = qa.shape[0]
+    if kva.shape != (B * S, 2 * W):
+        raise ValueError(f"expected kv [{B * S}, {2 * W}], got {kva.shape}")
+    out = np.empty((B, W), np.float32)
+    N.check(N.load().b200_debug_map_attention(device, _ptr(qa), _ptr(kva), B, S, W, H, _ptr(out)))
     return out

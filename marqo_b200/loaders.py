@@ -32,8 +32,8 @@ def _resolve_weights(props: dict, arch: dict, kind: str) -> Dict[str, np.ndarray
     w = props.get("weights")
     if w is None and props.get("random_init") is not None:
         seed = int(props["random_init"])
-        random = {"clip": weights_mod.random_clip_weights, "bert": weights_mod.random_bert_weights,
-                  "mpnet": weights_mod.random_mpnet_weights}[kind]
+        random = {"clip": weights_mod.random_clip_weights, "siglip": weights_mod.random_siglip_weights,
+                  "bert": weights_mod.random_bert_weights, "mpnet": weights_mod.random_mpnet_weights}[kind]
         return random(arch, seed)
     if w is None:
         raise ModelLoadError("model_properties needs `weights` (state dict or checkpoint path) or `random_init`; "
@@ -89,9 +89,13 @@ class B200OpenCLIP:
         if props.get("std") is not None:
             arch = dict(arch, std=tuple(props["std"]))
         self.arch = arch
-        self.model = Encoder("clip", arch, _resolve_weights(props, arch, "clip"), device=_validate_device(self.device),
+        # "siglip" (model_registry.SIGLIP_MODELS): the engine's SigLIP runtime, whose GPU resize squashes images to
+        # S x S; otherwise open_clip CLIP, shortest side -> S + centre crop
+        kind = arch.get("kind", "clip")
+        self.model = Encoder(kind, arch, _resolve_weights(props, arch, kind), device=_validate_device(self.device),
                              max_batch=int(props.get("max_batch", 256)))
-        self.tokenizer = props.get("tokenizer") or self._default_tokenizer()
+        # SigLIP's SentencePiece tokenizer is not restated here: its text needs model_properties["tokenizer"]
+        self.tokenizer = props.get("tokenizer") or (None if kind == "siglip" else self._default_tokenizer())
 
     def _default_tokenizer(self):
         if self.model_properties.get("merges_file"):
@@ -210,6 +214,9 @@ class B200OpenCLIP:
 
     def _tokenize(self, sentence) -> np.ndarray:
         if self.tokenizer is None:
+            if self.arch.get("kind") == "siglip":
+                raise ModelLoadError("no SigLIP tokenizer available: supply model_properties['tokenizer'], a callable "
+                                     "returning [n, 64] token ids (SigLIP's SentencePiece vocabulary is not bundled)")
             raise ModelLoadError("no CLIP tokenizer available: supply model_properties['tokenizer'] "
                                  "(open_clip's BPE vocabulary is not bundled)")
         text = self.tokenizer(sentence if isinstance(sentence, list) else [sentence])

@@ -21,7 +21,22 @@ table of their own, MPNET_MODELS, behind `find_model` / `all_models`: they are M
 "mpnet"`), which the same `b200_hf` loader serves with the MPNet runtime and tokenizer.  Their shapes come from the
 upstream config.json files and cannot be re-read offline (verify): width 768, 12 layers, 12 heads, mlp 3072, vocabulary
 30527, max_position_embeddings 514 (positions start after pad_token_id 1, so at most 512 tokens), layer_norm_eps 1e-5
-(MPNetConfig's default is 1e-12), 32 relative-attention buckets with max distance 128, mean pooling."""
+(MPNetConfig's default is 1e-12), 32 relative-attention buckets with max distance 128, mean pooling.
+
+The SigLIP entries (model_registry.py:385-433,489-494) live in SIGLIP_MODELS (`arch["kind"] == "siglip"`), served by
+the same `b200_open_clip` loader.  Their shapes come from open_clip 2.24.0's model_configs/ViT-{B,L}-16-SigLIP*.json,
+`pretrained._slpcfg` and timm's `AttentionPoolLatent`, none of which can be re-read offline (verify):
+    ViT-B-16-SigLIP{,-256,-384,-512}/webli, Marqo/marqo-fashionSigLIP
+        vision: timm vit_base_patch16_siglip_*: width 768, 12 layers, 12 heads, mlp 3072, patch 16, image 224 / 256 /
+        384 / 512 (fashionSigLIP: 224); text: width 768, 12 layers, 12 heads, mlp 3072, ctx 64, vocab 32000; embed 768
+    ViT-L-16-SigLIP-256/webli, ViT-L-16-SigLIP-384/webli
+        vision: width 1024, 24 layers, 16 heads, mlp 4096, patch 16, image 256 / 384; text: width 1024, 24 layers,
+        16 heads, mlp 4096, ctx 64, vocab 32000; embed 1024
+    Both towers: pre-LN blocks, LayerNorm eps 1e-6, erf-GELU.  Vision: no class token, patch conv with bias, no ln_pre,
+    final LN over all tokens, then the MAP head (a learned latent query attends over the tokens, proj, x + MLP(LN(x)),
+    MLP 4 x width); no projection (timm_proj "none").  Text: no causal mask, ln_final, last position pooled, Linear with
+    bias (proj_bias).  Preprocessing (_slpcfg): mean = std = 0.5, bicubic squash resize to S x S without a crop.
+ViT-SO400M-14-SigLIP-384 (width 1152, 16 heads: head_dim 72) is not served."""
 from __future__ import annotations
 
 import copy
@@ -138,16 +153,52 @@ def _mpnet_models() -> Dict[str, dict]:
 
 MPNET_MODELS: Dict[str, dict] = _mpnet_models()
 
+SIGLIP_MEAN = (0.5, 0.5, 0.5)   # open_clip pretrained._slpcfg (verify)
+SIGLIP_STD = (0.5, 0.5, 0.5)
+
+
+def _siglip_arch(w: int, layers: int, heads: int, image_size: int) -> dict:
+    """SigLIP ViT-{B,L}-16 (module docstring, verify): both towers share width, depth and heads."""
+    return {
+        "kind": "siglip", "embed_dim": w, "act": "gelu", "mean": SIGLIP_MEAN, "std": SIGLIP_STD,
+        "resize_mode": "squash", "ln_eps": 1e-6,
+        "vision": {"width": w, "layers": layers, "heads": heads, "mlp": 4 * w, "patch": 16, "image_size": image_size,
+                   "map_mlp": 4 * w},
+        "text": {"width": w, "layers": layers, "heads": heads, "mlp": 4 * w, "ctx": 64, "vocab": 32000},
+    }
+
+
+def _siglip_models() -> Dict[str, dict]:
+    m: Dict[str, dict] = {}
+    shapes = [(f"ViT-B-16-SigLIP{suffix}", 768, 12, 12, size)
+              for suffix, size in (("", 224), ("-256", 256), ("-384", 384), ("-512", 512))]
+    shapes += [(f"ViT-L-16-SigLIP-{size}", 1024, 24, 16, size) for size in (256, 384)]
+    for model, w, layers, heads, size in shapes:
+        name = f"open_clip/{model}/webli"
+        m[name] = {"name": name, "dimensions": w, "note": f"open_clip model: {model}/webli", "type": TYPE_OPEN_CLIP,
+                   "pretrained": "webli", "arch": _siglip_arch(w, layers, heads, size)}
+    # model_registry.py:489-494: an hf-hub open_clip model, no `pretrained` tag
+    m["Marqo/marqo-fashionSigLIP"] = {"name": "hf-hub:Marqo/marqo-fashionSigLIP", "dimensions": 768,
+                                      "note": "Marqo's fashionSigLIP model", "type": TYPE_OPEN_CLIP,
+                                      "arch": _siglip_arch(768, 12, 12, 224)}
+    return m
+
+
+SIGLIP_MODELS: Dict[str, dict] = _siglip_models()
+
 
 def find_model(model_name: str) -> Optional[dict]:
     """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
-    entry = MODELS.get(model_name)
-    return entry if entry is not None else MPNET_MODELS.get(model_name)
+    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS):
+        entry = table.get(model_name)
+        if entry is not None:
+            return entry
+    return None
 
 
 def all_models() -> Dict[str, dict]:
     """Every served registry entry by name (a new dict over the same entries)."""
-    return {**MODELS, **MPNET_MODELS}
+    return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS}
 
 
 def get_model_properties(model_name: str) -> dict:

@@ -99,6 +99,63 @@ def random_clip_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     return sd
 
 
+def random_siglip_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
+    """Seeded random weights under open_clip's SigLIP state-dict names (timm trunk + open_clip text tower; arch: the
+    registry's SigLIP block)."""
+    g = _rng(seed)
+    sd: Dict[str, np.ndarray] = {}
+    v, t, E = arch.get("vision"), arch.get("text"), arch["embed_dim"]
+    if v:
+        w, p, mlp = v["width"], v["patch"], v["mlp"]
+        grid = v["image_size"] // p
+        rg = 1.0 / math.sqrt(2.0 * v["layers"])
+        tr = "visual.trunk."
+        sd[tr + "patch_embed.proj.weight"] = g.standard_normal((w, 3, p, p), dtype=np.float32) / np.float32(
+            math.sqrt(3 * p * p))
+        sd[tr + "patch_embed.proj.bias"] = _vec(g, w)
+        sd[tr + "pos_embed"] = 0.5 * g.standard_normal((1, grid * grid, w), dtype=np.float32)
+        for i in range(v["layers"]):
+            b = f"{tr}blocks.{i}."
+            sd[b + "norm1.weight"] = _vec(g, w, 0.1, 1.0)
+            sd[b + "norm1.bias"] = _vec(g, w)
+            sd[b + "attn.qkv.weight"] = _lin(g, 3 * w, w, 1.5)
+            sd[b + "attn.qkv.bias"] = _vec(g, 3 * w)
+            sd[b + "attn.proj.weight"] = _lin(g, w, w, rg)
+            sd[b + "attn.proj.bias"] = _vec(g, w)
+            sd[b + "norm2.weight"] = _vec(g, w, 0.1, 1.0)
+            sd[b + "norm2.bias"] = _vec(g, w)
+            sd[b + "mlp.fc1.weight"] = _lin(g, mlp, w)
+            sd[b + "mlp.fc1.bias"] = _vec(g, mlp)
+            sd[b + "mlp.fc2.weight"] = _lin(g, w, mlp, rg)
+            sd[b + "mlp.fc2.bias"] = _vec(g, w)
+        sd[tr + "norm.weight"] = _vec(g, w, 0.1, 1.0)
+        sd[tr + "norm.bias"] = _vec(g, w)
+        a, hm = tr + "attn_pool.", v.get("map_mlp", 4 * w)
+        sd[a + "latent"] = g.standard_normal((1, 1, w), dtype=np.float32)
+        sd[a + "q.weight"] = _lin(g, w, w, 1.5)
+        sd[a + "q.bias"] = _vec(g, w)
+        sd[a + "kv.weight"] = _lin(g, 2 * w, w, 1.5)
+        sd[a + "kv.bias"] = _vec(g, 2 * w)
+        sd[a + "proj.weight"] = _lin(g, w, w)
+        sd[a + "proj.bias"] = _vec(g, w)
+        sd[a + "norm.weight"] = _vec(g, w, 0.1, 1.0)
+        sd[a + "norm.bias"] = _vec(g, w)
+        sd[a + "mlp.fc1.weight"] = _lin(g, hm, w)
+        sd[a + "mlp.fc1.bias"] = _vec(g, hm)
+        sd[a + "mlp.fc2.weight"] = _lin(g, w, hm)
+        sd[a + "mlp.fc2.bias"] = _vec(g, w)
+    if t:
+        w = t["width"]
+        sd["text.token_embedding.weight"] = g.standard_normal((t["vocab"], w), dtype=np.float32)
+        sd["text.positional_embedding"] = 0.5 * g.standard_normal((t["ctx"], w), dtype=np.float32)
+        _clip_blocks(g, "text.", t, sd)
+        sd["text.ln_final.weight"] = _vec(g, w, 0.1, 1.0)
+        sd["text.ln_final.bias"] = _vec(g, w)
+        sd["text.text_projection.weight"] = _lin(g, E, w)
+        sd["text.text_projection.bias"] = _vec(g, E)
+    return sd
+
+
 def random_bert_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     g = _rng(seed)
     w, mlp = arch["width"], arch["mlp"]
