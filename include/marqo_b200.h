@@ -443,23 +443,19 @@ int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16,
  * src/marqo/tensor_search/add_docs.py:129-134 folded into the operand load. */
 int b200_debug_patch_embed(int device, const uint8_t* hwc, int n, int S, int patch, const float* conv_w, int N,
                            const float* mean3, const float* std3, const float* cls, const float* pos, float* out);
-/* softmax(q k^T / 8 + mask) v over packed qkv fp32 [B*S, 3*W] (rounded to bf16); mask: 0 none, 1 causal,
- * 2 key length (kv_len int32 [B]).  out fp32 [B*S, W]. */
+/* softmax(q k^T / sqrt(head_dim) + mask + bias) v over packed qkv fp32 [B*S, 3*W] (rounded to bf16), head_dim = W / H
+ * (32 or 64); mask: 0 none, 1 causal, 2 key length (kv_len int32 [B]).  rel_bias (NULL: none) is MPNet's
+ * relative-position bias, fp32 [H, 2*smax - 1] (natural-log domain, as it enters softmax): rel_bias[h, j - i + smax - 1]
+ * is added to the logit of query i and key j; head_dim 64, mask 2, S <= smax.  out fp32 [B*S, W]. */
 int b200_debug_attention(int device, const float* qkv, int B, int S, int W, int H, int mask, const int32_t* kv_len,
-                         float* out);
-/* The same with key-length masking (kv_len int32 [B]) and MPNet's relative-position bias: rel_bias fp32 [H, 2*smax - 1]
- * (natural-log domain, as it enters softmax) adds rel_bias[h, j - i + smax - 1] to the logit of query i and key j.
- * head_dim 64, S <= smax. */
-int b200_debug_attention_bias(int device, const float* qkv, int B, int S, int W, int H, const int32_t* kv_len,
-                              const float* rel_bias, int smax, float* out);
-/* Mean device time (ms) of `iters` launches of the biased attention on device-generated data (all keys kept). */
-int b200_debug_attention_bias_time(int device, int B, int S, int W, int H, int iters, float* out_ms);
+                         const float* rel_bias, int smax, float* out);
 /* MPNet's relative_position_bucket as the model builds its bias table: out[d + max_len - 1] = bucket of
  * key - query = d for |d| < max_len (host-only). */
 int b200_debug_relative_position_buckets(int num_buckets, int max_distance, int max_len, int32_t* out);
+/* Mean device time (ms, CUDA events) of `iters` back-to-back attention launches on device-generated data, every key
+ * kept; rel_bias != 0 adds a generated relative-position bias table with smax = S (the bias runs with mask 2). */
+int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, int rel_bias, int iters, float* out_ms);
 /* LayerNorm over rows of fp32 [rows, w]. */
-/* Mean device time (ms, CUDA events) of `iters` back-to-back attention launches on device-generated data. */
-int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, int iters, float* out_ms);
 int b200_debug_layernorm(int device, const float* x, const float* gamma, const float* beta, float eps, int rows, int w,
                          float* out);
 /* The JPEG decoder's arithmetic (shared __host__ __device__ code of the two kernels) run on the host: lets the CPU test

@@ -118,11 +118,10 @@ _SIGNATURES = {
     "b200_debug_index_scan_kernel": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int)]),
     "b200_debug_gemm_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "b200_debug_patch_embed": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P]),
-    "b200_debug_attention": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
-    "b200_debug_attention_bias": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, _P]),
-    "b200_debug_attention_bias_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float)]),
+    "b200_debug_attention": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, _P]),
     "b200_debug_relative_position_buckets": (C.c_int, [C.c_int, C.c_int, C.c_int, _P]),
-    "b200_debug_attention_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float)]),
+    "b200_debug_attention_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                            C.POINTER(C.c_float)]),
     "b200_debug_layernorm": (C.c_int, [C.c_int, _P, _P, _P, C.c_float, C.c_int, C.c_int, _P]),
     "b200_debug_resize": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "b200_debug_resize_squash": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),

@@ -1,15 +1,15 @@
 #include "attention.cuh"
+#include "ptx.cuh"
 
 namespace mb {
 namespace attention {
 
-constexpr int BQ = 64;        // query rows per CTA (4 warps x 16)
 constexpr int BKV = 64;       // keys per block
-constexpr int THREADS = 128;
+constexpr int THREADS = 128;  // 4 warps x 16 query rows
 template <int HD>
 constexpr int CH_LOG2 = HD == 64 ? 3 : 2;   // log2 of the HD / 8 16-byte chunks per tile row
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+using ptx::smem_u32;
 
 __device__ __forceinline__ void cp_async16(void* dst, const void* src, bool valid) {
     const int sz = valid ? 16 : 0;
@@ -27,15 +27,12 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], const void* 
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
                  : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(p)));
 }
-__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+// d[0..3] (+)= A B: one m16n8 accumulator, chunk d / 4 of a flat accumulator array
+__device__ __forceinline__ void mma_bf16(float* d, const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
                  "{%0, %1, %2, %3};"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t pack2(float lo, float hi) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<uint32_t*>(&v);
 }
 
 // tile: 64 rows x HD bf16 (HD / 8 16-byte chunks per row), chunks XOR-swizzled so that the 8 rows one ldmatrix reads
@@ -82,11 +79,8 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
     const __nv_bfloat16* kbase = seq + W + h * HD;
     const __nv_bfloat16* vbase = seq + 2 * W + h * HD;
 
-    int len = S;
-    if (MASK == MASK_KEYLEN) len = min(S, max(kv_len[b], 0));
-    int kend = len;
-    if (MASK == MASK_CAUSAL) kend = min(len, q0 + BQ);
-    const int nkb = (kend + BKV - 1) / BKV;
+    const KeyRange kr = key_range<MASK, BKV>(S, kv_len, b, q0);
+    const int len = kr.len, nkb = kr.nkb;
 
     load_tile<HD>(sQ, qbase, q0, S, ld);
     if (nkb > 0) {
@@ -94,20 +88,14 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
         load_tile<HD>(sV[0], vbase, 0, len, ld);
     }
     cp_async_commit();
-    if constexpr (BIAS) {   // band entry t: key - query = t - (q0 + BQ - 1); read after the first block's barrier
-        const float* row = rel_bias + (size_t)h * (2 * bias_smax - 1);
-        for (int t = threadIdx.x; t < nkb * BKV + BQ; t += THREADS) sBias[t] = rel_bias_band_value(row, bias_smax, q0, t);
-    }
+    if constexpr (BIAS)   // read after the first block's barrier
+        stage_bias_band<BKV, THREADS>(sBias, rel_bias, bias_smax, h, q0, nkb);
 
     uint32_t qf[HD / 16][4];
-    float o[HD / 8][4];
+    float o[HD / 2];
 #pragma unroll
-    for (int i = 0; i < HD / 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) o[i][j] = 0.f;
-    float row_max[2] = {-INFINITY, -INFINITY};
-    float row_sum[2] = {0.f, 0.f};
-    const int qrow[2] = {q0 + warp * 16 + g, q0 + warp * 16 + g + 8};
+    for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+    OnlineSoftmax<MASK, BIAS> sm{{q0 + warp * 16 + g, q0 + warp * 16 + g + 8}, q0, len, scale_log2e, sBias};
 
     for (int kb = 0; kb < nkb; ++kb) {
         const int buf = kb & 1;
@@ -128,11 +116,9 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
             }
         }
         // ---- S = Q K^T (16 x 64 per warp)
-        float s[8][4];
+        float s[BKV / 2];
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
+        for (int i = 0; i < BKV / 2; ++i) s[i] = 0.f;
 #pragma unroll
         for (int ks = 0; ks < HD / 16; ++ks) {
 #pragma unroll
@@ -140,76 +126,22 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
                 uint32_t kf[4];
                 const int mat = lane >> 3, r = lane & 7;
                 ldmatrix_x4(kf, tile_ptr<HD>(sK[buf], np * 16 + (mat >> 1) * 8 + r, ks * 2 + (mat & 1)));
-                mma_bf16(s[2 * np], qf[ks], kf[0], kf[1]);
-                mma_bf16(s[2 * np + 1], qf[ks], kf[2], kf[3]);
+                mma_bf16(s + 8 * np, qf[ks], kf[0], kf[1]);
+                mma_bf16(s + 8 * np + 4, qf[ks], kf[2], kf[3]);
             }
         }
-        // ---- mask, scale (log2 domain), online softmax
-        float mx[2] = {row_max[0], row_max[1]};
+        uint32_t pa[BKV / 16][4];
+        sm.update(s, o, pa, kb * BKV);
+        // ---- O += P V, 16 output columns at a time (fewer registers than k-step by k-step)
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
+        for (int dp = 0; dp < HD / 16; ++dp) {
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int key = kb * BKV + nt * 8 + 2 * t + (e & 1);
-                const int rr = e >> 1;
-                bool ok = key < len;
-                if (MASK == MASK_CAUSAL) ok = ok && key <= qrow[rr];
-                float v;
-                if constexpr (BIAS)
-                    v = ok ? s[nt][e] * scale_log2e + sBias[key - qrow[rr] + (q0 + BQ - 1)] : -INFINITY;
-                else
-                    v = ok ? s[nt][e] * scale_log2e : -INFINITY;
-                s[nt][e] = v;
-                mx[rr] = fmaxf(mx[rr], v);
-            }
-        }
-#pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-            mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 1));
-            mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 2));
-        }
-        float corr[2], msafe[2];
-#pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-            msafe[rr] = mx[rr] == -INFINITY ? 0.f : mx[rr];
-            corr[rr] = exp2f(row_max[rr] - msafe[rr]);  // row_max = -inf on the first block -> 0
-            row_max[rr] = mx[rr];
-            row_sum[rr] *= corr[rr];
-        }
-#pragma unroll
-        for (int nt = 0; nt < HD / 8; ++nt) {
-            o[nt][0] *= corr[0];
-            o[nt][1] *= corr[0];
-            o[nt][2] *= corr[1];
-            o[nt][3] *= corr[1];
-        }
-        float ps[2] = {0.f, 0.f};
-#pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float pv = exp2f(s[nt][e] - msafe[e >> 1]);
-                s[nt][e] = pv;
-                ps[e >> 1] += pv;
-            }
-        }
-        row_sum[0] += ps[0];
-        row_sum[1] += ps[1];
-        // ---- O += P V
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-            uint32_t pa[4];
-            pa[0] = pack2(s[2 * ks][0], s[2 * ks][1]);
-            pa[1] = pack2(s[2 * ks][2], s[2 * ks][3]);
-            pa[2] = pack2(s[2 * ks + 1][0], s[2 * ks + 1][1]);
-            pa[3] = pack2(s[2 * ks + 1][2], s[2 * ks + 1][3]);
-#pragma unroll
-            for (int dp = 0; dp < HD / 16; ++dp) {
+            for (int ks = 0; ks < BKV / 16; ++ks) {
                 uint32_t vf[4];
                 const int mat = lane >> 3, r = lane & 7;
                 ldmatrix_x4_trans(vf, tile_ptr<HD>(sV[buf], ks * 16 + (mat & 1) * 8 + r, dp * 2 + (mat >> 1)));
-                mma_bf16(o[2 * dp], pa, vf[0], vf[1]);
-                mma_bf16(o[2 * dp + 1], pa, vf[2], vf[3]);
+                mma_bf16(o + 8 * dp, pa[ks], vf[0], vf[1]);
+                mma_bf16(o + 8 * dp + 4, pa[ks], vf[2], vf[3]);
             }
         }
         __syncthreads();
@@ -218,18 +150,16 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
         cp_async_wait<0>();
         __syncthreads();
     }
-    // ---- finalise: O /= rowsum (quad-reduced), stage through sQ (this warp's 16 rows), 16-byte coalesced stores
-#pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-        row_sum[rr] += __shfl_xor_sync(0xffffffffu, row_sum[rr], 1);
-        row_sum[rr] += __shfl_xor_sync(0xffffffffu, row_sum[rr], 2);
-    }
-    const float inv[2] = {row_sum[0] > 0.f ? 1.f / row_sum[0] : 0.f, row_sum[1] > 0.f ? 1.f / row_sum[1] : 0.f};
+    // ---- finalise: O /= row sum, stage through sQ (this warp's 16 rows), 16-byte coalesced stores
+    float inv[2];
+    sm.finish(inv);
 #pragma unroll
     for (int nt = 0; nt < HD / 8; ++nt) {
         const int r0 = warp * 16 + g;
-        *reinterpret_cast<uint32_t*>(tile_ptr<HD>(sQ, r0, nt) + 2 * t) = pack2(o[nt][0] * inv[0], o[nt][1] * inv[0]);
-        *reinterpret_cast<uint32_t*>(tile_ptr<HD>(sQ, r0 + 8, nt) + 2 * t) = pack2(o[nt][2] * inv[1], o[nt][3] * inv[1]);
+        *reinterpret_cast<uint32_t*>(tile_ptr<HD>(sQ, r0, nt) + 2 * t) =
+            pack_bf16x2(o[4 * nt] * inv[0], o[4 * nt + 1] * inv[0]);
+        *reinterpret_cast<uint32_t*>(tile_ptr<HD>(sQ, r0 + 8, nt) + 2 * t) =
+            pack_bf16x2(o[4 * nt + 2] * inv[1], o[4 * nt + 3] * inv[1]);
     }
     __syncwarp();
 #pragma unroll
@@ -244,52 +174,32 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
     }
 }
 
-template <int HD>
-void launch_hd(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask, const int32_t* kv_len,
-               cudaStream_t stream) {
-    const dim3 grid((S + BQ - 1) / BQ, H, B);
-    const float scale_log2e = head_scale_log2e(HD);
-    switch (mask) {
-        case MASK_NONE:
-            attention_kernel<HD, MASK_NONE, false>
-                <<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e, nullptr, 0);
-            break;
-        case MASK_CAUSAL:
-            attention_kernel<HD, MASK_CAUSAL, false>
-                <<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e, nullptr, 0);
-            break;
-        case MASK_KEYLEN:
-            if (!kv_len) fail(B200_ERR_INTERNAL, "attention: kv_len required for key-length masking");
-            attention_kernel<HD, MASK_KEYLEN, false>
-                <<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, scale_log2e, nullptr, 0);
-            break;
-        default:
-            fail(B200_ERR_INTERNAL, "attention: unknown mask mode %d", mask);
-    }
-}
-
 int launch(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask, const int32_t* kv_len,
-           cudaStream_t stream) {
+           const RelBias& bias, cudaStream_t stream) {
     if (B <= 0 || S <= 0) return 0;
-    if (S >= 128) return launch_wgmma(qkv, out, B, S, W, H, mask, kv_len, stream);
-    if (head_dim(W, H) == 64)
-        launch_hd<64>(qkv, out, B, S, W, H, mask, kv_len, stream);
-    else
-        launch_hd<32>(qkv, out, B, S, W, H, mask, kv_len, stream);
-    MB_CUDA(cudaGetLastError());
-    return 1;
-}
-
-int launch_rel_bias(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, const int32_t* kv_len,
-                    const RelBias& bias, cudaStream_t stream) {
-    if (B <= 0 || S <= 0) return 0;
-    if (head_dim(W, H) != 64) fail(B200_ERR_UNSUPPORTED, "attention: the relative bias is built for head_dim 64 only");
-    if (!kv_len || !bias.table) fail(B200_ERR_INTERNAL, "attention: the relative bias needs kv_len and a table");
-    if (S > bias.smax) fail(B200_ERR_INVALID_ARG, "attention: sequence %d is longer than the bias table (%d)", S, bias.smax);
-    if (S >= 128) return launch_wgmma_rel_bias(qkv, out, B, S, W, H, kv_len, bias, stream);
-    const dim3 grid((S + BQ - 1) / BQ, H, B);
-    attention_kernel<64, MASK_KEYLEN, true>
-        <<<grid, THREADS, 0, stream>>>(qkv, out, S, W, kv_len, head_scale_log2e(64), bias.table, bias.smax);
+    const int hd = head_dim(W, H);
+    if (bias.table) {
+        if (hd != 64 || mask != MASK_KEYLEN)
+            fail(B200_ERR_UNSUPPORTED, "attention: the relative bias is built for head_dim 64 with the key-length mask");
+        if (S > bias.smax)
+            fail(B200_ERR_INVALID_ARG, "attention: sequence %d is longer than the bias table (%d)", S, bias.smax);
+        if (S > MAX_BIAS_S)
+            fail(B200_ERR_UNSUPPORTED, "attention: the relative bias supports sequences of at most %d", MAX_BIAS_S);
+    }
+    if (B > 65535) fail(B200_ERR_UNSUPPORTED, "attention: batch %d is too large", B);
+    if (mask != MASK_NONE && mask != MASK_CAUSAL && mask != MASK_KEYLEN)
+        fail(B200_ERR_INTERNAL, "attention: unknown mask mode %d", mask);
+    if (mask == MASK_KEYLEN && !kv_len) fail(B200_ERR_INTERNAL, "attention: kv_len required for key-length masking");
+    if (S >= 128) {
+        launch_wgmma_kernel(qkv, out, B, S, W, H, hd, mask, kv_len, bias, stream);
+    } else {
+        dispatch(hd, mask, bias.table != nullptr, [&](auto d, auto m, auto with_bias) {
+            constexpr int HD = decltype(d)::value, MASK = decltype(m)::value;
+            constexpr bool BIAS = decltype(with_bias)::value;
+            attention_kernel<HD, MASK, BIAS><<<dim3((S + BQ - 1) / BQ, H, B), THREADS, 0, stream>>>(
+                qkv, out, S, W, kv_len, head_scale_log2e(HD), bias.table, bias.smax);
+        });
+    }
     MB_CUDA(cudaGetLastError());
     return 1;
 }

@@ -1,6 +1,6 @@
-// Host-side helpers shared by every translation unit of libmarqo_b200.so:
+// Helpers shared by every translation unit of libmarqo_b200.so:
 // status codes, thread-local error text, CUDA error checks, owners of device memory and CUDA handles,
-// TMA tensor-map encoding.
+// TMA tensor-map encoding, and the bf16x2 pack of the kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -160,5 +160,11 @@ CUtensorMap make_tmap_2d(const void* base, CUtensorMapDataType dtype, uint32_t e
 int sm_count(int device);
 
 inline size_t round_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// (lo, hi) rounded to bf16 (round to nearest even) in one 32-bit word, lo in the low half
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+    return *reinterpret_cast<uint32_t*>(&v);
+}
 
 }  // namespace mb

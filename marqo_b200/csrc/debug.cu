@@ -270,10 +270,11 @@ int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16,
 }
 
 int b200_debug_attention(int device, const float* qkv, int B, int S, int W, int H, int mask, const int32_t* kv_len,
-                         float* out) {
+                         const float* rel_bias, int smax, float* out) {
     return guarded([&] {
         MB_CHECK_ARG(qkv && out, "NULL buffer");
         MB_CHECK_ARG(B > 0 && S > 0 && W > 0 && H > 0, "B, S, W, H must be positive");
+        MB_CHECK_ARG(!rel_bias || smax > 0, "smax must be positive");
         require_device(device);
         DeviceGuard g(device);
         Scratch sc;
@@ -282,7 +283,15 @@ int b200_debug_attention(int device, const float* qkv, int B, int S, int W, int 
         __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>(M * W);
         float* dOut = sc.alloc<float>(M * W);
         const int32_t* dlen = kv_len ? sc.upload(kv_len, (size_t)B) : nullptr;
-        attention::launch(dq, dO, B, S, W, H, mask, dlen, sc.s);
+        attention::RelBias bias;
+        if (rel_bias) {
+            const size_t span = (size_t)H * (2 * smax - 1);
+            std::vector<float> scaled(rel_bias, rel_bias + span);   // the kernels add it in the log2 domain
+            for (float& v : scaled) v *= 1.4426950408889634f;
+            bias.table = sc.upload(scaled.data(), span);
+            bias.smax = smax;
+        }
+        attention::launch(dq, dO, B, S, W, H, mask, dlen, bias, sc.s);
         const long long n = (long long)M * W;
         bf16_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, sc.s>>>(dO, dOut, n);
         MB_CUDA(cudaGetLastError());
@@ -291,65 +300,7 @@ int b200_debug_attention(int device, const float* qkv, int B, int S, int W, int 
     });
 }
 
-int b200_debug_attention_bias(int device, const float* qkv, int B, int S, int W, int H, const int32_t* kv_len,
-                              const float* rel_bias, int smax, float* out) {
-    return guarded([&] {
-        MB_CHECK_ARG(qkv && kv_len && rel_bias && out, "NULL buffer");
-        MB_CHECK_ARG(B > 0 && S > 0 && W > 0 && H > 0 && smax > 0, "B, S, W, H, smax must be positive");
-        require_device(device);
-        DeviceGuard g(device);
-        Scratch sc;
-        const size_t M = (size_t)B * S, span = (size_t)H * (2 * smax - 1);
-        std::vector<float> scaled(rel_bias, rel_bias + span);   // the kernels add it in the log2 domain
-        for (float& v : scaled) v *= 1.4426950408889634f;
-        __nv_bfloat16* dq = sc.upload_bf16(qkv, M * 3 * W);
-        __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>(M * W);
-        float* dOut = sc.alloc<float>(M * W);
-        attention::RelBias bias;
-        bias.table = sc.upload(scaled.data(), span);
-        bias.smax = smax;
-        attention::launch_rel_bias(dq, dO, B, S, W, H, sc.upload(kv_len, (size_t)B), bias, sc.s);
-        const long long n = (long long)M * W;
-        bf16_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, sc.s>>>(dO, dOut, n);
-        MB_CUDA(cudaGetLastError());
-        MB_CUDA(cudaStreamSynchronize(sc.s));
-        MB_CUDA(cudaMemcpy(out, dOut, M * W * 4, cudaMemcpyDeviceToHost));
-    });
-}
-
-int b200_debug_attention_bias_time(int device, int B, int S, int W, int H, int iters, float* out_ms) {
-    return guarded([&] {
-        MB_CHECK_ARG(out_ms != nullptr, "NULL buffer");
-        MB_CHECK_ARG(B > 0 && S > 0 && W > 0 && H > 0 && iters > 0, "B, S, W, H, iters must be positive");
-        require_device(device);
-        DeviceGuard g(device);
-        Scratch sc;
-        const size_t M = (size_t)B * S;
-        __nv_bfloat16* dq = sc.alloc<__nv_bfloat16>(M * 3 * W);
-        __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>(M * W);
-        const long long n = (long long)(M * 3 * W), nb = (long long)H * (2 * S - 1);
-        fill_bf16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, sc.s>>>(dq, n, 12345u);
-        attention::RelBias bias;
-        float* table = sc.alloc<float>((size_t)nb);
-        fill_f32_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, sc.s>>>(table, nb, 99u);
-        bias.table = table;
-        bias.smax = S;
-        MB_CUDA(cudaGetLastError());
-        std::vector<int32_t> lens((size_t)B, S);
-        const int32_t* dlen = sc.upload(lens.data(), (size_t)B);
-        UniqueEvent e0 = make_event(), e1 = make_event();
-        for (int i = 0; i < 3; ++i) attention::launch_rel_bias(dq, dO, B, S, W, H, dlen, bias, sc.s);   // warm-up
-        MB_CUDA(cudaEventRecord(e0.get(), sc.s));
-        for (int i = 0; i < iters; ++i) attention::launch_rel_bias(dq, dO, B, S, W, H, dlen, bias, sc.s);
-        MB_CUDA(cudaEventRecord(e1.get(), sc.s));
-        MB_CUDA(cudaStreamSynchronize(sc.s));
-        float ms = 0.f;
-        MB_CUDA(cudaEventElapsedTime(&ms, e0.get(), e1.get()));
-        *out_ms = ms / (float)iters;
-    });
-}
-
-int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, int iters, float* out_ms) {
+int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, int rel_bias, int iters, float* out_ms) {
     return guarded([&] {
         MB_CHECK_ARG(out_ms != nullptr, "NULL buffer");
         MB_CHECK_ARG(B > 0 && S > 0 && W > 0 && H > 0 && iters > 0, "B, S, W, H, iters must be positive");
@@ -361,13 +312,21 @@ int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, 
         __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>(M * W);
         const long long n = (long long)(M * 3 * W);
         fill_bf16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, sc.s>>>(dq, n, 12345u);
+        attention::RelBias bias;
+        if (rel_bias) {
+            const long long nb = (long long)H * (2 * S - 1);
+            float* table = sc.alloc<float>((size_t)nb);
+            fill_f32_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, sc.s>>>(table, nb, 99u);
+            bias.table = table;
+            bias.smax = S;
+        }
         MB_CUDA(cudaGetLastError());
         std::vector<int32_t> lens((size_t)B, S);
         const int32_t* dlen = mask == attention::MASK_KEYLEN ? sc.upload(lens.data(), (size_t)B) : nullptr;
         UniqueEvent e0 = make_event(), e1 = make_event();
-        for (int i = 0; i < 3; ++i) attention::launch(dq, dO, B, S, W, H, mask, dlen, sc.s);   // warm-up
+        for (int i = 0; i < 3; ++i) attention::launch(dq, dO, B, S, W, H, mask, dlen, bias, sc.s);   // warm-up
         MB_CUDA(cudaEventRecord(e0.get(), sc.s));
-        for (int i = 0; i < iters; ++i) attention::launch(dq, dO, B, S, W, H, mask, dlen, sc.s);
+        for (int i = 0; i < iters; ++i) attention::launch(dq, dO, B, S, W, H, mask, dlen, bias, sc.s);
         MB_CUDA(cudaEventRecord(e1.get(), sc.s));
         MB_CUDA(cudaStreamSynchronize(sc.s));
         float ms = 0.f;

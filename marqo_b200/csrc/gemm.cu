@@ -149,11 +149,6 @@ __device__ __forceinline__ float quick_gelu(float x) {   // x * sigmoid(1.702 x)
     return x / (1.0f + ex2_approx(-1.702f * 1.44269504f * x));
 }
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<uint32_t*>(&v);
-}
-
 // Offset of bf16 element (row, k) inside a 128-row x 64-column K-major stage with the 128-byte swizzle TMA applies:
 // 16-byte unit u of row r lands at unit u ^ (r & 7).
 __device__ __forceinline__ uint32_t sw128_offset(int row, int unit) {

@@ -14,11 +14,6 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-    return *reinterpret_cast<uint32_t*>(&v);
-}
-
 // ------------------------------------------------------------------------------------------------ LayerNorm
 // One warp per row, the whole row lives in registers (two-pass mean / variance like torch's CPU kernel).
 constexpr int LN_MAX_V4 = 8;  // w <= 1024

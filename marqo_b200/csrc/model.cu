@@ -358,10 +358,7 @@ void linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, con
 void attend(b200_model* m, Counter& c, int B, int S, int w, int heads, int mask_mode, const int32_t* kv_len,
             const attention::RelBias& bias = {}) {
     ProfScope ps(m, 1);
-    if (bias.table)
-        c.n += attention::launch_rel_bias(m->qkv.get(), m->o.get(), B, S, w, heads, kv_len, bias, m->stream);
-    else
-        c.n += attention::launch(m->qkv.get(), m->o.get(), B, S, w, heads, mask_mode, kv_len, m->stream);
+    c.n += attention::launch(m->qkv.get(), m->o.get(), B, S, w, heads, mask_mode, kv_len, bias, m->stream);
 }
 
 // Pre-LN residual blocks (open_clip ResidualAttentionBlock).  x (fp32) is the residual stream, h (bf16) the LayerNorm

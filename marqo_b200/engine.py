@@ -575,23 +575,24 @@ def debug_attention(qkv, B: int, S: int, W: int, H: int, mask: int = 0, kv_len=N
     q = _as(qkv, np.float32)
     kl = None if kv_len is None else _as(kv_len, np.int32)
     out = np.empty((B * S, W), np.float32)
-    if rel_bias is None:
-        N.check(N.load().b200_debug_attention(device, _ptr(q), B, S, W, H, mask, _ptr(kl), _ptr(out)))
-        return out
-    rb = _as(rel_bias, np.float32)
-    if mask != 2 or kl is None:
-        raise ValueError("the relative bias runs with the key-length mask (mask=2, kv_len)")
-    if rb.ndim != 2 or rb.shape[0] != H or rb.shape[1] % 2 != 1:
-        raise ValueError(f"expected rel_bias [{H}, 2 * smax - 1], got {rb.shape}")
-    N.check(N.load().b200_debug_attention_bias(device, _ptr(q), B, S, W, H, _ptr(kl), _ptr(rb), (rb.shape[1] + 1) // 2,
-                                               _ptr(out)))
+    rb, smax = None, 0
+    if rel_bias is not None:
+        rb = _as(rel_bias, np.float32)
+        if mask != 2 or kl is None:
+            raise ValueError("the relative bias runs with the key-length mask (mask=2, kv_len)")
+        if rb.ndim != 2 or rb.shape[0] != H or rb.shape[1] % 2 != 1:
+            raise ValueError(f"expected rel_bias [{H}, 2 * smax - 1], got {rb.shape}")
+        smax = (rb.shape[1] + 1) // 2
+    N.check(N.load().b200_debug_attention(device, _ptr(q), B, S, W, H, mask, _ptr(kl), _ptr(rb), smax, _ptr(out)))
     return out
 
 
-def debug_attention_bias_time(B: int, S: int, W: int, H: int, iters: int = 20, device: int = 0) -> float:
-    """Mean device time (ms) of the biased attention launch on generated data."""
+def debug_attention_time(B: int, S: int, W: int, H: int, mask: int = 0, rel_bias: bool = False, iters: int = 20,
+                         device: int = 0) -> float:
+    """Mean device time (ms) of the attention launch on generated data, every key kept; rel_bias adds a generated
+    relative-position bias (with mask=2)."""
     ms = C.c_float(0)
-    N.check(N.load().b200_debug_attention_bias_time(device, B, S, W, H, iters, C.byref(ms)))
+    N.check(N.load().b200_debug_attention_time(device, B, S, W, H, mask, int(rel_bias), iters, C.byref(ms)))
     return ms.value
 
 

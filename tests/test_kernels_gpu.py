@@ -166,6 +166,17 @@ def test_attention_peaked_scores(gpu_required, B, S, H, mask):
     torch.testing.assert_close(got, ref, rtol=3e-2, atol=3e-2)
 
 
+def test_attention_refuses_more_than_65535_sequences(gpu_required):
+    """The batch is the grid's z dimension: B > 65535 is refused before any launch, on the short-sequence path too."""
+    from marqo_b200._native import ERR_UNSUPPORTED, NativeError
+    from marqo_b200.engine import debug_attention
+    B, S, H = 65536, 1, 1
+    qkv = np.zeros((B * S, 3 * H * 64), np.float32)
+    with pytest.raises(NativeError) as ei:
+        debug_attention(qkv, B, S, H * 64, H, 0)
+    assert ei.value.code == ERR_UNSUPPORTED
+
+
 @pytest.mark.parametrize("rows,w,eps", [(5, 128, 1e-5), (77, 512, 1e-5), (1000, 768, 1e-12), (33, 1024, 1e-5)])
 def test_layernorm_matches_torch(gpu_required, rows, w, eps):
     from marqo_b200.engine import debug_layernorm

@@ -1,14 +1,13 @@
 """Dev probe for the MPNet embedders (hf/all-mpnet-base-*), not a bench line.  Needs a GPU; prints JSON lines.
 
   1. attention kernel alone at the MPNet-base shape (12 heads of 64, key-length mask, every key valid), with and without
-     the relative-position bias (b200_debug_attention_bias_time / b200_debug_attention_time);
+     the relative-position bias (b200_debug_attention_time);
   2. device-resident forward (ids on the device, mean pooling + L2 normalise, seeded weights) vs transformers'
      MPNetModel built from the same config and weights, in fp32 (what the reference runs on CUDA) and in bf16.
 Times are host clocks around `iters` calls that end in a device synchronise, after `warmup` calls of the same shape.
 
     python tools/mpnet_probe.py [iters]
 """
-import ctypes as C
 import json
 import subprocess
 import sys
@@ -18,7 +17,7 @@ import torch
 
 sys.path.insert(0, ".")
 from marqo_b200 import _native as N, model_registry as R, weights as Wt  # noqa: E402
-from marqo_b200.engine import Encoder, debug_attention_bias_time  # noqa: E402
+from marqo_b200.engine import Encoder, debug_attention_time  # noqa: E402
 
 ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 50
 WARMUP = 5
@@ -45,11 +44,10 @@ def _wall(fn, iters):
 
 def attention(B, S, H=12, hd=64):
     W = H * hd
-    ms = C.c_float(0)
-    N.check(N.load().b200_debug_attention_time(0, B, S, W, H, 2, ITERS, C.byref(ms)))
-    biased = debug_attention_bias_time(B, S, W, H, ITERS)
-    return {"probe": "attention", "B": B, "S": S, "H": H, "head_dim": hd, "no_bias_us": ms.value * 1e3,
-            "rel_bias_us": biased * 1e3, "bias_overhead": biased / ms.value - 1.0}
+    plain = debug_attention_time(B, S, W, H, mask=2, iters=ITERS)
+    biased = debug_attention_time(B, S, W, H, mask=2, rel_bias=True, iters=ITERS)
+    return {"probe": "attention", "B": B, "S": S, "H": H, "head_dim": hd, "no_bias_us": plain * 1e3,
+            "rel_bias_us": biased * 1e3, "bias_overhead": biased / plain - 1.0}
 
 
 def forward(B, S):

@@ -1,6 +1,6 @@
 """Dev probe for the 384-wide BERT embedders (head_dim 32), not a bench line.  Needs a GPU; prints JSON lines.
 
-  1. attention kernel alone (b200_debug_attention_time, key-length mask, every key valid) vs
+  1. attention kernel alone (debug_attention_time, key-length mask, every key valid) vs
      torch.nn.functional.scaled_dot_product_attention in bf16 on q / k / v already split into [B, H, S, 32];
   2. device-resident forward (ids on the device, mean pooling + L2 normalise, seeded weights) vs HF BertModel built
      from the same config, in fp32 (what the reference runs on CUDA) and in bf16, both with transformers' SDPA attention.
@@ -8,7 +8,6 @@ Times are host clocks around `iters` calls that end in a device synchronise, aft
 
     python tools/small_bert_probe.py [iters]
 """
-import ctypes as C
 import json
 import subprocess
 import sys
@@ -18,7 +17,7 @@ import torch
 
 sys.path.insert(0, ".")
 from marqo_b200 import _native as N, model_registry as R, weights as Wt  # noqa: E402
-from marqo_b200.engine import Encoder  # noqa: E402
+from marqo_b200.engine import Encoder, debug_attention_time  # noqa: E402
 
 ITERS = int(sys.argv[1]) if len(sys.argv) > 1 else 50
 WARMUP = 5
@@ -44,13 +43,12 @@ def _wall(fn, iters):
 
 def attention(B, S, H=12, hd=32):
     W = H * hd
-    ms = C.c_float(0)
-    N.check(N.load().b200_debug_attention_time(0, B, S, W, H, 2, ITERS, C.byref(ms)))
+    ms = debug_attention_time(B, S, W, H, mask=2, iters=ITERS)
     q, k, v = (torch.randn(B, H, S, hd, device="cuda", dtype=torch.bfloat16) for _ in range(3))
     sdpa = _wall(lambda: torch.nn.functional.scaled_dot_product_attention(q, k, v), ITERS)
     flops = 4.0 * B * H * S * S * hd
-    return {"probe": "attention", "B": B, "S": S, "H": H, "head_dim": hd, "engine_us": ms.value * 1e3,
-            "sdpa_bf16_us": sdpa * 1e3, "engine_TFLOPs": flops / ms.value / 1e9, "speedup_vs_sdpa": sdpa / ms.value}
+    return {"probe": "attention", "B": B, "S": S, "H": H, "head_dim": hd, "engine_us": ms * 1e3,
+            "sdpa_bf16_us": sdpa * 1e3, "engine_TFLOPs": flops / ms / 1e9, "speedup_vs_sdpa": sdpa / ms}
 
 
 def forward(name, B, S):
