@@ -238,7 +238,8 @@ enum b200_arch {
     B200_ARCH_CLIP = 0, /* open_clip CLIP: vision tower + text tower */
     B200_ARCH_BERT = 1, /* HF BertModel + pooling */
     B200_ARCH_MPNET = 2, /* HF MPNetModel + pooling: BERT layers with a relative-position bias in the attention logits */
-    B200_ARCH_SIGLIP = 3 /* open_clip SigLIP: class-token-free ViT with a MAP pooling head + bidirectional text tower */
+    B200_ARCH_SIGLIP = 3, /* open_clip SigLIP: class-token-free ViT with a MAP pooling head + bidirectional text tower */
+    B200_ARCH_XLMR = 4    /* HF XLMRobertaModel + pooling: BERT layers, RoBERTa position ids, one token-type row */
 };
 enum b200_act { B200_ACT_GELU = 0, B200_ACT_QUICKGELU = 1 };
 enum b200_pool { B200_POOL_MEAN = 0, B200_POOL_CLS = 1 };
@@ -264,12 +265,14 @@ typedef struct b200_model_desc {
     float image_mean[3]; /* Normalize() constants, src/marqo/s2_inference/clip_utils.py:32-33 */
     float image_std[3];
     b200_tower_desc vision; /* CLIP only */
-    b200_tower_desc text;   /* CLIP text tower, or the BERT / MPNet encoder (MPNet: ctx = longest sequence, which is
-                               max_position_embeddings - pad_id - 1 because positions start after the pad id) */
-    /* MPNet (MPNetConfig) and SigLIP: */
-    float layer_norm_eps;     /* 1e-5 for the sentence-transformers MPNet checkpoints, 1e-6 for SigLIP */
-    /* MPNet only: */
+    b200_tower_desc text;   /* CLIP text tower, or the BERT / MPNet / XLM-R encoder (MPNet, XLM-R: ctx = longest
+                               sequence, which is max_position_embeddings - pad_id - 1 because positions start after
+                               the pad id) */
+    /* MPNet (MPNetConfig), XLM-R and SigLIP: */
+    float layer_norm_eps;     /* 1e-5 for the sentence-transformers MPNet checkpoints and XLM-R, 1e-6 for SigLIP */
+    /* MPNet and XLM-R: */
     int32_t pad_id;           /* pad_token_id (1): the position ids count from it */
+    /* MPNet only: */
     int32_t rel_buckets;      /* relative_attention_num_buckets (32) */
     int32_t rel_max_distance; /* max_distance of relative_position_bucket (128) */
 } b200_model_desc;
@@ -284,6 +287,9 @@ int b200_model_destroy(b200_model* m);
  * visual.trunk.attn_pool.{latent [1, 1, W], q, kv, proj, norm, mlp.fc1, mlp.fc2}.*, text.token_embedding.weight,
  * text.positional_embedding, text.transformer.resblocks.{i}.* (the CLIP block names), text.ln_final.*,
  * text.text_projection.{weight [E, W], bias}. */
+/* XLM-R: HF XLMRobertaModel names, as BERT's: embeddings.word_embeddings.weight [vocab, W],
+ * embeddings.position_embeddings.weight [ctx + pad_id + 1, W], embeddings.token_type_embeddings.weight [1, W],
+ * embeddings.LayerNorm.*, encoder.layer.{i}.* (a "roberta." prefix is dropped). */
 int b200_model_load_tensor(b200_model* m, const char* name, const float* data, int64_t numel);
 /* Verifies every required parameter has been supplied, builds derived buffers. */
 int b200_model_finalize(b200_model* m);
@@ -307,7 +313,8 @@ int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int nor
  * text projection; attn_mask is ignored (the tokenizer pads every row to the context length).
  * BERT: attn_mask int32 [n, seq] (1 = token, 0 = pad; NULL = all ones), token_type 0.
  * MPNet: as BERT, without token types; position ids follow the ids (HF create_position_ids_from_input_ids), the key
- * mask follows attn_mask.  seq > text.ctx is refused with B200_ERR_INVALID_ARG. */
+ * mask follows attn_mask.  XLM-R: as MPNet, plus token_type_embeddings row 0, LayerNorm eps layer_norm_eps.
+ * seq > text.ctx is refused with B200_ERR_INVALID_ARG. */
 int b200_model_encode_tokens(b200_model* m, const int32_t* ids, const int32_t* attn_mask, int n, int seq,
                              int normalize, float* out);
 /* Device-resident variants: inputs/outputs are device pointers on the model's device,
@@ -356,10 +363,17 @@ int b200_tokenizer_create_wordpiece_ex(const char* vocab_utf8, size_t nbytes, in
  * bpe_simple_vocab_16e6.txt (line 1 is a header; at most 49152-256-2 merges are used).  ftfy.fix_text is not
  * restated: text that ftfy would repair (mojibake) tokenises as written. */
 int b200_tokenizer_create_clip_bpe(const char* merges_utf8, size_t nbytes, b200_tokenizer** out);
+/* SentencePiece Unigram with XLM-RoBERTa's ids — XLMRobertaTokenizer on sentencepiece.bpe.model.  model_bytes: the
+ * serialized ModelProto (model_type UNIGRAM; no user-defined pieces).  Normalisation: the precompiled charsmap (longest
+ * match, the character itself when nothing matches), remove_extra_whitespaces, add_dummy_prefix, spaces -> U+2581;
+ * segmentation: Viterbi over the pieces, an unknown character scores min_score - 10 and adjacent unknowns merge.
+ * Ids: <s> 0, <pad> 1, </s> 2, <unk> 3, any other piece its SentencePiece id + 1 (fairseq's offset); vocab_size is
+ * pieces + 2 (<pad> and <mask>).  Special-token strings in the text are ordinary text. */
+int b200_tokenizer_create_unigram(const char* model_bytes, size_t nbytes, b200_tokenizer** out);
 int b200_tokenizer_destroy(b200_tokenizer* t);
 int b200_tokenizer_vocab_size(b200_tokenizer* t, int* out_size);
 /* Encode n UTF-8 strings (texts[i], text_bytes[i] bytes; invalid sequences decode as U+FFFD).
- * WordPiece: "[CLS] ids [SEP]", truncated to max_length, every row padded with [PAD] to the LONGEST row of this call
+ * WordPiece: "[CLS] ids [SEP]" (Unigram: "<s> ids </s>", padded with <pad>), truncated to max_length, every row padded with [PAD] to the LONGEST row of this call
  * (padding=True): *out_seq_len = that length <= max_length.  CLIP BPE: "<start_of_text> ids <end_of_text>", truncated
  * to max_length (= context_length) with the last id forced to <end_of_text>, zero padded: *out_seq_len = max_length.
  * out_ids / out_mask (mask may be NULL): caller buffers of n * max_length int32; rows are written back to back with

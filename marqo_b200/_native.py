@@ -14,7 +14,7 @@ _lock = threading.Lock()
 OK, ERR_INVALID_ARG, ERR_NO_DEVICE, ERR_CUDA, ERR_OOM, ERR_UNSUPPORTED, ERR_INTERNAL, ERR_MISSING_WEIGHT = range(8)
 
 METRIC_PRENORMALIZED_ANGULAR, METRIC_ANGULAR, METRIC_DOTPRODUCT, METRIC_EUCLIDEAN = range(4)
-ARCH_CLIP, ARCH_BERT, ARCH_MPNET, ARCH_SIGLIP = 0, 1, 2, 3
+ARCH_CLIP, ARCH_BERT, ARCH_MPNET, ARCH_SIGLIP, ARCH_XLMR = 0, 1, 2, 3, 4
 ACT_GELU, ACT_QUICKGELU = 0, 1
 POOL_MEAN, POOL_CLS = 0, 1
 GEMM_128x128, GEMM_PERSISTENT = 0, 1   # the GEMM kernel b200_debug_gemm_into reports
@@ -134,6 +134,7 @@ _SIGNATURES = {
     "b200_tokenizer_create_wordpiece_ex": (C.c_int, [C.c_char_p, C.c_size_t, C.c_int, C.c_char_p, C.c_char_p, C.c_char_p,
                                                      C.c_char_p, _P, C.c_int, C.POINTER(_P)]),
     "b200_tokenizer_create_clip_bpe": (C.c_int, [C.c_char_p, C.c_size_t, C.POINTER(_P)]),
+    "b200_tokenizer_create_unigram": (C.c_int, [C.c_char_p, C.c_size_t, C.POINTER(_P)]),
     "b200_tokenizer_destroy": (C.c_int, [_P]),
     "b200_tokenizer_vocab_size": (C.c_int, [_P, C.POINTER(C.c_int)]),
     "b200_tokenizer_encode": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, C.POINTER(C.c_int)]),

@@ -238,12 +238,14 @@ void bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, c
     MB_CUDA(cudaGetLastError());
 }
 
-__global__ void __launch_bounds__(256) mpnet_embed_ln_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ mask,
-                                                             const float* __restrict__ word, const float* __restrict__ pos,
-                                                             const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                             float eps, int n, int S, int w, int vocab, int pad,
-                                                             float* __restrict__ x, __nv_bfloat16* __restrict__ h,
-                                                             int32_t* __restrict__ kv_len) {
+// TYPE_ROW: XLM-R adds token_type_embeddings row 0 (HF: (inputs_embeds + token_type) + position, as BERT); MPNet has none.
+template <bool TYPE_ROW>
+__global__ void __launch_bounds__(256) roberta_embed_ln_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ mask,
+                                                               const float* __restrict__ word, const float* __restrict__ pos,
+                                                               const float* __restrict__ type0, const float* __restrict__ gamma,
+                                                               const float* __restrict__ beta, float eps, int n, int S, int w,
+                                                               int vocab, int pad, float* __restrict__ x,
+                                                               __nv_bfloat16* __restrict__ h, int32_t* __restrict__ kv_len) {
     const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= (long long)n * S) return;
@@ -259,13 +261,19 @@ __global__ void __launch_bounds__(256) mpnet_embed_ln_kernel(const int32_t* __re
     const int nv = w / 128;
     const float4* w4 = reinterpret_cast<const float4*>(word + (long long)id * w);
     const float4* p4 = reinterpret_cast<const float4*>(pos + (long long)p * w);
+    const float4* t4 = reinterpret_cast<const float4*>(type0);
     float4 v[LN_MAX_V4];
 #pragma unroll
     for (int j = 0; j < LN_MAX_V4; ++j)
         if (j < nv) {
             const int i4 = lane + 32 * j;
-            const float4 a = __ldg(w4 + i4), b = __ldg(p4 + i4);
-            v[j] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);   // HF: inputs_embeds + position_embeddings
+            float4 a = __ldg(w4 + i4);
+            const float4 b = __ldg(p4 + i4);
+            if (TYPE_ROW) {
+                const float4 c = __ldg(t4 + i4);
+                a = make_float4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w);
+            }
+            v[j] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);   // HF: inputs_embeds (+ type) + position
         }
     ln_row<true>(v, nv, w, gamma, beta, eps, lane, x + row * w, h + row * w);
     if (s == 0 && lane == 0) {
@@ -278,14 +286,19 @@ __global__ void __launch_bounds__(256) mpnet_embed_ln_kernel(const int32_t* __re
     }
 }
 
-void mpnet_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* gamma,
-                    const float* beta, float eps, int n, int S, int w, int vocab, int pad, float* x, __nv_bfloat16* h,
-                    int32_t* kv_len, cudaStream_t s) {
+void roberta_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
+                      const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, int pad, float* x,
+                      __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s) {
     if (n <= 0) return;
     check_ln_width(w);
     const long long rows = (long long)n * S;
-    mpnet_embed_ln_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(ids, mask, word, pos, gamma, beta, eps, n, S, w, vocab,
-                                                                    pad, x, h, kv_len);
+    const unsigned blocks = (unsigned)((rows + 7) / 8);
+    if (type0)
+        roberta_embed_ln_kernel<true><<<blocks, 256, 0, s>>>(ids, mask, word, pos, type0, gamma, beta, eps, n, S, w, vocab,
+                                                             pad, x, h, kv_len);
+    else
+        roberta_embed_ln_kernel<false><<<blocks, 256, 0, s>>>(ids, mask, word, pos, nullptr, gamma, beta, eps, n, S, w,
+                                                              vocab, pad, x, h, kv_len);
     MB_CUDA(cudaGetLastError());
 }
 

@@ -30,11 +30,12 @@ void bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, c
                    const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, float* x,
                    __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s);
 
-// MPNet: x = LN(word[ids] + position[p]) with HF's position rule p = pad + (non-pad ids among ids[b, 0..s]) for a
-// non-pad id and p = pad for a pad id (no token-type row); fp32 + bf16 copies.  kv_len[b] = sum(mask[b, :]) as above.
-void mpnet_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* gamma,
-                    const float* beta, float eps, int n, int S, int w, int vocab, int pad, float* x, __nv_bfloat16* h,
-                    int32_t* kv_len, cudaStream_t s);
+// RoBERTa-style embeddings (MPNet, XLM-R): x = LN(word[ids] (+ token_type[0]) + position[p]) with HF's position rule
+// p = pad + (non-pad ids among ids[b, 0..s]) for a non-pad id and p = pad for a pad id; type0 NULL (MPNet) adds no
+// token-type row.  fp32 + bf16 copies.  kv_len[b] = sum(mask[b, :]) as above.
+void roberta_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
+                      const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, int pad, float* x,
+                      __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s);
 
 // CLIP head: for image b take token row (b * S + row_in_seq[b]) (row_in_seq NULL -> 0), LayerNorm it, multiply by
 // proj [w, E] (fp32), optionally divide by the L2 norm (no epsilon: abstract_clip_model.py:83-85).

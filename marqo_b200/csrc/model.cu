@@ -1,4 +1,5 @@
-// Encoder runtime: CLIP ViT image tower, CLIP text tower, SigLIP towers, BERT (e5, MiniLM, bge), MPNet — SURVEY §8 a2-a5.
+// Encoder runtime: CLIP ViT image tower, CLIP text tower, SigLIP towers, BERT (e5, MiniLM, bge), MPNet, XLM-R
+// (multilingual-e5) — SURVEY §8 a2-a5.
 //
 // What the reference calls (third-party, restated in oracle/encoders.py):
 //   OPEN_CLIP.encode_image / encode_text   src/marqo/core/inference/embedding_models/open_clip_model.py:249-286
@@ -551,10 +552,11 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
         head_linear(m, c, m->h.get(), n, w, T.w_tproj, E, T.b_tproj, gemm::ACT_NONE, m->pooled.get(), true, false);
         kernels::l2_rows(m->pooled.get(), n, E, normalize, d_out, m->stream);
         c.n += 3;
-    } else if (m->desc.arch == B200_ARCH_MPNET) {
+    } else if (m->desc.arch == B200_ARCH_MPNET || m->desc.arch == B200_ARCH_XLMR) {
+        // RoBERTa position ids; XLM-R also adds its single token-type row (T.type0 is NULL for MPNet)
         const float eps = m->desc.layer_norm_eps;
-        kernels::mpnet_embed_ln(d_ids, d_mask, T.tok, T.pos, T.emb_ln_w, T.emb_ln_b, eps, n, S, w, T.d.vocab,
-                                m->desc.pad_id, m->x.get(), m->h.get(), m->aux.get(), m->stream);
+        kernels::roberta_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, eps, n, S, w, T.d.vocab,
+                                  m->desc.pad_id, m->x.get(), m->h.get(), m->aux.get(), m->stream);
         c.n += 1;
         run_bert_blocks(m, c, T, n, S, eps);
         kernels::bert_head(m->x.get(), m->aux.get(), n, S, w, m->desc.pool, normalize, d_out, m->stream);
@@ -696,7 +698,7 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         *out = nullptr;
         require_sm90_device(device);
         MB_CHECK_ARG(desc->arch == B200_ARCH_CLIP || desc->arch == B200_ARCH_BERT || desc->arch == B200_ARCH_MPNET ||
-                         desc->arch == B200_ARCH_SIGLIP,
+                         desc->arch == B200_ARCH_SIGLIP || desc->arch == B200_ARCH_XLMR,
                      "unknown arch %d", desc->arch);
         MB_CHECK_ARG(desc->max_batch > 0, "max_batch must be positive");
         MB_CHECK_ARG(desc->embed_dim > 0 && desc->embed_dim <= 4096, "embed_dim out of range");
@@ -726,7 +728,7 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
             check_tower(desc->text, "text");
             MB_CHECK_ARG(desc->text.ctx > 0 && desc->text.vocab > 0, "text.ctx and text.vocab must be positive");
             if (desc->arch != B200_ARCH_CLIP && !siglip)
-                MB_CHECK_ARG(desc->embed_dim == desc->text.width, "BERT / MPNet embed_dim must equal width");
+                MB_CHECK_ARG(desc->embed_dim == desc->text.width, "BERT / MPNet / XLM-R embed_dim must equal width");
             if (desc->arch == B200_ARCH_MPNET) {
                 MB_CHECK_ARG(desc->text.width == desc->text.heads * 64, "MPNet: head_dim must be 64 (width %d, heads %d)",
                              desc->text.width, desc->text.heads);
@@ -738,6 +740,11 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
                              desc->rel_max_distance);
                 MB_CHECK_ARG(desc->text.ctx <= 1024, "MPNet: sequences of up to 1024 tokens are supported (ctx %d)",
                              desc->text.ctx);
+            }
+            if (desc->arch == B200_ARCH_XLMR) {
+                MB_CHECK_ARG(desc->layer_norm_eps > 0.f, "XLM-R: layer_norm_eps must be positive");
+                MB_CHECK_ARG(desc->pad_id >= 0 && desc->pad_id < desc->text.vocab, "XLM-R: pad_id %d out of range",
+                             desc->pad_id);
             }
         }
         DeviceGuard g(device);
@@ -775,7 +782,10 @@ int b200_model_load_tensor(b200_model* m, const char* name, const float* data, i
         DeviceGuard g(m->device);
         DeviceBuffer<float> b((size_t)numel);
         MB_CUDA(cudaMemcpy(b.get(), data, (size_t)numel * sizeof(float), cudaMemcpyHostToDevice));
-        m->raw[name] = std::move(b);
+        std::string key = name;
+        // XLMRobertaModel checkpoints saved from a task head carry the encoder under "roberta."
+        if (m->desc.arch == B200_ARCH_XLMR && key.compare(0, 8, "roberta.") == 0) key.erase(0, 8);
+        m->raw[key] = std::move(b);
     });
 }
 
@@ -842,7 +852,7 @@ int b200_model_finalize(b200_model* m) {
                 T.ln_out_b = param(m, "text.ln_final.bias", w);
                 T.w_tproj = to_bf16(m, "text.text_projection.weight", E * w);
                 T.b_tproj = param(m, "text.text_projection.bias", E);
-            } else if (m->desc.arch == B200_ARCH_MPNET) {
+            } else if (m->desc.arch == B200_ARCH_MPNET || m->desc.arch == B200_ARCH_XLMR) {
                 T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
                 // positions run pad_id + 1 .. pad_id + ctx (pads take pad_id): the table has at least ctx + pad_id + 1 rows
                 const long long pos_rows = param_rows(m, "embeddings.position_embeddings.weight", w);
@@ -852,8 +862,13 @@ int b200_model_finalize(b200_model* m) {
                 T.pos = param(m, "embeddings.position_embeddings.weight", pos_rows * w);
                 T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
                 T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
-                build_bert_layers(m, T, MPNET_NAMES);
-                T.rel_bias = build_rel_bias(m, T);
+                if (m->desc.arch == B200_ARCH_XLMR) {
+                    T.type0 = param(m, "embeddings.token_type_embeddings.weight", w);   // type_vocab_size 1
+                    build_bert_layers(m, T, BERT_NAMES);
+                } else {
+                    build_bert_layers(m, T, MPNET_NAMES);
+                    T.rel_bias = build_rel_bias(m, T);
+                }
             } else {
                 T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
                 T.pos = param(m, "embeddings.position_embeddings.weight", (long long)T.d.ctx * w);

@@ -289,14 +289,15 @@ def _to_numpy_f32(t) -> np.ndarray:
 
 
 class Encoder:
-    """A CLIP or SigLIP (vision + text towers), BERT or MPNet encoder resident on one GPU.
+    """A CLIP or SigLIP (vision + text towers), BERT, MPNet or XLM-R encoder resident on one GPU.
 
     `config` keys — CLIP: embed_dim, act ("gelu"|"quickgelu"), mean, std, vision{width,layers,heads,mlp,patch,
     image_size}, text{width,layers,heads,mlp,ctx,vocab};  SigLIP: the CLIP keys plus ln_eps (embed_dim == vision
     width);  BERT: width, layers, heads, mlp, vocab, max_pos, type_vocab,
     pool ("mean"|"cls");  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
-    max_pos - pad_id - 1 tokens), pad_id, ln_eps, rel_buckets, rel_max_distance, pool.  `weights` maps checkpoint
-    parameter names (open_clip state_dict names / HF BertModel / MPNetModel names) to fp32 arrays or torch tensors.
+    max_pos - pad_id - 1 tokens), pad_id, ln_eps, rel_buckets, rel_max_distance, pool;  XLM-R: width, layers, heads,
+    mlp, vocab, max_pos (as MPNet), pad_id, ln_eps, pool.  `weights` maps checkpoint parameter names (open_clip
+    state_dict names / HF BertModel / MPNetModel / XLMRobertaModel names) to fp32 arrays or torch tensors.
     """
 
     def __init__(self, arch: str, config: dict, weights: dict, device: int = 0, max_batch: int = 256):
@@ -330,6 +331,16 @@ class Encoder:
             d.type_vocab = int(config.get("type_vocab", 2))
             d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"],
                                  config.get("max_pos", 512), config["vocab"], 0, 0)
+            self.image_size = 0
+        elif arch == "xlmr":
+            d.arch = N.ARCH_XLMR
+            d.embed_dim = int(config["width"])
+            d.pool = N.POOL_CLS if config.get("pool", "mean") == "cls" else N.POOL_MEAN
+            d.pad_id = int(config.get("pad_id", 1))
+            d.layer_norm_eps = float(config["ln_eps"])
+            ctx = int(config.get("max_pos", 514)) - d.pad_id - 1   # RoBERTa positions start after the pad id
+            d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"], ctx, config["vocab"],
+                                 0, 0)
             self.image_size = 0
         elif arch == "mpnet":
             d.arch = N.ARCH_MPNET

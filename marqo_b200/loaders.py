@@ -33,14 +33,15 @@ def _resolve_weights(props: dict, arch: dict, kind: str) -> Dict[str, np.ndarray
     if w is None and props.get("random_init") is not None:
         seed = int(props["random_init"])
         random = {"clip": weights_mod.random_clip_weights, "siglip": weights_mod.random_siglip_weights,
-                  "bert": weights_mod.random_bert_weights, "mpnet": weights_mod.random_mpnet_weights}[kind]
+                  "bert": weights_mod.random_bert_weights, "mpnet": weights_mod.random_mpnet_weights,
+                  "xlmr": weights_mod.random_xlmr_weights}[kind]
         return random(arch, seed)
     if w is None:
         raise ModelLoadError("model_properties needs `weights` (state dict or checkpoint path) or `random_init`; "
                              "checkpoint download is Marqo's job (open_clip_model.py:107-131) and out of scope here")
     if isinstance(w, (str, bytes)) or hasattr(w, "__fspath__"):
         w = weights_mod.load_state_dict(w)
-    if kind in ("bert", "mpnet"):
+    if kind in ("bert", "mpnet", "xlmr"):
         w = weights_mod.strip_hf_prefix(w)
     return w
 
@@ -293,14 +294,18 @@ class B200HuggingFace:
         if props.get("poolingMethod") or props.get("pooling_method"):  # hugging_face_model_properties.py
             arch = dict(arch, pool=(props.get("poolingMethod") or props.get("pooling_method")))
         self.arch = arch
-        kind = arch.get("kind", "bert")   # "mpnet": MPNetModel (model_registry.MPNET_MODELS); else BertModel
+        # "mpnet": MPNetModel (model_registry.MPNET_MODELS); "xlmr": XLMRobertaModel (XLMR_MODELS); else BertModel
+        kind = arch.get("kind", "bert")
         self._model = Encoder(kind, arch, _resolve_weights(props, arch, kind), device=_validate_device(self.device),
                               max_batch=int(props.get("max_batch", 256)))
         self._tokenizer = props.get("tokenizer") or self._default_tokenizer()
 
     def _default_tokenizer(self):
-        if self.model_properties.get("vocab_file"):
-            from .tokenizers import MPNetTokenizer, WordPieceTokenizer
+        vocab_file = self.model_properties.get("vocab_file")
+        if vocab_file:
+            from .tokenizers import MPNetTokenizer, WordPieceTokenizer, XLMRTokenizer, is_sentencepiece_model
+            if is_sentencepiece_model(vocab_file):   # sentencepiece.bpe.model (multilingual-e5)
+                return XLMRTokenizer(vocab_file)
             cls = MPNetTokenizer if self.arch.get("kind") == "mpnet" else WordPieceTokenizer
             return cls(self.model_properties["vocab_file"],
                        do_lower_case=bool(self.model_properties.get("do_lower_case", True)))

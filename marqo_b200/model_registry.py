@@ -36,7 +36,20 @@ the same `b200_open_clip` loader.  Their shapes come from open_clip 2.24.0's mod
     final LN over all tokens, then the MAP head (a learned latent query attends over the tokens, proj, x + MLP(LN(x)),
     MLP 4 x width); no projection (timm_proj "none").  Text: no causal mask, ln_final, last position pooled, Linear with
     bias (proj_bias).  Preprocessing (_slpcfg): mean = std = 0.5, bicubic squash resize to S x S without a crop.
-ViT-SO400M-14-SigLIP-384 (width 1152, 16 heads: head_dim 72) is not served."""
+ViT-SO400M-14-SigLIP-384 (width 1152, 16 heads: head_dim 72) is not served.
+
+The multilingual-e5 entries (model_registry.py:735-760,788-794) live in XLMR_MODELS, served by the `b200_hf` loader
+with the SentencePiece Unigram tokenizer of XLM-RoBERTa (fairseq id offset: <s> 0, <pad> 1, </s> 2, <unk> 3, every
+other piece at its SentencePiece id + 1).  Their shapes come from the upstream config.json files and cannot be re-read
+offline (verify):
+    multilingual-e5-base              XLMRobertaModel (`arch["kind"] == "xlmr"`): width 768, 12 layers, 12 heads,
+                                      mlp 3072, vocabulary 250002, max_position_embeddings 514 (positions start after
+                                      pad_token_id 1, so at most 512 tokens), one token type, layer_norm_eps 1e-5
+    multilingual-e5-large{,-instruct} the same at width 1024, 24 layers, 16 heads, mlp 4096
+    multilingual-e5-small             a BertModel (Multilingual-MiniLM-L12-H384, `arch["kind"]` absent): width 384,
+                                      12 layers, 12 heads, mlp 1536, vocabulary 250037, 512 positions, 2 token types,
+                                      layer_norm_eps 1e-12; it runs the BERT runtime unchanged
+All four mean-pool the last hidden state and erf-GELU their MLPs."""
 from __future__ import annotations
 
 import copy
@@ -187,9 +200,37 @@ def _siglip_models() -> Dict[str, dict]:
 SIGLIP_MODELS: Dict[str, dict] = _siglip_models()
 
 
+_E5_INSTRUCT_QUERY_PREFIX = "Instruct: Given a web search query, retrieve relevant passages that answer the query\nQuery: "
+
+
+def _xlmr_arch(w: int, layers: int, heads: int) -> dict:
+    """XLMRobertaModel (module docstring, verify)."""
+    return {"kind": "xlmr", "width": w, "layers": layers, "heads": heads, "mlp": 4 * w, "vocab": 250002, "max_pos": 514,
+            "pad_id": 1, "type_vocab": 1, "ln_eps": 1e-5, "pool": "mean"}
+
+
+def _xlmr_models() -> Dict[str, dict]:
+    m: Dict[str, dict] = {}
+    # Multilingual-MiniLM-L12-H384: a BertModel over the XLM-R SentencePiece vocabulary (module docstring, verify)
+    small = {**_bert_arch(*_BERT_SMALL), "vocab": 250037, "tokenizer": "xlmr"}
+    e5 = {"text_query_prefix": "query: ", "text_chunk_prefix": "passage: "}
+    for short, arch, props in (
+            ("multilingual-e5-small", small, {"model_size": 0.471, **e5}),
+            ("multilingual-e5-base", _xlmr_arch(768, 12, 12), {"model_size": 1.11, **e5}),
+            ("multilingual-e5-large", _xlmr_arch(1024, 24, 16), {"model_size": 2.24, **e5}),
+            ("multilingual-e5-large-instruct", _xlmr_arch(1024, 24, 16),
+             {"text_query_prefix": _E5_INSTRUCT_QUERY_PREFIX})):
+        m[f"hf/{short}"] = {"name": f"intfloat/{short}", "dimensions": arch["width"], "tokens": 512, "type": TYPE_HF,
+                            **props, "notes": "", "arch": arch}
+    return m
+
+
+XLMR_MODELS: Dict[str, dict] = _xlmr_models()
+
+
 def find_model(model_name: str) -> Optional[dict]:
     """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
-    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS):
+    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS):
         entry = table.get(model_name)
         if entry is not None:
             return entry
@@ -198,7 +239,7 @@ def find_model(model_name: str) -> Optional[dict]:
 
 def all_models() -> Dict[str, dict]:
     """Every served registry entry by name (a new dict over the same entries)."""
-    return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS}
+    return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS}
 
 
 def get_model_properties(model_name: str) -> dict:

@@ -5,10 +5,13 @@
   token_type_ids}.
 * `MPNetTokenizer` is the same WordPiece pipeline with MPNetTokenizer's special tokens ("<s> A </s>", <pad>, [UNK]) and
   the same call -> {input_ids, attention_mask}.
+* `XLMRTokenizer` is XLMRobertaTokenizer on a SentencePiece Unigram model (multilingual-e5): the same call ->
+  {input_ids, attention_mask}, rows "<s> A </s>" padded with <pad> (1).
 * `ClipBpeTokenizer` is called the way open_clip_model.py:277-279 calls open_clip's tokenizer:
   `tok(texts) -> int64 [n, context_length]`.
 
-Both take the vocabulary FILE Marqo's model cache already holds (vocab.txt / bpe_simple_vocab_16e6.txt[.gz])."""
+Each takes the vocabulary FILE Marqo's model cache already holds (vocab.txt / sentencepiece.bpe.model /
+bpe_simple_vocab_16e6.txt[.gz])."""
 from __future__ import annotations
 
 import ctypes as C
@@ -105,6 +108,27 @@ class MPNetTokenizer(WordPieceTokenizer):
         N.check(N.load().b200_tokenizer_create_wordpiece_ex(data, len(data), 1 if do_lower_case else 0, b"<s>", b"</s>",
                                                             b"<pad>", b"[UNK]", C.cast(specials, C.c_void_p),
                                                             len(self.SPECIALS), C.byref(h)))
+        _Tokenizer.__init__(self, h)
+        self.model_max_length = model_max_length
+
+
+def is_sentencepiece_model(path_or_bytes: Union[str, Path, bytes]) -> bool:
+    """True for a serialized SentencePiece ModelProto (sentencepiece.bpe.model, *.model), False for a text vocabulary."""
+    if isinstance(path_or_bytes, bytes):
+        return path_or_bytes[:1] == b"\x0a"   # field 1 (pieces), length-delimited: no vocab.txt line starts with LF
+    return str(path_or_bytes).endswith(".model")
+
+
+class XLMRTokenizer(WordPieceTokenizer):
+    """transformers' XLMRobertaTokenizer: SentencePiece Unigram (charsmap normalisation, Viterbi segmentation) with
+    fairseq's ids (<s> 0, <pad> 1, </s> 2, <unk> 3, piece id + 1), rows "<s> A </s>" padded with <pad>.  Special-token
+    strings in the text are tokenised as ordinary text.  No token_type_ids."""
+    _token_type_ids = False
+
+    def __init__(self, model_file: Union[str, Path, bytes], model_max_length: int = 512):
+        data = _read(model_file)
+        h = C.c_void_p()
+        N.check(N.load().b200_tokenizer_create_unigram(data, len(data), C.byref(h)))
         _Tokenizer.__init__(self, h)
         self.model_max_length = model_max_length
 

@@ -33,9 +33,9 @@ def load_state_dict(path: str) -> Dict[str, np.ndarray]:
 
 
 def strip_hf_prefix(sd: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
-    """HF checkpoints saved from BertForXxx / MPNetForXxx carry a 'bert.' / 'mpnet.' prefix; BertModel and MPNetModel
-    checkpoints do not."""
-    for prefix in ("bert.", "mpnet."):
+    """HF checkpoints saved from BertForXxx / MPNetForXxx / XLMRobertaForXxx carry a 'bert.' / 'mpnet.' / 'roberta.'
+    prefix; BertModel, MPNetModel and XLMRobertaModel checkpoints do not."""
+    for prefix in ("bert.", "mpnet.", "roberta."):
         if any(k.startswith(prefix) for k in sd):
             return {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
     return sd
@@ -181,6 +181,12 @@ def random_bert_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
         sd[p + "output.LayerNorm.weight"] = _vec(g, w, 0.1, 1.0)
         sd[p + "output.LayerNorm.bias"] = _vec(g, w)
     return sd
+
+
+def random_xlmr_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
+    """Seeded random weights under HF XLMRobertaModel parameter names (arch: the registry's XLM-R block): BertModel's
+    names with max_pos position rows and type_vocab (1) token-type rows."""
+    return random_bert_weights(arch, seed)
 
 
 def random_mpnet_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
