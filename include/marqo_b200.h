@@ -239,7 +239,8 @@ enum b200_arch {
     B200_ARCH_BERT = 1, /* HF BertModel + pooling */
     B200_ARCH_MPNET = 2, /* HF MPNetModel + pooling: BERT layers with a relative-position bias in the attention logits */
     B200_ARCH_SIGLIP = 3, /* open_clip SigLIP: class-token-free ViT with a MAP pooling head + bidirectional text tower */
-    B200_ARCH_XLMR = 4    /* HF XLMRobertaModel + pooling: BERT layers, RoBERTa position ids, one token-type row */
+    B200_ARCH_XLMR = 4,   /* HF XLMRobertaModel + pooling: BERT layers, RoBERTa position ids, one token-type row */
+    B200_ARCH_CLIP_RESNET = 5 /* OpenAI ResNet CLIP (open_clip ModifiedResNet image tower + the CLIP text tower) */
 };
 enum b200_act { B200_ACT_GELU = 0, B200_ACT_QUICKGELU = 1 };
 enum b200_pool { B200_POOL_MEAN = 0, B200_POOL_CLS = 1 };
@@ -275,6 +276,18 @@ typedef struct b200_model_desc {
     /* MPNet only: */
     int32_t rel_buckets;      /* relative_attention_num_buckets (32) */
     int32_t rel_max_distance; /* max_distance of relative_position_bucket (128) */
+    /* CLIP ResNet only (open_clip ModifiedResNet, verify): the image tower; `vision` is unused.
+     *   stem: conv1 3x3 stride 2 (3 -> width/2), conv2 3x3 (width/2 -> width/2), conv3 3x3 (width/2 -> width), each
+     *         without bias and followed by BatchNorm (eps 1e-5) and ReLU, then AvgPool2d(2);
+     *   stage s = 0..3 of resnet_layers[s] Bottlenecks with planes = width << s, stride 1, 2, 2, 2 on the first block:
+     *         ReLU(BN(conv3 1x1 (AvgPool(stride) (ReLU(BN(conv2 3x3 (ReLU(BN(conv1 1x1 (x))))))))) + identity), the
+     *         identity being BN(downsample 1x1 conv (AvgPool(stride) (x))) when stride > 1 or the channels change;
+     *   attention pool over the (S/32)^2 + 1 tokens [mean; pixels] + positional_embedding, resnet_heads heads of 64,
+     *         token 0 out of c_proj, embed_dim wide. */
+    int32_t resnet_layers[4];   /* Bottlenecks per stage: RN50 {3, 4, 6, 3}, RN101 {3, 4, 23, 3} */
+    int32_t resnet_width;       /* 64 (a power of two >= 64) */
+    int32_t resnet_heads;       /* attention-pool heads: width * 32 / 64 (head_dim 64) */
+    int32_t resnet_image_size;  /* 224 (a multiple of 32) */
 } b200_model_desc;
 
 int b200_model_create(int device, const b200_model_desc* desc, b200_model** out);
@@ -287,6 +300,12 @@ int b200_model_destroy(b200_model* m);
  * visual.trunk.attn_pool.{latent [1, 1, W], q, kv, proj, norm, mlp.fc1, mlp.fc2}.*, text.token_embedding.weight,
  * text.positional_embedding, text.transformer.resblocks.{i}.* (the CLIP block names), text.ln_final.*,
  * text.text_projection.{weight [E, W], bias}. */
+/* CLIP ResNet: open_clip ModifiedResNet names (verify): visual.{conv1,conv2,conv3}.weight,
+ * visual.{bn1,bn2,bn3}.{weight,bias,running_mean,running_var}, per block visual.layer{1-4}.{i}.{conv1,conv2,conv3}.weight
+ * and .bn{1,2,3}.*, the first block's .downsample.0.weight (1x1 conv) and .downsample.1.* (its BatchNorm),
+ * visual.attnpool.positional_embedding [(S/32)^2 + 1, 32 width], visual.attnpool.{q,k,v,c}_proj.{weight,bias}; the text
+ * tower under the CLIP names.  BatchNorm is folded into the convolutions by b200_model_finalize (num_batches_tracked is
+ * not needed). */
 /* XLM-R: HF XLMRobertaModel names, as BERT's: embeddings.word_embeddings.weight [vocab, W],
  * embeddings.position_embeddings.weight [ctx + pad_id + 1, W], embeddings.token_type_embeddings.weight [1, W],
  * embeddings.LayerNorm.*, encoder.layer.{i}.* (a "roberta." prefix is dropped). */
@@ -485,6 +504,17 @@ int b200_debug_resize_squash(int device, const uint8_t* hwc, int n, int h, int w
  * b, times v_{b,s}.  q fp32 [W] (one latent query, shared by every image); kv fp32 [B*S, 2W] (K columns then V columns,
  * rounded to bf16); head_dim 64.  out fp32 [B, W] (rounded to bf16). */
 int b200_debug_map_attention(int device, const float* q, const float* kv, int B, int S, int W, int H, float* out);
+/* The same with one query per image (the ResNet attention pool): q fp32 [B, W]. */
+int b200_debug_map_attention_per_image(int device, const float* q, const float* kv, int B, int S, int W, int H,
+                                       float* out);
+/* One convolution of the ResNet CLIP image tower, on the path the model runs it: out = act(conv(x) + bias (+ residual))
+ * rounded to bf16, NHWC fp32 in and out (x, w, bias and residual are rounded to bf16 first, the bias kept fp32).
+ * x [n, H, W, cin]; w [cout, cin, k, k] (torch layout); bias [cout] (NULL: zeros).  cin == 3: the stem conv1 (k 3,
+ * stride 2, padding 1; out [n, H/2, W/2, cout], x already normalised).  Otherwise k 1 (a GEMM over the pixels) or 3
+ * (the implicit GEMM, stride 1, padding 1, cin a power of two >= 32); out [n, H, W, cout].  relu != 0: ReLU, with the
+ * optional residual [n, H, W, cout] added before it; relu == 0 (1 x 1 and stem convs only) takes no residual. */
+int b200_debug_conv2d(int device, const float* x, int n, int H, int W, int cin, const float* w, int cout, int k,
+                      const float* bias, const float* residual, int relu, float* out);
 /* Bytes of device memory the library holds right now, over all devices and handles of this process (indexes,
  * exchanges, models and the scratch of calls in flight).  Memory from b200_host_alloc is not counted.  Returns to its
  * earlier value once every handle created in between is destroyed: a leak check. */

@@ -382,7 +382,8 @@ int b200_debug_resize_squash(int device, const uint8_t* hwc, int n, int h, int w
     });
 }
 
-int b200_debug_map_attention(int device, const float* q, const float* kv, int B, int S, int W, int H, float* out) {
+static int debug_map_attention(int device, const float* q, bool per_image, const float* kv, int B, int S, int W, int H,
+                               float* out) {
     return guarded([&] {
         MB_CHECK_ARG(q && kv && out, "NULL buffer");
         MB_CHECK_ARG(B > 0 && S > 0 && W > 0 && H > 0, "B, S, W, H must be positive");
@@ -391,16 +392,84 @@ int b200_debug_map_attention(int device, const float* q, const float* kv, int B,
         DeviceGuard g(device);
         Scratch sc;
         const size_t M = (size_t)B * S;
-        const float* dq = sc.upload(q, (size_t)W);
+        const float* dq = sc.upload(q, (size_t)W * (per_image ? B : 1));
         __nv_bfloat16* dkv = sc.upload_bf16(kv, M * 2 * W);
         __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>((size_t)B * W);
         float* dOut = sc.alloc<float>((size_t)B * W);
-        kernels::map_attention(dq, dkv, B, S, W, H, dO, sc.s);
+        kernels::map_attention(dq, per_image ? W : 0, dkv, B, S, W, H, dO, sc.s);
         const long long n = (long long)B * W;
         bf16_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, sc.s>>>(dO, dOut, n);
         MB_CUDA(cudaGetLastError());
         MB_CUDA(cudaStreamSynchronize(sc.s));
         MB_CUDA(cudaMemcpy(out, dOut, (size_t)B * W * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int b200_debug_map_attention(int device, const float* q, const float* kv, int B, int S, int W, int H, float* out) {
+    return debug_map_attention(device, q, false, kv, B, S, W, H, out);
+}
+
+int b200_debug_map_attention_per_image(int device, const float* q, const float* kv, int B, int S, int W, int H,
+                                       float* out) {
+    return debug_map_attention(device, q, true, kv, B, S, W, H, out);
+}
+
+int b200_debug_conv2d(int device, const float* x, int n, int H, int W, int cin, const float* w, int cout, int k,
+                      const float* bias, const float* residual, int relu, float* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && w && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && H > 0 && W > 0 && cout > 0, "n, H, W, cout must be positive");
+        MB_CHECK_ARG(cin == 3 ? k == 3 && H == W && H % 2 == 0 : (k == 1 || (k == 3 && H == W)),
+                     "unsupported conv: cin %d, k %d, %d x %d", cin, k, H, W);
+        MB_CHECK_ARG(relu || !residual, "a residual needs the ReLU");
+        MB_CHECK_ARG(relu || k == 1 || cin == 3, "the 3 x 3 gather conv runs with ReLU only");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const int K = gemm::conv_rows_k(cin, k);
+        std::vector<float> rows((size_t)cout * K);
+        gemm::conv_weight_rows(w, cout, cin, k, nullptr, rows.data());
+        __nv_bfloat16* dW = sc.upload_bf16(rows.data(), rows.size());
+        std::vector<float> zeros;
+        if (!bias) zeros.assign((size_t)cout, 0.f);
+        const float* dB = sc.upload(bias ? bias : zeros.data(), (size_t)cout);
+        const int Ho = cin == 3 ? H / 2 : H, Wo = cin == 3 ? W / 2 : W;
+        const size_t out_n = (size_t)n * Ho * Wo * cout;
+        gemm::Epilogue e;
+        e.bias = dB;
+        e.act = relu ? gemm::ACT_RELU : gemm::ACT_NONE;
+        e.residual = residual ? sc.upload_bf16(residual, out_n) : nullptr;
+        e.ldr = cout;
+        __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>(out_n);
+        e.out = dO;
+        e.ldo = cout;
+        if (cin == 3) {   // the stem: from already-normalised fp32 CHW, as b200_model_encode_images_f32 runs it
+            std::vector<float> chw((size_t)n * 3 * H * W);
+            for (int b = 0; b < n; ++b)
+                for (int c = 0; c < 3; ++c)
+                    for (int i = 0; i < H * W; ++i) chw[((size_t)b * 3 + c) * H * W + i] = x[((size_t)b * H * W + i) * 3 + c];
+            const float* dchw = sc.upload(chw.data(), chw.size());
+            __nv_bfloat16* dA = sc.alloc<__nv_bfloat16>((size_t)n * Ho * Wo * 64);
+            const float mean[3] = {0.f, 0.f, 0.f}, std1[3] = {1.f, 1.f, 1.f};
+            kernels::stem_im2col(nullptr, dchw, n, H, mean, std1, dA, sc.s);
+            gemm::launch(dA, K, dW, n * Ho * Wo, cout, K, e, sm_count(device), sc.s);
+        } else if (k == 3) {
+            gemm::ConvGather cg;
+            cg.act = sc.upload_bf16(x, (size_t)n * H * W * cin);
+            cg.n = n;
+            cg.H = H;
+            cg.W = W;
+            cg.cin = cin;
+            gemm::launch_conv3x3(cg, dW, cout, e, sc.s);
+        } else {
+            const __nv_bfloat16* dX = sc.upload_bf16(x, (size_t)n * H * W * cin);
+            gemm::launch(dX, cin, dW, n * H * W, cout, cin, e, sm_count(device), sc.s);
+        }
+        float* dOut = sc.alloc<float>(out_n);
+        bf16_to_f32_kernel<<<(unsigned)((out_n + 255) / 256), 256, 0, sc.s>>>(dO, dOut, (long long)out_n);
+        MB_CUDA(cudaGetLastError());
+        MB_CUDA(cudaStreamSynchronize(sc.s));
+        MB_CUDA(cudaMemcpy(out, dOut, out_n * 4, cudaMemcpyDeviceToHost));
     });
 }
 

@@ -19,8 +19,8 @@ namespace gemm {
 //   warps 0-7   two MMA warpgroups, 64 rows of the tile each (wgmma m64n128k16, fp32 accumulators in registers), then
 //               the epilogue;
 //   warps 8..   the producer: one warp issuing TMA loads of A and W k-blocks (128B swizzle) into a STAGES-deep smem ring,
-//               or, for the ViT patch embedding (GATHER), four warps that build the A stage from the uint8 image while
-//               one of them still loads W by TMA.
+//               or, for the ViT patch embedding (PROD_PATCH) and the 3 x 3 convolutions (PROD_CONV), four warps that
+//               build the A stage from the uint8 image or the NHWC activation while one of them still loads W by TMA.
 // Two CTAs share an SM (3 x 32 KB stages each), so one CTA's epilogue overlaps the other's main loop.
 // Warpgroup wg's 64 x 128 block of the output goes through one ring stage, the one of virtual k-block kblocks + wg:
 // the producer takes that stage through the usual empty/full protocol once the main loop has released it (k-block
@@ -71,6 +71,10 @@ constexpr size_t P_SMEM_BYTES = 1024 /*align*/ + P_RING_BYTES + 2 * EPI_BYTES + 
 static_assert(P_SMEM_BYTES <= 227 * 1024, "over the opt-in shared memory of an H100 CTA");
 static_assert(P_BN * 2 * EPI_ROWS == EPI_BYTES, "a warpgroup's bf16 64 x 256 block is one epilogue buffer");
 
+// How gemm_kernel's producer fills the A stages: TMA from an A matrix, or four gather warps building them from the
+// uint8 image (ViT patch embedding) or from an NHWC activation (3 x 3 convolution).
+enum Producer { PROD_TMA = 0, PROD_PATCH = 1, PROD_CONV = 2 };
+
 template <bool GATHER>
 constexpr int threads() { return MMA_THREADS + (GATHER ? 128 : 32); }
 
@@ -78,9 +82,12 @@ struct Params {
     int M, N, K;
     int tiles_m, tiles_n;
     Epilogue ep;
-    // GATHER only: uint8 HWC images [n, S, S, 3]; A row r = token t = r % (g*g + cls) of image r / (g*g + cls): zero
+    // PROD_PATCH: uint8 HWC images [n, S, S, 3]; A row r = token t = r % (g*g + cls) of image r / (g*g + cls): zero
     // for t < cls (the class token), else patch t - cls, row-major in the grid.
     // k index of the A row = dy * (64 * kbpd) + dx * 3 + c (kernels::patch_weight_rows lays W out the same way).
+    // PROD_CONV (gemm.cuh: ConvGather) reuses four of these fields rather than growing Params, whose layout every
+    // other instantiation's code depends on: img is the NHWC bf16 activation [n, H, W, cin], g = H, patch = W and
+    // kbpd = log2(cin).
     const uint8_t* img;
     int g;                  // patches per image side
     int patch;              // patch edge in pixels
@@ -188,6 +195,8 @@ __device__ __forceinline__ float2 act(float x0, float x1) {
         return make_float2(gelu_erf(x0), gelu_erf(x1));
     else if constexpr (ACT == ACT_QUICKGELU)
         return make_float2(quick_gelu(x0), quick_gelu(x1));
+    else if constexpr (ACT == ACT_RELU)
+        return make_float2(fmaxf(x0, 0.f), fmaxf(x1, 0.f));
     else
         return make_float2(x0, x1);
 }
@@ -195,10 +204,12 @@ __device__ __forceinline__ float2 act(float x0, float x1) {
 // The epilogue of COLS output columns of a warpgroup's 64 rows, held in acc[0, COLS / 2) (fragment i: columns
 // 8 i + 2 (lane & 3) + {0, 1} of rows rbase and rbase + 8): act(acc + bias) with the bias row at shared address bias_s,
 // plus the fp32 residual already in the buffer when there is one, written at epi_offset into the buffer at shared
-// address buf_s.
+// address buf_s.  ACT_RELU (bf16 only) adds its bf16 residual, already in the buffer in the output's layout, before
+// the activation.
 template <bool OUT_FP32, int ACT, int COLS>
 __device__ __forceinline__ void epilogue_to_smem(const float* acc, uint32_t bias_s, uint32_t buf_s, bool residual,
                                                  int rbase, int lane) {
+    static_assert(!(OUT_FP32 && ACT == ACT_RELU), "ACT_RELU writes bf16");
 #pragma unroll
     for (int i = 0; i < COLS / 8; ++i) {
         const int col = 8 * i + 2 * (lane & 3);
@@ -206,6 +217,19 @@ __device__ __forceinline__ void epilogue_to_smem(const float* acc, uint32_t bias
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int r = rbase + 8 * h;
+            if constexpr (ACT == ACT_RELU) {
+                const uint32_t dst = buf_s + epi_offset<2>(r, col);
+                float x0 = acc[4 * i + 2 * h] + bv.x, x1 = acc[4 * i + 2 * h + 1] + bv.y;
+                if (residual) {
+                    const uint32_t rv = ptx::ld_shared_u32(dst);
+                    const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rv));
+                    x0 += f.x;
+                    x1 += f.y;
+                }
+                const float2 y = act<false, ACT_RELU>(x0, x1);
+                ptx::st_shared_u32(dst, pack_bf16x2(y.x, y.y));
+                continue;
+            }
             float2 y = act<OUT_FP32, ACT>(acc[4 * i + 2 * h] + bv.x, acc[4 * i + 2 * h + 1] + bv.y);
             if constexpr (OUT_FP32) {
                 const uint32_t dst = buf_s + epi_offset<4>(r, col);
@@ -233,6 +257,15 @@ __device__ __forceinline__ void load_residual_boxes(const CUtensorMap* tmap_r, u
         ptx::tma_load_2d(buf + b * EPI_BOX_BYTES, tmap_r, bar, c0 + 32 * b, row0, ptx::kEvictNormal);
 }
 
+// The same for a bf16 residual (ACT_RELU): boxes of 64 columns, the output's layout.
+__device__ __forceinline__ void load_residual_boxes_bf16(const CUtensorMap* tmap_r, uint64_t* bar, uint8_t* buf,
+                                                         int row0, int c0, int M, int N) {
+    const int boxes = row0 < M && c0 < N ? min(2, (N - c0 + 63) / 64) : 0;
+    ptx::mbar_arrive_expect_tx(bar, (uint32_t)boxes * EPI_BOX_BYTES);
+    for (int b = 0; b < boxes; ++b)
+        ptx::tma_load_2d(buf + b * EPI_BOX_BYTES, tmap_r, bar, c0 + 64 * b, row0, ptx::kEvictNormal);
+}
+
 // TMA-stores the 64-row, COLS-column output block at (row0, c0) from its boxes in buf, clipped at M and N, as one bulk
 // group.
 template <bool OUT_FP32, int COLS>
@@ -247,11 +280,12 @@ __device__ __forceinline__ void store_output_boxes(const CUtensorMap* tmap_o, co
 
 // tmap_r / tmap_o: the fp32 residual and the output, boxes of EPI_ROWS rows x 128 bytes.  p is a grid constant so that
 // the gather's run-time index into p.nscale / p.nshift reads the parameter space instead of a local copy of p.
-template <bool GATHER, bool OUT_FP32, int ACT>
-__global__ void __launch_bounds__(threads<GATHER>(), GATHER ? 1 : 2)
+template <int PROD, bool OUT_FP32, int ACT>
+__global__ void __launch_bounds__(threads<PROD != PROD_TMA>(), PROD != PROD_TMA ? 1 : 2)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_o,
             const __grid_constant__ Params p) {
+    constexpr bool GATHER = PROD != PROD_TMA;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * STAGE_BYTES);
@@ -283,7 +317,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         if (!GATHER && pt >= 32) return;
         // GATHER: thread pt builds A row pt of every stage: token row m0 + pt, zero (prow == nullptr) for a class token
         const uint8_t* prow = nullptr;
-        if (GATHER) {
+        // PROD_CONV: thread pt builds A row pt, output pixel (b, cy, cx) = m0 + pt; cimg is image b (NULL: row >= M)
+        const __nv_bfloat16* cimg = nullptr;
+        int cy = 0, cx = 0;
+        const int cH = p.g, cW = p.patch, lg_cin = p.kbpd;   // PROD_CONV's meaning of these fields
+        if (PROD == PROD_CONV) {
+            const int r = m0 + pt;
+            if (r < p.M) {
+                const int hw = cH * cW;
+                const int b = r / hw, rem = r - b * hw;
+                cy = rem / cW;
+                cx = rem - cy * cW;
+                cimg = reinterpret_cast<const __nv_bfloat16*>(p.img) + ((size_t)b * hw << lg_cin);
+            }
+        }
+        if (PROD == PROD_PATCH) {
             const int r = m0 + pt;
             const int tokens = p.g * p.g + p.cls;
             const int b = r / tokens, t = r - b * tokens - p.cls;
@@ -303,7 +351,24 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                 if (!GATHER) ptx::tma_load_2d(sa, &tmap_a, &full[stage], kb * BK, m0, ptx::kEvictNormal);
                 ptx::tma_load_2d(sb, &tmap_b, &full[stage], kb * BK, n0, ptx::kEvictLast);
             }
-            if (GATHER) {
+            if (PROD == PROD_CONV) {
+                // 16-byte unit u holds k = 64 kb + 8 u .. + 7: channels c .. c + 7 of tap k >> lg_cin.  All eight
+                // loads are issued before the first store.
+                uint4 v[8];
+#pragma unroll
+                for (int u = 0; u < 8; ++u) {
+                    const int k = kb * 64 + u * 8;
+                    const int tap = k >> lg_cin, c = k & ((1 << lg_cin) - 1);
+                    const int iy = cy + tap / 3 - 1, ix = cx + tap % 3 - 1;
+                    v[u] = make_uint4(0u, 0u, 0u, 0u);
+                    if (cimg != nullptr && tap < 9 && (unsigned)iy < (unsigned)cH && (unsigned)ix < (unsigned)cW)
+                        v[u] = __ldg(reinterpret_cast<const uint4*>(cimg + (((size_t)iy * cW + ix) << lg_cin) + c));
+                }
+#pragma unroll
+                for (int u = 0; u < 8; ++u) *reinterpret_cast<uint4*>(sa + sw128_offset(pt, u)) = v[u];
+                ptx::fence_proxy_async_smem();   // generic-proxy stores -> visible to wgmma's operand reads
+                ptx::mbar_arrive(&full[stage]);
+            } else if (GATHER) {
                 // k-block kb covers k' = dy * 64 kbpd + j0 .. + 63 of the patch's pixel row dy
                 const int dy = kb / p.kbpd, j0 = (kb - dy * p.kbpd) * 64;
                 const uint8_t* src = prow ? prow + (size_t)dy * p.row_bytes + j0 : nullptr;
@@ -335,9 +400,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             uint8_t* s = smem + (size_t)stage * STAGE_BYTES;
             ptx::mbar_wait(&empty[stage], ((uint32_t)(kb / STAGES) & 1u) ^ 1);
             if (pt == 0) {
-                if (p.ep.residual != nullptr)
-                    load_residual_boxes(&tmap_r, &full[stage], s, m0 + EPI_ROWS * wg, n0, p.M, p.N);
-                else
+                if (p.ep.residual != nullptr) {
+                    if constexpr (ACT == ACT_RELU)
+                        load_residual_boxes_bf16(&tmap_r, &full[stage], s, m0 + EPI_ROWS * wg, n0, p.M, p.N);
+                    else
+                        load_residual_boxes(&tmap_r, &full[stage], s, m0 + EPI_ROWS * wg, n0, p.M, p.N);
+                } else
                     ptx::mbar_arrive(&full[stage]);
             }
             if (GATHER) ptx::mbar_arrive(&full[stage]);   // full[] also counts every gather thread
@@ -545,6 +613,10 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 // both launches and configure() take theirs.
 template <class F>
 static void dispatch(bool out_fp32, int act, F&& f) {
+    if (act == ACT_RELU) {   // bf16 only (check_epilogue)
+        f(std::false_type{}, std::integral_constant<int, ACT_RELU>{});
+        return;
+    }
     const auto with_act = [&](auto out) {
         if (act == ACT_GELU)
             f(out, std::integral_constant<int, ACT_GELU>{});
@@ -563,13 +635,14 @@ void configure() {
     static std::once_flag once;
     std::call_once(once, [] {
         const auto attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
-        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<true, true, ACT_NONE>, attr, (int)SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<PROD_PATCH, true, ACT_NONE>, attr, (int)SMEM_BYTES));
+        MB_CUDA(cudaFuncSetAttribute(gemm_kernel<PROD_CONV, false, ACT_RELU>, attr, (int)SMEM_BYTES));
         for (int out_fp32 = 0; out_fp32 < 2; ++out_fp32)
-            for (int act = ACT_NONE; act <= ACT_QUICKGELU; ++act)
+            for (int act = ACT_NONE; act <= ACT_RELU; ++act)
                 dispatch(out_fp32, act, [&](auto out, auto a) {
                     constexpr bool OUT_FP32 = decltype(out)::value;
                     constexpr int ACT = decltype(a)::value;
-                    MB_CUDA(cudaFuncSetAttribute(gemm_kernel<false, OUT_FP32, ACT>, attr, (int)SMEM_BYTES));
+                    MB_CUDA(cudaFuncSetAttribute(gemm_kernel<PROD_TMA, OUT_FP32, ACT>, attr, (int)SMEM_BYTES));
                     MB_CUDA(cudaFuncSetAttribute(gemm_persistent_kernel<OUT_FP32, ACT>, attr, (int)P_SMEM_BYTES));
                 });
     });
@@ -579,28 +652,39 @@ void configure() {
 static void check_epilogue(const Epilogue& ep) {
     if (ep.ldo % 8 != 0) fail(B200_ERR_INTERNAL, "gemm: ldo = %d must be a multiple of 8", ep.ldo);
     if ((reinterpret_cast<uintptr_t>(ep.out) & 15) != 0) fail(B200_ERR_INTERNAL, "gemm: output not 16-byte aligned");
-    if (ep.residual != nullptr &&
-        (!ep.out_fp32 || ep.ldr % 4 != 0 || (reinterpret_cast<uintptr_t>(ep.residual) & 15) != 0))
-        fail(B200_ERR_INTERNAL, "gemm: the residual needs an fp32 output, ldr %% 4 == 0 and 16-byte alignment");
+    if (ep.act == ACT_RELU && ep.out_fp32) fail(B200_ERR_INTERNAL, "gemm: ReLU writes a bf16 output");
+    if (ep.residual != nullptr && (ep.out_fp32 ? ep.ldr % 4 != 0 : ep.act != ACT_RELU || ep.ldr % 8 != 0))
+        fail(B200_ERR_INTERNAL, "gemm: the residual needs an fp32 output and ldr %% 4 == 0, or ReLU and ldr %% 8 == 0");
+    if (ep.residual != nullptr && (reinterpret_cast<uintptr_t>(ep.residual) & 15) != 0)
+        fail(B200_ERR_INTERNAL, "gemm: residual not 16-byte aligned");
 }
 
 // The epilogue's maps, boxes of EPI_ROWS rows x 128 bytes with the 128B swizzle: the fp32 residual (tr is left as it
 // is without one) and the output.
 static void epilogue_tmaps(const Epilogue& ep, int M, int N, CUtensorMap& tr, CUtensorMap& to) {
     if (ep.residual)
-        tr = make_tmap_2d(ep.residual, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
-                          (uint64_t)ep.ldr * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
+        tr = ep.out_fp32 ? make_tmap_2d(ep.residual, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
+                                        (uint64_t)ep.ldr * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B)
+                         : make_tmap_2d(ep.residual, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)N, (uint64_t)M,
+                                        (uint64_t)ep.ldr * 2, 64, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
     to = ep.out_fp32 ? make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (uint64_t)N, (uint64_t)M,
                                     (uint64_t)ep.ldo * 4, 32, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B)
                      : make_tmap_2d(ep.out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)N, (uint64_t)M,
                                     (uint64_t)ep.ldo * 2, 64, EPI_ROWS, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-template <bool GATHER, bool OUT_FP32, int ACT>
+template <int PROD, bool OUT_FP32, int ACT>
 static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep,
-                         cudaStream_t stream, const PatchGather* pg = nullptr) {
+                         cudaStream_t stream, const PatchGather* pg = nullptr, const ConvGather* cg = nullptr) {
+    constexpr bool GATHER = PROD != PROD_TMA;
     Params p{};
-    if (GATHER) {
+    if (PROD == PROD_CONV) {   // (Params: the fields PROD_CONV reuses)
+        p.img = reinterpret_cast<const uint8_t*>(cg->act);
+        p.g = cg->H;
+        p.patch = cg->W;
+        while ((1 << p.kbpd) < cg->cin) ++p.kbpd;
+    }
+    if (PROD == PROD_PATCH) {
         p.img = pg->img;
         p.patch = pg->patch;
         p.g = pg->S / pg->patch;
@@ -629,7 +713,7 @@ static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W
                                            (uint64_t)lda * 2, BK, BM, CU_TENSOR_MAP_SWIZZLE_128B);
     CUtensorMap tr = tb, to;
     epilogue_tmaps(ep, M, N, tr, to);
-    gemm_kernel<GATHER, OUT_FP32, ACT><<<(unsigned)tiles, threads<GATHER>(), SMEM_BYTES, stream>>>(ta, tb, tr, to, p);
+    gemm_kernel<PROD, OUT_FP32, ACT><<<(unsigned)tiles, threads<GATHER>(), SMEM_BYTES, stream>>>(ta, tb, tr, to, p);
     MB_CUDA(cudaGetLastError());
 }
 
@@ -669,7 +753,35 @@ void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, c
     const int g = pg.S / pg.patch;
     const long long M = (long long)pg.n * (g * g + pg.cls);
     if (M > 0x7fffffffLL) fail(B200_ERR_INVALID_ARG, "patch gather: batch of %d images is too large", pg.n);
-    launch_tiles<true, true, ACT_NONE>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
+    launch_tiles<PROD_PATCH, true, ACT_NONE>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
+}
+
+void launch_conv3x3(const ConvGather& cg, const __nv_bfloat16* Wc, int N, const Epilogue& ep, cudaStream_t stream) {
+    if (cg.n <= 0 || N <= 0) return;
+    if (cg.H <= 0 || cg.W <= 0 || cg.cin < 32 || (cg.cin & (cg.cin - 1)) != 0)
+        fail(B200_ERR_INTERNAL, "conv3x3: %d x %d x %d input (cin must be a power of two >= 32)", cg.H, cg.W, cg.cin);
+    if (N % 32 != 0) fail(B200_ERR_INTERNAL, "conv3x3: N = %d must be a multiple of 32", N);
+    if (ep.out_fp32 || ep.act != ACT_RELU) fail(B200_ERR_INTERNAL, "conv3x3: bf16 output with ReLU only");
+    if ((reinterpret_cast<uintptr_t>(cg.act) & 15) != 0) fail(B200_ERR_INTERNAL, "conv3x3: input not 16-byte aligned");
+    check_epilogue(ep);
+    configure();
+    const long long M = (long long)cg.n * cg.H * cg.W;
+    if (M > 0x7fffffffLL) fail(B200_ERR_INVALID_ARG, "conv3x3: batch of %d images is too large", cg.n);
+    launch_tiles<PROD_CONV, false, ACT_RELU>(nullptr, 0, Wc, (int)M, N, conv_gather_k(cg.cin), ep, stream, nullptr, &cg);
+}
+
+int conv_rows_k(int cin, int k) { return cin == 3 ? 64 : k == 1 ? cin : conv_gather_k(cin); }
+
+void conv_weight_rows(const float* w, int cout, int cin, int k, const double* scale, float* out) {
+    const int K = conv_rows_k(cin, k), taps = k * k;
+    for (int o = 0; o < cout; ++o) {
+        const double s = scale ? scale[o] : 1.0;
+        float* row = out + (size_t)o * K;
+        for (int j = 0; j < K; ++j) row[j] = 0.f;
+        for (int c = 0; c < cin; ++c)
+            for (int t = 0; t < taps; ++t)
+                row[t * cin + c] = (float)((double)w[((size_t)o * cin + c) * taps + t] * s);
+    }
 }
 
 int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep, int sms,
@@ -684,14 +796,15 @@ int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N
     // tile (all four ViT-L-14 layer GEMMs, K >= 1024), at least one full wave of tiles, and no half-empty 256-wide
     // column tile (the 384-wide BERTs run slower with one; DESIGN.md §7.5c).
     const long long tiles256 = (long long)((M + BM - 1) / BM) * (N / P_BN);
-    const bool persistent = K >= 1024 && N % P_BN == 0 && tiles256 >= sms;
+    // (the persistent kernel has no bf16 residual)
+    const bool persistent = K >= 1024 && N % P_BN == 0 && tiles256 >= sms && (ep.out_fp32 || ep.residual == nullptr);
     dispatch(ep.out_fp32, ep.act, [&](auto out, auto a) {
         constexpr bool OUT_FP32 = decltype(out)::value;
         constexpr int ACT = decltype(a)::value;
         if (persistent)
             launch_persistent<OUT_FP32, ACT>(A, lda, W, M, N, K, ep, sms, stream);
         else
-            launch_tiles<false, OUT_FP32, ACT>(A, lda, W, M, N, K, ep, stream);
+            launch_tiles<PROD_TMA, OUT_FP32, ACT>(A, lda, W, M, N, K, ep, stream);
     });
     return persistent ? KERNEL_PERSISTENT : KERNEL_128x128;
 }

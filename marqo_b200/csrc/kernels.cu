@@ -679,7 +679,7 @@ __device__ __forceinline__ float block_reduce_128(float v, float* red, bool is_m
     return is_max ? fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3])) : ((red[0] + red[1]) + red[2]) + red[3];
 }
 
-__global__ void __launch_bounds__(MAP_THREADS) map_attention_kernel(const float* __restrict__ q,
+__global__ void __launch_bounds__(MAP_THREADS) map_attention_kernel(const float* __restrict__ q, long long q_stride,
                                                                     const __nv_bfloat16* __restrict__ kv, int S, int W,
                                                                     __nv_bfloat16* __restrict__ out) {
     extern __shared__ float logit[];   // [S]
@@ -687,7 +687,7 @@ __global__ void __launch_bounds__(MAP_THREADS) map_attention_kernel(const float*
     __shared__ float red[4];
     __shared__ float part[4][64];
     const int b = blockIdx.x, h = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    if (tid < 64) qs[tid] = q[h * 64 + tid] * (0.125f * 1.4426950408889634f);
+    if (tid < 64) qs[tid] = q[b * q_stride + h * 64 + tid] * (0.125f * 1.4426950408889634f);
     __syncthreads();
     const long long ld = 2LL * W;
     const __nv_bfloat16* keys = kv + (long long)b * S * ld + h * 64;
@@ -734,13 +734,143 @@ __global__ void __launch_bounds__(MAP_THREADS) map_attention_kernel(const float*
     }
 }
 
-void map_attention(const float* q, const __nv_bfloat16* kv, int n, int S, int W, int heads, __nv_bfloat16* out,
-                   cudaStream_t s) {
+void map_attention(const float* q, long long q_stride, const __nv_bfloat16* kv, int n, int S, int W, int heads,
+                   __nv_bfloat16* out, cudaStream_t s) {
     if (n <= 0) return;
     if (W != heads * 64) fail(B200_ERR_UNSUPPORTED, "map_attention: head_dim must be 64 (width %d, heads %d)", W, heads);
     if (S <= 0 || S > MAP_MAX_TOKENS) fail(B200_ERR_UNSUPPORTED, "map_attention: %d tokens (1..%d)", S, MAP_MAX_TOKENS);
-    map_attention_kernel<<<dim3((unsigned)n, (unsigned)heads), MAP_THREADS, (size_t)S * sizeof(float), s>>>(q, kv, S, W,
-                                                                                                        out);
+    map_attention_kernel<<<dim3((unsigned)n, (unsigned)heads), MAP_THREADS, (size_t)S * sizeof(float), s>>>(
+        q, q_stride, kv, S, W, out);
+    MB_CUDA(cudaGetLastError());
+}
+
+// ------------------------------------------------------------------------------------------------ ResNet trunk
+// One thread = 8 consecutive k of one output pixel: k = tap * 3 + c (tap = 3 ky + kx), zero for k >= 27.  Input pixel
+// (2 oy - 1 + ky, 2 ox - 1 + kx), zero outside the image: the convolution pads the normalised image.
+__global__ void __launch_bounds__(256) stem_im2col_kernel(const uint8_t* __restrict__ u8, const float* __restrict__ chw,
+                                                          int n, int S, float3 nscale, float3 nshift,
+                                                          __nv_bfloat16* __restrict__ out) {
+    const int So = S / 2;
+    const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long total = (long long)n * So * So * 8;
+    if (gid >= total) return;
+    const int kg = (int)(gid & 7);
+    const long long pix = gid >> 3;
+    const long long b = pix / ((long long)So * So);
+    const int rem = (int)(pix - b * So * So), oy = rem / So, ox = rem - oy * So;
+    float f[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+        const int k = kg * 8 + e, tap = k / 3, c = k - tap * 3;
+        const int iy = 2 * oy - 1 + tap / 3, ix = 2 * ox - 1 + tap % 3;
+        float v = 0.f;
+        if (k < 27 && (unsigned)iy < (unsigned)S && (unsigned)ix < (unsigned)S) {
+            if (u8 != nullptr) {
+                const float sc = c == 0 ? nscale.x : c == 1 ? nscale.y : nscale.z;
+                const float sh = c == 0 ? nshift.x : c == 1 ? nshift.y : nshift.z;
+                v = fmaf((float)__ldg(u8 + ((b * S + iy) * S + ix) * 3 + c), sc, sh);
+            } else {
+                v = __ldg(chw + ((b * 3 + c) * S + iy) * S + ix);
+            }
+        }
+        f[e] = v;
+    }
+    reinterpret_cast<uint4*>(out)[gid] =
+        make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
+}
+
+void stem_im2col(const uint8_t* u8, const float* chw, int n, int S, const float* mean, const float* std,
+                 __nv_bfloat16* out, cudaStream_t s) {
+    if (n <= 0) return;
+    if (S % 2 != 0) fail(B200_ERR_INTERNAL, "stem_im2col: image size %d must be even", S);
+    float sc[3], sh[3];
+    for (int c = 0; c < 3; ++c) {   // the patch gather's constants (gemm.cu launch_tiles)
+        sc[c] = (float)(1.0 / (255.0 * (double)std[c]));
+        sh[c] = (float)(-(double)mean[c] / (double)std[c]);
+    }
+    const long long total = (long long)n * (S / 2) * (S / 2) * 8;
+    stem_im2col_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(u8, chw, n, S, make_float3(sc[0], sc[1], sc[2]),
+                                                                        make_float3(sh[0], sh[1], sh[2]), out);
+    MB_CUDA(cudaGetLastError());
+}
+
+// One thread = 8 channels of one output pixel; the four inputs are summed in fp32 and scaled by 1/4.
+__global__ void __launch_bounds__(256) avgpool2_kernel(const uint4* __restrict__ in, int n, int H, int W, int C8,
+                                                       uint4* __restrict__ out) {
+    const int Ho = H / 2, Wo = W / 2;
+    const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long total = (long long)n * Ho * Wo * C8;
+    if (gid >= total) return;
+    const int c = (int)(gid % C8);
+    const long long pix = gid / C8;
+    const long long b = pix / ((long long)Ho * Wo);
+    const int rem = (int)(pix - b * Ho * Wo), oy = rem / Wo, ox = rem - oy * Wo;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int d = 0; d < 4; ++d) {
+        const uint4 u = __ldg(in + ((b * H + 2 * oy + (d >> 1)) * W + 2 * ox + (d & 1)) * C8 + c);
+        const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&u);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = __bfloat1622float2(p2[e]);
+            acc[2 * e] += f.x;
+            acc[2 * e + 1] += f.y;
+        }
+    }
+    out[gid] = make_uint4(pack_bf16x2(0.25f * acc[0], 0.25f * acc[1]), pack_bf16x2(0.25f * acc[2], 0.25f * acc[3]),
+                          pack_bf16x2(0.25f * acc[4], 0.25f * acc[5]), pack_bf16x2(0.25f * acc[6], 0.25f * acc[7]));
+}
+
+void avgpool2_nhwc(const __nv_bfloat16* in, int n, int H, int W, int C, __nv_bfloat16* out, cudaStream_t s) {
+    if (n <= 0) return;
+    if (H % 2 != 0 || W % 2 != 0 || C % 8 != 0) fail(B200_ERR_INTERNAL, "avgpool2: %d x %d x %d", H, W, C);
+    const long long total = (long long)n * (H / 2) * (W / 2) * (C / 8);
+    avgpool2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(reinterpret_cast<const uint4*>(in), n, H, W, C / 8,
+                                                                     reinterpret_cast<uint4*>(out));
+    MB_CUDA(cudaGetLastError());
+}
+
+// One thread = 8 channels of one image: the fp32 mean over the HW pixels, then every token row.
+__global__ void __launch_bounds__(256) attnpool_tokens_kernel(const uint4* __restrict__ x, const float4* __restrict__ pos,
+                                                              int n, int HW, int C8, uint4* __restrict__ out) {
+    const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= (long long)n * C8) return;
+    const int c = (int)(gid % C8);
+    const long long b = gid / C8;
+    const uint4* src = x + b * HW * C8 + c;
+    uint4* dst = out + b * (HW + 1) * C8 + c;
+    float mean[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int s = 0; s < HW; ++s) {
+        const uint4 u = __ldg(src + (long long)s * C8);
+        const __nv_bfloat162* p2 = reinterpret_cast<const __nv_bfloat162*>(&u);
+        const float4 p0 = __ldg(pos + (long long)(1 + s) * 2 * C8 + 2 * c), p1 = __ldg(pos + (long long)(1 + s) * 2 * C8 + 2 * c + 1);
+        const float pv[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
+        float v[8];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = __bfloat1622float2(p2[e]);
+            mean[2 * e] += f.x;
+            mean[2 * e + 1] += f.y;
+            v[2 * e] = f.x + pv[2 * e];
+            v[2 * e + 1] = f.y + pv[2 * e + 1];
+        }
+        dst[(long long)(1 + s) * C8] = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
+                                                  pack_bf16x2(v[6], v[7]));
+    }
+    const float4 p0 = __ldg(pos + 2 * c), p1 = __ldg(pos + 2 * c + 1);
+    const float pv[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
+    float v[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = mean[e] / (float)HW + pv[e];
+    dst[0] = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+}
+
+void attnpool_tokens(const __nv_bfloat16* x, const float* pos, int n, int HW, int C, __nv_bfloat16* out, cudaStream_t s) {
+    if (n <= 0) return;
+    if (C % 8 != 0) fail(B200_ERR_INTERNAL, "attnpool_tokens: C = %d must be a multiple of 8", C);
+    const long long total = (long long)n * (C / 8);
+    attnpool_tokens_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
+        reinterpret_cast<const uint4*>(x), reinterpret_cast<const float4*>(pos), n, HW, C / 8, reinterpret_cast<uint4*>(out));
     MB_CUDA(cudaGetLastError());
 }
 

@@ -61,10 +61,22 @@ void resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst
 // The same resampling squashed to S x S (x and y scaled independently, no crop): PIL resize((S, S), BICUBIC).
 void resize_squash_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s);
 
-// SigLIP MAP pooling attention, one latent query per head: out[b, h*64 .. h*64+63] = softmax_s(q_h . k_{b,s} / 8) v_{b,s}
-// (bf16).  q fp32 [W] (shared by every image); kv bf16 [n*S, 2W] (K columns, then V columns, head-major); head_dim 64.
-void map_attention(const float* q, const __nv_bfloat16* kv, int n, int S, int W, int heads, __nv_bfloat16* out,
-                   cudaStream_t s);
+// Single-query attention pooling, one query per head: out[b, h*64 .. h*64+63] = softmax_s(q_h . k_{b,s} / 8) v_{b,s}
+// (bf16).  q fp32, image b's query at q + b * q_stride: q_stride 0 shares one query (SigLIP's latent), W gives one per
+// image (the ResNet attention pool's mean token); kv bf16 [n*S, 2W] (K columns, then V columns, head-major); head_dim 64.
+void map_attention(const float* q, long long q_stride, const __nv_bfloat16* kv, int n, int S, int W, int heads,
+                   __nv_bfloat16* out, cudaStream_t s);
+
+// ResNet stem conv1 (3 x 3, stride 2, padding 1, 3 input channels) as an im2col A matrix: bf16 [n * (S/2)^2, 64], row =
+// output pixel, k = (3 ky + kx) * 3 + c, zero for k >= 27.  Input: uint8 HWC [n, S, S, 3] normalised as the patch
+// gather does (u8 != NULL), or already-normalised fp32 CHW [n, 3, S, S].  Taps outside the image are 0.
+void stem_im2col(const uint8_t* u8, const float* chw, int n, int S, const float* mean, const float* std,
+                 __nv_bfloat16* out, cudaStream_t s);
+// AvgPool2d(2) over NHWC bf16 [n, H, W, C] -> [n, H/2, W/2, C] (H, W even, C % 8 == 0).
+void avgpool2_nhwc(const __nv_bfloat16* in, int n, int H, int W, int C, __nv_bfloat16* out, cudaStream_t s);
+// ResNet attention-pool tokens: x NHWC bf16 [n, HW, C] -> out bf16 [n * (HW + 1), C], row 0 of image b = mean_s x_s +
+// pos[0], row 1 + s = x_s + pos[1 + s]; pos fp32 [HW + 1, C].
+void attnpool_tokens(const __nv_bfloat16* x, const float* pos, int n, int HW, int C, __nv_bfloat16* out, cudaStream_t s);
 
 // out[b] = src[b] / |src[b]| if normalize (no epsilon: abstract_clip_model.py:83-85), else src[b]; rows of E floats.
 void l2_rows(const float* src, int n, int E, int normalize, float* out, cudaStream_t s);

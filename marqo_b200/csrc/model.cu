@@ -1,5 +1,5 @@
-// Encoder runtime: CLIP ViT image tower, CLIP text tower, SigLIP towers, BERT (e5, MiniLM, bge), MPNet, XLM-R
-// (multilingual-e5) — SURVEY §8 a2-a5.
+// Encoder runtime: CLIP ViT image tower, CLIP text tower, SigLIP towers, OpenAI ResNet CLIP image tower, BERT (e5,
+// MiniLM, bge), MPNet, XLM-R (multilingual-e5) — SURVEY §8 a2-a5.
 //
 // What the reference calls (third-party, restated in oracle/encoders.py):
 //   OPEN_CLIP.encode_image / encode_text   src/marqo/core/inference/embedding_models/open_clip_model.py:249-286
@@ -74,6 +74,33 @@ struct TowerW {
     attention::RelBias rel_bias;
 };
 
+// OpenAI ResNet CLIP image tower (open_clip ModifiedResNet, verify): every conv with its BatchNorm folded in at
+// finalize (w' = w g / sqrt(var + eps), b' = beta - mean g / sqrt(var + eps), in double), in the k order of the kernel
+// that runs it (gemm::conv_rows_k).
+struct ConvW {
+    const __nv_bfloat16* w = nullptr;   // bf16 [cout, conv_rows_k(cin, k)]
+    const float* b = nullptr;           // fp32 [cout]
+    int cin = 0, cout = 0, k = 0;
+};
+
+struct BottleneckW {
+    ConvW c1, c2, c3, ds;   // ds: the downsample conv (has_ds)
+    int stride = 1;
+    bool has_ds = false;
+};
+
+// Activations are NHWC bf16 in four buffers of max_batch * per_image elements, which the forward pass rotates through
+// (forward_resnet); fixed pointers, so captured CUDA graphs replay them.
+struct ResnetW {
+    ConvW stem[3];
+    std::vector<BottleneckW> blocks;
+    int C = 0, grid = 0;                 // trunk output channels and side
+    const float* pos = nullptr;          // attnpool.positional_embedding [grid^2 + 1, C]
+    const __nv_bfloat16 *w_kv = nullptr, *w_q = nullptr, *w_c = nullptr;   // [2C, C] (k_proj | v_proj), [C, C], [E, C]
+    const float *b_kv = nullptr, *b_q = nullptr, *b_c = nullptr;
+    DeviceBuffer<__nv_bfloat16> buf[4];
+};
+
 }  // namespace
 
 struct b200_model {
@@ -84,6 +111,7 @@ struct b200_model {
     std::map<std::string, DeviceBuffer<float>> raw;   // uploaded fp32 parameters by checkpoint name
     std::vector<DeviceBuffer<uint8_t>> derived;        // device buffers built from them by b200_model_finalize
     TowerW vision, text;
+    ResnetW resnet;   // B200_ARCH_CLIP_RESNET's image tower (vision.present, vision.tokens = grid^2 + 1)
     // workspaces (sized for max_tokens tokens)
     long long max_tokens = 0;
     DeviceBuffer<float> x;
@@ -326,6 +354,99 @@ void build_siglip_vision(b200_model* m, TowerW& T) {
     P.b_fc2 = param(m, a + "mlp.fc2.bias", w);
 }
 
+// conv + BatchNorm of the ResNet tower -> ConvW (see ConvW)
+ConvW fold_conv_bn(b200_model* m, const std::string& conv, const std::string& bn, int cin, int cout, int k) {
+    const long long nw = (long long)cout * cin * k * k;
+    const std::vector<float> w = to_host(param(m, conv + ".weight", nw), (size_t)nw);
+    const std::vector<float> g = to_host(param(m, bn + ".weight", cout), (size_t)cout);
+    const std::vector<float> beta = to_host(param(m, bn + ".bias", cout), (size_t)cout);
+    const std::vector<float> mean = to_host(param(m, bn + ".running_mean", cout), (size_t)cout);
+    const std::vector<float> var = to_host(param(m, bn + ".running_var", cout), (size_t)cout);
+    std::vector<double> scale((size_t)cout);
+    std::vector<float> bias((size_t)cout);
+    for (int o = 0; o < cout; ++o) {
+        scale[o] = (double)g[o] / std::sqrt((double)var[o] + 1e-5);
+        bias[o] = (float)((double)beta[o] - (double)mean[o] * scale[o]);
+    }
+    const int K = gemm::conv_rows_k(cin, k);
+    std::vector<float> rows((size_t)cout * K);
+    gemm::conv_weight_rows(w.data(), cout, cin, k, scale.data(), rows.data());
+    // Both copies go on the model's stream: a cudaMemcpy from pageable memory may return before its DMA lands, and the
+    // conversion below runs on the (non-blocking) model stream, which would not wait for it.
+    DeviceBuffer<float> tmp(rows.size());
+    MB_CUDA(cudaMemcpyAsync(tmp.get(), rows.data(), rows.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    __nv_bfloat16* wb = derived_buffer<__nv_bfloat16>(m, rows.size());
+    kernels::f32_to_bf16(tmp.get(), wb, (long long)rows.size(), m->stream);
+    float* db = derived_buffer<float>(m, bias.size());
+    MB_CUDA(cudaMemcpyAsync(db, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    MB_CUDA(cudaStreamSynchronize(m->stream));
+    m->raw.erase(conv + ".weight");
+    ConvW c;
+    c.w = wb;
+    c.b = db;
+    c.cin = cin;
+    c.cout = cout;
+    c.k = k;
+    return c;
+}
+
+// The ResNet tower's folded weights, the attention pool and the activation buffers (ResnetW).
+void build_resnet(b200_model* m, TowerW& T) {
+    ResnetW& R = m->resnet;
+    const b200_model_desc& d = m->desc;
+    const int width = d.resnet_width, S = d.resnet_image_size, E = d.embed_dim;
+    const std::string v = "visual.";
+    R.stem[0] = fold_conv_bn(m, v + "conv1", v + "bn1", 3, width / 2, 3);
+    R.stem[1] = fold_conv_bn(m, v + "conv2", v + "bn2", width / 2, width / 2, 3);
+    R.stem[2] = fold_conv_bn(m, v + "conv3", v + "bn3", width / 2, width, 3);
+    // per_image: the largest activation of one image (stem im2col rows are 64 wide)
+    long long H = S / 4, per_image = (long long)(S / 2) * (S / 2) * std::max(64, width);
+    int inplanes = width;
+    for (int s = 0; s < 4; ++s) {
+        const int planes = width << s;
+        for (int i = 0; i < d.resnet_layers[s]; ++i) {
+            const std::string p = v + "layer" + std::to_string(s + 1) + "." + std::to_string(i) + ".";
+            BottleneckW B;
+            B.stride = i == 0 && s > 0 ? 2 : 1;
+            B.c1 = fold_conv_bn(m, p + "conv1", p + "bn1", inplanes, planes, 1);
+            B.c2 = fold_conv_bn(m, p + "conv2", p + "bn2", planes, planes, 3);
+            B.c3 = fold_conv_bn(m, p + "conv3", p + "bn3", planes, 4 * planes, 1);
+            B.has_ds = B.stride > 1 || inplanes != 4 * planes;
+            if (B.has_ds) B.ds = fold_conv_bn(m, p + "downsample.0", p + "downsample.1", inplanes, 4 * planes, 1);
+            per_image = std::max({per_image, H * H * inplanes, H * H * planes});
+            H /= B.stride;
+            per_image = std::max(per_image, H * H * 4 * planes);
+            inplanes = 4 * planes;
+            R.blocks.push_back(B);
+        }
+    }
+    R.C = inplanes;
+    R.grid = (int)H;
+    const long long C = R.C, tokens = H * H + 1;
+    T.grid = (int)H;
+    T.tokens = (int)tokens;
+    per_image = std::max(per_image, tokens * 2 * C);   // the K|V rows (the tokens and the fp32 query are smaller)
+    const std::string a = v + "attnpool.";
+    R.pos = param(m, a + "positional_embedding", tokens * C);
+    __nv_bfloat16* wkv = derived_buffer<__nv_bfloat16>(m, (size_t)(2 * C * C));
+    float* bkv = derived_buffer<float>(m, (size_t)(2 * C));
+    const char* kv_names[2] = {"k_proj", "v_proj"};
+    for (int j = 0; j < 2; ++j) {
+        kernels::f32_to_bf16(param(m, a + kv_names[j] + ".weight", C * C), wkv + (size_t)j * C * C, C * C, m->stream);
+        MB_CUDA(cudaMemcpyAsync(bkv + (size_t)j * C, param(m, a + kv_names[j] + ".bias", C), (size_t)C * 4,
+                                cudaMemcpyDeviceToDevice, m->stream));
+    }
+    MB_CUDA(cudaStreamSynchronize(m->stream));
+    for (int j = 0; j < 2; ++j) m->raw.erase(a + kv_names[j] + ".weight");
+    R.w_kv = wkv;
+    R.b_kv = bkv;
+    R.w_q = to_bf16(m, a + "q_proj.weight", C * C);
+    R.b_q = param(m, a + "q_proj.bias", C);
+    R.w_c = to_bf16(m, a + "c_proj.weight", (long long)E * C);
+    R.b_c = param(m, a + "c_proj.bias", E);
+    for (auto& b : R.buf) b = DeviceBuffer<__nv_bfloat16>((size_t)d.max_batch * per_image);
+}
+
 struct Counter {
     int n = 0;
 };
@@ -459,6 +580,97 @@ void head_linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K
     linear(m, c, A, M, K, W, N, e);
 }
 
+// One folded ResNet conv over n images of H x H output pixels (NHWC bf16 x -> out): bias, then ReLU with the optional
+// bf16 residual added before it, or neither.  The stem conv (cin 3) takes stem_im2col's rows as x.
+void resnet_conv(b200_model* m, Counter& c, const ConvW& cw, const __nv_bfloat16* x, int n, int H,
+                 const __nv_bfloat16* residual, bool relu, __nv_bfloat16* out) {
+    gemm::Epilogue e;
+    e.bias = cw.b;
+    e.act = relu ? gemm::ACT_RELU : gemm::ACT_NONE;
+    e.residual = residual;
+    e.ldr = cw.cout;
+    e.out = out;
+    e.ldo = cw.cout;
+    ProfScope ps(m, 0);
+    if (cw.k == 3 && cw.cin != 3) {
+        gemm::ConvGather g;
+        g.act = x;
+        g.n = n;
+        g.H = g.W = H;
+        g.cin = cw.cin;
+        gemm::launch_conv3x3(g, cw.w, cw.cout, e, m->stream);
+    } else {
+        const int K = gemm::conv_rows_k(cw.cin, cw.k);
+        gemm::launch(x, K, cw.w, n * H * H, cw.cout, K, e, m->sms, m->stream);
+    }
+    ++c.n;
+}
+
+// The ResNet CLIP image tower over n images (uint8 HWC u8 or normalised fp32 CHW f32, at the model's size): buffers
+// A B C D rotate so that every block starts and ends in A.
+void forward_resnet(b200_model* m, Counter& c, const uint8_t* u8, const float* f32, int n, int normalize, float* d_out) {
+    ResnetW& R = m->resnet;
+    const b200_model_desc& d = m->desc;
+    __nv_bfloat16 *A = R.buf[0].get(), *B = R.buf[1].get(), *Cb = R.buf[2].get(), *D = R.buf[3].get();
+    const int S = d.resnet_image_size, width = d.resnet_width;
+    int H = S / 2;
+    kernels::stem_im2col(u8, f32, n, S, d.image_mean, d.image_std, B, m->stream);
+    resnet_conv(m, c, R.stem[0], B, n, H, nullptr, true, Cb);
+    resnet_conv(m, c, R.stem[1], Cb, n, H, nullptr, true, D);
+    resnet_conv(m, c, R.stem[2], D, n, H, nullptr, true, Cb);
+    kernels::avgpool2_nhwc(Cb, n, H, H, width, A, m->stream);
+    c.n += 2;
+    H /= 2;
+    for (const BottleneckW& blk : R.blocks) {
+        resnet_conv(m, c, blk.c1, A, n, H, nullptr, true, B);
+        resnet_conv(m, c, blk.c2, B, n, H, nullptr, true, Cb);
+        const __nv_bfloat16 *main = Cb, *identity = A;
+        if (blk.stride > 1) {
+            kernels::avgpool2_nhwc(Cb, n, H, H, blk.c2.cout, B, m->stream);
+            kernels::avgpool2_nhwc(A, n, H, H, blk.c1.cin, Cb, m->stream);
+            c.n += 2;
+            H /= 2;
+            main = B;
+            resnet_conv(m, c, blk.ds, Cb, n, H, nullptr, false, D);
+            identity = D;
+        } else if (blk.has_ds) {
+            resnet_conv(m, c, blk.ds, A, n, H, nullptr, false, D);
+            identity = D;
+        }
+        // in place over the identity when it is A: a tile reads the residual rows and columns it writes, nothing else
+        resnet_conv(m, c, blk.c3, main, n, H, identity, true, A);
+    }
+    // attention pool: tokens [mean; pixels] + pos -> B; K|V of every token -> Cb; q of token 0 (rows T C apart) -> D;
+    // one query per image and head -> A; c_proj -> pooled; L2
+    const int C = R.C, HW = R.grid * R.grid, T = HW + 1, E = d.embed_dim;
+    kernels::attnpool_tokens(A, R.pos, n, HW, C, B, m->stream);
+    ++c.n;
+    float* q = reinterpret_cast<float*>(D);
+    {
+        ProfScope ps(m, 0);
+        gemm::Epilogue e;
+        e.bias = R.b_kv;
+        e.out = Cb;
+        e.ldo = 2 * C;
+        gemm::launch(B, C, R.w_kv, n * T, 2 * C, C, e, m->sms, m->stream);
+        gemm::Epilogue eq;
+        eq.bias = R.b_q;
+        eq.out = q;
+        eq.ldo = C;
+        eq.out_fp32 = 1;
+        gemm::launch(B, T * C, R.w_q, n, C, C, eq, m->sms, m->stream);
+        c.n += 2;
+    }
+    {
+        ProfScope ps(m, 1);
+        kernels::map_attention(q, C, Cb, n, T, C, d.resnet_heads, A, m->stream);
+        ++c.n;
+    }
+    head_linear(m, c, A, n, C, R.w_c, E, R.b_c, gemm::ACT_NONE, m->pooled.get(), true, false);
+    kernels::l2_rows(m->pooled.get(), n, E, normalize, d_out, m->stream);
+    ++c.n;
+}
+
 // SigLIP vision head over the n * S token rows in x: final LayerNorm of every token -> h, K|V projection -> qkv
 // [n * S, 2w], one latent query per head attending over its image's tokens -> o [n, w], then proj -> pooled (fp32),
 // pooled + MLP(LN(pooled)), optional L2 -> d_out.
@@ -469,7 +681,7 @@ void map_head(b200_model* m, Counter& c, const TowerW& T, int n, int normalize, 
     head_linear(m, c, m->h.get(), M, w, P.w_kv, 2 * w, P.b_kv, gemm::ACT_NONE, m->qkv.get(), false, false);
     {
         ProfScope ps(m, 1);
-        kernels::map_attention(P.q, m->qkv.get(), n, S, w, T.d.heads, m->o.get(), m->stream);
+        kernels::map_attention(P.q, 0, m->qkv.get(), n, S, w, T.d.heads, m->o.get(), m->stream);
     }
     head_linear(m, c, m->o.get(), n, w, P.w_proj, w, P.b_proj, gemm::ACT_NONE, m->pooled.get(), true, false);
     kernels::layernorm(m->pooled.get(), w, P.ln_w, P.ln_b, T.eps, n, w, nullptr, m->h.get(), m->stream);
@@ -482,6 +694,10 @@ void map_head(b200_model* m, Counter& c, const TowerW& T, int n, int normalize, 
 // images already as device uint8 [n, S, S, 3] (u8 != nullptr) or device fp32 CHW (f32 != nullptr)
 void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const float* f32, int n, int normalize,
                           float* d_out) {
+    if (m->desc.arch == B200_ARCH_CLIP_RESNET) {
+        forward_resnet(m, c, u8, f32, n, normalize, d_out);
+        return;
+    }
     const TowerW& T = m->vision;
     const int S = T.d.image_size, p = T.d.patch, w = T.d.width;
     // x = positional embedding (+ class embedding on each image's first row), then conv1 (no bias) of every token row
@@ -535,7 +751,7 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
                           int normalize, float* d_out) {
     const TowerW& T = m->text;
     const int w = T.d.width;
-    if (m->desc.arch == B200_ARCH_CLIP) {
+    if (m->desc.arch == B200_ARCH_CLIP || m->desc.arch == B200_ARCH_CLIP_RESNET) {
         kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, m->x.get(), m->aux.get(), m->stream);
         c.n += 1;
         run_clip_blocks(m, c, T, n, S, attention::MASK_CAUSAL);
@@ -698,19 +914,34 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         *out = nullptr;
         require_sm90_device(device);
         MB_CHECK_ARG(desc->arch == B200_ARCH_CLIP || desc->arch == B200_ARCH_BERT || desc->arch == B200_ARCH_MPNET ||
-                         desc->arch == B200_ARCH_SIGLIP || desc->arch == B200_ARCH_XLMR,
+                         desc->arch == B200_ARCH_SIGLIP || desc->arch == B200_ARCH_XLMR ||
+                         desc->arch == B200_ARCH_CLIP_RESNET,
                      "unknown arch %d", desc->arch);
         MB_CHECK_ARG(desc->max_batch > 0, "max_batch must be positive");
         MB_CHECK_ARG(desc->embed_dim > 0 && desc->embed_dim <= 4096, "embed_dim out of range");
         const bool siglip = desc->arch == B200_ARCH_SIGLIP;
-        const bool has_vision = (desc->arch == B200_ARCH_CLIP || siglip) && desc->vision.layers > 0;
+        const bool resnet = desc->arch == B200_ARCH_CLIP_RESNET;
+        const bool has_vision = ((desc->arch == B200_ARCH_CLIP || siglip) && desc->vision.layers > 0) ||
+                                (resnet && desc->resnet_layers[0] > 0);
         if (siglip) {
             MB_CHECK_ARG(desc->layer_norm_eps > 0.f, "SigLIP: layer_norm_eps must be positive");
             MB_CHECK_ARG(desc->embed_dim % 32 == 0, "SigLIP: embed_dim %d must be a multiple of 32", desc->embed_dim);
         }
         const bool has_text = desc->text.layers > 0;
         MB_CHECK_ARG(has_vision || has_text, "model has no tower");
-        if (has_vision) {
+        if (has_vision && resnet) {
+            const int wd = desc->resnet_width, S = desc->resnet_image_size;
+            for (int s = 0; s < 4; ++s)
+                MB_CHECK_ARG(desc->resnet_layers[s] > 0 && desc->resnet_layers[s] <= 64, "resnet_layers[%d] = %d out of range",
+                             s, desc->resnet_layers[s]);
+            // the stem's 3 x 3 convs gather width / 2 channels: a power of two >= 32
+            MB_CHECK_ARG(wd >= 64 && wd <= 128 && (wd & (wd - 1)) == 0, "resnet_width %d must be 64 or 128", wd);
+            MB_CHECK_ARG(S > 0 && S % 32 == 0 && S <= 512, "resnet_image_size %d must be a multiple of 32, <= 512", S);
+            MB_CHECK_ARG(desc->resnet_heads * 64 == 32 * wd, "attention pool: head_dim must be 64 (%d channels, %d heads)",
+                         32 * wd, desc->resnet_heads);
+            MB_CHECK_ARG(desc->embed_dim % 32 == 0, "CLIP ResNet: embed_dim %d must be a multiple of 32", desc->embed_dim);
+            for (int i = 0; i < 3; ++i) MB_CHECK_ARG(desc->image_std[i] > 0.f, "image_std must be positive");
+        } else if (has_vision) {
             check_tower(desc->vision, "vision");
             MB_CHECK_ARG(desc->vision.patch > 0 && desc->vision.image_size % desc->vision.patch == 0,
                          "image_size must be a multiple of patch");
@@ -727,7 +958,7 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         if (has_text) {
             check_tower(desc->text, "text");
             MB_CHECK_ARG(desc->text.ctx > 0 && desc->text.vocab > 0, "text.ctx and text.vocab must be positive");
-            if (desc->arch != B200_ARCH_CLIP && !siglip)
+            if (desc->arch != B200_ARCH_CLIP && !siglip && !resnet)
                 MB_CHECK_ARG(desc->embed_dim == desc->text.width, "BERT / MPNet / XLM-R embed_dim must equal width");
             if (desc->arch == B200_ARCH_MPNET) {
                 MB_CHECK_ARG(desc->text.width == desc->text.heads * 64, "MPNet: head_dim must be 64 (width %d, heads %d)",
@@ -758,6 +989,7 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         m->ev1 = make_event();
         m->vision.present = has_vision;
         m->vision.d = desc->vision;
+        if (resnet) m->vision.d.image_size = desc->resnet_image_size;
         m->text.present = has_text;
         m->text.d = desc->text;
         gemm::configure();
@@ -799,7 +1031,12 @@ int b200_model_finalize(b200_model* m) {
         long long max_tok = 0, max_w = 0, max_mlp = 0;
         const bool siglip = m->desc.arch == B200_ARCH_SIGLIP;
         if (siglip) m->vision.eps = m->text.eps = m->desc.layer_norm_eps;
-        if (m->vision.present) {
+        if (m->vision.present && m->desc.arch == B200_ARCH_CLIP_RESNET) {
+            TowerW& T = m->vision;
+            build_resnet(m, T);
+            max_tok = std::max(max_tok, (long long)m->desc.max_batch * T.tokens);
+            m->resized = DeviceBuffer<uint8_t>((size_t)m->desc.max_batch * T.d.image_size * T.d.image_size * 3);
+        } else if (m->vision.present) {
             TowerW& T = m->vision;
             const long long w = T.d.width, p = T.d.patch;
             T.grid = T.d.image_size / T.d.patch;
@@ -837,7 +1074,7 @@ int b200_model_finalize(b200_model* m) {
             TowerW& T = m->text;
             const long long w = T.d.width;
             T.max_pos = T.d.ctx;
-            if (m->desc.arch == B200_ARCH_CLIP) {
+            if (m->desc.arch == B200_ARCH_CLIP || m->desc.arch == B200_ARCH_CLIP_RESNET) {
                 T.tok = param(m, "token_embedding.weight", (long long)T.d.vocab * w);
                 T.pos = param(m, "positional_embedding", (long long)T.d.ctx * w);
                 build_preln_layers(m, T, "transformer.resblocks.", OPEN_CLIP_BLOCK);
@@ -883,7 +1120,7 @@ int b200_model_finalize(b200_model* m) {
             max_mlp = std::max(max_mlp, (long long)T.d.mlp);
         }
         // cap the workspace at ~24 GB of activations: larger calls are processed in sub-batches
-        const long long bytes_per_tok = max_w * (4 + 2 + 6 + 2) + max_mlp * 2;
+        const long long bytes_per_tok = std::max<long long>(1, max_w * (4 + 2 + 6 + 2) + max_mlp * 2);
         const long long cap_tok = (24LL << 30) / bytes_per_tok;
         m->max_tokens = std::min(max_tok, std::max<long long>(cap_tok, 1024));
         m->x = DeviceBuffer<float>((size_t)m->max_tokens * max_w);
@@ -959,7 +1196,7 @@ int b200_model_encode_tokens(b200_model* m, const int32_t* ids, const int32_t* a
         require_ready(m);
         MB_CHECK_ARG(ids && out, "NULL buffer");
         check_tokens_args(m, n, seq);
-        if (attn_mask && m->desc.arch != B200_ARCH_CLIP) {
+        if (attn_mask && m->desc.arch != B200_ARCH_CLIP && m->desc.arch != B200_ARCH_CLIP_RESNET) {
             // the kernels implement prefix (right-padded) masks, which is what the tokenizer call at
             // hugging_face_model.py:179-185 produces
             for (int b = 0; b < n; ++b) {

@@ -21,6 +21,11 @@ __device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
 __device__ __forceinline__ void st_shared_f32x2(uint32_t addr, float x, float y) {
     asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
 }
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
 __device__ __forceinline__ float2 ld_shared_f32x2(uint32_t addr) {
     float2 v;
     asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");

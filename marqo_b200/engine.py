@@ -289,11 +289,13 @@ def _to_numpy_f32(t) -> np.ndarray:
 
 
 class Encoder:
-    """A CLIP or SigLIP (vision + text towers), BERT, MPNet or XLM-R encoder resident on one GPU.
+    """A CLIP, ResNet CLIP or SigLIP (vision + text towers), BERT, MPNet or XLM-R encoder resident on one GPU.
 
     `config` keys — CLIP: embed_dim, act ("gelu"|"quickgelu"), mean, std, vision{width,layers,heads,mlp,patch,
     image_size}, text{width,layers,heads,mlp,ctx,vocab};  SigLIP: the CLIP keys plus ln_eps (embed_dim == vision
-    width);  BERT: width, layers, heads, mlp, vocab, max_pos, type_vocab,
+    width);  ResNet CLIP ("clip_resnet"): embed_dim, act, mean, std, the text tower's width, layers, heads, mlp, ctx,
+    vocab at the top level (layers 0: no text tower), resnet{layers [4], width, heads, image_size} (None: no image
+    tower);  BERT: width, layers, heads, mlp, vocab, max_pos, type_vocab,
     pool ("mean"|"cls");  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
     max_pos - pad_id - 1 tokens), pad_id, ln_eps, rel_buckets, rel_max_distance, pool;  XLM-R: width, layers, heads,
     mlp, vocab, max_pos (as MPNet), pad_id, ln_eps, pool.  `weights` maps checkpoint parameter names (open_clip
@@ -324,6 +326,23 @@ class Encoder:
             if t:
                 d.text = N.TowerDesc(t["width"], t["layers"], t["heads"], t["mlp"], t["ctx"], t["vocab"], 0, 0)
             self.image_size = v.get("image_size", 224) if v else 0
+        elif arch == "clip_resnet":
+            d.arch = N.ARCH_CLIP_RESNET
+            d.embed_dim = int(config["embed_dim"])
+            d.act = N.ACT_QUICKGELU if config.get("act", "gelu") == "quickgelu" else N.ACT_GELU
+            for i in range(3):
+                d.image_mean[i] = float(np.float32(config["mean"][i]))
+                d.image_std[i] = float(np.float32(config["std"][i]))
+            r = config.get("resnet")
+            if r:
+                for i in range(4):
+                    d.resnet_layers[i] = int(r["layers"][i])
+                d.resnet_width, d.resnet_heads = int(r["width"]), int(r["heads"])
+                d.resnet_image_size = int(r.get("image_size", 224))
+            if config.get("layers"):
+                d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"], config["ctx"],
+                                     config["vocab"], 0, 0)
+            self.image_size = int(r.get("image_size", 224)) if r else 0
         elif arch == "bert":
             d.arch = N.ARCH_BERT
             d.embed_dim = int(config["width"])
@@ -638,12 +657,37 @@ def debug_resize_squash(hwc, S: int, device: int = 0) -> np.ndarray:
 
 
 def debug_map_attention(q, kv, B: int, S: int, H: int, device: int = 0) -> np.ndarray:
-    """SigLIP's MAP pooling attention: q fp32 [W] (one latent query), kv [B * S, 2W] (K then V columns, rounded to
-    bf16) -> fp32 [B, W], softmax(q_h k_h^T / 8) v_h per image and head (rounded to bf16)."""
+    """Single-query attention pooling: q fp32 [W] (SigLIP's one latent query, shared by every image) or [B, W] (one
+    query per image, the ResNet attention pool), kv [B * S, 2W] (K then V columns, rounded to bf16) -> fp32 [B, W],
+    softmax(q_h k_h^T / 8) v_h per image and head (rounded to bf16)."""
     qa, kva = _as(q, np.float32), _as(kv, np.float32)
-    W = qa.shape[0]
+    W = qa.shape[-1]
+    if qa.ndim not in (1, 2) or (qa.ndim == 2 and qa.shape[0] != B):
+        raise ValueError(f"expected q [{W}] or [{B}, {W}], got {qa.shape}")
     if kva.shape != (B * S, 2 * W):
         raise ValueError(f"expected kv [{B * S}, {2 * W}], got {kva.shape}")
     out = np.empty((B, W), np.float32)
-    N.check(N.load().b200_debug_map_attention(device, _ptr(qa), _ptr(kva), B, S, W, H, _ptr(out)))
+    fn = N.load().b200_debug_map_attention if qa.ndim == 1 else N.load().b200_debug_map_attention_per_image
+    N.check(fn(device, _ptr(qa), _ptr(kva), B, S, W, H, _ptr(out)))
+    return out
+
+
+def debug_conv2d(x, w, bias=None, residual=None, relu: bool = True, device: int = 0) -> np.ndarray:
+    """One convolution of the ResNet CLIP image tower on the path the model runs it: x NHWC fp32 [n, H, W, cin], w
+    [cout, cin, k, k] (torch layout), bias [cout] -> NHWC [n, Ho, Wo, cout] rounded to bf16: relu(conv + bias
+    (+ residual)), or conv + bias without relu (1 x 1 and stem convs, no residual).  cin 3 is the stem conv (3 x 3, stride 2, padding 1);
+    otherwise k 1 or 3 (stride 1, padding 1).  Operands are rounded to bf16 on the device."""
+    xa, wa = _as(x, np.float32), _as(w, np.float32)
+    n, H, W, cin = xa.shape
+    cout, k = wa.shape[0], wa.shape[2]
+    if wa.shape != (cout, cin, k, k):
+        raise ValueError(f"expected w [cout, {cin}, k, k], got {wa.shape}")
+    Ho, Wo = (H // 2, W // 2) if cin == 3 else (H, W)
+    b = None if bias is None else _as(bias, np.float32)
+    r = None if residual is None else _as(residual, np.float32)
+    if r is not None and r.shape != (n, Ho, Wo, cout):
+        raise ValueError(f"expected residual [{n}, {Ho}, {Wo}, {cout}], got {r.shape}")
+    out = np.empty((n, Ho, Wo, cout), np.float32)
+    N.check(N.load().b200_debug_conv2d(device, _ptr(xa), n, H, W, cin, _ptr(wa), cout, k, _ptr(b), _ptr(r), int(relu),
+                                       _ptr(out)))
     return out

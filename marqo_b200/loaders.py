@@ -33,6 +33,7 @@ def _resolve_weights(props: dict, arch: dict, kind: str) -> Dict[str, np.ndarray
     if w is None and props.get("random_init") is not None:
         seed = int(props["random_init"])
         random = {"clip": weights_mod.random_clip_weights, "siglip": weights_mod.random_siglip_weights,
+                  "clip_resnet": weights_mod.random_clip_resnet_weights,
                   "bert": weights_mod.random_bert_weights, "mpnet": weights_mod.random_mpnet_weights,
                   "xlmr": weights_mod.random_xlmr_weights}[kind]
         return random(arch, seed)
@@ -91,7 +92,8 @@ class B200OpenCLIP:
             arch = dict(arch, std=tuple(props["std"]))
         self.arch = arch
         # "siglip" (model_registry.SIGLIP_MODELS): the engine's SigLIP runtime, whose GPU resize squashes images to
-        # S x S; otherwise open_clip CLIP, shortest side -> S + centre crop
+        # S x S; "clip_resnet" (RESNET_MODELS): OpenAI's ResNet CLIP; otherwise open_clip CLIP; both shortest side -> S
+        # + centre crop
         kind = arch.get("kind", "clip")
         self.model = Encoder(kind, arch, _resolve_weights(props, arch, kind), device=_validate_device(self.device),
                              max_batch=int(props.get("max_batch", 256)))
@@ -101,7 +103,9 @@ class B200OpenCLIP:
     def _default_tokenizer(self):
         if self.model_properties.get("merges_file"):
             from .tokenizers import ClipBpeTokenizer
-            return ClipBpeTokenizer(self.model_properties["merges_file"], context_length=int(self.arch["text"]["ctx"]))
+            # the CLIP text tower's ctx: in its "text" block, or at the top level of a clip_resnet arch
+            ctx = self.arch["ctx"] if self.arch.get("kind") == "clip_resnet" else self.arch["text"]["ctx"]
+            return ClipBpeTokenizer(self.model_properties["merges_file"], context_length=int(ctx))
         try:
             import open_clip  # type: ignore
             return open_clip.get_tokenizer(self.model_properties.get("name", "").split("/")[1])

@@ -49,7 +49,17 @@ offline (verify):
     multilingual-e5-small             a BertModel (Multilingual-MiniLM-L12-H384, `arch["kind"]` absent): width 384,
                                       12 layers, 12 heads, mlp 1536, vocabulary 250037, 512 positions, 2 token types,
                                       layer_norm_eps 1e-12; it runs the BERT runtime unchanged
-All four mean-pool the last hidden state and erf-GELU their MLPs."""
+All four mean-pool the last hidden state and erf-GELU their MLPs.
+
+The OpenAI ResNet CLIP entries (model_registry.py:80-126) live in RESNET_MODELS (`arch["kind"] == "clip_resnet"`),
+served by the `b200_open_clip` loader.  Their shapes come from open_clip 2.24.0's model_configs/RN50.json, RN101.json
+and `ModifiedResNet`, which cannot be re-read offline (verify): image 224, width 64, stages of [3, 4, 6, 3] (RN50) or
+[3, 4, 23, 3] (RN101) Bottlenecks, a 7 x 7 x 2048 trunk output and an attention pool of 32 heads (head_dim 64) whose
+output is embed_dim wide (1024 / 512); the CLIP text tower (width 512, 12 layers, 8 heads, mlp 2048, ctx 77, vocab
+49408).  Every `openai` tag loads as QuickGELU (as ViT-B-32/openai does here), the `-quickgelu` names too; the
+yfcc15m / cc12m tags of the plain names run erf-GELU.  OpenAI mean and std, shortest side -> 224 + centre crop.  The
+arch block has no "vision" key: the text tower's fields sit at the top level, as in the BERT archs, and the CNN in its
+own "resnet" block."""
 from __future__ import annotations
 
 import copy
@@ -228,9 +238,32 @@ def _xlmr_models() -> Dict[str, dict]:
 XLMR_MODELS: Dict[str, dict] = _xlmr_models()
 
 
+def _resnet_arch(layers: list, embed: int, act: str) -> dict:
+    """OpenAI ResNet CLIP (module docstring, verify)."""
+    return {"kind": "clip_resnet", "embed_dim": embed, "act": act, "mean": OPENAI_MEAN, "std": OPENAI_STD,
+            "width": 512, "layers": 12, "heads": 8, "mlp": 2048, "ctx": 77, "vocab": 49408,
+            "resnet": {"layers": list(layers), "width": 64, "heads": 32, "image_size": 224}}
+
+
+def _resnet_models() -> Dict[str, dict]:
+    m: Dict[str, dict] = {}
+    for model, layers, embed, tags in (("RN50", [3, 4, 6, 3], 1024, ("openai", "yfcc15m", "cc12m")),
+                                       ("RN101", [3, 4, 23, 3], 512, ("openai", "yfcc15m"))):
+        for variant in (model, f"{model}-quickgelu"):
+            for tag in tags:
+                act = "quickgelu" if tag == "openai" or variant.endswith("-quickgelu") else "gelu"
+                name = f"open_clip/{variant}/{tag}"
+                m[name] = {"name": name, "dimensions": embed, "note": "open_clip models", "type": TYPE_OPEN_CLIP,
+                           "pretrained": tag, "arch": _resnet_arch(layers, embed, act)}
+    return m
+
+
+RESNET_MODELS: Dict[str, dict] = _resnet_models()
+
+
 def find_model(model_name: str) -> Optional[dict]:
     """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
-    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS):
+    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS):
         entry = table.get(model_name)
         if entry is not None:
             return entry
@@ -239,7 +272,7 @@ def find_model(model_name: str) -> Optional[dict]:
 
 def all_models() -> Dict[str, dict]:
     """Every served registry entry by name (a new dict over the same entries)."""
-    return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS}
+    return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS, **RESNET_MODELS}
 
 
 def get_model_properties(model_name: str) -> dict:

@@ -156,6 +156,55 @@ def random_siglip_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]
     return sd
 
 
+def _bn(g, prefix, c, sd):
+    sd[prefix + ".weight"] = _vec(g, c, 0.1, 1.0)
+    sd[prefix + ".bias"] = _vec(g, c)
+    sd[prefix + ".running_mean"] = _vec(g, c)
+    sd[prefix + ".running_var"] = (0.5 + g.random(c, dtype=np.float32)).astype(np.float32)
+
+
+def _conv(g, cout, cin, k):
+    return g.standard_normal((cout, cin, k, k), dtype=np.float32) / np.float32(math.sqrt(cin * k * k))
+
+
+def random_clip_resnet_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
+    """Seeded random weights under open_clip's ModifiedResNet CLIP names (arch: the registry's clip_resnet block;
+    arch["resnet"] None: no image tower, arch["layers"] 0: no text tower)."""
+    g = _rng(seed)
+    sd: Dict[str, np.ndarray] = {}
+    r, E = arch.get("resnet"), arch["embed_dim"]
+    if r:
+        w, v = r["width"], "visual."
+        for i, (cin, cout) in enumerate(((3, w // 2), (w // 2, w // 2), (w // 2, w)), start=1):
+            sd[f"{v}conv{i}.weight"] = _conv(g, cout, cin, 3)
+            _bn(g, f"{v}bn{i}", cout, sd)
+        inplanes = w
+        for s, depth in enumerate(r["layers"]):
+            planes = w << s
+            for i in range(depth):
+                p = f"{v}layer{s + 1}.{i}."
+                for j, (cin, cout, k) in enumerate(((inplanes, planes, 1), (planes, planes, 3), (planes, 4 * planes, 1)),
+                                                   start=1):
+                    sd[f"{p}conv{j}.weight"] = _conv(g, cout, cin, k)
+                    _bn(g, f"{p}bn{j}", cout, sd)
+                if i == 0:   # stride 2 (stages 2-4) or 64 -> 256 channels (stage 1): a downsample branch
+                    sd[f"{p}downsample.0.weight"] = _conv(g, 4 * planes, inplanes, 1)
+                    _bn(g, f"{p}downsample.1", 4 * planes, sd)
+                inplanes = 4 * planes
+        C, grid = 32 * w, r.get("image_size", 224) // 32
+        a = f"{v}attnpool."
+        sd[a + "positional_embedding"] = g.standard_normal((grid * grid + 1, C), dtype=np.float32) / np.float32(
+            math.sqrt(C))
+        for nm, out_f in (("q_proj", C), ("k_proj", C), ("v_proj", C), ("c_proj", E)):
+            sd[f"{a}{nm}.weight"] = _lin(g, out_f, C)
+            sd[f"{a}{nm}.bias"] = _vec(g, out_f)
+    if arch.get("layers"):
+        t = {k: arch[k] for k in ("width", "layers", "heads", "mlp", "ctx", "vocab")}
+        text = random_clip_weights({"embed_dim": E, "text": t}, seed + 1)
+        sd.update(text)
+    return sd
+
+
 def random_bert_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     g = _rng(seed)
     w, mlp = arch["width"], arch["mlp"]
