@@ -250,7 +250,7 @@ int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16,
             fill_f32_kernel<<<(unsigned)((no + 255) / 256), 256, 0, sc.s>>>(dOut, no, 4242u);
             ep.out = dOut;
             ep.out_fp32 = 1;
-            if (residual_in_place) {   // residual == out, as run_clip_blocks updates x
+            if (residual_in_place) {   // residual == out, as run_layers updates x
                 ep.residual = dOut;
                 ep.ldr = N;
             }
@@ -443,6 +443,7 @@ int b200_debug_conv2d(int device, const float* x, int n, int H, int W, int cin, 
         __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>(out_n);
         e.out = dO;
         e.ldo = cout;
+        const __nv_bfloat16* dX;
         if (cin == 3) {   // the stem: from already-normalised fp32 CHW, as b200_model_encode_images_f32 runs it
             std::vector<float> chw((size_t)n * 3 * H * W);
             for (int b = 0; b < n; ++b)
@@ -452,19 +453,11 @@ int b200_debug_conv2d(int device, const float* x, int n, int H, int W, int cin, 
             __nv_bfloat16* dA = sc.alloc<__nv_bfloat16>((size_t)n * Ho * Wo * 64);
             const float mean[3] = {0.f, 0.f, 0.f}, std1[3] = {1.f, 1.f, 1.f};
             kernels::stem_im2col(nullptr, dchw, n, H, mean, std1, dA, sc.s);
-            gemm::launch(dA, K, dW, n * Ho * Wo, cout, K, e, sm_count(device), sc.s);
-        } else if (k == 3) {
-            gemm::ConvGather cg;
-            cg.act = sc.upload_bf16(x, (size_t)n * H * W * cin);
-            cg.n = n;
-            cg.H = H;
-            cg.W = W;
-            cg.cin = cin;
-            gemm::launch_conv3x3(cg, dW, cout, e, sc.s);
+            dX = dA;
         } else {
-            const __nv_bfloat16* dX = sc.upload_bf16(x, (size_t)n * H * W * cin);
-            gemm::launch(dX, cin, dW, n * H * W, cout, cin, e, sm_count(device), sc.s);
+            dX = sc.upload_bf16(x, (size_t)n * H * W * cin);
         }
+        gemm::launch_conv(dX, n, Ho, Wo, cin, k, dW, cout, e, sm_count(device), sc.s);
         float* dOut = sc.alloc<float>(out_n);
         bf16_to_f32_kernel<<<(unsigned)((out_n + 255) / 256), 256, 0, sc.s>>>(dO, dOut, (long long)out_n);
         MB_CUDA(cudaGetLastError());

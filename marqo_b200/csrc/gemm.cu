@@ -741,8 +741,8 @@ static void launch_persistent(const __nv_bfloat16* A, int lda, const __nv_bfloat
     MB_CUDA(cudaGetLastError());
 }
 
-void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, const Epilogue& ep, cudaStream_t stream) {
-    if (pg.n <= 0 || N <= 0) return;
+int launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, const Epilogue& ep, cudaStream_t stream) {
+    if (pg.n <= 0 || N <= 0) return 0;
     if (pg.S <= 0 || pg.patch <= 0 || pg.S % pg.patch != 0)
         fail(B200_ERR_INTERNAL, "patch gather: image %d is not a multiple of patch %d", pg.S, pg.patch);
     if (N % 32 != 0) fail(B200_ERR_INTERNAL, "patch gather: N = %d must be a multiple of 32", N);
@@ -754,10 +754,11 @@ void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, c
     const long long M = (long long)pg.n * (g * g + pg.cls);
     if (M > 0x7fffffffLL) fail(B200_ERR_INVALID_ARG, "patch gather: batch of %d images is too large", pg.n);
     launch_tiles<PROD_PATCH, true, ACT_NONE>(nullptr, 0, Wg, (int)M, N, patch_gather_k(pg.patch), ep, stream, &pg);
+    return 1;
 }
 
-void launch_conv3x3(const ConvGather& cg, const __nv_bfloat16* Wc, int N, const Epilogue& ep, cudaStream_t stream) {
-    if (cg.n <= 0 || N <= 0) return;
+int launch_conv3x3(const ConvGather& cg, const __nv_bfloat16* Wc, int N, const Epilogue& ep, cudaStream_t stream) {
+    if (cg.n <= 0 || N <= 0) return 0;
     if (cg.H <= 0 || cg.W <= 0 || cg.cin < 32 || (cg.cin & (cg.cin - 1)) != 0)
         fail(B200_ERR_INTERNAL, "conv3x3: %d x %d x %d input (cin must be a power of two >= 32)", cg.H, cg.W, cg.cin);
     if (N % 32 != 0) fail(B200_ERR_INTERNAL, "conv3x3: N = %d must be a multiple of 32", N);
@@ -768,9 +769,25 @@ void launch_conv3x3(const ConvGather& cg, const __nv_bfloat16* Wc, int N, const 
     const long long M = (long long)cg.n * cg.H * cg.W;
     if (M > 0x7fffffffLL) fail(B200_ERR_INVALID_ARG, "conv3x3: batch of %d images is too large", cg.n);
     launch_tiles<PROD_CONV, false, ACT_RELU>(nullptr, 0, Wc, (int)M, N, conv_gather_k(cg.cin), ep, stream, nullptr, &cg);
+    return 1;
 }
 
 int conv_rows_k(int cin, int k) { return cin == 3 ? 64 : k == 1 ? cin : conv_gather_k(cin); }
+
+int launch_conv(const __nv_bfloat16* x, int n, int H, int W, int cin, int k, const __nv_bfloat16* Wc, int cout,
+                const Epilogue& ep, int sms, cudaStream_t stream) {
+    if (k == 3 && cin != 3) {
+        ConvGather g;
+        g.act = x;
+        g.n = n;
+        g.H = H;
+        g.W = W;
+        g.cin = cin;
+        return launch_conv3x3(g, Wc, cout, ep, stream);
+    }
+    const int K = conv_rows_k(cin, k);
+    return launch(x, K, Wc, n * H * W, cout, K, ep, sms, stream) == KERNEL_NONE ? 0 : 1;
+}
 
 void conv_weight_rows(const float* w, int cout, int cin, int k, const double* scale, float* out) {
     const int K = conv_rows_k(cin, k), taps = k * k;

@@ -40,7 +40,7 @@ int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N
 // normalised as ToTensor + Normalize.  cls is 1 for CLIP and 0 for the class-token-free SigLIP tower.  Wg [N,
 // patch_gather_k(patch)] is conv1.weight re-laid by kernels::patch_weight_rows.  No patch matrix exists in HBM: the
 // gather warps of the GEMM read the image rows, convert and write the swizzled smem A stage.  The epilogue must have an
-// fp32 output and no activation.
+// fp32 output and no activation.  Returns the number of kernels launched (0 without images, else 1).
 struct PatchGather {
     const uint8_t* img = nullptr;
     int n = 0, S = 0, patch = 0;
@@ -49,7 +49,7 @@ struct PatchGather {
 };
 inline int patch_gather_kbpd(int patch) { return (3 * patch + 63) / 64; }
 inline int patch_gather_k(int patch) { return patch * patch_gather_kbpd(patch) * 64; }
-void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, const Epilogue& ep, cudaStream_t stream);
+int launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, const Epilogue& ep, cudaStream_t stream);
 
 // 3 x 3 convolution, stride 1, zero padding 1, as an implicit GEMM over an NHWC bf16 activation [n, H, W, cin]:
 // row r of the virtual A matrix is output pixel (b, y, x) = r in row-major order (a 128-row tile may span images), and
@@ -57,18 +57,23 @@ void launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, c
 // The four gather warps of the GEMM copy 16-byte channel chunks into the swizzled A stage; k-block kb covers
 // k = 64 kb .. 64 kb + 63 (one tap of 64 channels, or two taps when cin = 32), and k >= 9 cin is zero.  W: bf16
 // [N, conv_gather_k(cin)] with the same k order (conv.weight [N, cin, 3, 3] permuted to [N, 3, 3, cin], zero padded).
-// cin must be a power of two >= 32; out is the NHWC [n, H, W, N] output.
+// cin must be a power of two >= 32; out is the NHWC [n, H, W, N] output.  Returns the number of kernels launched.
 struct ConvGather {
     const __nv_bfloat16* act = nullptr;
     int n = 0, H = 0, W = 0, cin = 0;
 };
 inline int conv_gather_k(int cin) { return (9 * cin + 63) / 64 * 64; }
-void launch_conv3x3(const ConvGather& cg, const __nv_bfloat16* Wc, int N, const Epilogue& ep, cudaStream_t stream);
+int launch_conv3x3(const ConvGather& cg, const __nv_bfloat16* Wc, int N, const Epilogue& ep, cudaStream_t stream);
 
 // The ResNet convolutions as the kernels run them: a k x k conv of cin channels has W rows of conv_rows_k(cin, k)
 // columns: cin for a 1 x 1 conv (a GEMM over the NHWC pixel rows), conv_gather_k(cin) for a 3 x 3 (launch_conv3x3),
 // 64 for the 3-channel stem conv (kernels::stem_im2col's k = tap * 3 + c).
 int conv_rows_k(int cin, int k);
+// One such conv over n images of H x W output pixels, x -> ep.out (NHWC bf16): a 3 x 3 conv (cin != 3) by
+// launch_conv3x3, any other by launch over x's rows, the NHWC pixel rows of a 1 x 1 conv or kernels::stem_im2col's rows
+// for the stem.  Wc: [cout, conv_rows_k(cin, k)] (conv_weight_rows).  Returns the number of kernels launched.
+int launch_conv(const __nv_bfloat16* x, int n, int H, int W, int cin, int k, const __nv_bfloat16* Wc, int cout,
+                const Epilogue& ep, int sms, cudaStream_t stream);
 // Host: conv.weight fp32 [cout, cin, k, k] times scale[o] (NULL: 1; the folded BatchNorm), in double, -> fp32 rows
 // [cout, conv_rows_k(cin, k)] with k index tap * cin + c (tap = k ky + kx), zero padded.
 void conv_weight_rows(const float* w, int cout, int cin, int k, const double* scale, float* out);

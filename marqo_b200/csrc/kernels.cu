@@ -76,13 +76,14 @@ static void check_ln_width(int w) {
     if (w % 128 != 0 || w > 128 * LN_MAX_V4) fail(B200_ERR_UNSUPPORTED, "width %d must be a multiple of 128 and <= 1024", w);
 }
 
-void layernorm(const float* x, long long in_stride, const float* gamma, const float* beta, float eps, int rows, int w,
-               float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s) {
-    if (rows <= 0) return;
+int layernorm(const float* x, long long in_stride, const float* gamma, const float* beta, float eps, int rows, int w,
+              float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s) {
+    if (rows <= 0) return 0;
     check_ln_width(w);
     static const int reverse = getenv("MARQO_B200_LN_FORWARD") == nullptr ? 1 : 0;
     layernorm_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, in_stride, gamma, beta, eps, rows, w, out_f32, out_bf16, reverse);
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 // ------------------------------------------------------------------------------------------------ im2col
@@ -119,12 +120,13 @@ __global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ c
         make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
 }
 
-void im2col_f32(const float* chw, int n, int S, int p, int kpad, int cls, __nv_bfloat16* out, cudaStream_t s) {
-    if (n <= 0) return;
+int im2col_f32(const float* chw, int n, int S, int p, int kpad, int cls, __nv_bfloat16* out, cudaStream_t s) {
+    if (n <= 0) return 0;
     const int g = S / p;
     const long long total = (long long)n * (g * g + cls) * (kpad / 8);
     im2col_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(chw, n, S, p, kpad, cls, out);
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 // ------------------------------------------------------------------------------------------------ embeddings
@@ -144,13 +146,14 @@ __global__ void __launch_bounds__(256) vit_embed_kernel(float4* __restrict__ x, 
     x[i] = v;
 }
 
-void vit_embed_rows(float* x, const float* cls, const float* pos, int n, int tokens_per_image, int w, cudaStream_t s) {
-    if (n <= 0) return;
+int vit_embed_rows(float* x, const float* cls, const float* pos, int n, int tokens_per_image, int w, cudaStream_t s) {
+    if (n <= 0) return 0;
     const long long total = (long long)n * tokens_per_image * (w / 4);
     vit_embed_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
         reinterpret_cast<float4*>(x), reinterpret_cast<const float4*>(cls), reinterpret_cast<const float4*>(pos), total,
         tokens_per_image, w / 4);
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 __global__ void __launch_bounds__(256) clip_text_embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ tok,
@@ -183,12 +186,13 @@ __global__ void __launch_bounds__(256) clip_text_embed_kernel(const int32_t* __r
     }
 }
 
-void clip_text_embed(const int32_t* ids, const float* tok, const float* pos, int n, int S, int w, int vocab, float* x,
-                     int32_t* eot, cudaStream_t s) {
-    if (n <= 0) return;
+int clip_text_embed(const int32_t* ids, const float* tok, const float* pos, int n, int S, int w, int vocab, float* x,
+                    int32_t* eot, cudaStream_t s) {
+    if (n <= 0) return 0;
     const long long rows = (long long)n * S;
     clip_text_embed_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(ids, tok, pos, n, S, w, vocab, x, eot);
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 __global__ void __launch_bounds__(256) bert_embed_ln_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ mask,
@@ -227,15 +231,16 @@ __global__ void __launch_bounds__(256) bert_embed_ln_kernel(const int32_t* __res
     }
 }
 
-void bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
-                   const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, float* x,
-                   __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s) {
-    if (n <= 0) return;
+int bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
+                  const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, float* x,
+                  __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s) {
+    if (n <= 0) return 0;
     check_ln_width(w);
     const long long rows = (long long)n * S;
     bert_embed_ln_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(ids, mask, word, pos, type0, gamma, beta, eps, n, S, w,
                                                                    vocab, x, h, kv_len);
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 // TYPE_ROW: XLM-R adds token_type_embeddings row 0 (HF: (inputs_embeds + token_type) + position, as BERT); MPNet has none.
@@ -286,10 +291,10 @@ __global__ void __launch_bounds__(256) roberta_embed_ln_kernel(const int32_t* __
     }
 }
 
-void roberta_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
-                      const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, int pad, float* x,
-                      __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s) {
-    if (n <= 0) return;
+int roberta_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
+                     const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, int pad, float* x,
+                     __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s) {
+    if (n <= 0) return 0;
     check_ln_width(w);
     const long long rows = (long long)n * S;
     const unsigned blocks = (unsigned)((rows + 7) / 8);
@@ -300,6 +305,7 @@ void roberta_embed_ln(const int32_t* ids, const int32_t* mask, const float* word
         roberta_embed_ln_kernel<false><<<blocks, 256, 0, s>>>(ids, mask, word, pos, nullptr, gamma, beta, eps, n, S, w,
                                                               vocab, pad, x, h, kv_len);
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 // ------------------------------------------------------------------------------------------------ heads
@@ -391,9 +397,9 @@ __global__ void __launch_bounds__(256) head_norm_kernel(float* __restrict__ out,
     for (int i = lane; i < E; i += 32) row[i] = row[i] / nrm;
 }
 
-void clip_head(const float* x, int S, const int32_t* row_in_seq, const float* gamma, const float* beta, float eps,
-               const float* proj, int n, int w, int E, int normalize, float* out, float* pooled_ws, cudaStream_t s) {
-    if (n <= 0) return;
+int clip_head(const float* x, int S, const int32_t* row_in_seq, const float* gamma, const float* beta, float eps,
+              const float* proj, int n, int w, int E, int normalize, float* out, float* pooled_ws, cudaStream_t s) {
+    if (n <= 0) return 0;
     if (w % 4 != 0 || (size_t)HEAD_IMGS * w * sizeof(float) > 40 * 1024)
         fail(B200_ERR_UNSUPPORTED, "clip_head: width %d unsupported", w);
     head_ln_kernel<<<(n + 7) / 8, 256, 0, s>>>(x, S, row_in_seq, gamma, beta, eps, n, w, pooled_ws);
@@ -401,10 +407,10 @@ void clip_head(const float* x, int S, const int32_t* row_in_seq, const float* ga
     const dim3 grid((n + HEAD_IMGS - 1) / HEAD_IMGS, (E + HEAD_COLS - 1) / HEAD_COLS);
     head_proj_kernel<<<grid, 256, (size_t)HEAD_IMGS * w * sizeof(float), s>>>(pooled_ws, proj, n, w, E, out);
     MB_CUDA(cudaGetLastError());
-    if (normalize) {
-        head_norm_kernel<<<(n + 7) / 8, 256, 0, s>>>(out, n, E);
-        MB_CUDA(cudaGetLastError());
-    }
+    if (!normalize) return 2;
+    head_norm_kernel<<<(n + 7) / 8, 256, 0, s>>>(out, n, E);
+    MB_CUDA(cudaGetLastError());
+    return 3;
 }
 
 __global__ void __launch_bounds__(256) bert_head_kernel(const float* __restrict__ x, const int32_t* __restrict__ kv_len, int S,
@@ -439,12 +445,13 @@ __global__ void __launch_bounds__(256) bert_head_kernel(const float* __restrict_
     }
 }
 
-void bert_head(const float* x, const int32_t* kv_len, int n, int S, int w, int pool, int normalize, float* out,
-               cudaStream_t s) {
-    if (n <= 0) return;
+int bert_head(const float* x, const int32_t* kv_len, int n, int S, int w, int pool, int normalize, float* out,
+              cudaStream_t s) {
+    if (n <= 0) return 0;
     if (w > 1024) fail(B200_ERR_UNSUPPORTED, "bert_head: width %d > 1024", w);
     bert_head_kernel<<<n, 256, 0, s>>>(x, kv_len, S, w, pool, normalize, out);
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 // ------------------------------------------------------------------------------------------------ conversions
@@ -609,8 +616,8 @@ __global__ void resample_v_kernel(const uint8_t* __restrict__ tmp, int n, int h,
 static int py_round_half_even(double v) { return (int)nearbyint(v); }
 
 // Resample [n, h, w, 3] to new_h x new_w and keep the S x S window at (top, left).
-static void resample_window_u8(const uint8_t* src, int n, int h, int w, int new_h, int new_w, int top, int left, int S,
-                               uint8_t* dst, cudaStream_t s) {
+static int resample_window_u8(const uint8_t* src, int n, int h, int w, int new_h, int new_w, int top, int left, int S,
+                              uint8_t* dst, cudaStream_t s) {
     const ResampleTable th = precompute(w, new_w);
     const ResampleTable tv = precompute(h, new_h);
     {   // stream-ordered temporaries, released on `s` at the end of this block
@@ -632,10 +639,11 @@ static void resample_window_u8(const uint8_t* src, int n, int h, int w, int new_
     }
     // the pageable host vectors above must outlive the async copies: synchronise before they go out of scope
     MB_CUDA(cudaStreamSynchronize(s));
+    return 2;
 }
 
-void resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s) {
-    if (n <= 0) return;
+int resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s) {
+    if (n <= 0) return 0;
     // torchvision Resize(S): shortest side -> S, the other int(S * long / short); CenterCrop(S)
     int new_w, new_h;
     if (w <= h) {
@@ -647,14 +655,14 @@ void resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst
     }
     const int left = py_round_half_even((new_w - S) / 2.0);
     const int top = py_round_half_even((new_h - S) / 2.0);
-    resample_window_u8(src, n, h, w, new_h, new_w, top, left, S, dst, s);
+    return resample_window_u8(src, n, h, w, new_h, new_w, top, left, S, dst, s);
 }
 
-void resize_squash_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s) {
-    if (n <= 0) return;
+int resize_squash_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s) {
+    if (n <= 0) return 0;
     // PIL resize((S, S), BICUBIC) = torchvision Resize((S, S)) on a PIL image: both axes to S, nothing cropped.  An axis
     // that already has S pixels gets the identity coefficients (a single 1.0 tap), so running its pass is exact.
-    resample_window_u8(src, n, h, w, S, S, 0, 0, S, dst, s);
+    return resample_window_u8(src, n, h, w, S, S, 0, 0, S, dst, s);
 }
 
 // ------------------------------------------------------------------------------------------------ SigLIP MAP head
@@ -734,14 +742,15 @@ __global__ void __launch_bounds__(MAP_THREADS) map_attention_kernel(const float*
     }
 }
 
-void map_attention(const float* q, long long q_stride, const __nv_bfloat16* kv, int n, int S, int W, int heads,
-                   __nv_bfloat16* out, cudaStream_t s) {
-    if (n <= 0) return;
+int map_attention(const float* q, long long q_stride, const __nv_bfloat16* kv, int n, int S, int W, int heads,
+                  __nv_bfloat16* out, cudaStream_t s) {
+    if (n <= 0) return 0;
     if (W != heads * 64) fail(B200_ERR_UNSUPPORTED, "map_attention: head_dim must be 64 (width %d, heads %d)", W, heads);
     if (S <= 0 || S > MAP_MAX_TOKENS) fail(B200_ERR_UNSUPPORTED, "map_attention: %d tokens (1..%d)", S, MAP_MAX_TOKENS);
     map_attention_kernel<<<dim3((unsigned)n, (unsigned)heads), MAP_THREADS, (size_t)S * sizeof(float), s>>>(
         q, q_stride, kv, S, W, out);
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 // ------------------------------------------------------------------------------------------------ ResNet trunk
@@ -779,9 +788,9 @@ __global__ void __launch_bounds__(256) stem_im2col_kernel(const uint8_t* __restr
         make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
 }
 
-void stem_im2col(const uint8_t* u8, const float* chw, int n, int S, const float* mean, const float* std,
-                 __nv_bfloat16* out, cudaStream_t s) {
-    if (n <= 0) return;
+int stem_im2col(const uint8_t* u8, const float* chw, int n, int S, const float* mean, const float* std,
+                __nv_bfloat16* out, cudaStream_t s) {
+    if (n <= 0) return 0;
     if (S % 2 != 0) fail(B200_ERR_INTERNAL, "stem_im2col: image size %d must be even", S);
     float sc[3], sh[3];
     for (int c = 0; c < 3; ++c) {   // the patch gather's constants (gemm.cu launch_tiles)
@@ -792,6 +801,7 @@ void stem_im2col(const uint8_t* u8, const float* chw, int n, int S, const float*
     stem_im2col_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(u8, chw, n, S, make_float3(sc[0], sc[1], sc[2]),
                                                                         make_float3(sh[0], sh[1], sh[2]), out);
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 // One thread = 8 channels of one output pixel; the four inputs are summed in fp32 and scaled by 1/4.
@@ -821,13 +831,14 @@ __global__ void __launch_bounds__(256) avgpool2_kernel(const uint4* __restrict__
                           pack_bf16x2(0.25f * acc[4], 0.25f * acc[5]), pack_bf16x2(0.25f * acc[6], 0.25f * acc[7]));
 }
 
-void avgpool2_nhwc(const __nv_bfloat16* in, int n, int H, int W, int C, __nv_bfloat16* out, cudaStream_t s) {
-    if (n <= 0) return;
+int avgpool2_nhwc(const __nv_bfloat16* in, int n, int H, int W, int C, __nv_bfloat16* out, cudaStream_t s) {
+    if (n <= 0) return 0;
     if (H % 2 != 0 || W % 2 != 0 || C % 8 != 0) fail(B200_ERR_INTERNAL, "avgpool2: %d x %d x %d", H, W, C);
     const long long total = (long long)n * (H / 2) * (W / 2) * (C / 8);
     avgpool2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(reinterpret_cast<const uint4*>(in), n, H, W, C / 8,
                                                                      reinterpret_cast<uint4*>(out));
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 // One thread = 8 channels of one image: the fp32 mean over the HW pixels, then every token row.
@@ -865,13 +876,14 @@ __global__ void __launch_bounds__(256) attnpool_tokens_kernel(const uint4* __res
     dst[0] = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
 }
 
-void attnpool_tokens(const __nv_bfloat16* x, const float* pos, int n, int HW, int C, __nv_bfloat16* out, cudaStream_t s) {
-    if (n <= 0) return;
+int attnpool_tokens(const __nv_bfloat16* x, const float* pos, int n, int HW, int C, __nv_bfloat16* out, cudaStream_t s) {
+    if (n <= 0) return 0;
     if (C % 8 != 0) fail(B200_ERR_INTERNAL, "attnpool_tokens: C = %d must be a multiple of 8", C);
     const long long total = (long long)n * (C / 8);
     attnpool_tokens_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
         reinterpret_cast<const uint4*>(x), reinterpret_cast<const float4*>(pos), n, HW, C / 8, reinterpret_cast<uint4*>(out));
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 __global__ void __launch_bounds__(256) l2_rows_kernel(const float* __restrict__ src, int n, int E, int normalize,
@@ -887,10 +899,11 @@ __global__ void __launch_bounds__(256) l2_rows_kernel(const float* __restrict__ 
     for (int i = lane; i < E; i += 32) out[(long long)b * E + i] = normalize ? row[i] / nrm : row[i];
 }
 
-void l2_rows(const float* src, int n, int E, int normalize, float* out, cudaStream_t s) {
-    if (n <= 0) return;
+int l2_rows(const float* src, int n, int E, int normalize, float* out, cudaStream_t s) {
+    if (n <= 0) return 0;
     l2_rows_kernel<<<(n + 7) / 8, 256, 0, s>>>(src, n, E, normalize, out);
     MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 }  // namespace kernels

@@ -1,5 +1,6 @@
 // Memory-bound helper kernels of the encoders (LayerNorm, embeddings, im2col, pooling + projection + L2 normalise,
-// dtype conversion).  All are coalesced / vectorised; none is GEMM-shaped.
+// dtype conversion).  All are coalesced / vectorised; none is GEMM-shaped.  The wrappers the encoders' forward passes
+// call return the number of kernels they launched (0 for an empty batch), which b200_model_last_timing reports.
 #pragma once
 #include "common.cuh"
 
@@ -8,45 +9,45 @@ namespace kernels {
 
 // y = LayerNorm(x) * gamma + beta over rows of width w (w % 128 == 0, w <= 1024).  Row r is read at
 // x + r * in_stride (floats).  Writes fp32 (out_f32, may alias x) and/or bf16 (out_bf16), both compact [rows, w].
-void layernorm(const float* x, long long in_stride, const float* gamma, const float* beta, float eps, int rows, int w,
-               float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s);
+int layernorm(const float* x, long long in_stride, const float* gamma, const float* beta, float eps, int rows, int w,
+              float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s);
 
 // Already-normalised fp32 CHW [n, 3, S, S] -> bf16 A matrix of the ViT token rows [n * (g*g + cls), kpad]: row
 // b * (g*g + cls) + t is zero for the class token t < cls (cls is 1 for CLIP, 0 for SigLIP), else patch t - cls
 // (row-major in the g x g grid) with k = c*p*p + dy*p + dx, zero for k >= 3*p*p.
-void im2col_f32(const float* chw, int n, int S, int p, int kpad, int cls, __nv_bfloat16* out, cudaStream_t s);
+int im2col_f32(const float* chw, int n, int S, int p, int kpad, int cls, __nv_bfloat16* out, cudaStream_t s);
 
 // x[b * tokens_per_image + t, :] = positional_embedding[t], plus class_embedding for t == 0 unless cls is NULL
 // (w % 4 == 0): the rows the patch-embed GEMM then adds conv1(patch) onto in place
-void vit_embed_rows(float* x, const float* cls, const float* pos, int n, int tokens_per_image, int w, cudaStream_t s);
+int vit_embed_rows(float* x, const float* cls, const float* pos, int n, int tokens_per_image, int w, cudaStream_t s);
 
 // CLIP text: x[b, s, :] = token_embedding[ids[b, s]] + positional_embedding[s]; also eot[b] = arg-max_s ids[b, s]
-void clip_text_embed(const int32_t* ids, const float* tok, const float* pos, int n, int S, int w, int vocab, float* x,
-                     int32_t* eot, cudaStream_t s);
+int clip_text_embed(const int32_t* ids, const float* tok, const float* pos, int n, int S, int w, int vocab, float* x,
+                    int32_t* eot, cudaStream_t s);
 
 // BERT: x = LN(word[ids] + position[s] + token_type[0]); fp32 + bf16 copies.  Also kv_len[b] = sum(mask[b, :])
 // (mask may be NULL = all ones).
-void bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
-                   const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, float* x,
-                   __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s);
+int bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
+                  const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, float* x,
+                  __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s);
 
 // RoBERTa-style embeddings (MPNet, XLM-R): x = LN(word[ids] (+ token_type[0]) + position[p]) with HF's position rule
 // p = pad + (non-pad ids among ids[b, 0..s]) for a non-pad id and p = pad for a pad id; type0 NULL (MPNet) adds no
 // token-type row.  fp32 + bf16 copies.  kv_len[b] = sum(mask[b, :]) as above.
-void roberta_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
-                      const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, int pad, float* x,
-                      __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s);
+int roberta_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
+                     const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, int pad, float* x,
+                     __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s);
 
 // CLIP head: for image b take token row (b * S + row_in_seq[b]) (row_in_seq NULL -> 0), LayerNorm it, multiply by
 // proj [w, E] (fp32), optionally divide by the L2 norm (no epsilon: abstract_clip_model.py:83-85).
-// pooled_ws: fp32 workspace [n, w].
-void clip_head(const float* x, int S, const int32_t* row_in_seq, const float* gamma, const float* beta, float eps,
-               const float* proj, int n, int w, int E, int normalize, float* out, float* pooled_ws, cudaStream_t s);
+// pooled_ws: fp32 workspace [n, w].  Three kernels with normalize, two without.
+int clip_head(const float* x, int S, const int32_t* row_in_seq, const float* gamma, const float* beta, float eps,
+              const float* proj, int n, int w, int E, int normalize, float* out, float* pooled_ws, cudaStream_t s);
 
 // BERT head: masked mean over the first kv_len[b] tokens (pool == 0) or the [CLS] row (pool == 1), then
 // x / max(|x|, 1e-12) if normalize (F.normalize, hugging_face_model.py:194-195).
-void bert_head(const float* x, const int32_t* kv_len, int n, int S, int w, int pool, int normalize, float* out,
-               cudaStream_t s);
+int bert_head(const float* x, const int32_t* kv_len, int n, int S, int w, int pool, int normalize, float* out,
+              cudaStream_t s);
 
 void f32_to_bf16(const float* src, __nv_bfloat16* dst, long long n, cudaStream_t s);
 // conv1.weight [w, 3*p*p] -> bf16 [w, kpad] zero padded
@@ -56,30 +57,31 @@ void pad_rows_to_bf16(const float* src, int rows, int k, int kpad, __nv_bfloat16
 // k' = dy * (64 * kbpd) + dx * 3 + c; the slots past 3 * p of every pixel row are zero.
 void patch_weight_rows(const float* src, int rows, int p, int kbpd, __nv_bfloat16* dst, cudaStream_t s);
 
-// PIL-compatible antialiased bicubic resize (shortest side -> S) + centre crop, uint8 HWC in/out.
-void resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s);
+// PIL-compatible antialiased bicubic resize (shortest side -> S) + centre crop, uint8 HWC in/out: a horizontal and a
+// vertical pass, two kernels.
+int resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s);
 // The same resampling squashed to S x S (x and y scaled independently, no crop): PIL resize((S, S), BICUBIC).
-void resize_squash_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s);
+int resize_squash_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s);
 
 // Single-query attention pooling, one query per head: out[b, h*64 .. h*64+63] = softmax_s(q_h . k_{b,s} / 8) v_{b,s}
 // (bf16).  q fp32, image b's query at q + b * q_stride: q_stride 0 shares one query (SigLIP's latent), W gives one per
 // image (the ResNet attention pool's mean token); kv bf16 [n*S, 2W] (K columns, then V columns, head-major); head_dim 64.
-void map_attention(const float* q, long long q_stride, const __nv_bfloat16* kv, int n, int S, int W, int heads,
-                   __nv_bfloat16* out, cudaStream_t s);
+int map_attention(const float* q, long long q_stride, const __nv_bfloat16* kv, int n, int S, int W, int heads,
+                  __nv_bfloat16* out, cudaStream_t s);
 
 // ResNet stem conv1 (3 x 3, stride 2, padding 1, 3 input channels) as an im2col A matrix: bf16 [n * (S/2)^2, 64], row =
 // output pixel, k = (3 ky + kx) * 3 + c, zero for k >= 27.  Input: uint8 HWC [n, S, S, 3] normalised as the patch
 // gather does (u8 != NULL), or already-normalised fp32 CHW [n, 3, S, S].  Taps outside the image are 0.
-void stem_im2col(const uint8_t* u8, const float* chw, int n, int S, const float* mean, const float* std,
-                 __nv_bfloat16* out, cudaStream_t s);
+int stem_im2col(const uint8_t* u8, const float* chw, int n, int S, const float* mean, const float* std,
+                __nv_bfloat16* out, cudaStream_t s);
 // AvgPool2d(2) over NHWC bf16 [n, H, W, C] -> [n, H/2, W/2, C] (H, W even, C % 8 == 0).
-void avgpool2_nhwc(const __nv_bfloat16* in, int n, int H, int W, int C, __nv_bfloat16* out, cudaStream_t s);
+int avgpool2_nhwc(const __nv_bfloat16* in, int n, int H, int W, int C, __nv_bfloat16* out, cudaStream_t s);
 // ResNet attention-pool tokens: x NHWC bf16 [n, HW, C] -> out bf16 [n * (HW + 1), C], row 0 of image b = mean_s x_s +
 // pos[0], row 1 + s = x_s + pos[1 + s]; pos fp32 [HW + 1, C].
-void attnpool_tokens(const __nv_bfloat16* x, const float* pos, int n, int HW, int C, __nv_bfloat16* out, cudaStream_t s);
+int attnpool_tokens(const __nv_bfloat16* x, const float* pos, int n, int HW, int C, __nv_bfloat16* out, cudaStream_t s);
 
 // out[b] = src[b] / |src[b]| if normalize (no epsilon: abstract_clip_model.py:83-85), else src[b]; rows of E floats.
-void l2_rows(const float* src, int n, int E, int normalize, float* out, cudaStream_t s);
+int l2_rows(const float* src, int n, int E, int normalize, float* out, cudaStream_t s);
 
 }  // namespace kernels
 }  // namespace mb

@@ -48,15 +48,27 @@ struct MapW {
     int mlp = 0;
 };
 
+// What runs a tower, resolved once from the model's arch (resolve_kinds).  Archs whose forward passes differ only in
+// data share a kind: MPNet and XLM-R are ROBERTA, and the ResNet CLIP's text tower is CLIP's.
+enum class VisionKind { NONE, CLIP_VIT, SIGLIP_VIT, RESNET };
+enum class TextKind { NONE, CLIP, SIGLIP, BERT, ROBERTA };
+struct Kinds {
+    VisionKind vision = VisionKind::NONE;
+    TextKind text = TextKind::NONE;
+    bool mpnet = false;   // ROBERTA: MPNet's layer names and relative-position bias, else XLM-R's token-type row
+};
+
 struct TowerW {
     b200_tower_desc d{};
-    bool present = false;
     std::vector<LayerW> layers;
     float eps = 1e-5f;                      // every LayerNorm of the tower
+    int act = gemm::ACT_GELU;               // the MLP's activation
+    // tokens per item: an image's token rows, or the longest sequence
+    int tokens = 0;
     // vision
     const __nv_bfloat16* conv_w = nullptr;  // [width, kpad]
     const __nv_bfloat16* conv_wg = nullptr; // [width, gemm::patch_gather_k(patch)]: gather GEMM order
-    int kpad = 0, grid = 0, tokens = 0;
+    int kpad = 0, grid = 0;
     int cls_rows = 1;                       // class-token rows per image: 1 (CLIP), 0 (SigLIP)
     // pos: CLIP positional_embedding [grid^2 + 1, width]; SigLIP pos_embed + the patch conv's bias [grid^2, width].
     // ln_pre is NULL for SigLIP.
@@ -69,8 +81,7 @@ struct TowerW {
     MapW map;
     // text / bert embeddings
     const float *tok = nullptr, *type0 = nullptr, *emb_ln_w = nullptr, *emb_ln_b = nullptr;
-    int max_pos = 0;
-    // MPNet: relative-position bias of every layer, fp32 [heads, 2 * max_pos - 1] pre-scaled by log2(e)
+    // MPNet: relative-position bias of every layer, fp32 [heads, 2 * ctx - 1] pre-scaled by log2(e)
     attention::RelBias rel_bias;
 };
 
@@ -110,8 +121,9 @@ struct b200_model {
     bool finalized = false;
     std::map<std::string, DeviceBuffer<float>> raw;   // uploaded fp32 parameters by checkpoint name
     std::vector<DeviceBuffer<uint8_t>> derived;        // device buffers built from them by b200_model_finalize
+    Kinds kind;
     TowerW vision, text;
-    ResnetW resnet;   // B200_ARCH_CLIP_RESNET's image tower (vision.present, vision.tokens = grid^2 + 1)
+    ResnetW resnet;   // VisionKind::RESNET's image tower (vision.tokens = grid^2 + 1)
     // workspaces (sized for max_tokens tokens)
     long long max_tokens = 0;
     DeviceBuffer<float> x;
@@ -164,6 +176,103 @@ void check_tower(const b200_tower_desc& t, const char* name) {
     MB_CHECK_ARG(t.heads > 0 && (t.width == t.heads * 32 || t.width == t.heads * 64),
                  "%s: head_dim must be 32 or 64 (width %d, heads %d)", name, t.width, t.heads);
     MB_CHECK_ARG(t.mlp > 0 && t.mlp % 64 == 0, "%s.mlp %d must be a multiple of 64", name, t.mlp);
+}
+
+// The only reader of desc.arch besides b200_model_create's unknown-arch check.
+Kinds resolve_kinds(const b200_model_desc& d) {
+    Kinds k;
+    const bool vit = d.vision.layers > 0, text = d.text.layers > 0;
+    switch (d.arch) {
+    case B200_ARCH_CLIP:
+        if (vit) k.vision = VisionKind::CLIP_VIT;
+        if (text) k.text = TextKind::CLIP;
+        break;
+    case B200_ARCH_CLIP_RESNET:
+        if (d.resnet_layers[0] > 0) k.vision = VisionKind::RESNET;
+        if (text) k.text = TextKind::CLIP;
+        break;
+    case B200_ARCH_SIGLIP:
+        if (vit) k.vision = VisionKind::SIGLIP_VIT;
+        if (text) k.text = TextKind::SIGLIP;
+        break;
+    case B200_ARCH_BERT:
+        if (text) k.text = TextKind::BERT;
+        break;
+    case B200_ARCH_MPNET:
+    case B200_ARCH_XLMR:
+        if (text) k.text = TextKind::ROBERTA;
+        k.mpnet = d.arch == B200_ARCH_MPNET;
+        break;
+    }
+    return k;
+}
+
+// the model-wide settings of a SigLIP tower
+void check_siglip(const b200_model_desc& d) {
+    MB_CHECK_ARG(d.layer_norm_eps > 0.f, "SigLIP: layer_norm_eps must be positive");
+    MB_CHECK_ARG(d.embed_dim % 32 == 0, "SigLIP: embed_dim %d must be a multiple of 32", d.embed_dim);
+}
+
+void check_vision(const b200_model_desc& d, VisionKind kind) {
+    if (kind == VisionKind::NONE) return;
+    for (int i = 0; i < 3; ++i) MB_CHECK_ARG(d.image_std[i] > 0.f, "image_std must be positive");
+    switch (kind) {
+    case VisionKind::RESNET: {
+        const int wd = d.resnet_width, S = d.resnet_image_size;
+        for (int s = 0; s < 4; ++s)
+            MB_CHECK_ARG(d.resnet_layers[s] > 0 && d.resnet_layers[s] <= 64, "resnet_layers[%d] = %d out of range", s,
+                         d.resnet_layers[s]);
+        // the stem's 3 x 3 convs gather width / 2 channels: a power of two >= 32
+        MB_CHECK_ARG(wd >= 64 && wd <= 128 && (wd & (wd - 1)) == 0, "resnet_width %d must be 64 or 128", wd);
+        MB_CHECK_ARG(S > 0 && S % 32 == 0 && S <= 512, "resnet_image_size %d must be a multiple of 32, <= 512", S);
+        MB_CHECK_ARG(d.resnet_heads * 64 == 32 * wd, "attention pool: head_dim must be 64 (%d channels, %d heads)",
+                     32 * wd, d.resnet_heads);
+        MB_CHECK_ARG(d.embed_dim % 32 == 0, "CLIP ResNet: embed_dim %d must be a multiple of 32", d.embed_dim);
+        break;
+    }
+    case VisionKind::SIGLIP_VIT:
+        check_siglip(d);
+        // the MAP head has no projection; its single-query attention runs head_dim 64 only
+        MB_CHECK_ARG(d.embed_dim == d.vision.width, "SigLIP: embed_dim %d must equal the vision width %d", d.embed_dim,
+                     d.vision.width);
+        MB_CHECK_ARG(d.vision.width == d.vision.heads * 64, "SigLIP: vision head_dim must be 64 (width %d, heads %d)",
+                     d.vision.width, d.vision.heads);
+        [[fallthrough]];
+    case VisionKind::CLIP_VIT:
+        check_tower(d.vision, "vision");
+        MB_CHECK_ARG(d.vision.patch > 0 && d.vision.image_size % d.vision.patch == 0,
+                     "image_size must be a multiple of patch");
+        break;
+    }
+}
+
+void check_text(const b200_model_desc& d, const Kinds& k) {
+    if (k.text == TextKind::NONE) return;
+    check_tower(d.text, "text");
+    MB_CHECK_ARG(d.text.ctx > 0 && d.text.vocab > 0, "text.ctx and text.vocab must be positive");
+    switch (k.text) {
+    case TextKind::SIGLIP:
+        check_siglip(d);
+        break;
+    case TextKind::ROBERTA: {
+        const char* name = k.mpnet ? "MPNet" : "XLM-R";
+        MB_CHECK_ARG(d.layer_norm_eps > 0.f, "%s: layer_norm_eps must be positive", name);
+        MB_CHECK_ARG(d.pad_id >= 0 && d.pad_id < d.text.vocab, "%s: pad_id %d out of range", name, d.pad_id);
+        if (k.mpnet) {
+            MB_CHECK_ARG(d.text.width == d.text.heads * 64, "MPNet: head_dim must be 64 (width %d, heads %d)",
+                         d.text.width, d.text.heads);
+            MB_CHECK_ARG(d.rel_buckets >= 4 && d.rel_buckets % 2 == 0 && d.rel_max_distance > d.rel_buckets / 4,
+                         "MPNet: bad relative-bias buckets (%d) / max distance (%d)", d.rel_buckets,
+                         d.rel_max_distance);
+            MB_CHECK_ARG(d.text.ctx <= 1024, "MPNet: sequences of up to 1024 tokens are supported (ctx %d)",
+                         d.text.ctx);
+        }
+        [[fallthrough]];
+    }
+    case TextKind::BERT:
+        MB_CHECK_ARG(d.embed_dim == d.text.width, "BERT / MPNet / XLM-R embed_dim must equal width");
+        break;
+    }
 }
 
 const float* param(b200_model* m, const std::string& name, long long numel) {
@@ -447,163 +556,194 @@ void build_resnet(b200_model* m, TowerW& T) {
     for (auto& b : R.buf) b = DeviceBuffer<__nv_bfloat16>((size_t)d.max_batch * per_image);
 }
 
+// the MLP activation of open_clip's towers
+int open_clip_act(const b200_model_desc& d) {
+    return d.act == B200_ACT_QUICKGELU ? gemm::ACT_QUICKGELU : gemm::ACT_GELU;
+}
+
+// open_clip's VisionTransformer or SigLIP's timm trunk: the patch conv (conv_name, no bias) in both GEMM layouts, then
+// the rest of the tower.
+void build_vit(b200_model* m, TowerW& T, const char* conv_name, int cls_rows) {
+    const long long w = T.d.width, p = T.d.patch;
+    T.grid = T.d.image_size / T.d.patch;
+    T.cls_rows = cls_rows;
+    T.tokens = T.grid * T.grid + T.cls_rows;
+    const int K = 3 * (int)p * (int)p;
+    T.kpad = (int)round_up((size_t)K, 64);
+    const float* conv = param(m, conv_name, w * K);
+    __nv_bfloat16* cw = derived_buffer<__nv_bfloat16>(m, (size_t)w * T.kpad);
+    kernels::pad_rows_to_bf16(conv, (int)w, K, T.kpad, cw, m->stream);
+    MB_CUDA(cudaStreamSynchronize(m->stream));
+    T.conv_w = cw;
+    __nv_bfloat16* cg = derived_buffer<__nv_bfloat16>(m, (size_t)w * gemm::patch_gather_k((int)p));
+    kernels::patch_weight_rows(conv, (int)w, (int)p, gemm::patch_gather_kbpd((int)p), cg, m->stream);
+    MB_CUDA(cudaStreamSynchronize(m->stream));
+    T.conv_wg = cg;
+}
+
+void build_vision(b200_model* m) {
+    TowerW& T = m->vision;
+    const long long w = T.d.width;
+    switch (m->kind.vision) {
+    case VisionKind::CLIP_VIT:
+        build_vit(m, T, "visual.conv1.weight", 1);
+        T.act = open_clip_act(m->desc);
+        T.cls = param(m, "visual.class_embedding", w);
+        T.pos = param(m, "visual.positional_embedding", (long long)T.tokens * w);
+        T.ln_pre_w = param(m, "visual.ln_pre.weight", w);
+        T.ln_pre_b = param(m, "visual.ln_pre.bias", w);
+        build_preln_layers(m, T, "visual.transformer.resblocks.", OPEN_CLIP_BLOCK);
+        T.ln_out_w = param(m, "visual.ln_post.weight", w);
+        T.ln_out_b = param(m, "visual.ln_post.bias", w);
+        T.proj = param(m, "visual.proj", w * m->desc.embed_dim);
+        break;
+    case VisionKind::SIGLIP_VIT:
+        build_vit(m, T, "visual.trunk.patch_embed.proj.weight", 0);
+        T.act = open_clip_act(m->desc);
+        T.eps = m->desc.layer_norm_eps;
+        build_siglip_vision(m, T);
+        break;
+    case VisionKind::RESNET:
+        build_resnet(m, T);
+        break;
+    }
+}
+
+void build_text(b200_model* m) {
+    TowerW& T = m->text;
+    const long long w = T.d.width, E = m->desc.embed_dim;
+    if (m->kind.text != TextKind::NONE) T.tokens = T.d.ctx;
+    switch (m->kind.text) {
+    case TextKind::CLIP:
+    case TextKind::SIGLIP: {
+        const bool siglip = m->kind.text == TextKind::SIGLIP;
+        const std::string p = siglip ? "text." : "";
+        T.act = open_clip_act(m->desc);
+        T.tok = param(m, p + "token_embedding.weight", (long long)T.d.vocab * w);
+        T.pos = param(m, p + "positional_embedding", (long long)T.d.ctx * w);
+        build_preln_layers(m, T, p + "transformer.resblocks.", OPEN_CLIP_BLOCK);
+        T.ln_out_w = param(m, p + "ln_final.weight", w);
+        T.ln_out_b = param(m, p + "ln_final.bias", w);
+        if (siglip) {
+            T.eps = m->desc.layer_norm_eps;
+            T.w_tproj = to_bf16(m, "text.text_projection.weight", E * w);
+            T.b_tproj = param(m, "text.text_projection.bias", E);
+        } else {
+            T.proj = param(m, "text_projection", w * E);
+        }
+        break;
+    }
+    case TextKind::BERT: {
+        T.eps = 1e-12f;   // BertConfig's layer_norm_eps
+        T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
+        T.pos = param(m, "embeddings.position_embeddings.weight", (long long)T.d.ctx * w);
+        const int tv = std::max(1, m->desc.type_vocab);
+        T.type0 = param(m, "embeddings.token_type_embeddings.weight", (long long)tv * w);  // row 0 is used
+        T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
+        T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
+        build_bert_layers(m, T, BERT_NAMES);
+        break;
+    }
+    case TextKind::ROBERTA: {
+        T.eps = m->desc.layer_norm_eps;
+        T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
+        // positions run pad_id + 1 .. pad_id + ctx (pads take pad_id): the table has at least ctx + pad_id + 1 rows
+        const long long pos_rows = param_rows(m, "embeddings.position_embeddings.weight", w);
+        MB_CHECK_ARG(pos_rows >= (long long)T.d.ctx + m->desc.pad_id + 1,
+                     "embeddings.position_embeddings has %lld rows; %d tokens with pad id %d need %d", pos_rows,
+                     T.d.ctx, m->desc.pad_id, T.d.ctx + m->desc.pad_id + 1);
+        T.pos = param(m, "embeddings.position_embeddings.weight", pos_rows * w);
+        T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
+        T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
+        if (m->kind.mpnet) {
+            build_bert_layers(m, T, MPNET_NAMES);
+            T.rel_bias = build_rel_bias(m, T);
+        } else {
+            T.type0 = param(m, "embeddings.token_type_embeddings.weight", w);   // type_vocab_size 1
+            build_bert_layers(m, T, BERT_NAMES);
+        }
+        break;
+    }
+    }
+}
+
 struct Counter {
     int n = 0;
 };
 
-struct ProfScope {
-    b200_model* m;
-    bool on;
-    ProfScope(b200_model* mm, int cls) : m(mm), on(mm->profiling) {
-        if (!on) return;
-        if ((size_t)(2 * m->prof_n + 2) > m->prof_ev.size()) {
-            for (int i = 0; i < 64; ++i) m->prof_ev.push_back(make_event());
-            m->prof_cls.resize(m->prof_ev.size() / 2);
-        }
-        m->prof_cls[m->prof_n] = cls;
-        MB_CUDA(cudaEventRecord(m->prof_ev[2 * m->prof_n].get(), m->stream));
+// A GEMM (cls 0) or attention (cls 1) launch: launch() returns the number of kernels it launched, which is counted;
+// while profiling, events bracket it for b200_model_profile.
+template <class Launch>
+void profiled(b200_model* m, Counter& c, int cls, Launch&& launch) {
+    if (!m->profiling) {
+        c.n += launch();
+        return;
     }
-    ~ProfScope() {
-        if (!on) return;
-        cudaEventRecord(m->prof_ev[2 * m->prof_n + 1].get(), m->stream);
-        ++m->prof_n;
+    if ((size_t)(2 * m->prof_n + 2) > m->prof_ev.size()) {
+        for (int i = 0; i < 64; ++i) m->prof_ev.push_back(make_event());
+        m->prof_cls.resize(m->prof_ev.size() / 2);
     }
-};
-
-void linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, const __nv_bfloat16* W, int N,
-            const gemm::Epilogue& ep) {
-    ProfScope ps(m, 0);
-    gemm::launch(A, K, W, M, N, K, ep, m->sms, m->stream);
-    ++c.n;
+    m->prof_cls[m->prof_n] = cls;
+    MB_CUDA(cudaEventRecord(m->prof_ev[2 * m->prof_n].get(), m->stream));
+    c.n += launch();
+    MB_CUDA(cudaEventRecord(m->prof_ev[2 * m->prof_n + 1].get(), m->stream));
+    ++m->prof_n;
 }
 
-void attend(b200_model* m, Counter& c, int B, int S, int w, int heads, int mask_mode, const int32_t* kv_len,
-            const attention::RelBias& bias = {}) {
-    ProfScope ps(m, 1);
-    c.n += attention::launch(m->qkv.get(), m->o.get(), B, S, w, heads, mask_mode, kv_len, bias, m->stream);
-}
-
-// Pre-LN residual blocks (open_clip ResidualAttentionBlock).  x (fp32) is the residual stream, h (bf16) the LayerNorm
-// output the next GEMM consumes.
-void run_clip_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, int mask_mode) {
-    const int M = B * S, w = T.d.width, mlp = T.d.mlp;
-    const int act = m->desc.act == B200_ACT_QUICKGELU ? gemm::ACT_QUICKGELU : gemm::ACT_GELU;
-    for (const LayerW& L : T.layers) {
-        kernels::layernorm(m->x.get(), w, L.ln1_w, L.ln1_b, T.eps, M, w, nullptr, m->h.get(), m->stream);
-        ++c.n;
-        gemm::Epilogue e1;
-        e1.bias = L.b_qkv;
-        e1.out = m->qkv.get();
-        e1.ldo = 3 * w;
-        linear(m, c, m->h.get(), M, w, L.w_qkv, 3 * w, e1);
-        attend(m, c, B, S, w, T.d.heads, mask_mode, nullptr);
-        gemm::Epilogue e2;
-        e2.bias = L.b_o;
-        e2.residual = m->x.get();
-        e2.ldr = w;
-        e2.out = m->x.get();
-        e2.ldo = w;
-        e2.out_fp32 = 1;
-        linear(m, c, m->o.get(), M, w, L.w_o, w, e2);
-        kernels::layernorm(m->x.get(), w, L.ln2_w, L.ln2_b, T.eps, M, w, nullptr, m->h.get(), m->stream);
-        ++c.n;
-        gemm::Epilogue e3;
-        e3.bias = L.b_fc;
-        e3.act = act;
-        e3.out = m->u.get();
-        e3.ldo = mlp;
-        linear(m, c, m->h.get(), M, w, L.w_fc, mlp, e3);
-        gemm::Epilogue e4;
-        e4.bias = L.b_proj;
-        e4.residual = m->x.get();
-        e4.ldr = w;
-        e4.out = m->x.get();
-        e4.ldo = w;
-        e4.out_fp32 = 1;
-        linear(m, c, m->u.get(), M, mlp, L.w_proj, w, e4);
-    }
-}
-
-// Post-LN blocks (HF BertLayer, MPNetLayer with the tower's relative-position bias); on entry x (fp32) and h (bf16)
-// both hold the embedding LayerNorm output.  Both LayerNorms of a layer rewrite x in place.
-void run_bert_blocks(b200_model* m, Counter& c, const TowerW& T, int B, int S, float eps) {
-    const int M = B * S, w = T.d.width, mlp = T.d.mlp;
-    for (const LayerW& L : T.layers) {
-        gemm::Epilogue e1;
-        e1.bias = L.b_qkv;
-        e1.out = m->qkv.get();
-        e1.ldo = 3 * w;
-        linear(m, c, m->h.get(), M, w, L.w_qkv, 3 * w, e1);
-        attend(m, c, B, S, w, T.d.heads, attention::MASK_KEYLEN, m->aux.get(), T.rel_bias);
-        gemm::Epilogue e2;
-        e2.bias = L.b_o;
-        e2.residual = m->x.get();
-        e2.ldr = w;
-        e2.out = m->x.get();
-        e2.ldo = w;
-        e2.out_fp32 = 1;
-        linear(m, c, m->o.get(), M, w, L.w_o, w, e2);
-        kernels::layernorm(m->x.get(), w, L.ln1_w, L.ln1_b, eps, M, w, m->x.get(), m->h.get(), m->stream);
-        ++c.n;
-        gemm::Epilogue e3;
-        e3.bias = L.b_fc;
-        e3.act = gemm::ACT_GELU;
-        e3.out = m->u.get();
-        e3.ldo = mlp;
-        linear(m, c, m->h.get(), M, w, L.w_fc, mlp, e3);
-        gemm::Epilogue e4;
-        e4.bias = L.b_proj;
-        e4.residual = m->x.get();
-        e4.ldr = w;
-        e4.out = m->x.get();
-        e4.ldo = w;
-        e4.out_fp32 = 1;
-        linear(m, c, m->u.get(), M, mlp, L.w_proj, w, e4);
-        kernels::layernorm(m->x.get(), w, L.ln2_w, L.ln2_b, eps, M, w, m->x.get(), m->h.get(), m->stream);
-        ++c.n;
-    }
-}
-
-// The small-M GEMMs of the SigLIP heads: out = act(A[M, K] W[N, K]^T + bias) (+ residual == out, fp32)
-void head_linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, const __nv_bfloat16* W, int N,
-                 const float* bias, int act, void* out, bool out_fp32, bool residual) {
+gemm::Epilogue epilogue(void* out, int ldo, const float* bias = nullptr, int act = gemm::ACT_NONE,
+                        bool out_fp32 = false, const void* residual = nullptr, int ldr = 0) {
     gemm::Epilogue e;
     e.bias = bias;
+    e.residual = residual;
+    e.ldr = ldr;
     e.act = act;
     e.out = out;
-    e.ldo = N;
+    e.ldo = ldo;
     e.out_fp32 = out_fp32 ? 1 : 0;
-    if (residual) {
-        e.residual = static_cast<const float*>(out);
-        e.ldr = N;
+    return e;
+}
+
+// out = ep(A[M, K] W[N, K]^T), A's rows lda elements apart (0: K)
+void linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, const __nv_bfloat16* W, int N,
+            const gemm::Epilogue& ep, int lda = 0) {
+    profiled(m, c, 0, [&] {
+        return gemm::launch(A, lda ? lda : K, W, M, N, K, ep, m->sms, m->stream) == gemm::KERNEL_NONE ? 0 : 1;
+    });
+}
+
+// The transformer layers of a tower.  x (fp32) is the residual stream, h (bf16) the LayerNorm output the next GEMM
+// consumes.  Pre-LN (open_clip ResidualAttentionBlock, timm's ViT Block): LN x -> h before the QKV and fc1 GEMMs.
+// Post-LN (HF BertLayer, MPNetLayer with the tower's relative-position bias): on entry x and h both hold the embedding
+// LayerNorm output, and LN rewrites x in place (x -> x and h) after each residual GEMM.
+void run_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S, int mask_mode, bool pre_ln) {
+    const int M = B * S, w = T.d.width, mlp = T.d.mlp;
+    float* x = m->x.get();
+    const int32_t* kv_len = mask_mode == attention::MASK_KEYLEN ? m->aux.get() : nullptr;
+    auto ln = [&](const float* g, const float* b) {
+        c.n += kernels::layernorm(x, w, g, b, T.eps, M, w, pre_ln ? nullptr : x, m->h.get(), m->stream);
+    };
+    for (const LayerW& L : T.layers) {
+        if (pre_ln) ln(L.ln1_w, L.ln1_b);
+        linear(m, c, m->h.get(), M, w, L.w_qkv, 3 * w, epilogue(m->qkv.get(), 3 * w, L.b_qkv));
+        profiled(m, c, 1, [&] {
+            return attention::launch(m->qkv.get(), m->o.get(), B, S, w, T.d.heads, mask_mode, kv_len, T.rel_bias,
+                                     m->stream);
+        });
+        linear(m, c, m->o.get(), M, w, L.w_o, w, epilogue(x, w, L.b_o, gemm::ACT_NONE, true, x, w));
+        ln(pre_ln ? L.ln2_w : L.ln1_w, pre_ln ? L.ln2_b : L.ln1_b);
+        linear(m, c, m->h.get(), M, w, L.w_fc, mlp, epilogue(m->u.get(), mlp, L.b_fc, T.act));
+        linear(m, c, m->u.get(), M, mlp, L.w_proj, w, epilogue(x, w, L.b_proj, gemm::ACT_NONE, true, x, w));
+        if (!pre_ln) ln(L.ln2_w, L.ln2_b);
     }
-    linear(m, c, A, M, K, W, N, e);
 }
 
 // One folded ResNet conv over n images of H x H output pixels (NHWC bf16 x -> out): bias, then ReLU with the optional
 // bf16 residual added before it, or neither.  The stem conv (cin 3) takes stem_im2col's rows as x.
 void resnet_conv(b200_model* m, Counter& c, const ConvW& cw, const __nv_bfloat16* x, int n, int H,
                  const __nv_bfloat16* residual, bool relu, __nv_bfloat16* out) {
-    gemm::Epilogue e;
-    e.bias = cw.b;
-    e.act = relu ? gemm::ACT_RELU : gemm::ACT_NONE;
-    e.residual = residual;
-    e.ldr = cw.cout;
-    e.out = out;
-    e.ldo = cw.cout;
-    ProfScope ps(m, 0);
-    if (cw.k == 3 && cw.cin != 3) {
-        gemm::ConvGather g;
-        g.act = x;
-        g.n = n;
-        g.H = g.W = H;
-        g.cin = cw.cin;
-        gemm::launch_conv3x3(g, cw.w, cw.cout, e, m->stream);
-    } else {
-        const int K = gemm::conv_rows_k(cw.cin, cw.k);
-        gemm::launch(x, K, cw.w, n * H * H, cw.cout, K, e, m->sms, m->stream);
-    }
-    ++c.n;
+    const gemm::Epilogue e =
+        epilogue(out, cw.cout, cw.b, relu ? gemm::ACT_RELU : gemm::ACT_NONE, false, residual, cw.cout);
+    profiled(m, c, 0, [&] { return gemm::launch_conv(x, n, H, H, cw.cin, cw.k, cw.w, cw.cout, e, m->sms, m->stream); });
 }
 
 // The ResNet CLIP image tower over n images (uint8 HWC u8 or normalised fp32 CHW f32, at the model's size): buffers
@@ -614,21 +754,19 @@ void forward_resnet(b200_model* m, Counter& c, const uint8_t* u8, const float* f
     __nv_bfloat16 *A = R.buf[0].get(), *B = R.buf[1].get(), *Cb = R.buf[2].get(), *D = R.buf[3].get();
     const int S = d.resnet_image_size, width = d.resnet_width;
     int H = S / 2;
-    kernels::stem_im2col(u8, f32, n, S, d.image_mean, d.image_std, B, m->stream);
+    c.n += kernels::stem_im2col(u8, f32, n, S, d.image_mean, d.image_std, B, m->stream);
     resnet_conv(m, c, R.stem[0], B, n, H, nullptr, true, Cb);
     resnet_conv(m, c, R.stem[1], Cb, n, H, nullptr, true, D);
     resnet_conv(m, c, R.stem[2], D, n, H, nullptr, true, Cb);
-    kernels::avgpool2_nhwc(Cb, n, H, H, width, A, m->stream);
-    c.n += 2;
+    c.n += kernels::avgpool2_nhwc(Cb, n, H, H, width, A, m->stream);
     H /= 2;
     for (const BottleneckW& blk : R.blocks) {
         resnet_conv(m, c, blk.c1, A, n, H, nullptr, true, B);
         resnet_conv(m, c, blk.c2, B, n, H, nullptr, true, Cb);
         const __nv_bfloat16 *main = Cb, *identity = A;
         if (blk.stride > 1) {
-            kernels::avgpool2_nhwc(Cb, n, H, H, blk.c2.cout, B, m->stream);
-            kernels::avgpool2_nhwc(A, n, H, H, blk.c1.cin, Cb, m->stream);
-            c.n += 2;
+            c.n += kernels::avgpool2_nhwc(Cb, n, H, H, blk.c2.cout, B, m->stream);
+            c.n += kernels::avgpool2_nhwc(A, n, H, H, blk.c1.cin, Cb, m->stream);
             H /= 2;
             main = B;
             resnet_conv(m, c, blk.ds, Cb, n, H, nullptr, false, D);
@@ -643,73 +781,25 @@ void forward_resnet(b200_model* m, Counter& c, const uint8_t* u8, const float* f
     // attention pool: tokens [mean; pixels] + pos -> B; K|V of every token -> Cb; q of token 0 (rows T C apart) -> D;
     // one query per image and head -> A; c_proj -> pooled; L2
     const int C = R.C, HW = R.grid * R.grid, T = HW + 1, E = d.embed_dim;
-    kernels::attnpool_tokens(A, R.pos, n, HW, C, B, m->stream);
-    ++c.n;
+    c.n += kernels::attnpool_tokens(A, R.pos, n, HW, C, B, m->stream);
     float* q = reinterpret_cast<float*>(D);
-    {
-        ProfScope ps(m, 0);
-        gemm::Epilogue e;
-        e.bias = R.b_kv;
-        e.out = Cb;
-        e.ldo = 2 * C;
-        gemm::launch(B, C, R.w_kv, n * T, 2 * C, C, e, m->sms, m->stream);
-        gemm::Epilogue eq;
-        eq.bias = R.b_q;
-        eq.out = q;
-        eq.ldo = C;
-        eq.out_fp32 = 1;
-        gemm::launch(B, T * C, R.w_q, n, C, C, eq, m->sms, m->stream);
-        c.n += 2;
-    }
-    {
-        ProfScope ps(m, 1);
-        kernels::map_attention(q, C, Cb, n, T, C, d.resnet_heads, A, m->stream);
-        ++c.n;
-    }
-    head_linear(m, c, A, n, C, R.w_c, E, R.b_c, gemm::ACT_NONE, m->pooled.get(), true, false);
-    kernels::l2_rows(m->pooled.get(), n, E, normalize, d_out, m->stream);
-    ++c.n;
+    linear(m, c, B, n * T, C, R.w_kv, 2 * C, epilogue(Cb, 2 * C, R.b_kv));
+    linear(m, c, B, n, C, R.w_q, C, epilogue(q, C, R.b_q, gemm::ACT_NONE, true), T * C);
+    profiled(m, c, 1, [&] { return kernels::map_attention(q, C, Cb, n, T, C, d.resnet_heads, A, m->stream); });
+    linear(m, c, A, n, C, R.w_c, E, epilogue(m->pooled.get(), E, R.b_c, gemm::ACT_NONE, true));
+    c.n += kernels::l2_rows(m->pooled.get(), n, E, normalize, d_out, m->stream);
 }
 
-// SigLIP vision head over the n * S token rows in x: final LayerNorm of every token -> h, K|V projection -> qkv
-// [n * S, 2w], one latent query per head attending over its image's tokens -> o [n, w], then proj -> pooled (fp32),
-// pooled + MLP(LN(pooled)), optional L2 -> d_out.
-void map_head(b200_model* m, Counter& c, const TowerW& T, int n, int normalize, float* d_out) {
-    const int S = T.tokens, w = T.d.width, M = n * S;
-    const MapW& P = T.map;
-    kernels::layernorm(m->x.get(), w, T.ln_out_w, T.ln_out_b, T.eps, M, w, nullptr, m->h.get(), m->stream);
-    head_linear(m, c, m->h.get(), M, w, P.w_kv, 2 * w, P.b_kv, gemm::ACT_NONE, m->qkv.get(), false, false);
-    {
-        ProfScope ps(m, 1);
-        kernels::map_attention(P.q, 0, m->qkv.get(), n, S, w, T.d.heads, m->o.get(), m->stream);
-    }
-    head_linear(m, c, m->o.get(), n, w, P.w_proj, w, P.b_proj, gemm::ACT_NONE, m->pooled.get(), true, false);
-    kernels::layernorm(m->pooled.get(), w, P.ln_w, P.ln_b, T.eps, n, w, nullptr, m->h.get(), m->stream);
-    head_linear(m, c, m->h.get(), n, w, P.w_fc1, P.mlp, P.b_fc1, gemm::ACT_GELU, m->u.get(), false, false);
-    head_linear(m, c, m->u.get(), n, P.mlp, P.w_fc2, w, P.b_fc2, gemm::ACT_NONE, m->pooled.get(), true, true);
-    kernels::l2_rows(m->pooled.get(), n, w, normalize, d_out, m->stream);
-    c.n += 4;
-}
-
-// images already as device uint8 [n, S, S, 3] (u8 != nullptr) or device fp32 CHW (f32 != nullptr)
-void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const float* f32, int n, int normalize,
-                          float* d_out) {
-    if (m->desc.arch == B200_ARCH_CLIP_RESNET) {
-        forward_resnet(m, c, u8, f32, n, normalize, d_out);
-        return;
-    }
-    const TowerW& T = m->vision;
+// A ViT trunk over n images (device uint8 [n, S, S, 3] u8, or device fp32 CHW f32): patch embedding, ln_pre (CLIP) and
+// the layers, leaving the n * T.tokens token rows in x.
+void forward_vit(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, const float* f32, int n) {
     const int S = T.d.image_size, p = T.d.patch, w = T.d.width;
+    float* x = m->x.get();
     // x = positional embedding (+ class embedding on each image's first row), then conv1 (no bias) of every token row
     // added onto it in place; a class-token row multiplies a zero A row.  SigLIP has no class row, and its conv bias is
     // already in T.pos.
-    kernels::vit_embed_rows(m->x.get(), T.cls, T.pos, n, T.tokens, w, m->stream);
-    gemm::Epilogue e;
-    e.residual = m->x.get();
-    e.ldr = w;
-    e.out = m->x.get();
-    e.ldo = w;
-    e.out_fp32 = 1;
+    c.n += kernels::vit_embed_rows(x, T.cls, T.pos, n, T.tokens, w, m->stream);
+    const gemm::Epilogue e = epilogue(x, w, nullptr, gemm::ACT_NONE, true, x, w);
     if (u8) {
         // uint8 pixels -> ToTensor + Normalize -> bf16 inside the GEMM's operand load: no patch matrix in HBM
         gemm::PatchGather pg;
@@ -722,68 +812,91 @@ void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const fl
             pg.mean[i] = m->desc.image_mean[i];
             pg.std[i] = m->desc.image_std[i];
         }
-        ProfScope ps(m, 0);
-        gemm::launch_patch_embed(pg, T.conv_wg, w, e, m->stream);
-        ++c.n;
+        profiled(m, c, 0, [&] { return gemm::launch_patch_embed(pg, T.conv_wg, w, e, m->stream); });
     } else {
         // preprocessed fp32 CHW tensors (the reference's parity path)
         if (!m->patches) m->patches = DeviceBuffer<__nv_bfloat16>((size_t)m->desc.max_batch * T.tokens * T.kpad);
-        kernels::im2col_f32(f32, n, S, p, T.kpad, T.cls_rows, m->patches.get(), m->stream);
+        c.n += kernels::im2col_f32(f32, n, S, p, T.kpad, T.cls_rows, m->patches.get(), m->stream);
         linear(m, c, m->patches.get(), n * T.tokens, T.kpad, T.conv_w, w, e);
-        ++c.n;
     }
-    ++c.n;
-    if (T.ln_pre_w) {
-        kernels::layernorm(m->x.get(), w, T.ln_pre_w, T.ln_pre_b, T.eps, n * T.tokens, w, m->x.get(), nullptr, m->stream);
-        ++c.n;
-    }
-    run_clip_blocks(m, c, T, n, T.tokens, attention::MASK_NONE);
-    if (m->desc.arch == B200_ARCH_SIGLIP) {
+    if (T.ln_pre_w)
+        c.n += kernels::layernorm(x, w, T.ln_pre_w, T.ln_pre_b, T.eps, n * T.tokens, w, x, nullptr, m->stream);
+    run_layers(m, c, T, n, T.tokens, attention::MASK_NONE, true);
+}
+
+// SigLIP vision head over the n * S token rows in x: final LayerNorm of every token -> h, K|V projection -> qkv
+// [n * S, 2w], one latent query per head attending over its image's tokens -> o [n, w], then proj -> pooled (fp32),
+// pooled + MLP(LN(pooled)), optional L2 -> d_out.
+void map_head(b200_model* m, Counter& c, const TowerW& T, int n, int normalize, float* d_out) {
+    const int S = T.tokens, w = T.d.width, M = n * S;
+    const MapW& P = T.map;
+    float* pooled = m->pooled.get();
+    c.n += kernels::layernorm(m->x.get(), w, T.ln_out_w, T.ln_out_b, T.eps, M, w, nullptr, m->h.get(), m->stream);
+    linear(m, c, m->h.get(), M, w, P.w_kv, 2 * w, epilogue(m->qkv.get(), 2 * w, P.b_kv));
+    __nv_bfloat16* o = m->o.get();
+    profiled(m, c, 1, [&] { return kernels::map_attention(P.q, 0, m->qkv.get(), n, S, w, T.d.heads, o, m->stream); });
+    linear(m, c, o, n, w, P.w_proj, w, epilogue(pooled, w, P.b_proj, gemm::ACT_NONE, true));
+    c.n += kernels::layernorm(pooled, w, P.ln_w, P.ln_b, T.eps, n, w, nullptr, m->h.get(), m->stream);
+    linear(m, c, m->h.get(), n, w, P.w_fc1, P.mlp, epilogue(m->u.get(), P.mlp, P.b_fc1, gemm::ACT_GELU));
+    linear(m, c, m->u.get(), n, P.mlp, P.w_fc2, w, epilogue(pooled, w, P.b_fc2, gemm::ACT_NONE, true, pooled, w));
+    c.n += kernels::l2_rows(pooled, n, w, normalize, d_out, m->stream);
+}
+
+// images already as device uint8 [n, S, S, 3] (u8 != nullptr) or device fp32 CHW (f32 != nullptr)
+void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const float* f32, int n, int normalize,
+                          float* d_out) {
+    const TowerW& T = m->vision;
+    switch (m->kind.vision) {
+    case VisionKind::CLIP_VIT:
+        forward_vit(m, c, T, u8, f32, n);
+        c.n += kernels::clip_head(m->x.get(), T.tokens, nullptr, T.ln_out_w, T.ln_out_b, T.eps, T.proj, n, T.d.width,
+                                  m->desc.embed_dim, normalize, d_out, m->pooled.get(), m->stream);
+        break;
+    case VisionKind::SIGLIP_VIT:
+        forward_vit(m, c, T, u8, f32, n);
         map_head(m, c, T, n, normalize, d_out);
-        return;
+        break;
+    case VisionKind::RESNET:
+        forward_resnet(m, c, u8, f32, n, normalize, d_out);
+        break;
     }
-    kernels::clip_head(m->x.get(), T.tokens, nullptr, T.ln_out_w, T.ln_out_b, T.eps, T.proj, n, w, m->desc.embed_dim,
-                       normalize, d_out, m->pooled.get(), m->stream);
-    c.n += 3;
 }
 
 void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const int32_t* d_mask, int n, int S,
                           int normalize, float* d_out) {
     const TowerW& T = m->text;
-    const int w = T.d.width;
-    if (m->desc.arch == B200_ARCH_CLIP || m->desc.arch == B200_ARCH_CLIP_RESNET) {
-        kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, m->x.get(), m->aux.get(), m->stream);
-        c.n += 1;
-        run_clip_blocks(m, c, T, n, S, attention::MASK_CAUSAL);
-        kernels::clip_head(m->x.get(), S, m->aux.get(), T.ln_out_w, T.ln_out_b, T.eps, T.proj, n, w, m->desc.embed_dim,
-                           normalize, d_out, m->pooled.get(), m->stream);
-        c.n += 3;
-    } else if (m->desc.arch == B200_ARCH_SIGLIP) {
-        // bidirectional blocks; ln_final of each sequence's last row (stride S rows) -> h [n, w], biased projection
-        const int E = m->desc.embed_dim;
-        kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, m->x.get(), m->aux.get(), m->stream);
-        run_clip_blocks(m, c, T, n, S, attention::MASK_NONE);
-        kernels::layernorm(m->x.get() + (size_t)(S - 1) * w, (long long)S * w, T.ln_out_w, T.ln_out_b, T.eps, n, w,
-                           nullptr, m->h.get(), m->stream);
-        head_linear(m, c, m->h.get(), n, w, T.w_tproj, E, T.b_tproj, gemm::ACT_NONE, m->pooled.get(), true, false);
-        kernels::l2_rows(m->pooled.get(), n, E, normalize, d_out, m->stream);
-        c.n += 3;
-    } else if (m->desc.arch == B200_ARCH_MPNET || m->desc.arch == B200_ARCH_XLMR) {
-        // RoBERTa position ids; XLM-R also adds its single token-type row (T.type0 is NULL for MPNet)
-        const float eps = m->desc.layer_norm_eps;
-        kernels::roberta_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, eps, n, S, w, T.d.vocab,
-                                  m->desc.pad_id, m->x.get(), m->h.get(), m->aux.get(), m->stream);
-        c.n += 1;
-        run_bert_blocks(m, c, T, n, S, eps);
-        kernels::bert_head(m->x.get(), m->aux.get(), n, S, w, m->desc.pool, normalize, d_out, m->stream);
-        c.n += 1;
-    } else {
-        kernels::bert_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, 1e-12f, n, S, w, T.d.vocab,
-                               m->x.get(), m->h.get(), m->aux.get(), m->stream);
-        c.n += 1;
-        run_bert_blocks(m, c, T, n, S, 1e-12f);
-        kernels::bert_head(m->x.get(), m->aux.get(), n, S, w, m->desc.pool, normalize, d_out, m->stream);
-        c.n += 1;
+    const int w = T.d.width, E = m->desc.embed_dim;
+    float* x = m->x.get();
+    int32_t* aux = m->aux.get();
+    switch (m->kind.text) {
+    case TextKind::CLIP:
+        // causal layers; ln_final of each sequence's eot row, projection, optional L2
+        c.n += kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, x, aux, m->stream);
+        run_layers(m, c, T, n, S, attention::MASK_CAUSAL, true);
+        c.n += kernels::clip_head(x, S, aux, T.ln_out_w, T.ln_out_b, T.eps, T.proj, n, w, E, normalize, d_out,
+                                  m->pooled.get(), m->stream);
+        break;
+    case TextKind::SIGLIP:
+        // bidirectional layers; ln_final of each sequence's last row (stride S rows) -> h [n, w], biased projection
+        c.n += kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, x, aux, m->stream);
+        run_layers(m, c, T, n, S, attention::MASK_NONE, true);
+        c.n += kernels::layernorm(x + (size_t)(S - 1) * w, (long long)S * w, T.ln_out_w, T.ln_out_b, T.eps, n, w,
+                                  nullptr, m->h.get(), m->stream);
+        linear(m, c, m->h.get(), n, w, T.w_tproj, E, epilogue(m->pooled.get(), E, T.b_tproj, gemm::ACT_NONE, true));
+        c.n += kernels::l2_rows(m->pooled.get(), n, E, normalize, d_out, m->stream);
+        break;
+    case TextKind::BERT:
+    case TextKind::ROBERTA:
+        // RoBERTa position ids count from pad_id; XLM-R also adds its single token-type row (T.type0 is NULL for MPNet)
+        if (m->kind.text == TextKind::BERT)
+            c.n += kernels::bert_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, T.eps, n, S, w,
+                                          T.d.vocab, x, m->h.get(), aux, m->stream);
+        else
+            c.n += kernels::roberta_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, T.eps, n, S,
+                                             w, T.d.vocab, m->desc.pad_id, x, m->h.get(), aux, m->stream);
+        run_layers(m, c, T, n, S, attention::MASK_KEYLEN, false);
+        c.n += kernels::bert_head(x, aux, n, S, w, m->desc.pool, normalize, d_out, m->stream);
+        break;
     }
 }
 
@@ -877,11 +990,10 @@ void encode_images_u8_dev(b200_model* m, Counter& c, const uint8_t* d_img, int n
         const int nb = std::min(cap, n - o);
         const uint8_t* src = d_img + (size_t)o * h * w * 3;
         if (h != S || w != S) {
-            if (m->desc.arch == B200_ARCH_SIGLIP)   // open_clip's SigLIP preprocessing squashes (no aspect, no crop)
-                kernels::resize_squash_u8(src, nb, h, w, S, m->resized.get(), m->stream);
+            if (m->kind.vision == VisionKind::SIGLIP_VIT)   // open_clip's SigLIP preprocessing squashes (no crop)
+                c.n += kernels::resize_squash_u8(src, nb, h, w, S, m->resized.get(), m->stream);
             else
-                kernels::resize_crop_u8(src, nb, h, w, S, m->resized.get(), m->stream);
-            c.n += 2;
+                c.n += kernels::resize_crop_u8(src, nb, h, w, S, m->resized.get(), m->stream);
             src = m->resized.get();
         }
         forward_images(m, c, src, nullptr, nb, normalize, d_out + (size_t)o * m->desc.embed_dim);
@@ -899,9 +1011,9 @@ void encode_tokens_dev(b200_model* m, Counter& c, const int32_t* d_ids, const in
 }
 
 void check_tokens_args(b200_model* m, int n, int S) {
-    MB_CHECK_ARG(m->text.present, "this model has no text tower");
+    MB_CHECK_ARG(m->kind.text != TextKind::NONE, "this model has no text tower");
     MB_CHECK_ARG(n > 0, "n must be positive");
-    MB_CHECK_ARG(S > 0 && S <= m->text.max_pos, "sequence length %d out of range (1..%d)", S, m->text.max_pos);
+    MB_CHECK_ARG(S > 0 && S <= m->text.tokens, "sequence length %d out of range (1..%d)", S, m->text.tokens);
 }
 
 }  // namespace
@@ -919,65 +1031,10 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
                      "unknown arch %d", desc->arch);
         MB_CHECK_ARG(desc->max_batch > 0, "max_batch must be positive");
         MB_CHECK_ARG(desc->embed_dim > 0 && desc->embed_dim <= 4096, "embed_dim out of range");
-        const bool siglip = desc->arch == B200_ARCH_SIGLIP;
-        const bool resnet = desc->arch == B200_ARCH_CLIP_RESNET;
-        const bool has_vision = ((desc->arch == B200_ARCH_CLIP || siglip) && desc->vision.layers > 0) ||
-                                (resnet && desc->resnet_layers[0] > 0);
-        if (siglip) {
-            MB_CHECK_ARG(desc->layer_norm_eps > 0.f, "SigLIP: layer_norm_eps must be positive");
-            MB_CHECK_ARG(desc->embed_dim % 32 == 0, "SigLIP: embed_dim %d must be a multiple of 32", desc->embed_dim);
-        }
-        const bool has_text = desc->text.layers > 0;
-        MB_CHECK_ARG(has_vision || has_text, "model has no tower");
-        if (has_vision && resnet) {
-            const int wd = desc->resnet_width, S = desc->resnet_image_size;
-            for (int s = 0; s < 4; ++s)
-                MB_CHECK_ARG(desc->resnet_layers[s] > 0 && desc->resnet_layers[s] <= 64, "resnet_layers[%d] = %d out of range",
-                             s, desc->resnet_layers[s]);
-            // the stem's 3 x 3 convs gather width / 2 channels: a power of two >= 32
-            MB_CHECK_ARG(wd >= 64 && wd <= 128 && (wd & (wd - 1)) == 0, "resnet_width %d must be 64 or 128", wd);
-            MB_CHECK_ARG(S > 0 && S % 32 == 0 && S <= 512, "resnet_image_size %d must be a multiple of 32, <= 512", S);
-            MB_CHECK_ARG(desc->resnet_heads * 64 == 32 * wd, "attention pool: head_dim must be 64 (%d channels, %d heads)",
-                         32 * wd, desc->resnet_heads);
-            MB_CHECK_ARG(desc->embed_dim % 32 == 0, "CLIP ResNet: embed_dim %d must be a multiple of 32", desc->embed_dim);
-            for (int i = 0; i < 3; ++i) MB_CHECK_ARG(desc->image_std[i] > 0.f, "image_std must be positive");
-        } else if (has_vision) {
-            check_tower(desc->vision, "vision");
-            MB_CHECK_ARG(desc->vision.patch > 0 && desc->vision.image_size % desc->vision.patch == 0,
-                         "image_size must be a multiple of patch");
-            for (int i = 0; i < 3; ++i) MB_CHECK_ARG(desc->image_std[i] > 0.f, "image_std must be positive");
-            if (siglip) {
-                // the MAP head has no projection; its single-query attention runs head_dim 64 only
-                MB_CHECK_ARG(desc->embed_dim == desc->vision.width, "SigLIP: embed_dim %d must equal the vision width %d",
-                             desc->embed_dim, desc->vision.width);
-                MB_CHECK_ARG(desc->vision.width == desc->vision.heads * 64,
-                             "SigLIP: vision head_dim must be 64 (width %d, heads %d)", desc->vision.width,
-                             desc->vision.heads);
-            }
-        }
-        if (has_text) {
-            check_tower(desc->text, "text");
-            MB_CHECK_ARG(desc->text.ctx > 0 && desc->text.vocab > 0, "text.ctx and text.vocab must be positive");
-            if (desc->arch != B200_ARCH_CLIP && !siglip && !resnet)
-                MB_CHECK_ARG(desc->embed_dim == desc->text.width, "BERT / MPNet / XLM-R embed_dim must equal width");
-            if (desc->arch == B200_ARCH_MPNET) {
-                MB_CHECK_ARG(desc->text.width == desc->text.heads * 64, "MPNet: head_dim must be 64 (width %d, heads %d)",
-                             desc->text.width, desc->text.heads);
-                MB_CHECK_ARG(desc->layer_norm_eps > 0.f, "MPNet: layer_norm_eps must be positive");
-                MB_CHECK_ARG(desc->pad_id >= 0 && desc->pad_id < desc->text.vocab, "MPNet: pad_id %d out of range",
-                             desc->pad_id);
-                MB_CHECK_ARG(desc->rel_buckets >= 4 && desc->rel_buckets % 2 == 0 && desc->rel_max_distance > desc->rel_buckets / 4,
-                             "MPNet: bad relative-bias buckets (%d) / max distance (%d)", desc->rel_buckets,
-                             desc->rel_max_distance);
-                MB_CHECK_ARG(desc->text.ctx <= 1024, "MPNet: sequences of up to 1024 tokens are supported (ctx %d)",
-                             desc->text.ctx);
-            }
-            if (desc->arch == B200_ARCH_XLMR) {
-                MB_CHECK_ARG(desc->layer_norm_eps > 0.f, "XLM-R: layer_norm_eps must be positive");
-                MB_CHECK_ARG(desc->pad_id >= 0 && desc->pad_id < desc->text.vocab, "XLM-R: pad_id %d out of range",
-                             desc->pad_id);
-            }
-        }
+        const Kinds kind = resolve_kinds(*desc);
+        MB_CHECK_ARG(kind.vision != VisionKind::NONE || kind.text != TextKind::NONE, "model has no tower");
+        check_vision(*desc, kind.vision);
+        check_text(*desc, kind);
         DeviceGuard g(device);
         std::unique_ptr<b200_model> m(new b200_model());   // released under the guard if the set-up fails
         m->device = device;
@@ -987,11 +1044,10 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         m->stream = m->own_stream.get();
         m->ev0 = make_event();
         m->ev1 = make_event();
-        m->vision.present = has_vision;
-        m->vision.d = desc->vision;
-        if (resnet) m->vision.d.image_size = desc->resnet_image_size;
-        m->text.present = has_text;
-        m->text.d = desc->text;
+        m->kind = kind;
+        if (kind.vision == VisionKind::CLIP_VIT || kind.vision == VisionKind::SIGLIP_VIT) m->vision.d = desc->vision;
+        if (kind.vision == VisionKind::RESNET) m->vision.d.image_size = desc->resnet_image_size;   // (no layers)
+        if (kind.text != TextKind::NONE) m->text.d = desc->text;
         gemm::configure();
         *out = m.release();
     });
@@ -1016,7 +1072,8 @@ int b200_model_load_tensor(b200_model* m, const char* name, const float* data, i
         MB_CUDA(cudaMemcpy(b.get(), data, (size_t)numel * sizeof(float), cudaMemcpyHostToDevice));
         std::string key = name;
         // XLMRobertaModel checkpoints saved from a task head carry the encoder under "roberta."
-        if (m->desc.arch == B200_ARCH_XLMR && key.compare(0, 8, "roberta.") == 0) key.erase(0, 8);
+        const bool xlmr = m->kind.text == TextKind::ROBERTA && !m->kind.mpnet;
+        if (xlmr && key.compare(0, 8, "roberta.") == 0) key.erase(0, 8);
         m->raw[key] = std::move(b);
     });
 }
@@ -1027,99 +1084,17 @@ int b200_model_finalize(b200_model* m) {
         std::lock_guard<std::mutex> lk(m->mu);
         if (m->finalized) return;
         DeviceGuard g(m->device);
-        const int E = m->desc.embed_dim;
+        build_vision(m);
+        build_text(m);
+        // workspaces for the towers' token rows, capped at ~24 GB of activations: larger calls are processed in
+        // sub-batches
+        const long long B = m->desc.max_batch, E = m->desc.embed_dim;
         long long max_tok = 0, max_w = 0, max_mlp = 0;
-        const bool siglip = m->desc.arch == B200_ARCH_SIGLIP;
-        if (siglip) m->vision.eps = m->text.eps = m->desc.layer_norm_eps;
-        if (m->vision.present && m->desc.arch == B200_ARCH_CLIP_RESNET) {
-            TowerW& T = m->vision;
-            build_resnet(m, T);
-            max_tok = std::max(max_tok, (long long)m->desc.max_batch * T.tokens);
-            m->resized = DeviceBuffer<uint8_t>((size_t)m->desc.max_batch * T.d.image_size * T.d.image_size * 3);
-        } else if (m->vision.present) {
-            TowerW& T = m->vision;
-            const long long w = T.d.width, p = T.d.patch;
-            T.grid = T.d.image_size / T.d.patch;
-            T.cls_rows = siglip ? 0 : 1;
-            T.tokens = T.grid * T.grid + T.cls_rows;
-            const int K = 3 * (int)p * (int)p;
-            T.kpad = (int)round_up((size_t)K, 64);
-            const float* conv = param(m, siglip ? "visual.trunk.patch_embed.proj.weight" : "visual.conv1.weight", w * K);
-            __nv_bfloat16* cw = derived_buffer<__nv_bfloat16>(m, (size_t)w * T.kpad);
-            kernels::pad_rows_to_bf16(conv, (int)w, K, T.kpad, cw, m->stream);
-            MB_CUDA(cudaStreamSynchronize(m->stream));
-            T.conv_w = cw;
-            __nv_bfloat16* cg = derived_buffer<__nv_bfloat16>(m, (size_t)w * gemm::patch_gather_k((int)p));
-            kernels::patch_weight_rows(conv, (int)w, (int)p, gemm::patch_gather_kbpd((int)p), cg, m->stream);
-            MB_CUDA(cudaStreamSynchronize(m->stream));
-            T.conv_wg = cg;
-            if (siglip) {
-                build_siglip_vision(m, T);
-            } else {
-                T.cls = param(m, "visual.class_embedding", w);
-                T.pos = param(m, "visual.positional_embedding", (long long)T.tokens * w);
-                T.ln_pre_w = param(m, "visual.ln_pre.weight", w);
-                T.ln_pre_b = param(m, "visual.ln_pre.bias", w);
-                build_preln_layers(m, T, "visual.transformer.resblocks.", OPEN_CLIP_BLOCK);
-                T.ln_out_w = param(m, "visual.ln_post.weight", w);
-                T.ln_out_b = param(m, "visual.ln_post.bias", w);
-                T.proj = param(m, "visual.proj", w * E);
-            }
-            max_tok = std::max(max_tok, (long long)m->desc.max_batch * T.tokens);
-            max_w = std::max(max_w, w);
-            max_mlp = std::max(max_mlp, (long long)std::max(T.d.mlp, T.map.mlp));
-            m->resized = DeviceBuffer<uint8_t>((size_t)m->desc.max_batch * T.d.image_size * T.d.image_size * 3);
+        for (const TowerW* T : {&m->vision, &m->text}) {
+            max_tok = std::max(max_tok, B * T->tokens);   // (0 for a missing tower)
+            max_w = std::max<long long>(max_w, T->d.width);
+            max_mlp = std::max<long long>({max_mlp, T->d.mlp, T->map.mlp});
         }
-        if (m->text.present) {
-            TowerW& T = m->text;
-            const long long w = T.d.width;
-            T.max_pos = T.d.ctx;
-            if (m->desc.arch == B200_ARCH_CLIP || m->desc.arch == B200_ARCH_CLIP_RESNET) {
-                T.tok = param(m, "token_embedding.weight", (long long)T.d.vocab * w);
-                T.pos = param(m, "positional_embedding", (long long)T.d.ctx * w);
-                build_preln_layers(m, T, "transformer.resblocks.", OPEN_CLIP_BLOCK);
-                T.ln_out_w = param(m, "ln_final.weight", w);
-                T.ln_out_b = param(m, "ln_final.bias", w);
-                T.proj = param(m, "text_projection", w * E);
-            } else if (siglip) {
-                T.tok = param(m, "text.token_embedding.weight", (long long)T.d.vocab * w);
-                T.pos = param(m, "text.positional_embedding", (long long)T.d.ctx * w);
-                build_preln_layers(m, T, "text.transformer.resblocks.", OPEN_CLIP_BLOCK);
-                T.ln_out_w = param(m, "text.ln_final.weight", w);
-                T.ln_out_b = param(m, "text.ln_final.bias", w);
-                T.w_tproj = to_bf16(m, "text.text_projection.weight", E * w);
-                T.b_tproj = param(m, "text.text_projection.bias", E);
-            } else if (m->desc.arch == B200_ARCH_MPNET || m->desc.arch == B200_ARCH_XLMR) {
-                T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
-                // positions run pad_id + 1 .. pad_id + ctx (pads take pad_id): the table has at least ctx + pad_id + 1 rows
-                const long long pos_rows = param_rows(m, "embeddings.position_embeddings.weight", w);
-                MB_CHECK_ARG(pos_rows >= (long long)T.d.ctx + m->desc.pad_id + 1,
-                             "embeddings.position_embeddings has %lld rows; %d tokens with pad id %d need %d", pos_rows,
-                             T.d.ctx, m->desc.pad_id, T.d.ctx + m->desc.pad_id + 1);
-                T.pos = param(m, "embeddings.position_embeddings.weight", pos_rows * w);
-                T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
-                T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
-                if (m->desc.arch == B200_ARCH_XLMR) {
-                    T.type0 = param(m, "embeddings.token_type_embeddings.weight", w);   // type_vocab_size 1
-                    build_bert_layers(m, T, BERT_NAMES);
-                } else {
-                    build_bert_layers(m, T, MPNET_NAMES);
-                    T.rel_bias = build_rel_bias(m, T);
-                }
-            } else {
-                T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
-                T.pos = param(m, "embeddings.position_embeddings.weight", (long long)T.d.ctx * w);
-                const int tv = std::max(1, m->desc.type_vocab);
-                T.type0 = param(m, "embeddings.token_type_embeddings.weight", (long long)tv * w);  // row 0 is used
-                T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
-                T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
-                build_bert_layers(m, T, BERT_NAMES);
-            }
-            max_tok = std::max(max_tok, (long long)m->desc.max_batch * T.d.ctx);
-            max_w = std::max(max_w, w);
-            max_mlp = std::max(max_mlp, (long long)T.d.mlp);
-        }
-        // cap the workspace at ~24 GB of activations: larger calls are processed in sub-batches
         const long long bytes_per_tok = std::max<long long>(1, max_w * (4 + 2 + 6 + 2) + max_mlp * 2);
         const long long cap_tok = (24LL << 30) / bytes_per_tok;
         m->max_tokens = std::min(max_tok, std::max<long long>(cap_tok, 1024));
@@ -1128,10 +1103,14 @@ int b200_model_finalize(b200_model* m) {
         m->qkv = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_w * 3);
         m->o = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_w);
         m->u = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_mlp);
+        if (m->kind.vision != VisionKind::NONE) {
+            const int S = m->vision.d.image_size;
+            m->resized = DeviceBuffer<uint8_t>((size_t)B * S * S * 3);
+        }
         MB_CUDA(cudaStreamSynchronize(m->stream));
-        m->aux = DeviceBuffer<int32_t>((size_t)m->desc.max_batch);
-        m->out_dev = DeviceBuffer<float>((size_t)m->desc.max_batch * E);
-        m->pooled = DeviceBuffer<float>((size_t)m->desc.max_batch * std::max<long long>(max_w, E));
+        m->aux = DeviceBuffer<int32_t>((size_t)B);
+        m->out_dev = DeviceBuffer<float>((size_t)B * E);
+        m->pooled = DeviceBuffer<float>((size_t)B * std::max(max_w, E));
         MB_CUDA(cudaStreamSynchronize(m->stream));
         m->finalized = true;
     });
@@ -1141,7 +1120,7 @@ int b200_model_encode_images_u8(b200_model* m, const uint8_t* hwc, int n, int h,
     return guarded([&] {
         require_ready(m);
         MB_CHECK_ARG(hwc && out, "NULL buffer");
-        MB_CHECK_ARG(m->vision.present, "this model has no vision tower");
+        MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
         MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
         std::lock_guard<std::mutex> lk(m->mu);
         DeviceGuard g(m->device);
@@ -1167,7 +1146,7 @@ int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int nor
     return guarded([&] {
         require_ready(m);
         MB_CHECK_ARG(chw && out, "NULL buffer");
-        MB_CHECK_ARG(m->vision.present, "this model has no vision tower");
+        MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
         MB_CHECK_ARG(n > 0, "n must be positive");
         std::lock_guard<std::mutex> lk(m->mu);
         DeviceGuard g(m->device);
@@ -1196,7 +1175,7 @@ int b200_model_encode_tokens(b200_model* m, const int32_t* ids, const int32_t* a
         require_ready(m);
         MB_CHECK_ARG(ids && out, "NULL buffer");
         check_tokens_args(m, n, seq);
-        if (attn_mask && m->desc.arch != B200_ARCH_CLIP && m->desc.arch != B200_ARCH_CLIP_RESNET) {
+        if (attn_mask && m->kind.text != TextKind::CLIP) {
             // the kernels implement prefix (right-padded) masks, which is what the tokenizer call at
             // hugging_face_model.py:179-185 produces
             for (int b = 0; b < n; ++b) {
@@ -1237,7 +1216,7 @@ int b200_model_encode_images_u8_device(b200_model* m, const uint8_t* d_hwc, int 
     return guarded([&] {
         require_ready(m);
         MB_CHECK_ARG(d_hwc && d_out, "NULL buffer");
-        MB_CHECK_ARG(m->vision.present, "this model has no vision tower");
+        MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
         MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
         std::lock_guard<std::mutex> lk(m->mu);
         DeviceGuard g(m->device);
