@@ -432,8 +432,9 @@ struct ExactParams {
     double* out_score;
 };
 
-// `val` is the exact ordering key of the re-score pass: the dot product, or minus the squared distance (euclidean)
-__device__ __forceinline__ double closeness_from_dot(double dot, int metric) {
+// `dot` is the exact dot product of the re-score pass, or minus the squared distance (euclidean).  Device code
+// takes CUDA's sqrt / acos, host code (host_finalize) libm's.
+__host__ __device__ __forceinline__ double closeness_from_dot(double dot, int metric) {
     switch (metric) {
         case B200_METRIC_EUCLIDEAN:
             return 1.0 / (1.0 + sqrt(fmax(-dot, 0.0)));
@@ -446,6 +447,73 @@ __device__ __forceinline__ double closeness_from_dot(double dot, int metric) {
         default:
             return dot;
     }
+}
+
+// Exact ordering key of a re-scored row: its dot product, or with score modifiers the modified score
+// mult * closeness + add of its document (separate multiply and add, no fma, as oracle/score_oracle.c computes it).
+// `doc` is read only with modifiers.
+__device__ __forceinline__ double exact_key(const ExactParams& p, double dot, const int32_t& doc) {
+    if (!p.mod64) return dot;
+    const double2 ma = p.mod64[doc];
+    return __dadd_rn(__dmul_rn(ma.x, closeness_from_dot(dot, p.metric)), ma.y);
+}
+
+// Score returned for an exact key: the modified score itself, or the closeness of the dot product.
+__host__ __device__ __forceinline__ double key_score(double key, int metric, bool modified) {
+    return modified ? key : closeness_from_dot(key, metric);
+}
+
+// Scan-domain key (what the scan's approximate key approximates) of an exact key: the modified score, the dot
+// product, or for euclidean -|q - e|^2 + |q|^2 = 2 q.e - |e|^2.  `qn2` (|q|^2) is read only for euclidean.
+__host__ __device__ __forceinline__ double scan_domain_key(double key, int metric, bool modified, const double& qn2) {
+    return modified ? key : (metric == B200_METRIC_EUCLIDEAN ? key + qn2 : key);
+}
+
+// Largest float <= x.
+__host__ __device__ __forceinline__ float float_rd(double x) {
+#ifdef __CUDA_ARCH__
+    return __double2float_rd(x);
+#else
+    const float f = (float)x;
+    return (double)f > x ? std::nextafterf(f, -INFINITY) : f;
+#endif
+}
+
+// Records query q's exact selection (nd distinct documents, k-th scan-domain key ek) and settles the query: either
+// resolved, or flagged for another collect pass with threshold next_L() (only evaluated then).  Returns true when
+// the query needs that pass; the caller counts it in n_need.
+template <class NextL>
+__host__ __device__ __forceinline__ bool settle(QState* qs, int q, int nd, double ek, bool resolved, NextL next_L) {
+    qs->ndocs[q] = nd;
+    qs->ek[q] = ek;
+    qs->cnt[q] = 0;
+    if (resolved) {
+        qs->status[q] = Q_RESOLVED;
+        qs->L[q] = INFINITY;
+    } else {
+        qs->L[q] = next_L();
+        qs->status[q] = Q_NEED;
+    }
+    return !resolved;
+}
+
+// Settles a query after an exact selection over every row the collect pass found at threshold L (finalize_kernel
+// and host_finalize).  A row that was not collected has approximate key < L, so exact key < L + eps: the top-k is
+// exact once the k-th exact key reaches L + eps, or when L = -inf collected every live row.  Otherwise the next
+// threshold is ek - eps rounded down (every row whose exact key can reach ek has approximate key >= it), or, with
+// fewer than k documents above L, L lowered by max(8 eps, 5 % of |L|); -inf (collect everything) when that is not
+// below L.
+__host__ __device__ __forceinline__ bool settle_collected(QState* qs, int q, int k, int nd, double ek) {
+    const float L = qs->L[q];
+    const float eps = qs->eps[q];
+    const bool resolved = (L == -INFINITY) || (nd >= k && ek >= (double)L + (double)eps);
+    return settle(qs, q, nd, ek, resolved, [&] {
+        float nl;
+        if (nd >= k) nl = float_rd(ek - (double)eps);
+        else nl = L - fmaxf(8.0f * eps, 0.05f * fabsf(L));
+        if (!(nl < L)) nl = -INFINITY;
+        return nl;
+    });
 }
 
 // Exact fp64 dot product (or minus squared distance) of query `qv` and corpus row `cv`, computed by one warp.
@@ -495,12 +563,7 @@ __device__ void exact_select(const ExactParams& p, int q, int n, const int32_t* 
         const double tot = warp_exact_dot(qv, p.corpus + (size_t)row * p.dim, p.dim, p.metric, lane);
         if (lane == 0) {
             x_dot[c] = tot;
-            double key = tot;
-            if (p.mod64) {   // the ordering key becomes the modified score (separate multiply and add, no fma)
-                const double2 ma = p.mod64[s_doc[c]];
-                key = __dadd_rn(__dmul_rn(ma.x, closeness_from_dot(tot, p.metric)), ma.y);
-            }
-            x_key[c] = key;
+            x_key[c] = exact_key(p, tot, s_doc[c]);
         }
     }
     if (threadIdx.x == 0) {
@@ -529,9 +592,8 @@ __device__ void exact_select(const ExactParams& p, int q, int n, const int32_t* 
             const size_t o = (size_t)q * p.k + rank;
             p.out_doc[o] = d + p.doc_offset;
             p.out_row[o] = s_row[i];
-            p.out_score[o] = p.mod64 ? v : closeness_from_dot(v, p.metric);
-            if (rank == p.k - 1)
-                *s_ek = p.mod64 ? v : (p.metric == B200_METRIC_EUCLIDEAN ? v + p.qs->qn2x[q] : v);
+            p.out_score[o] = key_score(v, p.metric, p.mod64);
+            if (rank == p.k - 1) *s_ek = scan_domain_key(v, p.metric, p.mod64, p.qs->qn2x[q]);
         }
     }
     __syncthreads();
@@ -690,19 +752,12 @@ __global__ void __launch_bounds__(MERGE_THREADS) merge_kernel(MergeParams p) {
         const float tau = fmaxf(key_flt(s_tail_max), tau_m);
         const int nd = s_ndocs;
         const bool resolved = nd >= k ? (s_ek > (double)tau + (double)eps) : (tau == -INFINITY);
-        qs->ndocs[q] = nd;
-        qs->ek[q] = s_ek;
-        qs->cnt[q] = 0;
-        if (resolved) {
-            qs->status[q] = Q_RESOLVED;
-            qs->L[q] = INFINITY;
-        } else {
+        const bool need = settle(qs, q, nd, s_ek, resolved, [&] {
             // every row whose exact key can reach the k-th one has approximate key >= ek - eps; with fewer than k
             // documents in hand start from the weakest list entry
-            qs->L[q] = nd >= k ? __double2float_rd(s_ek - (double)eps) : key_flt(s_union_min);
-            qs->status[q] = Q_NEED;
-            atomicAdd(&qs->n_need, 1);
-        }
+            return nd >= k ? float_rd(s_ek - (double)eps) : key_flt(s_union_min);
+        });
+        if (need) atomicAdd(&qs->n_need, 1);
     }
 }
 
@@ -743,27 +798,7 @@ __global__ void __launch_bounds__(FIN_THREADS) finalize_kernel(FinalizeParams p)
     __syncthreads();
     exact_select<FIN_THREADS>(p.ex, q, cnt, s_row, s_doc, x_dot, x_key, x_rep, &s_ndocs, &s_ek);
     __syncthreads();
-    if (threadIdx.x == 0) {
-        const float L = qs->L[q];
-        const float eps = qs->eps[q];
-        const int nd = s_ndocs;
-        // rows not collected have approximate key < L, i.e. exact key < L + eps
-        const bool resolved = (L == -INFINITY) || (nd >= k && s_ek >= (double)L + (double)eps);
-        qs->ndocs[q] = nd;
-        qs->ek[q] = s_ek;
-        qs->cnt[q] = 0;
-        if (resolved) {
-            qs->status[q] = Q_RESOLVED;
-            qs->L[q] = INFINITY;
-        } else {
-            float nl;
-            if (nd >= k) nl = __double2float_rd(s_ek - (double)eps);
-            else nl = L - fmaxf(8.0f * eps, 0.05f * fabsf(L));   // too few documents above L: look deeper
-            if (!(nl < L)) nl = -INFINITY;
-            qs->L[q] = nl;
-            atomicAdd(&qs->n_need, 1);
-        }
-    }
+    if (threadIdx.x == 0 && settle_collected(qs, q, k, s_ndocs, s_ek)) atomicAdd(&qs->n_need, 1);
 }
 
 // Host-finalize support: exact dot and key of every collected row of one query (warp per row).
@@ -776,11 +811,7 @@ __global__ void exact_keys_kernel(ExactParams p, int q, const int32_t* rows, int
     const double tot = warp_exact_dot(p.qh + (size_t)q * p.dim, p.corpus + (size_t)row * p.dim, p.dim, p.metric, lane);
     if (lane == 0) {
         const int d = p.doc_of_row[row];
-        double key = tot;
-        if (p.mod64) {
-            const double2 ma = p.mod64[d];
-            key = __dadd_rn(__dmul_rn(ma.x, closeness_from_dot(tot, p.metric)), ma.y);
-        }
+        const double key = exact_key(p, tot, d);
         out_dot[i] = tot;
         out_key[i] = key;
         out_doc[i] = d;
@@ -1252,6 +1283,14 @@ RowArrays alloc_rows(const b200_index* ix, int64_t cap) {
             ix->metric == B200_METRIC_EUCLIDEAN ? DeviceBuffer<float>((size_t)cap) : DeviceBuffer<float>()};
 }
 
+// Replaces the index's row arrays by `r` (capacity `cap`); the caller has copied the rows that stay.
+void adopt_rows(b200_index* ix, RowArrays&& r, int64_t cap) {
+    ix->corpus = std::move(r.corpus);
+    ix->doc_of_row = std::move(r.doc_of_row);
+    ix->row_n2 = std::move(r.row_n2);
+    ix->capacity = cap;
+}
+
 void ensure_capacity(b200_index* ix, int64_t need_rows) {
     if (need_rows <= ix->capacity) return;
     int64_t cap = std::max<int64_t>(need_rows, ix->capacity + ix->capacity / 2);
@@ -1267,10 +1306,7 @@ void ensure_capacity(b200_index* ix, int64_t need_rows) {
                                     cudaMemcpyDeviceToDevice, ix->stream));
     }
     MB_CUDA(cudaStreamSynchronize(ix->stream));
-    ix->corpus = std::move(r.corpus);
-    ix->doc_of_row = std::move(r.doc_of_row);
-    ix->row_n2 = std::move(r.row_n2);
-    ix->capacity = cap;
+    adopt_rows(ix, std::move(r), cap);
 }
 
 void ensure_out_k(b200_index* ix, int k) {
@@ -1482,7 +1518,8 @@ void fetch_qstate(b200_index* ix) {
 
 // Exact selection of one query's collected rows on the host (more rows than the device finalize holds in shared
 // memory: deep pagination, thousands of exact ties).  Keys are computed on the device (exact_keys_kernel); the
-// dedup / sort is the same rule as exact_select.  Returns true when the query is resolved.
+// dedup / sort is the same rule as exact_select, and the query is settled by the device finalize's rule
+// (settle_collected).  Returns true when the query needs another collect pass.
 bool host_finalize(b200_index* ix, int q, int nq, int k, const GroupOut& out, int cnt) {
     ++ix->stat_host_finalize;
     DeviceBuffer<double> d_dot((size_t)cnt), d_key((size_t)cnt);
@@ -1516,43 +1553,19 @@ bool host_finalize(b200_index* ix, int q, int nq, int k, const GroupOut& out, in
     std::sort(v.begin(), v.end(), [](const Hit& a, const Hit& b) { return a.key > b.key || (a.key == b.key && a.doc < b.doc); });
     const int nd = (int)v.size();
     QState* h = ix->h_qs.get();
-    const double L = h->L[q], eps = h->eps[q];
-    double ek = -std::numeric_limits<double>::infinity();
-    if (nd >= k) ek = ix->mod_active ? v[k - 1].key : (ix->metric == B200_METRIC_EUCLIDEAN ? v[k - 1].key + h->qn2x[q] : v[k - 1].key);
-    const bool resolved = std::isinf(L) ? (L < 0) : (nd >= k && ek >= L + eps);
+    const double ek = nd >= k ? scan_domain_key(v[k - 1].key, ix->metric, ix->mod_active, h->qn2x[q]) : -INFINITY;
     std::vector<int32_t> o_doc(k, -1), o_row(k, -1);
     std::vector<double> o_sc(k, -std::numeric_limits<double>::infinity());
     for (int i = 0; i < k && i < nd; ++i) {
         o_doc[i] = v[i].doc + ix->doc_offset;
         o_row[i] = v[i].row;
-        if (ix->mod_active) o_sc[i] = v[i].key;
-        else {
-            const double d = v[i].key;
-            switch (ix->metric) {   // same expressions as closeness_from_dot
-                case B200_METRIC_EUCLIDEAN: o_sc[i] = 1.0 / (1.0 + std::sqrt(std::max(-d, 0.0))); break;
-                case B200_METRIC_PRENORMALIZED_ANGULAR: o_sc[i] = 1.0 / (1.0 + (1.0 - d)); break;
-                case B200_METRIC_ANGULAR: o_sc[i] = 1.0 / (1.0 + std::acos(std::min(1.0, std::max(-1.0, d)))); break;
-                default: o_sc[i] = d;
-            }
-        }
+        o_sc[i] = key_score(v[i].key, ix->metric, ix->mod_active);
     }
     MB_CUDA(cudaMemcpyAsync(out.doc + (size_t)q * k, o_doc.data(), (size_t)k * 4, cudaMemcpyHostToDevice, ix->stream));
     MB_CUDA(cudaMemcpyAsync(out.row + (size_t)q * k, o_row.data(), (size_t)k * 4, cudaMemcpyHostToDevice, ix->stream));
     MB_CUDA(cudaMemcpyAsync(out.score + (size_t)q * k, o_sc.data(), (size_t)k * 8, cudaMemcpyHostToDevice, ix->stream));
     MB_CUDA(cudaStreamSynchronize(ix->stream));
-    h->ndocs[q] = nd;
-    h->ek[q] = ek;
-    if (resolved) {
-        h->status[q] = Q_RESOLVED;
-        h->L[q] = INFINITY;
-    } else {
-        float nl;
-        if (nd >= k) nl = std::nextafterf((float)(ek - eps), -INFINITY);
-        else nl = (float)L - std::max(8.0f * (float)eps, 0.05f * std::fabs((float)L));
-        if (!(nl < (float)L)) nl = -INFINITY;
-        h->L[q] = nl;
-    }
-    return resolved;
+    return settle_collected(h, q, k, nd, ek);
 }
 
 // One group of <= MQ queries already converted into ix->qh.get().
@@ -1628,11 +1641,8 @@ void search_group(b200_index* ix, int nq, int k, const GroupOut& out, bool recor
             fetch_qstate(ix);
         } else {
             int need = 0;
-            for (int q = 0; q < nq; ++q) {
-                if (h->status[q] != Q_NEED) continue;
-                if (!host_finalize(ix, q, nq, k, out, h->cnt[q])) ++need;
-                h->cnt[q] = 0;
-            }
+            for (int q = 0; q < nq; ++q)
+                if (h->status[q] == Q_NEED && host_finalize(ix, q, nq, k, out, h->cnt[q])) ++need;
             h->n_need = need;
         }
     }
@@ -1656,12 +1666,21 @@ void search_device(b200_index* ix, const float* d_q, int nq, int k, int32_t* d_o
     }
 }
 
-void check_search_args(b200_index* ix, const void* q, int nq, int k, const void* a, const void* b, const void* c) {
-    MB_CHECK_ARG(ix != nullptr, "index is NULL");
+void check_search_args(const void* q, int nq, int k, const void* a, const void* b, const void* c) {
     MB_CHECK_ARG(q && a && b && c, "NULL buffer");
     MB_CHECK_ARG(nq > 0, "nq must be positive (got %d)", nq);
     MB_CHECK_ARG(k > 0, "k must be positive (got %d)", k);
     MB_CHECK_ARG(k <= 11000, "k = %d exceeds 11000 (Marqo's own limit + offset cap, api/configs.py:24-25)", k);
+}
+
+// Largest of the caller's host document ids (-1 when n == 0); a negative id is rejected.
+int64_t max_doc_id(const int32_t* doc_ids, int64_t n) {
+    int64_t hi = -1;
+    for (int64_t i = 0; i < n; ++i) {
+        MB_CHECK_ARG(doc_ids[i] >= 0, "doc_ids[%lld] is negative", (long long)i);
+        hi = std::max<int64_t>(hi, doc_ids[i]);
+    }
+    return hi;
 }
 
 // largest document number among device-resident ids (ingest path; sizes the score-modifier tables)
@@ -1821,19 +1840,73 @@ void validate_opts(const b200_search_opts* o) {
     MB_CHECK_ARG(o->filter_bits != nullptr || o->filter_docs == 0, "filter_docs > 0 with filter_bits == NULL");
 }
 
-// Runs `append` (add_rows_device calls) and checks the appended values; nothing of a rejected batch stays searchable.
+// Body of an index entry point: `body` runs with the index locked and its device current; errors become the
+// returned status code.
 template <class F>
-void add_checked(b200_index* ix, F&& append) {
-    const int64_t rows_before = ix->n_rows;
-    const bool docs_before = ix->has_docs;
-    try {
-        append();
-        check_input_flags(ix, "embeddings");
-    } catch (...) {
-        ix->n_rows = rows_before;
-        ix->has_docs = docs_before;
-        throw;
-    }
+int with_index(b200_index* ix, const char* null_msg, F&& body) {
+    return guarded([&] {
+        MB_CHECK_ARG(ix != nullptr, "%s", null_msg);
+        std::lock_guard<std::mutex> lk(ix->mu);
+        DeviceGuard g(ix->device);
+        body();
+    });
+}
+template <class F>
+int with_index(b200_index* ix, F&& body) {
+    return with_index(ix, "index is NULL", body);
+}
+
+// The rows of one add call: vectors and optional document ids (nullptr: row i is document n_rows + i), each in host
+// or in device memory.
+struct AddRows {
+    const float* vecs;
+    bool vecs_on_host;
+    const int32_t* doc_ids;
+    bool ids_on_host;
+};
+
+// Body of the add entry points; `args_ok` / `null_msg` is the entry point's own NULL-argument check.  Host vectors
+// are staged through the device 64 Ki rows at a time.
+int add(b200_index* ix, const AddRows& a, int64_t m, bool args_ok, const char* null_msg) {
+    return with_index(ix, [&] {
+        MB_CHECK_ARG(m >= 0, "m must be >= 0");
+        if (m == 0) return;
+        MB_CHECK_ARG(args_ok, "%s", null_msg);
+        MB_CHECK_ARG(ix->n_rows + m < (int64_t)INT32_MAX, "row count would exceed 2^31-1");
+        const bool host_ids = a.doc_ids && a.ids_on_host;
+        const int64_t hi = host_ids ? std::max(ix->max_doc, max_doc_id(a.doc_ids, m)) : ix->max_doc;
+        const int64_t chunk = a.vecs_on_host ? std::min<int64_t>(m, 1 << 16) : m;
+        DeviceBuffer<float> d_v(a.vecs_on_host ? (size_t)chunk * ix->dim : 0);
+        DeviceBuffer<int32_t> d_d(host_ids ? (size_t)chunk : 0);
+        const int64_t rows_before = ix->n_rows;   // nothing of a rejected batch stays searchable
+        const bool docs_before = ix->has_docs;
+        try {
+            for (int64_t o = 0; o < m; o += chunk) {
+                const int64_t c = std::min(chunk, m - o);
+                const float* vecs = a.vecs + (size_t)o * ix->dim;
+                const int32_t* ids = a.doc_ids ? a.doc_ids + o : nullptr;
+                if (a.vecs_on_host) {
+                    MB_CUDA(cudaMemcpyAsync(d_v.get(), vecs, (size_t)c * ix->dim * sizeof(float),
+                                            cudaMemcpyHostToDevice, ix->stream));
+                    vecs = d_v.get();
+                }
+                if (host_ids) {
+                    MB_CUDA(cudaMemcpyAsync(d_d.get(), ids, (size_t)c * sizeof(int32_t), cudaMemcpyHostToDevice,
+                                            ix->stream));
+                    ids = d_d.get();
+                }
+                add_rows_device(ix, vecs, ids, c);
+                MB_CUDA(cudaStreamSynchronize(ix->stream));
+            }
+            check_input_flags(ix, "embeddings");
+        } catch (...) {
+            ix->n_rows = rows_before;
+            ix->has_docs = docs_before;
+            throw;
+        }
+        if (a.doc_ids && !a.ids_on_host) track_max_doc(ix, a.doc_ids, m);
+        else ix->max_doc = hi;
+    });
 }
 
 }  // namespace
@@ -1866,79 +1939,19 @@ int b200_index_destroy(b200_index* ix) {
 }
 
 int b200_index_add(b200_index* ix, const float* vecs, const int32_t* doc_ids, int64_t m) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr, "index is NULL");
-        MB_CHECK_ARG(m >= 0, "m must be >= 0");
-        if (m == 0) return;
-        MB_CHECK_ARG(vecs != nullptr, "vecs is NULL");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
-        MB_CHECK_ARG(ix->n_rows + m < (int64_t)INT32_MAX, "row count would exceed 2^31-1");
-        int64_t hi = ix->max_doc;
-        if (doc_ids)
-            for (int64_t i = 0; i < m; ++i) {
-                MB_CHECK_ARG(doc_ids[i] >= 0, "doc_ids[%lld] is negative", (long long)i);
-                hi = std::max<int64_t>(hi, doc_ids[i]);
-            }
-        const int64_t chunk = 1 << 16;
-        DeviceBuffer<float> d_v((size_t)std::min(m, chunk) * ix->dim);
-        DeviceBuffer<int32_t> d_d(doc_ids ? (size_t)std::min(m, chunk) : 0);
-        add_checked(ix, [&] {
-            for (int64_t o = 0; o < m; o += chunk) {
-                const int64_t c = std::min(chunk, m - o);
-                MB_CUDA(cudaMemcpyAsync(d_v.get(), vecs + (size_t)o * ix->dim, (size_t)c * ix->dim * sizeof(float),
-                                        cudaMemcpyHostToDevice, ix->stream));
-                if (doc_ids)
-                    MB_CUDA(cudaMemcpyAsync(d_d.get(), doc_ids + o, (size_t)c * sizeof(int32_t), cudaMemcpyHostToDevice,
-                                            ix->stream));
-                add_rows_device(ix, d_v.get(), doc_ids ? d_d.get() : nullptr, c);
-                MB_CUDA(cudaStreamSynchronize(ix->stream));
-            }
-        });
-        ix->max_doc = hi;
-    });
+    return add(ix, {vecs, true, doc_ids, true}, m, vecs != nullptr, "vecs is NULL");
 }
 
 int b200_index_add_device(b200_index* ix, const float* d_vecs, const int32_t* d_doc_ids, int64_t m) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr, "index is NULL");
-        MB_CHECK_ARG(m >= 0, "m must be >= 0");
-        if (m == 0) return;
-        MB_CHECK_ARG(d_vecs != nullptr, "d_vecs is NULL");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
-        MB_CHECK_ARG(ix->n_rows + m < (int64_t)INT32_MAX, "row count would exceed 2^31-1");
-        add_checked(ix, [&] { add_rows_device(ix, d_vecs, d_doc_ids, m); });
-        if (d_doc_ids) track_max_doc(ix, d_doc_ids, m);
-    });
+    return add(ix, {d_vecs, false, d_doc_ids, false}, m, d_vecs != nullptr, "d_vecs is NULL");
 }
 
 int b200_index_add_device_docs(b200_index* ix, const float* d_vecs, const int32_t* doc_ids, int64_t m) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr, "index is NULL");
-        MB_CHECK_ARG(m >= 0, "m must be >= 0");
-        if (m == 0) return;
-        MB_CHECK_ARG(d_vecs != nullptr && doc_ids != nullptr, "NULL argument");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
-        MB_CHECK_ARG(ix->n_rows + m < (int64_t)INT32_MAX, "row count would exceed 2^31-1");
-        int64_t hi = ix->max_doc;
-        for (int64_t i = 0; i < m; ++i) {
-            MB_CHECK_ARG(doc_ids[i] >= 0, "doc_ids[%lld] is negative", (long long)i);
-            hi = std::max<int64_t>(hi, doc_ids[i]);
-        }
-        DeviceBuffer<int32_t> d_d((size_t)m);
-        MB_CUDA(cudaMemcpyAsync(d_d.get(), doc_ids, (size_t)m * sizeof(int32_t), cudaMemcpyHostToDevice, ix->stream));
-        add_checked(ix, [&] { add_rows_device(ix, d_vecs, d_d.get(), m); });
-        ix->max_doc = hi;
-    });
+    return add(ix, {d_vecs, false, doc_ids, true}, m, d_vecs != nullptr && doc_ids != nullptr, "NULL argument");
 }
 
 int b200_index_delete_doc(b200_index* ix, int32_t doc_id) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr, "index is NULL");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
+    return with_index(ix, [&] {
         if (ix->n_rows == 0) return;
         tombstone_kernel<<<(unsigned)((ix->n_rows + 255) / 256), 256, 0, ix->stream>>>(ix->doc_of_row.get(), ix->n_rows,
                                                                                       doc_id);
@@ -1949,13 +1962,10 @@ int b200_index_delete_doc(b200_index* ix, int32_t doc_id) {
 }
 
 int b200_index_delete_rows(b200_index* ix, const int32_t* rows, int64_t n) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr, "index is NULL");
+    return with_index(ix, [&] {
         MB_CHECK_ARG(n >= 0, "n must be >= 0");
         if (n == 0) return;
         MB_CHECK_ARG(rows != nullptr, "rows is NULL");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
         for (int64_t i = 0; i < n; ++i)
             MB_CHECK_ARG(rows[i] >= 0 && rows[i] < ix->n_rows, "rows[%lld] = %d out of range", (long long)i, rows[i]);
         DeviceBuffer<int32_t> d_r((size_t)n);
@@ -1969,10 +1979,8 @@ int b200_index_delete_rows(b200_index* ix, const int32_t* rows, int64_t n) {
 }
 
 int b200_index_compact(b200_index* ix, int32_t* out_new_of_old, int64_t* out_rows) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr && out_new_of_old != nullptr && out_rows != nullptr, "NULL argument");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
+    return with_index(ix, "NULL argument", [&] {
+        MB_CHECK_ARG(out_new_of_old != nullptr && out_rows != nullptr, "NULL argument");
         const int64_t n = ix->n_rows;
         std::vector<int32_t> doc((size_t)n);
         if (n > 0) {
@@ -1996,19 +2004,15 @@ int b200_index_compact(b200_index* ix, int32_t* out_new_of_old, int64_t* out_row
             d_map.get(), n, ix->dim);
         MB_CUDA(cudaGetLastError());
         MB_CUDA(cudaStreamSynchronize(ix->stream));
-        ix->corpus = std::move(r.corpus);
-        ix->doc_of_row = std::move(r.doc_of_row);
-        ix->row_n2 = std::move(r.row_n2);
-        ix->capacity = cap;
+        adopt_rows(ix, std::move(r), cap);
         ix->n_rows = live;
         ix->dead_rows = 0;
     });
 }
 
 int b200_index_num_rows(b200_index* ix, int64_t* out_rows) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix && out_rows, "NULL argument");
-        std::lock_guard<std::mutex> lk(ix->mu);
+    return with_index(ix, "NULL argument", [&] {
+        MB_CHECK_ARG(out_rows, "NULL argument");
         *out_rows = ix->n_rows;
     });
 }
@@ -2027,12 +2031,10 @@ int b200_index_get_row(b200_index* ix, int64_t row, float* out_vec) {
 }
 
 int b200_index_get_rows(b200_index* ix, const int64_t* rows, int64_t n, float* out_vecs) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix && out_vecs && (rows || n == 0), "NULL argument");
+    return with_index(ix, "NULL argument", [&] {
+        MB_CHECK_ARG(out_vecs && (rows || n == 0), "NULL argument");
         MB_CHECK_ARG(n >= 0, "n must be >= 0");
         if (n == 0) return;
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
         std::vector<__half> tmp((size_t)n * ix->dim);
         for (int64_t i = 0; i < n; ++i) {
             MB_CHECK_ARG(rows[i] >= 0 && rows[i] < ix->n_rows, "row %lld out of range", (long long)rows[i]);
@@ -2046,11 +2048,9 @@ int b200_index_get_rows(b200_index* ix, const int64_t* rows, int64_t n, float* o
 
 int b200_index_search_ex(b200_index* ix, const float* q, int nq, int k, const b200_search_opts* opts, int32_t* out_doc,
                          int32_t* out_row, double* out_score) {
-    return guarded([&] {
-        check_search_args(ix, q, nq, k, out_doc, out_row, out_score);
+    return with_index(ix, [&] {
+        check_search_args(q, nq, k, out_doc, out_row, out_score);
         validate_opts(opts);
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
         const bool mod = opts && (opts->n_mult > 0 || opts->n_add > 0);
         const bool filt = opts && opts->filter_bits != nullptr;
         if (mod) prepare_modifiers(ix, opts->mult_cols, opts->mult_w, opts->n_mult, opts->add_cols, opts->add_w, opts->n_add);
@@ -2080,21 +2080,15 @@ int b200_index_search_modified(b200_index* ix, const float* q, int nq, int k, co
 }
 
 int b200_index_set_attributes(b200_index* ix, int column, const int32_t* doc_ids, const double* values, int64_t n) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr, "index is NULL");
+    return with_index(ix, [&] {
         MB_CHECK_ARG(n >= 0, "n must be >= 0");
         MB_CHECK_ARG(column >= -1 && column < B200_MAX_ATTRIBUTE_COLUMNS, "attribute column %d out of range", column);
         MB_CHECK_ARG(column >= 0 || values == nullptr, "column -1 (all columns) only clears: values must be NULL");
         if (n == 0) return;
         MB_CHECK_ARG(doc_ids != nullptr, "doc_ids is NULL");
-        int64_t hi = -1;
-        for (int64_t i = 0; i < n; ++i) {
-            MB_CHECK_ARG(doc_ids[i] >= 0, "doc_ids[%lld] is negative", (long long)i);
-            hi = std::max<int64_t>(hi, doc_ids[i]);
-            if (values) MB_CHECK_ARG(std::isfinite(values[i]), "values[%lld] is not finite", (long long)i);
-        }
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
+        const int64_t hi = max_doc_id(doc_ids, n);
+        if (values)
+            for (int64_t i = 0; i < n; ++i) MB_CHECK_ARG(std::isfinite(values[i]), "values[%lld] is not finite", (long long)i);
         if (column < 0 && ix->attr_cols.empty()) return;
         ensure_attr_capacity(ix, hi + 1);
         DeviceBuffer<int32_t> d_ids((size_t)n);
@@ -2119,23 +2113,18 @@ int b200_index_set_attributes(b200_index* ix, int column, const int32_t* doc_ids
 
 int b200_index_set_attributes_multi(b200_index* ix, const int32_t* columns, const int32_t* doc_ids, const double* values,
                                     int64_t n) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr, "index is NULL");
+    return with_index(ix, [&] {
         MB_CHECK_ARG(n >= 0, "n must be >= 0");
         if (n == 0) return;
         MB_CHECK_ARG(columns && doc_ids && values, "NULL argument");
-        int64_t hi = -1;
+        const int64_t hi = max_doc_id(doc_ids, n);
         int max_col = -1;
         for (int64_t i = 0; i < n; ++i) {
             MB_CHECK_ARG(columns[i] >= 0 && columns[i] < B200_MAX_ATTRIBUTE_COLUMNS, "columns[%lld] = %d out of range",
                          (long long)i, columns[i]);
-            MB_CHECK_ARG(doc_ids[i] >= 0, "doc_ids[%lld] is negative", (long long)i);
             MB_CHECK_ARG(std::isfinite(values[i]), "values[%lld] is not finite", (long long)i);
-            hi = std::max<int64_t>(hi, doc_ids[i]);
             max_col = std::max(max_col, columns[i]);
         }
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
         ensure_attr_capacity(ix, hi + 1);
         std::vector<char> used(max_col + 1, 0);
         for (int64_t i = 0; i < n; ++i) used[columns[i]] = 1;
@@ -2156,10 +2145,8 @@ int b200_index_set_attributes_multi(b200_index* ix, const int32_t* columns, cons
 
 int b200_index_search_device(b200_index* ix, const float* d_q, int nq, int k, int32_t* d_out_doc, int32_t* d_out_row,
                              double* d_out_score, int sync) {
-    return guarded([&] {
-        check_search_args(ix, d_q, nq, k, d_out_doc, d_out_row, d_out_score);
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
+    return with_index(ix, [&] {
+        check_search_args(d_q, nq, k, d_out_doc, d_out_row, d_out_score);
         search_device(ix, d_q, nq, k, d_out_doc, d_out_row, d_out_score, sync != 0);
         if (sync) MB_CUDA(cudaStreamSynchronize(ix->stream));
     });
@@ -2167,10 +2154,7 @@ int b200_index_search_device(b200_index* ix, const float* d_q, int nq, int k, in
 
 int b200_index_search_stats(b200_index* ix, int64_t* out_groups, int64_t* out_flagged, int64_t* out_collect_passes,
                             int64_t* out_unresolved) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr, "index is NULL");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
+    return with_index(ix, [&] {
         fetch_qstate(ix);
         if (out_groups) *out_groups = ix->stat_groups;
         if (out_flagged) *out_flagged = ix->stat_flagged;
@@ -2180,32 +2164,25 @@ int b200_index_search_stats(b200_index* ix, int64_t* out_groups, int64_t* out_fl
 }
 
 int b200_index_set_stream(b200_index* ix, void* cuda_stream, int use_external) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr, "index is NULL");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
+    return with_index(ix, [&] {
         MB_CUDA(cudaStreamSynchronize(ix->stream));
         ix->stream = use_external ? reinterpret_cast<cudaStream_t>(cuda_stream) : ix->own_stream.get();
     });
 }
 
 int b200_index_set_doc_offset(b200_index* ix, int32_t offset) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix != nullptr, "index is NULL");
+    return with_index(ix, [&] {
         MB_CHECK_ARG(offset >= 0, "offset must be >= 0");
-        std::lock_guard<std::mutex> lk(ix->mu);
         ix->doc_offset = offset;
     });
 }
 
 int b200_topk_merge_device(b200_index* ix, const void* d_gathered, int nshards, int nq, int k, int32_t* d_out_doc,
                            int32_t* d_out_row, double* d_out_score, int sync) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix && d_gathered && d_out_doc && d_out_row && d_out_score, "NULL argument");
+    return with_index(ix, "NULL argument", [&] {
+        MB_CHECK_ARG(d_gathered && d_out_doc && d_out_row && d_out_score, "NULL argument");
         MB_CHECK_ARG(nshards > 0 && nq > 0 && k > 0, "nshards, nq, k must be positive");
         if (nshards * k > 256) fail(B200_ERR_UNSUPPORTED, "device merge handles up to 256 candidates per query");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
         merge_shards_kernel<<<(nq + 3) / 4, 128, 0, ix->stream>>>(reinterpret_cast<const uint8_t*>(d_gathered), nshards, nq,
                                                                 k, d_out_doc, d_out_row, d_out_score);
         MB_CUDA(cudaGetLastError());
@@ -2214,10 +2191,8 @@ int b200_topk_merge_device(b200_index* ix, const void* d_gathered, int nshards, 
 }
 
 int b200_index_last_timing(b200_index* ix, float* scan_ms, float* merge_ms) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix && scan_ms && merge_ms, "NULL argument");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
+    return with_index(ix, "NULL argument", [&] {
+        MB_CHECK_ARG(scan_ms && merge_ms, "NULL argument");
         if (!ix->timing_valid) fail(B200_ERR_INVALID_ARG, "no search has been timed yet");
         MB_CUDA(cudaEventSynchronize(ix->ev[2].get()));
         MB_CUDA(cudaEventElapsedTime(scan_ms, ix->ev[0].get(), ix->ev[1].get()));
@@ -2312,16 +2287,14 @@ int b200_exchange_destroy(b200_exchange* ex) {
 
 int b200_index_search_exchange(b200_index* ix, b200_exchange* ex, const float* d_q, int nq, int k, void* d_local_block,
                                int32_t* d_out_doc, int32_t* d_out_row, double* d_out_score, int sync) {
-    return guarded([&] {
+    return with_index(ix, [&] {
         MB_CHECK_ARG(ex != nullptr && d_local_block != nullptr, "NULL argument");
-        check_search_args(ix, d_q, nq, k, d_out_doc, d_out_row, d_out_score);
+        check_search_args(d_q, nq, k, d_out_doc, d_out_row, d_out_score);
         MB_CHECK_ARG(nq <= MQ, "one exchange call handles at most %d queries", MQ);
         MB_CHECK_ARG((size_t)nq * k * 16 <= ex->slot_stride, "nq * k exceeds the exchange buffer's block size");
         MB_CHECK_ARG(ex->world * k <= 256, "world * k must be <= 256");
         MB_CHECK_ARG(ex->device == ix->device, "exchange buffer and index live on different devices");
         for (int s = 0; s < ex->world; ++s) MB_CHECK_ARG(ex->peer[s] != nullptr, "peer %d has not been opened", s);
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
         const size_t nk = (size_t)nq * k;
         uint8_t* blk = reinterpret_cast<uint8_t*>(d_local_block);
         search_device(ix, d_q, nq, k, reinterpret_cast<int32_t*>(blk), reinterpret_cast<int32_t*>(blk + nk * 4),
@@ -2363,10 +2336,8 @@ struct SnapshotHeader {
 }  // namespace
 
 int b200_index_save(b200_index* ix, const char* path) {
-    return guarded([&] {
-        MB_CHECK_ARG(ix && path, "NULL argument");
-        std::lock_guard<std::mutex> lk(ix->mu);
-        DeviceGuard g(ix->device);
+    return with_index(ix, "NULL argument", [&] {
+        MB_CHECK_ARG(path, "NULL argument");
         // written under a temporary name and renamed at the end: a crash or a short write never damages the previous
         // snapshot of the same name
         const std::string tmp_path = std::string(path) + ".tmp";
