@@ -488,9 +488,46 @@ int b200_debug_relative_position_buckets(int num_buckets, int max_distance, int 
 /* Mean device time (ms, CUDA events) of `iters` back-to-back attention launches on device-generated data, every key
  * kept; rel_bias != 0 adds a generated relative-position bias table with smax = S (the bias runs with mask 2). */
 int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, int rel_bias, int iters, float* out_ms);
-/* LayerNorm over rows of fp32 [rows, w]. */
-int b200_debug_layernorm(int device, const float* x, const float* gamma, const float* beta, float eps, int rows, int w,
+/* LayerNorm over `rows` rows of width w, row r read at x + r * in_stride (0: w); x holds (rows - 1) * in_stride + w
+ * floats.  out_f32 / out_bf16 (either may be NULL, not both) receive the fp32 and the bf16 output [rows, w], the bf16
+ * one as fp32.  in_place != 0 writes the fp32 output over x on the device (needs out_f32 and in_stride == w). */
+int b200_debug_layernorm(int device, const float* x, long long in_stride, const float* gamma, const float* beta, float eps,
+                         int rows, int w, int in_place, float* out_f32, float* out_bf16);
+/* CLIP / SigLIP text embedding: x fp32 [n*S, w] = tok[ids] + pos[s], eot int32 [n] = first arg-max of each ids row.
+ * tok [vocab, w], pos [S, w]. */
+int b200_debug_clip_text_embed(int device, const int32_t* ids, const float* tok, const float* pos, int n, int S, int w,
+                               int vocab, float* x, int32_t* eot);
+/* BERT embedding + LayerNorm: x fp32 [n*S, w] = LN(word[ids] + type0 + pos[s]), h = the bf16 copy (as fp32), kv_len
+ * int32 [n] = sum of each mask row (S when mask is NULL).  pos has pos_rows >= S rows; type0 [w] is required. */
+int b200_debug_bert_embed_ln(int device, const int32_t* ids, const int32_t* mask, const float* word, const float* pos,
+                             int pos_rows, const float* type0, const float* gamma, const float* beta, float eps, int n,
+                             int S, int w, int vocab, float* x, float* h, int32_t* kv_len);
+/* RoBERTa embedding + LayerNorm (XLM-R with type0, MPNet with type0 NULL): as above with HF's position ids counted from
+ * the ids and pad; pos has pos_rows >= pad + S + 1 rows. */
+int b200_debug_roberta_embed_ln(int device, const int32_t* ids, const int32_t* mask, const float* word, const float* pos,
+                                int pos_rows, const float* type0, const float* gamma, const float* beta, float eps, int n,
+                                int S, int w, int vocab, int pad, float* x, float* h, int32_t* kv_len);
+/* CLIP head over token rows x fp32 [n*S, w]: LN(row b*S + row_in_seq[b]) @ proj [w, E] (row_in_seq NULL: row 0), divided
+ * by its L2 norm if normalize.  out fp32 [n, E]. */
+int b200_debug_clip_head(int device, const float* x, int S, const int32_t* row_in_seq, const float* gamma,
+                         const float* beta, float eps, const float* proj, int n, int w, int E, int normalize, float* out);
+/* BERT head over x fp32 [n*S, w]: mean of the first kv_len[b] rows (pool 0) or row 0 (pool 1), then F.normalize if
+ * normalize.  out fp32 [n, w]. */
+int b200_debug_bert_head(int device, const float* x, const int32_t* kv_len, int n, int S, int w, int pool, int normalize,
                          float* out);
+/* out fp32 [n, E] = src / |src| per row if normalize, else src. */
+int b200_debug_l2_rows(int device, const float* src, int n, int E, int normalize, float* out);
+/* ResNet stem im2col: exactly one of hwc (uint8 [n,S,S,3], normalised with mean3 / std3) and chw (fp32 [n,3,S,S]) ->
+ * out fp32 [n*(S/2)^2, 64] (rounded to bf16). */
+int b200_debug_stem_im2col(int device, const uint8_t* hwc, const float* chw, int n, int S, const float* mean3,
+                           const float* std3, float* out);
+/* AvgPool2d(2) over NHWC x fp32 [n,H,W,C] (rounded to bf16) -> out fp32 [n,H/2,W/2,C] (rounded to bf16). */
+int b200_debug_avgpool2(int device, const float* x, int n, int H, int W, int C, float* out);
+/* ResNet attention-pool tokens: x fp32 [n,HW,C] (rounded to bf16), pos fp32 [HW+1, C] -> out fp32 [n*(HW+1), C]
+ * (rounded to bf16): row 0 = mean_s x_s + pos[0], row 1+s = x_s + pos[1+s]. */
+int b200_debug_attnpool_tokens(int device, const float* x, const float* pos, int n, int HW, int C, float* out);
+/* ViT im2col of fp32 CHW [n,3,S,S] -> out fp32 [n*((S/p)^2 + cls), kpad] (rounded to bf16), k = c*p*p + dy*p + dx. */
+int b200_debug_im2col_f32(int device, const float* chw, int n, int S, int p, int kpad, int cls, float* out);
 /* The JPEG decoder's arithmetic (shared __host__ __device__ code of the two kernels) run on the host: lets the CPU test
  * suite pin it against Pillow pixel for pixel.  A test hook, not a product path.  out_rgb == NULL: size query. */
 int b200_debug_jpeg_decode_host(const uint8_t* file, size_t nbytes, uint8_t* out_rgb, size_t out_capacity,

@@ -124,7 +124,20 @@ _SIGNATURES = {
     "b200_debug_relative_position_buckets": (C.c_int, [C.c_int, C.c_int, C.c_int, _P]),
     "b200_debug_attention_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                             C.POINTER(C.c_float)]),
-    "b200_debug_layernorm": (C.c_int, [C.c_int, _P, _P, _P, C.c_float, C.c_int, C.c_int, _P]),
+    "b200_debug_layernorm": (C.c_int, [C.c_int, _P, C.c_longlong, _P, _P, C.c_float, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_clip_text_embed": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_bert_embed_ln": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, _P, _P, _P, C.c_float, C.c_int, C.c_int,
+                                           C.c_int, C.c_int, _P, _P, _P]),
+    "b200_debug_roberta_embed_ln": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, _P, _P, _P, C.c_float, C.c_int, C.c_int,
+                                              C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "b200_debug_clip_head": (C.c_int, [C.c_int, _P, C.c_int, _P, _P, _P, C.c_float, _P, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       _P]),
+    "b200_debug_bert_head": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "b200_debug_l2_rows": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P]),
+    "b200_debug_stem_im2col": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
+    "b200_debug_avgpool2": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "b200_debug_attnpool_tokens": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
+    "b200_debug_im2col_f32": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "b200_debug_resize": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "b200_debug_resize_squash": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "b200_debug_map_attention": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),

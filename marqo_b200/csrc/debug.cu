@@ -39,6 +39,18 @@ __global__ void bf16_to_f32_kernel(const __nv_bfloat16* src, float* dst, long lo
     if (i < n) dst[i] = __bfloat162float(src[i]);
 }
 
+// Runs `launch` (which writes bf16 [m] into its argument) and downloads the result as fp32.
+template <class F>
+void run_bf16_out(Scratch& sc, size_t m, float* out, F&& launch) {
+    __nv_bfloat16* dO = sc.alloc<__nv_bfloat16>(m);
+    float* dOut = sc.alloc<float>(m);
+    launch(dO);
+    bf16_to_f32_kernel<<<(unsigned)((m + 255) / 256), 256, 0, sc.s>>>(dO, dOut, (long long)m);
+    MB_CUDA(cudaGetLastError());
+    MB_CUDA(cudaMemcpyAsync(out, dOut, m * 4, cudaMemcpyDeviceToHost, sc.s));
+    MB_CUDA(cudaStreamSynchronize(sc.s));
+}
+
 // pseudo-random values in [-1, 1) (kernel timing probes: no 200 MB host upload)
 __device__ __forceinline__ float fill_value(long long i, uint32_t seed) {
     uint32_t x = (uint32_t)i * 2654435761u + seed;
@@ -335,20 +347,221 @@ int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, 
     });
 }
 
-int b200_debug_layernorm(int device, const float* x, const float* gamma, const float* beta, float eps, int rows, int w,
-                         float* out) {
+int b200_debug_layernorm(int device, const float* x, long long in_stride, const float* gamma, const float* beta, float eps,
+                         int rows, int w, int in_place, float* out_f32, float* out_bf16) {
     return guarded([&] {
-        MB_CHECK_ARG(x && gamma && beta && out, "NULL buffer");
+        MB_CHECK_ARG(x && gamma && beta && (out_f32 || out_bf16), "NULL buffer");
+        MB_CHECK_ARG(rows > 0 && w > 0 && in_stride >= 0, "rows, w must be positive");
+        if (in_stride == 0) in_stride = w;
+        MB_CHECK_ARG(in_stride >= w, "in_stride %lld < w %d", in_stride, w);
+        MB_CHECK_ARG(!in_place || (out_f32 && in_stride == w), "in place needs the fp32 output and compact rows");
         require_device(device);
         DeviceGuard g(device);
         Scratch sc;
-        float* dx = sc.upload(x, (size_t)rows * w);
+        float* dx = sc.upload(x, (size_t)(rows - 1) * in_stride + w);
         float* dg = sc.upload(gamma, (size_t)w);
         float* db = sc.upload(beta, (size_t)w);
-        float* dout = sc.alloc<float>((size_t)rows * w);
-        kernels::layernorm(dx, w, dg, db, eps, rows, w, dout, nullptr, sc.s);
+        const size_t n = (size_t)rows * w;
+        float* dF = out_f32 ? (in_place ? dx : sc.alloc<float>(n)) : nullptr;
+        __nv_bfloat16* dB = out_bf16 ? sc.alloc<__nv_bfloat16>(n) : nullptr;
+        kernels::layernorm(dx, in_stride, dg, db, eps, rows, w, dF, dB, sc.s);
+        if (dB) {
+            float* dBf = sc.alloc<float>(n);
+            bf16_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, sc.s>>>(dB, dBf, (long long)n);
+            MB_CUDA(cudaGetLastError());
+            MB_CUDA(cudaMemcpyAsync(out_bf16, dBf, n * 4, cudaMemcpyDeviceToHost, sc.s));
+        }
+        if (dF) MB_CUDA(cudaMemcpyAsync(out_f32, dF, n * 4, cudaMemcpyDeviceToHost, sc.s));
         MB_CUDA(cudaStreamSynchronize(sc.s));
-        MB_CUDA(cudaMemcpy(out, dout, (size_t)rows * w * 4, cudaMemcpyDeviceToHost));
+    });
+}
+
+int b200_debug_clip_text_embed(int device, const int32_t* ids, const float* tok, const float* pos, int n, int S, int w,
+                               int vocab, float* x, int32_t* eot) {
+    return guarded([&] {
+        MB_CHECK_ARG(ids && tok && pos && x && eot, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && S > 0 && w > 0 && w % 4 == 0 && vocab > 0, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const size_t rows = (size_t)n * S;
+        const int32_t* dIds = sc.upload(ids, rows);
+        const float* dTok = sc.upload(tok, (size_t)vocab * w);
+        const float* dPos = sc.upload(pos, (size_t)S * w);
+        float* dX = sc.alloc<float>(rows * w);
+        int32_t* dEot = sc.alloc<int32_t>((size_t)n);
+        kernels::clip_text_embed(dIds, dTok, dPos, n, S, w, vocab, dX, dEot, sc.s);
+        MB_CUDA(cudaMemcpyAsync(x, dX, rows * w * 4, cudaMemcpyDeviceToHost, sc.s));
+        MB_CUDA(cudaMemcpyAsync(eot, dEot, (size_t)n * 4, cudaMemcpyDeviceToHost, sc.s));
+        MB_CUDA(cudaStreamSynchronize(sc.s));
+    });
+}
+
+// The BERT and RoBERTa embedding hooks: pos has pos_rows rows, which must cover every position the kernel reads.
+static int debug_embed_ln(int device, bool roberta, const int32_t* ids, const int32_t* mask, const float* word,
+                          const float* pos, int pos_rows, const float* type0, const float* gamma, const float* beta,
+                          float eps, int n, int S, int w, int vocab, int pad, float* x, float* h, int32_t* kv_len) {
+    return guarded([&] {
+        MB_CHECK_ARG(ids && word && pos && gamma && beta && x && h && kv_len, "NULL buffer");
+        MB_CHECK_ARG(roberta || type0, "the BERT embedding always adds token-type row 0");
+        MB_CHECK_ARG(n > 0 && S > 0 && w > 0 && vocab > 0, "bad shape");
+        MB_CHECK_ARG(roberta ? pad >= 0 && pos_rows >= pad + S + 1 : pos_rows >= S, "%d position rows are too few",
+                     pos_rows);
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const size_t rows = (size_t)n * S;
+        const int32_t* dIds = sc.upload(ids, rows);
+        const int32_t* dMask = mask ? sc.upload(mask, rows) : nullptr;
+        const float* dWord = sc.upload(word, (size_t)vocab * w);
+        const float* dPos = sc.upload(pos, (size_t)pos_rows * w);
+        const float* dType = type0 ? sc.upload(type0, (size_t)w) : nullptr;
+        const float* dG = sc.upload(gamma, (size_t)w);
+        const float* dB = sc.upload(beta, (size_t)w);
+        float* dX = sc.alloc<float>(rows * w);
+        __nv_bfloat16* dH = sc.alloc<__nv_bfloat16>(rows * w);
+        float* dHf = sc.alloc<float>(rows * w);
+        int32_t* dLen = sc.alloc<int32_t>((size_t)n);
+        if (roberta)
+            kernels::roberta_embed_ln(dIds, dMask, dWord, dPos, dType, dG, dB, eps, n, S, w, vocab, pad, dX, dH, dLen, sc.s);
+        else
+            kernels::bert_embed_ln(dIds, dMask, dWord, dPos, dType, dG, dB, eps, n, S, w, vocab, dX, dH, dLen, sc.s);
+        const long long m = (long long)(rows * w);
+        bf16_to_f32_kernel<<<(unsigned)((m + 255) / 256), 256, 0, sc.s>>>(dH, dHf, m);
+        MB_CUDA(cudaGetLastError());
+        MB_CUDA(cudaMemcpyAsync(x, dX, rows * w * 4, cudaMemcpyDeviceToHost, sc.s));
+        MB_CUDA(cudaMemcpyAsync(h, dHf, rows * w * 4, cudaMemcpyDeviceToHost, sc.s));
+        MB_CUDA(cudaMemcpyAsync(kv_len, dLen, (size_t)n * 4, cudaMemcpyDeviceToHost, sc.s));
+        MB_CUDA(cudaStreamSynchronize(sc.s));
+    });
+}
+
+int b200_debug_bert_embed_ln(int device, const int32_t* ids, const int32_t* mask, const float* word, const float* pos,
+                             int pos_rows, const float* type0, const float* gamma, const float* beta, float eps, int n,
+                             int S, int w, int vocab, float* x, float* h, int32_t* kv_len) {
+    return debug_embed_ln(device, false, ids, mask, word, pos, pos_rows, type0, gamma, beta, eps, n, S, w, vocab, 0, x, h,
+                          kv_len);
+}
+
+int b200_debug_roberta_embed_ln(int device, const int32_t* ids, const int32_t* mask, const float* word, const float* pos,
+                                int pos_rows, const float* type0, const float* gamma, const float* beta, float eps, int n,
+                                int S, int w, int vocab, int pad, float* x, float* h, int32_t* kv_len) {
+    return debug_embed_ln(device, true, ids, mask, word, pos, pos_rows, type0, gamma, beta, eps, n, S, w, vocab, pad, x,
+                          h, kv_len);
+}
+
+int b200_debug_clip_head(int device, const float* x, int S, const int32_t* row_in_seq, const float* gamma,
+                         const float* beta, float eps, const float* proj, int n, int w, int E, int normalize, float* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && gamma && beta && proj && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && S > 0 && w > 0 && E > 0, "bad shape");
+        for (int b = 0; row_in_seq && b < n; ++b)
+            MB_CHECK_ARG(row_in_seq[b] >= 0 && row_in_seq[b] < S, "row_in_seq[%d] = %d outside [0, %d)", b, row_in_seq[b], S);
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const float* dX = sc.upload(x, (size_t)n * S * w);
+        const int32_t* dRow = row_in_seq ? sc.upload(row_in_seq, (size_t)n) : nullptr;
+        const float* dG = sc.upload(gamma, (size_t)w);
+        const float* dB = sc.upload(beta, (size_t)w);
+        const float* dP = sc.upload(proj, (size_t)w * E);
+        float* dOut = sc.alloc<float>((size_t)n * E);
+        float* dPooled = sc.alloc<float>((size_t)n * w);
+        kernels::clip_head(dX, S, dRow, dG, dB, eps, dP, n, w, E, normalize, dOut, dPooled, sc.s);
+        MB_CUDA(cudaMemcpyAsync(out, dOut, (size_t)n * E * 4, cudaMemcpyDeviceToHost, sc.s));
+        MB_CUDA(cudaStreamSynchronize(sc.s));
+    });
+}
+
+int b200_debug_bert_head(int device, const float* x, const int32_t* kv_len, int n, int S, int w, int pool, int normalize,
+                         float* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && kv_len && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && S > 0 && w > 0 && (pool == 0 || pool == 1), "bad shape or pool");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const float* dX = sc.upload(x, (size_t)n * S * w);
+        const int32_t* dLen = sc.upload(kv_len, (size_t)n);
+        float* dOut = sc.alloc<float>((size_t)n * w);
+        kernels::bert_head(dX, dLen, n, S, w, pool, normalize, dOut, sc.s);
+        MB_CUDA(cudaMemcpyAsync(out, dOut, (size_t)n * w * 4, cudaMemcpyDeviceToHost, sc.s));
+        MB_CUDA(cudaStreamSynchronize(sc.s));
+    });
+}
+
+int b200_debug_l2_rows(int device, const float* src, int n, int E, int normalize, float* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(src && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && E > 0, "n, E must be positive");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const float* dS = sc.upload(src, (size_t)n * E);
+        float* dOut = sc.alloc<float>((size_t)n * E);
+        kernels::l2_rows(dS, n, E, normalize, dOut, sc.s);
+        MB_CUDA(cudaMemcpyAsync(out, dOut, (size_t)n * E * 4, cudaMemcpyDeviceToHost, sc.s));
+        MB_CUDA(cudaStreamSynchronize(sc.s));
+    });
+}
+
+int b200_debug_stem_im2col(int device, const uint8_t* hwc, const float* chw, int n, int S, const float* mean3,
+                           const float* std3, float* out) {
+    return guarded([&] {
+        MB_CHECK_ARG((hwc != nullptr) != (chw != nullptr), "exactly one of hwc and chw");
+        MB_CHECK_ARG(mean3 && std3 && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && S > 0 && S % 2 == 0, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const size_t px = (size_t)n * S * S * 3;
+        const uint8_t* dU8 = hwc ? sc.upload(hwc, px) : nullptr;
+        const float* dChw = chw ? sc.upload(chw, px) : nullptr;
+        run_bf16_out(sc, (size_t)n * (S / 2) * (S / 2) * 64, out, [&](__nv_bfloat16* o) {
+            kernels::stem_im2col(dU8, dChw, n, S, mean3, std3, o, sc.s);
+        });
+    });
+}
+
+int b200_debug_avgpool2(int device, const float* x, int n, int H, int W, int C, float* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && H > 0 && W > 0 && C > 0, "n, H, W, C must be positive");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const __nv_bfloat16* dX = sc.upload_bf16(x, (size_t)n * H * W * C);
+        run_bf16_out(sc, (size_t)n * (H / 2) * (W / 2) * C, out,
+                     [&](__nv_bfloat16* o) { kernels::avgpool2_nhwc(dX, n, H, W, C, o, sc.s); });
+    });
+}
+
+int b200_debug_attnpool_tokens(int device, const float* x, const float* pos, int n, int HW, int C, float* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && pos && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && HW > 0 && C > 0, "n, HW, C must be positive");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const __nv_bfloat16* dX = sc.upload_bf16(x, (size_t)n * HW * C);
+        const float* dPos = sc.upload(pos, (size_t)(HW + 1) * C);
+        run_bf16_out(sc, (size_t)n * (HW + 1) * C, out,
+                     [&](__nv_bfloat16* o) { kernels::attnpool_tokens(dX, dPos, n, HW, C, o, sc.s); });
+    });
+}
+
+int b200_debug_im2col_f32(int device, const float* chw, int n, int S, int p, int kpad, int cls, float* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(chw && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && p > 0 && S % p == 0 && S > 0 && (cls == 0 || cls == 1), "bad shape");
+        MB_CHECK_ARG(kpad % 8 == 0 && kpad >= 3 * p * p, "kpad %d must be a multiple of 8 and >= 3 p^2", kpad);
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const float* dChw = sc.upload(chw, (size_t)n * 3 * S * S);
+        const int g2 = (S / p) * (S / p);
+        run_bf16_out(sc, (size_t)n * (g2 + cls) * kpad, out,
+                     [&](__nv_bfloat16* o) { kernels::im2col_f32(dChw, n, S, p, kpad, cls, o, sc.s); });
     });
 }
 

@@ -45,7 +45,8 @@ int clip_head(const float* x, int S, const int32_t* row_in_seq, const float* gam
               const float* proj, int n, int w, int E, int normalize, float* out, float* pooled_ws, cudaStream_t s);
 
 // BERT head: masked mean over the first kv_len[b] tokens (pool == 0) or the [CLS] row (pool == 1), then
-// x / max(|x|, 1e-12) if normalize (F.normalize, hugging_face_model.py:194-195).
+// x / max(|x|, 1e-12) if normalize (F.normalize, hugging_face_model.py:194-195).  kv_len is clamped to [0, S]; 0 gives
+// a NaN row under mean pooling, as the reference's sum / mask.sum() does.
 int bert_head(const float* x, const int32_t* kv_len, int n, int S, int w, int pool, int normalize, float* out,
               cudaStream_t s);
 

@@ -634,10 +634,164 @@ def relative_position_buckets(max_len: int, num_buckets: int = 32, max_distance:
     return out
 
 
-def debug_layernorm(x, gamma, beta, eps: float, device: int = 0) -> np.ndarray:
-    x, g, b = _as(x, np.float32), _as(gamma, np.float32), _as(beta, np.float32)
-    out = np.empty_like(x)
-    N.check(N.load().b200_debug_layernorm(device, _ptr(x), _ptr(g), _ptr(b), eps, x.shape[0], x.shape[1], _ptr(out)))
+def debug_layernorm(x, gamma, beta, eps: float, rows: Optional[int] = None, in_stride: int = 0, outputs: str = "f32",
+                    in_place: bool = False, device: int = 0):
+    """LayerNorm of `rows` rows of width w = len(gamma), row r read at x.flat[r * in_stride] (in_stride 0: w; rows None:
+    x.size // in_stride).  outputs "f32" returns the fp32 output [rows, w], "bf16" the bf16 output (as fp32), "both"
+    the pair (fp32, bf16) of one launch.  in_place writes the fp32 output over x on the device, as ln_pre and BERT's
+    post-LN do."""
+    if outputs not in ("f32", "bf16", "both"):
+        raise ValueError(f"outputs must be 'f32', 'bf16' or 'both', got {outputs!r}")
+    xa, g, b = _as(x, np.float32).reshape(-1), _as(gamma, np.float32), _as(beta, np.float32)
+    w = g.size
+    stride = in_stride or w
+    if rows is None:
+        rows = xa.size // stride
+    if b.size != w or rows < 1 or stride < w or xa.size < (rows - 1) * stride + w:
+        raise ValueError(f"x of {xa.size} floats does not hold {rows} rows of {w} at stride {stride}")
+    if in_place and (outputs == "bf16" or stride != w):
+        raise ValueError("in place needs the fp32 output and compact rows")
+    f = np.empty((rows, w), np.float32) if outputs != "bf16" else None
+    h = np.empty((rows, w), np.float32) if outputs != "f32" else None
+    N.check(N.load().b200_debug_layernorm(device, _ptr(xa), in_stride, _ptr(g), _ptr(b), eps, rows, w, int(in_place),
+                                          _ptr(f), _ptr(h)))
+    return (f, h) if outputs == "both" else (f if h is None else h)
+
+
+def debug_clip_text_embed(ids, tok, pos, device: int = 0):
+    """CLIP / SigLIP text embedding of ids int32 [n, S]: (x fp32 [n*S, w] = tok[ids] + pos[s], eot int32 [n])."""
+    ia, t, p = _as(ids, np.int32), _as(tok, np.float32), _as(pos, np.float32)
+    n, S = ia.shape
+    vocab, w = t.shape
+    if p.shape != (S, w):
+        raise ValueError(f"expected pos [{S}, {w}], got {p.shape}")
+    x = np.empty((n * S, w), np.float32)
+    eot = np.empty(n, np.int32)
+    N.check(N.load().b200_debug_clip_text_embed(device, _ptr(ia), _ptr(t), _ptr(p), n, S, w, vocab, _ptr(x), _ptr(eot)))
+    return x, eot
+
+
+def debug_embed_ln(ids, mask, word, pos, type0, gamma, beta, eps: float, pad: Optional[int] = None, device: int = 0):
+    """BERT (pad None) or RoBERTa (pad = the pad id; type0 None for MPNet) embedding + LayerNorm of ids int32 [n, S]
+    with an optional mask [n, S] -> (x fp32 [n*S, w], its bf16 copy as fp32, kv_len int32 [n])."""
+    ia, wd, p = _as(ids, np.int32), _as(word, np.float32), _as(pos, np.float32)
+    n, S = ia.shape
+    vocab, w = wd.shape
+    m = None if mask is None else _as(mask, np.int32)
+    t = None if type0 is None else _as(type0, np.float32)
+    g, b = _as(gamma, np.float32), _as(beta, np.float32)
+    if m is not None and m.shape != ia.shape:
+        raise ValueError(f"expected mask {ia.shape}, got {m.shape}")
+    need = S if pad is None else pad + S + 1
+    if p.ndim != 2 or p.shape[1] != w or p.shape[0] < need:
+        raise ValueError(f"expected pos [>= {need}, {w}], got {p.shape}")
+    if (t is not None and t.size != w) or g.size != w or b.size != w:
+        raise ValueError(f"type0, gamma and beta must have {w} values")
+    x = np.empty((n * S, w), np.float32)
+    h = np.empty((n * S, w), np.float32)
+    kv_len = np.empty(n, np.int32)
+    lib = N.load()
+    if pad is None:
+        st = lib.b200_debug_bert_embed_ln(device, _ptr(ia), _ptr(m), _ptr(wd), _ptr(p), p.shape[0], _ptr(t), _ptr(g),
+                                          _ptr(b), eps, n, S, w, vocab, _ptr(x), _ptr(h), _ptr(kv_len))
+    else:
+        st = lib.b200_debug_roberta_embed_ln(device, _ptr(ia), _ptr(m), _ptr(wd), _ptr(p), p.shape[0], _ptr(t), _ptr(g),
+                                             _ptr(b), eps, n, S, w, vocab, pad, _ptr(x), _ptr(h), _ptr(kv_len))
+    N.check(st)
+    return x, h, kv_len
+
+
+def debug_clip_head(x, S: int, gamma, beta, eps: float, proj, row_in_seq=None, normalize: bool = True,
+                    device: int = 0) -> np.ndarray:
+    """CLIP head over token rows x fp32 [n*S, w]: LN(x[b*S + row_in_seq[b]]) @ proj [w, E] (row_in_seq None: row 0),
+    L2-normalised if normalize -> fp32 [n, E]."""
+    xa, pj = _as(x, np.float32), _as(proj, np.float32)
+    w, E = pj.shape
+    if xa.ndim != 2 or xa.shape[1] != w or xa.shape[0] % S != 0:
+        raise ValueError(f"expected x [n * {S}, {w}], got {xa.shape}")
+    n = xa.shape[0] // S
+    r = None if row_in_seq is None else _as(row_in_seq, np.int32)
+    if r is not None and (r.shape != (n,) or r.min() < 0 or r.max() >= S):
+        raise ValueError(f"row_in_seq must be [{n}] rows in [0, {S})")
+    g, b = _as(gamma, np.float32), _as(beta, np.float32)
+    out = np.empty((n, E), np.float32)
+    N.check(N.load().b200_debug_clip_head(device, _ptr(xa), S, _ptr(r), _ptr(g), _ptr(b), eps, _ptr(pj), n, w, E,
+                                          int(normalize), _ptr(out)))
+    return out
+
+
+def debug_bert_head(x, S: int, kv_len, pool: int = N.POOL_MEAN, normalize: bool = True, device: int = 0) -> np.ndarray:
+    """BERT head over x fp32 [n*S, w]: mean of the first kv_len[b] rows (POOL_MEAN) or row 0 (POOL_CLS), F.normalize'd
+    if normalize -> fp32 [n, w]."""
+    xa = _as(x, np.float32)
+    if xa.ndim != 2 or xa.shape[0] % S != 0:
+        raise ValueError(f"expected x [n * {S}, w], got {xa.shape}")
+    n, w = xa.shape[0] // S, xa.shape[1]
+    kl = _as(kv_len, np.int32)
+    if kl.shape != (n,):
+        raise ValueError(f"expected kv_len [{n}], got {kl.shape}")
+    out = np.empty((n, w), np.float32)
+    N.check(N.load().b200_debug_bert_head(device, _ptr(xa), _ptr(kl), n, S, w, pool, int(normalize), _ptr(out)))
+    return out
+
+
+def debug_l2_rows(src, normalize: bool = True, device: int = 0) -> np.ndarray:
+    """src fp32 [n, E] -> each row divided by its L2 norm if normalize, else a copy."""
+    a = _as(src, np.float32)
+    if a.ndim != 2:
+        raise ValueError(f"expected [n, E], got {a.shape}")
+    out = np.empty_like(a)
+    N.check(N.load().b200_debug_l2_rows(device, _ptr(a), a.shape[0], a.shape[1], int(normalize), _ptr(out)))
+    return out
+
+
+def debug_stem_im2col(images, mean=(0.0, 0.0, 0.0), std=(1.0, 1.0, 1.0), device: int = 0) -> np.ndarray:
+    """ResNet stem im2col of uint8 HWC [n, S, S, 3] (normalised with mean / std) or already-normalised fp32 CHW
+    [n, 3, S, S] -> fp32 [n * (S/2)^2, 64] (rounded to bf16), k = (3 ky + kx) * 3 + c."""
+    u8 = images.dtype == np.uint8
+    a = _as(images, np.uint8 if u8 else np.float32)
+    n, S = a.shape[0], a.shape[1] if u8 else a.shape[2]
+    if a.shape != ((n, S, S, 3) if u8 else (n, 3, S, S)) or S % 2 != 0:
+        raise ValueError(f"expected [n, S, S, 3] uint8 or [n, 3, S, S] fp32 with S even, got {a.shape}")
+    m3, s3 = _as(mean, np.float32), _as(std, np.float32)
+    out = np.empty((n * (S // 2) ** 2, 64), np.float32)
+    N.check(N.load().b200_debug_stem_im2col(device, _ptr(a) if u8 else None, None if u8 else _ptr(a), n, S, _ptr(m3),
+                                            _ptr(s3), _ptr(out)))
+    return out
+
+
+def debug_avgpool2(x, device: int = 0) -> np.ndarray:
+    """AvgPool2d(2) over NHWC fp32 [n, H, W, C] (rounded to bf16) -> [n, H/2, W/2, C] (rounded to bf16)."""
+    a = _as(x, np.float32)
+    n, H, W, Cc = a.shape
+    if H % 2 or W % 2 or Cc % 8:
+        raise ValueError(f"H, W must be even and C a multiple of 8, got {a.shape}")
+    out = np.empty((n, H // 2, W // 2, Cc), np.float32)
+    N.check(N.load().b200_debug_avgpool2(device, _ptr(a), n, H, W, Cc, _ptr(out)))
+    return out
+
+
+def debug_attnpool_tokens(x, pos, device: int = 0) -> np.ndarray:
+    """ResNet attention-pool tokens: x fp32 [n, HW, C] (rounded to bf16), pos fp32 [HW + 1, C] -> [n, HW + 1, C]
+    (rounded to bf16): row 0 = mean_s x_s + pos[0], row 1 + s = x_s + pos[1 + s]."""
+    a, p = _as(x, np.float32), _as(pos, np.float32)
+    n, HW, Cc = a.shape
+    if p.shape != (HW + 1, Cc) or Cc % 8:
+        raise ValueError(f"expected pos [{HW + 1}, {Cc}] and C a multiple of 8, got {p.shape}")
+    out = np.empty((n, HW + 1, Cc), np.float32)
+    N.check(N.load().b200_debug_attnpool_tokens(device, _ptr(a), _ptr(p), n, HW, Cc, _ptr(out)))
+    return out
+
+
+def debug_im2col_f32(chw, patch: int, kpad: int, cls: int, device: int = 0) -> np.ndarray:
+    """ViT im2col of fp32 CHW [n, 3, S, S] -> fp32 [n * ((S/p)^2 + cls), kpad] (rounded to bf16): the class rows
+    (cls = 1) and the columns past 3 p^2 are zero."""
+    a = _as(chw, np.float32)
+    n, c, S, S2 = a.shape
+    if c != 3 or S != S2 or S % patch or kpad % 8 or kpad < 3 * patch * patch or cls not in (0, 1):
+        raise ValueError(f"bad im2col shape {a.shape}, patch {patch}, kpad {kpad}, cls {cls}")
+    out = np.empty((n * ((S // patch) ** 2 + cls), kpad), np.float32)
+    N.check(N.load().b200_debug_im2col_f32(device, _ptr(a), n, S, patch, kpad, cls, _ptr(out)))
     return out
 
 

@@ -177,15 +177,58 @@ def test_attention_refuses_more_than_65535_sequences(gpu_required):
     assert ei.value.code == ERR_UNSUPPORTED
 
 
-@pytest.mark.parametrize("rows,w,eps", [(5, 128, 1e-5), (77, 512, 1e-5), (1000, 768, 1e-12), (33, 1024, 1e-5)])
-def test_layernorm_matches_torch(gpu_required, rows, w, eps):
+_LN_CASES = [
+    # compact rows, fp32 output
+    (5, 128, 1e-5, "f32"), (77, 512, 1e-5, "f32"), (1000, 768, 1e-12, "f32"), (33, 1024, 1e-5, "f32"),
+    (1, 384, 1e-12, "f32"), (7, 384, 1e-12, "f32"), (9, 384, 1e-5, "f32"),
+    # the last row of each 64-token sequence (in_stride = 64 w), as SigLIP text's ln_final reads it
+    (3, 768, 1e-6, "strided"), (9, 1024, 1e-6, "strided"), (1, 384, 1e-6, "strided"),
+    # bf16 output only (ln_out before SigLIP's MAP head, SigLIP text)
+    (7, 384, 1e-5, "bf16"), (257, 768, 1e-6, "bf16"),
+    # fp32 output over x plus the bf16 copy (BERT's post-LN; ln_pre has the fp32 output alone)
+    (9, 384, 1e-12, "in_place"), (1, 512, 1e-5, "in_place"),
+    # mean 1e4, std 1: the two-pass variance
+    (7, 1024, 1e-5, "offset"), (9, 768, 1e-12, "offset"),
+]
+
+
+@pytest.mark.parametrize("rows,w,eps,variant", _LN_CASES,
+                         ids=[f"{r}-{w}-{e}" + ("" if v == "f32" else f"-{v}") for r, w, e, v in _LN_CASES])
+def test_layernorm_matches_torch(gpu_required, rows, w, eps, variant):
+    """The LayerNorm launch vs fp64.  fp32 outputs are within 1e-5 + 1e-5 |y| (a few fp32 ulps of the mean, the
+    variance and y).  The bf16 output is the round-to-nearest-even of the fp32 result, bit for bit.
+    With mean 1e4 the fp32 sum of w values near 1e4 (partial sums up to 1e7, ulp 1) is off by a few units, the mean by
+    ~3e-3 at most, and each output by that times rstd * gamma ~ 1: 5e-3.  A one-pass E[x^2] - mean^2 would lose the
+    variance entirely (ulp(1e8) = 8)."""
     from marqo_b200.engine import debug_layernorm
     g = torch.Generator().manual_seed(rows)
-    x = torch.randn(rows, w, generator=g) * 3 + 1
-    gamma, beta = torch.randn(w, generator=g), torch.randn(w, generator=g)
-    ref = torch.nn.functional.layer_norm(x, (w,), gamma, beta, eps)
-    got = torch.from_numpy(debug_layernorm(x.numpy(), gamma.numpy(), beta.numpy(), eps))
-    torch.testing.assert_close(got, ref, rtol=1e-5, atol=1e-5)
+    if variant == "offset":
+        x = torch.randn(rows, w, generator=g) + 1e4
+        gamma, beta = 1.0 + 0.1 * torch.randn(w, generator=g), 0.1 * torch.randn(w, generator=g)
+    else:
+        x = torch.randn(rows, w, generator=g) * 3 + 1
+        gamma, beta = torch.randn(w, generator=g), torch.randn(w, generator=g)
+    ref = torch.nn.functional.layer_norm(x.double(), (w,), gamma.double(), beta.double(), eps)
+    tol = dict(rtol=0, atol=5e-3) if variant == "offset" else dict(rtol=1e-5, atol=1e-5)
+    args = (gamma.numpy(), beta.numpy(), eps)
+    got_b = None
+    if variant == "strided":
+        S = 64
+        seqs = torch.randn(rows, S, w, generator=g) * 3 + 1
+        seqs[:, S - 1] = x
+        got, got_b = debug_layernorm(seqs.reshape(-1)[(S - 1) * w:].numpy(), *args, rows=rows, in_stride=S * w,
+                                     outputs="both")
+    elif variant == "bf16":
+        got = debug_layernorm(x.numpy(), *args)
+        got_b = debug_layernorm(x.numpy(), *args, outputs="bf16")
+    elif variant == "in_place":
+        got, got_b = debug_layernorm(x.numpy(), *args, outputs="both", in_place=True)
+    else:
+        got = debug_layernorm(x.numpy(), *args)
+    got = torch.from_numpy(got)
+    torch.testing.assert_close(got.double(), ref, **tol)
+    if got_b is not None:
+        assert torch.equal(torch.from_numpy(got_b), _bf16(got))
 
 
 @pytest.mark.parametrize("h,w", [(480, 640), (640, 480), (224, 224), (300, 224), (256, 256), (1000, 750), (225, 400), (100, 150)])
