@@ -465,6 +465,14 @@ int b200_debug_gemm_into(int device, const float* A, const float* W, const float
  * dim 1024, streamed above), -1 leaves the setting unchanged.  *last_kernel (when not NULL) receives the kernel the last
  * search ran: 0 resident query block, 1 streamed query block, -1 no search yet. */
 int b200_debug_index_scan_kernel(b200_index* ix, int force_streamed, int* last_kernel);
+/* What the last search of ix left on the device for its last query group (read only: no search state changes).
+ * *nq and *grid (when not NULL) receive the group's size and the scan's grid, both 0 before any scan.  Each array
+ * that is not NULL receives, for that group: eps fp32 [nq], the per-query bound on |approximate - exact| scan key;
+ * queries fp32 [nq, dim], the fp16 query block as it was scanned; list_score fp32, list_row and list_doc int32
+ * [grid, nq, 16], every scan CTA's sorted list of its 16 best (approximate key, row, document) per query, unused
+ * entries -inf / -1 / -1.  The collect pass and the merge do not write the lists, so the keys are the scan's. */
+int b200_debug_index_last_scan(b200_index* ix, int* nq, int* grid, float* eps, float* queries, float* list_score,
+                               int32_t* list_row, int32_t* list_doc);
 /* Mean device time (ms, CUDA events) of `iters` back-to-back GEMM launches [M,K] x [N,K]^T on device-generated data,
  * with the epilogue given by act, out_bf16, has_bias and residual_in_place (residual == out, fp32 only). */
 int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16, int has_bias, int residual_in_place,

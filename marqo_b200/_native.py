@@ -19,6 +19,7 @@ ACT_GELU, ACT_QUICKGELU = 0, 1
 POOL_MEAN, POOL_CLS = 0, 1
 GEMM_128x128, GEMM_PERSISTENT = 0, 1   # the GEMM kernel b200_debug_gemm_into reports
 SCAN_RESIDENT_Q, SCAN_STREAMED_Q = 0, 1   # the scan kernel b200_debug_index_scan_kernel reports
+SCAN_LIST_LEN = 16   # entries per (scan CTA, query) list b200_debug_index_last_scan returns
 MAX_INDEX_DIM = 4096   # widest row store b200_index_create accepts (a multiple of 64)
 MAX_ATTRIBUTE_COLUMNS = 64
 MAX_MODIFIER_TERMS = 16
@@ -118,6 +119,7 @@ _SIGNATURES = {
     "b200_debug_gemm_into": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.c_int, _P, C.POINTER(C.c_int)]),
     "b200_debug_index_scan_kernel": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int)]),
+    "b200_debug_index_last_scan": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), _P, _P, _P, _P, _P]),
     "b200_debug_gemm_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "b200_debug_patch_embed": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P]),
     "b200_debug_attention": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, _P]),

@@ -233,6 +233,11 @@ int b200_debug_index_scan_kernel(b200_index* ix, int force_streamed, int* last_k
     return guarded([&] { score::debug_scan_kernel(ix, force_streamed, last_kernel); });
 }
 
+int b200_debug_index_last_scan(b200_index* ix, int* nq, int* grid, float* eps, float* queries, float* list_score,
+                               int32_t* list_row, int32_t* list_doc) {
+    return guarded([&] { score::debug_last_scan(ix, nq, grid, eps, queries, list_score, list_row, list_doc); });
+}
+
 int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16, int has_bias, int residual_in_place,
                          int iters, float* out_ms) {
     return guarded([&] {

@@ -822,6 +822,8 @@ __global__ void exact_keys_kernel(ExactParams p, int q, const int32_t* rows, int
 // tensor core adds them (16 per instruction, dim / 16 instructions) with at most one truncation per addend, so
 //   |approx dot - exact dot| <= dim * 2^-23 * sum|q_i e_i| <= dim * 2^-23 * |q| |e|.
 // The bound used is twice that (c = dim * 2^-22) with |e| <= sqrt(max_n2), the largest stored row norm.
+// Measured on the H100 (tests/test_score_bound_gpu.py): wgmma adds each group of four products exactly and truncates
+// the sum once, so the worst error seen is a quarter of the per-addend model, 1/8 of the dot-product eps.
 __global__ void query_prep_kernel(const __half* __restrict__ qh, int dim, int metric, int has_mod,
                                   const float* __restrict__ max_n2, const double* __restrict__ mod_max, QState* qs) {
     const int q = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -1263,6 +1265,8 @@ struct b200_index {
     // ran (-1 before the first scan)
     bool force_streamed_q = false;
     int last_scan_kernel = -1;
+    // the query group the last scan ran on (debug_last_scan): its size and the scan grid (0 / 0 before any scan)
+    int last_nq = 0, last_grid = 0;
     cudaStream_t stream = nullptr;   // own_stream, or the caller's stream set by b200_index_set_stream
     UniqueStream own_stream;
     UniqueEvent ev[4];
@@ -1490,6 +1494,8 @@ ScanLaunch prepare_scan(b200_index* ix, int nq) {
     const bool docs = ix->has_docs || ix->filter_active;   // the filter is applied where the document numbers are read
     L.fn_index = (docs ? 1 : 0) | (bias ? 2 : 0) | (mod ? 4 : 0) | (stream_q ? 8 : 0);
     ix->last_scan_kernel = stream_q ? SCAN_STREAMED_Q : SCAN_RESIDENT_Q;
+    ix->last_nq = nq;
+    ix->last_grid = L.grid;
     return L;
 }
 
@@ -1576,6 +1582,7 @@ void search_group(b200_index* ix, int nq, int k, const GroupOut& out, bool recor
     const int total = nq * k;
     ++ix->stat_groups;
     if (ix->n_rows == 0) {
+        ix->last_nq = ix->last_grid = 0;   // nothing is scanned
         fill_empty_kernel<<<(total + 255) / 256, 256, 0, ix->stream>>>(out.doc, out.row, out.score, total);
         MB_CUDA(cudaGetLastError());
         return;
@@ -1918,6 +1925,39 @@ void mb::score::debug_scan_kernel(b200_index* ix, int force_streamed, int* last_
     std::lock_guard<std::mutex> lk(ix->mu);
     if (force_streamed >= 0) ix->force_streamed_q = force_streamed != 0;
     if (last_kernel) *last_kernel = ix->last_scan_kernel;
+}
+
+// The COLLECT pass and merge_kernel only read the SELECT lists, so after a search they still hold the scan's
+// approximate keys; query_prep_kernel is the only writer of eps and nothing writes qh until the next search.
+void mb::score::debug_last_scan(b200_index* ix, int* nq, int* grid, float* eps, float* queries, float* list_score,
+                                int32_t* list_row, int32_t* list_doc) {
+    MB_CHECK_ARG(ix != nullptr, "index is NULL");
+    std::lock_guard<std::mutex> lk(ix->mu);
+    DeviceGuard g(ix->device);
+    MB_CUDA(cudaStreamSynchronize(ix->stream));
+    const int n = ix->last_nq, gr = ix->last_grid;
+    if (nq) *nq = n;
+    if (grid) *grid = gr;
+    if (n == 0) return;
+    if (eps) {
+        std::vector<float> e(MQ);
+        MB_CUDA(cudaMemcpy(e.data(), ix->qs.get()->eps, MQ * sizeof(float), cudaMemcpyDeviceToHost));
+        std::copy(e.begin(), e.begin() + n, eps);
+    }
+    if (queries) {
+        std::vector<__half> h((size_t)n * ix->dim);
+        MB_CUDA(cudaMemcpy(h.data(), ix->qh.get(), h.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < h.size(); ++i) queries[i] = __half2float(h[i]);
+    }
+    // device lists are [grid][MQ][KP]; the caller's are [grid][nq][KP]
+    auto lists = [&](void* dst, const void* src, size_t elem) {
+        if (!dst) return;
+        MB_CUDA(cudaMemcpy2D(dst, (size_t)n * KP * elem, src, (size_t)MQ * KP * elem, (size_t)n * KP * elem, (size_t)gr,
+                             cudaMemcpyDeviceToHost));
+    };
+    lists(list_score, ix->list_score.get(), sizeof(float));
+    lists(list_row, ix->list_row.get(), sizeof(int32_t));
+    lists(list_doc, ix->list_doc.get(), sizeof(int32_t));
 }
 
 extern "C" {

@@ -10,5 +10,9 @@ namespace score {
 // the kernel the last scan ran: 0 resident query block, 1 streamed, -1 no scan yet.
 void debug_scan_kernel(b200_index* ix, int force_streamed, int* last_kernel);
 
+// What the last scan of `ix` left on the device, for its query group (see b200_debug_index_last_scan).
+void debug_last_scan(b200_index* ix, int* nq, int* grid, float* eps, float* queries, float* list_score,
+                     int32_t* list_row, int32_t* list_doc);
+
 }  // namespace score
 }  // namespace mb

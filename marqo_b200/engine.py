@@ -564,6 +564,27 @@ def debug_scan_kernel(store: RowStore, force_streamed: Optional[bool] = None) ->
     return last.value
 
 
+def debug_last_scan(store: RowStore) -> dict:
+    """What `store`'s last search left on the device for its last query group (at most 64 queries):
+    {"nq", "grid", "eps" fp32 [nq] (bound on |approximate - exact| scan key), "queries" fp32 [nq, dim] (the fp16 query
+    block as scanned), "list_score" fp32 / "list_row" / "list_doc" int32 [grid, nq, _native.SCAN_LIST_LEN] (each scan
+    CTA's best approximate keys per query)}.  nq = grid = 0 before any search."""
+    lib, h = N.load(), store._handle()
+    nq, grid = C.c_int(0), C.c_int(0)
+    N.check(lib.b200_debug_index_last_scan(h, C.byref(nq), C.byref(grid), None, None, None, None, None))
+    n, g = nq.value, grid.value
+    eps = np.empty(n, np.float32)
+    queries = np.empty((n, store.dim), np.float32)
+    score = np.empty((g, n, N.SCAN_LIST_LEN), np.float32)
+    row = np.empty((g, n, N.SCAN_LIST_LEN), np.int32)
+    doc = np.empty((g, n, N.SCAN_LIST_LEN), np.int32)
+    N.check(lib.b200_debug_index_last_scan(h, C.byref(nq), C.byref(grid), _ptr(eps), _ptr(queries), _ptr(score),
+                                           _ptr(row), _ptr(doc)))
+    if (nq.value, grid.value) != (n, g):
+        raise RuntimeError("the store was searched between the two reads of its last scan")
+    return {"nq": n, "grid": g, "eps": eps, "queries": queries, "list_score": score, "list_row": row, "list_doc": doc}
+
+
 def debug_gemm_ln(A, W, bias, residual, gamma, beta, eps: float, in_place: bool = False, repeats: int = 1,
                   device: int = 0):
     """Residual GEMM followed by the LayerNorm launch -> (x fp32 [M, N], LayerNorm(x) rounded to bf16 [M, N])."""
