@@ -436,30 +436,22 @@ int b200_jpeg_decode_batch(int device, const uint8_t* const* files, const size_t
                            int32_t* heights, int32_t* widths, int32_t* status);
 
 /* ===================================================================================== */
-/* Diagnostics: run ONE kernel of the encoder on host data (used by the kernel-level     */
-/* numerics tests; not part of the reference-facing surface).                            */
+/* Diagnostics: run ONE kernel of the encoder (used by the kernel-level numerics tests;  */
+/* not part of the reference-facing surface).  The hooks with a `stream` argument take   */
+/* device buffers on `device`, bf16 ones typed void*, except where a comment says host;  */
+/* they run on `stream` (a cudaStream_t, 0: the legacy default stream) and synchronise   */
+/* it before they return.                                                                */
 /* ===================================================================================== */
 
-/* out[M,N] = act(A[M,K] @ W[N,K]^T + bias) (+ residual); A and W are rounded to bf16 on the device, fp32
- * accumulate; act: 0 none, 1 erf-GELU, 2 QuickGELU; bias/residual may be NULL; out_bf16 != 0 rounds the result to
- * bf16 before it is returned as fp32. */
-int b200_debug_gemm(int device, const float* A, const float* W, const float* bias, const float* residual, int M, int N,
-                    int K, int act, int out_bf16, float* out);
-/* Residual GEMM followed by the LayerNorm launch, as the encoder layers run them: out_x fp32 [M,N] = A W^T + bias
- * (+ residual); out_ln = LayerNorm(out_x) * gamma + beta rounded to bf16 (returned as fp32).  in_place != 0: the fp32
- * normalised rows also replace out_x (BERT post-LN).  The pair is repeated `repeats` times; with in_place == 0 every
- * repeat computes the same thing. */
-int b200_debug_gemm_ln(int device, const float* A, const float* W, const float* bias, const float* residual, int M, int N,
-                       int K, const float* gamma, const float* beta, float eps, int in_place, int repeats, float* out_x,
-                       float* out_ln);
-/* GEMM into an existing output buffer: io fp32 [out_rows, ldo] (out_rows >= M, ldo >= N) is uploaded (as bf16 when
- * out_bf16 != 0), rows [0, M) x columns [0, N) are overwritten with act(A W^T + bias) (+ the old contents when
- * residual_in_place != 0: residual == out, fp32 only), and the whole buffer is copied back into io.  The library picks
- * the kernel by its usual rule for an SM count of sms (0: the device's own); *kernel_out (when not NULL) receives the
- * kernel it ran: 0 the 128 x 128 tiles, 1 the persistent 128 x 256 tiles. */
-int b200_debug_gemm_into(int device, const float* A, const float* W, const float* bias, int M, int N, int K, int act,
-                         int out_bf16, int residual_in_place, int out_rows, int ldo, int sms, float* io,
-                         int* kernel_out);
+/* out = act(A @ W^T + bias) (+ residual) over rows [0, M) x columns [0, N): A bf16 [M, lda], W bf16 [N, K], fp32
+ * accumulate; act: 0 none, 1 erf-GELU, 2 QuickGELU; bias fp32 [N] and residual fp32 [M, ldr] may be NULL, and residual
+ * may be out itself (fp32 only), as the encoder layers update their residual stream.  out [M, ldo] is bf16 when
+ * out_bf16 != 0, fp32 otherwise.  The library picks the kernel by its usual rule for an SM count of sms (0: the
+ * device's own); *kernel_out (when not NULL) receives the kernel it ran: 0 the 128 x 128 tiles, 1 the persistent
+ * 128 x 256 tiles. */
+int b200_debug_gemm(int device, const void* A, int lda, const void* W, const float* bias, const float* residual, int ldr,
+                    void* out, int ldo, int out_bf16, int act, int M, int N, int K, int sms, int* kernel_out,
+                    void* stream);
 /* Scan kernel of a row store.  force_streamed: 1 makes every later search of ix scan with the streamed-query kernel
  * whatever its dim (so both kernels can run on one corpus), 0 restores the library's rule (resident query block up to
  * dim 1024, streamed above), -1 leaves the setting unchanged.  *last_kernel (when not NULL) receives the kernel the last
@@ -479,17 +471,18 @@ int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16,
                          int iters, float* out_ms);
 /* ViT patch embedding of uint8 HWC images [n,S,S,3], the token rows the image forward feeds to ln_pre: out fp32
  * [n*(G+1), N], row b*(G+1) = cls + pos[0], row b*(G+1)+1+i = conv1(patch i of image b) + pos[1+i], where the patch is
- * ToTensor + Normalize (mean3/std3)-ed and conv1 is conv_w fp32 [N, 3*patch*patch] without bias.  cls fp32 [N] and pos
- * fp32 [G+1, N] may be NULL (zeros).  The fused gather GEMM: no patch matrix in HBM,
+ * ToTensor + Normalize (mean3/std3, host fp32 [3])-ed and conv1 is conv_w fp32 [N, 3*patch*patch] without bias.
+ * cls fp32 [N], pos fp32 [G+1, N].  The fused gather GEMM: no patch matrix in HBM,
  * src/marqo/tensor_search/add_docs.py:129-134 folded into the operand load. */
 int b200_debug_patch_embed(int device, const uint8_t* hwc, int n, int S, int patch, const float* conv_w, int N,
-                           const float* mean3, const float* std3, const float* cls, const float* pos, float* out);
-/* softmax(q k^T / sqrt(head_dim) + mask + bias) v over packed qkv fp32 [B*S, 3*W] (rounded to bf16), head_dim = W / H
- * (32 or 64); mask: 0 none, 1 causal, 2 key length (kv_len int32 [B]).  rel_bias (NULL: none) is MPNet's
- * relative-position bias, fp32 [H, 2*smax - 1] (natural-log domain, as it enters softmax): rel_bias[h, j - i + smax - 1]
- * is added to the logit of query i and key j; head_dim 64, mask 2, S <= smax.  out fp32 [B*S, W]. */
-int b200_debug_attention(int device, const float* qkv, int B, int S, int W, int H, int mask, const int32_t* kv_len,
-                         const float* rel_bias, int smax, float* out);
+                           const float* mean3, const float* std3, const float* cls, const float* pos, float* out,
+                           void* stream);
+/* softmax(q k^T / sqrt(head_dim) + mask + bias) v over packed qkv bf16 [B*S, 3*W], head_dim = W / H (32 or 64);
+ * mask: 0 none, 1 causal, 2 key length (kv_len int32 [B]).  rel_bias (NULL: none) is MPNet's relative-position bias,
+ * a host array fp32 [H, 2*smax - 1] (natural-log domain, as it enters softmax): rel_bias[h, j - i + smax - 1] is added
+ * to the logit of query i and key j; head_dim 64, mask 2, S <= smax.  out bf16 [B*S, W]. */
+int b200_debug_attention(int device, const void* qkv, int B, int S, int W, int H, int mask, const int32_t* kv_len,
+                         const float* rel_bias, int smax, void* out, void* stream);
 /* MPNet's relative_position_bucket as the model builds its bias table: out[d + max_len - 1] = bucket of
  * key - query = d for |d| < max_len (host-only). */
 int b200_debug_relative_position_buckets(int num_buckets, int max_distance, int max_len, int32_t* out);
@@ -497,69 +490,68 @@ int b200_debug_relative_position_buckets(int num_buckets, int max_distance, int 
  * kept; rel_bias != 0 adds a generated relative-position bias table with smax = S (the bias runs with mask 2). */
 int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, int rel_bias, int iters, float* out_ms);
 /* LayerNorm over `rows` rows of width w, row r read at x + r * in_stride (0: w); x holds (rows - 1) * in_stride + w
- * floats.  out_f32 / out_bf16 (either may be NULL, not both) receive the fp32 and the bf16 output [rows, w], the bf16
- * one as fp32.  in_place != 0 writes the fp32 output over x on the device (needs out_f32 and in_stride == w). */
+ * floats.  out_f32 (fp32) and out_bf16 (bf16), either may be NULL but not both, receive the output [rows, w].
+ * out_f32 == x normalises in place (needs in_stride == w). */
 int b200_debug_layernorm(int device, const float* x, long long in_stride, const float* gamma, const float* beta, float eps,
-                         int rows, int w, int in_place, float* out_f32, float* out_bf16);
+                         int rows, int w, float* out_f32, void* out_bf16, void* stream);
 /* CLIP / SigLIP text embedding: x fp32 [n*S, w] = tok[ids] + pos[s], eot int32 [n] = first arg-max of each ids row.
  * tok [vocab, w], pos [S, w]. */
 int b200_debug_clip_text_embed(int device, const int32_t* ids, const float* tok, const float* pos, int n, int S, int w,
-                               int vocab, float* x, int32_t* eot);
-/* BERT embedding + LayerNorm: x fp32 [n*S, w] = LN(word[ids] + type0 + pos[s]), h = the bf16 copy (as fp32), kv_len
- * int32 [n] = sum of each mask row (S when mask is NULL).  pos has pos_rows >= S rows; type0 [w] is required. */
-int b200_debug_bert_embed_ln(int device, const int32_t* ids, const int32_t* mask, const float* word, const float* pos,
-                             int pos_rows, const float* type0, const float* gamma, const float* beta, float eps, int n,
-                             int S, int w, int vocab, float* x, float* h, int32_t* kv_len);
-/* RoBERTa embedding + LayerNorm (XLM-R with type0, MPNet with type0 NULL): as above with HF's position ids counted from
- * the ids and pad; pos has pos_rows >= pad + S + 1 rows. */
-int b200_debug_roberta_embed_ln(int device, const int32_t* ids, const int32_t* mask, const float* word, const float* pos,
-                                int pos_rows, const float* type0, const float* gamma, const float* beta, float eps, int n,
-                                int S, int w, int vocab, int pad, float* x, float* h, int32_t* kv_len);
-/* CLIP head over token rows x fp32 [n*S, w]: LN(row b*S + row_in_seq[b]) @ proj [w, E] (row_in_seq NULL: row 0), divided
- * by its L2 norm if normalize.  out fp32 [n, E]. */
+                               int vocab, float* x, int32_t* eot, void* stream);
+/* Embedding + LayerNorm: x fp32 [n*S, w] = LN(word[ids] + type0 + pos[p]), h bf16 [n*S, w] its bf16 copy, kv_len int32
+ * [n] = sum of each mask row (S when mask is NULL).  pad < 0: BERT, p = s, type0 [w] required, pos_rows >= S.
+ * pad >= 0: RoBERTa (XLM-R with type0, MPNet with type0 NULL), HF's position ids counted from the ids and pad,
+ * pos_rows >= pad + S + 1. */
+int b200_debug_embed_ln(int device, const int32_t* ids, const int32_t* mask, const float* word, const float* pos,
+                        int pos_rows, const float* type0, const float* gamma, const float* beta, float eps, int n, int S,
+                        int w, int vocab, int pad, float* x, void* h, int32_t* kv_len, void* stream);
+/* CLIP head over token rows x fp32 [n*S, w]: LN(row b*S + row_in_seq[b]) @ proj [w, E] (row_in_seq NULL: row 0;
+ * every entry must lie in [0, S)), divided by its L2 norm if normalize.  out fp32 [n, E]. */
 int b200_debug_clip_head(int device, const float* x, int S, const int32_t* row_in_seq, const float* gamma,
-                         const float* beta, float eps, const float* proj, int n, int w, int E, int normalize, float* out);
+                         const float* beta, float eps, const float* proj, int n, int w, int E, int normalize, float* out,
+                         void* stream);
 /* BERT head over x fp32 [n*S, w]: mean of the first kv_len[b] rows (pool 0) or row 0 (pool 1), then F.normalize if
  * normalize.  out fp32 [n, w]. */
 int b200_debug_bert_head(int device, const float* x, const int32_t* kv_len, int n, int S, int w, int pool, int normalize,
-                         float* out);
+                         float* out, void* stream);
 /* out fp32 [n, E] = src / |src| per row if normalize, else src. */
-int b200_debug_l2_rows(int device, const float* src, int n, int E, int normalize, float* out);
-/* ResNet stem im2col: exactly one of hwc (uint8 [n,S,S,3], normalised with mean3 / std3) and chw (fp32 [n,3,S,S]) ->
- * out fp32 [n*(S/2)^2, 64] (rounded to bf16). */
+int b200_debug_l2_rows(int device, const float* src, int n, int E, int normalize, float* out, void* stream);
+/* ResNet stem im2col: exactly one of hwc (uint8 [n,S,S,3], normalised with mean3 / std3, host fp32 [3]) and chw (fp32
+ * [n,3,S,S]) -> out bf16 [n*(S/2)^2, 64]. */
 int b200_debug_stem_im2col(int device, const uint8_t* hwc, const float* chw, int n, int S, const float* mean3,
-                           const float* std3, float* out);
-/* AvgPool2d(2) over NHWC x fp32 [n,H,W,C] (rounded to bf16) -> out fp32 [n,H/2,W/2,C] (rounded to bf16). */
-int b200_debug_avgpool2(int device, const float* x, int n, int H, int W, int C, float* out);
-/* ResNet attention-pool tokens: x fp32 [n,HW,C] (rounded to bf16), pos fp32 [HW+1, C] -> out fp32 [n*(HW+1), C]
- * (rounded to bf16): row 0 = mean_s x_s + pos[0], row 1+s = x_s + pos[1+s]. */
-int b200_debug_attnpool_tokens(int device, const float* x, const float* pos, int n, int HW, int C, float* out);
-/* ViT im2col of fp32 CHW [n,3,S,S] -> out fp32 [n*((S/p)^2 + cls), kpad] (rounded to bf16), k = c*p*p + dy*p + dx. */
-int b200_debug_im2col_f32(int device, const float* chw, int n, int S, int p, int kpad, int cls, float* out);
+                           const float* std3, void* out, void* stream);
+/* AvgPool2d(2) over NHWC x bf16 [n,H,W,C] -> out bf16 [n,H/2,W/2,C]. */
+int b200_debug_avgpool2(int device, const void* x, int n, int H, int W, int C, void* out, void* stream);
+/* ResNet attention-pool tokens: x bf16 [n,HW,C], pos fp32 [HW+1, C] -> out bf16 [n*(HW+1), C]: row 0 = mean_s x_s +
+ * pos[0], row 1+s = x_s + pos[1+s]. */
+int b200_debug_attnpool_tokens(int device, const void* x, const float* pos, int n, int HW, int C, void* out,
+                               void* stream);
+/* ViT im2col of fp32 CHW [n,3,S,S] -> out bf16 [n*((S/p)^2 + cls), kpad], k = c*p*p + dy*p + dx. */
+int b200_debug_im2col_f32(int device, const float* chw, int n, int S, int p, int kpad, int cls, void* out, void* stream);
 /* The JPEG decoder's arithmetic (shared __host__ __device__ code of the two kernels) run on the host: lets the CPU test
  * suite pin it against Pillow pixel for pixel.  A test hook, not a product path.  out_rgb == NULL: size query. */
 int b200_debug_jpeg_decode_host(const uint8_t* file, size_t nbytes, uint8_t* out_rgb, size_t out_capacity,
                                 int32_t* out_height, int32_t* out_width);
 /* Pillow-compatible bicubic resize (shortest side -> S) + centre crop of uint8 HWC images [n,h,w,3] -> [n,S,S,3]. */
-int b200_debug_resize(int device, const uint8_t* hwc, int n, int h, int w, int S, uint8_t* out);
+int b200_debug_resize(int device, const uint8_t* hwc, int n, int h, int w, int S, uint8_t* out, void* stream);
 /* The same bicubic resampling squashed to S x S (x and y scaled independently, no crop): PIL resize((S, S), BICUBIC),
  * SigLIP's preprocessing. */
-int b200_debug_resize_squash(int device, const uint8_t* hwc, int n, int h, int w, int S, uint8_t* out);
-/* SigLIP's MAP pooling attention: for image b and head h, softmax(q_h . k_{b,s} / sqrt(64)) over the S tokens of image
- * b, times v_{b,s}.  q fp32 [W] (one latent query, shared by every image); kv fp32 [B*S, 2W] (K columns then V columns,
- * rounded to bf16); head_dim 64.  out fp32 [B, W] (rounded to bf16). */
-int b200_debug_map_attention(int device, const float* q, const float* kv, int B, int S, int W, int H, float* out);
-/* The same with one query per image (the ResNet attention pool): q fp32 [B, W]. */
-int b200_debug_map_attention_per_image(int device, const float* q, const float* kv, int B, int S, int W, int H,
-                                       float* out);
-/* One convolution of the ResNet CLIP image tower, on the path the model runs it: out = act(conv(x) + bias (+ residual))
- * rounded to bf16, NHWC fp32 in and out (x, w, bias and residual are rounded to bf16 first, the bias kept fp32).
- * x [n, H, W, cin]; w [cout, cin, k, k] (torch layout); bias [cout] (NULL: zeros).  cin == 3: the stem conv1 (k 3,
- * stride 2, padding 1; out [n, H/2, W/2, cout], x already normalised).  Otherwise k 1 (a GEMM over the pixels) or 3
- * (the implicit GEMM, stride 1, padding 1, cin a power of two >= 32); out [n, H, W, cout].  relu != 0: ReLU, with the
- * optional residual [n, H, W, cout] added before it; relu == 0 (1 x 1 and stem convs only) takes no residual. */
-int b200_debug_conv2d(int device, const float* x, int n, int H, int W, int cin, const float* w, int cout, int k,
-                      const float* bias, const float* residual, int relu, float* out);
+int b200_debug_resize_squash(int device, const uint8_t* hwc, int n, int h, int w, int S, uint8_t* out, void* stream);
+/* Single-query attention pooling: for image b and head h, softmax(q_h . k_{b,s} / sqrt(64)) over the S tokens of image
+ * b, times v_{b,s}.  q fp32, image b's query at q + b * q_stride: q_stride 0 shares one latent query [W] by every
+ * image (SigLIP's MAP head), q_stride W gives one per image [B, W] (the ResNet attention pool).  kv bf16 [B*S, 2W]
+ * (K columns then V columns); head_dim 64.  out bf16 [B, W]. */
+int b200_debug_map_attention(int device, const float* q, int q_stride, const void* kv, int B, int S, int W, int H,
+                             void* out, void* stream);
+/* One convolution of the ResNet CLIP image tower, on the path the model runs it: out bf16 = act(conv(x) + bias
+ * (+ residual)).  w is a host array fp32 [cout, cin, k, k] (torch layout), laid out and rounded to bf16 as the model's
+ * finalize does; bias fp32 [cout].  cin == 3: the stem conv1 (k 3, stride 2, padding 1) of x fp32 CHW [n, 3, H, W],
+ * already normalised, as b200_model_encode_images_f32 receives it; out [n, H/2, W/2, cout].  Otherwise x bf16 NHWC
+ * [n, H, W, cin] and k 1 (a GEMM over the pixels) or 3 (the implicit GEMM, stride 1, padding 1, cin a power of two
+ * >= 32); out [n, H, W, cout].  relu != 0: ReLU, with the optional residual bf16 [n, H, W, cout] added before it;
+ * relu == 0 (1 x 1 and stem convs only) takes no residual. */
+int b200_debug_conv2d(int device, const void* x, int n, int H, int W, int cin, const float* w, int cout, int k,
+                      const float* bias, const void* residual, int relu, void* out, void* stream);
 /* Bytes of device memory the library holds right now, over all devices and handles of this process (indexes,
  * exchanges, models and the scratch of calls in flight).  Memory from b200_host_alloc is not counted.  Returns to its
  * earlier value once every handle created in between is destroyed: a leak check. */

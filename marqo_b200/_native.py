@@ -17,7 +17,7 @@ METRIC_PRENORMALIZED_ANGULAR, METRIC_ANGULAR, METRIC_DOTPRODUCT, METRIC_EUCLIDEA
 ARCH_CLIP, ARCH_BERT, ARCH_MPNET, ARCH_SIGLIP, ARCH_XLMR, ARCH_CLIP_RESNET = 0, 1, 2, 3, 4, 5
 ACT_GELU, ACT_QUICKGELU = 0, 1
 POOL_MEAN, POOL_CLS = 0, 1
-GEMM_128x128, GEMM_PERSISTENT = 0, 1   # the GEMM kernel b200_debug_gemm_into reports
+GEMM_128x128, GEMM_PERSISTENT = 0, 1   # the GEMM kernel b200_debug_gemm reports
 SCAN_RESIDENT_Q, SCAN_STREAMED_Q = 0, 1   # the scan kernel b200_debug_index_scan_kernel reports
 SCAN_LIST_LEN = 16   # entries per (scan CTA, query) list b200_debug_index_last_scan returns
 MAX_INDEX_DIM = 4096   # widest row store b200_index_create accepts (a multiple of 64)
@@ -114,38 +114,33 @@ _SIGNATURES = {
     "b200_model_set_profiling": (C.c_int, [_P, C.c_int]),
     "b200_model_profile": (C.c_int, [_P, C.POINTER(C.c_float), C.POINTER(C.c_int), C.POINTER(C.c_float), C.POINTER(C.c_int)]),
     "b200_model_last_timing": (C.c_int, [_P, C.POINTER(C.c_float), C.POINTER(C.c_int)]),
-    "b200_debug_gemm": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
-    "b200_debug_gemm_ln": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_float, C.c_int, C.c_int, _P, _P]),
-    "b200_debug_gemm_into": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                       C.c_int, _P, C.POINTER(C.c_int)]),
+    "b200_debug_gemm": (C.c_int, [C.c_int, _P, C.c_int, _P, _P, _P, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                  C.c_int, C.c_int, C.POINTER(C.c_int), _P]),
     "b200_debug_index_scan_kernel": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int)]),
     "b200_debug_index_last_scan": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), _P, _P, _P, _P, _P]),
     "b200_debug_gemm_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float)]),
-    "b200_debug_patch_embed": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P]),
-    "b200_debug_attention": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, _P]),
+    "b200_debug_patch_embed": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P]),
+    "b200_debug_attention": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P]),
     "b200_debug_relative_position_buckets": (C.c_int, [C.c_int, C.c_int, C.c_int, _P]),
     "b200_debug_attention_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                             C.POINTER(C.c_float)]),
-    "b200_debug_layernorm": (C.c_int, [C.c_int, _P, C.c_longlong, _P, _P, C.c_float, C.c_int, C.c_int, C.c_int, _P, _P]),
-    "b200_debug_clip_text_embed": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
-    "b200_debug_bert_embed_ln": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, _P, _P, _P, C.c_float, C.c_int, C.c_int,
-                                           C.c_int, C.c_int, _P, _P, _P]),
-    "b200_debug_roberta_embed_ln": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, _P, _P, _P, C.c_float, C.c_int, C.c_int,
-                                              C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "b200_debug_layernorm": (C.c_int, [C.c_int, _P, C.c_longlong, _P, _P, C.c_float, C.c_int, C.c_int, _P, _P, _P]),
+    "b200_debug_clip_text_embed": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "b200_debug_embed_ln": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, _P, _P, _P, C.c_float, C.c_int, C.c_int, C.c_int,
+                                      C.c_int, C.c_int, _P, _P, _P, _P]),
     "b200_debug_clip_head": (C.c_int, [C.c_int, _P, C.c_int, _P, _P, _P, C.c_float, _P, C.c_int, C.c_int, C.c_int, C.c_int,
-                                       _P]),
-    "b200_debug_bert_head": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
-    "b200_debug_l2_rows": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P]),
-    "b200_debug_stem_im2col": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P]),
-    "b200_debug_avgpool2": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
-    "b200_debug_attnpool_tokens": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
-    "b200_debug_im2col_f32": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
-    "b200_debug_resize": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
-    "b200_debug_resize_squash": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
-    "b200_debug_map_attention": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
-    "b200_debug_map_attention_per_image": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+                                       _P, _P]),
+    "b200_debug_bert_head": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_l2_rows": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_stem_im2col": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
+    "b200_debug_avgpool2": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_attnpool_tokens": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_im2col_f32": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_resize": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_resize_squash": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_map_attention": (C.c_int, [C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_conv2d": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, C.c_int,
-                                    _P]),
+                                    _P, _P]),
     "b200_debug_device_bytes": (C.c_int, [C.POINTER(C.c_int64)]),
     "b200_jpeg_info": (C.c_int, [_P, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200_jpeg_decode_batch": (C.c_int, [C.c_int, _P, _P, C.c_int, _P, _P, _P, _P]),

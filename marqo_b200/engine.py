@@ -523,16 +523,57 @@ class Encoder:
 # ---------------------------------------------------------------------------------------------------------
 # Kernel-level diagnostics (b200_debug_*)
 # ---------------------------------------------------------------------------------------------------------
+class _Staging:
+    """The device side of one b200_debug_* call: host arrays as torch tensors on cuda:{device}, and that device's
+    current stream, which the hook runs on and synchronises.  The library looks for the device before torch touches
+    CUDA, so without one the call fails with ERR_NO_DEVICE, as every compute entry point does."""
+
+    def __init__(self, device: int):
+        if not 0 <= device < N.device_count():
+            raise N.NativeError(N.ERR_NO_DEVICE, f"CUDA device {device} not available (marqo_b200 has no CPU fallback)")
+        import torch
+        self.torch, self.device = torch, device
+        self.dev = torch.device("cuda", device)
+        self.stream = torch.cuda.current_stream(self.dev).cuda_stream
+
+    def up(self, a, dtype: str = "float32"):
+        """a (None stays None) on the device as `dtype` (a torch dtype name); "bfloat16" rounds fp32 values to nearest
+        even, as __float2bfloat16_rn does."""
+        if a is None:
+            return None
+        t = self.torch.from_numpy(_as(a, np.float32 if dtype == "bfloat16" else dtype)).to(self.dev)
+        return t.to(getattr(self.torch, dtype))
+
+    def empty(self, shape, dtype: str = "float32"):
+        return self.torch.empty(shape, dtype=getattr(self.torch, dtype), device=self.dev)
+
+
+def _dptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def _host(t) -> np.ndarray:
+    """A device tensor as a host array, bf16 widened to fp32."""
+    return (t.float() if t.is_floating_point() else t).cpu().numpy()
+
+
+def _gemm(d: _Staging, a, w, bias, residual, out, act: int = 0, sms: int = 0) -> int:
+    """b200_debug_gemm: out[:M, :N] = act(a w^T + bias) (+ residual) for bf16 a [M, >= K], w [N, K] and out fp32 or
+    bf16 [>= M, >= N]; residual may be out itself.  Returns the kernel that ran."""
+    kernel = C.c_int(-1)
+    N.check(N.load().b200_debug_gemm(d.device, _dptr(a), a.stride(0), _dptr(w), _dptr(bias), _dptr(residual),
+                                     0 if residual is None else residual.stride(0), _dptr(out), out.stride(0),
+                                     int(out.dtype == d.torch.bfloat16), act, a.shape[0], w.shape[0], w.shape[1], sms,
+                                     C.byref(kernel), d.stream))
+    return kernel.value
+
+
 def debug_gemm(A, W, bias=None, residual=None, act: int = 0, out_bf16: bool = False, device: int = 0) -> np.ndarray:
-    A, W = _as(A, np.float32), _as(W, np.float32)
-    M, K = A.shape
-    Nn = W.shape[0]
-    b = None if bias is None else _as(bias, np.float32)
-    r = None if residual is None else _as(residual, np.float32)
-    out = np.empty((M, Nn), np.float32)
-    N.check(N.load().b200_debug_gemm(device, _ptr(A), _ptr(W), _ptr(b), _ptr(r), M, Nn, K, act, 1 if out_bf16 else 0,
-                                     _ptr(out)))
-    return out
+    d = _Staging(device)
+    a, w, b, r = d.up(A, "bfloat16"), d.up(W, "bfloat16"), d.up(bias), d.up(residual)
+    out = d.empty((a.shape[0], w.shape[0]), "bfloat16" if out_bf16 else "float32")
+    _gemm(d, a, w, b, r, out, act)
+    return _host(out)
 
 
 def debug_gemm_into(A, W, io, bias=None, act: int = 0, out_bf16: bool = False, residual_in_place: bool = False,
@@ -542,16 +583,14 @@ def debug_gemm_into(A, W, io, bias=None, act: int = 0, out_bf16: bool = False, r
     buffer is returned as the kernel left it.  The kernel is chosen by the library's rule for an SM count of sms (None:
     the device's own).  Returns the buffer, or with return_kernel (the buffer, the kernel that ran:
     _native.GEMM_128x128 or _native.GEMM_PERSISTENT)."""
-    A, W = _as(A, np.float32), _as(W, np.float32)
-    M, K = A.shape
-    Nn = W.shape[0]
-    b = None if bias is None else _as(bias, np.float32)
-    out = np.array(io, dtype=np.float32, order="C", copy=True)
-    kernel = C.c_int(-1)
-    N.check(N.load().b200_debug_gemm_into(device, _ptr(A), _ptr(W), _ptr(b), M, Nn, K, act, int(out_bf16),
-                                          int(residual_in_place), out.shape[0], out.shape[1], sms or 0, _ptr(out),
-                                          C.byref(kernel)))
-    return (out, kernel.value) if return_kernel else out
+    io = _as(io, np.float32)
+    if io.ndim != 2 or io.shape[0] < len(A) or io.shape[1] < len(W):
+        raise ValueError(f"io {io.shape} does not hold the [{len(A)}, {len(W)}] product")
+    d = _Staging(device)
+    a, w, b = d.up(A, "bfloat16"), d.up(W, "bfloat16"), d.up(bias)
+    out = d.up(io, "bfloat16" if out_bf16 else "float32")
+    kernel = _gemm(d, a, w, b, out if residual_in_place else None, out, act, sms or 0)
+    return (_host(out), kernel) if return_kernel else _host(out)
 
 
 def debug_scan_kernel(store: RowStore, force_streamed: Optional[bool] = None) -> int:
@@ -587,18 +626,21 @@ def debug_last_scan(store: RowStore) -> dict:
 
 def debug_gemm_ln(A, W, bias, residual, gamma, beta, eps: float, in_place: bool = False, repeats: int = 1,
                   device: int = 0):
-    """Residual GEMM followed by the LayerNorm launch -> (x fp32 [M, N], LayerNorm(x) rounded to bf16 [M, N])."""
-    A, W = _as(A, np.float32), _as(W, np.float32)
-    M, K = A.shape
-    Nn = W.shape[0]
-    b = None if bias is None else _as(bias, np.float32)
-    r = None if residual is None else _as(residual, np.float32)
-    g, be = _as(gamma, np.float32), _as(beta, np.float32)
-    out_x = np.empty((M, Nn), np.float32)
-    out_ln = np.empty((M, Nn), np.float32)
-    N.check(N.load().b200_debug_gemm_ln(device, _ptr(A), _ptr(W), _ptr(b), _ptr(r), M, Nn, K, _ptr(g), _ptr(be),
-                                        float(eps), 1 if in_place else 0, repeats, _ptr(out_x), _ptr(out_ln)))
-    return out_x, out_ln
+    """Residual GEMM followed by the LayerNorm launch, as the encoder layers run them, `repeats` times on the same
+    buffers -> (x fp32 [M, N], LayerNorm(x) rounded to bf16 [M, N]).  in_place: the normalised fp32 rows also replace x
+    (BERT's post-LN)."""
+    if repeats < 1:
+        raise ValueError(f"repeats must be positive, got {repeats}")
+    d = _Staging(device)
+    a, w, b, r = d.up(A, "bfloat16"), d.up(W, "bfloat16"), d.up(bias), d.up(residual)
+    g, be = d.up(gamma), d.up(beta)
+    M, Nn = a.shape[0], w.shape[0]
+    x, ln = d.empty((M, Nn)), d.empty((M, Nn), "bfloat16")
+    for _ in range(repeats):
+        _gemm(d, a, w, b, r, x)
+        N.check(N.load().b200_debug_layernorm(device, _dptr(x), Nn, _dptr(g), _dptr(be), float(eps), M, Nn,
+                                              _dptr(x) if in_place else None, _dptr(ln), d.stream))
+    return _host(x), _host(ln)
 
 
 def debug_patch_embed(images_u8, patch: int, conv_w, mean, std, pos=None, cls=None, device: int = 0) -> np.ndarray:
@@ -610,12 +652,14 @@ def debug_patch_embed(images_u8, patch: int, conv_w, mean, std, pos=None, cls=No
     Nn = w.shape[0]
     G = (S // patch) ** 2
     m3, s3 = _as(mean, np.float32), _as(std, np.float32)
-    cs = None if cls is None else _as(cls, np.float32)
-    ps = None if pos is None else _as(pos, np.float32)
-    out = np.empty((n * (G + 1), Nn), np.float32)
-    N.check(N.load().b200_debug_patch_embed(device, _ptr(img), n, S, patch, _ptr(w), Nn, _ptr(m3), _ptr(s3), _ptr(cs),
-                                            _ptr(ps), _ptr(out)))
-    return out
+    d = _Staging(device)
+    di, dw = d.up(img, "uint8"), d.up(w)
+    dc = d.up(np.zeros(Nn) if cls is None else cls)
+    dp = d.up(np.zeros((G + 1, Nn)) if pos is None else pos)
+    out = d.empty((n * (G + 1), Nn))
+    N.check(N.load().b200_debug_patch_embed(device, _dptr(di), n, S, patch, _dptr(dw), Nn, _ptr(m3), _ptr(s3),
+                                            _dptr(dc), _dptr(dp), _dptr(out), d.stream))
+    return _host(out)
 
 
 def debug_attention(qkv, B: int, S: int, W: int, H: int, mask: int = 0, kv_len=None, device: int = 0,
@@ -623,19 +667,20 @@ def debug_attention(qkv, B: int, S: int, W: int, H: int, mask: int = 0, kv_len=N
     """softmax(q k^T / sqrt(hd) + mask) v over packed qkv.  rel_bias: MPNet's relative-position bias, fp32
     [H, 2 * smax - 1], adds rel_bias[h, j - i + smax - 1] to the logit of query i and key j (key-length mask only,
     head_dim 64, S <= smax)."""
-    q = _as(qkv, np.float32)
-    kl = None if kv_len is None else _as(kv_len, np.int32)
-    out = np.empty((B * S, W), np.float32)
     rb, smax = None, 0
     if rel_bias is not None:
         rb = _as(rel_bias, np.float32)
-        if mask != 2 or kl is None:
+        if mask != 2 or kv_len is None:
             raise ValueError("the relative bias runs with the key-length mask (mask=2, kv_len)")
         if rb.ndim != 2 or rb.shape[0] != H or rb.shape[1] % 2 != 1:
             raise ValueError(f"expected rel_bias [{H}, 2 * smax - 1], got {rb.shape}")
         smax = (rb.shape[1] + 1) // 2
-    N.check(N.load().b200_debug_attention(device, _ptr(q), B, S, W, H, mask, _ptr(kl), _ptr(rb), smax, _ptr(out)))
-    return out
+    d = _Staging(device)
+    q, kl = d.up(qkv, "bfloat16"), d.up(kv_len, "int32")
+    out = d.empty((B * S, W), "bfloat16")
+    N.check(N.load().b200_debug_attention(device, _dptr(q), B, S, W, H, mask, _dptr(kl), _ptr(rb), smax, _dptr(out),
+                                          d.stream))
+    return _host(out)
 
 
 def debug_attention_time(B: int, S: int, W: int, H: int, mask: int = 0, rel_bias: bool = False, iters: int = 20,
@@ -672,10 +717,16 @@ def debug_layernorm(x, gamma, beta, eps: float, rows: Optional[int] = None, in_s
         raise ValueError(f"x of {xa.size} floats does not hold {rows} rows of {w} at stride {stride}")
     if in_place and (outputs == "bf16" or stride != w):
         raise ValueError("in place needs the fp32 output and compact rows")
-    f = np.empty((rows, w), np.float32) if outputs != "bf16" else None
-    h = np.empty((rows, w), np.float32) if outputs != "f32" else None
-    N.check(N.load().b200_debug_layernorm(device, _ptr(xa), in_stride, _ptr(g), _ptr(b), eps, rows, w, int(in_place),
-                                          _ptr(f), _ptr(h)))
+    d = _Staging(device)
+    dx, dg, db = d.up(xa), d.up(g), d.up(b)
+    f = h = None
+    if outputs != "bf16":
+        f = dx[:rows * w].view(rows, w) if in_place else d.empty((rows, w))
+    if outputs != "f32":
+        h = d.empty((rows, w), "bfloat16")
+    N.check(N.load().b200_debug_layernorm(device, _dptr(dx), in_stride, _dptr(dg), _dptr(db), eps, rows, w, _dptr(f),
+                                          _dptr(h), d.stream))
+    f, h = (None if t is None else _host(t) for t in (f, h))
     return (f, h) if outputs == "both" else (f if h is None else h)
 
 
@@ -686,10 +737,12 @@ def debug_clip_text_embed(ids, tok, pos, device: int = 0):
     vocab, w = t.shape
     if p.shape != (S, w):
         raise ValueError(f"expected pos [{S}, {w}], got {p.shape}")
-    x = np.empty((n * S, w), np.float32)
-    eot = np.empty(n, np.int32)
-    N.check(N.load().b200_debug_clip_text_embed(device, _ptr(ia), _ptr(t), _ptr(p), n, S, w, vocab, _ptr(x), _ptr(eot)))
-    return x, eot
+    d = _Staging(device)
+    di, dt, dp = d.up(ia, "int32"), d.up(t), d.up(p)
+    x, eot = d.empty((n * S, w)), d.empty(n, "int32")
+    N.check(N.load().b200_debug_clip_text_embed(device, _dptr(di), _dptr(dt), _dptr(dp), n, S, w, vocab, _dptr(x),
+                                                _dptr(eot), d.stream))
+    return _host(x), _host(eot)
 
 
 def debug_embed_ln(ids, mask, word, pos, type0, gamma, beta, eps: float, pad: Optional[int] = None, device: int = 0):
@@ -708,18 +761,14 @@ def debug_embed_ln(ids, mask, word, pos, type0, gamma, beta, eps: float, pad: Op
         raise ValueError(f"expected pos [>= {need}, {w}], got {p.shape}")
     if (t is not None and t.size != w) or g.size != w or b.size != w:
         raise ValueError(f"type0, gamma and beta must have {w} values")
-    x = np.empty((n * S, w), np.float32)
-    h = np.empty((n * S, w), np.float32)
-    kv_len = np.empty(n, np.int32)
-    lib = N.load()
-    if pad is None:
-        st = lib.b200_debug_bert_embed_ln(device, _ptr(ia), _ptr(m), _ptr(wd), _ptr(p), p.shape[0], _ptr(t), _ptr(g),
-                                          _ptr(b), eps, n, S, w, vocab, _ptr(x), _ptr(h), _ptr(kv_len))
-    else:
-        st = lib.b200_debug_roberta_embed_ln(device, _ptr(ia), _ptr(m), _ptr(wd), _ptr(p), p.shape[0], _ptr(t), _ptr(g),
-                                             _ptr(b), eps, n, S, w, vocab, pad, _ptr(x), _ptr(h), _ptr(kv_len))
-    N.check(st)
-    return x, h, kv_len
+    d = _Staging(device)
+    di, dm, dwd, dp, dt = d.up(ia, "int32"), d.up(m, "int32"), d.up(wd), d.up(p), d.up(t)
+    dg, db = d.up(g), d.up(b)
+    x, h, kv_len = d.empty((n * S, w)), d.empty((n * S, w), "bfloat16"), d.empty(n, "int32")
+    N.check(N.load().b200_debug_embed_ln(device, _dptr(di), _dptr(dm), _dptr(dwd), _dptr(dp), p.shape[0], _dptr(dt),
+                                         _dptr(dg), _dptr(db), eps, n, S, w, vocab, -1 if pad is None else pad, _dptr(x),
+                                         _dptr(h), _dptr(kv_len), d.stream))
+    return _host(x), _host(h), _host(kv_len)
 
 
 def debug_clip_head(x, S: int, gamma, beta, eps: float, proj, row_in_seq=None, normalize: bool = True,
@@ -735,10 +784,12 @@ def debug_clip_head(x, S: int, gamma, beta, eps: float, proj, row_in_seq=None, n
     if r is not None and (r.shape != (n,) or r.min() < 0 or r.max() >= S):
         raise ValueError(f"row_in_seq must be [{n}] rows in [0, {S})")
     g, b = _as(gamma, np.float32), _as(beta, np.float32)
-    out = np.empty((n, E), np.float32)
-    N.check(N.load().b200_debug_clip_head(device, _ptr(xa), S, _ptr(r), _ptr(g), _ptr(b), eps, _ptr(pj), n, w, E,
-                                          int(normalize), _ptr(out)))
-    return out
+    d = _Staging(device)
+    dx, dr, dg, db, dp = d.up(xa), d.up(r, "int32"), d.up(g), d.up(b), d.up(pj)
+    out = d.empty((n, E))
+    N.check(N.load().b200_debug_clip_head(device, _dptr(dx), S, _dptr(dr), _dptr(dg), _dptr(db), eps, _dptr(dp), n, w,
+                                          E, int(normalize), _dptr(out), d.stream))
+    return _host(out)
 
 
 def debug_bert_head(x, S: int, kv_len, pool: int = N.POOL_MEAN, normalize: bool = True, device: int = 0) -> np.ndarray:
@@ -751,9 +802,12 @@ def debug_bert_head(x, S: int, kv_len, pool: int = N.POOL_MEAN, normalize: bool 
     kl = _as(kv_len, np.int32)
     if kl.shape != (n,):
         raise ValueError(f"expected kv_len [{n}], got {kl.shape}")
-    out = np.empty((n, w), np.float32)
-    N.check(N.load().b200_debug_bert_head(device, _ptr(xa), _ptr(kl), n, S, w, pool, int(normalize), _ptr(out)))
-    return out
+    d = _Staging(device)
+    dx, dkl = d.up(xa), d.up(kl, "int32")
+    out = d.empty((n, w))
+    N.check(N.load().b200_debug_bert_head(device, _dptr(dx), _dptr(dkl), n, S, w, pool, int(normalize), _dptr(out),
+                                          d.stream))
+    return _host(out)
 
 
 def debug_l2_rows(src, normalize: bool = True, device: int = 0) -> np.ndarray:
@@ -761,9 +815,11 @@ def debug_l2_rows(src, normalize: bool = True, device: int = 0) -> np.ndarray:
     a = _as(src, np.float32)
     if a.ndim != 2:
         raise ValueError(f"expected [n, E], got {a.shape}")
-    out = np.empty_like(a)
-    N.check(N.load().b200_debug_l2_rows(device, _ptr(a), a.shape[0], a.shape[1], int(normalize), _ptr(out)))
-    return out
+    d = _Staging(device)
+    da, out = d.up(a), d.empty(a.shape)
+    N.check(N.load().b200_debug_l2_rows(device, _dptr(da), a.shape[0], a.shape[1], int(normalize), _dptr(out),
+                                        d.stream))
+    return _host(out)
 
 
 def debug_stem_im2col(images, mean=(0.0, 0.0, 0.0), std=(1.0, 1.0, 1.0), device: int = 0) -> np.ndarray:
@@ -775,10 +831,12 @@ def debug_stem_im2col(images, mean=(0.0, 0.0, 0.0), std=(1.0, 1.0, 1.0), device:
     if a.shape != ((n, S, S, 3) if u8 else (n, 3, S, S)) or S % 2 != 0:
         raise ValueError(f"expected [n, S, S, 3] uint8 or [n, 3, S, S] fp32 with S even, got {a.shape}")
     m3, s3 = _as(mean, np.float32), _as(std, np.float32)
-    out = np.empty((n * (S // 2) ** 2, 64), np.float32)
-    N.check(N.load().b200_debug_stem_im2col(device, _ptr(a) if u8 else None, None if u8 else _ptr(a), n, S, _ptr(m3),
-                                            _ptr(s3), _ptr(out)))
-    return out
+    d = _Staging(device)
+    da = d.up(a, "uint8" if u8 else "float32")
+    out = d.empty((n * (S // 2) ** 2, 64), "bfloat16")
+    N.check(N.load().b200_debug_stem_im2col(device, _dptr(da) if u8 else None, None if u8 else _dptr(da), n, S,
+                                            _ptr(m3), _ptr(s3), _dptr(out), d.stream))
+    return _host(out)
 
 
 def debug_avgpool2(x, device: int = 0) -> np.ndarray:
@@ -787,9 +845,10 @@ def debug_avgpool2(x, device: int = 0) -> np.ndarray:
     n, H, W, Cc = a.shape
     if H % 2 or W % 2 or Cc % 8:
         raise ValueError(f"H, W must be even and C a multiple of 8, got {a.shape}")
-    out = np.empty((n, H // 2, W // 2, Cc), np.float32)
-    N.check(N.load().b200_debug_avgpool2(device, _ptr(a), n, H, W, Cc, _ptr(out)))
-    return out
+    d = _Staging(device)
+    da, out = d.up(a, "bfloat16"), d.empty((n, H // 2, W // 2, Cc), "bfloat16")
+    N.check(N.load().b200_debug_avgpool2(device, _dptr(da), n, H, W, Cc, _dptr(out), d.stream))
+    return _host(out)
 
 
 def debug_attnpool_tokens(x, pos, device: int = 0) -> np.ndarray:
@@ -799,9 +858,10 @@ def debug_attnpool_tokens(x, pos, device: int = 0) -> np.ndarray:
     n, HW, Cc = a.shape
     if p.shape != (HW + 1, Cc) or Cc % 8:
         raise ValueError(f"expected pos [{HW + 1}, {Cc}] and C a multiple of 8, got {p.shape}")
-    out = np.empty((n, HW + 1, Cc), np.float32)
-    N.check(N.load().b200_debug_attnpool_tokens(device, _ptr(a), _ptr(p), n, HW, Cc, _ptr(out)))
-    return out
+    d = _Staging(device)
+    da, dp, out = d.up(a, "bfloat16"), d.up(p), d.empty((n, HW + 1, Cc), "bfloat16")
+    N.check(N.load().b200_debug_attnpool_tokens(device, _dptr(da), _dptr(dp), n, HW, Cc, _dptr(out), d.stream))
+    return _host(out)
 
 
 def debug_im2col_f32(chw, patch: int, kpad: int, cls: int, device: int = 0) -> np.ndarray:
@@ -811,24 +871,28 @@ def debug_im2col_f32(chw, patch: int, kpad: int, cls: int, device: int = 0) -> n
     n, c, S, S2 = a.shape
     if c != 3 or S != S2 or S % patch or kpad % 8 or kpad < 3 * patch * patch or cls not in (0, 1):
         raise ValueError(f"bad im2col shape {a.shape}, patch {patch}, kpad {kpad}, cls {cls}")
-    out = np.empty((n * ((S // patch) ** 2 + cls), kpad), np.float32)
-    N.check(N.load().b200_debug_im2col_f32(device, _ptr(a), n, S, patch, kpad, cls, _ptr(out)))
-    return out
+    d = _Staging(device)
+    da, out = d.up(a), d.empty((n * ((S // patch) ** 2 + cls), kpad), "bfloat16")
+    N.check(N.load().b200_debug_im2col_f32(device, _dptr(da), n, S, patch, kpad, cls, _dptr(out), d.stream))
+    return _host(out)
 
 
 def debug_resize(hwc, S: int, device: int = 0) -> np.ndarray:
     a = _as(hwc, np.uint8)
-    out = np.empty((a.shape[0], S, S, 3), np.uint8)
-    N.check(N.load().b200_debug_resize(device, _ptr(a), a.shape[0], a.shape[1], a.shape[2], S, _ptr(out)))
-    return out
+    d = _Staging(device)
+    da, out = d.up(a, "uint8"), d.empty((a.shape[0], S, S, 3), "uint8")
+    N.check(N.load().b200_debug_resize(device, _dptr(da), a.shape[0], a.shape[1], a.shape[2], S, _dptr(out), d.stream))
+    return _host(out)
 
 
 def debug_resize_squash(hwc, S: int, device: int = 0) -> np.ndarray:
     """uint8 [n, h, w, 3] -> [n, S, S, 3] as PIL resize((S, S), BICUBIC) does (SigLIP's squash resize)."""
     a = _as(hwc, np.uint8)
-    out = np.empty((a.shape[0], S, S, 3), np.uint8)
-    N.check(N.load().b200_debug_resize_squash(device, _ptr(a), a.shape[0], a.shape[1], a.shape[2], S, _ptr(out)))
-    return out
+    d = _Staging(device)
+    da, out = d.up(a, "uint8"), d.empty((a.shape[0], S, S, 3), "uint8")
+    N.check(N.load().b200_debug_resize_squash(device, _dptr(da), a.shape[0], a.shape[1], a.shape[2], S, _dptr(out),
+                                              d.stream))
+    return _host(out)
 
 
 def debug_map_attention(q, kv, B: int, S: int, H: int, device: int = 0) -> np.ndarray:
@@ -841,10 +905,11 @@ def debug_map_attention(q, kv, B: int, S: int, H: int, device: int = 0) -> np.nd
         raise ValueError(f"expected q [{W}] or [{B}, {W}], got {qa.shape}")
     if kva.shape != (B * S, 2 * W):
         raise ValueError(f"expected kv [{B * S}, {2 * W}], got {kva.shape}")
-    out = np.empty((B, W), np.float32)
-    fn = N.load().b200_debug_map_attention if qa.ndim == 1 else N.load().b200_debug_map_attention_per_image
-    N.check(fn(device, _ptr(qa), _ptr(kva), B, S, W, H, _ptr(out)))
-    return out
+    d = _Staging(device)
+    dq, dkv, out = d.up(qa), d.up(kva, "bfloat16"), d.empty((B, W), "bfloat16")
+    N.check(N.load().b200_debug_map_attention(device, _dptr(dq), 0 if qa.ndim == 1 else W, _dptr(dkv), B, S, W, H,
+                                              _dptr(out), d.stream))
+    return _host(out)
 
 
 def debug_conv2d(x, w, bias=None, residual=None, relu: bool = True, device: int = 0) -> np.ndarray:
@@ -858,11 +923,14 @@ def debug_conv2d(x, w, bias=None, residual=None, relu: bool = True, device: int 
     if wa.shape != (cout, cin, k, k):
         raise ValueError(f"expected w [cout, {cin}, k, k], got {wa.shape}")
     Ho, Wo = (H // 2, W // 2) if cin == 3 else (H, W)
-    b = None if bias is None else _as(bias, np.float32)
     r = None if residual is None else _as(residual, np.float32)
     if r is not None and r.shape != (n, Ho, Wo, cout):
         raise ValueError(f"expected residual [{n}, {Ho}, {Wo}, {cout}], got {r.shape}")
-    out = np.empty((n, Ho, Wo, cout), np.float32)
-    N.check(N.load().b200_debug_conv2d(device, _ptr(xa), n, H, W, cin, _ptr(wa), cout, k, _ptr(b), _ptr(r), int(relu),
-                                       _ptr(out)))
-    return out
+    d = _Staging(device)
+    # the stem reads fp32 CHW, as the fp32 image entry point receives it; the other convs a bf16 NHWC activation
+    dx = d.up(xa).permute(0, 3, 1, 2).contiguous() if cin == 3 else d.up(xa, "bfloat16")
+    db = d.up(np.zeros(cout) if bias is None else bias)
+    dr, out = d.up(r, "bfloat16"), d.empty((n, Ho, Wo, cout), "bfloat16")
+    N.check(N.load().b200_debug_conv2d(device, _dptr(dx), n, H, W, cin, _ptr(wa), cout, k, _dptr(db), _dptr(dr),
+                                       int(relu), _dptr(out), d.stream))
+    return _host(out)

@@ -1,7 +1,7 @@
 """The GEMM at the shapes and edges where its two kernels go wrong, each case pinned to the kernel it runs.
 
 The library runs the persistent 128 x 256 kernel for K >= 1024, N % 256 == 0 and at least one 128 x 256 tile per SM,
-and the 128 x 128 kernel otherwise (gemm.cu launch()).  b200_debug_gemm_into reports which one ran and takes the SM
+and the 128 x 128 kernel otherwise (gemm.cu launch()).  b200_debug_gemm reports which one ran and takes the SM
 count the rule is applied with, so a small count sends small shapes to the persistent kernel with each CTA walking
 many tiles, and a huge one sends any shape to the 128 x 128 kernel: no case runs a kernel where the rule would not.
 
