@@ -240,7 +240,8 @@ enum b200_arch {
     B200_ARCH_MPNET = 2, /* HF MPNetModel + pooling: BERT layers with a relative-position bias in the attention logits */
     B200_ARCH_SIGLIP = 3, /* open_clip SigLIP: class-token-free ViT with a MAP pooling head + bidirectional text tower */
     B200_ARCH_XLMR = 4,   /* HF XLMRobertaModel + pooling: BERT layers, RoBERTa position ids, one token-type row */
-    B200_ARCH_CLIP_RESNET = 5 /* OpenAI ResNet CLIP (open_clip ModifiedResNet image tower + the CLIP text tower) */
+    B200_ARCH_CLIP_RESNET = 5, /* OpenAI ResNet CLIP (open_clip ModifiedResNet image tower + the CLIP text tower) */
+    B200_ARCH_CLIP_CONVNEXT = 6 /* ConvNeXt CLIP (open_clip TimmModel over a timm ConvNeXt trunk + the CLIP text tower) */
 };
 enum b200_act { B200_ACT_GELU = 0, B200_ACT_QUICKGELU = 1 };
 enum b200_pool { B200_POOL_MEAN = 0, B200_POOL_CLS = 1 };
@@ -288,6 +289,20 @@ typedef struct b200_model_desc {
     int32_t resnet_width;       /* 64 (a power of two >= 64) */
     int32_t resnet_heads;       /* attention-pool heads: width * 32 / 64 (head_dim 64) */
     int32_t resnet_image_size;  /* 224 (a multiple of 32) */
+    /* CLIP ConvNeXt only (open_clip TimmModel over timm's ConvNeXt, verify): the image tower; `vision` is unused.
+     * Every LayerNorm is over the channels of one pixel, with eps layer_norm_eps (1e-6; 1e-5 for convnext_xxlarge).
+     *   stem: Conv2d(3, dims[0], 4, stride 4, bias), LayerNorm;
+     *   stage s = 0..3: for s > 0 LayerNorm, Conv2d(dims[s-1], dims[s], 2, stride 2, bias); then depths[s] blocks
+     *         x += gamma * fc2(GELU(fc1(LayerNorm(dwconv(x))))), dwconv the 7 x 7 depthwise conv (padding 3, bias),
+     *         fc1 dims[s] -> 4 dims[s] and fc2 back, both with bias, GELU the erf one;
+     *   head: mean over the pixels, LayerNorm, then convnext_head 0: a Linear without bias to embed_dim, or 1: an MLP
+     *         (fc1 with bias to 2 embed_dim, GELU, fc2 without bias to embed_dim).
+     * Shapes the kernels cover: dims multiples of 64 up to 3072, convnext_image_size a multiple of 32 up to 640, and
+     * embed_dim a multiple of 32; b200_model_create refuses others with B200_ERR_INVALID_ARG. */
+    int32_t convnext_dims[4];     /* channels per stage: base {128, 256, 512, 1024}, large {192, ...}, xxlarge {384, ...} */
+    int32_t convnext_depths[4];   /* blocks per stage: {3, 3, 27, 3}, xxlarge {3, 4, 30, 3} */
+    int32_t convnext_image_size;  /* 224, 256 or 320 */
+    int32_t convnext_head;        /* 0: linear projection, 1: MLP */
 } b200_model_desc;
 
 int b200_model_create(int device, const b200_model_desc* desc, b200_model** out);
@@ -306,6 +321,12 @@ int b200_model_destroy(b200_model* m);
  * visual.attnpool.positional_embedding [(S/32)^2 + 1, 32 width], visual.attnpool.{q,k,v,c}_proj.{weight,bias}; the text
  * tower under the CLIP names.  BatchNorm is folded into the convolutions by b200_model_finalize (num_batches_tracked is
  * not needed). */
+/* CLIP ConvNeXt: open_clip TimmModel names (verify): visual.trunk.stem.0.{weight [C0, 3, 4, 4], bias} (the conv),
+ * visual.trunk.stem.1.{weight,bias} (its LayerNorm), for s > 0 visual.trunk.stages.{s}.downsample.0.{weight,bias} (the
+ * LayerNorm) and .downsample.1.{weight [Cs, Cs-1, 2, 2], bias}, per block visual.trunk.stages.{s}.blocks.{i}.conv_dw.{weight
+ * [C, 1, 7, 7], bias}, .norm.*, .mlp.fc1.*, .mlp.fc2.* and .gamma [C], visual.trunk.head.norm.{weight,bias}, then
+ * visual.head.proj.weight [E, C3] (linear head) or visual.head.mlp.{fc1.weight [2E, C3], fc1.bias, fc2.weight [E, 2E]}
+ * (MLP head); the text tower under the CLIP names.  b200_model_finalize folds gamma into fc2's rows and bias. */
 /* XLM-R: HF XLMRobertaModel names, as BERT's: embeddings.word_embeddings.weight [vocab, W],
  * embeddings.position_embeddings.weight [ctx + pad_id + 1, W], embeddings.token_type_embeddings.weight [1, W],
  * embeddings.LayerNorm.*, encoder.layer.{i}.* (a "roberta." prefix is dropped). */
@@ -552,6 +573,20 @@ int b200_debug_map_attention(int device, const float* q, int q_stride, const voi
  * relu == 0 (1 x 1 and stem convs only) takes no residual. */
 int b200_debug_conv2d(int device, const void* x, int n, int H, int W, int cin, const float* w, int cout, int k,
                       const float* bias, const void* residual, int relu, void* out, void* stream);
+/* ConvNeXt block head: x fp32 NHWC [n, H, W, C] -> out bf16 [n*H*W, C] = LayerNorm over C (gamma, beta, eps) of the
+ * 7 x 7 depthwise conv with zero padding 3 plus bias; w fp32 [49, C], tap 7 dy + dx major (conv_dw.weight [C, 1, 7, 7]
+ * transposed).  C a multiple of 64, <= 3072. */
+int b200_debug_dwconv7_ln(int device, const float* x, int n, int H, int W, int C, const float* w, const float* bias,
+                          const float* gamma, const float* beta, float eps, void* out, void* stream);
+/* ConvNeXt per-pixel LayerNorm of x fp32 NHWC [n, H, W, C].  patchify 0: out fp32 [n*H*W, C] (may be x), the stem's
+ * norm; patchify 1 (H, W even): out bf16 [n*(H/2)*(W/2), 4C], the downsample conv's GEMM rows, pixel (y, x) at column
+ * ((y % 2) * 2 + x % 2) * C + c of row (y/2, x/2).  C a multiple of 64, <= 3072. */
+int b200_debug_ln_pixels(int device, const float* x, int n, int H, int W, int C, const float* gamma, const float* beta,
+                         float eps, int patchify, void* out, void* stream);
+/* ConvNeXt head input: mean over the HW pixel rows of each image of x fp32 [n, HW, C], then LayerNorm -> out bf16
+ * [n, C].  C a multiple of 64, <= 3072. */
+int b200_debug_pool_ln(int device, const float* x, int n, int HW, int C, const float* gamma, const float* beta, float eps,
+                       void* out, void* stream);
 /* Bytes of device memory the library holds right now, over all devices and handles of this process (indexes,
  * exchanges, models and the scratch of calls in flight).  Memory from b200_host_alloc is not counted.  Returns to its
  * earlier value once every handle created in between is destroyed: a leak check. */

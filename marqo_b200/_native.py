@@ -14,7 +14,7 @@ _lock = threading.Lock()
 OK, ERR_INVALID_ARG, ERR_NO_DEVICE, ERR_CUDA, ERR_OOM, ERR_UNSUPPORTED, ERR_INTERNAL, ERR_MISSING_WEIGHT = range(8)
 
 METRIC_PRENORMALIZED_ANGULAR, METRIC_ANGULAR, METRIC_DOTPRODUCT, METRIC_EUCLIDEAN = range(4)
-ARCH_CLIP, ARCH_BERT, ARCH_MPNET, ARCH_SIGLIP, ARCH_XLMR, ARCH_CLIP_RESNET = 0, 1, 2, 3, 4, 5
+ARCH_CLIP, ARCH_BERT, ARCH_MPNET, ARCH_SIGLIP, ARCH_XLMR, ARCH_CLIP_RESNET, ARCH_CLIP_CONVNEXT = 0, 1, 2, 3, 4, 5, 6
 ACT_GELU, ACT_QUICKGELU = 0, 1
 POOL_MEAN, POOL_CLS = 0, 1
 GEMM_128x128, GEMM_PERSISTENT = 0, 1   # the GEMM kernel b200_debug_gemm reports
@@ -49,6 +49,8 @@ class ModelDesc(C.Structure):
         ("layer_norm_eps", C.c_float), ("pad_id", C.c_int32), ("rel_buckets", C.c_int32), ("rel_max_distance", C.c_int32),
         ("resnet_layers", C.c_int32 * 4), ("resnet_width", C.c_int32), ("resnet_heads", C.c_int32),
         ("resnet_image_size", C.c_int32),
+        ("convnext_dims", C.c_int32 * 4), ("convnext_depths", C.c_int32 * 4), ("convnext_image_size", C.c_int32),
+        ("convnext_head", C.c_int32),
     ]
 
 
@@ -141,6 +143,11 @@ _SIGNATURES = {
     "b200_debug_map_attention": (C.c_int, [C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_conv2d": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, C.c_int,
                                     _P, _P]),
+    "b200_debug_dwconv7_ln": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, C.c_float, _P,
+                                        _P]),
+    "b200_debug_ln_pixels": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_float, C.c_int, _P,
+                                       _P]),
+    "b200_debug_pool_ln": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_float, _P, _P]),
     "b200_debug_device_bytes": (C.c_int, [C.POINTER(C.c_int64)]),
     "b200_jpeg_info": (C.c_int, [_P, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200_jpeg_decode_batch": (C.c_int, [C.c_int, _P, _P, C.c_int, _P, _P, _P, _P]),

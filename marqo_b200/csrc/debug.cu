@@ -456,4 +456,45 @@ int b200_debug_conv2d(int device, const void* x, int n, int H, int W, int cin, c
     });
 }
 
+int b200_debug_dwconv7_ln(int device, const float* x, int n, int H, int W, int C, const float* w, const float* bias,
+                          const float* gamma, const float* beta, float eps, void* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && w && bias && gamma && beta && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && H > 0 && W > 0 && C > 0, "n, H, W, C must be positive");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::dwconv7_ln(x, n, H, W, C, w, bias, gamma, beta, eps, static_cast<bf16*>(out), s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_ln_pixels(int device, const float* x, int n, int H, int W, int C, const float* gamma, const float* beta,
+                         float eps, int patchify, void* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && gamma && beta && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && H > 0 && W > 0 && C > 0, "n, H, W, C must be positive");
+        MB_CHECK_ARG(!patchify || (H % 2 == 0 && W % 2 == 0), "patchify needs an even H and W");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::ln_pixels(x, n, H, W, C, gamma, beta, eps, patchify ? nullptr : static_cast<float*>(out),
+                           patchify ? static_cast<bf16*>(out) : nullptr, s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_pool_ln(int device, const float* x, int n, int HW, int C, const float* gamma, const float* beta, float eps,
+                       void* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && gamma && beta && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && HW > 0 && C > 0, "n, HW, C must be positive");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::pool_ln(x, n, HW, C, gamma, beta, eps, static_cast<bf16*>(out), s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
 }  // extern "C"

@@ -906,5 +906,228 @@ int l2_rows(const float* src, int n, int E, int normalize, float* out, cudaStrea
     return 1;
 }
 
+// ------------------------------------------------------------------------------------------------ ConvNeXt
+// The image tower's memory-bound kernels over fp32 NHWC pixel rows x [pixels, C] (C % 64 == 0, C <= 3072).  A CTA has
+// one thread per 4 channels (rounded up to whole warps) and holds P pixels of them in registers; pixel_ln normalises
+// each pixel over its C channels (fp32 statistics, mean then variance, as layernorm_kernel does).
+constexpr int PX_MAX_C = 3072;
+
+static int px_threads(int C) { return (C / 4 + 31) / 32 * 32; }
+
+// v[p] (this thread's 4 channels of pixel p; zeros when !active) -> LayerNorm(pixel p) * gamma + beta.  red: shared
+// scratch of 32 * P floats.  Every thread of the CTA must call it.
+template <int P>
+__device__ __forceinline__ void pixel_ln(float4 (&v)[P], bool active, int C, const float* __restrict__ gamma,
+                                         const float* __restrict__ beta, float eps, float* red) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+    float mean[P], rstd[P];
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+        const float s = warp_sum(v[p].x + v[p].y + v[p].z + v[p].w);
+        if (lane == 0) red[warp * P + p] = s;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+        float s = 0.f;
+        for (int i = 0; i < nwarps; ++i) s += red[i * P + p];
+        mean[p] = s / (float)C;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+        const float a = v[p].x - mean[p], b = v[p].y - mean[p], c = v[p].z - mean[p], d = v[p].w - mean[p];
+        const float q = warp_sum(active ? a * a + b * b + c * c + d * d : 0.f);
+        if (lane == 0) red[warp * P + p] = q;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+        float q = 0.f;
+        for (int i = 0; i < nwarps; ++i) q += red[i * P + p];
+        rstd[p] = 1.0f / sqrtf(q / (float)C + eps);
+    }
+    if (!active) return;
+    const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + threadIdx.x);
+    const float4 b = __ldg(reinterpret_cast<const float4*>(beta) + threadIdx.x);
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+        v[p].x = (v[p].x - mean[p]) * rstd[p] * g.x + b.x;
+        v[p].y = (v[p].y - mean[p]) * rstd[p] * g.y + b.y;
+        v[p].z = (v[p].z - mean[p]) * rstd[p] * g.z + b.z;
+        v[p].w = (v[p].w - mean[p]) * rstd[p] * g.w + b.w;
+    }
+}
+
+__device__ __forceinline__ uint2 pack_bf16x4(const float4& y) {
+    return make_uint2(pack_bf16x2(y.x, y.y), pack_bf16x2(y.z, y.w));
+}
+
+__device__ __forceinline__ void fma4(float4& acc, const float4& w, const float4& x) {
+    acc.x = fmaf(w.x, x.x, acc.x);
+    acc.y = fmaf(w.y, x.y, acc.y);
+    acc.z = fmaf(w.z, x.z, acc.z);
+    acc.w = fmaf(w.w, x.w, acc.w);
+}
+
+// 7 x 7 depthwise conv (zero padding 3) + bias, then LayerNorm over C, of P consecutive pixels of one image row:
+// x fp32 [n, H, W, C], w fp32 [49, C] (tap-major), out bf16 [n * H * W, C].  Along a row the 7 taps slide over the
+// P + 6 input pixels in registers, so each input row is loaded once per output row (the other six output rows that
+// read it find it in L1 / L2); the conv result never leaves registers.
+template <int P>
+__global__ void __launch_bounds__(P == 8 ? 256 : 768, P == 8 ? 2 : 1) dwconv7_ln_kernel(
+    const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
+    const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int H, int W, int C, int xtiles,
+    __nv_bfloat16* __restrict__ out) {
+    __shared__ float red[32 * P];
+    const int xt = blockIdx.x % xtiles;
+    const long long row = blockIdx.x / xtiles;   // b * H + y
+    const int y = (int)(row % H), x0 = xt * P, C4 = C / 4, c4 = threadIdx.x;
+    const bool active = c4 < C4;
+    const long long img = row - y;               // b * H
+    float4 acc[P];
+    const float4 b4 = active ? __ldg(reinterpret_cast<const float4*>(bias) + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int p = 0; p < P; ++p) acc[p] = b4;
+    if (active) {
+        const float4* w4 = reinterpret_cast<const float4*>(w) + c4;
+        for (int dy = 0; dy < 7; ++dy) {
+            const int yy = y + dy - 3;
+            if (yy < 0 || yy >= H) continue;
+            const float4* src = reinterpret_cast<const float4*>(x) + (img + yy) * W * C4 + c4;
+            float4 wt[7];
+#pragma unroll
+            for (int dx = 0; dx < 7; ++dx) wt[dx] = __ldg(w4 + (dy * 7 + dx) * C4);
+#pragma unroll
+            for (int j = 0; j < P + 6; ++j) {
+                const int xx = x0 + j - 3;
+                const float4 in = xx >= 0 && xx < W ? __ldg(src + (long long)xx * C4) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+                for (int p = 0; p < P; ++p)
+                    if (j - p >= 0 && j - p < 7) fma4(acc[p], wt[j - p], in);
+            }
+        }
+    }
+    // (pixels past the row end take part in the reductions but are not written)
+    pixel_ln<P>(acc, active, C, gamma, beta, eps, red);
+    if (!active) return;
+    uint2* o = reinterpret_cast<uint2*>(out) + (row * W + x0) * C4 + c4;
+#pragma unroll
+    for (int p = 0; p < P; ++p)
+        if (x0 + p < W) o[(long long)p * C4] = pack_bf16x4(acc[p]);
+}
+
+static void check_px_width(int C) {
+    if (C <= 0 || C % 64 != 0 || C > PX_MAX_C)
+        fail(B200_ERR_UNSUPPORTED, "ConvNeXt: %d channels (a multiple of 64, <= %d, is needed)", C, PX_MAX_C);
+}
+
+int dwconv7_ln(const float* x, int n, int H, int W, int C, const float* w49, const float* bias, const float* gamma,
+               const float* beta, float eps, __nv_bfloat16* out, cudaStream_t s) {
+    if (n <= 0) return 0;
+    check_px_width(C);
+    // 8 pixels per thread up to 1024 channels (256 threads); 4 above, to stay within 80 registers at 768 threads
+    if (C <= 1024) {
+        const int xtiles = (W + 7) / 8;
+        dwconv7_ln_kernel<8><<<(unsigned)((long long)n * H * xtiles), px_threads(C), 0, s>>>(x, w49, bias, gamma, beta,
+                                                                                             eps, H, W, C, xtiles, out);
+    } else {
+        const int xtiles = (W + 3) / 4;
+        dwconv7_ln_kernel<4><<<(unsigned)((long long)n * H * xtiles), px_threads(C), 0, s>>>(x, w49, bias, gamma, beta,
+                                                                                             eps, H, W, C, xtiles, out);
+    }
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+// LayerNorm over C of LNP_P consecutive pixels of x fp32 [n, H, W, C] per CTA.  PATCHIFY: bf16 into the 2 x 2 stride-2
+// downsample's GEMM rows, pixel (b, y, x) -> row (b, y/2, x/2), columns ((y % 2) * 2 + x % 2) * C + c; otherwise fp32
+// back to the same pixel row (out may be x).
+constexpr int LNP_P = 4;
+
+template <bool PATCHIFY>
+__global__ void __launch_bounds__(768) ln_pixels_kernel(const float* x, long long pixels, int H, int W, int C,
+                                                        const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                        float eps, void* out) {
+    __shared__ float red[32 * LNP_P];
+    const int C4 = C / 4, c4 = threadIdx.x;
+    const bool active = c4 < C4;
+    const long long p0 = (long long)blockIdx.x * LNP_P;
+    float4 v[LNP_P];
+#pragma unroll
+    for (int p = 0; p < LNP_P; ++p)
+        v[p] = active && p0 + p < pixels ? reinterpret_cast<const float4*>(x)[(p0 + p) * C4 + c4]
+                                         : make_float4(0.f, 0.f, 0.f, 0.f);
+    pixel_ln<LNP_P>(v, active, C, gamma, beta, eps, red);
+    if (!active) return;
+#pragma unroll
+    for (int p = 0; p < LNP_P; ++p) {
+        const long long r = p0 + p;
+        if (r >= pixels) break;
+        if (PATCHIFY) {
+            const int xx = (int)(r % W);
+            const long long by = r / W;
+            const int yy = (int)(by % H);
+            const long long b = by / H;
+            const long long orow = (b * (H / 2) + yy / 2) * (W / 2) + xx / 2;
+            const int q = (yy & 1) * 2 + (xx & 1);
+            reinterpret_cast<uint2*>(out)[orow * C + (long long)q * C4 + c4] = pack_bf16x4(v[p]);
+        } else {
+            reinterpret_cast<float4*>(out)[r * C4 + c4] = v[p];
+        }
+    }
+}
+
+int ln_pixels(const float* x, int n, int H, int W, int C, const float* gamma, const float* beta, float eps,
+              float* out_f32, __nv_bfloat16* out_patch, cudaStream_t s) {
+    if (n <= 0) return 0;
+    check_px_width(C);
+    if ((out_f32 != nullptr) == (out_patch != nullptr)) fail(B200_ERR_INTERNAL, "ln_pixels: exactly one output");
+    if (out_patch && (H % 2 != 0 || W % 2 != 0)) fail(B200_ERR_INTERNAL, "ln_pixels: %d x %d is not even", H, W);
+    const long long pixels = (long long)n * H * W;
+    const unsigned grid = (unsigned)((pixels + LNP_P - 1) / LNP_P);
+    if (out_patch)
+        ln_pixels_kernel<true><<<grid, px_threads(C), 0, s>>>(x, pixels, H, W, C, gamma, beta, eps, out_patch);
+    else
+        ln_pixels_kernel<false><<<grid, px_threads(C), 0, s>>>(x, pixels, H, W, C, gamma, beta, eps, out_f32);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+// Global average pool of each image's HW pixel rows of x fp32 [n, HW, C], then LayerNorm over C -> bf16 [n, C] (the
+// head GEMM's A operand): one CTA per image.
+__global__ void __launch_bounds__(768) pool_ln_kernel(const float* __restrict__ x, int HW, int C,
+                                                      const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                      float eps, __nv_bfloat16* __restrict__ out) {
+    __shared__ float red[32];
+    const int C4 = C / 4, c4 = threadIdx.x;
+    const bool active = c4 < C4;
+    float4 v[1] = {make_float4(0.f, 0.f, 0.f, 0.f)};
+    if (active) {
+        const float4* src = reinterpret_cast<const float4*>(x) + (long long)blockIdx.x * HW * C4 + c4;
+        for (int i = 0; i < HW; ++i) {
+            const float4 a = __ldg(src + (long long)i * C4);
+            v[0].x += a.x;
+            v[0].y += a.y;
+            v[0].z += a.z;
+            v[0].w += a.w;
+        }
+        const float inv = 1.0f / (float)HW;
+        v[0] = make_float4(v[0].x * inv, v[0].y * inv, v[0].z * inv, v[0].w * inv);
+    }
+    pixel_ln<1>(v, active, C, gamma, beta, eps, red);
+    if (active) reinterpret_cast<uint2*>(out)[(long long)blockIdx.x * C4 + c4] = pack_bf16x4(v[0]);
+}
+
+int pool_ln(const float* x, int n, int HW, int C, const float* gamma, const float* beta, float eps, __nv_bfloat16* out,
+            cudaStream_t s) {
+    if (n <= 0) return 0;
+    check_px_width(C);
+    if (HW <= 0) fail(B200_ERR_INTERNAL, "pool_ln: %d pixels", HW);
+    pool_ln_kernel<<<n, px_threads(C), 0, s>>>(x, HW, C, gamma, beta, eps, out);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
 }  // namespace kernels
 }  // namespace mb

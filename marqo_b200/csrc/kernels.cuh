@@ -84,5 +84,19 @@ int attnpool_tokens(const __nv_bfloat16* x, const float* pos, int n, int HW, int
 // out[b] = src[b] / |src[b]| if normalize (no epsilon: abstract_clip_model.py:83-85), else src[b]; rows of E floats.
 int l2_rows(const float* src, int n, int E, int normalize, float* out, cudaStream_t s);
 
+// ConvNeXt image tower, over fp32 NHWC x [n, H, W, C] with C a multiple of 64, <= 3072; every LayerNorm is over the C
+// channels of one pixel.
+// Block head: 7 x 7 depthwise conv (zero padding 3) with bias, w49 fp32 [49, C] (tap 7 dy + dx major), then LayerNorm
+// -> bf16 out [n * H * W, C], the fc1 GEMM's A operand.
+int dwconv7_ln(const float* x, int n, int H, int W, int C, const float* w49, const float* bias, const float* gamma,
+               const float* beta, float eps, __nv_bfloat16* out, cudaStream_t s);
+// LayerNorm of every pixel, to exactly one of: out_f32 fp32 [n * H * W, C] (may be x: the stem's norm), or out_patch
+// bf16 [n * (H/2) * (W/2), 4C], the 2 x 2 stride-2 downsample conv's GEMM rows, column ((y % 2) * 2 + x % 2) * C + c.
+int ln_pixels(const float* x, int n, int H, int W, int C, const float* gamma, const float* beta, float eps,
+              float* out_f32, __nv_bfloat16* out_patch, cudaStream_t s);
+// Mean over each image's HW pixels of x fp32 [n, HW, C], then LayerNorm -> bf16 out [n, C].
+int pool_ln(const float* x, int n, int HW, int C, const float* gamma, const float* beta, float eps, __nv_bfloat16* out,
+            cudaStream_t s);
+
 }  // namespace kernels
 }  // namespace mb

@@ -1,4 +1,5 @@
-// Encoder runtime: CLIP ViT image tower, CLIP text tower, SigLIP towers, OpenAI ResNet CLIP image tower, BERT (e5,
+// Encoder runtime: CLIP ViT image tower, CLIP text tower, SigLIP towers, OpenAI ResNet CLIP and ConvNeXt CLIP image
+// towers, BERT (e5,
 // MiniLM, bge), MPNet, XLM-R (multilingual-e5) — SURVEY §8 a2-a5.
 //
 // What the reference calls (third-party, restated in oracle/encoders.py):
@@ -50,7 +51,7 @@ struct MapW {
 
 // What runs a tower, resolved once from the model's arch (resolve_kinds).  Archs whose forward passes differ only in
 // data share a kind: MPNet and XLM-R are ROBERTA, and the ResNet CLIP's text tower is CLIP's.
-enum class VisionKind { NONE, CLIP_VIT, SIGLIP_VIT, RESNET };
+enum class VisionKind { NONE, CLIP_VIT, SIGLIP_VIT, RESNET, CONVNEXT };
 enum class TextKind { NONE, CLIP, SIGLIP, BERT, ROBERTA };
 struct Kinds {
     VisionKind vision = VisionKind::NONE;
@@ -112,6 +113,38 @@ struct ResnetW {
     DeviceBuffer<__nv_bfloat16> buf[4];
 };
 
+// ConvNeXt CLIP image tower (open_clip TimmModel over timm's ConvNeXt, verify).  Its stem conv is the ViT patch
+// embedding at patch 4 without class rows (TowerW conv_w / conv_wg of m->vision).  A block is the MLP half of a pre-LN
+// transformer layer behind a depthwise conv: dwconv7_ln -> h, fc1 (+ GELU) -> u, fc2 with gamma folded into its rows
+// and bias, added onto the fp32 residual stream x in place.
+struct ConvnextBlockW {
+    const float *dw_w = nullptr, *dw_b = nullptr;   // fp32 [49, C] (tap-major), [C]
+    const float *ln_w = nullptr, *ln_b = nullptr, *b1 = nullptr, *b2 = nullptr;
+    const __nv_bfloat16 *w1 = nullptr, *w2 = nullptr;   // [4C, C], gamma-scaled [C, 4C]
+};
+
+struct ConvnextStageW {
+    int C = 0;
+    // downsample (stages > 0): LayerNorm, then the 2 x 2 stride-2 conv as a GEMM over ln_pixels' patch rows
+    const float *ds_ln_w = nullptr, *ds_ln_b = nullptr, *ds_b = nullptr;
+    const __nv_bfloat16* ds_w = nullptr;   // [C, 4 C_prev], column (dy * 2 + dx) * C_prev + c
+    std::vector<ConvnextBlockW> blocks;
+};
+
+// The activations live in x / h / u of max_images images at the first stage, the largest (every later stage has a
+// quarter of the pixels and twice the channels); fixed pointers, so captured CUDA graphs replay them.
+struct ConvnextW {
+    ConvnextStageW stages[4];
+    const float *stem_b = nullptr, *stem_ln_w = nullptr, *stem_ln_b = nullptr;
+    const float *head_ln_w = nullptr, *head_ln_b = nullptr;
+    const __nv_bfloat16* w_proj = nullptr;                              // linear head [E, C3]
+    const __nv_bfloat16 *w_fc1 = nullptr, *w_fc2 = nullptr;             // MLP head [2E, C3], [E, 2E]
+    const float* b_fc1 = nullptr;
+    int max_images = 0;
+    DeviceBuffer<float> x;                 // [pixels, C]
+    DeviceBuffer<__nv_bfloat16> h, u;      // [pixels, C], [pixels, 4C]
+};
+
 }  // namespace
 
 struct b200_model {
@@ -124,6 +157,7 @@ struct b200_model {
     Kinds kind;
     TowerW vision, text;
     ResnetW resnet;   // VisionKind::RESNET's image tower (vision.tokens = grid^2 + 1)
+    ConvnextW convnext;   // VisionKind::CONVNEXT's image tower (vision.tokens = the stem's (S/4)^2 pixels)
     // workspaces (sized for max_tokens tokens)
     long long max_tokens = 0;
     DeviceBuffer<float> x;
@@ -191,6 +225,10 @@ Kinds resolve_kinds(const b200_model_desc& d) {
         if (d.resnet_layers[0] > 0) k.vision = VisionKind::RESNET;
         if (text) k.text = TextKind::CLIP;
         break;
+    case B200_ARCH_CLIP_CONVNEXT:
+        if (d.convnext_depths[0] > 0) k.vision = VisionKind::CONVNEXT;
+        if (text) k.text = TextKind::CLIP;
+        break;
     case B200_ARCH_SIGLIP:
         if (vit) k.vision = VisionKind::SIGLIP_VIT;
         if (text) k.text = TextKind::SIGLIP;
@@ -228,6 +266,22 @@ void check_vision(const b200_model_desc& d, VisionKind kind) {
         MB_CHECK_ARG(d.resnet_heads * 64 == 32 * wd, "attention pool: head_dim must be 64 (%d channels, %d heads)",
                      32 * wd, d.resnet_heads);
         MB_CHECK_ARG(d.embed_dim % 32 == 0, "CLIP ResNet: embed_dim %d must be a multiple of 32", d.embed_dim);
+        break;
+    }
+    case VisionKind::CONVNEXT: {
+        // the per-pixel kernels take multiples of 64 channels up to 3072; the image halves four times after the stem
+        for (int s = 0; s < 4; ++s) {
+            MB_CHECK_ARG(d.convnext_dims[s] > 0 && d.convnext_dims[s] % 64 == 0 && d.convnext_dims[s] <= 3072,
+                         "convnext_dims[%d] = %d must be a multiple of 64, <= 3072", s, d.convnext_dims[s]);
+            MB_CHECK_ARG(d.convnext_depths[s] > 0 && d.convnext_depths[s] <= 64, "convnext_depths[%d] = %d out of range",
+                         s, d.convnext_depths[s]);
+        }
+        const int S = d.convnext_image_size;
+        MB_CHECK_ARG(S > 0 && S % 32 == 0 && S <= 640, "convnext_image_size %d must be a multiple of 32, <= 640", S);
+        MB_CHECK_ARG(d.convnext_head == 0 || d.convnext_head == 1, "convnext_head %d must be 0 (linear) or 1 (MLP)",
+                     d.convnext_head);
+        MB_CHECK_ARG(d.embed_dim % 32 == 0, "CLIP ConvNeXt: embed_dim %d must be a multiple of 32", d.embed_dim);
+        MB_CHECK_ARG(d.layer_norm_eps > 0.f, "CLIP ConvNeXt: layer_norm_eps must be positive");
         break;
     }
     case VisionKind::SIGLIP_VIT:
@@ -556,6 +610,17 @@ void build_resnet(b200_model* m, TowerW& T) {
     for (auto& b : R.buf) b = DeviceBuffer<__nv_bfloat16>((size_t)d.max_batch * per_image);
 }
 
+// host fp32 values -> an owned bf16 device copy.  The copy goes on the model's stream ahead of the conversion: a
+// cudaMemcpy from pageable memory may return before its DMA lands, and the non-blocking model stream would not wait.
+const __nv_bfloat16* upload_bf16(b200_model* m, const std::vector<float>& h) {
+    DeviceBuffer<float> tmp(h.size());
+    MB_CUDA(cudaMemcpyAsync(tmp.get(), h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    __nv_bfloat16* dst = derived_buffer<__nv_bfloat16>(m, h.size());
+    kernels::f32_to_bf16(tmp.get(), dst, (long long)h.size(), m->stream);
+    MB_CUDA(cudaStreamSynchronize(m->stream));
+    return dst;
+}
+
 // the MLP activation of open_clip's towers
 int open_clip_act(const b200_model_desc& d) {
     return d.act == B200_ACT_QUICKGELU ? gemm::ACT_QUICKGELU : gemm::ACT_GELU;
@@ -579,6 +644,84 @@ void build_vit(b200_model* m, TowerW& T, const char* conv_name, int cls_rows) {
     kernels::patch_weight_rows(conv, (int)w, (int)p, gemm::patch_gather_kbpd((int)p), cg, m->stream);
     MB_CUDA(cudaStreamSynchronize(m->stream));
     T.conv_wg = cg;
+}
+
+// The ConvNeXt tower's weights in the layouts its kernels read (ConvnextW) and its activation buffers.  T holds the
+// stem as a patch-4 ViT patch embedding.
+void build_convnext(b200_model* m, TowerW& T) {
+    ConvnextW& X = m->convnext;
+    const b200_model_desc& d = m->desc;
+    const long long E = d.embed_dim;
+    const std::string t = "visual.trunk.";
+    build_vit(m, T, "visual.trunk.stem.0.weight", 0);
+    X.stem_b = param(m, t + "stem.0.bias", T.d.width);
+    X.stem_ln_w = param(m, t + "stem.1.weight", T.d.width);
+    X.stem_ln_b = param(m, t + "stem.1.bias", T.d.width);
+    long long prev = 0;
+    for (int s = 0; s < 4; ++s) {
+        ConvnextStageW& st = X.stages[s];
+        const long long C = d.convnext_dims[s];
+        st.C = (int)C;
+        const std::string p = t + "stages." + std::to_string(s) + ".";
+        if (s > 0) {
+            st.ds_ln_w = param(m, p + "downsample.0.weight", prev);
+            st.ds_ln_b = param(m, p + "downsample.0.bias", prev);
+            // [C, C_prev, 2, 2] -> [C, (dy * 2 + dx) * C_prev + c]: ln_pixels' patch row order
+            const std::vector<float> w = to_host(param(m, p + "downsample.1.weight", C * prev * 4), (size_t)(C * prev * 4));
+            std::vector<float> rows(w.size());
+            for (long long o = 0; o < C; ++o)
+                for (long long c = 0; c < prev; ++c)
+                    for (int q = 0; q < 4; ++q) rows[(o * 4 + q) * prev + c] = w[(o * prev + c) * 4 + q];
+            st.ds_w = upload_bf16(m, rows);
+            m->raw.erase(p + "downsample.1.weight");
+            st.ds_b = param(m, p + "downsample.1.bias", C);
+        }
+        st.blocks.resize(d.convnext_depths[s]);
+        for (int i = 0; i < d.convnext_depths[s]; ++i) {
+            const std::string b = p + "blocks." + std::to_string(i) + ".";
+            ConvnextBlockW& B = st.blocks[i];
+            // conv_dw.weight [C, 1, 7, 7] -> [49, C]: a tap's channels contiguous
+            const std::vector<float> dw = to_host(param(m, b + "conv_dw.weight", C * 49), (size_t)(C * 49));
+            std::vector<float> taps(dw.size());
+            for (long long c = 0; c < C; ++c)
+                for (int k = 0; k < 49; ++k) taps[k * C + c] = dw[c * 49 + k];
+            B.dw_w = upload_derived(m, taps);
+            m->raw.erase(b + "conv_dw.weight");
+            B.dw_b = param(m, b + "conv_dw.bias", C);
+            B.ln_w = param(m, b + "norm.weight", C);
+            B.ln_b = param(m, b + "norm.bias", C);
+            B.w1 = to_bf16(m, b + "mlp.fc1.weight", 4 * C * C);
+            B.b1 = param(m, b + "mlp.fc1.bias", 4 * C);
+            // gamma * (u W2^T + b2) == u (gamma W2)^T + gamma b2
+            const std::vector<float> g = to_host(param(m, b + "gamma", C), (size_t)C);
+            std::vector<float> w2 = to_host(param(m, b + "mlp.fc2.weight", 4 * C * C), (size_t)(4 * C * C));
+            std::vector<float> b2 = to_host(param(m, b + "mlp.fc2.bias", C), (size_t)C);
+            for (long long o = 0; o < C; ++o) {
+                for (long long k = 0; k < 4 * C; ++k) w2[o * 4 * C + k] *= g[o];
+                b2[o] *= g[o];
+            }
+            B.w2 = upload_bf16(m, w2);
+            B.b2 = upload_derived(m, b2);
+            for (const char* nm : {"mlp.fc2.weight", "mlp.fc2.bias", "gamma"}) m->raw.erase(b + nm);
+        }
+        prev = C;
+    }
+    X.head_ln_w = param(m, t + "head.norm.weight", prev);
+    X.head_ln_b = param(m, t + "head.norm.bias", prev);
+    if (d.convnext_head == 0) {
+        X.w_proj = to_bf16(m, "visual.head.proj.weight", E * prev);
+    } else {
+        X.w_fc1 = to_bf16(m, "visual.head.mlp.fc1.weight", 2 * E * prev);
+        X.b_fc1 = param(m, "visual.head.mlp.fc1.bias", 2 * E);
+        X.w_fc2 = to_bf16(m, "visual.head.mlp.fc2.weight", E * 2 * E);
+    }
+    // x fp32, h bf16, u bf16 (4 C wide) of the first stage, capped at ~24 GB like the transformer workspaces; the
+    // head's rows (n x C3, n x 2E) fit in h and u
+    const long long per_image = (long long)T.tokens * T.d.width;
+    X.max_images = (int)std::max<long long>(1, std::min<long long>(d.max_batch, (24LL << 30) / (per_image * 14)));
+    X.x = DeviceBuffer<float>((size_t)X.max_images * per_image);
+    X.h = DeviceBuffer<__nv_bfloat16>((size_t)X.max_images * per_image);
+    X.u = DeviceBuffer<__nv_bfloat16>((size_t)X.max_images * per_image * 4);
 }
 
 void build_vision(b200_model* m) {
@@ -605,6 +748,9 @@ void build_vision(b200_model* m) {
         break;
     case VisionKind::RESNET:
         build_resnet(m, T);
+        break;
+    case VisionKind::CONVNEXT:
+        build_convnext(m, T);
         break;
     }
 }
@@ -790,16 +936,11 @@ void forward_resnet(b200_model* m, Counter& c, const uint8_t* u8, const float* f
     c.n += kernels::l2_rows(m->pooled.get(), n, E, normalize, d_out, m->stream);
 }
 
-// A ViT trunk over n images (device uint8 [n, S, S, 3] u8, or device fp32 CHW f32): patch embedding, ln_pre (CLIP) and
-// the layers, leaving the n * T.tokens token rows in x.
-void forward_vit(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, const float* f32, int n) {
+// The patch conv of T (no bias in its weights) over n images (device uint8 [n, S, S, 3] u8, or device fp32 CHW f32)
+// through epilogue e, into the n * T.tokens token rows.
+void patch_embed(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, const float* f32, int n,
+                 const gemm::Epilogue& e) {
     const int S = T.d.image_size, p = T.d.patch, w = T.d.width;
-    float* x = m->x.get();
-    // x = positional embedding (+ class embedding on each image's first row), then conv1 (no bias) of every token row
-    // added onto it in place; a class-token row multiplies a zero A row.  SigLIP has no class row, and its conv bias is
-    // already in T.pos.
-    c.n += kernels::vit_embed_rows(x, T.cls, T.pos, n, T.tokens, w, m->stream);
-    const gemm::Epilogue e = epilogue(x, w, nullptr, gemm::ACT_NONE, true, x, w);
     if (u8) {
         // uint8 pixels -> ToTensor + Normalize -> bf16 inside the GEMM's operand load: no patch matrix in HBM
         gemm::PatchGather pg;
@@ -819,6 +960,18 @@ void forward_vit(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, 
         c.n += kernels::im2col_f32(f32, n, S, p, T.kpad, T.cls_rows, m->patches.get(), m->stream);
         linear(m, c, m->patches.get(), n * T.tokens, T.kpad, T.conv_w, w, e);
     }
+}
+
+// A ViT trunk over n images (device uint8 [n, S, S, 3] u8, or device fp32 CHW f32): patch embedding, ln_pre (CLIP) and
+// the layers, leaving the n * T.tokens token rows in x.
+void forward_vit(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, const float* f32, int n) {
+    const int w = T.d.width;
+    float* x = m->x.get();
+    // x = positional embedding (+ class embedding on each image's first row), then conv1 (no bias) of every token row
+    // added onto it in place; a class-token row multiplies a zero A row.  SigLIP has no class row, and its conv bias is
+    // already in T.pos.
+    c.n += kernels::vit_embed_rows(x, T.cls, T.pos, n, T.tokens, w, m->stream);
+    patch_embed(m, c, T, u8, f32, n, epilogue(x, w, nullptr, gemm::ACT_NONE, true, x, w));
     if (T.ln_pre_w)
         c.n += kernels::layernorm(x, w, T.ln_pre_w, T.ln_pre_b, T.eps, n * T.tokens, w, x, nullptr, m->stream);
     run_layers(m, c, T, n, T.tokens, attention::MASK_NONE, true);
@@ -842,6 +995,49 @@ void map_head(b200_model* m, Counter& c, const TowerW& T, int n, int normalize, 
     c.n += kernels::l2_rows(pooled, n, w, normalize, d_out, m->stream);
 }
 
+// The ConvNeXt CLIP image tower over n images (device uint8 HWC u8 or normalised fp32 CHW f32, at the model's size).
+void forward_convnext(b200_model* m, Counter& c, const uint8_t* u8, const float* f32, int n, int normalize,
+                      float* d_out) {
+    const ConvnextW& X = m->convnext;
+    const TowerW& T = m->vision;
+    const b200_model_desc& d = m->desc;
+    const float eps = d.layer_norm_eps;
+    const int E = d.embed_dim, C0 = T.d.width;
+    float* x = X.x.get();
+    __nv_bfloat16 *h = X.h.get(), *u = X.u.get();
+    // stem: the 4 x 4 stride-4 conv with its bias -> x, then its LayerNorm in place: the residual stream
+    patch_embed(m, c, T, u8, f32, n, epilogue(x, C0, X.stem_b, gemm::ACT_NONE, true));
+    int H = T.grid;
+    c.n += kernels::ln_pixels(x, n, H, H, C0, X.stem_ln_w, X.stem_ln_b, eps, x, nullptr, m->stream);
+    int prev = C0;
+    for (const ConvnextStageW& st : X.stages) {
+        const int C = st.C;
+        if (st.ds_w) {
+            // LayerNorm + 2 x 2 patches -> h; the GEMM reads only h, so it may overwrite x
+            c.n += kernels::ln_pixels(x, n, H, H, prev, st.ds_ln_w, st.ds_ln_b, eps, nullptr, h, m->stream);
+            H /= 2;
+            linear(m, c, h, n * H * H, 4 * prev, st.ds_w, C, epilogue(x, C, st.ds_b, gemm::ACT_NONE, true));
+        }
+        const int M = n * H * H;
+        for (const ConvnextBlockW& B : st.blocks) {
+            c.n += kernels::dwconv7_ln(x, n, H, H, C, B.dw_w, B.dw_b, B.ln_w, B.ln_b, eps, h, m->stream);
+            linear(m, c, h, M, C, B.w1, 4 * C, epilogue(u, 4 * C, B.b1, gemm::ACT_GELU));
+            linear(m, c, u, M, 4 * C, B.w2, C, epilogue(x, C, B.b2, gemm::ACT_NONE, true, x, C));
+        }
+        prev = C;
+    }
+    // head: mean over the pixels + LayerNorm -> h [n, C3], then the projection or the MLP -> pooled, L2
+    float* pooled = m->pooled.get();
+    c.n += kernels::pool_ln(x, n, H * H, prev, X.head_ln_w, X.head_ln_b, eps, h, m->stream);
+    if (X.w_proj) {
+        linear(m, c, h, n, prev, X.w_proj, E, epilogue(pooled, E, nullptr, gemm::ACT_NONE, true));
+    } else {
+        linear(m, c, h, n, prev, X.w_fc1, 2 * E, epilogue(u, 2 * E, X.b_fc1, gemm::ACT_GELU));
+        linear(m, c, u, n, 2 * E, X.w_fc2, E, epilogue(pooled, E, nullptr, gemm::ACT_NONE, true));
+    }
+    c.n += kernels::l2_rows(pooled, n, E, normalize, d_out, m->stream);
+}
+
 // images already as device uint8 [n, S, S, 3] (u8 != nullptr) or device fp32 CHW (f32 != nullptr)
 void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const float* f32, int n, int normalize,
                           float* d_out) {
@@ -858,6 +1054,9 @@ void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const fl
         break;
     case VisionKind::RESNET:
         forward_resnet(m, c, u8, f32, n, normalize, d_out);
+        break;
+    case VisionKind::CONVNEXT:
+        forward_convnext(m, c, u8, f32, n, normalize, d_out);
         break;
     }
 }
@@ -969,6 +1168,11 @@ int batch_cap_tokens(b200_model* m, int tokens_per_item) {
     return (int)std::max<long long>(1, std::min<long long>(m->desc.max_batch, m->max_tokens / tokens_per_item));
 }
 
+// images per forward pass: what the image tower's activation buffers hold
+int image_batch_cap(b200_model* m) {
+    return m->kind.vision == VisionKind::CONVNEXT ? m->convnext.max_images : batch_cap_tokens(m, m->vision.tokens);
+}
+
 struct TimedRegion {
     b200_model* m;
     Counter c;
@@ -985,7 +1189,7 @@ void encode_images_u8_dev(b200_model* m, Counter& c, const uint8_t* d_img, int n
                           float* d_out) {
     const TowerW& T = m->vision;
     const int S = T.d.image_size;
-    const int cap = batch_cap_tokens(m, T.tokens);
+    const int cap = image_batch_cap(m);
     for (int o = 0; o < n; o += cap) {
         const int nb = std::min(cap, n - o);
         const uint8_t* src = d_img + (size_t)o * h * w * 3;
@@ -1027,7 +1231,7 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         require_sm90_device(device);
         MB_CHECK_ARG(desc->arch == B200_ARCH_CLIP || desc->arch == B200_ARCH_BERT || desc->arch == B200_ARCH_MPNET ||
                          desc->arch == B200_ARCH_SIGLIP || desc->arch == B200_ARCH_XLMR ||
-                         desc->arch == B200_ARCH_CLIP_RESNET,
+                         desc->arch == B200_ARCH_CLIP_RESNET || desc->arch == B200_ARCH_CLIP_CONVNEXT,
                      "unknown arch %d", desc->arch);
         MB_CHECK_ARG(desc->max_batch > 0, "max_batch must be positive");
         MB_CHECK_ARG(desc->embed_dim > 0 && desc->embed_dim <= 4096, "embed_dim out of range");
@@ -1047,6 +1251,11 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         m->kind = kind;
         if (kind.vision == VisionKind::CLIP_VIT || kind.vision == VisionKind::SIGLIP_VIT) m->vision.d = desc->vision;
         if (kind.vision == VisionKind::RESNET) m->vision.d.image_size = desc->resnet_image_size;   // (no layers)
+        if (kind.vision == VisionKind::CONVNEXT) {   // the stem, as a patch embedding (no layers)
+            m->vision.d.image_size = desc->convnext_image_size;
+            m->vision.d.patch = 4;
+            m->vision.d.width = desc->convnext_dims[0];
+        }
         if (kind.text != TextKind::NONE) m->text.d = desc->text;
         gemm::configure();
         *out = m.release();
@@ -1091,6 +1300,7 @@ int b200_model_finalize(b200_model* m) {
         const long long B = m->desc.max_batch, E = m->desc.embed_dim;
         long long max_tok = 0, max_w = 0, max_mlp = 0;
         for (const TowerW* T : {&m->vision, &m->text}) {
+            if (T == &m->vision && m->kind.vision == VisionKind::CONVNEXT) continue;   // its own buffers (ConvnextW)
             max_tok = std::max(max_tok, B * T->tokens);   // (0 for a missing tower)
             max_w = std::max<long long>(max_w, T->d.width);
             max_mlp = std::max<long long>({max_mlp, T->d.mlp, T->map.mlp});
@@ -1151,7 +1361,7 @@ int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int nor
         std::lock_guard<std::mutex> lk(m->mu);
         DeviceGuard g(m->device);
         const int E = m->desc.embed_dim, S = m->vision.d.image_size;
-        const int cap = batch_cap_tokens(m, m->vision.tokens);
+        const int cap = image_batch_cap(m);
         const size_t img_bytes = (size_t)3 * S * S * 4;
         ensure_in_dev(m, (size_t)std::min(n, cap) * img_bytes);
         TimedRegion tr(m);

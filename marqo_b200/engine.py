@@ -289,13 +289,16 @@ def _to_numpy_f32(t) -> np.ndarray:
 
 
 class Encoder:
-    """A CLIP, ResNet CLIP or SigLIP (vision + text towers), BERT, MPNet or XLM-R encoder resident on one GPU.
+    """A CLIP, ResNet CLIP, ConvNeXt CLIP or SigLIP (vision + text towers), BERT, MPNet or XLM-R encoder resident on one
+    GPU.
 
     `config` keys — CLIP: embed_dim, act ("gelu"|"quickgelu"), mean, std, vision{width,layers,heads,mlp,patch,
     image_size}, text{width,layers,heads,mlp,ctx,vocab};  SigLIP: the CLIP keys plus ln_eps (embed_dim == vision
     width);  ResNet CLIP ("clip_resnet"): embed_dim, act, mean, std, the text tower's width, layers, heads, mlp, ctx,
     vocab at the top level (layers 0: no text tower), resnet{layers [4], width, heads, image_size} (None: no image
-    tower);  BERT: width, layers, heads, mlp, vocab, max_pos, type_vocab,
+    tower);  ConvNeXt CLIP ("clip_convnext"): the ResNet CLIP keys with convnext{dims [4], depths [4], image_size,
+    ln_eps, head ("linear"|"mlp")} (None: no image tower) in place of resnet;  BERT: width, layers, heads, mlp, vocab,
+    max_pos, type_vocab,
     pool ("mean"|"cls");  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
     max_pos - pad_id - 1 tokens), pad_id, ln_eps, rel_buckets, rel_max_distance, pool;  XLM-R: width, layers, heads,
     mlp, vocab, max_pos (as MPNet), pad_id, ln_eps, pool.  `weights` maps checkpoint parameter names (open_clip
@@ -343,6 +346,24 @@ class Encoder:
                 d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"], config["ctx"],
                                      config["vocab"], 0, 0)
             self.image_size = int(r.get("image_size", 224)) if r else 0
+        elif arch == "clip_convnext":
+            d.arch = N.ARCH_CLIP_CONVNEXT
+            d.embed_dim = int(config["embed_dim"])
+            d.act = N.ACT_QUICKGELU if config.get("act", "gelu") == "quickgelu" else N.ACT_GELU
+            for i in range(3):
+                d.image_mean[i] = float(np.float32(config["mean"][i]))
+                d.image_std[i] = float(np.float32(config["std"][i]))
+            cx = config.get("convnext")
+            if cx:
+                for i in range(4):
+                    d.convnext_dims[i], d.convnext_depths[i] = int(cx["dims"][i]), int(cx["depths"][i])
+                d.convnext_image_size = int(cx["image_size"])
+                d.layer_norm_eps = float(cx["ln_eps"])
+                d.convnext_head = {"linear": 0, "mlp": 1}[cx["head"]]
+            if config.get("layers"):
+                d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"], config["ctx"],
+                                     config["vocab"], 0, 0)
+            self.image_size = int(cx["image_size"]) if cx else 0
         elif arch == "bert":
             d.arch = N.ARCH_BERT
             d.embed_dim = int(config["width"])
@@ -933,4 +954,58 @@ def debug_conv2d(x, w, bias=None, residual=None, relu: bool = True, device: int 
     dr, out = d.up(r, "bfloat16"), d.empty((n, Ho, Wo, cout), "bfloat16")
     N.check(N.load().b200_debug_conv2d(device, _dptr(dx), n, H, W, cin, _ptr(wa), cout, k, _dptr(db), _dptr(dr),
                                        int(relu), _dptr(out), d.stream))
+    return _host(out)
+
+
+def _ln_args(gamma, beta, C: int):
+    g, b = _as(gamma, np.float32), _as(beta, np.float32)
+    if g.shape != (C,) or b.shape != (C,):
+        raise ValueError(f"expected gamma and beta [{C}], got {g.shape} and {b.shape}")
+    return g, b
+
+
+def debug_dwconv7_ln(x, w, bias, gamma, beta, eps: float, device: int = 0) -> np.ndarray:
+    """ConvNeXt block head: x NHWC fp32 [n, H, W, C], w [C, 1, 7, 7] (conv_dw.weight), bias [C] -> fp32 [n * H * W, C]
+    (rounded to bf16) = LayerNorm over C of the 7 x 7 depthwise conv (zero padding 3) plus bias."""
+    xa, wa = _as(x, np.float32), _as(w, np.float32)
+    n, H, W, Cc = xa.shape
+    if wa.shape != (Cc, 1, 7, 7):
+        raise ValueError(f"expected w [{Cc}, 1, 7, 7], got {wa.shape}")
+    g, b = _ln_args(gamma, beta, Cc)
+    d = _Staging(device)
+    taps = np.ascontiguousarray(wa.reshape(Cc, 49).T)   # [49, C], as the model lays it out
+    dx, dw, db, dg, dbeta = d.up(xa), d.up(taps), d.up(bias), d.up(g), d.up(b)
+    out = d.empty((n * H * W, Cc), "bfloat16")
+    N.check(N.load().b200_debug_dwconv7_ln(device, _dptr(dx), n, H, W, Cc, _dptr(dw), _dptr(db), _dptr(dg), _dptr(dbeta),
+                                           float(eps), _dptr(out), d.stream))
+    return _host(out)
+
+
+def debug_ln_pixels(x, gamma, beta, eps: float, patchify: bool, device: int = 0) -> np.ndarray:
+    """ConvNeXt per-pixel LayerNorm of x NHWC fp32 [n, H, W, C].  patchify False: fp32 [n * H * W, C] (the stem's norm,
+    written in place over x on the device); True: [n * (H/2) * (W/2), 4C] rounded to bf16, the downsample conv's GEMM
+    rows, pixel (y, x) at columns ((y % 2) * 2 + x % 2) * C + c of row (y/2, x/2)."""
+    xa = _as(x, np.float32)
+    n, H, W, Cc = xa.shape
+    if patchify and (H % 2 or W % 2):
+        raise ValueError(f"patchify needs an even H and W, got {xa.shape}")
+    g, b = _ln_args(gamma, beta, Cc)
+    d = _Staging(device)
+    dx, dg, dbeta = d.up(xa), d.up(g), d.up(b)
+    out = d.empty((n * H * W // 4, 4 * Cc), "bfloat16") if patchify else dx
+    N.check(N.load().b200_debug_ln_pixels(device, _dptr(dx), n, H, W, Cc, _dptr(dg), _dptr(dbeta), float(eps),
+                                          int(patchify), _dptr(out), d.stream))
+    return _host(out).reshape(-1, 4 * Cc if patchify else Cc)
+
+
+def debug_pool_ln(x, gamma, beta, eps: float, device: int = 0) -> np.ndarray:
+    """ConvNeXt head input: x fp32 [n, HW, C] -> fp32 [n, C] (rounded to bf16) = LayerNorm over C of the mean over the
+    HW pixels of each image."""
+    xa = _as(x, np.float32)
+    n, HW, Cc = xa.shape
+    g, b = _ln_args(gamma, beta, Cc)
+    d = _Staging(device)
+    dx, dg, dbeta, out = d.up(xa), d.up(g), d.up(b), d.empty((n, Cc), "bfloat16")
+    N.check(N.load().b200_debug_pool_ln(device, _dptr(dx), n, HW, Cc, _dptr(dg), _dptr(dbeta), float(eps), _dptr(out),
+                                        d.stream))
     return _host(out)

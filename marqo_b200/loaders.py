@@ -34,6 +34,7 @@ def _resolve_weights(props: dict, arch: dict, kind: str) -> Dict[str, np.ndarray
         seed = int(props["random_init"])
         random = {"clip": weights_mod.random_clip_weights, "siglip": weights_mod.random_siglip_weights,
                   "clip_resnet": weights_mod.random_clip_resnet_weights,
+                  "clip_convnext": weights_mod.random_clip_convnext_weights,
                   "bert": weights_mod.random_bert_weights, "mpnet": weights_mod.random_mpnet_weights,
                   "xlmr": weights_mod.random_xlmr_weights}[kind]
         return random(arch, seed)
@@ -92,8 +93,8 @@ class B200OpenCLIP:
             arch = dict(arch, std=tuple(props["std"]))
         self.arch = arch
         # "siglip" (model_registry.SIGLIP_MODELS): the engine's SigLIP runtime, whose GPU resize squashes images to
-        # S x S; "clip_resnet" (RESNET_MODELS): OpenAI's ResNet CLIP; otherwise open_clip CLIP; both shortest side -> S
-        # + centre crop
+        # S x S; "clip_resnet" (RESNET_MODELS): OpenAI's ResNet CLIP; "clip_convnext" (CONVNEXT_MODELS): ConvNeXt
+        # CLIP; otherwise open_clip CLIP; all three shortest side -> S + centre crop
         kind = arch.get("kind", "clip")
         self.model = Encoder(kind, arch, _resolve_weights(props, arch, kind), device=_validate_device(self.device),
                              max_batch=int(props.get("max_batch", 256)))
@@ -103,8 +104,9 @@ class B200OpenCLIP:
     def _default_tokenizer(self):
         if self.model_properties.get("merges_file"):
             from .tokenizers import ClipBpeTokenizer
-            # the CLIP text tower's ctx: in its "text" block, or at the top level of a clip_resnet arch
-            ctx = self.arch["ctx"] if self.arch.get("kind") == "clip_resnet" else self.arch["text"]["ctx"]
+            # the CLIP text tower's ctx: in its "text" block, or at the top level of a clip_resnet / clip_convnext arch
+            top = self.arch.get("kind") in ("clip_resnet", "clip_convnext")
+            ctx = self.arch["ctx"] if top else self.arch["text"]["ctx"]
             return ClipBpeTokenizer(self.model_properties["merges_file"], context_length=int(ctx))
         try:
             import open_clip  # type: ignore
@@ -390,4 +392,4 @@ def register_with_marqo() -> None:
     """Install the two loader types into a live Marqo process (see INTEGRATION.md)."""
     from marqo.s2_inference import s2_inference as marqo_s2  # type: ignore
     marqo_s2.MODEL_PROPERTIES['loaders'].update(LOADERS)
-    marqo_s2.MODEL_PROPERTIES['models'].update(model_registry.all_models())
+    marqo_s2.MODEL_PROPERTIES['models'].update({**model_registry.all_models(), **model_registry.CONVNEXT_MODELS})

@@ -59,7 +59,26 @@ output is embed_dim wide (1024 / 512); the CLIP text tower (width 512, 12 layers
 49408).  Every `openai` tag loads as QuickGELU (as ViT-B-32/openai does here), the `-quickgelu` names too; the
 yfcc15m / cc12m tags of the plain names run erf-GELU.  OpenAI mean and std, shortest side -> 224 + centre crop.  The
 arch block has no "vision" key: the text tower's fields sit at the top level, as in the BERT archs, and the CNN in its
-own "resnet" block."""
+own "resnet" block.
+
+The ConvNeXt CLIP entries (model_registry.py:274-343) live in CONVNEXT_MODELS (`arch["kind"] == "clip_convnext"`),
+served by the `b200_open_clip` loader, in the clip_resnet layout with the trunk in a "convnext" block.  find_model
+finds them; all_models() leaves them out (see there).  Their shapes
+come from open_clip 2.24.0's model_configs/convnext_*.json, its `TimmModel` and timm's convnext.py, none of which can
+be re-read offline (verify):
+    convnext_base        timm convnext_base: dims 128, 256, 512, 1024, depths 3, 3, 27, 3; image 224; linear head;
+                         text width 512, 8 heads, 12 layers
+    convnext_base_w      the same trunk at image 256; text width 640, 10 heads, 12 layers
+    convnext_base_w_320  convnext_base_w at image 320
+    convnext_large_d     timm convnext_large: dims 192, 384, 768, 1536, depths 3, 3, 27, 3; image 256; MLP head
+                         (fc1 with bias to 2 embed, GELU, fc2 without bias); text width 768, 12 heads, 16 layers
+    convnext_large_d_320 convnext_large_d at image 320
+    convnext_xxlarge     timm convnext_xxlarge: dims 384, 768, 1536, 3072, depths 3, 4, 30, 3; image 256; linear
+                         head; trunk LayerNorm eps 1e-5 (timm's norm_eps for this model; 1e-6 for the others); text
+                         width 1024, 16 heads, 24 layers
+The heads pool with timm's own head (global average pool, then its LayerNorm), and the Linear head has no bias.  Every
+text tower has mlp 4 width, ctx 77, vocabulary 49408 and erf-GELU, as do the trunk's MLPs.  OpenAI mean and std,
+shortest side -> S + centre crop, as for CLIP (not SigLIP's squash)."""
 from __future__ import annotations
 
 import copy
@@ -261,9 +280,42 @@ def _resnet_models() -> Dict[str, dict]:
 RESNET_MODELS: Dict[str, dict] = _resnet_models()
 
 
+def _convnext_arch(trunk: str, image: int, head: str, embed: int, tw: int, tl: int, th: int) -> dict:
+    """ConvNeXt CLIP (module docstring, verify)."""
+    dims, depths, eps = {"base": ([128, 256, 512, 1024], [3, 3, 27, 3], 1e-6),
+                         "large": ([192, 384, 768, 1536], [3, 3, 27, 3], 1e-6),
+                         "xxlarge": ([384, 768, 1536, 3072], [3, 4, 30, 3], 1e-5)}[trunk]
+    return {"kind": "clip_convnext", "embed_dim": embed, "act": "gelu", "mean": OPENAI_MEAN, "std": OPENAI_STD,
+            "width": tw, "layers": tl, "heads": th, "mlp": 4 * tw, "ctx": 77, "vocab": 49408,
+            "convnext": {"dims": dims, "depths": depths, "image_size": image, "ln_eps": eps, "head": head}}
+
+
+def _convnext_models() -> Dict[str, dict]:
+    m: Dict[str, dict] = {}
+    base_w = ("laion2b_s13b_b82k", "laion2b_s13b_b82k_augreg", "laion_aesthetic_s13b_b82k")
+    for model, shape, tags in (
+            ("convnext_base", ("base", 224, "linear", 512, 512, 12, 8), ("laion400m_s13b_b51k",)),
+            ("convnext_base_w", ("base", 256, "linear", 640, 640, 12, 10), base_w),
+            ("convnext_base_w_320", ("base", 320, "linear", 640, 640, 12, 10),
+             ("laion_aesthetic_s13b_b82k", "laion_aesthetic_s13b_b82k_augreg")),
+            ("convnext_large_d", ("large", 256, "mlp", 768, 768, 16, 12), ("laion2b_s26b_b102k_augreg",)),
+            ("convnext_large_d_320", ("large", 320, "mlp", 768, 768, 16, 12),
+             ("laion2b_s29b_b131k_ft", "laion2b_s29b_b131k_ft_soup")),
+            ("convnext_xxlarge", ("xxlarge", 256, "linear", 1024, 1024, 24, 16),
+             ("laion2b_s34b_b82k_augreg", "laion2b_s34b_b82k_augreg_rewind", "laion2b_s34b_b82k_augreg_soup"))):
+        for tag in tags:
+            name = f"open_clip/{model}/{tag}"
+            m[name] = {"name": name, "dimensions": shape[3], "note": "open_clip models", "type": TYPE_OPEN_CLIP,
+                       "pretrained": tag, "arch": _convnext_arch(*shape)}
+    return m
+
+
+CONVNEXT_MODELS: Dict[str, dict] = _convnext_models()
+
+
 def find_model(model_name: str) -> Optional[dict]:
     """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
-    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS):
+    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS, CONVNEXT_MODELS):
         entry = table.get(model_name)
         if entry is not None:
             return entry
@@ -271,7 +323,11 @@ def find_model(model_name: str) -> Optional[dict]:
 
 
 def all_models() -> Dict[str, dict]:
-    """Every served registry entry by name (a new dict over the same entries)."""
+    """The served registry entries by name (a new dict over the same entries), except CONVNEXT_MODELS.  The layer
+    widths of these entries' towers are the served set the GEMM shape tests pin (384, 512, 768, 1024); the ConvNeXt
+    CLIP text towers add width 640, whose GEMMs tests/test_convnext_clip_gpu.py runs instead.  Callers that need every
+    served entry add CONVNEXT_MODELS to it, as loaders.register_with_marqo and s2_inference do; find_model looks in
+    every table."""
     return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS, **RESNET_MODELS}
 
 

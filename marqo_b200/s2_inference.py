@@ -104,7 +104,8 @@ def validate_model_properties(model_name: str, model_properties: Optional[dict])
     if "arch" not in props:
         base = model_registry.find_model(model_name)
         if base is None:
-            base = next((e for e in model_registry.all_models().values() if e["name"] == props.get("name")), None)
+            served = {**model_registry.all_models(), **model_registry.CONVNEXT_MODELS}
+            base = next((e for e in served.values() if e["name"] == props.get("name")), None)
         if base is None:
             raise InvalidModelPropertiesError(
                 f"model_properties for {model_name} needs an `arch` block (or a registry name) to size the encoder")

@@ -205,6 +205,52 @@ def random_clip_resnet_weights(arch: dict, seed: int = 1234) -> Dict[str, np.nda
     return sd
 
 
+def random_clip_convnext_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
+    """Seeded random weights under open_clip's TimmModel names for a timm ConvNeXt trunk (arch: the registry's
+    clip_convnext block; arch["convnext"] None: no image tower, arch["layers"] 0: no text tower)."""
+    g = _rng(seed)
+    sd: Dict[str, np.ndarray] = {}
+    cx, E = arch.get("convnext"), arch["embed_dim"]
+    if cx:
+        t, dims = "visual.trunk.", cx["dims"]
+
+        def ln(prefix, c):
+            sd[prefix + ".weight"] = _vec(g, c, 0.1, 1.0)
+            sd[prefix + ".bias"] = _vec(g, c)
+
+        sd[t + "stem.0.weight"] = _conv(g, dims[0], 3, 4)
+        sd[t + "stem.0.bias"] = _vec(g, dims[0])
+        ln(t + "stem.1", dims[0])
+        for s, (C, depth) in enumerate(zip(dims, cx["depths"])):
+            p = f"{t}stages.{s}."
+            if s > 0:
+                ln(p + "downsample.0", dims[s - 1])
+                sd[p + "downsample.1.weight"] = _conv(g, C, dims[s - 1], 2)
+                sd[p + "downsample.1.bias"] = _vec(g, C)
+            for i in range(depth):
+                b = f"{p}blocks.{i}."
+                sd[b + "conv_dw.weight"] = _conv(g, C, 1, 7)
+                sd[b + "conv_dw.bias"] = _vec(g, C)
+                ln(b + "norm", C)
+                sd[b + "mlp.fc1.weight"] = _lin(g, 4 * C, C)
+                sd[b + "mlp.fc1.bias"] = _vec(g, 4 * C)
+                sd[b + "mlp.fc2.weight"] = _lin(g, C, 4 * C)
+                sd[b + "mlp.fc2.bias"] = _vec(g, C)
+                # trained layer scales are small; these keep the residual stream from growing over 30 blocks
+                sd[b + "gamma"] = _vec(g, C, 0.1, 0.3)
+        ln(t + "head.norm", dims[3])
+        if cx["head"] == "mlp":
+            sd["visual.head.mlp.fc1.weight"] = _lin(g, 2 * E, dims[3])
+            sd["visual.head.mlp.fc1.bias"] = _vec(g, 2 * E)
+            sd["visual.head.mlp.fc2.weight"] = _lin(g, E, 2 * E)
+        else:
+            sd["visual.head.proj.weight"] = _lin(g, E, dims[3])
+    if arch.get("layers"):
+        text = {k: arch[k] for k in ("width", "layers", "heads", "mlp", "ctx", "vocab")}
+        sd.update(random_clip_weights({"embed_dim": E, "text": text}, seed + 1))
+    return sd
+
+
 def random_bert_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     g = _rng(seed)
     w, mlp = arch["width"], arch["mlp"]
