@@ -87,6 +87,19 @@ def tiny_bert(pool: str = "mean") -> BertCfg:
     return BertCfg(128, 2, 2, 512, vocab=1000, max_pos=64, pool=pool)
 
 
+def engine_config(cfg) -> dict:
+    """The Encoder("bert", ...) config of a BertCfg, or the Encoder("clip", ...) config of a ClipCfg."""
+    if isinstance(cfg, BertCfg):
+        return dict(width=cfg.width, layers=cfg.layers, heads=cfg.heads, mlp=cfg.mlp, vocab=cfg.vocab,
+                    max_pos=cfg.max_pos, type_vocab=cfg.type_vocab, pool=cfg.pool)
+
+    def tower(t):
+        return dict(width=t.width, layers=t.layers, heads=t.heads, mlp=t.mlp, ctx=t.ctx, vocab=t.vocab,
+                    image_size=t.image_size, patch=t.patch)
+    return dict(embed_dim=cfg.embed_dim, act=cfg.act, mean=cfg.mean, std=cfg.std, vision=tower(cfg.vision),
+                text=tower(cfg.text))
+
+
 # ------------------------------------------------------------------------------------------------ weights
 def _lin(g, out_f, in_f, gain=1.0):
     return torch.randn(out_f, in_f, generator=g) * (gain / math.sqrt(in_f))

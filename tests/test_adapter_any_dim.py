@@ -6,6 +6,7 @@ changes, and the padding never shows: get_batch returns d values and the error m
 import numpy as np
 import pytest
 
+import _checks as K
 from _filter_scenario import _doc, _yql
 
 
@@ -87,11 +88,6 @@ def gti(monkeypatch):
     return gti
 
 
-def _unit(rng, m, d):
-    x = rng.standard_normal((m, d)).astype(np.float32)
-    return x / np.linalg.norm(x, axis=1, keepdims=True)
-
-
 def _ask(ix, q, hits=5):
     return ix.query(_yql("s1", ["body"], hits), hits=hits, ranking="embedding_similarity", model_restrict="s1",
                     query_features={"marqo__query_embedding": np.asarray(q).tolist()})
@@ -110,7 +106,7 @@ def _expected(vecs, chunks, q, hits):
 def test_any_dimension_feeds_queries_reads_back_and_persists(gti, d, tmp_path):
     rng = np.random.default_rng(d)
     n, chunks = 30, 2
-    vecs = _unit(rng, n * chunks, d)
+    vecs = K.unit_rows(rng, n * chunks, d)
     ix = gti.GpuTensorIndex()
     docs = [_doc(f"d{i}", {}, {"body": (["c0", "c1"], vecs[i * chunks:(i + 1) * chunks])}) for i in range(n)]
     assert not ix.feed_batch(docs, "s1").errors
@@ -121,7 +117,7 @@ def test_any_dimension_feeds_queries_reads_back_and_persists(gti, d, tmp_path):
     for block in store.received:
         assert block.shape[1] == width and not block[:, d:].any()
     np.testing.assert_array_equal(np.concatenate(store.received)[:, :d], vecs)
-    q = _unit(rng, 1, d)[0]
+    q = K.unit_rows(rng, 1, d)[0]
     res = _ask(ix, q)
     ids, rel = _expected(vecs, chunks, q, 5)
     assert [h.id.split("::")[-1] for h in res.hits] == ids
@@ -146,9 +142,9 @@ def test_any_dimension_feeds_queries_reads_back_and_persists(gti, d, tmp_path):
 def test_wrong_dimension_documents_and_queries_are_rejected(gti, d):
     rng = np.random.default_rng(1)
     ix = gti.GpuTensorIndex()
-    assert not ix.feed_batch([_doc("a", {}, {"body": (["0"], _unit(rng, 1, d))})], "s1").errors
+    assert not ix.feed_batch([_doc("a", {}, {"body": (["0"], K.unit_rows(rng, 1, d))})], "s1").errors
     for bad in (d - 1, d + 1, -(-d // 64) * 64):      # the padded width is not the field's dimension either
-        r = ix.feed_batch([_doc("b", {}, {"body": (["0"], _unit(rng, 1, bad))})], "s1")
+        r = ix.feed_batch([_doc("b", {}, {"body": (["0"], K.unit_rows(rng, 1, bad))})], "s1")
         assert r.errors and r.responses[0].status == 400
         assert r.responses[0].message == f"field marqo__embeddings_body: embedding dimension {bad} != index dimension {d}"
         with pytest.raises(Exception, match=f"Expected a tensor of dimension {d} for query input but got {bad}"):
@@ -178,7 +174,7 @@ def test_manifest_without_a_recorded_dimension_loads_at_the_store_width(gti, tmp
     """Snapshots written before fields could be padded have no "dim" entry: the field's dimension is the store's."""
     import json
     rng = np.random.default_rng(2)
-    vecs = _unit(rng, 4, 128)
+    vecs = K.unit_rows(rng, 4, 128)
     ix = gti.GpuTensorIndex()
     ix.feed_batch([_doc(f"d{i}", {}, {"body": (["0"], vecs[i:i + 1])}) for i in range(4)], "s1")
     ix.save(str(tmp_path))

@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 import torch
 
+import _checks as K
 from oracle import encoders as E
 
 pytestmark = pytest.mark.gpu
@@ -14,33 +15,10 @@ TINY_CLIP_ARCH = dict(embed_dim=128, act="gelu", mean=E.OPENAI_CLIP_MEAN, std=E.
                       text=dict(width=128, layers=2, heads=2, mlp=512, ctx=77, vocab=1000))
 
 
-class WordTokenizer:
-    """Stand-in for AutoTokenizer (no vocab files offline): 'w<id>' words -> ids, [CLS]=2 ... [SEP]=3, pad 0."""
-
-    def __call__(self, sentences, padding=True, truncation=True, max_length=128, return_tensors="np"):
-        rows = []
-        for s in sentences:
-            ids = [2] + [5 + int(w[1:]) for w in s.split()][: max_length - 2] + [3]
-            rows.append(ids)
-        L = max(len(r) for r in rows)
-        ids = np.zeros((len(rows), L), np.int64)
-        mask = np.zeros((len(rows), L), np.int64)
-        for i, r in enumerate(rows):
-            ids[i, :len(r)] = r
-            mask[i, :len(r)] = 1
-        return {"input_ids": ids, "attention_mask": mask}
-
-
-def _cos_ok(got, ref):
-    got, ref = torch.as_tensor(np.asarray(got)).double(), torch.as_tensor(np.asarray(ref)).double()
-    cos = torch.nn.functional.cosine_similarity(got, ref)
-    assert float((1 - cos).max()) < 1e-3, float(cos.min())
-
-
 def test_vectorise_hf_loader_end_to_end(gpu_required, monkeypatch):
     from marqo_b200 import s2_inference as s2, weights as Wt
     s2.clear_loaded_models()
-    tok = WordTokenizer()
+    tok = K.WordTokenizer(2, 3, 5)
     props = {"name": "tiny-bert", "dimensions": 128, "type": "hf", "tokens": 32, "arch": TINY_BERT_ARCH,
              "random_init": 77, "tokenizer": tok}
     rng = np.random.default_rng(0)
@@ -54,10 +32,9 @@ def test_vectorise_hf_loader_end_to_end(gpu_required, monkeypatch):
     for i in range(0, 21, 8):                                            # the reference pads per sub-batch (Appendix A)
         t = tok(sentences[i:i + 8], max_length=32)
         ref.append(E.bert_encode(sd, cfg, torch.from_numpy(t["input_ids"]), torch.from_numpy(t["attention_mask"])))
-    _cos_ok(out, torch.cat(ref))
-    assert np.allclose(np.linalg.norm(np.asarray(out), axis=1), 1.0, atol=1e-5)
+    K.assert_embeddings_match(out, torch.cat(ref))
     one = s2.vectorise("tiny-bert", sentences[3], model_properties=props, device="cuda:0")
-    _cos_ok(one, torch.cat(ref)[3:4])                                    # str == [str] (test_encoding.py:28-60)
+    K.assert_embeddings_match(one, torch.cat(ref)[3:4], unit_norm=False)   # str == [str] (test_encoding.py:28-60)
     assert len(s2._available_models) == 1
     s2.eject_model("tiny-bert", "cuda:0", props)
     assert len(s2._available_models) == 0
@@ -89,7 +66,7 @@ def test_vectorise_clip_loader_images_and_text(gpu_required, monkeypatch):
     ref = E.clip_encode_image(sd, cfg, torch.stack([E.clip_preprocess_pil(p) for p in pil]))
     monkeypatch.setenv("MARQO_MAX_VECTORISE_BATCH_SIZE", "4")
     out = s2.vectorise("tiny-clip", pil, model_properties=props, device="cuda:0", modality=s2.Modality.IMAGE)
-    _cos_ok(out, ref)
+    K.assert_embeddings_match(out, ref, unit_norm=False)
     # what the download threads hand over: model.preprocess(pil) tensors (add_docs.py:129-134)
     key = next(iter(s2._available_models))
     model = s2._available_models[key]["model"]
@@ -99,11 +76,13 @@ def test_vectorise_clip_loader_images_and_text(gpu_required, monkeypatch):
     assert out2 == out
     # already-preprocessed float CHW tensors pass through unchanged (abstract_clip_model.py:108-111)
     chw = [E.clip_preprocess_pil(p) for p in pil[:3]]
-    _cos_ok(s2.vectorise("tiny-clip", chw, model_properties=props, device="cuda:0", modality=s2.Modality.IMAGE), ref[:3])
+    got = s2.vectorise("tiny-clip", chw, model_properties=props, device="cuda:0", modality=s2.Modality.IMAGE)
+    K.assert_embeddings_match(got, ref[:3], unit_norm=False)
     # text
     texts = ["1 2 3", "7", " ".join(str(i) for i in range(10, 60))]
     tref = E.clip_encode_text(sd, cfg, torch.from_numpy(clip_tok(texts)))
-    _cos_ok(s2.vectorise("tiny-clip", texts, model_properties=props, device="cuda:0"), tref)
+    got = s2.vectorise("tiny-clip", texts, model_properties=props, device="cuda:0")
+    K.assert_embeddings_match(got, tref, unit_norm=False)
     assert np.array_equal(model.encode_text(texts), model.encode(texts))         # test_encoding.py:334-370
     s2.clear_loaded_models()
 
@@ -126,7 +105,7 @@ def test_vectorise_with_cxx_tokenizers(gpu_required, tmp_path):
     ids, mask = OT.bert_encode_batch(OT.bert_wordpiece(words), sentences, 32)
     sd = {k: torch.from_numpy(v) for k, v in Wt.random_bert_weights(TINY_BERT_ARCH, 77).items()}
     ref = E.bert_encode(sd, E.BertCfg(128, 2, 2, 512, vocab=1000, max_pos=64), torch.from_numpy(ids), torch.from_numpy(mask))
-    _cos_ok(out, ref)
+    K.assert_embeddings_match(out, ref, unit_norm=False)
     # ---- CLIP text tower + byte-level BPE
     corpus = ["a photo of a cat", "a photo of a dog", "the quick brown fox", "hello world, it's me"] * 2
     merges = OT.train_toy_merges(corpus, 300)
@@ -140,7 +119,7 @@ def test_vectorise_with_cxx_tokenizers(gpu_required, tmp_path):
     assert tok_ids.max() < TINY_CLIP_ARCH["text"]["vocab"]
     csd = {k: torch.from_numpy(v) for k, v in Wt.random_clip_weights(TINY_CLIP_ARCH, 5).items()}
     s2.clear_loaded_models()
-    _cos_ok(got, E.clip_encode_text(csd, E.tiny_clip(), torch.from_numpy(tok_ids)))
+    K.assert_embeddings_match(got, E.clip_encode_text(csd, E.tiny_clip(), torch.from_numpy(tok_ids)), unit_norm=False)
 
 
 def _doc(doc_id, fields, embs):

@@ -7,9 +7,9 @@ import pytest
 import torch
 
 import _convnext_oracle as O
+from _checks import assert_embeddings_match, assert_index_search_matches
 
 pytestmark = pytest.mark.gpu
-COS_TOL = 1e-3
 BASE_W, LARGE_D = "open_clip/convnext_base_w/laion2b_s13b_b82k", "open_clip/convnext_large_d/laion2b_s26b_b102k_augreg"
 DIMS = {"base": [128, 256, 512, 1024], "large": [192, 384, 768, 1536], "xxlarge": [384, 768, 1536, 3072]}
 
@@ -20,15 +20,6 @@ def _fp32_oracle():
     torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
     yield
     torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
-
-
-def _check(got, ref):
-    got = torch.as_tensor(np.asarray(got)).cpu()
-    ref = torch.as_tensor(np.asarray(ref.cpu() if hasattr(ref, "cpu") else ref))
-    assert torch.isfinite(got).all()
-    c = torch.nn.functional.cosine_similarity(got.double(), ref.double(), dim=-1)
-    assert float((1 - c).max()) < COS_TOL, f"min cosine {float(c.min())}"
-    assert torch.allclose(got.norm(dim=-1), torch.ones(got.shape[0], dtype=got.dtype), atol=1e-5)
 
 
 def _ln64(y, g, b, eps):
@@ -166,7 +157,7 @@ def test_reduced_depth_tower(gpu_required, name):
         img = np.random.default_rng(3).integers(0, 256, (3, S, S, 3), dtype=np.uint8)
         got = enc.encode_images_u8(img)
         assert got.shape == (3, arch["embed_dim"])
-        _check(got, _ref_images(sd, arch, img))
+        assert_embeddings_match(got, _ref_images(sd, arch, img))
     finally:
         enc.close()
 
@@ -186,7 +177,7 @@ def test_base_w_every_input_path(gpu_required, base_w):
     at_size = rng.integers(0, 256, (40, 256, 256, 3), dtype=np.uint8)
     got = enc.encode_images_u8(at_size)
     rows = [0, 17, 39]
-    _check(got[rows], _ref_images(sd, arch, at_size[rows]))
+    assert_embeddings_match(got[rows], _ref_images(sd, arch, at_size[rows]))
     # device-resident uint8: the same bits
     d_in = torch.from_numpy(at_size).cuda()
     out = torch.empty((40, 640), dtype=torch.float32, device="cuda")
@@ -194,10 +185,10 @@ def test_base_w_every_input_path(gpu_required, base_w):
     np.testing.assert_array_equal(out.cpu().numpy(), got)
     # non-square images through the resize + centre crop
     other = rng.integers(0, 256, (3, 300, 171, 3), dtype=np.uint8)
-    _check(enc.encode_images_u8(other), _ref_images(sd, arch, other))
+    assert_embeddings_match(enc.encode_images_u8(other), _ref_images(sd, arch, other))
     # preprocessed fp32 CHW
     chw = E.clip_preprocess_u8(other, 256)
-    _check(enc.encode_images_f32(chw.numpy()), O.encode_image(sd, arch, chw.cuda()).cpu())
+    assert_embeddings_match(enc.encode_images_f32(chw.numpy()), O.encode_image(sd, arch, chw.cuda()).cpu())
 
 
 def test_base_w_single_image_graph_replay(gpu_required, base_w):
@@ -206,7 +197,7 @@ def test_base_w_single_image_graph_replay(gpu_required, base_w):
     first = enc.encode_images_u8(img)       # eager, then captured, then replayed
     np.testing.assert_array_equal(first, enc.encode_images_u8(img))
     np.testing.assert_array_equal(first, enc.encode_images_u8(img))
-    _check(first, _ref_images(sd, arch, img))
+    assert_embeddings_match(first, _ref_images(sd, arch, img))
 
 
 def _text_ids(n, seed):
@@ -229,7 +220,7 @@ def _text_check(arch, sd, enc, n):
     ids = _text_ids(n, w)
     got = enc.encode_tokens(ids.numpy())
     rows = [0, n // 2, n - 1]
-    _check(got[rows], E.clip_encode_text(tsd, cfg, ids[rows]))
+    assert_embeddings_match(got[rows], E.clip_encode_text(tsd, cfg, ids[rows]))
 
 
 def test_text_at_width_640(gpu_required, base_w):
@@ -257,7 +248,7 @@ def test_full_depth_tower(gpu_required, name):
     try:
         S = arch["convnext"]["image_size"]
         img = np.random.default_rng(4).integers(0, 256, (4, S, S, 3), dtype=np.uint8)
-        _check(enc.encode_images_u8(img), _ref_images(sd, arch, img))
+        assert_embeddings_match(enc.encode_images_u8(img), _ref_images(sd, arch, img))
     finally:
         enc.close()
 
@@ -367,14 +358,8 @@ def test_gemm_at_convnext_layer_shapes(gpu_required, M, N, K, act, out_bf16, res
 # ------------------------------------------------------------------------------------------------------------------
 # Through the seams: vectorise -> GpuTensorIndex -> search
 # ------------------------------------------------------------------------------------------------------------------
-def _doc(doc_id, vec):
-    return {"id": doc_id, "fields": {"marqo__id": doc_id, "marqo__chunks_body": ["c"],
-                                     "marqo__embeddings_body": {"0": vec.tolist()}}}
-
-
 def test_vectorise_base_w_into_index_and_search(gpu_required, score_oracle):
     from marqo_b200 import model_registry as R, s2_inference as s2
-    from marqo_b200.gpu_tensor_index import GpuTensorIndex
     from marqo_b200.s2_inference import Modality
     s2.clear_loaded_models()
     props = dict(R.get_model_properties(BASE_W), random_init=23, max_batch=32)
@@ -387,15 +372,4 @@ def test_vectorise_base_w_into_index_and_search(gpu_required, score_oracle):
     queries = np.asarray(s2.vectorise(BASE_W, images[:3], model_properties=props, device="cuda:0",
                                       normalize_embeddings=True, modality=Modality.IMAGE), np.float32)
     s2.clear_loaded_models()
-    ix = GpuTensorIndex()
-    assert not ix.feed_batch([_doc(f"d{i}", v) for i, v in enumerate(docs)], "s1").errors
-    k = 10
-    yql = (f"select * from s1 where (({{targetHits:{k}, approximate:False, hnsw.exploreAdditionalHits:0}}"
-           f"nearestNeighbor(marqo__embeddings_body, marqo__query_embedding)))")
-    edoc, _, escore = score_oracle.search(queries, docs, k, "prenormalized-angular")
-    for j in range(len(queries)):
-        res = ix.query(yql, hits=k, ranking="embedding_similarity", model_restrict="s1",
-                       query_features={"marqo__query_embedding": queries[j].tolist()})
-        assert [h.id.split("::")[-1] for h in res.hits] == [f"d{d}" for d in edoc[j]]
-        np.testing.assert_allclose([h.relevance for h in res.hits], escore[j], rtol=0, atol=1e-12)
-    ix.close()
+    assert_index_search_matches(score_oracle, docs, queries)

@@ -11,6 +11,7 @@ import math
 import pytest
 import torch
 
+from _checks import bf16
 from marqo_b200 import _native as N
 
 pytestmark = pytest.mark.gpu
@@ -18,11 +19,6 @@ pytestmark = pytest.mark.gpu
 F = torch.nn.functional
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
 CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
-
-
-def _bf16(x: torch.Tensor) -> torch.Tensor:
-    """Round to bf16 (round to nearest even) and back to fp32."""
-    return x.float().to(torch.bfloat16).float()
 
 
 def _assert_within_bf16_ulp(got: torch.Tensor, ref: torch.Tensor) -> None:
@@ -124,7 +120,7 @@ def test_bert_embed_ln(gpu_required, n, S, w, masked):
     e = (word[ids.long()].double() + type0.double()) + pos[:S].double()[None]
     ref = _layer_norm64(e, gamma, beta, eps).reshape(n * S, w)
     torch.testing.assert_close(x.double(), ref, **LN_TOL)
-    assert torch.equal(h, _bf16(x))
+    assert torch.equal(h, bf16(x))
     want = mask.sum(1).to(torch.int32) if masked else torch.full((n,), S, dtype=torch.int32)
     assert torch.equal(torch.from_numpy(kv_len), want)
 
@@ -198,7 +194,7 @@ def test_roberta_embed_ln(gpu_required, n, S, w, type_row, no_pads):
     e = e + pos.double()[p]
     ref = _layer_norm64(e, gamma, beta, eps).reshape(n * S, w)
     torch.testing.assert_close(x.double(), ref, **LN_TOL)
-    assert torch.equal(h, _bf16(x))
+    assert torch.equal(h, bf16(x))
     assert torch.equal(torch.from_numpy(kv_len), mask.sum(1).to(torch.int32))
 
 
@@ -318,7 +314,7 @@ def test_stem_im2col(gpu_required, n, S, u8):
     else:
         chw = torch.randn(n, 3, S, S, generator=g)
         got = torch.from_numpy(debug_stem_im2col(chw.numpy()))
-        assert torch.equal(got, _bf16(_stem_cols(chw)))
+        assert torch.equal(got, bf16(_stem_cols(chw)))
     assert not got[:, 27:].any()
 
 
@@ -329,7 +325,7 @@ def test_avgpool2_nhwc(gpu_required, n, H, W, C):
     """AvgPool2d(2) on NHWC bf16: each output within one bf16 ulp of the fp64 mean of its four bf16 inputs."""
     from marqo_b200.engine import debug_avgpool2
     g = torch.Generator().manual_seed(n + H * W + C)
-    x = _bf16(torch.randn(n, H, W, C, generator=g))
+    x = bf16(torch.randn(n, H, W, C, generator=g))
     got = torch.from_numpy(debug_avgpool2(x.numpy()))
     ref = x.double().view(n, H // 2, 2, W // 2, 2, C).mean(dim=(2, 4))
     _assert_within_bf16_ulp(got, ref)
@@ -343,7 +339,7 @@ def test_attnpool_tokens(gpu_required, n, HW, C):
     ulps."""
     from marqo_b200.engine import debug_attnpool_tokens
     g = torch.Generator().manual_seed(n + HW + C)
-    x = _bf16(4.0 + torch.randn(n, HW, C, generator=g))
+    x = bf16(4.0 + torch.randn(n, HW, C, generator=g))
     pos = torch.randn(HW + 1, C, generator=g)
     got = torch.from_numpy(debug_attnpool_tokens(x.numpy(), pos.numpy()))
     xd, pd = x.double(), pos.double()
@@ -365,4 +361,4 @@ def test_im2col_f32(gpu_required, n, S, p, cls):
     got = torch.from_numpy(debug_im2col_f32(chw.numpy(), p, kpad, cls))
     patches = F.unfold(chw, kernel_size=p, stride=p).transpose(1, 2)   # [n, g*g, K], k = c*p*p + dy*p + dx
     rows = F.pad(patches, (0, kpad - K, cls, 0))                       # zero columns, then zero class rows on top
-    assert torch.equal(got, _bf16(rows.reshape(-1, kpad)))
+    assert torch.equal(got, bf16(rows.reshape(-1, kpad)))

@@ -8,16 +8,13 @@ import math
 import pytest
 import torch
 
+from _checks import bf16
 from marqo_b200._native import GEMM_PERSISTENT
 
 pytestmark = pytest.mark.gpu
 
 SENTINEL = -7.5      # exact in bf16 and fp32
 GUARD_ROWS, GUARD_COLS = 5, 40
-
-
-def _bf16(x: torch.Tensor) -> torch.Tensor:
-    return x.to(torch.bfloat16).to(torch.float32)
 
 
 def _act(z: torch.Tensor, act: int) -> torch.Tensor:
@@ -42,8 +39,8 @@ def _act(z: torch.Tensor, act: int) -> torch.Tensor:
 def test_persistent_gemm_into_buffer(gpu_required, M, N, K, act, out_bf16, residual):
     from marqo_b200.engine import debug_gemm_into
     g = torch.Generator().manual_seed(M * 7 + N + K + act)
-    A = _bf16(torch.randn(M, K, generator=g))
-    W = _bf16(torch.randn(N, K, generator=g) / math.sqrt(K))
+    A = bf16(torch.randn(M, K, generator=g))
+    W = bf16(torch.randn(N, K, generator=g) / math.sqrt(K))
     b = torch.randn(N, generator=g)
     io = torch.full((M + GUARD_ROWS, N + GUARD_COLS), SENTINEL)
     res = torch.randn(M, N, generator=g)

@@ -13,6 +13,7 @@ import math
 import pytest
 import torch
 
+from _checks import bf16
 from marqo_b200 import model_registry
 from marqo_b200._native import GEMM_128x128, GEMM_PERSISTENT
 
@@ -33,10 +34,6 @@ def sm_count(gpu_required):
     return n
 
 
-def _bf16(x: torch.Tensor) -> torch.Tensor:
-    return x.to(torch.bfloat16).to(torch.float32)
-
-
 def _act(z: torch.Tensor, act: int) -> torch.Tensor:
     if act == GELU:
         return 0.5 * z * (1.0 + torch.erf(z / math.sqrt(2.0)))
@@ -50,8 +47,8 @@ def _run(M, N, K, act, out_bf16, residual, sms, seed, bias=True, alt_sms=None):
     of the same inputs with SM count alt_sms when given."""
     from marqo_b200.engine import debug_gemm_into
     g = torch.Generator().manual_seed(seed)
-    A = _bf16(torch.randn(M, K, generator=g))
-    W = _bf16(torch.randn(N, K, generator=g) / math.sqrt(K))
+    A = bf16(torch.randn(M, K, generator=g))
+    W = bf16(torch.randn(N, K, generator=g) / math.sqrt(K))
     b = torch.randn(N, generator=g) if bias else None
     io = torch.full((M + GUARD_ROWS, N + GUARD_COLS), SENTINEL)
     res = torch.randn(M, N, generator=g)

@@ -6,11 +6,9 @@ import numpy as np
 import pytest
 import torch
 
+from _checks import bf16
+
 pytestmark = pytest.mark.gpu
-
-
-def _bf16(x: torch.Tensor) -> torch.Tensor:
-    return x.to(torch.bfloat16).to(torch.float32)
 
 
 @pytest.mark.parametrize("M,N,K", [
@@ -20,8 +18,8 @@ def _bf16(x: torch.Tensor) -> torch.Tensor:
 def test_gemm_matches_torch(gpu_required, M, N, K):
     from marqo_b200.engine import debug_gemm
     g = torch.Generator().manual_seed(M + N + K)
-    A = _bf16(torch.randn(M, K, generator=g))
-    W = _bf16(torch.randn(N, K, generator=g) / math.sqrt(K))
+    A = bf16(torch.randn(M, K, generator=g))
+    W = bf16(torch.randn(N, K, generator=g) / math.sqrt(K))
     bias = torch.randn(N, generator=g)
     ref = A @ W.t() + bias
     got = torch.from_numpy(debug_gemm(A.numpy(), W.numpy(), bias.numpy()))
@@ -33,8 +31,8 @@ def test_gemm_epilogues(gpu_required, act):
     from marqo_b200.engine import debug_gemm
     g = torch.Generator().manual_seed(act)
     M, N, K = 333, 1024, 256
-    A = _bf16(torch.randn(M, K, generator=g))
-    W = _bf16(torch.randn(N, K, generator=g) / math.sqrt(K))
+    A = bf16(torch.randn(M, K, generator=g))
+    W = bf16(torch.randn(N, K, generator=g) / math.sqrt(K))
     bias = torch.randn(N, generator=g)
     res = torch.randn(M, N, generator=g)
     z = A @ W.t() + bias
@@ -57,8 +55,8 @@ def test_gemm_fused_layernorm(gpu_required, M, N, K, in_place):
     """The residual GEMM followed by the LayerNorm launch of the encoder layers (out_proj / fc2 -> ln), vs torch."""
     from marqo_b200.engine import debug_gemm_ln
     g = torch.Generator().manual_seed(M + N + K)
-    A = _bf16(torch.randn(M, K, generator=g))
-    W = _bf16(torch.randn(N, K, generator=g) / math.sqrt(K))
+    A = bf16(torch.randn(M, K, generator=g))
+    W = bf16(torch.randn(N, K, generator=g) / math.sqrt(K))
     bias = torch.randn(N, generator=g)
     res = torch.randn(M, N, generator=g)
     gamma = 1.0 + 0.1 * torch.randn(N, generator=g)
@@ -89,14 +87,14 @@ def test_patch_embed_token_rows_match_conv(gpu_required, n, S, patch, N):
     g = torch.Generator().manual_seed(n * 31 + patch)
     img = torch.randint(0, 256, (n, S, S, 3), generator=g, dtype=torch.uint8)
     K = 3 * patch * patch
-    w = _bf16(torch.randn(N, 3, patch, patch, generator=g) / math.sqrt(K))
+    w = bf16(torch.randn(N, 3, patch, patch, generator=g) / math.sqrt(K))
     G = (S // patch) ** 2
     pos = torch.randn(G + 1, N, generator=g)
     cls = torch.randn(N, generator=g)
     mean = torch.tensor([0.48145466, 0.4578275, 0.40821073])
     std = torch.tensor([0.26862954, 0.26130258, 0.27577711])
     x = (img.permute(0, 3, 1, 2).float() / 255.0 - mean[None, :, None, None]) / std[None, :, None, None]
-    ref = torch.nn.functional.conv2d(_bf16(x).double(), w.double(), stride=patch)       # [n, N, g, g]
+    ref = torch.nn.functional.conv2d(bf16(x).double(), w.double(), stride=patch)       # [n, N, g, g]
     ref = ref.flatten(2).transpose(1, 2) + pos[None, 1:, :].double()                      # [n, G, N]
     got = torch.from_numpy(debug_patch_embed(img.numpy(), patch, w.numpy(), mean.numpy(), std.numpy(), pos.numpy(),
                                              cls=cls.numpy()))
@@ -122,7 +120,7 @@ def test_attention_matches_torch(gpu_required, B, S, H, mask):
     from marqo_b200.engine import debug_attention
     g = torch.Generator().manual_seed(B * 1000 + S)
     W = H * 64
-    qkv = _bf16(torch.randn(B * S, 3 * W, generator=g))
+    qkv = bf16(torch.randn(B * S, 3 * W, generator=g))
     kv_len = None
     if mask == 2:
         kv_len = torch.randint(1, S + 1, (B,), generator=g).to(torch.int32)
@@ -148,7 +146,7 @@ def test_attention_peaked_scores(gpu_required, B, S, H, mask):
     W = H * 64
     qkv = torch.randn(B * S, 3 * W, generator=g)
     qkv[:, : 2 * W] *= 3.0                                          # q and k: score std 9, extremes beyond 40
-    qkv = _bf16(qkv)
+    qkv = bf16(qkv)
     kv_len = None
     if mask == 2:
         kv_len = torch.randint(1, S + 1, (B,), generator=g).to(torch.int32)
@@ -228,7 +226,7 @@ def test_layernorm_matches_torch(gpu_required, rows, w, eps, variant):
     got = torch.from_numpy(got)
     torch.testing.assert_close(got.double(), ref, **tol)
     if got_b is not None:
-        assert torch.equal(torch.from_numpy(got_b), _bf16(got))
+        assert torch.equal(torch.from_numpy(got_b), bf16(got))
 
 
 @pytest.mark.parametrize("h,w", [(480, 640), (640, 480), (224, 224), (300, 224), (256, 256), (1000, 750), (225, 400), (100, 150)])

@@ -7,15 +7,11 @@ import numpy as np
 import pytest
 import torch
 
+import _checks as K
 import _mpnet_oracle as M
 
 pytestmark = pytest.mark.gpu
-COS_TOL = 1e-3
 BASE = M.MPNET_BASE
-
-
-def _bf16(x):
-    return x.to(torch.bfloat16).to(torch.float32)
 
 
 def _attention_ref(qkv, B, S, H, kv_len, bias):
@@ -38,7 +34,7 @@ def test_attention_rel_bias_matches_torch(gpu_required, S, peaked):
     qkv = torch.randn(B * S, 3 * H * 64, generator=g)
     if peaked:
         qkv[:, : 2 * H * 64] *= 3.0                                  # score std 9: one key dominates most rows
-    qkv = _bf16(qkv)
+    qkv = K.bf16(qkv)
     bias = (torch.rand(H, 2 * smax - 1, generator=g) * 40 - 20) if peaked else torch.randn(H, 2 * smax - 1, generator=g)
     kv_len = torch.randint(1, S + 1, (B,), generator=g).to(torch.int32)
     kv_len[0] = S
@@ -61,14 +57,6 @@ def test_attention_rel_bias_refuses_longer_sequences_than_the_table(gpu_required
 # ------------------------------------------------------------------------------------------------------------------
 # The encoder through the C ABI vs the CPU fp32 oracle on the same seeded weights
 # ------------------------------------------------------------------------------------------------------------------
-def _check(got, ref):
-    got = torch.from_numpy(np.asarray(got))
-    assert torch.isfinite(got).all()
-    c = torch.nn.functional.cosine_similarity(got.double(), torch.as_tensor(np.asarray(ref)).double(), dim=-1)
-    assert float((1 - c).max()) < COS_TOL, f"min cosine {float(c.min())}"
-    assert torch.allclose(got.norm(dim=-1), torch.ones(got.shape[0], dtype=got.dtype), atol=1e-5)
-
-
 def _ids(g, B, S, lens=None):
     ids = torch.randint(5, 30000, (B, S), generator=g)
     ids[:, 0] = 0
@@ -98,7 +86,7 @@ def test_mpnet_base_batch_256_ragged(gpu_required, base_weights):
     got = enc.encode_tokens(ids.numpy(), mask.numpy())
     assert got.shape == (256, 768)
     pos = [0, 1, 37, 100, 200, 254, 255]
-    _check(got[pos], M.mpnet_encode(base_weights, BASE, ids[pos], mask[pos]))
+    K.assert_embeddings_match(got[pos], M.mpnet_encode(base_weights, BASE, ids[pos], mask[pos]))
     enc.close()
 
 
@@ -111,7 +99,7 @@ def test_mpnet_base_512_tokens_and_513_refused(gpu_required, base_weights):
     ids, mask = _ids(g, 8, 512, [512, 200, 312, 256, 1, 511, 256, 300])
     got = enc.encode_tokens(ids.numpy(), mask.numpy())
     sel = [0, 1, 4, 5]
-    _check(got[sel], M.mpnet_encode(base_weights, BASE, ids[sel], mask[sel]))
+    K.assert_embeddings_match(got[sel], M.mpnet_encode(base_weights, BASE, ids[sel], mask[sel]))
     with pytest.raises(NativeError) as ei:
         enc.encode_tokens(np.zeros((1, 513), np.int32))
     assert ei.value.code == ERR_INVALID_ARG
@@ -125,7 +113,8 @@ def test_mpnet_base_single_query_graph_replay(gpu_required, base_weights):
     g = torch.Generator().manual_seed(2)
     for i in range(3):
         ids, mask = _ids(g, 1, 16, [16 - 3 * i])
-        _check(enc.encode_tokens(ids.numpy(), mask.numpy()), M.mpnet_encode(base_weights, BASE, ids, mask))
+        K.assert_embeddings_match(enc.encode_tokens(ids.numpy(), mask.numpy()),
+                                  M.mpnet_encode(base_weights, BASE, ids, mask))
     enc.close()
 
 
@@ -147,10 +136,9 @@ def test_golden_vectors_through_the_c_abi(gpu_required):
     z = np.load(Path(__file__).resolve().parent / "golden" / "mpnet_golden.npz")
     cfg = M.tiny_mpnet()
     enc = Encoder("mpnet", M.engine_config(cfg), M.make_mpnet_weights(cfg, seed=int(z["seed"])), max_batch=8)
-    _check(enc.encode_tokens(z["ids"], z["mask"]), z["vec"])
+    K.assert_embeddings_match(enc.encode_tokens(z["ids"], z["mask"]), z["vec"])
     un = enc.encode_tokens(z["ids"], z["mask"], normalize=False)
-    c = torch.nn.functional.cosine_similarity(torch.from_numpy(un).double(), torch.from_numpy(z["vec_unnormalized"]).double())
-    assert float((1 - c).max()) < COS_TOL
+    K.assert_embeddings_match(un, z["vec_unnormalized"], unit_norm=False)
     np.testing.assert_allclose(np.linalg.norm(un, axis=1), np.linalg.norm(z["vec_unnormalized"], axis=1), rtol=1e-2)
     enc.close()
 
@@ -158,15 +146,9 @@ def test_golden_vectors_through_the_c_abi(gpu_required):
 # ------------------------------------------------------------------------------------------------------------------
 # Through the seams: vectorise("hf/all-mpnet-base-v2") with the C++ tokenizer -> GpuTensorIndex -> search
 # ------------------------------------------------------------------------------------------------------------------
-def _doc(doc_id, vec):
-    return {"id": doc_id, "fields": {"marqo__id": doc_id, "marqo__chunks_body": ["c"],
-                                     "marqo__embeddings_body": {"0": vec.tolist()}}}
-
-
 def test_vectorise_mpnet_into_index_and_search(gpu_required, score_oracle, monkeypatch, tmp_path):
     from transformers import MPNetTokenizer as HF
     from marqo_b200 import model_registry as R, s2_inference as s2, weights as Wt
-    from marqo_b200.gpu_tensor_index import GpuTensorIndex
     s2.clear_loaded_models()
     vf = tmp_path / "vocab.txt"
     vocab = M.synthetic_vocab(30527)
@@ -188,23 +170,12 @@ def test_vectorise_mpnet_into_index_and_search(gpu_required, score_oracle, monke
     for i in range(0, 64, 16):                                           # the reference pads per sub-batch
         t = hf(sentences[i:i + 16], padding=True, truncation=True, max_length=props["tokens"], return_tensors="pt")
         ref.append(M.mpnet_encode(sd, BASE, t["input_ids"], t["attention_mask"]))
-    _check(docs, torch.cat(ref))
+    K.assert_embeddings_match(docs, torch.cat(ref))
     queries = [" ".join(words[int(x)] for x in rng.integers(0, len(words), size=n)) for n in (3, 8, 14)]
     q = np.asarray(s2.vectorise(name, queries, model_properties=props, device="cuda:0", normalize_embeddings=True),
                    np.float32)
     t = hf(queries, padding=True, truncation=True, max_length=props["tokens"], return_tensors="pt")
-    _check(q, M.mpnet_encode(sd, BASE, t["input_ids"], t["attention_mask"]))
+    K.assert_embeddings_match(q, M.mpnet_encode(sd, BASE, t["input_ids"], t["attention_mask"]))
     s2.clear_loaded_models()
 
-    ix = GpuTensorIndex()
-    assert not ix.feed_batch([_doc(f"d{i}", v) for i, v in enumerate(docs)], "s1").errors
-    k = 10
-    yql = (f"select * from s1 where (({{targetHits:{k}, approximate:False, hnsw.exploreAdditionalHits:0}}"
-           f"nearestNeighbor(marqo__embeddings_body, marqo__query_embedding)))")
-    edoc, _, escore = score_oracle.search(q, docs, k, "prenormalized-angular")
-    for j in range(len(queries)):
-        res = ix.query(yql, hits=k, ranking="embedding_similarity", model_restrict="s1",
-                       query_features={"marqo__query_embedding": q[j].tolist()})
-        assert [h.id.split("::")[-1] for h in res.hits] == [f"d{d}" for d in edoc[j]]
-        np.testing.assert_allclose([h.relevance for h in res.hits], escore[j], rtol=0, atol=1e-12)
-    ix.close()
+    K.assert_index_search_matches(score_oracle, docs, q)

@@ -8,10 +8,10 @@ import numpy as np
 import pytest
 import torch
 
+import _checks as K
 import _resnet_oracle as O
 
 pytestmark = pytest.mark.gpu
-COS_TOL = 1e-3
 RN50, RN101 = "open_clip/RN50/openai", "open_clip/RN101/openai"
 
 
@@ -21,19 +21,6 @@ def _fp32_oracle():
     torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
     yield
     torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
-
-
-def _check(got, ref):
-    got = torch.as_tensor(np.asarray(got)).cpu()
-    ref = torch.as_tensor(np.asarray(ref.cpu() if hasattr(ref, "cpu") else ref))
-    assert torch.isfinite(got).all()
-    c = torch.nn.functional.cosine_similarity(got.double(), ref.double(), dim=-1)
-    assert float((1 - c).max()) < COS_TOL, f"min cosine {float(c.min())}"
-    assert torch.allclose(got.norm(dim=-1), torch.ones(got.shape[0], dtype=got.dtype), atol=1e-5)
-
-
-def _bf16(x):
-    return x.to(torch.bfloat16).to(torch.float32)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -69,7 +56,7 @@ def test_conv2d_matches_torch(gpu_required, cin, cout, k, H):
     w = torch.randn(cout, cin, k, k, generator=g) / (cin * k * k) ** 0.5
     b = torch.randn(cout, generator=g) * 0.1
     Ho = H // 2 if cin == 3 else H
-    xd, wd = _bf16(x).cuda().double(), _bf16(w).cuda().double()
+    xd, wd = K.bf16(x).cuda().double(), K.bf16(w).cuda().double()
     conv = torch.nn.functional.conv2d(xd.permute(0, 3, 1, 2), wd, stride=2 if cin == 3 else 1, padding=k // 2)
     conv = conv.permute(0, 2, 3, 1) + b.cuda().double()
     scale = float(conv.abs().max())
@@ -81,7 +68,7 @@ def test_conv2d_matches_torch(gpu_required, cin, cout, k, H):
     for relu, res in cases:
         got = torch.from_numpy(debug_conv2d(x.numpy(), w.numpy(), b.numpy(), None if res is None else res.numpy(),
                                             relu=relu)).cuda()
-        ref = conv + (_bf16(res).cuda().double() if res is not None else 0)
+        ref = conv + (K.bf16(res).cuda().double() if res is not None else 0)
         if relu:
             ref = torch.relu(ref)
         assert torch.isfinite(got).all()
@@ -100,7 +87,7 @@ def test_conv3x3_halo_on_every_border(gpu_required):
     w = np.random.default_rng(0).standard_normal((cout, cin, 3, 3)).astype(np.float32)
     got = debug_conv2d(x, w, relu=True)
     ref = torch.relu(torch.nn.functional.conv2d(torch.from_numpy(x).permute(0, 3, 1, 2).double(),
-                                                _bf16(torch.from_numpy(w)).double(), padding=1).permute(0, 2, 3, 1))
+                                                K.bf16(torch.from_numpy(w)).double(), padding=1).permute(0, 2, 3, 1))
     assert not got[0].any()
     torch.testing.assert_close(torch.from_numpy(got).double(), ref, rtol=2 ** -7, atol=1e-2)
 
@@ -111,7 +98,7 @@ def test_map_attention_per_image_queries(gpu_required, B):
     g = torch.Generator().manual_seed(B)
     H, W, S = 32, 2048, 50
     q = torch.randn(B, W, generator=g) * 2.0
-    kv = _bf16(torch.randn(B * S, 2 * W, generator=g))
+    kv = K.bf16(torch.randn(B * S, 2 * W, generator=g))
     got = torch.from_numpy(debug_map_attention(q.numpy(), kv.numpy(), B, S, H))
     k, v = kv.double().view(B, S, 2, H, 64).permute(2, 0, 3, 1, 4)
     att = (q.double().view(B, H, 1, 64) @ k.transpose(-1, -2)) / 8.0
@@ -155,7 +142,7 @@ def test_rn50_batch_256_every_input_path(gpu_required, rn50):
     rng = np.random.default_rng(1)
     at_size = rng.integers(0, 256, (256, 224, 224, 3), dtype=np.uint8)
     got = enc.encode_images_u8(at_size)
-    _check(got[ROWS], _ref_images(sd, arch, at_size[ROWS]))
+    K.assert_embeddings_match(got[ROWS], _ref_images(sd, arch, at_size[ROWS]))
     # device-resident, aligned and starting 1 byte past a 16-byte boundary: the same bits
     n_bytes = at_size.nbytes
     raw = torch.empty(n_bytes + 32, dtype=torch.uint8, device="cuda")
@@ -169,11 +156,11 @@ def test_rn50_batch_256_every_input_path(gpu_required, rn50):
         np.testing.assert_array_equal(out.cpu().numpy(), got)
     # non-square images through the resize + centre crop
     other = rng.integers(0, 256, (6, 300, 171, 3), dtype=np.uint8)
-    _check(enc.encode_images_u8(other), _ref_images(sd, arch, other))
+    K.assert_embeddings_match(enc.encode_images_u8(other), _ref_images(sd, arch, other))
     # preprocessed fp32 CHW
     from oracle import encoders as E
     chw = E.clip_preprocess_u8(other[:3])
-    _check(enc.encode_images_f32(chw.numpy()), O.encode_image(sd, arch, chw.cuda()).cpu())
+    K.assert_embeddings_match(enc.encode_images_f32(chw.numpy()), O.encode_image(sd, arch, chw.cuda()).cpu())
 
 
 def test_rn50_single_image_graph_replay(gpu_required, rn50):
@@ -182,7 +169,7 @@ def test_rn50_single_image_graph_replay(gpu_required, rn50):
     first = enc.encode_images_u8(img)       # eager, then captured, then replayed
     np.testing.assert_array_equal(first, enc.encode_images_u8(img))
     np.testing.assert_array_equal(first, enc.encode_images_u8(img))
-    _check(first, _ref_images(sd, arch, img))
+    K.assert_embeddings_match(first, _ref_images(sd, arch, img))
 
 
 @pytest.mark.parametrize("n", [256, 1])
@@ -202,7 +189,7 @@ def test_rn50_text(gpu_required, rn50, n):
     rows = [r for r in ROWS if r < n]
     for _ in range(3 if n == 1 else 1):
         got = enc.encode_tokens(ids.numpy())
-        _check(got[rows], E.clip_encode_text(tsd, cfg, ids[rows]))
+        K.assert_embeddings_match(got[rows], E.clip_encode_text(tsd, cfg, ids[rows]))
 
 
 def test_rn101_batch_16(gpu_required):
@@ -215,7 +202,7 @@ def test_rn101_batch_16(gpu_required):
         img = np.random.default_rng(101).integers(0, 256, (16, 224, 224, 3), dtype=np.uint8)
         got = enc.encode_images_u8(img)
         assert got.shape == (16, 512)
-        _check(got[[0, 7, 15]], _ref_images(sd, arch, img[[0, 7, 15]]))
+        K.assert_embeddings_match(got[[0, 7, 15]], _ref_images(sd, arch, img[[0, 7, 15]]))
     finally:
         enc.close()
 
@@ -223,14 +210,8 @@ def test_rn101_batch_16(gpu_required):
 # ------------------------------------------------------------------------------------------------------------------
 # Through the seams: vectorise("open_clip/RN50/openai") -> GpuTensorIndex -> search
 # ------------------------------------------------------------------------------------------------------------------
-def _doc(doc_id, vec):
-    return {"id": doc_id, "fields": {"marqo__id": doc_id, "marqo__chunks_body": ["c"],
-                                     "marqo__embeddings_body": {"0": vec.tolist()}}}
-
-
 def test_vectorise_rn50_into_index_and_search(gpu_required, score_oracle):
     from marqo_b200 import model_registry as R, s2_inference as s2
-    from marqo_b200.gpu_tensor_index import GpuTensorIndex
     from marqo_b200.s2_inference import Modality
     s2.clear_loaded_models()
     props = dict(R.get_model_properties(RN50), random_init=23)
@@ -243,15 +224,4 @@ def test_vectorise_rn50_into_index_and_search(gpu_required, score_oracle):
     queries = np.asarray(s2.vectorise(RN50, images[:3], model_properties=props, device="cuda:0",
                                       normalize_embeddings=True, modality=Modality.IMAGE), np.float32)
     s2.clear_loaded_models()
-    ix = GpuTensorIndex()
-    assert not ix.feed_batch([_doc(f"d{i}", v) for i, v in enumerate(docs)], "s1").errors
-    k = 10
-    yql = (f"select * from s1 where (({{targetHits:{k}, approximate:False, hnsw.exploreAdditionalHits:0}}"
-           f"nearestNeighbor(marqo__embeddings_body, marqo__query_embedding)))")
-    edoc, _, escore = score_oracle.search(queries, docs, k, "prenormalized-angular")
-    for j in range(len(queries)):
-        res = ix.query(yql, hits=k, ranking="embedding_similarity", model_restrict="s1",
-                       query_features={"marqo__query_embedding": queries[j].tolist()})
-        assert [h.id.split("::")[-1] for h in res.hits] == [f"d{d}" for d in edoc[j]]
-        np.testing.assert_allclose([h.relevance for h in res.hits], escore[j], rtol=0, atol=1e-12)
-    ix.close()
+    K.assert_index_search_matches(score_oracle, docs, queries)

@@ -8,22 +8,9 @@ fail it go through a threshold-collect pass.  These tests build inputs that fail
 import numpy as np
 import pytest
 
+import _checks as K
+
 pytestmark = pytest.mark.gpu
-
-
-def _unit_rows(rng, n, d):
-    x = rng.standard_normal((n, d)).astype(np.float32)
-    x /= np.linalg.norm(x, axis=1, keepdims=True)
-    return x
-
-
-def _check(store, so, q, corpus, k, metric="prenormalized-angular", doc_of_row=None, **kw):
-    doc, row, score = store.search(q, k, **kw)
-    edoc, erow, escore = so.search(q, corpus, k, metric, doc_of_row)
-    np.testing.assert_array_equal(doc, edoc)
-    np.testing.assert_array_equal(row, erow)
-    np.testing.assert_allclose(score, escore, rtol=0, atol=1e-12)
-    return doc, row, score
 
 
 def _ulp_family(base: np.ndarray, count: int, rng) -> np.ndarray:
@@ -47,21 +34,21 @@ def test_many_identical_rows_with_permuted_documents(gpu_required, score_oracle)
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(1)
     n, d = 40000, 256
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     dup_rows = rng.choice(n, size=40, replace=False)
     corpus[dup_rows] = corpus[dup_rows[0]]
     doc_of_row = rng.permutation(n).astype(np.int32)             # one chunk per document, shuffled numbering
-    q = _unit_rows(rng, 9, d)
+    q = K.unit_rows(rng, 9, d)
     q[0] = corpus[dup_rows[0]]
     store = RowStore(d)
     store.add(corpus, doc_of_row)
-    doc, _, score = _check(store, score_oracle, q, corpus, 10, doc_of_row=doc_of_row)
+    doc, _, score = K.assert_topk_equal(store.search(q, 10), score_oracle.search(q, corpus, 10, doc_of_row=doc_of_row))
     assert list(doc[0]) == sorted(doc_of_row[dup_rows])[:10]
     assert np.all(score[0] == score[0, 0])
     # 40 ties still fit the 64 candidates the merge re-scores exactly: answered in one pass, provably (guard held)
     assert store.search_stats()["flagged"] == 0
     for k in (1, 16, 39, 40, 41, 64):
-        _check(store, score_oracle, q, corpus, k, doc_of_row=doc_of_row)
+        K.assert_topk_equal(store.search(q, k), score_oracle.search(q, corpus, k, doc_of_row=doc_of_row))
     # 150 ties do not: the guard must notice (exact k-th key == bound of the unexamined rows) and the collect pass answer
     more = rng.choice(n, size=150, replace=False)
     corpus2 = corpus.copy()
@@ -70,12 +57,13 @@ def test_many_identical_rows_with_permuted_documents(gpu_required, score_oracle)
     q2[0] = corpus2[more[0]]
     store2 = RowStore(d)
     store2.add(corpus2, doc_of_row)
-    doc2, _, _ = _check(store2, score_oracle, q2, corpus2, 10, doc_of_row=doc_of_row)
+    doc2, _, _ = K.assert_topk_equal(store2.search(q2, 10),
+                                     score_oracle.search(q2, corpus2, 10, doc_of_row=doc_of_row))
     assert list(doc2[0]) == sorted(doc_of_row[more])[:10]
     st = store2.search_stats()
     assert st["flagged"] >= 1 and st["collect_passes"] >= 1
     for k in (64, 100, 149, 150, 151):
-        _check(store2, score_oracle, q2, corpus2, k, doc_of_row=doc_of_row)
+        K.assert_topk_equal(store2.search(q2, k), score_oracle.search(q2, corpus2, k, doc_of_row=doc_of_row))
 
 
 @pytest.mark.parametrize("spread", ["one_tile", "all_over"])
@@ -84,21 +72,21 @@ def test_near_ties_around_rank_k(gpu_required, score_oracle, spread):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(2)
     n, d = 60000, 768
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     base = corpus[77].copy()
     fam = _ulp_family(base, 30, rng)
     rows = np.arange(5000, 5030) if spread == "one_tile" else rng.choice(n, size=30, replace=False)
     corpus[rows] = fam
-    q = _unit_rows(rng, 5, d)
+    q = K.unit_rows(rng, 5, d)
     q[0] = base
     store = RowStore(d)
     store.add(corpus)
-    doc, _, score = _check(store, score_oracle, q, corpus, 10)
+    doc, _, score = K.assert_topk_equal(store.search(q, 10), score_oracle.search(q, corpus, 10))
     top = score[0]
     assert set(doc[0]).issubset(set(rows.tolist()) | {77})
     assert np.all(np.diff(top) <= 0) and (top[0] - top[-1]) < 1e-6       # really a near-tie cluster
     for k in (3, 16, 25):
-        _check(store, score_oracle, q, corpus, k)
+        K.assert_topk_equal(store.search(q, k), score_oracle.search(q, corpus, k))
 
 
 def test_near_tied_chunks_of_one_document(gpu_required, score_oracle):
@@ -107,18 +95,18 @@ def test_near_tied_chunks_of_one_document(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(3)
     n, d = 20000, 512
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     doc_of_row = (np.arange(n) // 4).astype(np.int32)
     base = corpus[4000].copy()
     fam = _ulp_family(base, 24, rng)
     corpus[4000:4004] = fam[:4]                                  # doc 1000: four chunks within 1e-8
     corpus[8000:8020] = fam[4:]                                  # docs 2000..2004: twenty more
-    q = _unit_rows(rng, 6, d)
+    q = K.unit_rows(rng, 6, d)
     q[0] = base
     store = RowStore(d)
     store.add(corpus, doc_of_row)
     for k in (1, 5, 10, 30):
-        _check(store, score_oracle, q, corpus, k, doc_of_row=doc_of_row)
+        K.assert_topk_equal(store.search(q, k), score_oracle.search(q, corpus, k, doc_of_row=doc_of_row))
 
 
 def test_ties_across_a_shard_boundary(gpu_required, score_oracle):
@@ -127,12 +115,12 @@ def test_ties_across_a_shard_boundary(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(4)
     n, d, nq, k = 30000, 256, 4, 10
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     base = corpus[5].copy()
     rows = np.concatenate([np.arange(100, 112), np.arange(20000, 20012)])
     corpus[rows] = _ulp_family(base, 24, rng)
     corpus[25000:25004] = base                                   # exact duplicates in the second shard
-    q = _unit_rows(rng, nq, d)
+    q = K.unit_rows(rng, nq, d)
     q[0] = base
     cut = 15000
     shards = [RowStore(d), RowStore(d)]
@@ -161,9 +149,9 @@ def test_async_entry_point_runs_the_fallback_without_host_help(gpu_required, sco
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(5)
     n, d, nq, k = 30000, 128, 8, 10
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     corpus[1000:1030] = corpus[3]
-    q = _unit_rows(rng, nq, d)
+    q = K.unit_rows(rng, nq, d)
     q[0] = corpus[3]
     store = RowStore(d)
     store.add(corpus)
@@ -186,23 +174,23 @@ def test_large_k(gpu_required, score_oracle, k):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(k)
     n, d = 100000, 128
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     corpus[100:140] = corpus[5]                                   # a run of exact ties
     doc_of_row = (np.arange(n) // 2).astype(np.int32)            # 2 chunks per doc
-    q = _unit_rows(rng, 7, d)
+    q = K.unit_rows(rng, 7, d)
     q[0] = corpus[5]
     store = RowStore(d)
     store.add(corpus, doc_of_row)
-    _check(store, score_oracle, q[1:], corpus, k, doc_of_row=doc_of_row)
+    K.assert_topk_equal(store.search(q[1:], k), score_oracle.search(q[1:], corpus, k, doc_of_row=doc_of_row))
     st = store.search_stats()
     if k <= 160:
         assert st["flagged"] == 0, st                             # single pass: nothing needed the fallback
-    _check(store, score_oracle, q, corpus, k, doc_of_row=doc_of_row)
+    K.assert_topk_equal(store.search(q, k), score_oracle.search(q, corpus, k, doc_of_row=doc_of_row))
     small = RowStore(d)
     small.add(corpus[:30])                                        # fewer documents than k
     doc, _, _ = small.search(q[:2], k)
     assert (doc[:, :30] >= 0).all() and (doc[:, 30:] == -1).all()
-    _check(small, score_oracle, q[:2], corpus[:30], k)
+    K.assert_topk_equal(small.search(q[:2], k), score_oracle.search(q[:2], corpus[:30], k))
 
 
 def test_document_filter_bitset(gpu_required, score_oracle):
@@ -210,10 +198,10 @@ def test_document_filter_bitset(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(7)
     n, d = 50000, 256
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     doc_of_row = (np.arange(n) // 2).astype(np.int32)
     ndocs = n // 2
-    q = _unit_rows(rng, 12, d)
+    q = K.unit_rows(rng, 12, d)
     for frac in (0.5, 0.01, 0.0002, 0.0):
         keep = rng.random(ndocs) < frac
         bits = np.packbits(keep, bitorder="little").view(np.uint8)
@@ -227,21 +215,24 @@ def test_document_filter_bitset(gpu_required, score_oracle):
                 b2 = np.packbits(keep_r, bitorder="little")
                 b2 = np.concatenate([b2, np.zeros((-len(b2)) % 4, np.uint8)]).view(np.uint32)
                 m2 = np.where(keep_r, np.arange(n), -1).astype(np.int32)
-                _check(store, score_oracle, q, corpus, 10, doc_of_row=m2, filter_bits=b2, filter_docs=n, filter_tag=11)
-                _check(store, score_oracle, q, corpus, 10, doc_of_row=m2, filter_bits=b2, filter_docs=n, filter_tag=11)
+                for _ in range(2):
+                    K.assert_topk_equal(store.search(q, 10, filter_bits=b2, filter_docs=n, filter_tag=11),
+                                        score_oracle.search(q, corpus, 10, doc_of_row=m2))
             else:
                 store.add(corpus, store_docs)
-                _check(store, score_oracle, q, corpus, 10, doc_of_row=masked, filter_bits=bits, filter_docs=ndocs)
-                _check(store, score_oracle, q, corpus, 200, doc_of_row=masked, filter_bits=bits, filter_docs=ndocs)
-            _check(store, score_oracle, q, corpus, 10, doc_of_row=store_docs)   # and the filter is gone afterwards
+                for k in (10, 200):
+                    K.assert_topk_equal(store.search(q, k, filter_bits=bits, filter_docs=ndocs),
+                                        score_oracle.search(q, corpus, k, doc_of_row=masked))
+            # and the filter is gone afterwards
+            K.assert_topk_equal(store.search(q, 10), score_oracle.search(q, corpus, 10, doc_of_row=store_docs))
 
 
 def test_filter_with_modifiers(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(8)
     n, d = 20000, 128
-    corpus = _unit_rows(rng, n, d)
-    q = _unit_rows(rng, 5, d)
+    corpus = K.unit_rows(rng, n, d)
+    q = K.unit_rows(rng, 5, d)
     store = RowStore(d)
     store.add(corpus)
     vals = rng.uniform(0.5, 2.0, size=n)
@@ -250,36 +241,35 @@ def test_filter_with_modifiers(gpu_required, score_oracle):
     bits = np.packbits(keep, bitorder="little")
     bits = np.concatenate([bits, np.zeros((-len(bits)) % 4, np.uint8)]).view(np.uint32)
     mod = score_oracle.modifiers(vals[None, :], [(0, 1.5)], [(0, 0.01)])
-    doc, row, score = store.search(q, 10, mult=[(0, 1.5)], add=[(0, 0.01)], filter_bits=bits, filter_docs=n)
     masked = np.where(keep, np.arange(n), -1).astype(np.int32)
-    ed, er, es = score_oracle.search_modified(q, corpus, 10, mod, doc_of_row=masked)
-    np.testing.assert_array_equal(doc, ed)
-    np.testing.assert_array_equal(row, er)
-    np.testing.assert_allclose(score, es, rtol=0, atol=1e-12)
+    K.assert_topk_equal(store.search(q, 10, mult=[(0, 1.5)], add=[(0, 0.01)], filter_bits=bits, filter_docs=n),
+                        score_oracle.search_modified(q, corpus, 10, mod, doc_of_row=masked))
 
 
 def test_delete_rows_and_compact(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(9)
     n, d = 12000, 128
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     doc_of_row = (np.arange(n) // 3).astype(np.int32)
-    q = _unit_rows(rng, 10, d)
+    q = K.unit_rows(rng, 10, d)
     store = RowStore(d, metric="euclidean")
     store.add(corpus, doc_of_row)
     dead = rng.choice(n, size=5000, replace=False)
     store.delete_rows(dead)
     masked = doc_of_row.copy()
     masked[dead] = -1
-    _check(store, score_oracle, q, corpus, 10, metric="euclidean", doc_of_row=masked)
+    K.assert_topk_equal(store.search(q, 10), score_oracle.search(q, corpus, 10, metric="euclidean", doc_of_row=masked))
     new_of_old = store.compact()
     assert len(store) == n - 5000 and (new_of_old[dead] == -1).all()
     live = np.flatnonzero(masked >= 0)
     assert np.array_equal(new_of_old[live], np.arange(len(live)))
-    _check(store, score_oracle, q, corpus[live], 10, metric="euclidean", doc_of_row=masked[live])
+    K.assert_topk_equal(store.search(q, 10),
+                        score_oracle.search(q, corpus[live], 10, metric="euclidean", doc_of_row=masked[live]))
     store.add(corpus[:10], np.arange(4000, 4010, dtype=np.int32))
-    _check(store, score_oracle, q, np.concatenate([corpus[live], corpus[:10]]), 10, metric="euclidean",
-           doc_of_row=np.concatenate([masked[live], np.arange(4000, 4010, dtype=np.int32)]))
+    grown = np.concatenate([corpus[live], corpus[:10]])
+    grown_docs = np.concatenate([masked[live], np.arange(4000, 4010, dtype=np.int32)])
+    K.assert_topk_equal(store.search(q, 10), score_oracle.search(q, grown, 10, "euclidean", grown_docs))
 
 
 def test_non_finite_and_out_of_range_rows_are_rejected(gpu_required):
@@ -312,17 +302,14 @@ def test_ties_other_metrics_and_modifiers(gpu_required, score_oracle, metric):
     store = RowStore(d, metric=metric)
     store.add(corpus)
     for k in (10, 45):
-        _check(store, score_oracle, q, corpus, k, metric=metric)
+        K.assert_topk_equal(store.search(q, k), score_oracle.search(q, corpus, k, metric=metric))
     vals = rng.uniform(0.9, 1.1, size=n)
     vals[200:240] = 1.0
     vals[17] = 1.0
     store.set_attributes(0, np.arange(n, dtype=np.int32), vals)
     mod = score_oracle.modifiers(vals[None, :], [(0, 1.0)], [])
-    doc, row, score = store.search(q, 10, mult=[(0, 1.0)])
-    ed, er, es = score_oracle.search_modified(q, corpus, 10, mod, metric=metric)
-    np.testing.assert_array_equal(doc, ed)
-    np.testing.assert_array_equal(row, er)
-    np.testing.assert_allclose(score, es, rtol=0, atol=1e-9)
+    K.assert_topk_equal(store.search(q, 10, mult=[(0, 1.0)]),
+                        score_oracle.search_modified(q, corpus, 10, mod, metric=metric), atol=1e-9)
 
 
 def test_two_million_rows_768(gpu_required, score_oracle):
@@ -344,12 +331,8 @@ def test_two_million_rows_768(gpu_required, score_oracle):
     q = torch.nn.functional.normalize(torch.randn(nq, d, device="cuda", generator=g), dim=1).cpu().numpy()
     q[0] = host[7].astype(np.float32)
     q[1] = host[1_999_999].astype(np.float32)
-    doc, row, score = store.search(q, 10)
     qh = q.astype(np.float16).view(np.uint16)
-    edoc, erow, escore = score_oracle.search_half(qh, host.view(np.uint16), 10)
-    np.testing.assert_array_equal(doc, edoc)
-    np.testing.assert_array_equal(row, erow)
-    np.testing.assert_allclose(score, escore, rtol=0, atol=1e-12)
+    doc, _, _ = K.assert_topk_equal(store.search(q, 10), score_oracle.search_half(qh, host.view(np.uint16), 10))
     assert doc[0, 0] == 7 and list(doc[0, 1:10]) == list(range(1000, 1009)) and doc[1, 0] == 1_999_999
     d100, _, _ = store.search(q[:2], 100)
     e100, _, _ = score_oracle.search_half(qh[:2], host.view(np.uint16), 100)

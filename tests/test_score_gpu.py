@@ -5,21 +5,9 @@ Bar: doc ids and arg-max rows bit-exact; closeness equal to 1e-12 (fp64; acos ma
 import numpy as np
 import pytest
 
+import _checks as K
+
 pytestmark = pytest.mark.gpu
-
-
-def _unit_rows(rng, n, d):
-    x = rng.standard_normal((n, d)).astype(np.float32)
-    x /= np.linalg.norm(x, axis=1, keepdims=True)
-    return x
-
-
-def _check(store, so, q, corpus, k, metric, doc_of_row=None):
-    doc, row, score = store.search(q, k)
-    edoc, erow, escore = so.search(q, corpus, k, metric, doc_of_row)
-    np.testing.assert_array_equal(doc, edoc)
-    np.testing.assert_array_equal(row, erow)
-    np.testing.assert_allclose(score, escore, rtol=0, atol=1e-12)
 
 
 @pytest.mark.parametrize("n,d,nq,k", [
@@ -29,12 +17,12 @@ def _check(store, so, q, corpus, k, metric, doc_of_row=None):
 def test_topk_matches_oracle(gpu_required, score_oracle, n, d, nq, k):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(n * 31 + d)
-    corpus = _unit_rows(rng, n, d)
-    q = _unit_rows(rng, nq, d)
+    corpus = K.unit_rows(rng, n, d)
+    q = K.unit_rows(rng, nq, d)
     store = RowStore(d)
     store.add(corpus)
     assert len(store) == n
-    _check(store, score_oracle, q, corpus, k, "prenormalized-angular")
+    K.assert_topk_equal(store.search(q, k), score_oracle.search(q, corpus, k, "prenormalized-angular"))
 
 
 def test_self_match_and_duplicates(gpu_required, score_oracle):
@@ -43,10 +31,10 @@ def test_self_match_and_duplicates(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(5)
     n, d = 30000, 768
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     corpus[20000:20050] = corpus[123]          # 50 exact duplicates of row 123
     corpus[777] = corpus[29999]
-    q = _unit_rows(rng, 64, d)
+    q = K.unit_rows(rng, 64, d)
     q[:8] = corpus[[123, 5, 999, 15000, 29999, 4242, 64, 127]]
     store = RowStore(d)
     store.add(corpus)
@@ -54,7 +42,7 @@ def test_self_match_and_duplicates(gpu_required, score_oracle):
     assert doc[0, 0] == 123 and list(doc[0, 1:10]) == list(range(20000, 20009))
     assert doc[4, 0] == 777 and doc[4, 1] == 29999
     assert np.all(np.abs(score[:8, 0] - 1.0) < 2e-3)
-    _check(store, score_oracle, q, corpus, 10, "prenormalized-angular")
+    K.assert_topk_equal(store.search(q, 10), score_oracle.search(q, corpus, 10, "prenormalized-angular"))
 
 
 @pytest.mark.parametrize("metric", ["angular", "dotproduct", "euclidean"])
@@ -66,11 +54,11 @@ def test_other_metrics(gpu_required, score_oracle, metric):
     store = RowStore(256, metric=metric)
     store.add(corpus[:1000])
     store.add(corpus[1000:])
-    _check(store, score_oracle, q, corpus, 10, metric)
+    K.assert_topk_equal(store.search(q, 10), score_oracle.search(q, corpus, 10, metric))
     doc_of_row = (np.arange(3000) // 2).astype(np.int32)
     chunks = RowStore(256, metric=metric)
     chunks.add(corpus, doc_of_row)
-    _check(chunks, score_oracle, q, corpus, 25, metric, doc_of_row)
+    K.assert_topk_equal(chunks.search(q, 25), score_oracle.search(q, corpus, 25, metric, doc_of_row))
     if metric == "euclidean":
         d, r, s = store.search(corpus[5:6], 1)
         # distance to its own fp16-rounded copy is tiny but not 0 (query is rounded too -> identical -> exactly 0)
@@ -82,10 +70,10 @@ def test_max_over_chunks_and_delete(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(11)
     n, d = 9000, 256
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     doc_of_row = (np.arange(n) // 3).astype(np.int32)            # 3 chunks per doc
     doc_of_row[6000:] = rng.integers(0, 3000, size=3000)          # plus scattered extra chunks
-    q = _unit_rows(rng, 40, d)
+    q = K.unit_rows(rng, 40, d)
     q[0] = corpus[4]                                              # doc 1, chunk row 4
     store = RowStore(d)
     store.add(corpus[:5000], doc_of_row[:5000])
@@ -94,13 +82,13 @@ def test_max_over_chunks_and_delete(gpu_required, score_oracle):
     assert doc[0, 0] == 1 and row[0, 0] == 4
     for qi in range(doc.shape[0]):
         assert len(set(doc[qi])) == 10                            # one hit per document
-    _check(store, score_oracle, q, corpus, 10, "prenormalized-angular", doc_of_row)
+    K.assert_topk_equal(store.search(q, 10), score_oracle.search(q, corpus, 10, "prenormalized-angular", doc_of_row))
     store.delete_doc(1)
     dd = doc_of_row.copy()
     dd[dd == 1] = -1
     doc2, _, _ = store.search(q, 10)
     assert 1 not in doc2[0]
-    _check(store, score_oracle, q, corpus, 10, "prenormalized-angular", dd)
+    K.assert_topk_equal(store.search(q, 10), score_oracle.search(q, corpus, 10, "prenormalized-angular", dd))
 
 
 @pytest.mark.parametrize("k", [11, 16, 50, 200])
@@ -109,19 +97,19 @@ def test_large_k_multi_round(gpu_required, score_oracle, k):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(k)
     n, d = 6000, 128
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     corpus[100:140] = corpus[5]                                   # a run of exact ties across the round boundary
     doc_of_row = (np.arange(n) // 2).astype(np.int32)            # 2 chunks per doc
-    q = _unit_rows(rng, 7, d)
+    q = K.unit_rows(rng, 7, d)
     q[0] = corpus[5]
     store = RowStore(d)
     store.add(corpus, doc_of_row)
-    _check(store, score_oracle, q, corpus, k, "prenormalized-angular", doc_of_row)
+    K.assert_topk_equal(store.search(q, k), score_oracle.search(q, corpus, k, "prenormalized-angular", doc_of_row))
     small = RowStore(d)
     small.add(corpus[:30])                                        # fewer documents than k
     doc, row, score = small.search(q[:2], k)
     assert (doc[:, :30] >= 0).all() and (doc[:, 30:] == -1).all()
-    _check(small, score_oracle, q[:2], corpus[:30], k, "prenormalized-angular")
+    K.assert_topk_equal(small.search(q[:2], k), score_oracle.search(q[:2], corpus[:30], k, "prenormalized-angular"))
 
 
 def test_empty_and_small(gpu_required):
@@ -140,18 +128,18 @@ def test_growth_and_snapshot(gpu_required, score_oracle, tmp_path):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(3)
     d = 128
-    corpus = _unit_rows(rng, 2500, d)
+    corpus = K.unit_rows(rng, 2500, d)
     store = RowStore(d, capacity=10)
     for lo in range(0, 2500, 700):
         store.add(corpus[lo:lo + 700])
-    q = _unit_rows(rng, 6, d)
-    _check(store, score_oracle, q, corpus, 10, "prenormalized-angular")
+    q = K.unit_rows(rng, 6, d)
+    K.assert_topk_equal(store.search(q, 10), score_oracle.search(q, corpus, 10, "prenormalized-angular"))
     np.testing.assert_array_equal(store.get_row(17), corpus[17].astype(np.float16).astype(np.float32))
     p = tmp_path / "snap.b200"
     store.save(str(p))
     again = RowStore.load(str(p))
     assert len(again) == 2500 and again.dim == d
-    _check(again, score_oracle, q, corpus, 10, "prenormalized-angular")
+    K.assert_topk_equal(again.search(q, 10), score_oracle.search(q, corpus, 10, "prenormalized-angular"))
 
 
 def test_argument_errors(gpu_required):
@@ -173,9 +161,9 @@ def test_doc_offset_and_device_shard_merge(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(21)
     n, d, nq, k = 5000, 128, 33, 10
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     corpus[4000] = corpus[10]                                   # cross-shard tie: lower doc id first
-    q = _unit_rows(rng, nq, d)
+    q = K.unit_rows(rng, nq, d)
     q[0] = corpus[10]
     cut = 2300
     shards = [RowStore(d), RowStore(d)]

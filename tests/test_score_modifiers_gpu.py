@@ -7,13 +7,9 @@ Bar: doc ids and arg-max rows bit-exact; modified scores equal to 1e-12 (fp64, s
 import numpy as np
 import pytest
 
+import _checks as K
+
 pytestmark = pytest.mark.gpu
-
-
-def _unit_rows(rng, n, d):
-    x = rng.standard_normal((n, d)).astype(np.float32)
-    x /= np.linalg.norm(x, axis=1, keepdims=True)
-    return x
 
 
 def _attrs(rng, n_cols, n_docs, coverage=0.7, lo=0.0, hi=3.0):
@@ -28,39 +24,32 @@ def _feed_attrs(store, attrs):
         store.set_attributes(c, ids, attrs[c, ids])
 
 
-def _check(store, so, q, corpus, k, metric, attrs, mult, add, doc_of_row=None, atol=1e-12):
-    doc, row, score = store.search_modified(q, k, mult, add)
-    mod = so.modifiers(attrs, mult, add)
-    edoc, erow, escore = so.search_modified(q, corpus, k, mod, metric, doc_of_row)
-    np.testing.assert_array_equal(doc, edoc)
-    np.testing.assert_array_equal(row, erow)
-    np.testing.assert_allclose(score, escore, rtol=0, atol=atol)
-    return doc, row, score
+def _search_modified(store, so, q, corpus, k, attrs, mult, add, metric="prenormalized-angular", doc_of_row=None):
+    """(the store's, the oracle's) top-k of the same modified search."""
+    got = store.search_modified(q, k, mult, add)
+    return got, so.search_modified(q, corpus, k, so.modifiers(attrs, mult, add), metric, doc_of_row)
 
 
 @pytest.mark.parametrize("n,d,nq,k", [(300, 64, 3, 5), (20000, 128, 5, 10), (50000, 768, 64, 10), (4097, 384, 70, 10)])
 def test_modified_topk_matches_oracle(gpu_required, score_oracle, n, d, nq, k):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(n + d)
-    corpus = _unit_rows(rng, n, d)
-    q = _unit_rows(rng, nq, d)
+    corpus = K.unit_rows(rng, n, d)
+    q = K.unit_rows(rng, nq, d)
     attrs = _attrs(rng, 3, n)
     store = RowStore(d)
     store.add(corpus)
     _feed_attrs(store, attrs)
-    doc, _, _ = _check(store, score_oracle, q, corpus, k, "prenormalized-angular", attrs, [(0, 1.5), (1, 0.25)], [(2, 0.3)])
+    doc, _, _ = K.assert_topk_equal(*_search_modified(store, score_oracle, q, corpus, k, attrs, [(0, 1.5), (1, 0.25)],
+                                                      [(2, 0.3)]))
     # the modifiers really re-rank: the unmodified top-k differs
     plain, _, _ = store.search(q, k)
     assert not np.array_equal(doc, plain)
     # add-only and mult-only
-    _check(store, score_oracle, q, corpus, k, "prenormalized-angular", attrs, [], [(2, 0.3), (0, -0.05)])
-    _check(store, score_oracle, q, corpus, k, "prenormalized-angular", attrs, [(1, 2.0)], [])
+    K.assert_topk_equal(*_search_modified(store, score_oracle, q, corpus, k, attrs, [], [(2, 0.3), (0, -0.05)]))
+    K.assert_topk_equal(*_search_modified(store, score_oracle, q, corpus, k, attrs, [(1, 2.0)], []))
     # no terms at all == plain search (multiplier 1, addend 0)
-    d2, r2, s2 = store.search_modified(q, k, [], [])
-    p2, pr2, ps2 = store.search(q, k)
-    np.testing.assert_array_equal(d2, p2)
-    np.testing.assert_array_equal(r2, pr2)
-    np.testing.assert_allclose(s2, ps2, rtol=0, atol=1e-15)
+    K.assert_topk_equal(store.search_modified(q, k, [], []), store.search(q, k), atol=1e-15)
 
 
 def test_missing_cells_and_unset_columns(gpu_required, score_oracle):
@@ -68,26 +57,27 @@ def test_missing_cells_and_unset_columns(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(3)
     n, d = 5000, 128
-    corpus = _unit_rows(rng, n, d)
-    q = _unit_rows(rng, 4, d)
+    corpus = K.unit_rows(rng, n, d)
+    q = K.unit_rows(rng, 4, d)
     attrs = np.full((6, n), np.nan)
     attrs[0, ::2] = rng.uniform(0.5, 2.0, size=n // 2)   # only even documents carry attribute 0
     store = RowStore(d)
     store.add(corpus)
     _feed_attrs(store, attrs)
-    _check(store, score_oracle, q, corpus, 10, "prenormalized-angular", attrs, [(0, 3.0), (5, 7.0)], [(4, 1.0)])
+    K.assert_topk_equal(*_search_modified(store, score_oracle, q, corpus, 10, attrs, [(0, 3.0), (5, 7.0)], [(4, 1.0)]))
     # zero attribute value -> product 0 -> score == addend only
     attrs[1, :] = 0.0
     store.set_attributes(1, np.arange(n, dtype=np.int32), attrs[1])
-    doc, _, score = _check(store, score_oracle, q, corpus, 10, "prenormalized-angular", attrs, [(1, 5.0)], [(0, 1.0)])
+    doc, _, score = K.assert_topk_equal(*_search_modified(store, score_oracle, q, corpus, 10, attrs, [(1, 5.0)],
+                                                          [(0, 1.0)]))
     assert np.all(score[doc >= 0] >= 0.0)
     # removing cells
     store.set_attributes(0, np.arange(0, n, 4, dtype=np.int32), None)
     attrs[0, 0:n:4] = np.nan
-    _check(store, score_oracle, q, corpus, 10, "prenormalized-angular", attrs, [(0, 3.0)], [(0, 0.5)])
+    K.assert_topk_equal(*_search_modified(store, score_oracle, q, corpus, 10, attrs, [(0, 3.0)], [(0, 0.5)]))
     store.set_attributes(-1, np.arange(100, dtype=np.int32), None)
     attrs[:, :100] = np.nan
-    _check(store, score_oracle, q, corpus, 10, "prenormalized-angular", attrs, [(0, 3.0)], [(1, 0.5)])
+    K.assert_topk_equal(*_search_modified(store, score_oracle, q, corpus, 10, attrs, [(0, 3.0)], [(1, 0.5)]))
 
 
 @pytest.mark.parametrize("metric", ["angular", "dotproduct", "euclidean"])
@@ -103,8 +93,9 @@ def test_modified_other_metrics_and_chunks(gpu_required, score_oracle, metric):
     store.add(corpus, doc_of_row)
     _feed_attrs(store, attrs)
     atol = 1e-9 if metric == "angular" else 1e-12       # acos differs in the last ulps between libm and CUDA
-    _check(store, score_oracle, q, corpus, 10, metric, attrs, [(0, 1.25)], [(1, 0.01)], doc_of_row, atol=atol)
-    _check(store, score_oracle, q, corpus, 37, metric, attrs, [(0, 1.25)], [(1, 0.01)], doc_of_row, atol=atol)  # multi-round
+    for k in (10, 37):   # 37: multi-round
+        K.assert_topk_equal(*_search_modified(store, score_oracle, q, corpus, k, attrs, [(0, 1.25)], [(1, 0.01)],
+                                              metric, doc_of_row), atol=atol)
 
 
 def test_negative_multiplier(gpu_required, score_oracle):
@@ -112,13 +103,13 @@ def test_negative_multiplier(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(23)
     n, d = 4000, 128
-    corpus = _unit_rows(rng, n, d)
-    q = _unit_rows(rng, 3, d)
+    corpus = K.unit_rows(rng, n, d)
+    q = K.unit_rows(rng, 3, d)
     attrs = _attrs(rng, 1, n, coverage=0.5, lo=0.5, hi=1.5)
     store = RowStore(d)
     store.add(corpus)                       # one chunk per document: the best chunk is THE chunk, any sign works
     _feed_attrs(store, attrs)
-    _check(store, score_oracle, q, corpus, 10, "prenormalized-angular", attrs, [(0, -1.0)], [])
+    K.assert_topk_equal(*_search_modified(store, score_oracle, q, corpus, 10, attrs, [(0, -1.0)], []))
     chunks = RowStore(d)
     chunks.add(corpus, (np.arange(n) // 2).astype(np.int32))
     _feed_attrs(chunks, attrs[:, : n // 2])
@@ -154,8 +145,8 @@ def test_snapshot_keeps_attributes(gpu_required, score_oracle, tmp_path):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(31)
     n, d = 3000, 128
-    corpus = _unit_rows(rng, n, d)
-    q = _unit_rows(rng, 3, d)
+    corpus = K.unit_rows(rng, n, d)
+    q = K.unit_rows(rng, 3, d)
     attrs = _attrs(rng, 2, n)
     store = RowStore(d)
     store.add(corpus)
@@ -163,4 +154,4 @@ def test_snapshot_keeps_attributes(gpu_required, score_oracle, tmp_path):
     path = tmp_path / "snap.b200idx"
     store.save(str(path))
     again = RowStore.load(str(path))
-    _check(again, score_oracle, q, corpus, 10, "prenormalized-angular", attrs, [(0, 2.0)], [(1, 0.1)])
+    K.assert_topk_equal(*_search_modified(again, score_oracle, q, corpus, 10, attrs, [(0, 2.0)], [(1, 0.1)]))

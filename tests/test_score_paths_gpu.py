@@ -9,6 +9,8 @@
 import numpy as np
 import pytest
 
+import _checks as K
+
 pytestmark = pytest.mark.gpu
 
 METRICS = ("prenormalized-angular", "angular", "dotproduct", "euclidean")
@@ -17,27 +19,15 @@ NAN_MSG = ("embeddings contain a value that is not finite or does not fit the fp
            "normalisation)")
 
 
-def _unit_rows(rng, n, d):
-    x = rng.standard_normal((n, d)).astype(np.float32)
-    x /= np.linalg.norm(x, axis=1, keepdims=True)
-    return x
-
-
 def _tie_corpus(run, seed=0):
     """`run` identical rows (the first query's best match) among 8000 random unit rows; queries: that row and two
     random ones."""
     rng = np.random.default_rng(seed)
-    corpus = _unit_rows(rng, 8000 + run, DIM)
+    corpus = K.unit_rows(rng, 8000 + run, DIM)
     start = 3000
     corpus[start:start + run] = corpus[start]
-    q = np.concatenate([corpus[start:start + 1], _unit_rows(rng, 2, DIM)])
+    q = np.concatenate([corpus[start:start + 1], K.unit_rows(rng, 2, DIM)])
     return corpus, q
-
-
-def _assert_same(got, want):
-    np.testing.assert_array_equal(got[0], want[0])
-    np.testing.assert_array_equal(got[1], want[1])
-    np.testing.assert_allclose(got[2], want[2], rtol=0, atol=1e-12)
 
 
 @pytest.mark.parametrize("run", [4000, 5000], ids=["device-finalize", "host-finalize"])
@@ -52,7 +42,7 @@ def test_tied_run_both_sides_of_finalize_capacity(gpu_required, score_oracle, ru
         store.add(corpus, doc_of_row)
         for k in (10, 1000, 4999):
             before = store.search_stats()["collect_passes"]
-            _assert_same(store.search(q, k), score_oracle.search(q, corpus, k, metric, doc_of_row))
+            K.assert_topk_equal(store.search(q, k), score_oracle.search(q, corpus, k, metric, doc_of_row))
             assert store.search_stats()["collect_passes"] >= before + 1
     finally:
         store.close()
@@ -80,7 +70,7 @@ def test_tied_run_with_score_modifiers(gpu_required, score_oracle, run):
         for k in (10, 1000):
             before = store.search_stats()["collect_passes"]
             got = store.search_modified(q, k, mult, add)
-            _assert_same(got, score_oracle.search_modified(q, corpus, k, mod, metric, doc_of_row))
+            K.assert_topk_equal(got, score_oracle.search_modified(q, corpus, k, mod, metric, doc_of_row))
             assert store.search_stats()["collect_passes"] >= before + 1
     finally:
         store.close()
@@ -92,7 +82,7 @@ M = 70000   # more than one 64 Ki-row staging chunk of the host add
 
 def _add_corpus():
     rng = np.random.default_rng(5)
-    vecs = _unit_rows(rng, M, DIM)
+    vecs = K.unit_rows(rng, M, DIM)
     ids = rng.permutation(M // 2).astype(np.int32)[np.arange(M) // 2]   # two chunks per document, shuffled numbers
     return vecs, ids
 
@@ -128,7 +118,7 @@ def _snapshot(store, q, tmp_path, name):
 def test_every_add_path_leaves_the_same_index(gpu_required, tmp_path):
     from marqo_b200.engine import RowStore
     vecs, ids = _add_corpus()
-    q = _unit_rows(np.random.default_rng(7), 5, DIM)
+    q = K.unit_rows(np.random.default_rng(7), 5, DIM)
     snaps = {}
     for path in ("add_ids", "add_device_ids", "add_device_docs", "add", "add_device"):
         store = RowStore(DIM)
@@ -157,8 +147,8 @@ def test_rejected_batch_leaves_nothing_behind(gpu_required, path):
     from marqo_b200 import _native as N
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(8)
-    base, base_ids = _unit_rows(rng, 500, DIM), np.arange(500, dtype=np.int32)
-    q = _unit_rows(rng, 3, DIM)
+    base, base_ids = K.unit_rows(rng, 500, DIM), np.arange(500, dtype=np.int32)
+    q = K.unit_rows(rng, 3, DIM)
     store = RowStore(DIM, "dotproduct")
     try:
         _fill(store, path, base, base_ids)
@@ -166,7 +156,7 @@ def test_rejected_batch_leaves_nothing_behind(gpu_required, path):
         for kind, (msg, spoil) in BAD_BATCHES.items():
             if kind == "negative-id" and path not in HOST_ID_PATHS:
                 continue
-            vecs, ids = _unit_rows(rng, 40, DIM), np.arange(500, 540, dtype=np.int32)
+            vecs, ids = K.unit_rows(rng, 40, DIM), np.arange(500, 540, dtype=np.int32)
             spoil(vecs, ids)
             with pytest.raises(N.NativeError) as e:
                 _fill(store, path, vecs, ids)
@@ -175,7 +165,7 @@ def test_rejected_batch_leaves_nothing_behind(gpu_required, path):
             got = store.search(q, 20)
             for a, b in zip(got, want):
                 np.testing.assert_array_equal(a, b)
-        _fill(store, path, _unit_rows(rng, 40, DIM), np.arange(500, 540, dtype=np.int32))
+        _fill(store, path, K.unit_rows(rng, 40, DIM), np.arange(500, 540, dtype=np.int32))
         assert len(store) == 540
     finally:
         store.close()

@@ -7,22 +7,18 @@ force the streamed kernel at any dim, so both kernels are run on one corpus here
 import numpy as np
 import pytest
 
+import _checks as K
+
 pytestmark = pytest.mark.gpu
 
 WIDE_DIMS = [1088, 1152, 1536, 2048, 3072, 4096]
 METRICS = ["prenormalized-angular", "angular", "dotproduct", "euclidean"]
 
 
-def _unit_rows(rng, n, d):
-    x = rng.standard_normal((n, d)).astype(np.float32)
-    x /= np.linalg.norm(x, axis=1, keepdims=True)
-    return x
-
-
 def _rows_for(metric, rng, n, d):
     if metric in ("prenormalized-angular", "angular"):
-        return _unit_rows(rng, n, d)
-    return _unit_rows(rng, n, d) * np.float32(0.7)     # not unit: the dot product and distance use the norms
+        return K.unit_rows(rng, n, d)
+    return K.unit_rows(rng, n, d) * np.float32(0.7)     # not unit: the dot product and distance use the norms
 
 
 def _expect(so, q, corpus, k, metric="prenormalized-angular", doc_of_row=None, got=None):
@@ -81,8 +77,8 @@ def test_many_tiles_per_sm(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(11)
     n, d = 200_000, 1536
-    corpus = _unit_rows(rng, n, d)
-    q = _unit_rows(rng, 8, d)
+    corpus = K.unit_rows(rng, n, d)
+    q = K.unit_rows(rng, 8, d)
     q[0] = corpus[n - 1]
     store = RowStore(d)
     store.add(corpus)
@@ -95,10 +91,10 @@ def test_filter_and_modifiers_1536(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(12)
     n, d = 16_000, 1536
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     doc_of_row = (np.arange(n) // 2).astype(np.int32)
     ndocs = n // 2
-    q = _unit_rows(rng, 5, d)
+    q = K.unit_rows(rng, 5, d)
     store = RowStore(d)
     store.add(corpus, doc_of_row)
     keep = rng.random(ndocs) < 0.2
@@ -127,7 +123,7 @@ def test_ties_and_near_ties_3072(gpu_required, score_oracle):
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(13)
     n, d = 60_000, 3072
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     # 20 identical rows in one tile (more than one CTA's 16-entry list holds) and 80 more elsewhere (more than the 64
     # candidates the merge re-scores for k <= 10)
     ties = np.concatenate([np.arange(2000, 2020), rng.choice(np.arange(3000, n), size=80, replace=False)])
@@ -142,7 +138,7 @@ def test_ties_and_near_ties_3072(gpu_required, score_oracle):
         fam[i] = bits.view(np.float16)
     near = rng.choice(np.setdiff1d(np.arange(n), ties), size=30, replace=False)
     corpus[near] = fam.astype(np.float32)
-    q = _unit_rows(rng, 4, d)
+    q = K.unit_rows(rng, 4, d)
     q[0] = corpus[ties[0]]
     q[1] = base
     store = RowStore(d)
@@ -160,9 +156,9 @@ def test_async_compact_save_load_rows_and_device_merge_1536(gpu_required, score_
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(14)
     n, d, nq, k = 12_000, 1536, 6, 10
-    corpus = _unit_rows(rng, n, d)
+    corpus = K.unit_rows(rng, n, d)
     corpus[500:530] = corpus[9]
-    q = _unit_rows(rng, nq, d)
+    q = K.unit_rows(rng, nq, d)
     q[0] = corpus[9]
     store = RowStore(d)
     store.add(corpus)
@@ -253,13 +249,13 @@ def test_adapter_pads_narrow_fields(gpu_required, score_oracle, d, tmp_path):
     from marqo_b200.gpu_tensor_index import GpuTensorIndex
     rng = np.random.default_rng(d)
     n_docs, chunks = 400, 2
-    vecs = _unit_rows(rng, n_docs * chunks, d)
+    vecs = K.unit_rows(rng, n_docs * chunks, d)
     ix = GpuTensorIndex()
     docs = [_doc(f"d{i}", {}, {"body": ([f"c{j}" for j in range(chunks)], vecs[i * chunks:(i + 1) * chunks])})
             for i in range(n_docs)]
     resp = ix.feed_batch(docs, "s1")
     assert not resp.errors
-    q = _unit_rows(rng, 3, d)
+    q = K.unit_rows(rng, 3, d)
     doc_of_row = (np.arange(n_docs * chunks) // chunks).astype(np.int32)
     w = -(-d // 64) * 64                      # the oracle's summation order needs a multiple of 8: pad as the adapter does
     pad = lambda x: np.concatenate([x, np.zeros((x.shape[0], w - d), np.float32)], axis=1)

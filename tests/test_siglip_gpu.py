@@ -7,22 +7,10 @@ import numpy as np
 import pytest
 import torch
 
+import _checks as K
 import _siglip_oracle as O
 
 pytestmark = pytest.mark.gpu
-COS_TOL = 1e-3
-
-
-def _check(got, ref):
-    got = torch.as_tensor(np.asarray(got))
-    assert torch.isfinite(got).all()
-    c = torch.nn.functional.cosine_similarity(got.double(), torch.as_tensor(np.asarray(ref)).double(), dim=-1)
-    assert float((1 - c).max()) < COS_TOL, f"min cosine {float(c.min())}"
-    assert torch.allclose(got.norm(dim=-1), torch.ones(got.shape[0], dtype=got.dtype), atol=1e-5)
-
-
-def _bf16(x):
-    return x.to(torch.bfloat16).to(torch.float32)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -35,7 +23,7 @@ def test_map_attention_matches_torch(gpu_required, S, B):
     g = torch.Generator().manual_seed(S * 10 + B)
     H, W = 12, 768
     q = torch.randn(W, generator=g) * 2.0                          # logit std ~2: peaked but not one-hot
-    kv = _bf16(torch.randn(B * S, 2 * W, generator=g))
+    kv = K.bf16(torch.randn(B * S, 2 * W, generator=g))
     got = torch.from_numpy(debug_map_attention(q.numpy(), kv.numpy(), B, S, H))
     k, v = kv.double().view(B, S, 2, H, 64).permute(2, 0, 3, 1, 4)     # [B, H, S, 64]
     att = (q.double().view(1, H, 1, 64) @ k.transpose(-1, -2)) / 8.0  # [B, H, 1, S]
@@ -87,7 +75,7 @@ def test_b16_224_batch_256_every_input_path(gpu_required, b16):
     rng = np.random.default_rng(1)
     at_size = rng.integers(0, 256, (256, 224, 224, 3), dtype=np.uint8)
     got = enc.encode_images_u8(at_size)
-    _check(got[ROWS], O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(at_size[ROWS], 224)))
+    K.assert_embeddings_match(got[ROWS], O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(at_size[ROWS], 224)))
     # the same batch from a device-resident tensor gives the same bits
     dev = torch.from_numpy(at_size).cuda()
     out = torch.empty((256, 768), dtype=torch.float32, device="cuda")
@@ -96,15 +84,15 @@ def test_b16_224_batch_256_every_input_path(gpu_required, b16):
     np.testing.assert_array_equal(out.cpu().numpy(), got)
     # squash resize of another size on the way in
     other = rng.integers(0, 256, (8, 300, 171, 3), dtype=np.uint8)
-    _check(enc.encode_images_u8(other), O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(other, 224)))
+    K.assert_embeddings_match(enc.encode_images_u8(other),
+                              O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(other, 224)))
     # preprocessed fp32 CHW
     chw = O.siglip_preprocess_u8(other[:3], 224)
-    _check(enc.encode_images_f32(chw.numpy()), O.siglip_encode_image(sd, cfg, chw))
+    K.assert_embeddings_match(enc.encode_images_f32(chw.numpy()), O.siglip_encode_image(sd, cfg, chw))
     # unnormalised output is the pooled vector itself
     raw = enc.encode_images_f32(chw.numpy(), normalize=False)
     ref = O.siglip_encode_image(sd, cfg, chw, normalize=False)
-    c = torch.nn.functional.cosine_similarity(torch.from_numpy(raw).double(), ref.double(), dim=-1)
-    assert float((1 - c).max()) < COS_TOL
+    K.assert_embeddings_match(raw, ref, unit_norm=False)
     torch.testing.assert_close(torch.from_numpy(raw).norm(dim=-1), ref.norm(dim=-1), rtol=1e-2, atol=0)
 
 
@@ -116,7 +104,7 @@ def test_b16_single_image_graph_replay(gpu_required, b16):
     third = enc.encode_images_u8(img)
     np.testing.assert_array_equal(first, second)
     np.testing.assert_array_equal(first, third)
-    _check(first, O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(img, 224)))
+    K.assert_embeddings_match(first, O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(img, 224)))
 
 
 @pytest.mark.parametrize("n", [256, 1])
@@ -126,7 +114,7 @@ def test_b16_text(gpu_required, b16, n):
     rows = [r for r in ROWS if r < n]
     for _ in range(3 if n == 1 else 1):     # a single query also runs eagerly, captured and replayed
         got = enc.encode_tokens(ids.numpy())
-        _check(got[rows], O.siglip_encode_text(sd, cfg, ids[rows]))
+        K.assert_embeddings_match(got[rows], O.siglip_encode_text(sd, cfg, ids[rows]))
 
 
 @pytest.mark.parametrize("size,n", [(256, 32), (384, 16), (512, 4)])
@@ -138,10 +126,11 @@ def test_b16_larger_images(gpu_required, size, n):
         rng = np.random.default_rng(size)
         at_size = rng.integers(0, 256, (n, size, size, 3), dtype=np.uint8)
         rows = [0, n - 1]
-        _check(enc.encode_images_u8(at_size)[rows],
-               O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(at_size[rows], size)))
+        K.assert_embeddings_match(enc.encode_images_u8(at_size)[rows],
+                                  O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(at_size[rows], size)))
         squashed = rng.integers(0, 256, (2, 200, 333, 3), dtype=np.uint8)
-        _check(enc.encode_images_u8(squashed), O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(squashed, size)))
+        K.assert_embeddings_match(enc.encode_images_u8(squashed),
+                                  O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(squashed, size)))
     finally:
         enc.close()
 
@@ -153,7 +142,8 @@ def test_l16_256(gpu_required):
     try:
         img = np.random.default_rng(16).integers(0, 256, (64, 320, 240, 3), dtype=np.uint8)
         got = enc.encode_images_u8(img)
-        _check(got[[0, 63]], O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(img[[0, 63]], 256)))
+        K.assert_embeddings_match(got[[0, 63]],
+                                  O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(img[[0, 63]], 256)))
     finally:
         enc.close()
 
@@ -183,11 +173,6 @@ def test_missing_map_head_weight_is_reported(gpu_required):
 # ------------------------------------------------------------------------------------------------------------------
 # Through the seams: vectorise("Marqo/marqo-fashionSigLIP") -> GpuTensorIndex -> search
 # ------------------------------------------------------------------------------------------------------------------
-def _doc(doc_id, vec):
-    return {"id": doc_id, "fields": {"marqo__id": doc_id, "marqo__chunks_body": ["c"],
-                                     "marqo__embeddings_body": {"0": vec.tolist()}}}
-
-
 def _tokenizer(texts):
     """Stand-in for SigLIP's SentencePiece tokenizer: [n, 64] ids from a hash of the words, zero padded."""
     out = np.zeros((len(texts), 64), np.int64)
@@ -199,7 +184,6 @@ def _tokenizer(texts):
 
 def test_vectorise_fashion_siglip_into_index_and_search(gpu_required, score_oracle):
     from marqo_b200 import model_registry as R, s2_inference as s2, weights as Wt
-    from marqo_b200.gpu_tensor_index import GpuTensorIndex
     from marqo_b200.s2_inference import Modality
     s2.clear_loaded_models()
     name = "Marqo/marqo-fashionSigLIP"
@@ -216,20 +200,9 @@ def test_vectorise_fashion_siglip_into_index_and_search(gpu_required, score_orac
     cfg = O.SiglipCfg()
     sd = {k: torch.from_numpy(v) for k, v in Wt.random_siglip_weights(props["arch"], 17).items()}
     rows = [0, 47]
-    _check(docs[rows], O.siglip_encode_image(sd, cfg, torch.cat([O.siglip_preprocess_u8(images[r][None], 224)
-                                                                  for r in rows])))
-    _check(q, O.siglip_encode_text(sd, cfg, torch.from_numpy(_tokenizer(queries))))
+    px = torch.cat([O.siglip_preprocess_u8(images[r][None], 224) for r in rows])
+    K.assert_embeddings_match(docs[rows], O.siglip_encode_image(sd, cfg, px))
+    K.assert_embeddings_match(q, O.siglip_encode_text(sd, cfg, torch.from_numpy(_tokenizer(queries))))
     s2.clear_loaded_models()
 
-    ix = GpuTensorIndex()
-    assert not ix.feed_batch([_doc(f"d{i}", v) for i, v in enumerate(docs)], "s1").errors
-    k = 10
-    yql = (f"select * from s1 where (({{targetHits:{k}, approximate:False, hnsw.exploreAdditionalHits:0}}"
-           f"nearestNeighbor(marqo__embeddings_body, marqo__query_embedding)))")
-    edoc, _, escore = score_oracle.search(q, docs, k, "prenormalized-angular")
-    for j in range(len(queries)):
-        res = ix.query(yql, hits=k, ranking="embedding_similarity", model_restrict="s1",
-                       query_features={"marqo__query_embedding": q[j].tolist()})
-        assert [h.id.split("::")[-1] for h in res.hits] == [f"d{d}" for d in edoc[j]]
-        np.testing.assert_allclose([h.relevance for h in res.hits], escore[j], rtol=0, atol=1e-12)
-    ix.close()
+    K.assert_index_search_matches(score_oracle, docs, q)

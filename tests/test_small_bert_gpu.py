@@ -7,16 +7,12 @@ import numpy as np
 import pytest
 import torch
 
+import _checks as K
 from oracle import encoders as E
 
 pytestmark = pytest.mark.gpu
-COS_TOL = 1e-3
 MINILM_L6 = E.BertCfg(384, 6, 12, 1536)
 E5_SMALL = E.BertCfg(384, 12, 12, 1536)
-
-
-def _bf16(x: torch.Tensor) -> torch.Tensor:
-    return x.to(torch.bfloat16).to(torch.float32)
 
 
 def _kv_len(g, B, S, mask):
@@ -52,7 +48,7 @@ def test_attention_hd32_matches_torch(gpu_required, B, S, H, mask):
     from marqo_b200.engine import debug_attention
     g = torch.Generator().manual_seed(B * 1000 + S + 7 * mask)
     W = H * 32
-    qkv = _bf16(torch.randn(B * S, 3 * W, generator=g))
+    qkv = K.bf16(torch.randn(B * S, 3 * W, generator=g))
     kv_len = _kv_len(g, B, S, mask)
     ref = _attention_ref(qkv, B, S, H, mask, kv_len)
     got = torch.from_numpy(debug_attention(qkv.numpy(), B, S, W, H, mask, None if kv_len is None else kv_len.numpy()))
@@ -69,7 +65,7 @@ def test_attention_hd32_peaked_scores(gpu_required, B, S, H, mask):
     W = H * 32
     qkv = torch.randn(B * S, 3 * W, generator=g)
     qkv[:, : 2 * W] *= 3.0                                          # q and k: score std 9, extremes beyond 40
-    qkv = _bf16(qkv)
+    qkv = K.bf16(qkv)
     kv_len = _kv_len(g, B, S, mask)
     ref = _attention_ref(qkv, B, S, H, mask, kv_len, dtype=torch.float64)
     got = torch.from_numpy(debug_attention(qkv.numpy(), B, S, W, H, mask, None if kv_len is None else kv_len.numpy()))
@@ -93,31 +89,9 @@ def test_attention_other_head_dims_are_unsupported(gpu_required, hd, S):
 # ------------------------------------------------------------------------------------------------------------------
 # Encoders through the C ABI vs the CPU fp32 oracle on the same seeded weights
 # ------------------------------------------------------------------------------------------------------------------
-def _cos(a, b):
-    a, b = torch.as_tensor(np.asarray(a)).double(), torch.as_tensor(np.asarray(b)).double()
-    return torch.nn.functional.cosine_similarity(a, b, dim=-1)
-
-
-def _check(got, ref):
-    got = torch.from_numpy(np.asarray(got))
-    assert torch.isfinite(got).all()
-    c = _cos(got, ref)
-    assert float((1 - c).max()) < COS_TOL, f"min cosine {float(c.min())}"
-    assert torch.allclose(got.norm(dim=-1), torch.ones(got.shape[0], dtype=got.dtype), atol=1e-5)
-
-
-def _bert_config(cfg: E.BertCfg) -> dict:
-    return dict(width=cfg.width, layers=cfg.layers, heads=cfg.heads, mlp=cfg.mlp, vocab=cfg.vocab, max_pos=cfg.max_pos,
-                type_vocab=cfg.type_vocab, pool=cfg.pool)
-
-
 def _ids(g, B, S):
     return torch.cat([torch.full((B, 1), 101), torch.randint(1000, 30000, (B, S - 2), generator=g),
                       torch.full((B, 1), 102)], 1)
-
-
-def _sample_positions(n, m):
-    return sorted(set([0, n - 1] + [int(x) for x in np.linspace(1, n - 2, m - 2)]))
 
 
 def test_minilm_l6_batch_256_ragged(gpu_required):
@@ -125,7 +99,7 @@ def test_minilm_l6_batch_256_ragged(gpu_required):
     from marqo_b200.engine import Encoder
     cfg = MINILM_L6
     sd = E.make_bert_weights(cfg, seed=1234)
-    enc = Encoder("bert", _bert_config(cfg), sd, max_batch=256)
+    enc = Encoder("bert", E.engine_config(cfg), sd, max_batch=256)
     g = torch.Generator().manual_seed(0)
     ids = _ids(g, 256, 128)
     mask = torch.ones(256, 128, dtype=torch.int64)
@@ -136,10 +110,10 @@ def test_minilm_l6_batch_256_ragged(gpu_required):
         ids[b, int(lens[b]):] = 0
     got = enc.encode_tokens(ids.numpy(), mask.numpy())
     assert got.shape == (256, 384)
-    pos = _sample_positions(256, 6) + [100]
-    _check(got[pos], E.bert_encode(sd, cfg, ids[pos], mask[pos]))
+    pos = K.sample_positions(256, 6) + [100]
+    K.assert_embeddings_match(got[pos], E.bert_encode(sd, cfg, ids[pos], mask[pos]))
     full = enc.encode_tokens(ids[:4].numpy())                     # no mask: every key counts
-    _check(full, E.bert_encode(sd, cfg, ids[:4]))
+    K.assert_embeddings_match(full, E.bert_encode(sd, cfg, ids[:4]))
     enc.close()
 
 
@@ -148,18 +122,18 @@ def test_e5_small_v2_512_tokens(gpu_required):
     from marqo_b200.engine import Encoder
     cfg = E5_SMALL
     sd = E.make_bert_weights(cfg, seed=1234)
-    enc = Encoder("bert", _bert_config(cfg), sd, max_batch=8)
+    enc = Encoder("bert", E.engine_config(cfg), sd, max_batch=8)
     g = torch.Generator().manual_seed(1)
     ids = _ids(g, 8, 512)
     got = enc.encode_tokens(ids.numpy())
-    _check(got[[0, 7]], E.bert_encode(sd, cfg, ids[[0, 7]]))
+    K.assert_embeddings_match(got[[0, 7]], E.bert_encode(sd, cfg, ids[[0, 7]]))
     mask = torch.ones(8, 512, dtype=torch.int64)
     for b, L in enumerate([256, 200, 312, 256, 1, 511, 256, 300]):
         mask[b, L:] = 0
         ids[b, L:] = 0
     gm = enc.encode_tokens(ids.numpy(), mask.numpy())
     sel = [1, 4, 5]
-    _check(gm[sel], E.bert_encode(sd, cfg, ids[sel], mask[sel]))
+    K.assert_embeddings_match(gm[sel], E.bert_encode(sd, cfg, ids[sel], mask[sel]))
     enc.close()
 
 
@@ -168,46 +142,26 @@ def test_single_short_query(gpu_required, cfg):
     """b1 x 16 tokens: the search-latency shape (mma.sync attention), eager then replayed from a CUDA graph."""
     from marqo_b200.engine import Encoder
     sd = E.make_bert_weights(cfg, seed=77)
-    enc = Encoder("bert", _bert_config(cfg), sd, max_batch=16)
+    enc = Encoder("bert", E.engine_config(cfg), sd, max_batch=16)
     g = torch.Generator().manual_seed(2)
     for _ in range(3):
         ids = _ids(g, 1, 16)
-        _check(enc.encode_tokens(ids.numpy()), E.bert_encode(sd, cfg, ids))
+        K.assert_embeddings_match(enc.encode_tokens(ids.numpy()), E.bert_encode(sd, cfg, ids))
     ids = _ids(g, 1, 16)
     mask = torch.ones(1, 16, dtype=torch.int64)
     mask[0, 11:] = 0
     ids[0, 11:] = 0
-    _check(enc.encode_tokens(ids.numpy(), mask.numpy()), E.bert_encode(sd, cfg, ids, mask))
+    K.assert_embeddings_match(enc.encode_tokens(ids.numpy(), mask.numpy()), E.bert_encode(sd, cfg, ids, mask))
     enc.close()
 
 
 # ------------------------------------------------------------------------------------------------------------------
 # Through the seams: vectorise("hf/all-MiniLM-L6-v2") -> GpuTensorIndex at D = 384 -> search
 # ------------------------------------------------------------------------------------------------------------------
-class WordTokenizer:
-    """Stand-in for AutoTokenizer (no vocab files offline): 'w<id>' words -> ids, [CLS]=101 ... [SEP]=102, pad 0."""
-
-    def __call__(self, sentences, padding=True, truncation=True, max_length=128, return_tensors="np"):
-        rows = [[101] + [1000 + int(w[1:]) for w in s.split()][: max_length - 2] + [102] for s in sentences]
-        L = max(len(r) for r in rows)
-        ids = np.zeros((len(rows), L), np.int64)
-        mask = np.zeros((len(rows), L), np.int64)
-        for i, r in enumerate(rows):
-            ids[i, :len(r)] = r
-            mask[i, :len(r)] = 1
-        return {"input_ids": ids, "attention_mask": mask}
-
-
-def _doc(doc_id, vec):
-    return {"id": doc_id, "fields": {"marqo__id": doc_id, "marqo__chunks_body": ["c"],
-                                     "marqo__embeddings_body": {"0": vec.tolist()}}}
-
-
 def test_vectorise_minilm_into_index_and_search(gpu_required, score_oracle, monkeypatch):
     from marqo_b200 import model_registry as R, s2_inference as s2, weights as Wt
-    from marqo_b200.gpu_tensor_index import GpuTensorIndex
     s2.clear_loaded_models()
-    tok = WordTokenizer()
+    tok = K.WordTokenizer(101, 102, 1000)
     name = "hf/all-MiniLM-L6-v2"
     props = dict(R.get_model_properties(name), random_init=31, tokenizer=tok)
     rng = np.random.default_rng(3)
@@ -223,22 +177,11 @@ def test_vectorise_minilm_into_index_and_search(gpu_required, score_oracle, monk
     for i in range(0, 64, 16):                                           # the reference pads per sub-batch
         t = tok(sentences[i:i + 16], max_length=props["tokens"])
         ref.append(E.bert_encode(sd, MINILM_L6, torch.from_numpy(t["input_ids"]), torch.from_numpy(t["attention_mask"])))
-    _check(docs, torch.cat(ref))
+    K.assert_embeddings_match(docs, torch.cat(ref))
     queries = [" ".join(f"w{int(x)}" for x in rng.integers(0, 28000, size=n)) for n in (3, 8, 14)]
     q = np.asarray(s2.vectorise(name, queries, model_properties=props, device="cuda:0", normalize_embeddings=True),
                    np.float32)
-    _check(q, E.bert_encode(sd, MINILM_L6, *[torch.from_numpy(v) for v in tok(queries).values()]))
+    K.assert_embeddings_match(q, E.bert_encode(sd, MINILM_L6, *[torch.from_numpy(v) for v in tok(queries).values()]))
     s2.clear_loaded_models()
 
-    ix = GpuTensorIndex()
-    assert not ix.feed_batch([_doc(f"d{i}", v) for i, v in enumerate(docs)], "s1").errors
-    k = 10
-    yql = (f"select * from s1 where (({{targetHits:{k}, approximate:False, hnsw.exploreAdditionalHits:0}}"
-           f"nearestNeighbor(marqo__embeddings_body, marqo__query_embedding)))")
-    edoc, _, escore = score_oracle.search(q, docs, k, "prenormalized-angular")
-    for j in range(len(queries)):
-        res = ix.query(yql, hits=k, ranking="embedding_similarity", model_restrict="s1",
-                       query_features={"marqo__query_embedding": q[j].tolist()})
-        assert [h.id.split("::")[-1] for h in res.hits] == [f"d{d}" for d in edoc[j]]
-        np.testing.assert_allclose([h.relevance for h in res.hits], escore[j], rtol=0, atol=1e-12)
-    ix.close()
+    K.assert_index_search_matches(score_oracle, docs, q)

@@ -8,19 +8,11 @@ import numpy as np
 import pytest
 import torch
 
+import _checks as K
 import _xlmr_oracle as X
 
 pytestmark = pytest.mark.gpu
-COS_TOL = 1e-3
 MODEL_FILE = Path(__file__).resolve().parent / "golden" / "unigram_golden.model"
-
-
-def _check(got, ref):
-    got = torch.from_numpy(np.asarray(got))
-    assert torch.isfinite(got).all()
-    c = torch.nn.functional.cosine_similarity(got.double(), torch.as_tensor(np.asarray(ref)).double(), dim=-1)
-    assert float((1 - c).max()) < COS_TOL, f"min cosine {float(c.min())}"
-    assert torch.allclose(got.norm(dim=-1), torch.ones(got.shape[0], dtype=got.dtype), atol=1e-5)
 
 
 def _encoder(cfg, sd, max_batch):
@@ -44,7 +36,7 @@ def test_xlmr_base_full_depth_ragged(gpu_required):
     got = enc.encode_tokens(ids.numpy(), mask.numpy())
     assert got.shape == (16, 768)
     sel = [0, 1, 2, 3, 4, 5, 15]
-    _check(got[sel], X.xlmr_encode(sd, cfg, ids[sel], mask[sel]))
+    K.assert_embeddings_match(got[sel], X.xlmr_encode(sd, cfg, ids[sel], mask[sel]))
     enc.close()
 
 
@@ -61,7 +53,7 @@ def test_xlmr_large_two_layers_b64(gpu_required):
     got = enc.encode_tokens(ids.numpy(), mask.numpy())
     assert got.shape == (64, 1024)
     sel = [0, 17, 40, 63]
-    _check(got[sel], X.xlmr_encode(sd, cfg, ids[sel], mask[sel]))
+    K.assert_embeddings_match(got[sel], X.xlmr_encode(sd, cfg, ids[sel], mask[sel]))
     enc.close()
 
 
@@ -75,7 +67,7 @@ def test_xlmr_large_full_depth_and_513_refused(gpu_required):
     ids, mask = X.ragged_ids(g, 8, 512, [512, 100, 512, 37, 256, 511, 3, 400], cfg.vocab)
     got = enc.encode_tokens(ids.numpy(), mask.numpy())
     sel = [0, 3]
-    _check(got[sel], X.xlmr_encode(sd, cfg, ids[sel], mask[sel]))
+    K.assert_embeddings_match(got[sel], X.xlmr_encode(sd, cfg, ids[sel], mask[sel]))
     with pytest.raises(NativeError) as ei:
         enc.encode_tokens(np.zeros((1, 513), np.int32))
     assert ei.value.code == ERR_INVALID_ARG
@@ -97,7 +89,7 @@ def test_xlmr_small_runs_the_bert_runtime(gpu_required):
     got = enc.encode_tokens(ids.numpy(), mask.numpy())
     cfg = BertCfg(384, 12, 12, 1536, vocab=250037, max_pos=512, type_vocab=2)
     sel = [0, 1, 2, 3]
-    _check(got[sel], bert_encode(sd, cfg, ids[sel], mask[sel]))
+    K.assert_embeddings_match(got[sel], bert_encode(sd, cfg, ids[sel], mask[sel]))
     enc.close()
 
 
@@ -109,7 +101,7 @@ def test_roberta_prefix_and_missing_type_row(gpu_required):
     g = torch.Generator().manual_seed(4)
     ids, mask = X.ragged_ids(g, 4, 64, [64, 1, 33, 10], cfg.vocab)
     ids[1, 0] = 2
-    _check(enc.encode_tokens(ids.numpy(), mask.numpy()), X.xlmr_encode(sd, cfg, ids, mask))
+    K.assert_embeddings_match(enc.encode_tokens(ids.numpy(), mask.numpy()), X.xlmr_encode(sd, cfg, ids, mask))
     enc.close()
     del sd["embeddings.token_type_embeddings.weight"]
     with pytest.raises(NativeError) as ei:
@@ -120,15 +112,9 @@ def test_roberta_prefix_and_missing_type_row(gpu_required):
 # ------------------------------------------------------------------------------------------------------------------
 # Through the seams: vectorise("hf/multilingual-e5-base") with the Unigram tokenizer -> GpuTensorIndex -> search
 # ------------------------------------------------------------------------------------------------------------------
-def _doc(doc_id, vec):
-    return {"id": doc_id, "fields": {"marqo__id": doc_id, "marqo__chunks_body": ["c"],
-                                     "marqo__embeddings_body": {"0": vec.tolist()}}}
-
-
 def test_vectorise_multilingual_e5_into_index_and_search(gpu_required, score_oracle, monkeypatch):
     import sentencepiece as spm
     from marqo_b200 import model_registry as R, s2_inference as s2
-    from marqo_b200.gpu_tensor_index import GpuTensorIndex
     s2.clear_loaded_models()
     name = "hf/multilingual-e5-base"
     props = dict(R.get_model_properties(name), random_init=41, vocab_file=str(MODEL_FILE))
@@ -154,22 +140,11 @@ def test_vectorise_multilingual_e5_into_index_and_search(gpu_required, score_ora
         return X.xlmr_encode(sd, cfg, ids, mask)
 
     sel = [0, 3, 17, 39, 40, 63]
-    _check(docs[sel], oracle([sentences[i] for i in sel]))
+    K.assert_embeddings_match(docs[sel], oracle([sentences[i] for i in sel]))
     queries = ["東京 大学", "привет мир", "ﬁne café", "αβγ"]
     q = np.asarray(s2.vectorise(name, queries, model_properties=props, device="cuda:0", normalize_embeddings=True),
                    np.float32)
-    _check(q, oracle(queries))
+    K.assert_embeddings_match(q, oracle(queries))
     s2.clear_loaded_models()
 
-    ix = GpuTensorIndex()
-    assert not ix.feed_batch([_doc(f"d{i}", v) for i, v in enumerate(docs)], "s1").errors
-    k = 10
-    yql = (f"select * from s1 where (({{targetHits:{k}, approximate:False, hnsw.exploreAdditionalHits:0}}"
-           f"nearestNeighbor(marqo__embeddings_body, marqo__query_embedding)))")
-    edoc, _, escore = score_oracle.search(q, docs, k, "prenormalized-angular")
-    for j in range(len(queries)):
-        res = ix.query(yql, hits=k, ranking="embedding_similarity", model_restrict="s1",
-                       query_features={"marqo__query_embedding": q[j].tolist()})
-        assert [h.id.split("::")[-1] for h in res.hits] == [f"d{d}" for d in edoc[j]]
-        np.testing.assert_allclose([h.relevance for h in res.hits], escore[j], rtol=0, atol=1e-12)
-    ix.close()
+    K.assert_index_search_matches(score_oracle, docs, q)
