@@ -247,9 +247,11 @@ enum b200_act { B200_ACT_GELU = 0, B200_ACT_QUICKGELU = 1 };
 enum b200_pool { B200_POOL_MEAN = 0, B200_POOL_CLS = 1 };
 
 typedef struct b200_tower_desc {
-    int32_t width;      /* hidden size */
+    int32_t width;      /* hidden size: a multiple of 128, <= 1664 for the CLIP towers, <= 1024 for the others */
     int32_t layers;     /* transformer blocks */
-    int32_t heads;      /* head_dim = width / heads must be 32 or 64 */
+    int32_t heads;      /* head_dim = width / heads must be 32 or 64; a CLIP vision tower of at least 128 tokens
+                           may also have 80, 88 or 104 (ViT-H-14, ViT-g-14, ViT-bigG-14), which run zero-padded to
+                           96, 96 and 128 */
     int32_t mlp;        /* MLP hidden size */
     int32_t ctx;        /* text: context length (77 / 512); vision: unused */
     int32_t vocab;      /* text: vocabulary size; vision: unused */
@@ -303,6 +305,10 @@ typedef struct b200_model_desc {
     int32_t convnext_depths[4];   /* blocks per stage: {3, 3, 27, 3}, xxlarge {3, 4, 30, 3} */
     int32_t convnext_image_size;  /* 224, 256 or 320 */
     int32_t convnext_head;        /* 0: linear projection, 1: MLP */
+    /* CLIP ViT: how a uint8 image of another size becomes image_size x image_size: 0 resizes the shortest side and
+     * centre-crops (open_clip's default), 1 squashes it, x and y scaled independently without a crop (open_clip's
+     * resize_mode "squash": the DFN5B models).  SigLIP always squashes. */
+    int32_t resize_squash;
 } b200_model_desc;
 
 int b200_model_create(int device, const b200_model_desc* desc, b200_model** out);
@@ -504,6 +510,10 @@ int b200_debug_patch_embed(int device, const uint8_t* hwc, int n, int S, int pat
  * to the logit of query i and key j; head_dim 64, mask 2, S <= smax.  out bf16 [B*S, W]. */
 int b200_debug_attention(int device, const void* qkv, int B, int S, int W, int H, int mask, const int32_t* kv_len,
                          const float* rel_bias, int smax, void* out, void* stream);
+/* b200_debug_attention (without a bias) over heads of W / H columns whose logits take the scale 1 / sqrt(model_hd):
+ * the zero-padded heads of the ViT-H / g / bigG vision towers (model_hd 80, 88 or 104 in heads of 96 or 128). */
+int b200_debug_attention_padded(int device, const void* qkv, int B, int S, int W, int H, int model_hd, int mask,
+                                const int32_t* kv_len, void* out, void* stream);
 /* MPNet's relative_position_bucket as the model builds its bias table: out[d + max_len - 1] = bucket of
  * key - query = d for |d| < max_len (host-only). */
 int b200_debug_relative_position_buckets(int num_buckets, int max_distance, int max_len, int32_t* out);

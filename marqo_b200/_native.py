@@ -50,7 +50,7 @@ class ModelDesc(C.Structure):
         ("resnet_layers", C.c_int32 * 4), ("resnet_width", C.c_int32), ("resnet_heads", C.c_int32),
         ("resnet_image_size", C.c_int32),
         ("convnext_dims", C.c_int32 * 4), ("convnext_depths", C.c_int32 * 4), ("convnext_image_size", C.c_int32),
-        ("convnext_head", C.c_int32),
+        ("convnext_head", C.c_int32), ("resize_squash", C.c_int32),
     ]
 
 
@@ -123,6 +123,8 @@ _SIGNATURES = {
     "b200_debug_gemm_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "b200_debug_patch_embed": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, _P]),
     "b200_debug_attention": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P]),
+    "b200_debug_attention_padded": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P,
+                                              _P]),
     "b200_debug_relative_position_buckets": (C.c_int, [C.c_int, C.c_int, C.c_int, _P]),
     "b200_debug_attention_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                             C.POINTER(C.c_float)]),

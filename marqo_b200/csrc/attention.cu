@@ -175,9 +175,14 @@ attention_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
 }
 
 int launch(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask, const int32_t* kv_len,
-           const RelBias& bias, cudaStream_t stream) {
+           const RelBias& bias, cudaStream_t stream, int model_hd) {
     if (B <= 0 || S <= 0) return 0;
     const int hd = head_dim(W, H);
+    if (hd > 64 && S < 128)
+        fail(B200_ERR_UNSUPPORTED, "attention: head_dim %d runs sequences of at least 128 tokens (S = %d)", hd, S);
+    if (model_hd < 0 || model_hd > hd)
+        fail(B200_ERR_INVALID_ARG, "attention: model head_dim %d does not fit kernel head_dim %d", model_hd, hd);
+    const float scale_log2e = head_scale_log2e(model_hd ? model_hd : hd);
     if (bias.table) {
         if (hd != 64 || mask != MASK_KEYLEN)
             fail(B200_ERR_UNSUPPORTED, "attention: the relative bias is built for head_dim 64 with the key-length mask");
@@ -191,13 +196,13 @@ int launch(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, in
         fail(B200_ERR_INTERNAL, "attention: unknown mask mode %d", mask);
     if (mask == MASK_KEYLEN && !kv_len) fail(B200_ERR_INTERNAL, "attention: kv_len required for key-length masking");
     if (S >= 128) {
-        launch_wgmma_kernel(qkv, out, B, S, W, H, hd, mask, kv_len, bias, stream);
+        launch_wgmma_kernel(qkv, out, B, S, W, H, hd, mask, kv_len, bias, scale_log2e, stream);
     } else {
-        dispatch(hd, mask, bias.table != nullptr, [&](auto d, auto m, auto with_bias) {
+        dispatch<false>(hd, mask, bias.table != nullptr, [&](auto d, auto m, auto with_bias) {
             constexpr int HD = decltype(d)::value, MASK = decltype(m)::value;
             constexpr bool BIAS = decltype(with_bias)::value;
             attention_kernel<HD, MASK, BIAS><<<dim3((S + BQ - 1) / BQ, H, B), THREADS, 0, stream>>>(
-                qkv, out, S, W, kv_len, head_scale_log2e(HD), bias.table, bias.smax);
+                qkv, out, S, W, kv_len, scale_log2e, bias.table, bias.smax);
         });
     }
     MB_CUDA(cudaGetLastError());

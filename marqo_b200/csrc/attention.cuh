@@ -1,11 +1,14 @@
-// Multi-head attention over packed QKV (head_dim 32 or 64), flash-style online softmax in fp32, one CTA per (64 queries, head,
-// sequence).  launch() validates the arguments once and picks the kernel:
+// Multi-head attention over packed QKV (head_dim 32 or 64; 96 or 128 for S >= 128), flash-style online softmax in fp32,
+// one CTA per (64 queries, head, sequence).  launch() validates the arguments once and picks the kernel:
 //   S >= 128: wgmma kernel (attention_wgmma.cu) — TMA-fed 128-key K / V tiles, one MMA warpgroup, P from registers.
 //   S <  128: warp-level kernel (attention.cu, mma.sync m16n8k16, 64-key blocks) — a ViT-B-32 (50 tokens) or CLIP text
 //             (77 tokens) sequence would leave 40-60 % of a 128-key wgmma tile masked.
+// Head dims 96 and 128 serve the ViT-H / g / bigG vision towers (257 or 730 tokens), whose heads of 80, 88 and 104
+// columns the model pads with zero columns (model.cu: pad_heads); the logits keep the model head dim's scale.
 // Both kernels hold the scores in the same register layout and run the online softmax below on it (OnlineSoftmax); each
 // keeps only its data movement, its MMAs and its output stores.
 #pragma once
+#include <cmath>
 #include <type_traits>
 
 #include "common.cuh"
@@ -28,32 +31,40 @@ struct RelBias {
 constexpr int MAX_BIAS_S = 1024;   // the wgmma kernel's shared-memory limit covers the band of up to this many keys
 
 // qkv: bf16 [B*S, 3*W] rows = tokens, columns = [q | k | v], head h occupies columns h*D..h*D+D-1 of each part, where
-// D = W / H is the head dim, 32 or 64; both kernels take it as the compile-time parameter HD.
+// D = W / H is the kernel head dim, 32 or 64 (either kernel) or 96 or 128 (S >= 128); the kernels take it as the
+// compile-time parameter HD.  model_hd: the head dim whose 1 / sqrt scales the logits, when the heads carry zero pad
+// columns up to D; 0 means D.
 // out: bf16 [B*S, W].  kv_len: int32 [B] valid key count per sequence (MASK_KEYLEN only).
-// Errors: a head dim other than 32 / 64, B > 65535 (gridDim.z), a bias without head_dim 64 and MASK_KEYLEN or with
-// S > MAX_BIAS_S: B200_ERR_UNSUPPORTED; a bias with S > smax: B200_ERR_INVALID_ARG; an unknown mask or MASK_KEYLEN
-// without kv_len: B200_ERR_INTERNAL.  Returns the number of kernels launched.
+// Errors: a head dim other than 32 / 64 / 96 / 128, head dim 96 / 128 with S < 128, B > 65535 (gridDim.z), a bias
+// without head_dim 64 and MASK_KEYLEN or with S > MAX_BIAS_S: B200_ERR_UNSUPPORTED; a bias with S > smax or a model_hd
+// outside 1..D: B200_ERR_INVALID_ARG; an unknown mask or MASK_KEYLEN without kv_len: B200_ERR_INTERNAL.  Returns the
+// number of kernels launched.
 int launch(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int mask, const int32_t* kv_len,
-           const RelBias& bias, cudaStream_t stream);
+           const RelBias& bias, cudaStream_t stream, int model_hd = 0);
 
 // The wgmma kernel's launch (attention_wgmma.cu), for arguments launch() has validated; launch() runs it for S >= 128.
 void launch_wgmma_kernel(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int hd, int mask,
-                         const int32_t* kv_len, const RelBias& bias, cudaStream_t stream);
+                         const int32_t* kv_len, const RelBias& bias, float scale_log2e, cudaStream_t stream);
 
-// W / H when it is a head dim the kernels are built for (32 or 64); anything else fails with B200_ERR_UNSUPPORTED.
+// W / H when it is a head dim the kernels are built for (32, 64, 96 or 128); anything else fails with
+// B200_ERR_UNSUPPORTED.
 inline int head_dim(int W, int H) {
-    if (H > 0 && W == H * 64) return 64;
-    if (H > 0 && W == H * 32) return 32;
-    fail(B200_ERR_UNSUPPORTED, "attention: head_dim must be 32 or 64 (width %d, heads %d)", W, H);
+    for (int hd : {64, 32, 96, 128})
+        if (H > 0 && W == H * hd) return hd;
+    fail(B200_ERR_UNSUPPORTED, "attention: head_dim must be 32, 64, 96 or 128 (width %d, heads %d)", W, H);
 }
 
-// softmax scale 1/sqrt(head_dim), times log2(e): the kernels exponentiate with exp2
-inline float head_scale_log2e(int hd) { return (hd == 64 ? 0.125f : 0.17677669529663687f) * 1.4426950408889634f; }
+// softmax scale 1/sqrt(hd), times log2(e): the kernels exponentiate with exp2.  hd 32 and 64 keep their fp32 constants.
+inline float head_scale_log2e(int hd) {
+    const float scale = hd == 64 ? 0.125f : hd == 32 ? 0.17677669529663687f : (float)(1.0 / std::sqrt((double)hd));
+    return scale * 1.4426950408889634f;
+}
 
 // Calls f(std::integral_constant<int, HD>, std::integral_constant<int, MASK>, std::bool_constant<BIAS>) for the
-// instantiation of (hd, mask, bias) that launch() has accepted: the one list of the instantiations both kernels serve,
-// {32, 64} x {none, causal, key length} without the bias, and <64, MASK_KEYLEN, true>.
-template <class F>
+// instantiation of (hd, mask, bias) that launch() has accepted: the one list of the instantiations the kernels serve,
+// {32, 64} x {none, causal, key length} without the bias, and <64, MASK_KEYLEN, true>; WIDE (the wgmma kernel only)
+// adds {96, 128} x {none, causal, key length} without the bias.
+template <bool WIDE, class F>
 void dispatch(int hd, int mask, bool bias, F&& f) {
     if (bias) return f(std::integral_constant<int, 64>{}, std::integral_constant<int, MASK_KEYLEN>{}, std::true_type{});
     const auto with_mask = [&](auto d) {
@@ -64,6 +75,10 @@ void dispatch(int hd, int mask, bool bias, F&& f) {
         else
             f(d, std::integral_constant<int, MASK_KEYLEN>{}, std::false_type{});
     };
+    if constexpr (WIDE) {
+        if (hd == 96) return with_mask(std::integral_constant<int, 96>{});
+        if (hd == 128) return with_mask(std::integral_constant<int, 128>{});
+    }
     if (hd == 64)
         with_mask(std::integral_constant<int, 64>{});
     else

@@ -5,8 +5,11 @@
 //               (attention.cuh: OnlineSoftmax) on the accumulator registers, then O += P V with
 //               wgmma m64n{HD}k16 taking P from registers (bf16, the m16n8k16 A fragment the S accumulator layout maps
 //               to) and V as the transposed (MN-major) B operand.
-// The head dim HD (32 or 64) is a template parameter.  A Q / K / V row is HD * 2 bytes, so HD = 64 tiles use the 128-byte
-// swizzle and HD = 32 tiles the 64-byte one, in the tensor maps and in the wgmma descriptors alike.
+// The head dim HD (32, 64, 96 or 128) is a template parameter.  A tile's HD columns are stored as one or two column blocks
+// (Tiles), each its own TMA box: block 0 holds the first min(HD, 64) columns, block 1 the HD - 64 after them (HD 96:
+// 32, HD 128: 64).  A block of 64 columns (128-byte rows) uses the 128-byte swizzle and one of 32 the 64-byte one, in
+// the tensor maps and in the wgmma descriptors alike.  QK^T takes each 16-column k-step from the block it falls in;
+// P V issues one wgmma per block, each into its own columns of O.
 // Keys past the sequence's length (S, kv_len[b]) and, for MASK_CAUSAL, past the query are masked to -inf; the tiles TMA
 // reads beyond a sequence belong to the next one (or are zero-filled past the matrix) and only ever meet masked scores.
 #include <mutex>
@@ -25,28 +28,42 @@ constexpr int THREADS = 160;
 
 template <int HD>
 struct Tiles {
+    static constexpr int C0 = HD < 64 ? HD : 64;   // columns of block 0
+    static constexpr int C1 = HD - C0;             // columns of block 1 (0: none)
+    static constexpr int NB = C1 > 0 ? 2 : 1;      // column blocks
     static constexpr uint32_t Q_BYTES = BQ * HD * 2;
+    static constexpr uint32_t Q1_OFFSET = BQ * C0 * 2;       // block 1 of the Q tile
     static constexpr uint32_t KV_TILE_BYTES = BKV * HD * 2;
+    static constexpr uint32_t KV1_OFFSET = BKV * C0 * 2;     // block 1 of a K / V tile
     static constexpr uint32_t STAGE_BYTES = 2 * KV_TILE_BYTES;   // K then V
     static constexpr size_t SMEM_BYTES = Q_BYTES + KV_STAGES * STAGE_BYTES + 1024 /*align*/ + 64 /*barriers*/;
+    // every block starts on a multiple of the 128-byte swizzle's 1024-byte atom
+    static_assert(Q1_OFFSET % 1024 == 0 && Q_BYTES % 1024 == 0 && KV1_OFFSET % 1024 == 0 && KV_TILE_BYTES % 1024 == 0);
 };
 
-// K-major descriptor of a Q / K tile, and MN-major descriptor of a V tile, for the swizzle that goes with HD
+// The TMA descriptors of the Q tiles and of the K / V tiles, one pair per column block
 template <int HD>
+struct TensorMaps {
+    CUtensorMap q[Tiles<HD>::NB], kv[Tiles<HD>::NB];
+};
+
+// K-major descriptor of a Q / K column block, and MN-major descriptor of a V column block, of C columns: the swizzle
+// that goes with C
+template <int C>
 __device__ __forceinline__ uint64_t desc_k(uint32_t smem_addr) {
-    if constexpr (HD == 64) return ptx::make_desc_k_sw128(smem_addr);
+    if constexpr (C == 64) return ptx::make_desc_k_sw128(smem_addr);
     else return ptx::make_desc_k_sw64(smem_addr);
 }
-template <int HD>
+template <int C>
 __device__ __forceinline__ uint64_t desc_mn(uint32_t smem_addr) {
-    if constexpr (HD == 64) return ptx::make_desc_mn_sw128(smem_addr, 0);
+    if constexpr (C == 64) return ptx::make_desc_mn_sw128(smem_addr, 0);
     else return ptx::make_desc_mn_sw64(smem_addr, 0);
 }
 
-// O[64 x HD] += P[64 x 16] V[16 x HD]
-template <int HD>
-__device__ __forceinline__ void wgmma_pv(float (&o)[HD / 2], const uint32_t (&a)[4], uint64_t desc_v) {
-    if constexpr (HD == 64) ptx::wgmma_m64n64k16_bf16_rs_tb(o, a, desc_v, 1u);
+// O[64 x C] += P[64 x 16] V[16 x C]: C columns of O, one column block of V
+template <int C>
+__device__ __forceinline__ void wgmma_pv(float (&o)[C / 2], const uint32_t (&a)[4], uint64_t desc_v) {
+    if constexpr (C == 64) ptx::wgmma_m64n64k16_bf16_rs_tb(o, a, desc_v, 1u);
     else ptx::wgmma_m64n32k16_bf16_rs_tb(o, a, desc_v, 1u);
 }
 
@@ -57,12 +74,14 @@ inline size_t bias_band_bytes(int S) { return ((size_t)(S + BKV - 1) / BKV * BKV
 // staged in shared memory behind the barriers.
 template <int HD, int MASK, bool BIAS>
 __global__ void __launch_bounds__(THREADS)
-attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
-                       __nv_bfloat16* __restrict__ out, int S, int W, const int32_t* __restrict__ kv_len,
-                       float scale_log2e, const float* __restrict__ rel_bias, int bias_smax) {
-    constexpr uint32_t Q_BYTES = Tiles<HD>::Q_BYTES;
-    constexpr uint32_t KV_TILE_BYTES = Tiles<HD>::KV_TILE_BYTES;
-    constexpr uint32_t STAGE_BYTES = Tiles<HD>::STAGE_BYTES;
+attention_wgmma_kernel(const __grid_constant__ TensorMaps<HD> tmaps, __nv_bfloat16* __restrict__ out, int S, int W,
+                       const int32_t* __restrict__ kv_len, float scale_log2e, const float* __restrict__ rel_bias,
+                       int bias_smax) {
+    using T = Tiles<HD>;
+    constexpr int C0 = T::C0, C1 = T::C1;
+    constexpr uint32_t Q_BYTES = T::Q_BYTES;
+    constexpr uint32_t KV_TILE_BYTES = T::KV_TILE_BYTES;
+    constexpr uint32_t STAGE_BYTES = T::STAGE_BYTES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sq = smem;
@@ -93,14 +112,22 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
         // ------------------------------------------------------------ TMA producer
         if (lane == 0 && nkb > 0) {
             ptx::mbar_arrive_expect_tx(qfull, Q_BYTES);
-            ptx::tma_load_2d(sq, &tmap_q, qfull, h * HD, row0 + q0, ptx::kEvictFirst);
+            ptx::tma_load_2d(sq, &tmaps.q[0], qfull, h * HD, row0 + q0, ptx::kEvictFirst);
+            if constexpr (C1 > 0)
+                ptx::tma_load_2d(sq + T::Q1_OFFSET, &tmaps.q[1], qfull, h * HD + C0, row0 + q0, ptx::kEvictFirst);
             for (int j = 0; j < nkb; ++j) {
                 const int st = j % KV_STAGES;
                 ptx::mbar_wait(&empty[st], ((uint32_t)(j / KV_STAGES) & 1u) ^ 1u);
                 ptx::mbar_arrive_expect_tx(&full[st], STAGE_BYTES);
                 uint8_t* dst = skv + (size_t)st * STAGE_BYTES;
-                ptx::tma_load_2d(dst, &tmap_kv, &full[st], W + h * HD, row0 + j * BKV, ptx::kEvictLast);
-                ptx::tma_load_2d(dst + KV_TILE_BYTES, &tmap_kv, &full[st], 2 * W + h * HD, row0 + j * BKV, ptx::kEvictLast);
+                ptx::tma_load_2d(dst, &tmaps.kv[0], &full[st], W + h * HD, row0 + j * BKV, ptx::kEvictLast);
+                ptx::tma_load_2d(dst + KV_TILE_BYTES, &tmaps.kv[0], &full[st], 2 * W + h * HD, row0 + j * BKV, ptx::kEvictLast);
+                if constexpr (C1 > 0) {
+                    ptx::tma_load_2d(dst + T::KV1_OFFSET, &tmaps.kv[1], &full[st], W + h * HD + C0, row0 + j * BKV,
+                                     ptx::kEvictLast);
+                    ptx::tma_load_2d(dst + KV_TILE_BYTES + T::KV1_OFFSET, &tmaps.kv[1], &full[st], 2 * W + h * HD + C0,
+                                     row0 + j * BKV, ptx::kEvictLast);
+                }
             }
         }
         return;
@@ -123,16 +150,27 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
         float s[BKV / 2];
         ptx::wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < HD / 16; ++k)
-            ptx::wgmma_m64n128k16_bf16(s, desc_k<HD>(q_base + k * 32), desc_k<HD>(k_base + k * 32), k != 0 ? 1u : 0u);
+        for (int k = 0; k < C0 / 16; ++k)
+            ptx::wgmma_m64n128k16_bf16(s, desc_k<C0>(q_base + k * 32), desc_k<C0>(k_base + k * 32), k != 0 ? 1u : 0u);
+        if constexpr (C1 > 0) {
+#pragma unroll
+            for (int k = 0; k < C1 / 16; ++k)
+                ptx::wgmma_m64n128k16_bf16(s, desc_k<C1>(q_base + T::Q1_OFFSET + k * 32),
+                                           desc_k<C1>(k_base + T::KV1_OFFSET + k * 32), 1u);
+        }
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         uint32_t pa[BKV / 16][4];
         sm.update(s, o, pa, j * BKV);
-        // ---- O += P V (64 x HD, K = 128 keys; 16 keys = 16 V rows of HD * 2 bytes per k-step)
+        // ---- O += P V (64 x HD, K = 128 keys; 16 keys = 16 V rows of C * 2 bytes of each column block per k-step)
         ptx::wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BKV / 16; ++k) wgmma_pv<HD>(o, pa[k], desc_mn<HD>(v_base + k * 32 * HD));
+        for (int k = 0; k < BKV / 16; ++k) {
+            wgmma_pv<C0>(*reinterpret_cast<float(*)[C0 / 2]>(o), pa[k], desc_mn<C0>(v_base + k * 32 * C0));
+            if constexpr (C1 > 0)
+                wgmma_pv<C1>(*reinterpret_cast<float(*)[C1 / 2]>(o + C0 / 2), pa[k],
+                             desc_mn<C1>(v_base + T::KV1_OFFSET + k * 32 * C1));
+        }
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         __syncwarp();
@@ -152,20 +190,27 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_
     }
 }
 
-// Q tiles of BQ rows and K / V tiles of BKV rows out of the packed qkv matrix
+// Q tiles of BQ rows and K / V tiles of BKV rows out of the packed qkv matrix, per column block
 template <int HD>
-void make_tmaps(const __nv_bfloat16* qkv, int B, int S, int W, CUtensorMap& tq, CUtensorMap& tkv) {
+TensorMaps<HD> make_tmaps(const __nv_bfloat16* qkv, int B, int S, int W) {
     const uint64_t rows = (uint64_t)B * S;
-    const CUtensorMapSwizzle swz = HD == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-    tq = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows, (uint64_t)3 * W * 2, HD, BQ, swz);
-    tkv = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows, (uint64_t)3 * W * 2, HD, BKV, swz);
+    TensorMaps<HD> t;
+    for (int i = 0; i < Tiles<HD>::NB; ++i) {
+        const uint32_t cols = i == 0 ? Tiles<HD>::C0 : Tiles<HD>::C1;
+        const CUtensorMapSwizzle swz = cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+        t.q[i] = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows, (uint64_t)3 * W * 2, cols,
+                              BQ, swz);
+        t.kv[i] = make_tmap_2d(qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (uint64_t)3 * W, rows, (uint64_t)3 * W * 2,
+                               cols, BKV, swz);
+    }
+    return t;
 }
 
 }  // namespace
 
 void launch_wgmma_kernel(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int S, int W, int H, int hd, int mask,
-                         const int32_t* kv_len, const RelBias& bias, cudaStream_t stream) {
-    dispatch(hd, mask, bias.table != nullptr, [&](auto d, auto m, auto with_bias) {
+                         const int32_t* kv_len, const RelBias& bias, float scale_log2e, cudaStream_t stream) {
+    dispatch<true>(hd, mask, bias.table != nullptr, [&](auto d, auto m, auto with_bias) {
         constexpr int HD = decltype(d)::value, MASK = decltype(m)::value;
         constexpr bool BIAS = decltype(with_bias)::value;
         constexpr size_t BASE = Tiles<HD>::SMEM_BYTES;
@@ -175,11 +220,9 @@ void launch_wgmma_kernel(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, in
                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)(BASE + (BIAS ? bias_band_bytes(MAX_BIAS_S) : 0))));
         });
-        CUtensorMap tq, tkv;
-        make_tmaps<HD>(qkv, B, S, W, tq, tkv);
         attention_wgmma_kernel<HD, MASK, BIAS>
             <<<dim3((S + BQ - 1) / BQ, H, B), THREADS, BASE + (BIAS ? bias_band_bytes(S) : 0), stream>>>(
-                tq, tkv, out, S, W, kv_len, head_scale_log2e(HD), bias.table, bias.smax);
+                make_tmaps<HD>(qkv, B, S, W), out, S, W, kv_len, scale_log2e, bias.table, bias.smax);
     });
 }
 

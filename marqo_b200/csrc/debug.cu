@@ -195,6 +195,20 @@ int b200_debug_attention(int device, const void* qkv, int B, int S, int W, int H
     });
 }
 
+int b200_debug_attention_padded(int device, const void* qkv, int B, int S, int W, int H, int model_hd, int mask,
+                                const int32_t* kv_len, void* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(qkv && out, "NULL buffer");
+        MB_CHECK_ARG(B > 0 && S > 0 && W > 0 && H > 0 && model_hd > 0, "B, S, W, H, model_hd must be positive");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        attention::launch(static_cast<const bf16*>(qkv), static_cast<bf16*>(out), B, S, W, H, mask, kv_len,
+                          attention::RelBias{}, s, model_hd);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
 int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, int rel_bias, int iters, float* out_ms) {
     return guarded([&] {
         MB_CHECK_ARG(out_ms != nullptr, "NULL buffer");

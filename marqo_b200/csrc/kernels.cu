@@ -16,26 +16,28 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 // ------------------------------------------------------------------------------------------------ LayerNorm
 // One warp per row, the whole row lives in registers (two-pass mean / variance like torch's CPU kernel).
-constexpr int LN_MAX_V4 = 8;  // w <= 1024
+constexpr int LN_MAX_V4 = 8;        // w <= 1024: every tower but the ViT-H / g / bigG ones
+constexpr int LN_WIDE_MAX_V4 = 13;  // w <= 1664: layernorm() only, in its own instantiation so that the rows of up to
+                                    // 1024 keep their code (and bits)
 
-template <bool GATHER_EMBED>
-__device__ __forceinline__ void ln_row(float4 (&v)[LN_MAX_V4], int nv, int w, const float* gamma, const float* beta,
+template <bool GATHER_EMBED, int MAXV = LN_MAX_V4>
+__device__ __forceinline__ void ln_row(float4 (&v)[MAXV], int nv, int w, const float* gamma, const float* beta,
                                        float eps, int lane, float* of, __nv_bfloat16* ob) {
     float s = 0.f;
 #pragma unroll
-    for (int j = 0; j < LN_MAX_V4; ++j)
+    for (int j = 0; j < MAXV; ++j)
         if (j < nv) s += v[j].x + v[j].y + v[j].z + v[j].w;
     const float mean = warp_sum(s) / (float)w;
     float q = 0.f;
 #pragma unroll
-    for (int j = 0; j < LN_MAX_V4; ++j)
+    for (int j = 0; j < MAXV; ++j)
         if (j < nv) {
             const float a = v[j].x - mean, b = v[j].y - mean, c = v[j].z - mean, d = v[j].w - mean;
             q += a * a + b * b + c * c + d * d;
         }
     const float rstd = 1.0f / sqrtf(warp_sum(q) / (float)w + eps);
 #pragma unroll
-    for (int j = 0; j < LN_MAX_V4; ++j)
+    for (int j = 0; j < MAXV; ++j)
         if (j < nv) {
             const int i4 = lane + 32 * j;
             const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + i4);
@@ -54,6 +56,7 @@ __device__ __forceinline__ void ln_row(float4 (&v)[LN_MAX_V4], int nv, int w, co
 // order, so the rows it wrote last — the ones most likely still in the 126 MB L2 — are read first, and the bf16 rows this
 // kernel writes last are the low ones the next GEMM (ascending again) starts with.  `reverse` = 0 restores the forward order
 // (MARQO_B200_LN_FORWARD=1, A/B timing).
+template <int MAXV>
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ x, long long in_stride,
                                                         const float* __restrict__ gamma, const float* __restrict__ beta,
                                                         float eps, int rows, int w, float* out_f32,
@@ -64,24 +67,30 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
     if (reverse) row = rows - 1 - row;
     const int nv = w / 128;
     const float4* src = reinterpret_cast<const float4*>(x + (long long)row * in_stride);
-    float4 v[LN_MAX_V4];
+    float4 v[MAXV];
 #pragma unroll
-    for (int j = 0; j < LN_MAX_V4; ++j)
+    for (int j = 0; j < MAXV; ++j)
         if (j < nv) v[j] = src[lane + 32 * j];
-    ln_row<false>(v, nv, w, gamma, beta, eps, lane, out_f32 ? out_f32 + (long long)row * w : nullptr,
-                  out_bf16 ? out_bf16 + (long long)row * w : nullptr);
+    ln_row<false, MAXV>(v, nv, w, gamma, beta, eps, lane, out_f32 ? out_f32 + (long long)row * w : nullptr,
+                        out_bf16 ? out_bf16 + (long long)row * w : nullptr);
 }
 
-static void check_ln_width(int w) {
-    if (w % 128 != 0 || w > 128 * LN_MAX_V4) fail(B200_ERR_UNSUPPORTED, "width %d must be a multiple of 128 and <= 1024", w);
+static void check_ln_width(int w, int max_v4 = LN_MAX_V4) {
+    if (w % 128 != 0 || w > 128 * max_v4)
+        fail(B200_ERR_UNSUPPORTED, "width %d must be a multiple of 128 and <= %d", w, 128 * max_v4);
 }
 
 int layernorm(const float* x, long long in_stride, const float* gamma, const float* beta, float eps, int rows, int w,
               float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s) {
     if (rows <= 0) return 0;
-    check_ln_width(w);
+    check_ln_width(w, LN_WIDE_MAX_V4);
     static const int reverse = getenv("MARQO_B200_LN_FORWARD") == nullptr ? 1 : 0;
-    layernorm_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, in_stride, gamma, beta, eps, rows, w, out_f32, out_bf16, reverse);
+    if (w <= 128 * LN_MAX_V4)
+        layernorm_kernel<LN_MAX_V4>
+            <<<(rows + 7) / 8, 256, 0, s>>>(x, in_stride, gamma, beta, eps, rows, w, out_f32, out_bf16, reverse);
+    else
+        layernorm_kernel<LN_WIDE_MAX_V4>
+            <<<(rows + 7) / 8, 256, 0, s>>>(x, in_stride, gamma, beta, eps, rows, w, out_f32, out_bf16, reverse);
     MB_CUDA(cudaGetLastError());
     return 1;
 }

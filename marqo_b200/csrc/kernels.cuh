@@ -7,7 +7,7 @@
 namespace mb {
 namespace kernels {
 
-// y = LayerNorm(x) * gamma + beta over rows of width w (w % 128 == 0, w <= 1024).  Row r is read at
+// y = LayerNorm(x) * gamma + beta over rows of width w (w % 128 == 0, w <= 1664).  Row r is read at
 // x + r * in_stride (floats).  Writes fp32 (out_f32, may alias x) and/or bf16 (out_bf16), both compact [rows, w].
 int layernorm(const float* x, long long in_stride, const float* gamma, const float* beta, float eps, int rows, int w,
               float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s);

@@ -11,8 +11,8 @@
 //             embeddings / projections
 //   x         fp32 [tokens, width]   residual stream (kept fp32 end to end)
 //   h         bf16 [tokens, width]   LayerNorm output = GEMM A operand
-//   qkv       bf16 [tokens, 3*width] fused QKV projection
-//   o         bf16 [tokens, width]   attention output
+//   qkv       bf16 [tokens, 3*aw]    fused QKV projection (aw: TowerW::aw, the width with zero-padded heads)
+//   o         bf16 [tokens, aw]      attention output
 //   u         bf16 [tokens, mlp]     MLP hidden
 //   patches   bf16 [images * (grid^2 + 1), kpad]  im2col of preprocessed fp32 CHW input (zero class-token rows)
 // Every Linear is the wgmma GEMM of gemm.cu with bias / activation / residual-add fused into its epilogue.
@@ -61,6 +61,9 @@ struct Kinds {
 
 struct TowerW {
     b200_tower_desc d{};
+    // the attention width heads * kernel_head_dim(width / heads): width, or for the ViT-H / g / bigG vision towers the
+    // width with every head zero-padded to the kernel's head dim (pad_heads)
+    int aw = 0;
     std::vector<LayerW> layers;
     float eps = 1e-5f;                      // every LayerNorm of the tower
     int act = gemm::ACT_GELU;               // the MLP's activation
@@ -203,12 +206,21 @@ T* derived_buffer(b200_model* m, size_t n) {
     return reinterpret_cast<T*>(m->derived.back().get());
 }
 
-void check_tower(const b200_tower_desc& t, const char* name) {
-    MB_CHECK_ARG(t.width > 0 && t.width % 128 == 0 && t.width <= 1024, "%s.width %d must be a multiple of 128, <= 1024",
-                 name, t.width);
+// The attention kernels' head dim for a tower's head dim hd: hd itself for 32 and 64; 80 and 88 run as 96 and 104 as
+// 128, each head padded with zero columns (pad_heads).
+int kernel_head_dim(int hd) { return hd <= 64 ? hd : hd <= 96 ? 96 : 128; }
+
+// max_width: 1664 for the CLIP towers (their LayerNorm and head kernels), 1024 for the others.  padded_heads: the tower
+// may have head dims 80, 88 and 104, which only the wgmma attention kernel runs (kernel_head_dim), so only a vision
+// tower of at least 128 tokens takes them.
+void check_tower(const b200_tower_desc& t, const char* name, int max_width = 1024, bool padded_heads = false) {
+    MB_CHECK_ARG(t.width > 0 && t.width % 128 == 0 && t.width <= max_width, "%s.width %d must be a multiple of 128, <= %d",
+                 name, t.width, max_width);
     MB_CHECK_ARG(t.layers > 0, "%s.layers must be positive", name);
-    MB_CHECK_ARG(t.heads > 0 && (t.width == t.heads * 32 || t.width == t.heads * 64),
-                 "%s: head_dim must be 32 or 64 (width %d, heads %d)", name, t.width, t.heads);
+    const int hd = t.heads > 0 && t.width % t.heads == 0 ? t.width / t.heads : 0;
+    const bool padded = padded_heads && (hd == 80 || hd == 88 || hd == 104);
+    MB_CHECK_ARG(hd == 32 || hd == 64 || padded, "%s: head_dim must be 32 or 64%s (width %d, heads %d)", name,
+                 padded_heads ? ", or 80, 88 or 104" : "", t.width, t.heads);
     MB_CHECK_ARG(t.mlp > 0 && t.mlp % 64 == 0, "%s.mlp %d must be a multiple of 64", name, t.mlp);
 }
 
@@ -292,17 +304,21 @@ void check_vision(const b200_model_desc& d, VisionKind kind) {
         MB_CHECK_ARG(d.vision.width == d.vision.heads * 64, "SigLIP: vision head_dim must be 64 (width %d, heads %d)",
                      d.vision.width, d.vision.heads);
         [[fallthrough]];
-    case VisionKind::CLIP_VIT:
-        check_tower(d.vision, "vision");
+    case VisionKind::CLIP_VIT: {
         MB_CHECK_ARG(d.vision.patch > 0 && d.vision.image_size % d.vision.patch == 0,
                      "image_size must be a multiple of patch");
+        const bool clip = kind == VisionKind::CLIP_VIT;
+        const int grid = d.vision.image_size / d.vision.patch;
+        check_tower(d.vision, "vision", clip ? 1664 : 1024, clip && grid * grid + 1 >= 128);
         break;
     }
+    }
+    MB_CHECK_ARG(d.resize_squash == 0 || d.resize_squash == 1, "resize_squash %d must be 0 or 1", d.resize_squash);
 }
 
 void check_text(const b200_model_desc& d, const Kinds& k) {
     if (k.text == TextKind::NONE) return;
-    check_tower(d.text, "text");
+    check_tower(d.text, "text", k.text == TextKind::CLIP ? 1664 : 1024);
     MB_CHECK_ARG(d.text.ctx > 0 && d.text.vocab > 0, "text.ctx and text.vocab must be positive");
     switch (k.text) {
     case TextKind::SIGLIP:
@@ -357,18 +373,51 @@ const PreLnNames OPEN_CLIP_BLOCK{"ln_1", "attn.in_proj_weight", "attn.in_proj_bi
                                  "mlp.c_proj"};
 const PreLnNames TIMM_BLOCK{"norm1", "attn.qkv.weight", "attn.qkv.bias", "attn.proj", "norm2", "mlp.fc1", "mlp.fc2"};
 
+// fp32 parameter `name`, [rows, nb * blk] row-major, with column block i moved to columns i * pblk .. i * pblk + blk - 1
+// of [rows, nb * pblk] and zeros in the other columns: replaces the uploaded parameter.
+void pad_blocks(b200_model* m, const std::string& name, long long rows, int nb, long long blk, long long pblk) {
+    const float* src = param(m, name, rows * nb * blk);
+    DeviceBuffer<float> dst((size_t)(rows * nb * pblk));
+    MB_CUDA(cudaMemsetAsync(dst.get(), 0, dst.size() * sizeof(float), m->stream));
+    for (int i = 0; i < nb; ++i) {
+        if (rows == 1)
+            MB_CUDA(cudaMemcpyAsync(dst.get() + i * pblk, src + i * blk, blk * sizeof(float), cudaMemcpyDeviceToDevice,
+                                    m->stream));
+        else
+            MB_CUDA(cudaMemcpy2DAsync(dst.get() + i * pblk, nb * pblk * sizeof(float), src + i * blk,
+                                      nb * blk * sizeof(float), blk * sizeof(float), rows, cudaMemcpyDeviceToDevice,
+                                      m->stream));
+    }
+    MB_CUDA(cudaStreamSynchronize(m->stream));
+    m->raw[name] = std::move(dst);
+}
+
+// The zero-padded head layout of a tower whose attention width T.aw exceeds its width (kernel_head_dim): head h of q,
+// k and v takes rows h * hdp .. h * hdp + hd - 1 of its part's H * hdp rows of the QKV weight and bias, zero rows and
+// zero bias after them, and the out-projection's K dimension has zero columns at the same places.  The QKV GEMM then
+// writes exact zeros into the pad columns, QK^T gains exact 0 * 0 terms, the pad columns of the attention output are
+// P * 0 = 0 and meet zero weights in the out-projection: the result is the unpadded one up to fp32 summation order.
+void pad_heads(b200_model* m, const TowerW& T, const std::string& p, const PreLnNames& nm) {
+    const long long w = T.d.width, H = T.d.heads, hd = w / H, hdp = T.aw / H;
+    if (hdp == hd) return;
+    pad_blocks(m, p + nm.qkv_w, 1, (int)(3 * H), hd * w, hdp * w);
+    pad_blocks(m, p + nm.qkv_b, 1, (int)(3 * H), hd, hdp);
+    pad_blocks(m, p + nm.out + ".weight", w, (int)H, hd, hdp);
+}
+
 // blocks: the prefix of block i's names up to the index ("visual.transformer.resblocks.", "visual.trunk.blocks.", ...)
 void build_preln_layers(b200_model* m, TowerW& T, const std::string& blocks, const PreLnNames& nm) {
-    const long long w = T.d.width, mlp = T.d.mlp;
+    const long long w = T.d.width, aw = T.aw, mlp = T.d.mlp;
     T.layers.resize(T.d.layers);
     for (int i = 0; i < T.d.layers; ++i) {
         const std::string p = blocks + std::to_string(i) + ".";
         LayerW& L = T.layers[i];
         L.ln1_w = param(m, p + nm.ln1 + ".weight", w);
         L.ln1_b = param(m, p + nm.ln1 + ".bias", w);
-        L.w_qkv = to_bf16(m, p + nm.qkv_w, 3 * w * w);
-        L.b_qkv = param(m, p + nm.qkv_b, 3 * w);
-        L.w_o = to_bf16(m, p + nm.out + ".weight", w * w);
+        pad_heads(m, T, p, nm);
+        L.w_qkv = to_bf16(m, p + nm.qkv_w, 3 * aw * w);
+        L.b_qkv = param(m, p + nm.qkv_b, 3 * aw);
+        L.w_o = to_bf16(m, p + nm.out + ".weight", w * aw);
         L.b_o = param(m, p + nm.out + ".bias", w);
         L.ln2_w = param(m, p + nm.ln2 + ".weight", w);
         L.ln2_b = param(m, p + nm.ln2 + ".bias", w);
@@ -862,7 +911,7 @@ void linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, con
 // Post-LN (HF BertLayer, MPNetLayer with the tower's relative-position bias): on entry x and h both hold the embedding
 // LayerNorm output, and LN rewrites x in place (x -> x and h) after each residual GEMM.
 void run_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S, int mask_mode, bool pre_ln) {
-    const int M = B * S, w = T.d.width, mlp = T.d.mlp;
+    const int M = B * S, w = T.d.width, aw = T.aw, mlp = T.d.mlp;
     float* x = m->x.get();
     const int32_t* kv_len = mask_mode == attention::MASK_KEYLEN ? m->aux.get() : nullptr;
     auto ln = [&](const float* g, const float* b) {
@@ -870,12 +919,12 @@ void run_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S, int ma
     };
     for (const LayerW& L : T.layers) {
         if (pre_ln) ln(L.ln1_w, L.ln1_b);
-        linear(m, c, m->h.get(), M, w, L.w_qkv, 3 * w, epilogue(m->qkv.get(), 3 * w, L.b_qkv));
+        linear(m, c, m->h.get(), M, w, L.w_qkv, 3 * aw, epilogue(m->qkv.get(), 3 * aw, L.b_qkv));
         profiled(m, c, 1, [&] {
-            return attention::launch(m->qkv.get(), m->o.get(), B, S, w, T.d.heads, mask_mode, kv_len, T.rel_bias,
-                                     m->stream);
+            return attention::launch(m->qkv.get(), m->o.get(), B, S, aw, T.d.heads, mask_mode, kv_len, T.rel_bias,
+                                     m->stream, w / T.d.heads);
         });
-        linear(m, c, m->o.get(), M, w, L.w_o, w, epilogue(x, w, L.b_o, gemm::ACT_NONE, true, x, w));
+        linear(m, c, m->o.get(), M, aw, L.w_o, w, epilogue(x, w, L.b_o, gemm::ACT_NONE, true, x, w));
         ln(pre_ln ? L.ln2_w : L.ln1_w, pre_ln ? L.ln2_b : L.ln1_b);
         linear(m, c, m->h.get(), M, w, L.w_fc, mlp, epilogue(m->u.get(), mlp, L.b_fc, T.act));
         linear(m, c, m->u.get(), M, mlp, L.w_proj, w, epilogue(x, w, L.b_proj, gemm::ACT_NONE, true, x, w));
@@ -1194,7 +1243,8 @@ void encode_images_u8_dev(b200_model* m, Counter& c, const uint8_t* d_img, int n
         const int nb = std::min(cap, n - o);
         const uint8_t* src = d_img + (size_t)o * h * w * 3;
         if (h != S || w != S) {
-            if (m->kind.vision == VisionKind::SIGLIP_VIT)   // open_clip's SigLIP preprocessing squashes (no crop)
+            // open_clip's SigLIP and DFN5B preprocessing squashes (no crop); every other tower crops
+            if (m->kind.vision == VisionKind::SIGLIP_VIT || m->desc.resize_squash)
                 c.n += kernels::resize_squash_u8(src, nb, h, w, S, m->resized.get(), m->stream);
             else
                 c.n += kernels::resize_crop_u8(src, nb, h, w, S, m->resized.get(), m->stream);
@@ -1257,6 +1307,8 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
             m->vision.d.width = desc->convnext_dims[0];
         }
         if (kind.text != TextKind::NONE) m->text.d = desc->text;
+        for (TowerW* T : {&m->vision, &m->text})
+            if (T->d.heads > 0) T->aw = T->d.heads * kernel_head_dim(T->d.width / T->d.heads);
         gemm::configure();
         *out = m.release();
     });
@@ -1298,20 +1350,21 @@ int b200_model_finalize(b200_model* m) {
         // workspaces for the towers' token rows, capped at ~24 GB of activations: larger calls are processed in
         // sub-batches
         const long long B = m->desc.max_batch, E = m->desc.embed_dim;
-        long long max_tok = 0, max_w = 0, max_mlp = 0;
+        long long max_tok = 0, max_w = 0, max_aw = 0, max_mlp = 0;
         for (const TowerW* T : {&m->vision, &m->text}) {
             if (T == &m->vision && m->kind.vision == VisionKind::CONVNEXT) continue;   // its own buffers (ConvnextW)
             max_tok = std::max(max_tok, B * T->tokens);   // (0 for a missing tower)
             max_w = std::max<long long>(max_w, T->d.width);
+            max_aw = std::max<long long>({max_aw, T->d.width, T->aw});   // qkv and o: padded heads are wider
             max_mlp = std::max<long long>({max_mlp, T->d.mlp, T->map.mlp});
         }
-        const long long bytes_per_tok = std::max<long long>(1, max_w * (4 + 2 + 6 + 2) + max_mlp * 2);
+        const long long bytes_per_tok = std::max<long long>(1, max_w * (4 + 2) + max_aw * (6 + 2) + max_mlp * 2);
         const long long cap_tok = (24LL << 30) / bytes_per_tok;
         m->max_tokens = std::min(max_tok, std::max<long long>(cap_tok, 1024));
         m->x = DeviceBuffer<float>((size_t)m->max_tokens * max_w);
         m->h = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_w);
-        m->qkv = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_w * 3);
-        m->o = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_w);
+        m->qkv = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_aw * 3);
+        m->o = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_aw);
         m->u = DeviceBuffer<__nv_bfloat16>((size_t)m->max_tokens * max_mlp);
         if (m->kind.vision != VisionKind::NONE) {
             const int S = m->vision.d.image_size;

@@ -292,8 +292,9 @@ class Encoder:
     """A CLIP, ResNet CLIP, ConvNeXt CLIP or SigLIP (vision + text towers), BERT, MPNet or XLM-R encoder resident on one
     GPU.
 
-    `config` keys — CLIP: embed_dim, act ("gelu"|"quickgelu"), mean, std, vision{width,layers,heads,mlp,patch,
-    image_size}, text{width,layers,heads,mlp,ctx,vocab};  SigLIP: the CLIP keys plus ln_eps (embed_dim == vision
+    `config` keys — CLIP: embed_dim, act ("gelu"|"quickgelu"), mean, std, resize_mode (optional: "squash" resizes
+    images of another size without a crop), vision{width,layers,heads,mlp,patch,image_size},
+    text{width,layers,heads,mlp,ctx,vocab};  SigLIP: the CLIP keys plus ln_eps (embed_dim == vision
     width);  ResNet CLIP ("clip_resnet"): embed_dim, act, mean, std, the text tower's width, layers, heads, mlp, ctx,
     vocab at the top level (layers 0: no text tower), resnet{layers [4], width, heads, image_size} (None: no image
     tower);  ConvNeXt CLIP ("clip_convnext"): the ResNet CLIP keys with convnext{dims [4], depths [4], image_size,
@@ -328,6 +329,9 @@ class Encoder:
                                        v["patch"])
             if t:
                 d.text = N.TowerDesc(t["width"], t["layers"], t["heads"], t["mlp"], t["ctx"], t["vocab"], 0, 0)
+            # open_clip's resize_mode "squash" (SigLIP, the DFN5B CLIP models): the GPU resize scales x and y to
+            # image_size independently instead of cropping
+            d.resize_squash = int(config.get("resize_mode") == "squash")
             self.image_size = v.get("image_size", 224) if v else 0
         elif arch == "clip_resnet":
             d.arch = N.ARCH_CLIP_RESNET

@@ -392,4 +392,4 @@ def register_with_marqo() -> None:
     """Install the two loader types into a live Marqo process (see INTEGRATION.md)."""
     from marqo.s2_inference import s2_inference as marqo_s2  # type: ignore
     marqo_s2.MODEL_PROPERTIES['loaders'].update(LOADERS)
-    marqo_s2.MODEL_PROPERTIES['models'].update({**model_registry.all_models(), **model_registry.CONVNEXT_MODELS})
+    marqo_s2.MODEL_PROPERTIES['models'].update(model_registry.served_models())

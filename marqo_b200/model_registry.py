@@ -78,7 +78,25 @@ be re-read offline (verify):
                          width 1024, 16 heads, 24 layers
 The heads pool with timm's own head (global average pool, then its LayerNorm), and the Linear head has no bias.  Every
 text tower has mlp 4 width, ctx 77, vocabulary 49408 and erf-GELU, as do the trunk's MLPs.  OpenAI mean and std,
-shortest side -> S + centre crop, as for CLIP (not SigLIP's squash)."""
+shortest side -> S + centre crop, as for CLIP (not SigLIP's squash).
+
+The big open_clip ViTs (model_registry.py:237-256,378-384,392-398) live in BIG_VIT_MODELS, in the CLIP layout of
+MODELS, served by the `b200_open_clip` loader.  find_model finds them; all_models() leaves them out (see there).
+Their shapes come from open_clip 2.24.0's model_configs/ViT-{H,g,bigG}-14*.json (head_width, mlp_ratio 4.3637 for g
+and 4.9231 for bigG) and their DFN5B preprocessing from its pretrained.py, none of which can be re-read offline
+(verify):
+    ViT-H-14/laion2b_s32b_b79k          vision width 1280, 32 layers, 16 heads (head_dim 80), mlp 5120, image 224;
+                                        text width 1024, 24 layers, 16 heads, mlp 4096; embed 1024; erf-GELU
+    ViT-H-14-quickgelu/dfn5b            the same with QuickGELU and the bicubic squash resize (resize_mode "squash")
+    ViT-H-14-378-quickgelu/dfn5b        ViT-H-14-quickgelu/dfn5b at image 378 (27 x 27 + 1 = 730 tokens)
+    ViT-g-14/laion2b_s{12b_b42k,34b_b88k} vision width 1408, 40 layers, 16 heads (head_dim 88), mlp 6144, image 224;
+                                        text as ViT-H-14; embed 1024; erf-GELU
+    ViT-bigG-14/laion2b_s39b_b160k      vision width 1664, 48 layers, 16 heads (head_dim 104), mlp 8192, image 224;
+                                        text width 1280, 32 layers, 20 heads, mlp 5120; embed 1280; erf-GELU
+All use patch 14, the class token, ln_pre / ln_post, LayerNorm eps 1e-5, OpenAI mean and std, ctx 77, vocabulary
+49408 and the causal CLIP text tower.  The vision heads of 80, 88 and 104 run zero-padded to the attention kernel's
+96, 96 and 128.  The entries carry no model_size: Marqo derives 5, 5 and 6 GB from the names.  ViT-SO400M-14-SigLIP-384
+(head_dim 72) and xlm-roberta-large-ViT-H-14 are not served."""
 from __future__ import annotations
 
 import copy
@@ -313,9 +331,42 @@ def _convnext_models() -> Dict[str, dict]:
 CONVNEXT_MODELS: Dict[str, dict] = _convnext_models()
 
 
+def _big_vit_arch(vw: int, vl: int, mlp: int, image: int, act: str, text: tuple, embed: int) -> dict:
+    """ViT-H / g / bigG-14 CLIP (module docstring, verify): 16 vision heads, patch 14."""
+    tw, tl, th = text
+    arch = _clip_arch(embed, vw, vl, 16, 14, tw, tl, th, act=act)
+    arch["vision"].update(mlp=mlp, image_size=image)
+    return arch
+
+
+def _big_vit_models() -> Dict[str, dict]:
+    m: Dict[str, dict] = {}
+    h_text, big_g_text = (1024, 24, 16), (1280, 32, 20)
+    for model, tag, shape in (
+            ("ViT-H-14", "laion2b_s32b_b79k", (1280, 32, 5120, 224, "gelu", h_text, 1024)),
+            ("ViT-H-14-quickgelu", "dfn5b", (1280, 32, 5120, 224, "quickgelu", h_text, 1024)),
+            ("ViT-H-14-378-quickgelu", "dfn5b", (1280, 32, 5120, 378, "quickgelu", h_text, 1024)),
+            ("ViT-g-14", "laion2b_s12b_b42k", (1408, 40, 6144, 224, "gelu", h_text, 1024)),
+            ("ViT-g-14", "laion2b_s34b_b88k", (1408, 40, 6144, 224, "gelu", h_text, 1024)),
+            ("ViT-bigG-14", "laion2b_s39b_b160k", (1664, 48, 8192, 224, "gelu", big_g_text, 1280))):
+        name = f"open_clip/{model}/{tag}"
+        arch = _big_vit_arch(*shape)
+        dfn = tag == "dfn5b"
+        if dfn:
+            arch["resize_mode"] = "squash"
+        # the DFN5B entries have the note style of the reference's newer entries (model_registry.py:378-398)
+        m[name] = {"name": name, "dimensions": shape[-1],
+                   "note": f"open_clip model: {model}/{tag}" if dfn else "open_clip models", "type": TYPE_OPEN_CLIP,
+                   "pretrained": tag, "arch": arch}
+    return m
+
+
+BIG_VIT_MODELS: Dict[str, dict] = _big_vit_models()
+
+
 def find_model(model_name: str) -> Optional[dict]:
     """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
-    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS, CONVNEXT_MODELS):
+    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS, CONVNEXT_MODELS, BIG_VIT_MODELS):
         entry = table.get(model_name)
         if entry is not None:
             return entry
@@ -323,12 +374,19 @@ def find_model(model_name: str) -> Optional[dict]:
 
 
 def all_models() -> Dict[str, dict]:
-    """The served registry entries by name (a new dict over the same entries), except CONVNEXT_MODELS.  The layer
-    widths of these entries' towers are the served set the GEMM shape tests pin (384, 512, 768, 1024); the ConvNeXt
-    CLIP text towers add width 640, whose GEMMs tests/test_convnext_clip_gpu.py runs instead.  Callers that need every
-    served entry add CONVNEXT_MODELS to it, as loaders.register_with_marqo and s2_inference do; find_model looks in
-    every table."""
+    """The served registry entries by name (a new dict over the same entries), except CONVNEXT_MODELS and
+    BIG_VIT_MODELS.  The layer widths of these entries' towers are the served set the GEMM shape tests pin (384, 512,
+    768, 1024), and their attention shapes the set the attention tests enumerate; the ConvNeXt CLIP text towers add
+    width 640, and the big ViTs widths 1280 to 1664, padded head dims and 20 text heads, which
+    tests/test_convnext_clip_gpu.py and tests/test_big_vit_gpu.py run instead.  served_models() has every served
+    entry; find_model looks in every table."""
     return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS, **RESNET_MODELS}
+
+
+def served_models() -> Dict[str, dict]:
+    """Every served registry entry by name (a new dict over the same entries): all_models() and the tables it leaves
+    out."""
+    return {**all_models(), **CONVNEXT_MODELS, **BIG_VIT_MODELS}
 
 
 def get_model_properties(model_name: str) -> dict:

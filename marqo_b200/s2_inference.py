@@ -104,7 +104,7 @@ def validate_model_properties(model_name: str, model_properties: Optional[dict])
     if "arch" not in props:
         base = model_registry.find_model(model_name)
         if base is None:
-            served = {**model_registry.all_models(), **model_registry.CONVNEXT_MODELS}
+            served = model_registry.served_models()
             base = next((e for e in served.values() if e["name"] == props.get("name")), None)
         if base is None:
             raise InvalidModelPropertiesError(
