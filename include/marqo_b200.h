@@ -241,7 +241,8 @@ enum b200_arch {
     B200_ARCH_SIGLIP = 3, /* open_clip SigLIP: class-token-free ViT with a MAP pooling head + bidirectional text tower */
     B200_ARCH_XLMR = 4,   /* HF XLMRobertaModel + pooling: BERT layers, RoBERTa position ids, one token-type row */
     B200_ARCH_CLIP_RESNET = 5, /* OpenAI ResNet CLIP (open_clip ModifiedResNet image tower + the CLIP text tower) */
-    B200_ARCH_CLIP_CONVNEXT = 6 /* ConvNeXt CLIP (open_clip TimmModel over a timm ConvNeXt trunk + the CLIP text tower) */
+    B200_ARCH_CLIP_CONVNEXT = 6, /* ConvNeXt CLIP (open_clip TimmModel over a timm ConvNeXt trunk + the CLIP text tower) */
+    B200_ARCH_CLIP_EVA = 7 /* EVA02 CLIP (open_clip TimmModel over a timm Eva trunk + the CLIP text tower) */
 };
 enum b200_act { B200_ACT_GELU = 0, B200_ACT_QUICKGELU = 1 };
 enum b200_pool { B200_POOL_MEAN = 0, B200_POOL_CLS = 1 };
@@ -309,6 +310,22 @@ typedef struct b200_model_desc {
      * centre-crops (open_clip's default), 1 squashes it, x and y scaled independently without a crop (open_clip's
      * resize_mode "squash": the DFN5B models).  SigLIP always squashes. */
     int32_t resize_squash;
+    /* EVA02 CLIP only (open_clip CustomTextCLIP over TimmModel and timm's Eva, verify).  `vision` is the trunk:
+     * width <= 1024, head_dim 64, mlp the SwiGLU hidden size H (<= 3072 rounded up to 64: 2048 for EVA02-B-16, 2730
+     * for EVA02-L-14), patch, image_size; `text` is the causal CLIP text tower, whose LayerNorms keep eps 1e-5.  Every
+     * trunk LayerNorm has eps layer_norm_eps (1e-6).  G = image_size / patch, N = G^2 + 1 tokens:
+     *   x = [cls_token; patch_embed(img) + its bias] + pos_embed (no ln_pre);
+     *   per block: h = norm1(x); q = h Wq^T + bq, k = h Wk^T (no bias), v = h Wv^T + bv; q and k of tokens 1..N-1 rotated
+     *         by the 2-D RoPE below (token 0 is not); o = softmax(q k^T / 8) v per head;
+     *         x += attn.proj(attn.norm(o)), attn.norm a LayerNorm over the full width of o;
+     *         h = norm2(x); u = SiLU(h Wg^T + bg) * (h Wx^T + bx); x += mlp.fc2(mlp.norm(u)), mlp.norm over the H
+     *         columns of u;
+     *   head: norm(x) of token 0, head Linear [embed_dim, width] with bias, then the CLIP L2 rule.
+     * RoPE (timm RotaryEmbeddingCat, in_pixels False, ref_feat_shape (ref, ref)): the patch at grid row r and column c
+     * is token 1 + r G + c, s = ref / G.  In each head, pair i = 0..31 (columns 2i, 2i+1) turns by theta = p 10000^(-j/16)
+     * with j = i mod 16, p = r s for i < 16 and c s for i >= 16: (a, b) -> (a cos - b sin, b cos + a sin).  The
+     * table is built by the engine (it is not in the checkpoint). */
+    int32_t eva_rope_ref_grid;    /* ref_feat_shape: 16 */
 } b200_model_desc;
 
 int b200_model_create(int device, const b200_model_desc* desc, b200_model** out);
@@ -336,6 +353,15 @@ int b200_model_destroy(b200_model* m);
 /* XLM-R: HF XLMRobertaModel names, as BERT's: embeddings.word_embeddings.weight [vocab, W],
  * embeddings.position_embeddings.weight [ctx + pad_id + 1, W], embeddings.token_type_embeddings.weight [1, W],
  * embeddings.LayerNorm.*, encoder.layer.{i}.* (a "roberta." prefix is dropped). */
+/* CLIP EVA02: open_clip CustomTextCLIP names over TimmModel (verify): visual.trunk.patch_embed.proj.{weight [W, 3, P, P],
+ * bias}, visual.trunk.cls_token [1, 1, W], visual.trunk.pos_embed [1, N, W], per block visual.trunk.blocks.{i}.norm1.*,
+ * .attn.q_proj.{weight,bias}, .attn.k_proj.weight, .attn.v_proj.{weight,bias}, .attn.norm.*, .attn.proj.*, .norm2.*,
+ * .mlp.fc1_g.{weight [H, W], bias}, .mlp.fc1_x.*, .mlp.norm.{weight,bias} [H], .mlp.fc2.{weight [W, H], bias},
+ * visual.trunk.norm.*, visual.trunk.head.{weight [E, W], bias}; the text tower under the CLIP block names with a
+ * "text." prefix (text.token_embedding.weight, ..., text.ln_final.*) and text.text_projection [W, E].
+ * b200_model_finalize fuses q | k | v (k with a zero bias), folds the patch bias into pos_embed's patch rows, fuses
+ * fc1_g | fc1_x with the hidden size padded to a multiple of 64 by zero rows (and fc2 by zero columns), and builds the
+ * RoPE table.  A checkpoint whose fc1_g has other than vision.mlp rows is refused with B200_ERR_INVALID_ARG. */
 int b200_model_load_tensor(b200_model* m, const char* name, const float* data, int64_t numel);
 /* Verifies every required parameter has been supplied, builds derived buffers. */
 int b200_model_finalize(b200_model* m);
@@ -525,6 +551,17 @@ int b200_debug_attention_time(int device, int B, int S, int W, int H, int mask, 
  * out_f32 == x normalises in place (needs in_stride == w). */
 int b200_debug_layernorm(int device, const float* x, long long in_stride, const float* gamma, const float* beta, float eps,
                          int rows, int w, float* out_f32, void* out_bf16, void* stream);
+/* b200_debug_layernorm over bf16 rows x (EVA02's attn.norm): out bf16 [rows, w]; w a multiple of 128, <= 1664. */
+int b200_debug_layernorm_bf16(int device, const void* x, long long in_stride, const float* gamma, const float* beta,
+                              float eps, int rows, int w, void* out, void* stream);
+/* EVA02's rotary embedding in place on qkv bf16 [n*S, 3w] (heads of 64, S = G^2 + 1 tokens per image), with the
+ * (cos, sin) table the model builds for grid G and reference grid ref (see b200_model_desc).  Class rows and v
+ * columns are left as they are. */
+int b200_debug_rope_qk(int device, void* qkv, int n, int G, int w, int ref, void* stream);
+/* EVA02's SwiGLU + LayerNorm: in bf16 [rows, 2 hp] (gate | x, hp = h rounded up to 64), gamma / beta fp32 [h] ->
+ * out bf16 [rows, hp] at row stride ldo (out may be in with ldo = 2 hp), pad columns 0. */
+int b200_debug_swiglu_ln(int device, const void* in, int rows, int h, const float* gamma, const float* beta, float eps,
+                         void* out, long long ldo, void* stream);
 /* CLIP / SigLIP text embedding: x fp32 [n*S, w] = tok[ids] + pos[s], eot int32 [n] = first arg-max of each ids row.
  * tok [vocab, w], pos [S, w]. */
 int b200_debug_clip_text_embed(int device, const int32_t* ids, const float* tok, const float* pos, int n, int S, int w,

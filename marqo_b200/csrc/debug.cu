@@ -264,6 +264,53 @@ int b200_debug_layernorm(int device, const float* x, long long in_stride, const 
     });
 }
 
+int b200_debug_layernorm_bf16(int device, const void* x, long long in_stride, const float* gamma, const float* beta,
+                              float eps, int rows, int w, void* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && gamma && beta && out, "NULL buffer");
+        MB_CHECK_ARG(rows > 0 && w > 0 && in_stride >= 0, "rows, w must be positive");
+        if (in_stride == 0) in_stride = w;
+        MB_CHECK_ARG(in_stride >= w, "in_stride %lld < w %d", in_stride, w);
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::layernorm_bf16(static_cast<const bf16*>(x), in_stride, gamma, beta, eps, rows, w, static_cast<bf16*>(out),
+                                s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_rope_qk(int device, void* qkv, int n, int G, int w, int ref, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(qkv != nullptr, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && G > 0 && ref > 0 && w > 0 && w % 64 == 0, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        std::vector<float> table((size_t)G * G * 64);
+        kernels::rope_table(G, ref, table.data());
+        DeviceBuffer<float> dt(table.size());
+        MB_CUDA(cudaMemcpyAsync(dt.get(), table.data(), table.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+        kernels::rope_qk(static_cast<bf16*>(qkv), n, G * G + 1, w, dt.get(), s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_swiglu_ln(int device, const void* in, int rows, int h, const float* gamma, const float* beta, float eps,
+                         void* out, long long ldo, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(in && gamma && beta && out, "NULL buffer");
+        MB_CHECK_ARG(rows > 0 && h > 0, "rows, h must be positive");
+        const int hp = (int)round_up((size_t)h, 64);
+        MB_CHECK_ARG(ldo >= hp && ldo % 8 == 0, "ldo %lld must be a multiple of 8, >= %d", ldo, hp);
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::swiglu_ln(static_cast<const bf16*>(in), rows, hp, h, gamma, beta, eps, static_cast<bf16*>(out), ldo, s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
 int b200_debug_clip_text_embed(int device, const int32_t* ids, const float* tok, const float* pos, int n, int S, int w,
                                int vocab, float* x, int32_t* eot, void* stream) {
     return guarded([&] {

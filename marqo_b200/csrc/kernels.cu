@@ -52,12 +52,22 @@ __device__ __forceinline__ void ln_row(float4 (&v)[MAXV], int nv, int w, const f
         }
 }
 
+// Elements 4 i4 .. 4 i4 + 3 of a row as fp32: a float4 load, or four bf16 (8 bytes) widened exactly.
+__device__ __forceinline__ float4 load4(const float* __restrict__ row, int i4) {
+    return reinterpret_cast<const float4*>(row)[i4];
+}
+__device__ __forceinline__ float4 load4(const __nv_bfloat16* __restrict__ row, int i4) {
+    const uint2 u = reinterpret_cast<const uint2*>(row)[i4];
+    return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u), __uint_as_float(u.y << 16),
+                       __uint_as_float(u.y & 0xffff0000u));
+}
+
 // Rows are visited LAST FIRST (block 0 takes the highest rows): the GEMM that produced x wrote its row bands in ascending
 // order, so the rows it wrote last — the ones most likely still in the 126 MB L2 — are read first, and the bf16 rows this
 // kernel writes last are the low ones the next GEMM (ascending again) starts with.  `reverse` = 0 restores the forward order
-// (MARQO_B200_LN_FORWARD=1, A/B timing).
-template <int MAXV>
-__global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ x, long long in_stride,
+// (MARQO_B200_LN_FORWARD=1, A/B timing).  TIn: fp32 rows (the residual stream) or bf16 rows (EVA02's attention output).
+template <int MAXV, class TIn = float>
+__global__ void __launch_bounds__(256) layernorm_kernel(const TIn* __restrict__ x, long long in_stride,
                                                         const float* __restrict__ gamma, const float* __restrict__ beta,
                                                         float eps, int rows, int w, float* out_f32,
                                                         __nv_bfloat16* out_bf16, int reverse) {
@@ -66,11 +76,11 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
     if (row >= rows) return;
     if (reverse) row = rows - 1 - row;
     const int nv = w / 128;
-    const float4* src = reinterpret_cast<const float4*>(x + (long long)row * in_stride);
+    const TIn* src = x + (long long)row * in_stride;
     float4 v[MAXV];
 #pragma unroll
     for (int j = 0; j < MAXV; ++j)
-        if (j < nv) v[j] = src[lane + 32 * j];
+        if (j < nv) v[j] = load4(src, lane + 32 * j);
     ln_row<false, MAXV>(v, nv, w, gamma, beta, eps, lane, out_f32 ? out_f32 + (long long)row * w : nullptr,
                         out_bf16 ? out_bf16 + (long long)row * w : nullptr);
 }
@@ -91,6 +101,162 @@ int layernorm(const float* x, long long in_stride, const float* gamma, const flo
     else
         layernorm_kernel<LN_WIDE_MAX_V4>
             <<<(rows + 7) / 8, 256, 0, s>>>(x, in_stride, gamma, beta, eps, rows, w, out_f32, out_bf16, reverse);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int layernorm_bf16(const __nv_bfloat16* x, long long in_stride, const float* gamma, const float* beta, float eps,
+                   int rows, int w, __nv_bfloat16* out, cudaStream_t s) {
+    if (rows <= 0) return 0;
+    check_ln_width(w, LN_WIDE_MAX_V4);
+    static const int reverse = getenv("MARQO_B200_LN_FORWARD") == nullptr ? 1 : 0;
+    if (w <= 128 * LN_MAX_V4)
+        layernorm_kernel<LN_MAX_V4, __nv_bfloat16>
+            <<<(rows + 7) / 8, 256, 0, s>>>(x, in_stride, gamma, beta, eps, rows, w, nullptr, out, reverse);
+    else
+        layernorm_kernel<LN_WIDE_MAX_V4, __nv_bfloat16>
+            <<<(rows + 7) / 8, 256, 0, s>>>(x, in_stride, gamma, beta, eps, rows, w, nullptr, out, reverse);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+// ------------------------------------------------------------------------------------------------ EVA02
+// 2-D rotary position embedding of q and k in place: one thread rotates 4 pairs (8 bf16 columns) of q and the same
+// columns of k of one patch row.  The pair index inside a head is (column % 64) / 2, so 8-column groups never straddle
+// a head.  v and the class rows are not read or written.
+__global__ void __launch_bounds__(256) rope_qk_kernel(__nv_bfloat16* __restrict__ qkv, int S, int w,
+                                                      const float2* __restrict__ table, long long total) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int groups = w / 8;
+    const int g = (int)(i % groups);
+    const long long prow = i / groups;               // patch row over the batch
+    const int patch = (int)(prow % (S - 1));
+    const long long row = prow + prow / (S - 1) + 1;   // skip each image's class row
+    const float4* tab = reinterpret_cast<const float4*>(table + (long long)patch * 32 + (g % 8) * 4);
+    const float4 t01 = __ldg(tab), t23 = __ldg(tab + 1);   // (cos, sin) of the 4 pairs
+    const float cs[4] = {t01.x, t01.z, t23.x, t23.z}, sn[4] = {t01.y, t01.w, t23.y, t23.w};
+#pragma unroll
+    for (int part = 0; part < 2; ++part) {   // q, then k
+        uint4* p = reinterpret_cast<uint4*>(qkv + row * 3 * w + (long long)part * w) + g;
+        const uint4 u = *p;
+        uint32_t in[4] = {u.x, u.y, u.z, u.w}, out[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float a = __uint_as_float(in[e] << 16), b = __uint_as_float(in[e] & 0xffff0000u);
+            out[e] = pack_bf16x2(a * cs[e] - b * sn[e], b * cs[e] + a * sn[e]);
+        }
+        *p = make_uint4(out[0], out[1], out[2], out[3]);
+    }
+}
+
+void rope_table(int G, int ref, float* out) {
+    const double s = (double)ref / G;
+    for (int r = 0; r < G; ++r)
+        for (int c = 0; c < G; ++c)
+            for (int i = 0; i < 32; ++i) {
+                const double theta = (i < 16 ? r : c) * s * std::pow(10000.0, -(double)(i % 16) / 16.0);
+                float* o = out + ((long long)(r * G + c) * 32 + i) * 2;
+                o[0] = (float)std::cos(theta);
+                o[1] = (float)std::sin(theta);
+            }
+}
+
+int rope_qk(__nv_bfloat16* qkv, int n, int S, int w, const float* table, cudaStream_t s) {
+    if (n <= 0 || S <= 1) return 0;
+    if (w % 64 != 0) fail(B200_ERR_UNSUPPORTED, "rope_qk: width %d must be a multiple of 64", w);
+    const long long total = (long long)n * (S - 1) * (w / 8);
+    rope_qk_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(qkv, S, w, reinterpret_cast<const float2*>(table),
+                                                                   total);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+// SwiGLU + LayerNorm: one 128-thread block per row, each thread holding up to SWIGLU_V groups of 8 hidden columns in
+// registers.  The whole row is read before any of it is written, so out may be the gate half of in (ldo = 2 hp).
+constexpr int SWIGLU_THREADS = 128, SWIGLU_V = 3;
+static_assert(SWIGLU_THREADS * SWIGLU_V * 8 == SWIGLU_MAX_HP, "swiglu_ln's registers hold SWIGLU_MAX_HP columns");
+
+__device__ __forceinline__ float block_sum(float v, float* red) {
+    v = warp_sum(v);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    __syncthreads();   // red may still be read from the previous sum
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    float t = 0.f;
+#pragma unroll
+    for (int i = 0; i < SWIGLU_THREADS / 32; ++i) t += red[i];
+    return t;
+}
+
+__global__ void __launch_bounds__(SWIGLU_THREADS) swiglu_ln_kernel(const __nv_bfloat16* in, int hp, int h,
+                                                                    const float* __restrict__ gamma,
+                                                                    const float* __restrict__ beta, float eps,
+                                                                    __nv_bfloat16* out, long long ldo) {
+    __shared__ float red[SWIGLU_THREADS / 32];
+    const long long row = blockIdx.x;
+    const __nv_bfloat16* g_row = in + row * 2 * hp;
+    const __nv_bfloat16* x_row = g_row + hp;
+    const int groups = hp / 8;
+    float u[SWIGLU_V][8];
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < SWIGLU_V; ++j) {
+        const int c8 = threadIdx.x + SWIGLU_THREADS * j;
+        if (c8 < groups) {
+            const uint4 gv = reinterpret_cast<const uint4*>(g_row)[c8];
+            const uint4 xv = reinterpret_cast<const uint4*>(x_row)[c8];
+            const uint32_t gw[4] = {gv.x, gv.y, gv.z, gv.w}, xw[4] = {xv.x, xv.y, xv.z, xv.w};
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const uint32_t gb = gw[e / 2], xb = xw[e / 2];
+                const float gf = __uint_as_float(e % 2 ? gb & 0xffff0000u : gb << 16);
+                const float xf = __uint_as_float(e % 2 ? xb & 0xffff0000u : xb << 16);
+                // SiLU(g) x = g x / (1 + e^-g); the pad columns (zero weights and bias) give exactly 0
+                u[j][e] = gf / (1.0f + expf(-gf)) * xf;
+                if (c8 * 8 + e < h) s += u[j][e];
+            }
+        }
+    }
+    const float mean = block_sum(s, red) / (float)h;
+    float q = 0.f;
+#pragma unroll
+    for (int j = 0; j < SWIGLU_V; ++j) {
+        const int c8 = threadIdx.x + SWIGLU_THREADS * j;
+        if (c8 < groups)
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+                if (c8 * 8 + e < h) {
+                    const float d = u[j][e] - mean;
+                    q += d * d;
+                }
+    }
+    const float rstd = 1.0f / sqrtf(block_sum(q, red) / (float)h + eps);
+    __nv_bfloat16* o_row = out + row * ldo;
+#pragma unroll
+    for (int j = 0; j < SWIGLU_V; ++j) {
+        const int c8 = threadIdx.x + SWIGLU_THREADS * j;
+        if (c8 < groups) {
+            float y[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const int c = c8 * 8 + e;
+                y[e] = c < h ? (u[j][e] - mean) * rstd * __ldg(gamma + c) + __ldg(beta + c) : 0.f;
+            }
+            reinterpret_cast<uint4*>(o_row)[c8] = make_uint4(pack_bf16x2(y[0], y[1]), pack_bf16x2(y[2], y[3]),
+                                                             pack_bf16x2(y[4], y[5]), pack_bf16x2(y[6], y[7]));
+        }
+    }
+}
+
+int swiglu_ln(const __nv_bfloat16* in, int rows, int hp, int h, const float* gamma, const float* beta, float eps,
+              __nv_bfloat16* out, long long ldo, cudaStream_t s) {
+    if (rows <= 0) return 0;
+    if (hp % 64 != 0 || hp > SWIGLU_MAX_HP || h <= hp - 64 || h > hp)
+        fail(B200_ERR_UNSUPPORTED, "swiglu_ln: hidden %d padded to %d must round up to a multiple of 64, <= %d", h, hp,
+             SWIGLU_MAX_HP);
+    if (ldo < hp || ldo % 8 != 0) fail(B200_ERR_INTERNAL, "swiglu_ln: ldo %lld", ldo);
+    swiglu_ln_kernel<<<(unsigned)rows, SWIGLU_THREADS, 0, s>>>(in, hp, h, gamma, beta, eps, out, ldo);
     MB_CUDA(cudaGetLastError());
     return 1;
 }

@@ -11,6 +11,26 @@ namespace kernels {
 // x + r * in_stride (floats).  Writes fp32 (out_f32, may alias x) and/or bf16 (out_bf16), both compact [rows, w].
 int layernorm(const float* x, long long in_stride, const float* gamma, const float* beta, float eps, int rows, int w,
               float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s);
+// The same over bf16 rows (widened exactly to fp32), bf16 out [rows, w]: EVA02's LayerNorm of the attention output.
+int layernorm_bf16(const __nv_bfloat16* x, long long in_stride, const float* gamma, const float* beta, float eps,
+                   int rows, int w, __nv_bfloat16* out, cudaStream_t s);
+
+// EVA02 2-D rotary position embedding, in place on qkv bf16 [n * S, 3w] (q | k | v, heads of 64): for each image's
+// patch rows 1 .. S - 1 (patch p = row - 1), pair i of every q and k head (columns 2i, 2i + 1) becomes
+// (a cos - b sin, b cos + a sin) with (cos, sin) = table[p * 32 + i] (fp32 pairs [S - 1, 32]), computed in fp32 and
+// rounded once.  The class rows and the v columns are left untouched.  w % 64 == 0.
+int rope_qk(__nv_bfloat16* qkv, int n, int S, int w, const float* table, cudaStream_t s);
+// rope_qk's table for a G x G patch grid and timm's ref_feat_shape (ref, ref), on the host, computed in fp64:
+// out[(p * 32 + i) * 2 + {0, 1}] = (cos, sin) of pair i of patch p (b200_model_desc: eva_rope_ref_grid).
+void rope_table(int G, int ref, float* out);
+
+// EVA02 SwiGLU + its LayerNorm: in bf16 [rows, 2 hp] holds the gate g (columns 0 .. hp - 1) and x (hp .. 2hp - 1);
+// u = SiLU(g) x in fp32, LayerNorm over the h true columns (mean, then variance about it), * gamma + beta [h] -> bf16
+// out [rows, hp] at row stride ldo, the pad columns h .. hp - 1 exactly 0.  hp is h rounded up to 64, <= SWIGLU_MAX_HP.
+// out may be in itself (ldo = 2 hp): a row is read whole before it is written.
+constexpr int SWIGLU_MAX_HP = 3072;
+int swiglu_ln(const __nv_bfloat16* in, int rows, int hp, int h, const float* gamma, const float* beta, float eps,
+              __nv_bfloat16* out, long long ldo, cudaStream_t s);
 
 // Already-normalised fp32 CHW [n, 3, S, S] -> bf16 A matrix of the ViT token rows [n * (g*g + cls), kpad]: row
 // b * (g*g + cls) + t is zero for the class token t < cls (cls is 1 for CLIP, 0 for SigLIP), else patch t - cls

@@ -1,5 +1,5 @@
-// Encoder runtime: CLIP ViT image tower, CLIP text tower, SigLIP towers, OpenAI ResNet CLIP and ConvNeXt CLIP image
-// towers, BERT (e5,
+// Encoder runtime: CLIP ViT image tower, CLIP text tower, SigLIP towers, OpenAI ResNet CLIP, ConvNeXt CLIP and EVA02
+// CLIP image towers, BERT (e5,
 // MiniLM, bge), MPNet, XLM-R (multilingual-e5) — SURVEY §8 a2-a5.
 //
 // What the reference calls (third-party, restated in oracle/encoders.py):
@@ -13,7 +13,7 @@
 //   h         bf16 [tokens, width]   LayerNorm output = GEMM A operand
 //   qkv       bf16 [tokens, 3*aw]    fused QKV projection (aw: TowerW::aw, the width with zero-padded heads)
 //   o         bf16 [tokens, aw]      attention output
-//   u         bf16 [tokens, mlp]     MLP hidden
+//   u         bf16 [tokens, mlp]     MLP hidden (EVA02: [tokens, 2 hp], the SwiGLU gate | x, see run_eva_layers)
 //   patches   bf16 [images * (grid^2 + 1), kpad]  im2col of preprocessed fp32 CHW input (zero class-token rows)
 // Every Linear is the wgmma GEMM of gemm.cu with bias / activation / residual-add fused into its epilogue.
 #include <algorithm>
@@ -38,6 +38,8 @@ struct LayerW {
     const float *ln1_w = nullptr, *ln1_b = nullptr, *ln2_w = nullptr, *ln2_b = nullptr;
     const float *b_qkv = nullptr, *b_o = nullptr, *b_fc = nullptr, *b_proj = nullptr;
     const __nv_bfloat16 *w_qkv = nullptr, *w_o = nullptr, *w_fc = nullptr, *w_proj = nullptr;
+    // EVA02: attn.norm over the attention output [width] and mlp.norm over the SwiGLU hidden row [swiglu_h]
+    const float *ln_attn_w = nullptr, *ln_attn_b = nullptr, *ln_mlp_w = nullptr, *ln_mlp_b = nullptr;
 };
 
 // SigLIP's MAP pooling head (timm AttentionPoolLatent with one latent): q = latent W_q^T + b_q is batch-independent and
@@ -51,7 +53,7 @@ struct MapW {
 
 // What runs a tower, resolved once from the model's arch (resolve_kinds).  Archs whose forward passes differ only in
 // data share a kind: MPNet and XLM-R are ROBERTA, and the ResNet CLIP's text tower is CLIP's.
-enum class VisionKind { NONE, CLIP_VIT, SIGLIP_VIT, RESNET, CONVNEXT };
+enum class VisionKind { NONE, CLIP_VIT, SIGLIP_VIT, RESNET, CONVNEXT, EVA_VIT };
 enum class TextKind { NONE, CLIP, SIGLIP, BERT, ROBERTA };
 struct Kinds {
     VisionKind vision = VisionKind::NONE;
@@ -79,10 +81,14 @@ struct TowerW {
     const float *cls = nullptr, *pos = nullptr, *ln_pre_w = nullptr, *ln_pre_b = nullptr;
     // final LN (ln_post / ln_final / trunk.norm) and CLIP's projection [width, embed]
     const float *ln_out_w = nullptr, *ln_out_b = nullptr, *proj = nullptr;
-    // SigLIP text projection (nn.Linear [embed, width] + bias) and vision MAP head
+    // SigLIP text projection and EVA02's vision head (nn.Linear [embed, width] + bias); SigLIP's vision MAP head
     const __nv_bfloat16* w_tproj = nullptr;
     const float* b_tproj = nullptr;
     MapW map;
+    // EVA02 vision: the SwiGLU hidden size (from the checkpoint) and it rounded up to 64 (T.d.mlp after finalize), and
+    // the RoPE table, fp32 (cos, sin) pairs [grid^2, 32] (kernels::rope_table)
+    int swiglu_h = 0, swiglu_hp = 0;
+    const float* rope = nullptr;
     // text / bert embeddings
     const float *tok = nullptr, *type0 = nullptr, *emb_ln_w = nullptr, *emb_ln_b = nullptr;
     // MPNet: relative-position bias of every layer, fp32 [heads, 2 * ctx - 1] pre-scaled by log2(e)
@@ -241,6 +247,10 @@ Kinds resolve_kinds(const b200_model_desc& d) {
         if (d.convnext_depths[0] > 0) k.vision = VisionKind::CONVNEXT;
         if (text) k.text = TextKind::CLIP;
         break;
+    case B200_ARCH_CLIP_EVA:
+        if (vit) k.vision = VisionKind::EVA_VIT;
+        if (text) k.text = TextKind::CLIP;
+        break;
     case B200_ARCH_SIGLIP:
         if (vit) k.vision = VisionKind::SIGLIP_VIT;
         if (text) k.text = TextKind::SIGLIP;
@@ -294,6 +304,24 @@ void check_vision(const b200_model_desc& d, VisionKind kind) {
                      d.convnext_head);
         MB_CHECK_ARG(d.embed_dim % 32 == 0, "CLIP ConvNeXt: embed_dim %d must be a multiple of 32", d.embed_dim);
         MB_CHECK_ARG(d.layer_norm_eps > 0.f, "CLIP ConvNeXt: layer_norm_eps must be positive");
+        break;
+    }
+    case VisionKind::EVA_VIT: {
+        // heads of 64 (the RoPE pairs), widths up to 1024, and a SwiGLU hidden size of any value whose round-up to 64
+        // swiglu_ln holds; the GEMMs run it padded (build_eva_vision)
+        MB_CHECK_ARG(d.vision.patch > 0 && d.vision.image_size % d.vision.patch == 0,
+                     "image_size must be a multiple of patch");
+        MB_CHECK_ARG(d.vision.mlp > 0 && (int)round_up((size_t)d.vision.mlp, 64) <= kernels::SWIGLU_MAX_HP,
+                     "EVA02: vision.mlp %d must be positive and round up to at most %d", d.vision.mlp,
+                     kernels::SWIGLU_MAX_HP);
+        b200_tower_desc t = d.vision;
+        t.mlp = (int)round_up((size_t)t.mlp, 64);
+        check_tower(t, "vision");
+        MB_CHECK_ARG(d.vision.width == d.vision.heads * 64, "EVA02: vision head_dim must be 64 (width %d, heads %d)",
+                     d.vision.width, d.vision.heads);
+        MB_CHECK_ARG(d.layer_norm_eps > 0.f, "EVA02: layer_norm_eps must be positive");
+        MB_CHECK_ARG(d.eva_rope_ref_grid > 0, "EVA02: eva_rope_ref_grid %d must be positive", d.eva_rope_ref_grid);
+        MB_CHECK_ARG(d.embed_dim % 32 == 0, "EVA02: embed_dim %d must be a multiple of 32", d.embed_dim);
         break;
     }
     case VisionKind::SIGLIP_VIT:
@@ -695,6 +723,87 @@ void build_vit(b200_model* m, TowerW& T, const char* conv_name, int cls_rows) {
     T.conv_wg = cg;
 }
 
+// The EVA02 trunk (open_clip TimmModel over timm's Eva, verify) in the layouts run_eva_layers reads:
+//   pos       pos_embed with the patch conv's bias folded into the patch rows (the class row has no conv term);
+//   w_qkv     q_proj | k_proj | v_proj [3w, w], b_qkv q bias | 0 | v bias (k_proj has no bias);
+//   w_fc      fc1_g | fc1_x [2 hp, w] with zero rows and zero bias after each part's h rows, so the gate and x halves
+//             start at columns 0 and hp of the GEMM's output and its pad columns are exact zeros;
+//   w_proj    fc2 [w, hp] with zero K columns h .. hp - 1, which meet swiglu_ln's zero pad columns: exact, as for
+//             pad_heads;
+//   rope      the RoPE table of the grid, built in fp64 on the host;
+//   w_tproj   the head Linear [E, w] with its bias.
+void build_eva_vision(b200_model* m, TowerW& T) {
+    const std::string t = "visual.trunk.";
+    build_vit(m, T, "visual.trunk.patch_embed.proj.weight", 1);
+    const long long w = T.d.width, E = m->desc.embed_dim;
+    T.eps = m->desc.layer_norm_eps;
+    T.cls = param(m, t + "cls_token", w);
+    std::vector<float> pos = to_host(param(m, t + "pos_embed", (long long)T.tokens * w), (size_t)T.tokens * w);
+    const std::vector<float> bias = to_host(param(m, t + "patch_embed.proj.bias", w), (size_t)w);
+    for (long long i = w; i < (long long)pos.size(); ++i) pos[i] += bias[i % w];
+    T.pos = upload_derived(m, pos);
+    std::vector<float> rope((size_t)T.grid * T.grid * 64);
+    kernels::rope_table(T.grid, m->desc.eva_rope_ref_grid, rope.data());
+    T.rope = upload_derived(m, rope);
+    // the SwiGLU hidden size is the checkpoint's; it must be the one the model was created with
+    const long long h = param_rows(m, t + "blocks.0.mlp.fc1_g.weight", w), hp = (long long)round_up((size_t)h, 64);
+    MB_CHECK_ARG(h == T.d.mlp, "EVA02: %sblocks.0.mlp.fc1_g has %lld rows, vision.mlp is %d", t.c_str(), h, T.d.mlp);
+    T.swiglu_h = (int)h;
+    T.swiglu_hp = (int)hp;
+    T.d.mlp = (int)hp;
+    T.layers.resize(T.d.layers);
+    for (int i = 0; i < T.d.layers; ++i) {
+        const std::string p = t + "blocks." + std::to_string(i) + ".";
+        LayerW& L = T.layers[i];
+        L.ln1_w = param(m, p + "norm1.weight", w);
+        L.ln1_b = param(m, p + "norm1.bias", w);
+        __nv_bfloat16* wqkv = derived_buffer<__nv_bfloat16>(m, (size_t)(3 * w * w));
+        float* bqkv = derived_buffer<float>(m, (size_t)(3 * w));
+        const char* qkv_names[3] = {"attn.q_proj", "attn.k_proj", "attn.v_proj"};
+        MB_CUDA(cudaMemsetAsync(bqkv, 0, (size_t)(3 * w) * sizeof(float), m->stream));
+        for (int j = 0; j < 3; ++j) {
+            const std::string base = p + qkv_names[j];
+            kernels::f32_to_bf16(param(m, base + ".weight", w * w), wqkv + (size_t)(j * w * w), w * w, m->stream);
+            if (j != 1)
+                MB_CUDA(cudaMemcpyAsync(bqkv + j * w, param(m, base + ".bias", w), (size_t)w * sizeof(float),
+                                        cudaMemcpyDeviceToDevice, m->stream));
+        }
+        L.w_qkv = wqkv;
+        L.b_qkv = bqkv;
+        L.ln_attn_w = param(m, p + "attn.norm.weight", w);
+        L.ln_attn_b = param(m, p + "attn.norm.bias", w);
+        L.ln2_w = param(m, p + "norm2.weight", w);
+        L.ln2_b = param(m, p + "norm2.bias", w);
+        __nv_bfloat16* wfc = derived_buffer<__nv_bfloat16>(m, (size_t)(2 * hp * w));
+        float* bfc = derived_buffer<float>(m, (size_t)(2 * hp));
+        MB_CUDA(cudaMemsetAsync(wfc, 0, (size_t)(2 * hp * w) * sizeof(__nv_bfloat16), m->stream));
+        MB_CUDA(cudaMemsetAsync(bfc, 0, (size_t)(2 * hp) * sizeof(float), m->stream));
+        const char* fc1_names[2] = {"mlp.fc1_g", "mlp.fc1_x"};
+        for (int j = 0; j < 2; ++j) {
+            const std::string base = p + fc1_names[j];
+            kernels::f32_to_bf16(param(m, base + ".weight", h * w), wfc + (size_t)(j * hp * w), h * w, m->stream);
+            MB_CUDA(cudaMemcpyAsync(bfc + j * hp, param(m, base + ".bias", h), (size_t)h * sizeof(float),
+                                    cudaMemcpyDeviceToDevice, m->stream));
+        }
+        L.w_fc = wfc;
+        L.b_fc = bfc;
+        MB_CUDA(cudaStreamSynchronize(m->stream));
+        for (int j = 0; j < 3; ++j) m->raw.erase(p + qkv_names[j] + ".weight");
+        for (int j = 0; j < 2; ++j) m->raw.erase(p + fc1_names[j] + ".weight");
+        L.w_o = to_bf16(m, p + "attn.proj.weight", w * w);
+        L.b_o = param(m, p + "attn.proj.bias", w);
+        L.ln_mlp_w = param(m, p + "mlp.norm.weight", h);
+        L.ln_mlp_b = param(m, p + "mlp.norm.bias", h);
+        pad_blocks(m, p + "mlp.fc2.weight", w, 1, h, hp);
+        L.w_proj = to_bf16(m, p + "mlp.fc2.weight", w * hp);
+        L.b_proj = param(m, p + "mlp.fc2.bias", w);
+    }
+    T.ln_out_w = param(m, t + "norm.weight", w);
+    T.ln_out_b = param(m, t + "norm.bias", w);
+    T.w_tproj = to_bf16(m, t + "head.weight", E * w);
+    T.b_tproj = param(m, t + "head.bias", E);
+}
+
 // The ConvNeXt tower's weights in the layouts its kernels read (ConvnextW) and its activation buffers.  T holds the
 // stem as a patch-4 ViT patch embedding.
 void build_convnext(b200_model* m, TowerW& T) {
@@ -801,6 +910,9 @@ void build_vision(b200_model* m) {
     case VisionKind::CONVNEXT:
         build_convnext(m, T);
         break;
+    case VisionKind::EVA_VIT:
+        build_eva_vision(m, T);
+        break;
     }
 }
 
@@ -812,7 +924,8 @@ void build_text(b200_model* m) {
     case TextKind::CLIP:
     case TextKind::SIGLIP: {
         const bool siglip = m->kind.text == TextKind::SIGLIP;
-        const std::string p = siglip ? "text." : "";
+        // SigLIP and EVA02 (open_clip CustomTextCLIP) keep the text tower under "text."
+        const std::string p = siglip || m->desc.arch == B200_ARCH_CLIP_EVA ? "text." : "";
         T.act = open_clip_act(m->desc);
         T.tok = param(m, p + "token_embedding.weight", (long long)T.d.vocab * w);
         T.pos = param(m, p + "positional_embedding", (long long)T.d.ctx * w);
@@ -824,7 +937,7 @@ void build_text(b200_model* m) {
             T.w_tproj = to_bf16(m, "text.text_projection.weight", E * w);
             T.b_tproj = param(m, "text.text_projection.bias", E);
         } else {
-            T.proj = param(m, "text_projection", w * E);
+            T.proj = param(m, p + "text_projection", w * E);
         }
         break;
     }
@@ -932,6 +1045,32 @@ void run_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S, int ma
     }
 }
 
+// The EVA02 trunk's layers over B images of S tokens (open_clip TimmModel over timm's Eva, verify): pre-LN blocks whose
+// q and k are rotated after the QKV GEMM (rope_qk), whose attention output is LayerNorm-ed (attn.norm) before the
+// out-projection, and whose MLP is a SwiGLU with a LayerNorm over its hidden row (mlp.norm).  fc1 writes the gate and
+// x halves, 2 hp columns, into u; swiglu_ln overwrites each row's gate half with the normalised hidden row, which fc2
+// reads at row stride 2 hp.
+void run_eva_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S) {
+    const int M = B * S, w = T.d.width, hp = T.swiglu_hp;
+    float* x = m->x.get();
+    __nv_bfloat16 *h = m->h.get(), *qkv = m->qkv.get(), *o = m->o.get(), *u = m->u.get();
+    for (const LayerW& L : T.layers) {
+        c.n += kernels::layernorm(x, w, L.ln1_w, L.ln1_b, T.eps, M, w, nullptr, h, m->stream);
+        linear(m, c, h, M, w, L.w_qkv, 3 * w, epilogue(qkv, 3 * w, L.b_qkv));
+        c.n += kernels::rope_qk(qkv, B, S, w, T.rope, m->stream);
+        profiled(m, c, 1, [&] {
+            return attention::launch(qkv, o, B, S, w, T.d.heads, attention::MASK_NONE, nullptr, attention::RelBias{},
+                                     m->stream);
+        });
+        c.n += kernels::layernorm_bf16(o, w, L.ln_attn_w, L.ln_attn_b, T.eps, M, w, h, m->stream);
+        linear(m, c, h, M, w, L.w_o, w, epilogue(x, w, L.b_o, gemm::ACT_NONE, true, x, w));
+        c.n += kernels::layernorm(x, w, L.ln2_w, L.ln2_b, T.eps, M, w, nullptr, h, m->stream);
+        linear(m, c, h, M, w, L.w_fc, 2 * hp, epilogue(u, 2 * hp, L.b_fc));
+        c.n += kernels::swiglu_ln(u, M, hp, T.swiglu_h, L.ln_mlp_w, L.ln_mlp_b, T.eps, u, 2 * hp, m->stream);
+        linear(m, c, u, M, hp, L.w_proj, w, epilogue(x, w, L.b_proj, gemm::ACT_NONE, true, x, w), 2 * hp);
+    }
+}
+
 // One folded ResNet conv over n images of H x H output pixels (NHWC bf16 x -> out): bias, then ReLU with the optional
 // bf16 residual added before it, or neither.  The stem conv (cin 3) takes stem_im2col's rows as x.
 void resnet_conv(b200_model* m, Counter& c, const ConvW& cw, const __nv_bfloat16* x, int n, int H,
@@ -1012,18 +1151,21 @@ void patch_embed(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, 
 }
 
 // A ViT trunk over n images (device uint8 [n, S, S, 3] u8, or device fp32 CHW f32): patch embedding, ln_pre (CLIP) and
-// the layers, leaving the n * T.tokens token rows in x.
+// the layers (EVA02's own, which have a RoPE table), leaving the n * T.tokens token rows in x.
 void forward_vit(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, const float* f32, int n) {
     const int w = T.d.width;
     float* x = m->x.get();
     // x = positional embedding (+ class embedding on each image's first row), then conv1 (no bias) of every token row
-    // added onto it in place; a class-token row multiplies a zero A row.  SigLIP has no class row, and its conv bias is
-    // already in T.pos.
+    // added onto it in place; a class-token row multiplies a zero A row.  SigLIP has no class row; its conv bias, and
+    // EVA02's, is already in T.pos.
     c.n += kernels::vit_embed_rows(x, T.cls, T.pos, n, T.tokens, w, m->stream);
     patch_embed(m, c, T, u8, f32, n, epilogue(x, w, nullptr, gemm::ACT_NONE, true, x, w));
     if (T.ln_pre_w)
         c.n += kernels::layernorm(x, w, T.ln_pre_w, T.ln_pre_b, T.eps, n * T.tokens, w, x, nullptr, m->stream);
-    run_layers(m, c, T, n, T.tokens, attention::MASK_NONE, true);
+    if (T.rope)
+        run_eva_layers(m, c, T, n, T.tokens);
+    else
+        run_layers(m, c, T, n, T.tokens, attention::MASK_NONE, true);
 }
 
 // SigLIP vision head over the n * S token rows in x: final LayerNorm of every token -> h, K|V projection -> qkv
@@ -1107,6 +1249,16 @@ void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const fl
     case VisionKind::CONVNEXT:
         forward_convnext(m, c, u8, f32, n, normalize, d_out);
         break;
+    case VisionKind::EVA_VIT: {
+        // trunk.norm of each image's class row (rows T.tokens apart) -> h [n, w], the head Linear with its bias, L2
+        const int w = T.d.width, E = m->desc.embed_dim;
+        forward_vit(m, c, T, u8, f32, n);
+        c.n += kernels::layernorm(m->x.get(), (long long)T.tokens * w, T.ln_out_w, T.ln_out_b, T.eps, n, w, nullptr,
+                                  m->h.get(), m->stream);
+        linear(m, c, m->h.get(), n, w, T.w_tproj, E, epilogue(m->pooled.get(), E, T.b_tproj, gemm::ACT_NONE, true));
+        c.n += kernels::l2_rows(m->pooled.get(), n, E, normalize, d_out, m->stream);
+        break;
+    }
     }
 }
 
@@ -1281,7 +1433,8 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         require_sm90_device(device);
         MB_CHECK_ARG(desc->arch == B200_ARCH_CLIP || desc->arch == B200_ARCH_BERT || desc->arch == B200_ARCH_MPNET ||
                          desc->arch == B200_ARCH_SIGLIP || desc->arch == B200_ARCH_XLMR ||
-                         desc->arch == B200_ARCH_CLIP_RESNET || desc->arch == B200_ARCH_CLIP_CONVNEXT,
+                         desc->arch == B200_ARCH_CLIP_RESNET || desc->arch == B200_ARCH_CLIP_CONVNEXT ||
+                         desc->arch == B200_ARCH_CLIP_EVA,
                      "unknown arch %d", desc->arch);
         MB_CHECK_ARG(desc->max_batch > 0, "max_batch must be positive");
         MB_CHECK_ARG(desc->embed_dim > 0 && desc->embed_dim <= 4096, "embed_dim out of range");
@@ -1299,7 +1452,9 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         m->ev0 = make_event();
         m->ev1 = make_event();
         m->kind = kind;
-        if (kind.vision == VisionKind::CLIP_VIT || kind.vision == VisionKind::SIGLIP_VIT) m->vision.d = desc->vision;
+        if (kind.vision == VisionKind::CLIP_VIT || kind.vision == VisionKind::SIGLIP_VIT ||
+            kind.vision == VisionKind::EVA_VIT)
+            m->vision.d = desc->vision;
         if (kind.vision == VisionKind::RESNET) m->vision.d.image_size = desc->resnet_image_size;   // (no layers)
         if (kind.vision == VisionKind::CONVNEXT) {   // the stem, as a patch embedding (no layers)
             m->vision.d.image_size = desc->convnext_image_size;
@@ -1356,7 +1511,7 @@ int b200_model_finalize(b200_model* m) {
             max_tok = std::max(max_tok, B * T->tokens);   // (0 for a missing tower)
             max_w = std::max<long long>(max_w, T->d.width);
             max_aw = std::max<long long>({max_aw, T->d.width, T->aw});   // qkv and o: padded heads are wider
-            max_mlp = std::max<long long>({max_mlp, T->d.mlp, T->map.mlp});
+            max_mlp = std::max<long long>({max_mlp, T->d.mlp, T->map.mlp, 2LL * T->swiglu_hp});   // EVA02: gate | x
         }
         const long long bytes_per_tok = std::max<long long>(1, max_w * (4 + 2) + max_aw * (6 + 2) + max_mlp * 2);
         const long long cap_tok = (24LL << 30) / bytes_per_tok;

@@ -289,8 +289,8 @@ def _to_numpy_f32(t) -> np.ndarray:
 
 
 class Encoder:
-    """A CLIP, ResNet CLIP, ConvNeXt CLIP or SigLIP (vision + text towers), BERT, MPNet or XLM-R encoder resident on one
-    GPU.
+    """A CLIP, ResNet CLIP, ConvNeXt CLIP, EVA02 CLIP or SigLIP (vision + text towers), BERT, MPNet or XLM-R encoder
+    resident on one GPU.
 
     `config` keys — CLIP: embed_dim, act ("gelu"|"quickgelu"), mean, std, resize_mode (optional: "squash" resizes
     images of another size without a crop), vision{width,layers,heads,mlp,patch,image_size},
@@ -298,7 +298,9 @@ class Encoder:
     width);  ResNet CLIP ("clip_resnet"): embed_dim, act, mean, std, the text tower's width, layers, heads, mlp, ctx,
     vocab at the top level (layers 0: no text tower), resnet{layers [4], width, heads, image_size} (None: no image
     tower);  ConvNeXt CLIP ("clip_convnext"): the ResNet CLIP keys with convnext{dims [4], depths [4], image_size,
-    ln_eps, head ("linear"|"mlp")} (None: no image tower) in place of resnet;  BERT: width, layers, heads, mlp, vocab,
+    ln_eps, head ("linear"|"mlp")} (None: no image tower) in place of resnet;  EVA02 CLIP ("clip_eva"): the ResNet
+    CLIP keys with eva{width, layers, heads, mlp (the SwiGLU hidden size), patch, image_size, ln_eps, rope_ref_grid}
+    (None: no image tower) in place of resnet;  BERT: width, layers, heads, mlp, vocab,
     max_pos, type_vocab,
     pool ("mean"|"cls");  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
     max_pos - pad_id - 1 tokens), pad_id, ln_eps, rel_buckets, rel_max_distance, pool;  XLM-R: width, layers, heads,
@@ -368,6 +370,23 @@ class Encoder:
                 d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"], config["ctx"],
                                      config["vocab"], 0, 0)
             self.image_size = int(cx["image_size"]) if cx else 0
+        elif arch == "clip_eva":
+            d.arch = N.ARCH_CLIP_EVA
+            d.embed_dim = int(config["embed_dim"])
+            d.act = N.ACT_QUICKGELU if config.get("act", "gelu") == "quickgelu" else N.ACT_GELU
+            for i in range(3):
+                d.image_mean[i] = float(np.float32(config["mean"][i]))
+                d.image_std[i] = float(np.float32(config["std"][i]))
+            ev = config.get("eva")
+            if ev:
+                d.vision = N.TowerDesc(ev["width"], ev["layers"], ev["heads"], ev["mlp"], 0, 0, ev["image_size"],
+                                       ev["patch"])
+                d.layer_norm_eps = float(ev["ln_eps"])
+                d.eva_rope_ref_grid = int(ev["rope_ref_grid"])
+            if config.get("layers"):
+                d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"], config["ctx"],
+                                     config["vocab"], 0, 0)
+            self.image_size = int(ev["image_size"]) if ev else 0
         elif arch == "bert":
             d.arch = N.ARCH_BERT
             d.embed_dim = int(config["width"])

@@ -35,6 +35,7 @@ def _resolve_weights(props: dict, arch: dict, kind: str) -> Dict[str, np.ndarray
         random = {"clip": weights_mod.random_clip_weights, "siglip": weights_mod.random_siglip_weights,
                   "clip_resnet": weights_mod.random_clip_resnet_weights,
                   "clip_convnext": weights_mod.random_clip_convnext_weights,
+                  "clip_eva": weights_mod.random_eva02_weights,
                   "bert": weights_mod.random_bert_weights, "mpnet": weights_mod.random_mpnet_weights,
                   "xlmr": weights_mod.random_xlmr_weights}[kind]
         return random(arch, seed)
@@ -94,7 +95,8 @@ class B200OpenCLIP:
         self.arch = arch
         # "siglip" (model_registry.SIGLIP_MODELS): the engine's SigLIP runtime, whose GPU resize squashes images to
         # S x S; "clip_resnet" (RESNET_MODELS): OpenAI's ResNet CLIP; "clip_convnext" (CONVNEXT_MODELS): ConvNeXt
-        # CLIP; otherwise open_clip CLIP; all three shortest side -> S + centre crop
+        # CLIP; "clip_eva" (EVA02_MODELS): EVA02 CLIP; otherwise open_clip CLIP; all four shortest side -> S + centre
+        # crop (unless the arch asks for the squash)
         kind = arch.get("kind", "clip")
         self.model = Encoder(kind, arch, _resolve_weights(props, arch, kind), device=_validate_device(self.device),
                              max_batch=int(props.get("max_batch", 256)))
@@ -104,8 +106,9 @@ class B200OpenCLIP:
     def _default_tokenizer(self):
         if self.model_properties.get("merges_file"):
             from .tokenizers import ClipBpeTokenizer
-            # the CLIP text tower's ctx: in its "text" block, or at the top level of a clip_resnet / clip_convnext arch
-            top = self.arch.get("kind") in ("clip_resnet", "clip_convnext")
+            # the CLIP text tower's ctx: in its "text" block, or at the top level of a clip_resnet / clip_convnext /
+            # clip_eva arch
+            top = self.arch.get("kind") in ("clip_resnet", "clip_convnext", "clip_eva")
             ctx = self.arch["ctx"] if top else self.arch["text"]["ctx"]
             return ClipBpeTokenizer(self.model_properties["merges_file"], context_length=int(ctx))
         try:

@@ -96,7 +96,32 @@ and 4.9231 for bigG) and their DFN5B preprocessing from its pretrained.py, none 
 All use patch 14, the class token, ln_pre / ln_post, LayerNorm eps 1e-5, OpenAI mean and std, ctx 77, vocabulary
 49408 and the causal CLIP text tower.  The vision heads of 80, 88 and 104 run zero-padded to the attention kernel's
 96, 96 and 128.  The entries carry no model_size: Marqo derives 5, 5 and 6 GB from the names.  ViT-SO400M-14-SigLIP-384
-(head_dim 72) and xlm-roberta-large-ViT-H-14 are not served."""
+(head_dim 72) and xlm-roberta-large-ViT-H-14 are not served.
+
+The EVA02 CLIP entries (model_registry.py:441-461) live in EVA02_MODELS (`arch["kind"] == "clip_eva"`), served by the
+`b200_open_clip` loader, in the clip_resnet layout: the text tower's fields at the top level and the trunk in an "eva"
+block.  Their shapes come from open_clip 2.24.0's model_configs/EVA02-*.json, its `TimmModel` / `CustomTextCLIP` and
+timm's eva.py (`Eva`, `EvaAttention`, `SwiGLU`, `RotaryEmbeddingCat`), none of which can be re-read offline (verify):
+    EVA02-B-16/merged2b_s8b_b131k      trunk width 768, 12 layers, 12 heads, SwiGLU hidden 2048, patch 16, image 224
+                                       (197 tokens); text width 512, 12 layers, 8 heads; embed 512
+    EVA02-L-14/merged2b_s4b_b131k      trunk width 1024, 24 layers, 16 heads, SwiGLU hidden 2730, patch 14, image 224
+                                       (257 tokens); text width 768, 12 layers, 12 heads; embed 768
+    EVA02-L-14-336/merged2b_s6b_b61k   EVA02-L-14 at image 336 (577 tokens)
+The hidden size is int(width * 4 * 2 / 3).  Every head is 64 wide; every trunk LayerNorm has eps 1e-6.  The trunk:
+    x = [cls_token ; patch_embed(img) + its bias] + pos_embed            (no ln_pre, no layer scale)
+    per block:  h = norm1(x);  q = h Wq^T + bq,  k = h Wk^T (no bias),  v = h Wv^T + bv
+                q and k of tokens 1..N-1 rotated (RoPE below), token 0 not;  o = softmax(q k^T / 8) v per head
+                x += attn.proj(attn.norm(o))                            (LayerNorm over the full width of o)
+                h = norm2(x);  u = SiLU(h Wg^T + bg) * (h Wx^T + bx)
+                x += mlp.fc2(mlp.norm(u))                               (LayerNorm over the hidden row)
+    out = head(norm(x)[token 0]), head a Linear [E, W] with bias, then the CLIP L2 rule (no epsilon).
+RoPE (timm build_fourier_pos_embed with the "ij" grid, repeat_interleave(2), apply_rot_embed_cat; in_pixels False,
+ref_feat_shape (16, 16)): the patch at grid row r and column c is token 1 + r G + c, s = 16 / G.  Pair i = 0..31 of
+a head (columns 2i, 2i + 1) turns by theta = p 10000^(-j/16), j = i mod 16, p = r s for i < 16 and c s for i >= 16:
+(a, b) -> (a cos - b sin, b cos + a sin).  The table is a non-persistent buffer, so the engine builds it.  The text
+tower is the causal CLIP tower (erf-GELU, LayerNorm eps 1e-5, ctx 77, vocabulary 49408, EOT pooling, ln_final, a
+[W, E] projection without bias) under the "text." prefix.  OpenAI mean and std, shortest side -> S + centre crop.  The
+entries carry no model_size: Marqo derives 1 GB from the open_clip type."""
 from __future__ import annotations
 
 import copy
@@ -364,9 +389,34 @@ def _big_vit_models() -> Dict[str, dict]:
 BIG_VIT_MODELS: Dict[str, dict] = _big_vit_models()
 
 
+def _eva02_arch(embed: int, width: int, layers: int, heads: int, patch: int, image: int, text: tuple) -> dict:
+    """EVA02 CLIP (module docstring, verify): the CLIP text tower at the top level, the timm Eva trunk in "eva"."""
+    tw, tl, th = text
+    return {"kind": "clip_eva", "embed_dim": embed, "act": "gelu", "mean": OPENAI_MEAN, "std": OPENAI_STD,
+            "width": tw, "layers": tl, "heads": th, "mlp": 4 * tw, "ctx": 77, "vocab": 49408,
+            "eva": {"width": width, "layers": layers, "heads": heads, "mlp": int(width * 4 * 2 / 3), "patch": patch,
+                    "image_size": image, "ln_eps": 1e-6, "rope_ref_grid": 16}}
+
+
+def _eva02_models() -> Dict[str, dict]:
+    m: Dict[str, dict] = {}
+    for model, tag, shape in (
+            ("EVA02-B-16", "merged2b_s8b_b131k", (512, 768, 12, 12, 16, 224, (512, 12, 8))),
+            ("EVA02-L-14", "merged2b_s4b_b131k", (768, 1024, 24, 16, 14, 224, (768, 12, 12))),
+            ("EVA02-L-14-336", "merged2b_s6b_b61k", (768, 1024, 24, 16, 14, 336, (768, 12, 12)))):
+        name = f"open_clip/{model}/{tag}"
+        m[name] = {"name": name, "dimensions": shape[0], "note": f"open_clip model: {model}/{tag}",
+                   "type": TYPE_OPEN_CLIP, "pretrained": tag, "arch": _eva02_arch(*shape)}
+    return m
+
+
+EVA02_MODELS: Dict[str, dict] = _eva02_models()
+
+
 def find_model(model_name: str) -> Optional[dict]:
     """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
-    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS, CONVNEXT_MODELS, BIG_VIT_MODELS):
+    for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS, CONVNEXT_MODELS, BIG_VIT_MODELS,
+                  EVA02_MODELS):
         entry = table.get(model_name)
         if entry is not None:
             return entry
@@ -378,9 +428,11 @@ def all_models() -> Dict[str, dict]:
     BIG_VIT_MODELS.  The layer widths of these entries' towers are the served set the GEMM shape tests pin (384, 512,
     768, 1024), and their attention shapes the set the attention tests enumerate; the ConvNeXt CLIP text towers add
     width 640, and the big ViTs widths 1280 to 1664, padded head dims and 20 text heads, which
-    tests/test_convnext_clip_gpu.py and tests/test_big_vit_gpu.py run instead.  served_models() has every served
-    entry; find_model looks in every table."""
-    return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS, **RESNET_MODELS}
+    tests/test_convnext_clip_gpu.py and tests/test_big_vit_gpu.py run instead.  EVA02_MODELS is in: its arch blocks
+    keep the text tower (512 and 768 wide) at the top level, as the ResNet CLIP ones do, and its trunk in an "eva"
+    block, whose layer shapes tests/test_eva02_kernels_gpu.py runs.  served_models() has every served entry;
+    find_model looks in every table."""
+    return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS, **RESNET_MODELS, **EVA02_MODELS}
 
 
 def served_models() -> Dict[str, dict]:

@@ -251,6 +251,55 @@ def random_clip_convnext_weights(arch: dict, seed: int = 1234) -> Dict[str, np.n
     return sd
 
 
+def random_eva02_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
+    """Seeded random weights under open_clip's CustomTextCLIP names over a timm Eva trunk (arch: the registry's
+    clip_eva block; arch["eva"] None: no image tower, arch["layers"] 0: no text tower)."""
+    g = _rng(seed)
+    sd: Dict[str, np.ndarray] = {}
+    ev, E = arch.get("eva"), arch["embed_dim"]
+    if ev:
+        w, p, hid, L = ev["width"], ev["patch"], ev["mlp"], ev["layers"]
+        grid = ev["image_size"] // p
+        rg = 1.0 / math.sqrt(2.0 * L)
+        tr = "visual.trunk."
+
+        def ln(prefix, n):
+            sd[prefix + ".weight"] = _vec(g, n, 0.1, 1.0)
+            sd[prefix + ".bias"] = _vec(g, n)
+
+        sd[tr + "patch_embed.proj.weight"] = _conv(g, w, 3, p)
+        sd[tr + "patch_embed.proj.bias"] = _vec(g, w)
+        sd[tr + "cls_token"] = 0.5 * g.standard_normal((1, 1, w), dtype=np.float32)
+        sd[tr + "pos_embed"] = 0.5 * g.standard_normal((1, grid * grid + 1, w), dtype=np.float32)
+        for i in range(L):
+            b = f"{tr}blocks.{i}."
+            ln(b + "norm1", w)
+            sd[b + "attn.q_proj.weight"] = _lin(g, w, w, 1.5)
+            sd[b + "attn.q_proj.bias"] = _vec(g, w)
+            sd[b + "attn.k_proj.weight"] = _lin(g, w, w, 1.5)
+            sd[b + "attn.v_proj.weight"] = _lin(g, w, w, 1.5)
+            sd[b + "attn.v_proj.bias"] = _vec(g, w)
+            ln(b + "attn.norm", w)
+            sd[b + "attn.proj.weight"] = _lin(g, w, w, rg)
+            sd[b + "attn.proj.bias"] = _vec(g, w)
+            ln(b + "norm2", w)
+            sd[b + "mlp.fc1_g.weight"] = _lin(g, hid, w)
+            sd[b + "mlp.fc1_g.bias"] = _vec(g, hid)
+            sd[b + "mlp.fc1_x.weight"] = _lin(g, hid, w)
+            sd[b + "mlp.fc1_x.bias"] = _vec(g, hid)
+            ln(b + "mlp.norm", hid)
+            sd[b + "mlp.fc2.weight"] = _lin(g, w, hid, rg)
+            sd[b + "mlp.fc2.bias"] = _vec(g, w)
+        ln(tr + "norm", w)
+        sd[tr + "head.weight"] = _lin(g, E, w)
+        sd[tr + "head.bias"] = _vec(g, E)
+    if arch.get("layers"):
+        t = {k: arch[k] for k in ("width", "layers", "heads", "mlp", "ctx", "vocab")}
+        text = random_clip_weights({"embed_dim": E, "text": t}, seed + 1)
+        sd.update({"text." + k: v for k, v in text.items()})
+    return sd
+
+
 def random_bert_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     g = _rng(seed)
     w, mlp = arch["width"], arch["mlp"]
