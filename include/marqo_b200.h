@@ -242,7 +242,9 @@ enum b200_arch {
     B200_ARCH_XLMR = 4,   /* HF XLMRobertaModel + pooling: BERT layers, RoBERTa position ids, one token-type row */
     B200_ARCH_CLIP_RESNET = 5, /* OpenAI ResNet CLIP (open_clip ModifiedResNet image tower + the CLIP text tower) */
     B200_ARCH_CLIP_CONVNEXT = 6, /* ConvNeXt CLIP (open_clip TimmModel over a timm ConvNeXt trunk + the CLIP text tower) */
-    B200_ARCH_CLIP_EVA = 7 /* EVA02 CLIP (open_clip TimmModel over a timm Eva trunk + the CLIP text tower) */
+    B200_ARCH_CLIP_EVA = 7, /* EVA02 CLIP (open_clip TimmModel over a timm Eva trunk + the CLIP text tower) */
+    B200_ARCH_GTE = 8 /* Alibaba's NewModel (gte-v1.5 architecture, the Stella embedders) + pooling: post-LN layers with
+                         rotary q and k and a GeGLU MLP */
 };
 enum b200_act { B200_ACT_GELU = 0, B200_ACT_QUICKGELU = 1 };
 enum b200_pool { B200_POOL_MEAN = 0, B200_POOL_CLS = 1 };
@@ -326,6 +328,19 @@ typedef struct b200_model_desc {
      * with j = i mod 16, p = r s for i < 16 and c s for i >= 16: (a, b) -> (a cos - b sin, b cos + a sin).  The
      * table is built by the engine (it is not in the checkpoint). */
     int32_t eva_rope_ref_grid;    /* ref_feat_shape: 16 */
+    /* GTE only (NewModel with position_embedding_type "rope", verify).  `text` is the encoder: width <= 1024, head_dim
+     * 64, mlp the GeGLU hidden size M, ctx <= 512; embed_dim == width; every LayerNorm has eps layer_norm_eps (1e-12);
+     * pool as BERT's; token_type_embeddings row 0 is added (type_vocab rows).  Over right-padded ids [B, S]:
+     *   x = LN_emb(word[ids] + token_type[0])                        (no position table);
+     *   per layer (post-LN): q | k | v = x Wqkv^T + bqkv, heads of 64; q and k of position s = 0..S-1 rotated by the
+     *         RoPE below; o = softmax(q k^T / 8 + key mask) v; x = attn_ln(x + o Wo^T + bo);
+     *         up | gate = x Wug^T (no bias, up first); x = mlp_ln(x + (GELU_erf(gate) * up) Wd^T + bd);
+     *   out = masked mean of x, then F.normalize (as BERT).
+     * RoPE (NTKScalingRotaryEmbedding, rotate-half): in each head, pair j = 0..31 (columns j and j + 32) turns by s f_j,
+     * f_j = (rope_theta rope_ntk_factor)^(-2j/64) / rope_ntk_factor^(2/64): (a, b) -> (a cos - b sin, b cos + a sin).
+     * The table is built by the engine. */
+    float rope_theta;             /* 160000 */
+    float rope_ntk_factor;        /* rope_scaling factor (type "ntk"): 2; 1 for no scaling */
 } b200_model_desc;
 
 int b200_model_create(int device, const b200_model_desc* desc, b200_model** out);
@@ -353,6 +368,11 @@ int b200_model_destroy(b200_model* m);
 /* XLM-R: HF XLMRobertaModel names, as BERT's: embeddings.word_embeddings.weight [vocab, W],
  * embeddings.position_embeddings.weight [ctx + pad_id + 1, W], embeddings.token_type_embeddings.weight [1, W],
  * embeddings.LayerNorm.*, encoder.layer.{i}.* (a "roberta." prefix is dropped). */
+/* GTE: NewModel names (verify): embeddings.word_embeddings.weight [vocab, W], embeddings.token_type_embeddings.weight
+ * [type_vocab, W], embeddings.LayerNorm.*, per layer encoder.layer.{i}.attention.qkv_proj.{weight [3W, W], bias},
+ * .attention.o_proj.{weight,bias}, .attn_ln.{weight,bias}, .mlp.up_gate_proj.weight [2M, W] (up rows, then gate rows;
+ * no bias), .mlp.down_proj.{weight [W, M], bias}, .mlp_ln.{weight,bias} (a "new." prefix is dropped; pooler weights are
+ * not needed).  An up_gate_proj without 2 text.mlp rows is refused with B200_ERR_INVALID_ARG. */
 /* CLIP EVA02: open_clip CustomTextCLIP names over TimmModel (verify): visual.trunk.patch_embed.proj.{weight [W, 3, P, P],
  * bias}, visual.trunk.cls_token [1, 1, W], visual.trunk.pos_embed [1, N, W], per block visual.trunk.blocks.{i}.norm1.*,
  * .attn.q_proj.{weight,bias}, .attn.k_proj.weight, .attn.v_proj.{weight,bias}, .attn.norm.*, .attn.proj.*, .norm2.*,
@@ -386,6 +406,7 @@ int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int nor
  * BERT: attn_mask int32 [n, seq] (1 = token, 0 = pad; NULL = all ones), token_type 0.
  * MPNet: as BERT, without token types; position ids follow the ids (HF create_position_ids_from_input_ids), the key
  * mask follows attn_mask.  XLM-R: as MPNet, plus token_type_embeddings row 0, LayerNorm eps layer_norm_eps.
+ * GTE: as BERT, without a position table; q and k rotated by position.
  * seq > text.ctx is refused with B200_ERR_INVALID_ARG. */
 int b200_model_encode_tokens(b200_model* m, const int32_t* ids, const int32_t* attn_mask, int n, int seq,
                              int normalize, float* out);
@@ -558,6 +579,13 @@ int b200_debug_layernorm_bf16(int device, const void* x, long long in_stride, co
  * (cos, sin) table the model builds for grid G and reference grid ref (see b200_model_desc).  Class rows and v
  * columns are left as they are. */
 int b200_debug_rope_qk(int device, void* qkv, int n, int G, int w, int ref, void* stream);
+/* GTE's rotary embedding in place on qkv bf16 [n*S, 3w] (heads of 64): rotate-half pairs (columns j, j + 32) of every
+ * row's q and k, position s = 0..S-1 of each sequence, with the table the model builds from rope_theta = theta and
+ * rope_ntk_factor = ntk_factor (see b200_model_desc).  v columns are left as they are. */
+int b200_debug_rope_qk_half(int device, void* qkv, int n, int S, int w, float theta, float ntk_factor, void* stream);
+/* GTE's GeGLU: in bf16 [rows, 2h] (up | gate) -> out bf16 [rows, h] = GELU_erf(gate) * up at row stride ldo (out may be
+ * in with ldo = 2h).  h a multiple of 8. */
+int b200_debug_geglu(int device, const void* in, int rows, int h, void* out, long long ldo, void* stream);
 /* EVA02's SwiGLU + LayerNorm: in bf16 [rows, 2 hp] (gate | x, hp = h rounded up to 64), gamma / beta fp32 [h] ->
  * out bf16 [rows, hp] at row stride ldo (out may be in with ldo = 2 hp), pad columns 0. */
 int b200_debug_swiglu_ln(int device, const void* in, int rows, int h, const float* gamma, const float* beta, float eps,
@@ -567,7 +595,8 @@ int b200_debug_swiglu_ln(int device, const void* in, int rows, int h, const floa
 int b200_debug_clip_text_embed(int device, const int32_t* ids, const float* tok, const float* pos, int n, int S, int w,
                                int vocab, float* x, int32_t* eot, void* stream);
 /* Embedding + LayerNorm: x fp32 [n*S, w] = LN(word[ids] + type0 + pos[p]), h bf16 [n*S, w] its bf16 copy, kv_len int32
- * [n] = sum of each mask row (S when mask is NULL).  pad < 0: BERT, p = s, type0 [w] required, pos_rows >= S.
+ * [n] = sum of each mask row (S when mask is NULL).  pad < 0: BERT, p = s, type0 [w] required, pos_rows >= S, or pos
+ * NULL for no position row (GTE).
  * pad >= 0: RoBERTa (XLM-R with type0, MPNet with type0 NULL), HF's position ids counted from the ids and pad,
  * pos_rows >= pad + S + 1. */
 int b200_debug_embed_ln(int device, const int32_t* ids, const int32_t* mask, const float* word, const float* pos,

@@ -16,6 +16,7 @@ OK, ERR_INVALID_ARG, ERR_NO_DEVICE, ERR_CUDA, ERR_OOM, ERR_UNSUPPORTED, ERR_INTE
 METRIC_PRENORMALIZED_ANGULAR, METRIC_ANGULAR, METRIC_DOTPRODUCT, METRIC_EUCLIDEAN = range(4)
 ARCH_CLIP, ARCH_BERT, ARCH_MPNET, ARCH_SIGLIP, ARCH_XLMR, ARCH_CLIP_RESNET, ARCH_CLIP_CONVNEXT = 0, 1, 2, 3, 4, 5, 6
 ARCH_CLIP_EVA = 7
+ARCH_GTE = 8
 ACT_GELU, ACT_QUICKGELU = 0, 1
 POOL_MEAN, POOL_CLS = 0, 1
 GEMM_128x128, GEMM_PERSISTENT = 0, 1   # the GEMM kernel b200_debug_gemm reports
@@ -52,6 +53,7 @@ class ModelDesc(C.Structure):
         ("resnet_image_size", C.c_int32),
         ("convnext_dims", C.c_int32 * 4), ("convnext_depths", C.c_int32 * 4), ("convnext_image_size", C.c_int32),
         ("convnext_head", C.c_int32), ("resize_squash", C.c_int32), ("eva_rope_ref_grid", C.c_int32),
+        ("rope_theta", C.c_float), ("rope_ntk_factor", C.c_float),
     ]
 
 
@@ -132,6 +134,8 @@ _SIGNATURES = {
     "b200_debug_layernorm": (C.c_int, [C.c_int, _P, C.c_longlong, _P, _P, C.c_float, C.c_int, C.c_int, _P, _P, _P]),
     "b200_debug_layernorm_bf16": (C.c_int, [C.c_int, _P, C.c_longlong, _P, _P, C.c_float, C.c_int, C.c_int, _P, _P]),
     "b200_debug_rope_qk": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "b200_debug_rope_qk_half": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, _P]),
+    "b200_debug_geglu": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, _P, C.c_longlong, _P]),
     "b200_debug_swiglu_ln": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, _P, _P, C.c_float, _P, C.c_longlong, _P]),
     "b200_debug_clip_text_embed": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "b200_debug_embed_ln": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, _P, _P, _P, C.c_float, C.c_int, C.c_int, C.c_int,

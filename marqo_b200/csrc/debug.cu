@@ -291,7 +291,37 @@ int b200_debug_rope_qk(int device, void* qkv, int n, int G, int w, int ref, void
         kernels::rope_table(G, ref, table.data());
         DeviceBuffer<float> dt(table.size());
         MB_CUDA(cudaMemcpyAsync(dt.get(), table.data(), table.size() * sizeof(float), cudaMemcpyHostToDevice, s));
-        kernels::rope_qk(static_cast<bf16*>(qkv), n, G * G + 1, w, dt.get(), s);
+        kernels::rope_qk(static_cast<bf16*>(qkv), n, G * G + 1, 1, w, dt.get(), kernels::RopePairing::INTERLEAVED, s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_rope_qk_half(int device, void* qkv, int n, int S, int w, float theta, float ntk_factor, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(qkv != nullptr, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && S > 0 && w > 0 && w % 64 == 0, "bad shape");
+        MB_CHECK_ARG(theta > 0.f && ntk_factor >= 1.f, "rope_theta must be positive and rope_ntk_factor >= 1");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        std::vector<float> table((size_t)S * 64);
+        kernels::rope_table_ntk(S, theta, ntk_factor, table.data());
+        DeviceBuffer<float> dt(table.size());
+        MB_CUDA(cudaMemcpyAsync(dt.get(), table.data(), table.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+        kernels::rope_qk(static_cast<bf16*>(qkv), n, S, 0, w, dt.get(), kernels::RopePairing::HALF, s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_geglu(int device, const void* in, int rows, int h, void* out, long long ldo, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(in && out, "NULL buffer");
+        MB_CHECK_ARG(rows > 0 && h > 0 && h % 8 == 0, "rows must be positive and h a positive multiple of 8");
+        MB_CHECK_ARG(ldo >= h && ldo % 8 == 0, "ldo %lld must be a multiple of 8, >= %d", ldo, h);
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::geglu(static_cast<const bf16*>(in), rows, h, static_cast<bf16*>(out), ldo, s);
         MB_CUDA(cudaStreamSynchronize(s));
     });
 }
@@ -329,10 +359,11 @@ int b200_debug_embed_ln(int device, const int32_t* ids, const int32_t* mask, con
                         int w, int vocab, int pad, float* x, void* h, int32_t* kv_len, void* stream) {
     return guarded([&] {
         const bool roberta = pad >= 0;
-        MB_CHECK_ARG(ids && word && pos && gamma && beta && x && h && kv_len, "NULL buffer");
+        // pos NULL: the BERT embedding without a position row (GTE)
+        MB_CHECK_ARG(ids && word && (pos || !roberta) && gamma && beta && x && h && kv_len, "NULL buffer");
         MB_CHECK_ARG(roberta || type0, "the BERT embedding always adds token-type row 0");
         MB_CHECK_ARG(n > 0 && S > 0 && w > 0 && vocab > 0, "bad shape");
-        MB_CHECK_ARG(pos_rows >= (roberta ? pad + S + 1 : S), "%d position rows are too few", pos_rows);
+        MB_CHECK_ARG(!pos || pos_rows >= (roberta ? pad + S + 1 : S), "%d position rows are too few", pos_rows);
         require_device(device);
         DeviceGuard g(device);
         const cudaStream_t s = static_cast<cudaStream_t>(stream);

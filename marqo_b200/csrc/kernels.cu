@@ -120,33 +120,70 @@ int layernorm_bf16(const __nv_bfloat16* x, long long in_stride, const float* gam
     return 1;
 }
 
-// ------------------------------------------------------------------------------------------------ EVA02
-// 2-D rotary position embedding of q and k in place: one thread rotates 4 pairs (8 bf16 columns) of q and the same
-// columns of k of one patch row.  The pair index inside a head is (column % 64) / 2, so 8-column groups never straddle
-// a head.  v and the class rows are not read or written.
+// ------------------------------------------------------------------------------------------------ EVA02, GTE
+// Rotary position embedding of q and k in place.  INTERLEAVED (EVA02): one thread rotates 4 pairs (8 bf16 columns) of q
+// and the same columns of k of one row; the pair index inside a head is (column % 64) / 2, so 8-column groups never
+// straddle a head.  HALF (NewModel's rotate-half): one thread rotates pairs j0 .. j0 + 7 of one head, columns j0 .. j0 + 7
+// and j0 + 32 .. j0 + 39, of q and of k.  The first FIRST rows of each sequence (EVA02's class row), and v, are not read
+// or written.
+template <RopePairing PAIRING, int FIRST>
 __global__ void __launch_bounds__(256) rope_qk_kernel(__nv_bfloat16* __restrict__ qkv, int S, int w,
                                                       const float2* __restrict__ table, long long total) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
-    const int groups = w / 8;
+    constexpr bool HALF = PAIRING == RopePairing::HALF;
+    const int groups = w / (HALF ? 16 : 8);
     const int g = (int)(i % groups);
-    const long long prow = i / groups;               // patch row over the batch
-    const int patch = (int)(prow % (S - 1));
-    const long long row = prow + prow / (S - 1) + 1;   // skip each image's class row
-    const float4* tab = reinterpret_cast<const float4*>(table + (long long)patch * 32 + (g % 8) * 4);
-    const float4 t01 = __ldg(tab), t23 = __ldg(tab + 1);   // (cos, sin) of the 4 pairs
-    const float cs[4] = {t01.x, t01.z, t23.x, t23.z}, sn[4] = {t01.y, t01.w, t23.y, t23.w};
+    const long long prow = i / groups;                             // rotated row over the batch
+    const int pos = (int)(prow % (S - FIRST));                     // its table row
+    const long long row = prow + prow / (S - FIRST) * FIRST + FIRST;   // skip each sequence's first FIRST rows
+    if constexpr (!HALF) {
+        const float4* tab = reinterpret_cast<const float4*>(table + (long long)pos * 32 + (g % 8) * 4);
+        const float4 t01 = __ldg(tab), t23 = __ldg(tab + 1);   // (cos, sin) of the 4 pairs
+        const float cs[4] = {t01.x, t01.z, t23.x, t23.z}, sn[4] = {t01.y, t01.w, t23.y, t23.w};
 #pragma unroll
-    for (int part = 0; part < 2; ++part) {   // q, then k
-        uint4* p = reinterpret_cast<uint4*>(qkv + row * 3 * w + (long long)part * w) + g;
-        const uint4 u = *p;
-        uint32_t in[4] = {u.x, u.y, u.z, u.w}, out[4];
+        for (int part = 0; part < 2; ++part) {   // q, then k
+            uint4* p = reinterpret_cast<uint4*>(qkv + row * 3 * w + (long long)part * w) + g;
+            const uint4 u = *p;
+            uint32_t in[4] = {u.x, u.y, u.z, u.w}, out[4];
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const float a = __uint_as_float(in[e] << 16), b = __uint_as_float(in[e] & 0xffff0000u);
-            out[e] = pack_bf16x2(a * cs[e] - b * sn[e], b * cs[e] + a * sn[e]);
+            for (int e = 0; e < 4; ++e) {
+                const float a = __uint_as_float(in[e] << 16), b = __uint_as_float(in[e] & 0xffff0000u);
+                out[e] = pack_bf16x2(a * cs[e] - b * sn[e], b * cs[e] + a * sn[e]);
+            }
+            *p = make_uint4(out[0], out[1], out[2], out[3]);
         }
-        *p = make_uint4(out[0], out[1], out[2], out[3]);
+    } else {
+        const int head = g / 4, j0 = (g % 4) * 8;
+        const float4* tab = reinterpret_cast<const float4*>(table + (long long)pos * 32 + j0);
+        float cs[8], sn[8];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {   // (cos, sin) of pairs j0 + 2t and j0 + 2t + 1
+            const float4 v = __ldg(tab + t);
+            cs[2 * t] = v.x;
+            sn[2 * t] = v.y;
+            cs[2 * t + 1] = v.z;
+            sn[2 * t + 1] = v.w;
+        }
+#pragma unroll
+        for (int part = 0; part < 2; ++part) {   // q, then k
+            __nv_bfloat16* base = qkv + row * 3 * w + (long long)part * w + head * 64 + j0;
+            uint4* pa = reinterpret_cast<uint4*>(base);        // the first halves a of the 8 pairs
+            uint4* pb = reinterpret_cast<uint4*>(base + 32);   // their second halves b
+            const uint4 ua = *pa, ub = *pb;
+            const uint32_t ia[4] = {ua.x, ua.y, ua.z, ua.w}, ib[4] = {ub.x, ub.y, ub.z, ub.w};
+            uint32_t oa[4], ob[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float a0 = __uint_as_float(ia[e] << 16), a1 = __uint_as_float(ia[e] & 0xffff0000u);
+                const float b0 = __uint_as_float(ib[e] << 16), b1 = __uint_as_float(ib[e] & 0xffff0000u);
+                const float c0 = cs[2 * e], s0 = sn[2 * e], c1 = cs[2 * e + 1], s1 = sn[2 * e + 1];
+                oa[e] = pack_bf16x2(a0 * c0 - b0 * s0, a1 * c1 - b1 * s1);
+                ob[e] = pack_bf16x2(b0 * c0 + a0 * s0, b1 * c1 + a1 * s1);
+            }
+            *pa = make_uint4(oa[0], oa[1], oa[2], oa[3]);
+            *pb = make_uint4(ob[0], ob[1], ob[2], ob[3]);
+        }
     }
 }
 
@@ -162,12 +199,74 @@ void rope_table(int G, int ref, float* out) {
             }
 }
 
-int rope_qk(__nv_bfloat16* qkv, int n, int S, int w, const float* table, cudaStream_t s) {
-    if (n <= 0 || S <= 1) return 0;
+void rope_table_ntk(int ctx, double base, double factor, float* out) {
+    for (int j = 0; j < 32; ++j) {
+        const double f = std::pow(base * factor, -2.0 * j / 64.0) / std::pow(factor, 2.0 / 64.0);
+        for (int s = 0; s < ctx; ++s) {
+            float* o = out + ((long long)s * 32 + j) * 2;
+            o[0] = (float)std::cos(s * f);
+            o[1] = (float)std::sin(s * f);
+        }
+    }
+}
+
+template <RopePairing PAIRING, int FIRST>
+void launch_rope_qk(__nv_bfloat16* qkv, int S, int w, const float* table, long long total, cudaStream_t s) {
+    rope_qk_kernel<PAIRING, FIRST><<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
+        qkv, S, w, reinterpret_cast<const float2*>(table), total);
+}
+
+int rope_qk(__nv_bfloat16* qkv, int n, int S, int first, int w, const float* table, RopePairing pairing,
+            cudaStream_t s) {
+    if (first != 0 && first != 1) fail(B200_ERR_INTERNAL, "rope_qk: first rotated row %d must be 0 or 1", first);
+    if (n <= 0 || S <= first) return 0;
     if (w % 64 != 0) fail(B200_ERR_UNSUPPORTED, "rope_qk: width %d must be a multiple of 64", w);
-    const long long total = (long long)n * (S - 1) * (w / 8);
-    rope_qk_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(qkv, S, w, reinterpret_cast<const float2*>(table),
-                                                                   total);
+    const bool half = pairing == RopePairing::HALF;
+    const long long total = (long long)n * (S - first) * (w / (half ? 16 : 8));
+    if (half)
+        first ? launch_rope_qk<RopePairing::HALF, 1>(qkv, S, w, table, total, s)
+              : launch_rope_qk<RopePairing::HALF, 0>(qkv, S, w, table, total, s);
+    else
+        first ? launch_rope_qk<RopePairing::INTERLEAVED, 1>(qkv, S, w, table, total, s)
+              : launch_rope_qk<RopePairing::INTERLEAVED, 0>(qkv, S, w, table, total, s);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+// GeGLU: one thread per 8 columns of a row, reading the up and gate groups before writing over the up group, so out may
+// be the up half of in itself (ldo = 2h).
+__global__ void __launch_bounds__(256) geglu_kernel(const __nv_bfloat16* in, int h, __nv_bfloat16* out, long long ldo,
+                                                    long long total) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int groups = h / 8;
+    const long long row = i / groups;
+    const int c8 = (int)(i % groups);
+    const uint4 uv = reinterpret_cast<const uint4*>(in + row * 2 * h)[c8];
+    const uint4 gv = reinterpret_cast<const uint4*>(in + row * 2 * h + h)[c8];
+    const uint32_t uw[4] = {uv.x, uv.y, uv.z, uv.w}, gw[4] = {gv.x, gv.y, gv.z, gv.w};
+    uint32_t o[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        float y[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const float u = __uint_as_float(k ? uw[e] & 0xffff0000u : uw[e] << 16);
+            const float g = __uint_as_float(k ? gw[e] & 0xffff0000u : gw[e] << 16);
+            // torch's exact GELU: g / 2 (1 + erf(g / sqrt 2))
+            y[k] = 0.5f * g * (1.0f + erff(g * 0.70710678118654752440f)) * u;
+        }
+        o[e] = pack_bf16x2(y[0], y[1]);
+    }
+    reinterpret_cast<uint4*>(out + row * ldo)[c8] = make_uint4(o[0], o[1], o[2], o[3]);
+}
+
+int geglu(const __nv_bfloat16* in, int rows, int h, __nv_bfloat16* out, long long ldo, cudaStream_t s) {
+    if (rows <= 0) return 0;
+    if (h <= 0 || h % 8 != 0) fail(B200_ERR_UNSUPPORTED, "geglu: hidden size %d must be a positive multiple of 8", h);
+    if (ldo < h || ldo % 8 != 0) fail(B200_ERR_INTERNAL, "geglu: ldo %lld", ldo);
+    const long long total = (long long)rows * (h / 8);
+    geglu_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, h, out, ldo, total);
     MB_CUDA(cudaGetLastError());
     return 1;
 }
@@ -370,6 +469,8 @@ int clip_text_embed(const int32_t* ids, const float* tok, const float* pos, int 
     return 1;
 }
 
+// POS: BERT's position_embeddings row s is added; GTE (NewModel, rotary positions) has no position table.
+template <bool POS>
 __global__ void __launch_bounds__(256) bert_embed_ln_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ mask,
                                                             const float* __restrict__ word, const float* __restrict__ pos,
                                                             const float* __restrict__ type0, const float* __restrict__ gamma,
@@ -384,17 +485,27 @@ __global__ void __launch_bounds__(256) bert_embed_ln_kernel(const int32_t* __res
     id = min(max(id, 0), vocab - 1);
     const int nv = w / 128;
     const float4* w4 = reinterpret_cast<const float4*>(word + (long long)id * w);
-    const float4* p4 = reinterpret_cast<const float4*>(pos + (long long)s * w);
     const float4* t4 = reinterpret_cast<const float4*>(type0);
     float4 v[LN_MAX_V4];
+    if constexpr (POS) {
+        const float4* p4 = reinterpret_cast<const float4*>(pos + (long long)s * w);
 #pragma unroll
-    for (int j = 0; j < LN_MAX_V4; ++j)
-        if (j < nv) {
-            const int i4 = lane + 32 * j;
-            const float4 a = __ldg(w4 + i4), b = __ldg(p4 + i4), c = __ldg(t4 + i4);
-            // HF: inputs_embeds + token_type_embeddings, then + position_embeddings
-            v[j] = make_float4((a.x + c.x) + b.x, (a.y + c.y) + b.y, (a.z + c.z) + b.z, (a.w + c.w) + b.w);
-        }
+        for (int j = 0; j < LN_MAX_V4; ++j)
+            if (j < nv) {
+                const int i4 = lane + 32 * j;
+                const float4 a = __ldg(w4 + i4), b = __ldg(p4 + i4), c = __ldg(t4 + i4);
+                // HF: inputs_embeds + token_type_embeddings, then + position_embeddings
+                v[j] = make_float4((a.x + c.x) + b.x, (a.y + c.y) + b.y, (a.z + c.z) + b.z, (a.w + c.w) + b.w);
+            }
+    } else {
+#pragma unroll
+        for (int j = 0; j < LN_MAX_V4; ++j)
+            if (j < nv) {
+                const int i4 = lane + 32 * j;
+                const float4 a = __ldg(w4 + i4), c = __ldg(t4 + i4);
+                v[j] = make_float4(a.x + c.x, a.y + c.y, a.z + c.z, a.w + c.w);   // NewEmbeddings: word + token type
+            }
+    }
     ln_row<true>(v, nv, w, gamma, beta, eps, lane, x + row * w, h + row * w);
     if (s == 0 && lane == 0) {
         int cnt = S;
@@ -412,8 +523,13 @@ int bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, co
     if (n <= 0) return 0;
     check_ln_width(w);
     const long long rows = (long long)n * S;
-    bert_embed_ln_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(ids, mask, word, pos, type0, gamma, beta, eps, n, S, w,
-                                                                   vocab, x, h, kv_len);
+    const unsigned blocks = (unsigned)((rows + 7) / 8);
+    if (pos)
+        bert_embed_ln_kernel<true><<<blocks, 256, 0, s>>>(ids, mask, word, pos, type0, gamma, beta, eps, n, S, w, vocab, x,
+                                                           h, kv_len);
+    else
+        bert_embed_ln_kernel<false><<<blocks, 256, 0, s>>>(ids, mask, word, nullptr, type0, gamma, beta, eps, n, S, w,
+                                                            vocab, x, h, kv_len);
     MB_CUDA(cudaGetLastError());
     return 1;
 }

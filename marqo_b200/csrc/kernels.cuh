@@ -15,14 +15,25 @@ int layernorm(const float* x, long long in_stride, const float* gamma, const flo
 int layernorm_bf16(const __nv_bfloat16* x, long long in_stride, const float* gamma, const float* beta, float eps,
                    int rows, int w, __nv_bfloat16* out, cudaStream_t s);
 
-// EVA02 2-D rotary position embedding, in place on qkv bf16 [n * S, 3w] (q | k | v, heads of 64): for each image's
-// patch rows 1 .. S - 1 (patch p = row - 1), pair i of every q and k head (columns 2i, 2i + 1) becomes
-// (a cos - b sin, b cos + a sin) with (cos, sin) = table[p * 32 + i] (fp32 pairs [S - 1, 32]), computed in fp32 and
-// rounded once.  The class rows and the v columns are left untouched.  w % 64 == 0.
-int rope_qk(__nv_bfloat16* qkv, int n, int S, int w, const float* table, cudaStream_t s);
+// Rotary position embedding, in place on qkv bf16 [n * S, 3w] (q | k | v, heads of 64): rows first .. S - 1 of each
+// sequence (first 1: EVA02, whose class row is not rotated; 0: GTE) are rotated, row s by table row s - first (fp32
+// (cos, sin) pairs [S - first, 32]).  Pair j of every q and k head, columns (a, b), becomes (a cos - b sin, b cos + a sin)
+// with (cos, sin) = table[(s - first) * 32 + j], computed in fp32 and rounded once.  The columns of pair j are 2j and
+// 2j + 1 (INTERLEAVED: EVA02, timm's apply_rot_embed_cat) or j and j + 32 (HALF: NewModel's rotate_half).  The first
+// rows and the v columns are left untouched.  w % 64 == 0.
+enum class RopePairing { INTERLEAVED, HALF };
+int rope_qk(__nv_bfloat16* qkv, int n, int S, int first, int w, const float* table, RopePairing pairing, cudaStream_t s);
 // rope_qk's table for a G x G patch grid and timm's ref_feat_shape (ref, ref), on the host, computed in fp64:
 // out[(p * 32 + i) * 2 + {0, 1}] = (cos, sin) of pair i of patch p (b200_model_desc: eva_rope_ref_grid).
 void rope_table(int G, int ref, float* out);
+// rope_qk's table for GTE's 1-D positions 0 .. ctx - 1 (NewModel's NTKScalingRotaryEmbedding, heads of 64, verify), on
+// the host, in fp64: out[(s * 32 + j) * 2 + {0, 1}] = (cos, sin) of s f_j with
+// f_j = (base factor)^(-2j / 64) / factor^(2 / 64) (b200_model_desc: rope_theta, rope_ntk_factor).
+void rope_table_ntk(int ctx, double base, double factor, float* out);
+
+// GeGLU: in bf16 [rows, 2h] holds up (columns 0 .. h - 1) and gate (h .. 2h - 1); out bf16 [rows, h] at row stride ldo
+// = GELU_erf(gate) * up, computed in fp32 and rounded once.  out may be the up half of in (ldo = 2h).  h % 8 == 0.
+int geglu(const __nv_bfloat16* in, int rows, int h, __nv_bfloat16* out, long long ldo, cudaStream_t s);
 
 // EVA02 SwiGLU + its LayerNorm: in bf16 [rows, 2 hp] holds the gate g (columns 0 .. hp - 1) and x (hp .. 2hp - 1);
 // u = SiLU(g) x in fp32, LayerNorm over the h true columns (mean, then variance about it), * gamma + beta [h] -> bf16
@@ -45,7 +56,7 @@ int vit_embed_rows(float* x, const float* cls, const float* pos, int n, int toke
 int clip_text_embed(const int32_t* ids, const float* tok, const float* pos, int n, int S, int w, int vocab, float* x,
                     int32_t* eot, cudaStream_t s);
 
-// BERT: x = LN(word[ids] + position[s] + token_type[0]); fp32 + bf16 copies.  Also kv_len[b] = sum(mask[b, :])
+// BERT: x = LN(word[ids] + position[s] + token_type[0]); pos NULL (GTE) adds no position row.  fp32 + bf16 copies.  Also kv_len[b] = sum(mask[b, :])
 // (mask may be NULL = all ones).
 int bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
                   const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, float* x,

@@ -1,6 +1,6 @@
 // Encoder runtime: CLIP ViT image tower, CLIP text tower, SigLIP towers, OpenAI ResNet CLIP, ConvNeXt CLIP and EVA02
 // CLIP image towers, BERT (e5,
-// MiniLM, bge), MPNet, XLM-R (multilingual-e5) — SURVEY §8 a2-a5.
+// MiniLM, bge), MPNet, XLM-R (multilingual-e5), GTE (Stella) — SURVEY §8 a2-a5.
 //
 // What the reference calls (third-party, restated in oracle/encoders.py):
 //   OPEN_CLIP.encode_image / encode_text   src/marqo/core/inference/embedding_models/open_clip_model.py:249-286
@@ -13,7 +13,8 @@
 //   h         bf16 [tokens, width]   LayerNorm output = GEMM A operand
 //   qkv       bf16 [tokens, 3*aw]    fused QKV projection (aw: TowerW::aw, the width with zero-padded heads)
 //   o         bf16 [tokens, aw]      attention output
-//   u         bf16 [tokens, mlp]     MLP hidden (EVA02: [tokens, 2 hp], the SwiGLU gate | x, see run_eva_layers)
+//   u         bf16 [tokens, mlp]     MLP hidden (EVA02: [tokens, 2 hp], the SwiGLU gate | x, see run_eva_layers; GTE:
+//                                    [tokens, 2 mlp], up | gate, see run_gte_layers)
 //   patches   bf16 [images * (grid^2 + 1), kpad]  im2col of preprocessed fp32 CHW input (zero class-token rows)
 // Every Linear is the wgmma GEMM of gemm.cu with bias / activation / residual-add fused into its epilogue.
 #include <algorithm>
@@ -54,7 +55,7 @@ struct MapW {
 // What runs a tower, resolved once from the model's arch (resolve_kinds).  Archs whose forward passes differ only in
 // data share a kind: MPNet and XLM-R are ROBERTA, and the ResNet CLIP's text tower is CLIP's.
 enum class VisionKind { NONE, CLIP_VIT, SIGLIP_VIT, RESNET, CONVNEXT, EVA_VIT };
-enum class TextKind { NONE, CLIP, SIGLIP, BERT, ROBERTA };
+enum class TextKind { NONE, CLIP, SIGLIP, BERT, ROBERTA, GTE };
 struct Kinds {
     VisionKind vision = VisionKind::NONE;
     TextKind text = TextKind::NONE;
@@ -86,7 +87,8 @@ struct TowerW {
     const float* b_tproj = nullptr;
     MapW map;
     // EVA02 vision: the SwiGLU hidden size (from the checkpoint) and it rounded up to 64 (T.d.mlp after finalize), and
-    // the RoPE table, fp32 (cos, sin) pairs [grid^2, 32] (kernels::rope_table)
+    // the RoPE table, fp32 (cos, sin) pairs [grid^2, 32] (kernels::rope_table); GTE: the RoPE table [ctx, 32]
+    // (kernels::rope_table_ntk)
     int swiglu_h = 0, swiglu_hp = 0;
     const float* rope = nullptr;
     // text / bert embeddings
@@ -263,6 +265,9 @@ Kinds resolve_kinds(const b200_model_desc& d) {
         if (text) k.text = TextKind::ROBERTA;
         k.mpnet = d.arch == B200_ARCH_MPNET;
         break;
+    case B200_ARCH_GTE:
+        if (text) k.text = TextKind::GTE;
+        break;
     }
     return k;
 }
@@ -369,6 +374,17 @@ void check_text(const b200_model_desc& d, const Kinds& k) {
     }
     case TextKind::BERT:
         MB_CHECK_ARG(d.embed_dim == d.text.width, "BERT / MPNet / XLM-R embed_dim must equal width");
+        break;
+    case TextKind::GTE:
+        // heads of 64 (the rotate-half pairs j, j + 32); the engine's sequences stop at 512 tokens
+        MB_CHECK_ARG(d.text.width == d.text.heads * 64, "GTE: head_dim must be 64 (width %d, heads %d)", d.text.width,
+                     d.text.heads);
+        MB_CHECK_ARG(d.embed_dim == d.text.width, "GTE: embed_dim %d must equal width %d", d.embed_dim, d.text.width);
+        MB_CHECK_ARG(d.text.ctx <= 512, "GTE: sequences of up to 512 tokens are supported (ctx %d)", d.text.ctx);
+        MB_CHECK_ARG(d.layer_norm_eps > 0.f, "GTE: layer_norm_eps must be positive");
+        MB_CHECK_ARG(d.rope_theta > 0.f && d.rope_ntk_factor >= 1.f,
+                     "GTE: rope_theta (%g) must be positive and rope_ntk_factor (%g) at least 1", d.rope_theta,
+                     d.rope_ntk_factor);
         break;
     }
 }
@@ -507,6 +523,31 @@ long long param_rows(b200_model* m, const std::string& name, long long w) {
         fail(B200_ERR_INVALID_ARG, "parameter '%s' has %zu elements, not a multiple of %lld", name.c_str(),
              it->second.size(), w);
     return (long long)it->second.size() / w;
+}
+
+// NewModel's layers (GTE, verify) in the layouts run_gte_layers reads: the fused qkv_proj and up_gate_proj as they are
+// (up_gate_proj has no bias), attn_ln in ln1 and mlp_ln in ln2.
+void build_gte_layers(b200_model* m, TowerW& T) {
+    const long long w = T.d.width, mlp = T.d.mlp;
+    T.layers.resize(T.d.layers);
+    for (int i = 0; i < T.d.layers; ++i) {
+        const std::string p = "encoder.layer." + std::to_string(i) + ".";
+        LayerW& L = T.layers[i];
+        L.w_qkv = to_bf16(m, p + "attention.qkv_proj.weight", 3 * w * w);
+        L.b_qkv = param(m, p + "attention.qkv_proj.bias", 3 * w);
+        L.w_o = to_bf16(m, p + "attention.o_proj.weight", w * w);
+        L.b_o = param(m, p + "attention.o_proj.bias", w);
+        L.ln1_w = param(m, p + "attn_ln.weight", w);
+        L.ln1_b = param(m, p + "attn_ln.bias", w);
+        const std::string ug = p + "mlp.up_gate_proj.weight";
+        const long long rows = param_rows(m, ug, w);
+        MB_CHECK_ARG(rows == 2 * mlp, "GTE: %s has %lld rows, 2 * text.mlp = %lld are needed", ug.c_str(), rows, 2 * mlp);
+        L.w_fc = to_bf16(m, ug, 2 * mlp * w);
+        L.w_proj = to_bf16(m, p + "mlp.down_proj.weight", w * mlp);
+        L.b_proj = param(m, p + "mlp.down_proj.bias", w);
+        L.ln2_w = param(m, p + "mlp_ln.weight", w);
+        L.ln2_b = param(m, p + "mlp_ln.bias", w);
+    }
 }
 
 // transformers MPNetEncoder.relative_position_bucket for relative_position = key - query, in the same fp32 arithmetic:
@@ -972,6 +1013,19 @@ void build_text(b200_model* m) {
         }
         break;
     }
+    case TextKind::GTE: {
+        T.eps = m->desc.layer_norm_eps;
+        T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
+        const int tv = std::max(1, m->desc.type_vocab);
+        T.type0 = param(m, "embeddings.token_type_embeddings.weight", (long long)tv * w);  // row 0 is used
+        T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
+        T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
+        build_gte_layers(m, T);
+        std::vector<float> rope((size_t)T.d.ctx * 64);
+        kernels::rope_table_ntk(T.d.ctx, m->desc.rope_theta, m->desc.rope_ntk_factor, rope.data());
+        T.rope = upload_derived(m, rope);
+        break;
+    }
     }
 }
 
@@ -1057,7 +1111,7 @@ void run_eva_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S) {
     for (const LayerW& L : T.layers) {
         c.n += kernels::layernorm(x, w, L.ln1_w, L.ln1_b, T.eps, M, w, nullptr, h, m->stream);
         linear(m, c, h, M, w, L.w_qkv, 3 * w, epilogue(qkv, 3 * w, L.b_qkv));
-        c.n += kernels::rope_qk(qkv, B, S, w, T.rope, m->stream);
+        c.n += kernels::rope_qk(qkv, B, S, 1, w, T.rope, kernels::RopePairing::INTERLEAVED, m->stream);
         profiled(m, c, 1, [&] {
             return attention::launch(qkv, o, B, S, w, T.d.heads, attention::MASK_NONE, nullptr, attention::RelBias{},
                                      m->stream);
@@ -1068,6 +1122,31 @@ void run_eva_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S) {
         linear(m, c, h, M, w, L.w_fc, 2 * hp, epilogue(u, 2 * hp, L.b_fc));
         c.n += kernels::swiglu_ln(u, M, hp, T.swiglu_h, L.ln_mlp_w, L.ln_mlp_b, T.eps, u, 2 * hp, m->stream);
         linear(m, c, u, M, hp, L.w_proj, w, epilogue(x, w, L.b_proj, gemm::ACT_NONE, true, x, w), 2 * hp);
+    }
+}
+
+// GTE's layers over B sequences of S tokens (NewModel, verify): post-LN as run_layers' BERT path, with q and k rotated
+// after the QKV GEMM (rope_qk, rotate-half pairs) and a GeGLU MLP.  On entry x and h both hold the embedding LayerNorm
+// output.  up_gate_proj writes up | gate, 2 mlp columns, into u; geglu overwrites each row's up half with
+// GELU(gate) * up, which down_proj reads at row stride 2 mlp.
+void run_gte_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S) {
+    const int M = B * S, w = T.d.width, mlp = T.d.mlp;
+    float* x = m->x.get();
+    __nv_bfloat16 *h = m->h.get(), *qkv = m->qkv.get(), *o = m->o.get(), *u = m->u.get();
+    const int32_t* kv_len = m->aux.get();
+    for (const LayerW& L : T.layers) {
+        linear(m, c, h, M, w, L.w_qkv, 3 * w, epilogue(qkv, 3 * w, L.b_qkv));
+        c.n += kernels::rope_qk(qkv, B, S, 0, w, T.rope, kernels::RopePairing::HALF, m->stream);
+        profiled(m, c, 1, [&] {
+            return attention::launch(qkv, o, B, S, w, T.d.heads, attention::MASK_KEYLEN, kv_len, attention::RelBias{},
+                                     m->stream);
+        });
+        linear(m, c, o, M, w, L.w_o, w, epilogue(x, w, L.b_o, gemm::ACT_NONE, true, x, w));
+        c.n += kernels::layernorm(x, w, L.ln1_w, L.ln1_b, T.eps, M, w, x, h, m->stream);
+        linear(m, c, h, M, w, L.w_fc, 2 * mlp, epilogue(u, 2 * mlp));
+        c.n += kernels::geglu(u, M, mlp, u, 2 * mlp, m->stream);
+        linear(m, c, u, M, mlp, L.w_proj, w, epilogue(x, w, L.b_proj, gemm::ACT_NONE, true, x, w), 2 * mlp);
+        c.n += kernels::layernorm(x, w, L.ln2_w, L.ln2_b, T.eps, M, w, x, h, m->stream);
     }
 }
 
@@ -1297,6 +1376,13 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
         run_layers(m, c, T, n, S, attention::MASK_KEYLEN, false);
         c.n += kernels::bert_head(x, aux, n, S, w, m->desc.pool, normalize, d_out, m->stream);
         break;
+    case TextKind::GTE:
+        // BERT's embedding without a position row, the rotary layers, BERT's pooling
+        c.n += kernels::bert_embed_ln(d_ids, d_mask, T.tok, nullptr, T.type0, T.emb_ln_w, T.emb_ln_b, T.eps, n, S, w,
+                                      T.d.vocab, x, m->h.get(), aux, m->stream);
+        run_gte_layers(m, c, T, n, S);
+        c.n += kernels::bert_head(x, aux, n, S, w, m->desc.pool, normalize, d_out, m->stream);
+        break;
     }
 }
 
@@ -1434,7 +1520,7 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         MB_CHECK_ARG(desc->arch == B200_ARCH_CLIP || desc->arch == B200_ARCH_BERT || desc->arch == B200_ARCH_MPNET ||
                          desc->arch == B200_ARCH_SIGLIP || desc->arch == B200_ARCH_XLMR ||
                          desc->arch == B200_ARCH_CLIP_RESNET || desc->arch == B200_ARCH_CLIP_CONVNEXT ||
-                         desc->arch == B200_ARCH_CLIP_EVA,
+                         desc->arch == B200_ARCH_CLIP_EVA || desc->arch == B200_ARCH_GTE,
                      "unknown arch %d", desc->arch);
         MB_CHECK_ARG(desc->max_batch > 0, "max_batch must be positive");
         MB_CHECK_ARG(desc->embed_dim > 0 && desc->embed_dim <= 4096, "embed_dim out of range");
@@ -1490,6 +1576,8 @@ int b200_model_load_tensor(b200_model* m, const char* name, const float* data, i
         // XLMRobertaModel checkpoints saved from a task head carry the encoder under "roberta."
         const bool xlmr = m->kind.text == TextKind::ROBERTA && !m->kind.mpnet;
         if (xlmr && key.compare(0, 8, "roberta.") == 0) key.erase(0, 8);
+        // and NewModel checkpoints saved from a task head under "new."
+        if (m->kind.text == TextKind::GTE && key.compare(0, 4, "new.") == 0) key.erase(0, 4);
         m->raw[key] = std::move(b);
     });
 }
@@ -1511,7 +1599,9 @@ int b200_model_finalize(b200_model* m) {
             max_tok = std::max(max_tok, B * T->tokens);   // (0 for a missing tower)
             max_w = std::max<long long>(max_w, T->d.width);
             max_aw = std::max<long long>({max_aw, T->d.width, T->aw});   // qkv and o: padded heads are wider
-            max_mlp = std::max<long long>({max_mlp, T->d.mlp, T->map.mlp, 2LL * T->swiglu_hp});   // EVA02: gate | x
+            // EVA02: gate | x; GTE: up | gate
+            const long long gte_u = T == &m->text && m->kind.text == TextKind::GTE ? 2LL * T->d.mlp : 0;
+            max_mlp = std::max<long long>({max_mlp, T->d.mlp, T->map.mlp, 2LL * T->swiglu_hp, gte_u});
         }
         const long long bytes_per_tok = std::max<long long>(1, max_w * (4 + 2) + max_aw * (6 + 2) + max_mlp * 2);
         const long long cap_tok = (24LL << 30) / bytes_per_tok;

@@ -289,8 +289,8 @@ def _to_numpy_f32(t) -> np.ndarray:
 
 
 class Encoder:
-    """A CLIP, ResNet CLIP, ConvNeXt CLIP, EVA02 CLIP or SigLIP (vision + text towers), BERT, MPNet or XLM-R encoder
-    resident on one GPU.
+    """A CLIP, ResNet CLIP, ConvNeXt CLIP, EVA02 CLIP or SigLIP (vision + text towers), BERT, MPNet, XLM-R or GTE
+    encoder resident on one GPU.
 
     `config` keys — CLIP: embed_dim, act ("gelu"|"quickgelu"), mean, std, resize_mode (optional: "squash" resizes
     images of another size without a crop), vision{width,layers,heads,mlp,patch,image_size},
@@ -304,8 +304,10 @@ class Encoder:
     max_pos, type_vocab,
     pool ("mean"|"cls");  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
     max_pos - pad_id - 1 tokens), pad_id, ln_eps, rel_buckets, rel_max_distance, pool;  XLM-R: width, layers, heads,
-    mlp, vocab, max_pos (as MPNet), pad_id, ln_eps, pool.  `weights` maps checkpoint parameter names (open_clip
-    state_dict names / HF BertModel / MPNetModel / XLMRobertaModel names) to fp32 arrays or torch tensors.
+    mlp, vocab, max_pos (as MPNet), pad_id, ln_eps, pool;  GTE (NewModel: the Stella embedders): width, layers, heads,
+    mlp (the GeGLU hidden size), vocab, type_vocab, ctx, ln_eps, rope_theta, rope_ntk_factor, pool.  `weights` maps
+    checkpoint parameter names (open_clip state_dict names / HF BertModel / MPNetModel / XLMRobertaModel / NewModel
+    names) to fp32 arrays or torch tensors.
     """
 
     def __init__(self, arch: str, config: dict, weights: dict, device: int = 0, max_batch: int = 256):
@@ -416,6 +418,17 @@ class Encoder:
             ctx = int(config.get("max_pos", 514)) - d.pad_id - 1
             d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"], ctx, config["vocab"],
                                  0, 0)
+            self.image_size = 0
+        elif arch == "gte":
+            d.arch = N.ARCH_GTE
+            d.embed_dim = int(config["width"])
+            d.pool = N.POOL_CLS if config.get("pool", "mean") == "cls" else N.POOL_MEAN
+            d.type_vocab = int(config.get("type_vocab", 2))
+            d.layer_norm_eps = float(config["ln_eps"])
+            d.rope_theta = float(config["rope_theta"])
+            d.rope_ntk_factor = float(config["rope_ntk_factor"])
+            d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"], config["ctx"],
+                                 config["vocab"], 0, 0)
             self.image_size = 0
         else:
             raise ValueError(f"unknown arch {arch!r}")
@@ -790,9 +803,11 @@ def debug_clip_text_embed(ids, tok, pos, device: int = 0):
 
 
 def debug_embed_ln(ids, mask, word, pos, type0, gamma, beta, eps: float, pad: Optional[int] = None, device: int = 0):
-    """BERT (pad None) or RoBERTa (pad = the pad id; type0 None for MPNet) embedding + LayerNorm of ids int32 [n, S]
-    with an optional mask [n, S] -> (x fp32 [n*S, w], its bf16 copy as fp32, kv_len int32 [n])."""
-    ia, wd, p = _as(ids, np.int32), _as(word, np.float32), _as(pos, np.float32)
+    """BERT (pad None; pos None for GTE, which has no position table) or RoBERTa (pad = the pad id; type0 None for
+    MPNet) embedding + LayerNorm of ids int32 [n, S] with an optional mask [n, S] -> (x fp32 [n*S, w], its bf16 copy as
+    fp32, kv_len int32 [n])."""
+    ia, wd = _as(ids, np.int32), _as(word, np.float32)
+    p = None if pos is None else _as(pos, np.float32)
     n, S = ia.shape
     vocab, w = wd.shape
     m = None if mask is None else _as(mask, np.int32)
@@ -801,7 +816,7 @@ def debug_embed_ln(ids, mask, word, pos, type0, gamma, beta, eps: float, pad: Op
     if m is not None and m.shape != ia.shape:
         raise ValueError(f"expected mask {ia.shape}, got {m.shape}")
     need = S if pad is None else pad + S + 1
-    if p.ndim != 2 or p.shape[1] != w or p.shape[0] < need:
+    if p is not None and (p.ndim != 2 or p.shape[1] != w or p.shape[0] < need):
         raise ValueError(f"expected pos [>= {need}, {w}], got {p.shape}")
     if (t is not None and t.size != w) or g.size != w or b.size != w:
         raise ValueError(f"type0, gamma and beta must have {w} values")
@@ -809,7 +824,8 @@ def debug_embed_ln(ids, mask, word, pos, type0, gamma, beta, eps: float, pad: Op
     di, dm, dwd, dp, dt = d.up(ia, "int32"), d.up(m, "int32"), d.up(wd), d.up(p), d.up(t)
     dg, db = d.up(g), d.up(b)
     x, h, kv_len = d.empty((n * S, w)), d.empty((n * S, w), "bfloat16"), d.empty(n, "int32")
-    N.check(N.load().b200_debug_embed_ln(device, _dptr(di), _dptr(dm), _dptr(dwd), _dptr(dp), p.shape[0], _dptr(dt),
+    N.check(N.load().b200_debug_embed_ln(device, _dptr(di), _dptr(dm), _dptr(dwd), _dptr(dp),
+                                         0 if p is None else p.shape[0], _dptr(dt),
                                          _dptr(dg), _dptr(db), eps, n, S, w, vocab, -1 if pad is None else pad, _dptr(x),
                                          _dptr(h), _dptr(kv_len), d.stream))
     return _host(x), _host(h), _host(kv_len)

@@ -9,6 +9,8 @@ surface on top of the C ABI:
   B200OpenCLIP    <-> OPEN_CLIP        (src/marqo/core/inference/embedding_models/open_clip_model.py:249-286,
                                         abstract_clip_model.py:56-112)
   B200HuggingFace <-> HuggingFaceModel (src/marqo/core/inference/embedding_models/hugging_face_model.py:172-214)
+  B200HuggingFaceStella <-> HuggingFaceStellaModel (hugging_face_stella_model.py): B200HuggingFace over the GTE
+                        runtime, refusing properties without trustRemoteCode
 
 Weights: `model_properties["weights"]` is a state dict (checkpoint names) or a path to one; `"random_init": seed`
 builds seeded random weights (benchmarks / self-test).  Tokenisers, in order of preference:
@@ -37,7 +39,7 @@ def _resolve_weights(props: dict, arch: dict, kind: str) -> Dict[str, np.ndarray
                   "clip_convnext": weights_mod.random_clip_convnext_weights,
                   "clip_eva": weights_mod.random_eva02_weights,
                   "bert": weights_mod.random_bert_weights, "mpnet": weights_mod.random_mpnet_weights,
-                  "xlmr": weights_mod.random_xlmr_weights}[kind]
+                  "xlmr": weights_mod.random_xlmr_weights, "gte": weights_mod.random_gte_weights}[kind]
         return random(arch, seed)
     if w is None:
         raise ModelLoadError("model_properties needs `weights` (state dict or checkpoint path) or `random_init`; "
@@ -303,7 +305,8 @@ class B200HuggingFace:
         if props.get("poolingMethod") or props.get("pooling_method"):  # hugging_face_model_properties.py
             arch = dict(arch, pool=(props.get("poolingMethod") or props.get("pooling_method")))
         self.arch = arch
-        # "mpnet": MPNetModel (model_registry.MPNET_MODELS); "xlmr": XLMRobertaModel (XLMR_MODELS); else BertModel
+        # "mpnet": MPNetModel (model_registry.MPNET_MODELS); "xlmr": XLMRobertaModel (XLMR_MODELS); "gte": NewModel
+        # (GTE_MODELS); else BertModel
         kind = arch.get("kind", "bert")
         self._model = Encoder(kind, arch, _resolve_weights(props, arch, kind), device=_validate_device(self.device),
                               max_batch=int(props.get("max_batch", 256)))
@@ -377,9 +380,23 @@ class B200HuggingFace:
         return out
 
 
+class B200HuggingFaceStella(B200HuggingFace):
+    """The Stella embedder's loader type (model_registry.GTE_MODELS).  The reference loads its checkpoint with
+    trust_remote_code and refuses model properties without `trustRemoteCode: True` when the loader is constructed
+    (hugging_face_model.py:54-59); so does this one, before any GPU work."""
+
+    def __init__(self, device: Optional[str] = None, model_properties: Optional[dict] = None, model_auth=None):
+        if not (model_properties or {}).get("trustRemoteCode"):
+            raise InvalidModelPropertiesError(
+                "The specified model requires the 'trustRemoteCode' attribute to be set to True. Setting this "
+                "attribute to True may have security implications.")
+        super().__init__(device=device, model_properties=model_properties, model_auth=model_auth)
+
+
 LOADERS = {
     model_registry.TYPE_OPEN_CLIP: B200OpenCLIP,
     model_registry.TYPE_HF: B200HuggingFace,
+    model_registry.TYPE_HF_STELLA: B200HuggingFaceStella,
 }
 
 
@@ -392,7 +409,7 @@ def get_model_loader(model_name: Optional[str], model_properties: dict):
 
 
 def register_with_marqo() -> None:
-    """Install the two loader types into a live Marqo process (see INTEGRATION.md)."""
+    """Install the three loader types into a live Marqo process (see INTEGRATION.md)."""
     from marqo.s2_inference import s2_inference as marqo_s2  # type: ignore
     marqo_s2.MODEL_PROPERTIES['loaders'].update(LOADERS)
     marqo_s2.MODEL_PROPERTIES['models'].update(model_registry.served_models())

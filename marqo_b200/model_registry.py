@@ -2,8 +2,8 @@
 
 Property dicts (`name`, `dimensions`, `type`, `tokens`, `model_size`, prefixes, `poolingMethod`, `notes`) are the
 reference's registry entries (src/marqo/s2_inference/model_registry.py:142-231 for open_clip/*, :616-851 for hf/*);
-`type` is rewritten to the engine's loader types ("b200_open_clip" / "b200_hf") so that both engines can be registered
-side by side in MODEL_PROPERTIES['loaders'] (model_registry.py:2133-2145).  The `arch` blocks are the shapes that live
+`type` is rewritten to the engine's loader types ("b200_open_clip" / "b200_hf" / "b200_hf_stella") so that both
+engines can be registered side by side in MODEL_PROPERTIES['loaders'] (model_registry.py:2133-2145).  The `arch` blocks are the shapes that live
 in open_clip 2.24.0 `model_configs/*.json` and the HF `config.json` files (SURVEY.md §8).
 
 The hf/* shapes come from the upstream HF `config.json` files, which cannot be re-read offline (like the ViT shapes of
@@ -121,7 +121,25 @@ a head (columns 2i, 2i + 1) turns by theta = p 10000^(-j/16), j = i mod 16, p = 
 (a, b) -> (a cos - b sin, b cos + a sin).  The table is a non-persistent buffer, so the engine builds it.  The text
 tower is the causal CLIP tower (erf-GELU, LayerNorm eps 1e-5, ctx 77, vocabulary 49408, EOT pooling, ln_final, a
 [W, E] projection without bias) under the "text." prefix.  OpenAI mean and std, shortest side -> S + centre crop.  The
-entries carry no model_size: Marqo derives 1 GB from the open_clip type."""
+entries carry no model_size: Marqo derives 1 GB from the open_clip type.
+
+The Stella embedder Marqo/dunzhang-stella_en_400M_v5 (model_registry.py:898-904) lives in GTE_MODELS (`arch["kind"] ==
+"gte"`), served by its own loader type "b200_hf_stella" (the reference's "hf_stella": HuggingFaceStellaModel, a
+HuggingFaceModel that requires trustRemoteCode and loads with use_memory_efficient_attention False and unpad_inputs
+False).  The checkpoint is Alibaba's NewModel (the gte-v1.5 architecture, trust_remote_code).  Its shapes come from
+its config.json and modeling.py, which cannot be re-read offline (verify): width 1024, 24 layers, 16 heads (head_dim
+64), GeGLU hidden 4096, vocabulary 30528, 2 token types, erf-GELU, LayerNorm eps 1e-12, position_embedding_type "rope"
+with rope_theta 160000 and rope_scaling {type "ntk", factor 2.0}, max_position_embeddings 8192, no logn attention
+scale; mean pooling of the last hidden state (no 2_Dense projection), then F.normalize.  Over right-padded ids:
+    x = LN_emb(word[ids] + token_type[0])                               (no position table)
+    per layer (post-LN):  q | k | v = x Wqkv^T + bqkv;  q, k rotated by position s (RoPE below)
+                          x = attn_ln(x + attention(q, k, v) Wo^T + bo)  (padded keys masked, scale 1/8)
+                          up | gate = x Wug^T (no bias);  x = mlp_ln(x + (GELU(gate) * up) Wd^T + bd)
+RoPE (NTKScalingRotaryEmbedding, rotate_half): the cache is built at 8192 * 2 positions, beyond
+max_position_embeddings, so the NTK branch applies: pair j = 0..31 of a head (columns j and j + 32) turns by s f_j,
+f_j = (160000 * 2)^(-2j/64) / 2^(2/64): (a, b) -> (a cos - b sin, b cos + a sin).  The uncased BERT WordPiece
+tokenizer ([CLS] 101, [SEP] 102, pad 0) is the engine's WordPieceTokenizer.  The entry carries no model_size: Marqo
+has no size for the hf_stella type and takes its default, 0.66 GB."""
 from __future__ import annotations
 
 import copy
@@ -132,6 +150,7 @@ OPENAI_STD = (0.26862954, 0.26130258, 0.27577711)
 
 TYPE_OPEN_CLIP = "b200_open_clip"
 TYPE_HF = "b200_hf"
+TYPE_HF_STELLA = "b200_hf_stella"
 
 
 def _clip_arch(embed, vw, vl, vh, patch, tw, tl, th, act="gelu"):
@@ -413,10 +432,22 @@ def _eva02_models() -> Dict[str, dict]:
 EVA02_MODELS: Dict[str, dict] = _eva02_models()
 
 
+def _gte_arch() -> dict:
+    """NewModel as the Stella embedder configures it (module docstring, verify)."""
+    return {"kind": "gte", "width": 1024, "layers": 24, "heads": 16, "mlp": 4096, "vocab": 30528, "type_vocab": 2,
+            "ctx": 512, "ln_eps": 1e-12, "rope_theta": 160000.0, "rope_ntk_factor": 2.0, "pool": "mean"}
+
+
+GTE_MODELS: Dict[str, dict] = {
+    "Marqo/dunzhang-stella_en_400M_v5": {"name": "Marqo/dunzhang-stella_en_400M_v5", "dimensions": 1024, "tokens": 512,
+                                         "type": TYPE_HF_STELLA, "trustRemoteCode": True, "arch": _gte_arch()},
+}
+
+
 def find_model(model_name: str) -> Optional[dict]:
     """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
     for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS, CONVNEXT_MODELS, BIG_VIT_MODELS,
-                  EVA02_MODELS):
+                  EVA02_MODELS, GTE_MODELS):
         entry = table.get(model_name)
         if entry is not None:
             return entry
@@ -430,9 +461,10 @@ def all_models() -> Dict[str, dict]:
     width 640, and the big ViTs widths 1280 to 1664, padded head dims and 20 text heads, which
     tests/test_convnext_clip_gpu.py and tests/test_big_vit_gpu.py run instead.  EVA02_MODELS is in: its arch blocks
     keep the text tower (512 and 768 wide) at the top level, as the ResNet CLIP ones do, and its trunk in an "eva"
-    block, whose layer shapes tests/test_eva02_kernels_gpu.py runs.  served_models() has every served entry;
-    find_model looks in every table."""
-    return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS, **RESNET_MODELS, **EVA02_MODELS}
+    block, whose layer shapes tests/test_eva02_kernels_gpu.py runs.  GTE_MODELS is in: its encoder is 1024 wide with a
+    4096 hidden size, as the BERT-large models; its fused up | gate GEMM runs in tests/test_gte_kernels_gpu.py.
+    served_models() has every served entry; find_model looks in every table."""
+    return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS, **RESNET_MODELS, **EVA02_MODELS, **GTE_MODELS}
 
 
 def served_models() -> Dict[str, dict]:

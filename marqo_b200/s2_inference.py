@@ -86,7 +86,7 @@ def _create_model_cache_key(model_name: str, device: str, model_properties: dict
 
 
 def validate_model_properties(model_name: str, model_properties: Optional[dict]) -> dict:
-    """s2_inference.py:340-407 reduced to the two loader types this engine serves: explicit properties must carry
+    """s2_inference.py:340-407 reduced to the three loader types this engine serves: explicit properties must carry
     `dimensions` and a known `type`; otherwise the name is looked up in the registry."""
     if model_properties is None:
         return model_registry.get_model_properties(model_name)
@@ -96,11 +96,12 @@ def validate_model_properties(model_name: str, model_properties: Optional[dict])
     if "dimensions" not in props:
         raise InvalidModelPropertiesError(f"model_properties for {model_name} is missing the required key `dimensions`")
     mtype = props.get("type")
-    alias = {"open_clip": model_registry.TYPE_OPEN_CLIP, "hf": model_registry.TYPE_HF}
+    alias = {"open_clip": model_registry.TYPE_OPEN_CLIP, "hf": model_registry.TYPE_HF,
+             "hf_stella": model_registry.TYPE_HF_STELLA}
     props["type"] = alias.get(mtype, mtype)
-    if props["type"] not in (model_registry.TYPE_OPEN_CLIP, model_registry.TYPE_HF):
+    if props["type"] not in alias.values():
         raise InvalidModelPropertiesError(
-            f"model type `{mtype}` is not served by the H100 engine (supported: open_clip, hf)")
+            f"model type `{mtype}` is not served by the H100 engine (supported: open_clip, hf, hf_stella)")
     if "arch" not in props:
         base = model_registry.find_model(model_name)
         if base is None:
@@ -111,7 +112,7 @@ def validate_model_properties(model_name: str, model_properties: Optional[dict])
                 f"model_properties for {model_name} needs an `arch` block (or a registry name) to size the encoder")
         import copy
         props["arch"] = copy.deepcopy(base["arch"])
-    if props["type"] == model_registry.TYPE_HF:
+    if props["type"] in (model_registry.TYPE_HF, model_registry.TYPE_HF_STELLA):
         props.setdefault("tokens", 128)  # hugging_face_model_properties.py: default 128
     return props
 
@@ -158,7 +159,8 @@ def get_model_size(model_name: str, model_properties: dict):
 
 def _reference_type_name(t):
     """this engine's loader types carry a b200_ prefix in the registry; sizes are declared per reference type"""
-    return {model_registry.TYPE_OPEN_CLIP: "open_clip", model_registry.TYPE_HF: "hf"}.get(t, t)
+    return {model_registry.TYPE_OPEN_CLIP: "open_clip", model_registry.TYPE_HF: "hf",
+            model_registry.TYPE_HF_STELLA: "hf_stella"}.get(t, t)
 
 
 def _check_memory_threshold_for_model(device: str, model_size) -> bool:

@@ -333,6 +333,34 @@ def random_xlmr_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     return random_bert_weights(arch, seed)
 
 
+def random_gte_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
+    """Seeded random weights under NewModel parameter names (arch: the registry's GTE block): the fused qkv_proj, the
+    fused up_gate_proj [2 mlp, width] without bias, no position table.  up_gate_proj and down_proj have gains 0.7 and
+    0.5: the GeGLU product of two Gaussian columns is heavier-tailed than a GELU's input, and at gain 1 the 24 post-LN
+    layers amplify bf16 rounding to cosines near 0.99 against fp32 (trained checkpoints are not that sensitive)."""
+    g = _rng(seed)
+    w, mlp = arch["width"], arch["mlp"]
+    sd: Dict[str, np.ndarray] = {}
+    sd["embeddings.word_embeddings.weight"] = g.standard_normal((arch["vocab"], w), dtype=np.float32)
+    sd["embeddings.token_type_embeddings.weight"] = 0.5 * g.standard_normal((arch.get("type_vocab", 2), w), dtype=np.float32)
+    sd["embeddings.LayerNorm.weight"] = _vec(g, w, 0.1, 1.0)
+    sd["embeddings.LayerNorm.bias"] = _vec(g, w)
+    for i in range(arch["layers"]):
+        p = f"encoder.layer.{i}."
+        sd[p + "attention.qkv_proj.weight"] = _lin(g, 3 * w, w, 1.5)
+        sd[p + "attention.qkv_proj.bias"] = _vec(g, 3 * w)
+        sd[p + "attention.o_proj.weight"] = _lin(g, w, w)
+        sd[p + "attention.o_proj.bias"] = _vec(g, w)
+        sd[p + "attn_ln.weight"] = _vec(g, w, 0.1, 1.0)
+        sd[p + "attn_ln.bias"] = _vec(g, w)
+        sd[p + "mlp.up_gate_proj.weight"] = _lin(g, 2 * mlp, w, 0.7)
+        sd[p + "mlp.down_proj.weight"] = _lin(g, w, mlp, 0.5)
+        sd[p + "mlp.down_proj.bias"] = _vec(g, w)
+        sd[p + "mlp_ln.weight"] = _vec(g, w, 0.1, 1.0)
+        sd[p + "mlp_ln.bias"] = _vec(g, w)
+    return sd
+
+
 def random_mpnet_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     """Seeded random weights under HF MPNetModel parameter names (arch: the registry's MPNet block)."""
     g = _rng(seed)
