@@ -13,8 +13,7 @@
 //   h         bf16 [tokens, width]   LayerNorm output = GEMM A operand
 //   qkv       bf16 [tokens, 3*aw]    fused QKV projection (aw: TowerW::aw, the width with zero-padded heads)
 //   o         bf16 [tokens, aw]      attention output
-//   u         bf16 [tokens, mlp]     MLP hidden (EVA02: [tokens, 2 hp], the SwiGLU gate | x, see run_eva_layers; GTE:
-//                                    [tokens, 2 mlp], up | gate, see run_gte_layers)
+//   u         bf16 [tokens, fc1_cols] MLP hidden: mlp columns, or both halves of a gated MLP (2 mlp, see Mlp)
 //   patches   bf16 [images * (grid^2 + 1), kpad]  im2col of preprocessed fp32 CHW input (zero class-token rows)
 // Every Linear is the wgmma GEMM of gemm.cu with bias / activation / residual-add fused into its epilogue.
 #include <algorithm>
@@ -39,9 +38,14 @@ struct LayerW {
     const float *ln1_w = nullptr, *ln1_b = nullptr, *ln2_w = nullptr, *ln2_b = nullptr;
     const float *b_qkv = nullptr, *b_o = nullptr, *b_fc = nullptr, *b_proj = nullptr;
     const __nv_bfloat16 *w_qkv = nullptr, *w_o = nullptr, *w_fc = nullptr, *w_proj = nullptr;
-    // EVA02: attn.norm over the attention output [width] and mlp.norm over the SwiGLU hidden row [swiglu_h]
+    // EVA02: attn.norm over the attention output [width] and mlp.norm over the SwiGLU hidden row [TowerW::mlp_h]
     const float *ln_attn_w = nullptr, *ln_attn_b = nullptr, *ln_mlp_w = nullptr, *ln_mlp_b = nullptr;
 };
+
+// A layer's MLP: fc1 with the tower's activation in its epilogue, or a gated unit over the 2 mlp columns fc1 writes
+// without one (EVA02's SwiGLU with its LayerNorm, GTE's GeGLU), run in place over one half, which fc2 reads at row
+// stride 2 mlp.
+enum class Mlp { ACT, SWIGLU_LN, GEGLU };
 
 // SigLIP's MAP pooling head (timm AttentionPoolLatent with one latent): q = latent W_q^T + b_q is batch-independent and
 // built once by b200_model_finalize.
@@ -69,7 +73,18 @@ struct TowerW {
     int aw = 0;
     std::vector<LayerW> layers;
     float eps = 1e-5f;                      // every LayerNorm of the tower
-    int act = gemm::ACT_GELU;               // the MLP's activation
+    // pre-LN layers (open_clip, timm) normalise before attention and the MLP; post-LN ones (BERT family, GTE) after
+    bool pre_ln = true;
+    Mlp mlp_form = Mlp::ACT;
+    int act = gemm::ACT_GELU;               // Mlp::ACT: the activation in fc1's epilogue
+    // the MLP's hidden size; T.d.mlp, the width its GEMMs run, is EVA02's rounded up to 64
+    int mlp_h = 0;
+    // RoPE on q and k after the QKV GEMM (kernels::rope_qk): fp32 (cos, sin) pairs, EVA02's [grid^2, 32]
+    // (kernels::rope_table), GTE's [ctx, 32] (kernels::rope_table_ntk); the rows before rope_first of every sequence
+    // (EVA02's class row) are not rotated
+    const float* rope = nullptr;
+    kernels::RopePairing rope_pairing = kernels::RopePairing::INTERLEAVED;
+    int rope_first = 0;
     // tokens per item: an image's token rows, or the longest sequence
     int tokens = 0;
     // vision
@@ -86,11 +101,6 @@ struct TowerW {
     const __nv_bfloat16* w_tproj = nullptr;
     const float* b_tproj = nullptr;
     MapW map;
-    // EVA02 vision: the SwiGLU hidden size (from the checkpoint) and it rounded up to 64 (T.d.mlp after finalize), and
-    // the RoPE table, fp32 (cos, sin) pairs [grid^2, 32] (kernels::rope_table); GTE: the RoPE table [ctx, 32]
-    // (kernels::rope_table_ntk)
-    int swiglu_h = 0, swiglu_hp = 0;
-    const float* rope = nullptr;
     // text / bert embeddings
     const float *tok = nullptr, *type0 = nullptr, *emb_ln_w = nullptr, *emb_ln_b = nullptr;
     // MPNet: relative-position bias of every layer, fp32 [heads, 2 * ctx - 1] pre-scaled by log2(e)
@@ -408,14 +418,46 @@ const __nv_bfloat16* to_bf16(b200_model* m, const std::string& name, long long n
     return dst;
 }
 
-// Checkpoint names of a pre-LN block: open_clip ResidualAttentionBlock and timm's ViT Block (SigLIP's vision trunk)
-// have the same arithmetic and the same fused q|k|v layout.
-struct PreLnNames {
-    const char *ln1, *qkv_w, *qkv_b, *out, *ln2, *fc, *proj;
+// Rows of a parameter stored as [rows, w]; its element count must be a multiple of w.
+long long param_rows(b200_model* m, const std::string& name, long long w) {
+    auto it = m->raw.find(name);
+    if (it == m->raw.end()) fail(B200_ERR_MISSING_WEIGHT, "missing parameter '%s'", name.c_str());
+    if ((long long)it->second.size() % w != 0)
+        fail(B200_ERR_INVALID_ARG, "parameter '%s' has %zu elements, not a multiple of %lld", name.c_str(),
+             it->second.size(), w);
+    return (long long)it->second.size() / w;
+}
+
+// Checkpoint names of a transformer layer, each the prefix of its parameters' names up to "weight" / "bias" below the
+// layer's own prefix (nullptr: the layer has no such module).  qkv and fc are Linears given as their parts in the
+// checkpoint: one fused Linear, or q, k and v, or the gate and x halves; bit j of qkv_bias / fc_bias says part j has a
+// bias.
+struct LayerNames {
+    const char *ln1, *ln2;   // pre-LN: before attention and the MLP; post-LN: after them
+    const char* qkv[3];
+    const char *out, *attn_ln;
+    const char* fc[2];
+    const char *mlp_ln, *proj;
+    unsigned qkv_bias = 0b111, fc_bias = 0b11;
 };
-const PreLnNames OPEN_CLIP_BLOCK{"ln_1", "attn.in_proj_weight", "attn.in_proj_bias", "attn.out_proj", "ln_2", "mlp.c_fc",
-                                 "mlp.c_proj"};
-const PreLnNames TIMM_BLOCK{"norm1", "attn.qkv.weight", "attn.qkv.bias", "attn.proj", "norm2", "mlp.fc1", "mlp.fc2"};
+// open_clip ResidualAttentionBlock and timm's ViT Block (SigLIP's vision trunk) have the same arithmetic and the same
+// fused q|k|v layout
+const LayerNames OPEN_CLIP_BLOCK{"ln_1.", "ln_2.", {"attn.in_proj_"}, "attn.out_proj.", nullptr, {"mlp.c_fc."}, nullptr,
+                                 "mlp.c_proj."};
+const LayerNames TIMM_BLOCK{"norm1.", "norm2.", {"attn.qkv."}, "attn.proj.", nullptr, {"mlp.fc1."}, nullptr, "mlp.fc2."};
+// HF BertLayer and MPNetLayer differ only in their attention half
+const LayerNames BERT_LAYER{"attention.output.LayerNorm.", "output.LayerNorm.",
+                            {"attention.self.query.", "attention.self.key.", "attention.self.value."},
+                            "attention.output.dense.", nullptr, {"intermediate.dense."}, nullptr, "output.dense."};
+const LayerNames MPNET_LAYER{"attention.LayerNorm.", "output.LayerNorm.",
+                             {"attention.attn.q.", "attention.attn.k.", "attention.attn.v."}, "attention.attn.o.",
+                             nullptr, {"intermediate.dense."}, nullptr, "output.dense."};
+// NewModel (GTE, verify): up_gate_proj is fused up | gate and has no bias
+const LayerNames GTE_LAYER{"attn_ln.", "mlp_ln.", {"attention.qkv_proj."}, "attention.o_proj.", nullptr,
+                           {"mlp.up_gate_proj."}, nullptr, "mlp.down_proj.", 0b111, 0b00};
+// timm's Eva block (EVA02, verify): k_proj has no bias
+const LayerNames EVA_BLOCK{"norm1.", "norm2.", {"attn.q_proj.", "attn.k_proj.", "attn.v_proj."}, "attn.proj.",
+                           "attn.norm.", {"mlp.fc1_g.", "mlp.fc1_x."}, "mlp.norm.", "mlp.fc2.", 0b101};
 
 // fp32 parameter `name`, [rows, nb * blk] row-major, with column block i moved to columns i * pblk .. i * pblk + blk - 1
 // of [rows, nb * pblk] and zeros in the other columns: replaces the uploaded parameter.
@@ -441,112 +483,80 @@ void pad_blocks(b200_model* m, const std::string& name, long long rows, int nb, 
 // zero bias after them, and the out-projection's K dimension has zero columns at the same places.  The QKV GEMM then
 // writes exact zeros into the pad columns, QK^T gains exact 0 * 0 terms, the pad columns of the attention output are
 // P * 0 = 0 and meet zero weights in the out-projection: the result is the unpadded one up to fp32 summation order.
-void pad_heads(b200_model* m, const TowerW& T, const std::string& p, const PreLnNames& nm) {
+// Only the CLIP vision towers, whose q|k|v is one fused Linear, have padded heads (check_tower).
+void pad_heads(b200_model* m, const TowerW& T, const std::string& p, const LayerNames& nm) {
     const long long w = T.d.width, H = T.d.heads, hd = w / H, hdp = T.aw / H;
     if (hdp == hd) return;
-    pad_blocks(m, p + nm.qkv_w, 1, (int)(3 * H), hd * w, hdp * w);
-    pad_blocks(m, p + nm.qkv_b, 1, (int)(3 * H), hd, hdp);
-    pad_blocks(m, p + nm.out + ".weight", w, (int)H, hd, hdp);
+    pad_blocks(m, p + nm.qkv[0] + "weight", 1, (int)(3 * H), hd * w, hdp * w);
+    pad_blocks(m, p + nm.qkv[0] + "bias", 1, (int)(3 * H), hd, hdp);
+    pad_blocks(m, p + nm.out + "weight", w, (int)H, hd, hdp);
 }
 
-// blocks: the prefix of block i's names up to the index ("visual.transformer.resblocks.", "visual.trunk.blocks.", ...)
-void build_preln_layers(b200_model* m, TowerW& T, const std::string& blocks, const PreLnNames& nm) {
-    const long long w = T.d.width, aw = T.aw, mlp = T.d.mlp;
+// The Linear whose n parts, each [rows, in], are parts[j] under prefix p, as one bf16 weight [n * stride, in] with part
+// j at row j * stride and zero rows after each part's own, and its fp32 bias [n * stride] with zeros for a part without
+// one (bias_mask), or nullptr when no part has one.  A Linear fused in the checkpoint (one part, no padding) is only
+// converted to bf16 and keeps its uploaded bias.  The fp32 weights are released.
+void stack_linear(b200_model* m, const std::string& p, const char* const* parts, int n, unsigned bias_mask,
+                  long long rows, long long stride, long long in, const __nv_bfloat16*& w_out, const float*& b_out) {
+    b_out = nullptr;
+    if (n == 1 && rows == stride) {
+        w_out = to_bf16(m, p + parts[0] + "weight", rows * in);
+        if (bias_mask) b_out = param(m, p + parts[0] + "bias", rows);
+        return;
+    }
+    __nv_bfloat16* w = derived_buffer<__nv_bfloat16>(m, (size_t)(n * stride * in));
+    float* b = bias_mask ? derived_buffer<float>(m, (size_t)(n * stride)) : nullptr;
+    MB_CUDA(cudaMemsetAsync(w, 0, (size_t)(n * stride * in) * sizeof(__nv_bfloat16), m->stream));
+    if (b) MB_CUDA(cudaMemsetAsync(b, 0, (size_t)(n * stride) * sizeof(float), m->stream));
+    for (int j = 0; j < n; ++j) {
+        const std::string base = p + parts[j];
+        kernels::f32_to_bf16(param(m, base + "weight", rows * in), w + (size_t)(j * stride * in), rows * in, m->stream);
+        if ((bias_mask >> j) & 1)
+            MB_CUDA(cudaMemcpyAsync(b + j * stride, param(m, base + "bias", rows), (size_t)rows * sizeof(float),
+                                    cudaMemcpyDeviceToDevice, m->stream));
+    }
+    MB_CUDA(cudaStreamSynchronize(m->stream));
+    for (int j = 0; j < n; ++j) m->raw.erase(p + parts[j] + "weight");
+    w_out = w;
+    b_out = b;
+}
+
+// The columns fc1 writes per token: mlp, or both halves of a gated MLP
+int fc1_cols(const TowerW& T) { return T.mlp_form == Mlp::ACT ? T.d.mlp : 2 * T.d.mlp; }
+
+// The layers of T in the layouts run_layers reads.  blocks: the prefix of layer i's names up to the index
+// ("visual.transformer.resblocks.", "encoder.layer.", ...).  fc1's parts each have mlp_h rows at a stride of mlp
+// (EVA02's gate and x halves, zero rows after each), unless it is one fused Linear of fc1_cols rows; fc2 then gets zero
+// K columns at the pad positions, which meet the gated unit's zero pad columns: exact, as for pad_heads.
+void build_layers(b200_model* m, TowerW& T, const std::string& blocks, const LayerNames& nm) {
+    const long long w = T.d.width, aw = T.aw, mlp = T.d.mlp, fc = fc1_cols(T);
+    const int n_qkv = nm.qkv[1] ? 3 : 1, n_fc = nm.fc[1] ? 2 : 1;
+    const long long fc_rows = n_fc == 1 ? fc : T.mlp_h;
+    auto norm = [&](const std::string& p, const char* name, long long n, const float*& g, const float*& b) {
+        g = param(m, p + name + "weight", n);
+        b = param(m, p + name + "bias", n);
+    };
     T.layers.resize(T.d.layers);
     for (int i = 0; i < T.d.layers; ++i) {
         const std::string p = blocks + std::to_string(i) + ".";
         LayerW& L = T.layers[i];
-        L.ln1_w = param(m, p + nm.ln1 + ".weight", w);
-        L.ln1_b = param(m, p + nm.ln1 + ".bias", w);
+        norm(p, nm.ln1, w, L.ln1_w, L.ln1_b);
         pad_heads(m, T, p, nm);
-        L.w_qkv = to_bf16(m, p + nm.qkv_w, 3 * aw * w);
-        L.b_qkv = param(m, p + nm.qkv_b, 3 * aw);
-        L.w_o = to_bf16(m, p + nm.out + ".weight", w * aw);
-        L.b_o = param(m, p + nm.out + ".bias", w);
-        L.ln2_w = param(m, p + nm.ln2 + ".weight", w);
-        L.ln2_b = param(m, p + nm.ln2 + ".bias", w);
-        L.w_fc = to_bf16(m, p + nm.fc + ".weight", mlp * w);
-        L.b_fc = param(m, p + nm.fc + ".bias", mlp);
-        L.w_proj = to_bf16(m, p + nm.proj + ".weight", w * mlp);
-        L.b_proj = param(m, p + nm.proj + ".bias", w);
-    }
-}
-
-// Checkpoint names of the attention half of a post-LN layer: HF BertLayer and MPNetLayer differ only there.
-struct PostLnNames {
-    const char* qkv[3];    // query / key / value Linear, under encoder.layer.{i}.
-    const char* out;       // attention output Linear
-    const char* out_ln;    // LayerNorm after the attention residual
-};
-const PostLnNames BERT_NAMES{{"attention.self.query", "attention.self.key", "attention.self.value"},
-                             "attention.output.dense", "attention.output.LayerNorm"};
-const PostLnNames MPNET_NAMES{{"attention.attn.q", "attention.attn.k", "attention.attn.v"}, "attention.attn.o",
-                              "attention.LayerNorm"};
-
-void build_bert_layers(b200_model* m, TowerW& T, const PostLnNames& nm) {
-    const long long w = T.d.width, mlp = T.d.mlp;
-    T.layers.resize(T.d.layers);
-    for (int i = 0; i < T.d.layers; ++i) {
-        const std::string p = "encoder.layer." + std::to_string(i) + ".";
-        LayerW& L = T.layers[i];
-        // fuse query / key / value into one [3w, w] weight and one [3w] bias
-        __nv_bfloat16* wq = derived_buffer<__nv_bfloat16>(m, (size_t)3 * w * w);
-        float* bq = derived_buffer<float>(m, (size_t)3 * w);
-        for (int j = 0; j < 3; ++j) {
-            const std::string base = p + nm.qkv[j];
-            kernels::f32_to_bf16(param(m, base + ".weight", w * w), wq + (size_t)j * w * w, w * w, m->stream);
-            MB_CUDA(cudaMemcpyAsync(bq + (size_t)j * w, param(m, base + ".bias", w), (size_t)w * 4, cudaMemcpyDeviceToDevice,
-                                    m->stream));
+        stack_linear(m, p, nm.qkv, n_qkv, nm.qkv_bias, 3 * aw / n_qkv, 3 * aw / n_qkv, w, L.w_qkv, L.b_qkv);
+        L.w_o = to_bf16(m, p + nm.out + "weight", w * aw);
+        L.b_o = param(m, p + nm.out + "bias", w);
+        if (nm.attn_ln) norm(p, nm.attn_ln, w, L.ln_attn_w, L.ln_attn_b);
+        if (n_fc == 1 && fc != mlp) {   // a fused gated fc1 (GTE's up | gate) holds both halves
+            const std::string fw = p + nm.fc[0] + "weight";
+            const long long rows = param_rows(m, fw, w);
+            MB_CHECK_ARG(rows == fc, "%s has %lld rows, 2 * mlp = %lld are needed", fw.c_str(), rows, fc);
         }
-        MB_CUDA(cudaStreamSynchronize(m->stream));
-        for (int j = 0; j < 3; ++j) m->raw.erase(p + nm.qkv[j] + ".weight");
-        L.w_qkv = wq;
-        L.b_qkv = bq;
-        L.w_o = to_bf16(m, p + nm.out + ".weight", w * w);
-        L.b_o = param(m, p + nm.out + ".bias", w);
-        L.ln1_w = param(m, p + nm.out_ln + ".weight", w);  // post-LN after attention
-        L.ln1_b = param(m, p + nm.out_ln + ".bias", w);
-        L.w_fc = to_bf16(m, p + "intermediate.dense.weight", mlp * w);
-        L.b_fc = param(m, p + "intermediate.dense.bias", mlp);
-        L.w_proj = to_bf16(m, p + "output.dense.weight", w * mlp);
-        L.b_proj = param(m, p + "output.dense.bias", w);
-        L.ln2_w = param(m, p + "output.LayerNorm.weight", w);  // post-LN after the MLP
-        L.ln2_b = param(m, p + "output.LayerNorm.bias", w);
-    }
-}
-
-// Rows of a parameter stored as [rows, w]; its element count must be a multiple of w.
-long long param_rows(b200_model* m, const std::string& name, long long w) {
-    auto it = m->raw.find(name);
-    if (it == m->raw.end()) fail(B200_ERR_MISSING_WEIGHT, "missing parameter '%s'", name.c_str());
-    if ((long long)it->second.size() % w != 0)
-        fail(B200_ERR_INVALID_ARG, "parameter '%s' has %zu elements, not a multiple of %lld", name.c_str(),
-             it->second.size(), w);
-    return (long long)it->second.size() / w;
-}
-
-// NewModel's layers (GTE, verify) in the layouts run_gte_layers reads: the fused qkv_proj and up_gate_proj as they are
-// (up_gate_proj has no bias), attn_ln in ln1 and mlp_ln in ln2.
-void build_gte_layers(b200_model* m, TowerW& T) {
-    const long long w = T.d.width, mlp = T.d.mlp;
-    T.layers.resize(T.d.layers);
-    for (int i = 0; i < T.d.layers; ++i) {
-        const std::string p = "encoder.layer." + std::to_string(i) + ".";
-        LayerW& L = T.layers[i];
-        L.w_qkv = to_bf16(m, p + "attention.qkv_proj.weight", 3 * w * w);
-        L.b_qkv = param(m, p + "attention.qkv_proj.bias", 3 * w);
-        L.w_o = to_bf16(m, p + "attention.o_proj.weight", w * w);
-        L.b_o = param(m, p + "attention.o_proj.bias", w);
-        L.ln1_w = param(m, p + "attn_ln.weight", w);
-        L.ln1_b = param(m, p + "attn_ln.bias", w);
-        const std::string ug = p + "mlp.up_gate_proj.weight";
-        const long long rows = param_rows(m, ug, w);
-        MB_CHECK_ARG(rows == 2 * mlp, "GTE: %s has %lld rows, 2 * text.mlp = %lld are needed", ug.c_str(), rows, 2 * mlp);
-        L.w_fc = to_bf16(m, ug, 2 * mlp * w);
-        L.w_proj = to_bf16(m, p + "mlp.down_proj.weight", w * mlp);
-        L.b_proj = param(m, p + "mlp.down_proj.bias", w);
-        L.ln2_w = param(m, p + "mlp_ln.weight", w);
-        L.ln2_b = param(m, p + "mlp_ln.bias", w);
+        stack_linear(m, p, nm.fc, n_fc, nm.fc_bias, fc_rows, fc / n_fc, w, L.w_fc, L.b_fc);
+        if (nm.mlp_ln) norm(p, nm.mlp_ln, T.mlp_h, L.ln_mlp_w, L.ln_mlp_b);
+        if (T.mlp_h != mlp) pad_blocks(m, p + nm.proj + "weight", w, 1, T.mlp_h, mlp);
+        L.w_proj = to_bf16(m, p + nm.proj + "weight", w * mlp);
+        L.b_proj = param(m, p + nm.proj + "bias", w);
+        norm(p, nm.ln2, w, L.ln2_w, L.ln2_b);
     }
 }
 
@@ -595,17 +605,24 @@ const float* upload_derived(b200_model* m, const std::vector<float>& h) {
     return d;
 }
 
-// SigLIP's timm trunk after the patch conv (open_clip names, verify): pos_embed with the conv bias folded in (the bias
-// is the same for every token, so pos[t] + bias + conv(patch) == pos'[t] + conv(patch)), the blocks, the final norm and
-// the MAP head, whose latent query projection q = latent W_q^T + b_q is computed here once, in double.
+// A timm trunk's pos_embed with the patch conv's bias folded into its patch rows: the bias is the same for every patch,
+// so pos[t] + bias + conv(patch) == pos'[t] + conv(patch); the class rows have no conv term.
+const float* fold_patch_bias(b200_model* m, const TowerW& T, const std::string& trunk) {
+    const long long w = T.d.width;
+    std::vector<float> pos = to_host(param(m, trunk + "pos_embed", (long long)T.tokens * w), (size_t)T.tokens * w);
+    const std::vector<float> bias = to_host(param(m, trunk + "patch_embed.proj.bias", w), (size_t)w);
+    for (long long i = T.cls_rows * w; i < (long long)pos.size(); ++i) pos[i] += bias[i % w];
+    return upload_derived(m, pos);
+}
+
+// SigLIP's timm trunk after the patch conv (open_clip names, verify): pos_embed with the conv bias folded in, the
+// blocks, the final norm and the MAP head, whose latent query projection q = latent W_q^T + b_q is computed here once,
+// in double.
 void build_siglip_vision(b200_model* m, TowerW& T) {
     const long long w = T.d.width;
     const std::string t = "visual.trunk.";
-    std::vector<float> pos = to_host(param(m, t + "pos_embed", (long long)T.tokens * w), (size_t)T.tokens * w);
-    const std::vector<float> bias = to_host(param(m, t + "patch_embed.proj.bias", w), (size_t)w);
-    for (long long i = 0; i < (long long)pos.size(); ++i) pos[i] += bias[i % w];
-    T.pos = upload_derived(m, pos);
-    build_preln_layers(m, T, t + "blocks.", TIMM_BLOCK);
+    T.pos = fold_patch_bias(m, T, t);
+    build_layers(m, T, t + "blocks.", TIMM_BLOCK);
     T.ln_out_w = param(m, t + "norm.weight", w);
     T.ln_out_b = param(m, t + "norm.bias", w);
     const std::string a = t + "attn_pool.";
@@ -764,81 +781,26 @@ void build_vit(b200_model* m, TowerW& T, const char* conv_name, int cls_rows) {
     T.conv_wg = cg;
 }
 
-// The EVA02 trunk (open_clip TimmModel over timm's Eva, verify) in the layouts run_eva_layers reads:
-//   pos       pos_embed with the patch conv's bias folded into the patch rows (the class row has no conv term);
-//   w_qkv     q_proj | k_proj | v_proj [3w, w], b_qkv q bias | 0 | v bias (k_proj has no bias);
-//   w_fc      fc1_g | fc1_x [2 hp, w] with zero rows and zero bias after each part's h rows, so the gate and x halves
-//             start at columns 0 and hp of the GEMM's output and its pad columns are exact zeros;
-//   w_proj    fc2 [w, hp] with zero K columns h .. hp - 1, which meet swiglu_ln's zero pad columns: exact, as for
-//             pad_heads;
-//   rope      the RoPE table of the grid, built in fp64 on the host;
-//   w_tproj   the head Linear [E, w] with its bias.
+// The EVA02 trunk (open_clip TimmModel over timm's Eva, verify): pos_embed with the patch conv's bias folded in, the
+// RoPE table of the grid (built in fp64 on the host), the blocks (EVA_BLOCK: q | k | v with a zero k bias, fc1_g | fc1_x
+// with the hidden size padded to a multiple of 64), the final norm and the head Linear [E, w] with its bias.
 void build_eva_vision(b200_model* m, TowerW& T) {
     const std::string t = "visual.trunk.";
     build_vit(m, T, "visual.trunk.patch_embed.proj.weight", 1);
     const long long w = T.d.width, E = m->desc.embed_dim;
     T.eps = m->desc.layer_norm_eps;
     T.cls = param(m, t + "cls_token", w);
-    std::vector<float> pos = to_host(param(m, t + "pos_embed", (long long)T.tokens * w), (size_t)T.tokens * w);
-    const std::vector<float> bias = to_host(param(m, t + "patch_embed.proj.bias", w), (size_t)w);
-    for (long long i = w; i < (long long)pos.size(); ++i) pos[i] += bias[i % w];
-    T.pos = upload_derived(m, pos);
+    T.pos = fold_patch_bias(m, T, t);
     std::vector<float> rope((size_t)T.grid * T.grid * 64);
     kernels::rope_table(T.grid, m->desc.eva_rope_ref_grid, rope.data());
     T.rope = upload_derived(m, rope);
+    T.rope_first = 1;
+    T.mlp_form = Mlp::SWIGLU_LN;
     // the SwiGLU hidden size is the checkpoint's; it must be the one the model was created with
-    const long long h = param_rows(m, t + "blocks.0.mlp.fc1_g.weight", w), hp = (long long)round_up((size_t)h, 64);
+    const long long h = param_rows(m, t + "blocks.0.mlp.fc1_g.weight", w);
     MB_CHECK_ARG(h == T.d.mlp, "EVA02: %sblocks.0.mlp.fc1_g has %lld rows, vision.mlp is %d", t.c_str(), h, T.d.mlp);
-    T.swiglu_h = (int)h;
-    T.swiglu_hp = (int)hp;
-    T.d.mlp = (int)hp;
-    T.layers.resize(T.d.layers);
-    for (int i = 0; i < T.d.layers; ++i) {
-        const std::string p = t + "blocks." + std::to_string(i) + ".";
-        LayerW& L = T.layers[i];
-        L.ln1_w = param(m, p + "norm1.weight", w);
-        L.ln1_b = param(m, p + "norm1.bias", w);
-        __nv_bfloat16* wqkv = derived_buffer<__nv_bfloat16>(m, (size_t)(3 * w * w));
-        float* bqkv = derived_buffer<float>(m, (size_t)(3 * w));
-        const char* qkv_names[3] = {"attn.q_proj", "attn.k_proj", "attn.v_proj"};
-        MB_CUDA(cudaMemsetAsync(bqkv, 0, (size_t)(3 * w) * sizeof(float), m->stream));
-        for (int j = 0; j < 3; ++j) {
-            const std::string base = p + qkv_names[j];
-            kernels::f32_to_bf16(param(m, base + ".weight", w * w), wqkv + (size_t)(j * w * w), w * w, m->stream);
-            if (j != 1)
-                MB_CUDA(cudaMemcpyAsync(bqkv + j * w, param(m, base + ".bias", w), (size_t)w * sizeof(float),
-                                        cudaMemcpyDeviceToDevice, m->stream));
-        }
-        L.w_qkv = wqkv;
-        L.b_qkv = bqkv;
-        L.ln_attn_w = param(m, p + "attn.norm.weight", w);
-        L.ln_attn_b = param(m, p + "attn.norm.bias", w);
-        L.ln2_w = param(m, p + "norm2.weight", w);
-        L.ln2_b = param(m, p + "norm2.bias", w);
-        __nv_bfloat16* wfc = derived_buffer<__nv_bfloat16>(m, (size_t)(2 * hp * w));
-        float* bfc = derived_buffer<float>(m, (size_t)(2 * hp));
-        MB_CUDA(cudaMemsetAsync(wfc, 0, (size_t)(2 * hp * w) * sizeof(__nv_bfloat16), m->stream));
-        MB_CUDA(cudaMemsetAsync(bfc, 0, (size_t)(2 * hp) * sizeof(float), m->stream));
-        const char* fc1_names[2] = {"mlp.fc1_g", "mlp.fc1_x"};
-        for (int j = 0; j < 2; ++j) {
-            const std::string base = p + fc1_names[j];
-            kernels::f32_to_bf16(param(m, base + ".weight", h * w), wfc + (size_t)(j * hp * w), h * w, m->stream);
-            MB_CUDA(cudaMemcpyAsync(bfc + j * hp, param(m, base + ".bias", h), (size_t)h * sizeof(float),
-                                    cudaMemcpyDeviceToDevice, m->stream));
-        }
-        L.w_fc = wfc;
-        L.b_fc = bfc;
-        MB_CUDA(cudaStreamSynchronize(m->stream));
-        for (int j = 0; j < 3; ++j) m->raw.erase(p + qkv_names[j] + ".weight");
-        for (int j = 0; j < 2; ++j) m->raw.erase(p + fc1_names[j] + ".weight");
-        L.w_o = to_bf16(m, p + "attn.proj.weight", w * w);
-        L.b_o = param(m, p + "attn.proj.bias", w);
-        L.ln_mlp_w = param(m, p + "mlp.norm.weight", h);
-        L.ln_mlp_b = param(m, p + "mlp.norm.bias", h);
-        pad_blocks(m, p + "mlp.fc2.weight", w, 1, h, hp);
-        L.w_proj = to_bf16(m, p + "mlp.fc2.weight", w * hp);
-        L.b_proj = param(m, p + "mlp.fc2.bias", w);
-    }
+    T.d.mlp = (int)round_up((size_t)h, 64);
+    build_layers(m, T, t + "blocks.", EVA_BLOCK);
     T.ln_out_w = param(m, t + "norm.weight", w);
     T.ln_out_b = param(m, t + "norm.bias", w);
     T.w_tproj = to_bf16(m, t + "head.weight", E * w);
@@ -934,7 +896,7 @@ void build_vision(b200_model* m) {
         T.pos = param(m, "visual.positional_embedding", (long long)T.tokens * w);
         T.ln_pre_w = param(m, "visual.ln_pre.weight", w);
         T.ln_pre_b = param(m, "visual.ln_pre.bias", w);
-        build_preln_layers(m, T, "visual.transformer.resblocks.", OPEN_CLIP_BLOCK);
+        build_layers(m, T, "visual.transformer.resblocks.", OPEN_CLIP_BLOCK);
         T.ln_out_w = param(m, "visual.ln_post.weight", w);
         T.ln_out_b = param(m, "visual.ln_post.bias", w);
         T.proj = param(m, "visual.proj", w * m->desc.embed_dim);
@@ -970,7 +932,7 @@ void build_text(b200_model* m) {
         T.act = open_clip_act(m->desc);
         T.tok = param(m, p + "token_embedding.weight", (long long)T.d.vocab * w);
         T.pos = param(m, p + "positional_embedding", (long long)T.d.ctx * w);
-        build_preln_layers(m, T, p + "transformer.resblocks.", OPEN_CLIP_BLOCK);
+        build_layers(m, T, p + "transformer.resblocks.", OPEN_CLIP_BLOCK);
         T.ln_out_w = param(m, p + "ln_final.weight", w);
         T.ln_out_b = param(m, p + "ln_final.bias", w);
         if (siglip) {
@@ -984,17 +946,19 @@ void build_text(b200_model* m) {
     }
     case TextKind::BERT: {
         T.eps = 1e-12f;   // BertConfig's layer_norm_eps
+        T.pre_ln = false;
         T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
         T.pos = param(m, "embeddings.position_embeddings.weight", (long long)T.d.ctx * w);
         const int tv = std::max(1, m->desc.type_vocab);
         T.type0 = param(m, "embeddings.token_type_embeddings.weight", (long long)tv * w);  // row 0 is used
         T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
         T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
-        build_bert_layers(m, T, BERT_NAMES);
+        build_layers(m, T, "encoder.layer.", BERT_LAYER);
         break;
     }
     case TextKind::ROBERTA: {
         T.eps = m->desc.layer_norm_eps;
+        T.pre_ln = false;
         T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
         // positions run pad_id + 1 .. pad_id + ctx (pads take pad_id): the table has at least ctx + pad_id + 1 rows
         const long long pos_rows = param_rows(m, "embeddings.position_embeddings.weight", w);
@@ -1005,25 +969,28 @@ void build_text(b200_model* m) {
         T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
         T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
         if (m->kind.mpnet) {
-            build_bert_layers(m, T, MPNET_NAMES);
+            build_layers(m, T, "encoder.layer.", MPNET_LAYER);
             T.rel_bias = build_rel_bias(m, T);
         } else {
             T.type0 = param(m, "embeddings.token_type_embeddings.weight", w);   // type_vocab_size 1
-            build_bert_layers(m, T, BERT_NAMES);
+            build_layers(m, T, "encoder.layer.", BERT_LAYER);
         }
         break;
     }
     case TextKind::GTE: {
         T.eps = m->desc.layer_norm_eps;
+        T.pre_ln = false;
+        T.mlp_form = Mlp::GEGLU;
         T.tok = param(m, "embeddings.word_embeddings.weight", (long long)T.d.vocab * w);
         const int tv = std::max(1, m->desc.type_vocab);
         T.type0 = param(m, "embeddings.token_type_embeddings.weight", (long long)tv * w);  // row 0 is used
         T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
         T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
-        build_gte_layers(m, T);
+        build_layers(m, T, "encoder.layer.", GTE_LAYER);
         std::vector<float> rope((size_t)T.d.ctx * 64);
         kernels::rope_table_ntk(T.d.ctx, m->desc.rope_theta, m->desc.rope_ntk_factor, rope.data());
         T.rope = upload_derived(m, rope);
+        T.rope_pairing = kernels::RopePairing::HALF;
         break;
     }
     }
@@ -1074,79 +1041,38 @@ void linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, con
 }
 
 // The transformer layers of a tower.  x (fp32) is the residual stream, h (bf16) the LayerNorm output the next GEMM
-// consumes.  Pre-LN (open_clip ResidualAttentionBlock, timm's ViT Block): LN x -> h before the QKV and fc1 GEMMs.
-// Post-LN (HF BertLayer, MPNetLayer with the tower's relative-position bias): on entry x and h both hold the embedding
-// LayerNorm output, and LN rewrites x in place (x -> x and h) after each residual GEMM.
-void run_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S, int mask_mode, bool pre_ln) {
-    const int M = B * S, w = T.d.width, aw = T.aw, mlp = T.d.mlp;
+// consumes.  Pre-LN (open_clip ResidualAttentionBlock, timm's ViT and Eva Blocks): LN x -> h before the QKV and fc1
+// GEMMs.  Post-LN (HF BertLayer, MPNetLayer with the tower's relative-position bias, NewModel): on entry x and h both
+// hold the embedding LayerNorm output, and LN rewrites x in place (x -> x and h) after each residual GEMM.  A tower may
+// rotate q and k after the QKV GEMM (T.rope), LayerNorm the attention output before the out-projection (EVA02's
+// attn.norm) and run a gated MLP (Mlp).
+void run_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S, int mask_mode) {
+    const int M = B * S, w = T.d.width, aw = T.aw, mlp = T.d.mlp, fc1 = fc1_cols(T);
     float* x = m->x.get();
+    __nv_bfloat16 *h = m->h.get(), *qkv = m->qkv.get(), *o = m->o.get(), *u = m->u.get();
     const int32_t* kv_len = mask_mode == attention::MASK_KEYLEN ? m->aux.get() : nullptr;
     auto ln = [&](const float* g, const float* b) {
-        c.n += kernels::layernorm(x, w, g, b, T.eps, M, w, pre_ln ? nullptr : x, m->h.get(), m->stream);
+        c.n += kernels::layernorm(x, w, g, b, T.eps, M, w, T.pre_ln ? nullptr : x, h, m->stream);
     };
     for (const LayerW& L : T.layers) {
-        if (pre_ln) ln(L.ln1_w, L.ln1_b);
-        linear(m, c, m->h.get(), M, w, L.w_qkv, 3 * aw, epilogue(m->qkv.get(), 3 * aw, L.b_qkv));
+        if (T.pre_ln) ln(L.ln1_w, L.ln1_b);
+        linear(m, c, h, M, w, L.w_qkv, 3 * aw, epilogue(qkv, 3 * aw, L.b_qkv));
+        if (T.rope) c.n += kernels::rope_qk(qkv, B, S, T.rope_first, aw, T.rope, T.rope_pairing, m->stream);
         profiled(m, c, 1, [&] {
-            return attention::launch(m->qkv.get(), m->o.get(), B, S, aw, T.d.heads, mask_mode, kv_len, T.rel_bias,
-                                     m->stream, w / T.d.heads);
+            return attention::launch(qkv, o, B, S, aw, T.d.heads, mask_mode, kv_len, T.rel_bias, m->stream,
+                                     w / T.d.heads);
         });
-        linear(m, c, m->o.get(), M, aw, L.w_o, w, epilogue(x, w, L.b_o, gemm::ACT_NONE, true, x, w));
-        ln(pre_ln ? L.ln2_w : L.ln1_w, pre_ln ? L.ln2_b : L.ln1_b);
-        linear(m, c, m->h.get(), M, w, L.w_fc, mlp, epilogue(m->u.get(), mlp, L.b_fc, T.act));
-        linear(m, c, m->u.get(), M, mlp, L.w_proj, w, epilogue(x, w, L.b_proj, gemm::ACT_NONE, true, x, w));
-        if (!pre_ln) ln(L.ln2_w, L.ln2_b);
-    }
-}
-
-// The EVA02 trunk's layers over B images of S tokens (open_clip TimmModel over timm's Eva, verify): pre-LN blocks whose
-// q and k are rotated after the QKV GEMM (rope_qk), whose attention output is LayerNorm-ed (attn.norm) before the
-// out-projection, and whose MLP is a SwiGLU with a LayerNorm over its hidden row (mlp.norm).  fc1 writes the gate and
-// x halves, 2 hp columns, into u; swiglu_ln overwrites each row's gate half with the normalised hidden row, which fc2
-// reads at row stride 2 hp.
-void run_eva_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S) {
-    const int M = B * S, w = T.d.width, hp = T.swiglu_hp;
-    float* x = m->x.get();
-    __nv_bfloat16 *h = m->h.get(), *qkv = m->qkv.get(), *o = m->o.get(), *u = m->u.get();
-    for (const LayerW& L : T.layers) {
-        c.n += kernels::layernorm(x, w, L.ln1_w, L.ln1_b, T.eps, M, w, nullptr, h, m->stream);
-        linear(m, c, h, M, w, L.w_qkv, 3 * w, epilogue(qkv, 3 * w, L.b_qkv));
-        c.n += kernels::rope_qk(qkv, B, S, 1, w, T.rope, kernels::RopePairing::INTERLEAVED, m->stream);
-        profiled(m, c, 1, [&] {
-            return attention::launch(qkv, o, B, S, w, T.d.heads, attention::MASK_NONE, nullptr, attention::RelBias{},
-                                     m->stream);
-        });
-        c.n += kernels::layernorm_bf16(o, w, L.ln_attn_w, L.ln_attn_b, T.eps, M, w, h, m->stream);
-        linear(m, c, h, M, w, L.w_o, w, epilogue(x, w, L.b_o, gemm::ACT_NONE, true, x, w));
-        c.n += kernels::layernorm(x, w, L.ln2_w, L.ln2_b, T.eps, M, w, nullptr, h, m->stream);
-        linear(m, c, h, M, w, L.w_fc, 2 * hp, epilogue(u, 2 * hp, L.b_fc));
-        c.n += kernels::swiglu_ln(u, M, hp, T.swiglu_h, L.ln_mlp_w, L.ln_mlp_b, T.eps, u, 2 * hp, m->stream);
-        linear(m, c, u, M, hp, L.w_proj, w, epilogue(x, w, L.b_proj, gemm::ACT_NONE, true, x, w), 2 * hp);
-    }
-}
-
-// GTE's layers over B sequences of S tokens (NewModel, verify): post-LN as run_layers' BERT path, with q and k rotated
-// after the QKV GEMM (rope_qk, rotate-half pairs) and a GeGLU MLP.  On entry x and h both hold the embedding LayerNorm
-// output.  up_gate_proj writes up | gate, 2 mlp columns, into u; geglu overwrites each row's up half with
-// GELU(gate) * up, which down_proj reads at row stride 2 mlp.
-void run_gte_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S) {
-    const int M = B * S, w = T.d.width, mlp = T.d.mlp;
-    float* x = m->x.get();
-    __nv_bfloat16 *h = m->h.get(), *qkv = m->qkv.get(), *o = m->o.get(), *u = m->u.get();
-    const int32_t* kv_len = m->aux.get();
-    for (const LayerW& L : T.layers) {
-        linear(m, c, h, M, w, L.w_qkv, 3 * w, epilogue(qkv, 3 * w, L.b_qkv));
-        c.n += kernels::rope_qk(qkv, B, S, 0, w, T.rope, kernels::RopePairing::HALF, m->stream);
-        profiled(m, c, 1, [&] {
-            return attention::launch(qkv, o, B, S, w, T.d.heads, attention::MASK_KEYLEN, kv_len, attention::RelBias{},
-                                     m->stream);
-        });
-        linear(m, c, o, M, w, L.w_o, w, epilogue(x, w, L.b_o, gemm::ACT_NONE, true, x, w));
-        c.n += kernels::layernorm(x, w, L.ln1_w, L.ln1_b, T.eps, M, w, x, h, m->stream);
-        linear(m, c, h, M, w, L.w_fc, 2 * mlp, epilogue(u, 2 * mlp));
-        c.n += kernels::geglu(u, M, mlp, u, 2 * mlp, m->stream);
-        linear(m, c, u, M, mlp, L.w_proj, w, epilogue(x, w, L.b_proj, gemm::ACT_NONE, true, x, w), 2 * mlp);
-        c.n += kernels::layernorm(x, w, L.ln2_w, L.ln2_b, T.eps, M, w, x, h, m->stream);
+        if (L.ln_attn_w) c.n += kernels::layernorm_bf16(o, w, L.ln_attn_w, L.ln_attn_b, T.eps, M, w, h, m->stream);
+        linear(m, c, L.ln_attn_w ? h : o, M, aw, L.w_o, w, epilogue(x, w, L.b_o, gemm::ACT_NONE, true, x, w));
+        ln(T.pre_ln ? L.ln2_w : L.ln1_w, T.pre_ln ? L.ln2_b : L.ln1_b);
+        linear(m, c, h, M, w, L.w_fc, fc1,
+               epilogue(u, fc1, L.b_fc, T.mlp_form == Mlp::ACT ? T.act : gemm::ACT_NONE));
+        if (T.mlp_form == Mlp::SWIGLU_LN)
+            c.n += kernels::swiglu_ln(u, M, mlp, T.mlp_h, L.ln_mlp_w, L.ln_mlp_b, T.eps, u, fc1, m->stream);
+        else if (T.mlp_form == Mlp::GEGLU)
+            c.n += kernels::geglu(u, M, mlp, u, fc1, m->stream);
+        linear(m, c, u, M, mlp, L.w_proj, w, epilogue(x, w, L.b_proj, gemm::ACT_NONE, true, x, w), fc1);
+        if (!T.pre_ln) ln(L.ln2_w, L.ln2_b);
     }
 }
 
@@ -1230,7 +1156,7 @@ void patch_embed(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, 
 }
 
 // A ViT trunk over n images (device uint8 [n, S, S, 3] u8, or device fp32 CHW f32): patch embedding, ln_pre (CLIP) and
-// the layers (EVA02's own, which have a RoPE table), leaving the n * T.tokens token rows in x.
+// the layers, leaving the n * T.tokens token rows in x.
 void forward_vit(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, const float* f32, int n) {
     const int w = T.d.width;
     float* x = m->x.get();
@@ -1241,10 +1167,7 @@ void forward_vit(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, 
     patch_embed(m, c, T, u8, f32, n, epilogue(x, w, nullptr, gemm::ACT_NONE, true, x, w));
     if (T.ln_pre_w)
         c.n += kernels::layernorm(x, w, T.ln_pre_w, T.ln_pre_b, T.eps, n * T.tokens, w, x, nullptr, m->stream);
-    if (T.rope)
-        run_eva_layers(m, c, T, n, T.tokens);
-    else
-        run_layers(m, c, T, n, T.tokens, attention::MASK_NONE, true);
+    run_layers(m, c, T, n, T.tokens, attention::MASK_NONE);
 }
 
 // SigLIP vision head over the n * S token rows in x: final LayerNorm of every token -> h, K|V projection -> qkv
@@ -1351,14 +1274,14 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
     case TextKind::CLIP:
         // causal layers; ln_final of each sequence's eot row, projection, optional L2
         c.n += kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, x, aux, m->stream);
-        run_layers(m, c, T, n, S, attention::MASK_CAUSAL, true);
+        run_layers(m, c, T, n, S, attention::MASK_CAUSAL);
         c.n += kernels::clip_head(x, S, aux, T.ln_out_w, T.ln_out_b, T.eps, T.proj, n, w, E, normalize, d_out,
                                   m->pooled.get(), m->stream);
         break;
     case TextKind::SIGLIP:
         // bidirectional layers; ln_final of each sequence's last row (stride S rows) -> h [n, w], biased projection
         c.n += kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, x, aux, m->stream);
-        run_layers(m, c, T, n, S, attention::MASK_NONE, true);
+        run_layers(m, c, T, n, S, attention::MASK_NONE);
         c.n += kernels::layernorm(x + (size_t)(S - 1) * w, (long long)S * w, T.ln_out_w, T.ln_out_b, T.eps, n, w,
                                   nullptr, m->h.get(), m->stream);
         linear(m, c, m->h.get(), n, w, T.w_tproj, E, epilogue(m->pooled.get(), E, T.b_tproj, gemm::ACT_NONE, true));
@@ -1366,21 +1289,16 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
         break;
     case TextKind::BERT:
     case TextKind::ROBERTA:
-        // RoBERTa position ids count from pad_id; XLM-R also adds its single token-type row (T.type0 is NULL for MPNet)
-        if (m->kind.text == TextKind::BERT)
+    case TextKind::GTE:
+        // RoBERTa position ids count from pad_id; XLM-R also adds its single token-type row (T.type0 is NULL for
+        // MPNet); GTE has no position table (T.pos is NULL)
+        if (m->kind.text != TextKind::ROBERTA)
             c.n += kernels::bert_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, T.eps, n, S, w,
                                           T.d.vocab, x, m->h.get(), aux, m->stream);
         else
             c.n += kernels::roberta_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, T.eps, n, S,
                                              w, T.d.vocab, m->desc.pad_id, x, m->h.get(), aux, m->stream);
-        run_layers(m, c, T, n, S, attention::MASK_KEYLEN, false);
-        c.n += kernels::bert_head(x, aux, n, S, w, m->desc.pool, normalize, d_out, m->stream);
-        break;
-    case TextKind::GTE:
-        // BERT's embedding without a position row, the rotary layers, BERT's pooling
-        c.n += kernels::bert_embed_ln(d_ids, d_mask, T.tok, nullptr, T.type0, T.emb_ln_w, T.emb_ln_b, T.eps, n, S, w,
-                                      T.d.vocab, x, m->h.get(), aux, m->stream);
-        run_gte_layers(m, c, T, n, S);
+        run_layers(m, c, T, n, S, attention::MASK_KEYLEN);
         c.n += kernels::bert_head(x, aux, n, S, w, m->desc.pool, normalize, d_out, m->stream);
         break;
     }
@@ -1548,8 +1466,10 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
             m->vision.d.width = desc->convnext_dims[0];
         }
         if (kind.text != TextKind::NONE) m->text.d = desc->text;
-        for (TowerW* T : {&m->vision, &m->text})
+        for (TowerW* T : {&m->vision, &m->text}) {
             if (T->d.heads > 0) T->aw = T->d.heads * kernel_head_dim(T->d.width / T->d.heads);
+            T->mlp_h = T->d.mlp;
+        }
         gemm::configure();
         *out = m.release();
     });
@@ -1599,9 +1519,7 @@ int b200_model_finalize(b200_model* m) {
             max_tok = std::max(max_tok, B * T->tokens);   // (0 for a missing tower)
             max_w = std::max<long long>(max_w, T->d.width);
             max_aw = std::max<long long>({max_aw, T->d.width, T->aw});   // qkv and o: padded heads are wider
-            // EVA02: gate | x; GTE: up | gate
-            const long long gte_u = T == &m->text && m->kind.text == TextKind::GTE ? 2LL * T->d.mlp : 0;
-            max_mlp = std::max<long long>({max_mlp, T->d.mlp, T->map.mlp, 2LL * T->swiglu_hp, gte_u});
+            max_mlp = std::max<long long>({max_mlp, fc1_cols(*T), T->map.mlp});
         }
         const long long bytes_per_tok = std::max<long long>(1, max_w * (4 + 2) + max_aw * (6 + 2) + max_mlp * 2);
         const long long cap_tok = (24LL << 30) / bytes_per_tok;

@@ -8,6 +8,7 @@ import torch
 from torch.autograd import DeviceType
 from torch.profiler import ProfilerActivity, profile
 
+import _eva02_oracle as V
 import _mpnet_oracle as M
 import _siglip_oracle as O
 import _xlmr_oracle as X
@@ -39,6 +40,12 @@ def _clip_resnet():
     return "clip_resnet", arch, random_clip_resnet_weights(arch, seed=3), 1000
 
 
+def _clip_eva():
+    from marqo_b200.weights import random_eva02_weights
+    arch = V.arch(V.B16, eva_layers=1, text_layers=1)
+    return "clip_eva", arch, random_eva02_weights(arch, seed=7), arch["vocab"]
+
+
 def _bert():
     cfg = E.tiny_bert("mean")
     arch = dict(width=cfg.width, layers=cfg.layers, heads=cfg.heads, mlp=cfg.mlp, vocab=cfg.vocab, max_pos=cfg.max_pos,
@@ -54,6 +61,13 @@ def _mpnet():
 def _xlmr():
     cfg = X.tiny_xlmr()
     return "xlmr", X.engine_config(cfg), X.make_xlmr_weights(cfg, seed=6), cfg.vocab
+
+
+def _gte():
+    from marqo_b200 import model_registry as R
+    from marqo_b200.weights import random_gte_weights
+    arch = dict(R.get_model_properties("Marqo/dunzhang-stella_en_400M_v5")["arch"], layers=2)
+    return "gte", arch, random_gte_weights(arch, seed=8), arch["vocab"]
 
 
 def _kernels(fn):
@@ -94,8 +108,8 @@ def _calls(enc, vocab, rng):
     return calls
 
 
-@pytest.mark.parametrize("make", [_clip, _siglip, _clip_resnet, _bert, _mpnet, _xlmr],
-                         ids=["clip", "siglip", "clip_resnet", "bert", "mpnet", "xlmr"])
+@pytest.mark.parametrize("make", [_clip, _siglip, _clip_resnet, _clip_eva, _bert, _mpnet, _xlmr, _gte],
+                         ids=["clip", "siglip", "clip_resnet", "clip_eva", "bert", "mpnet", "xlmr", "gte"])
 def test_reported_launches_equal_the_kernels_run(gpu_required, make):
     from marqo_b200.engine import Encoder
     arch_name, arch, sd, vocab = make()
