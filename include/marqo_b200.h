@@ -663,6 +663,28 @@ int b200_debug_ln_pixels(int device, const float* x, int n, int H, int W, int C,
  * [n, C].  C a multiple of 64, <= 3072. */
 int b200_debug_pool_ln(int device, const float* x, int n, int HW, int C, const float* gamma, const float* beta, float eps,
                        void* out, void* stream);
+/* Transformer layers [first, first + count) of a finalized model's vision (tower 0) or text (tower 1) tower, through
+ * the layer runner the encode calls use, with the tower's own mask: none for vision and SigLIP text, causal for CLIP
+ * text, key lengths for the BERT family, MPNet, XLM-R and GTE.  x_in fp32 [B*S, width] is the residual stream the
+ * first layer reads (a post-LN tower also gets h = bf16(x_in), as its embedding LayerNorm leaves them); kv_len int32
+ * [B] (NULL: S for every sequence), each in 0..S, is read by the key-length towers only.  S must be the vision
+ * tower's token count, or 1..ctx for a text tower.  The call first waits for the model's own stream (an encode call
+ * with sync = 0 may still use the workspaces), then runs on `stream`.  Afterwards, each output that is not NULL
+ * receives what the last layer left: x_out fp32 [B*S, width] the residual stream; h_out bf16 [B*S, width] the last
+ * LayerNorm output (pre-LN: bf16(LN2(x_mid)), fc1's input; post-LN: bf16(x_out)); qkv_out bf16 [B*S, 3*aw] the QKV
+ * projection after any rotary embedding; o_out bf16 [B*S, aw] the attention output; u_out bf16 [B*S, fc1] the MLP
+ * hidden rows after the activation or gate (a gated MLP's result in the first fc1 / 2 columns).  width, aw and fc1
+ * come from b200_debug_layer_cols.  Nothing but the model's workspaces and the outputs is written.
+ * B200_ERR_INVALID_ARG for a tower the model lacks, a range outside the tower, B above max_batch, B*S above the
+ * workspace, a bad S or a key length outside 0..S. */
+int b200_debug_layers(b200_model* m, int tower, int first, int count, const float* x_in, int B, int S,
+                      const int32_t* kv_len, float* x_out, void* h_out, void* qkv_out, void* o_out, void* u_out,
+                      void* stream);
+/* The row widths of b200_debug_layers' outputs for a finalized model's tower: out[0] the width, out[1] aw (heads times
+ * the attention kernel's head dim: the tower's, or 96 for 80 and 88 and 128 for 104, zero-padded), out[2] fc1 (mlp, or
+ * for a gated MLP both halves of mlp rounded up to 64).  out: host int32 [3].  B200_ERR_INVALID_ARG for a tower the
+ * model lacks. */
+int b200_debug_layer_cols(b200_model* m, int tower, int32_t* out);
 /* Bytes of device memory the library holds right now, over all devices and handles of this process (indexes,
  * exchanges, models and the scratch of calls in flight).  Memory from b200_host_alloc is not counted.  Returns to its
  * earlier value once every handle created in between is destroyed: a leak check. */

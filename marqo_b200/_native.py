@@ -158,6 +158,8 @@ _SIGNATURES = {
     "b200_debug_ln_pixels": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, C.c_float, C.c_int, _P,
                                        _P]),
     "b200_debug_pool_ln": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_float, _P, _P]),
+    "b200_debug_layers": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P]),
+    "b200_debug_layer_cols": (C.c_int, [_P, C.c_int, _P]),
     "b200_debug_device_bytes": (C.c_int, [C.POINTER(C.c_int64)]),
     "b200_jpeg_info": (C.c_int, [_P, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200_jpeg_decode_batch": (C.c_int, [C.c_int, _P, _P, C.c_int, _P, _P, _P, _P]),

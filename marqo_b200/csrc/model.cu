@@ -1045,16 +1045,19 @@ void linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, con
 // GEMMs.  Post-LN (HF BertLayer, MPNetLayer with the tower's relative-position bias, NewModel): on entry x and h both
 // hold the embedding LayerNorm output, and LN rewrites x in place (x -> x and h) after each residual GEMM.  A tower may
 // rotate q and k after the QKV GEMM (T.rope), LayerNorm the attention output before the out-projection (EVA02's
-// attn.norm) and run a gated MLP (Mlp).
-void run_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S, int mask_mode) {
+// attn.norm) and run a gated MLP (Mlp).  Layers [first, first + count) run (count < 0: to the last one).
+void run_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S, int mask_mode, int first = 0,
+                int count = -1) {
     const int M = B * S, w = T.d.width, aw = T.aw, mlp = T.d.mlp, fc1 = fc1_cols(T);
+    const int end = count < 0 ? (int)T.layers.size() : first + count;
     float* x = m->x.get();
     __nv_bfloat16 *h = m->h.get(), *qkv = m->qkv.get(), *o = m->o.get(), *u = m->u.get();
     const int32_t* kv_len = mask_mode == attention::MASK_KEYLEN ? m->aux.get() : nullptr;
     auto ln = [&](const float* g, const float* b) {
         c.n += kernels::layernorm(x, w, g, b, T.eps, M, w, T.pre_ln ? nullptr : x, h, m->stream);
     };
-    for (const LayerW& L : T.layers) {
+    for (int i = first; i < end; ++i) {
+        const LayerW& L = T.layers[i];
         if (T.pre_ln) ln(L.ln1_w, L.ln1_b);
         linear(m, c, h, M, w, L.w_qkv, 3 * aw, epilogue(qkv, 3 * aw, L.b_qkv));
         if (T.rope) c.n += kernels::rope_qk(qkv, B, S, T.rope_first, aw, T.rope, T.rope_pairing, m->stream);
@@ -1426,6 +1429,16 @@ void check_tokens_args(b200_model* m, int n, int S) {
     MB_CHECK_ARG(S > 0 && S <= m->text.tokens, "sequence length %d out of range (1..%d)", S, m->text.tokens);
 }
 
+// The transformer tower b200_debug_layers runs: 0 vision, 1 text, if the model has one with layers.
+const TowerW& layer_tower(b200_model* m, int tower) {
+    MB_CHECK_ARG(tower == 0 || tower == 1, "tower %d must be 0 (vision) or 1 (text)", tower);
+    const VisionKind vk = m->kind.vision;
+    MB_CHECK_ARG(tower == 0 ? vk == VisionKind::CLIP_VIT || vk == VisionKind::SIGLIP_VIT || vk == VisionKind::EVA_VIT
+                            : m->kind.text != TextKind::NONE,
+                 "this model has no transformer %s tower", tower == 0 ? "vision" : "text");
+    return tower == 0 ? m->vision : m->text;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1716,6 +1729,79 @@ int b200_debug_relative_position_buckets(int num_buckets, int max_distance, int 
                      "bad bucket parameters");
         for (int d = -(max_len - 1); d <= max_len - 1; ++d)
             out[d + max_len - 1] = relative_position_bucket(d, num_buckets, max_distance);
+    });
+}
+
+int b200_debug_layer_cols(b200_model* m, int tower, int32_t* out) {
+    return guarded([&] {
+        require_ready(m);
+        MB_CHECK_ARG(out != nullptr, "NULL buffer");
+        const TowerW& T = layer_tower(m, tower);
+        out[0] = T.d.width;
+        out[1] = T.aw;
+        out[2] = fc1_cols(T);
+    });
+}
+
+int b200_debug_layers(b200_model* m, int tower, int first, int count, const float* x_in, int B, int S,
+                      const int32_t* kv_len, float* x_out, void* h_out, void* qkv_out, void* o_out, void* u_out,
+                      void* stream) {
+    return guarded([&] {
+        require_ready(m);
+        MB_CHECK_ARG(x_in != nullptr, "NULL buffer");
+        std::lock_guard<std::mutex> lk(m->mu);
+        const TowerW& T = layer_tower(m, tower);
+        const bool vision = tower == 0;
+        const TextKind tk = m->kind.text;
+        const int L = (int)T.layers.size();
+        MB_CHECK_ARG(first >= 0 && count > 0 && first <= L - count, "layers [%d, %d + %d) outside the tower's %d", first,
+                     first, count, L);
+        MB_CHECK_ARG(B > 0 && B <= m->desc.max_batch, "B %d out of range (1..%d)", B, m->desc.max_batch);
+        MB_CHECK_ARG(vision ? S == T.tokens : S > 0 && S <= T.tokens, "S %d: the %s tower takes %s%d tokens", S,
+                     vision ? "vision" : "text", vision ? "" : "1..", T.tokens);
+        MB_CHECK_ARG((long long)B * S <= m->max_tokens, "B * S = %lld rows exceed the workspace's %lld",
+                     (long long)B * S, m->max_tokens);
+        // the mask of the tower's forward pass (forward_vit, forward_tokens_eager)
+        const int mask = vision || tk == TextKind::SIGLIP ? attention::MASK_NONE
+                         : tk == TextKind::CLIP             ? attention::MASK_CAUSAL
+                                                            : attention::MASK_KEYLEN;
+        DeviceGuard g(m->device);
+        // an encode call with sync = 0 may still be using the workspaces on the model's stream
+        MB_CUDA(cudaStreamSynchronize(m->stream));
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        std::vector<int32_t> lens((size_t)B, S);
+        if (mask == attention::MASK_KEYLEN && kv_len) {
+            MB_CUDA(cudaMemcpyAsync(lens.data(), kv_len, lens.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+            MB_CUDA(cudaStreamSynchronize(s));
+            for (int b = 0; b < B; ++b)
+                MB_CHECK_ARG(lens[b] >= 0 && lens[b] <= S, "kv_len[%d] = %d outside 0..%d", b, lens[b], S);
+        }
+        const cudaStream_t saved = m->stream;
+        m->stream = s;
+        try {
+            const size_t M = (size_t)B * S, w = T.d.width;
+            MB_CUDA(cudaMemcpyAsync(m->x.get(), x_in, M * w * sizeof(float), cudaMemcpyDeviceToDevice, s));
+            // a post-LN tower's layers start from the embedding LayerNorm's two outputs, x and h = bf16(x)
+            if (!T.pre_ln) kernels::f32_to_bf16(m->x.get(), m->h.get(), (long long)(M * w), s);
+            if (mask == attention::MASK_KEYLEN) {
+                MB_CUDA(cudaMemcpyAsync(m->aux.get(), lens.data(), lens.size() * sizeof(int32_t), cudaMemcpyHostToDevice,
+                                        s));
+                MB_CUDA(cudaStreamSynchronize(s));   // `lens` is pageable
+            }
+            Counter c;
+            run_layers(m, c, T, B, S, mask, first, count);
+            const size_t aw = T.aw, fc1 = fc1_cols(T);
+            if (x_out) MB_CUDA(cudaMemcpyAsync(x_out, m->x.get(), M * w * sizeof(float), cudaMemcpyDeviceToDevice, s));
+            if (h_out) MB_CUDA(cudaMemcpyAsync(h_out, m->h.get(), M * w * 2, cudaMemcpyDeviceToDevice, s));
+            if (qkv_out) MB_CUDA(cudaMemcpyAsync(qkv_out, m->qkv.get(), M * 3 * aw * 2, cudaMemcpyDeviceToDevice, s));
+            if (o_out) MB_CUDA(cudaMemcpyAsync(o_out, m->o.get(), M * aw * 2, cudaMemcpyDeviceToDevice, s));
+            if (u_out) MB_CUDA(cudaMemcpyAsync(u_out, m->u.get(), M * fc1 * 2, cudaMemcpyDeviceToDevice, s));
+            MB_CUDA(cudaStreamSynchronize(s));
+        } catch (...) {
+            m->stream = saved;
+            throw;
+        }
+        m->stream = saved;
     });
 }
 

@@ -719,6 +719,37 @@ def debug_patch_embed(images_u8, patch: int, conv_w, mean, std, pos=None, cls=No
     return _host(out)
 
 
+def layer_cols(enc: Encoder, tower: str) -> Tuple[int, int, int]:
+    """(width, aw, fc1) of a transformer tower's layer buffers, as the library lays them out (b200_debug_layer_cols):
+    aw the attention width with every head zero-padded to the attention kernel's head dim, fc1 the columns fc1
+    writes."""
+    out = np.zeros(3, np.int32)
+    N.check(enc._lib.b200_debug_layer_cols(enc._handle(), 0 if tower == "vision" else 1, _ptr(out)))
+    return int(out[0]), int(out[1]), int(out[2])
+
+
+def debug_layers(enc: Encoder, tower: str, first: int, count: int, x_in, S: int, kv_len=None) -> dict:
+    """Layers [first, first + count) of enc's "vision" or "text" tower through the encoder's own layer runner, from
+    the residual rows x_in fp32 [B * S, width] (a torch tensor on the encoder's device, or a host array), with key
+    lengths kv_len [B] (each in 0..S) for the key-length towers (None: S each).  Returns what the last layer left, as
+    device tensors: {"x": fp32 [B * S, width], "h": bf16 [B * S, width] the last LayerNorm output (pre-LN: fc1's
+    input), "qkv": bf16 [B * S, 3 aw] after any rotary embedding, "o": bf16 [B * S, aw], "u": bf16 [B * S, fc1] after
+    the activation or gate} (layer_cols gives aw and fc1)."""
+    w, aw, fc1 = layer_cols(enc, tower)
+    d = _Staging(enc.device)
+    x = x_in.to(device=d.dev, dtype=d.torch.float32).contiguous() if hasattr(x_in, "to") else d.up(x_in)
+    if x.dim() != 2 or x.shape[1] != w or S < 1 or x.shape[0] % S != 0:
+        raise ValueError(f"expected x_in [B * {S}, {w}], got {tuple(x.shape)}")
+    M = x.shape[0]
+    kl = None if kv_len is None else d.up(kv_len, "int32")
+    out = {"x": d.empty((M, w)), "h": d.empty((M, w), "bfloat16"), "qkv": d.empty((M, 3 * aw), "bfloat16"),
+           "o": d.empty((M, aw), "bfloat16"), "u": d.empty((M, fc1), "bfloat16")}
+    N.check(enc._lib.b200_debug_layers(enc._handle(), 0 if tower == "vision" else 1, first, count, _dptr(x), M // S,
+                                       S, _dptr(kl), _dptr(out["x"]), _dptr(out["h"]), _dptr(out["qkv"]),
+                                       _dptr(out["o"]), _dptr(out["u"]), d.stream))
+    return out
+
+
 def debug_attention(qkv, B: int, S: int, W: int, H: int, mask: int = 0, kv_len=None, device: int = 0,
                     rel_bias=None) -> np.ndarray:
     """softmax(q k^T / sqrt(hd) + mask) v over packed qkv.  rel_bias: MPNet's relative-position bias, fp32
