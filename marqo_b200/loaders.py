@@ -33,14 +33,7 @@ from .s2_inference import Modality, UnidentifiedImageError, _is_image, _is_tenso
 def _resolve_weights(props: dict, arch: dict, kind: str) -> Dict[str, np.ndarray]:
     w = props.get("weights")
     if w is None and props.get("random_init") is not None:
-        seed = int(props["random_init"])
-        random = {"clip": weights_mod.random_clip_weights, "siglip": weights_mod.random_siglip_weights,
-                  "clip_resnet": weights_mod.random_clip_resnet_weights,
-                  "clip_convnext": weights_mod.random_clip_convnext_weights,
-                  "clip_eva": weights_mod.random_eva02_weights,
-                  "bert": weights_mod.random_bert_weights, "mpnet": weights_mod.random_mpnet_weights,
-                  "xlmr": weights_mod.random_xlmr_weights, "gte": weights_mod.random_gte_weights}[kind]
-        return random(arch, seed)
+        return weights_mod.random_weights(kind, arch, int(props["random_init"]))
     if w is None:
         raise ModelLoadError("model_properties needs `weights` (state dict or checkpoint path) or `random_init`; "
                              "checkpoint download is Marqo's job (open_clip_model.py:107-131) and out of scope here")

@@ -388,3 +388,12 @@ def random_mpnet_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
         sd[p + "output.LayerNorm.weight"] = _vec(g, w, 0.1, 1.0)
         sd[p + "output.LayerNorm.bias"] = _vec(g, w)
     return sd
+
+
+def random_weights(kind: str, arch: dict, seed: int) -> Dict[str, np.ndarray]:
+    """Seeded random weights for an Encoder of `kind` ("clip", "siglip", "clip_resnet", "clip_convnext", "clip_eva",
+    "bert", "mpnet", "xlmr" or "gte"); KeyError for any other kind."""
+    return {"clip": random_clip_weights, "siglip": random_siglip_weights, "clip_resnet": random_clip_resnet_weights,
+            "clip_convnext": random_clip_convnext_weights, "clip_eva": random_eva02_weights,
+            "bert": random_bert_weights, "mpnet": random_mpnet_weights, "xlmr": random_xlmr_weights,
+            "gte": random_gte_weights}[kind](arch, seed)

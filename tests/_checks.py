@@ -1,7 +1,9 @@
-"""Checks and inputs shared by the test files: embedding parity against an oracle, top-k parity against the score
-oracle, and the vectorise -> GpuTensorIndex -> search seam, each written once so that every model family is held to the
-same bar."""
+"""Checks and inputs shared by the test files: embedding parity against an oracle, every input path of an image tower,
+refusals at create time, top-k parity against the score oracle, and the vectorise -> GpuTensorIndex -> search seam,
+each written once so that every model family is held to the same bar.  A file whose torch oracle runs on the GPU
+imports the autouse fixture fp32_oracle by name."""
 import numpy as np
+import pytest
 import torch
 
 COS_TOL = 1e-3   # BASELINE.json north_star: cosine >= 1 - 1e-3 per vector
@@ -31,6 +33,78 @@ def assert_embeddings_match(got, ref, tol=COS_TOL, unit_norm=True):
     assert float((1 - c).max()) < tol, f"min cosine {float(c.min())}"
     if unit_norm:
         assert torch.allclose(got.norm(dim=-1), torch.ones(got.shape[0], dtype=got.dtype), atol=1e-5)
+
+
+@pytest.fixture(autouse=True)
+def fp32_oracle():
+    """TF32 off for torch's matmuls and cuDNN convolutions while a test runs, so that a GPU oracle computes in fp32."""
+    old = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+    yield
+    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+
+
+def _assert_rows_match(got, ref, unit_norm):
+    """assert_embeddings_match, and every row's norm within 1 % of ref's, so that normalised and unnormalised rows
+    cannot stand in for each other."""
+    assert_embeddings_match(got, ref, unit_norm=unit_norm)
+    torch.testing.assert_close(_cpu(got).double().norm(dim=-1), _cpu(ref).double().norm(dim=-1), rtol=1e-2, atol=0)
+
+
+def check_image_input_paths(enc, at_size, photo, preprocess, ref, rows=None, resize=None):
+    """Encoder enc's image tower on every input path against ref(chw, normalize), the oracle on preprocess(u8), fp32
+    [n, 3, S, S]:
+
+      - uint8 images at the model's size, the given rows of them (all by default) against ref;
+      - the same images from device memory: the same bits;
+      - photo (uint8 of another size) through the model's resize; with resize (that resize kernel alone), also the bits
+        of photo resized by it first;
+      - photo's first three rows preprocessed to fp32;
+      - unnormalised rows from the uint8 and the fp32 path.
+
+    Returns the embeddings of at_size."""
+    n, S = len(at_size), enc.image_size
+    rows = list(range(n)) if rows is None else rows
+    got = enc.encode_images_u8(at_size)
+    assert got.shape == (n, enc.embed_dim)
+    _assert_rows_match(got[rows], ref(preprocess(at_size[rows]), normalize=True), True)
+    d_in = torch.from_numpy(at_size).cuda()
+    out = torch.empty((n, enc.embed_dim), dtype=torch.float32, device="cuda")
+    torch.cuda.synchronize()
+    enc.encode_images_u8_device(d_in.data_ptr(), n, S, S, out.data_ptr(), sync=True)
+    np.testing.assert_array_equal(out.cpu().numpy(), got)
+    resized = enc.encode_images_u8(photo)
+    _assert_rows_match(resized, ref(preprocess(photo), normalize=True), True)
+    if resize is not None:
+        np.testing.assert_array_equal(resized, enc.encode_images_u8(resize(photo, S)))
+    chw = preprocess(photo[:3])
+    _assert_rows_match(enc.encode_images_f32(chw.numpy()), ref(chw, normalize=True), True)
+    raw = enc.encode_images_u8(at_size[:2], normalize=False)
+    _assert_rows_match(raw, ref(preprocess(at_size[:2]), normalize=False), False)
+    _assert_rows_match(enc.encode_images_f32(chw.numpy(), normalize=False), ref(chw, normalize=False), False)
+    return got
+
+
+def clip_text_ids(n, seed):
+    """n CLIP token rows of 77: start 49406, 1 to 68 random ids, end 49407, zero padding."""
+    ids = torch.zeros(n, 77, dtype=torch.int64)
+    g = torch.Generator().manual_seed(seed)
+    for i in range(n):
+        L = int(torch.randint(2, 70, (1,), generator=g))
+        ids[i, 0] = 49406
+        ids[i, 1:L] = torch.randint(1, 49000, (L - 1,), generator=g)
+        ids[i, L] = 49407
+    return ids
+
+
+def assert_refused(kind, arch, weights, code, in_message=None):
+    """Encoder(kind, arch, weights) is refused with NativeError code, whose message names in_message if given."""
+    from marqo_b200._native import NativeError
+    from marqo_b200.engine import Encoder
+    with pytest.raises(NativeError) as e:
+        Encoder(kind, arch, weights, max_batch=2)
+    assert e.value.code == code, e.value
+    assert in_message is None or in_message in e.value.message, e.value
 
 
 def assert_topk_equal(got, expected, atol=1e-12):

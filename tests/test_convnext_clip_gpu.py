@@ -1,25 +1,21 @@
 """ConvNeXt CLIP on the GPU: its three per-pixel kernels through their debug hooks against torch fp64, the towers
 through the C ABI against the fp32 oracle (cosine >= 1 - 1e-3, unit norm) at every distinct trunk shape and on every
-input path, the CLIP text tower at widths 640 and 1024, the launch count, device memory after destroy, and
-vectorise -> GpuTensorIndex against the score oracle.  The oracle runs on the GPU in fp32 with TF32 off."""
+input path, the CLIP text tower at widths 640 and 1024, the shapes refused at create time, the GEMM at every layer
+shape, and vectorise -> GpuTensorIndex against the score oracle.  The oracle runs on the GPU in fp32 with TF32 off.
+The launch count is in tests/test_model_launches_gpu.py and device memory after close in
+tests/test_device_memory_gpu.py."""
 import numpy as np
 import pytest
 import torch
 
 import _convnext_oracle as O
-from _checks import assert_embeddings_match, assert_index_search_matches
+from _checks import (assert_embeddings_match, assert_index_search_matches, assert_refused, check_image_input_paths,
+                     clip_text_ids, fp32_oracle)  # noqa: F401 (fp32_oracle: autouse)
+from marqo_b200._native import ERR_INVALID_ARG
 
 pytestmark = pytest.mark.gpu
 BASE_W, LARGE_D = "open_clip/convnext_base_w/laion2b_s13b_b82k", "open_clip/convnext_large_d/laion2b_s26b_b102k_augreg"
 DIMS = {"base": [128, 256, 512, 1024], "large": [192, 384, 768, 1536], "xxlarge": [384, 768, 1536, 3072]}
-
-
-@pytest.fixture(autouse=True)
-def _fp32_oracle():
-    old = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
-    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
 
 
 def _ln64(y, g, b, eps):
@@ -175,20 +171,10 @@ def test_base_w_every_input_path(gpu_required, base_w):
     arch, sd, enc = base_w
     rng = np.random.default_rng(1)
     at_size = rng.integers(0, 256, (40, 256, 256, 3), dtype=np.uint8)
-    got = enc.encode_images_u8(at_size)
-    rows = [0, 17, 39]
-    assert_embeddings_match(got[rows], _ref_images(sd, arch, at_size[rows]))
-    # device-resident uint8: the same bits
-    d_in = torch.from_numpy(at_size).cuda()
-    out = torch.empty((40, 640), dtype=torch.float32, device="cuda")
-    enc.encode_images_u8_device(d_in.data_ptr(), 40, 256, 256, out.data_ptr(), sync=True)
-    np.testing.assert_array_equal(out.cpu().numpy(), got)
-    # non-square images through the resize + centre crop
-    other = rng.integers(0, 256, (3, 300, 171, 3), dtype=np.uint8)
-    assert_embeddings_match(enc.encode_images_u8(other), _ref_images(sd, arch, other))
-    # preprocessed fp32 CHW
-    chw = E.clip_preprocess_u8(other, 256)
-    assert_embeddings_match(enc.encode_images_f32(chw.numpy()), O.encode_image(sd, arch, chw.cuda()).cpu())
+    other = rng.integers(0, 256, (3, 300, 171, 3), dtype=np.uint8)   # through the resize + centre crop
+    check_image_input_paths(enc, at_size, other, lambda u8: E.clip_preprocess_u8(u8, 256),
+                            lambda chw, normalize: O.encode_image(sd, arch, chw.cuda(), normalize=normalize).cpu(),
+                            rows=[0, 17, 39])
 
 
 def test_base_w_single_image_graph_replay(gpu_required, base_w):
@@ -200,24 +186,13 @@ def test_base_w_single_image_graph_replay(gpu_required, base_w):
     assert_embeddings_match(first, _ref_images(sd, arch, img))
 
 
-def _text_ids(n, seed):
-    ids = torch.zeros(n, 77, dtype=torch.int64)
-    g = torch.Generator().manual_seed(seed)
-    for i in range(n):
-        L = int(torch.randint(2, 70, (1,), generator=g))
-        ids[i, 0] = 49406
-        ids[i, 1:L] = torch.randint(1, 49000, (L - 1,), generator=g)
-        ids[i, L] = 49407
-    return ids
-
-
 def _text_check(arch, sd, enc, n):
     from oracle import encoders as E
     w, layers, heads = arch["width"], arch["layers"], arch["heads"]
     cfg = E.ClipCfg(embed_dim=arch["embed_dim"], vision=E.TowerCfg(64, 1, 1, 64),
                     text=E.TowerCfg(w, layers, heads, 4 * w, ctx=77, vocab=49408), act=arch["act"])
     tsd = {k: torch.as_tensor(v) for k, v in sd.items() if not k.startswith("visual.")}
-    ids = _text_ids(n, w)
+    ids = clip_text_ids(n, w)
     got = enc.encode_tokens(ids.numpy())
     rows = [0, n // 2, n - 1]
     assert_embeddings_match(got[rows], E.clip_encode_text(tsd, cfg, ids[rows]))
@@ -254,75 +229,17 @@ def test_full_depth_tower(gpu_required, name):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# Launches, memory, bad shapes
+# Refusals
 # ------------------------------------------------------------------------------------------------------------------
-# Run in a process of its own: a torch.profiler session leaves CUPTI in a state in which a later session of the same
-# process can miss the first kernels of a new model's stream, which would upset the other launch-count tests.
-_LAUNCHES_CHILD = """
-import json, sys
-import numpy as np, torch
-from torch.profiler import ProfilerActivity, profile
-from marqo_b200 import model_registry as R
-from marqo_b200.engine import Encoder
-from marqo_b200.weights import random_clip_convnext_weights
-arch = R.get_model_properties(sys.argv[1])["arch"]
-arch["layers"] = 0
-arch["convnext"]["depths"] = [1, 1, 2, 1]
-enc = Encoder("clip_convnext", arch, random_clip_convnext_weights(arch, seed=5), max_batch=4)
-img = np.random.default_rng(5).integers(0, 256, (4, 256, 256, 3), dtype=np.uint8)
-enc.encode_images_u8(img)   # warm-up
-with profile(activities=[ProfilerActivity.CUDA]) as prof:
-    enc.encode_images_u8(img)
-    torch.cuda.synchronize()
-ran = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
-       and not e.name.startswith(("Memcpy", "Memset"))]
-print(json.dumps({"reported": enc.last_timing()[1], "ran": ran}))
-enc.close()
-"""
-
-
-def test_reported_launches_equal_the_kernels_run(gpu_required):
-    import json
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([root, os.environ.get("PYTHONPATH", "")]))
-    r = subprocess.run([sys.executable, "-c", _LAUNCHES_CHILD, LARGE_D], cwd=root, env=env, capture_output=True,
-                       text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-2000:]
-    out = json.loads(r.stdout.strip().splitlines()[-1])
-    # stem GEMM + LN, 3 x (LN-patchify + GEMM), 5 blocks x 3, pool_ln, the MLP head's 2 GEMMs, l2
-    assert out["reported"] == 2 + 3 * 2 + 5 * 3 + 1 + 2 + 1
-    assert len(out["ran"]) == out["reported"], out["ran"]
-
-
-def test_device_bytes_return_after_destroy(gpu_required):
-    from marqo_b200 import _native as N
-    import ctypes as C
-    before = C.c_int64(0)
-    N.check(N.load().b200_debug_device_bytes(C.byref(before)))
-    sd, enc = _encoder(_arch(BASE_W, depths=[1, 1, 1, 1]), seed=9, max_batch=8)
-    enc.encode_images_u8(np.zeros((2, 256, 256, 3), np.uint8))
-    enc.close()
-    after = C.c_int64(0)
-    N.check(N.load().b200_debug_device_bytes(C.byref(after)))
-    assert after.value == before.value
-
-
 @pytest.mark.parametrize("field,value", [("dims", [96, 256, 512, 1024]), ("dims", [128, 256, 512, 4096]),
                                          ("image_size", 240), ("embed_dim", 500)])
 def test_bad_shapes_are_refused_at_create(gpu_required, field, value):
-    from marqo_b200 import _native as N
-    from marqo_b200.engine import Encoder
     arch = _arch(BASE_W, depths=[1, 1, 1, 1])
     if field == "embed_dim":
         arch["embed_dim"] = value
     else:
         arch["convnext"][field] = value
-    with pytest.raises(N.NativeError) as e:
-        Encoder("clip_convnext", arch, {}, max_batch=2)
-    assert e.value.code == N.ERR_INVALID_ARG
+    assert_refused("clip_convnext", arch, {}, ERR_INVALID_ARG)
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -1,7 +1,8 @@
 """Every device buffer the library allocates is released again.  Each scenario reads the library's own count of live
 device bytes (b200_debug_device_bytes) before and after, and the difference must come back to zero: index life cycles
 with every growth path, calls rejected after they allocated, the exchange buffer, an encoder (also one whose finalize
-fails), the JPEG decoder and the resize temporaries.  cudaMemGetInfo is not used: other processes share the card."""
+fails), one encoder of each of the EVA02, big-ViT, ConvNeXt and GTE kinds through its encode calls, the JPEG decoder
+and the resize temporaries.  cudaMemGetInfo is not used: other processes share the card."""
 import contextlib
 import ctypes as C
 import gc
@@ -9,7 +10,12 @@ import io
 
 import numpy as np
 import pytest
+import torch
 
+import _big_vit_oracle as B
+import _eva02_oracle as V
+import _gte_oracle as G
+from _checks import clip_text_ids
 from marqo_b200 import _native as N
 
 pytestmark = pytest.mark.gpu
@@ -42,7 +48,6 @@ def _raises(code, fn, *args, **kwargs):
 
 @pytest.mark.parametrize("metric", ["prenormalized-angular", "euclidean"])
 def test_index_life_cycle(gpu_required, tmp_path, metric):
-    import torch
     from marqo_b200.engine import RowStore
     rng = np.random.default_rng(0)
     with _released() as before:
@@ -167,6 +172,51 @@ def test_encoder_life_cycle(gpu_required):
         for _ in range(3):   # eager, captured into a CUDA graph, replayed
             out = enc.encode_tokens(ids)
         assert out.shape == (4, arch["width"]) and np.isfinite(out).all()
+        enc.close()
+
+
+def _convnext_arch():
+    from marqo_b200 import model_registry as R
+    a = R.get_model_properties("open_clip/convnext_base_w/laion2b_s13b_b82k")["arch"]
+    a["convnext"]["depths"], a["layers"] = [1, 1, 1, 1], 0
+    return a
+
+
+def _photos(enc):
+    enc.encode_images_u8(np.zeros((2, 300, 200, 3), np.uint8))
+
+
+def _clip_text(enc):
+    enc.encode_tokens(clip_text_ids(2, 1).numpy())
+
+
+def _gte_ragged(enc):
+    ids, mask = G.ragged_ids(torch.Generator().manual_seed(3), [200, 5], 200, G.STELLA.vocab)
+    enc.encode_tokens(ids.numpy(), mask.numpy())
+
+
+# kind, arch (one layer per tower), the encode calls; seeded weights, max_batch 8
+_TOWERS = {
+    "eva02": ("clip_eva", lambda: V.arch(V.L14, eva_layers=1, text_layers=1), (_photos, _clip_text)),
+    "big_vit": ("clip", lambda: B.arch(B.BIG_G, vision_layers=1, text_layers=1), (_photos, _clip_text)),
+    "convnext": ("clip_convnext", _convnext_arch,
+                 (lambda enc: enc.encode_images_u8(np.zeros((2, 256, 256, 3), np.uint8)),)),
+    "gte": ("gte", lambda: G.engine_config(G.GteCfg(layers=1)), (_gte_ragged,)),
+}
+
+
+@pytest.mark.parametrize("tower", list(_TOWERS))
+def test_tower_kind_life_cycle(gpu_required, tower):
+    from marqo_b200.engine import Encoder
+    from marqo_b200.weights import random_weights
+    kind, arch, calls = _TOWERS[tower]
+    arch = arch()
+    sd = random_weights(kind, arch, 9)
+    with _released() as before:
+        enc = Encoder(kind, arch, sd, max_batch=8)
+        assert _live_bytes() > before
+        for call in calls:
+            call(enc)
         enc.close()
 
 

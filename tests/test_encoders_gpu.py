@@ -122,14 +122,11 @@ def test_e5_base_cfg1(gpu_required):
 
 
 def test_missing_weight_is_an_error(gpu_required):
-    from marqo_b200.engine import Encoder
-    from marqo_b200._native import NativeError, ERR_MISSING_WEIGHT
+    from marqo_b200._native import ERR_MISSING_WEIGHT
     cfg = E.tiny_bert()
     sd = E.make_bert_weights(cfg, seed=1)
     del sd["encoder.layer.1.output.dense.bias"]
-    with pytest.raises(NativeError) as ei:
-        Encoder("bert", E.engine_config(cfg), sd)
-    assert ei.value.code == ERR_MISSING_WEIGHT
+    K.assert_refused("bert", E.engine_config(cfg), sd, ERR_MISSING_WEIGHT)
 
 
 # ------------------------------------------------------------------------------------------------------------------

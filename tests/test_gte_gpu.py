@@ -1,23 +1,18 @@
 """The Stella embedder (GTE encoder) on the GPU: the full 24 layers at b16 x 512 with ragged lengths against the fp32
 oracle (cosine >= 1 - 1e-3, unit norm), a single 16-token query through the eager, captured and replayed graph paths,
-the launch count, device memory after destroy, the refusals, and vectorise(stella) with the C++ WordPiece tokenizer ->
-GpuTensorIndex against the score oracle.  The oracle runs on the GPU in fp32 with TF32 off."""
+the refusals, and vectorise(stella) with the C++ WordPiece tokenizer ->
+GpuTensorIndex against the score oracle.  The oracle runs on the GPU in fp32 with TF32 off.  The launch count at
+2 layers is in tests/test_model_launches_gpu.py and device memory after close in tests/test_device_memory_gpu.py."""
 import numpy as np
 import pytest
 import torch
 
 import _gte_oracle as G
-from _checks import assert_embeddings_match, assert_index_search_matches, cosine
+from _checks import (assert_embeddings_match, assert_index_search_matches, assert_refused, cosine,
+                     fp32_oracle)  # noqa: F401 (fp32_oracle: autouse)
+from marqo_b200._native import ERR_INVALID_ARG, ERR_MISSING_WEIGHT, NativeError
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(autouse=True)
-def _fp32_oracle():
-    old = torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32 = old
 
 
 def _encoder(cfg, sd, max_batch):
@@ -80,99 +75,32 @@ def test_single_query_graph_path(gpu_required):
         enc.close()
 
 
-# Run in a process of its own: a torch.profiler session leaves CUPTI in a state in which a later session of the same
-# process can miss the first kernels of a new model's stream (tests/test_convnext_clip_gpu.py).
-_LAUNCHES_CHILD = """
-import json
-import numpy as np, torch
-from torch.profiler import ProfilerActivity, profile
-from marqo_b200 import model_registry as R
-from marqo_b200.engine import Encoder
-from marqo_b200.weights import random_gte_weights
-arch = dict(R.get_model_properties("Marqo/dunzhang-stella_en_400M_v5")["arch"], layers=2)
-enc = Encoder("gte", arch, random_gte_weights(arch, seed=5), max_batch=8)
-ids = np.random.default_rng(5).integers(103, 30000, (8, 300)).astype(np.int32)
-mask = np.ones_like(ids)
-mask[3, 100:] = 0
-enc.encode_tokens(ids, mask)   # warm-up
-with profile(activities=[ProfilerActivity.CUDA]) as prof:
-    enc.encode_tokens(ids, mask)
-    torch.cuda.synchronize()
-ran = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
-       and not e.name.startswith(("Memcpy", "Memset"))]
-print(json.dumps({"reported": enc.last_timing()[1], "ran": ran}))
-enc.close()
-"""
-
-
-def test_reported_launches_equal_the_kernels_run(gpu_required):
-    import json
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([root, os.environ.get("PYTHONPATH", "")]))
-    r = subprocess.run([sys.executable, "-c", _LAUNCHES_CHILD], cwd=root, env=env, capture_output=True, text=True,
-                       timeout=600)
-    assert r.returncode == 0, r.stderr[-2000:]
-    out = json.loads(r.stdout.strip().splitlines()[-1])
-    assert out["reported"] == 1 + 2 * 9 + 1
-    assert len(out["ran"]) == out["reported"], out["ran"]
-    for kernel in ("rope_qk_kernel", "geglu_kernel"):
-        assert sum(kernel in k for k in out["ran"]) == 2, kernel
-    assert sum("bert_embed_ln_kernel" in k for k in out["ran"]) == 1
-
-
-def test_device_bytes_return_after_destroy(gpu_required):
-    from marqo_b200 import _native as N
-    import ctypes as C
-    before = C.c_int64(0)
-    N.check(N.load().b200_debug_device_bytes(C.byref(before)))
-    cfg = G.GteCfg(layers=1)
-    enc = _encoder(cfg, G.make_gte_weights(cfg, seed=9), 8)
-    ids, mask = G.ragged_ids(torch.Generator().manual_seed(3), [200, 5], 200, cfg.vocab)
-    enc.encode_tokens(ids.numpy(), mask.numpy())
-    enc.close()
-    after = C.c_int64(0)
-    N.check(N.load().b200_debug_device_bytes(C.byref(after)))
-    assert after.value == before.value
-
-
 # ------------------------------------------------------------------------------------------------------------------
 # Refusals
 # ------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("case", ["head_dim_32", "width_1280", "ctx_1024", "no_eps", "no_theta", "ntk_below_1"])
 def test_bad_shapes_are_refused_at_create(gpu_required, case):
-    from marqo_b200 import _native as N
-    from marqo_b200.engine import Encoder
     a = G.engine_config(G.GteCfg(layers=1))
     a.update({"head_dim_32": dict(heads=32), "width_1280": dict(width=1280, heads=20), "ctx_1024": dict(ctx=1024),
               "no_eps": dict(ln_eps=0.0), "no_theta": dict(rope_theta=0.0), "ntk_below_1": dict(rope_ntk_factor=0.5)
               }[case])
-    with pytest.raises(N.NativeError) as e:
-        Encoder("gte", a, {}, max_batch=2)
-    assert e.value.code == N.ERR_INVALID_ARG
+    assert_refused("gte", a, {}, ERR_INVALID_ARG)
 
 
 def test_missing_weight_wrong_up_gate_and_long_sequence(gpu_required):
-    from marqo_b200 import _native as N
     cfg = G.tiny_gte()
-    sd = G.make_gte_weights(cfg, seed=6)
+    a, sd = G.engine_config(cfg), G.make_gte_weights(cfg, seed=6)
     missing = {k: v for k, v in sd.items() if k != "encoder.layer.1.mlp_ln.bias"}
-    with pytest.raises(N.NativeError) as e:
-        _encoder(cfg, missing, 2)
-    assert e.value.code == N.ERR_MISSING_WEIGHT and "mlp_ln.bias" in str(e.value)
+    assert_refused("gte", a, missing, ERR_MISSING_WEIGHT, "mlp_ln.bias")
     # an up_gate_proj of mlp rows (no gate half)
     wrong = dict(sd)
     wrong["encoder.layer.0.mlp.up_gate_proj.weight"] = sd["encoder.layer.0.mlp.up_gate_proj.weight"][:cfg.mlp]
-    with pytest.raises(N.NativeError) as e:
-        _encoder(cfg, wrong, 2)
-    assert e.value.code == N.ERR_INVALID_ARG
+    assert_refused("gte", a, wrong, ERR_INVALID_ARG)
     enc = _encoder(cfg, sd, 2)
     try:
-        with pytest.raises(N.NativeError) as e:
+        with pytest.raises(NativeError) as e:
             enc.encode_tokens(np.zeros((1, cfg.ctx + 1), np.int32))
-        assert e.value.code == N.ERR_INVALID_ARG
+        assert e.value.code == ERR_INVALID_ARG
     finally:
         enc.close()
 

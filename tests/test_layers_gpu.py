@@ -168,11 +168,6 @@ def test_served_layer_variants():
 
 
 # ---------------------------------------------------------------------------------------------------- the models
-_RANDOM = {"clip": Wt.random_clip_weights, "siglip": Wt.random_siglip_weights, "clip_eva": Wt.random_eva02_weights,
-           "bert": Wt.random_bert_weights, "xlmr": Wt.random_xlmr_weights, "mpnet": Wt.random_mpnet_weights,
-           "gte": Wt.random_gte_weights}
-
-
 @pytest.fixture(scope="module")
 def sm_count(gpu_required):
     return torch.cuda.get_device_properties(0).multi_processor_count
@@ -200,7 +195,7 @@ def layer_model(request, sm_count):
     from marqo_b200.engine import Encoder
     c = VARIANTS[request.param]
     seed = zlib.crc32(c["id"].encode())
-    sd = _RANDOM[c["kind"]](c["arch"], seed)
+    sd = Wt.random_weights(c["kind"], c["arch"], seed)
     max_batch = max(max(b for b, _, _ in _shapes(c, sm_count)), 4)
     enc = Encoder(c["kind"], c["arch"], sd, max_batch=max_batch)
     from marqo_b200.engine import layer_cols
@@ -568,8 +563,8 @@ def test_debug_layers_refuses_bad_arguments(gpu_required):
     vit = VARIANTS["clip-vision-768-3072-gelu-50"]
     encs = []
     try:
-        eb = Encoder("bert", bert["arch"], _RANDOM["bert"](bert["arch"], 1), max_batch=2)
-        ev = Encoder("clip", vit["arch"], _RANDOM["clip"](vit["arch"], 2), max_batch=2)
+        eb = Encoder("bert", bert["arch"], Wt.random_weights("bert", bert["arch"], 1), max_batch=2)
+        ev = Encoder("clip", vit["arch"], Wt.random_weights("clip", vit["arch"], 2), max_batch=2)
         encs += [eb, ev]
         xb = torch.zeros(2 * 16, 384, device="cuda")
         xv = torch.zeros(50, 768, device="cuda")

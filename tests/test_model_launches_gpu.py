@@ -1,7 +1,13 @@
 """The launch count b200_model_last_timing reports, and the GEMM / attention launches b200_model_profile brackets, equal
 the kernels the device ran (torch.profiler's CUDA kernel events) for one small model of every tower kind, through
 every encode entry point, with and without L2 normalisation; and a replayed CUDA graph reports the count of the eager
-pass it was captured from."""
+pass it was captured from.  Served models at reduced depth report the count their layers add up to, with the
+variant-specific kernels (rotary, SwiGLU, GeGLU, wgmma attention) run as often as the layers call them."""
+import json
+import os
+import subprocess
+import sys
+
 import numpy as np
 import pytest
 import torch
@@ -134,3 +140,83 @@ def test_reported_launches_equal_the_kernels_run(gpu_required, make):
             assert prof["attention_launches"] == sum("attention" in b for b in base), f"{name}: {base}"
     finally:
         enc.close()
+
+
+# Run in a process of its own: a torch.profiler session leaves CUPTI in a state in which a later session of the same
+# process can miss the first kernels of a new model's stream.  argv[1]: [registry name, kind, arch edits, input].
+_LAUNCHES_CHILD = """
+import json, sys
+import numpy as np, torch
+from torch.profiler import ProfilerActivity, profile
+from marqo_b200 import model_registry as R
+from marqo_b200.engine import Encoder
+from marqo_b200.weights import random_weights
+name, kind, edits, (inp, shape) = json.loads(sys.argv[1])
+arch = R.get_model_properties(name)["arch"]
+for path, value in edits.items():
+    *outer, key = path.split(".")
+    d = arch
+    for k in outer:
+        d = d[k]
+    d[key] = value
+enc = Encoder(kind, arch, random_weights(kind, arch, 5), max_batch=shape[0])
+rng = np.random.default_rng(5)
+if inp == "u8":
+    img = rng.integers(0, 256, tuple(shape) + (3,), dtype=np.uint8)
+    run = lambda: enc.encode_images_u8(img)
+else:   # token ids, row 3 masked after 100 tokens
+    ids = rng.integers(103, 30000, tuple(shape)).astype(np.int32)
+    mask = np.ones_like(ids)
+    mask[3, 100:] = 0
+    run = lambda: enc.encode_tokens(ids, mask)
+run()   # warm-up
+with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    run()
+    torch.cuda.synchronize()
+ran = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+       and not e.name.startswith(("Memcpy", "Memset"))]
+print(json.dumps({"reported": enc.last_timing()[1], "ran": ran}))
+enc.close()
+"""
+
+_PHOTOS = ("u8", [4, 480, 640])
+_EVA02 = {"rope_qk_kernel": 2, "swiglu_ln_kernel": 2, "attention_wgmma_kernel": 2}
+# (registry name, kind, arch edits, input, reported launches, launches of named kernels)
+_SERVED = {
+    # the resize's two passes, embed rows, patch GEMM, 2 layers x (LN, QKV, rope, attention, attn.norm, out-proj, LN,
+    # fc1, swiglu_ln, fc2), the head's LN, GEMM and L2
+    "EVA02-B-16": ("open_clip/EVA02-B-16/merged2b_s8b_b131k", "clip_eva", {"layers": 0, "eva.layers": 2}, _PHOTOS,
+                   2 + 2 + 2 * 10 + 3, _EVA02),
+    "EVA02-L-14-336": ("open_clip/EVA02-L-14-336/merged2b_s6b_b61k", "clip_eva", {"layers": 0, "eva.layers": 2},
+                       _PHOTOS, 2 + 2 + 2 * 10 + 3, _EVA02),
+    # the resize's two passes, embed rows, patch GEMM, ln_pre, 2 layers x (LN, QKV, attention, out-proj, LN, fc1,
+    # fc2), the head's 3
+    "ViT-H-14-378": ("open_clip/ViT-H-14-378-quickgelu/dfn5b", "clip", {"text": None, "vision.layers": 2}, _PHOTOS,
+                     2 + 3 + 2 * 7 + 3, {"attention_wgmma_kernel": 2}),
+    "ViT-bigG-14": ("open_clip/ViT-bigG-14/laion2b_s39b_b160k", "clip", {"text": None, "vision.layers": 2}, _PHOTOS,
+                    2 + 3 + 2 * 7 + 3, {"attention_wgmma_kernel": 2}),
+    # stem GEMM + LN, 3 x (LN-patchify + GEMM), 5 blocks x 3, pool_ln, the MLP head's 2 GEMMs, l2
+    "convnext_large_d": ("open_clip/convnext_large_d/laion2b_s26b_b102k_augreg", "clip_convnext",
+                         {"layers": 0, "convnext.depths": [1, 1, 2, 1]}, ("u8", [4, 256, 256]),
+                         2 + 3 * 2 + 5 * 3 + 1 + 2 + 1, {}),
+    # embed, 2 layers x (QKV, rope, attention, o_proj, attn_ln, up_gate, geglu, down, mlp_ln), the head
+    "Stella": ("Marqo/dunzhang-stella_en_400M_v5", "gte", {"layers": 2}, ("ids", [8, 300]), 1 + 2 * 9 + 1,
+               {"rope_qk_kernel": 2, "geglu_kernel": 2, "bert_embed_ln_kernel": 1}),
+}
+
+
+@pytest.mark.parametrize("row", list(_SERVED))
+def test_served_model_launches(gpu_required, row):
+    """4 images (ConvNeXt at its own size, the others 480 x 640 through the resize) or 8 x 300 ids with one row
+    masked, after a warm-up call."""
+    name, kind, edits, inp, reported, kernels = _SERVED[row]
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    env = dict(os.environ, PYTHONPATH=os.pathsep.join([root, os.environ.get("PYTHONPATH", "")]))
+    r = subprocess.run([sys.executable, "-c", _LAUNCHES_CHILD, json.dumps([name, kind, edits, inp])], cwd=root,
+                       env=env, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0, r.stderr[-2000:]
+    out = json.loads(r.stdout.strip().splitlines()[-1])
+    assert out["reported"] == reported
+    assert len(out["ran"]) == out["reported"], out["ran"]
+    for kernel, n in kernels.items():
+        assert sum(kernel in k for k in out["ran"]) == n, kernel

@@ -119,14 +119,11 @@ def test_mpnet_base_single_query_graph_replay(gpu_required, base_weights):
 
 
 def test_missing_relative_attention_bias(gpu_required):
-    from marqo_b200._native import ERR_MISSING_WEIGHT, NativeError
-    from marqo_b200.engine import Encoder
+    from marqo_b200._native import ERR_MISSING_WEIGHT
     cfg = M.tiny_mpnet()
     sd = M.make_mpnet_weights(cfg, seed=3)
     del sd["encoder.relative_attention_bias.weight"]
-    with pytest.raises(NativeError) as ei:
-        Encoder("mpnet", M.engine_config(cfg), sd, max_batch=2)
-    assert ei.value.code == ERR_MISSING_WEIGHT
+    K.assert_refused("mpnet", M.engine_config(cfg), sd, ERR_MISSING_WEIGHT)
 
 
 def test_golden_vectors_through_the_c_abi(gpu_required):

@@ -1,6 +1,7 @@
 """OpenAI ResNet CLIP on the GPU: every distinct convolution of RN50 and RN101 through debug_conv2d (the model's own
 path) against torch fp64 on the bf16-rounded operands, the attention pool's per-image queries, and the RN50 / RN101
-towers through the C ABI against the fp32 oracle (cosine >= 1 - 1e-3, unit norm) on every input path, plus
+towers through the C ABI against the fp32 oracle (cosine >= 1 - 1e-3, unit norm) on every input path (the device
+uint8 batch also one byte past a 16-byte boundary), plus
 vectorise("open_clip/RN50/openai") -> GpuTensorIndex against the score oracle.
 
 The full-size oracle runs on the GPU in fp32 with TF32 off, on a few rows of each batch (rows are independent)."""
@@ -10,17 +11,11 @@ import torch
 
 import _checks as K
 import _resnet_oracle as O
+from _checks import fp32_oracle  # noqa: F401 (autouse)
+from oracle import encoders as E
 
 pytestmark = pytest.mark.gpu
 RN50, RN101 = "open_clip/RN50/openai", "open_clip/RN101/openai"
-
-
-@pytest.fixture(autouse=True)
-def _fp32_oracle():
-    old = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
-    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -130,7 +125,6 @@ def rn50():
 
 
 def _ref_images(sd, arch, u8):
-    from oracle import encoders as E
     return O.encode_image(sd, arch, E.clip_preprocess_u8(u8).cuda()).cpu()
 
 
@@ -141,8 +135,10 @@ def test_rn50_batch_256_every_input_path(gpu_required, rn50):
     arch, sd, enc = rn50
     rng = np.random.default_rng(1)
     at_size = rng.integers(0, 256, (256, 224, 224, 3), dtype=np.uint8)
-    got = enc.encode_images_u8(at_size)
-    K.assert_embeddings_match(got[ROWS], _ref_images(sd, arch, at_size[ROWS]))
+    other = rng.integers(0, 256, (6, 300, 171, 3), dtype=np.uint8)   # through the resize + centre crop
+    got = K.check_image_input_paths(enc, at_size, other, E.clip_preprocess_u8,
+                                    lambda chw, normalize: O.encode_image(sd, arch, chw.cuda(), normalize).cpu(),
+                                    rows=ROWS)
     # device-resident, aligned and starting 1 byte past a 16-byte boundary: the same bits
     n_bytes = at_size.nbytes
     raw = torch.empty(n_bytes + 32, dtype=torch.uint8, device="cuda")
@@ -154,13 +150,6 @@ def test_rn50_batch_256_every_input_path(gpu_required, rn50):
         torch.cuda.synchronize()
         enc.encode_images_u8_device(base + off, 256, 224, 224, out.data_ptr(), sync=True)
         np.testing.assert_array_equal(out.cpu().numpy(), got)
-    # non-square images through the resize + centre crop
-    other = rng.integers(0, 256, (6, 300, 171, 3), dtype=np.uint8)
-    K.assert_embeddings_match(enc.encode_images_u8(other), _ref_images(sd, arch, other))
-    # preprocessed fp32 CHW
-    from oracle import encoders as E
-    chw = E.clip_preprocess_u8(other[:3])
-    K.assert_embeddings_match(enc.encode_images_f32(chw.numpy()), O.encode_image(sd, arch, chw.cuda()).cpu())
 
 
 def test_rn50_single_image_graph_replay(gpu_required, rn50):
@@ -174,15 +163,8 @@ def test_rn50_single_image_graph_replay(gpu_required, rn50):
 
 @pytest.mark.parametrize("n", [256, 1])
 def test_rn50_text(gpu_required, rn50, n):
-    from oracle import encoders as E
     arch, sd, enc = rn50
-    ids = torch.zeros(n, 77, dtype=torch.int64)
-    g = torch.Generator().manual_seed(n)
-    for i in range(n):
-        L = int(torch.randint(2, 70, (1,), generator=g))
-        ids[i, 0] = 49406
-        ids[i, 1:L] = torch.randint(1, 49000, (L - 1,), generator=g)
-        ids[i, L] = 49407
+    ids = K.clip_text_ids(n, n)
     cfg = E.ClipCfg(embed_dim=1024, vision=E.TowerCfg(64, 1, 1, 64),
                     text=E.TowerCfg(512, 12, 8, 2048, ctx=77, vocab=49408), act=arch["act"])
     tsd = {k: torch.as_tensor(v) for k, v in sd.items() if not k.startswith("visual.")}

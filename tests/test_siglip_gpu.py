@@ -1,6 +1,7 @@
 """SigLIP on the GPU: the MAP pooling kernel vs torch, the squash resize vs Pillow bit for bit, the SigLIP towers
-through the C ABI vs the CPU fp32 oracle (cosine >= 1 - 1e-3, unit norm) on every input path, the refusal of head_dim
-72 (SO400M), and vectorise("Marqo/marqo-fashionSigLIP") -> GpuTensorIndex vs the score oracle.
+through the C ABI vs the CPU fp32 oracle (cosine >= 1 - 1e-3, unit norm) on every input path, the refusals of head_dim
+72 (SO400M) and of a missing MAP head weight, and vectorise("Marqo/marqo-fashionSigLIP") -> GpuTensorIndex vs the score
+oracle.
 
 The oracle is run on a few rows of each batch (rows are independent), so the engine still runs the full batch."""
 import numpy as np
@@ -9,6 +10,7 @@ import torch
 
 import _checks as K
 import _siglip_oracle as O
+from marqo_b200._native import ERR_INVALID_ARG, ERR_MISSING_WEIGHT
 
 pytestmark = pytest.mark.gpu
 
@@ -71,29 +73,15 @@ ROWS = [0, 101, 255]
 
 
 def test_b16_224_batch_256_every_input_path(gpu_required, b16):
+    """Every input path (_checks.check_image_input_paths): unnormalised output is the pooled vector itself, its norm
+    within 1 % of the oracle's."""
     cfg, sd, enc = b16
     rng = np.random.default_rng(1)
     at_size = rng.integers(0, 256, (256, 224, 224, 3), dtype=np.uint8)
-    got = enc.encode_images_u8(at_size)
-    K.assert_embeddings_match(got[ROWS], O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(at_size[ROWS], 224)))
-    # the same batch from a device-resident tensor gives the same bits
-    dev = torch.from_numpy(at_size).cuda()
-    out = torch.empty((256, 768), dtype=torch.float32, device="cuda")
-    torch.cuda.synchronize()
-    enc.encode_images_u8_device(dev.data_ptr(), 256, 224, 224, out.data_ptr(), sync=True)
-    np.testing.assert_array_equal(out.cpu().numpy(), got)
-    # squash resize of another size on the way in
-    other = rng.integers(0, 256, (8, 300, 171, 3), dtype=np.uint8)
-    K.assert_embeddings_match(enc.encode_images_u8(other),
-                              O.siglip_encode_image(sd, cfg, O.siglip_preprocess_u8(other, 224)))
-    # preprocessed fp32 CHW
-    chw = O.siglip_preprocess_u8(other[:3], 224)
-    K.assert_embeddings_match(enc.encode_images_f32(chw.numpy()), O.siglip_encode_image(sd, cfg, chw))
-    # unnormalised output is the pooled vector itself
-    raw = enc.encode_images_f32(chw.numpy(), normalize=False)
-    ref = O.siglip_encode_image(sd, cfg, chw, normalize=False)
-    K.assert_embeddings_match(raw, ref, unit_norm=False)
-    torch.testing.assert_close(torch.from_numpy(raw).norm(dim=-1), ref.norm(dim=-1), rtol=1e-2, atol=0)
+    other = rng.integers(0, 256, (8, 300, 171, 3), dtype=np.uint8)   # squash resize of another size on the way in
+    K.check_image_input_paths(enc, at_size, other, lambda u8: O.siglip_preprocess_u8(u8, 224),
+                              lambda chw, normalize: O.siglip_encode_image(sd, cfg, chw, normalize=normalize),
+                              rows=ROWS)
 
 
 def test_b16_single_image_graph_replay(gpu_required, b16):
@@ -151,23 +139,16 @@ def test_l16_256(gpu_required):
 @pytest.mark.parametrize("tower", ["vision", "text"])
 def test_head_dim_72_refused(gpu_required, tower):
     """ViT-SO400M-14-SigLIP-384: width 1152, 16 heads (head_dim 72) is refused when the model is built."""
-    from marqo_b200._native import ERR_INVALID_ARG, NativeError
-    from marqo_b200.engine import Encoder
     arch = O.SiglipCfg(width=1152, heads=16, mlp=4304, image_size=384).arch()
     arch["vision" if tower == "text" else "text"] = None
-    with pytest.raises(NativeError) as ei:
-        Encoder("siglip", arch, {})
-    assert ei.value.code == ERR_INVALID_ARG
+    K.assert_refused("siglip", arch, {}, ERR_INVALID_ARG)
 
 
 def test_missing_map_head_weight_is_reported(gpu_required):
-    from marqo_b200._native import ERR_MISSING_WEIGHT, NativeError
     cfg = O.tiny_siglip(64)
     sd = O.make_siglip_weights(cfg)
     del sd["visual.trunk.attn_pool.kv.bias"]
-    with pytest.raises(NativeError) as ei:
-        _encoder(cfg, sd)
-    assert ei.value.code == ERR_MISSING_WEIGHT and "visual.trunk.attn_pool.kv.bias" in ei.value.message
+    K.assert_refused("siglip", cfg.arch(), sd, ERR_MISSING_WEIGHT, "visual.trunk.attn_pool.kv.bias")
 
 
 # ------------------------------------------------------------------------------------------------------------------

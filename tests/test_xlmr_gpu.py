@@ -94,7 +94,7 @@ def test_xlmr_small_runs_the_bert_runtime(gpu_required):
 
 
 def test_roberta_prefix_and_missing_type_row(gpu_required):
-    from marqo_b200._native import ERR_MISSING_WEIGHT, NativeError
+    from marqo_b200._native import ERR_MISSING_WEIGHT
     cfg = X.tiny_xlmr()
     sd = X.make_xlmr_weights(cfg, seed=15)
     enc = _encoder(cfg, {"roberta." + k: v for k, v in sd.items()}, 4)
@@ -104,9 +104,7 @@ def test_roberta_prefix_and_missing_type_row(gpu_required):
     K.assert_embeddings_match(enc.encode_tokens(ids.numpy(), mask.numpy()), X.xlmr_encode(sd, cfg, ids, mask))
     enc.close()
     del sd["embeddings.token_type_embeddings.weight"]
-    with pytest.raises(NativeError) as ei:
-        _encoder(cfg, sd, 2)
-    assert ei.value.code == ERR_MISSING_WEIGHT
+    K.assert_refused("xlmr", X.engine_config(cfg), sd, ERR_MISSING_WEIGHT)
 
 
 # ------------------------------------------------------------------------------------------------------------------
