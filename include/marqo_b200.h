@@ -543,14 +543,20 @@ int b200_debug_index_last_scan(b200_index* ix, int* nq, int* grid, float* eps, f
  * with the epilogue given by act, out_bf16, has_bias and residual_in_place (residual == out, fp32 only). */
 int b200_debug_gemm_time(int device, int M, int N, int K, int act, int out_bf16, int has_bias, int residual_in_place,
                          int iters, float* out_ms);
-/* ViT patch embedding of uint8 HWC images [n,S,S,3], the token rows the image forward feeds to ln_pre: out fp32
- * [n*(G+1), N], row b*(G+1) = cls + pos[0], row b*(G+1)+1+i = conv1(patch i of image b) + pos[1+i], where the patch is
- * ToTensor + Normalize (mean3/std3, host fp32 [3])-ed and conv1 is conv_w fp32 [N, 3*patch*patch] without bias.
- * cls fp32 [N], pos fp32 [G+1, N].  The fused gather GEMM: no patch matrix in HBM,
- * src/marqo/tensor_search/add_docs.py:129-134 folded into the operand load. */
+/* The patch embedding of uint8 HWC images [n,S,S,3] (G = (S/patch)^2 patches each) by the fused gather GEMM: each
+ * patch is ToTensor + Normalize (mean3/std3, host fp32 [3])-ed inside the operand load, no patch matrix in HBM
+ * (src/marqo/tensor_search/add_docs.py:129-134), and conv1 is conv_w fp32 [N, 3*patch*patch] without bias.  The
+ * three forms the image forwards run:
+ *   pos != NULL, the ViT form (CLIP, EVA02, the big ViTs, SigLIP): the token rows fed to ln_pre, T = G + (cls != NULL)
+ *     per image, out fp32 [n*T, N] (ldo == N): with a class row (cls fp32 [N]) row b*T = cls + pos[0] and row
+ *     b*T+1+i = conv1(patch i of image b) + pos[1+i]; without one (SigLIP) row b*T+i = conv1(patch i) + pos[i].
+ *     pos fp32 [T, N]; bias must be NULL.
+ *   pos == NULL, the ConvNeXt stem form: row b*G+i of out fp32 [n*G, ldo] (ldo >= N, a multiple of 8) =
+ *     conv1(patch i of image b) + bias (fp32 [N], NULL: none); cls must be NULL.
+ * Nothing of out outside those n*T or n*G rows and their first N columns is written. */
 int b200_debug_patch_embed(int device, const uint8_t* hwc, int n, int S, int patch, const float* conv_w, int N,
-                           const float* mean3, const float* std3, const float* cls, const float* pos, float* out,
-                           void* stream);
+                           const float* mean3, const float* std3, const float* cls, const float* pos,
+                           const float* bias, float* out, int ldo, void* stream);
 /* softmax(q k^T / sqrt(head_dim) + mask + bias) v over packed qkv bf16 [B*S, 3*W], head_dim = W / H (32 or 64);
  * mask: 0 none, 1 causal, 2 key length (kv_len int32 [B]).  rel_bias (NULL: none) is MPNet's relative-position bias,
  * a host array fp32 [H, 2*smax - 1] (natural-log domain, as it enters softmax): rel_bias[h, j - i + smax - 1] is added

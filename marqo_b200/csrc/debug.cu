@@ -55,30 +55,41 @@ void require_device(int device) {
 extern "C" {
 
 int b200_debug_patch_embed(int device, const uint8_t* hwc, int n, int S, int patch, const float* conv_w, int N,
-                           const float* mean3, const float* std3, const float* cls, const float* pos, float* out,
-                           void* stream) {
+                           const float* mean3, const float* std3, const float* cls, const float* pos,
+                           const float* bias, float* out, int ldo, void* stream) {
     return guarded([&] {
-        MB_CHECK_ARG(hwc && conv_w && mean3 && std3 && cls && pos && out, "NULL buffer");
+        MB_CHECK_ARG(hwc && conv_w && mean3 && std3 && out, "NULL buffer");
         MB_CHECK_ARG(n > 0 && S > 0 && patch > 0 && S % patch == 0 && N > 0 && N % 32 == 0, "bad shape");
+        const bool vit = pos != nullptr;
+        if (vit)
+            MB_CHECK_ARG(bias == nullptr && ldo == N, "the ViT form has no bias and compact rows (ldo %d, N %d)", ldo, N);
+        else
+            MB_CHECK_ARG(cls == nullptr && ldo >= N && ldo % 8 == 0,
+                         "the stem form has no class row, and ldo %d must be a multiple of 8, >= N %d", ldo, N);
         require_device(device);
         DeviceGuard g(device);
         const cudaStream_t s = static_cast<cudaStream_t>(stream);
         const int G = (S / patch) * (S / patch);
         DeviceBuffer<bf16> wg((size_t)N * gemm::patch_gather_k(patch));
         kernels::patch_weight_rows(conv_w, N, patch, gemm::patch_gather_kbpd(patch), wg.get(), s);
-        // as the ViT forward does: x = pos (+ cls), then the gather GEMM adds conv1 onto it in place
-        kernels::vit_embed_rows(out, cls, pos, n, G + 1, N, s);
         gemm::Epilogue ep;
-        ep.residual = out;
-        ep.ldr = N;
         ep.out = out;
-        ep.ldo = N;
+        ep.ldo = ldo;
         ep.out_fp32 = 1;
+        if (vit) {
+            // as forward_vit does: x = pos (+ cls), then the gather GEMM adds conv1 onto it in place
+            kernels::vit_embed_rows(out, cls, pos, n, G + (cls != nullptr), N, s);
+            ep.residual = out;
+            ep.ldr = N;
+        } else {
+            ep.bias = bias;   // as forward_convnext's stem: conv + bias, no residual
+        }
         gemm::PatchGather pg;
         pg.img = hwc;
         pg.n = n;
         pg.S = S;
         pg.patch = patch;
+        pg.cls = cls != nullptr;
         for (int i = 0; i < 3; ++i) {
             pg.mean[i] = mean3[i];
             pg.std[i] = std3[i];

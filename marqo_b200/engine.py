@@ -700,22 +700,35 @@ def debug_gemm_ln(A, W, bias, residual, gamma, beta, eps: float, in_place: bool 
     return _host(x), _host(ln)
 
 
-def debug_patch_embed(images_u8, patch: int, conv_w, mean, std, pos=None, cls=None, device: int = 0) -> np.ndarray:
-    """ViT patch embedding of uint8 HWC images [n, S, S, 3] -> the token rows fp32 [n * (G + 1), N] the image forward
-    feeds to ln_pre: cls + pos[0] for the class rows, conv1(patch) + pos[1:] for the others (cls / pos None: zeros)."""
+def debug_patch_embed(images_u8, patch: int, conv_w, mean, std, io, pos=None, cls=None, bias=None,
+                      device: int = 0) -> np.ndarray:
+    """The patch embedding of uint8 HWC images [n, S, S, 3] (G patches each) by the fused gather GEMM, into a copy of io
+    (fp32 [rows >= M, cols >= N], N = len(conv_w)), in one of the forms the image forwards run
+    (b200_debug_patch_embed):
+
+      - pos given (fp32 [T, N]), the ViT form: rows [0, M = n T) become the token rows fed to ln_pre, T = G + 1 with a
+        class row (cls fp32 [N]: cls + pos[0], then conv1(patch i) + pos[1 + i]), T = G without one (SigLIP:
+        conv1(patch i) + pos[i]); io must have exactly N columns;
+      - pos None, the ConvNeXt stem form: rows [0, M = n G) x columns [0, N) become conv1(patch i) + bias (None: no
+        bias); cls must be None.
+
+    Returns the whole buffer, the rest of it as the kernels left it."""
     img = _as(images_u8, np.uint8)
     n, S = img.shape[0], img.shape[1]
-    w = _as(conv_w, np.float32).reshape(conv_w.shape[0], -1)
+    w = _as(conv_w, np.float32).reshape(len(conv_w), -1)
     Nn = w.shape[0]
-    G = (S // patch) ** 2
+    T = (S // patch) ** 2 + (cls is not None)
+    io = _as(io, np.float32)
+    if io.ndim != 2 or io.shape[0] < n * T or io.shape[1] < Nn:
+        raise ValueError(f"io {io.shape} does not hold the [{n * T}, {Nn}] token rows")
+    if pos is not None and np.shape(pos) != (T, Nn):
+        raise ValueError(f"pos {np.shape(pos)} is not [{T}, {Nn}]")
     m3, s3 = _as(mean, np.float32), _as(std, np.float32)
     d = _Staging(device)
-    di, dw = d.up(img, "uint8"), d.up(w)
-    dc = d.up(np.zeros(Nn) if cls is None else cls)
-    dp = d.up(np.zeros((G + 1, Nn)) if pos is None else pos)
-    out = d.empty((n * (G + 1), Nn))
+    di, dw, out = d.up(img, "uint8"), d.up(w), d.up(io)
+    dc, dp, db = d.up(cls), d.up(pos), d.up(bias)
     N.check(N.load().b200_debug_patch_embed(device, _dptr(di), n, S, patch, _dptr(dw), Nn, _ptr(m3), _ptr(s3),
-                                            _dptr(dc), _dptr(dp), _dptr(out), d.stream))
+                                            _dptr(dc), _dptr(dp), _dptr(db), _dptr(out), io.shape[1], d.stream))
     return _host(out)
 
 

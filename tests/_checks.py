@@ -144,6 +144,19 @@ def unit_rows(rng, n, d):
     return x
 
 
+def served_resize_sizes(mode):
+    """The image sizes S that the served image towers resize to in `mode`: "crop" (the shortest side to S, then the
+    centre S x S) or "squash" (both sides to S), as each entry's arch.get("resize_mode") says (crop by default)."""
+    from marqo_b200 import model_registry as R
+    sizes = set()
+    for e in R.served_models().values():
+        a = e["arch"]
+        tower = next((t for t in a.values() if isinstance(t, dict) and "image_size" in t), None)
+        if tower is not None and (a.get("resize_mode") or "crop") == mode:
+            sizes.add(tower["image_size"])
+    return sorted(sizes)
+
+
 def sample_positions(n, m):
     """Up to m positions spread over a batch of n, the first and the last among them, in ascending order."""
     return sorted(set([0, n - 1] + [int(x) for x in np.linspace(1, n - 2, m - 2)]))

@@ -349,7 +349,10 @@ def test_attnpool_tokens(gpu_required, n, HW, C):
 
 # ------------------------------------------------------------------------------------------------ im2col_f32
 @pytest.mark.parametrize("n,S,p,cls", [(3, 224, 14, 1), (1, 224, 16, 0), (5, 224, 32, 1), (2, 256, 16, 0),
-                                       (9, 224, 16, 1), (2, 224, 32, 0)])
+                                       (9, 224, 16, 1), (2, 224, 32, 0),
+                                       # the ConvNeXt stems (patch 4, kpad 64), the served sizes above 256
+                                       (2, 224, 4, 0), (2, 256, 4, 0), (1, 320, 4, 0), (1, 336, 14, 1), (1, 378, 14, 1),
+                                       (1, 384, 16, 0), (1, 512, 16, 0)])
 def test_im2col_f32(gpu_required, n, S, p, cls):
     """The ViT patch rows of fp32 CHW input, bit for bit the bf16 of the patch in k = c*p*p + dy*p + dx order (the
     order of conv1.weight.reshape(w, -1)); the class row (cls = 1) and the columns 3 p^2 .. kpad are zero."""

@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 import torch
 
-from _checks import bf16
+from _checks import bf16, served_resize_sizes
 
 pytestmark = pytest.mark.gpu
 
@@ -70,40 +70,6 @@ def test_gemm_fused_layernorm(gpu_required, M, N, K, in_place):
     x, ln = torch.from_numpy(x).double(), torch.from_numpy(ln).double()
     torch.testing.assert_close(ln, ln_ref, rtol=1e-2, atol=1e-2)            # bf16 output rounding
     torch.testing.assert_close(x, ln_ref if in_place else x_ref, rtol=3e-4, atol=3e-4)
-
-
-@pytest.mark.parametrize("n,S,patch,N", [
-    (3, 224, 14, 1024),    # ViT-L-14: 42-byte pixel rows, one 64-slot k-block each (zero padded past byte 42)
-    (5, 224, 32, 768),     # ViT-B-32: 96-byte pixel rows = 2 k-blocks, a 128-row tile straddles images (49 per image)
-    (2, 224, 16, 128),     # ViT-B-16 grid, one N tile
-    (300, 224, 32, 128),   # more tiles than SMs
-    (1, 112, 8, 256),      # small image: 336-byte rows
-])
-def test_patch_embed_token_rows_match_conv(gpu_required, n, S, patch, N):
-    """SURVEY §8 (a2): uint8 HWC -> ToTensor -> Normalize -> conv1 fused into the GEMM's operand load, added onto the
-    positional (+ class) embedding rows in place.  Reference: the torchvision formula (u8/255 - mean)/std in fp32,
-    rounded to bf16 like the kernel's A operand, conv2d in fp32."""
-    from marqo_b200.engine import debug_patch_embed
-    g = torch.Generator().manual_seed(n * 31 + patch)
-    img = torch.randint(0, 256, (n, S, S, 3), generator=g, dtype=torch.uint8)
-    K = 3 * patch * patch
-    w = bf16(torch.randn(N, 3, patch, patch, generator=g) / math.sqrt(K))
-    G = (S // patch) ** 2
-    pos = torch.randn(G + 1, N, generator=g)
-    cls = torch.randn(N, generator=g)
-    mean = torch.tensor([0.48145466, 0.4578275, 0.40821073])
-    std = torch.tensor([0.26862954, 0.26130258, 0.27577711])
-    x = (img.permute(0, 3, 1, 2).float() / 255.0 - mean[None, :, None, None]) / std[None, :, None, None]
-    ref = torch.nn.functional.conv2d(bf16(x).double(), w.double(), stride=patch)       # [n, N, g, g]
-    ref = ref.flatten(2).transpose(1, 2) + pos[None, 1:, :].double()                      # [n, G, N]
-    got = torch.from_numpy(debug_patch_embed(img.numpy(), patch, w.numpy(), mean.numpy(), std.numpy(), pos.numpy(),
-                                             cls=cls.numpy()))
-    got = got.view(n, G + 1, N)
-    assert torch.equal(got[:, 0], (cls + pos[0]).expand(n, N))       # class rows: a zero A row adds nothing
-    # the kernel normalises with one fma (u * 1/(255 std) - mean/std): a few values land on the other side of a bf16
-    # rounding boundary (2^-9 relative) -> compare at bf16-product accuracy
-    torch.testing.assert_close(got[:, 1:].double(), ref, rtol=0, atol=2e-2)
-    assert float((got[:, 1:].double() - ref).abs().mean()) < 1e-3
 
 
 @pytest.mark.parametrize("B,S,H,mask", [
@@ -229,22 +195,37 @@ def test_layernorm_matches_torch(gpu_required, rows, w, eps, variant):
         assert torch.equal(torch.from_numpy(got_b), bf16(got))
 
 
-@pytest.mark.parametrize("h,w", [(480, 640), (640, 480), (224, 224), (300, 224), (256, 256), (1000, 750), (225, 400), (100, 150)])
+# photo-like sizes, then the edges: sides of 1 and 2 pixels (every output from one or two source pixels; the other side
+# short, since the crop resizes it by as much), the shortest side S (identity passes) and S +- 1, 1:20, and a
+# 3024 x 4032 photo (a filter about 2 * ceil(2 * 4032 / 224) + 1 taps wide)
+@pytest.mark.parametrize("h,w", [(480, 640), (640, 480), (224, 224), (300, 224), (256, 256), (1000, 750), (225, 400), (100, 150),
+                                 (1, 1), (1, 3), (2, 5), (6, 2), ("S", "S"), ("S", 1000), ("S+1", 1000), (900, "S-1"),
+                                 (50, 1000), (1000, 50), (3024, 4032)])
 def test_resize_matches_pillow_bit_exact(gpu_required, h, w):
-    """Resize(224, BICUBIC) + CenterCrop(224) on PIL images (clip_utils.py:48-67) — Pillow is the third-party
-    implementation the reference runs; the CUDA kernel restates its fixed-point two-pass resampler bit for bit."""
+    """Resize(S, BICUBIC) + CenterCrop(S) on PIL images (clip_utils.py:48-67) at every S a served model crops to —
+    Pillow is the third-party implementation the reference runs; the CUDA kernel restates its fixed-point two-pass
+    resampler bit for bit."""
     from PIL import Image
     from torchvision.transforms import CenterCrop, InterpolationMode, Resize
     from marqo_b200.engine import debug_resize
-    rng = np.random.default_rng(h * 7 + w)
-    imgs = rng.integers(0, 256, size=(3, h, w, 3), dtype=np.uint8)
-    imgs[1] = (np.linspace(0, 255, w)[None, :, None] * np.ones((h, 1, 3))).astype(np.uint8)   # smooth gradient
-    tf = [Resize(224, interpolation=InterpolationMode.BICUBIC), CenterCrop(224)]
-    ref = []
-    for a in imgs:
-        im = Image.fromarray(a)
-        for t in tf:
-            im = t(im)
-        ref.append(np.asarray(im.convert("RGB")))
-    got = debug_resize(imgs, 224)
-    np.testing.assert_array_equal(got, np.stack(ref))
+    sizes = served_resize_sizes("crop")
+    assert sizes == [224, 256, 320, 336]
+    for S in sizes:
+        hs, ws = _side(h, S), _side(w, S)
+        rng = np.random.default_rng(hs * 7 + ws)
+        imgs = rng.integers(0, 256, size=(1 if hs * ws > 4_000_000 else 3, hs, ws, 3), dtype=np.uint8)
+        if len(imgs) > 1:
+            imgs[1] = (np.linspace(0, 255, ws)[None, :, None] * np.ones((hs, 1, 3))).astype(np.uint8)   # smooth gradient
+        tf = [Resize(S, interpolation=InterpolationMode.BICUBIC), CenterCrop(S)]
+        ref = []
+        for a in imgs:
+            im = Image.fromarray(a)
+            for t in tf:
+                im = t(im)
+            ref.append(np.asarray(im.convert("RGB")))
+        np.testing.assert_array_equal(debug_resize(imgs, S), np.stack(ref), err_msg=f"S = {S}, {hs} x {ws}")
+
+
+def _side(x, S):
+    """An image side of the resize cases: a number of pixels, or "S", "S+1", "S-1" relative to the target size."""
+    return x if isinstance(x, int) else S + {"S": 0, "S+1": 1, "S-1": -1}[x]

@@ -35,18 +35,35 @@ def test_map_attention_matches_torch(gpu_required, S, B):
     assert (got - ref).abs().mean() < 2e-3
 
 
-@pytest.mark.parametrize("h,w", [(480, 640), (640, 480), (224, 224), (300, 224), (256, 256), (1000, 750), (225, 400), (100, 150)])
+# photo-like sizes, then the edges: sides of 1 and 2 pixels (every output from one or two source pixels), a side of
+# exactly S (an identity pass) and S +- 1, 1:20, and a 3024 x 4032 photo (a filter about 2 * ceil(2 * 4032 / 224) + 1
+# taps wide)
+@pytest.mark.parametrize("h,w", [(480, 640), (640, 480), (224, 224), (300, 224), (256, 256), (1000, 750), (225, 400), (100, 150),
+                                 (1, 640), (480, 2), (1, 1), (2, 2), ("S", 640), (480, "S"), ("S+1", "S-1"),
+                                 ("S-1", "S+1"), (40, 800), (800, 40), (3024, 4032)])
 def test_resize_squash_matches_pillow_bit_exact(gpu_required, h, w):
     """PIL resize((S, S), BICUBIC) — what torchvision's Resize((S, S)) does to a PIL image in open_clip's SigLIP
-    transform: independent x and y scales, no crop."""
+    transform: independent x and y scales, no crop — at every S a served model squashes to.
+
+    The reference is the one call to Pillow's two-pass resampler (horizontal pass, then vertical) that Image.resize
+    makes for an image of any ordinary shape.  Pillow 12.2 (newer than the 10.4 the reference pins) instead resizes an
+    image more than 100 times taller than wide in two calls, the vertical one first, and so rounds to uint8 between
+    the passes in the other order: for 480 x 2 to 224 x 224 that moves about a fifth of the pixels, by up to 15.  The
+    kernel restates the single call."""
     from PIL import Image
     from marqo_b200.engine import debug_resize_squash
-    rng = np.random.default_rng(h * 7 + w)
-    imgs = rng.integers(0, 256, size=(3, h, w, 3), dtype=np.uint8)
-    imgs[1] = (np.linspace(0, 255, w)[None, :, None] * np.ones((h, 1, 3))).astype(np.uint8)   # smooth gradient
-    for S in (224, 384):
-        ref = np.stack([np.asarray(Image.fromarray(a).resize((S, S), Image.BICUBIC)) for a in imgs])
-        np.testing.assert_array_equal(debug_resize_squash(imgs, S), ref)
+    from test_kernels_gpu import _side
+    sizes = K.served_resize_sizes("squash")
+    assert sizes == [224, 256, 378, 384, 512]
+    for S in sizes:
+        hs, ws = _side(h, S), _side(w, S)
+        rng = np.random.default_rng(hs * 7 + ws)
+        imgs = rng.integers(0, 256, size=(1 if hs * ws > 4_000_000 else 3, hs, ws, 3), dtype=np.uint8)
+        if len(imgs) > 1:
+            imgs[1] = (np.linspace(0, 255, ws)[None, :, None] * np.ones((hs, 1, 3))).astype(np.uint8)   # smooth gradient
+        pil = [Image.fromarray(a) for a in imgs]
+        ref = np.stack([np.asarray(im._new(im.im.resize((S, S), Image.BICUBIC, (0, 0) + im.size))) for im in pil])
+        np.testing.assert_array_equal(debug_resize_squash(imgs, S), ref, err_msg=f"S = {S}, {hs} x {ws}")
 
 
 # ------------------------------------------------------------------------------------------------------------------
