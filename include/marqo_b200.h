@@ -438,6 +438,20 @@ int b200_model_encode_images_u8_device(b200_model* m, const uint8_t* d_hwc, int 
                                        float* d_out, int sync);
 int b200_model_encode_tokens_device(b200_model* m, const int32_t* d_ids, const int32_t* d_attn_mask, int n,
                                     int seq, int normalize, float* d_out, int sync);
+/* Images of mixed sizes in one call (every vision tower that takes uint8 images): image i is uint8 HWC
+ * [heights[i], widths[i], 3] at hwc[i]; hwc, heights and widths are host arrays of n.  The images are resized to the
+ * model's S x S by the tower's rule (shortest side + centre crop, or the squash) in one pass over each sub-batch, two
+ * kernels whatever the mix of sizes, and the tower runs once per sub-batch; images already S x S pass through
+ * unchanged.  out: fp32 host [n, embed_dim], row i for image i.  The host variant copies each sub-batch's images to the
+ * device, one copy per run of images that lie back to back in host memory.  NULL arrays or entries, n <= 0, a height
+ * or width <= 0, or a model without a vision tower: B200_ERR_INVALID_ARG, nothing written. */
+int b200_model_encode_images_u8_ragged(b200_model* m, const uint8_t* const* hwc, const int32_t* heights,
+                                       const int32_t* widths, int n, int normalize, float* out);
+/* The same with device-resident images: d_hwc is a host array of n device pointers on the model's device; d_out fp32
+ * device [n, embed_dim]; asynchronous on the model's stream unless sync != 0 (the call's host-side tables have been
+ * uploaded by the time it returns). */
+int b200_model_encode_images_u8_ragged_device(b200_model* m, const uint8_t* const* d_hwc, const int32_t* heights,
+                                              const int32_t* widths, int n, int normalize, float* d_out, int sync);
 int b200_model_set_stream(b200_model* m, void* cuda_stream, int use_external);
 /* Optional per-kernel-class device timing: when enabled every GEMM / attention launch of an encode call is
  * bracketed by CUDA events on the handle's stream; b200_model_profile returns their sums over every encode call
@@ -667,6 +681,12 @@ int b200_debug_resize(int device, const uint8_t* hwc, int n, int h, int w, int S
 /* The same bicubic resampling squashed to S x S (x and y scaled independently, no crop): PIL resize((S, S), BICUBIC),
  * SigLIP's preprocessing. */
 int b200_debug_resize_squash(int device, const uint8_t* hwc, int n, int h, int w, int S, uint8_t* out, void* stream);
+/* The resize of n images of any sizes in one pass, as b200_model_encode_images_u8_ragged runs it: image i is uint8 HWC
+ * [heights[i], widths[i], 3] at device pointer d_hwc[i] (d_hwc, heights and widths are host arrays) -> out
+ * [n, S, S, 3]; squash 0: shortest side -> S + centre crop, as b200_debug_resize; squash 1: as
+ * b200_debug_resize_squash. */
+int b200_debug_resize_ragged(int device, const uint8_t* const* d_hwc, const int32_t* heights, const int32_t* widths,
+                             int n, int S, int squash, uint8_t* out, void* stream);
 /* Single-query attention pooling: for image b and head h, softmax(q_h . k_{b,s} / sqrt(D)) over the S tokens of image
  * b, times v_{b,s}, D = W / H.  q fp32, image b's query at q + b * q_stride: q_stride 0 shares one latent query [W] by
  * every image (SigLIP's MAP head, CoCa's pooler), q_stride W gives one per image [B, W] (the ResNet attention pool).

@@ -116,6 +116,8 @@ _SIGNATURES = {
     "b200_model_encode_tokens": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "b200_model_encode_images_u8_device": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
     "b200_model_encode_tokens_device": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
+    "b200_model_encode_images_u8_ragged": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P]),
+    "b200_model_encode_images_u8_ragged_device": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int]),
     "b200_model_set_stream": (C.c_int, [_P, _P, C.c_int]),
     "b200_model_set_profiling": (C.c_int, [_P, C.c_int]),
     "b200_model_profile": (C.c_int, [_P, C.POINTER(C.c_float), C.POINTER(C.c_int), C.POINTER(C.c_float), C.POINTER(C.c_int)]),
@@ -154,6 +156,7 @@ _SIGNATURES = {
     "b200_debug_im2col_f32": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_resize": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_resize_squash": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_resize_ragged": (C.c_int, [C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_map_attention": (C.c_int, [C.c_int, _P, C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_conv2d": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, C.c_int,
                                     _P, _P]),

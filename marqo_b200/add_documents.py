@@ -57,8 +57,9 @@ def add_documents_device(index: GpuTensorIndex, schema: str, docs: Sequence[Dict
     (model loader object, 'image' | 'text').  Every tensor field is vectorised in ONE encode_to_device call over the
     batch (one chunk per document and field: images are not patch-chunked, captions are single chunks — the cfg3
     shape), the embeddings stay in HBM, and the batch is fed with one feed_batch.
-    `device_contents[field]`: optional pre-assembled batch content for the field (a uint8 [n, H, W, 3] CUDA tensor or an
-    int32 [n, seq] token-id array) replacing the per-document contents — what a loader that decodes / tokenises in bulk
+    `device_contents[field]`: optional pre-assembled batch content for the field (a uint8 [n, H, W, 3] CUDA tensor, a
+    list of n uint8 [H_i, W_i, 3] CUDA tensors of any sizes such as decode_images_to_device returns, or an int32
+    [n, seq] token-id array) replacing the per-document contents — what a loader that decodes / tokenises in bulk
     hands over.  Returns feed_batch's FeedBatchResponse."""
     vectorisers: Dict[str, DeviceBatchVectoriser] = {}
     for field, (model, modality) in tensor_fields.items():

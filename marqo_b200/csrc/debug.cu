@@ -517,6 +517,24 @@ int b200_debug_resize_squash(int device, const uint8_t* hwc, int n, int h, int w
     });
 }
 
+int b200_debug_resize_ragged(int device, const uint8_t* const* d_hwc, const int32_t* heights, const int32_t* widths,
+                             int n, int S, int squash, uint8_t* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(d_hwc && heights && widths && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && S > 0, "n, S must be positive");
+        for (int i = 0; i < n; ++i) {
+            MB_CHECK_ARG(d_hwc[i] != nullptr, "image %d is NULL", i);
+            MB_CHECK_ARG(heights[i] > 0 && widths[i] > 0, "image %d: height %d and width %d must be positive", i,
+                         heights[i], widths[i]);
+        }
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::resize_u8(d_hwc, heights, widths, n, S, squash != 0, out, s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
 int b200_debug_map_attention(int device, const float* q, int q_stride, const void* kv, int B, int S, int W, int H,
                              void* out, void* stream) {
     return guarded([&] {

@@ -2,7 +2,10 @@
 
 #include <cmath>
 #include <cstdlib>
+#include <cstring>
+#include <map>
 #include <mutex>
+#include <tuple>
 #include <vector>
 
 namespace mb {
@@ -862,17 +865,20 @@ static double bicubic_filter(double x) {
     return 0.0;
 }
 
-static ResampleTable precompute(int in_size, int out_size) {
+// Rows first .. first + count - 1 of the table for in_size -> out_size: a row depends on its index and the two sizes
+// only, so the S rows a crop keeps are computed without the rest of the resized image's.
+static ResampleTable precompute(int in_size, int out_size, int first, int count) {
     ResampleTable t;
     const double scale = (double)in_size / (double)out_size;
     double filterscale = scale;
     if (filterscale < 1.0) filterscale = 1.0;
     const double support = 2.0 * filterscale;
     t.ksize = (int)ceil(support) * 2 + 1;
-    t.bounds.assign((size_t)out_size * 2, 0);
-    t.coeffs.assign((size_t)out_size * t.ksize, 0);
+    t.bounds.assign((size_t)count * 2, 0);
+    t.coeffs.assign((size_t)count * t.ksize, 0);
     std::vector<double> k(t.ksize);
-    for (int xx = 0; xx < out_size; ++xx) {
+    for (int r = 0; r < count; ++r) {
+        const int xx = first + r;
         const double center = (xx + 0.5) * scale;
         double ww = 0.0;
         const double ss = 1.0 / filterscale;
@@ -890,11 +896,11 @@ static ResampleTable precompute(int in_size, int out_size) {
             if (ww != 0.0) k[x] /= ww;
         for (int x = 0; x < t.ksize; ++x) {
             const double v = x < xmax ? k[x] : 0.0;
-            t.coeffs[(size_t)xx * t.ksize + x] =
+            t.coeffs[(size_t)r * t.ksize + x] =
                 v < 0 ? (int)(-0.5 + v * (1 << PRECISION_BITS)) : (int)(0.5 + v * (1 << PRECISION_BITS));
         }
-        t.bounds[xx * 2] = xmin;
-        t.bounds[xx * 2 + 1] = xmax;
+        t.bounds[(size_t)r * 2] = xmin;
+        t.bounds[(size_t)r * 2 + 1] = xmax;
     }
     return t;
 }
@@ -904,18 +910,45 @@ __device__ __forceinline__ uint8_t clip8(int v) {
     return (uint8_t)min(max(v, 0), 255);
 }
 
-// horizontal: src [n, h, w, 3] -> tmp [n, h, S, 3] for output columns x_off .. x_off + S - 1 of the resized image
-__global__ void resample_h_kernel(const uint8_t* __restrict__ src, int n, int h, int w, int S, int x_off,
-                                  const int* __restrict__ bounds, const int* __restrict__ coeffs, int ksize,
-                                  uint8_t* __restrict__ tmp) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (long long)n * h * S) return;
-    const int xo = (int)(i % S);
-    const long long rowi = i / S;  // (image, y)
-    const int xx = xo + x_off;
-    const int xmin = bounds[xx * 2], cnt = bounds[xx * 2 + 1];
-    const int* k = coeffs + (long long)xx * ksize;
-    const uint8_t* line = src + rowi * w * 3;
+// One image of a ragged resize.  Its tables hold the S rows of the window kept: bounds [S][2] = (first source pixel,
+// taps) and coeffs [S][ksize], at int offsets into the packed table block.
+struct ResizeDesc {
+    const uint8_t* src;   // [h, w, 3]
+    long long row0;       // its first row in the intermediate [sum_i h_i, S, 3]
+    long long hb, hc;     // horizontal table: output column xo of the window
+    long long vb, vc;     // vertical table: output row yo of the window
+    int h, w, hk, vk;
+};
+
+// Image of intermediate row r: the last descriptor whose row0 <= r (row0 ascends, descriptor 0's is 0).
+__device__ __forceinline__ int image_of_row(const ResizeDesc* __restrict__ d, int n, long long r) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (d[mid].row0 <= r) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// horizontal: every source row of every image -> tmp [rows, S, 3], the S output columns of its window
+__global__ void resample_h_kernel(const ResizeDesc* __restrict__ d, int n, long long rows, int S,
+                                  const int* __restrict__ tab, uint8_t* __restrict__ tmp) {
+    // one search per block for the image of its first row; a block spans a few rows, so its threads step from there
+    __shared__ int first;
+    const long long i0 = (long long)blockIdx.x * blockDim.x;
+    if (threadIdx.x == 0) first = image_of_row(d, n, i0 / S);
+    __syncthreads();
+    const long long i = i0 + threadIdx.x;
+    if (i >= rows * S) return;
+    const long long r = i / S;
+    const int xo = (int)(i - r * S);
+    int b = first;
+    while (b + 1 < n && d[b + 1].row0 <= r) ++b;
+    const ResizeDesc& D = d[b];
+    const int xmin = tab[D.hb + 2 * xo], cnt = tab[D.hb + 2 * xo + 1];
+    const int* k = tab + D.hc + (long long)xo * D.hk;
+    const uint8_t* line = D.src + (r - D.row0) * D.w * 3;
     int s0 = 1 << (PRECISION_BITS - 1), s1 = s0, s2 = s0;
     for (int x = 0; x < cnt; ++x) {
         const int c = k[x];
@@ -930,22 +963,23 @@ __global__ void resample_h_kernel(const uint8_t* __restrict__ src, int n, int h,
     o[2] = clip8(s2);
 }
 
-// vertical: tmp [n, h, S, 3] -> dst [n, S, S, 3] for output rows y_off .. y_off + S - 1
-__global__ void resample_v_kernel(const uint8_t* __restrict__ tmp, int n, int h, int S, int y_off,
-                                  const int* __restrict__ bounds, const int* __restrict__ coeffs, int ksize,
-                                  uint8_t* __restrict__ dst) {
+// vertical: tmp [rows, S, 3] -> dst [n, S, S, 3], the S output rows of each image's window
+__global__ void resample_v_kernel(const ResizeDesc* __restrict__ d, int n, int S, const int* __restrict__ tab,
+                                  const uint8_t* __restrict__ tmp, uint8_t* __restrict__ dst) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (long long)n * S * S) return;
-    const int xo = (int)(i % S);
-    const int yo = (int)((i / S) % S);
-    const long long b = i / ((long long)S * S);
-    const int yy = yo + y_off;
-    const int ymin = bounds[yy * 2], cnt = bounds[yy * 2 + 1];
-    const int* k = coeffs + (long long)yy * ksize;
+    const long long SS = (long long)S * S;
+    if (i >= n * SS) return;
+    const long long b = i / SS;
+    const int p = (int)(i - b * SS);
+    const int yo = p / S, xo = p - yo * S;
+    const ResizeDesc& D = d[b];
+    const int ymin = tab[D.vb + 2 * yo], cnt = tab[D.vb + 2 * yo + 1];
+    const int* k = tab + D.vc + (long long)yo * D.vk;
+    const uint8_t* col = tmp + ((D.row0 + ymin) * S + xo) * 3;
     int s0 = 1 << (PRECISION_BITS - 1), s1 = s0, s2 = s0;
     for (int y = 0; y < cnt; ++y) {
         const int c = k[y];
-        const uint8_t* px = tmp + ((b * h + ymin + y) * S + xo) * 3;
+        const uint8_t* px = col + (long long)y * S * 3;
         s0 += px[0] * c;
         s1 += px[1] * c;
         s2 += px[2] * c;
@@ -958,54 +992,87 @@ __global__ void resample_v_kernel(const uint8_t* __restrict__ tmp, int n, int h,
 
 static int py_round_half_even(double v) { return (int)nearbyint(v); }
 
-// Resample [n, h, w, 3] to new_h x new_w and keep the S x S window at (top, left).
-static int resample_window_u8(const uint8_t* src, int n, int h, int w, int new_h, int new_w, int top, int left, int S,
-                              uint8_t* dst, cudaStream_t s) {
-    const ResampleTable th = precompute(w, new_w);
-    const ResampleTable tv = precompute(h, new_h);
+int resize_u8(const uint8_t* const* src, const int32_t* h, const int32_t* w, int n, int S, bool squash, uint8_t* dst,
+              cudaStream_t s) {
+    if (n <= 0) return 0;
+    // descriptors, then the tables, in one block: one upload
+    const size_t desc_bytes = (size_t)n * sizeof(ResizeDesc);
+    static_assert(sizeof(ResizeDesc) % sizeof(int) == 0, "the tables follow the descriptors int-aligned");
+    std::vector<ResizeDesc> desc((size_t)n);
+    std::vector<int> tab;
+    // (in, out, first) -> offsets of (bounds, coeffs) and ksize: one table per distinct resize of an axis in the call
+    std::map<std::tuple<int, int, int>, std::tuple<long long, long long, int>> tables;
+    auto table = [&](int in, int out, int first, long long& b, long long& c, int& k) {
+        auto it = tables.find({in, out, first});
+        if (it == tables.end()) {
+            const ResampleTable t = precompute(in, out, first, S);
+            const long long at = (long long)tab.size();
+            tab.insert(tab.end(), t.bounds.begin(), t.bounds.end());
+            tab.insert(tab.end(), t.coeffs.begin(), t.coeffs.end());
+            it = tables.emplace(std::make_tuple(in, out, first), std::make_tuple(at, at + 2LL * S, t.ksize)).first;
+        }
+        std::tie(b, c, k) = it->second;
+    };
+    long long rows = 0;
+    for (int i = 0; i < n; ++i) {
+        int new_h = S, new_w = S, top = 0, left = 0;
+        if (!squash) {
+            // torchvision Resize(S): shortest side -> S, the other int(S * long / short); CenterCrop(S)
+            if (w[i] <= h[i])
+                new_h = (int)((double)((long long)S * h[i]) / (double)w[i]);   // int(S * long / short): true division
+            else
+                new_w = (int)((double)((long long)S * w[i]) / (double)h[i]);
+            left = py_round_half_even((new_w - S) / 2.0);
+            top = py_round_half_even((new_h - S) / 2.0);
+        }
+        // squash: PIL resize((S, S), BICUBIC) = torchvision Resize((S, S)) on a PIL image, nothing cropped.  An axis
+        // that already has S pixels gets the identity coefficients (a single 1.0 tap), so running its pass is exact.
+        ResizeDesc& D = desc[i];
+        D.src = src[i];
+        D.row0 = rows;
+        D.h = h[i];
+        D.w = w[i];
+        table(w[i], new_w, left, D.hb, D.hc, D.hk);
+        table(h[i], new_h, top, D.vb, D.vc, D.vk);
+        rows += h[i];
+    }
+    std::vector<uint8_t> block(desc_bytes + tab.size() * sizeof(int));
+    std::memcpy(block.data(), desc.data(), desc_bytes);
+    std::memcpy(block.data() + desc_bytes, tab.data(), tab.size() * sizeof(int));
     {   // stream-ordered temporaries, released on `s` at the end of this block
-        auto up = [&](const std::vector<int>& v) {
-            DeviceBuffer<int> d(v.size(), s);
-            MB_CUDA(cudaMemcpyAsync(d.get(), v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-            return d;
-        };
-        const DeviceBuffer<int> d_hb = up(th.bounds), d_hc = up(th.coeffs), d_vb = up(tv.bounds), d_vc = up(tv.coeffs);
-        const DeviceBuffer<uint8_t> tmp((size_t)n * h * S * 3, s);
-        const long long nh = (long long)n * h * S;
-        resample_h_kernel<<<(unsigned)((nh + 255) / 256), 256, 0, s>>>(src, n, h, w, S, left, d_hb.get(), d_hc.get(),
-                                                                       th.ksize, tmp.get());
+        const DeviceBuffer<uint8_t> d_block(block.size(), s);
+        MB_CUDA(cudaMemcpyAsync(d_block.get(), block.data(), block.size(), cudaMemcpyHostToDevice, s));
+        // `block` is pageable and freed on return: the copy must be done before the kernels are even queued
+        MB_CUDA(cudaStreamSynchronize(s));
+        const ResizeDesc* d_desc = reinterpret_cast<const ResizeDesc*>(d_block.get());
+        const int* d_tab = reinterpret_cast<const int*>(d_block.get() + desc_bytes);
+        const DeviceBuffer<uint8_t> tmp((size_t)rows * S * 3, s);
+        const long long nh = rows * S;
+        resample_h_kernel<<<(unsigned)((nh + 255) / 256), 256, 0, s>>>(d_desc, n, rows, S, d_tab, tmp.get());
         MB_CUDA(cudaGetLastError());
         const long long nv = (long long)n * S * S;
-        resample_v_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, s>>>(tmp.get(), n, h, S, top, d_vb.get(), d_vc.get(),
-                                                                       tv.ksize, dst);
+        resample_v_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, s>>>(d_desc, n, S, d_tab, tmp.get(), dst);
         MB_CUDA(cudaGetLastError());
     }
-    // the pageable host vectors above must outlive the async copies: synchronise before they go out of scope
-    MB_CUDA(cudaStreamSynchronize(s));
     return 2;
 }
 
-int resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s) {
+// the uniform batch [n, h, w, 3]: every image's pointer into it, one size
+static int resize_uniform_u8(const uint8_t* src, int n, int h, int w, int S, bool squash, uint8_t* dst,
+                             cudaStream_t s) {
     if (n <= 0) return 0;
-    // torchvision Resize(S): shortest side -> S, the other int(S * long / short); CenterCrop(S)
-    int new_w, new_h;
-    if (w <= h) {
-        new_w = S;
-        new_h = (int)((double)((long long)S * h) / (double)w);  // int(S * long / short): Python true division
-    } else {
-        new_h = S;
-        new_w = (int)((double)((long long)S * w) / (double)h);
-    }
-    const int left = py_round_half_even((new_w - S) / 2.0);
-    const int top = py_round_half_even((new_h - S) / 2.0);
-    return resample_window_u8(src, n, h, w, new_h, new_w, top, left, S, dst, s);
+    std::vector<const uint8_t*> ptr((size_t)n);
+    for (int i = 0; i < n; ++i) ptr[i] = src + (size_t)i * h * w * 3;
+    const std::vector<int32_t> hs((size_t)n, h), ws((size_t)n, w);
+    return resize_u8(ptr.data(), hs.data(), ws.data(), n, S, squash, dst, s);
+}
+
+int resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s) {
+    return resize_uniform_u8(src, n, h, w, S, false, dst, s);
 }
 
 int resize_squash_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s) {
-    if (n <= 0) return 0;
-    // PIL resize((S, S), BICUBIC) = torchvision Resize((S, S)) on a PIL image: both axes to S, nothing cropped.  An axis
-    // that already has S pixels gets the identity coefficients (a single 1.0 tap), so running its pass is exact.
-    return resample_window_u8(src, n, h, w, S, S, 0, 0, S, dst, s);
+    return resize_uniform_u8(src, n, h, w, S, true, dst, s);
 }
 
 // ------------------------------------------------------------------------------------------------ SigLIP MAP head

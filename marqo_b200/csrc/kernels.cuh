@@ -93,10 +93,16 @@ void pad_rows_to_bf16(const float* src, int rows, int k, int kpad, __nv_bfloat16
 // k' = dy * (64 * kbpd) + dx * 3 + c; the slots past 3 * p of every pixel row are zero.
 void patch_weight_rows(const float* src, int rows, int p, int kbpd, __nv_bfloat16* dst, cudaStream_t s);
 
-// PIL-compatible antialiased bicubic resize (shortest side -> S) + centre crop, uint8 HWC in/out: a horizontal and a
-// vertical pass, two kernels.
+// PIL-compatible antialiased bicubic resize of n images of any sizes to dst uint8 [n, S, S, 3]: image i is uint8 HWC
+// [h[i], w[i], 3] at device pointer src[i] (src, h and w are host arrays).  squash false: shortest side -> S, then the
+// centre S x S (torchvision Resize(S) + CenterCrop(S)); true: x and y scaled independently to S, no crop (PIL
+// resize((S, S), BICUBIC)).  A horizontal and a vertical pass over the whole batch, two kernels whatever the sizes;
+// the coefficient tables are computed on the host once per distinct resize of an axis and uploaded with the
+// per-image descriptors in one copy, which has finished when the call returns.
+int resize_u8(const uint8_t* const* src, const int32_t* h, const int32_t* w, int n, int S, bool squash, uint8_t* dst,
+              cudaStream_t s);
+// resize_u8 of the uniform batch [n, h, w, 3] at src: shortest side + centre crop, and the squash.
 int resize_crop_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s);
-// The same resampling squashed to S x S (x and y scaled independently, no crop): PIL resize((S, S), BICUBIC).
 int resize_squash_u8(const uint8_t* src, int n, int h, int w, int S, uint8_t* dst, cudaStream_t s);
 
 // Single-query attention pooling, one query per head of D = W / heads columns: out[b, h*D .. h*D+D-1] =

@@ -1497,6 +1497,9 @@ struct TimedRegion {
     }
 };
 
+// open_clip's SigLIP and DFN5B preprocessing squashes (no crop); every other tower crops
+bool resize_squashes(b200_model* m) { return m->kind.vision == VisionKind::SIGLIP_VIT || m->desc.resize_squash; }
+
 // device-resident uint8 images of size h x w -> embeddings
 void encode_images_u8_dev(b200_model* m, Counter& c, const uint8_t* d_img, int n, int h, int w, int normalize,
                           float* d_out) {
@@ -1507,14 +1510,37 @@ void encode_images_u8_dev(b200_model* m, Counter& c, const uint8_t* d_img, int n
         const int nb = std::min(cap, n - o);
         const uint8_t* src = d_img + (size_t)o * h * w * 3;
         if (h != S || w != S) {
-            // open_clip's SigLIP and DFN5B preprocessing squashes (no crop); every other tower crops
-            if (m->kind.vision == VisionKind::SIGLIP_VIT || m->desc.resize_squash)
+            if (resize_squashes(m))
                 c.n += kernels::resize_squash_u8(src, nb, h, w, S, m->resized.get(), m->stream);
             else
                 c.n += kernels::resize_crop_u8(src, nb, h, w, S, m->resized.get(), m->stream);
             src = m->resized.get();
         }
         forward_images(m, c, src, nullptr, nb, normalize, d_out + (size_t)o * m->desc.embed_dim);
+    }
+}
+
+// device-resident uint8 images of any sizes (d_img, h, w: host arrays of n) -> embeddings: each sub-batch is resized
+// into m->resized in one kernel pair, images already S x S included (their taps are the identity)
+void encode_images_u8_ragged_dev(b200_model* m, Counter& c, const uint8_t* const* d_img, const int32_t* h,
+                                 const int32_t* w, int n, int normalize, float* d_out) {
+    const int S = m->vision.d.image_size;
+    const int cap = image_batch_cap(m);
+    for (int o = 0; o < n; o += cap) {
+        const int nb = std::min(cap, n - o);
+        c.n += kernels::resize_u8(d_img + o, h + o, w + o, nb, S, resize_squashes(m), m->resized.get(), m->stream);
+        forward_images(m, c, m->resized.get(), nullptr, nb, normalize, d_out + (size_t)o * m->desc.embed_dim);
+    }
+}
+
+// the arguments of a ragged image call, all checked before anything is written
+void check_ragged_args(b200_model* m, const uint8_t* const* imgs, const int32_t* h, const int32_t* w, int n) {
+    MB_CHECK_ARG(imgs && h && w, "NULL array");
+    MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
+    MB_CHECK_ARG(n > 0, "n must be positive");
+    for (int i = 0; i < n; ++i) {
+        MB_CHECK_ARG(imgs[i] != nullptr, "image %d is NULL", i);
+        MB_CHECK_ARG(h[i] > 0 && w[i] > 0, "image %d: height %d and width %d must be positive", i, h[i], w[i]);
     }
 }
 
@@ -1692,6 +1718,52 @@ int b200_model_encode_images_u8(b200_model* m, const uint8_t* hwc, int n, int h,
     });
 }
 
+int b200_model_encode_images_u8_ragged(b200_model* m, const uint8_t* const* hwc, const int32_t* heights,
+                                       const int32_t* widths, int n, int normalize, float* out) {
+    return guarded([&] {
+        require_ready(m);
+        MB_CHECK_ARG(out != nullptr, "NULL buffer");
+        check_ragged_args(m, hwc, heights, widths, n);
+        std::lock_guard<std::mutex> lk(m->mu);
+        DeviceGuard g(m->device);
+        const int E = m->desc.embed_dim;
+        const int cap = image_batch_cap(m);
+        auto bytes = [&](int i) { return (size_t)heights[i] * widths[i] * 3; };
+        size_t most = 0;   // the largest sub-batch's pixels: what in_dev must hold
+        for (int o = 0; o < n; o += cap) {
+            size_t sum = 0;
+            for (int i = o; i < std::min(n, o + cap); ++i) sum += bytes(i);
+            most = std::max(most, sum);
+        }
+        ensure_in_dev(m, most);
+        std::vector<const uint8_t*> d_img((size_t)n);
+        TimedRegion tr(m);
+        for (int o = 0; o < n; o += cap) {
+            const int nb = std::min(cap, n - o);
+            size_t off = 0;
+            for (int i = o; i < o + nb;) {
+                // one copy per run of images that lie back to back in host memory
+                size_t run = bytes(i);
+                d_img[i] = m->in_dev.get() + off;
+                int j = i + 1;
+                for (; j < o + nb && hwc[j] == hwc[j - 1] + bytes(j - 1); ++j) {
+                    d_img[j] = d_img[i] + run;
+                    run += bytes(j);
+                }
+                MB_CUDA(cudaMemcpyAsync(m->in_dev.get() + off, hwc[i], run, cudaMemcpyHostToDevice, m->stream));
+                off += run;
+                i = j;
+            }
+            encode_images_u8_ragged_dev(m, tr.c, d_img.data() + o, heights + o, widths + o, nb, normalize,
+                                        m->out_dev.get());
+            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
+                                    m->stream));
+            MB_CUDA(cudaStreamSynchronize(m->stream));
+        }
+        tr.finish();
+    });
+}
+
 int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int normalize, float* out) {
     return guarded([&] {
         require_ready(m);
@@ -1772,6 +1844,21 @@ int b200_model_encode_images_u8_device(b200_model* m, const uint8_t* d_hwc, int 
         DeviceGuard g(m->device);
         TimedRegion tr(m);
         encode_images_u8_dev(m, tr.c, d_hwc, n, h, w, normalize, d_out);
+        tr.finish();
+        if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
+    });
+}
+
+int b200_model_encode_images_u8_ragged_device(b200_model* m, const uint8_t* const* d_hwc, const int32_t* heights,
+                                              const int32_t* widths, int n, int normalize, float* d_out, int sync) {
+    return guarded([&] {
+        require_ready(m);
+        MB_CHECK_ARG(d_out != nullptr, "NULL buffer");
+        check_ragged_args(m, d_hwc, heights, widths, n);
+        std::lock_guard<std::mutex> lk(m->mu);
+        DeviceGuard g(m->device);
+        TimedRegion tr(m);
+        encode_images_u8_ragged_dev(m, tr.c, d_hwc, heights, widths, n, normalize, d_out);
         tr.finish();
         if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
     });

@@ -500,20 +500,49 @@ class Encoder:
                 if a.shape != (h, w, 3) or a.dtype != np.uint8:
                     raise ValueError(f"image {i}: expected uint8 [{h}, {w}, 3], got {a.dtype} {a.shape}")
 
-            def fill(lo: int, hi: int) -> None:
-                for i in range(lo, hi):
-                    np.copyto(buf[i], images[i])   # releases the GIL for the memcpy
-
-            if n * h * w * 3 >= (8 << 20):   # a 38 MB batch: ~4 ms on one core, < 1 ms on eight
-                if self._pool is None:
-                    from concurrent.futures import ThreadPoolExecutor
-                    self._pool = ThreadPoolExecutor(8, thread_name_prefix="b200-stage")
-                step = (n + 7) // 8
-                list(self._pool.map(lambda lo: fill(lo, min(n, lo + step)), range(0, n, step)))
-            else:
-                fill(0, n)
+            self._fill(n, n * h * w * 3, lambda i: np.copyto(buf[i], images[i]))
             N.check(self._lib.b200_model_encode_images_u8(self._handle(), C.c_void_p(self._stage_ptr.value), n, h, w,
                                                           1 if normalize else 0, _ptr(out)))
+        return out
+
+    def _fill(self, n: int, nbytes: int, copy) -> None:
+        """copy(i) for i < n: the staging copies of n images of nbytes in all (np.copyto releases the GIL for the
+        memcpy), on eight threads from 8 MB up."""
+        def fill(lo: int, hi: int) -> None:
+            for i in range(lo, hi):
+                copy(i)
+
+        if nbytes >= (8 << 20):   # a 38 MB batch: ~4 ms on one core, < 1 ms on eight
+            if self._pool is None:
+                from concurrent.futures import ThreadPoolExecutor
+                self._pool = ThreadPoolExecutor(8, thread_name_prefix="b200-stage")
+            step = (n + 7) // 8
+            list(self._pool.map(lambda lo: fill(lo, min(n, lo + step)), range(0, n, step)))
+        else:
+            fill(0, n)
+
+    def encode_images_u8_ragged(self, images: Sequence[np.ndarray], normalize: bool = True) -> np.ndarray:
+        """uint8 HWC images of any sizes, [h_i, w_i, 3] each, in one call: they are packed back to back into the
+        page-locked staging buffer (one H2D copy per sub-batch), resized together on the GPU and encoded in one tower
+        pass per sub-batch.  Row i of the result is image i's embedding."""
+        n = len(images)
+        if n == 0:
+            raise ValueError("expected at least one image")
+        for i, a in enumerate(images):
+            if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+                raise ValueError(f"image {i}: expected uint8 [H, W, 3], got {a.dtype} {a.shape}")
+        sizes = [a.shape[0] * a.shape[1] * 3 for a in images]
+        offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        heights = np.array([a.shape[0] for a in images], np.int32)
+        widths = np.array([a.shape[1] for a in images], np.int32)
+        out = np.empty((n, self.embed_dim), np.float32)
+        with self._stage_lock:
+            buf = self._staging(int(offsets[-1]))
+            self._fill(n, int(offsets[-1]),
+                       lambda i: np.copyto(buf[offsets[i]:offsets[i + 1]].reshape(images[i].shape), images[i]))
+            ptrs = (C.c_void_p * n)(*[self._stage_ptr.value + int(o) for o in offsets[:-1]])
+            N.check(self._lib.b200_model_encode_images_u8_ragged(self._handle(), ptrs, _ptr(heights), _ptr(widths), n,
+                                                                 1 if normalize else 0, _ptr(out)))
         return out
 
     def encode_images_u8(self, hwc: np.ndarray, normalize: bool = True) -> np.ndarray:
@@ -553,6 +582,19 @@ class Encoder:
         N.check(self._lib.b200_model_encode_images_u8_device(self._handle(), C.c_void_p(d_ptr), n, h, w,
                                                              1 if normalize else 0, C.c_void_p(d_out_ptr),
                                                              1 if sync else 0))
+
+    def encode_images_u8_ragged_device(self, ptrs: Sequence[int], heights: Sequence[int], widths: Sequence[int],
+                                       d_out_ptr: int, normalize: bool = True, sync: bool = True) -> None:
+        """Device-resident uint8 HWC images of any sizes: image i at device pointer ptrs[i], heights[i] x widths[i];
+        d_out_ptr: fp32 device [n, embed_dim]."""
+        n = len(ptrs)
+        if len(heights) != n or len(widths) != n:
+            raise ValueError(f"{n} pointers, {len(heights)} heights and {len(widths)} widths")
+        p = (C.c_void_p * max(n, 1))(*[int(x) for x in ptrs])
+        N.check(self._lib.b200_model_encode_images_u8_ragged_device(self._handle(), p, _ptr(_as(heights, np.int32)),
+                                                                    _ptr(_as(widths, np.int32)), n,
+                                                                    1 if normalize else 0, C.c_void_p(d_out_ptr),
+                                                                    1 if sync else 0))
 
     def encode_tokens_device(self, d_ids_ptr: int, d_mask_ptr: Optional[int], n: int, seq: int, d_out_ptr: int,
                              normalize: bool = True, sync: bool = True) -> None:
@@ -1006,6 +1048,21 @@ def debug_resize_squash(hwc, S: int, device: int = 0) -> np.ndarray:
     da, out = d.up(a, "uint8"), d.empty((a.shape[0], S, S, 3), "uint8")
     N.check(N.load().b200_debug_resize_squash(device, _dptr(da), a.shape[0], a.shape[1], a.shape[2], S, _dptr(out),
                                               d.stream))
+    return _host(out)
+
+
+def debug_resize_ragged(images, S: int, squash: bool = False, device: int = 0) -> np.ndarray:
+    """uint8 HWC images of any sizes -> uint8 [n, S, S, 3] in one ragged resize: the shortest side to S and the centre
+    crop (as debug_resize), or with squash both sides to S (as debug_resize_squash)."""
+    imgs = [_as(a, np.uint8) for a in images]
+    d = _Staging(device)
+    dev = [d.up(a, "uint8") for a in imgs]
+    heights = np.array([a.shape[0] for a in imgs], np.int32)
+    widths = np.array([a.shape[1] for a in imgs], np.int32)
+    out = d.empty((len(imgs), S, S, 3), "uint8")
+    ptrs = (C.c_void_p * max(len(imgs), 1))(*[t.data_ptr() for t in dev])
+    N.check(N.load().b200_debug_resize_ragged(device, ptrs, _ptr(heights), _ptr(widths), len(imgs), S, int(squash),
+                                              _dptr(out), d.stream))
     return _host(out)
 
 

@@ -243,7 +243,9 @@ class B200OpenCLIP:
         """encode() whose result is a CUDA fp32 tensor [n, dim] on the model's device instead of a host ndarray: the
         vectors go from the projection + L2 epilogue straight into the row store (b200_index_add_device_docs), never
         through `List[List[float]]`.  Same routing rules as encode() (abstract_clip_model.py:56-75).  Images: uint8 HWC
-        arrays / tensors of ONE size per call; texts: strings, or an int32 [n, ctx] array of token ids."""
+        arrays / tensors; a sub-batch of one size is stacked into one block, one of mixed sizes goes to the ragged entry
+        point in one call (CUDA tensors by pointer, host arrays in one packed upload).  Texts: strings, or an int32
+        [n, ctx] array of token ids."""
         import torch
         if self.model is None:
             self.load()
@@ -251,20 +253,25 @@ class B200OpenCLIP:
         items = inputs if isinstance(inputs, list) else [inputs]
         is_ids = isinstance(inputs, np.ndarray) and inputs.dtype.kind in "iu" and inputs.ndim == 2
         is_image = not is_ids and ((infer and _is_image(inputs)) or default == 'image')
-        dev = torch.device("cuda", self.model.device)
+        dev = self._torch_device()
         n = inputs.shape[0] if is_ids else len(items)
         out = torch.empty((n, self.model.embed_dim), dtype=torch.float32, device=dev)
         step = max(1, min(int(sub_batch), int(self.model_properties.get("max_batch", 256))))
         if is_image:
             for lo in range(0, n, step):
                 part = items[lo:lo + step]
-                if all(self._on_model_device(it) for it in part):
+                on_device = all(self._on_model_device(it) for it in part)
+                if not on_device:
+                    part = [np.asarray(it.cpu() if _is_tensor(it) else
+                                       (it.convert("RGB") if type(it).__module__.startswith("PIL.") else it),
+                                       dtype=np.uint8) for it in part]
+                if len({tuple(it.shape) for it in part}) > 1:
+                    self._encode_ragged_to_device(part, on_device, out[lo:], bool(normalize))
+                    continue
+                if on_device:
                     batch = torch.stack(part).contiguous()
                 else:
-                    host = np.stack([np.asarray(it.cpu() if _is_tensor(it) else
-                                                (it.convert("RGB") if type(it).__module__.startswith("PIL.") else it),
-                                                dtype=np.uint8) for it in part])
-                    batch = torch.from_numpy(host).to(dev, non_blocking=False)
+                    batch = torch.from_numpy(np.stack(part)).to(dev, non_blocking=False)
                 if batch.ndim != 4 or batch.shape[3] != 3:
                     raise UnidentifiedImageError(f"expected uint8 [n, H, W, 3] images, got {tuple(batch.shape)}")
                 self._sync_device(dev)
@@ -279,6 +286,31 @@ class B200OpenCLIP:
                 self.model.encode_tokens_device(d_ids[lo:].data_ptr(), None, m, int(ids.shape[1]), out[lo:].data_ptr(),
                                                 normalize=bool(normalize), sync=True)
         return out
+
+    def _encode_ragged_to_device(self, part, on_device: bool, out, normalize: bool) -> None:
+        """Images of mixed sizes (CUDA tensors on the model's device, or host arrays) -> rows out[:len(part)] through
+        one ragged call; host arrays are packed back to back and uploaded in one copy."""
+        import torch
+        for it in part:
+            if it.ndim != 3 or it.shape[2] != 3:
+                raise UnidentifiedImageError(f"expected uint8 [H, W, 3] images, got {tuple(it.shape)}")
+        if on_device:
+            keep = [t.contiguous() for t in part]
+            ptrs = [t.data_ptr() for t in keep]
+        else:
+            keep = torch.from_numpy(np.concatenate([a.reshape(-1) for a in part])).to(self._torch_device(),
+                                                                                      non_blocking=False)
+            offsets = np.cumsum([0] + [a.size for a in part[:-1]])
+            ptrs = [keep.data_ptr() + int(o) for o in offsets]
+        self._sync_device(out.device)
+        self.model.encode_images_u8_ragged_device(ptrs, [int(it.shape[0]) for it in part],
+                                                  [int(it.shape[1]) for it in part], out.data_ptr(),
+                                                  normalize=normalize, sync=True)
+
+    def _torch_device(self):
+        """The torch device of the model's GPU, where encode_to_device's results live."""
+        import torch
+        return torch.device("cuda", self.model.device)
 
 
 class B200HuggingFace:
