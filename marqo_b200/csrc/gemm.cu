@@ -87,7 +87,7 @@ struct Params {
     // k index of the A row = dy * (64 * kbpd) + dx * 3 + c (kernels::patch_weight_rows lays W out the same way).
     // PROD_CONV (gemm.cuh: ConvGather) reuses four of these fields rather than growing Params, whose layout every
     // other instantiation's code depends on: img is the NHWC bf16 activation [n, H, W, cin], g = H, patch = W and
-    // kbpd = log2(cin).
+    // kbpd = cin.
     const uint8_t* img;
     int g;                  // patches per image side
     int patch;              // patch edge in pixels
@@ -296,7 +296,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     const int lane = threadIdx.x & 31;
     const int tile_m = blockIdx.x / p.tiles_n, tile_n = blockIdx.x % p.tiles_n;
     const int m0 = tile_m * BM, n0 = tile_n * BN;
-    const int kblocks = p.K / BK;
+    // K need only be a multiple of 8: the last k-block's columns past K are zero-filled by TMA in A and W alike
+    const int kblocks = (p.K + BK - 1) / BK;
 
     if (threadIdx.x == MMA_THREADS) {
         ptx::prefetch_tmap(&tmap_b);
@@ -320,7 +321,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         // PROD_CONV: thread pt builds A row pt, output pixel (b, cy, cx) = m0 + pt; cimg is image b (NULL: row >= M)
         const __nv_bfloat16* cimg = nullptr;
         int cy = 0, cx = 0;
-        const int cH = p.g, cW = p.patch, lg_cin = p.kbpd;   // PROD_CONV's meaning of these fields
+        const int cH = p.g, cW = p.patch, cin = p.kbpd;   // PROD_CONV's meaning of these fields
         if (PROD == PROD_CONV) {
             const int r = m0 + pt;
             if (r < p.M) {
@@ -328,7 +329,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                 const int b = r / hw, rem = r - b * hw;
                 cy = rem / cW;
                 cx = rem - cy * cW;
-                cimg = reinterpret_cast<const __nv_bfloat16*>(p.img) + ((size_t)b * hw << lg_cin);
+                cimg = reinterpret_cast<const __nv_bfloat16*>(p.img) + (size_t)b * hw * cin;
             }
         }
         if (PROD == PROD_PATCH) {
@@ -352,17 +353,23 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
                 ptx::tma_load_2d(sb, &tmap_b, &full[stage], kb * BK, n0, ptx::kEvictLast);
             }
             if (PROD == PROD_CONV) {
-                // 16-byte unit u holds k = 64 kb + 8 u .. + 7: channels c .. c + 7 of tap k >> lg_cin.  All eight
+                // 16-byte unit u holds k = 64 kb + 8 u .. + 7: channels c .. c + 7 of tap t, k = t cin + c.  cin is
+                // a multiple of 8, so a unit never straddles two taps: (t, c) walks the k-block in 8-channel steps,
+                // onto the next tap whenever c reaches cin (more than once per k-block when cin < 64).  All eight
                 // loads are issued before the first store.
+                int tap = kb * 64 / cin, c = kb * 64 - tap * cin;
                 uint4 v[8];
 #pragma unroll
                 for (int u = 0; u < 8; ++u) {
-                    const int k = kb * 64 + u * 8;
-                    const int tap = k >> lg_cin, c = k & ((1 << lg_cin) - 1);
                     const int iy = cy + tap / 3 - 1, ix = cx + tap % 3 - 1;
                     v[u] = make_uint4(0u, 0u, 0u, 0u);
                     if (cimg != nullptr && tap < 9 && (unsigned)iy < (unsigned)cH && (unsigned)ix < (unsigned)cW)
-                        v[u] = __ldg(reinterpret_cast<const uint4*>(cimg + (((size_t)iy * cW + ix) << lg_cin) + c));
+                        v[u] = __ldg(reinterpret_cast<const uint4*>(cimg + ((size_t)iy * cW + ix) * cin + c));
+                    c += 8;
+                    if (c == cin) {
+                        c = 0;
+                        ++tap;
+                    }
                 }
 #pragma unroll
                 for (int u = 0; u < 8; ++u) *reinterpret_cast<uint4*>(sa + sw128_offset(pt, u)) = v[u];
@@ -682,7 +689,7 @@ static void launch_tiles(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W
         p.img = reinterpret_cast<const uint8_t*>(cg->act);
         p.g = cg->H;
         p.patch = cg->W;
-        while ((1 << p.kbpd) < cg->cin) ++p.kbpd;
+        p.kbpd = cg->cin;
     }
     if (PROD == PROD_PATCH) {
         p.img = pg->img;
@@ -759,9 +766,9 @@ int launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, co
 
 int launch_conv3x3(const ConvGather& cg, const __nv_bfloat16* Wc, int N, const Epilogue& ep, cudaStream_t stream) {
     if (cg.n <= 0 || N <= 0) return 0;
-    if (cg.H <= 0 || cg.W <= 0 || cg.cin < 32 || (cg.cin & (cg.cin - 1)) != 0)
-        fail(B200_ERR_INTERNAL, "conv3x3: %d x %d x %d input (cin must be a power of two >= 32)", cg.H, cg.W, cg.cin);
-    if (N % 32 != 0) fail(B200_ERR_INTERNAL, "conv3x3: N = %d must be a multiple of 32", N);
+    if (cg.H <= 0 || cg.W <= 0 || cg.cin < 8 || cg.cin % 8 != 0)
+        fail(B200_ERR_INTERNAL, "conv3x3: %d x %d x %d input (cin must be a positive multiple of 8)", cg.H, cg.W, cg.cin);
+    if (N % 8 != 0) fail(B200_ERR_INTERNAL, "conv3x3: N = %d must be a multiple of 8", N);
     if (ep.out_fp32 || ep.act != ACT_RELU) fail(B200_ERR_INTERNAL, "conv3x3: bf16 output with ReLU only");
     if ((reinterpret_cast<uintptr_t>(cg.act) & 15) != 0) fail(B200_ERR_INTERNAL, "conv3x3: input not 16-byte aligned");
     check_epilogue(ep);
@@ -804,8 +811,12 @@ void conv_weight_rows(const float* w, int cout, int cin, int k, const double* sc
 int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep, int sms,
            cudaStream_t stream) {
     if (M <= 0 || N <= 0) return KERNEL_NONE;
-    if (K <= 0 || K % BK != 0) fail(B200_ERR_INTERNAL, "gemm: K = %d must be a positive multiple of %d", K, BK);
-    if (N % 32 != 0) fail(B200_ERR_INTERNAL, "gemm: N = %d must be a multiple of 32", N);
+    // TMA needs 16-byte row pitches: K % 8 == 0; a partial last k-block is zero-filled past K in both operands.  The
+    // bf16 output's last 64-column box is clipped at N by the TMA store, as at M; the fp32 epilogue keeps whole
+    // 32-column boxes.
+    if (K <= 0 || K % 8 != 0) fail(B200_ERR_INTERNAL, "gemm: K = %d must be a positive multiple of 8", K);
+    if (N % (ep.out_fp32 ? 32 : 8) != 0)
+        fail(B200_ERR_INTERNAL, "gemm: N = %d must be a multiple of %d", N, ep.out_fp32 ? 32 : 8);
     if (lda % 8 != 0) fail(B200_ERR_INTERNAL, "gemm: lda = %d must be a multiple of 8", lda);
     check_epilogue(ep);
     configure();
@@ -814,7 +825,8 @@ int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N
     // column tile (the 384-wide BERTs run slower with one; DESIGN.md §7.5c).
     const long long tiles256 = (long long)((M + BM - 1) / BM) * (N / P_BN);
     // (the persistent kernel has no bf16 residual)
-    const bool persistent = K >= 1024 && N % P_BN == 0 && tiles256 >= sms && (ep.out_fp32 || ep.residual == nullptr);
+    const bool persistent = K >= 1024 && K % BK == 0 && N % P_BN == 0 && tiles256 >= sms &&
+                            (ep.out_fp32 || ep.residual == nullptr);
     dispatch(ep.out_fp32, ep.act, [&](auto out, auto a) {
         constexpr bool OUT_FP32 = decltype(out)::value;
         constexpr int ACT = decltype(a)::value;

@@ -26,8 +26,10 @@ struct Epilogue {
 };
 
 // A: bf16 [M, K] row-major with leading dimension lda (elements); W: bf16 [N, K] row-major (nn.Linear layout).
-// Requirements: K % 64 == 0, N % 32 == 0, lda % 8 == 0.
-// Returns the kernel it launched: KERNEL_PERSISTENT for K >= 1024, N % 256 == 0 and at least sm_count 128 x 256 tiles,
+// Requirements: K % 8 == 0 (the last 64-wide k-block is zero-filled past K in A and W by TMA), N % 8 == 0 for a bf16
+// output and N % 32 == 0 for an fp32 one (the last output box is clipped at N), lda % 8 == 0.
+// Returns the kernel it launched: KERNEL_PERSISTENT for K >= 1024, K % 64 == 0, N % 256 == 0 and at least sm_count
+// 128 x 256 tiles,
 // KERNEL_128x128 otherwise, KERNEL_NONE when M or N is 0.
 enum Kernel { KERNEL_NONE = -1, KERNEL_128x128 = 0, KERNEL_PERSISTENT = 1 };
 int launch(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int M, int N, int K, const Epilogue& ep,
@@ -55,9 +57,10 @@ int launch_patch_embed(const PatchGather& pg, const __nv_bfloat16* Wg, int N, co
 // row r of the virtual A matrix is output pixel (b, y, x) = r in row-major order (a 128-row tile may span images), and
 // its k index tap * cin + c, tap = 3 (dy + 1) + (dx + 1), reads input pixel (y + dy, x + dx), zero outside the image.
 // The four gather warps of the GEMM copy 16-byte channel chunks into the swizzled A stage; k-block kb covers
-// k = 64 kb .. 64 kb + 63 (one tap of 64 channels, or two taps when cin = 32), and k >= 9 cin is zero.  W: bf16
-// [N, conv_gather_k(cin)] with the same k order (conv.weight [N, cin, 3, 3] permuted to [N, 3, 3, cin], zero padded).
-// cin must be a power of two >= 32; out is the NHWC [n, H, W, N] output.  Returns the number of kernels launched.
+// k = 64 kb .. 64 kb + 63 (part of a tap, or parts of several taps when cin is not a multiple of 64), and k >= 9 cin
+// is zero.  W: bf16 [N, conv_gather_k(cin)] with the same k order (conv.weight [N, cin, 3, 3] permuted to
+// [N, 3, 3, cin], zero padded).  cin and N must be multiples of 8 (the ResNets' 40 ... 768); out is the NHWC
+// [n, H, W, N] output.  Returns the number of kernels launched.
 struct ConvGather {
     const __nv_bfloat16* act = nullptr;
     int n = 0, H = 0, W = 0, cin = 0;

@@ -299,8 +299,8 @@ void check_vision(const b200_model_desc& d, VisionKind kind) {
         for (int s = 0; s < 4; ++s)
             MB_CHECK_ARG(d.resnet_layers[s] > 0 && d.resnet_layers[s] <= 64, "resnet_layers[%d] = %d out of range", s,
                          d.resnet_layers[s]);
-        // the stem's 3 x 3 convs gather width / 2 channels: a power of two >= 32
-        MB_CHECK_ARG(wd >= 64 && wd <= 128 && (wd & (wd - 1)) == 0, "resnet_width %d must be 64 or 128", wd);
+        // the stem's 3 x 3 convs gather width / 2 channels and write width / 2 columns: a multiple of 8
+        MB_CHECK_ARG(wd >= 64 && wd <= 128 && wd % 16 == 0, "resnet_width %d must be a multiple of 16 in [64, 128]", wd);
         MB_CHECK_ARG(S > 0 && S % 32 == 0 && S <= 512, "resnet_image_size %d must be a multiple of 32, <= 512", S);
         MB_CHECK_ARG(d.resnet_heads * 64 == 32 * wd, "attention pool: head_dim must be 64 (%d channels, %d heads)",
                      32 * wd, d.resnet_heads);

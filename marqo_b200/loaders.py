@@ -11,6 +11,9 @@ surface on top of the C ABI:
   B200HuggingFace <-> HuggingFaceModel (src/marqo/core/inference/embedding_models/hugging_face_model.py:172-214)
   B200HuggingFaceStella <-> HuggingFaceStellaModel (hugging_face_stella_model.py): B200HuggingFace over the GTE
                         runtime, refusing properties without trustRemoteCode
+  B200Clip        <-> CLIP             (src/marqo/s2_inference/clip_utils.py:295-492): B200OpenCLIP over OpenAI's
+                                        checkpoints, whose arch it reads from a custom checkpoint's shapes
+  B200Fp16Clip    <-> FP16_CLIP        (clip_utils.py:495-518): B200Clip returning float16 vectors
 
 Weights: `model_properties["weights"]` is a state dict (checkpoint names) or a path to one; `"random_init": seed`
 builds seeded random weights (benchmarks / self-test).  Tokenisers, in order of preference:
@@ -21,12 +24,13 @@ CLIP loader `open_clip.get_tokenizer` — both need files that only exist where 
 """
 from __future__ import annotations
 
+import os
 from typing import Callable, Dict, List, Optional, Union
 
 import numpy as np
 
 from . import model_registry, weights as weights_mod
-from .errors import InvalidModelPropertiesError, ModelLoadError, VectoriseError
+from .errors import InternalError, InvalidModelPropertiesError, ModelLoadError, VectoriseError
 from .s2_inference import Modality, UnidentifiedImageError, _is_image, _is_tensor, _validate_device
 
 
@@ -78,6 +82,11 @@ class B200OpenCLIP:
         self.preprocess_config = None
 
     def load(self) -> None:
+        self._load(None)
+
+    def _load(self, state_dict: Optional[Dict[str, np.ndarray]]) -> None:
+        """load(), with the weights already read when state_dict is given: the Encoder takes them, and nothing keeps
+        the host copy once it is built."""
         from .engine import Encoder
         props = self.model_properties
         arch = props.get("arch")
@@ -93,7 +102,8 @@ class B200OpenCLIP:
         # CLIP; "clip_eva" (EVA02_MODELS): EVA02 CLIP; otherwise open_clip CLIP; all four shortest side -> S + centre
         # crop (unless the arch asks for the squash)
         kind = arch.get("kind", "clip")
-        self.model = Encoder(kind, arch, _resolve_weights(props, arch, kind), device=_validate_device(self.device),
+        weights = state_dict if state_dict is not None else _resolve_weights(props, arch, kind)
+        self.model = Encoder(kind, arch, weights, device=_validate_device(self.device),
                              max_batch=int(props.get("max_batch", 256)))
         # SigLIP's SentencePiece tokenizer is not restated here: its text needs model_properties["tokenizer"]
         self.tokenizer = props.get("tokenizer") or (None if kind == "siglip" else self._default_tokenizer())
@@ -421,10 +431,97 @@ class B200HuggingFaceStella(B200HuggingFace):
         super().__init__(device=device, model_properties=model_properties, model_auth=model_auth)
 
 
+WIDE_RESNET_MAX_BATCH = 64   # B200Clip's default max_batch for ResNets wider than 64 (RN50x4, RN50x16, RN50x64)
+
+
+class B200Clip(B200OpenCLIP):
+    """The reference's `clip` loader type (model_registry.OPENAI_CLIP_MODELS: "ViT-B/32", "RN50", ...).  The networks
+    are the open_clip */openai ones, run by the same encoders; what differs is the loader's own behaviour:
+      - construction without a device raises InternalError, not ModelLoadError (clip_utils.py:305-306);
+      - a custom model names its checkpoint by `localpath` (or the engine's own `weights`); `url` and
+        `model_location` are refused with ModelLoadError, as downloading is Marqo's job, and more than one of the three
+        with InvalidModelPropertiesError (clip_utils.py:360-364);
+      - without an `arch` block the arch is read from the checkpoint's shapes (model_registry.openai_clip_arch), as
+        clip.load builds the model from its state dict, so any OpenAI-format checkpoint (RN50x4 too) is served;
+      - the tokenizer is clip.tokenize(truncate=True): the CLIP BPE at context 77 with EOT forced into the last slot,
+        from `merges_file`, else the `clip` package's own when it is importable."""
+
+    def __init__(self, device: Optional[str] = None, model_properties: Optional[dict] = None, model_auth=None):
+        if not device:
+            raise InternalError("`device` is required for loading CLIP models!")
+        super().__init__(device=device, model_properties=model_properties, model_auth=model_auth)
+
+    def load(self) -> None:
+        props = self.model_properties
+        given = [k for k in ("localpath", "url", "model_location") if props.get(k)]
+        if len(given) > 1:
+            raise InvalidModelPropertiesError(
+                "Only one of `url`, `localpath` or `model_location` can be specified in model_properties. Please "
+                "ensure that only one of these is specified in model_properties and retry.")
+        if given and given[0] != "localpath":
+            raise ModelLoadError(f"model_properties[{given[0]!r}]: downloading the checkpoint is Marqo's job; pass "
+                                 "the downloaded file as `localpath`")
+        if given:
+            path = props["localpath"]
+            if not os.path.isfile(path):
+                raise InvalidModelPropertiesError(f"Marqo can not load the custom clip model. The provided model path "
+                                                  f"`{path}` is not a local file.")
+            props = dict(props, weights=path)
+        sd = None   # the checkpoint, when it has to be read for its arch; handed to the Encoder, never stored
+        if props.get("arch") is None and props.get("weights") is not None:
+            sd = props["weights"]
+            if isinstance(sd, (str, bytes)) or hasattr(sd, "__fspath__"):
+                sd = weights_mod.load_state_dict(sd)
+            arch = model_registry.openai_clip_arch(sd)
+            if props.get("dimensions") is not None and int(props["dimensions"]) != arch["embed_dim"]:
+                raise InvalidModelPropertiesError(
+                    f"model_properties declares dimensions {props['dimensions']}, but the checkpoint's "
+                    f"text_projection gives embeddings of {arch['embed_dim']}")
+            props = dict(props, arch=arch)
+        r = (props.get("arch") or {}).get("resnet")
+        if r is not None and r["width"] > 64 and props.get("max_batch") is None:
+            # the wide ResNets' four activation buffers hold max_batch x (S/2)^2 x width bf16 values each: 7.1 MB
+            # (RN50x16) and 12.8 MB (RN50x64) per image, 7.2 and 13 GB at the usual 256 images; at 64 images the
+            # models hold 2.2 and 4.2 GB of device memory in all and every trunk GEMM still has >= 9216 rows
+            # (DESIGN.md §6)
+            props = dict(props, max_batch=WIDE_RESNET_MAX_BATCH)
+        self.model_properties = props
+        self._load(sd)
+
+    def _default_tokenizer(self):
+        if self.model_properties.get("merges_file"):
+            return super()._default_tokenizer()
+        try:
+            import clip  # type: ignore
+        except Exception:
+            return None  # encode_text raises a clear error if text arrives without a tokenizer
+        return lambda texts: clip.tokenize(texts, truncate=True)
+
+
+class B200Fp16Clip(B200Clip):
+    """The reference's `fp16_clip` loader type ("fp16/ViT-B/32", ...).  On CUDA the reference runs the model in fp16
+    and returns float16 arrays (clip_utils.py:393-397, 512-518); this loader runs the same encoder as the fp32 name and
+    returns its vectors rounded to float16 (encode_to_device: the rounded values, as fp32 for the row store).
+    `fp16_clip` is not a preprocess-image type (constants.py:31), so Marqo hands its images over undecoded."""
+
+    def encode_image(self, images, image_download_headers: Optional[Dict] = None, normalize=True) -> np.ndarray:
+        return super().encode_image(images, image_download_headers=image_download_headers,
+                                    normalize=normalize).astype(np.float16)
+
+    def encode_text(self, sentence: Union[str, List[str]], normalize=True) -> np.ndarray:
+        return super().encode_text(sentence, normalize=normalize).astype(np.float16)
+
+    def encode_to_device(self, inputs, default: str = 'text', normalize=True, sub_batch: int = 256, **kwargs):
+        out = super().encode_to_device(inputs, default=default, normalize=normalize, sub_batch=sub_batch, **kwargs)
+        return out.half().float()
+
+
 LOADERS = {
     model_registry.TYPE_OPEN_CLIP: B200OpenCLIP,
     model_registry.TYPE_HF: B200HuggingFace,
     model_registry.TYPE_HF_STELLA: B200HuggingFaceStella,
+    model_registry.TYPE_CLIP: B200Clip,
+    model_registry.TYPE_FP16_CLIP: B200Fp16Clip,
 }
 
 
@@ -437,7 +534,7 @@ def get_model_loader(model_name: Optional[str], model_properties: dict):
 
 
 def register_with_marqo() -> None:
-    """Install the three loader types into a live Marqo process (see INTEGRATION.md)."""
+    """Install the engine's loader types into a live Marqo process (see INTEGRATION.md)."""
     from marqo.s2_inference import s2_inference as marqo_s2  # type: ignore
     marqo_s2.MODEL_PROPERTIES['loaders'].update(LOADERS)
     marqo_s2.MODEL_PROPERTIES['models'].update(model_registry.served_models())

@@ -160,7 +160,22 @@ causal except that the CLS row keeps key 0 and each key k with ids[k - 1] != 0 (
 pools that row through ln_final and text_projection [W, embed].  encode_image / encode_text F.normalize their output
 (normalize=True is their default and Marqo does not pass it), so the vectors are unit whatever Marqo's normalize says.
 The text decoder and logit_scale are not used.  The entries carry no model_size: Marqo derives 1 GB (B-32, from the
-open_clip type) and 1.5 GB (L-14, from the "vit-l-14" name rule)."""
+open_clip type) and 1.5 GB (L-14, from the "vit-l-14" name rule).
+
+The OpenAI CLIP entries of the reference's `clip` and `fp16_clip` loaders (model_registry.py:16-73, 2069-2091) live in
+OPENAI_CLIP_MODELS, field for field, under the loader types "b200_clip" and "b200_fp16_clip", plus an arch block:
+    ViT-B/32, ViT-B/16, ViT-L/14      the arch of open_clip/ViT-{B-32,B-16,L-14}/openai (QuickGELU)
+    ViT-L/14@336px                    ViT-L/14 at image 336 (577 tokens)
+    RN50, RN101                       the arch of open_clip/RN50/openai, RN101/openai
+    fp16/ViT-B/32, -B/16, -L/14       the arch of the fp32 name
+The wide ResNets' archs (OpenAI's build_model shapes; open_clip RN50x*.json, verify) are in WIDE_RESNET_ARCHS:
+    RN50x4    [4, 6, 10, 6] blocks of width 80 at 288 px; embed 640, text 640 wide, 10 heads, 12 layers
+    RN50x16   [6, 8, 18, 8] blocks of width 96 at 384 px; embed 768, text 768 wide, 12 heads, 12 layers
+    RN50x64   [3, 15, 36, 10] blocks of width 128 at 448 px; embed 1024, text 1024 wide, 16 heads, 12 layers
+each with an attention pool of width / 2 heads of 64.  Their names are not registered (DESIGN.md §6): the `clip`
+loader serves them from a custom checkpoint, whose arch openai_clip_arch reads from its shapes.  No entry carries a
+model_size: Marqo derives 1 GB from the clip type, the 0.66 GB default for fp16_clip, and 1.5 GB for the ViT-L/14
+names."""
 from __future__ import annotations
 
 import copy
@@ -172,12 +187,14 @@ OPENAI_STD = (0.26862954, 0.26130258, 0.27577711)
 TYPE_OPEN_CLIP = "b200_open_clip"
 TYPE_HF = "b200_hf"
 TYPE_HF_STELLA = "b200_hf_stella"
+TYPE_CLIP = "b200_clip"
+TYPE_FP16_CLIP = "b200_fp16_clip"
 
 
-def _clip_arch(embed, vw, vl, vh, patch, tw, tl, th, act="gelu"):
+def _clip_arch(embed, vw, vl, vh, patch, tw, tl, th, act="gelu", image_size=224):
     return {
         "embed_dim": embed, "act": act, "mean": OPENAI_MEAN, "std": OPENAI_STD,
-        "vision": {"width": vw, "layers": vl, "heads": vh, "mlp": 4 * vw, "patch": patch, "image_size": 224},
+        "vision": {"width": vw, "layers": vl, "heads": vh, "mlp": 4 * vw, "patch": patch, "image_size": image_size},
         "text": {"width": tw, "layers": tl, "heads": th, "mlp": 4 * tw, "ctx": 77, "vocab": 49408},
     }
 
@@ -340,11 +357,14 @@ def _xlmr_models() -> Dict[str, dict]:
 XLMR_MODELS: Dict[str, dict] = _xlmr_models()
 
 
-def _resnet_arch(layers: list, embed: int, act: str) -> dict:
-    """OpenAI ResNet CLIP (module docstring, verify)."""
+def _resnet_arch(layers: list, embed: int, act: str, width: int = 64, image_size: int = 224,
+                 text: tuple = (512, 12, 8)) -> dict:
+    """OpenAI ResNet CLIP (module docstring, verify): the attention pool has width / 2 heads of 64 over 32 width
+    channels; text is the CLIP text tower's (width, layers, heads)."""
+    tw, tl, th = text
     return {"kind": "clip_resnet", "embed_dim": embed, "act": act, "mean": OPENAI_MEAN, "std": OPENAI_STD,
-            "width": 512, "layers": 12, "heads": 8, "mlp": 2048, "ctx": 77, "vocab": 49408,
-            "resnet": {"layers": list(layers), "width": 64, "heads": 32, "image_size": 224}}
+            "width": tw, "layers": tl, "heads": th, "mlp": 4 * tw, "ctx": 77, "vocab": 49408,
+            "resnet": {"layers": list(layers), "width": width, "heads": width // 2, "image_size": image_size}}
 
 
 def _resnet_models() -> Dict[str, dict]:
@@ -480,10 +500,84 @@ def _coca_models() -> Dict[str, dict]:
 COCA_MODELS: Dict[str, dict] = _coca_models()
 
 
+# The wide OpenAI ResNets by their `clip` names (module docstring): served through a custom checkpoint, whose arch
+# openai_clip_arch reads, and by these blocks in tests and tools; their names are not registered.
+WIDE_RESNET_ARCHS: Dict[str, dict] = {
+    "RN50x4": _resnet_arch([4, 6, 10, 6], 640, "quickgelu", 80, 288, (640, 12, 10)),
+    "RN50x16": _resnet_arch([6, 8, 18, 8], 768, "quickgelu", 96, 384, (768, 12, 12)),
+    "RN50x64": _resnet_arch([3, 15, 36, 10], 1024, "quickgelu", 128, 448, (1024, 12, 16)),
+}
+
+_OPENAI_NOTE_FP16 = "The faster version (fp16, load from `cuda`) of openai clip model"
+
+
+def _openai_clip_models() -> Dict[str, dict]:
+    """The reference's `clip` and `fp16_clip` entries (module docstring), field for field, plus their arch."""
+    m: Dict[str, dict] = {}
+    q = "quickgelu"
+    archs = {
+        "RN50": (1024, "CLIP resnet50", _resnet_arch([3, 4, 6, 3], 1024, q)),
+        "RN101": (512, "CLIP resnet101", _resnet_arch([3, 4, 23, 3], 512, q)),
+        "ViT-B/32": (512, "CLIP ViT-B/32", _clip_arch(**_VIT_B_32, act=q)),
+        "ViT-B/16": (512, "CLIP ViT-B/16", _clip_arch(**_VIT_B_16, act=q)),
+        "ViT-L/14": (768, "CLIP ViT-L/14", _clip_arch(**_VIT_L_14, act=q)),
+        "ViT-L/14@336px": (768, "CLIP ViT-L/14@336px", _clip_arch(**_VIT_L_14, act=q, image_size=336)),
+    }
+    for name, (dims, notes, arch) in archs.items():
+        m[name] = {"name": name, "dimensions": dims, "notes": notes, "type": TYPE_CLIP, "arch": arch}
+    for name in ("ViT-L/14", "ViT-B/32", "ViT-B/16"):
+        fp16 = f"fp16/{name}"
+        m[fp16] = {"name": fp16, "dimensions": m[name]["dimensions"], "type": TYPE_FP16_CLIP, "notes": _OPENAI_NOTE_FP16,
+                   "arch": copy.deepcopy(m[name]["arch"])}
+    return m
+
+
+OPENAI_CLIP_MODELS: Dict[str, dict] = _openai_clip_models()
+
+
+def _count(sd: dict, prefix: str) -> int:
+    """The number of distinct indices i among the keys prefix + "i.*"."""
+    return len({k[len(prefix):].split(".")[0] for k in sd if k.startswith(prefix)})
+
+
+def openai_clip_arch(sd: dict) -> dict:
+    """The arch block of an OpenAI-format CLIP state dict (the names of OpenAI's released checkpoints), read from its
+    shapes by the rules of OpenAI's clip.model.build_model: the ViT's width and patch from visual.conv1 and its grid
+    from visual.positional_embedding; the ResNet's width from visual.layer1.0.conv1, its block counts from the
+    visual.layer{1..4}.* names and its image size from visual.attnpool.positional_embedding (the trunk downsamples
+    32 times); the text tower from text_projection, positional_embedding, token_embedding and ln_final.  Heads are
+    width / 64 in both towers (width / 2 in the attention pool); every OpenAI model is QuickGELU.  A state dict
+    without one of these names (an open_clip timm or HF checkpoint, say) raises InvalidModelPropertiesError naming it."""
+    from .errors import InvalidModelPropertiesError
+
+    def shape(k):
+        if k not in sd:
+            raise InvalidModelPropertiesError(f"not an OpenAI-format CLIP checkpoint: it has no `{k}`, which the arch "
+                                              f"of a custom `clip` model is read from")
+        return tuple(sd[k].shape)
+
+    embed = shape("text_projection")[1]
+    tw = shape("ln_final.weight")[0]
+    text = (tw, _count(sd, "transformer.resblocks."), tw // 64)
+    if "visual.proj" in sd:
+        vw, _, patch, _ = shape("visual.conv1.weight")
+        grid = round((shape("visual.positional_embedding")[0] - 1) ** 0.5)
+        arch = _clip_arch(embed, vw, _count(sd, "visual.transformer.resblocks."), vw // 64, patch, *text,
+                          act="quickgelu", image_size=patch * grid)
+        arch["text"].update(ctx=shape("positional_embedding")[0], vocab=shape("token_embedding.weight")[0])
+    else:
+        layers = [_count(sd, f"visual.layer{b}.") for b in (1, 2, 3, 4)]
+        width = shape("visual.layer1.0.conv1.weight")[0]
+        grid = round((shape("visual.attnpool.positional_embedding")[0] - 1) ** 0.5)
+        arch = _resnet_arch(layers, embed, "quickgelu", width, 32 * grid, text)
+        arch.update(ctx=shape("positional_embedding")[0], vocab=shape("token_embedding.weight")[0])
+    return arch
+
+
 def find_model(model_name: str) -> Optional[dict]:
     """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
     for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS, CONVNEXT_MODELS, BIG_VIT_MODELS,
-                  EVA02_MODELS, GTE_MODELS, COCA_MODELS):
+                  EVA02_MODELS, GTE_MODELS, COCA_MODELS, OPENAI_CLIP_MODELS):
         entry = table.get(model_name)
         if entry is not None:
             return entry
@@ -500,9 +594,11 @@ def all_models() -> Dict[str, dict]:
     block, whose layer shapes tests/test_eva02_kernels_gpu.py runs.  GTE_MODELS is in: its encoder is 1024 wide with a
     4096 hidden size, as the BERT-large models; its fused up | gate GEMM runs in tests/test_gte_kernels_gpu.py.
     COCA_MODELS is in: its towers are the ViT-B-32 and ViT-L-14 CLIP shapes; its pooler GEMMs and attention run in
-    tests/test_coca_kernels_gpu.py.  served_models() has every served entry; find_model looks in every table."""
+    tests/test_coca_kernels_gpu.py.  OPENAI_CLIP_MODELS is in: its text towers are 512, 768 and 1024 wide, and its
+    one new layer shape (ViT-L/14@336px's vision layers at 577 tokens) runs in tests/test_layers_gpu.py.
+    served_models() has every served entry; find_model looks in every table."""
     return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS, **RESNET_MODELS, **EVA02_MODELS, **GTE_MODELS,
-            **COCA_MODELS}
+            **COCA_MODELS, **OPENAI_CLIP_MODELS}
 
 
 def served_models() -> Dict[str, dict]:

@@ -86,8 +86,10 @@ def _create_model_cache_key(model_name: str, device: str, model_properties: dict
 
 
 def validate_model_properties(model_name: str, model_properties: Optional[dict]) -> dict:
-    """s2_inference.py:340-407 reduced to the three loader types this engine serves: explicit properties must carry
-    `dimensions` and a known `type`; otherwise the name is looked up in the registry."""
+    """s2_inference.py:340-407 reduced to the loader types this engine serves: explicit properties must carry
+    `dimensions` and a known `type`; otherwise the name is looked up in the registry.  A custom `clip` model with a
+    checkpoint (`localpath`, `url`, `model_location` or `weights`) and no `arch` keeps it so: its loader reads the
+    arch from the checkpoint's shapes (model_registry.openai_clip_arch), as clip.load builds the model from them."""
     if model_properties is None:
         return model_registry.get_model_properties(model_name)
     if not isinstance(model_properties, dict):
@@ -97,12 +99,15 @@ def validate_model_properties(model_name: str, model_properties: Optional[dict])
         raise InvalidModelPropertiesError(f"model_properties for {model_name} is missing the required key `dimensions`")
     mtype = props.get("type")
     alias = {"open_clip": model_registry.TYPE_OPEN_CLIP, "hf": model_registry.TYPE_HF,
-             "hf_stella": model_registry.TYPE_HF_STELLA}
+             "hf_stella": model_registry.TYPE_HF_STELLA, "clip": model_registry.TYPE_CLIP,
+             "fp16_clip": model_registry.TYPE_FP16_CLIP}
     props["type"] = alias.get(mtype, mtype)
     if props["type"] not in alias.values():
-        raise InvalidModelPropertiesError(
-            f"model type `{mtype}` is not served by the H100 engine (supported: open_clip, hf, hf_stella)")
-    if "arch" not in props:
+        raise InvalidModelPropertiesError(f"model type `{mtype}` is not served by the H100 engine (supported: "
+                                          f"open_clip, hf, hf_stella, clip, fp16_clip)")
+    custom_clip = props["type"] == model_registry.TYPE_CLIP and any(
+        props.get(k) is not None for k in ("localpath", "url", "model_location", "weights"))
+    if "arch" not in props and not custom_clip:
         base = model_registry.find_model(model_name)
         if base is None:
             served = model_registry.served_models()
@@ -160,7 +165,8 @@ def get_model_size(model_name: str, model_properties: dict):
 def _reference_type_name(t):
     """this engine's loader types carry a b200_ prefix in the registry; sizes are declared per reference type"""
     return {model_registry.TYPE_OPEN_CLIP: "open_clip", model_registry.TYPE_HF: "hf",
-            model_registry.TYPE_HF_STELLA: "hf_stella"}.get(t, t)
+            model_registry.TYPE_HF_STELLA: "hf_stella", model_registry.TYPE_CLIP: "clip",
+            model_registry.TYPE_FP16_CLIP: "fp16_clip"}.get(t, t)
 
 
 def _check_memory_threshold_for_model(device: str, model_size) -> bool:
@@ -260,7 +266,8 @@ def clear_loaded_models() -> None:
 
 
 def is_preprocess_image_model(model_properties: dict = None) -> bool:
-    """s2_inference.py:180-185 (constants.PREPROCESS_IMAGE_MODEL_LIST = CLIP-type models; here: the open_clip loader)."""
+    """s2_inference.py:180-185 (constants.PREPROCESS_IMAGE_MODEL_LIST = [clip, open_clip]: the open_clip and clip
+    loaders; not fp16_clip)."""
     return _reference_type_name((model_properties or {}).get("type")) in ("open_clip", "clip")
 
 

@@ -13,7 +13,7 @@ import numpy as np
 
 
 def load_state_dict(path: str) -> Dict[str, np.ndarray]:
-    """.npz, torch .pt/.bin/.pth or .safetensors -> {name: fp32 ndarray}."""
+    """.npz, torch .pt/.bin/.pth (a state dict or a TorchScript archive) or .safetensors -> {name: fp32 ndarray}."""
     p = str(path)
     if p.endswith(".npz"):
         with np.load(p) as z:
@@ -22,7 +22,12 @@ def load_state_dict(path: str) -> Dict[str, np.ndarray]:
         from safetensors.numpy import load_file  # optional dependency
         return {k: np.asarray(v, dtype=np.float32) for k, v in load_file(p).items()}
     import torch
-    sd = torch.load(p, map_location="cpu", weights_only=True)
+    if _is_torchscript(p):
+        # OpenAI's released CLIP checkpoints (and open_clip's */openai files) are TorchScript archives, which
+        # torch.load(weights_only=True) refuses; the scripted module's state dict has the names clip.load reads
+        sd = torch.jit.load(p, map_location="cpu").state_dict()
+    else:
+        sd = torch.load(p, map_location="cpu", weights_only=True)
     if isinstance(sd, dict) and "state_dict" in sd and isinstance(sd["state_dict"], dict):
         sd = sd["state_dict"]
     out = {}
@@ -30,6 +35,16 @@ def load_state_dict(path: str) -> Dict[str, np.ndarray]:
         if hasattr(v, "is_floating_point") and v.is_floating_point():
             out[k[len("module."):] if k.startswith("module.") else k] = v.float().numpy()
     return out
+
+
+def _is_torchscript(path: str) -> bool:
+    """A torch.jit.save archive: a zip whose records include the scripted code's constants.pkl (a plain torch.save
+    zip has data.pkl only)."""
+    import zipfile
+    if not zipfile.is_zipfile(path):
+        return False
+    with zipfile.ZipFile(path) as z:
+        return any(n.endswith("/constants.pkl") for n in z.namelist())
 
 
 def strip_hf_prefix(sd: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
