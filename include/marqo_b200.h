@@ -356,6 +356,13 @@ typedef struct b200_model_desc {
      * by its norm again when normalize is set.  A CLS text tower needs head_dim 64 and ctx <= 127. */
     int32_t attn_pool_heads;      /* 8; 0: the class-token head */
     int32_t text_embed_cls;       /* 1: CoCa's appended CLS row */
+    /* M-CLIP's text tower (pt_multilingual_clip MultilingualCLIP, verify), arch B200_ARCH_BERT or B200_ARCH_XLMR with
+     * pool B200_POOL_MEAN.  text_proj_dim > 0 replaces the pooling head: the masked mean of the last hidden state over
+     * each row's tokens, then LinearTransformation (nn.Linear [text_proj_dim, width] with bias), then, when normalize is
+     * set, the division by the L2 norm without an epsilon (the reference's CLIP.normalize).  embed_dim must equal
+     * text_proj_dim.  Weights: the encoder's names under an optional "transformer." prefix (dropped), and
+     * LinearTransformation.weight [E, width] and LinearTransformation.bias [E].  0: the usual head. */
+    int32_t text_proj_dim;
 } b200_model_desc;
 
 int b200_model_create(int device, const b200_model_desc* desc, b200_model** out);
@@ -658,6 +665,11 @@ int b200_debug_clip_head(int device, const float* x, int S, const int32_t* row_i
  * normalize.  out fp32 [n, w]. */
 int b200_debug_bert_head(int device, const float* x, const int32_t* kv_len, int n, int S, int w, int pool, int normalize,
                          float* out, void* stream);
+/* M-CLIP's text head over x fp32 [n*S, w]: the mean of the first kv_len[b] rows, then @ proj [w, E] (the transposed
+ * LinearTransformation.weight) + bias [E] (NULL: none), divided by its L2 norm if normalize.  out fp32 [n, E].
+ * w a multiple of 4, <= 1024. */
+int b200_debug_text_head(int device, const float* x, const int32_t* kv_len, int n, int S, int w, const float* proj,
+                         const float* bias, int E, int normalize, float* out, void* stream);
 /* out fp32 [n, E] = src / |src| per row if normalize, else src. */
 int b200_debug_l2_rows(int device, const float* src, int n, int E, int normalize, float* out, void* stream);
 /* ResNet stem im2col: exactly one of hwc (uint8 [n,S,S,3], normalised with mean3 / std3, host fp32 [3]) and chw (fp32

@@ -54,7 +54,7 @@ class ModelDesc(C.Structure):
         ("convnext_dims", C.c_int32 * 4), ("convnext_depths", C.c_int32 * 4), ("convnext_image_size", C.c_int32),
         ("convnext_head", C.c_int32), ("resize_squash", C.c_int32), ("eva_rope_ref_grid", C.c_int32),
         ("rope_theta", C.c_float), ("rope_ntk_factor", C.c_float),
-        ("attn_pool_heads", C.c_int32), ("text_embed_cls", C.c_int32),
+        ("attn_pool_heads", C.c_int32), ("text_embed_cls", C.c_int32), ("text_proj_dim", C.c_int32),
     ]
 
 
@@ -149,6 +149,7 @@ _SIGNATURES = {
     "b200_debug_clip_head": (C.c_int, [C.c_int, _P, C.c_int, _P, _P, _P, C.c_float, _P, C.c_int, C.c_int, C.c_int, C.c_int,
                                        _P, _P]),
     "b200_debug_bert_head": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_text_head": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P]),
     "b200_debug_l2_rows": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_stem_im2col": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
     "b200_debug_avgpool2": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),

@@ -429,6 +429,20 @@ int b200_debug_bert_head(int device, const float* x, const int32_t* kv_len, int 
     });
 }
 
+int b200_debug_text_head(int device, const float* x, const int32_t* kv_len, int n, int S, int w, const float* proj,
+                         const float* bias, int E, int normalize, float* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && kv_len && proj && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && S > 0 && w > 0 && E > 0, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        DeviceBuffer<float> pooled((size_t)n * w);
+        kernels::text_head(x, kv_len, n, S, w, proj, bias, E, normalize, out, pooled.get(), s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
 int b200_debug_l2_rows(int device, const float* src, int n, int E, int normalize, float* out, void* stream) {
     return guarded([&] {
         MB_CHECK_ARG(src && out, "NULL buffer");

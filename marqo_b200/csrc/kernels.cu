@@ -667,8 +667,10 @@ __global__ void __launch_bounds__(256) head_ln_kernel(const float* __restrict__ 
     for (int i = lane; i < w; i += 32) pooled[(long long)b * w + i] = (src[i] - mean) * rstd * gamma[i] + beta[i];
 }
 
-__global__ void __launch_bounds__(256) head_proj_kernel(const float* __restrict__ pooled, const float* __restrict__ proj, int n,
-                                                        int w, int E, float* __restrict__ out) {
+// bias (fp32 [E], NULL: none) is added after the four K-slices are summed
+__global__ void __launch_bounds__(256) head_proj_kernel(const float* __restrict__ pooled, const float* __restrict__ proj,
+                                                        const float* __restrict__ bias, int n, int w, int E,
+                                                        float* __restrict__ out) {
     __shared__ float part[4][HEAD_IMGS][HEAD_COLS];
     extern __shared__ float s_pool[];   // [HEAD_IMGS][w]
     const int b0 = blockIdx.x * HEAD_IMGS;
@@ -700,7 +702,8 @@ __global__ void __launch_bounds__(256) head_proj_kernel(const float* __restrict_
             if (b0 + k < n) {
                 const int c = threadIdx.x & (HEAD_COLS - 1);
                 // fixed order: the result does not depend on scheduling
-                out[(long long)(b0 + k) * E + e] = ((part[0][k][c] + part[1][k][c]) + part[2][k][c]) + part[3][k][c];
+                const float v = ((part[0][k][c] + part[1][k][c]) + part[2][k][c]) + part[3][k][c];
+                out[(long long)(b0 + k) * E + e] = bias ? v + bias[e] : v;
             }
     }
 }
@@ -746,7 +749,7 @@ int clip_head(const float* x, int S, const int32_t* row_in_seq, const float* gam
     head_ln_kernel<<<(n + 7) / 8, 256, 0, s>>>(x, S, row_in_seq, gamma, beta, eps, n, w, pooled_ws);
     MB_CUDA(cudaGetLastError());
     const dim3 grid((n + HEAD_IMGS - 1) / HEAD_IMGS, (E + HEAD_COLS - 1) / HEAD_COLS);
-    head_proj_kernel<<<grid, 256, (size_t)HEAD_IMGS * w * sizeof(float), s>>>(pooled_ws, proj, n, w, E, out);
+    head_proj_kernel<<<grid, 256, (size_t)HEAD_IMGS * w * sizeof(float), s>>>(pooled_ws, proj, nullptr, n, w, E, out);
     MB_CUDA(cudaGetLastError());
     if (unit) {
         head_unit_kernel<<<(n + 7) / 8, 256, 0, s>>>(out, n, E, normalize);
@@ -798,6 +801,21 @@ int bert_head(const float* x, const int32_t* kv_len, int n, int S, int w, int po
     bert_head_kernel<<<n, 256, 0, s>>>(x, kv_len, S, w, pool, normalize, out);
     MB_CUDA(cudaGetLastError());
     return 1;
+}
+
+int text_head(const float* x, const int32_t* kv_len, int n, int S, int w, const float* proj, const float* bias, int E,
+              int normalize, float* out, float* pooled_ws, cudaStream_t s) {
+    if (n <= 0) return 0;
+    if (w > 1024 || w % 4 != 0) fail(B200_ERR_UNSUPPORTED, "text_head: width %d unsupported", w);
+    bert_head_kernel<<<n, 256, 0, s>>>(x, kv_len, S, w, 0, 0, pooled_ws);
+    MB_CUDA(cudaGetLastError());
+    const dim3 grid((n + HEAD_IMGS - 1) / HEAD_IMGS, (E + HEAD_COLS - 1) / HEAD_COLS);
+    head_proj_kernel<<<grid, 256, (size_t)HEAD_IMGS * w * sizeof(float), s>>>(pooled_ws, proj, bias, n, w, E, out);
+    MB_CUDA(cudaGetLastError());
+    if (!normalize) return 2;
+    head_norm_kernel<<<(n + 7) / 8, 256, 0, s>>>(out, n, E);
+    MB_CUDA(cudaGetLastError());
+    return 3;
 }
 
 // ------------------------------------------------------------------------------------------------ conversions

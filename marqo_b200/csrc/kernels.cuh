@@ -85,6 +85,13 @@ int clip_head(const float* x, int S, const int32_t* row_in_seq, const float* gam
 int bert_head(const float* x, const int32_t* kv_len, int n, int S, int w, int pool, int normalize, float* out,
               cudaStream_t s);
 
+// M-CLIP's text head (pt_multilingual_clip MultilingualCLIP.forward, verify): the masked mean over the first kv_len[b]
+// token rows into pooled_ws (fp32 [n, w], bert_head's loop without its normalisation), then pooled @ proj [w, E] + bias
+// (fp32 [E], NULL: none), then, if normalize, the division by the L2 norm without an epsilon (clip_utils.py:400-401).
+// Three kernels with normalize, two without.
+int text_head(const float* x, const int32_t* kv_len, int n, int S, int w, const float* proj, const float* bias, int E,
+              int normalize, float* out, float* pooled_ws, cudaStream_t s);
+
 void f32_to_bf16(const float* src, __nv_bfloat16* dst, long long n, cudaStream_t s);
 // conv1.weight [w, 3*p*p] -> bf16 [w, kpad] zero padded
 void pad_rows_to_bf16(const float* src, int rows, int k, int kpad, __nv_bfloat16* dst, cudaStream_t s);

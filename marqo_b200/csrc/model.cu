@@ -96,7 +96,8 @@ struct TowerW {
     // pos: CLIP positional_embedding [grid^2 + 1, width]; SigLIP pos_embed + the patch conv's bias [grid^2, width].
     // ln_pre is NULL for SigLIP.
     const float *cls = nullptr, *pos = nullptr, *ln_pre_w = nullptr, *ln_pre_b = nullptr;
-    // final LN (ln_post / ln_final / trunk.norm) and CLIP's projection [width, embed]
+    // final LN (ln_post / ln_final / trunk.norm) and CLIP's projection [width, embed] (M-CLIP's text head: its
+    // LinearTransformation transposed, with b_tproj its bias)
     const float *ln_out_w = nullptr, *ln_out_b = nullptr, *proj = nullptr;
     // SigLIP text projection and EVA02's vision head (nn.Linear [embed, width] + bias); SigLIP's vision MAP head and
     // CoCa's attentional pooler
@@ -373,6 +374,9 @@ void check_vision(const b200_model_desc& d, VisionKind kind) {
 }
 
 void check_text(const b200_model_desc& d, const Kinds& k) {
+    MB_CHECK_ARG(d.text_proj_dim >= 0, "text_proj_dim %d must not be negative", d.text_proj_dim);
+    MB_CHECK_ARG(d.text_proj_dim == 0 || d.arch == B200_ARCH_BERT || d.arch == B200_ARCH_XLMR,
+                 "text_proj_dim: only the BERT and XLM-R text towers take a projected head");
     if (k.text == TextKind::NONE) return;
     check_tower(d.text, "text", k.text == TextKind::CLIP || k.text == TextKind::COCA ? 1664 : 1024);
     MB_CHECK_ARG(d.text.ctx > 0 && d.text.vocab > 0, "text.ctx and text.vocab must be positive");
@@ -403,6 +407,13 @@ void check_text(const b200_model_desc& d, const Kinds& k) {
         [[fallthrough]];
     }
     case TextKind::BERT:
+        if (d.text_proj_dim > 0) {
+            // M-CLIP's text head: the masked mean, projected (text_head)
+            MB_CHECK_ARG(d.pool == B200_POOL_MEAN, "text_proj_dim: the projected head pools by the masked mean");
+            MB_CHECK_ARG(d.embed_dim == d.text_proj_dim, "embed_dim %d must equal text_proj_dim %d", d.embed_dim,
+                         d.text_proj_dim);
+            break;
+        }
         MB_CHECK_ARG(d.embed_dim == d.text.width, "BERT / MPNet / XLM-R embed_dim must equal width");
         break;
     case TextKind::GTE:
@@ -1065,6 +1076,16 @@ void build_text(b200_model* m) {
         break;
     }
     }
+    if (m->desc.text_proj_dim > 0) {
+        // M-CLIP's LinearTransformation (nn.Linear [E, w] with bias), transposed to the [w, E] text_head reads
+        const std::vector<float> lin = to_host(param(m, "LinearTransformation.weight", E * w), (size_t)(E * w));
+        std::vector<float> proj((size_t)(E * w));
+        for (long long e = 0; e < E; ++e)
+            for (long long i = 0; i < w; ++i) proj[(size_t)(i * E + e)] = lin[(size_t)(e * w + i)];
+        T.proj = upload_derived(m, proj);
+        m->raw.erase("LinearTransformation.weight");
+        T.b_tproj = param(m, "LinearTransformation.bias", E);
+    }
 }
 
 struct Counter {
@@ -1407,7 +1428,11 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
             c.n += kernels::roberta_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, T.eps, n, S,
                                              w, T.d.vocab, m->desc.pad_id, x, m->h.get(), aux, m->stream);
         run_layers(m, c, T, n, S, attention::MASK_KEYLEN);
-        c.n += kernels::bert_head(x, aux, n, S, w, m->desc.pool, normalize, d_out, m->stream);
+        if (T.proj)   // M-CLIP: the masked mean, projected
+            c.n += kernels::text_head(x, aux, n, S, w, T.proj, T.b_tproj, E, normalize, d_out, m->pooled.get(),
+                                      m->stream);
+        else
+            c.n += kernels::bert_head(x, aux, n, S, w, m->desc.pool, normalize, d_out, m->stream);
         break;
     }
 }
@@ -1648,6 +1673,8 @@ int b200_model_load_tensor(b200_model* m, const char* name, const float* data, i
         if (xlmr && key.compare(0, 8, "roberta.") == 0) key.erase(0, 8);
         // and NewModel checkpoints saved from a task head under "new."
         if (m->kind.text == TextKind::GTE && key.compare(0, 4, "new.") == 0) key.erase(0, 4);
+        // and M-CLIP checkpoints (MultilingualCLIP) under "transformer.", beside their LinearTransformation
+        if (m->desc.text_proj_dim > 0 && key.compare(0, 12, "transformer.") == 0) key.erase(0, 12);
         m->raw[key] = std::move(b);
     });
 }

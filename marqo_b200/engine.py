@@ -303,9 +303,10 @@ class Encoder:
     CLIP keys with eva{width, layers, heads, mlp (the SwiGLU hidden size), patch, image_size, ln_eps, rope_ref_grid}
     (None: no image tower) in place of resnet;  BERT: width, layers, heads, mlp, vocab,
     max_pos, type_vocab,
-    pool ("mean"|"cls");  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
+    pool ("mean"|"cls"), proj_dim (optional: M-CLIP's projected text head of that many outputs, whose weights are
+    LinearTransformation.weight [proj_dim, width] and .bias);  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
     max_pos - pad_id - 1 tokens), pad_id, ln_eps, rel_buckets, rel_max_distance, pool;  XLM-R: width, layers, heads,
-    mlp, vocab, max_pos (as MPNet), pad_id, ln_eps, pool;  GTE (NewModel: the Stella embedders): width, layers, heads,
+    mlp, vocab, max_pos (as MPNet), pad_id, ln_eps, pool, proj_dim (as BERT);  GTE (NewModel: the Stella embedders): width, layers, heads,
     mlp (the GeGLU hidden size), vocab, type_vocab, ctx, ln_eps, rope_theta, rope_ntk_factor, pool.  `weights` maps
     checkpoint parameter names (open_clip state_dict names / HF BertModel / MPNetModel / XLMRobertaModel / NewModel
     names) to fp32 arrays or torch tensors.
@@ -394,7 +395,8 @@ class Encoder:
             self.image_size = int(ev["image_size"]) if ev else 0
         elif arch == "bert":
             d.arch = N.ARCH_BERT
-            d.embed_dim = int(config["width"])
+            d.embed_dim = int(config.get("proj_dim") or config["width"])
+            d.text_proj_dim = int(config.get("proj_dim") or 0)
             d.pool = N.POOL_CLS if config.get("pool", "mean") == "cls" else N.POOL_MEAN
             d.type_vocab = int(config.get("type_vocab", 2))
             d.text = N.TowerDesc(config["width"], config["layers"], config["heads"], config["mlp"],
@@ -402,7 +404,8 @@ class Encoder:
             self.image_size = 0
         elif arch == "xlmr":
             d.arch = N.ARCH_XLMR
-            d.embed_dim = int(config["width"])
+            d.embed_dim = int(config.get("proj_dim") or config["width"])
+            d.text_proj_dim = int(config.get("proj_dim") or 0)
             d.pool = N.POOL_CLS if config.get("pool", "mean") == "cls" else N.POOL_MEAN
             d.pad_id = int(config.get("pad_id", 1))
             d.layer_norm_eps = float(config["ln_eps"])
@@ -963,6 +966,26 @@ def debug_bert_head(x, S: int, kv_len, pool: int = N.POOL_MEAN, normalize: bool 
     out = d.empty((n, w))
     N.check(N.load().b200_debug_bert_head(device, _dptr(dx), _dptr(dkl), n, S, w, pool, int(normalize), _dptr(out),
                                           d.stream))
+    return _host(out)
+
+
+def debug_text_head(x, S: int, kv_len, proj, bias=None, normalize: bool = True, device: int = 0) -> np.ndarray:
+    """M-CLIP's text head over x fp32 [n*S, w]: the mean of the first kv_len[b] rows @ proj [w, E] + bias [E] (None:
+    none), divided by its L2 norm if normalize -> fp32 [n, E]."""
+    xa, pj = _as(x, np.float32), _as(proj, np.float32)
+    w, E = pj.shape
+    if xa.ndim != 2 or xa.shape[1] != w or xa.shape[0] % S != 0:
+        raise ValueError(f"expected x [n * {S}, {w}], got {xa.shape}")
+    n = xa.shape[0] // S
+    kl = _as(kv_len, np.int32)
+    if kl.shape != (n,):
+        raise ValueError(f"expected kv_len [{n}], got {kl.shape}")
+    b = None if bias is None else _as(bias, np.float32)
+    d = _Staging(device)
+    dx, dkl, dp, dbias = d.up(xa), d.up(kl, "int32"), d.up(pj), d.up(b)
+    out = d.empty((n, E))
+    N.check(N.load().b200_debug_text_head(device, _dptr(dx), _dptr(dkl), n, S, w, _dptr(dp), _dptr(dbias), E,
+                                          int(normalize), _dptr(out), d.stream))
     return _host(out)
 
 

@@ -14,6 +14,8 @@ surface on top of the C ABI:
   B200Clip        <-> CLIP             (src/marqo/s2_inference/clip_utils.py:295-492): B200OpenCLIP over OpenAI's
                                         checkpoints, whose arch it reads from a custom checkpoint's shapes
   B200Fp16Clip    <-> FP16_CLIP        (clip_utils.py:495-518): B200Clip returning float16 vectors
+  B200MultilingualClip <-> MULTILINGUAL_CLIP (clip_utils.py:521-596): B200Clip's image tower beside M-CLIP's XLM-R or
+                                        LaBSE text tower with its projected head
 
 Weights: `model_properties["weights"]` is a state dict (checkpoint names) or a path to one; `"random_init": seed`
 builds seeded random weights (benchmarks / self-test).  Tokenisers, in order of preference:
@@ -516,12 +518,134 @@ class B200Fp16Clip(B200Clip):
         return out.half().float()
 
 
+class B200MultilingualClip(B200OpenCLIP):
+    """The reference's `multilingual_clip` loader type (model_registry.MULTILINGUAL_CLIP_MODELS).  Two Encoders:
+      - the image tower, exactly the one B200Clip builds for the entry's `visual` name (clip.load's visual(x));
+      - the text tower, M-CLIP's XLM-R or BERT encoder with its masked-mean LinearTransformation head, run over
+        tokenizer(texts, padding=True): the batch padded to its longest text.
+    Weights: `visual_weights`, an OpenAI-format CLIP checkpoint of which only visual.* is read, and `textual_weights`,
+    the MultilingualCLIP checkpoint (state dicts or paths); `random_init` seeds both instead, the image tower as B200Clip
+    seeds it.  Tokenizer: model_properties["tokenizer"] (a callable), else `vocab_file` (XLM-R: sentencepiece.bpe.model
+    -> XLMRTokenizer; LaBSE: vocab.txt -> the cased WordPieceTokenizer), else transformers.AutoTokenizer of the
+    entry's textual_model.  The reference's tokenizer call does not truncate, so a text longer than the encoder's 512
+    positions fails there inside the embedding (torch's IndexError for XLM-R, a size mismatch for LaBSE); here it is
+    refused with VectoriseError before any GPU work, never truncated."""
+
+    def __init__(self, device: Optional[str] = None, model_properties: Optional[dict] = None, model_auth=None):
+        if not device:
+            raise InternalError("`device` is required for loading MULTILINGUAL CLIP models!")
+        super().__init__(device=device, model_properties=model_properties, model_auth=model_auth)
+        self.text_model = None
+
+    def load(self) -> None:
+        from .engine import Encoder
+        props = self.model_properties
+        arch = props.get("arch")
+        if arch is None:
+            raise InvalidModelPropertiesError("model_properties has no `arch` block")
+        seed = props.get("random_init")
+        for k in ("visual_weights", "textual_weights"):
+            if props.get(k) is None and seed is None:
+                raise ModelLoadError(f"model_properties needs `{k}` (state dict or checkpoint path) or `random_init`; "
+                                     "checkpoint download is Marqo's job")
+        # B200Clip's image tower: the OPENAI_CLIP_MODELS arch without its text tower
+        self.arch = dict(model_registry.OPENAI_CLIP_MODELS[arch["visual"]]["arch"], text=None)
+        device, max_batch = _validate_device(self.device), int(props.get("max_batch", 256))
+        vis = props.get("visual_weights")
+        if vis is None:
+            vis = weights_mod.random_clip_weights(self.arch, int(seed))
+        elif isinstance(vis, (str, bytes)) or hasattr(vis, "__fspath__"):
+            vis = weights_mod.load_state_dict(vis)
+        txt = props.get("textual_weights")
+        if txt is None:
+            txt = weights_mod.random_mclip_text_weights(arch, int(seed) + 1)
+        elif isinstance(txt, (str, bytes)) or hasattr(txt, "__fspath__"):
+            txt = weights_mod.load_state_dict(txt)
+        self.model = Encoder("clip", self.arch, {k: v for k, v in vis.items() if k.startswith("visual.")},
+                             device=device, max_batch=max_batch)
+        try:
+            self.text_model = Encoder(arch["text_kind"], arch, txt, device=device, max_batch=max_batch)
+        except Exception:
+            self.close()
+            raise
+        # the encoder's positions: XLM-R's start after the pad id
+        self.max_tokens = arch["max_pos"] - (arch["pad_id"] + 1 if arch["text_kind"] == "xlmr" else 0)
+        self.tokenizer = props.get("tokenizer") or self._default_tokenizer()
+
+    def _default_tokenizer(self):
+        props, kind = self.model_properties, self.model_properties["arch"]["text_kind"]
+        if props.get("vocab_file"):
+            from .tokenizers import WordPieceTokenizer, XLMRTokenizer
+            if kind == "xlmr":
+                return XLMRTokenizer(props["vocab_file"])
+            return WordPieceTokenizer(props["vocab_file"], do_lower_case=False)
+        try:
+            from transformers import AutoTokenizer
+            return AutoTokenizer.from_pretrained(props["textual_model"])
+        except Exception:
+            return None  # encode_text raises a clear error if text arrives without a tokenizer
+
+    def close(self) -> None:
+        super().close()
+        if self.text_model is not None:
+            self.text_model.close()
+            self.text_model = None
+
+    def _tokens(self, sentences: List[str]):
+        """ids and mask int32 [n, L], L the longest text's tokens; a text over max_tokens is refused."""
+        if self.tokenizer is None:
+            raise ModelLoadError("no M-CLIP tokenizer available: supply model_properties['tokenizer'] or 'vocab_file'")
+        # one token past the limit shows a text that does not fit without tokenizing all of a long one
+        tok = self.tokenizer(sentences, padding=True, truncation=True, max_length=self.max_tokens + 1,
+                             return_tensors="np")
+        ids = np.ascontiguousarray(tok["input_ids"], dtype=np.int32)
+        mask = np.ascontiguousarray(tok["attention_mask"], dtype=np.int32)
+        lens = mask.sum(axis=1)
+        if lens.max() > self.max_tokens:
+            i = int(np.argmax(lens > self.max_tokens))
+            raise VectoriseError(f"text {i} is longer than the {self.max_tokens} tokens the multilingual_clip text "
+                                 f"encoder takes; it is not truncated, as the reference's M-CLIP tokenizer call does not "
+                                 f"truncate either")
+        return ids, mask
+
+    def encode_text(self, sentence: Union[str, List[str]], normalize=True) -> np.ndarray:
+        """clip_utils.py:555-570: MultilingualCLIP.forward, then / |out| when normalize is set"""
+        if self.text_model is None:
+            self.load()
+        ids, mask = self._tokens(sentence if isinstance(sentence, list) else [sentence])
+        return self.text_model.encode_tokens(ids, mask, normalize=bool(normalize))
+
+    def encode_to_device(self, inputs, default: str = 'text', normalize=True, sub_batch: int = 256, **kwargs):
+        """B200OpenCLIP.encode_to_device for images; texts (strings, tokenized per sub-batch) run the text Encoder."""
+        import torch
+        infer = kwargs.get('infer', True)
+        is_ids = isinstance(inputs, np.ndarray) and inputs.dtype.kind in "iu" and inputs.ndim == 2
+        if is_ids or (infer and _is_image(inputs)) or default == 'image':
+            if is_ids:
+                raise VectoriseError("multilingual_clip takes texts as strings: token ids carry no attention mask")
+            return super().encode_to_device(inputs, default=default, normalize=normalize, sub_batch=sub_batch, **kwargs)
+        if self.text_model is None:
+            self.load()
+        items = inputs if isinstance(inputs, list) else [inputs]
+        dev = self._torch_device()
+        out = torch.empty((len(items), self.text_model.embed_dim), dtype=torch.float32, device=dev)
+        step = max(1, min(int(sub_batch), int(self.model_properties.get("max_batch", 256))))
+        for lo in range(0, len(items), step):
+            ids, mask = self._tokens(items[lo:lo + step])
+            d_ids, d_mask = torch.from_numpy(ids).to(dev), torch.from_numpy(mask).to(dev)
+            self._sync_device(dev)
+            self.text_model.encode_tokens_device(d_ids.data_ptr(), d_mask.data_ptr(), ids.shape[0], ids.shape[1],
+                                                 out[lo:].data_ptr(), normalize=bool(normalize), sync=True)
+        return out
+
+
 LOADERS = {
     model_registry.TYPE_OPEN_CLIP: B200OpenCLIP,
     model_registry.TYPE_HF: B200HuggingFace,
     model_registry.TYPE_HF_STELLA: B200HuggingFaceStella,
     model_registry.TYPE_CLIP: B200Clip,
     model_registry.TYPE_FP16_CLIP: B200Fp16Clip,
+    model_registry.TYPE_MULTILINGUAL_CLIP: B200MultilingualClip,
 }
 
 

@@ -2,7 +2,7 @@
 
 Property dicts (`name`, `dimensions`, `type`, `tokens`, `model_size`, prefixes, `poolingMethod`, `notes`) are the
 reference's registry entries (src/marqo/s2_inference/model_registry.py:142-231 for open_clip/*, :616-851 for hf/*);
-`type` is rewritten to the engine's loader types ("b200_open_clip" / "b200_hf" / "b200_hf_stella") so that both
+`type` is rewritten to the engine's loader types ("b200_open_clip", "b200_hf", ...) so that both
 engines can be registered side by side in MODEL_PROPERTIES['loaders'] (model_registry.py:2133-2145).  The `arch` blocks are the shapes that live
 in open_clip 2.24.0 `model_configs/*.json` and the HF `config.json` files (SURVEY.md §8).
 
@@ -175,7 +175,25 @@ The wide ResNets' archs (OpenAI's build_model shapes; open_clip RN50x*.json, ver
 each with an attention pool of width / 2 heads of 64.  Their names are not registered (DESIGN.md §6): the `clip`
 loader serves them from a custom checkpoint, whose arch openai_clip_arch reads from its shapes.  No entry carries a
 model_size: Marqo derives 1 GB from the clip type, the 0.66 GB default for fp16_clip, and 1.5 GB for the ViT-L/14
-names."""
+names.
+
+The M-CLIP entries of the reference's `multilingual_clip` loader (get_multilingual_clip_properties, clip_utils.py:599-
+640) live in MULTILINGUAL_CLIP_MODELS, field for field, under the loader type "b200_multilingual_clip", plus an arch
+block (`arch["kind"] == "mclip"`) in the clip_resnet layout: the text tower's fields at the top level, and the image
+tower as the name of the OPENAI_CLIP_MODELS entry it is ("visual": "ViT-L/14"), not a copied ViT block.  The text
+towers' shapes come from the upstream config.json files, which cannot be re-read offline (verify):
+    XLM-Roberta-Large-Vit-L-14, -Vit-B-32   XLMRobertaModel (`text_kind` "xlmr"): width 1024, 24 layers, 16 heads, mlp
+                                            4096, vocabulary 250002, max_position_embeddings 514, pad_token_id 1, one
+                                            token type, layer_norm_eps 1e-5; proj_dim 768 and 512
+    LABSE-Vit-L-14                          a cased BertModel (`text_kind` "bert"): width 768, 12 layers, 12 heads, mlp
+                                            3072, vocabulary 501153, 512 positions, 2 token types, pad 0,
+                                            layer_norm_eps 1e-12; proj_dim 768
+Both erf-GELU their MLPs.  pt_multilingual_clip's MultilingualCLIP (verify) keeps the encoder under "transformer." and
+runs tokenizer(texts, padding=True) (no truncation) -> transformer(...)[0] -> the masked mean over each row's tokens ->
+LinearTransformation (nn.Linear [proj_dim, width] with bias); the loader then divides by the norm without an epsilon
+when normalize is set.  "multilingual-clip/XLM-R Large Vit-B/16+" is not served: its image tower, open_clip
+ViT-B-16-plus-240, is 896 wide at 240 px (DESIGN.md §6).  No entry carries a model_size: Marqo derives 1.5 GB for the
+two names with "vit-l-14" and 5 GB from the multilingual_clip type for the other."""
 from __future__ import annotations
 
 import copy
@@ -189,6 +207,7 @@ TYPE_HF = "b200_hf"
 TYPE_HF_STELLA = "b200_hf_stella"
 TYPE_CLIP = "b200_clip"
 TYPE_FP16_CLIP = "b200_fp16_clip"
+TYPE_MULTILINGUAL_CLIP = "b200_multilingual_clip"
 
 
 def _clip_arch(embed, vw, vl, vh, patch, tw, tl, th, act="gelu", image_size=224):
@@ -535,6 +554,31 @@ def _openai_clip_models() -> Dict[str, dict]:
 OPENAI_CLIP_MODELS: Dict[str, dict] = _openai_clip_models()
 
 
+def _mclip_arch(text_kind: str, proj_dim: int, visual: str) -> dict:
+    """An M-CLIP model (module docstring, verify): the text tower at the top level, the image tower by its `clip` name."""
+    if text_kind == "xlmr":
+        text = _xlmr_arch(1024, 24, 16)
+    else:   # LaBSE: a cased BertModel over a 501153-piece WordPiece vocabulary
+        text = {**_bert_arch(*_BERT_BASE), "vocab": 501153, "pad_id": 0, "ln_eps": 1e-12}
+    return {**text, "kind": "mclip", "text_kind": text_kind, "proj_dim": proj_dim, "visual": visual}
+
+
+def _multilingual_clip_models() -> Dict[str, dict]:
+    """The reference's `multilingual_clip` entries (module docstring), field for field, plus their arch."""
+    m: Dict[str, dict] = {}
+    for model, visual, textual, dims, text_kind in (
+            ("XLM-Roberta-Large-Vit-L-14", "ViT-L/14", "M-CLIP/XLM-Roberta-Large-Vit-L-14", 768, "xlmr"),
+            ("XLM-Roberta-Large-Vit-B-32", "ViT-B/32", "M-CLIP/XLM-Roberta-Large-Vit-B-32", 512, "xlmr"),
+            ("LABSE-Vit-L-14", "ViT-L/14", "M-CLIP/LABSE-Vit-L-14", 768, "bert")):
+        name = f"multilingual-clip/{model}"
+        m[name] = {"name": name, "visual_model": f"openai/{visual}", "textual_model": textual, "dimensions": dims,
+                   "type": TYPE_MULTILINGUAL_CLIP, "arch": _mclip_arch(text_kind, dims, visual)}
+    return m
+
+
+MULTILINGUAL_CLIP_MODELS: Dict[str, dict] = _multilingual_clip_models()
+
+
 def _count(sd: dict, prefix: str) -> int:
     """The number of distinct indices i among the keys prefix + "i.*"."""
     return len({k[len(prefix):].split(".")[0] for k in sd if k.startswith(prefix)})
@@ -577,7 +621,7 @@ def openai_clip_arch(sd: dict) -> dict:
 def find_model(model_name: str) -> Optional[dict]:
     """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
     for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS, CONVNEXT_MODELS, BIG_VIT_MODELS,
-                  EVA02_MODELS, GTE_MODELS, COCA_MODELS, OPENAI_CLIP_MODELS):
+                  EVA02_MODELS, GTE_MODELS, COCA_MODELS, OPENAI_CLIP_MODELS, MULTILINGUAL_CLIP_MODELS):
         entry = table.get(model_name)
         if entry is not None:
             return entry
@@ -596,9 +640,11 @@ def all_models() -> Dict[str, dict]:
     COCA_MODELS is in: its towers are the ViT-B-32 and ViT-L-14 CLIP shapes; its pooler GEMMs and attention run in
     tests/test_coca_kernels_gpu.py.  OPENAI_CLIP_MODELS is in: its text towers are 512, 768 and 1024 wide, and its
     one new layer shape (ViT-L/14@336px's vision layers at 577 tokens) runs in tests/test_layers_gpu.py.
+    MULTILINGUAL_CLIP_MODELS is in: its text towers are multilingual-e5-large's and a BERT-base, 1024 and 768 wide, and
+    its image towers are named OPENAI_CLIP_MODELS entries, not blocks of their own.
     served_models() has every served entry; find_model looks in every table."""
     return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS, **RESNET_MODELS, **EVA02_MODELS, **GTE_MODELS,
-            **COCA_MODELS, **OPENAI_CLIP_MODELS}
+            **COCA_MODELS, **OPENAI_CLIP_MODELS, **MULTILINGUAL_CLIP_MODELS}
 
 
 def served_models() -> Dict[str, dict]:

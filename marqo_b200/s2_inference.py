@@ -89,7 +89,8 @@ def validate_model_properties(model_name: str, model_properties: Optional[dict])
     """s2_inference.py:340-407 reduced to the loader types this engine serves: explicit properties must carry
     `dimensions` and a known `type`; otherwise the name is looked up in the registry.  A custom `clip` model with a
     checkpoint (`localpath`, `url`, `model_location` or `weights`) and no `arch` keeps it so: its loader reads the
-    arch from the checkpoint's shapes (model_registry.openai_clip_arch), as clip.load builds the model from them."""
+    arch from the checkpoint's shapes (model_registry.openai_clip_arch), as clip.load builds the model from them.
+    `multilingual_clip` serves the names of model_registry.MULTILINGUAL_CLIP_MODELS only."""
     if model_properties is None:
         return model_registry.get_model_properties(model_name)
     if not isinstance(model_properties, dict):
@@ -100,11 +101,18 @@ def validate_model_properties(model_name: str, model_properties: Optional[dict])
     mtype = props.get("type")
     alias = {"open_clip": model_registry.TYPE_OPEN_CLIP, "hf": model_registry.TYPE_HF,
              "hf_stella": model_registry.TYPE_HF_STELLA, "clip": model_registry.TYPE_CLIP,
-             "fp16_clip": model_registry.TYPE_FP16_CLIP}
+             "fp16_clip": model_registry.TYPE_FP16_CLIP, "multilingual_clip": model_registry.TYPE_MULTILINGUAL_CLIP}
     props["type"] = alias.get(mtype, mtype)
     if props["type"] not in alias.values():
         raise InvalidModelPropertiesError(f"model type `{mtype}` is not served by the H100 engine (supported: "
-                                          f"open_clip, hf, hf_stella, clip, fp16_clip)")
+                                          f"open_clip, hf, hf_stella, clip, fp16_clip, multilingual_clip)")
+    if (props["type"] == model_registry.TYPE_MULTILINGUAL_CLIP
+            and model_name not in model_registry.MULTILINGUAL_CLIP_MODELS):
+        # the reference's MULTILINGUAL_CLIP reads its towers from get_multilingual_clip_properties()[model_name]
+        # (clip_utils.py:527): only its own names load
+        raise InvalidModelPropertiesError(
+            f"multilingual_clip model `{model_name}` is not served by the H100 engine (served: "
+            f"{', '.join(model_registry.MULTILINGUAL_CLIP_MODELS)})")
     custom_clip = props["type"] == model_registry.TYPE_CLIP and any(
         props.get(k) is not None for k in ("localpath", "url", "model_location", "weights"))
     if "arch" not in props and not custom_clip:
@@ -166,7 +174,8 @@ def _reference_type_name(t):
     """this engine's loader types carry a b200_ prefix in the registry; sizes are declared per reference type"""
     return {model_registry.TYPE_OPEN_CLIP: "open_clip", model_registry.TYPE_HF: "hf",
             model_registry.TYPE_HF_STELLA: "hf_stella", model_registry.TYPE_CLIP: "clip",
-            model_registry.TYPE_FP16_CLIP: "fp16_clip"}.get(t, t)
+            model_registry.TYPE_FP16_CLIP: "fp16_clip",
+            model_registry.TYPE_MULTILINGUAL_CLIP: "multilingual_clip"}.get(t, t)
 
 
 def _check_memory_threshold_for_model(device: str, model_size) -> bool:

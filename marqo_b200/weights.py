@@ -366,6 +366,16 @@ def random_xlmr_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     return random_bert_weights(arch, seed)
 
 
+def random_mclip_text_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
+    """Seeded random weights of an M-CLIP text tower under MultilingualCLIP's names (arch: the registry's M-CLIP
+    block): the BERT / XLM-R encoder under "transformer." and LinearTransformation [proj_dim, width] with its bias."""
+    sd = {"transformer." + k: v for k, v in random_bert_weights(arch, seed).items()}
+    g = _rng(seed + 1)
+    sd["LinearTransformation.weight"] = _lin(g, arch["proj_dim"], arch["width"])
+    sd["LinearTransformation.bias"] = _vec(g, arch["proj_dim"])
+    return sd
+
+
 def random_gte_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     """Seeded random weights under NewModel parameter names (arch: the registry's GTE block): the fused qkv_proj, the
     fused up_gate_proj [2 mlp, width] without bias, no position table.  up_gate_proj and down_proj have gains 0.7 and
