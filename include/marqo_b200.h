@@ -363,6 +363,19 @@ typedef struct b200_model_desc {
      * text_proj_dim.  Weights: the encoder's names under an optional "transformer." prefix (dropped), and
      * LinearTransformation.weight [E, width] and LinearTransformation.bias [E].  0: the usual head. */
     int32_t text_proj_dim;
+    /* A BERT cross-encoder (transformers BertForSequenceClassification, eval mode; verify), arch B200_ARCH_BERT only.
+     * cls_labels > 0 replaces the pooling head: over a pair batch of ids, mask and token-type ids [n, S]
+     *   x = LN_emb(word[ids] + token_type[type_ids] + position[s])   (type ids clamped to [0, type_vocab - 1]);
+     *   the BERT layers (key mask from attn_mask, erf-GELU);
+     *   p = tanh(pooler.dense(x[CLS])), x[CLS] the row of position 0;
+     *   out[b] = classifier(p) [cls_labels], then the activation b200_model_classify_tokens asks for.
+     * embed_dim must equal cls_labels.  Weights: BertForSequenceClassification's names with the "bert." prefix dropped
+     * (embeddings.*, encoder.layer.*, pooler.dense.{weight [W, W], bias}), classifier.{weight [cls_labels, W], bias};
+     * b200_model_finalize refuses a missing one with B200_ERR_MISSING_WEIGHT, as every other required parameter.
+     * Such a model is run by b200_model_classify_tokens only; b200_model_encode_tokens refuses it with
+     * B200_ERR_INVALID_ARG, and b200_model_create refuses cls_labels on any other arch the same way.  0: the usual
+     * head. */
+    int32_t cls_labels;
 } b200_model_desc;
 
 int b200_model_create(int device, const b200_model_desc* desc, b200_model** out);
@@ -445,6 +458,16 @@ int b200_model_encode_images_u8_device(b200_model* m, const uint8_t* d_hwc, int 
                                        float* d_out, int sync);
 int b200_model_encode_tokens_device(b200_model* m, const int32_t* d_ids, const int32_t* d_attn_mask, int n,
                                     int seq, int normalize, float* d_out, int sync);
+/* A cross-encoder's scores (cls_labels > 0, see b200_model_desc): sentence pairs as ids, attn_mask (NULL: all ones, else
+ * a right-padded prefix mask as b200_model_encode_tokens takes) and type_ids (0 up to the first [SEP], 1 after it;
+ * NULL: all 0), each int32 [n, seq] on the host.  activation 0 returns the logits, 1 their sigmoid
+ * (sentence-transformers' CrossEncoder default for one label).  out: fp32 host [n, cls_labels].  A model without a
+ * classification head, or any other activation: B200_ERR_INVALID_ARG. */
+int b200_model_classify_tokens(b200_model* m, const int32_t* ids, const int32_t* attn_mask, const int32_t* type_ids,
+                               int n, int seq, int activation, float* out);
+/* The same with device-resident inputs and output, asynchronous on the model's stream unless sync != 0. */
+int b200_model_classify_tokens_device(b200_model* m, const int32_t* d_ids, const int32_t* d_attn_mask,
+                                      const int32_t* d_type_ids, int n, int seq, int activation, float* d_out, int sync);
 /* Images of mixed sizes in one call (every vision tower that takes uint8 images): image i is uint8 HWC
  * [heights[i], widths[i], 3] at hwc[i]; hwc, heights and widths are host arrays of n.  The images are resized to the
  * model's S x S by the tower's rule (shortest side + centre crop, or the squash) in one pass over each sub-batch, two
@@ -516,6 +539,17 @@ int b200_tokenizer_vocab_size(b200_tokenizer* t, int* out_size);
  * stride *out_seq_len.  max_length >= 2.  Thread-safe (the handle is immutable after creation). */
 int b200_tokenizer_encode(b200_tokenizer* t, const char* const* texts, const int64_t* text_bytes, int n, int max_length,
                           int32_t* out_ids, int32_t* out_mask, int* out_seq_len);
+/* WordPiece sentence pairs, what a cross-encoder's tokenizer(texts_a, texts_b, padding=True, truncation='longest_first',
+ * max_length=max_length) gives: row i is "[CLS] A [SEP] B [SEP]" for A = texts_a[i], B = texts_b[i], type ids 0 through
+ * the first [SEP] and 1 after it, padded with [PAD] (type 0, mask 0) to the longest row of the call.  Truncation is
+ * HF tokenizers' longest_first over the budget m = max_length - 3: with n1 <= n2 the two lengths (the shorter first),
+ * when n1 + n2 > m, n2 = n1 if n1 > m, else max(n1, m - n1); if n1 + n2 is still over m, n1 = m / 2 and n2 = n1 + m % 2;
+ * each side then keeps its first min(its length, its share) ids.  out_ids, out_mask, out_type_ids (mask and type ids
+ * may be NULL): caller buffers of n * max_length int32, rows back to back with stride *out_seq_len.  max_length >= 3.
+ * WordPiece tokenizers only (B200_ERR_INVALID_ARG otherwise). */
+int b200_tokenizer_encode_pairs(b200_tokenizer* t, const char* const* texts_a, const int64_t* bytes_a,
+                                const char* const* texts_b, const int64_t* bytes_b, int n, int max_length,
+                                int32_t* out_ids, int32_t* out_mask, int32_t* out_type_ids, int* out_seq_len);
 
 /* Recommender interpolation (SURVEY §8 f3): src/marqo/core/utils/vector_interpolation.py —
  * Lerp.interpolate :49-88 (sum_i (w_i / sum w) v_i), Nlerp.interpolate :91-119 (Lerp, then / |.|),
@@ -652,10 +686,13 @@ int b200_debug_clip_text_embed_cls(int device, const int32_t* ids, const float* 
  * [n] = sum of each mask row (S when mask is NULL).  pad < 0: BERT, p = s, type0 [w] required, pos_rows >= S, or pos
  * NULL for no position row (GTE).
  * pad >= 0: RoBERTa (XLM-R with type0, MPNet with type0 NULL), HF's position ids counted from the ids and pad,
- * pos_rows >= pad + S + 1. */
+ * pos_rows >= pad + S + 1.
+ * type_ids (BERT with positions only; NULL: none): int32 [n, S], and type0 is then the whole token-type table
+ * [type_rows, w], row type_ids[b, s] (clamped to [0, type_rows - 1]) added in place of row 0. */
 int b200_debug_embed_ln(int device, const int32_t* ids, const int32_t* mask, const float* word, const float* pos,
                         int pos_rows, const float* type0, const float* gamma, const float* beta, float eps, int n, int S,
-                        int w, int vocab, int pad, float* x, void* h, int32_t* kv_len, void* stream);
+                        int w, int vocab, int pad, float* x, void* h, int32_t* kv_len, const int32_t* type_ids,
+                        int type_rows, void* stream);
 /* CLIP head over token rows x fp32 [n*S, w]: LN(row b*S + row_in_seq[b]) @ proj [w, E] (row_in_seq NULL: row 0;
  * every entry must lie in [0, S)), divided by its L2 norm if normalize.  out fp32 [n, E]. */
 int b200_debug_clip_head(int device, const float* x, int S, const int32_t* row_in_seq, const float* gamma,
@@ -670,6 +707,11 @@ int b200_debug_bert_head(int device, const float* x, const int32_t* kv_len, int 
  * w a multiple of 4, <= 1024. */
 int b200_debug_text_head(int device, const float* x, const int32_t* kv_len, int n, int S, int w, const float* proj,
                          const float* bias, int E, int normalize, float* out, void* stream);
+/* BertForSequenceClassification's head over x fp32 [n*S, w]: p = tanh(pool_w [w, w] . x[b*S] + pool_b [w]), then
+ * out[b, l] = cls_w[l] . p + cls_b[l] for cls_w [L, w], cls_b [L], through the sigmoid if sigmoid != 0.  out fp32
+ * [n, L].  w <= 1024. */
+int b200_debug_cls_head(int device, const float* x, int n, int S, int w, const float* pool_w, const float* pool_b,
+                        const float* cls_w, const float* cls_b, int L, int sigmoid, float* out, void* stream);
 /* out fp32 [n, E] = src / |src| per row if normalize, else src. */
 int b200_debug_l2_rows(int device, const float* src, int n, int E, int normalize, float* out, void* stream);
 /* ResNet stem im2col: exactly one of hwc (uint8 [n,S,S,3], normalised with mean3 / std3, host fp32 [3]) and chw (fp32

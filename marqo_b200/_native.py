@@ -55,6 +55,7 @@ class ModelDesc(C.Structure):
         ("convnext_head", C.c_int32), ("resize_squash", C.c_int32), ("eva_rope_ref_grid", C.c_int32),
         ("rope_theta", C.c_float), ("rope_ntk_factor", C.c_float),
         ("attn_pool_heads", C.c_int32), ("text_embed_cls", C.c_int32), ("text_proj_dim", C.c_int32),
+        ("cls_labels", C.c_int32),
     ]
 
 
@@ -116,6 +117,8 @@ _SIGNATURES = {
     "b200_model_encode_tokens": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "b200_model_encode_images_u8_device": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
     "b200_model_encode_tokens_device": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
+    "b200_model_classify_tokens": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
+    "b200_model_classify_tokens_device": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
     "b200_model_encode_images_u8_ragged": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P]),
     "b200_model_encode_images_u8_ragged_device": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int]),
     "b200_model_set_stream": (C.c_int, [_P, _P, C.c_int]),
@@ -145,11 +148,12 @@ _SIGNATURES = {
     "b200_debug_clip_text_embed_cls": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P,
                                                  _P]),
     "b200_debug_embed_ln": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_int, _P, _P, _P, C.c_float, C.c_int, C.c_int, C.c_int,
-                                      C.c_int, C.c_int, _P, _P, _P, _P]),
+                                      C.c_int, C.c_int, _P, _P, _P, _P, C.c_int, _P]),
     "b200_debug_clip_head": (C.c_int, [C.c_int, _P, C.c_int, _P, _P, _P, C.c_float, _P, C.c_int, C.c_int, C.c_int, C.c_int,
                                        _P, _P]),
     "b200_debug_bert_head": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_text_head": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_cls_head": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P]),
     "b200_debug_l2_rows": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_stem_im2col": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
     "b200_debug_avgpool2": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
@@ -180,6 +184,7 @@ _SIGNATURES = {
     "b200_tokenizer_destroy": (C.c_int, [_P]),
     "b200_tokenizer_vocab_size": (C.c_int, [_P, C.POINTER(C.c_int)]),
     "b200_tokenizer_encode": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, C.POINTER(C.c_int)]),
+    "b200_tokenizer_encode_pairs": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, C.POINTER(C.c_int)]),
     "b200_fuse_vectors": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "b200_interpolate_vectors": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.POINTER(C.c_int)]),
 }

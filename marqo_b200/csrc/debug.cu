@@ -380,9 +380,11 @@ int b200_debug_clip_text_embed_cls(int device, const int32_t* ids, const float* 
 
 int b200_debug_embed_ln(int device, const int32_t* ids, const int32_t* mask, const float* word, const float* pos,
                         int pos_rows, const float* type0, const float* gamma, const float* beta, float eps, int n, int S,
-                        int w, int vocab, int pad, float* x, void* h, int32_t* kv_len, void* stream) {
+                        int w, int vocab, int pad, float* x, void* h, int32_t* kv_len, const int32_t* type_ids,
+                        int type_rows, void* stream) {
     return guarded([&] {
         const bool roberta = pad >= 0;
+        MB_CHECK_ARG(!type_ids || (!roberta && pos && type_rows > 0), "token-type ids: BERT with positions and rows");
         // pos NULL: the BERT embedding without a position row (GTE)
         MB_CHECK_ARG(ids && word && (pos || !roberta) && gamma && beta && x && h && kv_len, "NULL buffer");
         MB_CHECK_ARG(roberta || type0, "the BERT embedding always adds token-type row 0");
@@ -396,7 +398,7 @@ int b200_debug_embed_ln(int device, const int32_t* ids, const int32_t* mask, con
                                       static_cast<bf16*>(h), kv_len, s);
         else
             kernels::bert_embed_ln(ids, mask, word, pos, type0, gamma, beta, eps, n, S, w, vocab, x, static_cast<bf16*>(h),
-                                   kv_len, s);
+                                   kv_len, s, type_ids, type_ids ? type_rows : 1);
         MB_CUDA(cudaStreamSynchronize(s));
     });
 }
@@ -439,6 +441,19 @@ int b200_debug_text_head(int device, const float* x, const int32_t* kv_len, int 
         const cudaStream_t s = static_cast<cudaStream_t>(stream);
         DeviceBuffer<float> pooled((size_t)n * w);
         kernels::text_head(x, kv_len, n, S, w, proj, bias, E, normalize, out, pooled.get(), s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_cls_head(int device, const float* x, int n, int S, int w, const float* pool_w, const float* pool_b,
+                        const float* cls_w, const float* cls_b, int L, int sigmoid, float* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && pool_w && pool_b && cls_w && cls_b && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && S > 0 && w > 0 && L > 0, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::cls_head(x, S, n, w, pool_w, pool_b, cls_w, cls_b, L, sigmoid, out, s);
         MB_CUDA(cudaStreamSynchronize(s));
     });
 }

@@ -498,13 +498,18 @@ int clip_text_embed(const int32_t* ids, const float* tok, const float* pos, int 
 }
 
 // POS: BERT's position_embeddings row s is added; GTE (NewModel, rotary positions) has no position table.
-template <bool POS>
+// TYPES: each token adds row type_ids[row] (clamped to [0, type_vocab - 1]) of the token-type table `type0`
+// [type_vocab, w] (a sentence pair); without it every token adds row 0, and the instantiation is the one the encoders
+// have always run.
+template <bool POS, bool TYPES = false>
 __global__ void __launch_bounds__(256) bert_embed_ln_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ mask,
                                                             const float* __restrict__ word, const float* __restrict__ pos,
                                                             const float* __restrict__ type0, const float* __restrict__ gamma,
                                                             const float* __restrict__ beta, float eps, int n, int S, int w,
                                                             int vocab, float* __restrict__ x, __nv_bfloat16* __restrict__ h,
-                                                            int32_t* __restrict__ kv_len) {
+                                                            int32_t* __restrict__ kv_len,
+                                                            const int32_t* __restrict__ type_ids = nullptr,
+                                                            int type_vocab = 1) {
     const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= (long long)n * S) return;
@@ -513,7 +518,9 @@ __global__ void __launch_bounds__(256) bert_embed_ln_kernel(const int32_t* __res
     id = min(max(id, 0), vocab - 1);
     const int nv = w / 128;
     const float4* w4 = reinterpret_cast<const float4*>(word + (long long)id * w);
-    const float4* t4 = reinterpret_cast<const float4*>(type0);
+    const float* trow = type0;
+    if constexpr (TYPES) trow += (long long)min(max(type_ids[row], 0), type_vocab - 1) * w;
+    const float4* t4 = reinterpret_cast<const float4*>(trow);
     float4 v[LN_MAX_V4];
     if constexpr (POS) {
         const float4* p4 = reinterpret_cast<const float4*>(pos + (long long)s * w);
@@ -547,12 +554,16 @@ __global__ void __launch_bounds__(256) bert_embed_ln_kernel(const int32_t* __res
 
 int bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
                   const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, float* x,
-                  __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s) {
+                  __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s, const int32_t* type_ids, int type_vocab) {
     if (n <= 0) return 0;
     check_ln_width(w);
     const long long rows = (long long)n * S;
     const unsigned blocks = (unsigned)((rows + 7) / 8);
-    if (pos)
+    if (type_ids) {
+        if (!pos || type_vocab < 1) fail(B200_ERR_INTERNAL, "bert_embed_ln: token types need positions and a table");
+        bert_embed_ln_kernel<true, true><<<blocks, 256, 0, s>>>(ids, mask, word, pos, type0, gamma, beta, eps, n, S, w,
+                                                                 vocab, x, h, kv_len, type_ids, type_vocab);
+    } else if (pos)
         bert_embed_ln_kernel<true><<<blocks, 256, 0, s>>>(ids, mask, word, pos, type0, gamma, beta, eps, n, S, w, vocab, x,
                                                            h, kv_len);
     else
@@ -816,6 +827,62 @@ int text_head(const float* x, const int32_t* kv_len, int n, int S, int w, const 
     head_norm_kernel<<<(n + 7) / 8, 256, 0, s>>>(out, n, E);
     MB_CUDA(cudaGetLastError());
     return 3;
+}
+
+// BertForSequenceClassification's head, CLS_SEQS sequences per CTA so that each pooler row is read once per CTA: the
+// CLS rows in shared memory, one warp per pooler output (every warp's lanes stride over a coalesced weight row, then a
+// butterfly sum: a fixed order), tanh, then one warp per (sequence, label) for the classifier.  Everything is fp32.
+constexpr int CLS_SEQS = 4;
+
+__global__ void __launch_bounds__(256) cls_head_kernel(const float* __restrict__ x, int S, int n, int w,
+                                                       const float* __restrict__ wp, const float* __restrict__ bp,
+                                                       const float* __restrict__ wc, const float* __restrict__ bc, int L,
+                                                       int sigmoid, float* __restrict__ out) {
+    extern __shared__ float sm[];   // cls [CLS_SEQS][w], then pooled [CLS_SEQS][w]
+    float* cls = sm;
+    float* pooled = sm + CLS_SEQS * w;
+    const int b0 = blockIdx.x * CLS_SEQS, nb = min(CLS_SEQS, n - b0);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int i = threadIdx.x; i < CLS_SEQS * w; i += 256) {
+        const int k = i / w, c = i - k * w;
+        cls[i] = k < nb ? x[(long long)(b0 + k) * S * w + c] : 0.f;   // token 0 of sequence b0 + k
+    }
+    __syncthreads();
+    for (int o = warp; o < w; o += 8) {
+        const float* row = wp + (long long)o * w;
+        float acc[CLS_SEQS];
+#pragma unroll
+        for (int k = 0; k < CLS_SEQS; ++k) acc[k] = 0.f;
+        for (int i = lane; i < w; i += 32) {
+            const float a = __ldg(row + i);
+#pragma unroll
+            for (int k = 0; k < CLS_SEQS; ++k) acc[k] = fmaf(a, cls[k * w + i], acc[k]);
+        }
+#pragma unroll
+        for (int k = 0; k < CLS_SEQS; ++k) {
+            const float v = warp_sum(acc[k]);
+            if (lane == 0) pooled[k * w + o] = tanhf(v + bp[o]);
+        }
+    }
+    __syncthreads();
+    for (int j = warp; j < nb * L; j += 8) {
+        const int k = j / L, l = j - k * L;
+        const float* row = wc + (long long)l * w;
+        float acc = 0.f;
+        for (int i = lane; i < w; i += 32) acc = fmaf(__ldg(row + i), pooled[k * w + i], acc);
+        acc = warp_sum(acc) + bc[l];
+        if (lane == 0) out[(long long)(b0 + k) * L + l] = sigmoid ? 1.f / (1.f + expf(-acc)) : acc;
+    }
+}
+
+int cls_head(const float* x, int S, int n, int w, const float* wp, const float* bp, const float* wc, const float* bc,
+             int L, int sigmoid, float* out, cudaStream_t s) {
+    if (n <= 0) return 0;
+    if (w <= 0 || w > 1024 || L <= 0) fail(B200_ERR_UNSUPPORTED, "cls_head: width %d, %d labels unsupported", w, L);
+    const size_t smem = (size_t)2 * CLS_SEQS * w * sizeof(float);   // <= 32 KB
+    cls_head_kernel<<<(n + CLS_SEQS - 1) / CLS_SEQS, 256, smem, s>>>(x, S, n, w, wp, bp, wc, bc, L, sigmoid, out);
+    MB_CUDA(cudaGetLastError());
+    return 1;
 }
 
 // ------------------------------------------------------------------------------------------------ conversions

@@ -59,10 +59,13 @@ int clip_text_embed(const int32_t* ids, const float* tok, const float* pos, int 
                     int32_t* eot, cudaStream_t s, const float* cls = nullptr);
 
 // BERT: x = LN(word[ids] + position[s] + token_type[0]); pos NULL (GTE) adds no position row.  fp32 + bf16 copies.  Also kv_len[b] = sum(mask[b, :])
-// (mask may be NULL = all ones).
+// (mask may be NULL = all ones).  type_ids (int32 [n, S], a sentence pair's segments; needs pos): token_type
+// [type_ids[b, s]] instead of row 0, type0 then being the whole table [type_vocab, w] and each id clamped to
+// [0, type_vocab - 1] as the word ids are to the vocabulary.
 int bert_embed_ln(const int32_t* ids, const int32_t* mask, const float* word, const float* pos, const float* type0,
                   const float* gamma, const float* beta, float eps, int n, int S, int w, int vocab, float* x,
-                  __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s);
+                  __nv_bfloat16* h, int32_t* kv_len, cudaStream_t s, const int32_t* type_ids = nullptr,
+                  int type_vocab = 1);
 
 // RoBERTa-style embeddings (MPNet, XLM-R): x = LN(word[ids] (+ token_type[0]) + position[p]) with HF's position rule
 // p = pad + (non-pad ids among ids[b, 0..s]) for a non-pad id and p = pad for a pad id; type0 NULL (MPNet) adds no
@@ -91,6 +94,13 @@ int bert_head(const float* x, const int32_t* kv_len, int n, int S, int w, int po
 // Three kernels with normalize, two without.
 int text_head(const float* x, const int32_t* kv_len, int n, int S, int w, const float* proj, const float* bias, int E,
               int normalize, float* out, float* pooled_ws, cudaStream_t s);
+
+// BertForSequenceClassification's head (transformers BertPooler + classifier, eval mode), one kernel: for sequence b,
+// c = x[b * S] (its [CLS] row of the fp32 residual stream [n * S, w]), p = tanh(wp c + bp) with the pooler
+// wp [w, w] (nn.Linear layout) and bp [w], then out[b, l] = wc[l] . p + bc[l] for the L labels of wc [L, w], bc [L],
+// through the sigmoid when `sigmoid` is set.  fp32 throughout; out fp32 [n, L].  w <= 1024.
+int cls_head(const float* x, int S, int n, int w, const float* wp, const float* bp, const float* wc, const float* bc,
+             int L, int sigmoid, float* out, cudaStream_t s);
 
 void f32_to_bf16(const float* src, __nv_bfloat16* dst, long long n, cudaStream_t s);
 // conv1.weight [w, 3*p*p] -> bf16 [w, kpad] zero padded

@@ -108,6 +108,9 @@ struct TowerW {
     const float *tok = nullptr, *type0 = nullptr, *emb_ln_w = nullptr, *emb_ln_b = nullptr, *text_cls = nullptr;
     // MPNet: relative-position bias of every layer, fp32 [heads, 2 * ctx - 1] pre-scaled by log2(e)
     attention::RelBias rel_bias;
+    // BertForSequenceClassification (cls_labels > 0): the pooler [width, width] and [width], the classifier
+    // [cls_labels, width] and [cls_labels], all fp32 as uploaded
+    const float *pool_w = nullptr, *pool_b = nullptr, *cls_w = nullptr, *cls_b = nullptr;
 };
 
 // OpenAI ResNet CLIP image tower (open_clip ModifiedResNet, verify): every conv with its BatchNorm folded in at
@@ -205,8 +208,10 @@ struct b200_model {
     struct GraphKey {
         int kind, n, S, normalize;
         const void *in0, *in1, *out;
+        const void* in2 = nullptr;   // token-type ids of a classified pair batch
         bool operator<(const GraphKey& o) const {
-            return std::tie(kind, n, S, normalize, in0, in1, out) < std::tie(o.kind, o.n, o.S, o.normalize, o.in0, o.in1, o.out);
+            return std::tie(kind, n, S, normalize, in0, in1, out, in2) <
+                   std::tie(o.kind, o.n, o.S, o.normalize, o.in0, o.in1, o.out, o.in2);
         }
     };
     struct GraphEntry {
@@ -377,6 +382,9 @@ void check_text(const b200_model_desc& d, const Kinds& k) {
     MB_CHECK_ARG(d.text_proj_dim >= 0, "text_proj_dim %d must not be negative", d.text_proj_dim);
     MB_CHECK_ARG(d.text_proj_dim == 0 || d.arch == B200_ARCH_BERT || d.arch == B200_ARCH_XLMR,
                  "text_proj_dim: only the BERT and XLM-R text towers take a projected head");
+    MB_CHECK_ARG(d.cls_labels >= 0, "cls_labels %d must not be negative", d.cls_labels);
+    MB_CHECK_ARG(d.cls_labels == 0 || d.arch == B200_ARCH_BERT,
+                 "cls_labels: only the BERT arch takes a sequence-classification head");
     if (k.text == TextKind::NONE) return;
     check_tower(d.text, "text", k.text == TextKind::CLIP || k.text == TextKind::COCA ? 1664 : 1024);
     MB_CHECK_ARG(d.text.ctx > 0 && d.text.vocab > 0, "text.ctx and text.vocab must be positive");
@@ -407,6 +415,13 @@ void check_text(const b200_model_desc& d, const Kinds& k) {
         [[fallthrough]];
     }
     case TextKind::BERT:
+        if (d.cls_labels > 0) {
+            // BertForSequenceClassification: the pooler and classifier (cls_head) write cls_labels scores per pair
+            MB_CHECK_ARG(d.text_proj_dim == 0, "cls_labels and text_proj_dim are two different heads");
+            MB_CHECK_ARG(d.embed_dim == d.cls_labels, "embed_dim %d must equal cls_labels %d", d.embed_dim,
+                         d.cls_labels);
+            break;
+        }
         if (d.text_proj_dim > 0) {
             // M-CLIP's text head: the masked mean, projected (text_head)
             MB_CHECK_ARG(d.pool == B200_POOL_MEAN, "text_proj_dim: the projected head pools by the masked mean");
@@ -1036,6 +1051,12 @@ void build_text(b200_model* m) {
         T.emb_ln_w = param(m, "embeddings.LayerNorm.weight", w);
         T.emb_ln_b = param(m, "embeddings.LayerNorm.bias", w);
         build_layers(m, T, "encoder.layer.", BERT_LAYER);
+        if (m->desc.cls_labels > 0) {
+            T.pool_w = param(m, "pooler.dense.weight", w * w);
+            T.pool_b = param(m, "pooler.dense.bias", w);
+            T.cls_w = param(m, "classifier.weight", E * w);   // E == cls_labels
+            T.cls_b = param(m, "classifier.bias", E);
+        }
         break;
     }
     case TextKind::ROBERTA: {
@@ -1383,8 +1404,10 @@ void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const fl
     }
 }
 
-void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const int32_t* d_mask, int n, int S,
-                          int normalize, float* d_out) {
+// d_types: token-type ids [n, S] of a classifier (NULL: all 0); normalize is then the classifier's activation (0
+// identity, 1 sigmoid)
+void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const int32_t* d_mask, const int32_t* d_types,
+                          int n, int S, int normalize, float* d_out) {
     const TowerW& T = m->text;
     const int w = T.d.width, E = m->desc.embed_dim;
     float* x = m->x.get();
@@ -1423,12 +1446,15 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
         // MPNet); GTE has no position table (T.pos is NULL)
         if (m->kind.text != TextKind::ROBERTA)
             c.n += kernels::bert_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, T.eps, n, S, w,
-                                          T.d.vocab, x, m->h.get(), aux, m->stream);
+                                          T.d.vocab, x, m->h.get(), aux, m->stream, d_types,
+                                          std::max(1, m->desc.type_vocab));
         else
             c.n += kernels::roberta_embed_ln(d_ids, d_mask, T.tok, T.pos, T.type0, T.emb_ln_w, T.emb_ln_b, T.eps, n, S,
                                              w, T.d.vocab, m->desc.pad_id, x, m->h.get(), aux, m->stream);
         run_layers(m, c, T, n, S, attention::MASK_KEYLEN);
-        if (T.proj)   // M-CLIP: the masked mean, projected
+        if (T.cls_w)   // BertForSequenceClassification: pooler, classifier, activation
+            c.n += kernels::cls_head(x, S, n, w, T.pool_w, T.pool_b, T.cls_w, T.cls_b, E, normalize, d_out, m->stream);
+        else if (T.proj)   // M-CLIP: the masked mean, projected
             c.n += kernels::text_head(x, aux, n, S, w, T.proj, T.b_tproj, E, normalize, d_out, m->pooled.get(),
                                       m->stream);
         else
@@ -1490,11 +1516,11 @@ void forward_images(b200_model* m, Counter& c, const uint8_t* u8, const float* f
                 [&](Counter& cc) { forward_images_eager(m, cc, u8, f32, n, normalize, d_out); });
 }
 
-void forward_tokens(b200_model* m, Counter& c, const int32_t* d_ids, const int32_t* d_mask, int n, int S, int normalize,
-                    float* d_out) {
-    const b200_model::GraphKey key{1, n, S, normalize, d_ids, d_mask, d_out};
+void forward_tokens(b200_model* m, Counter& c, const int32_t* d_ids, const int32_t* d_mask, const int32_t* d_types, int n,
+                    int S, int normalize, float* d_out) {
+    const b200_model::GraphKey key{1, n, S, normalize, d_ids, d_mask, d_out, d_types};
     run_graphed(m, c, key, (long long)n * S,
-                [&](Counter& cc) { forward_tokens_eager(m, cc, d_ids, d_mask, n, S, normalize, d_out); });
+                [&](Counter& cc) { forward_tokens_eager(m, cc, d_ids, d_mask, d_types, n, S, normalize, d_out); });
 }
 
 void require_ready(b200_model* m) {
@@ -1572,22 +1598,74 @@ void check_ragged_args(b200_model* m, const uint8_t* const* imgs, const int32_t*
 // The token rows a sequence of `seq` ids takes in the workspaces: CoCa's text tower appends its CLS row.
 int token_rows(b200_model* m, int seq) { return m->kind.text == TextKind::COCA ? seq + 1 : seq; }
 
-void encode_tokens_dev(b200_model* m, Counter& c, const int32_t* d_ids, const int32_t* d_mask, int n, int S, int normalize,
-                       float* d_out) {
+void encode_tokens_dev(b200_model* m, Counter& c, const int32_t* d_ids, const int32_t* d_mask, const int32_t* d_types,
+                       int n, int S, int normalize, float* d_out) {
     const int cap = batch_cap_tokens(m, token_rows(m, S));
     for (int o = 0; o < n; o += cap) {
         const int nb = std::min(cap, n - o);
-        forward_tokens(m, c, d_ids + (size_t)o * S, d_mask ? d_mask + (size_t)o * S : nullptr, nb, S, normalize,
+        forward_tokens(m, c, d_ids + (size_t)o * S, d_mask ? d_mask + (size_t)o * S : nullptr,
+                       d_types ? d_types + (size_t)o * S : nullptr, nb, S, normalize,
                        d_out + (size_t)o * m->desc.embed_dim);
     }
 }
 
-void check_tokens_args(b200_model* m, int n, int S) {
+// classify: the call is b200_model_classify_tokens*, which only a classifier (cls_labels > 0) takes; the encode calls
+// refuse one
+void check_tokens_args(b200_model* m, int n, int S, bool classify = false) {
     MB_CHECK_ARG(m->kind.text != TextKind::NONE, "this model has no text tower");
+    MB_CHECK_ARG(!classify || m->desc.cls_labels > 0, "this model has no classification head (cls_labels 0)");
+    MB_CHECK_ARG(classify || m->desc.cls_labels == 0, "this model is a classifier (cls_labels %d): classify its tokens",
+                 m->desc.cls_labels);
     MB_CHECK_ARG(n > 0, "n must be positive");
     MB_CHECK_ARG(S > 0 && S <= m->text.tokens, "sequence length %d out of range (1..%d)", S, m->text.tokens);
     if (m->kind.text == TextKind::COCA)   // open_clip's CoCa tokenizer pads every text to ctx - 1 ids
         MB_CHECK_ARG(S == m->text.tokens - 1, "CoCa text: ids must be %d wide (got %d)", m->text.tokens - 1, S);
+}
+
+// b200_model_encode_tokens and b200_model_classify_tokens: host ids, mask and token types (either may be NULL) in
+// sub-batches through the staging buffer; `normalize` is the classifier's activation when classify is set
+void tokens_host(b200_model* m, const int32_t* ids, const int32_t* attn_mask, const int32_t* types, int n, int seq,
+                 int normalize, float* out, bool classify) {
+    require_ready(m);
+    MB_CHECK_ARG(ids && out, "NULL buffer");
+    check_tokens_args(m, n, seq, classify);
+    if (attn_mask && m->kind.text != TextKind::CLIP && m->kind.text != TextKind::COCA) {
+        // the kernels implement prefix (right-padded) masks, which is what the tokenizer call at
+        // hugging_face_model.py:179-185 produces
+        for (int b = 0; b < n; ++b) {
+            bool seen_zero = false;
+            for (int s = 0; s < seq; ++s) {
+                const bool on = attn_mask[(size_t)b * seq + s] != 0;
+                if (on && seen_zero) fail(B200_ERR_UNSUPPORTED, "attention mask of item %d is not a prefix mask", b);
+                seen_zero |= !on;
+            }
+        }
+    }
+    std::lock_guard<std::mutex> lk(m->mu);
+    DeviceGuard g(m->device);
+    const int E = m->desc.embed_dim;
+    const int cap = batch_cap_tokens(m, token_rows(m, seq));
+    const size_t row_bytes = (size_t)seq * 4, block = (size_t)std::min(n, cap) * seq;
+    ensure_in_dev(m, block * 4 * (types ? 3 : 2));
+    int32_t* d_ids = reinterpret_cast<int32_t*>(m->in_dev.get());
+    int32_t* d_mask = d_ids + block;
+    int32_t* d_types = types ? d_mask + block : nullptr;
+    TimedRegion tr(m);
+    for (int o = 0; o < n; o += cap) {
+        const int nb = std::min(cap, n - o);
+        MB_CUDA(cudaMemcpyAsync(d_ids, ids + (size_t)o * seq, (size_t)nb * row_bytes, cudaMemcpyHostToDevice, m->stream));
+        if (attn_mask)
+            MB_CUDA(cudaMemcpyAsync(d_mask, attn_mask + (size_t)o * seq, (size_t)nb * row_bytes, cudaMemcpyHostToDevice,
+                                    m->stream));
+        if (types)
+            MB_CUDA(cudaMemcpyAsync(d_types, types + (size_t)o * seq, (size_t)nb * row_bytes, cudaMemcpyHostToDevice,
+                                    m->stream));
+        forward_tokens(m, tr.c, d_ids, attn_mask ? d_mask : nullptr, d_types, nb, seq, normalize, m->out_dev.get());
+        MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
+                                m->stream));
+        MB_CUDA(cudaStreamSynchronize(m->stream));
+    }
+    tr.finish();
 }
 
 // The transformer tower b200_debug_layers runs: 0 vision, 1 text, if the model has one with layers.
@@ -1675,6 +1753,8 @@ int b200_model_load_tensor(b200_model* m, const char* name, const float* data, i
         if (m->kind.text == TextKind::GTE && key.compare(0, 4, "new.") == 0) key.erase(0, 4);
         // and M-CLIP checkpoints (MultilingualCLIP) under "transformer.", beside their LinearTransformation
         if (m->desc.text_proj_dim > 0 && key.compare(0, 12, "transformer.") == 0) key.erase(0, 12);
+        // and BertForSequenceClassification checkpoints under "bert.", beside their classifier
+        if (m->kind.text == TextKind::BERT && key.compare(0, 5, "bert.") == 0) key.erase(0, 5);
         m->raw[key] = std::move(b);
     });
 }
@@ -1820,43 +1900,14 @@ int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int nor
 
 int b200_model_encode_tokens(b200_model* m, const int32_t* ids, const int32_t* attn_mask, int n, int seq, int normalize,
                              float* out) {
+    return guarded([&] { tokens_host(m, ids, attn_mask, nullptr, n, seq, normalize, out, false); });
+}
+
+int b200_model_classify_tokens(b200_model* m, const int32_t* ids, const int32_t* attn_mask, const int32_t* type_ids,
+                               int n, int seq, int activation, float* out) {
     return guarded([&] {
-        require_ready(m);
-        MB_CHECK_ARG(ids && out, "NULL buffer");
-        check_tokens_args(m, n, seq);
-        if (attn_mask && m->kind.text != TextKind::CLIP && m->kind.text != TextKind::COCA) {
-            // the kernels implement prefix (right-padded) masks, which is what the tokenizer call at
-            // hugging_face_model.py:179-185 produces
-            for (int b = 0; b < n; ++b) {
-                bool seen_zero = false;
-                for (int s = 0; s < seq; ++s) {
-                    const bool on = attn_mask[(size_t)b * seq + s] != 0;
-                    if (on && seen_zero) fail(B200_ERR_UNSUPPORTED, "attention mask of item %d is not a prefix mask", b);
-                    seen_zero |= !on;
-                }
-            }
-        }
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        const int E = m->desc.embed_dim;
-        const int cap = batch_cap_tokens(m, token_rows(m, seq));
-        const size_t row_bytes = (size_t)seq * 4;
-        ensure_in_dev(m, (size_t)std::min(n, cap) * row_bytes * 2);
-        int32_t* d_ids = reinterpret_cast<int32_t*>(m->in_dev.get());
-        int32_t* d_mask = d_ids + (size_t)std::min(n, cap) * seq;
-        TimedRegion tr(m);
-        for (int o = 0; o < n; o += cap) {
-            const int nb = std::min(cap, n - o);
-            MB_CUDA(cudaMemcpyAsync(d_ids, ids + (size_t)o * seq, (size_t)nb * row_bytes, cudaMemcpyHostToDevice, m->stream));
-            if (attn_mask)
-                MB_CUDA(cudaMemcpyAsync(d_mask, attn_mask + (size_t)o * seq, (size_t)nb * row_bytes, cudaMemcpyHostToDevice,
-                                        m->stream));
-            forward_tokens(m, tr.c, d_ids, attn_mask ? d_mask : nullptr, nb, seq, normalize, m->out_dev.get());
-            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
-                                    m->stream));
-            MB_CUDA(cudaStreamSynchronize(m->stream));
-        }
-        tr.finish();
+        MB_CHECK_ARG(activation == 0 || activation == 1, "activation %d must be 0 (identity) or 1 (sigmoid)", activation);
+        tokens_host(m, ids, attn_mask, type_ids, n, seq, activation, out, true);
     });
 }
 
@@ -1900,7 +1951,23 @@ int b200_model_encode_tokens_device(b200_model* m, const int32_t* d_ids, const i
         std::lock_guard<std::mutex> lk(m->mu);
         DeviceGuard g(m->device);
         TimedRegion tr(m);
-        encode_tokens_dev(m, tr.c, d_ids, d_attn_mask, n, seq, normalize, d_out);
+        encode_tokens_dev(m, tr.c, d_ids, d_attn_mask, nullptr, n, seq, normalize, d_out);
+        tr.finish();
+        if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
+    });
+}
+
+int b200_model_classify_tokens_device(b200_model* m, const int32_t* d_ids, const int32_t* d_attn_mask,
+                                      const int32_t* d_type_ids, int n, int seq, int activation, float* d_out, int sync) {
+    return guarded([&] {
+        require_ready(m);
+        MB_CHECK_ARG(d_ids && d_out, "NULL buffer");
+        MB_CHECK_ARG(activation == 0 || activation == 1, "activation %d must be 0 (identity) or 1 (sigmoid)", activation);
+        check_tokens_args(m, n, seq, true);
+        std::lock_guard<std::mutex> lk(m->mu);
+        DeviceGuard g(m->device);
+        TimedRegion tr(m);
+        encode_tokens_dev(m, tr.c, d_ids, d_attn_mask, d_type_ids, n, seq, activation, d_out);
         tr.finish();
         if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
     });

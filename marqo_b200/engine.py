@@ -304,7 +304,8 @@ class Encoder:
     (None: no image tower) in place of resnet;  BERT: width, layers, heads, mlp, vocab,
     max_pos, type_vocab,
     pool ("mean"|"cls"), proj_dim (optional: M-CLIP's projected text head of that many outputs, whose weights are
-    LinearTransformation.weight [proj_dim, width] and .bias);  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
+    LinearTransformation.weight [proj_dim, width] and .bias), num_labels (optional: a BertForSequenceClassification
+    cross-encoder of that many labels, run by classify_tokens, whose weights add pooler.dense.* and classifier.*);  MPNet: width, layers, heads, mlp, vocab, max_pos (max_position_embeddings: sequences of up to
     max_pos - pad_id - 1 tokens), pad_id, ln_eps, rel_buckets, rel_max_distance, pool;  XLM-R: width, layers, heads,
     mlp, vocab, max_pos (as MPNet), pad_id, ln_eps, pool, proj_dim (as BERT);  GTE (NewModel: the Stella embedders): width, layers, heads,
     mlp (the GeGLU hidden size), vocab, type_vocab, ctx, ln_eps, rope_theta, rope_ntk_factor, pool.  `weights` maps
@@ -395,7 +396,8 @@ class Encoder:
             self.image_size = int(ev["image_size"]) if ev else 0
         elif arch == "bert":
             d.arch = N.ARCH_BERT
-            d.embed_dim = int(config.get("proj_dim") or config["width"])
+            d.cls_labels = int(config.get("num_labels") or 0)
+            d.embed_dim = int(d.cls_labels or config.get("proj_dim") or config["width"])
             d.text_proj_dim = int(config.get("proj_dim") or 0)
             d.pool = N.POOL_CLS if config.get("pool", "mean") == "cls" else N.POOL_MEAN
             d.type_vocab = int(config.get("type_vocab", 2))
@@ -579,6 +581,31 @@ class Encoder:
         N.check(self._lib.b200_model_encode_tokens(self._handle(), _ptr(i), _ptr(mk), i.shape[0], i.shape[1],
                                                    1 if normalize else 0, _ptr(out)))
         return out
+
+    def classify_tokens(self, ids, attn_mask=None, type_ids=None, sigmoid: bool = True) -> np.ndarray:
+        """A cross-encoder's scores (num_labels in the config) of sentence pairs: ids, attn_mask and type_ids int
+        [n, seq] (None: all ones / all zeros) -> fp32 [n, num_labels], the logits through the sigmoid if sigmoid."""
+        i = _as(ids.cpu().numpy() if hasattr(ids, "cpu") else ids, np.int32)
+        if i.ndim != 2:
+            raise ValueError(f"expected int [n, seq] token ids, got {i.shape}")
+        extra = []
+        for a in (attn_mask, type_ids):
+            a = None if a is None else _as(a.cpu().numpy() if hasattr(a, "cpu") else a, np.int32)
+            if a is not None and a.shape != i.shape:
+                raise ValueError("attention mask and token-type ids must have the shape of the ids")
+            extra.append(a)
+        out = np.empty((i.shape[0], self.embed_dim), np.float32)
+        N.check(self._lib.b200_model_classify_tokens(self._handle(), _ptr(i), _ptr(extra[0]), _ptr(extra[1]), i.shape[0],
+                                                     i.shape[1], 1 if sigmoid else 0, _ptr(out)))
+        return out
+
+    def classify_tokens_device(self, d_ids_ptr: int, d_mask_ptr: Optional[int], d_types_ptr: Optional[int], n: int,
+                               seq: int, d_out_ptr: int, sigmoid: bool = True, sync: bool = True) -> None:
+        N.check(self._lib.b200_model_classify_tokens_device(self._handle(), C.c_void_p(d_ids_ptr),
+                                                            C.c_void_p(d_mask_ptr) if d_mask_ptr else None,
+                                                            C.c_void_p(d_types_ptr) if d_types_ptr else None, n, seq,
+                                                            1 if sigmoid else 0, C.c_void_p(d_out_ptr),
+                                                            1 if sync else 0))
 
     def encode_images_u8_device(self, d_ptr: int, n: int, h: int, w: int, d_out_ptr: int, normalize: bool = True,
                                 sync: bool = True) -> None:
@@ -901,32 +928,39 @@ def debug_clip_text_embed(ids, tok, pos, device: int = 0, cls=None):
     return _host(x), _host(eot)
 
 
-def debug_embed_ln(ids, mask, word, pos, type0, gamma, beta, eps: float, pad: Optional[int] = None, device: int = 0):
+def debug_embed_ln(ids, mask, word, pos, type0, gamma, beta, eps: float, pad: Optional[int] = None, device: int = 0,
+                   type_ids=None):
     """BERT (pad None; pos None for GTE, which has no position table) or RoBERTa (pad = the pad id; type0 None for
     MPNet) embedding + LayerNorm of ids int32 [n, S] with an optional mask [n, S] -> (x fp32 [n*S, w], its bf16 copy as
-    fp32, kv_len int32 [n])."""
+    fp32, kv_len int32 [n]).  type_ids (BERT with positions: a sentence pair's int32 [n, S]): type0 is the whole
+    token-type table [rows, w] and each token adds its own row."""
     ia, wd = _as(ids, np.int32), _as(word, np.float32)
     p = None if pos is None else _as(pos, np.float32)
     n, S = ia.shape
     vocab, w = wd.shape
     m = None if mask is None else _as(mask, np.int32)
     t = None if type0 is None else _as(type0, np.float32)
+    ti = None if type_ids is None else _as(type_ids, np.int32)
     g, b = _as(gamma, np.float32), _as(beta, np.float32)
     if m is not None and m.shape != ia.shape:
         raise ValueError(f"expected mask {ia.shape}, got {m.shape}")
+    if ti is not None and (ti.shape != ia.shape or t is None or t.ndim != 2 or t.shape[1] != w):
+        raise ValueError(f"type_ids must be {ia.shape} with a token-type table [rows, {w}]")
+    type_rows = 0 if ti is None else t.shape[0]
     need = S if pad is None else pad + S + 1
     if p is not None and (p.ndim != 2 or p.shape[1] != w or p.shape[0] < need):
         raise ValueError(f"expected pos [>= {need}, {w}], got {p.shape}")
-    if (t is not None and t.size != w) or g.size != w or b.size != w:
+    if (t is not None and ti is None and t.size != w) or g.size != w or b.size != w:
         raise ValueError(f"type0, gamma and beta must have {w} values")
     d = _Staging(device)
     di, dm, dwd, dp, dt = d.up(ia, "int32"), d.up(m, "int32"), d.up(wd), d.up(p), d.up(t)
+    dti = d.up(ti, "int32")
     dg, db = d.up(g), d.up(b)
     x, h, kv_len = d.empty((n * S, w)), d.empty((n * S, w), "bfloat16"), d.empty(n, "int32")
     N.check(N.load().b200_debug_embed_ln(device, _dptr(di), _dptr(dm), _dptr(dwd), _dptr(dp),
                                          0 if p is None else p.shape[0], _dptr(dt),
                                          _dptr(dg), _dptr(db), eps, n, S, w, vocab, -1 if pad is None else pad, _dptr(x),
-                                         _dptr(h), _dptr(kv_len), d.stream))
+                                         _dptr(h), _dptr(kv_len), _dptr(dti), type_rows, d.stream))
     return _host(x), _host(h), _host(kv_len)
 
 
@@ -986,6 +1020,24 @@ def debug_text_head(x, S: int, kv_len, proj, bias=None, normalize: bool = True, 
     out = d.empty((n, E))
     N.check(N.load().b200_debug_text_head(device, _dptr(dx), _dptr(dkl), n, S, w, _dptr(dp), _dptr(dbias), E,
                                           int(normalize), _dptr(out), d.stream))
+    return _host(out)
+
+
+def debug_cls_head(x, S: int, pool_w, pool_b, cls_w, cls_b, sigmoid: bool = False, device: int = 0) -> np.ndarray:
+    """BertForSequenceClassification's head over x fp32 [n*S, w]: tanh(pool_w [w, w] . x[b*S] + pool_b) through the
+    classifier cls_w [L, w], cls_b [L], then the sigmoid if sigmoid -> fp32 [n, L]."""
+    xa, pw, pb, cw, cb = (_as(a, np.float32) for a in (x, pool_w, pool_b, cls_w, cls_b))
+    w, L = pw.shape[0], cw.shape[0]
+    if xa.ndim != 2 or xa.shape[1] != w or xa.shape[0] % S != 0:
+        raise ValueError(f"expected x [n * {S}, {w}], got {xa.shape}")
+    if pw.shape != (w, w) or pb.shape != (w,) or cw.shape != (L, w) or cb.shape != (L,):
+        raise ValueError("expected pool_w [w, w], pool_b [w], cls_w [L, w], cls_b [L]")
+    n = xa.shape[0] // S
+    d = _Staging(device)
+    dx, dpw, dpb, dcw, dcb = d.up(xa), d.up(pw), d.up(pb), d.up(cw), d.up(cb)
+    out = d.empty((n, L))
+    N.check(N.load().b200_debug_cls_head(device, _dptr(dx), n, S, w, _dptr(dpw), _dptr(dpb), _dptr(dcw), _dptr(dcb), L,
+                                         int(sigmoid), _dptr(out), d.stream))
     return _host(out)
 
 

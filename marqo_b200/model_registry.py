@@ -579,6 +579,31 @@ def _multilingual_clip_models() -> Dict[str, dict]:
 MULTILINGUAL_CLIP_MODELS: Dict[str, dict] = _multilingual_clip_models()
 
 
+def _cross_encoder_arch(width: int, layers: int, heads: int) -> dict:
+    """A cross-encoder's BertForSequenceClassification shape (config.json, verify): uncased vocabulary 30522, 512
+    positions, 2 token types, mlp 4 x width, one label."""
+    return {**_bert_arch(width, layers, heads), "num_labels": 1}
+
+
+# The BERT cross-encoders Marqo's text reranker (`reRanker` in a search: reranking/cross_encoders.py ReRankerText)
+# loads through sentence-transformers' CrossEncoder, which cross_encoder.B200CrossEncoder serves.  They are scorers of
+# (query, passage) pairs, not embedders, so this table is kept apart from the vectorise registry: find_model,
+# all_models and served_models do not read it.  Shapes from the config.json files (verify); TinyBERT-L-2 runs at width
+# 128 with heads of 64, the MiniLMs at width 384 with heads of 32.  ms-marco-TinyBERT-L-4 (312 wide, head dim 26) and
+# the non-BERT cross-encoders are not served.
+CROSS_ENCODER_MODELS: Dict[str, dict] = {
+    name: {"name": name, "arch": _cross_encoder_arch(*shape)}
+    for name, shape in (
+        ("cross-encoder/ms-marco-TinyBERT-L-2", (128, 2, 2)),
+        ("cross-encoder/ms-marco-TinyBERT-L-2-v2", (128, 2, 2)),
+        ("cross-encoder/ms-marco-MiniLM-L-2-v2", (384, 2, 12)),
+        ("cross-encoder/ms-marco-MiniLM-L-4-v2", (384, 4, 12)),
+        ("cross-encoder/ms-marco-MiniLM-L-6-v2", (384, 6, 12)),
+        ("cross-encoder/ms-marco-MiniLM-L-12-v2", (384, 12, 12)),
+    )
+}
+
+
 def _count(sd: dict, prefix: str) -> int:
     """The number of distinct indices i among the keys prefix + "i.*"."""
     return len({k[len(prefix):].split(".")[0] for k in sd if k.startswith(prefix)})

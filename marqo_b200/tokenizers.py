@@ -2,7 +2,8 @@
 
 * `WordPieceTokenizer` is called the way hugging_face_model.py:179-185 calls its AutoTokenizer:
   `tok(sentences, padding=True, truncation=True, max_length=N, return_tensors="np")` -> {input_ids, attention_mask,
-  token_type_ids}.
+  token_type_ids}; and the way sentence-transformers' CrossEncoder calls it on sentence pairs:
+  `tok(texts_a, texts_b, padding=True, truncation='longest_first', max_length=N)` -> rows "[CLS] A [SEP] B [SEP]".
 * `MPNetTokenizer` is the same WordPiece pipeline with MPNetTokenizer's special tokens ("<s> A </s>", <pad>, [UNK]) and
   the same call -> {input_ids, attention_mask}.
 * `XLMRTokenizer` is XLMRobertaTokenizer on a SentencePiece Unigram model (multilingual-e5): the same call ->
@@ -60,6 +61,23 @@ class _Tokenizer:
         L = L.value
         return ids.reshape(-1)[: n * L].reshape(n, L), mask.reshape(-1)[: n * L].reshape(n, L)
 
+    def _encode_pairs(self, texts_a: Sequence[str], texts_b: Sequence[str], max_length: int):
+        if len(texts_a) != len(texts_b):
+            raise ValueError(f"{len(texts_a)} first texts and {len(texts_b)} second texts")
+        a = [t.encode("utf-8", "replace") for t in texts_a]
+        b = [t.encode("utf-8", "replace") for t in texts_b]
+        n = len(a)
+        pa, pb = (C.c_char_p * n)(*a), (C.c_char_p * n)(*b)
+        la = np.asarray([len(x) for x in a], dtype=np.int64)
+        lb = np.asarray([len(x) for x in b], dtype=np.int64)
+        out = [np.empty(n * max_length, dtype=np.int32) for _ in range(3)]
+        L = C.c_int(0)
+        N.check(self._lib.b200_tokenizer_encode_pairs(self._h, C.cast(pa, C.c_void_p), la.ctypes.data_as(C.c_void_p),
+                                                      C.cast(pb, C.c_void_p), lb.ctypes.data_as(C.c_void_p), n,
+                                                      int(max_length), *[o.ctypes.data_as(C.c_void_p) for o in out],
+                                                      C.byref(L)))
+        return tuple(o[: n * L.value].reshape(n, L.value) for o in out)
+
 
 def _read(path_or_bytes: Union[str, Path, bytes]) -> bytes:
     if isinstance(path_or_bytes, bytes):
@@ -78,16 +96,24 @@ class WordPieceTokenizer(_Tokenizer):
         super().__init__(h)
         self.model_max_length = model_max_length
 
-    def __call__(self, sentences: Union[str, List[str]], padding=True, truncation=True, max_length: int = None,
-                 return_tensors: str = "np") -> Dict[str, np.ndarray]:
-        if padding is not True or truncation is not True:
-            raise ValueError("WordPieceTokenizer implements the reference's call only: padding=True, truncation=True")
-        single = isinstance(sentences, str)
-        ids, mask = self._encode([sentences] if single else list(sentences), max_length or self.model_max_length)
-        out = {"input_ids": ids.astype(np.int64)}
-        if self._token_type_ids:
-            out["token_type_ids"] = np.zeros_like(ids, dtype=np.int64)
-        out["attention_mask"] = mask.astype(np.int64)
+    def __call__(self, sentences: Union[str, List[str]], text_pair: List[str] = None, padding=True, truncation=True,
+                 max_length: int = None, return_tensors: str = "np") -> Dict[str, np.ndarray]:
+        if text_pair is not None:
+            if padding is not True or truncation != "longest_first" or not self._token_type_ids:
+                raise ValueError("sentence pairs are encoded as CrossEncoder asks only: a BERT WordPiece tokenizer, "
+                                 "padding=True, truncation='longest_first'")
+            ids, mask, types = self._encode_pairs(list(sentences), list(text_pair), max_length or self.model_max_length)
+            out = {"input_ids": ids.astype(np.int64), "token_type_ids": types.astype(np.int64),
+                   "attention_mask": mask.astype(np.int64)}
+        else:
+            if padding is not True or truncation is not True:
+                raise ValueError("WordPieceTokenizer implements the reference's call only: padding=True, truncation=True")
+            single = isinstance(sentences, str)
+            ids, mask = self._encode([sentences] if single else list(sentences), max_length or self.model_max_length)
+            out = {"input_ids": ids.astype(np.int64)}
+            if self._token_type_ids:
+                out["token_type_ids"] = np.zeros_like(ids, dtype=np.int64)
+            out["attention_mask"] = mask.astype(np.int64)
         if return_tensors == "pt":
             import torch
             return {k: torch.from_numpy(v) for k, v in out.items()}

@@ -360,6 +360,19 @@ def random_bert_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     return sd
 
 
+def random_cross_encoder_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
+    """Seeded random weights of a BERT cross-encoder under BertForSequenceClassification's names (arch: the registry's
+    cross-encoder block): random_bert_weights under "bert.", the pooler and the classifier of num_labels rows."""
+    w, labels = arch["width"], arch["num_labels"]
+    sd = {"bert." + k: v for k, v in random_bert_weights(arch, seed).items()}
+    g = _rng(seed + 1)
+    sd["bert.pooler.dense.weight"] = _lin(g, w, w, 1.5)
+    sd["bert.pooler.dense.bias"] = _vec(g, w)
+    sd["classifier.weight"] = _lin(g, labels, w, 2.0)
+    sd["classifier.bias"] = _vec(g, labels)
+    return sd
+
+
 def random_xlmr_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     """Seeded random weights under HF XLMRobertaModel parameter names (arch: the registry's XLM-R block): BertModel's
     names with max_pos position rows and type_vocab (1) token-type rows."""
