@@ -376,6 +376,24 @@ typedef struct b200_model_desc {
      * B200_ERR_INVALID_ARG, and b200_model_create refuses cls_labels on any other arch the same way.  0: the usual
      * head. */
     int32_t cls_labels;
+    /* OWL-ViT's open-vocabulary detector (transformers OwlViTForObjectDetection, eval mode; verify), arch
+     * B200_ARCH_CLIP only, with a CLIP ViT vision tower and the CLIP text tower.  owl_detect = 1 replaces the image
+     * embedding head: with G = image_size / patch and the trunk's N = G^2 + 1 token rows x of an image,
+     *   e = ln_post(x) (every row);  f_p = layer_norm(e_p * e_0) for the patches p = 1 .. G^2 (row-major, token
+     *   1 + r G + c);
+     *   logit_p = (c^ . q^ + logit_shift(f_p)) * (ELU(logit_scale(f_p)) + 1), c^ = c / (|c| + 1e-6) for
+     *   c = class_head.dense0(f_p) [embed_dim], and q^ = u / (|u| + 1e-6) for the query's unit text embedding
+     *   u = t / |t| (t: ln_final of the query's EOT row, at argmax(id), times text_projection);
+     *   box_p = sigmoid(box_head.dense2(GELU(dense1(GELU(dense0(f_p))))) + box_bias[p]) as (cx, cy, w, h), box_bias
+     *   being the logits of the patch's corner ((c + 1) / G, (r + 1) / G) and of its size 1 / G, each + 1e-4.
+     * Weights: the CLIP names of both towers without visual.proj, and the detector's own layer_norm.{weight, bias}
+     * [width], class_head.dense0.{weight [embed_dim, width], bias}, class_head.logit_shift.{weight [1, width], bias
+     * [1]}, class_head.logit_scale.{weight, bias} (the same shapes), box_head.dense0 / dense1.{weight [width, width],
+     * bias} and box_head.dense2.{weight [4, width], bias [4]}; b200_model_finalize refuses a missing one with
+     * B200_ERR_MISSING_WEIGHT.  resize_squash must be 1, vision.width <= 1024 and embed_dim + 2 rounded up to 64 at
+     * most vision.width.  Such a model is run by b200_model_detect_images_u8 only; every encode call refuses it
+     * with B200_ERR_INVALID_ARG.  0: the usual heads. */
+    int32_t owl_detect;
 } b200_model_desc;
 
 int b200_model_create(int device, const b200_model_desc* desc, b200_model** out);
@@ -468,6 +486,13 @@ int b200_model_classify_tokens(b200_model* m, const int32_t* ids, const int32_t*
 /* The same with device-resident inputs and output, asynchronous on the model's stream unless sync != 0. */
 int b200_model_classify_tokens_device(b200_model* m, const int32_t* d_ids, const int32_t* d_attn_mask,
                                       const int32_t* d_type_ids, int n, int seq, int activation, float* d_out, int sync);
+/* OWL-ViT detection (owl_detect = 1, see b200_model_desc): one text query, query_ids int32 [seq] on the host (seq <=
+ * text.ctx), scored against each of n uint8 HWC images [h, w, 3] (hwc, host), which are squashed to image_size by the
+ * Pillow-exact resize.  logits: fp32 host [n, G^2], what OwlViTForObjectDetection returns as logits[..., 0]; boxes: fp32
+ * host [n, G^2, 4], its pred_boxes (cx, cy, w, h in [0, 1]).  n larger than the batch the workspaces hold runs in
+ * sub-batches.  A model without the detector, seq outside 1 .. text.ctx, or n, h or w <= 0: B200_ERR_INVALID_ARG. */
+int b200_model_detect_images_u8(b200_model* m, const uint8_t* hwc, int n, int h, int w, const int32_t* query_ids,
+                                int seq, float* logits, float* boxes);
 /* Images of mixed sizes in one call (every vision tower that takes uint8 images): image i is uint8 HWC
  * [heights[i], widths[i], 3] at hwc[i]; hwc, heights and widths are host arrays of n.  The images are resized to the
  * model's S x S by the tower's rule (shortest side + centre crop, or the squash) in one pass over each sub-batch, two
@@ -707,6 +732,24 @@ int b200_debug_bert_head(int device, const float* x, const int32_t* kv_len, int 
  * w a multiple of 4, <= 1024. */
 int b200_debug_text_head(int device, const float* x, const int32_t* kv_len, int n, int S, int w, const float* proj,
                          const float* bias, int E, int normalize, float* out, void* stream);
+/* OWL-ViT's patch features over the trunk rows x fp32 [n*N, w] (N = G^2 + 1 rows per image, class row first):
+ * out[b*G^2 + p - 1] = LN_det(LN_post(x[b*N + p]) * LN_post(x[b*N])) for p = 1 .. G^2, LN_post by post_g / post_b and
+ * LN_det by det_g / det_b (both eps).  out bf16 [n*G^2, w].  w a multiple of 128, <= 1024. */
+int b200_debug_owl_merge_ln(int device, const float* x, int n, int N, int w, const float* post_g, const float* post_b,
+                            const float* det_g, const float* det_b, float eps, void* out, void* stream);
+/* OWL-ViT's class logits from the class head GEMM's rows c fp32 [M, ldc] (columns 0 .. E-1 dense0 with its bias, E
+ * logit_shift, E + 1 logit_scale) and the query's text embedding t fp32 [E] (not normalised): out[r] = (c^ . q^ +
+ * shift) * (ELU(scale) + 1) with c^ = c / (|c| + 1e-6), u = t / |t| and q^ = u / (|u| + 1e-6).  out fp32 [M]. */
+int b200_debug_owl_class_logits(int device, const float* c, int ldc, int M, int E, const float* t, float* out,
+                                void* stream);
+/* OWL-ViT's boxes from the box head's second hidden rows a bf16 [M, w] (after its GELU): out[r, j] = sigmoid(w2[j] . a[r]
+ * + b2[j] + box_bias[r % P, j]) for w2 fp32 [4, w], b2 [4], box_bias fp32 [P, 4].  out fp32 [M, 4]. */
+int b200_debug_owl_boxes(int device, const void* a, int M, int w, int P, const float* w2, const float* b2,
+                         const float* box_bias, float* out, void* stream);
+/* OWL-ViT's box bias of a G x G grid as the model builds it, in fp64 rounded to fp32 (host-only): out fp32 [G^2, 4],
+ * row r G + c = (logit((c + 1) / G), logit((r + 1) / G), logit(1 / G), logit(1 / G)) with logit(v) = log(v + 1e-4) -
+ * log1p(-v + 1e-4). */
+int b200_debug_owl_box_bias(int G, float* out);
 /* BertForSequenceClassification's head over x fp32 [n*S, w]: p = tanh(pool_w [w, w] . x[b*S] + pool_b [w]), then
  * out[b, l] = cls_w[l] . p + cls_b[l] for cls_w [L, w], cls_b [L], through the sigmoid if sigmoid != 0.  out fp32
  * [n, L].  w <= 1024. */

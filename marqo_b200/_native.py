@@ -55,7 +55,7 @@ class ModelDesc(C.Structure):
         ("convnext_head", C.c_int32), ("resize_squash", C.c_int32), ("eva_rope_ref_grid", C.c_int32),
         ("rope_theta", C.c_float), ("rope_ntk_factor", C.c_float),
         ("attn_pool_heads", C.c_int32), ("text_embed_cls", C.c_int32), ("text_proj_dim", C.c_int32),
-        ("cls_labels", C.c_int32),
+        ("cls_labels", C.c_int32), ("owl_detect", C.c_int32),
     ]
 
 
@@ -119,6 +119,7 @@ _SIGNATURES = {
     "b200_model_encode_tokens_device": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
     "b200_model_classify_tokens": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "b200_model_classify_tokens_device": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
+    "b200_model_detect_images_u8": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "b200_model_encode_images_u8_ragged": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P]),
     "b200_model_encode_images_u8_ragged_device": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int]),
     "b200_model_set_stream": (C.c_int, [_P, _P, C.c_int]),
@@ -154,6 +155,10 @@ _SIGNATURES = {
     "b200_debug_bert_head": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_text_head": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P]),
     "b200_debug_cls_head": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_owl_merge_ln": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, C.c_float, _P, _P]),
+    "b200_debug_owl_class_logits": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
+    "b200_debug_owl_boxes": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
+    "b200_debug_owl_box_bias": (C.c_int, [C.c_int, _P]),
     "b200_debug_l2_rows": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_stem_im2col": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
     "b200_debug_avgpool2": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),

@@ -458,6 +458,53 @@ int b200_debug_cls_head(int device, const float* x, int n, int S, int w, const f
     });
 }
 
+int b200_debug_owl_merge_ln(int device, const float* x, int n, int N, int w, const float* post_g, const float* post_b,
+                            const float* det_g, const float* det_b, float eps, void* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && post_g && post_b && det_g && det_b && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && N >= 2 && w > 0, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::owl_merge_ln(x, n, N, w, post_g, post_b, det_g, det_b, eps, static_cast<bf16*>(out), s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_owl_class_logits(int device, const float* c, int ldc, int M, int E, const float* t, float* out,
+                                void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(c && t && out, "NULL buffer");
+        MB_CHECK_ARG(M > 0 && E > 0 && ldc >= E + 2, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::owl_class_logits(c, ldc, M, E, t, out, s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_owl_boxes(int device, const void* a, int M, int w, int P, const float* w2, const float* b2,
+                         const float* box_bias, float* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(a && w2 && b2 && box_bias && out, "NULL buffer");
+        MB_CHECK_ARG(M > 0 && w > 0 && w % 4 == 0 && P > 0, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::owl_boxes(static_cast<const bf16*>(a), M, w, P, w2, b2, box_bias, out, s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_owl_box_bias(int G, float* out) {
+    return guarded([&] {
+        MB_CHECK_ARG(out != nullptr, "NULL buffer");
+        MB_CHECK_ARG(G > 0 && G <= 1024, "grid %d out of range", G);
+        kernels::owl_box_bias(G, out);
+    });
+}
+
 int b200_debug_l2_rows(int device, const float* src, int n, int E, int normalize, float* out, void* stream) {
     return guarded([&] {
         MB_CHECK_ARG(src && out, "NULL buffer");

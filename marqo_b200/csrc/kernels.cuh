@@ -102,6 +102,22 @@ int text_head(const float* x, const int32_t* kv_len, int n, int S, int w, const 
 int cls_head(const float* x, int S, int n, int w, const float* wp, const float* bp, const float* wc, const float* bc,
              int L, int sigmoid, float* out, cudaStream_t s);
 
+// OWL-ViT's detection head (transformers OwlViTForObjectDetection, verify).  owl_merge_ln: for the trunk rows x fp32
+// [n * N, w] of n images (N = P + 1, class row first), out[b * P + p - 1] = LN(LN_post(x[b N + p]) * LN_post(x[b N]))
+// with (post_g, post_b) and then (det_g, det_b), both at eps, for p = 1 .. P; out bf16 [n * P, w], w <= 1024.
+int owl_merge_ln(const float* x, int n, int N, int w, const float* post_g, const float* post_b, const float* det_g,
+                 const float* det_b, float eps, __nv_bfloat16* out, cudaStream_t s);
+// Class logits from the class-head GEMM rows c fp32 [M, ldc] (dense0 in columns 0 .. E-1, logit_shift in E,
+// logit_scale in E + 1, biases included) and the query's text embedding t fp32 [E]: out[r] = (c^ . q^ + shift) *
+// (ELU(scale) + 1), c^ = c / (|c| + 1e-6), q^ = u / (|u| + 1e-6) for u = t / |t|.  out fp32 [M].
+int owl_class_logits(const float* c, int ldc, int M, int E, const float* t, float* out, cudaStream_t s);
+// Boxes from the box head's second GELU rows a bf16 [M, w]: out[r] = sigmoid(w2 a[r] + b2 + box_bias[r % P]) for w2
+// fp32 [4, w], b2 [4] and box_bias fp32 [P, 4]; out fp32 [M, 4].
+int owl_boxes(const __nv_bfloat16* a, int M, int w, int P, const float* w2, const float* b2, const float* box_bias,
+              float* out, cudaStream_t s);
+// The box bias table of a G x G grid (HF compute_box_bias), built in fp64 on the host: out fp32 [G^2, 4].
+void owl_box_bias(int G, float* out);
+
 void f32_to_bf16(const float* src, __nv_bfloat16* dst, long long n, cudaStream_t s);
 // conv1.weight [w, 3*p*p] -> bf16 [w, kpad] zero padded
 void pad_rows_to_bf16(const float* src, int rows, int k, int kpad, __nv_bfloat16* dst, cudaStream_t s);

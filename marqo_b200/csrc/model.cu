@@ -172,6 +172,17 @@ struct ConvnextW {
     DeviceBuffer<__nv_bfloat16> h, u;      // [pixels, C], [pixels, 4C]
 };
 
+// OWL-ViT's detection head (owl_detect): the detector's LayerNorm; the class head as one Linear [ncls, width] whose
+// rows are class_head.dense0 (embed_dim rows), logit_shift, logit_scale and zero rows up to a multiple of 64, with its
+// fp32 bias; box_head.dense0 / dense1 (bf16, GELU in their epilogues) and dense2 (fp32 [4, width], owl_boxes); the
+// box bias table fp32 [G^2, 4].
+struct OwlW {
+    const float *ln_w = nullptr, *ln_b = nullptr, *b_cls = nullptr, *b_box0 = nullptr, *b_box1 = nullptr;
+    const float *w_box2 = nullptr, *b_box2 = nullptr, *box_bias = nullptr;
+    const __nv_bfloat16 *w_cls = nullptr, *w_box0 = nullptr, *w_box1 = nullptr;
+    int ncls = 0;
+};
+
 }  // namespace
 
 struct b200_model {
@@ -185,6 +196,8 @@ struct b200_model {
     TowerW vision, text;
     ResnetW resnet;   // VisionKind::RESNET's image tower (vision.tokens = grid^2 + 1)
     ConvnextW convnext;   // VisionKind::CONVNEXT's image tower (vision.tokens = the stem's (S/4)^2 pixels)
+    OwlW owl;             // owl_detect's head
+    DeviceBuffer<float> det;   // owl_detect: [max_batch, G^2] logits, then [max_batch, G^2, 4] boxes
     // workspaces (sized for max_tokens tokens)
     long long max_tokens = 0;
     DeviceBuffer<float> x;
@@ -376,6 +389,21 @@ void check_vision(const b200_model_desc& d, VisionKind kind) {
     }
     }
     MB_CHECK_ARG(d.resize_squash == 0 || d.resize_squash == 1, "resize_squash %d must be 0 or 1", d.resize_squash);
+}
+
+// OWL-ViT's detector: the CLIP ViT and text towers, squashed images, the merge LayerNorm's width limit, and a class
+// head of embed_dim + 2 rows padded to 64 whose fp32 output fits the trunk's residual rows
+void check_owl(const b200_model_desc& d, const Kinds& k) {
+    MB_CHECK_ARG(d.owl_detect == 0 || d.owl_detect == 1, "owl_detect %d must be 0 or 1", d.owl_detect);
+    if (!d.owl_detect) return;
+    MB_CHECK_ARG(d.arch == B200_ARCH_CLIP, "owl_detect: only the CLIP arch takes OWL-ViT's detection head");
+    MB_CHECK_ARG(k.vision == VisionKind::CLIP_VIT && k.text == TextKind::CLIP,
+                 "owl_detect: the detector needs the CLIP ViT vision tower and the CLIP text tower");
+    MB_CHECK_ARG(d.resize_squash == 1, "owl_detect: OWL-ViT squashes its images (resize_squash 1)");
+    MB_CHECK_ARG(d.vision.width <= 1024, "owl_detect: vision.width %d must be <= 1024", d.vision.width);
+    MB_CHECK_ARG((int)round_up((size_t)d.embed_dim + 2, 64) <= d.vision.width,
+                 "owl_detect: embed_dim %d + 2 rounded up to 64 must be at most vision.width %d", d.embed_dim,
+                 d.vision.width);
 }
 
 void check_text(const b200_model_desc& d, const Kinds& k) {
@@ -974,6 +1002,42 @@ void build_coca_pooler(b200_model* m, TowerW& T) {
     T.proj = param(m, "visual.proj", d * m->desc.embed_dim);
 }
 
+// OWL-ViT's detection head (OwlW) under the checkpoint's own names, and its box bias table, built in fp64 on the host.
+void build_owl(b200_model* m, const TowerW& T) {
+    OwlW& D = m->owl;
+    const long long w = T.d.width, E = m->desc.embed_dim;
+    D.ln_w = param(m, "layer_norm.weight", w);
+    D.ln_b = param(m, "layer_norm.bias", w);
+    D.ncls = (int)round_up((size_t)E + 2, 64);
+    std::vector<float> rows((size_t)D.ncls * w, 0.f), bias((size_t)D.ncls, 0.f);
+    const struct {
+        const char* name;
+        long long n;
+    } parts[3] = {{"class_head.dense0.", E}, {"class_head.logit_shift.", 1}, {"class_head.logit_scale.", 1}};
+    long long at = 0;
+    for (const auto& pt : parts) {
+        const std::string p = pt.name;
+        const std::vector<float> wt = to_host(param(m, p + "weight", pt.n * w), (size_t)(pt.n * w));
+        const std::vector<float> bt = to_host(param(m, p + "bias", pt.n), (size_t)pt.n);
+        std::copy(wt.begin(), wt.end(), rows.begin() + at * w);
+        std::copy(bt.begin(), bt.end(), bias.begin() + at);
+        m->raw.erase(p + "weight");
+        m->raw.erase(p + "bias");
+        at += pt.n;
+    }
+    D.w_cls = upload_bf16(m, rows);
+    D.b_cls = upload_derived(m, bias);
+    D.w_box0 = to_bf16(m, "box_head.dense0.weight", w * w);
+    D.b_box0 = param(m, "box_head.dense0.bias", w);
+    D.w_box1 = to_bf16(m, "box_head.dense1.weight", w * w);
+    D.b_box1 = param(m, "box_head.dense1.bias", w);
+    D.w_box2 = param(m, "box_head.dense2.weight", 4 * w);
+    D.b_box2 = param(m, "box_head.dense2.bias", 4);
+    std::vector<float> bb((size_t)T.grid * T.grid * 4);
+    kernels::owl_box_bias(T.grid, bb.data());
+    D.box_bias = upload_derived(m, bb);
+}
+
 void build_vision(b200_model* m) {
     TowerW& T = m->vision;
     const long long w = T.d.width;
@@ -993,7 +1057,10 @@ void build_vision(b200_model* m) {
         }
         T.ln_out_w = param(m, "visual.ln_post.weight", w);
         T.ln_out_b = param(m, "visual.ln_post.bias", w);
-        T.proj = param(m, "visual.proj", w * m->desc.embed_dim);
+        if (m->desc.owl_detect)
+            build_owl(m, T);
+        else
+            T.proj = param(m, "visual.proj", w * m->desc.embed_dim);
         break;
     case VisionKind::SIGLIP_VIT:
         build_vit(m, T, "visual.trunk.patch_embed.proj.weight", 0);
@@ -1404,6 +1471,25 @@ void forward_images_eager(b200_model* m, Counter& c, const uint8_t* u8, const fl
     }
 }
 
+// OWL-ViT's detection over n images (device uint8 [n, S, S, 3]) and the query's text embedding t [E] (device): the
+// trunk's rows in x; the merged patch features -> h; the class head GEMM -> x (fp32 [M, ncls], the trunk's rows are
+// no longer read) and the logits; box_head dense0 -> u, dense1 -> o, then dense2 and the box bias -> boxes.
+void forward_detect_eager(b200_model* m, Counter& c, const uint8_t* u8, int n, const float* t, float* logits,
+                          float* boxes) {
+    const TowerW& T = m->vision;
+    const OwlW& D = m->owl;
+    const int w = T.d.width, P = T.grid * T.grid, M = n * P;
+    float* x = m->x.get();
+    __nv_bfloat16 *h = m->h.get(), *u = m->u.get(), *o = m->o.get();
+    forward_vit(m, c, T, u8, nullptr, n);
+    c.n += kernels::owl_merge_ln(x, n, T.tokens, w, T.ln_out_w, T.ln_out_b, D.ln_w, D.ln_b, T.eps, h, m->stream);
+    linear(m, c, h, M, w, D.w_cls, D.ncls, epilogue(x, D.ncls, D.b_cls, gemm::ACT_NONE, true));
+    c.n += kernels::owl_class_logits(x, D.ncls, M, m->desc.embed_dim, t, logits, m->stream);
+    linear(m, c, h, M, w, D.w_box0, w, epilogue(u, w, D.b_box0, gemm::ACT_GELU));
+    linear(m, c, u, M, w, D.w_box1, w, epilogue(o, w, D.b_box1, gemm::ACT_GELU));
+    c.n += kernels::owl_boxes(o, M, w, P, D.w_box2, D.b_box2, D.box_bias, boxes, m->stream);
+}
+
 // d_types: token-type ids [n, S] of a classifier (NULL: all 0); normalize is then the classifier's activation (0
 // identity, 1 sigmoid)
 void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const int32_t* d_mask, const int32_t* d_types,
@@ -1523,6 +1609,12 @@ void forward_tokens(b200_model* m, Counter& c, const int32_t* d_ids, const int32
                 [&](Counter& cc) { forward_tokens_eager(m, cc, d_ids, d_mask, d_types, n, S, normalize, d_out); });
 }
 
+void forward_detect(b200_model* m, Counter& c, const uint8_t* u8, int n, const float* t, float* logits, float* boxes) {
+    const b200_model::GraphKey key{2, n, 0, 0, u8, t, logits, boxes};
+    run_graphed(m, c, key, (long long)n * m->vision.tokens,
+                [&](Counter& cc) { forward_detect_eager(m, cc, u8, n, t, logits, boxes); });
+}
+
 void require_ready(b200_model* m) {
     MB_CHECK_ARG(m != nullptr, "model is NULL");
     if (!m->finalized) fail(B200_ERR_INVALID_ARG, "b200_model_finalize has not been called");
@@ -1584,10 +1676,16 @@ void encode_images_u8_ragged_dev(b200_model* m, Counter& c, const uint8_t* const
     }
 }
 
+// every image encode call: a vision tower with an embedding head
+void check_encodes_images(b200_model* m) {
+    MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
+    MB_CHECK_ARG(!m->desc.owl_detect, "this model is an OWL-ViT detector: detect images with a query");
+}
+
 // the arguments of a ragged image call, all checked before anything is written
 void check_ragged_args(b200_model* m, const uint8_t* const* imgs, const int32_t* h, const int32_t* w, int n) {
     MB_CHECK_ARG(imgs && h && w, "NULL array");
-    MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
+    check_encodes_images(m);
     MB_CHECK_ARG(n > 0, "n must be positive");
     for (int i = 0; i < n; ++i) {
         MB_CHECK_ARG(imgs[i] != nullptr, "image %d is NULL", i);
@@ -1613,6 +1711,7 @@ void encode_tokens_dev(b200_model* m, Counter& c, const int32_t* d_ids, const in
 // refuse one
 void check_tokens_args(b200_model* m, int n, int S, bool classify = false) {
     MB_CHECK_ARG(m->kind.text != TextKind::NONE, "this model has no text tower");
+    MB_CHECK_ARG(!m->desc.owl_detect, "this model is an OWL-ViT detector: detect images with a query");
     MB_CHECK_ARG(!classify || m->desc.cls_labels > 0, "this model has no classification head (cls_labels 0)");
     MB_CHECK_ARG(classify || m->desc.cls_labels == 0, "this model is a classifier (cls_labels %d): classify its tokens",
                  m->desc.cls_labels);
@@ -1699,6 +1798,7 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         MB_CHECK_ARG(kind.vision != VisionKind::NONE || kind.text != TextKind::NONE, "model has no tower");
         check_vision(*desc, kind.vision);
         check_text(*desc, kind);
+        check_owl(*desc, kind);
         DeviceGuard g(device);
         std::unique_ptr<b200_model> m(new b200_model());   // released under the guard if the set-up fails
         m->device = device;
@@ -1790,6 +1890,7 @@ int b200_model_finalize(b200_model* m) {
             const int S = m->vision.d.image_size;
             m->resized = DeviceBuffer<uint8_t>((size_t)B * S * S * 3);
         }
+        if (m->desc.owl_detect) m->det = DeviceBuffer<float>((size_t)B * m->vision.grid * m->vision.grid * 5);
         MB_CUDA(cudaStreamSynchronize(m->stream));
         m->aux = DeviceBuffer<int32_t>((size_t)B);
         m->out_dev = DeviceBuffer<float>((size_t)B * E);
@@ -1803,7 +1904,7 @@ int b200_model_encode_images_u8(b200_model* m, const uint8_t* hwc, int n, int h,
     return guarded([&] {
         require_ready(m);
         MB_CHECK_ARG(hwc && out, "NULL buffer");
-        MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
+        check_encodes_images(m);
         MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
         std::lock_guard<std::mutex> lk(m->mu);
         DeviceGuard g(m->device);
@@ -1818,6 +1919,49 @@ int b200_model_encode_images_u8(b200_model* m, const uint8_t* hwc, int n, int h,
                                     cudaMemcpyHostToDevice, m->stream));
             encode_images_u8_dev(m, tr.c, m->in_dev.get(), nb, h, w, normalize, m->out_dev.get());
             MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
+                                    m->stream));
+            MB_CUDA(cudaStreamSynchronize(m->stream));
+        }
+        tr.finish();
+    });
+}
+
+int b200_model_detect_images_u8(b200_model* m, const uint8_t* hwc, int n, int h, int w, const int32_t* query_ids,
+                                int seq, float* logits, float* boxes) {
+    return guarded([&] {
+        require_ready(m);
+        MB_CHECK_ARG(hwc && query_ids && logits && boxes, "NULL buffer");
+        MB_CHECK_ARG(m->desc.owl_detect, "this model has no OWL-ViT detection head (owl_detect 0)");
+        MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
+        MB_CHECK_ARG(seq > 0 && seq <= m->text.tokens, "query length %d out of range (1..%d)", seq, m->text.tokens);
+        std::lock_guard<std::mutex> lk(m->mu);
+        DeviceGuard g(m->device);
+        const TowerW& T = m->vision;
+        const int S = T.d.image_size, P = T.grid * T.grid;
+        const int cap = image_batch_cap(m);
+        const size_t img_bytes = (size_t)h * w * 3, ids_bytes = round_up((size_t)seq * 4, 256);
+        ensure_in_dev(m, ids_bytes + (size_t)std::min(n, cap) * img_bytes);
+        const int32_t* d_ids = reinterpret_cast<const int32_t*>(m->in_dev.get());
+        uint8_t* d_img = m->in_dev.get() + ids_bytes;
+        float* d_logits = m->det.get();
+        float* d_boxes = d_logits + (size_t)m->desc.max_batch * P;
+        float* t = m->out_dev.get();   // the query's text embedding [embed_dim]
+        TimedRegion tr(m);
+        MB_CUDA(cudaMemcpyAsync(m->in_dev.get(), query_ids, (size_t)seq * 4, cudaMemcpyHostToDevice, m->stream));
+        forward_tokens(m, tr.c, d_ids, nullptr, nullptr, 1, seq, 0, t);
+        for (int o = 0; o < n; o += cap) {
+            const int nb = std::min(cap, n - o);
+            MB_CUDA(cudaMemcpyAsync(d_img, hwc + (size_t)o * img_bytes, (size_t)nb * img_bytes, cudaMemcpyHostToDevice,
+                                    m->stream));
+            const uint8_t* src = d_img;
+            if (h != S || w != S) {
+                tr.c.n += kernels::resize_squash_u8(src, nb, h, w, S, m->resized.get(), m->stream);
+                src = m->resized.get();
+            }
+            forward_detect(m, tr.c, src, nb, t, d_logits, d_boxes);
+            MB_CUDA(cudaMemcpyAsync(logits + (size_t)o * P, d_logits, (size_t)nb * P * 4, cudaMemcpyDeviceToHost,
+                                    m->stream));
+            MB_CUDA(cudaMemcpyAsync(boxes + (size_t)o * P * 4, d_boxes, (size_t)nb * P * 16, cudaMemcpyDeviceToHost,
                                     m->stream));
             MB_CUDA(cudaStreamSynchronize(m->stream));
         }
@@ -1875,7 +2019,7 @@ int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int nor
     return guarded([&] {
         require_ready(m);
         MB_CHECK_ARG(chw && out, "NULL buffer");
-        MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
+        check_encodes_images(m);
         MB_CHECK_ARG(n > 0, "n must be positive");
         std::lock_guard<std::mutex> lk(m->mu);
         DeviceGuard g(m->device);
@@ -1916,7 +2060,7 @@ int b200_model_encode_images_u8_device(b200_model* m, const uint8_t* d_hwc, int 
     return guarded([&] {
         require_ready(m);
         MB_CHECK_ARG(d_hwc && d_out, "NULL buffer");
-        MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
+        check_encodes_images(m);
         MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
         std::lock_guard<std::mutex> lk(m->mu);
         DeviceGuard g(m->device);

@@ -295,7 +295,8 @@ class Encoder:
     `config` keys — CLIP: embed_dim, act ("gelu"|"quickgelu"), mean, std, resize_mode (optional: "squash" resizes
     images of another size without a crop), vision{width,layers,heads,mlp,patch,image_size},
     text{width,layers,heads,mlp,ctx,vocab}; CoCa is CLIP with vision.attn_pool_heads (its attentional pooler) and
-    text.embed_cls (its appended CLS row; ctx counts it, so the ids are ctx - 1 wide);  SigLIP: the CLIP keys plus ln_eps (embed_dim == vision
+    text.embed_cls (its appended CLS row; ctx counts it, so the ids are ctx - 1 wide); OWL-ViT is CLIP with
+    owl_detect (the detection head in place of visual.proj, run by detect_images_u8);  SigLIP: the CLIP keys plus ln_eps (embed_dim == vision
     width);  ResNet CLIP ("clip_resnet"): embed_dim, act, mean, std, the text tower's width, layers, heads, mlp, ctx,
     vocab at the top level (layers 0: no text tower), resnet{layers [4], width, heads, image_size} (None: no image
     tower);  ConvNeXt CLIP ("clip_convnext"): the ResNet CLIP keys with convnext{dims [4], depths [4], image_size,
@@ -341,7 +342,9 @@ class Encoder:
             # open_clip's resize_mode "squash" (SigLIP, the DFN5B CLIP models): the GPU resize scales x and y to
             # image_size independently instead of cropping
             d.resize_squash = int(config.get("resize_mode") == "squash")
+            d.owl_detect = int(bool(config.get("owl_detect", False)))
             self.image_size = v.get("image_size", 224) if v else 0
+            self.grid = self.image_size // v["patch"] if v else 0
         elif arch == "clip_resnet":
             d.arch = N.ARCH_CLIP_RESNET
             d.embed_dim = int(config["embed_dim"])
@@ -598,6 +601,21 @@ class Encoder:
         N.check(self._lib.b200_model_classify_tokens(self._handle(), _ptr(i), _ptr(extra[0]), _ptr(extra[1]), i.shape[0],
                                                      i.shape[1], 1 if sigmoid else 0, _ptr(out)))
         return out
+
+    def detect_images_u8(self, hwc, query_ids) -> Tuple[np.ndarray, np.ndarray]:
+        """OWL-ViT detection (owl_detect in the config): uint8 [n, H, W, 3] images, squashed to image_size on the GPU,
+        against one query's int ids [seq] (seq <= text ctx) -> (logits fp32 [n, G^2], boxes fp32 [n, G^2, 4] as
+        (cx, cy, w, h) in [0, 1]), what OwlViTForObjectDetection returns as logits[..., 0] and pred_boxes."""
+        a = _as(hwc, np.uint8)
+        if a.ndim != 4 or a.shape[3] != 3:
+            raise ValueError(f"expected uint8 [n, H, W, 3], got {a.shape}")
+        q = _as(query_ids.cpu().numpy() if hasattr(query_ids, "cpu") else query_ids, np.int32).reshape(-1)
+        P = self.grid * self.grid
+        logits = np.empty((a.shape[0], P), np.float32)
+        boxes = np.empty((a.shape[0], P, 4), np.float32)
+        N.check(self._lib.b200_model_detect_images_u8(self._handle(), _ptr(a), a.shape[0], a.shape[1], a.shape[2],
+                                                      _ptr(q), q.size, _ptr(logits), _ptr(boxes)))
+        return logits, boxes
 
     def classify_tokens_device(self, d_ids_ptr: int, d_mask_ptr: Optional[int], d_types_ptr: Optional[int], n: int,
                                seq: int, d_out_ptr: int, sigmoid: bool = True, sync: bool = True) -> None:
@@ -1039,6 +1057,50 @@ def debug_cls_head(x, S: int, pool_w, pool_b, cls_w, cls_b, sigmoid: bool = Fals
     N.check(N.load().b200_debug_cls_head(device, _dptr(dx), n, S, w, _dptr(dpw), _dptr(dpb), _dptr(dcw), _dptr(dcb), L,
                                          int(sigmoid), _dptr(out), d.stream))
     return _host(out)
+
+
+def debug_owl_merge_ln(x, N_rows: int, post_g, post_b, det_g, det_b, eps: float = 1e-5, device: int = 0) -> np.ndarray:
+    """OWL-ViT's patch features over trunk rows x fp32 [n * N_rows, w] (class row first per image): LN_det(LN_post(patch)
+    * LN_post(class)) -> fp32 [n * (N_rows - 1), w] (the kernel's bf16 values, widened)."""
+    xa = _as(x, np.float32)
+    w = xa.shape[1]
+    n = xa.shape[0] // N_rows
+    d = _Staging(device)
+    dx, g1, b1, g2, b2 = (d.up(a) for a in (xa, post_g, post_b, det_g, det_b))
+    out = d.empty((n * (N_rows - 1), w), "bfloat16")
+    N.check(N.load().b200_debug_owl_merge_ln(device, _dptr(dx), n, N_rows, w, _dptr(g1), _dptr(b1), _dptr(g2), _dptr(b2),
+                                             float(eps), _dptr(out), d.stream))
+    return _host(out.float())
+
+
+def debug_owl_class_logits(c, E: int, t, device: int = 0) -> np.ndarray:
+    """OWL-ViT's class logits from class-head GEMM rows c fp32 [M, ldc] (dense0 | shift | scale | padding) and the
+    query's text embedding t fp32 [E] -> fp32 [M]."""
+    ca, ta = _as(c, np.float32), _as(t, np.float32)
+    d = _Staging(device)
+    dc, dt = d.up(ca), d.up(ta)
+    out = d.empty((ca.shape[0],))
+    N.check(N.load().b200_debug_owl_class_logits(device, _dptr(dc), ca.shape[1], ca.shape[0], int(E), _dptr(dt),
+                                                 _dptr(out), d.stream))
+    return _host(out)
+
+
+def debug_owl_boxes(a, P: int, w2, b2, box_bias, device: int = 0) -> np.ndarray:
+    """OWL-ViT's boxes from the box head's second GELU rows a [M, w] (rounded to bf16) -> fp32 [M, 4]."""
+    aa = _as(a, np.float32)
+    d = _Staging(device)
+    da, dw, db, dbb = d.up(aa, "bfloat16"), d.up(w2), d.up(b2), d.up(box_bias)
+    out = d.empty((aa.shape[0], 4))
+    N.check(N.load().b200_debug_owl_boxes(device, _dptr(da), aa.shape[0], aa.shape[1], int(P), _dptr(dw), _dptr(db),
+                                          _dptr(dbb), _dptr(out), d.stream))
+    return _host(out)
+
+
+def owl_box_bias(G: int) -> np.ndarray:
+    """The engine's OWL-ViT box bias table of a G x G grid, fp32 [G^2, 4] (built on the host: no device needed)."""
+    out = np.empty((G * G, 4), np.float32)
+    N.check(N.load().b200_debug_owl_box_bias(int(G), _ptr(out)))
+    return out
 
 
 def debug_l2_rows(src, normalize: bool = True, device: int = 0) -> np.ndarray:

@@ -604,6 +604,41 @@ CROSS_ENCODER_MODELS: Dict[str, dict] = {
 }
 
 
+
+def _owlvit_arch(width: int, layers: int, heads: int, patch: int, image_size: int, text_width: int) -> dict:
+    """An OWL-ViT detector's shape (OwlViTConfig of the checkpoint, verify): the engine's CLIP block with QuickGELU in
+    both towers, CLIP's mean and std, squashed images, a 16-token text context over the CLIP BPE vocabulary and the
+    text width as the embedding (projection) width."""
+    return {"embed_dim": text_width, "act": "quickgelu", "resize_mode": "squash", "owl_detect": True,
+            "mean": (0.48145466, 0.4578275, 0.40821073), "std": (0.26862954, 0.26130258, 0.27577711),
+            "vision": {"width": width, "layers": layers, "heads": heads, "mlp": 4 * width, "patch": patch,
+                       "image_size": image_size},
+            "text": {"width": text_width, "layers": 12, "heads": text_width // 64, "mlp": 4 * text_width, "ctx": 16,
+                     "vocab": 49408}}
+
+
+# The OWL-ViT detectors Marqo's image reranker (`reRanker` "owl/..." in a search: reranking/cross_encoders.py
+# ReRankerOwl) loads through transformers' OwlViTForObjectDetection, which owl_reranker.B200OwlDetector serves: the
+# six names of ReRankerOwl._get_model_mapping, three checkpoints.  They score image hits against the query, so, like
+# CROSS_ENCODER_MODELS, this table is kept apart from the vectorise registry: find_model, all_models and
+# served_models do not read it.
+_OWLVIT_CHECKPOINTS = {
+    "google/owlvit-base-patch32": _owlvit_arch(768, 12, 12, 32, 768, 512),
+    "google/owlvit-base-patch16": _owlvit_arch(768, 12, 12, 16, 768, 512),
+    "google/owlvit-large-patch14": _owlvit_arch(1024, 24, 16, 14, 840, 768),
+}
+OWL_VIT_MODELS: Dict[str, dict] = {
+    name: {"name": name, "checkpoint": ckpt, "arch": _OWLVIT_CHECKPOINTS[ckpt]}
+    for name, ckpt in (
+        ("google/owlvit-base-patch32", "google/owlvit-base-patch32"),
+        ("google/owlvit-base-patch16", "google/owlvit-base-patch16"),
+        ("google/owlvit-large-patch14", "google/owlvit-large-patch14"),
+        ("owl/ViT-B/32", "google/owlvit-base-patch32"),
+        ("owl/ViT-B/16", "google/owlvit-base-patch16"),
+        ("owl/ViT-L/14", "google/owlvit-large-patch14"),
+    )
+}
+
 def _count(sd: dict, prefix: str) -> int:
     """The number of distinct indices i among the keys prefix + "i.*"."""
     return len({k[len(prefix):].split(".")[0] for k in sd if k.startswith(prefix)})

@@ -373,6 +373,132 @@ def random_cross_encoder_weights(arch: dict, seed: int = 1234) -> Dict[str, np.n
     return sd
 
 
+# transformers' CLIP-style encoder layer names -> open_clip's (the engine's) below a tower's resblock prefix
+_OWL_LAYER_NAMES = {"layer_norm1.": "ln_1.", "layer_norm2.": "ln_2.", "self_attn.out_proj.": "attn.out_proj.",
+                    "mlp.fc1.": "mlp.c_fc.", "mlp.fc2.": "mlp.c_proj."}
+# the two OWL-ViT tensors the detector never reads: the CLIP image projection and the contrastive temperature
+OWLVIT_UNUSED = ("owlvit.visual_projection.weight", "owlvit.logit_scale")
+
+
+def owlvit_state_dict_to_engine(sd: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
+    """An OwlViTForObjectDetection state dict under the engine's CLIP names (b200_model_desc owl_detect): q | k | v of
+    every layer stacked into in_proj_weight / in_proj_bias, text_projection.weight transposed to text_projection
+    [width, E], pre_layrnorm (also spelt pre_layernorm) -> visual.ln_pre, post_layernorm -> visual.ln_post, and the
+    detector's layer_norm.*, class_head.* and box_head.* kept as they are.  Every tensor is used but OWLVIT_UNUSED and
+    the position_ids buffers; any other name raises KeyError."""
+    sd = {k: v for k, v in sd.items() if not k.endswith("position_ids") and k not in OWLVIT_UNUSED}
+    out: Dict[str, np.ndarray] = {}
+    qkv: Dict[str, Dict[str, np.ndarray]] = {}
+    towers = (("owlvit.vision_model.", "visual."), ("owlvit.text_model.", ""))
+    fixed = {"owlvit.vision_model.embeddings.class_embedding": "visual.class_embedding",
+             "owlvit.vision_model.embeddings.patch_embedding.weight": "visual.conv1.weight",
+             "owlvit.vision_model.embeddings.position_embedding.weight": "visual.positional_embedding",
+             "owlvit.text_model.embeddings.token_embedding.weight": "token_embedding.weight",
+             "owlvit.text_model.embeddings.position_embedding.weight": "positional_embedding"}
+    for k, v in sd.items():
+        a = np.asarray(v.detach().cpu().numpy() if hasattr(v, "detach") else v, dtype=np.float32)
+        if k in fixed:
+            out[fixed[k]] = a
+        elif k == "owlvit.text_projection.weight":
+            out["text_projection"] = np.ascontiguousarray(a.T)
+        elif k.startswith(("layer_norm.", "class_head.", "box_head.")):
+            out[k] = a
+        else:
+            for src, dst in towers:
+                if not k.startswith(src):
+                    continue
+                rest = k[len(src):]
+                for a_name, b_name in (("pre_layrnorm.", "ln_pre."), ("pre_layernorm.", "ln_pre."),
+                                       ("post_layernorm.", "ln_post."), ("final_layer_norm.", "ln_final.")):
+                    if rest.startswith(a_name):
+                        out[dst + b_name + rest[len(a_name):]] = a
+                        break
+                else:
+                    if not rest.startswith("encoder.layers."):
+                        raise KeyError(f"{k}: not an OwlViTForObjectDetection parameter the engine knows")
+                    i, sub = rest[len("encoder.layers."):].split(".", 1)
+                    p = f"{dst}transformer.resblocks.{i}."
+                    if sub.startswith("self_attn.") and sub[10:12] in ("q_", "k_", "v_"):
+                        qkv.setdefault(p + "attn.in_proj_" + sub.rsplit(".", 1)[1], {})[sub[10]] = a
+                        break
+                    for a_name, b_name in _OWL_LAYER_NAMES.items():
+                        if sub.startswith(a_name):
+                            out[p + b_name + sub[len(a_name):]] = a
+                            break
+                    else:
+                        raise KeyError(f"{k}: not an OwlViTForObjectDetection parameter the engine knows")
+                break
+            else:
+                raise KeyError(f"{k}: not an OwlViTForObjectDetection parameter the engine knows")
+    for name, parts in qkv.items():
+        out[name] = np.concatenate([parts["q"], parts["k"], parts["v"]], axis=0)
+    return out
+
+
+def random_owlvit_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
+    """Seeded random weights of an OWL-ViT detector under OwlViTForObjectDetection's names (arch: the registry's
+    OWL-ViT block, the CLIP block of Encoder("clip")), including the two tensors the detector does not read."""
+    g = _rng(seed)
+    v, t, E = arch["vision"], arch["text"], arch["embed_dim"]
+    sd: Dict[str, np.ndarray] = {}
+
+    def layers(prefix, tw):
+        w, mlp, L = tw["width"], tw["mlp"], tw["layers"]
+        rg = 1.0 / math.sqrt(2.0 * L)
+        for i in range(L):
+            p = f"{prefix}encoder.layers.{i}."
+            for nm in ("layer_norm1", "layer_norm2"):
+                sd[p + nm + ".weight"] = _vec(g, w, 0.1, 1.0)
+                sd[p + nm + ".bias"] = _vec(g, w)
+            for nm in ("q_proj", "k_proj", "v_proj"):
+                sd[p + f"self_attn.{nm}.weight"] = _lin(g, w, w, 1.5)
+                sd[p + f"self_attn.{nm}.bias"] = _vec(g, w)
+            sd[p + "self_attn.out_proj.weight"] = _lin(g, w, w, rg)
+            sd[p + "self_attn.out_proj.bias"] = _vec(g, w)
+            sd[p + "mlp.fc1.weight"] = _lin(g, mlp, w)
+            sd[p + "mlp.fc1.bias"] = _vec(g, mlp)
+            sd[p + "mlp.fc2.weight"] = _lin(g, w, mlp, rg)
+            sd[p + "mlp.fc2.bias"] = _vec(g, w)
+
+    w, p = v["width"], v["patch"]
+    grid = v["image_size"] // p
+    vm = "owlvit.vision_model."
+    sd[vm + "embeddings.class_embedding"] = _vec(g, w, 0.5)
+    sd[vm + "embeddings.patch_embedding.weight"] = (g.standard_normal((w, 3, p, p), dtype=np.float32) /
+                                                    np.float32(math.sqrt(3 * p * p)))
+    sd[vm + "embeddings.position_embedding.weight"] = 0.5 * g.standard_normal((grid * grid + 1, w), dtype=np.float32)
+    sd[vm + "pre_layrnorm.weight"] = _vec(g, w, 0.1, 1.0)
+    sd[vm + "pre_layrnorm.bias"] = _vec(g, w)
+    layers(vm, v)
+    sd[vm + "post_layernorm.weight"] = _vec(g, w, 0.1, 1.0)
+    sd[vm + "post_layernorm.bias"] = _vec(g, w)
+    tw = t["width"]
+    tm = "owlvit.text_model."
+    sd[tm + "embeddings.token_embedding.weight"] = g.standard_normal((t["vocab"], tw), dtype=np.float32)
+    sd[tm + "embeddings.position_embedding.weight"] = 0.5 * g.standard_normal((t["ctx"], tw), dtype=np.float32)
+    layers(tm, t)
+    sd[tm + "final_layer_norm.weight"] = _vec(g, tw, 0.1, 1.0)
+    sd[tm + "final_layer_norm.bias"] = _vec(g, tw)
+    sd["owlvit.text_projection.weight"] = _lin(g, E, tw)
+    sd["owlvit.visual_projection.weight"] = _lin(g, E, w)
+    sd["owlvit.logit_scale"] = np.array(2.6592, np.float32)
+    sd["layer_norm.weight"] = _vec(g, w, 0.1, 1.0)
+    sd["layer_norm.bias"] = _vec(g, w)
+    sd["class_head.dense0.weight"] = _lin(g, E, w)
+    sd["class_head.dense0.bias"] = _vec(g, E)
+    # shift and scale spread around 0 so that both branches of the ELU occur among the patches
+    sd["class_head.logit_shift.weight"] = _lin(g, 1, w)
+    sd["class_head.logit_shift.bias"] = _vec(g, 1)
+    sd["class_head.logit_scale.weight"] = _lin(g, 1, w)
+    sd["class_head.logit_scale.bias"] = _vec(g, 1)
+    for nm in ("dense0", "dense1"):
+        sd[f"box_head.{nm}.weight"] = _lin(g, w, w)
+        sd[f"box_head.{nm}.bias"] = _vec(g, w)
+    sd["box_head.dense2.weight"] = _lin(g, 4, w)
+    sd["box_head.dense2.bias"] = _vec(g, 4)
+    return sd
+
+
 def random_xlmr_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
     """Seeded random weights under HF XLMRobertaModel parameter names (arch: the registry's XLM-R block): BertModel's
     names with max_pos position rows and type_vocab (1) token-type rows."""
