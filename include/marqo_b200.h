@@ -394,6 +394,23 @@ typedef struct b200_model_desc {
      * most vision.width.  Such a model is run by b200_model_detect_images_u8 only; every encode call refuses it
      * with B200_ERR_INVALID_ARG.  0: the usual heads. */
     int32_t owl_detect;
+    /* LanguageBind's video model (languagebind LanguageBindVideo, eval mode; verify), arch B200_ARCH_CLIP only, with a
+     * CLIP ViT of heads of 64 (width <= 1024) and the CLIP text tower.  video_frames = T in 1..16 makes the vision
+     * tower a video tower over T frames of N = (image_size / patch)^2 + 1 token rows each, laid out (b T + t) N + token:
+     *   x = the CLIP ViT embedding of every frame (conv1 without bias; frame t's class row is class_embedding[t] when
+     *       that is [T, width], else class_embedding [width]) + positional_embedding, then ln_pre;
+     *   per block, before the CLIP block: x += temporal_embedding[t] on every row of frame t (not when T = 1);
+     *       x += out_proj(MHA over the T frames of each (video, token) pair of temporal_ln_1(x)), no mask, heads of 64
+     *       with q / k / v / out biases;
+     *   head: ln_post of the T class rows, their mean, visual.proj [width, embed_dim], v / |v| * exp(logit_scale), and,
+     *       when normalize is set, the division by the norm again (no epsilons).
+     * The text tower is the causal CLIP one; its head is LanguageBind's: ln_final of the EOT row (first arg-max id),
+     * text_projection, v / |v|, then the division again when normalize is set.  Weights: the CLIP names, visual.proj
+     * [width, E], per block visual.transformer.resblocks.{i}.temporal_embedding [T, width], .temporal_ln_1.{weight,
+     * bias}, .temporal_attn.in_proj_{weight [3 width, width], bias}, .temporal_attn.out_proj.{weight, bias}, and
+     * logit_scale [1].  Such a model encodes uint8 videos by b200_model_encode_videos_u8 and text by the token calls;
+     * the image encode calls refuse it with B200_ERR_INVALID_ARG.  0: no video tower. */
+    int32_t video_frames;
 } b200_model_desc;
 
 int b200_model_create(int device, const b200_model_desc* desc, b200_model** out);
@@ -493,6 +510,17 @@ int b200_model_classify_tokens_device(b200_model* m, const int32_t* d_ids, const
  * sub-batches.  A model without the detector, seq outside 1 .. text.ctx, or n, h or w <= 0: B200_ERR_INVALID_ARG. */
 int b200_model_detect_images_u8(b200_model* m, const uint8_t* hwc, int n, int h, int w, const int32_t* query_ids,
                                 int seq, float* logits, float* boxes);
+/* LanguageBind videos (video_frames > 0, see b200_model_desc): n videos of t frames, uint8 RGB thwc [n, t, h, w, 3]
+ * (host), t == video_frames.  Each frame goes through LanguageBind's video transform on the GPU (ShortSideScale to
+ * image_size, bilinear, align_corners False, no antialias; CenterCropVideo with Python's round; / 255; Normalize by
+ * image_mean / image_std; the training-time random horizontal flip the reference also applies is not), then the video
+ * tower.  out: fp32 host [n, embed_dim].  A model without a video tower, t != video_frames, or n, h or w <= 0:
+ * B200_ERR_INVALID_ARG. */
+int b200_model_encode_videos_u8(b200_model* m, const uint8_t* thwc, int n, int t, int h, int w, int normalize,
+                                float* out);
+/* The same with the videos and the output on the model's device, asynchronous on its stream unless sync != 0. */
+int b200_model_encode_videos_u8_device(b200_model* m, const uint8_t* d_thwc, int n, int t, int h, int w, int normalize,
+                                       float* d_out, int sync);
 /* Images of mixed sizes in one call (every vision tower that takes uint8 images): image i is uint8 HWC
  * [heights[i], widths[i], 3] at hwc[i]; hwc, heights and widths are host arrays of n.  The images are resized to the
  * model's S x S by the tower's rule (shortest side + centre crop, or the squash) in one pass over each sub-batch, two
@@ -755,6 +783,26 @@ int b200_debug_owl_box_bias(int G, float* out);
  * [n, L].  w <= 1024. */
 int b200_debug_cls_head(int device, const float* x, int n, int S, int w, const float* pool_w, const float* pool_b,
                         const float* cls_w, const float* cls_b, int L, int sigmoid, float* out, void* stream);
+/* LanguageBind's heads over x fp32 [n*T*N, w]: for item b the mean over t < T of LN(x[(b T + t) N + r]) (r =
+ * row_in_seq[b], NULL: 0; gamma, beta, eps) @ proj [w, E], then v / |v| * scale, then / its norm if normalize.  The
+ * video head is r = 0 with scale exp(logit_scale); the text head T = 1, r = the EOT row, scale 1.  out fp32 [n, E]. */
+int b200_debug_frame_mean_head(int device, const float* x, int N, int T, const int32_t* row_in_seq, const float* gamma,
+                               const float* beta, float eps, const float* proj, int n, int w, int E, float scale,
+                               int normalize, float* out, void* stream);
+/* LanguageBind's temporal step over x fp32 [rows, w] (rows (b T + t) N + token): x[r] += temb[(r / N) % T] in place
+ * (temb fp32 [T, w]; NULL: nothing), then h bf16 [rows, w] = LN(x[r]).  w a multiple of 128, <= 1024. */
+int b200_debug_temporal_embed_ln(int device, float* x, const float* temb, int N, int T, const float* gamma,
+                                 const float* beta, float eps, int rows, int w, void* h, void* stream);
+/* Attention over the T frames (1..16) of every (video, token) pair: qkv bf16 [n*T*N, 3W] (q | k | v, rows (b T + t) N
+ * + token), heads of 64 (W = 64 H), no mask, scale 1/8 -> out bf16 [n*T*N, W] in the same row order. */
+int b200_debug_temporal_attention(int device, const void* qkv, int n, int T, int N, int W, int H, void* out,
+                                  void* stream);
+/* Mean device time (ms, CUDA events) of `iters` back-to-back temporal_attention launches on device-generated data. */
+int b200_debug_temporal_attention_time(int device, int n, int T, int N, int W, int H, int iters, float* out_ms);
+/* LanguageBind's video transform of uint8 RGB frames [frames, h, w, 3] -> out fp32 CHW [frames, 3, S, S] (see
+ * b200_model_encode_videos_u8); mean3 / std3 host fp32 [3]. */
+int b200_debug_video_resize_crop(int device, const uint8_t* frames_hwc, int frames, int h, int w, int S,
+                                 const float* mean3, const float* std3, float* out, void* stream);
 /* out fp32 [n, E] = src / |src| per row if normalize, else src. */
 int b200_debug_l2_rows(int device, const float* src, int n, int E, int normalize, float* out, void* stream);
 /* ResNet stem im2col: exactly one of hwc (uint8 [n,S,S,3], normalised with mean3 / std3, host fp32 [3]) and chw (fp32

@@ -55,7 +55,7 @@ class ModelDesc(C.Structure):
         ("convnext_head", C.c_int32), ("resize_squash", C.c_int32), ("eva_rope_ref_grid", C.c_int32),
         ("rope_theta", C.c_float), ("rope_ntk_factor", C.c_float),
         ("attn_pool_heads", C.c_int32), ("text_embed_cls", C.c_int32), ("text_proj_dim", C.c_int32),
-        ("cls_labels", C.c_int32), ("owl_detect", C.c_int32),
+        ("cls_labels", C.c_int32), ("owl_detect", C.c_int32), ("video_frames", C.c_int32),
     ]
 
 
@@ -120,6 +120,8 @@ _SIGNATURES = {
     "b200_model_classify_tokens": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "b200_model_classify_tokens_device": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
     "b200_model_detect_images_u8": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
+    "b200_model_encode_videos_u8": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "b200_model_encode_videos_u8_device": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int]),
     "b200_model_encode_images_u8_ragged": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P]),
     "b200_model_encode_images_u8_ragged_device": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, C.c_int]),
     "b200_model_set_stream": (C.c_int, [_P, _P, C.c_int]),
@@ -159,6 +161,14 @@ _SIGNATURES = {
     "b200_debug_owl_class_logits": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P]),
     "b200_debug_owl_boxes": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "b200_debug_owl_box_bias": (C.c_int, [C.c_int, _P]),
+    "b200_debug_frame_mean_head": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, C.c_float, _P, C.c_int, C.c_int,
+                                             C.c_int, C.c_float, C.c_int, _P, _P]),
+    "b200_debug_temporal_embed_ln": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_float, C.c_int, C.c_int,
+                                               _P, _P]),
+    "b200_debug_temporal_attention": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),
+    "b200_debug_temporal_attention_time": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                     C.POINTER(C.c_float)]),
+    "b200_debug_video_resize_crop": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P]),
     "b200_debug_l2_rows": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, _P, _P]),
     "b200_debug_stem_im2col": (C.c_int, [C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
     "b200_debug_avgpool2": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, _P]),

@@ -505,6 +505,84 @@ int b200_debug_owl_box_bias(int G, float* out) {
     });
 }
 
+int b200_debug_frame_mean_head(int device, const float* x, int N, int T, const int32_t* row_in_seq, const float* gamma,
+                               const float* beta, float eps, const float* proj, int n, int w, int E, float scale,
+                               int normalize, float* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && gamma && beta && proj && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && N > 0 && T > 0 && w > 0 && E > 0, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        DeviceBuffer<float> pooled((size_t)n * w);
+        kernels::frame_mean_head(x, N, T, row_in_seq, gamma, beta, eps, proj, n, w, E, scale, normalize, out,
+                                 pooled.get(), s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_temporal_embed_ln(int device, float* x, const float* temb, int N, int T, const float* gamma,
+                                 const float* beta, float eps, int rows, int w, void* h, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(x && gamma && beta && h, "NULL buffer");
+        MB_CHECK_ARG(rows > 0 && N > 0 && T > 0 && w > 0, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::temporal_embed_ln(x, temb, N, T, gamma, beta, eps, rows, w, static_cast<bf16*>(h), s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_temporal_attention(int device, const void* qkv, int n, int T, int N, int W, int H, void* out,
+                                  void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(qkv && out, "NULL buffer");
+        MB_CHECK_ARG(n > 0 && N > 0, "n and N must be positive");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::temporal_attention(static_cast<const bf16*>(qkv), n, T, N, W, H, static_cast<bf16*>(out), s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
+int b200_debug_temporal_attention_time(int device, int n, int T, int N, int W, int H, int iters, float* out_ms) {
+    return guarded([&] {
+        MB_CHECK_ARG(out_ms && n > 0 && N > 0 && iters > 0, "bad argument");
+        require_device(device);
+        DeviceGuard g(device);
+        Scratch sc;
+        const long long rows = (long long)n * T * N;
+        bf16* qkv = sc.alloc<bf16>((size_t)rows * 3 * W);
+        bf16* o = sc.alloc<bf16>((size_t)rows * W);
+        fill_bf16_kernel<<<(unsigned)((rows * 3 * W + 255) / 256), 256, 0, sc.s>>>(qkv, rows * 3 * W, 7u);
+        MB_CUDA(cudaGetLastError());
+        kernels::temporal_attention(qkv, n, T, N, W, H, o, sc.s);   // warm-up
+        UniqueEvent e0 = make_event(), e1 = make_event();
+        MB_CUDA(cudaEventRecord(e0.get(), sc.s));
+        for (int i = 0; i < iters; ++i) kernels::temporal_attention(qkv, n, T, N, W, H, o, sc.s);
+        MB_CUDA(cudaEventRecord(e1.get(), sc.s));
+        MB_CUDA(cudaEventSynchronize(e1.get()));
+        float ms = 0.f;
+        MB_CUDA(cudaEventElapsedTime(&ms, e0.get(), e1.get()));
+        *out_ms = ms / iters;
+    });
+}
+
+int b200_debug_video_resize_crop(int device, const uint8_t* frames_hwc, int frames, int h, int w, int S,
+                                 const float* mean3, const float* std3, float* out, void* stream) {
+    return guarded([&] {
+        MB_CHECK_ARG(frames_hwc && mean3 && std3 && out, "NULL buffer");
+        MB_CHECK_ARG(frames > 0 && h > 0 && w > 0 && S > 0, "bad shape");
+        require_device(device);
+        DeviceGuard g(device);
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        kernels::video_resize_crop(frames_hwc, frames, h, w, S, mean3, std3, out, s);
+        MB_CUDA(cudaStreamSynchronize(s));
+    });
+}
+
 int b200_debug_l2_rows(int device, const float* src, int n, int E, int normalize, float* out, void* stream) {
     return guarded([&] {
         MB_CHECK_ARG(src && out, "NULL buffer");

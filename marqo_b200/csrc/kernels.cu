@@ -1824,5 +1824,265 @@ int pool_ln(const float* x, int n, int HW, int C, const float* gamma, const floa
     return 1;
 }
 
+// ------------------------------------------------------------------------------------------------ LanguageBind video
+// LanguageBind's heads (languagebind/__init__.py:55-64, video/modeling_video.py:766-771):
+//   (1) frame_mean_ln_kernel  one warp per item: LayerNorm of each of its T pooled rows, then their mean -> pooled
+//   (2) head_proj_kernel      the CLIP head's projection
+//   (3) head_scale_kernel     one warp per item: v / |v| * scale, then, if normalize, / its norm again (no epsilons)
+__global__ void __launch_bounds__(256) frame_mean_ln_kernel(const float* __restrict__ x, int N, int T,
+                                                            const int32_t* __restrict__ row_in_seq,
+                                                            const float* __restrict__ gamma,
+                                                            const float* __restrict__ beta, float eps, int n, int w,
+                                                            float* __restrict__ pooled) {
+    const int b = blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (b >= n) return;
+    const int r = row_in_seq ? row_in_seq[b] : 0;
+    float* dst = pooled + (long long)b * w;
+    for (int t = 0; t < T; ++t) {
+        const float* src = x + (((long long)b * T + t) * N + r) * w;
+        float s = 0.f;
+        for (int i = lane; i < w; i += 32) s += src[i];
+        const float mean = warp_sum(s) / (float)w;
+        float q = 0.f;
+        for (int i = lane; i < w; i += 32) {
+            const float d = src[i] - mean;
+            q += d * d;
+        }
+        const float rstd = 1.0f / sqrtf(warp_sum(q) / (float)w + eps);
+        // each lane owns the same columns for every t: the sum needs no synchronisation
+        for (int i = lane; i < w; i += 32) {
+            const float y = (src[i] - mean) * rstd * gamma[i] + beta[i];
+            dst[i] = t == 0 ? y : dst[i] + y;
+        }
+    }
+    for (int i = lane; i < w; i += 32) dst[i] = dst[i] / (float)T;
+}
+
+__global__ void __launch_bounds__(256) head_scale_kernel(float* __restrict__ out, int n, int E, float scale,
+                                                         int normalize) {
+    const int b = blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (b >= n) return;
+    float* row = out + (long long)b * E;
+    float ss = 0.f;
+    for (int i = lane; i < E; i += 32) ss += row[i] * row[i];
+    const float nrm = sqrtf(warp_sum(ss));
+    ss = 0.f;
+    for (int i = lane; i < E; i += 32) {
+        const float v = row[i] / nrm * scale;
+        row[i] = v;
+        ss += v * v;
+    }
+    if (!normalize) return;
+    const float nrm2 = sqrtf(warp_sum(ss));
+    for (int i = lane; i < E; i += 32) row[i] = row[i] / nrm2;
+}
+
+int frame_mean_head(const float* x, int N, int T, const int32_t* row_in_seq, const float* gamma, const float* beta,
+                    float eps, const float* proj, int n, int w, int E, float scale, int normalize, float* out,
+                    float* pooled_ws, cudaStream_t s) {
+    if (n <= 0) return 0;
+    if (w % 4 != 0 || (size_t)HEAD_IMGS * w * sizeof(float) > 40 * 1024)
+        fail(B200_ERR_UNSUPPORTED, "frame_mean_head: width %d unsupported", w);
+    if (T < 1) fail(B200_ERR_INVALID_ARG, "frame_mean_head: T %d must be positive", T);
+    frame_mean_ln_kernel<<<(n + 7) / 8, 256, 0, s>>>(x, N, T, row_in_seq, gamma, beta, eps, n, w, pooled_ws);
+    MB_CUDA(cudaGetLastError());
+    const dim3 grid((n + HEAD_IMGS - 1) / HEAD_IMGS, (E + HEAD_COLS - 1) / HEAD_COLS);
+    head_proj_kernel<<<grid, 256, (size_t)HEAD_IMGS * w * sizeof(float), s>>>(pooled_ws, proj, nullptr, n, w, E, out);
+    MB_CUDA(cudaGetLastError());
+    head_scale_kernel<<<(n + 7) / 8, 256, 0, s>>>(out, n, E, scale, normalize);
+    MB_CUDA(cudaGetLastError());
+    return 3;
+}
+
+// x[r] += temb[(r / N) % T] (when temb != NULL), then h[r] = bf16(LN(x[r])): one warp per row, the row read once.
+__global__ void __launch_bounds__(256) temporal_embed_ln_kernel(float* __restrict__ x, const float* __restrict__ temb,
+                                                                int N, int T, const float* __restrict__ gamma,
+                                                                const float* __restrict__ beta, float eps, int rows,
+                                                                int w, __nv_bfloat16* __restrict__ h) {
+    const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (row >= rows) return;
+    const int nv = w / 128;
+    float* src = x + (long long)row * w;
+    float4 v[LN_MAX_V4];
+#pragma unroll
+    for (int j = 0; j < LN_MAX_V4; ++j)
+        if (j < nv) v[j] = load4(src, lane + 32 * j);
+    if (temb) {
+        const float* e = temb + (long long)((row / N) % T) * w;
+#pragma unroll
+        for (int j = 0; j < LN_MAX_V4; ++j)
+            if (j < nv) {
+                const float4 a = __ldg(reinterpret_cast<const float4*>(e) + lane + 32 * j);
+                v[j] = make_float4(v[j].x + a.x, v[j].y + a.y, v[j].z + a.z, v[j].w + a.w);
+                reinterpret_cast<float4*>(src)[lane + 32 * j] = v[j];
+            }
+    }
+    ln_row<false, LN_MAX_V4>(v, nv, w, gamma, beta, eps, lane, nullptr, h + (long long)row * w);
+}
+
+int temporal_embed_ln(float* x, const float* temb, int N, int T, const float* gamma, const float* beta, float eps,
+                      int rows, int w, __nv_bfloat16* h, cudaStream_t s) {
+    if (rows <= 0) return 0;
+    check_ln_width(w);
+    if (N <= 0 || T <= 0) fail(B200_ERR_INVALID_ARG, "temporal_embed_ln: N %d and T %d must be positive", N, T);
+    temporal_embed_ln_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, temb, N, T, gamma, beta, eps, rows, w, h);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+// Eight lanes per (item, token, head): lane l owns columns 8 l .. 8 l + 7 of the head, read as 16-byte loads.  For
+// each query frame i the group reads q_i and the T frames' k and v rows (k and v again for every query, from L1 / L2:
+// held in registers across the queries they would take 128 of them at T = 8), sums each score over its 8 lanes by
+// shuffles, and takes the softmax in fp32 (exp2 of logits pre-scaled by log2(e) / sqrt(64)), the weighted sum of v and
+// one 16-byte bf16 store.  Frame t of an (item, token) pair is row (b T + t) N + token of the packed buffers: no
+// (b n) t copy.  A group past the end reads the last group's rows (every lane of a warp takes part in the shuffles) and
+// stores nothing.
+__device__ __forceinline__ void unpack8(const uint4 u, float (&f)[8]) {
+    const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        f[2 * i] = __uint_as_float(w4[i] << 16);
+        f[2 * i + 1] = __uint_as_float(w4[i] & 0xffff0000u);
+    }
+}
+
+template <int TMAX>
+__global__ void __launch_bounds__(256) temporal_attention_kernel(const __nv_bfloat16* __restrict__ qkv, int N, int T,
+                                                                 int H, long long groups, float scale_log2,
+                                                                 __nv_bfloat16* __restrict__ out) {
+    const long long g0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 3;
+    const bool valid = g0 < groups;
+    const long long g = valid ? g0 : groups - 1;
+    const int l = threadIdx.x & 7;
+    const int h = (int)(g % H);
+    const long long bn = g / H;
+    const int tok = (int)(bn % N);
+    const long long b = bn / N;
+    const int W = H * 64;
+    const long long ld = 3LL * W, step = (long long)N * ld;   // frame t's row: row0 + t N
+    const long long row0 = b * T * N + tok;
+    const __nv_bfloat16* base = qkv + row0 * ld + h * 64 + l * 8;
+    for (int i = 0; i < T; ++i) {
+        float q[8];
+        unpack8(__ldg(reinterpret_cast<const uint4*>(base + i * step)), q);
+        float s[TMAX];
+        float m = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < TMAX; ++j)
+            if (j < T) {
+                float kf[8];
+                unpack8(__ldg(reinterpret_cast<const uint4*>(base + j * step + W)), kf);
+                float d = 0.f;
+#pragma unroll
+                for (int c = 0; c < 8; ++c) d = fmaf(q[c], kf[c], d);
+                d += __shfl_xor_sync(0xffffffffu, d, 1);
+                d += __shfl_xor_sync(0xffffffffu, d, 2);
+                d += __shfl_xor_sync(0xffffffffu, d, 4);
+                s[j] = d * scale_log2;
+                m = fmaxf(m, s[j]);
+            }
+        float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        float sum = 0.f;
+#pragma unroll
+        for (int j = 0; j < TMAX; ++j)
+            if (j < T) {
+                const float p = exp2f(s[j] - m);
+                sum += p;
+                float vf[8];
+                unpack8(__ldg(reinterpret_cast<const uint4*>(base + j * step + 2 * W)), vf);
+#pragma unroll
+                for (int c = 0; c < 8; ++c) acc[c] = fmaf(p, vf[c], acc[c]);
+            }
+        if (valid) {
+            const float inv = 1.0f / sum;
+            uint4 o;
+            o.x = pack_bf16x2(acc[0] * inv, acc[1] * inv);
+            o.y = pack_bf16x2(acc[2] * inv, acc[3] * inv);
+            o.z = pack_bf16x2(acc[4] * inv, acc[5] * inv);
+            o.w = pack_bf16x2(acc[6] * inv, acc[7] * inv);
+            *reinterpret_cast<uint4*>(out + (row0 + (long long)i * N) * W + h * 64 + l * 8) = o;
+        }
+    }
+}
+
+int temporal_attention(const __nv_bfloat16* qkv, int n, int T, int N, int W, int heads, __nv_bfloat16* out,
+                       cudaStream_t s) {
+    if (n <= 0) return 0;
+    if (T < 1 || T > TEMPORAL_MAX_FRAMES)
+        fail(B200_ERR_INVALID_ARG, "temporal_attention: T %d must be 1..%d", T, TEMPORAL_MAX_FRAMES);
+    if (heads <= 0 || W != heads * 64 || N <= 0)
+        fail(B200_ERR_UNSUPPORTED, "temporal_attention: heads of 64 only (W %d, heads %d, N %d)", W, heads, N);
+    const long long groups = (long long)n * N * heads;
+    const unsigned blocks = (unsigned)((groups * 8 + 255) / 256);
+    const float scale_log2 = 0.125f * 1.4426950408889634f;
+    if (T <= 8)
+        temporal_attention_kernel<8><<<blocks, 256, 0, s>>>(qkv, N, T, heads, groups, scale_log2, out);
+    else
+        temporal_attention_kernel<TEMPORAL_MAX_FRAMES>
+            <<<blocks, 256, 0, s>>>(qkv, N, T, heads, groups, scale_log2, out);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+// One thread per output pixel (f, y, x) of the S x S crop, all three channels: the source point in the frame of the
+// resized pixel (y + top, x + left) by F.interpolate's rule (align_corners False: (dst + 0.5) h / nh - 0.5 as one fma,
+// clamped at 0; the far tap clamped to the last row / column), bilinear over the uint8 values in fp32, then / 255 and Normalize.
+// The reference normalises before it resizes; the bilinear weights sum to 1, so the two orders differ by rounding.
+__global__ void __launch_bounds__(256) video_resize_crop_kernel(const uint8_t* __restrict__ src, long long total, int H,
+                                                                int W, int S, int top, int left, float sy, float sx,
+                                                                float3 mean, float3 stdv, float* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const long long plane = (long long)S * S;
+    const long long f = i / plane;
+    const int p = (int)(i - f * plane), y = p / S, x = p - y * S;
+    const float fy = fmaxf(fmaf(sy, (float)(y + top) + 0.5f, -0.5f), 0.f);
+    const float fx = fmaxf(fmaf(sx, (float)(x + left) + 0.5f, -0.5f), 0.f);
+    const int y0 = (int)fy, x0 = (int)fx;
+    const int y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
+    const float ly = fy - (float)y0, lx = fx - (float)x0, hy = 1.f - ly, hx = 1.f - lx;
+    const uint8_t* img = src + f * H * W * 3;
+    const uint8_t *a = img + ((long long)y0 * W + x0) * 3, *b = img + ((long long)y0 * W + x1) * 3;
+    const uint8_t *c = img + ((long long)y1 * W + x0) * 3, *d = img + ((long long)y1 * W + x1) * 3;
+    const float m[3] = {mean.x, mean.y, mean.z}, sd[3] = {stdv.x, stdv.y, stdv.z};
+    float* o = out + f * 3 * plane + p;
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+        const float v = hy * (hx * (float)a[ch] + lx * (float)b[ch]) + ly * (hx * (float)c[ch] + lx * (float)d[ch]);
+        o[ch * plane] = (v / 255.f - m[ch]) / sd[ch];
+    }
+}
+
+void video_resize_geometry(int h, int w, int S, int* nh, int* nw, int* top, int* left) {
+    // pytorchvideo's short_side_scale: the short side to S, the long one to floor(long / short * S) in double
+    if (w < h) {
+        *nh = (int)std::floor((double)h / w * S);
+        *nw = S;
+    } else {
+        *nh = S;
+        *nw = (int)std::floor((double)w / h * S);
+    }
+    // torchvision's CenterCropVideo: int(round((size - S) / 2.0)), Python's round (half to even)
+    *top = py_round_half_even((*nh - S) / 2.0);
+    *left = py_round_half_even((*nw - S) / 2.0);
+}
+
+int video_resize_crop(const uint8_t* src, long long frames, int h, int w, int S, const float* mean, const float* std_,
+                      float* out, cudaStream_t s) {
+    if (frames <= 0) return 0;
+    if (h <= 0 || w <= 0 || S <= 0) fail(B200_ERR_INVALID_ARG, "video_resize_crop: bad size %d x %d -> %d", h, w, S);
+    int nh, nw, top, left;
+    video_resize_geometry(h, w, S, &nh, &nw, &top, &left);
+    const long long total = frames * S * S;
+    video_resize_crop_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(
+        src, total, h, w, S, top, left, (float)h / (float)nh, (float)w / (float)nw,
+        make_float3(mean[0], mean[1], mean[2]), make_float3(std_[0], std_[1], std_[2]), out);
+    MB_CUDA(cudaGetLastError());
+    return 1;
+}
+
 }  // namespace kernels
 }  // namespace mb

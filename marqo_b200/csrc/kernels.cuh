@@ -82,6 +82,34 @@ int clip_head(const float* x, int S, const int32_t* row_in_seq, const float* gam
               const float* proj, int n, int w, int E, int normalize, float* out, float* pooled_ws, cudaStream_t s,
               bool unit = false);
 
+// LanguageBind's heads (languagebind/__init__.py:55-64): for item b, the mean over t < T of LN(x[(b T + t) N + r])
+// (r = row_in_seq[b], NULL: 0) into pooled_ws (fp32 [n, w]), then @ proj [w, E] (fp32), then v / |v| * scale and, if
+// normalize, a second division by the norm (no epsilons).  The video head is T frames of N token rows with r = 0 and
+// scale exp(logit_scale) (video/modeling_video.py:766-771); the text head is T = 1, N = S, r = the EOT row, scale 1.
+// Always three kernels.  w % 4 == 0, w <= 2560.
+int frame_mean_head(const float* x, int N, int T, const int32_t* row_in_seq, const float* gamma, const float* beta,
+                    float eps, const float* proj, int n, int w, int E, float scale, int normalize, float* out,
+                    float* pooled_ws, cudaStream_t s);
+
+// LanguageBind's temporal step, over the fp32 residual stream x [rows, w] whose rows are (b T + t) N + token: row r
+// gains temb[(r / N) % T] in place (fp32 [T, w]; NULL adds nothing: a single frame, video/modeling_video.py:214-219),
+// then h[r] = bf16(LN(x[r])) by gamma, beta, eps (temporal_layer_norm1).  w % 128 == 0, w <= 1024.
+int temporal_embed_ln(float* x, const float* temb, int N, int T, const float* gamma, const float* beta, float eps,
+                      int rows, int w, __nv_bfloat16* h, cudaStream_t s);
+// Attention over the T frames of every (item, token) pair and head of 64 columns, no mask (video/modeling_video.py:
+// 221-232): with qkv bf16 [n T N, 3W] (q | k | v) and rows (b T + t) N + token, out bf16 [n T N, W] row (b T + i) N +
+// token, head h = softmax_j(q_i . k_j / 8) v_j over j < T, in fp32, rounded once.  T in 1 .. TEMPORAL_MAX_FRAMES.
+constexpr int TEMPORAL_MAX_FRAMES = 16;
+int temporal_attention(const __nv_bfloat16* qkv, int n, int T, int N, int W, int heads, __nv_bfloat16* out,
+                       cudaStream_t s);
+// LanguageBind's video transform (video/processing_video.py:20-45) of uint8 RGB frames [frames, h, w, 3] -> fp32 CHW
+// [frames, 3, S, S]: pytorchvideo ShortSideScale(S) (bilinear, align_corners False, no antialias), CenterCropVideo(S)
+// (offsets rounded half to even), / 255 and NormalizeVideo(mean, std) (host fp32 [3]); the resize runs on the raw
+// values, normalised afterwards, in fp32.  video_resize_geometry gives the resized size and the crop's offsets.
+int video_resize_crop(const uint8_t* src, long long frames, int h, int w, int S, const float* mean, const float* std_,
+                      float* out, cudaStream_t s);
+void video_resize_geometry(int h, int w, int S, int* nh, int* nw, int* top, int* left);
+
 // BERT head: masked mean over the first kv_len[b] tokens (pool == 0) or the [CLS] row (pool == 1), then
 // x / max(|x|, 1e-12) if normalize (F.normalize, hugging_face_model.py:194-195).  kv_len is clamped to [0, S]; 0 gives
 // a NaN row under mean pooling, as the reference's sum / mask.sum() does.

@@ -40,6 +40,10 @@ struct LayerW {
     const __nv_bfloat16 *w_qkv = nullptr, *w_o = nullptr, *w_fc = nullptr, *w_proj = nullptr;
     // EVA02: attn.norm over the attention output [width] and mlp.norm over the SwiGLU hidden row [TowerW::mlp_h]
     const float *ln_attn_w = nullptr, *ln_attn_b = nullptr, *ln_mlp_w = nullptr, *ln_mlp_b = nullptr;
+    // LanguageBind's temporal step (TowerW::frames > 0): temporal_embedding [frames, width] (NULL for one frame, which
+    // adds none), temporal_layer_norm1, temporal_attn's fused q | k | v [3 width, width] and out_proj
+    const float *temb = nullptr, *tln_w = nullptr, *tln_b = nullptr, *b_tqkv = nullptr, *b_to = nullptr;
+    const __nv_bfloat16 *w_tqkv = nullptr, *w_to = nullptr;
 };
 
 // A layer's MLP: fc1 with the tower's activation in its epilogue, or a gated unit over the 2 mlp columns fc1 writes
@@ -59,7 +63,7 @@ struct MapW {
 
 // What runs a tower, resolved once from the model's arch (resolve_kinds).  Archs whose forward passes differ only in
 // data share a kind: MPNet and XLM-R are ROBERTA, and the ResNet CLIP's text tower is CLIP's.
-enum class VisionKind { NONE, CLIP_VIT, SIGLIP_VIT, RESNET, CONVNEXT, EVA_VIT, COCA_VIT };
+enum class VisionKind { NONE, CLIP_VIT, SIGLIP_VIT, RESNET, CONVNEXT, EVA_VIT, COCA_VIT, VIDEO_VIT };
 enum class TextKind { NONE, CLIP, SIGLIP, BERT, ROBERTA, GTE, COCA };
 struct Kinds {
     VisionKind vision = VisionKind::NONE;
@@ -86,8 +90,11 @@ struct TowerW {
     const float* rope = nullptr;
     kernels::RopePairing rope_pairing = kernels::RopePairing::INTERLEAVED;
     int rope_first = 0;
-    // tokens per item: an image's token rows, or the longest sequence
+    // tokens per item: an image's token rows, or the longest sequence (a video tower: one frame's)
     int tokens = 0;
+    // LanguageBind's video tower: frames per video (0: not a video tower), and the factor exp(logit_scale) of its head
+    int frames = 0;
+    float out_scale = 1.f;
     // vision
     const __nv_bfloat16* conv_w = nullptr;  // [width, kpad]
     const __nv_bfloat16* conv_wg = nullptr; // [width, gemm::patch_gather_k(patch)]: gather GEMM order
@@ -207,6 +214,7 @@ struct b200_model {
     DeviceBuffer<float> pooled;       // [max_batch, width] LayerNorm-ed pooled rows (CLIP heads)
     DeviceBuffer<uint8_t> in_dev;     // staging for host inputs
     DeviceBuffer<uint8_t> resized;    // [max_batch, S, S, 3]
+    DeviceBuffer<float> video_f32;    // a video model's transformed frames: fp32 CHW [videos per pass * frames, 3, S, S]
     cudaStream_t stream = nullptr;
     UniqueStream own_stream;          // created by the handle; `stream` may be replaced by a caller's stream
     UniqueEvent ev0, ev1;
@@ -269,7 +277,10 @@ Kinds resolve_kinds(const b200_model_desc& d) {
     const bool vit = d.vision.layers > 0, text = d.text.layers > 0;
     switch (d.arch) {
     case B200_ARCH_CLIP:
-        if (vit) k.vision = d.attn_pool_heads > 0 ? VisionKind::COCA_VIT : VisionKind::CLIP_VIT;
+        if (vit)
+            k.vision = d.attn_pool_heads > 0 ? VisionKind::COCA_VIT
+                       : d.video_frames > 0  ? VisionKind::VIDEO_VIT
+                                             : VisionKind::CLIP_VIT;
         if (text) k.text = d.text_embed_cls ? TextKind::COCA : TextKind::CLIP;
         break;
     case B200_ARCH_CLIP_RESNET:
@@ -379,10 +390,18 @@ void check_vision(const b200_model_desc& d, VisionKind kind) {
                          d.embed_dim, d.vision.width);
         }
         [[fallthrough]];
+    case VisionKind::VIDEO_VIT:
+        if (kind == VisionKind::VIDEO_VIT) {
+            // the temporal kernels: heads of 64, the LayerNorm's rows of up to 1024 in registers
+            MB_CHECK_ARG(d.vision.width == d.vision.heads * 64 && d.vision.width <= 1024,
+                         "video: vision head_dim must be 64 and width <= 1024 (width %d, heads %d)", d.vision.width,
+                         d.vision.heads);
+        }
+        [[fallthrough]];
     case VisionKind::CLIP_VIT: {
         MB_CHECK_ARG(d.vision.patch > 0 && d.vision.image_size % d.vision.patch == 0,
                      "image_size must be a multiple of patch");
-        const bool clip = kind == VisionKind::CLIP_VIT || kind == VisionKind::COCA_VIT;
+        const bool clip = kind == VisionKind::CLIP_VIT || kind == VisionKind::COCA_VIT || kind == VisionKind::VIDEO_VIT;
         const int grid = d.vision.image_size / d.vision.patch;
         check_tower(d.vision, "vision", clip ? 1664 : 1024, clip && grid * grid + 1 >= 128);
         break;
@@ -404,6 +423,17 @@ void check_owl(const b200_model_desc& d, const Kinds& k) {
     MB_CHECK_ARG((int)round_up((size_t)d.embed_dim + 2, 64) <= d.vision.width,
                  "owl_detect: embed_dim %d + 2 rounded up to 64 must be at most vision.width %d", d.embed_dim,
                  d.vision.width);
+}
+
+// LanguageBind's video model: the CLIP ViT with the temporal step, its frame-mean head and the CLIP text tower
+void check_video(const b200_model_desc& d, const Kinds& k) {
+    MB_CHECK_ARG(d.video_frames >= 0 && d.video_frames <= kernels::TEMPORAL_MAX_FRAMES,
+                 "video_frames %d must be 0..%d", d.video_frames, kernels::TEMPORAL_MAX_FRAMES);
+    if (!d.video_frames) return;
+    MB_CHECK_ARG(d.arch == B200_ARCH_CLIP, "video_frames: only the CLIP arch takes LanguageBind's video tower");
+    MB_CHECK_ARG(d.attn_pool_heads == 0 && !d.owl_detect && !d.text_embed_cls,
+                 "video_frames: CoCa's pooler and OWL-ViT's detector are other heads");
+    MB_CHECK_ARG(k.vision == VisionKind::VIDEO_VIT, "video_frames: the model needs a vision tower");
 }
 
 void check_text(const b200_model_desc& d, const Kinds& k) {
@@ -1038,6 +1068,53 @@ void build_owl(b200_model* m, const TowerW& T) {
     D.box_bias = upload_derived(m, bb);
 }
 
+// LanguageBind's video tower (languagebind/video/modeling_video.py:698-785, verify) under the CLIP ViT names, its frames
+// laid out (b T + t) N + token.  visual.class_embedding is [width] (CLIPVisionEmbeddings) or one row per frame [T,
+// width] (CLIPVisionEmbeddings3D with tube 1); it and visual.positional_embedding become one table of a video's T N rows
+// (frame t's class row: class_embedding[t] + positional_embedding[0], its patch rows: positional_embedding), which
+// vit_embed_rows writes and the patch GEMM adds conv1 onto.  Per layer the temporal step's weights (LayerW), and the
+// head: ln_post, visual.proj [width, E] and exp(logit_scale).
+void build_video_vision(b200_model* m, TowerW& T) {
+    const long long w = T.d.width, F = m->desc.video_frames;
+    build_vit(m, T, "visual.conv1.weight", 1);
+    T.act = open_clip_act(m->desc);
+    T.frames = (int)F;
+    const long long N = T.tokens;
+    const long long cls_rows = param_rows(m, "visual.class_embedding", w);
+    MB_CHECK_ARG(cls_rows == 1 || cls_rows == F, "visual.class_embedding has %lld rows: 1 or video_frames (%lld)",
+                 cls_rows, F);
+    const std::vector<float> cls = to_host(param(m, "visual.class_embedding", cls_rows * w), (size_t)(cls_rows * w));
+    const std::vector<float> pos = to_host(param(m, "visual.positional_embedding", N * w), (size_t)(N * w));
+    std::vector<float> table((size_t)(F * N * w));
+    for (long long t = 0; t < F; ++t) {
+        std::copy(pos.begin(), pos.end(), table.begin() + t * N * w);
+        const float* c = cls.data() + (cls_rows == 1 ? 0 : t * w);
+        for (long long i = 0; i < w; ++i) table[(size_t)(t * N * w + i)] = c[i] + pos[(size_t)i];
+    }
+    T.pos = upload_derived(m, table);
+    m->raw.erase("visual.class_embedding");
+    m->raw.erase("visual.positional_embedding");
+    T.ln_pre_w = param(m, "visual.ln_pre.weight", w);
+    T.ln_pre_b = param(m, "visual.ln_pre.bias", w);
+    build_layers(m, T, "visual.transformer.resblocks.", OPEN_CLIP_BLOCK);
+    static const char* const tqkv[1] = {"temporal_attn.in_proj_"};
+    for (int i = 0; i < T.d.layers; ++i) {
+        const std::string p = "visual.transformer.resblocks." + std::to_string(i) + ".";
+        LayerW& L = T.layers[i];
+        const float* temb = param(m, p + "temporal_embedding", F * w);
+        L.temb = F > 1 ? temb : nullptr;   // one frame adds none (modeling_video.py:214)
+        L.tln_w = param(m, p + "temporal_ln_1.weight", w);
+        L.tln_b = param(m, p + "temporal_ln_1.bias", w);
+        stack_linear(m, p, tqkv, 1, 0b1, 3 * w, 3 * w, w, L.w_tqkv, L.b_tqkv);
+        L.w_to = to_bf16(m, p + "temporal_attn.out_proj.weight", w * w);
+        L.b_to = param(m, p + "temporal_attn.out_proj.bias", w);
+    }
+    T.ln_out_w = param(m, "visual.ln_post.weight", w);
+    T.ln_out_b = param(m, "visual.ln_post.bias", w);
+    T.proj = param(m, "visual.proj", w * m->desc.embed_dim);
+    T.out_scale = std::exp(to_host(param(m, "logit_scale", 1), 1)[0]);
+}
+
 void build_vision(b200_model* m) {
     TowerW& T = m->vision;
     const long long w = T.d.width;
@@ -1076,6 +1153,9 @@ void build_vision(b200_model* m) {
         break;
     case VisionKind::EVA_VIT:
         build_eva_vision(m, T);
+        break;
+    case VisionKind::VIDEO_VIT:
+        build_video_vision(m, T);
         break;
     }
 }
@@ -1225,7 +1305,9 @@ void linear(b200_model* m, Counter& c, const __nv_bfloat16* A, int M, int K, con
 // GEMMs.  Post-LN (HF BertLayer, MPNetLayer with the tower's relative-position bias, NewModel): on entry x and h both
 // hold the embedding LayerNorm output, and LN rewrites x in place (x -> x and h) after each residual GEMM.  A tower may
 // rotate q and k after the QKV GEMM (T.rope), LayerNorm the attention output before the out-projection (EVA02's
-// attn.norm) and run a gated MLP (Mlp).  Layers [first, first + count) run (count < 0: to the last one).
+// attn.norm) and run a gated MLP (Mlp).  A video tower (T.frames > 0, B = videos * frames) runs LanguageBind's temporal
+// step first (modeling_video.py:209-232): x += temporal_embedding[t], then x += out_proj(attention over the frames of
+// each token position (temporal_layer_norm1(x))).  Layers [first, first + count) run (count < 0: to the last one).
 // MASK_CLS reads the sequences' token ids, cls_ids [B, S - 1].
 void run_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S, int mask_mode, int first = 0,
                 int count = -1, const int32_t* cls_ids = nullptr) {
@@ -1241,6 +1323,14 @@ void run_layers(b200_model* m, Counter& c, const TowerW& T, int B, int S, int ma
     };
     for (int i = first; i < end; ++i) {
         const LayerW& L = T.layers[i];
+        if (T.frames) {
+            c.n += kernels::temporal_embed_ln(x, L.temb, S, T.frames, L.tln_w, L.tln_b, T.eps, M, w, h, m->stream);
+            linear(m, c, h, M, w, L.w_tqkv, 3 * w, epilogue(qkv, 3 * w, L.b_tqkv));
+            profiled(m, c, 1, [&] {
+                return kernels::temporal_attention(qkv, B / T.frames, T.frames, S, w, T.d.heads, o, m->stream);
+            });
+            linear(m, c, o, M, w, L.w_to, w, epilogue(x, w, L.b_to, gemm::ACT_NONE, true, x, w));
+        }
         if (T.pre_ln) ln(L.ln1_w, L.ln1_b);
         linear(m, c, h, M, w, L.w_qkv, 3 * aw, epilogue(qkv, 3 * aw, L.b_qkv));
         if (T.rope) c.n += kernels::rope_qk(qkv, B, S, T.rope_first, aw, T.rope, T.rope_pairing, m->stream);
@@ -1335,21 +1425,23 @@ void patch_embed(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, 
         profiled(m, c, 0, [&] { return gemm::launch_patch_embed(pg, T.conv_wg, w, e, m->stream); });
     } else {
         // preprocessed fp32 CHW tensors (the reference's parity path)
-        if (!m->patches) m->patches = DeviceBuffer<__nv_bfloat16>((size_t)m->desc.max_batch * T.tokens * T.kpad);
+        if (!m->patches)
+            m->patches =
+                DeviceBuffer<__nv_bfloat16>((size_t)m->desc.max_batch * std::max(1, T.frames) * T.tokens * T.kpad);
         c.n += kernels::im2col_f32(f32, n, S, p, T.kpad, T.cls_rows, m->patches.get(), m->stream);
         linear(m, c, m->patches.get(), n * T.tokens, T.kpad, T.conv_w, w, e);
     }
 }
 
 // A ViT trunk over n images (device uint8 [n, S, S, 3] u8, or device fp32 CHW f32): patch embedding, ln_pre (CLIP) and
-// the layers, leaving the n * T.tokens token rows in x.
+// the layers, leaving the n * T.tokens token rows in x.  A video tower's images are the frames of n / T.frames videos.
 void forward_vit(b200_model* m, Counter& c, const TowerW& T, const uint8_t* u8, const float* f32, int n) {
-    const int w = T.d.width;
+    const int w = T.d.width, per = std::max(1, T.frames);
     float* x = m->x.get();
     // x = positional embedding (+ class embedding on each image's first row), then conv1 (no bias) of every token row
     // added onto it in place; a class-token row multiplies a zero A row.  SigLIP has no class row; its conv bias, and
-    // EVA02's, is already in T.pos.
-    c.n += kernels::vit_embed_rows(x, T.cls, T.pos, n, T.tokens, w, m->stream);
+    // EVA02's, is already in T.pos; a video tower's T.pos spans a video's frames, class rows included.
+    c.n += kernels::vit_embed_rows(x, T.cls, T.pos, n / per, per * T.tokens, w, m->stream);
     patch_embed(m, c, T, u8, f32, n, epilogue(x, w, nullptr, gemm::ACT_NONE, true, x, w));
     if (T.ln_pre_w)
         c.n += kernels::layernorm(x, w, T.ln_pre_w, T.ln_pre_b, T.eps, n * T.tokens, w, x, nullptr, m->stream);
@@ -1500,11 +1592,16 @@ void forward_tokens_eager(b200_model* m, Counter& c, const int32_t* d_ids, const
     int32_t* aux = m->aux.get();
     switch (m->kind.text) {
     case TextKind::CLIP:
-        // causal layers; ln_final of each sequence's eot row, projection, optional L2
+        // causal layers; ln_final of each sequence's eot row, projection, optional L2 (LanguageBind: always L2, then
+        // optionally once more)
         c.n += kernels::clip_text_embed(d_ids, T.tok, T.pos, n, S, w, T.d.vocab, x, aux, m->stream);
         run_layers(m, c, T, n, S, attention::MASK_CAUSAL);
-        c.n += kernels::clip_head(x, S, aux, T.ln_out_w, T.ln_out_b, T.eps, T.proj, n, w, E, normalize, d_out,
-                                  m->pooled.get(), m->stream);
+        if (m->desc.video_frames)
+            c.n += kernels::frame_mean_head(x, S, 1, aux, T.ln_out_w, T.ln_out_b, T.eps, T.proj, n, w, E, 1.f, normalize,
+                                            d_out, m->pooled.get(), m->stream);
+        else
+            c.n += kernels::clip_head(x, S, aux, T.ln_out_w, T.ln_out_b, T.eps, T.proj, n, w, E, normalize, d_out,
+                                      m->pooled.get(), m->stream);
         break;
     case TextKind::COCA: {
         // ids [n, S]; the CLS row appended after them is the last of St token rows, pooled (aux = St - 1) through
@@ -1615,6 +1712,19 @@ void forward_detect(b200_model* m, Counter& c, const uint8_t* u8, int n, const f
                 [&](Counter& cc) { forward_detect_eager(m, cc, u8, n, t, logits, boxes); });
 }
 
+// n videos of T.frames transformed frames each (device fp32 CHW [n * frames, 3, S, S]): the trunk, then LanguageBind's
+// head (the mean of the frames' ln_post class rows, visual.proj, L2 times exp(logit_scale), optional L2)
+void forward_videos(b200_model* m, Counter& c, const float* f32, int n, int normalize, float* d_out) {
+    const TowerW& T = m->vision;
+    const b200_model::GraphKey key{3, n, 0, normalize, nullptr, f32, d_out};
+    run_graphed(m, c, key, (long long)n * T.frames * T.tokens, [&](Counter& cc) {
+        forward_vit(m, cc, T, nullptr, f32, n * T.frames);
+        cc.n += kernels::frame_mean_head(m->x.get(), T.tokens, T.frames, nullptr, T.ln_out_w, T.ln_out_b, T.eps, T.proj,
+                                         n, T.d.width, m->desc.embed_dim, T.out_scale, normalize, d_out,
+                                         m->pooled.get(), m->stream);
+    });
+}
+
 void require_ready(b200_model* m) {
     MB_CHECK_ARG(m != nullptr, "model is NULL");
     if (!m->finalized) fail(B200_ERR_INVALID_ARG, "b200_model_finalize has not been called");
@@ -1627,6 +1737,29 @@ int batch_cap_tokens(b200_model* m, int tokens_per_item) {
 // images per forward pass: what the image tower's activation buffers hold
 int image_batch_cap(b200_model* m) {
     return m->kind.vision == VisionKind::CONVNEXT ? m->convnext.max_images : batch_cap_tokens(m, m->vision.tokens);
+}
+
+// videos per forward pass: what the workspaces hold
+int video_batch_cap(b200_model* m) { return batch_cap_tokens(m, m->vision.frames * m->vision.tokens); }
+
+// device-resident uint8 videos [n, frames, h, w, 3] -> embeddings: each sub-batch's frames transformed into video_f32,
+// then one forward pass
+void encode_videos_u8_dev(b200_model* m, Counter& c, const uint8_t* d_vid, int n, int h, int w, int normalize,
+                          float* d_out) {
+    const TowerW& T = m->vision;
+    const int cap = video_batch_cap(m), F = T.frames;
+    for (int o = 0; o < n; o += cap) {
+        const int nb = std::min(cap, n - o);
+        c.n += kernels::video_resize_crop(d_vid + (size_t)o * F * h * w * 3, (long long)nb * F, h, w, T.d.image_size,
+                                          m->desc.image_mean, m->desc.image_std, m->video_f32.get(), m->stream);
+        forward_videos(m, c, m->video_f32.get(), nb, normalize, d_out + (size_t)o * m->desc.embed_dim);
+    }
+}
+
+void check_videos_args(b200_model* m, int n, int t, int h, int w) {
+    MB_CHECK_ARG(m->kind.vision == VisionKind::VIDEO_VIT, "this model has no video tower (video_frames 0)");
+    MB_CHECK_ARG(t == m->vision.frames, "videos of %d frames: the model takes %d", t, m->vision.frames);
+    MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
 }
 
 struct TimedRegion {
@@ -1680,6 +1813,8 @@ void encode_images_u8_ragged_dev(b200_model* m, Counter& c, const uint8_t* const
 void check_encodes_images(b200_model* m) {
     MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
     MB_CHECK_ARG(!m->desc.owl_detect, "this model is an OWL-ViT detector: detect images with a query");
+    MB_CHECK_ARG(m->kind.vision != VisionKind::VIDEO_VIT, "this model is a video model: encode videos of %d frames",
+                 m->vision.frames);
 }
 
 // the arguments of a ragged image call, all checked before anything is written
@@ -1772,7 +1907,7 @@ const TowerW& layer_tower(b200_model* m, int tower) {
     MB_CHECK_ARG(tower == 0 || tower == 1, "tower %d must be 0 (vision) or 1 (text)", tower);
     const VisionKind vk = m->kind.vision;
     MB_CHECK_ARG(tower == 0 ? vk == VisionKind::CLIP_VIT || vk == VisionKind::SIGLIP_VIT || vk == VisionKind::EVA_VIT ||
-                                  vk == VisionKind::COCA_VIT
+                                  vk == VisionKind::COCA_VIT || vk == VisionKind::VIDEO_VIT
                             : m->kind.text != TextKind::NONE,
                  "this model has no transformer %s tower", tower == 0 ? "vision" : "text");
     return tower == 0 ? m->vision : m->text;
@@ -1799,6 +1934,7 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         check_vision(*desc, kind.vision);
         check_text(*desc, kind);
         check_owl(*desc, kind);
+        check_video(*desc, kind);
         DeviceGuard g(device);
         std::unique_ptr<b200_model> m(new b200_model());   // released under the guard if the set-up fails
         m->device = device;
@@ -1810,7 +1946,8 @@ int b200_model_create(int device, const b200_model_desc* desc, b200_model** out)
         m->ev1 = make_event();
         m->kind = kind;
         if (kind.vision == VisionKind::CLIP_VIT || kind.vision == VisionKind::SIGLIP_VIT ||
-            kind.vision == VisionKind::EVA_VIT || kind.vision == VisionKind::COCA_VIT)
+            kind.vision == VisionKind::EVA_VIT || kind.vision == VisionKind::COCA_VIT ||
+            kind.vision == VisionKind::VIDEO_VIT)
             m->vision.d = desc->vision;
         if (kind.vision == VisionKind::RESNET) m->vision.d.image_size = desc->resnet_image_size;   // (no layers)
         if (kind.vision == VisionKind::CONVNEXT) {   // the stem, as a patch embedding (no layers)
@@ -1873,7 +2010,7 @@ int b200_model_finalize(b200_model* m) {
         long long max_tok = 0, max_w = 0, max_aw = 0, max_mlp = 0;
         for (const TowerW* T : {&m->vision, &m->text}) {
             if (T == &m->vision && m->kind.vision == VisionKind::CONVNEXT) continue;   // its own buffers (ConvnextW)
-            max_tok = std::max(max_tok, B * T->tokens);   // (0 for a missing tower)
+            max_tok = std::max(max_tok, B * std::max(1, T->frames) * T->tokens);   // (0 for a missing tower)
             max_w = std::max<long long>(max_w, T->d.width);
             max_aw = std::max<long long>({max_aw, T->d.width, T->aw});   // qkv and o: padded heads are wider
             max_mlp = std::max<long long>({max_mlp, fc1_cols(*T), T->map.mlp});
@@ -1891,6 +2028,10 @@ int b200_model_finalize(b200_model* m) {
             m->resized = DeviceBuffer<uint8_t>((size_t)B * S * S * 3);
         }
         if (m->desc.owl_detect) m->det = DeviceBuffer<float>((size_t)B * m->vision.grid * m->vision.grid * 5);
+        if (m->kind.vision == VisionKind::VIDEO_VIT) {
+            const size_t S = m->vision.d.image_size;
+            m->video_f32 = DeviceBuffer<float>((size_t)video_batch_cap(m) * m->vision.frames * 3 * S * S);
+        }
         MB_CUDA(cudaStreamSynchronize(m->stream));
         m->aux = DeviceBuffer<int32_t>((size_t)B);
         m->out_dev = DeviceBuffer<float>((size_t)B * E);
@@ -1923,6 +2064,47 @@ int b200_model_encode_images_u8(b200_model* m, const uint8_t* hwc, int n, int h,
             MB_CUDA(cudaStreamSynchronize(m->stream));
         }
         tr.finish();
+    });
+}
+
+int b200_model_encode_videos_u8(b200_model* m, const uint8_t* thwc, int n, int t, int h, int w, int normalize,
+                                float* out) {
+    return guarded([&] {
+        require_ready(m);
+        MB_CHECK_ARG(thwc && out, "NULL buffer");
+        check_videos_args(m, n, t, h, w);
+        std::lock_guard<std::mutex> lk(m->mu);
+        DeviceGuard g(m->device);
+        const int E = m->desc.embed_dim;
+        const int cap = video_batch_cap(m);
+        const size_t video_bytes = (size_t)t * h * w * 3;
+        ensure_in_dev(m, (size_t)std::min(n, cap) * video_bytes);
+        TimedRegion tr(m);
+        for (int o = 0; o < n; o += cap) {
+            const int nb = std::min(cap, n - o);
+            MB_CUDA(cudaMemcpyAsync(m->in_dev.get(), thwc + (size_t)o * video_bytes, (size_t)nb * video_bytes,
+                                    cudaMemcpyHostToDevice, m->stream));
+            encode_videos_u8_dev(m, tr.c, m->in_dev.get(), nb, h, w, normalize, m->out_dev.get());
+            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
+                                    m->stream));
+            MB_CUDA(cudaStreamSynchronize(m->stream));
+        }
+        tr.finish();
+    });
+}
+
+int b200_model_encode_videos_u8_device(b200_model* m, const uint8_t* d_thwc, int n, int t, int h, int w, int normalize,
+                                       float* d_out, int sync) {
+    return guarded([&] {
+        require_ready(m);
+        MB_CHECK_ARG(d_thwc && d_out, "NULL buffer");
+        check_videos_args(m, n, t, h, w);
+        std::lock_guard<std::mutex> lk(m->mu);
+        DeviceGuard g(m->device);
+        TimedRegion tr(m);
+        encode_videos_u8_dev(m, tr.c, d_thwc, n, h, w, normalize, d_out);
+        tr.finish();
+        if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
     });
 }
 
@@ -2192,7 +2374,9 @@ int b200_debug_layers(b200_model* m, int tower, int first, int count, const floa
         const int L = (int)T.layers.size();
         MB_CHECK_ARG(first >= 0 && count > 0 && first <= L - count, "layers [%d, %d + %d) outside the tower's %d", first,
                      first, count, L);
-        MB_CHECK_ARG(B > 0 && B <= m->desc.max_batch, "B %d out of range (1..%d)", B, m->desc.max_batch);
+        const int per = vision ? std::max(1, T.frames) : 1;   // a video tower's sequences are its videos' frames
+        MB_CHECK_ARG(B > 0 && B % per == 0 && B / per <= m->desc.max_batch, "B %d out of range (1..%d%s)", B,
+                     m->desc.max_batch * per, per > 1 ? ", a multiple of the frames" : "");
         MB_CHECK_ARG(vision ? S == T.tokens : S > 0 && S <= T.tokens, "S %d: the %s tower takes %s%d tokens", S,
                      vision ? "vision" : "text", vision ? "" : "1..", T.tokens);
         MB_CHECK_ARG((long long)B * S <= m->max_tokens, "B * S = %lld rows exceed the workspace's %lld",

@@ -296,7 +296,8 @@ class Encoder:
     images of another size without a crop), vision{width,layers,heads,mlp,patch,image_size},
     text{width,layers,heads,mlp,ctx,vocab}; CoCa is CLIP with vision.attn_pool_heads (its attentional pooler) and
     text.embed_cls (its appended CLS row; ctx counts it, so the ids are ctx - 1 wide); OWL-ViT is CLIP with
-    owl_detect (the detection head in place of visual.proj, run by detect_images_u8);  SigLIP: the CLIP keys plus ln_eps (embed_dim == vision
+    owl_detect (the detection head in place of visual.proj, run by detect_images_u8); LanguageBind's video model is CLIP
+    with video_frames (the vision tower a video tower, run by encode_videos_u8);  SigLIP: the CLIP keys plus ln_eps (embed_dim == vision
     width);  ResNet CLIP ("clip_resnet"): embed_dim, act, mean, std, the text tower's width, layers, heads, mlp, ctx,
     vocab at the top level (layers 0: no text tower), resnet{layers [4], width, heads, image_size} (None: no image
     tower);  ConvNeXt CLIP ("clip_convnext"): the ResNet CLIP keys with convnext{dims [4], depths [4], image_size,
@@ -343,6 +344,9 @@ class Encoder:
             # image_size independently instead of cropping
             d.resize_squash = int(config.get("resize_mode") == "squash")
             d.owl_detect = int(bool(config.get("owl_detect", False)))
+            # LanguageBind's video model: the vision tower runs over video_frames frames with its temporal layers
+            d.video_frames = int(config.get("video_frames") or 0)
+            self.video_frames = int(d.video_frames)
             self.image_size = v.get("image_size", 224) if v else 0
             self.grid = self.image_size // v["patch"] if v else 0
         elif arch == "clip_resnet":
@@ -616,6 +620,23 @@ class Encoder:
         N.check(self._lib.b200_model_detect_images_u8(self._handle(), _ptr(a), a.shape[0], a.shape[1], a.shape[2],
                                                       _ptr(q), q.size, _ptr(logits), _ptr(boxes)))
         return logits, boxes
+
+    def encode_videos_u8(self, thwc, normalize: bool = True) -> np.ndarray:
+        """LanguageBind videos (video_frames in the config): uint8 RGB [n, T, H, W, 3] with T the model's frames,
+        transformed on the GPU (short side to image_size, bilinear; centre crop; Normalize) -> fp32 [n, embed_dim]."""
+        a = _as(thwc, np.uint8)
+        if a.ndim != 5 or a.shape[4] != 3:
+            raise ValueError(f"expected uint8 [n, T, H, W, 3], got {a.shape}")
+        out = np.empty((a.shape[0], self.embed_dim), np.float32)
+        N.check(self._lib.b200_model_encode_videos_u8(self._handle(), _ptr(a), a.shape[0], a.shape[1], a.shape[2],
+                                                      a.shape[3], 1 if normalize else 0, _ptr(out)))
+        return out
+
+    def encode_videos_u8_device(self, d_ptr: int, n: int, t: int, h: int, w: int, d_out_ptr: int,
+                                normalize: bool = True, sync: bool = True) -> None:
+        N.check(self._lib.b200_model_encode_videos_u8_device(self._handle(), C.c_void_p(d_ptr), n, t, h, w,
+                                                             1 if normalize else 0, C.c_void_p(d_out_ptr),
+                                                             1 if sync else 0))
 
     def classify_tokens_device(self, d_ids_ptr: int, d_mask_ptr: Optional[int], d_types_ptr: Optional[int], n: int,
                                seq: int, d_out_ptr: int, sigmoid: bool = True, sync: bool = True) -> None:
@@ -1101,6 +1122,67 @@ def owl_box_bias(G: int) -> np.ndarray:
     out = np.empty((G * G, 4), np.float32)
     N.check(N.load().b200_debug_owl_box_bias(int(G), _ptr(out)))
     return out
+
+
+def debug_frame_mean_head(x, N_rows: int, T: int, gamma, beta, eps: float, proj, scale: float = 1.0,
+                          row_in_seq=None, normalize: bool = True, device: int = 0) -> np.ndarray:
+    """LanguageBind's heads over x fp32 [n * T * N_rows, w]: the mean over the T rows (b T + t) N_rows + r (r =
+    row_in_seq[b], None: 0) of their LayerNorm, @ proj [w, E], v / |v| * scale, then / its norm if normalize."""
+    d = _Staging(device)
+    xa = _as(x, np.float32)
+    pr = _as(proj, np.float32)
+    w, E = xa.shape[1], pr.shape[1]
+    n = xa.shape[0] // (T * N_rows)
+    dx, dg, db, dp = d.up(xa), d.up(gamma), d.up(beta), d.up(pr)
+    dr = d.up(row_in_seq, "int32")
+    out = d.empty((n, E))
+    N.check(N.load().b200_debug_frame_mean_head(device, _dptr(dx), N_rows, T, _dptr(dr), _dptr(dg), _dptr(db), eps,
+                                                _dptr(dp), n, w, E, float(scale), 1 if normalize else 0, _dptr(out),
+                                                d.stream))
+    return _host(out)
+
+
+def debug_temporal_embed_ln(x, temb, N_rows: int, T: int, gamma, beta, eps: float, device: int = 0):
+    """LanguageBind's temporal step: (x + temb[(r / N_rows) % T] fp32 [rows, w], bf16 LN of it as fp32)."""
+    d = _Staging(device)
+    xa = _as(x, np.float32)
+    rows, w = xa.shape
+    dx, dt, dg, db = d.up(xa), d.up(temb), d.up(gamma), d.up(beta)
+    h = d.empty((rows, w), "bfloat16")
+    N.check(N.load().b200_debug_temporal_embed_ln(device, _dptr(dx), _dptr(dt), N_rows, T, _dptr(dg), _dptr(db), eps,
+                                                  rows, w, _dptr(h), d.stream))
+    return _host(dx), _host(h.float())
+
+
+def debug_temporal_attention(qkv, n: int, T: int, N_rows: int, H: int, device: int = 0) -> np.ndarray:
+    """Attention over the T frames of each (video, token) pair: qkv [n * T * N_rows, 3W] (rounded to bf16), heads of
+    64 -> out [n * T * N_rows, W] (bf16 values as fp32)."""
+    d = _Staging(device)
+    q = d.up(qkv, "bfloat16")
+    W = q.shape[1] // 3
+    out = d.empty((q.shape[0], W), "bfloat16")
+    N.check(N.load().b200_debug_temporal_attention(device, _dptr(q), n, T, N_rows, W, H, _dptr(out), d.stream))
+    return _host(out.float())
+
+
+def debug_temporal_attention_time(n: int, T: int, N_rows: int, W: int, H: int, iters: int = 50,
+                                  device: int = 0) -> float:
+    ms = C.c_float(0)
+    N.check(N.load().b200_debug_temporal_attention_time(device, n, T, N_rows, W, H, iters, C.byref(ms)))
+    return ms.value
+
+
+def debug_video_resize_crop(frames, S: int, mean, std, device: int = 0) -> np.ndarray:
+    """LanguageBind's video transform of uint8 RGB frames [f, h, w, 3] -> fp32 CHW [f, 3, S, S]."""
+    d = _Staging(device)
+    a = _as(frames, np.uint8)
+    f, h, w, _ = a.shape
+    da = d.up(a, "uint8")
+    out = d.empty((f, 3, S, S))
+    m3, s3 = np.asarray(mean, np.float32), np.asarray(std, np.float32)
+    N.check(N.load().b200_debug_video_resize_crop(device, _dptr(da), f, h, w, S, _ptr(m3), _ptr(s3), _dptr(out),
+                                                  d.stream))
+    return _host(out)
 
 
 def debug_l2_rows(src, normalize: bool = True, device: int = 0) -> np.ndarray:

@@ -639,6 +639,179 @@ class B200MultilingualClip(B200OpenCLIP):
         return out
 
 
+def _read_video_frames(path: str, num_frames: int) -> np.ndarray:
+    """LanguageBind's opencv decode (languagebind/video/processing_video.py:80-93): frame ids np.linspace(0, count - 1,
+    num_frames, dtype=int) of CAP_PROP_FRAME_COUNT, each read after seeking to it and turned BGR -> RGB.  uint8
+    [num_frames, H, W, 3]."""
+    import cv2
+    cap = cv2.VideoCapture(str(path))
+    try:
+        count = int(cap.get(cv2.CAP_PROP_FRAME_COUNT))
+        frames = []
+        for idx in np.linspace(0, count - 1, num_frames, dtype=int):
+            cap.set(cv2.CAP_PROP_POS_FRAMES, int(idx))
+            ok, frame = cap.read()
+            if not ok or frame is None:
+                raise VectoriseError(f"Could not read frame {int(idx)} of video {path}")
+            frames.append(cv2.cvtColor(frame, cv2.COLOR_BGR2RGB))
+    finally:
+        cap.release()
+    return np.stack(frames)
+
+
+class LanguageBindVideoPreprocessor:
+    """What LanguageBindVideoProcessor(config)(paths) does on the host (processing_video.py:48-99): decode and sample
+    the frames of each video file.  Returns {"pixel_values": uint8 [n, T, H, W, 3]} for videos of one size; the
+    transform (ShortSideScale, CenterCropVideo, Normalize) runs on the GPU in B200LanguageBind.encode."""
+
+    def __init__(self, num_frames: int):
+        self.num_frames = int(num_frames)
+
+    def __call__(self, images=None, return_tensors=None, **kwargs):
+        paths = images if isinstance(images, (list, tuple)) else [images]
+        videos = [_read_video_frames(p, self.num_frames) for p in paths]
+        if len({v.shape for v in videos}) != 1:
+            raise VectoriseError("videos of different sizes: preprocess them one at a time")
+        return {"pixel_values": np.stack(videos)}
+
+
+class B200LanguageBind:
+    """Marqo's `languagebind` loader (multimodal_model_load.py:204-299, LanguageBindEncoder) for
+    LanguageBind/Video_V1.5_FT on the engine: the video tower (LanguageBindVideo.vision_model with its temporal layers,
+    video_frames in the arch) and the checkpoint's CLIP text tower in one Encoder.
+
+    Weights: model_properties["weights"] (a LanguageBindVideo state dict or checkpoint file), or `localpath`, a snapshot
+    directory with config.json and pytorch_model.bin / model.safetensors, or `random_init` (a seed).  config.json, when
+    there is one, gives num_frames, hidden_act, layer_norm_eps and the embedding form (clip_type "vl" or "vl_new", whose
+    tube_size must be 1), each checked against the arch; the tensors' shapes are checked by the engine.  Nothing is
+    downloaded.  Text is tokenised by model_properties["tokenizer"] or the CLIP BPE of `merges_file` at context 77.
+
+    Outputs follow LanguageBind.forward and the encoder's _normalize: every vector is v / |v|; a video vector is then
+    multiplied by exp(logit_scale); normalize=True divides by the norm once more.  Unlike the reference, the video
+    transform does not apply RandomHorizontalFlipVideo(p=0.5), which the reference runs at inference and which makes
+    its video embeddings random; the engine's are those of the unflipped frames."""
+
+    def __init__(self, device: Optional[str] = None, model_properties: Optional[dict] = None, model_auth=None):
+        if device is None:
+            raise ModelLoadError("`device` is required for loading LanguageBind models!")
+        self.device = device
+        self.model_properties = dict(model_properties or {})
+        self.model = None
+        self.tokenizer: Optional[Callable] = None
+        self._preprocessors: Dict[Modality, Callable] = {}
+
+    @staticmethod
+    def _check_config(cfg: dict, arch: dict) -> dict:
+        """The arch with the act of the checkpoint's config.json (both towers must agree), after checking the fields
+        the engine fixes: 8 frames as the arch says, eps 1e-5, a tube of one frame."""
+        v, t = cfg.get("vision_config", {}), cfg.get("text_config", {})
+        acts = {v.get("hidden_act", "quick_gelu"), t.get("hidden_act", "quick_gelu")}
+        if len(acts) != 1 or not acts <= {"gelu", "quick_gelu"}:
+            raise InvalidModelPropertiesError(f"LanguageBind: hidden_act {sorted(acts)} is not one gelu / quick_gelu")
+        frames = int(v.get("num_frames", 1))
+        if frames != arch["video_frames"]:
+            raise InvalidModelPropertiesError(f"LanguageBind: num_frames {frames} != the arch's {arch['video_frames']}")
+        for c in (v, t):
+            if float(c.get("layer_norm_eps", 1e-5)) != 1e-5:
+                raise InvalidModelPropertiesError("LanguageBind: the engine's CLIP towers take layer_norm_eps 1e-5")
+        if v.get("clip_type", "vl") == "vl_new" and int(v.get("tube_size", 1)) != 1:
+            raise InvalidModelPropertiesError("LanguageBind: a patch embedding over tubes of more than one frame")
+        return dict(arch, act="gelu" if acts == {"gelu"} else "quickgelu")
+
+    def load(self) -> None:
+        import json
+        from .engine import Encoder
+        props = self.model_properties
+        arch = props.get("arch")
+        if arch is None or not arch.get("video_frames"):
+            raise InvalidModelPropertiesError("model_properties has no LanguageBind `arch` block (video_frames)")
+        w = props.get("weights")
+        local = props.get("localpath")
+        if local and os.path.isdir(local):
+            cfg_path = os.path.join(local, "config.json")
+            if os.path.exists(cfg_path):
+                with open(cfg_path) as f:
+                    arch = self._check_config(json.load(f), arch)
+            if w is None:
+                for fn in ("model.safetensors", "pytorch_model.bin"):
+                    if os.path.exists(os.path.join(local, fn)):
+                        w = os.path.join(local, fn)
+                        break
+        if w is None and props.get("random_init") is not None:
+            w = weights_mod.random_languagebind_video_weights(arch, int(props["random_init"]))
+        if w is None:
+            raise ModelLoadError("model_properties needs `weights`, a `localpath` snapshot or `random_init`; "
+                                 "checkpoint download is Marqo's job and out of scope here")
+        if isinstance(w, (str, bytes)) or hasattr(w, "__fspath__"):
+            w = weights_mod.load_state_dict(w)
+        self.arch = arch
+        self.model = Encoder("clip", arch, weights_mod.languagebind_video_state_dict_to_engine(w),
+                             device=_validate_device(self.device), max_batch=int(props.get("max_batch", 32)))
+        self.tokenizer = props.get("tokenizer")
+        if self.tokenizer is None and props.get("merges_file"):
+            from .tokenizers import ClipBpeTokenizer
+            self.tokenizer = ClipBpeTokenizer(props["merges_file"], context_length=int(arch["text"]["ctx"]))
+
+    def close(self) -> None:
+        if self.model is not None:
+            self.model.close()
+            self.model = None
+
+    def preprocessor(self, modality):
+        """The host preprocessor of a modality this model has (video), else None, as LanguageBindEncoder.preprocessor
+        returns for a modality outside its clip_type."""
+        if Modality(modality) != Modality.VIDEO:
+            return None
+        if Modality.VIDEO not in self._preprocessors:
+            self._preprocessors[Modality.VIDEO] = LanguageBindVideoPreprocessor(self.arch["video_frames"])
+        return self._preprocessors[Modality.VIDEO]
+
+    def _encode_videos(self, videos: List[np.ndarray], normalize: bool) -> np.ndarray:
+        """uint8 [T, H, W, 3] videos, grouped by size into one engine call each, rows returned in the input order."""
+        out = np.empty((len(videos), self.model.embed_dim), np.float32)
+        groups: Dict[tuple, List[int]] = {}
+        for i, v in enumerate(videos):
+            groups.setdefault(v.shape, []).append(i)
+        for idx in groups.values():
+            out[idx] = self.model.encode_videos_u8(np.stack([videos[i] for i in idx]), normalize=normalize)
+        return out
+
+    def encode(self, content, modality=Modality.TEXT, normalize=True, **kwargs) -> np.ndarray:
+        modality = Modality(modality) if modality is not None else Modality.TEXT
+        if modality == Modality.TEXT:
+            if self.tokenizer is None:
+                raise VectoriseError("LanguageBind text needs model_properties['tokenizer'] or a merges_file")
+            texts = [content] if isinstance(content, str) else list(content)
+            ids = np.asarray(self.tokenizer(texts), dtype=np.int32)
+            return self.model.encode_tokens(ids, normalize=normalize)
+        if modality == Modality.VIDEO:
+            items = [content] if isinstance(content, (str, dict)) or hasattr(content, "__fspath__") else list(content)
+            videos: List[np.ndarray] = []
+            for it in items:
+                if isinstance(it, dict) and "pixel_values" in it:
+                    pv = it["pixel_values"]
+                    pv = np.asarray(pv.cpu().numpy() if hasattr(pv, "cpu") else pv)
+                    if pv.dtype != np.uint8 or pv.ndim != 5 or pv.shape[-1] != 3:
+                        raise ValueError(f"pixel_values must be uint8 [n, T, H, W, 3], got {pv.dtype} {pv.shape}")
+                    videos.extend(pv)
+                elif isinstance(it, str) and "http" in it:
+                    raise ValueError(f"Unsupported video content: {it} (downloading is Marqo's host code)")
+                elif isinstance(it, str) or hasattr(it, "__fspath__"):
+                    videos.append(_read_video_frames(it, self.arch["video_frames"]))
+                else:
+                    raise ValueError(f"Unsupported {modality.value} content type: {type(it)}, content: {it}")
+            return self._encode_videos(videos, normalize)
+        if modality == Modality.IMAGE and isinstance(content, (str, list)):
+            first = content[0] if isinstance(content, list) else content
+            if isinstance(first, str) and "http" not in first:   # the reference encodes such content as text
+                return self.encode([first], modality=Modality.TEXT, normalize=normalize)
+        if modality in (Modality.IMAGE, Modality.AUDIO):
+            # the reference calls preprocessor(modality), which is None for a model without that tower
+            raise TypeError(f"'NoneType' object is not callable: {self.model_properties.get('name')} has no "
+                            f"{modality.value} tower")
+        raise ValueError(f"Unsupported modality {modality}")
+
+
 LOADERS = {
     model_registry.TYPE_OPEN_CLIP: B200OpenCLIP,
     model_registry.TYPE_HF: B200HuggingFace,
@@ -646,6 +819,7 @@ LOADERS = {
     model_registry.TYPE_CLIP: B200Clip,
     model_registry.TYPE_FP16_CLIP: B200Fp16Clip,
     model_registry.TYPE_MULTILINGUAL_CLIP: B200MultilingualClip,
+    model_registry.TYPE_LANGUAGEBIND: B200LanguageBind,
 }
 
 

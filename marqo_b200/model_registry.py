@@ -208,6 +208,7 @@ TYPE_HF_STELLA = "b200_hf_stella"
 TYPE_CLIP = "b200_clip"
 TYPE_FP16_CLIP = "b200_fp16_clip"
 TYPE_MULTILINGUAL_CLIP = "b200_multilingual_clip"
+TYPE_LANGUAGEBIND = "b200_languagebind"
 
 
 def _clip_arch(embed, vw, vl, vh, patch, tw, tl, th, act="gelu", image_size=224):
@@ -639,6 +640,28 @@ OWL_VIT_MODELS: Dict[str, dict] = {
     )
 }
 
+# Marqo's `languagebind` entries (model_registry.py:2003-2064).  The engine serves LanguageBind/Video_V1.5_FT, the video
+# + language model: a CLIP ViT-L/14 video tower over 8 frames with a temporal attention sub-layer in every block, and
+# the CLIP text tower (loaders.B200LanguageBind).  The five other names need the audio tower (a Kaldi fbank front end)
+# or the LanguageBind_Image tower with its own text tower, and stay unserved: find_model does not know them.  The arch
+# block keeps the CLIP layout (vision 1024 x 24 x 16, text 768 x 12 x 12, the OpenAI mean and std), so the registry
+# walks of the GEMM, layer and patch-embedding tests see no new shape; video_frames says it is the video tower, and
+# the loader checks every field against the checkpoint's config.json.
+LANGUAGEBIND_UNSERVED = ("LanguageBind/Video_V1.5_FT_Audio_FT_Image", "LanguageBind/Video_V1.5_FT_Audio_FT",
+                         "LanguageBind/Video_V1.5_FT_Image", "LanguageBind/Audio_FT_Image", "LanguageBind/Audio_FT")
+
+
+def _languagebind_models() -> Dict[str, dict]:
+    arch = dict(_clip_arch(**_VIT_L_14), video_frames=8)
+    name = "LanguageBind/Video_V1.5_FT"
+    return {name: {"name": name, "dimensions": 768, "type": TYPE_LANGUAGEBIND, "loader": "languagebind",
+                   "model_size": 2, "supported_modalities": ["video", "language"], "video_chunk_length": 20,
+                   "audio_chunk_length": 10, "arch": arch}}
+
+
+LANGUAGEBIND_MODELS: Dict[str, dict] = _languagebind_models()
+
+
 def _count(sd: dict, prefix: str) -> int:
     """The number of distinct indices i among the keys prefix + "i.*"."""
     return len({k[len(prefix):].split(".")[0] for k in sd if k.startswith(prefix)})
@@ -681,7 +704,8 @@ def openai_clip_arch(sd: dict) -> dict:
 def find_model(model_name: str) -> Optional[dict]:
     """The registry entry of `model_name` (not a copy), or None: the one lookup over every table of served models."""
     for table in (MODELS, MPNET_MODELS, SIGLIP_MODELS, XLMR_MODELS, RESNET_MODELS, CONVNEXT_MODELS, BIG_VIT_MODELS,
-                  EVA02_MODELS, GTE_MODELS, COCA_MODELS, OPENAI_CLIP_MODELS, MULTILINGUAL_CLIP_MODELS):
+                  EVA02_MODELS, GTE_MODELS, COCA_MODELS, OPENAI_CLIP_MODELS, MULTILINGUAL_CLIP_MODELS,
+                  LANGUAGEBIND_MODELS):
         entry = table.get(model_name)
         if entry is not None:
             return entry
@@ -701,10 +725,11 @@ def all_models() -> Dict[str, dict]:
     tests/test_coca_kernels_gpu.py.  OPENAI_CLIP_MODELS is in: its text towers are 512, 768 and 1024 wide, and its
     one new layer shape (ViT-L/14@336px's vision layers at 577 tokens) runs in tests/test_layers_gpu.py.
     MULTILINGUAL_CLIP_MODELS is in: its text towers are multilingual-e5-large's and a BERT-base, 1024 and 768 wide, and
-    its image towers are named OPENAI_CLIP_MODELS entries, not blocks of their own.
+    its image towers are named OPENAI_CLIP_MODELS entries, not blocks of their own.  LANGUAGEBIND_MODELS is in: its
+    towers are the ViT-L/14 CLIP shapes, and its temporal GEMMs have the shapes of the spatial attention's.
     served_models() has every served entry; find_model looks in every table."""
     return {**MODELS, **MPNET_MODELS, **SIGLIP_MODELS, **XLMR_MODELS, **RESNET_MODELS, **EVA02_MODELS, **GTE_MODELS,
-            **COCA_MODELS, **OPENAI_CLIP_MODELS, **MULTILINGUAL_CLIP_MODELS}
+            **COCA_MODELS, **OPENAI_CLIP_MODELS, **MULTILINGUAL_CLIP_MODELS, **LANGUAGEBIND_MODELS}
 
 
 def served_models() -> Dict[str, dict]:

@@ -101,11 +101,18 @@ def validate_model_properties(model_name: str, model_properties: Optional[dict])
     mtype = props.get("type")
     alias = {"open_clip": model_registry.TYPE_OPEN_CLIP, "hf": model_registry.TYPE_HF,
              "hf_stella": model_registry.TYPE_HF_STELLA, "clip": model_registry.TYPE_CLIP,
-             "fp16_clip": model_registry.TYPE_FP16_CLIP, "multilingual_clip": model_registry.TYPE_MULTILINGUAL_CLIP}
+             "fp16_clip": model_registry.TYPE_FP16_CLIP, "multilingual_clip": model_registry.TYPE_MULTILINGUAL_CLIP,
+             "languagebind": model_registry.TYPE_LANGUAGEBIND}
     props["type"] = alias.get(mtype, mtype)
     if props["type"] not in alias.values():
         raise InvalidModelPropertiesError(f"model type `{mtype}` is not served by the H100 engine (supported: "
-                                          f"open_clip, hf, hf_stella, clip, fp16_clip, multilingual_clip)")
+                                          f"open_clip, hf, hf_stella, clip, fp16_clip, multilingual_clip, "
+                                          f"languagebind)")
+    if props["type"] == model_registry.TYPE_LANGUAGEBIND and model_name not in model_registry.LANGUAGEBIND_MODELS:
+        # the reference's LanguageBind loads the towers its name lists; the engine has the video one only
+        raise InvalidModelPropertiesError(
+            f"languagebind model `{model_name}` is not served by the H100 engine (served: "
+            f"{', '.join(model_registry.LANGUAGEBIND_MODELS)})")
     if (props["type"] == model_registry.TYPE_MULTILINGUAL_CLIP
             and model_name not in model_registry.MULTILINGUAL_CLIP_MODELS):
         # the reference's MULTILINGUAL_CLIP reads its towers from get_multilingual_clip_properties()[model_name]
@@ -175,7 +182,8 @@ def _reference_type_name(t):
     return {model_registry.TYPE_OPEN_CLIP: "open_clip", model_registry.TYPE_HF: "hf",
             model_registry.TYPE_HF_STELLA: "hf_stella", model_registry.TYPE_CLIP: "clip",
             model_registry.TYPE_FP16_CLIP: "fp16_clip",
-            model_registry.TYPE_MULTILINGUAL_CLIP: "multilingual_clip"}.get(t, t)
+            model_registry.TYPE_MULTILINGUAL_CLIP: "multilingual_clip",
+            model_registry.TYPE_LANGUAGEBIND: "languagebind"}.get(t, t)
 
 
 def _check_memory_threshold_for_model(device: str, model_size) -> bool:
@@ -295,7 +303,10 @@ def load_multimodal_model_and_get_preprocessors(model_name: str, model_propertie
     model = _available_models[model_cache_key][AvailableModelsKey.model]
     preprocessors = {
         "image": getattr(model, "preprocess", None) if is_preprocess_image_model(model_properties) else None,
-        "video": None,
+        # LanguageBind's video preprocessor (multimodal_model_load.py:236-250): cv2 decode and frame sampling on the
+        # host; the transform runs on the GPU
+        "video": (model.preprocessor(Modality.VIDEO)
+                  if model_properties.get("type") == model_registry.TYPE_LANGUAGEBIND else None),
         "audio": None,
         "text": None,
     }

@@ -376,8 +376,47 @@ def random_cross_encoder_weights(arch: dict, seed: int = 1234) -> Dict[str, np.n
 # transformers' CLIP-style encoder layer names -> open_clip's (the engine's) below a tower's resblock prefix
 _OWL_LAYER_NAMES = {"layer_norm1.": "ln_1.", "layer_norm2.": "ln_2.", "self_attn.out_proj.": "attn.out_proj.",
                     "mlp.fc1.": "mlp.c_fc.", "mlp.fc2.": "mlp.c_proj."}
+# and LanguageBind's temporal sub-layer (languagebind/video/modeling_video.py:180-187), whose q | k | v go to
+# temporal_attn.in_proj_* as self_attn's go to attn.in_proj_*
+_TEMPORAL_LAYER_NAMES = {"temporal_layer_norm1.": "temporal_ln_1.", "temporal_attn.out_proj.": "temporal_attn.out_proj.",
+                         "temporal_embedding": "temporal_embedding"}
 # the two OWL-ViT tensors the detector never reads: the CLIP image projection and the contrastive temperature
 OWLVIT_UNUSED = ("owlvit.visual_projection.weight", "owlvit.logit_scale")
+
+
+def _hf_clip_tower_tensor(key: str, rest: str, dst: str, a: np.ndarray, out: dict, qkv: dict, what: str,
+                          layer_names: dict, attns: dict) -> None:
+    """One tensor of a transformers CLIP-style tower, `rest` its name below the tower's prefix, under the engine's
+    names below `dst`: pre_layrnorm (also spelt pre_layernorm) -> ln_pre, post_layernorm -> ln_post, final_layer_norm
+    -> ln_final, a layer's q / k / v parts of each attention in `attns` (its transformers prefix -> the engine's fused
+    in_proj_ prefix) collected in qkv, its other parts renamed by layer_names.  Any other name raises KeyError."""
+    for a_name, b_name in (("pre_layrnorm.", "ln_pre."), ("pre_layernorm.", "ln_pre."),
+                           ("post_layernorm.", "ln_post."), ("final_layer_norm.", "ln_final.")):
+        if rest.startswith(a_name):
+            out[dst + b_name + rest[len(a_name):]] = a
+            return
+    if not rest.startswith("encoder.layers."):
+        raise KeyError(f"{key}: not {what} parameter the engine knows")
+    i, sub = rest[len("encoder.layers."):].split(".", 1)
+    p = f"{dst}transformer.resblocks.{i}."
+    for src, fused in attns.items():
+        if sub.startswith(src) and sub[len(src):len(src) + 2] in ("q_", "k_", "v_"):
+            qkv.setdefault(p + fused + sub.rsplit(".", 1)[1], {})[sub[len(src)]] = a
+            return
+    for a_name, b_name in layer_names.items():
+        if sub.startswith(a_name):
+            out[p + b_name + sub[len(a_name):]] = a
+            return
+    raise KeyError(f"{key}: not {what} parameter the engine knows")
+
+
+def _stack_qkv(qkv: dict, out: dict) -> None:
+    for name, parts in qkv.items():
+        out[name] = np.concatenate([parts["q"], parts["k"], parts["v"]], axis=0)
+
+
+def _f32(v) -> np.ndarray:
+    return np.asarray(v.detach().cpu().numpy() if hasattr(v, "detach") else v, dtype=np.float32)
 
 
 def owlvit_state_dict_to_engine(sd: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
@@ -396,7 +435,7 @@ def owlvit_state_dict_to_engine(sd: Dict[str, np.ndarray]) -> Dict[str, np.ndarr
              "owlvit.text_model.embeddings.token_embedding.weight": "token_embedding.weight",
              "owlvit.text_model.embeddings.position_embedding.weight": "positional_embedding"}
     for k, v in sd.items():
-        a = np.asarray(v.detach().cpu().numpy() if hasattr(v, "detach") else v, dtype=np.float32)
+        a = _f32(v)
         if k in fixed:
             out[fixed[k]] = a
         elif k == "owlvit.text_projection.weight":
@@ -405,34 +444,122 @@ def owlvit_state_dict_to_engine(sd: Dict[str, np.ndarray]) -> Dict[str, np.ndarr
             out[k] = a
         else:
             for src, dst in towers:
-                if not k.startswith(src):
-                    continue
-                rest = k[len(src):]
-                for a_name, b_name in (("pre_layrnorm.", "ln_pre."), ("pre_layernorm.", "ln_pre."),
-                                       ("post_layernorm.", "ln_post."), ("final_layer_norm.", "ln_final.")):
-                    if rest.startswith(a_name):
-                        out[dst + b_name + rest[len(a_name):]] = a
-                        break
-                else:
-                    if not rest.startswith("encoder.layers."):
-                        raise KeyError(f"{k}: not an OwlViTForObjectDetection parameter the engine knows")
-                    i, sub = rest[len("encoder.layers."):].split(".", 1)
-                    p = f"{dst}transformer.resblocks.{i}."
-                    if sub.startswith("self_attn.") and sub[10:12] in ("q_", "k_", "v_"):
-                        qkv.setdefault(p + "attn.in_proj_" + sub.rsplit(".", 1)[1], {})[sub[10]] = a
-                        break
-                    for a_name, b_name in _OWL_LAYER_NAMES.items():
-                        if sub.startswith(a_name):
-                            out[p + b_name + sub[len(a_name):]] = a
-                            break
-                    else:
-                        raise KeyError(f"{k}: not an OwlViTForObjectDetection parameter the engine knows")
-                break
+                if k.startswith(src):
+                    _hf_clip_tower_tensor(k, k[len(src):], dst, a, out, qkv, "an OwlViTForObjectDetection",
+                                          _OWL_LAYER_NAMES, {"self_attn.": "attn.in_proj_"})
+                    break
             else:
                 raise KeyError(f"{k}: not an OwlViTForObjectDetection parameter the engine knows")
-    for name, parts in qkv.items():
-        out[name] = np.concatenate([parts["q"], parts["k"], parts["v"]], axis=0)
+    _stack_qkv(qkv, out)
     return out
+
+
+def languagebind_video_state_dict_to_engine(sd: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
+    """A LanguageBindVideo state dict (languagebind/video/modeling_video.py:842-873) under the engine's names
+    (b200_model_desc video_frames): the CLIP renames of owlvit_state_dict_to_engine for both towers, plus each vision
+    layer's temporal_embedding [1, T, W] -> [T, W], temporal_layer_norm1 -> temporal_ln_1 and temporal_attn's q | k | v
+    stacked into temporal_attn.in_proj_*; visual_projection.weight [E, W] and text_projection.weight transposed to
+    visual.proj and text_projection [W, E]; logit_scale as [1].  A Conv3d patch embedding [W, 3, tube, P, P] of tube 1
+    (CLIPVisionEmbeddings3D) loses its tube axis; one of tube > 1 keeps it, and the engine refuses its size.  Every
+    tensor is used but the position_ids buffers; any other name raises KeyError."""
+    out: Dict[str, np.ndarray] = {}
+    qkv: Dict[str, Dict[str, np.ndarray]] = {}
+    towers = (("vision_model.", "visual."), ("text_model.", ""))
+    fixed = {"vision_model.embeddings.class_embedding": "visual.class_embedding",
+             "vision_model.embeddings.position_embedding.weight": "visual.positional_embedding",
+             "text_model.embeddings.token_embedding.weight": "token_embedding.weight",
+             "text_model.embeddings.position_embedding.weight": "positional_embedding"}
+    layer_names = {**_OWL_LAYER_NAMES, **_TEMPORAL_LAYER_NAMES}
+    attns = {"self_attn.": "attn.in_proj_", "temporal_attn.": "temporal_attn.in_proj_"}
+    for k, v in sd.items():
+        if k.endswith("position_ids"):
+            continue
+        a = _f32(v)
+        if k in fixed:
+            out[fixed[k]] = a
+        elif k == "vision_model.embeddings.patch_embedding.weight":
+            out["visual.conv1.weight"] = a[:, :, 0] if a.ndim == 5 and a.shape[2] == 1 else a
+        elif k in ("visual_projection.weight", "text_projection.weight"):
+            out["visual.proj" if k[0] == "v" else "text_projection"] = np.ascontiguousarray(a.T)
+        elif k == "logit_scale":
+            out[k] = a.reshape(1)
+        else:
+            for src, dst in towers:
+                if k.startswith(src):
+                    _hf_clip_tower_tensor(k, k[len(src):], dst, a, out, qkv, "a LanguageBindVideo", layer_names,
+                                          attns)
+                    break
+            else:
+                raise KeyError(f"{k}: not a LanguageBindVideo parameter the engine knows")
+    for name in [n for n in out if n.endswith(".temporal_embedding")]:
+        out[name] = out[name].reshape(-1, out[name].shape[-1])
+    _stack_qkv(qkv, out)
+    return out
+
+
+def random_languagebind_video_weights(arch: dict, seed: int = 1234, form: str = "vl_new") -> Dict[str, np.ndarray]:
+    """Seeded random weights of a LanguageBindVideo under its checkpoint's names and shapes (arch: the registry's
+    LanguageBind block, the CLIP block of Encoder("clip") with video_frames T).  form "vl_new": CLIPVisionEmbeddings3D's
+    class_embedding [T, W] and Conv3d patch_embedding [W, 3, 1, P, P]; "vl": CLIPVisionEmbeddings' [W] and
+    [W, 3, P, P].  Every temporal_embedding is [1, T, W]; logit_scale a scalar near log(100)."""
+    g = _rng(seed)
+    v, t, E, T = arch["vision"], arch["text"], arch["embed_dim"], arch["video_frames"]
+    sd: Dict[str, np.ndarray] = {}
+
+    def attention(p, w, rg):
+        for nm in ("q_proj", "k_proj", "v_proj"):
+            sd[p + f"{nm}.weight"] = _lin(g, w, w, 1.5)
+            sd[p + f"{nm}.bias"] = _vec(g, w)
+        sd[p + "out_proj.weight"] = _lin(g, w, w, rg)
+        sd[p + "out_proj.bias"] = _vec(g, w)
+
+    def layers(prefix, tw, temporal):
+        w, mlp, L = tw["width"], tw["mlp"], tw["layers"]
+        rg = 1.0 / math.sqrt(2.0 * L)
+        for i in range(L):
+            p = f"{prefix}encoder.layers.{i}."
+            for nm in ("layer_norm1", "layer_norm2"):
+                sd[p + nm + ".weight"] = _vec(g, w, 0.1, 1.0)
+                sd[p + nm + ".bias"] = _vec(g, w)
+            attention(p + "self_attn.", w, rg)
+            sd[p + "mlp.fc1.weight"] = _lin(g, mlp, w)
+            sd[p + "mlp.fc1.bias"] = _vec(g, mlp)
+            sd[p + "mlp.fc2.weight"] = _lin(g, w, mlp, rg)
+            sd[p + "mlp.fc2.bias"] = _vec(g, w)
+            if temporal:
+                sd[p + "temporal_embedding"] = (g.standard_normal((1, T, w), dtype=np.float32) *
+                                                np.float32(w ** -0.5))
+                sd[p + "temporal_layer_norm1.weight"] = _vec(g, w, 0.1, 1.0)
+                sd[p + "temporal_layer_norm1.bias"] = _vec(g, w)
+                attention(p + "temporal_attn.", w, rg)
+
+    w, p = v["width"], v["patch"]
+    grid = v["image_size"] // p
+    vm = "vision_model."
+    conv = g.standard_normal((w, 3, p, p), dtype=np.float32) / np.float32(math.sqrt(3 * p * p))
+    if form == "vl_new":
+        sd[vm + "embeddings.class_embedding"] = np.stack([_vec(g, w, 0.5) for _ in range(T)])
+        sd[vm + "embeddings.patch_embedding.weight"] = np.ascontiguousarray(conv[:, :, None])
+    else:
+        sd[vm + "embeddings.class_embedding"] = _vec(g, w, 0.5)
+        sd[vm + "embeddings.patch_embedding.weight"] = conv
+    sd[vm + "embeddings.position_embedding.weight"] = 0.5 * g.standard_normal((grid * grid + 1, w), dtype=np.float32)
+    sd[vm + "pre_layrnorm.weight"] = _vec(g, w, 0.1, 1.0)
+    sd[vm + "pre_layrnorm.bias"] = _vec(g, w)
+    layers(vm, v, True)
+    sd[vm + "post_layernorm.weight"] = _vec(g, w, 0.1, 1.0)
+    sd[vm + "post_layernorm.bias"] = _vec(g, w)
+    tw = t["width"]
+    tm = "text_model."
+    sd[tm + "embeddings.token_embedding.weight"] = g.standard_normal((t["vocab"], tw), dtype=np.float32)
+    sd[tm + "embeddings.position_embedding.weight"] = 0.5 * g.standard_normal((t["ctx"], tw), dtype=np.float32)
+    layers(tm, t, False)
+    sd[tm + "final_layer_norm.weight"] = _vec(g, tw, 0.1, 1.0)
+    sd[tm + "final_layer_norm.bias"] = _vec(g, tw)
+    sd["visual_projection.weight"] = _lin(g, E, w)
+    sd["text_projection.weight"] = _lin(g, E, tw)
+    sd["logit_scale"] = np.array(4.6052, np.float32)
+    return sd
 
 
 def random_owlvit_weights(arch: dict, seed: int = 1234) -> Dict[str, np.ndarray]:
