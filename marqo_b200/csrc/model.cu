@@ -71,6 +71,11 @@ struct Kinds {
     bool mpnet = false;   // ROBERTA: MPNet's layer names and relative-position bias, else XLM-R's token-type row
 };
 
+// The model calls of the C ABI by what they run, which decides whether a model takes them (require_accepts): IMAGES
+// every image encode (u8, u8 device, ragged, ragged device, f32), TOKENS encode_tokens(_device), CLASSIFY
+// classify_tokens(_device), DETECT detect_images_u8, VIDEOS encode_videos_u8(_device).
+enum class Call { IMAGES, TOKENS, CLASSIFY, DETECT, VIDEOS };
+
 struct TowerW {
     b200_tower_desc d{};
     // the attention width heads * kernel_head_dim(width / heads): width, or for the ViT-H / g / bigG vision towers the
@@ -227,12 +232,13 @@ struct b200_model {
     int prof_n = 0;
     // CUDA graphs of small (launch-bound) forward passes, keyed by everything the captured launches depend on
     struct GraphKey {
-        int kind, n, S, normalize;
+        Call pass;   // forward_images (IMAGES), forward_tokens (TOKENS), forward_detect or forward_videos
+        int n, S, normalize;
         const void *in0, *in1, *out;
         const void* in2 = nullptr;   // token-type ids of a classified pair batch
         bool operator<(const GraphKey& o) const {
-            return std::tie(kind, n, S, normalize, in0, in1, out, in2) <
-                   std::tie(o.kind, o.n, o.S, o.normalize, o.in0, o.in1, o.out, o.in2);
+            return std::tie(pass, n, S, normalize, in0, in1, out, in2) <
+                   std::tie(o.pass, o.n, o.S, o.normalize, o.in0, o.in1, o.out, o.in2);
         }
     };
     struct GraphEntry {
@@ -1689,25 +1695,21 @@ void run_graphed(b200_model* m, Counter& c, const b200_model::GraphKey& key, lon
     c.n += it->second.launches;
 }
 
-void ensure_in_dev(b200_model* m, size_t bytes) {
-    if (bytes > m->in_dev.size()) m->in_dev = DeviceBuffer<uint8_t>(bytes);
-}
-
 void forward_images(b200_model* m, Counter& c, const uint8_t* u8, const float* f32, int n, int normalize, float* d_out) {
-    const b200_model::GraphKey key{0, n, 0, normalize, u8, f32, d_out};
+    const b200_model::GraphKey key{Call::IMAGES, n, 0, normalize, u8, f32, d_out};
     run_graphed(m, c, key, (long long)n * m->vision.tokens,
                 [&](Counter& cc) { forward_images_eager(m, cc, u8, f32, n, normalize, d_out); });
 }
 
 void forward_tokens(b200_model* m, Counter& c, const int32_t* d_ids, const int32_t* d_mask, const int32_t* d_types, int n,
                     int S, int normalize, float* d_out) {
-    const b200_model::GraphKey key{1, n, S, normalize, d_ids, d_mask, d_out, d_types};
+    const b200_model::GraphKey key{Call::TOKENS, n, S, normalize, d_ids, d_mask, d_out, d_types};
     run_graphed(m, c, key, (long long)n * S,
                 [&](Counter& cc) { forward_tokens_eager(m, cc, d_ids, d_mask, d_types, n, S, normalize, d_out); });
 }
 
 void forward_detect(b200_model* m, Counter& c, const uint8_t* u8, int n, const float* t, float* logits, float* boxes) {
-    const b200_model::GraphKey key{2, n, 0, 0, u8, t, logits, boxes};
+    const b200_model::GraphKey key{Call::DETECT, n, 0, 0, u8, t, logits, boxes};
     run_graphed(m, c, key, (long long)n * m->vision.tokens,
                 [&](Counter& cc) { forward_detect_eager(m, cc, u8, n, t, logits, boxes); });
 }
@@ -1716,7 +1718,7 @@ void forward_detect(b200_model* m, Counter& c, const uint8_t* u8, int n, const f
 // head (the mean of the frames' ln_post class rows, visual.proj, L2 times exp(logit_scale), optional L2)
 void forward_videos(b200_model* m, Counter& c, const float* f32, int n, int normalize, float* d_out) {
     const TowerW& T = m->vision;
-    const b200_model::GraphKey key{3, n, 0, normalize, nullptr, f32, d_out};
+    const b200_model::GraphKey key{Call::VIDEOS, n, 0, normalize, nullptr, f32, d_out};
     run_graphed(m, c, key, (long long)n * T.frames * T.tokens, [&](Counter& cc) {
         forward_vit(m, cc, T, nullptr, f32, n * T.frames);
         cc.n += kernels::frame_mean_head(m->x.get(), T.tokens, T.frames, nullptr, T.ln_out_w, T.ln_out_b, T.eps, T.proj,
@@ -1728,6 +1730,93 @@ void forward_videos(b200_model* m, Counter& c, const float* f32, int n, int norm
 void require_ready(b200_model* m) {
     MB_CHECK_ARG(m != nullptr, "model is NULL");
     if (!m->finalized) fail(B200_ERR_INVALID_ARG, "b200_model_finalize has not been called");
+}
+
+// Which calls a model takes: an OWL-ViT detector only detects, a video model encodes videos (and its text), and a text
+// tower with a classification head classifies instead of encoding.
+void require_accepts(b200_model* m, Call call) {
+    const VisionKind vk = m->kind.vision;
+    const char* owl = "this model is an OWL-ViT detector: detect images with a query";
+    switch (call) {
+    case Call::IMAGES:
+        MB_CHECK_ARG(vk != VisionKind::NONE, "this model has no vision tower");
+        MB_CHECK_ARG(!m->desc.owl_detect, "%s", owl);
+        MB_CHECK_ARG(vk != VisionKind::VIDEO_VIT, "this model is a video model: encode videos of %d frames",
+                     m->vision.frames);
+        break;
+    case Call::TOKENS:
+    case Call::CLASSIFY:
+        MB_CHECK_ARG(m->kind.text != TextKind::NONE, "this model has no text tower");
+        MB_CHECK_ARG(!m->desc.owl_detect, "%s", owl);
+        if (call == Call::CLASSIFY)
+            MB_CHECK_ARG(m->desc.cls_labels > 0, "this model has no classification head (cls_labels 0)");
+        else
+            MB_CHECK_ARG(m->desc.cls_labels == 0, "this model is a classifier (cls_labels %d): classify its tokens",
+                         m->desc.cls_labels);
+        break;
+    case Call::DETECT:
+        MB_CHECK_ARG(m->desc.owl_detect, "this model has no OWL-ViT detection head (owl_detect 0)");
+        break;
+    case Call::VIDEOS:
+        MB_CHECK_ARG(vk == VisionKind::VIDEO_VIT, "this model has no video tower (video_frames 0)");
+        break;
+    }
+}
+
+// Every model call.  All its refusals come first, so that a refused call writes nothing and leaves last_timing as it
+// was: readiness, whether the model takes `call`, then `check`, the call's own argument checks, which returns the bytes
+// of host input the call stages in in_dev (0 for device inputs).  Then, under the model's lock on its device, in_dev
+// is sized and `body` runs on the model's stream, timed into last_timing, with a final synchronise if `sync`.
+template <class Check, class Body>
+int model_call(b200_model* m, Call call, int sync, Check&& check, Body&& body) {
+    return guarded([&] {
+        require_ready(m);
+        require_accepts(m, call);
+        const size_t staged = check();
+        std::lock_guard<std::mutex> lk(m->mu);
+        DeviceGuard g(m->device);
+        if (staged > m->in_dev.size()) m->in_dev = DeviceBuffer<uint8_t>(staged);
+        Counter c;
+        MB_CUDA(cudaEventRecord(m->ev0.get(), m->stream));
+        body(c);
+        MB_CUDA(cudaEventRecord(m->ev1.get(), m->stream));
+        m->timing_valid = true;
+        m->last_launches = c.n;
+        if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
+    });
+}
+
+void to_device(b200_model* m, void* dst, const void* src, size_t bytes) {
+    MB_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, m->stream));
+}
+
+// A device output of a host call and where it goes: `per` floats of each item.
+struct HostOut {
+    float* host;
+    const float* dev;
+    size_t per;
+};
+
+// A host call's n items in sub-batches of up to cap: stage(o, nb) copies the inputs of items o .. o + nb - 1 into
+// in_dev, run(o, nb) runs the device path over them, and every output's nb items come back before the synchronise
+// that frees in_dev for the next sub-batch.
+template <class Stage, class Run>
+void host_batches(b200_model* m, int n, int cap, Stage&& stage, Run&& run, std::initializer_list<HostOut> outs) {
+    for (int o = 0; o < n; o += cap) {
+        const int nb = std::min(cap, n - o);
+        stage(o, nb);
+        run(o, nb);
+        for (const HostOut& r : outs)
+            MB_CUDA(cudaMemcpyAsync(r.host + (size_t)o * r.per, r.dev, (size_t)nb * r.per * sizeof(float),
+                                    cudaMemcpyDeviceToHost, m->stream));
+        MB_CUDA(cudaStreamSynchronize(m->stream));
+    }
+}
+
+// the n, h, w and buffers of a uint8 image or video call
+void check_u8_args(bool buffers, int n, int h, int w) {
+    MB_CHECK_ARG(buffers, "NULL buffer");
+    MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
 }
 
 int batch_cap_tokens(b200_model* m, int tokens_per_item) {
@@ -1756,43 +1845,28 @@ void encode_videos_u8_dev(b200_model* m, Counter& c, const uint8_t* d_vid, int n
     }
 }
 
-void check_videos_args(b200_model* m, int n, int t, int h, int w) {
-    MB_CHECK_ARG(m->kind.vision == VisionKind::VIDEO_VIT, "this model has no video tower (video_frames 0)");
-    MB_CHECK_ARG(t == m->vision.frames, "videos of %d frames: the model takes %d", t, m->vision.frames);
-    MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
-}
-
-struct TimedRegion {
-    b200_model* m;
-    Counter c;
-    explicit TimedRegion(b200_model* mm) : m(mm) { MB_CUDA(cudaEventRecord(m->ev0.get(), m->stream)); }
-    void finish() {
-        MB_CUDA(cudaEventRecord(m->ev1.get(), m->stream));
-        m->timing_valid = true;
-        m->last_launches = c.n;
-    }
-};
-
 // open_clip's SigLIP and DFN5B preprocessing squashes (no crop); every other tower crops
 bool resize_squashes(b200_model* m) { return m->kind.vision == VisionKind::SIGLIP_VIT || m->desc.resize_squash; }
+
+// nb device uint8 images of h x w as the image tower takes them, S x S: resized into m->resized, unless already S x S
+const uint8_t* resize_images(b200_model* m, Counter& c, const uint8_t* src, int nb, int h, int w) {
+    const int S = m->vision.d.image_size;
+    if (h == S && w == S) return src;
+    if (resize_squashes(m))
+        c.n += kernels::resize_squash_u8(src, nb, h, w, S, m->resized.get(), m->stream);
+    else
+        c.n += kernels::resize_crop_u8(src, nb, h, w, S, m->resized.get(), m->stream);
+    return m->resized.get();
+}
 
 // device-resident uint8 images of size h x w -> embeddings
 void encode_images_u8_dev(b200_model* m, Counter& c, const uint8_t* d_img, int n, int h, int w, int normalize,
                           float* d_out) {
-    const TowerW& T = m->vision;
-    const int S = T.d.image_size;
     const int cap = image_batch_cap(m);
     for (int o = 0; o < n; o += cap) {
         const int nb = std::min(cap, n - o);
-        const uint8_t* src = d_img + (size_t)o * h * w * 3;
-        if (h != S || w != S) {
-            if (resize_squashes(m))
-                c.n += kernels::resize_squash_u8(src, nb, h, w, S, m->resized.get(), m->stream);
-            else
-                c.n += kernels::resize_crop_u8(src, nb, h, w, S, m->resized.get(), m->stream);
-            src = m->resized.get();
-        }
-        forward_images(m, c, src, nullptr, nb, normalize, d_out + (size_t)o * m->desc.embed_dim);
+        forward_images(m, c, resize_images(m, c, d_img + (size_t)o * h * w * 3, nb, h, w), nullptr, nb, normalize,
+                       d_out + (size_t)o * m->desc.embed_dim);
     }
 }
 
@@ -1809,18 +1883,9 @@ void encode_images_u8_ragged_dev(b200_model* m, Counter& c, const uint8_t* const
     }
 }
 
-// every image encode call: a vision tower with an embedding head
-void check_encodes_images(b200_model* m) {
-    MB_CHECK_ARG(m->kind.vision != VisionKind::NONE, "this model has no vision tower");
-    MB_CHECK_ARG(!m->desc.owl_detect, "this model is an OWL-ViT detector: detect images with a query");
-    MB_CHECK_ARG(m->kind.vision != VisionKind::VIDEO_VIT, "this model is a video model: encode videos of %d frames",
-                 m->vision.frames);
-}
-
 // the arguments of a ragged image call, all checked before anything is written
-void check_ragged_args(b200_model* m, const uint8_t* const* imgs, const int32_t* h, const int32_t* w, int n) {
+void check_ragged_args(const uint8_t* const* imgs, const int32_t* h, const int32_t* w, int n) {
     MB_CHECK_ARG(imgs && h && w, "NULL array");
-    check_encodes_images(m);
     MB_CHECK_ARG(n > 0, "n must be positive");
     for (int i = 0; i < n; ++i) {
         MB_CHECK_ARG(imgs[i] != nullptr, "image %d is NULL", i);
@@ -1842,64 +1907,56 @@ void encode_tokens_dev(b200_model* m, Counter& c, const int32_t* d_ids, const in
     }
 }
 
-// classify: the call is b200_model_classify_tokens*, which only a classifier (cls_labels > 0) takes; the encode calls
-// refuse one
-void check_tokens_args(b200_model* m, int n, int S, bool classify = false) {
-    MB_CHECK_ARG(m->kind.text != TextKind::NONE, "this model has no text tower");
-    MB_CHECK_ARG(!m->desc.owl_detect, "this model is an OWL-ViT detector: detect images with a query");
-    MB_CHECK_ARG(!classify || m->desc.cls_labels > 0, "this model has no classification head (cls_labels 0)");
-    MB_CHECK_ARG(classify || m->desc.cls_labels == 0, "this model is a classifier (cls_labels %d): classify its tokens",
-                 m->desc.cls_labels);
+// the arguments of a token call
+void check_tokens_args(b200_model* m, int n, int S) {
     MB_CHECK_ARG(n > 0, "n must be positive");
     MB_CHECK_ARG(S > 0 && S <= m->text.tokens, "sequence length %d out of range (1..%d)", S, m->text.tokens);
     if (m->kind.text == TextKind::COCA)   // open_clip's CoCa tokenizer pads every text to ctx - 1 ids
         MB_CHECK_ARG(S == m->text.tokens - 1, "CoCa text: ids must be %d wide (got %d)", m->text.tokens - 1, S);
 }
 
-// b200_model_encode_tokens and b200_model_classify_tokens: host ids, mask and token types (either may be NULL) in
-// sub-batches through the staging buffer; `normalize` is the classifier's activation when classify is set
-void tokens_host(b200_model* m, const int32_t* ids, const int32_t* attn_mask, const int32_t* types, int n, int seq,
-                 int normalize, float* out, bool classify) {
-    require_ready(m);
-    MB_CHECK_ARG(ids && out, "NULL buffer");
-    check_tokens_args(m, n, seq, classify);
-    if (attn_mask && m->kind.text != TextKind::CLIP && m->kind.text != TextKind::COCA) {
-        // the kernels implement prefix (right-padded) masks, which is what the tokenizer call at
-        // hugging_face_model.py:179-185 produces
-        for (int b = 0; b < n; ++b) {
-            bool seen_zero = false;
-            for (int s = 0; s < seq; ++s) {
-                const bool on = attn_mask[(size_t)b * seq + s] != 0;
-                if (on && seen_zero) fail(B200_ERR_UNSUPPORTED, "attention mask of item %d is not a prefix mask", b);
-                seen_zero |= !on;
-            }
+// The kernels implement prefix (right-padded) masks, which is what the tokenizer call at hugging_face_model.py:179-185
+// produces.
+void check_prefix_mask(const int32_t* mask, int n, int seq) {
+    for (int b = 0; b < n; ++b) {
+        bool seen_zero = false;
+        for (int s = 0; s < seq; ++s) {
+            const bool on = mask[(size_t)b * seq + s] != 0;
+            if (on && seen_zero) fail(B200_ERR_UNSUPPORTED, "attention mask of item %d is not a prefix mask", b);
+            seen_zero |= !on;
         }
     }
-    std::lock_guard<std::mutex> lk(m->mu);
-    DeviceGuard g(m->device);
-    const int E = m->desc.embed_dim;
-    const int cap = batch_cap_tokens(m, token_rows(m, seq));
-    const size_t row_bytes = (size_t)seq * 4, block = (size_t)std::min(n, cap) * seq;
-    ensure_in_dev(m, block * 4 * (types ? 3 : 2));
-    int32_t* d_ids = reinterpret_cast<int32_t*>(m->in_dev.get());
-    int32_t* d_mask = d_ids + block;
-    int32_t* d_types = types ? d_mask + block : nullptr;
-    TimedRegion tr(m);
-    for (int o = 0; o < n; o += cap) {
-        const int nb = std::min(cap, n - o);
-        MB_CUDA(cudaMemcpyAsync(d_ids, ids + (size_t)o * seq, (size_t)nb * row_bytes, cudaMemcpyHostToDevice, m->stream));
-        if (attn_mask)
-            MB_CUDA(cudaMemcpyAsync(d_mask, attn_mask + (size_t)o * seq, (size_t)nb * row_bytes, cudaMemcpyHostToDevice,
-                                    m->stream));
-        if (types)
-            MB_CUDA(cudaMemcpyAsync(d_types, types + (size_t)o * seq, (size_t)nb * row_bytes, cudaMemcpyHostToDevice,
-                                    m->stream));
-        forward_tokens(m, tr.c, d_ids, attn_mask ? d_mask : nullptr, d_types, nb, seq, normalize, m->out_dev.get());
-        MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
-                                m->stream));
-        MB_CUDA(cudaStreamSynchronize(m->stream));
-    }
-    tr.finish();
+}
+
+// b200_model_encode_tokens and b200_model_classify_tokens: host ids, mask and token types (either may be NULL) in
+// sub-batches through in_dev; `normalize` is the classifier's activation for CLASSIFY
+int tokens_host(b200_model* m, Call call, const int32_t* ids, const int32_t* attn_mask, const int32_t* types, int n,
+                int seq, int normalize, float* out) {
+    int cap = 0;
+    size_t block = 0;   // the ids of a sub-batch; the mask and the token types follow them in in_dev
+    return model_call(m, call, 0, [&] {
+        MB_CHECK_ARG(ids && out, "NULL buffer");
+        MB_CHECK_ARG(call == Call::TOKENS || normalize == 0 || normalize == 1,
+                     "activation %d must be 0 (identity) or 1 (sigmoid)", normalize);
+        check_tokens_args(m, n, seq);
+        if (attn_mask && m->kind.text != TextKind::CLIP && m->kind.text != TextKind::COCA)
+            check_prefix_mask(attn_mask, n, seq);
+        cap = batch_cap_tokens(m, token_rows(m, seq));
+        block = (size_t)std::min(n, cap) * seq;
+        return block * 4 * (types ? 3 : 2);
+    }, [&](Counter& c) {
+        int32_t* d_ids = reinterpret_cast<int32_t*>(m->in_dev.get());
+        int32_t* d_mask = d_ids + block;
+        int32_t* d_types = types ? d_mask + block : nullptr;
+        const size_t row_bytes = (size_t)seq * 4;
+        host_batches(m, n, cap, [&](int o, int nb) {
+            to_device(m, d_ids, ids + (size_t)o * seq, nb * row_bytes);
+            if (attn_mask) to_device(m, d_mask, attn_mask + (size_t)o * seq, nb * row_bytes);
+            if (types) to_device(m, d_types, types + (size_t)o * seq, nb * row_bytes);
+        }, [&](int, int nb) {
+            encode_tokens_dev(m, c, d_ids, attn_mask ? d_mask : nullptr, d_types, nb, seq, normalize, m->out_dev.get());
+        }, {{out, m->out_dev.get(), (size_t)m->desc.embed_dim}});
+    });
 }
 
 // The transformer tower b200_debug_layers runs: 0 vision, 1 text, if the model has one with layers.
@@ -2042,137 +2099,87 @@ int b200_model_finalize(b200_model* m) {
 }
 
 int b200_model_encode_images_u8(b200_model* m, const uint8_t* hwc, int n, int h, int w, int normalize, float* out) {
-    return guarded([&] {
-        require_ready(m);
-        MB_CHECK_ARG(hwc && out, "NULL buffer");
-        check_encodes_images(m);
-        MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        const int E = m->desc.embed_dim;
-        const int cap = m->desc.max_batch;
-        const size_t img_bytes = (size_t)h * w * 3;
-        ensure_in_dev(m, (size_t)std::min(n, cap) * img_bytes);
-        TimedRegion tr(m);
-        for (int o = 0; o < n; o += cap) {
-            const int nb = std::min(cap, n - o);
-            MB_CUDA(cudaMemcpyAsync(m->in_dev.get(), hwc + (size_t)o * img_bytes, (size_t)nb * img_bytes,
-                                    cudaMemcpyHostToDevice, m->stream));
-            encode_images_u8_dev(m, tr.c, m->in_dev.get(), nb, h, w, normalize, m->out_dev.get());
-            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
-                                    m->stream));
-            MB_CUDA(cudaStreamSynchronize(m->stream));
-        }
-        tr.finish();
+    const size_t img_bytes = (size_t)h * w * 3;
+    return model_call(m, Call::IMAGES, 0, [&] {
+        check_u8_args(hwc && out, n, h, w);
+        return (size_t)std::min(n, m->desc.max_batch) * img_bytes;
+    }, [&](Counter& c) {
+        host_batches(m, n, m->desc.max_batch, [&](int o, int nb) {
+            to_device(m, m->in_dev.get(), hwc + (size_t)o * img_bytes, nb * img_bytes);
+        }, [&](int, int nb) {
+            encode_images_u8_dev(m, c, m->in_dev.get(), nb, h, w, normalize, m->out_dev.get());
+        }, {{out, m->out_dev.get(), (size_t)m->desc.embed_dim}});
     });
 }
 
 int b200_model_encode_videos_u8(b200_model* m, const uint8_t* thwc, int n, int t, int h, int w, int normalize,
                                 float* out) {
-    return guarded([&] {
-        require_ready(m);
-        MB_CHECK_ARG(thwc && out, "NULL buffer");
-        check_videos_args(m, n, t, h, w);
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        const int E = m->desc.embed_dim;
-        const int cap = video_batch_cap(m);
-        const size_t video_bytes = (size_t)t * h * w * 3;
-        ensure_in_dev(m, (size_t)std::min(n, cap) * video_bytes);
-        TimedRegion tr(m);
-        for (int o = 0; o < n; o += cap) {
-            const int nb = std::min(cap, n - o);
-            MB_CUDA(cudaMemcpyAsync(m->in_dev.get(), thwc + (size_t)o * video_bytes, (size_t)nb * video_bytes,
-                                    cudaMemcpyHostToDevice, m->stream));
-            encode_videos_u8_dev(m, tr.c, m->in_dev.get(), nb, h, w, normalize, m->out_dev.get());
-            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
-                                    m->stream));
-            MB_CUDA(cudaStreamSynchronize(m->stream));
-        }
-        tr.finish();
+    const size_t video_bytes = (size_t)t * h * w * 3;
+    return model_call(m, Call::VIDEOS, 0, [&] {
+        check_u8_args(thwc && out, n, h, w);
+        MB_CHECK_ARG(t == m->vision.frames, "videos of %d frames: the model takes %d", t, m->vision.frames);
+        return (size_t)std::min(n, video_batch_cap(m)) * video_bytes;
+    }, [&](Counter& c) {
+        host_batches(m, n, video_batch_cap(m), [&](int o, int nb) {
+            to_device(m, m->in_dev.get(), thwc + (size_t)o * video_bytes, nb * video_bytes);
+        }, [&](int, int nb) {
+            encode_videos_u8_dev(m, c, m->in_dev.get(), nb, h, w, normalize, m->out_dev.get());
+        }, {{out, m->out_dev.get(), (size_t)m->desc.embed_dim}});
     });
 }
 
 int b200_model_encode_videos_u8_device(b200_model* m, const uint8_t* d_thwc, int n, int t, int h, int w, int normalize,
                                        float* d_out, int sync) {
-    return guarded([&] {
-        require_ready(m);
-        MB_CHECK_ARG(d_thwc && d_out, "NULL buffer");
-        check_videos_args(m, n, t, h, w);
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        TimedRegion tr(m);
-        encode_videos_u8_dev(m, tr.c, d_thwc, n, h, w, normalize, d_out);
-        tr.finish();
-        if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
-    });
+    return model_call(m, Call::VIDEOS, sync, [&] {
+        check_u8_args(d_thwc && d_out, n, h, w);
+        MB_CHECK_ARG(t == m->vision.frames, "videos of %d frames: the model takes %d", t, m->vision.frames);
+        return 0;
+    }, [&](Counter& c) { encode_videos_u8_dev(m, c, d_thwc, n, h, w, normalize, d_out); });
 }
 
 int b200_model_detect_images_u8(b200_model* m, const uint8_t* hwc, int n, int h, int w, const int32_t* query_ids,
                                 int seq, float* logits, float* boxes) {
-    return guarded([&] {
-        require_ready(m);
-        MB_CHECK_ARG(hwc && query_ids && logits && boxes, "NULL buffer");
-        MB_CHECK_ARG(m->desc.owl_detect, "this model has no OWL-ViT detection head (owl_detect 0)");
-        MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
+    const size_t img_bytes = (size_t)h * w * 3;
+    size_t ids_bytes = 0;   // in_dev holds the query's ids, then the images
+    return model_call(m, Call::DETECT, 0, [&] {
+        check_u8_args(hwc && query_ids && logits && boxes, n, h, w);
         MB_CHECK_ARG(seq > 0 && seq <= m->text.tokens, "query length %d out of range (1..%d)", seq, m->text.tokens);
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        const TowerW& T = m->vision;
-        const int S = T.d.image_size, P = T.grid * T.grid;
-        const int cap = image_batch_cap(m);
-        const size_t img_bytes = (size_t)h * w * 3, ids_bytes = round_up((size_t)seq * 4, 256);
-        ensure_in_dev(m, ids_bytes + (size_t)std::min(n, cap) * img_bytes);
+        ids_bytes = round_up((size_t)seq * 4, 256);
+        return ids_bytes + (size_t)std::min(n, image_batch_cap(m)) * img_bytes;
+    }, [&](Counter& c) {
+        const int P = m->vision.grid * m->vision.grid;
         const int32_t* d_ids = reinterpret_cast<const int32_t*>(m->in_dev.get());
         uint8_t* d_img = m->in_dev.get() + ids_bytes;
         float* d_logits = m->det.get();
         float* d_boxes = d_logits + (size_t)m->desc.max_batch * P;
         float* t = m->out_dev.get();   // the query's text embedding [embed_dim]
-        TimedRegion tr(m);
-        MB_CUDA(cudaMemcpyAsync(m->in_dev.get(), query_ids, (size_t)seq * 4, cudaMemcpyHostToDevice, m->stream));
-        forward_tokens(m, tr.c, d_ids, nullptr, nullptr, 1, seq, 0, t);
-        for (int o = 0; o < n; o += cap) {
-            const int nb = std::min(cap, n - o);
-            MB_CUDA(cudaMemcpyAsync(d_img, hwc + (size_t)o * img_bytes, (size_t)nb * img_bytes, cudaMemcpyHostToDevice,
-                                    m->stream));
-            const uint8_t* src = d_img;
-            if (h != S || w != S) {
-                tr.c.n += kernels::resize_squash_u8(src, nb, h, w, S, m->resized.get(), m->stream);
-                src = m->resized.get();
-            }
-            forward_detect(m, tr.c, src, nb, t, d_logits, d_boxes);
-            MB_CUDA(cudaMemcpyAsync(logits + (size_t)o * P, d_logits, (size_t)nb * P * 4, cudaMemcpyDeviceToHost,
-                                    m->stream));
-            MB_CUDA(cudaMemcpyAsync(boxes + (size_t)o * P * 4, d_boxes, (size_t)nb * P * 16, cudaMemcpyDeviceToHost,
-                                    m->stream));
-            MB_CUDA(cudaStreamSynchronize(m->stream));
-        }
-        tr.finish();
+        to_device(m, m->in_dev.get(), query_ids, (size_t)seq * 4);
+        forward_tokens(m, c, d_ids, nullptr, nullptr, 1, seq, 0, t);
+        host_batches(m, n, image_batch_cap(m), [&](int o, int nb) {
+            to_device(m, d_img, hwc + (size_t)o * img_bytes, nb * img_bytes);
+        }, [&](int, int nb) {
+            forward_detect(m, c, resize_images(m, c, d_img, nb, h, w), nb, t, d_logits, d_boxes);
+        }, {{logits, d_logits, (size_t)P}, {boxes, d_boxes, (size_t)P * 4}});
     });
 }
 
 int b200_model_encode_images_u8_ragged(b200_model* m, const uint8_t* const* hwc, const int32_t* heights,
                                        const int32_t* widths, int n, int normalize, float* out) {
-    return guarded([&] {
-        require_ready(m);
+    auto bytes = [&](int i) { return (size_t)heights[i] * widths[i] * 3; };
+    return model_call(m, Call::IMAGES, 0, [&] {
         MB_CHECK_ARG(out != nullptr, "NULL buffer");
-        check_ragged_args(m, hwc, heights, widths, n);
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        const int E = m->desc.embed_dim;
+        check_ragged_args(hwc, heights, widths, n);
         const int cap = image_batch_cap(m);
-        auto bytes = [&](int i) { return (size_t)heights[i] * widths[i] * 3; };
         size_t most = 0;   // the largest sub-batch's pixels: what in_dev must hold
         for (int o = 0; o < n; o += cap) {
             size_t sum = 0;
             for (int i = o; i < std::min(n, o + cap); ++i) sum += bytes(i);
             most = std::max(most, sum);
         }
-        ensure_in_dev(m, most);
+        return most;
+    }, [&](Counter& c) {
         std::vector<const uint8_t*> d_img((size_t)n);
-        TimedRegion tr(m);
-        for (int o = 0; o < n; o += cap) {
-            const int nb = std::min(cap, n - o);
+        host_batches(m, n, image_batch_cap(m), [&](int o, int nb) {
             size_t off = 0;
             for (int i = o; i < o + nb;) {
                 // one copy per run of images that lie back to back in host memory
@@ -2183,120 +2190,77 @@ int b200_model_encode_images_u8_ragged(b200_model* m, const uint8_t* const* hwc,
                     d_img[j] = d_img[i] + run;
                     run += bytes(j);
                 }
-                MB_CUDA(cudaMemcpyAsync(m->in_dev.get() + off, hwc[i], run, cudaMemcpyHostToDevice, m->stream));
+                to_device(m, m->in_dev.get() + off, hwc[i], run);
                 off += run;
                 i = j;
             }
-            encode_images_u8_ragged_dev(m, tr.c, d_img.data() + o, heights + o, widths + o, nb, normalize,
-                                        m->out_dev.get());
-            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
-                                    m->stream));
-            MB_CUDA(cudaStreamSynchronize(m->stream));
-        }
-        tr.finish();
+        }, [&](int o, int nb) {
+            encode_images_u8_ragged_dev(m, c, d_img.data() + o, heights + o, widths + o, nb, normalize, m->out_dev.get());
+        }, {{out, m->out_dev.get(), (size_t)m->desc.embed_dim}});
     });
 }
 
 int b200_model_encode_images_f32(b200_model* m, const float* chw, int n, int normalize, float* out) {
-    return guarded([&] {
-        require_ready(m);
+    size_t img = 0;   // floats per image
+    return model_call(m, Call::IMAGES, 0, [&] {
         MB_CHECK_ARG(chw && out, "NULL buffer");
-        check_encodes_images(m);
         MB_CHECK_ARG(n > 0, "n must be positive");
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        const int E = m->desc.embed_dim, S = m->vision.d.image_size;
-        const int cap = image_batch_cap(m);
-        const size_t img_bytes = (size_t)3 * S * S * 4;
-        ensure_in_dev(m, (size_t)std::min(n, cap) * img_bytes);
-        TimedRegion tr(m);
-        for (int o = 0; o < n; o += cap) {
-            const int nb = std::min(cap, n - o);
-            MB_CUDA(cudaMemcpyAsync(m->in_dev.get(), chw + (size_t)o * 3 * S * S, (size_t)nb * img_bytes,
-                                    cudaMemcpyHostToDevice, m->stream));
-            forward_images(m, tr.c, nullptr, reinterpret_cast<const float*>(m->in_dev.get()), nb, normalize,
-                           m->out_dev.get());
-            MB_CUDA(cudaMemcpyAsync(out + (size_t)o * E, m->out_dev.get(), (size_t)nb * E * 4, cudaMemcpyDeviceToHost,
-                                    m->stream));
-            MB_CUDA(cudaStreamSynchronize(m->stream));
-        }
-        tr.finish();
+        img = (size_t)3 * m->vision.d.image_size * m->vision.d.image_size;
+        return (size_t)std::min(n, image_batch_cap(m)) * img * 4;
+    }, [&](Counter& c) {
+        const float* d_chw = reinterpret_cast<const float*>(m->in_dev.get());
+        host_batches(m, n, image_batch_cap(m), [&](int o, int nb) {
+            to_device(m, m->in_dev.get(), chw + (size_t)o * img, nb * img * 4);
+        }, [&](int, int nb) {
+            forward_images(m, c, nullptr, d_chw, nb, normalize, m->out_dev.get());
+        }, {{out, m->out_dev.get(), (size_t)m->desc.embed_dim}});
     });
 }
 
 int b200_model_encode_tokens(b200_model* m, const int32_t* ids, const int32_t* attn_mask, int n, int seq, int normalize,
                              float* out) {
-    return guarded([&] { tokens_host(m, ids, attn_mask, nullptr, n, seq, normalize, out, false); });
+    return tokens_host(m, Call::TOKENS, ids, attn_mask, nullptr, n, seq, normalize, out);
 }
 
 int b200_model_classify_tokens(b200_model* m, const int32_t* ids, const int32_t* attn_mask, const int32_t* type_ids,
                                int n, int seq, int activation, float* out) {
-    return guarded([&] {
-        MB_CHECK_ARG(activation == 0 || activation == 1, "activation %d must be 0 (identity) or 1 (sigmoid)", activation);
-        tokens_host(m, ids, attn_mask, type_ids, n, seq, activation, out, true);
-    });
+    return tokens_host(m, Call::CLASSIFY, ids, attn_mask, type_ids, n, seq, activation, out);
 }
 
 int b200_model_encode_images_u8_device(b200_model* m, const uint8_t* d_hwc, int n, int h, int w, int normalize,
                                        float* d_out, int sync) {
-    return guarded([&] {
-        require_ready(m);
-        MB_CHECK_ARG(d_hwc && d_out, "NULL buffer");
-        check_encodes_images(m);
-        MB_CHECK_ARG(n > 0 && h > 0 && w > 0, "n, h, w must be positive");
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        TimedRegion tr(m);
-        encode_images_u8_dev(m, tr.c, d_hwc, n, h, w, normalize, d_out);
-        tr.finish();
-        if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
-    });
+    return model_call(m, Call::IMAGES, sync, [&] {
+        check_u8_args(d_hwc && d_out, n, h, w);
+        return 0;
+    }, [&](Counter& c) { encode_images_u8_dev(m, c, d_hwc, n, h, w, normalize, d_out); });
 }
 
 int b200_model_encode_images_u8_ragged_device(b200_model* m, const uint8_t* const* d_hwc, const int32_t* heights,
                                               const int32_t* widths, int n, int normalize, float* d_out, int sync) {
-    return guarded([&] {
-        require_ready(m);
+    return model_call(m, Call::IMAGES, sync, [&] {
         MB_CHECK_ARG(d_out != nullptr, "NULL buffer");
-        check_ragged_args(m, d_hwc, heights, widths, n);
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        TimedRegion tr(m);
-        encode_images_u8_ragged_dev(m, tr.c, d_hwc, heights, widths, n, normalize, d_out);
-        tr.finish();
-        if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
-    });
+        check_ragged_args(d_hwc, heights, widths, n);
+        return 0;
+    }, [&](Counter& c) { encode_images_u8_ragged_dev(m, c, d_hwc, heights, widths, n, normalize, d_out); });
 }
 
 int b200_model_encode_tokens_device(b200_model* m, const int32_t* d_ids, const int32_t* d_attn_mask, int n, int seq,
                                     int normalize, float* d_out, int sync) {
-    return guarded([&] {
-        require_ready(m);
+    return model_call(m, Call::TOKENS, sync, [&] {
         MB_CHECK_ARG(d_ids && d_out, "NULL buffer");
         check_tokens_args(m, n, seq);
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        TimedRegion tr(m);
-        encode_tokens_dev(m, tr.c, d_ids, d_attn_mask, nullptr, n, seq, normalize, d_out);
-        tr.finish();
-        if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
-    });
+        return 0;
+    }, [&](Counter& c) { encode_tokens_dev(m, c, d_ids, d_attn_mask, nullptr, n, seq, normalize, d_out); });
 }
 
 int b200_model_classify_tokens_device(b200_model* m, const int32_t* d_ids, const int32_t* d_attn_mask,
                                       const int32_t* d_type_ids, int n, int seq, int activation, float* d_out, int sync) {
-    return guarded([&] {
-        require_ready(m);
+    return model_call(m, Call::CLASSIFY, sync, [&] {
         MB_CHECK_ARG(d_ids && d_out, "NULL buffer");
         MB_CHECK_ARG(activation == 0 || activation == 1, "activation %d must be 0 (identity) or 1 (sigmoid)", activation);
-        check_tokens_args(m, n, seq, true);
-        std::lock_guard<std::mutex> lk(m->mu);
-        DeviceGuard g(m->device);
-        TimedRegion tr(m);
-        encode_tokens_dev(m, tr.c, d_ids, d_attn_mask, d_type_ids, n, seq, activation, d_out);
-        tr.finish();
-        if (sync) MB_CUDA(cudaStreamSynchronize(m->stream));
-    });
+        check_tokens_args(m, n, seq);
+        return 0;
+    }, [&](Counter& c) { encode_tokens_dev(m, c, d_ids, d_attn_mask, d_type_ids, n, seq, activation, d_out); });
 }
 
 int b200_model_set_stream(b200_model* m, void* cuda_stream, int use_external) {
